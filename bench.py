@@ -1,7 +1,8 @@
-"""bench.py - FullSubNet inference throughput on B200 (BASELINE.json metric: frames/s and x real-time,
+"""bench.py - FullSubNet inference throughput on H100 (BASELINE.json metric: frames/s and x real-time,
 16 kHz, n_fft=512, hop=256) for the workload `configs[1]`: batch = 256 x 4 s synthetic clips per GPU.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--precision auto|fp32|f16x3_tc|f16_tc] [--no-extras]
+                  [--dump-outputs DIR]
   python bench.py --impl reference      # the CPU arm (oracle port of the reference path, all host threads)
 
 One "step" = one pass of the hot path (stft -> model -> decompress/mask -> istft) over one batch.
@@ -9,6 +10,8 @@ One "step" = one pass of the hot path (stft -> model -> decompress/mask -> istft
 buffers, the H2D copy of the waveforms and the D2H copy of the result inside the timed region.
 Multi-GPU: one process per GPU (torchrun), clips sharded over ranks, no data-path collective (weak
 scaling: every rank enhances its own B clips); time = max over ranks.
+--dump-outputs DIR writes what the last timed step returned (the enhanced waveforms, float32) as DIR/wav.npy, a fixed
+seeded sample of at most 64 MB; the inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -20,7 +23,10 @@ import sys
 import threading
 import time
 
-import torch
+# The training extra frees and re-allocates its ~41 GB activation workspace every step; without expandable segments the
+# caching allocator splits the freed block for small tensors and the next step no longer fits in 80 GB.
+os.environ.setdefault("PYTORCH_CUDA_ALLOC_CONF", "expandable_segments:True")
+import torch  # noqa: E402
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
@@ -36,11 +42,12 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 / FP16 989 TFLOP/s - data-sheet figures, not measured
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "fallback"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -169,6 +176,26 @@ def run_reference(args):
     print(json.dumps(line))
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor of the last timed step.  Rows (clips) beyond the size limit are sampled with a fixed
+    seed, sorted, and their indices stored beside them as <name>_rows.npy."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        a = a.reshape(a.shape[0], -1)
+        rows = a.shape[0]
+        keep = max(1, min(rows, DUMP_LIMIT_BYTES // max(1, a[0].nbytes)))
+        if keep < rows:
+            idx = np.sort(np.random.default_rng(0).choice(rows, size=keep, replace=False))
+            a = a[idx]
+            np.save(os.path.join(out_dir, f"{name}_rows.npy"), idx.astype(np.float64))
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -186,8 +213,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the `precisions`, `latency_b1` and `train_dp` objects")
     ap.add_argument("--no-train", action="store_true", help="skip the `train_dp` object")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output of the last timed step as DIR/<name>.npy (float32, <= 64 MB)")
     args = ap.parse_args()
     if args.model == "fullsubnet_train":
+        if args.dump_outputs:
+            ap.error("--dump-outputs covers the inference workloads")
         import bench_train
         return bench_train.main(args)
     if args.impl == "reference":
@@ -248,7 +279,7 @@ def main():
     host_in = O.make_noisy(B, L, seed=rank).pin_memory()  # every rank enhances its own clips
     host_out = torch.empty(B, L, dtype=torch.float32).pin_memory()
     x_dev = host_in.to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         if dist is not None:
@@ -280,14 +311,17 @@ def main():
             ms = float(t.item())
         return ms / steps, [s / steps for s in stage]
 
+    last = {}
+
     def step_resident():
         if args.model == "fullsubnet":
-            model.enhance(x_dev, N_FFT, HOP, WIN)
+            out = model.enhance(x_dev, N_FFT, HOP, WIN)
         elif args.model == "improved_fullsubnet":
             with torch.no_grad():
-                model(x_dev)  # wav -> wav (improved_fullsubnet/model.py:541-591)
+                out = model(x_dev)  # wav -> wav (improved_fullsubnet/model.py:541-591)
         else:
-            inf.enhance_batch(x_dev)
+            out = inf.enhance_batch(x_dev)
+        last["wav"] = out
 
     def step_e2e():
         if args.model == "improved_fullsubnet":
@@ -302,6 +336,8 @@ def main():
     sampler.start()
     ms_step, _ = timed(step_resident, args.steps, args.warmup)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     launches = int(lib.fsn_last_launch_count())
     # second pass with stage events on (separate from the headline timing)
     _, stage_ms = timed(step_resident, max(2, min(args.steps, 3)), 1, prof=True)
@@ -321,9 +357,7 @@ def main():
         number of MMA passes the precision needs) over the CUDA-event time of the stage."""
         achieved = sb_flops / (sb_ms * 1e-3) / 1e12 if sb_ms > 0 else None
         passes = {"f16x3_tc": 3, "f16_tc": 1}.get(prec)
-        key = {"f16x3_tc": "sb_lstm_tc2_kernel<x3>", "f16_tc": "sb_lstm_tc2_kernel"}.get(prec)
-        if prec == "f16_tc" and os.environ.get("FSN_TC_PAIR", "1") == "0":
-            key = "sb_lstm_tc_kernel"
+        key = {"f16x3_tc": "sb_lstm_tc_kernel<x3>", "f16_tc": "sb_lstm_tc_kernel"}.get(prec)
         r = {"kernel": f"sub-band LSTM stack ({prec})", "bound": "tensor" if passes else "fma", "achieved": achieved,
              "peak": peak_tf, "unit": "TFLOP/s", "frac": (achieved / peak_tf) if achieved else None,
              "traffic": tj.get(key, {}).get("dram_bytes_per_launch") if (key and B == 256) else None,
@@ -407,7 +441,7 @@ def main():
                 "fullband_weight_stream": {
                     "bytes_per_step": fb_bytes, "achieved_gbs": fb_bytes / (1e-3 * st[1] / (T + 2)) / 1e9,
                     "hbm_peak_gbs": peaks.get("hbm_gbs"),
-                    "frac_of_hbm_peak": fb_bytes / (1e-3 * st[1] / (T + 2)) / 1e9 / peaks.get("hbm_gbs", 6582.5),
+                    "frac_of_hbm_peak": fb_bytes / (1e-3 * st[1] / (T + 2)) / 1e9 / peaks.get("hbm_gbs", 3350.0),
                     "note": "the persistent kernel keeps the weights in shared memory for all 253 steps (HBM is read "
                             "once, 15.2 MB per launch); the figure is the SMEM-resident weight bytes one step consumes "
                             "over the step time, i.e. what an HBM-streaming GEMV would have to sustain to keep up; "

@@ -1,4 +1,4 @@
-"""bench_train.py - FullSubNet TRAINING step on B200 (BASELINE configs[2]: batch = 64 x 3 s clips per GPU, cIRM MSE
+"""bench_train.py - FullSubNet TRAINING step on H100 (BASELINE configs[2]: batch = 64 x 3 s clips per GPU, cIRM MSE
 loss, data-parallel with one gradient all-reduce).  Same JSON contract as bench.py (which dispatches here for
 ``--model fullsubnet_train``).
 
@@ -197,16 +197,15 @@ def measure(args, dist, dev, rank, world, local, cpu_leg=True):
         "e2e": {"value": e2e_value, "unit": "frames/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": 2 * B * L * 4,
                 "d2h_bytes_per_step": 4},
         "gpu_launches": launches, "clocks": clocks,
-        "roofline": {"kernel": "whole training step; tcgen05 kernels: lstm_fwd_step_kernel (fused recurrent GEMM + cell, "
-                               "kind::f16 / tf32) and tgemm_tma_kernel (kind::tf32: BPTT and weight-gradient GEMMs), "
-                               "together about 60 % of the step (profiles/r02h_train_step_launches_summary.txt)"
+        "roofline": {"kernel": "whole training step; wgmma kernels: lstm_fwd_step_kernel (fused recurrent GEMM + cell, "
+                               "f16 / tf32) and tgemm_tma_kernel (tf32: BPTT and weight-gradient GEMMs)"
                                if precision == "tf32_tc" else "whole training step (fp32 FMA GEMMs)",
                      "bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
                      "frac": achieved / peak_tf, "traffic": traffic,
                      "peak_source": f"{peak_kind} bf16_tflops_sustained (the dense tf32 rate is half of it)",
                      "flops_per_launch": flops, "ms_per_launch": ms_step,
                      "note": "achieved = algorithmic FLOPs of the whole step (3 x forward) / step time; traffic = DRAM "
-                             "bytes of one BPTT-step GEMM launch (profiles/traffic.json)"},
+                             "bytes of one BPTT-step GEMM launch (profiles/traffic.json when present)"},
     }
     line["allreduce"] = allreduce
     if rank == 0 and cpu_leg and world == 1:

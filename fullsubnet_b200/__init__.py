@@ -1,4 +1,4 @@
-"""fullsubnet_b200 - B200 (sm_100a) implementation of FullSubNet's enhancement hot path behind
+"""fullsubnet_b200 - H100 (sm_90a) implementation of FullSubNet's enhancement hot path behind
 the reference's own Python API (Audio-WestlakeU/FullSubNet, recipes/dns_interspeech_2020).
 
 Layout mirrors the reference so that TOML ``path`` strings keep working:

@@ -150,7 +150,7 @@ def load() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"fullsubnet_b200: {LIB_PATH} is missing. Build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a). There is no CPU/PyTorch fallback for this path.")
+                "g.build()'` (nvcc, sm_90a). There is no CPU/PyTorch fallback for this path.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(lib, name)  # AttributeError if the ABI is incomplete

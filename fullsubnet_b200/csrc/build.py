@@ -1,4 +1,4 @@
-"""Builds libfsn_b200.so in-tree with nvcc for sm_100a (no torch headers: the library is a
+"""Builds libfsn_b200.so in-tree with nvcc for sm_90a (H100) (no torch headers: the library is a
 plain C-ABI CUDA library; the Python host binds it with ctypes)."""
 from __future__ import annotations
 
@@ -7,11 +7,11 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["fsn_dsp.cu", "fsn_dsp_dft.cu", "fsn_lstm_simt.cu", "fsn_subband_tc.cu", "fsn_subband_tc2.cu", "fsn_subband_tc4.cu", "fsn_fullband.cu", "fsn_lstm_rec_tc.cu", "fsn_fast_model.cu", "fsn_improved.cu", "fsn_fullband_baseline.cu", "fsn_train.cu", "fsn_mix.cu", "fsn_tgemm.cu", "fsn_model.cu"]
+SOURCES = ["fsn_dsp.cu", "fsn_dsp_dft.cu", "fsn_lstm_simt.cu", "fsn_subband_tc.cu", "fsn_fullband.cu", "fsn_lstm_rec_tc.cu", "fsn_fast_model.cu", "fsn_improved.cu", "fsn_fullband_baseline.cu", "fsn_train.cu", "fsn_mix.cu", "fsn_tgemm.cu", "fsn_model.cu"]
 LIB = os.path.join(HERE, "libfsn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC", "-DFSN_BUILT_ARCH=100", "--use_fast_math=false"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-DFSN_BUILT_ARCH=90", "--use_fast_math=false"]
 
 
 def needs_build() -> bool:
@@ -42,7 +42,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             print(out)
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {s}")
-    subprocess.check_call([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([NVCC, "-shared", "-o", LIB, *objs, *ARCH])
     return LIB
 
 

@@ -334,7 +334,7 @@ __global__ void si_sdr_kernel(const float* __restrict__ ref, const float* __rest
 
 static int ew_grid(int64_t n) {
   int64_t g = (n + 255) / 256;
-  return (int)(g < 1 ? 1 : (g > 148 * 16 ? 148 * 16 : g));
+  return (int)(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
 }
 
 static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }

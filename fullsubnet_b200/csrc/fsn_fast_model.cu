@@ -84,7 +84,7 @@ struct FastDims { int B, T, Tp, F, M, K, Ts, S; };
 
 static bool fast_tc_ok(const fsn_fast_desc* d) {
   const int K = (2 * d->noisy_num_neighbors + 1) + (2 * d->enc_num_neighbors + 1);
-  return sb_tc2_enabled() && d->bn_hidden == 384 && d->bn_layers == 2 && K <= 32;
+  return d->bn_hidden == 384 && d->bn_layers == 2 && K <= 32;
 }
 static bool fast_x3(const fsn_fast_desc* d) { return d->precision == FSN_PREC_F16X3_TC; }
 
@@ -183,7 +183,7 @@ static int run_lstm_pair(const fsn_lstm_layer& la, int Ka, int Ha, const fsn_lst
   int rc;
   static const bool stepwise = getenv("FSN_FB_STEPWISE") != nullptr;
   if (!stepwise && tc && tc_mid && x_step_stride == (size_t)Ka && x_row_stride == (size_t)steps * Ka) {
-    // tensor cores: per layer one hoisted input-projection GEMM + the persistent tcgen05 recurrence
+    // tensor cores: per layer one hoisted input-projection GEMM + the persistent wgmma recurrence
     if ((rc = lstm_layer_tc(la, x, (size_t)Ka, Ka, row_scale, steps, 0, R, steps, Ha, x3, *tc, tc_mid, st))) return rc;
     return lstm_layer_tc(lb, tc_mid, (size_t)Ha, Ha, nullptr, 1, 0, R, steps, Hb, x3, *tc, hb_all, st);
   }
@@ -235,7 +235,7 @@ extern "C" size_t fsn_fast_workspace_bytes(const fsn_fast_desc* d, int B, int T)
   return w.bytes;
 }
 
-extern "C" size_t fsn_fast_packed_bytes(const fsn_fast_desc* d) { return fast_tc_ok(d) ? sb_tc2_packed_bytes(fast_x3(d)) : 0; }
+extern "C" size_t fsn_fast_packed_bytes(const fsn_fast_desc* d) { return fast_tc_ok(d) ? sb_tc_packed_bytes_raw(d->bn_hidden, fast_x3(d)) : 0; }
 
 extern "C" int fsn_fast_pack_bn_weights(const fsn_fast_desc* d, const fsn_fast_weights* wt, void* packed,
                                         fsn_stream_t stream) {
@@ -244,7 +244,7 @@ extern "C" int fsn_fast_pack_bn_weights(const fsn_fast_desc* d, const fsn_fast_w
   for (int l = 0; l < 2; ++l) { s.w_ih[l] = wt->bn[l].w_ih; s.w_hh[l] = wt->bn[l].w_hh; s.b_ih[l] = wt->bn[l].b_ih; s.b_hh[l] = wt->bn[l].b_hh; }
   s.fc_w = wt->bn_fc_w; s.fc_b = wt->bn_fc_b;
   const int K = (2 * d->noisy_num_neighbors + 1) + (2 * d->enc_num_neighbors + 1);
-  return sb_tc2_pack_raw(&s, K, /*fc_out=*/1, packed, (cudaStream_t)stream, fast_x3(d));
+  return sb_tc_pack_raw(&s, d->bn_hidden, K, /*fc_out=*/1, packed, (cudaStream_t)stream, fast_x3(d));
 }
 
 extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* mix_mag, int B,
@@ -291,7 +291,7 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   const int Hb = d->bn_hidden;
   int bn_bstride = M;
   if (fast_is_tc(d)) {
-    // tcgen05 CTA-pair kernel of the fullsubnet sub-band stack: same stack shape (K<=32 -> 384 -> 384), the gather
+    // tensor-core kernel of the fullsubnet sub-band stack: same stack shape (K<=32 -> 384 -> 384), the gather
     // does the unfold AND the time down-sampling on the fly from melT / encT, Linear output 1 of 2 is zero-padded
     FSN_REQUIRE(wt->bn_packed && fast_tc_ok(d), FSN_ERR_UNSUPPORTED,
                 "fast model: the tensor-core precisions need packed bottleneck weights, bn_hidden = 384 and input width <= 32");
@@ -299,9 +299,9 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
     memset(&a, 0, sizeof(a));
     a.packed = wt->bn_packed; a.magT = w.melT; a.fbT = w.encT; a.inv2 = w.inv2; a.crm = w.bn_out;
     a.B = B; a.F = M; a.Tp = Tp; a.la = 0; a.Ns = d->noisy_num_neighbors; a.Nf = d->enc_num_neighbors;
-    a.H = Hb; a.act = FSN_ACT_RELU; a.steps = m.Ts; a.shrink = m.S; a.pair = true; a.x3 = fast_x3(d);
+    a.H = Hb; a.act = FSN_ACT_RELU; a.steps = m.Ts; a.shrink = m.S; a.x3 = fast_x3(d);
     a.map = RowMap{B, M, M, 1};
-    if ((rc = sb_tc2_forward(a, st))) return rc;
+    if ((rc = sb_tc_forward(a, st))) return rc;
     bn_bstride = 2 * M;
   } else {
   for (int t = 0; t < m.Ts; ++t) {
@@ -331,7 +331,7 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   {
     const size_t n = (size_t)B * Tp * 2 * M;
     int g = (int)((n + 255) / 256);
-    if (g > 148 * 16) g = 148 * 16;
+    if (g > 132 * 16) g = 132 * 16;
     fast_dec_input_kernel<<<g, 256, 0, st>>>(w.encT, w.bn_out, bn_bstride, B, Tp, M, m.S, m.Ts, w.dec_in);
     FSN_CHECK_LAUNCH("fast_dec_input_kernel");
   }

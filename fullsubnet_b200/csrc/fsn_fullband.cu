@@ -252,7 +252,7 @@ size_t fb_persistent_smem(int F, int H0, int H1) {
 }
 
 bool fb_persistent_supported(int F, int H0, int H1) {
-  static int coop = -1, max_smem = 0, sms = 148;
+  static int coop = -1, max_smem = 0, sms = 132;
   if (coop < 0) {
     int dev = 0;
     cudaGetDevice(&dev);
@@ -273,7 +273,7 @@ int fb_persistent_launch(const fsn_seq_weights* w, const float* x_chunk, const f
   for (int l = 0; l < 2; ++l) { a.w_ih[l] = w->w_ih[l]; a.w_hh[l] = w->w_hh[l]; a.b_ih[l] = w->b_ih[l]; a.b_hh[l] = w->b_hh[l]; }
   a.x = x_chunk; a.inv1 = inv1_chunk; a.h0buf = h0buf; a.h1all = h1all_chunk; a.barrier = barrier;
   a.B = nb; a.F = F; a.H0 = H0; a.H1 = H1; a.Tp = Tp;
-  int sms = 148;
+  int sms = 132;
   { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
   const int Hm = H0 > H1 ? H0 : H1;
   int upc = 1;

@@ -130,7 +130,7 @@ extern "C" int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_l
   if ((rc = fc_gemm_launch(last, fc_w, fc_b, w.y, B * Tp, H, 2 * F, d->activation, st))) return rc;
   const size_t n = (size_t)B * 2 * F * T;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   fbb_output_kernel<<<blocks, 256, 0, st>>>(w.y, out, B, F, T, Tp, d->look_ahead);
   FSN_CHECK_LAUNCH("fbb_output_kernel");
   return FSN_OK;

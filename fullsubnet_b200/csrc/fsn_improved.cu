@@ -225,7 +225,7 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
   if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)Fu * T, 1.f, w.inv1, nullptr, st, eps))) return rc;
   const bool fb_tc = w.fbtc_mid != nullptr;
   if (fb_tc) {
-    // tensor cores: per layer one hoisted input-projection GEMM (tf32) + the persistent tcgen05 recurrence, Linear likewise
+    // tensor cores: per layer one hoisted input-projection GEMM (tf32) + the persistent wgmma recurrence, Linear likewise
     fsn_lstm_layer L0{wt->fb.w_ih[0], wt->fb.w_hh[0], wt->fb.b_ih[0], wt->fb.b_hh[0]};
     fsn_lstm_layer L1{wt->fb.w_ih[1], wt->fb.w_hh[1], wt->fb.b_ih[1], wt->fb.b_hh[1]};
     if ((rc = lstm_layer_tc(L0, w.magc, (size_t)Fu, Fu, w.inv1, T, 0, B, T, Hf, false, w.fbtc, w.fbtc_mid, st))) return rc;
@@ -276,12 +276,12 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
     if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)g.N * g.W * T, 1.f, w.invs, nullptr, st, eps))) return rc;
     const fsn_seq_weights& sw = wt->sb[s];
     if (d->precision == FSN_PREC_TF32_TC) {
-      // layer by layer over all steps: hoisted input projection + per-step recurrent GEMM on tcgen05 (tf32), fused cell
+      // layer by layer over all steps: hoisted input projection + per-step recurrent GEMM on wgmma (tf32), fused cell
       LayerSave l1{w.tc.G, w.tc.C, w.tc_h1};
       {  // scale X by the section norm in place (the tensor-core GEMM reads plain fp32 rows)
         const size_t n = (size_t)T * R * g.W;
         int blocks = (int)((n + 255) / 256);
-        if (blocks > 148 * 16) blocks = 148 * 16;
+        if (blocks > 132 * 16) blocks = 132 * 16;
         imp_scale_rows_kernel<<<blocks, 256, 0, st>>>(w.X, w.invs, n, (size_t)R * g.W, (size_t)g.N * g.W, B);
         FSN_CHECK_LAUNCH("imp_scale_rows_kernel");
       }

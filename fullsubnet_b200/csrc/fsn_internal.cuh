@@ -56,7 +56,7 @@ int cum_clip_scale_launch(const float2* fs, int B, int Tp, int F, float eps, flo
 int cum_unit_scale_launch(const float* magT, const float* fbT, RowMap map, int R, int Tp, int Ns, int Nf, float eps,
                           float* scaleT, cudaStream_t st, bool time_major = false);
 
-// tf32 tcgen05 GEMM (fsn_tgemm.cu): C[M,N] (+)= A[M,K] B[N,K]^T, fp32 row-major operands with 16-byte aligned rows
+// tf32 wgmma GEMM (fsn_tgemm.cu): C[M,N] (+)= A[M,K] B[N,K]^T, fp32 row-major operands with 16-byte aligned rows
 bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, int K);
 int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
                  bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st);
@@ -140,7 +140,7 @@ int fb_persistent_launch(const fsn_seq_weights* w, const float* x_chunk, const f
                          cudaStream_t st);
 
 // tensor-core LSTM layer for a small batch of sequences (fsn_lstm_rec_tc.cu): hoisted input projection on the tf32
-// GEMM (x3: three passes on tf32 hi/lo splits) + persistent cooperative tcgen05 recurrence (x3: fp16 hi/lo splits)
+// GEMM (x3: three passes on tf32 hi/lo splits) + persistent cooperative wgmma recurrence (x3: fp16 hi/lo splits)
 bool lstm_rec_tc_supported(int H, bool x3);
 int lstm_rec_tc_rows_per_launch(int H);
 size_t lstm_rec_tc_scratch_bytes(int H, bool x3);
@@ -161,35 +161,23 @@ int linear_tc(const float* x, size_t ldx, int K, const float* W, const float* bi
 int gemm_tc_split_launch(const float* a, size_t lda, const float* W, int N, int K, float* w, float* C, size_t ldc, size_t M,
                          bool x3, cudaStream_t st);
 
-// tcgen05 sub-band stack (fsn_subband_tc.cu)
+// tensor-core sub-band stack (fsn_subband_tc.cu)
 struct SbTcArgs {
-  const void* packed;       // tile-ordered fp16 weights (fsn_pack_sb_weights)
+  const void* packed;       // tile-ordered fp16 weights (fsn_pack_sb_weights / sb_tc_pack_raw)
   const float* magT; const float* fbT; const float* inv2;
   const float* unit_scale;  // nullable: per-row scale of this step (cumulative norm) instead of inv2[clip]
   float* crm;
   int B, F, Tp, la, Ns, Nf, H, act;
-  int steps, shrink;      // pair kernel only: LSTM steps (0 = Tp) and time down-sampling of the gathered input (0/1 = none)
-  bool pair;              // packed for / run by the CTA-pair kernel
-  bool x3;                // pair kernel only: error-compensated variant (FSN_PREC_F16X3_TC image)
-  bool quad;              // packed for / run by the 6-CTA-cluster kernel (fsn_subband_tc4.cu)
+  int steps, shrink;      // LSTM steps (0 = Tp) and time down-sampling of the gathered input (0/1 = none)
+  bool x3;                // error-compensated variant (FSN_PREC_F16X3_TC image)
   RowMap map;
 };
 size_t sb_tc_packed_bytes(const fsn_model_desc* d);
+size_t sb_tc_packed_bytes_raw(int H, bool x3);
 int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed, cudaStream_t st);
+// weights of a 2-layer stack of hidden size H over Ksb inputs with a Linear(H -> fc_out <= 2) on top
+int sb_tc_pack_raw(const fsn_seq_weights* sb, int H, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3);
 int sb_tc_forward(const SbTcArgs& a, cudaStream_t st);
 bool sb_tc_supported(const fsn_model_desc* d);
-
-// CTA-pair (cta_group::2) variant (fsn_subband_tc2.cu); preferred when the shape allows (H = 384)
-bool sb_tc2_supported(const fsn_model_desc* d);
-size_t sb_tc2_packed_bytes(bool x3 = false);
-int sb_tc2_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed, cudaStream_t st);
-int sb_tc2_forward(const SbTcArgs& a, cudaStream_t st);
-int sb_tc2_pack_raw(const fsn_seq_weights* sb, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3 = false);
-// cluster (three pairs = 6 CTAs, N = 128) variant (fsn_subband_tc4.cu); experimental, single fp16 pass, H = 384; FSN_TC_CLUSTER4=1
-bool sb_tc4_supported(const fsn_model_desc* d);
-size_t sb_tc4_packed_bytes();
-int sb_tc4_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed, cudaStream_t st);
-int sb_tc4_forward(const SbTcArgs& a, cudaStream_t st);
-bool sb_tc2_enabled();  // H = 384 stacks may use the pair kernel (FSN_TC_PAIR != 0)
 
 }  // namespace fsn

@@ -1,4 +1,4 @@
-// One LSTM layer for a SMALL batch of sequences (rows = clips) on the tensor cores (tcgen05, sm_100a):
+// One LSTM layer for a SMALL batch of sequences (rows = clips) on the tensor cores (wgmma, sm_90a):
 //   1. the input projection of ALL steps hoisted into one GEMM  P[r,t,:] = x[r,t,:] W_ih^T   (tgemm_tma_kernel, tf32;
 //      three passes on tf32 hi/lo splits for the fp32 error class), and
 //   2. the recurrence  gates_t = P_t + b + h_{t-1} W_hh^T  as ONE persistent cooperative kernel (this file).
@@ -8,14 +8,15 @@
 //
 // Mapping of the recurrence.  The batch is small (<= 128 rows per group) and the steps are serial, so the HIDDEN
 // dimension is spread over the chip: CTA j of a group owns 8 hidden units = 32 gate columns and keeps that slice of
-// W_hh resident in shared memory for the whole sequence (fp16, UMMA K-major 128B-swizzled; compensated mode: hi and lo
-// parts).  Per step every CTA needs ALL of h_{t-1}: the epilogues publish h_t as fp16 (hi [+ lo]) in a ping-pong array
+// W_hh resident in shared memory for the whole sequence (fp16, K-major 128B-swizzled; compensated mode: hi and lo
+// parts).  Per step every CTA needs ALL of h_{t-1}: the consumers publish h_t as fp16 (hi [+ lo]) in a ping-pong array
 // in global memory (it lives in L2), a per-group counter is the step barrier, and each CTA's producer warp streams the
-// [128 rows x K] state through a TMA ring.  Rows sit on the M side of the MMA:
-//     D[128 rows, 32 | 64 gate columns] += h_hi[128, 16] . [W_hi ; W_lo]^T   (one MMA, N = 64: the lo product lands in
-//     D[128 rows, 32]                    += h_lo[128, 16] . W_hi^T             columns 32..63 and is added in the epilogue)
-// so the thread that owns TMEM lane r sees all four gates of the CTA's 8 units for row r: c stays in 8 registers, no
-// exchange.  Two groups of 64 CTAs cover 256 clips with H = 512.
+// [128 rows x K] state through a TMA ring.  Rows sit on the M side of the MMA (two m64 halves per warpgroup):
+//     D[64 rows, 32 | 64 gate columns] += h_hi[64, 16] . [W_hi ; W_lo]^T   (N = 64: the lo product lands in
+//     D[64 rows, 32]                    += h_lo[64, 16] . W_hi^T             columns 32..63 and is added in the cell)
+// Column block j (8 columns) of D is gate j % 4, so the thread that holds a row's fragment holds all four gates of
+// the same two units: c stays in 8 registers (4 rows x 2 units), no exchange.  Groups of 64 CTAs cover 128 clips
+// each with H = 512.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <string.h>
@@ -23,23 +24,22 @@
 
 #include "fsn_internal.cuh"
 #include "fsn_tc_ptx.cuh"
+#include "fsn_wgmma.cuh"
 
 namespace fsn {
 namespace rec {
 using namespace ptx;
 
-constexpr int MR = 128;               // rows per group (MMA M)
+constexpr int MR = 128;               // rows per group (two m64 MMA halves)
 constexpr int U = 8;                  // hidden units per CTA
 constexpr int NG = 4 * U;             // gate columns per CTA
 constexpr int KB = 64;                // k-block: one 128-byte swizzled row of fp16
 constexpr int A_TILE = MR * KB * 2;   // 16 KB
-constexpr int NTHREADS = 192;         // warp 0: TMA producer, warp 1: MMA issue + TMEM, warps 2-5: epilogue
+constexpr int NTHREADS = 160;         // warps 0-3: MMA + cell (one warpgroup), warp 4: TMA producer
 constexpr int MAX_STAGES = 6;
 
 struct Bars {
   uint64_t full[MAX_STAGES], empty[MAX_STAGES];
-  uint64_t acc_full, acc_empty;
-  uint32_t tmem_base;
 };
 
 struct Args {
@@ -50,16 +50,6 @@ struct Args {
   unsigned int* barrier;                                      // one counter per group, 32 words apart
   int R, T, H, Kp, Rpad, C, stages, fence_all;
 };
-
-__device__ __forceinline__ void tc_mma1_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 
 template <bool X3> __device__ __forceinline__ float act_sigmoid(float x) {
   return X3 ? 1.0f / (1.0f + expf(-x)) : fast_sigmoid(x);
@@ -74,8 +64,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
   constexpr int STAGE_BYTES = PARTS * A_TILE;
   constexpr int WB_ROWS = PARTS * NG;          // rows of the resident weight operand per k-block: [W_hi ; W_lo]
   constexpr int WB_BYTES = WB_ROWS * 128;
-  constexpr uint32_t kIdescMain = (1u << 4) | ((uint32_t)(WB_ROWS >> 3) << 17) | ((128u >> 4) << 24);
-  constexpr uint32_t kIdescLo = (1u << 4) | ((uint32_t)(NG >> 3) << 17) | ((128u >> 4) << 24);
+  constexpr int NACC = WB_ROWS / 2;            // accumulator registers per m64 half
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int nkb = a.Kp / KB;
@@ -88,16 +77,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
   const int H = a.H, T = a.T;
   unsigned int* counter = a.barrier + g * 32;
 
-  // ---------------- one-time setup: barriers, TMEM, resident weight slice
+  // ---------------- one-time setup: barriers, resident weight slice
   if (threadIdx.x == 0) {
-    for (int s = 0; s < a.stages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 1); }
-    mbar_init(&bars.acc_full, 1);
-    mbar_init(&bars.acc_empty, 128);
+    for (int s = 0; s < a.stages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 64;" ::"r"(smem_u32(&bars.tmem_base)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   // weight operand: k-block kb = rows [W_hi (gate col n = gate*8 + ul) ; W_lo] x 64 k, 128B swizzle
   for (int idx = threadIdx.x; idx < nkb * NG * (KB / 8); idx += NTHREADS) {
@@ -118,12 +101,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
     if (X3) *reinterpret_cast<uint4*>(blk + swz128_off(NG + n, ch * 8)) = *reinterpret_cast<const uint4*>(lo);
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars.tmem_base;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ================= producer: after the group has published h_{p-1}, stream it through the ring
     uint32_t it = 0;
     for (int p = 1; p < T; ++p) {
@@ -132,7 +112,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
         unsigned int v, spins = 0;
         do {
           asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(counter) : "memory");
-          if (++spins > (1u << 27)) { printf("fsn rec: step barrier timeout (block %d step %d)\n", blockIdx.x, p); __trap(); }
+          if (++spins > (1u << 27)) asm volatile("trap;");  // a lost publication traps instead of hanging
         } while (v < target);
       }
       __syncwarp();
@@ -151,120 +131,124 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
         __syncwarp();
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issue (converged warp, one elected lane)
-    uint32_t it = 0;
-    const uint64_t wdesc0 = desc_sw128(smem_u32(wsm));
-    const uint64_t adesc0 = desc_sw128(smem_u32(ring));
-    for (int p = 1; p < T; ++p) {
-      mbar_wait<false>(&bars.acc_empty, (p - 1) & 1);  // the epilogue of step p-1 has drained the accumulator
-      tc_fence_after();
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        const uint32_t s = it % (uint32_t)a.stages, use = it / (uint32_t)a.stages;
-        mbar_wait<false>(&bars.full[s], use & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t ad = adesc0 + (uint64_t)((s * STAGE_BYTES) >> 4);
-          const uint64_t wd = wdesc0 + (uint64_t)(((uint32_t)kb * WB_BYTES) >> 4);
-#pragma unroll
-          for (int k = 0; k < KB / 16; ++k) {
-            tc_mma1_f16(tmem_base, ad + (uint64_t)(2 * k), wd + (uint64_t)(2 * k), kIdescMain, (kb | k) ? 1u : 0u);
-            if (X3) tc_mma1_f16(tmem_base, ad + (uint64_t)((A_TILE >> 4) + 2 * k), wd + (uint64_t)(2 * k), kIdescLo, 1u);
-          }
-          tc_commit1(&bars.empty[s]);
-        }
-        __syncwarp();
-      }
-      if (elect_one()) tc_commit1(&bars.acc_full);
-      __syncwarp();
-    }
   } else {
-    // ================= epilogue: thread = row (TMEM lane), 8 units x 4 gates in its columns
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int r = g * MR + row;
-    const bool valid = r < a.R;
-    const bool vec_ok = (H & 3) == 0 && (a.p_row & 3) == 0 && (a.p_t & 3) == 0 && (a.h_row & 3) == 0 && (a.h_t & 3) == 0;
-    float bias[NG];
+    // ================= consumers: MMA, then the cell on the fragment.  Thread rows: 16 warp + lane/4 + 8 hh + 64 half;
+    // units u0 + 2 (lane % 4) + e; gate = column block % 4 (block + 4: the lo product of X3)
+    const int q = warp;
+    const int ul0 = 2 * (lane & 3);
+    const bool vec_ok = (H & 1) == 0 && (a.p_row & 1) == 0 && (a.p_t & 1) == 0 && (a.h_row & 1) == 0 && (a.h_t & 1) == 0;
+    float bias[4][2];
 #pragma unroll
-    for (int n = 0; n < NG; ++n) {
-      const int gate = n / U, u = u0 + (n % U);
-      bias[n] = (u < H) ? a.b_ih[gate * H + u] + a.b_hh[gate * H + u] : 0.f;
-    }
-    float c[U];
+    for (int gate = 0; gate < 4; ++gate)
 #pragma unroll
-    for (int i = 0; i < U; ++i) c[i] = 0.f;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
+      for (int e = 0; e < 2; ++e) {
+        const int u = u0 + ul0 + e;
+        bias[gate][e] = (u < H) ? a.b_ih[gate * H + u] + a.b_hh[gate * H + u] : 0.f;
+      }
+    float c[4][2];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) c[i][0] = c[i][1] = 0.f;
     const int nu = (H - u0 < U) ? (H - u0) : U;  // real units of this CTA
+    const bool u_ok0 = ul0 < nu, u_ok1 = ul0 + 1 < nu;
+    uint32_t it = 0;
+    const uint32_t wbase = smem_u32(wsm), rbase = smem_u32(ring);
     for (int p = 0; p < T; ++p) {
-      float pre[NG];
-      if (valid) {  // input projection of this step (issued before the wait below: the latency hides behind the MMAs)
-        const float* pp = a.P + (size_t)r * a.p_row + (size_t)p * a.p_t + u0;
-        if (vec_ok && nu == U) {
+      float pre[4][4][2];  // [row slot][gate][unit]
 #pragma unroll
-          for (int gate = 0; gate < 4; ++gate) {
-            const float4 v0 = __ldg(reinterpret_cast<const float4*>(pp + (size_t)gate * H));
-            const float4 v1 = __ldg(reinterpret_cast<const float4*>(pp + (size_t)gate * H + 4));
-            pre[gate * U + 0] = v0.x; pre[gate * U + 1] = v0.y; pre[gate * U + 2] = v0.z; pre[gate * U + 3] = v0.w;
-            pre[gate * U + 4] = v1.x; pre[gate * U + 5] = v1.y; pre[gate * U + 6] = v1.z; pre[gate * U + 7] = v1.w;
+      for (int rs = 0; rs < 4; ++rs) {  // input projection of this step (loads in flight under the MMAs)
+        const int r = g * MR + 64 * (rs >> 1) + 16 * q + (lane >> 2) + 8 * (rs & 1);
+        const bool valid = r < a.R;
+        const float* pp = a.P + (size_t)r * a.p_row + (size_t)p * a.p_t + u0 + ul0;
+#pragma unroll
+        for (int gate = 0; gate < 4; ++gate) {
+          if (valid && vec_ok && u_ok1) {
+            const float2 v = __ldg(reinterpret_cast<const float2*>(pp + (size_t)gate * H));
+            pre[rs][gate][0] = v.x; pre[rs][gate][1] = v.y;
+          } else {
+            pre[rs][gate][0] = (valid && u_ok0) ? __ldg(pp + (size_t)gate * H) : 0.f;
+            pre[rs][gate][1] = (valid && u_ok1) ? __ldg(pp + (size_t)gate * H + 1) : 0.f;
           }
-        } else {
-#pragma unroll
-          for (int n = 0; n < NG; ++n) pre[n] = ((n % U) < nu) ? __ldg(pp + (size_t)(n / U) * H + (n % U)) : 0.f;
         }
-      } else {
-#pragma unroll
-        for (int n = 0; n < NG; ++n) pre[n] = 0.f;
       }
       if (p > 0) {
-        mbar_wait<true>(&bars.acc_full, (p - 1) & 1);
-        tc_fence_after();
+        float acc[2][NACC];
+        float accl[2][NG / 2];
 #pragma unroll
-        for (int cb = 0; cb < NG; cb += 8) {
-          float d[8];
-          tc_ld8(taddr + cb, d);
-          tc_wait_ld();
+        for (int hf = 0; hf < 2; ++hf) {
 #pragma unroll
-          for (int e = 0; e < 8; ++e) pre[cb + e] += d[e];
-          if (X3) {
-            tc_ld8(taddr + NG + cb, d);
-            tc_wait_ld();
+          for (int i = 0; i < NACC; ++i) acc[hf][i] = 0.f;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) pre[cb + e] += d[e];
-          }
+          for (int i = 0; i < NG / 2; ++i) accl[hf][i] = 0.f;
+          wg::fence_operand(acc[hf]);
+          wg::fence_operand(accl[hf]);
         }
-        tc_fence_before();
-      }
-      mbar_arrive(&bars.acc_empty);
-      float h[U];
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const uint32_t s = it % (uint32_t)a.stages, use = it / (uint32_t)a.stages;
+          mbar_wait_mma(&bars.full[s], use & 1);
+          wg::fence();
+          const uint32_t sa = rbase + s * STAGE_BYTES;
+          const uint64_t wd = wg::desc_sw128(wbase + (uint32_t)kb * WB_BYTES);
 #pragma unroll
-      for (int i = 0; i < U; ++i) {
-        const float gi = pre[0 * U + i] + bias[0 * U + i], gf = pre[1 * U + i] + bias[1 * U + i];
-        const float gg = pre[2 * U + i] + bias[2 * U + i], go = pre[3 * U + i] + bias[3 * U + i];
-        const float cn = act_sigmoid<X3>(gf) * c[i] + act_sigmoid<X3>(gi) * act_tanh<X3>(gg);
-        c[i] = cn;
-        h[i] = act_sigmoid<X3>(go) * act_tanh<X3>(cn);
-      }
-      if (valid) {
-        float* hp = a.hall + (size_t)r * a.h_row + (size_t)p * a.h_t + u0;
-        if (vec_ok && nu == U) {
-          *reinterpret_cast<float4*>(hp) = make_float4(h[0], h[1], h[2], h[3]);
-          *reinterpret_cast<float4*>(hp + 4) = make_float4(h[4], h[5], h[6], h[7]);
-        } else {
+          for (int hf = 0; hf < 2; ++hf) {
+            const uint64_t ad = wg::desc_sw128(sa + hf * (64 * 128));
 #pragma unroll
-          for (int i = 0; i < U; ++i) if (i < nu) hp[i] = h[i];
-        }
-        if (p + 1 < T) {  // publish h_p for the next step: fp16 hi (and lo), 16 bytes each
-          __half hi[U], lo[U];
-#pragma unroll
-          for (int i = 0; i < U; ++i) {
-            const float v = (i < nu) ? h[i] : 0.f;
-            hi[i] = __float2half_rn(v);
-            lo[i] = __float2half_rn(v - __half2float(hi[i]));
+            for (int k = 0; k < KB / 16; ++k) {
+              if constexpr (X3) {
+                wg::mma_f16_n64(acc[hf], ad + (uint64_t)(2 * k), wd + (uint64_t)(2 * k), 1u);
+                wg::mma_f16_n32(accl[hf], ad + (uint64_t)((A_TILE >> 4) + 2 * k), wd + (uint64_t)(2 * k), 1u);
+              } else {
+                wg::mma_f16_n32(acc[hf], ad + (uint64_t)(2 * k), wd + (uint64_t)(2 * k), 1u);
+              }
+            }
           }
-          __half* sp = a.state + ((size_t)((p & 1) * PARTS) * a.Rpad + r) * a.Kp + u0;
-          *reinterpret_cast<uint4*>(sp) = *reinterpret_cast<const uint4*>(hi);
-          if (X3) *reinterpret_cast<uint4*>(sp + (size_t)a.Rpad * a.Kp) = *reinterpret_cast<const uint4*>(lo);
+          wg::commit();
+          wg::wait<0>();
+          if (lane == 0) mbar_arrive(&bars.empty[s]);
+        }
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          wg::fence_operand(acc[hf]);
+          wg::fence_operand(accl[hf]);
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+            for (int gate = 0; gate < 4; ++gate)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                float v = acc[hf][4 * gate + 2 * hh + e];
+                if (X3) v += acc[hf][4 * (gate + 4) + 2 * hh + e] + accl[hf][4 * gate + 2 * hh + e];
+                pre[2 * hf + hh][gate][e] += v;
+              }
+        }
+      }
+#pragma unroll
+      for (int rs = 0; rs < 4; ++rs) {
+        const int r = g * MR + 64 * (rs >> 1) + 16 * q + (lane >> 2) + 8 * (rs & 1);
+        float h[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float gi = pre[rs][0][e] + bias[0][e], gf = pre[rs][1][e] + bias[1][e];
+          const float gg = pre[rs][2][e] + bias[2][e], go = pre[rs][3][e] + bias[3][e];
+          const float cn = act_sigmoid<X3>(gf) * c[rs][e] + act_sigmoid<X3>(gi) * act_tanh<X3>(gg);
+          c[rs][e] = cn;
+          h[e] = act_sigmoid<X3>(go) * act_tanh<X3>(cn);
+        }
+        if (r < a.R) {
+          float* hp = a.hall + (size_t)r * a.h_row + (size_t)p * a.h_t + u0 + ul0;
+          if (vec_ok && u_ok1) {
+            *reinterpret_cast<float2*>(hp) = make_float2(h[0], h[1]);
+          } else {
+            if (u_ok0) hp[0] = h[0];
+            if (u_ok1) hp[1] = h[1];
+          }
+          if (p + 1 < T) {  // publish h_p for the next step: fp16 hi (and lo)
+            const float v0 = u_ok0 ? h[0] : 0.f, v1 = u_ok1 ? h[1] : 0.f;
+            const __half2 hi = __floats2half2_rn(v0, v1);
+            const __half2 lo = __floats2half2_rn(v0 - __low2float(hi), v1 - __high2float(hi));
+            __half* sp = a.state + ((size_t)((p & 1) * PARTS) * a.Rpad + r) * a.Kp + u0 + ul0;
+            *reinterpret_cast<__half2*>(sp) = hi;
+            if (X3) *reinterpret_cast<__half2*>(sp + (size_t)a.Rpad * a.Kp) = lo;
+          }
         }
       }
       if (p + 1 < T) {
@@ -280,14 +264,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
         }
       }
     }
-  }
-
-  // ---------------- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 64;" ::"r"(tmem_base));
   }
 }
 
@@ -364,7 +340,7 @@ static size_t smem_bytes(int Kp, bool x3, int stages) {
 }  // namespace rec
 
 static int rec_sm_count() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;
@@ -380,7 +356,7 @@ bool lstm_rec_tc_supported(int H, bool x3) {
   cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   const int Kp = (H + rec::KB - 1) / rec::KB * rec::KB;
-  return coop == 1 && major == 10 && cdiv(H, rec::U) <= rec_sm_count() && rec::smem_bytes(Kp, x3, 2) <= (size_t)max_smem;
+  return coop == 1 && major == 9 && cdiv(H, rec::U) <= rec_sm_count() && rec::smem_bytes(Kp, x3, 2) <= (size_t)max_smem;
 }
 
 // rows one launch covers (groups of 128 that fit on the chip next to each other)
@@ -461,7 +437,7 @@ int split_tf32_launch(const float* in, size_t rows, int K, size_t ldi, const flo
   if (rows == 0) return FSN_OK;
   const size_t n = rows * (size_t)Kp;
   size_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > rec_sm_count() * 16) blocks = (size_t)rec_sm_count() * 16;
   rec::split_tf32_kernel<<<(int)blocks, 256, 0, st>>>(in, rows, K, ldi, row_scale, rows_per_scale < 1 ? 1 : rows_per_scale,
                                                       scale_B, out, Kp, cat);
   FSN_CHECK_LAUNCH("split_tf32_kernel");
@@ -472,7 +448,7 @@ int bias_act_launch(float* x, size_t rows, int N, size_t ld, const float* bias, 
   if (rows == 0) return FSN_OK;
   const size_t n = rows * (size_t)N;
   size_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > rec_sm_count() * 16) blocks = (size_t)rec_sm_count() * 16;
   rec::bias_act_kernel<<<(int)blocks, 256, 0, st>>>(x, rows, N, ld, bias, act);
   FSN_CHECK_LAUNCH("bias_act_kernel");
   return FSN_OK;

@@ -134,7 +134,7 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
 }
 
 // Full-band stack on the tensor cores (model.py:92-95; sequence_model.py:106-125): per layer the input projection of
-// all steps as one tf32 GEMM (three passes on hi/lo splits when x3) and the recurrence in the persistent tcgen05
+// all steps as one tf32 GEMM (three passes on hi/lo splits when x3) and the recurrence in the persistent wgmma
 // kernel; Linear(Hf -> F) + activation as the same GEMM + a bias/activation pass.  x3 keeps the fp32 error class.
 static int fb_tc_forward(const fsn_model_desc* d, const fsn_seq_weights* fb, const Dims& m, const ModelWs& w, cudaStream_t st) {
   const int F = m.F, Tp = m.Tp, B = m.B, Hf = d->fb_hidden;
@@ -221,9 +221,8 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
     memset(&a, 0, sizeof(a));
     a.packed = sb_packed; a.magT = w.magT; a.fbT = w.fbT; a.inv2 = w.inv2; a.crm = crm;
     a.B = B; a.F = F; a.Tp = Tp; a.la = d->look_ahead; a.Ns = d->sb_num_neighbors; a.Nf = d->fb_num_neighbors;
-    a.H = Hs; a.act = d->sb_activation; a.map = map; a.pair = sb_tc2_supported(d); a.x3 = d->precision == FSN_PREC_F16X3_TC;
+    a.H = Hs; a.act = d->sb_activation; a.map = map; a.x3 = d->precision == FSN_PREC_F16X3_TC;
     a.unit_scale = cum ? w.cum2 : nullptr;
-    a.quad = sb_tc4_supported(d);
     rc = sb_tc_forward(a, st);
     prof_mark(3, st);
     return rc;
@@ -321,7 +320,7 @@ extern "C" int fsn_model_forward(const fsn_model_desc* d, const fsn_seq_weights*
   int rc = make_dims(d, B, T, m);
   if (rc) return rc;
   FSN_REQUIRE(d->precision == FSN_PREC_FP32 || sb_tc_supported(d), FSN_ERR_UNSUPPORTED,
-              "FSN_PREC_F16_TC needs sb_hidden %% 128 == 0 (FSN_PREC_F16X3_TC: sb_hidden = 384) and sub-band input width <= 32");
+              "FSN_PREC_F16_TC / FSN_PREC_F16X3_TC need sb_hidden in {128,256,384} and sub-band input width <= 32");
   ModelWs w;
   carve_model(d, m, workspace, w);
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
@@ -385,7 +384,7 @@ static int enhance_impl(const fsn_model_desc* d, const fsn_seq_weights* fb, cons
   int rc = carve_enhance(&dd, B, L, n_fft, hop, workspace, e, m);
   if (rc) return rc;
   FSN_REQUIRE(dd.precision == FSN_PREC_FP32 || sb_tc_supported(&dd), FSN_ERR_UNSUPPORTED,
-              "FSN_PREC_F16_TC needs sb_hidden %% 128 == 0 (FSN_PREC_F16X3_TC: sb_hidden = 384) and sub-band input width <= 32");
+              "FSN_PREC_F16_TC / FSN_PREC_F16X3_TC need sb_hidden in {128,256,384} and sub-band input width <= 32");
   FSN_REQUIRE(workspace && workspace_bytes >= e.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, e.bytes);
   ModelWs w;

@@ -1,210 +1,72 @@
-// Sub-band LSTM stack on the 5th-gen tensor cores (tcgen05 + TMEM), sm_100a only.
+// Sub-band LSTM stack on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Reference semantics: recipes/dns_interspeech_2020/fullsubnet/model.py:98-135 (unfold, concat,
 // norm, drop_band, 2xLSTM(H) + Linear(H->2), re-layout, look-ahead slice) with
 // audio_zen/model/module/sequence_model.py:106-125 and audio_zen/model/base_model.py:13-46.
+// The same stack shape is the fast_fullsubnet bottleneck (fsn_fast_model.cu): there the gather also down-samples
+// time (`shrink`) and the Linear layer has one output (the packer zero-pads the second).
 //
 // Formulation ("weights as the M operand").  A CTA owns NB sub-band units (rows of the
 // [B*F', .] batch) for all T' steps and both layers.  Per step and layer it needs
 //     gates^T [4H, NB] = W [4H, K] . S^T [K, NB],      S = [x_t | h_{t-1}]  (layer 0)
 //                                                      S = [h0_t | h1_{t-1}] (layer 1)
-// which runs as tcgen05.mma kind::f16 with M = 128 gate rows (one gate type of 128 hidden
-// units), N = NB, K = 16 per instruction:
-//   * A operand  = 16 KB fp16 weight tiles [128 x 64], pre-swizzled (128B) by the packer and
-//                  streamed from L2 with cp.async.bulk (TMA engine) through a ring of stages;
-//   * B operand  = the recurrent state S, fp16, resident in shared memory in the same K-major
-//                  128B-swizzled layout, written in place by the epilogue (h) and the gather warp (x);
-//   * D          = fp32 accumulators in TMEM: lane = hidden unit, column = unit-in-CTA, one
-//                  128-column buffer (4 gates x NB) per 128-unit slice m.
-// The epilogue thread that owns hidden unit u (TMEM lane) keeps that unit's cell state c for
-// all NB rows and both layers in registers, applies the gate non-linearities in fp32 and
-// writes h (fp16) straight back into the B-operand layout.  Layer 1 runs one step behind
-// layer 0 in the MMA issue order so that every epilogue overlaps the other layer's MMAs.
+// which runs as wgmma m64nNBk16 (fp16 operands, fp32 accumulate), two m64 halves per gate of a
+// 128-unit slice m:
+//   * A operand  = 32 KB fp16 weight stages [4 gates x 128 x 32 k], pre-swizzled (64B) by the packer and
+//                  streamed from L2 with cp.async.bulk (TMA engine) through a ring; a cluster of CL CTAs
+//                  consumes the same stream, each loads 1/CL of a stage and multicasts it to all;
+//   * B operand  = the recurrent state S, fp16, resident in shared memory (K-major, 128B-swizzled),
+//                  written in place by the consumers (h) and the gather warp (x);
+//   * D          = fp32 accumulators in the registers of consumer warpgroup m, which owns hidden units
+//                  [128m, 128m+128): it issues the MMAs of its slice, keeps that slice's cell state c for all NB
+//                  rows and both layers in registers, applies the gate non-linearities in fp32 and writes h (fp16)
+//                  straight back into the B-operand layout.  While one warpgroup runs its cell, the next one's
+//                  MMAs consume the weight stream.
+// X3 (FSN_PREC_F16X3_TC) is the ERROR-COMPENSATED variant: weights and state are each split into two fp16 terms
+// (hi = rn(v), lo = rn(v - hi)) and every product is issued as W_hi.S_hi + W_hi.S_lo + W_lo.S_hi into the same fp32
+// accumulator (the dropped W_lo.S_lo term is 2^-22 relative); the stream carries a hi and a lo stage per k range and
+// the gate non-linearities use expf / IEEE division.
 // Nothing but the NB x 2 mask values per step ever leaves the SM.
 //
-// Warp roles (512 threads): 0 = weight-tile producer, 1 = MMA issuer, 2 = x_t gather
-// (+ TMEM alloc), 3 = Linear(H->2) + output staging, 4..15 = epilogue (3 warpgroups, one per
-// 128-unit slice m).
+// Warp roles (128 + 128 MT threads): 0 = weight-stage producer, 1 = idle, 2 = x_t gather, 3 = Linear(H->2) + output
+// staging, 4.. = consumer warpgroups (one per 128-unit slice m).
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include "fsn_internal.cuh"
+#include "fsn_tc_ptx.cuh"
+#include "fsn_wgmma.cuh"
 
 namespace fsn {
 namespace tc {
 
-constexpr int NB = 32;                 // sub-band units per CTA (MMA N)
+using namespace ptx;
+
+constexpr int NB = 16;                 // sub-band units per CTA (MMA N)
 constexpr int KB = 64;                 // fp16 elements per 128-byte swizzle row
 constexpr int KS = 32;                 // k elements per weight stage
 constexpr int W_SUB = 128 * KS * 2;    // 8192 B: [128 gate rows x 32 k] of one gate, 64B-swizzled
-constexpr int W_TILE = 4 * W_SUB;      // 32768 B: one ring stage = the 4 gates (i,f,g,o) of one (slice m, k range)
-constexpr int S_KBLK = NB * KB * 2;    // 4096 B: one k-block of the state operand
-constexpr int MAX_STAGES = 4;        // weight ring depth is a launch parameter (default 3)
+constexpr int W_TILE = 4 * W_SUB;      // 32768 B: one ring stage = the 4 gates (i,f,g,o) of one (slice m, k range, part)
+constexpr int S_KBLK = NB * KB * 2;    // 2048 B: one k-block of the state operand
+constexpr int MAX_STAGES = 4;          // weight ring depth (FSN_TC_STAGES, default 4)
 constexpr int MAX_MT = 3;
 constexpr int OUT_T = 8;               // output frames staged before a store
 constexpr int NTHREADS = 128 + 128 * MAX_MT;
 
-// ---------------------------------------------------------------- PTX helpers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {  // non-blocking probe
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// spin with a watchdog: a protocol bug traps (launch error) instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 27)) {
-      printf("fsn sb_tc: mbarrier timeout (block %d thread %d bar %p parity %u)\n", blockIdx.x, threadIdx.x,
-             (void*)bar, parity);
-      __trap();
-    }
-  }
-}
-// same, for warps that are off the critical issue path: back off between probes so the spinning does not
-// steal issue slots from the MMA-issuing warp that shares the SM sub-partition
-__device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(64);
-    if (++spins > (1u << 24)) {
-      printf("fsn sb_tc: mbarrier timeout (block %d thread %d bar %p parity %u)\n", blockIdx.x, threadIdx.x,
-             (void*)bar, parity);
-      __trap();
-    }
-  }
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void bulk_g2s_mc(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
-          smem_u32(dst)),
-      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// one lane of a converged warp (the tcgen05 / TMA issue idiom: the warp stays converged so that the
-// operands live in uniform registers, only the issuing instruction is predicated)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128B-swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-// start>>4 | LBO(=1) <<16 | SBO(=1024 B >>4) <<32 | version 1 <<46 | SWIZZLE_128B (2) <<61
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// same for the 64B-swizzled weight sub-tiles (rows of 64 B, 8-row groups 512 B apart): SWIZZLE_64B = 4
-__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (32ull << 32) | (1ull << 46) | (4ull << 61);
-}
-// byte offset of element (row, k<32) inside a [128 x 32] K-major 64B-swizzled sub-tile (Swizzle<2,4,3>)
-__host__ __device__ __forceinline__ int swz64_off(int row, int k) {
-  return (row >> 3) * 512 + (row & 7) * 64 + ((((k >> 3) ^ ((row >> 1) & 3)) & 3) << 4) + (k & 7) * 2;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=f16, both K-major, M=128, N=NB
-constexpr uint32_t kIdesc = (1u << 4) | ((uint32_t)(NB >> 3) << 17) | ((128u >> 4) << 24);
-
-// byte offset of element (row, k) inside a K-major 128B-swizzled k-block whose rows are 128 B
-__host__ __device__ __forceinline__ int swz_off(int row, int k) {
-  return (row >> 3) * 1024 + (row & 7) * 128 + ((((k >> 3) ^ (row & 7)) & 7) << 4) + (k & 7) * 2;
-}
-
-__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-__device__ __forceinline__ float fast_tanh(float x) { return 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * x)); }
-
 struct PackedLayout {
-  int H, MT, nkb0, nkb1, kx16;
-  size_t tiles0, tiles1;  // per layer
+  int H, MT, nkb0, nkb1, parts;
+  size_t tiles0, tiles1;  // stages per step, per layer
   size_t off_bias, off_fcw, off_fcb, bytes;
 };
 
-__host__ __device__ inline PackedLayout packed_layout(int H, int Ksb) {
+__host__ __device__ inline PackedLayout packed_layout(int H, bool x3) {
   PackedLayout L;
   L.H = H; L.MT = H / 128;
-  L.nkb0 = 1 + H / KS; L.nkb1 = 2 * H / KS;  // stages (k ranges of 32) per slice m
-  L.kx16 = (Ksb + 15) / 16;
-  L.tiles0 = (size_t)L.MT * L.nkb0;          // stages per step, layer 0 / layer 1
-  L.tiles1 = (size_t)L.MT * L.nkb1;
+  L.nkb0 = 1 + H / KS; L.nkb1 = 2 * H / KS;  // k ranges of 32 per slice m
+  L.parts = x3 ? 2 : 1;
+  L.tiles0 = (size_t)L.MT * L.nkb0 * L.parts;
+  L.tiles1 = (size_t)L.MT * L.nkb1 * L.parts;
   L.off_bias = (L.tiles0 + L.tiles1) * W_TILE;
   L.off_fcw = L.off_bias + (size_t)2 * 4 * H * sizeof(float);
   L.off_fcb = L.off_fcw + (size_t)2 * H * sizeof(float);
@@ -213,14 +75,14 @@ __host__ __device__ inline PackedLayout packed_layout(int H, int Ksb) {
 }
 
 // ---------------------------------------------------------------- weight packer
-// stage order = consumption order: layer, m (128-unit slice), k range of 32; 4 gate sub-tiles per stage
+// stage order = consumption order: layer, m (128-unit slice), k range of 32, part (hi, lo); 4 gate sub-tiles per stage
 __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restrict__ whh0,
                             const float* __restrict__ wih1, const float* __restrict__ whh1,
                             const float* __restrict__ bih0, const float* __restrict__ bhh0,
                             const float* __restrict__ bih1, const float* __restrict__ bhh1,
-                            const float* __restrict__ fcw, const float* __restrict__ fcb, int H, int Ksb,
-                            uint8_t* __restrict__ out) {
-  const PackedLayout L = packed_layout(H, Ksb);
+                            const float* __restrict__ fcw, const float* __restrict__ fcb, int H, int Ksb, int x3,
+                            int fc_out, uint8_t* __restrict__ out) {
+  const PackedLayout L = packed_layout(H, x3 != 0);
   const size_t nstages = L.tiles0 + L.tiles1;
   const size_t total = nstages * 4 * 128 * 4;  // one thread per (stage, gate, row, 16-byte chunk)
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -231,6 +93,8 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
     size_t st = st_abs;
     const int layer = st >= L.tiles0;
     if (layer) st -= L.tiles0;
+    const int part = (int)(st % L.parts);
+    st /= L.parts;
     const int nkb = layer ? L.nkb1 : L.nkb0;
     const int kb = (int)(st % nkb);
     const int m = (int)(st / nkb);
@@ -247,12 +111,13 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
         const int k = kb * KS + kk;
         w = (k < H) ? wih1[(size_t)wrow * H + k] : whh1[(size_t)wrow * H + (k - H)];
       }
-      v[e] = __float2half_rn(w);
+      const __half hi = __float2half_rn(w);
+      v[e] = part ? __float2half_rn(w - __half2float(hi)) : hi;
     }
     uint8_t* dst = out + st_abs * W_TILE + g * W_SUB + swz64_off(r, c * 8);
     *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(v);
   }
-  // biases (b_ih + b_hh, fp32) and the Linear layer
+  // biases (b_ih + b_hh, fp32) and the Linear layer (outputs beyond fc_out are zero)
   float* bias = reinterpret_cast<float*>(out + L.off_bias);
   float* pfcw = reinterpret_cast<float*>(out + L.off_fcw);
   float* pfcb = reinterpret_cast<float*>(out + L.off_fcb);
@@ -260,15 +125,16 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
     bias[i] = bih0[i] + bhh0[i];
     bias[4 * H + i] = bih1[i] + bhh1[i];
   }
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * H; i += gridDim.x * blockDim.x) pfcw[i] = fcw[i];
-  if (blockIdx.x == 0 && threadIdx.x < 2) pfcb[threadIdx.x] = fcb[threadIdx.x];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * H; i += gridDim.x * blockDim.x)
+    pfcw[i] = (i < fc_out * H) ? fcw[i] : 0.f;
+  if (blockIdx.x == 0 && threadIdx.x < 2) pfcb[threadIdx.x] = ((int)threadIdx.x < fc_out) ? fcb[threadIdx.x] : 0.f;
 }
 
 // ---------------------------------------------------------------- shared-memory plan
 struct Smem {
-  uint32_t w, x, h0, h1, fcw, outst, rows, bars, total;
+  uint32_t w, x, h0, h1, lo, fcw, outst, rows, bars, total;
 };
-__host__ __device__ inline Smem smem_plan(int H, int stages) {
+__host__ __device__ inline Smem smem_plan(int H, int stages, bool x3) {
   Smem s;
   const int nkh = H / KB;
   uint32_t o = 0;
@@ -276,7 +142,8 @@ __host__ __device__ inline Smem smem_plan(int H, int stages) {
   s.x = o; o += 2 * S_KBLK;
   s.h0 = o; o += 2 * nkh * S_KBLK;
   s.h1 = o; o += nkh * S_KBLK;  // single buffer: h1_t overwrites h1_{t-1} once every layer-1 MMA of step t is done
-  s.fcw = o; o += 4 * MAX_MT * 2 * NB * 4;  // Linear partial sums [epilogue warp][o][row]
+  s.lo = o; o += x3 ? (o - s.x) : 0;  // X3: lo copies of x, h0, h1 at offset (lo - x) from the hi copies
+  s.fcw = o; o += 4 * MAX_MT * 2 * NB * 4;  // Linear partial sums [consumer warp][o][row]
   s.outst = o; o += NB * 2 * OUT_T * 4;
   s.rows = o; o += NB * 16;
   s.bars = o; o += 256;
@@ -287,10 +154,11 @@ __host__ __device__ inline Smem smem_plan(int H, int stages) {
 struct Bars {
   uint64_t w_full[MAX_STAGES], w_empty[MAX_STAGES];
   uint64_t x_full[2], x_empty[2];
-  uint64_t acc_full[MAX_MT], acc_empty[MAX_MT];
   uint64_t h0_ready, h1_ready, fc_done;
   uint64_t l1_done;   // all layer-1 MMAs of a step have completed (h1 may be overwritten)
-  uint32_t tmem_base;
+  // turn[m]: warpgroup m may wait on the weight ring - its predecessor in the stream has seen all of its own
+  // stages land.  The ring's parity waits are only sound one phase ahead, so the warpgroups take the ring in turn
+  uint64_t turn[MAX_MT];
 };
 static_assert(sizeof(Bars) <= 256, "barrier block too large");
 
@@ -300,18 +168,13 @@ struct RowInfo {
   int out_idx;        // crm index of (b', o=0, f', t=0) divided by T  (= (b'*2)*Fsub + f')
 };
 
-// debug event trace: rec = (event id << 48) | (it << 32 ... ) kept simple: [slot] = clock, ids fixed per slot
-__device__ __forceinline__ void trace_ev(long long* tr, int it, int ev) {
-  if (tr && blockIdx.x == 0 && it >= 8 && it < 16) tr[(it - 8) * 32 + ev] = clock64();
-}
-
 struct KArgs {
   const uint8_t* packed;
   const float* magT; const float* fbT; const float* inv2;
   const float* unit_scale;  // nullable: cumulative norm, scale of (step t, row r) at [t*R + r] instead of inv2[clip]
   float* crm;
   int R, F, Tp, la, T, Ns, Nf, H, Ksb, act, Fsub, stages, cluster;
-  long long* trace;  // debug: clock64 event trace of CTA 0 (FSN_TC_TRACE), else nullptr
+  int src_T, shrink;  // frames in magT/fbT; x_t = mean of `shrink` source frames (fast_fullsubnet down-sampling), 1 = none
   RowMap map;
 };
 
@@ -323,8 +186,14 @@ __device__ __forceinline__ float act_apply(float v, int act) {
     default: return v;
   }
 }
+// MUFU-class forms for the single-pass variant, whose fp16 products are 1e-3 class anyway; expf + IEEE division
+// for the compensated one, whose whole point is the fp32 error class
+template <bool X3> __device__ __forceinline__ float sg(float x) { return X3 ? 1.0f / (1.0f + expf(-x)) : fast_sigmoid(x); }
+template <bool X3> __device__ __forceinline__ float th(float x) { return X3 ? 1.0f - 2.0f / (1.0f + expf(2.0f * x)) : fast_tanh(x); }
 
+template <bool X3>
 __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) {
+  constexpr int PARTS = X3 ? 2 : 1;
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzle atoms need 1024-byte alignment in the shared window
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -332,13 +201,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
   const int MT = H / 128;
   const int nkh = H / KB;
   const int STAGES = a.stages;
-  // CL CTAs of a cluster consume the same weight stream in lock step: each loads 1/CL of every tile and
-  // multicasts it to all of them, so one L2 read feeds CL SMs
   const int CL = a.cluster;
   const uint16_t cl_mask = (uint16_t)((1u << CL) - 1u);
   const uint32_t cl_rank = (CL > 1) ? cluster_ctarank() : 0u;
-  const Smem sp = smem_plan(H, STAGES);
-  const PackedLayout PL = packed_layout(H, a.Ksb);
+  const Smem sp = smem_plan(H, STAGES, X3);
+  const uint32_t LO = sp.lo - sp.x;  // byte offset of a lo copy from its hi copy
+  const PackedLayout PL = packed_layout(H, X3);
   Bars& bars = *reinterpret_cast<Bars*>(smem + sp.bars);
   RowInfo* rows = reinterpret_cast<RowInfo*>(smem + sp.rows);
   float* fc_part = reinterpret_cast<float*>(smem + sp.fcw);
@@ -349,18 +217,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
 
   // ---------------- one-time setup
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.w_full[s], 1); mbar_init(&bars.w_empty[s], CL); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&bars.x_full[i], 1); mbar_init(&bars.x_empty[i], 1); }
-    for (int m = 0; m < MAX_MT; ++m) { mbar_init(&bars.acc_full[m], 1); mbar_init(&bars.acc_empty[m], 4); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.w_full[s], 1); mbar_init(&bars.w_empty[s], 4 * CL); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&bars.x_full[i], 1); mbar_init(&bars.x_empty[i], 4 * MT); }
     mbar_init(&bars.h0_ready, 4 * MT);
     mbar_init(&bars.h1_ready, 4 * MT);
     mbar_init(&bars.fc_done, 1);
-    mbar_init(&bars.l1_done, 1);
+    mbar_init(&bars.l1_done, 4 * MT);
+    for (int m = 0; m < MAX_MT; ++m) mbar_init(&bars.turn[m], 4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) {  // TMEM: 512 columns (3 accumulator buffers of 4*NB columns are used)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&bars.tmem_base)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   if (threadIdx.x < NB) {
     RowInfo ri;
@@ -379,177 +243,96 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
     const int n16 = (sp.fcw - sp.x) / 16;
     for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
   }
-  fence_async_smem();
-  tc_fence_before();
+  fence_proxy_async();
   __syncthreads();
   if (CL > 1) cluster_sync_all();  // peers' barriers are initialised before any multicast reaches them
-  tc_fence_after();
-  const uint32_t tmem_base = bars.tmem_base;
 
   if (warp < 4) {
-    // warpgroup 0 (producer / MMA / gather / Linear) needs few registers: hand the rest to the epilogue
+    // warpgroup 0 (producer / gather / Linear) needs few registers: hand the rest to the consumers
     asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
   if (warp == 0) {
-    // ================= weight-tile producer: the same (layer 0, layer 1) tile stream every step
-    {
-      uint32_t stage = 0, phase = 0;
-      for (int it = 0; it <= Tp; ++it) {
-        const size_t t_begin = (it < Tp) ? 0 : PL.tiles0;
-        const size_t t_end = (it >= 1) ? PL.tiles0 + PL.tiles1 : PL.tiles0;
-        const uint8_t* src = a.packed + t_begin * W_TILE;
-        for (size_t tile = t_begin; tile < t_end; ++tile, src += W_TILE) {
-          mbar_wait_relaxed(&bars.w_empty[stage], phase ^ 1);  // all CL consumers have drained this stage
-          if (elect_one()) {
-            mbar_expect_tx(&bars.w_full[stage], W_TILE);
-            if (CL == 1) {
-              bulk_g2s(smem + sp.w + stage * W_TILE, src, W_TILE, &bars.w_full[stage]);
-            } else {
-              const uint32_t slice = W_TILE / CL, off = cl_rank * slice;
-              bulk_g2s_mc(smem + sp.w + stage * W_TILE + off, src + off, slice, &bars.w_full[stage], cl_mask);
-            }
-          }
-          __syncwarp();
-          if (++stage == (uint32_t)STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer (converged warp, one elected lane issues).  Order per iteration:
-    // layer0(step it), layer1(step it-1)
-    {
-      uint32_t stage = 0, phase = 0;
-      bool w_ready = false;
-      const uint64_t adesc0 = make_desc_sw64(smem_u32(smem + sp.w));
-      uint32_t jobs[MAX_MT] = {0, 0, 0};
-      // every mbarrier phase is waited on exactly once, in order (a parity wait on a phase that is two
-      // behind the barrier would block on the wrong phase), so count the phases already observed
-      int h0_seen = 0, h1_seen = 0;
-      for (int it = 0; it <= Tp; ++it) {
-        for (int layer = 0; layer < 2; ++layer) {
-          const int t = it - layer;
-          if (t < 0 || t >= Tp) continue;
-          // operands of this step must be complete in shared memory
-          if (layer == 0) {
-            mbar_wait(&bars.x_full[t & 1], (t >> 1) & 1);
-            for (; h0_seen < t; ++h0_seen) mbar_wait(&bars.h0_ready, h0_seen & 1);      // h0_{t-1}
+    // ================= weight-stage producer: the same (layer 0, layer 1) stream every step
+    uint32_t stage = 0, phase = 0;
+    for (int it = 0; it <= Tp; ++it) {
+      const size_t t_begin = (it < Tp) ? 0 : PL.tiles0;
+      const size_t t_end = (it >= 1) ? PL.tiles0 + PL.tiles1 : PL.tiles0;
+      const uint8_t* src = a.packed + t_begin * W_TILE;
+      for (size_t tile = t_begin; tile < t_end; ++tile, src += W_TILE) {
+        mbar_wait<true>(&bars.w_empty[stage], phase ^ 1);  // all CL CTAs' consumers have drained this stage
+        if (elect_one()) {
+          mbar_expect_tx(&bars.w_full[stage], W_TILE);
+          if (CL == 1) {
+            bulk_g2s(smem + sp.w + stage * W_TILE, src, W_TILE, &bars.w_full[stage]);
           } else {
-            for (; h0_seen < t + 1; ++h0_seen) mbar_wait(&bars.h0_ready, h0_seen & 1);  // h0_t
-            for (; h1_seen < t; ++h1_seen) mbar_wait(&bars.h1_ready, h1_seen & 1);      // h1_{t-1}
+            const uint32_t slice = W_TILE / CL, off = cl_rank * slice;
+            bulk_g2s_mc(smem + sp.w + stage * W_TILE + off, src + off, slice, &bars.w_full[stage], cl_mask);
           }
-          tc_fence_after();
-          const uint32_t x_addr = smem_u32(smem + sp.x + (t & 1) * S_KBLK);
-          const uint32_t h0_cur = smem_u32(smem + sp.h0 + (t & 1) * nkh * S_KBLK);        // h0_t
-          const uint32_t h0_prev = smem_u32(smem + sp.h0 + ((t + 1) & 1) * nkh * S_KBLK);  // h0_{t-1}
-          const uint32_t h1_prev = smem_u32(smem + sp.h1);                                    // h1_{t-1}
-          // B operand (state, K-major 128B-swizzled blocks of 64 k): layer 0: [x_t (32 k)] [h0_{t-1} (H)];
-          // layer 1: [h0_t (H)] [h1_{t-1} (H)].  One weight stage covers 32 k = half a block.
-          const uint64_t bd_a = make_desc(layer ? h0_cur : x_addr);
-          const uint64_t bd_b = make_desc(layer ? h1_prev : h0_prev);
-          const int n_a = layer ? H / KS : 1;
-          const int n_b = H / KS;
-          // one stage: 2 k16 slices x 4 gates; consecutive MMAs hit different accumulators, so the
-          // accumulate dependency of each gate is 4 instructions apart
-          auto issue_stage = [&](uint32_t d0, uint64_t bd, bool first) {
-            if (!w_ready) mbar_wait(&bars.w_full[stage], phase);
-            tc_fence_after();
-            const uint64_t ad = adesc0 + (uint64_t)(stage * (W_TILE >> 4));
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 2; ++k)
-#pragma unroll
-                for (int g = 0; g < 4; ++g)
-                  tc_mma_f16(d0 + (uint32_t)(g * NB), ad + (uint64_t)(g * (W_SUB >> 4) + 2 * k), bd + (uint64_t)(2 * k),
-                             kIdesc, (first && k == 0) ? 0u : 1u);
-              // stage free (in every CTA that fills it) once these MMAs have read it
-              if (CL == 1) tc_commit(&bars.w_empty[stage]); else tc_commit_mc(&bars.w_empty[stage], cl_mask);
-            }
-            __syncwarp();
-            if (++stage == (uint32_t)STAGES) { stage = 0; phase ^= 1; }
-            w_ready = mbar_test_wait(&bars.w_full[stage], phase);  // probe the next stage early
-          };
-          for (int m = 0; m < MT; ++m) {
-            if (lane == 0) trace_ev(a.trace, it, (layer * 3 + m) * 2);
-            mbar_wait(&bars.acc_empty[m], (jobs[m] & 1) ^ 1);
-            tc_fence_after();
-            if (lane == 0) trace_ev(a.trace, it, 24 + layer * 3 + m);
-            const uint32_t d0 = tmem_base + (uint32_t)(m * 4 * NB);
-            uint64_t bd = bd_a;
-#pragma unroll 1
-            for (int j = 0; j < n_a; ++j) {
-              issue_stage(d0, bd, j == 0);
-              bd += (j & 1) ? (uint64_t)((S_KBLK >> 4) - 4) : 4ull;  // +64 B inside a block, then next block
-            }
-            bd = bd_b;
-#pragma unroll 1
-            for (int j = 0; j < n_b; ++j) {
-              issue_stage(d0, bd, false);
-              bd += (j & 1) ? (uint64_t)((S_KBLK >> 4) - 4) : 4ull;
-            }
-            if (elect_one()) tc_commit(&bars.acc_full[m]);
-            __syncwarp();
-            if (lane == 0) trace_ev(a.trace, it, (layer * 3 + m) * 2 + 1);
-            jobs[m]++;
-          }
-          if (elect_one()) {
-            if (layer == 0) tc_commit(&bars.x_empty[t & 1]);
-            else tc_commit(&bars.l1_done);  // every layer-1 MMA of step t has read h1_{t-1}
-          }
-          __syncwarp();
         }
+        __syncwarp();
+        if (++stage == (uint32_t)STAGES) { stage = 0; phase ^= 1; }
       }
     }
   } else if (warp == 2) {
     // ================= x_t gather: sub-band unit = 2Ns+1 reflected magnitude rows + 2Nf+1 full-band rows,
-    // scaled by 1/(mu'+1e-5)  (base_model.py:35-44, model.py:98-111), fp16, B-operand layout
+    // scaled by 1/(mu'+1e-5)  (base_model.py:35-44, model.py:98-111), fp16 (X3: + lo), B-operand layout
     const int nmag = 2 * a.Ns + 1;
     for (int t = 0; t < Tp; ++t) {
-      mbar_wait_relaxed(&bars.x_empty[t & 1], ((t >> 1) & 1) ^ 1);
+      mbar_wait<true>(&bars.x_empty[t & 1], ((t >> 1) & 1) ^ 1);
       uint8_t* xb = smem + sp.x + (t & 1) * S_KBLK;
+      // source frames of step t: itself, or (fast_fullsubnet/model.py:108-129) frame 0 alone, then blocks of
+      // `shrink` frames, the last one over its own length
+      int f0 = t, f1 = t + 1;
+      if (a.shrink > 1 && t > 0) { f0 = 1 + (t - 1) * a.shrink; f1 = min(f0 + a.shrink, a.src_T); }
+      const float wmean = 1.0f / (float)(f1 - f0);
 #pragma unroll 4
       for (int n = 0; n < NB; ++n) {
         const RowInfo ri = rows[n];
-        const float scale = (a.unit_scale && ri.src_b >= 0) ? a.unit_scale[(size_t)t * a.R + row0 + n] : ri.scale;
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-          const int k = lane + 32 * kk;
-          float v = 0.f;
-          if (ri.src_b >= 0 && k < a.Ksb) {
-            const size_t base = ((size_t)ri.src_b * Tp + t) * a.F;
-            if (k < nmag) v = a.magT[base + reflect_idx(ri.src_f + k - a.Ns, a.F)];
-            else          v = a.fbT[base + reflect_idx(ri.src_f + (k - nmag) - a.Nf, a.F)];
-            v *= scale;
+        float v = 0.f;
+        if (ri.src_b >= 0 && lane < a.Ksb) {
+          const int col = (lane < nmag) ? reflect_idx(ri.src_f + lane - a.Ns, a.F)
+                                        : reflect_idx(ri.src_f + (lane - nmag) - a.Nf, a.F);
+          const float* src = (lane < nmag) ? a.magT : a.fbT;
+          if (a.shrink <= 1) {
+            v = src[((size_t)ri.src_b * a.src_T + t) * a.F + col];
+            v *= a.unit_scale ? a.unit_scale[(size_t)t * a.R + row0 + n] : ri.scale;
+          } else {
+            for (int fr = f0; fr < f1; ++fr) v += src[((size_t)ri.src_b * a.src_T + fr) * a.F + col];
+            v *= wmean * ri.scale;
           }
-          *reinterpret_cast<__half*>(xb + swz_off(n, k)) = __float2half_rn(v);
         }
+        const __half hi = __float2half_rn(v);
+        *reinterpret_cast<__half*>(xb + swz128_off(n, lane)) = hi;
+        if (X3) *reinterpret_cast<__half*>(xb + LO + swz128_off(n, lane)) = __float2half_rn(v - __half2float(hi));
       }
-      fence_async_smem();
+      fence_proxy_async();
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars.x_full[t & 1]);
     }
   } else if (warp == 3) {
-    // ================= Linear(H -> 2): sums the fp32 partial dot products of the epilogue warps, adds
+    // ================= Linear(H -> 2): sums the fp32 partial dot products of the consumer warps, adds
     // the bias, stages OUT_T frames and stores crm[b', o, f', t - la]  (model.py:129-135 fused)
     const float fcb0 = reinterpret_cast<const float*>(a.packed + PL.off_fcb)[0];
     const float fcb1 = reinterpret_cast<const float*>(a.packed + PL.off_fcb)[1];
-    const RowInfo ri = rows[lane];
+    const int ln = lane < NB ? lane : 0;
+    const RowInfo ri = rows[ln];
     int staged = 0, t_stage0 = 0;
     for (int t = 0; t < Tp; ++t) {
-      mbar_wait_relaxed(&bars.h1_ready, t & 1);
+      mbar_wait<true>(&bars.h1_ready, t & 1);
       if (t >= a.la) {
         float s0 = fcb0, s1 = fcb1;
         for (int w = 0; w < 4 * MT; ++w) {
-          s0 += fc_part[(w * 2 + 0) * NB + lane];
-          s1 += fc_part[(w * 2 + 1) * NB + lane];
+          s0 += fc_part[(w * 2 + 0) * NB + ln];
+          s1 += fc_part[(w * 2 + 1) * NB + ln];
         }
         if (staged == 0) t_stage0 = t - a.la;
-        outst[(lane * 2 + 0) * OUT_T + staged] = act_apply(s0, a.act);
-        outst[(lane * 2 + 1) * OUT_T + staged] = act_apply(s1, a.act);
+        outst[(ln * 2 + 0) * OUT_T + staged] = act_apply(s0, a.act);
+        outst[(ln * 2 + 1) * OUT_T + staged] = act_apply(s1, a.act);
         ++staged;
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars.fc_done);
       if (staged == OUT_T || (t == Tp - 1 && staged > 0)) {
-        if (ri.src_b >= 0) {
+        if (lane < NB && ri.src_b >= 0) {
 #pragma unroll
           for (int o = 0; o < 2; ++o) {
             float* dst = a.crm + ((size_t)ri.out_idx + (size_t)o * a.Fsub) * a.T + t_stage0;
@@ -561,158 +344,256 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
     }
   }
   } else {
-    // ================= epilogue warpgroup m: owns hidden units [128m, 128m+128) of both layers
+    // ================= consumer warpgroup m: MMAs and cells of hidden units [128m, 128m+128) of both layers.
+    // Fragment of thread (warp q, lane l): unit 128 m + 64 hf + 16 q + l/4 + 8 hh, row n = 8 j + 2 (l%4) + e,
+    // register acc[g][hf][4 j + 2 hh + e]
     asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
     const int m = (warp - 4) >> 2;
     const int q = warp & 3;
     if (m < MT) {
-      const int u = m * 128 + q * 32 + lane;
       const float* bias_g = reinterpret_cast<const float*>(a.packed + PL.off_bias);
-      float b0[4], b1[4];
-#pragma unroll
-      for (int g = 0; g < 4; ++g) { b0[g] = bias_g[g * H + u]; b1[g] = bias_g[4 * H + g * H + u]; }
-      const float wfc0 = reinterpret_cast<const float*>(a.packed + PL.off_fcw)[u];
-      const float wfc1 = reinterpret_cast<const float*>(a.packed + PL.off_fcw)[H + u];
+      const float* fcw = reinterpret_cast<const float*>(a.packed + PL.off_fcw);
       float* my_part = fc_part + (size_t)(warp - 4) * 2 * NB;
-      float c0[NB], c1[NB];
+      float c0[16], c1[16];
 #pragma unroll
-      for (int i = 0; i < NB; ++i) c0[i] = c1[i] = 0.f;
-      const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(m * 4 * NB);
-      // thread-constant part of the h store address: k-block u/64, 16-byte chunk (u%64)/8, element u%8
-      const int kbu = u >> 6, chunk = (u & 63) >> 3, el = u & 7;
-      uint32_t job = 0;
+      for (int i = 0; i < 16; ++i) c0[i] = c1[i] = 0.f;
+      const uint32_t wbase = smem_u32(smem + sp.w);
+      int h0_seen = 0, h1_seen = 0, turns = 0;
+      bool first_block = true;
+      size_t tile_base = 0;  // global index (in the producer's stream) of this iteration's first stage
       for (int it = 0; it <= Tp; ++it) {
         for (int layer = 0; layer < 2; ++layer) {
           const int t = it - layer;
           if (t < 0 || t >= Tp) continue;
-          mbar_wait_relaxed(&bars.acc_full[m], job & 1);
-          ++job;
-          tc_fence_after();
-          if (q == 0 && lane == 0) trace_ev(a.trace, it, 12 + (layer * 3 + m) * 2);
-          if (layer == 1 && t >= 1) mbar_wait_relaxed(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read h1[(t+1)&1]
-          uint8_t* hb = smem + (layer ? sp.h1 : sp.h0 + (t & 1) * nkh * S_KBLK) + kbu * S_KBLK + el * 2;
-          __half2 hst[NB / 2];  // layer 1: h1_t is held back until every layer-1 MMA of this step is done
+          // operands of this step complete in shared memory (every phase waited on once, in order)
+          if (layer == 0) {
+            mbar_wait_mma(&bars.x_full[t & 1], (t >> 1) & 1);
+            for (; h0_seen < t; ++h0_seen) mbar_wait_mma(&bars.h0_ready, h0_seen & 1);      // h0_{t-1}
+          } else {
+            for (; h0_seen < t + 1; ++h0_seen) mbar_wait_mma(&bars.h0_ready, h0_seen & 1);  // h0_t
+            for (; h1_seen < t; ++h1_seen) mbar_wait_mma(&bars.h1_ready, h1_seen & 1);      // h1_{t-1}
+          }
+          const uint32_t x_addr = smem_u32(smem + sp.x + (t & 1) * S_KBLK);
+          const uint32_t h0_cur = smem_u32(smem + sp.h0 + (t & 1) * nkh * S_KBLK);        // h0_t
+          const uint32_t h0_prev = smem_u32(smem + sp.h0 + ((t + 1) & 1) * nkh * S_KBLK);  // h0_{t-1}
+          const uint32_t h1_prev = smem_u32(smem + sp.h1);                                    // h1_{t-1}
+          // B operand k ranges: layer 0: [x_t (32 k)] [h0_{t-1} (H)]; layer 1: [h0_t (H)] [h1_{t-1} (H)]
+          const int nkb = layer ? PL.nkb1 : PL.nkb0;
+          const size_t first = tile_base + (layer ? ((it < Tp) ? PL.tiles0 : 0) : 0) + (size_t)m * nkb * PARTS;
+          float acc[4][2][8];
 #pragma unroll
-          for (int j0 = 0; j0 < NB; j0 += 8) {
-            float gi[8], gf[8], gg[8], go[8];
-            tc_ld8(tacc + 0 * NB + j0, gi);
-            tc_ld8(tacc + 1 * NB + j0, gf);
-            tc_ld8(tacc + 2 * NB + j0, gg);
-            tc_ld8(tacc + 3 * NB + j0, go);
-            tc_wait_ld();
+          for (int g = 0; g < 4; ++g)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float cp, bi, bf, bg, bo;
-              if (layer == 0) { cp = c0[j0 + j]; bi = b0[0]; bf = b0[1]; bg = b0[2]; bo = b0[3]; }
-              else            { cp = c1[j0 + j]; bi = b1[0]; bf = b1[1]; bg = b1[2]; bo = b1[3]; }
-              const float cn = fast_sigmoid(gf[j] + bf) * cp + fast_sigmoid(gi[j] + bi) * fast_tanh(gg[j] + bg);
-              if (layer == 0) c0[j0 + j] = cn; else c1[j0 + j] = cn;
-              const float h = fast_sigmoid(go[j] + bo) * fast_tanh(cn);
-              // row n = j0 + j: (n>>3)*1024 + (n&7)*128 + ((chunk ^ (n&7)) << 4)
-              if (layer == 0)
-                *reinterpret_cast<__half*>(hb + (j0 >> 3) * 1024 + j * 128 + ((chunk ^ j) << 4)) = __float2half_rn(h);
-              go[j] = h;  // keep the fp32 h for the Linear layer
+            for (int hf = 0; hf < 2; ++hf) {
+#pragma unroll
+              for (int i = 0; i < 8; ++i) acc[g][hf][i] = 0.f;
+              wg::fence_operand(acc[g][hf]);
             }
-            if (layer == 1) {
+          int prev_stage = -1;
+          if (m > 0 || !first_block) { mbar_wait_mma(&bars.turn[m], turns & 1); ++turns; }
+          first_block = false;
+          for (int j = 0; j < nkb; ++j) {
+            uint32_t sb;  // state address of k range j
+            if (layer == 0) sb = (j == 0) ? x_addr : h0_prev + ((j - 1) >> 1) * S_KBLK + ((j - 1) & 1) * 64;
+            else sb = (j < H / KS) ? h0_cur + (j >> 1) * S_KBLK + (j & 1) * 64
+                                   : h1_prev + ((j - H / KS) >> 1) * S_KBLK + ((j - H / KS) & 1) * 64;
 #pragma unroll
-              for (int j = 0; j < 8; j += 2) hst[(j0 + j) >> 1] = __floats2half2_rn(go[j], go[j + 1]);
-            }
-            if (layer == 1) {
-              // Linear(H->2) in fp32: 16 products (2 outputs x 8 rows) summed over the warp's 32 hidden
-              // units with a halving exchange (8+4+2+1 shuffles) + one final pair add
-              float v[16];
+            for (int part = 0; part < PARTS; ++part) {
+              const size_t gi = first + (size_t)j * PARTS + part;
+              const int stage = (int)(gi % (size_t)STAGES);
+              mbar_wait_mma(&bars.w_full[stage], (uint32_t)((gi / (size_t)STAGES) & 1));
+              if (j == nkb - 1 && part == PARTS - 1 && lane == 0) mbar_arrive(&bars.turn[m + 1 < MT ? m + 1 : 0]);
+              wg::fence();
+              const uint32_t wa = wbase + stage * W_TILE;
 #pragma unroll
-              for (int j = 0; j < 8; ++j) { v[j] = go[j] * wfc0; v[8 + j] = go[j] * wfc1; }
+              for (int kk = 0; kk < 2; ++kk) {
+                const uint64_t bd = wg::desc_sw128(sb + kk * 32);
 #pragma unroll
-              for (int half = 8, off = 16; half >= 1; half >>= 1, off >>= 1) {
-                const bool up = (lane & off) != 0;
+                for (int g = 0; g < 4; ++g)
 #pragma unroll
-                for (int i = 0; i < half; ++i) {
-                  const float send = up ? v[i] : v[i + half];
-                  const float keep = up ? v[i + half] : v[i];
-                  v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                }
+                  for (int hf = 0; hf < 2; ++hf) {
+                    const uint64_t ad = wg::desc_sw64(wa + g * W_SUB + hf * (64 * 64) + kk * 32);
+                    wg::mma_f16_n16(acc[g][hf], ad, bd, 1u);
+                    if (X3 && part == 0) wg::mma_f16_n16(acc[g][hf], ad, wg::desc_sw128(sb + LO + kk * 32), 1u);
+                  }
               }
-              v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
-              // lane bits (4,3,2,1) select (output, row bit2, bit1, bit0)
-              if ((lane & 1) == 0) my_part[((lane >> 4) & 1) * NB + j0 + ((lane >> 1) & 7)] = v[0];
+              wg::commit();
+              wg::wait<1>();  // the MMAs of the previous stage have read it
+              if (prev_stage >= 0 && lane == 0) {
+                if (CL == 1) mbar_arrive(&bars.w_empty[prev_stage]);
+                else for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&bars.w_empty[prev_stage], (uint32_t)r);
+              }
+              prev_stage = stage;
             }
           }
-          tc_fence_before();
-          if (layer == 1) {
-            // TMEM is drained: release the accumulators first, then wait until the last layer-1 MMA of this
-            // step has consumed h1_{t-1} and overwrite it with h1_t
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bars.acc_empty[m]);
-            mbar_wait_relaxed(&bars.l1_done, t & 1);
+          wg::wait<0>();
 #pragma unroll
-            for (int n = 0; n < NB; n += 2) {
-              *reinterpret_cast<__half*>(hb + (n >> 3) * 1024 + (n & 7) * 128 + ((chunk ^ (n & 7)) << 4)) = __low2half(hst[n >> 1]);
-              *reinterpret_cast<__half*>(hb + ((n + 1) >> 3) * 1024 + ((n + 1) & 7) * 128 + ((chunk ^ ((n + 1) & 7)) << 4)) =
-                  __high2half(hst[n >> 1]);
-            }
-          }
-          fence_async_smem();
-          __syncwarp();
+          for (int g = 0; g < 4; ++g)
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) wg::fence_operand(acc[g][hf]);
           if (lane == 0) {
-            if (layer == 0) mbar_arrive(&bars.acc_empty[m]);
-            mbar_arrive(layer ? &bars.h1_ready : &bars.h0_ready);
-            if (q == 0) trace_ev(a.trace, it, 12 + (layer * 3 + m) * 2 + 1);
+            if (CL == 1) mbar_arrive(&bars.w_empty[prev_stage]);
+            else for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&bars.w_empty[prev_stage], (uint32_t)r);
+            // this warpgroup's MMAs of the step have consumed x_t / h1_{t-1}
+            mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
           }
+          if (layer == 1 && t >= 1) mbar_wait_mma(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
+          float fsum[2][4];  // Linear partials [o][row slot j*2+e]
+#pragma unroll
+          for (int i = 0; i < 8; ++i) fsum[i >> 2][i & 3] = 0.f;
+          __half hv[2][2][4];  // h (fp16 hi) [hf][hh][row slot], held back for layer 1
+          __half lv[2][2][4];
+          uint8_t* hb = smem + (layer ? sp.h1 : sp.h0 + (t & 1) * nkh * S_KBLK);
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int u = m * 128 + 64 * hf + 16 * q + (lane >> 2) + 8 * hh;
+              const float* bl = bias_g + (layer ? 4 * H : 0);
+              const float bi = bl[u], bff = bl[H + u], bg = bl[2 * H + u], bo = bl[3 * H + u];
+              const float w0 = fcw[u], w1 = fcw[H + u];
+#pragma unroll
+              for (int j = 0; j < 2; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int ri = 4 * j + 2 * hh + e;
+                  const int ci = hf * 8 + hh * 4 + j * 2 + e;
+                  const float cp = layer ? c1[ci] : c0[ci];
+                  const float cn = sg<X3>(acc[1][hf][ri] + bff) * cp + sg<X3>(acc[0][hf][ri] + bi) * th<X3>(acc[2][hf][ri] + bg);
+                  if (layer) c1[ci] = cn; else c0[ci] = cn;
+                  const float h = sg<X3>(acc[3][hf][ri] + bo) * th<X3>(cn);
+                  const __half hi = __float2half_rn(h);
+                  hv[hf][hh][j * 2 + e] = hi;
+                  lv[hf][hh][j * 2 + e] = __float2half_rn(h - __half2float(hi));
+                  if (layer) { fsum[0][j * 2 + e] += h * w0; fsum[1][j * 2 + e] += h * w1; }
+                }
+            }
+          if (layer == 1) {
+            // Linear(H->2) in fp32: sum over the warp's units (lanes with equal lane % 4 hold the same rows)
+#pragma unroll
+            for (int o = 0; o < 2; ++o)
+#pragma unroll
+              for (int s = 0; s < 4; ++s) {
+                float v = fsum[o][s];
+                v += __shfl_xor_sync(0xffffffffu, v, 4);
+                v += __shfl_xor_sync(0xffffffffu, v, 8);
+                v += __shfl_xor_sync(0xffffffffu, v, 16);
+                fsum[o][s] = v;
+              }
+            if (lane < 4) {
+#pragma unroll
+              for (int o = 0; o < 2; ++o)
+#pragma unroll
+                for (int s = 0; s < 4; ++s) my_part[o * NB + 8 * (s >> 1) + 2 * lane + (s & 1)] = fsum[o][s];
+            }
+            // every layer-1 MMA of this step (all warpgroups) has consumed h1_{t-1}: overwrite it with h1_t
+            mbar_wait_mma(&bars.l1_done, t & 1);
+          }
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int u = m * 128 + 64 * hf + 16 * q + (lane >> 2) + 8 * hh;
+              uint8_t* ub = hb + (u >> 6) * S_KBLK + (u & 7) * 2;
+              const int chunk = (u & 63) >> 3;
+#pragma unroll
+              for (int j = 0; j < 2; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int n = 8 * j + 2 * (lane & 3) + e;
+                  uint8_t* p = ub + (n >> 3) * 1024 + (n & 7) * 128 + ((chunk ^ (n & 7)) << 4);
+                  *reinterpret_cast<__half*>(p) = hv[hf][hh][j * 2 + e];
+                  if (X3) *reinterpret_cast<__half*>(p + LO) = lv[hf][hh][j * 2 + e];
+                }
+            }
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(layer ? &bars.h1_ready : &bars.h0_ready);
         }
+        tile_base += ((it < Tp) ? PL.tiles0 : 0) + ((it >= 1) ? PL.tiles1 : 0);
       }
     }
   }
 
   // ---------------- teardown
-  tc_fence_before();
   __syncthreads();
   if (CL > 1) cluster_sync_all();  // no CTA leaves while a peer may still signal its barriers
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base));
-  }
 }
 
 }  // namespace tc
 
+static int sb_ksb(const fsn_model_desc* d) { return (2 * d->sb_num_neighbors + 1) + (2 * d->fb_num_neighbors + 1); }
+
+static bool sb_tc_shape_ok(int H, int Ksb) { return H % 128 == 0 && H / 128 <= tc::MAX_MT && H >= 128 && Ksb <= tc::KS; }
+
 bool sb_tc_supported(const fsn_model_desc* d) {
   if (d->cell_type != FSN_CELL_LSTM) return false;  // GRU: fp32 kernels only
-  const int Ksb = (2 * d->sb_num_neighbors + 1) + (2 * d->fb_num_neighbors + 1);
-  if (d->precision == FSN_PREC_F16X3_TC) return sb_tc2_supported(d);  // compensated variant: pair kernel only
-  return d->sb_hidden % 128 == 0 && d->sb_hidden / 128 <= tc::MAX_MT && d->sb_hidden >= 128 && Ksb <= tc::KS;
+  return sb_tc_shape_ok(d->sb_hidden, sb_ksb(d));
 }
+
+size_t sb_tc_packed_bytes_raw(int H, bool x3) { return tc::packed_layout(H, x3).bytes; }
 
 size_t sb_tc_packed_bytes(const fsn_model_desc* d) {
   if (!sb_tc_supported(d)) return 0;
-  if (sb_tc4_supported(d)) return sb_tc4_packed_bytes();
-  if (sb_tc2_supported(d)) return sb_tc2_packed_bytes(d->precision == FSN_PREC_F16X3_TC);
-  const int Ksb = (2 * d->sb_num_neighbors + 1) + (2 * d->fb_num_neighbors + 1);
-  return tc::packed_layout(d->sb_hidden, Ksb).bytes;
+  return sb_tc_packed_bytes_raw(d->sb_hidden, d->precision == FSN_PREC_F16X3_TC);
 }
 
-int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed, cudaStream_t st) {
-  FSN_REQUIRE(sb_tc_supported(d), FSN_ERR_UNSUPPORTED,
-              "FSN_PREC_F16_TC needs sb_hidden in {128,256,384} and sub-band input width <= 32");
-  if (sb_tc4_supported(d)) return sb_tc4_pack(d, sb, packed, st);
-  if (sb_tc2_supported(d)) return sb_tc2_pack(d, sb, packed, st);
-  const int Ksb = (2 * d->sb_num_neighbors + 1) + (2 * d->fb_num_neighbors + 1);
-  tc::pack_kernel<<<148 * 4, 256, 0, st>>>(sb->w_ih[0], sb->w_hh[0], sb->w_ih[1], sb->w_hh[1], sb->b_ih[0],
-                                           sb->b_hh[0], sb->b_ih[1], sb->b_hh[1], sb->fc_w, sb->fc_b, d->sb_hidden,
-                                           Ksb, (uint8_t*)packed);
+int sb_tc_pack_raw(const fsn_seq_weights* sb, int H, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3) {
+  FSN_REQUIRE(sb_tc_shape_ok(H, Ksb), FSN_ERR_UNSUPPORTED,
+              "the fp16 tensor-core LSTM stack needs a hidden size in {128,256,384} and an input width <= 32");
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  tc::pack_kernel<<<sms * 4, 256, 0, st>>>(sb->w_ih[0], sb->w_hh[0], sb->w_ih[1], sb->w_hh[1], sb->b_ih[0], sb->b_hh[0],
+                                           sb->b_ih[1], sb->b_hh[1], sb->fc_w, sb->fc_b, H, Ksb, x3 ? 1 : 0, fc_out,
+                                           (uint8_t*)packed);
   FSN_CHECK_LAUNCH("sb pack_kernel");
   return FSN_OK;
 }
 
+int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed, cudaStream_t st) {
+  FSN_REQUIRE(sb_tc_supported(d), FSN_ERR_UNSUPPORTED,
+              "FSN_PREC_F16_TC / FSN_PREC_F16X3_TC need sb_hidden in {128,256,384} and sub-band input width <= 32");
+  return sb_tc_pack_raw(sb, d->sb_hidden, sb_ksb(d), 2, packed, st, d->precision == FSN_PREC_F16X3_TC);
+}
+
+template <bool X3>
+static int sb_tc_launch(const tc::KArgs& a, int H, cudaStream_t st) {
+  const tc::Smem sp = tc::smem_plan(H, a.stages, X3);
+  const size_t smem = sp.total + 1024;  // slack for the 1024-byte alignment of the dynamic segment
+  int rc = check_cuda(cudaFuncSetAttribute(tc::sb_lstm_tc_kernel<X3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)smem), "sb_lstm_tc smem attr");
+  if (rc) return rc;
+  const int tiles = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;  // padding CTAs own no valid row
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(tiles);
+  cfg.blockDim = dim3(128 + 128 * (H / 128));
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = a.cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  rc = check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_lstm_tc_kernel<X3>, a), "sb_lstm_tc_kernel launch");
+  if (rc) return rc;
+  FSN_CHECK_LAUNCH("sb_lstm_tc_kernel");
+  return FSN_OK;
+}
+
 int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
-  if (s.quad) return sb_tc4_forward(s, st);
-  if (s.pair) return sb_tc2_forward(s, st);
   tc::KArgs a;
   a.packed = (const uint8_t*)s.packed;
-  a.magT = s.magT; a.fbT = s.fbT; a.inv2 = s.inv2; a.unit_scale = s.unit_scale; a.crm = s.crm;
-  a.R = s.map.B * s.map.Fsub; a.F = s.F; a.Tp = s.Tp; a.la = s.la; a.T = s.Tp - s.la;
+  a.magT = s.magT; a.fbT = s.fbT; a.inv2 = s.inv2; a.unit_scale = s.shrink > 1 ? nullptr : s.unit_scale; a.crm = s.crm;
+  a.R = s.map.B * s.map.Fsub; a.F = s.F; a.Tp = s.steps > 0 ? s.steps : s.Tp; a.la = s.la; a.T = a.Tp - s.la;
+  a.src_T = s.Tp; a.shrink = s.shrink > 1 ? s.shrink : 1;
   a.Ns = s.Ns; a.Nf = s.Nf; a.H = s.H; a.Ksb = (2 * s.Ns + 1) + (2 * s.Nf + 1); a.act = s.act;
   a.Fsub = s.map.Fsub; a.map = s.map;
+  FSN_REQUIRE(sb_tc_shape_ok(a.H, a.Ksb), FSN_ERR_UNSUPPORTED, "sb_lstm_tc: unsupported hidden size %d / input width %d",
+              a.H, a.Ksb);
   static int stages_env = -1;
   if (stages_env < 0) {
     const char* e = getenv("FSN_TC_STAGES");
@@ -728,50 +609,7 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
     if (cluster_env != 1 && cluster_env != 2 && cluster_env != 4) cluster_env = 2;
   }
   a.cluster = cluster_env;
-  a.trace = nullptr;
-  static long long* trace_buf = nullptr;
-  if (getenv("FSN_TC_TRACE")) {  // debug only: 8 iterations x 32 event slots of clock64
-    if (!trace_buf) { cudaMalloc(&trace_buf, 8 * 32 * sizeof(long long)); cudaMemset(trace_buf, 0, 8 * 32 * sizeof(long long)); }
-    a.trace = trace_buf;
-  }
-  const tc::Smem sp = tc::smem_plan(s.H, a.stages);
-  const size_t smem = sp.total + 1024;  // slack for the 1024-byte alignment of the dynamic segment
-  int rc = check_cuda(cudaFuncSetAttribute(tc::sb_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)smem), "sb_lstm_tc smem attr");
-  if (rc) return rc;
-  const int tiles = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;  // padding CTAs own no valid row
-  const int threads = 128 + 128 * (s.H / 128);
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(tiles);
-  cfg.blockDim = dim3(threads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = a.cluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  rc = check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_lstm_tc_kernel, a), "sb_lstm_tc_kernel launch");
-  if (rc) return rc;
-  FSN_CHECK_LAUNCH("sb_lstm_tc_kernel");
-  if (a.trace) {
-    long long h[8 * 32];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, a.trace, sizeof(h), cudaMemcpyDeviceToHost);
-    const long long t0 = h[0];
-    static const char* names[6] = {"L0m0", "L0m1", "L0m2", "L1m0", "L1m1", "L1m2"};
-    for (int it = 0; it < 3; ++it) {
-      fprintf(stderr, "[trace it=%d]\n", it + 8);
-      for (int j = 0; j < 6; ++j)
-        fprintf(stderr, "  %s issue_begin %7lld acc_empty_ok %7lld issue_end %7lld | epi_begin %7lld epi_end %7lld\n", names[j],
-                h[it * 32 + j * 2] - t0, h[it * 32 + 24 + j] - t0, h[it * 32 + j * 2 + 1] - t0,
-                h[it * 32 + 12 + j * 2] - t0, h[it * 32 + 12 + j * 2 + 1] - t0);
-    }
-  }
-  return FSN_OK;
+  return s.x3 ? sb_tc_launch<true>(a, s.H, st) : sb_tc_launch<false>(a, s.H, st);
 }
 
 }  // namespace fsn

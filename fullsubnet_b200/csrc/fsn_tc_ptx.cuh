@@ -1,4 +1,4 @@
-// PTX helpers shared by the tcgen05 kernels (mbarrier, bulk copy, tcgen05, cluster / DSMEM).
+// PTX helpers shared by the tensor-core kernels (mbarrier, bulk copy / TMA, cp.async, cluster / DSMEM).
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -76,18 +76,22 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// spin with a watchdog: a protocol bug traps (launch error) instead of hanging the GPU
+// spin with a watchdog: a protocol bug traps (launch error) instead of hanging the GPU.  No printf here: any call in a
+// kernel makes ptxas serialise all of its wgmma instructions
 template <bool RELAXED>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (RELAXED) __nanosleep(64);
-    if (++spins > (RELAXED ? (1u << 24) : (1u << 27))) {
-      printf("fsn tc: mbarrier timeout (block %d thread %d bar off %u parity %u)\n", blockIdx.x, threadIdx.x,
-             smem_u32(bar) & 0xffffu, parity);
-      __trap();
-    }
+    if (++spins > (RELAXED ? (1u << 24) : (1u << 27))) asm volatile("trap;");
   }
+}
+
+// same without the back-off variants, for the threads that issue wgmma
+__device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity))
+    if (++spins > (1u << 27)) asm volatile("trap;");
 }
 
 // ---- TMA engine (non-tensor bulk copy) and proxy fence
@@ -96,6 +100,14 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                    smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
+}
+// same, multicast to the CTAs of `mask` in the cluster (same offset, each CTA's barrier at the same offset)
+__device__ __forceinline__ void bulk_g2s_mc(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(dst)),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
+      : "memory");
 }
 // TMA tiled 2-D load (tensor map in kernel parameter space): box at element coordinates (c0 = inner, c1 = row)
 __device__ __forceinline__ void tma_load_2d(void* dst, const void* tmap, int c0, int c1, uint64_t* bar) {
@@ -107,36 +119,8 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const void* tmap, int c0,
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
-// ---- tcgen05
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// cta_group::1 forms
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_commit1(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, tf32 operands (fp32 bits, low 13 mantissa bits ignored), fp32 accumulate, K = 8
-__device__ __forceinline__ void tc_mma1_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same tile shape, fp16 operands (K = 16 per instruction), fp32 accumulate
-__device__ __forceinline__ void tc_mma1_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
 }
 // 16-byte asynchronous copy global -> shared; bytes beyond src_bytes (0..16) are zero-filled
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
@@ -146,40 +130,6 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void tc_mma2_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit2_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major shared-memory matrix descriptors (cute::UMMA::SmemDescriptor): start>>4 | LBO(1)<<16 | SBO>>4 <<32 |
-// version 1 <<46 | layout <<61.  128B swizzle: 8-row groups 1024 B apart; 64B swizzle: 512 B apart.
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ uint64_t desc_sw64(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (32ull << 32) | (1ull << 46) | (4ull << 61);
-}
 // byte offset of element (row, k) in a K-major 128B-swizzled block of 64 k (rows of 128 B)
 __host__ __device__ __forceinline__ int swz128_off(int row, int k) {
   return (row >> 3) * 1024 + (row & 7) * 128 + ((((k >> 3) ^ (row & 7)) & 7) << 4) + (k & 7) * 2;

@@ -1,18 +1,18 @@
 // tf32 tensor-core GEMM for the training path:  C[M,N] (+)= A[M,K] * B[N,K]^T, all fp32 in global memory, both
-// operands K-contiguous ("K-major"), tcgen05.mma kind::tf32 with the accumulator in TMEM.
+// operands K-contiguous ("K-major"), Hopper warpgroup MMA (wgmma.mma_async, tf32) with the accumulators in registers.
 //
 // One CTA = one 128 x BN output tile (BN = 128 or 256), optional split-K slice (blockIdx.z).
-//   warps 0-3  producers: every thread owns one row of the A tile and one (BN=128) or two (BN=256) rows of the B
-//              tile; per k-step (32 floats = one 128-byte swizzle row) it issues 16-byte cp.async copies straight
-//              into the 128B-swizzled K-major layout the UMMA descriptors expect (chunk ^= row & 7); rows / k beyond
-//              the matrix are zero-filled.  cp.async.wait_group + fence.proxy.async + mbarrier arrive hand the stage
-//              to the tensor core.  After the last k-step the same warps drain TMEM (warp w <-> lanes 32w..32w+31).
-//   warp 4     MMA issue (converged warp, one elected lane): 4 MMAs (K = 8) per stage, tcgen05.commit frees it.
+//   warpgroups 0-1  consumers: warpgroup h multiplies rows 64h..64h+63 of the tile (m64nBNk8, 4 per stage), releases each
+//                   stage once the wgmma that read it has retired (wait_group 1), and writes its accumulator fragment
+//                   straight from registers after the last stage.
+//   producers       tgemm_tma_kernel: one warp, one elected lane issues the TMA tiled loads (128B swizzle, rows / k beyond
+//                   the matrix zero-filled by the tensor map) of a stage.  tgemm_kernel: a third warpgroup whose threads
+//                   copy 16-byte chunks with cp.async straight into the same 128B-swizzled K-major layout (chunk ^= row & 7).
 // No operand conversion pass: the tensor core reads fp32 bits as tf32 (10-bit mantissa, truncation).
 //
 // Also in this file, built from the same pieces (DESIGN.md 4.2):
-//   tgemm_tma_kernel        the same tile fed by TMA (default); BlockedOps mode streams block-tiled operand copies
-//                           (transpose_blocked_kernel) for the long-K weight-gradient GEMMs dW = dG^T X
+//   tgemm_tma_kernel        BlockedOps mode streams block-tiled operand copies (transpose_blocked_kernel) for the long-K
+//                           weight-gradient GEMMs dW = dG^T X
 //   lstm_fwd_step_kernel    one LSTM step of the training forward: [x_t | h_{t-1}] [W_ih | W_hh]^T (fp16 / tf32 operands)
 //                           and the cell in one launch; tile = 128 rows x (4 gates x 32 hidden units)
 #include <cuda.h>
@@ -21,6 +21,7 @@
 
 #include "fsn_internal.cuh"
 #include "fsn_tc_ptx.cuh"
+#include "fsn_wgmma.cuh"
 
 namespace fsn {
 namespace tg {
@@ -29,14 +30,15 @@ using namespace ptx;
 
 constexpr int BM = 128, BK = 32;
 constexpr int A_BYTES = BM * BK * 4;  // 16 KB
+constexpr int CONSUMERS = 256;        // two warpgroups of 64 tile rows each
 
 template <int BN> struct Cfg {
+  static_assert(BN == 128 || BN == 256, "wgmma tile width");
   static constexpr int B_BYTES = BN * BK * 4;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // BN = 128: 3 stages (96 KB) so two CTAs share an SM - one drains its accumulator while the other runs its main loop
-  static constexpr int STAGES = (BN == 128) ? 3 : (BN == 256 ? 4 : 3);
-  static constexpr int TMEM_COLS = (BN <= 128) ? 128 : (BN <= 256 ? 256 : 512);
-  static constexpr int LAG = (BN == 128) ? 2 : 3;      // cp.async groups in flight per thread
+  // BN = 128: 3 stages (96 KB) so two CTAs share an SM - one writes its tile while the other runs its main loop
+  static constexpr int STAGES = (BN == 128) ? 3 : 4;
+  static constexpr int LAG = (BN == 128) ? 2 : 3;      // cp.async groups in flight per producer thread
   static constexpr int MIN_CTAS = (BN == 128) ? 2 : 1;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
@@ -47,83 +49,66 @@ struct BlockedOps { int on, a_nkb, b_nkb, a_kb0, b_kb0; };
 struct Bars {
   uint64_t full[8];
   uint64_t empty[8];
-  uint64_t acc_full;
-  uint32_t tmem_base;
 };
 
-// drain the accumulator: TMEM -> registers -> per-warp padded smem slab -> full 128-byte rows in global memory
-// (all MMAs have completed, so the stage buffers are free)
+// consumer warpgroups: the tile's MMAs over nk stages into acc (rows 64 * warpgroup + fragment row)
 template <int BN>
-__device__ __forceinline__ void epilogue(uint8_t* smem, Bars& bars, uint32_t tmem_base, float* __restrict__ C, size_t ldc,
-                                         int M, int N, int m0, int n0, int accumulate, size_t split_stride) {
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  mbar_wait<true>(&bars.acc_full, 0);
-  tc_fence_after();
-  float* slab = reinterpret_cast<float*>(smem) + warp * (32 * 33);
-  float* cbase = C + (size_t)blockIdx.z * split_stride;
-  const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-  for (int cb = 0; cb < BN / 32; ++cb) {
-    if (n0 + cb * 32 >= N) break;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      float v[8];
-      tc_ld8(taddr + cb * 32 + q * 8, v);
-      tc_wait_ld();
-#pragma unroll
-      for (int j = 0; j < 8; ++j) slab[lane * 33 + q * 8 + j] = v[j];
-    }
-    __syncwarp();
-    const int col = n0 + cb * 32 + lane;
-    if (col < N) {
-      const int row0 = m0 + warp * 32;
-#pragma unroll
-      for (int r8 = 0; r8 < 32; r8 += 8) {
-        float old[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j)  // batch the read-modify-write loads: one memory round trip per 8 rows
-          old[j] = (accumulate && row0 + r8 + j < M) ? cbase[(size_t)(row0 + r8 + j) * ldc + col] : 0.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (row0 + r8 + j < M) cbase[(size_t)(row0 + r8 + j) * ldc + col] = old[j] + slab[(r8 + j) * 33 + lane];
-      }
-    }
-    __syncwarp();
-  }
-}
-
-template <int BN>
-__device__ __forceinline__ void mma_loop(uint8_t* smem, Bars& bars, uint32_t tmem_base, int nk) {
+__device__ __forceinline__ void mma_loop(uint8_t* smem, Bars& bars, int nk, float (&acc)[BN / 2]) {
   using CF = Cfg<BN>;
   constexpr int STAGES = CF::STAGES;
-  constexpr int N0 = BN > 256 ? 256 : BN, N1 = BN - N0;  // one MMA covers at most 256 columns
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N0 >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-  const uint32_t idesc1 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((N1 > 0 ? N1 : 8) >> 3) << 17) |
-                          ((uint32_t)(BM >> 4) << 24);
+  const int wgi = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const uint32_t smem_base = smem_u32(smem);
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  wg::fence_operand(acc);
   for (int i = 0; i < nk; ++i) {
     const int s = i % STAGES;
-    mbar_wait<false>(&bars.full[s], (uint32_t)((i / STAGES) & 1));
-    tc_fence_after();
-    if (elect_one()) {
-      const uint32_t sa = smem_base + s * CF::STAGE_BYTES;
-      const uint32_t sb = sa + A_BYTES;
+    mbar_wait_mma(&bars.full[s], (uint32_t)((i / STAGES) & 1));
+    const uint32_t sa = smem_base + s * CF::STAGE_BYTES + wgi * (64 * 128);
+    const uint32_t sb = smem_base + s * CF::STAGE_BYTES + A_BYTES;
+    wg::fence();
 #pragma unroll
-      for (int kk = 0; kk < BK / 8; ++kk) {
-        tc_mma1_tf32(tmem_base, desc_sw128(sa + kk * 32), desc_sw128(sb + kk * 32), idesc, (i > 0 || kk > 0) ? 1u : 0u);
-        if (N1 > 0)  // columns 256.. of the tile: B rows 256.. start 256 * 128 bytes further
-          tc_mma1_tf32(tmem_base + 256, desc_sw128(sa + kk * 32), desc_sw128(sb + 256 * 128 + kk * 32), idesc1,
-                       (i > 0 || kk > 0) ? 1u : 0u);
-      }
-      tc_commit1(&bars.empty[s]);
+    for (int kk = 0; kk < BK / 8; ++kk) {
+      if constexpr (BN == 256) wg::mma_tf32_n256(acc, wg::desc_sw128(sa + kk * 32), wg::desc_sw128(sb + kk * 32), 1u);
+      else                     wg::mma_tf32_n128(acc, wg::desc_sw128(sa + kk * 32), wg::desc_sw128(sb + kk * 32), 1u);
     }
-    __syncwarp();
+    wg::commit();
+    wg::wait<1>();  // the MMAs of stage i-1 have read their operands
+    if (i > 0 && lane == 0) mbar_arrive(&bars.empty[(i - 1) % STAGES]);
   }
-  if (elect_one()) tc_commit1(&bars.acc_full);
-  __syncwarp();
+  wg::wait<0>();
+  wg::fence_operand(acc);
+}
+
+// accumulator fragment -> global memory (all MMAs have completed)
+template <int BN>
+__device__ __forceinline__ void epilogue(const float (&acc)[BN / 2], float* __restrict__ C, size_t ldc, int M, int N, int m0,
+                                         int n0, int accumulate, size_t split_stride) {
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31, wgi = threadIdx.x >> 7;
+  float* cbase = C + (size_t)blockIdx.z * split_stride;
+  const int rbase = m0 + 64 * wgi + 16 * w + (l >> 2);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (l & 3);
+    if (col >= N) continue;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = rbase + 8 * hh;
+      if (row >= M) continue;
+      float* p = cbase + (size_t)row * ldc + col;
+      float v0 = acc[4 * j + 2 * hh], v1 = acc[4 * j + 2 * hh + 1];
+      if (accumulate) v0 += p[0];
+      p[0] = v0;
+      if (col + 1 < N) {
+        if (accumulate) v1 += p[1];
+        p[1] = v1;
+      }
+    }
+  }
 }
 
 template <int BN>
-__global__ void __launch_bounds__(160, Cfg<BN>::MIN_CTAS)
+__global__ void __launch_bounds__(CONSUMERS + 128, 1)
 tgemm_kernel(const float* __restrict__ A, size_t lda, const float* __restrict__ Bm, size_t ldb, float* __restrict__ C,
              size_t ldc, int M, int N, int K, int k_per_split, int accumulate, size_t split_stride) {
   using CF = Cfg<BN>;
@@ -131,30 +116,21 @@ tgemm_kernel(const float* __restrict__ A, size_t lda, const float* __restrict__ 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   Bars& bars = *reinterpret_cast<Bars*>(smem + STAGES * CF::STAGE_BYTES);
-  const int tid = threadIdx.x, warp = tid >> 5;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   const int kb = blockIdx.z * k_per_split;
   const int ke = (kb + k_per_split < K) ? kb + k_per_split : K;
   const int nk = (ke - kb + BK - 1) / BK;
 
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 128); mbar_init(&bars.empty[s], 1); }
-    mbar_init(&bars.acc_full, 1);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 128); mbar_init(&bars.empty[s], CONSUMERS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars.tmem_base)),
-                 "n"(BN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars.tmem_base;
 
-  if (warp < 4) {
+  if (threadIdx.x >= CONSUMERS) {
     // ------------------------------------------------------------------ producers
-    // lane -> (16-byte chunk c = tid & 7 of a 128-byte row, rows (tid >> 3) + 16 j): 8 lanes read one full line
+    // thread -> (16-byte chunk c = tid & 7 of a 128-byte row, rows (tid >> 3) + 16 j): 8 threads read one full line
+    const int tid = threadIdx.x - CONSUMERS;
     const int c = tid & 7, rbase = tid >> 3;
     const uint32_t sw = (uint32_t)(rbase & 7);  // (rbase + 16 j) & 7
     const uint32_t dst_off = (uint32_t)((rbase >> 3) * 1024 + (rbase & 7) * 128) + (((uint32_t)c ^ sw) << 4);
@@ -164,7 +140,7 @@ tgemm_kernel(const float* __restrict__ A, size_t lda, const float* __restrict__ 
     for (int i = 0; i < nk + LAG; ++i) {
       if (i < nk) {
         const int s = i % STAGES;
-        if (i >= STAGES) mbar_wait<false>(&bars.empty[s], (uint32_t)(((i / STAGES) - 1) & 1));
+        if (i >= STAGES) mbar_wait<true>(&bars.empty[s], (uint32_t)(((i / STAGES) - 1) & 1));
         const int k0 = kb + i * BK;
         int rem = (ke - (k0 + c * 4)) * 4;
         rem = rem < 0 ? 0 : (rem > 16 ? 16 : rem);
@@ -188,83 +164,61 @@ tgemm_kernel(const float* __restrict__ A, size_t lda, const float* __restrict__ 
         mbar_arrive(&bars.full[(i - LAG) % STAGES]);
       }
     }
-    epilogue<BN>(smem, bars, tmem_base, C, ldc, M, N, m0, n0, accumulate, split_stride);
   } else {
-    mma_loop<BN>(smem, bars, tmem_base, nk);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(BN));
+    float acc[BN / 2];
+    mma_loop<BN>(smem, bars, nk, acc);
+    epilogue<BN>(acc, C, ldc, M, N, m0, n0, accumulate, split_stride);
   }
 }
 
-// Same tile, operands fed by TMA: one elected lane issues two tiled loads per stage (128B hardware swizzle, rows / k
+// Same tile, operands fed by TMA: one elected lane issues the tiled loads of a stage (128B hardware swizzle, rows / k
 // beyond the matrix zero-filled by the tensor map), the full barrier counts the transaction bytes.
 template <int BN>
-__global__ void __launch_bounds__(160, Cfg<BN>::MIN_CTAS)
+__global__ void __launch_bounds__(CONSUMERS + 32, Cfg<BN>::MIN_CTAS)
 tgemm_tma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmB2, float* __restrict__ C, size_t ldc, int M, int N, int K,
                  int k_per_split, int accumulate, size_t split_stride, BlockedOps bo) {
   using CF = Cfg<BN>;
   constexpr int STAGES = CF::STAGES;
+  (void)tmB2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   Bars& bars = *reinterpret_cast<Bars*>(smem + STAGES * CF::STAGE_BYTES);
-  const int tid = threadIdx.x, warp = tid >> 5;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   const int kb = blockIdx.z * k_per_split;
   const int ke = (kb + k_per_split < K) ? kb + k_per_split : K;
   const int nk = (ke - kb + BK - 1) / BK;
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 1); }
-    mbar_init(&bars.acc_full, 1);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], CONSUMERS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars.tmem_base)),
-                 "n"(CF::TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars.tmem_base;
-  if (warp < 4) {
-    if (warp == 0) {
-      for (int i = 0; i < nk; ++i) {
-        const int s = i % STAGES;
-        if (i >= STAGES) mbar_wait<false>(&bars.empty[s], (uint32_t)(((i / STAGES) - 1) & 1));
-        if (elect_one()) {
-          uint8_t* sa = smem + s * CF::STAGE_BYTES;
-          mbar_expect_tx(&bars.full[s], CF::STAGE_BYTES);
-          if (bo.on) {
-            // block-tiled operands: tile (128 rows, k block of 32) = 16 contiguous KB, see tgemm_blocked_launch
-            const int kblk = (kb >> 5) + i;
-            tma_load_2d(sa, &tmA, 0, (blockIdx.x * bo.a_nkb + bo.a_kb0 + kblk) * 128, &bars.full[s]);
+  if (threadIdx.x >= CONSUMERS) {
+    for (int i = 0; i < nk; ++i) {
+      const int s = i % STAGES;
+      if (i >= STAGES) mbar_wait<false>(&bars.empty[s], (uint32_t)(((i / STAGES) - 1) & 1));
+      if (elect_one()) {
+        uint8_t* sa = smem + s * CF::STAGE_BYTES;
+        mbar_expect_tx(&bars.full[s], CF::STAGE_BYTES);
+        if (bo.on) {
+          // block-tiled operands: tile (128 rows, k block of 32) = 16 contiguous KB, see tgemm_blocked_launch
+          const int kblk = (kb >> 5) + i;
+          tma_load_2d(sa, &tmA, 0, (blockIdx.x * bo.a_nkb + bo.a_kb0 + kblk) * 128, &bars.full[s]);
 #pragma unroll
-            for (int j = 0; j < BN / 128; ++j)
-              tma_load_2d(sa + A_BYTES + j * 128 * 128, &tmB, 0, ((blockIdx.y * (BN / 128) + j) * bo.b_nkb + bo.b_kb0 + kblk) * 128,
-                          &bars.full[s]);
-          } else {
-            tma_load_2d(sa, &tmA, kb + i * BK, m0, &bars.full[s]);
-            tma_load_2d(sa + A_BYTES, &tmB, kb + i * BK, n0, &bars.full[s]);
-            if (BN > 256) tma_load_2d(sa + A_BYTES + 256 * 128, &tmB2, kb + i * BK, n0 + 256, &bars.full[s]);
-          }
+          for (int j = 0; j < BN / 128; ++j)
+            tma_load_2d(sa + A_BYTES + j * 128 * 128, &tmB, 0, ((blockIdx.y * (BN / 128) + j) * bo.b_nkb + bo.b_kb0 + kblk) * 128,
+                        &bars.full[s]);
+        } else {
+          tma_load_2d(sa, &tmA, kb + i * BK, m0, &bars.full[s]);
+          tma_load_2d(sa + A_BYTES, &tmB, kb + i * BK, n0, &bars.full[s]);
         }
-        __syncwarp();
       }
+      __syncwarp();
     }
-    epilogue<BN>(smem, bars, tmem_base, C, ldc, M, N, m0, n0, accumulate, split_stride);
   } else {
-    mma_loop<BN>(smem, bars, tmem_base, nk);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(CF::TMEM_COLS));
+    float acc[BN / 2];
+    mma_loop<BN>(smem, bars, nk, acc);
+    epilogue<BN>(acc, C, ldc, M, N, m0, n0, accumulate, split_stride);
   }
 }
 
@@ -272,11 +226,11 @@ tgemm_tma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 // One LSTM step of the training forward, GEMM and cell in one kernel (torch.nn.LSTM forward, saved for autograd):
 //   z = P_t + b_ih + b_hh + h_{t-1} W_hh^T;  (i,f,g,o) = act(z);  c_t = f c_{t-1} + i g;  h_t = o tanh(c_t)
 // The CTA tile is 128 rows x 128 gate columns = the FOUR gates of 32 hidden units: the B operand is four 32-row TMA
-// boxes of W_hh (rows g*H + 32 j ..), so the accumulator holds everything the cell of those units needs and the
-// recurrent product never goes to memory.  The epilogue turns the accumulator through shared memory so that every
-// global access is a full 128-byte row piece: reads P_t (the hoisted input projection, overwritten in place by the
-// post-activation gates the backward pass needs) and c_{t-1}, writes gates, c_t, h_t.  Two CTAs per SM: one drains
-// while the other multiplies.
+// boxes of W_hh (rows g*H + 32 j ..), so column 32 g + u of the accumulator is gate g of unit u0 + u.  In the wgmma
+// fragment a thread holds columns 8 j + 2 (lane % 4) + {0, 1}, i.e. the same 8 units in all four gate blocks: the cell
+// runs straight on the accumulator registers and the recurrent product never goes to memory.  The cell reads P_t (the
+// hoisted input projection, overwritten in place by the post-activation gates the backward pass needs) and c_{t-1},
+// writes gates, c_t, h_t.  Two CTAs per SM: one runs its cell while the other multiplies.
 // 1 / (1 + 2^(-x log2 e)) and 2 sigmoid(2x) - 1 on the MUFU unit (ex2.approx + rcp.approx: ~2 ulp; saturate correctly:
 // ex2 -> inf gives rcp -> 0, ex2 -> 0 gives 1)
 __device__ __forceinline__ float sigmoid_mufu(float x) {
@@ -292,15 +246,14 @@ __device__ __forceinline__ float tanh_mufu(float x) {
   return fmaf(2.0f, r, -1.0f);
 }
 
-// HT: hidden size known at compile time (0: runtime) - every stride of the epilogue becomes an immediate offset
-// ST: TMA stages (3: 2 CTAs per SM; 2: 3 CTAs per SM - the kernel is bound by the latency chain of one CTA - load, multiply,
-// drain, cell - not by any unit, so more CTAs in flight is what raises the throughput)
+// HT: hidden size known at compile time (0: runtime) - the strides of the cell become immediate offsets
+// ST: TMA stages
 template <int ST> struct StepCfg {
-  static constexpr int MAIN = (ST * Cfg<128>::STAGE_BYTES > 4 * 4 * 32 * 33 * 4 ? ST * Cfg<128>::STAGE_BYTES : 4 * 4 * 32 * 33 * 4 + 1023) & ~1023;
+  static constexpr int MAIN = ST * Cfg<128>::STAGE_BYTES;
   static constexpr int SMEM = MAIN + 1024 /*align*/ + 256 /*barriers*/;
 };
 template <bool FOLD, int HT, int ST>
-__global__ void __launch_bounds__(192, (ST == 2 && HT != 0 && FOLD) ? 3 : 2)
+__global__ void __launch_bounds__(CONSUMERS + 32, 2)
 lstm_fwd_step_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmWx, float* __restrict__ G,
                      const float* __restrict__ b_ih, const float* __restrict__ b_hh, const float* __restrict__ C_prev,
@@ -312,27 +265,17 @@ lstm_fwd_step_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   Bars& bars = *reinterpret_cast<Bars*>(smem + StepCfg<ST>::MAIN);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.x * BM, u0 = blockIdx.y * 32;
   // k blocks: first nkx of x_t W_ih^T (a narrow layer input is folded in here instead of a hoisted projection: G then
   // carries no P and is only written), then nkh of h_{t-1} W_hh^T (0 at the first step)
   const int nk = nkx + nkh;
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 1); }
-    mbar_init(&bars.acc_full, 1);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], CONSUMERS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars.tmem_base)),
-                 "n"(CF::TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars.tmem_base;
-  if (warp == 5) {
-    // TMA producer (its own warp: the four epilogue warps start their global loads right away)
+  if (threadIdx.x >= CONSUMERS) {
+    // TMA producer
     for (int i = 0; i < nk; ++i) {
       const int s = i % STAGES;
       if (i >= STAGES) mbar_wait<false>(&bars.empty[s], (uint32_t)(((i / STAGES) - 1) & 1));
@@ -349,132 +292,66 @@ lstm_fwd_step_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
       }
       __syncwarp();
     }
-  } else if (warp < 4) {
-    // ---- epilogue: lane = hidden unit u0 + lane (H % 32 == 0), the warp walks its 32 rows in batches of 8.  Kept
-    // small on purpose: the straight-line version of this loop overflowed the instruction cache (ncu: 29 % of the
-    // samples on stall_no_inst) and the cell costs more issue slots than the MMAs
-    const int u = u0 + lane;
-    const int row0 = m0 + warp * 32;
-    const int nrows = R - row0 < 32 ? R - row0 : 32;  // may be <= 0: nothing to do but the barriers
-    constexpr int RB = 8;
-    const unsigned H4 = 4u * (unsigned)H;
-    float b[4];
+    return;
+  }
+  // ---- consumers: MMA (per stage four instructions over 32 bytes of k each: 8 tf32 or 16 fp16 values; both kinds
+  // accumulate into the same fp32 registers), then the cell on the fragment
+  const int wgi = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+  float acc[64];
 #pragma unroll
-    for (int g = 0; g < 4; ++g) b[g] = b_ih[g * H + u] + b_hh[g * H + u];
-    const float* cp_ptr = C_prev ? C_prev + (size_t)row0 * H + u : nullptr;
-    float* g_ptr = G + (size_t)row0 * H4 + u;
-    float cp[RB], pz[FOLD ? 1 : RB][4];
-    auto load_rows = [&](int r0) {
-#pragma unroll
-      for (int j = 0; j < RB; ++j) {
-        const bool ok = r0 + j < nrows;
-        cp[j] = (ok && cp_ptr) ? (cp_ptr + (size_t)r0 * H)[j * H] : 0.f;
-        if (!FOLD) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) pz[j][g] = ok ? (g_ptr + (size_t)r0 * H4)[j * 4 * H + g * H] : 0.f;
-        }
-      }
-    };
-    load_rows(0);  // in flight while the main loop runs
-    mbar_wait<true>(&bars.acc_full, 0);
-    tc_fence_after();
-    // accumulator -> per-warp slab [gate][row][33] in the (now free) stage buffers, shared-space addresses
-    const uint32_t slab = smem_u32(smem) + (uint32_t)warp * (4 * 32 * 33 * 4);
-    const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      float v[4][8];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) tc_ld8(taddr + g * 32 + q * 8, v[q]);
-      tc_wait_ld();
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          asm volatile("st.shared.f32 [%0], %1;" ::"r"(slab + (uint32_t)(((g * 32 + lane) * 33 + q * 8 + j) * 4)), "f"(v[q][j]));
-    }
-    __syncwarp();
-    float* c_ptr = C_out + (size_t)row0 * H + u;
-    float* h_ptr = H_out + (size_t)row0 * H + u;
-    __half* h16_ptr = H16_out ? H16_out + (size_t)row0 * H + u : nullptr;
-#pragma unroll 1
-    for (int r0 = 0; r0 < 32; r0 += RB) {
-      float gi[RB], gf[RB], gg[RB], go[RB], cn[RB], hn[RB];
-#pragma unroll
-      for (int j = 0; j < RB; ++j) {
-        float z[4];
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float a;
-          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(a) : "r"(slab + (uint32_t)(((g * 32 + r0 + j) * 33 + lane) * 4)));
-          z[g] = FOLD ? a + b[g] : (pz[j][g] + b[g]) + a;
-        }
-        // ex2 + rcp forms (2 ulp class; the tf32 / fp16 products around them are 1e-3 class).  FSN_TRAIN_FAST_ACT=0
-        // selects the unfused GEMM + lstm_cell_fwd_kernel path with expf / IEEE division instead
-        gi[j] = sigmoid_mufu(z[0]); gf[j] = sigmoid_mufu(z[1]); gg[j] = tanh_mufu(z[2]); go[j] = sigmoid_mufu(z[3]);
-        cn[j] = fmaf(gf[j], cp[j], gi[j] * gg[j]);
-        hn[j] = go[j] * tanh_mufu(cn[j]);
-      }
-      // one base per array and batch, everything else an offset (immediate when HT != 0)
-      float* gr = g_ptr + (size_t)r0 * H4;
-      float* cr = c_ptr + (size_t)r0 * H;
-      float* hr = h_ptr + (size_t)r0 * H;
-      __half* h16r = h16_ptr + (size_t)r0 * H;
-      if (r0 + RB < 32) load_rows(r0 + RB);  // next batch in flight under this batch's stores
-      if (r0 + RB <= nrows) {                // whole batch inside the matrix: no per-row predicates
-#pragma unroll
-        for (int j = 0; j < RB; ++j) {
-          gr[j * 4 * H] = gi[j]; gr[j * 4 * H + H] = gf[j]; gr[j * 4 * H + 2 * H] = gg[j]; gr[j * 4 * H + 3 * H] = go[j];
-          cr[j * H] = cn[j];
-          hr[j * H] = hn[j];
-        }
-        if (h16_ptr) {
-#pragma unroll
-          for (int j = 0; j < RB; ++j) h16r[j * H] = __float2half_rn(hn[j]);  // next step's / next layer's MMA operand
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < RB; ++j) {
-          if (r0 + j < nrows) {
-            gr[j * 4 * H] = gi[j]; gr[j * 4 * H + H] = gf[j]; gr[j * 4 * H + 2 * H] = gg[j]; gr[j * 4 * H + 3 * H] = go[j];
-            cr[j * H] = cn[j];
-            hr[j * H] = hn[j];
-            if (h16_ptr) h16r[j * H] = __float2half_rn(hn[j]);
-          }
-        }
-      }
-    }
-  } else if (warp == 4) {
-    // MMA issue: per stage four instructions over 32 bytes of k each (8 tf32 or 16 fp16 values); both kinds accumulate
-    // into the same fp32 tile
-    const uint32_t idesc32 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-    const uint32_t idesc16 = (1u << 4) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  wg::fence_operand(acc);
+  {
     const uint32_t smem_base = smem_u32(smem);
     for (int i = 0; i < nk; ++i) {
       const int s = i % STAGES;
-      mbar_wait<false>(&bars.full[s], (uint32_t)((i / STAGES) & 1));
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_base + s * CF::STAGE_BYTES;
-        const uint32_t sb = sa + A_BYTES;
-        const bool half_blk = i < nkx ? (x16 != 0) : (h16 != 0);
+      mbar_wait_mma(&bars.full[s], (uint32_t)((i / STAGES) & 1));
+      const uint32_t sa = smem_base + s * CF::STAGE_BYTES + wgi * (64 * 128);
+      const uint32_t sb = smem_base + s * CF::STAGE_BYTES + A_BYTES;
+      const bool half_blk = i < nkx ? (x16 != 0) : (h16 != 0);
+      wg::fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          if (half_blk) tc_mma1_f16(tmem_base, desc_sw128(sa + kk * 32), desc_sw128(sb + kk * 32), idesc16, (i > 0 || kk > 0) ? 1u : 0u);
-          else          tc_mma1_tf32(tmem_base, desc_sw128(sa + kk * 32), desc_sw128(sb + kk * 32), idesc32, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        tc_commit1(&bars.empty[s]);
+      for (int kk = 0; kk < 4; ++kk) {
+        if (half_blk) wg::mma_f16_n128(acc, wg::desc_sw128(sa + kk * 32), wg::desc_sw128(sb + kk * 32), 1u);
+        else          wg::mma_tf32_n128(acc, wg::desc_sw128(sa + kk * 32), wg::desc_sw128(sb + kk * 32), 1u);
       }
-      __syncwarp();
+      wg::commit();
+      wg::wait<1>();
+      if (i > 0 && l == 0) mbar_arrive(&bars.empty[(i - 1) % STAGES]);
     }
-    if (elect_one()) tc_commit1(&bars.acc_full);
-    __syncwarp();
+    wg::wait<0>();
+    wg::fence_operand(acc);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(CF::TMEM_COLS));
+  const unsigned H4 = 4u * (unsigned)H;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int row = m0 + 64 * wgi + 16 * w + (l >> 2) + 8 * hh;
+    if (row >= R) continue;
+    float* gr = G + (size_t)row * H4;
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int u = u0 + 8 * jj + 2 * (l & 3) + e;
+        float z[4];
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          const float a = acc[4 * (g * 4 + jj) + 2 * hh + e];
+          const float b = b_ih[g * H + u] + b_hh[g * H + u];
+          z[g] = FOLD ? a + b : (gr[g * H + u] + b) + a;
+        }
+        // ex2 + rcp forms (2 ulp class; the tf32 / fp16 products around them are 1e-3 class).  FSN_TRAIN_FAST_ACT=0
+        // selects the unfused GEMM + lstm_cell_fwd_kernel path with expf / IEEE division instead
+        const float gi = sigmoid_mufu(z[0]), gf = sigmoid_mufu(z[1]), gg = tanh_mufu(z[2]), go = sigmoid_mufu(z[3]);
+        const float cp = C_prev ? C_prev[(size_t)row * H + u] : 0.f;
+        const float cn = fmaf(gf, cp, gi * gg);
+        const float hn = go * tanh_mufu(cn);
+        gr[u] = gi; gr[H + u] = gf; gr[2 * H + u] = gg; gr[3 * H + u] = go;
+        C_out[(size_t)row * H + u] = cn;
+        H_out[(size_t)row * H + u] = hn;
+        if (H16_out) H16_out[(size_t)row * H + u] = __float2half_rn(hn);  // next step's / next layer's MMA operand
+      }
+    }
   }
 }
 
@@ -523,6 +400,19 @@ static bool make_tmap16(CUtensorMap* m, const __half* base, int K, int rows, siz
          CUDA_SUCCESS;
 }
 
+constexpr int TGEMM_THREADS = tg::CONSUMERS + 32;      // TMA-fed kernels: two consumer warpgroups + producer warp
+constexpr int TGEMM_CP_THREADS = tg::CONSUMERS + 128;  // cp.async-fed kernel: producer warpgroup
+
+static int tgemm_sm_count() {
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return sms;
+}
+
 // fixed-order sum of split-K slabs (fsn_train.cu)
 int splitk_reduce_launch(const float* part, int S, int M, int N, float* C, size_t ldc, bool accumulate, cudaStream_t st);
 
@@ -533,7 +423,7 @@ bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, in
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    ok = (major == 10 && smem >= tg::Cfg<128>::SMEM && getenv("FSN_NO_TGEMM") == nullptr) ? 1 : 0;
+    ok = (major == 9 && smem >= tg::Cfg<128>::SMEM && getenv("FSN_NO_TGEMM") == nullptr) ? 1 : 0;
   }
   return ok == 1 && K >= 4 && (lda & 3) == 0 && (ldb & 3) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
          (reinterpret_cast<uintptr_t>(Bm) & 15) == 0;
@@ -544,7 +434,7 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
                  bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st) {
   if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
   FSN_REQUIRE(tgemm_supported(A, lda, Bm, ldb, K), FSN_ERR_UNSUPPORTED, "tgemm: operands must be 16-byte aligned rows");
-  static const int force_bn = getenv("FSN_TGEMM_BN") ? atoi(getenv("FSN_TGEMM_BN")) : 0;
+  static const int force_bn = getenv("FSN_TGEMM_BN") && atoi(getenv("FSN_TGEMM_BN")) == 128 ? 128 : 0;
   int BN = force_bn ? force_bn : ((N >= 256 && N % 256 == 0) ? 256 : 128);
   // a handful of tiles (per-step GEMMs of the full-band stack, 64 rows): narrow tiles + split-K so that the weight
   // matrix is streamed by ~64 CTAs instead of 2-8
@@ -554,14 +444,11 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
   // epilogue overlaps the other's main loop (measured 1081 -> 945 us at K = 384, 778 -> 522 us at K = 32 per 195 k rows)
   static const int smallk_bn = getenv("FSN_TGEMM_SMALLK_BN") ? atoi(getenv("FSN_TGEMM_SMALLK_BN")) : 128;
   if (!force_bn && K <= 512 && BN == 256 && cdiv(M, tg::BM) >= 1024) BN = smallk_bn == 256 ? 256 : 128;
-  // long-K, narrow output (weight gradients): the whole N extent in one CTA so the big A operand is read exactly once
-  static const bool wide = getenv("FSN_TGEMM_NO384") == nullptr;
-  if (!force_bn && wide && tmap_encoder() && scratch && K >= 65536 && N > 256 && N <= 384) BN = 384;
   const int tiles = cdiv(M, tg::BM) * cdiv(N, BN);
   int S = 1;
   if (scratch && K >= 8192 && tiles < 296) {
     // minimise waves(tiles * S) / S over the SM slots (1 or 2 resident CTAs per SM), slices of >= 2048 k
-    const int slots = 148 * (BN == 128 ? 2 : 1);  // resident CTAs
+    const int slots = tgemm_sm_count() * (BN == 128 ? 2 : 1);  // resident CTAs
     double best = 1e30;
     for (int s = 1; s <= 64 && s <= cdiv(K, 2048); ++s) {
       if ((size_t)s * M * N > scratch_floats) break;
@@ -595,25 +482,18 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
       if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                 tg::Cfg<128>::SMEM), "tgemm smem attr")))
         return rc;
-      if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<384>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                tg::Cfg<384>::SMEM), "tgemm smem attr")))
-        return rc;
       attr = true;
     }
-    if (BN == 384)
-      tg::tgemm_tma_kernel<384><<<grid, 160, tg::Cfg<384>::SMEM, st>>>(tmA, tmB, tmB2, dst, ldd, M, N, K, kps, acc,
-                                                                       (size_t)M * N, tg::BlockedOps{0, 0, 0, 0, 0});
-    else if (BN == 256)
-      tg::tgemm_tma_kernel<256><<<grid, 160, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, tmB2, dst, ldd, M, N, K, kps, acc,
+    if (BN == 256)
+      tg::tgemm_tma_kernel<256><<<grid, TGEMM_THREADS, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, tmB2, dst, ldd, M, N, K, kps, acc,
                                                                        (size_t)M * N, tg::BlockedOps{0, 0, 0, 0, 0});
     else
-      tg::tgemm_tma_kernel<128><<<grid, 160, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, tmB2, dst, ldd, M, N, K, kps, acc,
+      tg::tgemm_tma_kernel<128><<<grid, TGEMM_THREADS, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, tmB2, dst, ldd, M, N, K, kps, acc,
                                                                        (size_t)M * N, tg::BlockedOps{0, 0, 0, 0, 0});
     FSN_CHECK_LAUNCH("tgemm_tma_kernel");
     if (S > 1) return splitk_reduce_launch(scratch, S, M, N, C, ldc, accumulate, st);
     return FSN_OK;
   }
-  FSN_REQUIRE(BN != 384, FSN_ERR_CUDA, "tgemm: tensor-map encoding failed for the 128x384 tile");
   if (BN == 256) {
     static bool attr_by_dev[64] = {};  // the opt-in is per device
     int cur_dev_ = 0; cudaGetDevice(&cur_dev_); bool& attr = attr_by_dev[cur_dev_ & 63];
@@ -623,7 +503,7 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
         return rc;
       attr = true;
     }
-    tg::tgemm_kernel<256><<<grid, 160, tg::Cfg<256>::SMEM, st>>>(A, lda, Bm, ldb, dst, ldd, M, N, K, kps, acc,
+    tg::tgemm_kernel<256><<<grid, TGEMM_CP_THREADS, tg::Cfg<256>::SMEM, st>>>(A, lda, Bm, ldb, dst, ldd, M, N, K, kps, acc,
                                                                  (size_t)M * N);
   } else {
     static bool attr_by_dev[64] = {};  // the opt-in is per device
@@ -634,7 +514,7 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
         return rc;
       attr = true;
     }
-    tg::tgemm_kernel<128><<<grid, 160, tg::Cfg<128>::SMEM, st>>>(A, lda, Bm, ldb, dst, ldd, M, N, K, kps, acc,
+    tg::tgemm_kernel<128><<<grid, TGEMM_CP_THREADS, tg::Cfg<128>::SMEM, st>>>(A, lda, Bm, ldb, dst, ldd, M, N, K, kps, acc,
                                                                  (size_t)M * N);
   }
   FSN_CHECK_LAUNCH("tgemm_kernel");
@@ -704,11 +584,11 @@ int lstm_fwd_step_launch(const float* Hprev, const float* w_hh, const float* Xt,
 #define FSN_STEP_LAUNCH(FOLD, HT)                                                                                              \
   do {                                                                                                                         \
     if (stages == 2)                                                                                                           \
-      tg::lstm_fwd_step_kernel<FOLD, HT, 2><<<grid, 192, tg::StepCfg<2>::SMEM, st>>>(                                          \
+      tg::lstm_fwd_step_kernel<FOLD, HT, 2><<<grid, TGEMM_THREADS, tg::StepCfg<2>::SMEM, st>>>(                                          \
           tmA, tmB, tmX, tmWx, Gt, b_ih, b_hh, C_prev, C_out, H_out, h16 ? h->H16_out : nullptr, R, H, nkx, nkh, x16 ? 1 : 0,  \
           h16 ? 1 : 0);                                                                                                        \
     else                                                                                                                       \
-      tg::lstm_fwd_step_kernel<FOLD, HT, 3><<<grid, 192, tg::StepCfg<3>::SMEM, st>>>(                                          \
+      tg::lstm_fwd_step_kernel<FOLD, HT, 3><<<grid, TGEMM_THREADS, tg::StepCfg<3>::SMEM, st>>>(                                          \
           tmA, tmB, tmX, tmWx, Gt, b_ih, b_hh, C_prev, C_out, H_out, h16 ? h->H16_out : nullptr, R, H, nkx, nkh, x16 ? 1 : 0,  \
           h16 ? 1 : 0);                                                                                                        \
   } while (0)
@@ -731,7 +611,7 @@ __global__ void to_half_kernel(const float* __restrict__ in, size_t n, __half* _
 }  // namespace tg
 int to_half_launch(const float* in, size_t n, __half* out, cudaStream_t st) {
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > tgemm_sm_count() * 8) blocks = tgemm_sm_count() * 8;
   tg::to_half_kernel<<<blocks, 256, 0, st>>>(in, n, out);
   FSN_CHECK_LAUNCH("to_half_kernel");
   return FSN_OK;
@@ -814,11 +694,11 @@ int tgemm_blocked_launch(const float* Ablk, int nkb_a, int a_kb0, const float* B
   if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
   PFN_cuTensorMapEncodeTiled_v12000 fn = tmap_encoder();
   FSN_REQUIRE(fn, FSN_ERR_UNSUPPORTED, "tgemm_blocked: cuTensorMapEncodeTiled unavailable");
-  int BN = (N > 256 && N <= 384) ? 384 : ((N > 128 && N <= 256) || N % 256 == 0 ? 256 : 128);
+  int BN = (N > 128) ? 256 : 128;
   const int tiles = cdiv(M, tg::BM) * cdiv(N, BN);
   int S = 1;
   if (scratch && K >= 8192 && tiles < 296) {
-    const int slots = 148 * (BN == 128 ? 2 : 1);
+    const int slots = tgemm_sm_count() * (BN == 128 ? 2 : 1);
     double best = 1e30;
     for (int s = 1; s <= 64 && s <= cdiv(K, 2048); ++s) {
       if ((size_t)s * M * N > scratch_floats) break;
@@ -843,23 +723,20 @@ int tgemm_blocked_launch(const float* Ablk, int nkb_a, int a_kb0, const float* B
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS,
               FSN_ERR_CUDA, "tgemm_blocked: tensor-map encoding failed");
   int rc;
-  if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, tg::Cfg<384>::SMEM), "tgemm smem attr"))) return rc;
   if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, tg::Cfg<256>::SMEM), "tgemm smem attr"))) return rc;
   if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, tg::Cfg<128>::SMEM), "tgemm smem attr"))) return rc;
   const tg::BlockedOps bo{1, nkb_a, nkb_b, a_kb0, b_kb0};
-  if (BN == 384)
-    tg::tgemm_tma_kernel<384><<<grid, 160, tg::Cfg<384>::SMEM, st>>>(tmA, tmB, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
-  else if (BN == 256)
-    tg::tgemm_tma_kernel<256><<<grid, 160, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
+  if (BN == 256)
+    tg::tgemm_tma_kernel<256><<<grid, TGEMM_THREADS, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
   else
-    tg::tgemm_tma_kernel<128><<<grid, 160, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
+    tg::tgemm_tma_kernel<128><<<grid, TGEMM_THREADS, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
   FSN_CHECK_LAUNCH("tgemm_tma_kernel");
   if (S > 1) return splitk_reduce_launch(scratch, S, M, N, C, ldc, accumulate, st);
   return FSN_OK;
 }
 }  // namespace fsn
 
-// debug / unit-test entry point (tests/test_gpu_train.py): C[M,N] (+)= A[M,K] B[N,K]^T on the tcgen05 path
+// debug / unit-test entry point (tests/test_gpu_train.py): C[M,N] (+)= A[M,K] B[N,K]^T on the wgmma path
 extern "C" int fsn_debug_tgemm(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M,
                                int N, int K, int accumulate, float* scratch, int64_t scratch_floats,
                                fsn_stream_t stream) {

@@ -109,7 +109,7 @@ static int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, si
   if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
   const int tiles = cdiv(M, 64) * cdiv(N, 64);
   int S = 1;
-  if (scratch && K >= 4096 && tiles < 592) {  // fill 148 SMs x 4 CTAs; slices of >= 1024 k
+  if (scratch && K >= 4096 && tiles < 528) {  // fill 132 SMs x 4 CTAs; slices of >= 1024 k
     S = cdiv(592, tiles);
     if (S > cdiv(K, 1024)) S = cdiv(K, 1024);
     while (S > 1 && (size_t)S * M * N > SPLITK_SCRATCH_FLOATS) --S;
@@ -604,7 +604,7 @@ static int layer_forward_save(const fsn_seq_weights* w, int l, const float* X, i
 }
 
 // tensor-core variant.  Default: ONE kernel per step (lstm_fwd_step_kernel, fsn_tgemm.cu): [x_t | h_{t-1}] [W_ih | W_hh]^T on
-// tcgen05 and the cell in its epilogue, gates / cell / hidden saved.  Fallbacks, step by step: a layer input whose rows
+// wgmma and the cell on its accumulators, gates / cell / hidden saved.  Fallbacks, step by step: a layer input whose rows
 // are not 16-byte aligned keeps a hoisted projection of all steps (one GEMM into the gate buffer) that the step kernel
 // adds; with the fused kernel switched off (or H % 32 != 0) every step is a recurrent GEMM into `rec` + lstm_cell_fwd_kernel
 int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp,
@@ -633,10 +633,10 @@ int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R
   }
   const size_t n = (size_t)R * H;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   for (int t = 0; t < Tp; ++t) {
     float* Gt = s.G + (size_t)t * R * 4 * H;
-    if (fused && (t > 0 || fold)) {  // GEMM + cell in one kernel, the recurrent product stays in TMEM
+    if (fused && (t > 0 || fold)) {  // GEMM + cell in one kernel, the recurrent product stays in registers
       LstmStepHalf hs{nullptr, nullptr, nullptr, nullptr, nullptr};
       if (h16) {
         hs.Hprev16 = t > 0 ? half->H16 + (size_t)(t - 1) * R * H : nullptr;
@@ -691,7 +691,7 @@ static int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_abov
   p.dout = dout; p.fc_w = fc_w; p.O = O;
   const size_t n = (size_t)L.R * L.H;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   lstm_bwd_point_kernel<<<blocks, 256, 0, st>>>(p);
   FSN_CHECK_LAUNCH("lstm_bwd_point_kernel");
   int rc;
@@ -807,7 +807,7 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
     train_frame_sum_kernel<<<cdiv(Tp * B, 8), 256, 0, st>>>(w.raw, B, F, Tp, w.fs);
     FSN_CHECK_LAUNCH("train_frame_sum_kernel");
     if ((rc = cum_clip_scale_launch(w.fs, B, Tp, F, cum_eps, w.cum1, st))) return rc;
-    train_scale_tm_kernel<<<148 * 8, 256, 0, st>>>(w.raw, w.cum1, F, (size_t)Tp * B * F, w.xfb);
+    train_scale_tm_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.cum1, F, (size_t)Tp * B * F, w.xfb);
     FSN_CHECK_LAUNCH("train_scale_tm_kernel");
   }
   // full-band stack + Linear/activation (model.py:92-95)
@@ -832,7 +832,7 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   if (cum && (rc = cum_unit_scale_launch(w.raw, w.fbz, map, m.R, Tp, d->sb_num_neighbors, d->fb_num_neighbors, cum_eps, w.cum2,
                                          st, /*time_major=*/true)))
     return rc;
-  train_gather_kernel<<<148 * 8, 256, 0, st>>>(w.raw, w.fbz, w.inv2, cum ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,
+  train_gather_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.fbz, w.inv2, cum ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,
                                                d->sb_num_neighbors, d->fb_num_neighbors);
   FSN_CHECK_LAUNCH("train_gather_kernel");
   if (tc_sb) {
@@ -892,7 +892,7 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   const int Tp = m.Tp, F = m.F, R = m.R, Hf = d->fb_hidden, Hs = d->sb_hidden, K = m.Ksb;
   RowMap map{B, F, m.Fsub, m.G};
   // ---- sub-band Linear (model.py:129-135 backwards)
-  train_dout_kernel<<<148 * 8, 256, 0, st>>>(dcrm, w.dout, R, m.Fsub, T, Tp, d->look_ahead);
+  train_dout_kernel<<<132 * 8, 256, 0, st>>>(dcrm, w.dout, R, m.Fsub, T, Tp, d->look_ahead);
   FSN_CHECK_LAUNCH("train_dout_kernel");
   {  // dW of the 2-output Linear: one streaming pass over h1 (2.4 GB at config 3)
     const size_t rows = (size_t)Tp * R;
@@ -944,12 +944,12 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
     train_cum_unit_bwd_kernel<<<cdiv(R, 128), 128, 0, st2>>>(w.dxsb, w.xsb, w.cum2, Tp, R, K, w.dunit);
     FSN_CHECK_LAUNCH("train_cum_unit_bwd_kernel");
-    train_dfbz_cum_kernel<<<148 * 8, 256, 0, st2>>>(w.dunit, w.fbz, map, Tp, R, d->fb_activation, w.dz);
+    train_dfbz_cum_kernel<<<132 * 8, 256, 0, st2>>>(w.dunit, w.fbz, map, Tp, R, d->fb_activation, w.dz);
     FSN_CHECK_LAUNCH("train_dfbz_cum_kernel");
   } else {
     train_dot_kernel<<<B, 256, 0, st2>>>(w.dxsb, w.xsb, Tp, R, m.Fsub, K, w.dot);
     FSN_CHECK_LAUNCH("train_dot_kernel");
-    train_dfbz_kernel<<<148 * 8, 256, 0, st2>>>(w.dxsb, w.fbz, w.inv2, w.dot, map, Tp, R, K, (float)F * K * Tp,
+    train_dfbz_kernel<<<132 * 8, 256, 0, st2>>>(w.dxsb, w.fbz, w.inv2, w.dot, map, Tp, R, K, (float)F * K * Tp,
                                                 d->fb_activation, w.dz);
     FSN_CHECK_LAUNCH("train_dfbz_kernel");
   }

@@ -69,7 +69,7 @@ class Model(BaseModel):
         self.norm = self.norm_wrapper(norm_type)
         # arithmetic: 'fp32' (FMA kernels) | 'f16x3_tc' (tensor cores, hi+lo split operands, the fp32 error class) |
         # 'f16_tc' (tensor cores, single pass, ~1e-4) | 'auto' = f16x3_tc when the shape allows, else fp32.  The
-        # tensor-core modes run the bottleneck on the tcgen05 pair kernel and the encoder / decoder LSTMs + Linears
+        # tensor-core modes run the bottleneck on the wgmma sub-band kernel and the encoder / decoder LSTMs + Linears
         # on the hoisted-GEMM + persistent-recurrence kernels (fsn_lstm_rec_tc.cu)
         self.precision = precision or os.environ.get("FSN_PRECISION", "auto")
         self._packed = None

@@ -98,12 +98,12 @@ class Model(BaseModel):
         self.num_groups_in_drop_band = num_groups_in_drop_band
         # arithmetic of the sub-band stack (99 % of the FLOPs):
         #   "fp32"     fp32 FMA kernels
-        #   "f16x3_tc" tcgen05, fp16 hi+lo split of weights and state, 3 MMAs per product: the fp32 error class
+        #   "f16x3_tc" wgmma, fp16 hi+lo split of weights and state, 3 MMAs per product: the fp32 error class
         #              (cRM ~1e-6 rel, waveform <= 1e-4 abs even where decompress_cIRM amplifies x100)
-        #   "f16_tc"   tcgen05, single fp16 pass: 3x faster, cRM within 1e-3 rel; opt-in
+        #   "f16_tc"   wgmma, single fp16 pass: about 2x faster, cRM within 1e-3 rel; opt-in
         #   "auto"     f16x3_tc when the shape allows, else fp32 -- the default never trades the reference's accuracy
         self.precision = precision or os.environ.get("FSN_PRECISION", "auto")
-        # arithmetic of the training step's GEMMs: "fp32" (FMA) or "tf32_tc" (tcgen05 kind::tf32); the reference
+        # arithmetic of the training step's GEMMs: "fp32" (FMA) or "tf32_tc" (wgmma tf32); the reference
         # trains under fp16 autocast (trainer.py:56), so both are at least its precision
         self.train_precision = os.environ.get("FSN_TRAIN_PRECISION", "auto")
         self._packed = None

@@ -57,7 +57,7 @@ class Model(BaseModel):
             # model.py:226-236 also offers cumulative_laplace_norm / offline_gaussian_norm
             raise NotImplementedError("libfsn_b200 builds offline_laplace_norm for improved_fullsubnet")
         self.norm_type = norm_type
-        # arithmetic of the sub-band sections (98 % of the FLOPs): "fp32" (FMA kernels), "tf32_tc" (tcgen05 kind::tf32
+        # arithmetic of the sub-band sections (98 % of the FLOPs): "fp32" (FMA kernels), "tf32_tc" (wgmma tf32
         # GEMMs, fp32 accumulate; waveform within 1e-4 of the reference) or "auto" (= tf32_tc when sb_hidden % 4 == 0)
         self.precision = os.environ.get("FSN_IMPROVED_PRECISION", "auto")
 

@@ -20,5 +20,5 @@ def initialize_module(path: str, args: Optional[dict] = None, initialize: bool =
 
 def prepare_device(n_gpu: int, keep_reproducibility=False):
     if n_gpu == 0:
-        raise RuntimeError("fullsubnet_b200 has no CPU path: a CUDA device (B200) is required.")
+        raise RuntimeError("fullsubnet_b200 has no CPU path: a CUDA device (H100) is required.")
     return torch.device("cuda:0")

@@ -1,5 +1,5 @@
 /*
- * fsn_b200.h - C ABI of libfsn_b200.so: the B200 (sm_100a) implementation of FullSubNet's
+ * fsn_b200.h - C ABI of libfsn_b200.so: the H100 (sm_90a) implementation of FullSubNet's
  * enhancement hot path (SURVEY.md section 8).
  *
  * The reference (Audio-WestlakeU/FullSubNet) is pure Python and has no FFI; its "operator"
@@ -49,12 +49,12 @@ enum { FSN_CELL_LSTM = 0, FSN_CELL_GRU = 1 };
 /* arithmetic of the sub-band LSTM stack (99 % of the FLOPs):
  *   FSN_PREC_FP32     - fp32 FMA everywhere (bit-for-bit class of the reference CPU path, ~1e-6)
  *   FSN_PREC_TF32_TC  - training step only (fsn_train_*): every GEMM of the forward, of back-propagation through
- *                       time and of the weight gradients on tcgen05 kind::tf32 (fp32 data read as tf32, fp32
- *                       accumulate in TMEM); gate / cell arithmetic and all reductions stay fp32
+ *                       time and of the weight gradients on wgmma tf32 (fp32 data read as tf32, fp32
+ *                       accumulate); gate / cell arithmetic and all reductions stay fp32
  *   FSN_PREC_F16_TC   - fp16 operands (11-bit significand, like TF32) x fp32 accumulate on the
- *                       tcgen05 tensor cores, fp32 cell state; cRM within 1e-3 rel (tests)
+ *                       wgmma tensor cores, fp32 cell state; cRM within 1e-3 rel (tests)
  *   FSN_PREC_F16X3_TC - error-compensated tensor-core path: weights and state split into fp16 hi + lo terms, every
- *                       product issued as W_hi.S_hi + W_hi.S_lo + W_lo.S_hi into one fp32 TMEM accumulator (22
+ *                       product issued as W_hi.S_hi + W_hi.S_lo + W_lo.S_hi into one fp32 accumulator (22
  *                       significand bits per operand), libm-class gate functions; the fp32 error class (cRM ~1e-6
  *                       rel), needed where decompress_cIRM amplifies mask errors x100 (|cRM| near the 9.9 clip) */
 enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F16X3_TC = 3 };
@@ -138,7 +138,7 @@ typedef struct fsn_seq_weights {
 size_t fsn_model_workspace_bytes(const fsn_model_desc* d, int B, int T);
 
 /* FSN_PREC_F16_TC / FSN_PREC_F16X3_TC only: bytes of, and packer for, the tile-ordered fp16 image of the sub-band
- * weights that the tcgen05 kernel streams (cache it keyed on the parameters' version AND the precision: the
+ * weights that the tensor-core kernel streams (cache it keyed on the parameters' version AND the precision: the
  * compensated image carries a hi and a lo stage per k range). */
 size_t fsn_sb_packed_bytes(const fsn_model_desc* d);
 int fsn_pack_sb_weights(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed, fsn_stream_t stream);
@@ -230,7 +230,7 @@ typedef struct fsn_improved_desc {
   int32_t sb_num_center[FSN_IMP_MAX_SECTIONS], sb_num_neighbor[FSN_IMP_MAX_SECTIONS];
   int32_t fb_num_center[FSN_IMP_MAX_SECTIONS], fb_num_neighbor[FSN_IMP_MAX_SECTIONS];
   int32_t fb_hidden, sb_hidden, fb_activation, sb_activation;
-  int32_t precision; /* FSN_PREC_FP32, or FSN_PREC_TF32_TC: the sub-band sections' GEMMs on tcgen05 kind::tf32 */
+  int32_t precision; /* FSN_PREC_FP32, or FSN_PREC_TF32_TC: the sub-band sections' GEMMs on wgmma tf32 */
 } fsn_improved_desc;
 
 typedef struct fsn_improved_weights {
@@ -351,7 +351,7 @@ int fsn_debug_row_to_unit(int B, int F, int G, int r, int* b, int* f);
 int fsn_debug_unit_to_row(int B, int F, int G, int b, int f);
 int fsn_debug_reflect_count(int r, int F, int N);
 
-/* unit-test hook for the tf32 tcgen05 GEMM of the training path: C[M,N] (+)= A[M,K] B[N,K]^T, fp32 row-major
+/* unit-test hook for the tf32 wgmma GEMM of the training path: C[M,N] (+)= A[M,K] B[N,K]^T, fp32 row-major
  * operands with 16-byte aligned rows; scratch (optional) enables split-K */
 int fsn_debug_tgemm(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N,
                     int K, int accumulate, float* scratch, int64_t scratch_floats, fsn_stream_t stream);
@@ -374,7 +374,7 @@ int fsn_debug_lstm_fwd_step(const float* h_prev, const float* w_hh, const float*
 
 /* unit-test hooks for the tensor-core LSTM layer of the full-band stacks (fsn_lstm_rec_tc.cu;
  * audio_zen/model/module/sequence_model.py:52-58,117): hall[r,t,:] of nn.LSTM(K -> H, 1 layer) over x [R,T,K]
- * (hoisted input-projection GEMM + persistent tcgen05 recurrence), and out = act(x W^T + b) for x [rows,K], W [N,K];
+ * (hoisted input-projection GEMM + persistent wgmma recurrence), and out = act(x W^T + b) for x [rows,K], W [N,K];
  * x3 != 0 selects the compensated (fp32-class) arithmetic.  Workspace of the Linear hook: the LSTM one with
  * R*T = rows, H = max(8, ceil(N/4)). */
 size_t fsn_debug_lstm_tc_workspace_bytes(int R, int T, int K, int H, int x3);

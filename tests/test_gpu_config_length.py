@@ -33,7 +33,7 @@ def check_fp(y, fp):
 def test_fullsubnet_4s_clip_both_weight_sets(golden, dev, tag, gain, precision, crm_tol):
     from fullsubnet_b200.fullsubnet.model import Model
     from oracle import fullsubnet_oracle as O
-    g = golden("model_full_4s")
+    g = {**golden("model_full_4s_wa"), **golden("model_full_4s_wb")}
     y = O.make_noisy(1, 64000, seed=40, speechlike=True)
     check_fp(y, g["y_fp"])
     m = Model(**O.DEFAULT_MODEL_ARGS, precision=precision)
@@ -50,7 +50,7 @@ def test_fullsubnet_4s_single_pass_f16_mask_gate(golden, dev):
     """The opt-in single-pass mode at T = 251: cRM gate on both weight sets, waveform gate on W-a."""
     from fullsubnet_b200.fullsubnet.model import Model
     from oracle import fullsubnet_oracle as O
-    g = golden("model_full_4s")
+    g = {**golden("model_full_4s_wa"), **golden("model_full_4s_wb")}
     y = O.make_noisy(1, 64000, seed=40, speechlike=True).to(dev)
     for tag, gain in (("wa", 1.0), ("wb", WB_GAIN)):
         m = Model(**O.DEFAULT_MODEL_ARGS, precision="f16_tc")

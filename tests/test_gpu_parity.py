@@ -306,7 +306,7 @@ def test_cumulative_laplace_norm_matches_reference(golden, dev):
         assert rel_max(m(mag).cpu(), g["small_g2"]) < 2e-5  # B=3: drop_band + per-unit running means
     full = dict(O.DEFAULT_MODEL_ARGS, norm_type="cumulative_laplace_norm")
     for prec, tol in (("fp32", 5e-5), ("auto", 5e-5), ("f16_tc", CRM_TOL)):
-        # auto = the compensated tensor-core path: per-step unit scales inside the tcgen05 gather warp
+        # auto = the compensated tensor-core path: per-step unit scales inside the tensor-core gather warp
         mf = make_model(full, O.make_state_dict(seed=0, args=full, sb_fc_gain=60.0), dev, prec)
         if prec == "auto":
             assert mf._resolve_precision() == "f16x3_tc"
@@ -450,22 +450,3 @@ def test_batched_file_loop_matches_reference_host_loop(dev, tmp_path):
     _lib.check(_lib.load().fsn_peak_normalize_int16(enh.data_ptr(), 3, 6000, 0.8 * 32767.0, pcm2.data_ptr(),
                                                     torch.cuda.current_stream().cuda_stream))
     assert torch.equal(pcm, pcm2) and torch.equal(enh, m.enhance(y))
-
-
-def test_cluster_kernel_variant_in_a_subprocess(dev):
-    """The experimental 6-CTA-cluster sub-band kernel (FSN_TC_CLUSTER4=1, read once per process; precision f16_tc):
-    cRM within the mask gate of the fp32 kernels at 4 s, incl. a batch that spans several clusters and a partial one."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, FSN_TC_CLUSTER4="1")
-    out = subprocess.run([sys.executable, os.path.join(root, "tools", "tc4_check.py"), "3", "64000"], env=env, capture_output=True,
-                         text=True, timeout=300)
-    assert out.returncode == 0, out.stderr[-2000:]
-    line = [l for l in out.stdout.splitlines() if l.startswith("B=3")][-1]
-    assert "cluster4=1" in line and "finite True" in line, line
-    crm_err = float(line.split("cRM max-rel ")[1].split()[0])
-    l2_err = float(line.split("rel-l2 ")[1].split(";")[0])
-    wav_err = float(line.split("wav max-abs ")[1].split(";")[0])
-    assert crm_err < CRM_TOL and l2_err < CRM_TOL and wav_err < WAV_TOL, line

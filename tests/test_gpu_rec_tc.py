@@ -1,5 +1,5 @@
 """GPU: the tensor-core LSTM layer / Linear layer of the full-band stacks (fsn_lstm_rec_tc.cu: hoisted tf32 GEMM +
-persistent tcgen05 recurrence) against float64 torch on the CPU (audio_zen/model/module/sequence_model.py:52-58,117).
+persistent wgmma recurrence) against float64 torch on the CPU (audio_zen/model/module/sequence_model.py:52-58,117).
 x3 = compensated arithmetic (fp32 error class), single pass = fp16/tf32 operands (~1e-3)."""
 import numpy as np
 import pytest

@@ -188,7 +188,7 @@ def test_trainer_step_and_checkpoint_roundtrip(golden, dev, tmp_path):
 
 
 def test_tf32_tensor_core_gemm_matches_truncated_reference(dev):
-    """fsn_debug_tgemm: C (+)= A B^T on tcgen05 kind::tf32 == fp64 GEMM of the tf32-truncated operands."""
+    """fsn_debug_tgemm: C (+)= A B^T on wgmma tf32 == fp64 GEMM of the tf32-truncated operands."""
     from fullsubnet_b200 import _lib
     lib = _lib.load()
 

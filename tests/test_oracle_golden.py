@@ -259,7 +259,7 @@ def _fingerprint(y):
 
 def test_oracle_at_config_length_4s(golden):
     """T = 251 (BASELINE configs 0/1 clip length), both weight sets: oracle vs the unmodified reference."""
-    g = golden("model_full_4s")
+    g = {**golden("model_full_4s_wa"), **golden("model_full_4s_wb")}
     y = O.make_noisy(1, 64000, seed=40, speechlike=True)
     assert np.allclose(_fingerprint(y), g["y_fp"], rtol=0, atol=1e-9)
     torch.set_num_threads(8)

@@ -1,4 +1,4 @@
-"""Diagnostic (GPU): compare the tcgen05 sub-band path against the fp32 path on a tiny case."""
+"""Diagnostic (GPU): compare the tensor-core sub-band path against the fp32 path on a tiny case."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

@@ -1,4 +1,4 @@
-"""Times the tf32 tcgen05 GEMM on the shapes of the training step (config 3): python tools/tgemm_shapes.py
+"""Times the tf32 wgmma GEMM on the shapes of the training step (config 3): python tools/tgemm_shapes.py
 (FSN_TGEMM_BN / FSN_TGEMM_SMALLK_BN select tile widths per process)."""
 import sys
 

@@ -1,4 +1,4 @@
-"""Checks the tf32 tcgen05 GEMM (fsn_debug_tgemm) against an exact tf32-truncated reference and times it."""
+"""Checks the tf32 wgmma GEMM (fsn_debug_tgemm) against an exact tf32-truncated reference and times it."""
 import ctypes as C
 import sys
 
