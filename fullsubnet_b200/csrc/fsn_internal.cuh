@@ -171,6 +171,7 @@ struct SbTcArgs {
   int steps, shrink;      // LSTM steps (0 = Tp) and time down-sampling of the gathered input (0/1 = none)
   bool x3;                // error-compensated variant (FSN_PREC_F16X3_TC image)
   RowMap map;
+  int stages, cluster;    // weight ring depth (2..4) and CTAs per cluster (1, 2, 4); 0 = FSN_TC_STAGES / FSN_TC_CLUSTER
 };
 size_t sb_tc_packed_bytes(const fsn_model_desc* d);
 size_t sb_tc_packed_bytes_raw(int H, bool x3);

@@ -601,15 +601,62 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
     if (stages_env < 2) stages_env = 2;
     if (stages_env > tc::MAX_STAGES) stages_env = tc::MAX_STAGES;
   }
-  a.stages = stages_env;
   static int cluster_env = -1;
   if (cluster_env < 0) {
     const char* e = getenv("FSN_TC_CLUSTER");
     cluster_env = e ? atoi(e) : 2;
     if (cluster_env != 1 && cluster_env != 2 && cluster_env != 4) cluster_env = 2;
   }
-  a.cluster = cluster_env;
+  // an explicit launch configuration (the unit-test hook) overrides the environment
+  a.stages = s.stages ? s.stages : stages_env;
+  a.cluster = s.cluster ? s.cluster : cluster_env;
   return s.x3 ? sb_tc_launch<true>(a, s.H, st) : sb_tc_launch<false>(a, s.H, st);
 }
 
 }  // namespace fsn
+
+// unit-test hook (tests/test_gpu_subband_tc.py): the sub-band stack on caller-provided inputs and launch configuration
+extern "C" size_t fsn_debug_sb_lstm_tc_packed_bytes(int H, int x3) {
+  return fsn::sb_tc_shape_ok(H, 0) ? fsn::sb_tc_packed_bytes_raw(H, x3 != 0) : 0;
+}
+
+extern "C" int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
+                                    const float* magT, const float* fbT, int B, int F, int src_T, int G,
+                                    const float* inv2, const float* unit_scale, int la, int steps, int shrink, int stages,
+                                    int cluster, void* packed, float* crm, fsn_stream_t stream) {
+  using namespace fsn;
+  // every check precedes the first CUDA call
+  FSN_REQUIRE(cluster == 0 || cluster == 1 || cluster == 2 || cluster == 4, FSN_ERR_UNSUPPORTED,
+              "sb_lstm_tc: cluster size %d (0, 1, 2 or 4)", cluster);
+  FSN_REQUIRE(stages == 0 || (stages >= 2 && stages <= tc::MAX_STAGES), FSN_ERR_UNSUPPORTED,
+              "sb_lstm_tc: ring depth %d (0, 2, 3 or 4)", stages);
+  FSN_REQUIRE(sb && magT && fbT && inv2 && packed && crm, FSN_ERR_SHAPE, "sb_lstm_tc: missing buffer");
+  FSN_REQUIRE(B > 0 && F > 1 && src_T > 0 && Ns >= 0 && Nf >= 0 && Ns < F && Nf < F, FSN_ERR_SHAPE,
+              "sb_lstm_tc: bad shape B=%d F=%d src_T=%d Ns=%d Nf=%d", B, F, src_T, Ns, Nf);
+  FSN_REQUIRE(fc_out == 1 || fc_out == 2, FSN_ERR_SHAPE, "sb_lstm_tc: fc_out %d (1 or 2)", fc_out);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "sb_lstm_tc: activation %d", act);
+  FSN_REQUIRE(shrink >= 1 && G >= 1, FSN_ERR_SHAPE, "sb_lstm_tc: shrink %d / groups %d", shrink, G);
+  // drop_band as make_dims applies it
+  const int g = (B > 1 && G > 1) ? G : 1;
+  FSN_REQUIRE(B == 1 || B > G, FSN_ERR_SHAPE, "sb_lstm_tc: batch size %d <= num_groups %d", B, G);
+  const int Fsub = g > 1 ? F / g : F;
+  FSN_REQUIRE(Fsub > 0, FSN_ERR_SHAPE, "sb_lstm_tc: num_freqs < num_groups");
+  // steps read frames [0, steps) of the source, or with shrink > 1 frame 0 then blocks of `shrink` frames
+  const int max_steps = shrink > 1 ? 1 + cdiv(src_T - 1, shrink) : src_T;
+  FSN_REQUIRE(steps > 0 && steps <= max_steps && la >= 0 && la < steps, FSN_ERR_SHAPE,
+              "sb_lstm_tc: steps %d / look-ahead %d for %d source frames (shrink %d)", steps, la, src_T, shrink);
+  FSN_REQUIRE(!(unit_scale && shrink > 1), FSN_ERR_UNSUPPORTED, "sb_lstm_tc: per-step scales with time down-sampling");
+  FSN_REQUIRE(sb_tc_shape_ok(H, (2 * Ns + 1) + (2 * Nf + 1)), FSN_ERR_UNSUPPORTED,
+              "sb_lstm_tc: unsupported hidden size %d / input width %d", H, (2 * Ns + 1) + (2 * Nf + 1));
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = sb_tc_pack_raw(sb, H, (2 * Ns + 1) + (2 * Nf + 1), fc_out, packed, st, x3 != 0);
+  if (rc) return rc;
+  SbTcArgs a;
+  memset(&a, 0, sizeof(a));
+  a.packed = packed; a.magT = magT; a.fbT = fbT; a.inv2 = inv2; a.unit_scale = unit_scale; a.crm = crm;
+  a.B = B; a.F = F; a.Tp = src_T; a.la = la; a.Ns = Ns; a.Nf = Nf; a.H = H; a.act = act;
+  a.steps = steps; a.shrink = shrink; a.x3 = x3 != 0;
+  a.map = RowMap{B, F, Fsub, g};
+  a.stages = stages; a.cluster = cluster;
+  return sb_tc_forward(a, st);
+}

@@ -384,6 +384,20 @@ int fsn_debug_lstm_layer_tc(const float* w_ih, const float* w_hh, const float* b
 int fsn_debug_linear_tc(const float* x, int rows, int K, const float* W, const float* bias, int N, int act, int x3,
                         float* out, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
+/* unit-test hook for the sub-band tensor-core stack (fsn_subband_tc.cu; model.py:98-135): packs sb (2 LSTM layers of
+ * hidden size H over Ksb = (2Ns+1)+(2Nf+1) inputs, Linear(H -> fc_out <= 2)) into `packed`
+ * (fsn_debug_sb_lstm_tc_packed_bytes, 0 = unsupported H) and runs the stack on magT, fbT [B, src_T, F] (time-major):
+ * unit (b', f') of the drop_band map (G groups, as Model.forward applies them) gathers the reflected rows of its source
+ * clip, scaled by inv2[clip] or, when unit_scale [steps, B*Fsub] is given, by unit_scale[t*R + r]; shrink > 1
+ * down-samples time like fast_fullsubnet.  crm [B, 2, Fsub, steps - la] receives act(Linear) of steps la..steps-1
+ * (outputs beyond fc_out are act(0)).  stages (2..4) and cluster (1, 2, 4) choose the launch configuration, 0 = the
+ * FSN_TC_STAGES / FSN_TC_CLUSTER default.  Arguments are checked before any CUDA call. */
+size_t fsn_debug_sb_lstm_tc_packed_bytes(int H, int x3);
+int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
+                         const float* magT, const float* fbT, int B, int F, int src_T, int G,
+                         const float* inv2, const float* unit_scale, int la, int steps, int shrink,
+                         int stages, int cluster, void* packed, float* crm, fsn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
