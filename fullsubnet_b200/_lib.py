@@ -35,7 +35,7 @@ class LstmLayer(C.Structure):
 class FastDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "num_freqs", "look_ahead", "shrink_size", "num_mels", "enc1_hidden", "enc2_hidden", "bn_hidden", "bn_layers",
-        "dec_hidden", "noisy_num_neighbors", "enc_num_neighbors", "precision")]
+        "dec_hidden", "noisy_num_neighbors", "enc_num_neighbors", "precision", "cell_type")]
 
 
 class FastWeights(C.Structure):
@@ -48,6 +48,16 @@ class FastWeights(C.Structure):
 class SeqGrads(C.Structure):
     _fields_ = [("w_ih", C.c_void_p * 2), ("w_hh", C.c_void_p * 2), ("b_ih", C.c_void_p * 2),
                 ("b_hh", C.c_void_p * 2), ("fc_w", C.c_void_p), ("fc_b", C.c_void_p)]
+
+
+class LstmGrads(C.Structure):
+    _fields_ = [("w_ih", C.c_void_p), ("w_hh", C.c_void_p), ("b_ih", C.c_void_p), ("b_hh", C.c_void_p)]
+
+
+class FastGrads(C.Structure):
+    _fields_ = [("enc1", LstmGrads), ("enc2", LstmGrads), ("enc_fc_w", C.c_void_p), ("enc_fc_b", C.c_void_p),
+                ("bn", LstmGrads * 2), ("bn_fc_w", C.c_void_p), ("bn_fc_b", C.c_void_p),
+                ("dec1", LstmGrads), ("dec2", LstmGrads), ("dec_fc_w", C.c_void_p), ("dec_fc_b", C.c_void_p)]
 
 
 MAX_PARAM_TENSORS = 64
@@ -113,6 +123,10 @@ _SIGNATURES = {
                                     _P, _S, _P]),
     "fsn_train_backward": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _I, _I,
                                      C.POINTER(SeqGrads), C.POINTER(SeqGrads), _P, _S, _P]),
+    "fsn_fast_train_workspace_bytes": (_S, [C.POINTER(FastDesc), _I, _I]),
+    "fsn_fast_train_forward": (C.c_int, [C.POINTER(FastDesc), C.POINTER(FastWeights), _P, _I, _I, _P, _P, _S, _P]),
+    "fsn_fast_train_backward": (C.c_int, [C.POINTER(FastDesc), C.POINTER(FastWeights), _P, _I, _I, C.POINTER(FastGrads), _P,
+                                          _S, _P]),
     "fsn_mse_loss_scratch_bytes": (_S, []),
     "fsn_mse_loss": (C.c_int, [_P, _P, _I, _I, _I, _P, _P, _P, _S, _P]),
     "fsn_clip_adam_scratch_bytes": (_S, []),

@@ -80,8 +80,6 @@ __global__ void fast_output_kernel(const float* __restrict__ dec, int B, int Tp,
   }
 }
 
-struct FastDims { int B, T, Tp, F, M, K, Ts, S; };
-
 static bool fast_tc_ok(const fsn_fast_desc* d) {
   const int K = (2 * d->noisy_num_neighbors + 1) + (2 * d->enc_num_neighbors + 1);
   return d->bn_hidden == 384 && d->bn_layers == 2 && K <= 32;
@@ -119,7 +117,7 @@ struct FCarver {
   }
 };
 
-static int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m) {
+int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m) {
   FSN_REQUIRE(d && d->num_freqs > 1 && d->num_mels > 1 && d->shrink_size >= 1 && d->look_ahead >= 0, FSN_ERR_SHAPE,
               "fast model: bad descriptor");
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "fast model: empty input (B=%d, T=%d)", B, T);

@@ -1,0 +1,475 @@
+// Training step of fast_fullsubnet (recipes/dns_interspeech_2020/fast_fullsubnet/trainer.py:45-56, model.py:143-202):
+//   fsn_fast_train_forward   Model.forward in train mode, keeping what back-propagation through time needs
+//   fsn_fast_train_backward  Linear(2F) -> decoder BPTT -> up-sampling transpose -> ReLU' -> bottleneck BPTT -> second
+//                            norm + down-sampling + unfold (closed form, gather) -> ReLU' -> Linear(M) -> encoder BPTT;
+//                            weight gradients of every LSTM layer through layer_weight_grads (fsn_train.cu)
+// Everything is time-major ([Tp, rows, .], the bottleneck [Ts, B*M, .]) like fsn_train.cu, so the LSTM layers reuse its
+// activation-saving forward, its per-step backward and its weight-gradient GEMMs.  Every reduction runs in a fixed order:
+// two runs give identical bits.  oracle/fast_fullsubnet_oracle.py:fast_model_forward under CPU autograd is the reference.
+#include <string.h>
+
+#include "fsn_internal.cuh"
+
+namespace fsn {
+
+// ------------------------------------------------------------------------------------------ forward kernels
+// mag [B,F,T] -> magT [Tp,B,F], zero look-ahead frames (model.py:161)
+__global__ void ftr_transpose_kernel(const float* __restrict__ mag, float* __restrict__ magT, int B, int F, int T, int Tp) {
+  __shared__ float tile[32][33];
+  const int b = blockIdx.z, f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  for (int i = ty; i < 32; i += 8) {
+    const int f = f0 + i, t = t0 + tx;
+    tile[i][tx] = (f < F && t < T) ? mag[((size_t)b * F + f) * T + t] : 0.f;
+  }
+  __syncthreads();
+  for (int i = ty; i < 32; i += 8) {
+    const int t = t0 + i, f = f0 + tx;
+    if (t < Tp && f < F) magT[((size_t)t * B + b) * F + f] = tile[tx][i];
+  }
+}
+
+// out[i] = in[i] * scale[(i / cols) % B / div]  (rows of a [steps, B*div, cols] tensor scaled per clip)
+__global__ void ftr_scale_kernel(const float* __restrict__ in, const float* __restrict__ scale, size_t n, int cols, int rows,
+                                 int div, float* __restrict__ out) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    out[i] = in[i] * scale[(int)((i / cols) % rows) / div];
+}
+
+// first frame of shrunk step ts and the number of frames averaged into it (model.py:108-129)
+__device__ __forceinline__ void shrink_block(int ts, int S, int Tp, int& t0, int& len) {
+  if (ts == 0) { t0 = 0; len = 1; return; }
+  t0 = 1 + (ts - 1) * S;
+  len = min(t0 + S, Tp) - t0;
+}
+
+// bottleneck input before its norm (model.py:174-187), time-major sources melT / encT [Tp,B,M]: row (b,m) of shrunk step
+// ts, feature k = 2Nn+1 reflected noisy-mel rows || 2Ne+1 reflected encoder rows, averaged over the block of ts.  One CTA
+// per (b, ts): bn[ts][b*M+m][k] and the fixed-order sum fs[b*Ts+ts] (the layout clip_reduce_only_launch reads)
+__global__ void ftr_bn_input_kernel(const float* __restrict__ melT, const float* __restrict__ encT, int B, int Tp, int M,
+                                    int Nn, int Ne, int S, int Ts, float* __restrict__ bn, float2* __restrict__ fs) {
+  __shared__ float red[256];
+  const int b = blockIdx.x / Ts, ts = blockIdx.x % Ts;
+  const int K = (2 * Nn + 1) + (2 * Ne + 1);
+  int t0, len;
+  shrink_block(ts, S, Tp, t0, len);
+  const float inv = 1.0f / (float)len;
+  float local = 0.f;
+  for (int i = threadIdx.x; i < M * K; i += blockDim.x) {
+    const int m = i / K, k = i - m * K;
+    float acc = 0.f;
+    for (int t = t0; t < t0 + len; ++t) {
+      const size_t base = ((size_t)t * B + b) * M;
+      acc += (k < 2 * Nn + 1) ? melT[base + reflect_idx(m + k - Nn, M)]
+                              : encT[base + reflect_idx(m + (k - (2 * Nn + 1)) - Ne, M)];
+    }
+    const float v = acc * inv;
+    bn[((size_t)ts * B * M + (size_t)b * M + m) * K + k] = v;
+    local += v;
+  }
+  red[threadIdx.x] = local;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) fs[(size_t)b * Ts + ts] = make_float2(red[0], red[0]);
+}
+
+// decoder input dec_in [Tp,B,2M] = [encoder output | up-sampled bottleneck output] (model.py:191-194): frame t reads shrunk
+// step min(t/S, Ts-1) of bn_out [Ts, B*M]
+__global__ void ftr_dec_input_kernel(const float* __restrict__ encT, const float* __restrict__ bn_out, int B, int Tp, int M,
+                                     int S, int Ts, float* __restrict__ dec_in) {
+  const size_t n = (size_t)Tp * B * 2 * M;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % (2 * M));
+    const size_t tb = i / (2 * M);
+    const int b = (int)(tb % B), t = (int)(tb / B);
+    dec_in[i] = c < M ? encT[tb * M + c] : bn_out[(size_t)min(t / S, Ts - 1) * B * M + (size_t)b * M + (c - M)];
+  }
+}
+
+// dec [Tp,B,2F] (channel c*F+f) -> out [B,2,F,T], dropping the first `la` frames (model.py:197-200)
+__global__ void ftr_output_kernel(const float* __restrict__ dec, int B, int Tp, int F, int la, float* __restrict__ out) {
+  __shared__ float tile[32][33];
+  const int T = Tp - la;
+  const int b = blockIdx.z >> 1, c = blockIdx.z & 1;
+  const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  for (int i = ty; i < 32; i += 8) {
+    const int t = t0 + i, f = f0 + tx;
+    tile[i][tx] = (t < T && f < F) ? dec[((size_t)(t + la) * B + b) * (2 * F) + c * F + f] : 0.f;
+  }
+  __syncthreads();
+  for (int i = ty; i < 32; i += 8) {
+    const int f = f0 + i, t = t0 + tx;
+    if (f < F && t < T) out[(((size_t)b * 2 + c) * F + f) * T + t] = tile[tx][i];
+  }
+}
+
+// ------------------------------------------------------------------------------------------ backward kernels
+// dY [Tp,B,2F] from dout [B,2,F,T]; zero on the look-ahead frames
+__global__ void ftr_dy_kernel(const float* __restrict__ dout, int B, int F, int T, int Tp, int la, float* __restrict__ dY) {
+  const size_t n = (size_t)Tp * B * 2 * F;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int cf = (int)(i % (2 * F));
+    const size_t tb = i / (2 * F);
+    const int b = (int)(tb % B), t = (int)(tb / B);
+    dY[i] = t >= la ? dout[((size_t)b * 2 * F + cf) * T + (t - la)] : 0.f;
+  }
+}
+
+// transpose of the up-sampling (frame t <- shrunk step min(t/S, Ts-1)) on the bottleneck half of d dec_in, times ReLU' of
+// the bottleneck output: dbn[ts, r] = [bn_out > 0] * sum over the frames that read ts (ascending t)
+__global__ void ftr_dbn_kernel(const float* __restrict__ ddec, const float* __restrict__ bn_out, int B, int Tp, int M, int S,
+                               int Ts, float* __restrict__ dbn) {
+  const size_t R = (size_t)B * M, n = (size_t)Ts * R;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int ts = (int)(i / R);
+    const int r = (int)(i % R), b = r / M, m = r - b * M;
+    const int t0 = ts * S, t1 = ts == Ts - 1 ? Tp : min(t0 + S, Tp);
+    float acc = 0.f;
+    for (int t = t0; t < t1; ++t) acc += ddec[((size_t)t * B + b) * 2 * M + M + m];
+    dbn[i] = bn_out[i] > 0.f ? acc : 0.f;
+  }
+}
+
+// d encT [Tp,B,M] = ReLU'(encT) * ( ddec[t,b,m] (decoder input, columns < M)
+//   + inv2[b] * sum_{(m',k) : reflect(m' + k - Ne) = m} dX[ts(t), b*M+m', 2Nn+1+k] / len(ts)    (unfold^T . down-sampling^T)
+//   - inv2[b] * dot[b] * c_Ne[m] / (M K Ts len(ts)) )                                           (second-norm backward)
+// gather form: the (m', k) pairs of m are the direct, left-reflected and right-reflected sources of each offset k - Ne
+__global__ void ftr_denc_kernel(const float* __restrict__ ddec, const float* __restrict__ dX, const float* __restrict__ encT,
+                                const float* __restrict__ inv2, const float* __restrict__ dot, int B, int Tp, int M, int Nn,
+                                int Ne, int S, float cnt2, float* __restrict__ denc) {
+  const int K = (2 * Nn + 1) + (2 * Ne + 1);
+  const size_t n = (size_t)Tp * B * M;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int m = (int)(i % M);
+    const size_t tb = i / M;
+    const int b = (int)(tb % B), t = (int)(tb / B);
+    const int ts = t == 0 ? 0 : 1 + (t - 1) / S;
+    int t0, len;
+    shrink_block(ts, S, Tp, t0, len);
+    const float* dx = dX + ((size_t)ts * B * M + (size_t)b * M) * K + (2 * Nn + 1);
+    float acc = 0.f;
+    for (int k = 0; k <= 2 * Ne; ++k) {
+      const int o = k - Ne;
+      int src = m - o;                                        // m' + o = m
+      if (src >= 0 && src < M) acc += dx[(size_t)src * K + k];
+      src = -m - o;                                           // m' + o = -m < 0
+      if (m > 0 && src >= 0 && src < M) acc += dx[(size_t)src * K + k];
+      src = 2 * (M - 1) - m - o;                              // m' + o = 2(M-1) - m >= M
+      if (m < M - 1 && src >= 0 && src < M) acc += dx[(size_t)src * K + k];
+    }
+    const float s = inv2[b], fl = (float)len;
+    float v = ddec[tb * 2 * M + m] + s * acc / fl - s * dot[b] * (float)reflect_count(m, M, Ne) / (cnt2 * fl);
+    denc[i] = encT[i] > 0.f ? v : 0.f;
+  }
+}
+
+// ------------------------------------------------------------------------------------------ workspace
+enum { L_ENC1, L_ENC2, L_BN0, L_BN1, L_DEC1, L_DEC2, NL };
+
+struct FastTrainWs {
+  float *magT, *melT, *xenc, *encT, *xbn, *bn_out, *dec_in, *dec_out;
+  float *inv1, *inv2, *dot;
+  float2 *sums1, *sums2, *fs;
+  LayerSave L[NL];
+  float *dY, *dH, *ddec, *dbn, *dxbn, *denc;
+  float *dh_rec[2], *dc[2], *dh_mid;
+  float *splitk, *colsum, *gT, *xT, *rec;
+  float *whhT[NL], *wihT[NL];  // FSN_PREC_TF32_TC: transposed weights of the tensor-core layers
+  __half *h16[NL], *w16;       // fp16 MMA operands of the forward step kernel
+  size_t bytes;
+};
+
+struct LayerShape { int R, K0, H, steps; };
+
+struct FCarverT {
+  char* base; size_t off;
+  explicit FCarverT(void* p) : base((char*)p), off(0) {}
+  template <class T> T* take(size_t n) {
+    T* r = base ? (T*)(base + off) : nullptr;
+    off = align_up(off + n * sizeof(T), 256);
+    return r;
+  }
+};
+
+static void layer_shapes(const fsn_fast_desc* d, const FastDims& m, LayerShape* s) {
+  const int R = m.B * m.M;
+  s[L_ENC1] = {m.B, m.M, d->enc1_hidden, m.Tp};
+  s[L_ENC2] = {m.B, d->enc1_hidden, d->enc2_hidden, m.Tp};
+  s[L_BN0] = {R, m.K, d->bn_hidden, m.Ts};
+  s[L_BN1] = {R, d->bn_hidden, d->bn_hidden, m.Ts};
+  s[L_DEC1] = {m.B, 2 * m.M, d->dec_hidden, m.Tp};
+  s[L_DEC2] = {m.B, d->dec_hidden, d->dec_hidden, m.Tp};
+}
+
+// the same per-layer choice as fsn_train_forward / fsn_train_backward
+static bool tc_layer(const fsn_fast_desc* d, int H) { return d->precision == FSN_PREC_TF32_TC && (H & 3) == 0; }
+
+// the encoder input (normalised mel spectrogram) needs no gradient: no dx GEMM, no transposed W_ih
+static bool dx_tf32(int l) { return l != L_ENC1; }
+
+static size_t smax(size_t a, size_t b) { return a > b ? a : b; }
+
+static void carve_fast_train(const fsn_fast_desc* d, const FastDims& m, void* base, FastTrainWs& w) {
+  FCarverT c(base);
+  const size_t Tp = m.Tp, B = m.B, F = m.F, M = m.M, K = m.K, Ts = m.Ts, R = (size_t)m.B * m.M;
+  LayerShape s[NL];
+  layer_shapes(d, m, s);
+  w.magT = c.take<float>(Tp * B * F);
+  w.melT = c.take<float>(Tp * B * M);
+  w.xenc = c.take<float>(Tp * B * M);
+  w.encT = c.take<float>(Tp * B * M);
+  w.xbn = c.take<float>(Ts * R * K);
+  w.bn_out = c.take<float>(Ts * R);
+  w.dec_in = c.take<float>(Tp * B * 2 * M);
+  w.dec_out = c.take<float>(Tp * B * 2 * F);
+  w.inv1 = c.take<float>(B); w.inv2 = c.take<float>(B); w.dot = c.take<float>(B);
+  w.sums1 = c.take<float2>(B); w.sums2 = c.take<float2>(B); w.fs = c.take<float2>(B * Ts);
+  size_t rh = 0, hmax = 0, wmax = 0, g_blk = 0, x_blk = 0;
+  for (int l = 0; l < NL; ++l) {
+    const size_t rows = (size_t)s[l].steps * s[l].R, H = s[l].H;
+    w.L[l].G = c.take<float>(rows * 4 * H); w.L[l].C = c.take<float>(rows * H); w.L[l].H = c.take<float>(rows * H);
+    rh = smax(rh, (size_t)s[l].R * H);
+    hmax = smax(hmax, H);
+    wmax = smax(wmax, 4 * H * (H + s[l].K0));
+    if (tc_layer(d, s[l].H)) {
+      g_blk = smax(g_blk, tgemm_blocked_floats(rows, 4 * s[l].H));
+      x_blk = smax(x_blk, tgemm_blocked_floats(rows, s[l].K0 > s[l].H ? s[l].K0 : s[l].H));
+    }
+  }
+  w.dY = c.take<float>(Tp * B * 2 * F);
+  w.dH = c.take<float>(Tp * B * smax(d->dec_hidden, d->enc2_hidden));
+  w.ddec = c.take<float>(Tp * B * 2 * M);
+  w.dbn = c.take<float>(Ts * R);
+  w.dxbn = c.take<float>(Ts * R * K);
+  w.denc = c.take<float>(Tp * B * M);
+  for (int i = 0; i < 2; ++i) { w.dh_rec[i] = c.take<float>(rh); w.dc[i] = c.take<float>(rh); }
+  w.dh_mid = c.take<float>(rh);
+  w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
+  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * smax(4 * hmax, 2 * F));
+  w.gT = w.xT = w.rec = nullptr;
+  w.w16 = nullptr;
+  for (int l = 0; l < NL; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
+  if (d->precision == FSN_PREC_TF32_TC) {
+    for (int l = 0; l < NL; ++l) {
+      if (!tc_layer(d, s[l].H)) continue;
+      const size_t H = s[l].H;
+      w.whhT[l] = c.take<float>(H * 4 * H);
+      if (dx_tf32(l)) w.wihT[l] = c.take<float>((size_t)s[l].K0 * 4 * H);
+      w.h16[l] = c.take<__half>((size_t)s[l].steps * s[l].R * H);
+    }
+    w.gT = c.take<float>(g_blk);
+    w.xT = c.take<float>(x_blk);
+    w.rec = c.take<float>(4 * rh);
+    w.w16 = c.take<__half>(wmax);
+  }
+  w.bytes = c.off;
+}
+
+static int fast_train_check(const fsn_fast_desc* d, int B, int T, FastDims& m) {
+  FSN_REQUIRE(d, FSN_ERR_SHAPE, "fast training: no descriptor");
+  FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "fast training: the GRU cell is not built");
+  FSN_REQUIRE(d->precision == FSN_PREC_FP32 || d->precision == FSN_PREC_TF32_TC, FSN_ERR_UNSUPPORTED,
+              "fast training: precision must be fp32 or tf32_tc");
+  int rc = fast_dims(d, B, T, m);
+  if (rc) return rc;
+  FSN_REQUIRE(d->noisy_num_neighbors >= 0 && d->enc_num_neighbors >= 0 && d->enc1_hidden > 0 && d->enc2_hidden > 0 &&
+                  d->bn_hidden > 0 && d->dec_hidden > 0,
+              FSN_ERR_SHAPE, "fast training: bad descriptor");
+  FSN_REQUIRE(m.Ts <= 65535, FSN_ERR_SHAPE, "fast training: too many frames");
+  return FSN_OK;
+}
+
+static void seq_of(const fsn_lstm_layer& l, fsn_seq_weights& s) {
+  memset(&s, 0, sizeof(s));
+  s.w_ih[0] = l.w_ih; s.w_hh[0] = l.w_hh; s.b_ih[0] = l.b_ih; s.b_hh[0] = l.b_hh;
+}
+
+static const fsn_lstm_layer& layer_weights(const fsn_fast_weights* wt, int l) {
+  switch (l) {
+    case L_ENC1: return wt->enc1;
+    case L_ENC2: return wt->enc2;
+    case L_BN0: return wt->bn[0];
+    case L_BN1: return wt->bn[1];
+    case L_DEC1: return wt->dec1;
+    default: return wt->dec2;
+  }
+}
+
+// forward of layer l over its steps from X [steps, R, K0]; X16 = fp16 copy of X left by the layer below (or nullptr)
+static int fast_layer_forward(const fsn_fast_desc* d, const fsn_fast_weights* wt, const FastTrainWs& w, const LayerShape* s,
+                              int l, const float* X, const __half* X16, cudaStream_t st) {
+  fsn_seq_weights sw;
+  seq_of(layer_weights(wt, l), sw);
+  const LayerShape& q = s[l];
+  if (!tc_layer(d, q.H)) return layer_forward_save(&sw, 0, X, q.R, q.K0, q.H, q.steps, w.L[l], st);
+  const LayerHalf half{w.h16[l], X16, w.w16};
+  return layer_forward_save_tc(&sw, 0, X, q.R, q.K0, q.H, q.steps, w.L[l], w.rec, st, w.splitk, SPLITK_SCRATCH_FLOATS, &half);
+}
+
+static LayerBwd layer_bwd(const fsn_fast_desc* d, const fsn_fast_weights* wt, const FastTrainWs& w, const LayerShape* s,
+                          int l, int slot) {
+  const fsn_lstm_layer& lw = layer_weights(wt, l);
+  const bool tc = tc_layer(d, s[l].H);
+  return LayerBwd{lw.w_ih, lw.w_hh, w.L[l], s[l].R, s[l].K0, s[l].H, w.dh_rec[slot], w.dc[slot],
+                  tc ? w.whhT[l] : nullptr, tc ? w.wihT[l] : nullptr, w.splitk};
+}
+
+static int transpose_weights(const fsn_fast_desc* d, const fsn_fast_weights* wt, const FastTrainWs& w, const LayerShape* s,
+                             int l, cudaStream_t st) {
+  if (!tc_layer(d, s[l].H)) return FSN_OK;
+  const fsn_lstm_layer& lw = layer_weights(wt, l);
+  int rc;
+  if ((rc = transpose_launch(lw.w_hh, (size_t)4 * s[l].H, s[l].H, w.whhT[l], st))) return rc;
+  if (w.wihT[l] && (rc = transpose_launch(lw.w_ih, (size_t)4 * s[l].H, s[l].K0, w.wihT[l], st))) return rc;
+  return FSN_OK;
+}
+
+// BPTT of a two-layer pair (upper `hi` fed by lower `lo`, one step apart as in fsn_train_backward); d h of the upper layer
+// from dh_above [steps, R, Hhi] or from an O-output Linear on top (dout [steps, R, O], fc_w [O, Hhi]); dx of the lower
+// layer into dx [steps, R, K0lo] when given
+static int pair_bwd(const LayerBwd& hi, const LayerBwd& lo, int steps, const float* dh_above, const float* dout,
+                    const float* fc_w, int O, float* dh_mid, float* dx, cudaStream_t st) {
+  int rc;
+  for (int t = steps - 1; t >= 0; --t) {
+    if ((rc = layer_bwd_step(hi, t, steps, dh_above ? dh_above + (size_t)t * hi.R * hi.H : nullptr,
+                             dout ? dout + (size_t)t * hi.R * O : nullptr, fc_w, O, dh_mid, st)))
+      return rc;
+    if ((rc = layer_bwd_step(lo, t, steps, dh_mid, nullptr, nullptr, 0, dx ? dx + (size_t)t * lo.R * lo.K0 : nullptr, st)))
+      return rc;
+  }
+  return FSN_OK;
+}
+
+static int grid_for(size_t n) {
+  size_t g = (n + 255) / 256;
+  return (int)(g > 132 * 16 ? 132 * 16 : (g ? g : 1));
+}
+
+}  // namespace fsn
+
+using namespace fsn;
+
+extern "C" size_t fsn_fast_train_workspace_bytes(const fsn_fast_desc* d, int B, int T) {
+  FastDims m;
+  if (fast_train_check(d, B, T, m)) return 0;
+  FastTrainWs w;
+  carve_fast_train(d, m, nullptr, w);
+  return w.bytes;
+}
+
+extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* mix_mag, int B, int T,
+                                      float* out, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FastDims m;
+  int rc = fast_train_check(d, B, T, m);
+  if (rc) return rc;
+  FSN_REQUIRE(wt && mix_mag && out, FSN_ERR_SHAPE, "fast training: null argument");
+  FastTrainWs w;
+  carve_fast_train(d, m, workspace, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes,
+              w.bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Tp = m.Tp, F = m.F, M = m.M, K = m.K, Ts = m.Ts, R = B * M;
+  LayerShape s[NL];
+  layer_shapes(d, m, s);
+  // look-ahead pad + time-major layout, Mel filtering (model.py:161-166)
+  ftr_transpose_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(mix_mag, w.magT, B, F, T, Tp);
+  FSN_CHECK_LAUNCH("ftr_transpose_kernel");
+  if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, Tp * B, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true))) return rc;
+  // first norm (model.py:170): the mel spectrogram has no parameter behind it, only the normalised copy is kept
+  train_tm_stats_kernel<<<B, 256, 0, st>>>(w.melT, B, M, Tp, 0, w.sums1);
+  FSN_CHECK_LAUNCH("train_tm_stats_kernel");
+  if ((rc = norm_scales_launch(w.sums1, w.sums1, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) return rc;
+  ftr_scale_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.melT, w.inv1, (size_t)Tp * B * M, M, B, 1, w.xenc);
+  FSN_CHECK_LAUNCH("ftr_scale_kernel");
+  // encoder: LSTM(M->He1), LSTM(He1->He2) + Linear(M) + ReLU (model.py:35-54,171)
+  if ((rc = fast_layer_forward(d, wt, w, s, L_ENC1, w.xenc, nullptr, st))) return rc;
+  if ((rc = fast_layer_forward(d, wt, w, s, L_ENC2, w.L[L_ENC1].H, nullptr, st))) return rc;  // He1 != He2: no shared fp16 path
+  if ((rc = fc_gemm_launch(w.L[L_ENC2].H, wt->enc_fc_w, wt->enc_fc_b, w.encT, Tp * B, d->enc2_hidden, M, FSN_ACT_RELU, st)))
+    return rc;
+  // bottleneck input: unfold + concat + down-sampling, its norm; the normalised input is kept (model.py:174-187)
+  ftr_bn_input_kernel<<<B * Ts, 256, 0, st>>>(w.melT, w.encT, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
+                                              Ts, w.xbn, w.fs);
+  FSN_CHECK_LAUNCH("ftr_bn_input_kernel");
+  if ((rc = clip_reduce_only_launch(w.fs, B, Ts, w.sums2, st))) return rc;
+  if ((rc = norm_scales_launch(w.sums2, w.sums2, B, (float)M * K * Ts, 1.f, w.inv2, nullptr, st))) return rc;
+  ftr_scale_kernel<<<grid_for((size_t)Ts * R * K), 256, 0, st>>>(w.xbn, w.inv2, (size_t)Ts * R * K, K, R, M, w.xbn);
+  FSN_CHECK_LAUNCH("ftr_scale_kernel");
+  // bottleneck 2xLSTM(K->Hb->Hb) + Linear(1) + ReLU over Ts steps (model.py:188-189)
+  if ((rc = fast_layer_forward(d, wt, w, s, L_BN0, w.xbn, nullptr, st))) return rc;
+  if ((rc = fast_layer_forward(d, wt, w, s, L_BN1, w.L[L_BN0].H, w.h16[L_BN0], st))) return rc;
+  if ((rc = rows_fc_launch(w.L[L_BN1].H, Ts * R, d->bn_hidden, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out, 1, 0, st)))
+    return rc;
+  // up-sampling + concat, decoder LSTM(2M->Hd), LSTM(Hd->Hd) + Linear(2F) (model.py:191-196)
+  ftr_dec_input_kernel<<<grid_for((size_t)Tp * B * 2 * M), 256, 0, st>>>(w.encT, w.bn_out, B, Tp, M, m.S, Ts, w.dec_in);
+  FSN_CHECK_LAUNCH("ftr_dec_input_kernel");
+  if ((rc = fast_layer_forward(d, wt, w, s, L_DEC1, w.dec_in, nullptr, st))) return rc;
+  if ((rc = fast_layer_forward(d, wt, w, s, L_DEC2, w.L[L_DEC1].H, w.h16[L_DEC1], st))) return rc;
+  if ((rc = fc_gemm_launch(w.L[L_DEC2].H, wt->dec_fc_w, wt->dec_fc_b, w.dec_out, Tp * B, d->dec_hidden, 2 * F, FSN_ACT_NONE, st)))
+    return rc;
+  ftr_output_kernel<<<dim3(cdiv(T, 32), cdiv(F, 32), B * 2), dim3(32, 8), 0, st>>>(w.dec_out, B, Tp, F, d->look_ahead, out);
+  FSN_CHECK_LAUNCH("ftr_output_kernel");
+  return FSN_OK;
+}
+
+extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* dout, int B, int T,
+                                       const fsn_fast_grads* g, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FastDims m;
+  int rc = fast_train_check(d, B, T, m);
+  if (rc) return rc;
+  FSN_REQUIRE(wt && dout && g, FSN_ERR_SHAPE, "fast training: null argument");
+  FastTrainWs w;
+  carve_fast_train(d, m, workspace, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes,
+              w.bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Tp = m.Tp, F = m.F, M = m.M, K = m.K, Ts = m.Ts, R = B * M;
+  const int Hd = d->dec_hidden, He2 = d->enc2_hidden, Hb = d->bn_hidden;
+  LayerShape s[NL];
+  layer_shapes(d, m, s);
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  for (int l = 0; l < NL; ++l)
+    if ((rc = transpose_weights(d, wt, w, s, l, st))) return rc;
+  // ---- decoder Linear(2F) (model.py:196-200 backwards): dW = dY^T H, db = colsum dY, dH = dY W
+  ftr_dy_kernel<<<grid_for((size_t)Tp * B * 2 * F), 256, 0, st>>>(dout, B, F, T, Tp, d->look_ahead, w.dY);
+  FSN_CHECK_LAUNCH("ftr_dy_kernel");
+  if ((rc = sgemm_launch(true, w.dY, 2 * F, w.L[L_DEC2].H, Hd, g->dec_fc_w, Hd, 2 * F, Hd, Tp * B, false, w.splitk, st)))
+    return rc;
+  if ((rc = colsum_launch(w.dY, (size_t)Tp * B, 2 * F, 2 * F, g->dec_fc_b, nullptr, w.colsum, st))) return rc;
+  if ((rc = sgemm_launch(false, w.dY, 2 * F, wt->dec_fc_w, Hd, w.dH, Hd, Tp * B, Hd, 2 * F, false, nullptr, st))) return rc;
+  // ---- decoder BPTT, d dec_in
+  const LayerBwd d2 = layer_bwd(d, wt, w, s, L_DEC2, 1), d1 = layer_bwd(d, wt, w, s, L_DEC1, 0);
+  if ((rc = pair_bwd(d2, d1, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, w.ddec, st))) return rc;
+  if ((rc = layer_weight_grads(d2, Tp, w.L[L_DEC1].H, g->dec2.w_ih, g->dec2.w_hh, g->dec2.b_ih, g->dec2.b_hh, wg, st))) return rc;
+  if ((rc = layer_weight_grads(d1, Tp, w.dec_in, g->dec1.w_ih, g->dec1.w_hh, g->dec1.b_ih, g->dec1.b_hh, wg, st))) return rc;
+  // ---- up-sampling transpose + ReLU' of the bottleneck output, its Linear(1)
+  ftr_dbn_kernel<<<grid_for((size_t)Ts * R), 256, 0, st>>>(w.ddec, w.bn_out, B, Tp, M, m.S, Ts, w.dbn);
+  FSN_CHECK_LAUNCH("ftr_dbn_kernel");
+  if ((rc = sgemm_launch(true, w.dbn, 1, w.L[L_BN1].H, Hb, g->bn_fc_w, Hb, 1, Hb, Ts * R, false, w.splitk, st))) return rc;
+  if ((rc = colsum_launch(w.dbn, (size_t)Ts * R, 1, 1, g->bn_fc_b, nullptr, w.colsum, st))) return rc;
+  // ---- bottleneck BPTT (the Linear(1) backward folded into layer 1's point kernel), d X_bn
+  const LayerBwd b1 = layer_bwd(d, wt, w, s, L_BN1, 1), b0 = layer_bwd(d, wt, w, s, L_BN0, 0);
+  if ((rc = pair_bwd(b1, b0, Ts, nullptr, w.dbn, wt->bn_fc_w, 1, w.dh_mid, w.dxbn, st))) return rc;
+  if ((rc = layer_weight_grads(b1, Ts, w.L[L_BN0].H, g->bn[1].w_ih, g->bn[1].w_hh, g->bn[1].b_ih, g->bn[1].b_hh, wg, st))) return rc;
+  if ((rc = layer_weight_grads(b0, Ts, w.xbn, g->bn[0].w_ih, g->bn[0].w_hh, g->bn[0].b_ih, g->bn[0].b_hh, wg, st))) return rc;
+  // ---- second norm + down-sampling + unfold backward, ReLU' of the encoder output, its Linear(M)
+  train_dot_kernel<<<B, 256, 0, st>>>(w.dxbn, w.xbn, Ts, R, M, K, w.dot);
+  FSN_CHECK_LAUNCH("train_dot_kernel");
+  ftr_denc_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.ddec, w.dxbn, w.encT, w.inv2, w.dot, B, Tp, M,
+                                                                d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
+                                                                (float)M * K * Ts, w.denc);
+  FSN_CHECK_LAUNCH("ftr_denc_kernel");
+  if ((rc = sgemm_launch(true, w.denc, M, w.L[L_ENC2].H, He2, g->enc_fc_w, He2, M, He2, Tp * B, false, w.splitk, st))) return rc;
+  if ((rc = colsum_launch(w.denc, (size_t)Tp * B, M, M, g->enc_fc_b, nullptr, w.colsum, st))) return rc;
+  if ((rc = sgemm_launch(false, w.denc, M, wt->enc_fc_w, He2, w.dH, He2, Tp * B, He2, M, false, nullptr, st))) return rc;
+  // ---- encoder BPTT (its input is the normalised mel spectrogram: no dx)
+  const LayerBwd e2 = layer_bwd(d, wt, w, s, L_ENC2, 1), e1 = layer_bwd(d, wt, w, s, L_ENC1, 0);
+  if ((rc = pair_bwd(e2, e1, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, st))) return rc;
+  if ((rc = layer_weight_grads(e2, Tp, w.L[L_ENC1].H, g->enc2.w_ih, g->enc2.w_hh, g->enc2.b_ih, g->enc2.b_hh, wg, st))) return rc;
+  return layer_weight_grads(e1, Tp, w.xenc, g->enc1.w_ih, g->enc1.w_hh, g->enc1.b_ih, g->enc1.b_hh, wg, st);
+}

@@ -92,6 +92,47 @@ struct LayerHalf { __half* H16; const __half* X16; __half* w16; };
 int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp,
                           const LayerSave& s, float* rec, cudaStream_t st, float* splitk = nullptr, size_t splitk_floats = 0,
                           const LayerHalf* half = nullptr);
+// fp32 variant: one SIMT step kernel per step (lstm_step_launch with save_gates)
+int layer_forward_save(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+                       cudaStream_t st);
+
+// ---- back-propagation through time of one LSTM layer (fsn_train.cu), shared by the fullsubnet and fast_fullsubnet steps
+static const size_t SPLITK_SCRATCH_FLOATS = (size_t)16 << 20;  // 64 MB of split-K partial sums
+static const int COLSUM_MAX_S = 512;                            // row slabs of a column sum
+struct LayerBwd {
+  const float *w_ih, *w_hh;
+  LayerSave s;
+  int R, K0, H;
+  float *dh_rec, *dc;
+  const float *w_hhT, *w_ihT;  // tensor-core path: [H,4H] / [K0,4H] transposed copies (else nullptr)
+  float* splitk;               // split-K space of the per-step GEMMs (used when the layer has only a few tiles)
+};
+// scratch of layer_weight_grads: K-major copies of dG / layer input (tensor-core path, tgemm_blocked_floats of the largest
+// layer), split-K space (SPLITK_SCRATCH_FLOATS) and column-sum partials (COLSUM_MAX_S x 4H)
+struct WgradScratch { float *gT, *xT, *splitk, *colsum; };
+// step t of one layer: pointwise gate gradients (d h from above = dh_above + dout W_fc for an O-output Linear on top),
+// then dh_rec = dG W_hh and, when dx != nullptr, dx = dG W_ih
+int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, const float* dout, const float* fc_w, int O,
+                   float* dx, cudaStream_t st);
+// weight / bias gradients of one layer from dG [Tp*R,4H] (in L.s.G), its input X [Tp*R,K0] and hidden states
+int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih, float* g_w_hh, float* g_b_ih, float* g_b_hh,
+                       const WgradScratch& w, cudaStream_t st);
+// fp32 SIMT GEMM C[M,N] (+)= op(A) B (op(A) = A^T when ta), split-K over `scratch` for long K (deterministic)
+int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
+                 bool accumulate, float* scratch, cudaStream_t st);
+// out[c] (and out2[c] when given) = sum_r X[r*ldx + c], fixed order
+int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch, cudaStream_t st);
+// out [cols, rows] = in [rows, cols]^T
+int transpose_launch(const float* in, size_t rows, int cols, float* out, cudaStream_t st);
+// per-clip (sum, sum_f c_N[f] * row sum) of a time-major x [Tp,B,F], one CTA per clip
+__global__ void train_tm_stats_kernel(const float* __restrict__ x, int B, int F, int Tp, int N, float2* __restrict__ sums);
+// dot[b'] = sum over the rows [b'*Fsub, (b'+1)*Fsub) of every step of dX * X  (laplace-norm backward), one CTA per clip
+__global__ void train_dot_kernel(const float* __restrict__ dX, const float* __restrict__ X, int Tp, int R, int Fsub, int K,
+                                 float* __restrict__ dot);
+
+// shapes of one fast_fullsubnet Model.forward call (fsn_fast_model.cu): Ts = shrunk steps of the bottleneck
+struct FastDims { int B, T, Tp, F, M, K, Ts, S; };
+int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m);
 
 // shapes of one Model.forward call (fsn_model.cu)
 struct Dims {

@@ -102,9 +102,7 @@ int splitk_reduce_launch(const float* part, int S, int M, int N, float* C, size_
   return FSN_OK;
 }
 
-static const size_t SPLITK_SCRATCH_FLOATS = (size_t)16 << 20;  // 64 MB
-
-static int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M,
+int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M,
                         int N, int K, bool accumulate, float* scratch, cudaStream_t st) {
   if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
   const int tiles = cdiv(M, 64) * cdiv(N, 64);
@@ -159,7 +157,6 @@ __global__ void colsum_final_kernel(const float* __restrict__ part, int S, int c
   out[c] = s;
   if (out2) out2[c] = s;
 }
-static const int COLSUM_MAX_S = 512;
 
 // dW [O,H] = dout^T Hm for a Linear with a few outputs (the sub-band Linear, O = 2; model.py:129-135 backwards):
 // dout [rows,O], Hm [rows,H].  One pass over Hm: a CTA owns a slab of rows, a thread one column; part [S][O][H], then
@@ -193,7 +190,7 @@ __global__ void __launch_bounds__(128) small_out_wgrad_kernel(const float* __res
     for (int o = 0; o < O; ++o) part[((size_t)blockIdx.y * O + o) * H + c] = acc[o];
   }
 }
-static int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch,
+int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch,
                          cudaStream_t st) {
   int S = (int)((rows + 2047) / 2048);
   if (S > COLSUM_MAX_S) S = COLSUM_MAX_S;
@@ -385,7 +382,7 @@ __global__ void transpose_kernel(const float* __restrict__ in, size_t rows, int 
     if (c < cols && r < rows) out[(size_t)c * rows + r] = tile[threadIdx.x][i];
   }
 }
-static int transpose_launch(const float* in, size_t rows, int cols, float* out, cudaStream_t st) {
+int transpose_launch(const float* in, size_t rows, int cols, float* out, cudaStream_t st) {
   dim3 grid((unsigned)((rows + 31) / 32), cdiv(cols, 32));
   transpose_kernel<<<grid, dim3(32, 8), 0, st>>>(in, rows, cols, out);
   FSN_CHECK_LAUNCH("transpose_kernel");
@@ -584,8 +581,8 @@ static int train_check(const fsn_model_desc* d) {
 }
 
 // one layer forward over all steps, saving gates / cell / hidden:  X [Tp,R,K0] (row_scale == nullptr)
-static int layer_forward_save(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp,
-                              const LayerSave& s, cudaStream_t st) {
+int layer_forward_save(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+                       cudaStream_t st) {
   for (int t = 0; t < Tp; ++t) {
     StepParams p;
     memset(&p, 0, sizeof(p));
@@ -667,17 +664,8 @@ int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R
 
 static bool tc_layer_ok(const fsn_model_desc* d, int H) { return d->precision == FSN_PREC_TF32_TC && (H & 3) == 0; }
 
-struct LayerBwd {
-  const float *w_ih, *w_hh;
-  LayerSave s;
-  int R, K0, H;
-  float *dh_rec, *dc;
-  const float *w_hhT, *w_ihT;  // tensor-core path: [H,4H] / [K0,4H] transposed copies (else nullptr)
-  float* splitk;               // split-K space of the per-step GEMMs (used when the layer has only a few tiles)
-};
-
 // step t of one layer: pointwise gate gradients, then dh_rec = dG W_hh and (optionally) dx = dG W_ih
-static int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, const float* dout, const float* fc_w,
+int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, const float* dout, const float* fc_w,
                           int O, float* dx, cudaStream_t st) {
   BwdPoint p;
   memset(&p, 0, sizeof(p));
@@ -709,8 +697,8 @@ static int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_abov
 }
 
 // weight / bias gradients of one layer from dG [Tp*R,4H] (in L.s.G), its input X [Tp*R,K0] and hidden states
-static int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih, float* g_w_hh, float* g_b_ih,
-                              float* g_b_hh, const TrainWs& w, cudaStream_t st) {
+int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih, float* g_w_hh, float* g_b_ih,
+                       float* g_b_hh, const WgradScratch& w, cudaStream_t st) {
   const int H4 = 4 * L.H;
   const int rows = Tp * L.R;
   int rc;
@@ -937,9 +925,10 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
     if ((rc = check_cuda(cudaStreamWaitEvent(side->s, side->fork, 0), "stream wait"))) return rc;
     st2 = side->s; splitk2 = w.splitk2; colsum2 = w.colsum2;
   }
-  if ((rc = layer_weight_grads(s1, Tp, w.sb[0].H, gsb->w_ih[1], gsb->w_hh[1], gsb->b_ih[1], gsb->b_hh[1], w, st)))
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  if ((rc = layer_weight_grads(s1, Tp, w.sb[0].H, gsb->w_ih[1], gsb->w_hh[1], gsb->b_ih[1], gsb->b_hh[1], wg, st)))
     return rc;
-  if ((rc = layer_weight_grads(s0, Tp, w.xsb, gsb->w_ih[0], gsb->w_hh[0], gsb->b_ih[0], gsb->b_hh[0], w, st))) return rc;
+  if ((rc = layer_weight_grads(s0, Tp, w.xsb, gsb->w_ih[0], gsb->w_hh[0], gsb->b_ih[0], gsb->b_hh[0], wg, st))) return rc;
   // ---- second norm + drop_band + full-band Linear/activation
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
     train_cum_unit_bwd_kernel<<<cdiv(R, 128), 128, 0, st2>>>(w.dxsb, w.xsb, w.cum2, Tp, R, K, w.dunit);
@@ -968,9 +957,9 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
     if ((rc = check_cuda(cudaEventRecord(side->join, side->s), "event record"))) return rc;
     if ((rc = check_cuda(cudaStreamWaitEvent(st, side->join, 0), "stream wait"))) return rc;
   }
-  if ((rc = layer_weight_grads(f1, Tp, w.fb[0].H, gfb->w_ih[1], gfb->w_hh[1], gfb->b_ih[1], gfb->b_hh[1], w, st)))
+  if ((rc = layer_weight_grads(f1, Tp, w.fb[0].H, gfb->w_ih[1], gfb->w_hh[1], gfb->b_ih[1], gfb->b_hh[1], wg, st)))
     return rc;
-  return layer_weight_grads(f0, Tp, w.xfb, gfb->w_ih[0], gfb->w_hh[0], gfb->b_ih[0], gfb->b_hh[0], w, st);
+  return layer_weight_grads(f0, Tp, w.xfb, gfb->w_ih[0], gfb->w_hh[0], gfb->b_ih[0], gfb->b_hh[0], wg, st);
 }
 
 // ------------------------------------------------------------------------------------------ loss

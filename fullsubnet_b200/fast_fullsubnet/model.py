@@ -2,7 +2,9 @@
 
 Same constructor kwargs and the same 31 ``state_dict`` entries (incl. the ``mel_scale.fb`` buffer that
 torchaudio's MelScale registers); ``forward(mix_mag [B,1,F,T]) -> [B,2,F,T]`` is one call into libfsn_b200
-(``fsn_fast_model_forward``, fp32 kernels)."""
+(``fsn_fast_model_forward``).  In train mode with gradients enabled the forward keeps its activations
+(``fsn_fast_train_forward``) and ``loss.backward()`` runs back-propagation through time in the library
+(``fsn_fast_train_backward``), the training step of fast_fullsubnet/trainer.py:45-56."""
 from __future__ import annotations
 
 import ctypes as C
@@ -27,6 +29,73 @@ def melscale_fbanks(n_freqs: int, n_mels: int, sample_rate: int = 16000, f_min: 
     f_diff = f_pts[1:] - f_pts[:-1]
     slopes = f_pts.unsqueeze(0) - all_freqs.unsqueeze(1)
     return torch.max(torch.zeros(1), torch.min((-1.0 * slopes[:, :-2]) / f_diff[:-1], slopes[:, 2:] / f_diff[1:]))
+
+
+_LAYERS = (("enc1", "encoder.0.", 0), ("enc2", "encoder.1.", 0), ("dec1", "decoder_lstm.0.", 0),
+           ("dec2", "decoder_lstm.1.", 0))
+_LINEARS = (("enc_fc", "encoder.1."), ("bn_fc", "bottleneck."), ("dec_fc", "decoder_lstm.1."))
+
+
+def _lstm_grads(grads: dict, prefix: str, l: int) -> "_lib.LstmGrads":
+    return _lib.LstmGrads(*(grads[f"{prefix}sequence_model.{n}_l{l}"].data_ptr()
+                            for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")))
+
+
+def _grad_struct(grads: dict) -> "_lib.FastGrads":
+    g = _lib.FastGrads()
+    for field, prefix, l in _LAYERS:
+        setattr(g, field, _lstm_grads(grads, prefix, l))
+    for l in range(2):
+        g.bn[l] = _lstm_grads(grads, "bottleneck.", l)
+    for field, prefix in _LINEARS:
+        setattr(g, field + "_w", grads[f"{prefix}fc_output_layer.weight"].data_ptr())
+        setattr(g, field + "_b", grads[f"{prefix}fc_output_layer.bias"].data_ptr())
+    return g
+
+
+class _TrainForward(torch.autograd.Function):
+    """Model.forward in train mode with back-propagation through time in libfsn_b200 (fsn_fast_train_forward /
+    fsn_fast_train_backward).  The parameters are passed as inputs so autograd (and DDP's hooks) route the gradients to
+    them exactly as for the reference's nn.LSTM / nn.Linear modules."""
+
+    @staticmethod
+    def forward(ctx, model, x, *params):
+        B, _, F, T = x.shape
+        device = x.device
+        lib = _lib.load()
+        with torch.cuda.device(device):
+            d = model._desc(_lib.PREC[model._resolve_train_precision()])
+            w = model._weight_struct()
+            n = lib.fsn_fast_train_workspace_bytes(C.byref(d), B, T)
+            if n == 0:
+                _lib.check_workspace(n)
+            ws = torch.empty(n, dtype=torch.uint8, device=device)
+            out = torch.empty(B, 2, F, T, dtype=torch.float32, device=device)
+            _lib.check(lib.fsn_fast_train_forward(C.byref(d), C.byref(w), x.data_ptr(), B, T, out.data_ptr(),
+                                                  ws.data_ptr(), n, _lib.stream_ptr(device)))
+        ctx.model, ctx.ws, ctx.dims, ctx.desc = model, ws, (B, T), d
+        ctx.versions = model._version_key()
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        model, (B, T) = ctx.model, ctx.dims
+        if ctx.versions != model._version_key():
+            raise RuntimeError("fullsubnet_b200: a parameter was modified in place between forward and backward")
+        if ctx.ws is None:
+            raise RuntimeError("fullsubnet_b200: backward through the same forward twice (activations were released)")
+        dout = dout.contiguous().float()
+        device = dout.device
+        lib = _lib.load()
+        names = [k for k, _ in model.named_parameters()]
+        _, grads = model._new_flat_grads(device)
+        with torch.cuda.device(device):
+            w = model._weight_struct()
+            g = _grad_struct(grads)
+            _lib.check(lib.fsn_fast_train_backward(C.byref(ctx.desc), C.byref(w), dout.data_ptr(), B, T, C.byref(g),
+                                                   ctx.ws.data_ptr(), ctx.ws.numel(), _lib.stream_ptr(device)))
+        ctx.ws = None
+        return (None, None) + tuple(grads[k] for k in names)
 
 
 class _MelScale(nn.Module):
@@ -72,6 +141,10 @@ class Model(BaseModel):
         # tensor-core modes run the bottleneck on the wgmma sub-band kernel and the encoder / decoder LSTMs + Linears
         # on the hoisted-GEMM + persistent-recurrence kernels (fsn_lstm_rec_tc.cu)
         self.precision = precision or os.environ.get("FSN_PRECISION", "auto")
+        # arithmetic of the training step's GEMMs: "fp32" (FMA) | "tf32_tc" (wgmma tf32 for every LSTM layer whose hidden
+        # size is a multiple of 4; enc2 with 257 units stays fp32) | "auto" = tf32_tc when the bottleneck allows it
+        self.train_precision = os.environ.get("FSN_TRAIN_PRECISION", "auto")
+        self.sequence_model_type = sequence_model
         self._packed = None
         self._packed_key = None
         if num_mels != 64 or encoder_input_size != 257:
@@ -90,16 +163,26 @@ class Model(BaseModel):
             raise NotImplementedError("the tensor-core precisions need bottleneck_hidden_size = 384, 2 layers and input width <= 32")
         return self.precision
 
+    def _resolve_train_precision(self) -> str:
+        if self.train_precision == "auto":
+            return "tf32_tc" if self.bottleneck.hidden_size % 4 == 0 else "fp32"
+        if self.train_precision not in ("fp32", "tf32_tc"):
+            raise ValueError("train_precision must be 'fp32', 'tf32_tc' or 'auto'")
+        return self.train_precision
+
+    def _version_key(self):
+        return tuple((p.data_ptr(), p._version) for p in self.parameters())
+
     def _desc(self, prec: int):
         return _lib.FastDesc(num_freqs=self.encoder_input_size, look_ahead=self.look_ahead, shrink_size=self.shrink_size,
                           num_mels=self.num_mels, enc1_hidden=384, enc2_hidden=257,
                           bn_hidden=self.bottleneck.hidden_size, bn_layers=self.bottleneck.num_layers, dec_hidden=512,
                           noisy_num_neighbors=self.noisy_input_num_neighbors,
-                          enc_num_neighbors=self.enc_output_num_neighbors, precision=prec)
+                          enc_num_neighbors=self.enc_output_num_neighbors, precision=prec,
+                          cell_type=_lib.CELL[self.sequence_model_type])
 
-    def _structs(self, device):
-        prec = self._resolve_precision()
-        d = self._desc(_lib.PREC[prec])
+    def _weight_struct(self):
+        """Raw device pointers of every parameter (fsn_fast_weights, no packed bottleneck image)."""
         w = _lib.FastWeights()
         fb = self.mel_scale.fb
         if not fb.is_cuda:
@@ -113,6 +196,12 @@ class Model(BaseModel):
         w.dec1, w.dec2 = self.decoder_lstm[0].layer_struct(0), self.decoder_lstm[1].layer_struct(0)
         w.dec_fc_w, w.dec_fc_b = self.decoder_lstm[1].fc_ptrs()
         w.bn_packed = None
+        return w
+
+    def _structs(self, device):
+        prec = self._resolve_precision()
+        d = self._desc(_lib.PREC[prec])
+        w = self._weight_struct()
         if prec != "fp32":  # tile-ordered fp16 image of the bottleneck weights, rebuilt when a parameter changes
             key = (self.bottleneck.version_key(), str(device), prec)
             if self._packed is None or self._packed_key != key:
@@ -129,9 +218,12 @@ class Model(BaseModel):
         batch_size, num_channels, num_freqs, num_frames = mix_mag.size()
         assert num_channels == 1, f"{self.__class__.__name__} takes a magnitude feature as the input."
         assert num_freqs == self.encoder_input_size
-        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("fullsubnet_b200: backward kernels are not built yet; use torch.no_grad()/eval().")
         x = _lib.require_cuda(mix_mag, "mix_mag")
+        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            # training step (fast_fullsubnet/trainer.py:45-56): kernels that keep the activations for BPTT
+            if not all(p.requires_grad for p in self.parameters()):
+                raise NotImplementedError("fullsubnet_b200: partially frozen models are not built")
+            return _TrainForward.apply(self, x, *self.parameters())
         lib = _lib.load()
         with torch.cuda.device(x.device):
             d, w = self._structs(x.device)

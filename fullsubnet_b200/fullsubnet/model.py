@@ -185,38 +185,6 @@ class Model(BaseModel):
                                              ws_bytes, _lib.stream_ptr(device)))
         return out
 
-    def flat_grad(self):
-        """Makes every ``p.grad`` a view into one persistent flat fp32 buffer (keeping current values) and returns
-        the buffer: one ``all_reduce`` then moves all 20 gradients (SURVEY 8e)."""
-        params = list(self.parameters())
-        flat = getattr(self, "_flat", None)
-        ok = flat is not None and flat.device == params[0].device and all(
-            p.grad is not None and p.grad.data_ptr() == flat.data_ptr() + 4 * off
-            for p, off in zip(params, self._flat_offsets))
-        if not ok:
-            flat = torch.zeros(sum(p.numel() for p in params), dtype=torch.float32, device=params[0].device)
-            offs, off = [], 0
-            for p in params:
-                view = flat[off:off + p.numel()].view_as(p)
-                if p.grad is not None:
-                    view.copy_(p.grad)
-                p.grad = view
-                offs.append(off)
-                off += p.numel()
-            self._flat, self._flat_offsets = flat, offs
-        return flat
-
-    def _new_flat_grads(self, device):
-        """One flat fp32 buffer holding every gradient in parameter order (what the single all-reduce of
-        base_trainer.py:32 / SURVEY 8e moves) and the per-parameter views into it."""
-        params = list(self.named_parameters())
-        flat = torch.empty(sum(p.numel() for _, p in params), dtype=torch.float32, device=device)
-        views, off = {}, 0
-        for k, p in params:
-            views[k] = flat[off:off + p.numel()].view_as(p)
-            off += p.numel()
-        return flat, views
-
     @torch.no_grad()
     def enhance(self, noisy, n_fft=512, hop_length=256, win_length=512, return_crm=False):
         """Fused wav -> wav path of Inferencer.full_band_crm_mask (recipes/.../inferencer.py:130-145),

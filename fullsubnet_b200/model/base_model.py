@@ -1,7 +1,9 @@
 """Host-side pieces of audio_zen/model/base_model.py that the drop-in Model needs:
-norm_wrapper (:356-372) name checking and weight_init (:374-439, CPU-side initialisation)."""
+norm_wrapper (:356-372) name checking and weight_init (:374-439, CPU-side initialisation); plus the flat-gradient
+buffers the training steps of fullsubnet and fast_fullsubnet share."""
 from __future__ import annotations
 
+import torch
 import torch.nn as nn
 import torch.nn.init as init
 
@@ -33,3 +35,35 @@ class BaseModel(nn.Module):
                     init.orthogonal_(param.data)
                 else:
                     init.normal_(param.data)
+
+    def flat_grad(self):
+        """Makes every ``p.grad`` a view into one persistent flat fp32 buffer (keeping current values) and returns
+        the buffer: one ``all_reduce`` then moves every gradient of the model (SURVEY 8e)."""
+        params = list(self.parameters())
+        flat = getattr(self, "_flat", None)
+        ok = flat is not None and flat.device == params[0].device and all(
+            p.grad is not None and p.grad.data_ptr() == flat.data_ptr() + 4 * off
+            for p, off in zip(params, self._flat_offsets))
+        if not ok:
+            flat = torch.zeros(sum(p.numel() for p in params), dtype=torch.float32, device=params[0].device)
+            offs, off = [], 0
+            for p in params:
+                view = flat[off:off + p.numel()].view_as(p)
+                if p.grad is not None:
+                    view.copy_(p.grad)
+                p.grad = view
+                offs.append(off)
+                off += p.numel()
+            self._flat, self._flat_offsets = flat, offs
+        return flat
+
+    def _new_flat_grads(self, device):
+        """One flat fp32 buffer holding every gradient in parameter order (what the single all-reduce of
+        base_trainer.py:32 / SURVEY 8e moves) and the per-parameter views into it."""
+        params = list(self.named_parameters())
+        flat = torch.empty(sum(p.numel() for _, p in params), dtype=torch.float32, device=device)
+        views, off = {}, 0
+        for k, p in params:
+            views[k] = flat[off:off + p.numel()].view_as(p)
+            off += p.numel()
+        return flat, views

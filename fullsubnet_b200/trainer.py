@@ -1,4 +1,5 @@
-"""Mirror of recipes/dns_interspeech_2020/fullsubnet/trainer.py:14-181 on top of
+"""Mirror of recipes/dns_interspeech_2020/fullsubnet/trainer.py:14-181 (and of fast_fullsubnet/trainer.py, the same loop
+without drop_band) on top of
 audio_zen/trainer/base_trainer.py:28-218 - the parts of the trainer that are arithmetic on the hot path (SURVEY 8a row
 A11, 8f rank 4): STFT of noisy/clean, cIRM target + drop_band, Model.forward, MSE, backward, gradient mean over
 ranks, clip, Adam; and the B=1 validation loop (enhance + loss + SI-SDR, all on the device).
@@ -100,7 +101,8 @@ class Trainer:
         noisy_mag, _, noisy_real, noisy_imag = self.torch_stft(noisy)
         _, _, clean_real, clean_imag = self.torch_stft(clean)
         cIRM = build_complex_ideal_ratio_mask(noisy_real, noisy_imag, clean_real, clean_imag)  # [B, F, T, 2]
-        cIRM = drop_band(cIRM.permute(0, 3, 1, 2), core.num_groups_in_drop_band).permute(0, 2, 3, 1)
+        if hasattr(core, "num_groups_in_drop_band"):  # fullsubnet; fast_fullsubnet/trainer.py:45-56 has no drop_band
+            cIRM = drop_band(cIRM.permute(0, 3, 1, 2), core.num_groups_in_drop_band).permute(0, 2, 3, 1)
         cRM = model(noisy_mag.unsqueeze(1)).permute(0, 2, 3, 1)
         loss = self.loss_function(cIRM, cRM)
         loss.backward()  # under DDP the gradient mean over ranks happens in here (base_trainer.py:32)

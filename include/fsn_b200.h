@@ -193,6 +193,7 @@ typedef struct fsn_fast_desc {
   int32_t noisy_num_neighbors; /* noisy_input_num_neighbors */
   int32_t enc_num_neighbors;   /* encoder_output_num_neighbors */
   int32_t precision;           /* FSN_PREC_* for the bottleneck stack (the tensor-core path needs bn_hidden = 384) */
+  int32_t cell_type;           /* FSN_CELL_* (`sequence_model`); the training step is built for LSTM only */
 } fsn_fast_desc;
 
 typedef struct fsn_fast_weights {
@@ -287,6 +288,26 @@ int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
 int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
                        const float* dcrm, int B, int T, const fsn_seq_grads* gfb, const fsn_seq_grads* gsb,
                        void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+
+/* Training step of recipes/dns_interspeech_2020/fast_fullsubnet/trainer.py:45-56 (the fast recipe), same conventions as
+ * fsn_train_*: the caller allocates the workspace and passes the same untouched buffer from forward to backward; the
+ * gradients of the 30 parameters are OVERWRITTEN; no host synchronisation; arguments are checked before any CUDA call.
+ *   fsn_fast_train_forward  = Model.forward in train mode (fast_fullsubnet/model.py:143-202): out [B,2,F,T], keeping the
+ *                             activations back-propagation through time needs (time-major [Tp, rows, .])
+ *   fsn_fast_train_backward = loss.backward() from dout = d loss / d out [B,2,F,T]
+ * d->precision: FSN_PREC_FP32, or FSN_PREC_TF32_TC (every LSTM layer with H % 4 == 0 on the wgmma tf32 GEMMs, as in
+ * fsn_train_*); any other precision, bn_layers != 2 or the GRU cell -> FSN_ERR_UNSUPPORTED. */
+typedef struct fsn_lstm_grads { float *w_ih, *w_hh, *b_ih, *b_hh; } fsn_lstm_grads;
+typedef struct fsn_fast_grads {
+  fsn_lstm_grads enc1, enc2;  float *enc_fc_w, *enc_fc_b;
+  fsn_lstm_grads bn[2];       float *bn_fc_w,  *bn_fc_b;
+  fsn_lstm_grads dec1, dec2;  float *dec_fc_w, *dec_fc_b;
+} fsn_fast_grads;
+size_t fsn_fast_train_workspace_bytes(const fsn_fast_desc* d, int B, int T);
+int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_weights* w, const float* mix_mag, int B, int T,
+                           float* out, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_weights* w, const float* dout, int B, int T,
+                            const fsn_fast_grads* g, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 size_t fsn_mse_loss_scratch_bytes(void);
 int fsn_mse_loss(const float* cirm, const float* crm, int B, int Fsub, int T, float* loss, float* dcrm,
