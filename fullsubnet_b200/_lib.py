@@ -71,7 +71,11 @@ class ParamList(C.Structure):
 
 class FullbandDesc(C.Structure):
     _fields_ = [("num_freqs", C.c_int32), ("hidden", C.c_int32), ("num_layers", C.c_int32), ("look_ahead", C.c_int32),
-                ("activation", C.c_int32), ("norm_type", C.c_int32)]
+                ("activation", C.c_int32), ("norm_type", C.c_int32), ("precision", C.c_int32), ("cell_type", C.c_int32)]
+
+
+class FullbandGrads(C.Structure):
+    _fields_ = [("layer", LstmGrads * 8), ("fc_w", C.c_void_p), ("fc_b", C.c_void_p)]
 
 
 IMP_MAX_SECTIONS = 8
@@ -133,6 +137,10 @@ _SIGNATURES = {
     "fsn_clip_adam": (C.c_int, [C.POINTER(ParamList), _F, _F, _F, _F, _F, _F, _I, _P, _P, _S, _P]),
     "fsn_fullband_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
     "fsn_fullband_forward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, _P, _P, _S, _P]),
+    "fsn_fullband_train_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
+    "fsn_fullband_train_forward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, _P, _P, _S, _P]),
+    "fsn_fullband_train_backward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, C.POINTER(FullbandGrads), _P,
+                                              _S, _P]),
     "fsn_peak_normalize_int16": (C.c_int, [_P, _I, _I, _F, _P, _P]),
     "fsn_si_sdr": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "fsn_rir_convolve": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P]),

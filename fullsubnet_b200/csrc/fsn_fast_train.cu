@@ -89,36 +89,7 @@ __global__ void ftr_dec_input_kernel(const float* __restrict__ encT, const float
   }
 }
 
-// dec [Tp,B,2F] (channel c*F+f) -> out [B,2,F,T], dropping the first `la` frames (model.py:197-200)
-__global__ void ftr_output_kernel(const float* __restrict__ dec, int B, int Tp, int F, int la, float* __restrict__ out) {
-  __shared__ float tile[32][33];
-  const int T = Tp - la;
-  const int b = blockIdx.z >> 1, c = blockIdx.z & 1;
-  const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  for (int i = ty; i < 32; i += 8) {
-    const int t = t0 + i, f = f0 + tx;
-    tile[i][tx] = (t < T && f < F) ? dec[((size_t)(t + la) * B + b) * (2 * F) + c * F + f] : 0.f;
-  }
-  __syncthreads();
-  for (int i = ty; i < 32; i += 8) {
-    const int f = f0 + i, t = t0 + tx;
-    if (f < F && t < T) out[(((size_t)b * 2 + c) * F + f) * T + t] = tile[tx][i];
-  }
-}
-
 // ------------------------------------------------------------------------------------------ backward kernels
-// dY [Tp,B,2F] from dout [B,2,F,T]; zero on the look-ahead frames
-__global__ void ftr_dy_kernel(const float* __restrict__ dout, int B, int F, int T, int Tp, int la, float* __restrict__ dY) {
-  const size_t n = (size_t)Tp * B * 2 * F;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int cf = (int)(i % (2 * F));
-    const size_t tb = i / (2 * F);
-    const int b = (int)(tb % B), t = (int)(tb / B);
-    dY[i] = t >= la ? dout[((size_t)b * 2 * F + cf) * T + (t - la)] : 0.f;
-  }
-}
-
 // transpose of the up-sampling (frame t <- shrunk step min(t/S, Ts-1)) on the bottleneck half of d dec_in, times ReLU' of
 // the bottleneck output: dbn[ts, r] = [bn_out > 0] * sum over the frames that read ts (ascending t)
 __global__ void ftr_dbn_kernel(const float* __restrict__ ddec, const float* __restrict__ bn_out, int B, int Tp, int M, int S,
@@ -328,22 +299,6 @@ static int transpose_weights(const fsn_fast_desc* d, const fsn_fast_weights* wt,
   return FSN_OK;
 }
 
-// BPTT of a two-layer pair (upper `hi` fed by lower `lo`, one step apart as in fsn_train_backward); d h of the upper layer
-// from dh_above [steps, R, Hhi] or from an O-output Linear on top (dout [steps, R, O], fc_w [O, Hhi]); dx of the lower
-// layer into dx [steps, R, K0lo] when given
-static int pair_bwd(const LayerBwd& hi, const LayerBwd& lo, int steps, const float* dh_above, const float* dout,
-                    const float* fc_w, int O, float* dh_mid, float* dx, cudaStream_t st) {
-  int rc;
-  for (int t = steps - 1; t >= 0; --t) {
-    if ((rc = layer_bwd_step(hi, t, steps, dh_above ? dh_above + (size_t)t * hi.R * hi.H : nullptr,
-                             dout ? dout + (size_t)t * hi.R * O : nullptr, fc_w, O, dh_mid, st)))
-      return rc;
-    if ((rc = layer_bwd_step(lo, t, steps, dh_mid, nullptr, nullptr, 0, dx ? dx + (size_t)t * lo.R * lo.K0 : nullptr, st)))
-      return rc;
-  }
-  return FSN_OK;
-}
-
 static int grid_for(size_t n) {
   size_t g = (n + 255) / 256;
   return (int)(g > 132 * 16 ? 132 * 16 : (g ? g : 1));
@@ -411,9 +366,7 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   if ((rc = fast_layer_forward(d, wt, w, s, L_DEC2, w.L[L_DEC1].H, w.h16[L_DEC1], st))) return rc;
   if ((rc = fc_gemm_launch(w.L[L_DEC2].H, wt->dec_fc_w, wt->dec_fc_b, w.dec_out, Tp * B, d->dec_hidden, 2 * F, FSN_ACT_NONE, st)))
     return rc;
-  ftr_output_kernel<<<dim3(cdiv(T, 32), cdiv(F, 32), B * 2), dim3(32, 8), 0, st>>>(w.dec_out, B, Tp, F, d->look_ahead, out);
-  FSN_CHECK_LAUNCH("ftr_output_kernel");
-  return FSN_OK;
+  return train_output_launch(w.dec_out, B, Tp, F, d->look_ahead, out, st);
 }
 
 extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* dout, int B, int T,
@@ -436,15 +389,15 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   for (int l = 0; l < NL; ++l)
     if ((rc = transpose_weights(d, wt, w, s, l, st))) return rc;
   // ---- decoder Linear(2F) (model.py:196-200 backwards): dW = dY^T H, db = colsum dY, dH = dY W
-  ftr_dy_kernel<<<grid_for((size_t)Tp * B * 2 * F), 256, 0, st>>>(dout, B, F, T, Tp, d->look_ahead, w.dY);
-  FSN_CHECK_LAUNCH("ftr_dy_kernel");
+  if ((rc = train_dy_launch(dout, nullptr, FSN_ACT_NONE, B, F, T, Tp, d->look_ahead, w.dY, st))) return rc;
   if ((rc = sgemm_launch(true, w.dY, 2 * F, w.L[L_DEC2].H, Hd, g->dec_fc_w, Hd, 2 * F, Hd, Tp * B, false, w.splitk, st)))
     return rc;
   if ((rc = colsum_launch(w.dY, (size_t)Tp * B, 2 * F, 2 * F, g->dec_fc_b, nullptr, w.colsum, st))) return rc;
   if ((rc = sgemm_launch(false, w.dY, 2 * F, wt->dec_fc_w, Hd, w.dH, Hd, Tp * B, Hd, 2 * F, false, nullptr, st))) return rc;
   // ---- decoder BPTT, d dec_in
-  const LayerBwd d2 = layer_bwd(d, wt, w, s, L_DEC2, 1), d1 = layer_bwd(d, wt, w, s, L_DEC1, 0);
-  if ((rc = pair_bwd(d2, d1, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, w.ddec, st))) return rc;
+  const LayerBwd dec[2] = {layer_bwd(d, wt, w, s, L_DEC1, 0), layer_bwd(d, wt, w, s, L_DEC2, 1)};
+  const LayerBwd &d1 = dec[0], &d2 = dec[1];
+  if ((rc = stack_bwd(dec, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, w.ddec, st))) return rc;
   if ((rc = layer_weight_grads(d2, Tp, w.L[L_DEC1].H, g->dec2.w_ih, g->dec2.w_hh, g->dec2.b_ih, g->dec2.b_hh, wg, st))) return rc;
   if ((rc = layer_weight_grads(d1, Tp, w.dec_in, g->dec1.w_ih, g->dec1.w_hh, g->dec1.b_ih, g->dec1.b_hh, wg, st))) return rc;
   // ---- up-sampling transpose + ReLU' of the bottleneck output, its Linear(1)
@@ -453,8 +406,9 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   if ((rc = sgemm_launch(true, w.dbn, 1, w.L[L_BN1].H, Hb, g->bn_fc_w, Hb, 1, Hb, Ts * R, false, w.splitk, st))) return rc;
   if ((rc = colsum_launch(w.dbn, (size_t)Ts * R, 1, 1, g->bn_fc_b, nullptr, w.colsum, st))) return rc;
   // ---- bottleneck BPTT (the Linear(1) backward folded into layer 1's point kernel), d X_bn
-  const LayerBwd b1 = layer_bwd(d, wt, w, s, L_BN1, 1), b0 = layer_bwd(d, wt, w, s, L_BN0, 0);
-  if ((rc = pair_bwd(b1, b0, Ts, nullptr, w.dbn, wt->bn_fc_w, 1, w.dh_mid, w.dxbn, st))) return rc;
+  const LayerBwd bn[2] = {layer_bwd(d, wt, w, s, L_BN0, 0), layer_bwd(d, wt, w, s, L_BN1, 1)};
+  const LayerBwd &b0 = bn[0], &b1 = bn[1];
+  if ((rc = stack_bwd(bn, 2, Ts, nullptr, w.dbn, wt->bn_fc_w, 1, w.dh_mid, nullptr, w.dxbn, st))) return rc;
   if ((rc = layer_weight_grads(b1, Ts, w.L[L_BN0].H, g->bn[1].w_ih, g->bn[1].w_hh, g->bn[1].b_ih, g->bn[1].b_hh, wg, st))) return rc;
   if ((rc = layer_weight_grads(b0, Ts, w.xbn, g->bn[0].w_ih, g->bn[0].w_hh, g->bn[0].b_ih, g->bn[0].b_hh, wg, st))) return rc;
   // ---- second norm + down-sampling + unfold backward, ReLU' of the encoder output, its Linear(M)
@@ -468,8 +422,9 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   if ((rc = colsum_launch(w.denc, (size_t)Tp * B, M, M, g->enc_fc_b, nullptr, w.colsum, st))) return rc;
   if ((rc = sgemm_launch(false, w.denc, M, wt->enc_fc_w, He2, w.dH, He2, Tp * B, He2, M, false, nullptr, st))) return rc;
   // ---- encoder BPTT (its input is the normalised mel spectrogram: no dx)
-  const LayerBwd e2 = layer_bwd(d, wt, w, s, L_ENC2, 1), e1 = layer_bwd(d, wt, w, s, L_ENC1, 0);
-  if ((rc = pair_bwd(e2, e1, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, st))) return rc;
+  const LayerBwd enc[2] = {layer_bwd(d, wt, w, s, L_ENC1, 0), layer_bwd(d, wt, w, s, L_ENC2, 1)};
+  const LayerBwd &e1 = enc[0], &e2 = enc[1];
+  if ((rc = stack_bwd(enc, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st))) return rc;
   if ((rc = layer_weight_grads(e2, Tp, w.L[L_ENC1].H, g->enc2.w_ih, g->enc2.w_hh, g->enc2.b_ih, g->enc2.b_hh, wg, st))) return rc;
   return layer_weight_grads(e1, Tp, w.xenc, g->enc1.w_ih, g->enc1.w_hh, g->enc1.b_ih, g->enc1.b_hh, wg, st);
 }

@@ -117,6 +117,25 @@ int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, cons
 // weight / bias gradients of one layer from dG [Tp*R,4H] (in L.s.G), its input X [Tp*R,K0] and hidden states
 int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih, float* g_w_hh, float* g_b_ih, float* g_b_hh,
                        const WgradScratch& w, cudaStream_t st);
+// BPTT of a stack of n layers (L[0] at the bottom), one step at a time from the top: every layer at step t before any at
+// t-1.  The top layer's d h comes from dh_above [steps, R, H] or from an O-output Linear on top (dout [steps, R, O],
+// fc_w [O, H]); layer l < n-1 takes layer l+1's dx of the same step through dh_mid0 / dh_mid1 (alternating; dh_mid1 is
+// used only when n > 2); layer 0's dx goes to dx [steps, R, K0] when given.  Each L[l] carries its own dh_rec / dc slot.
+int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const float* dout, const float* fc_w, int O,
+              float* dh_mid0, float* dh_mid1, float* dx, cudaStream_t st);
+// input of a training step (fullsubnet/model.py:85-92, fullband_baseline/model.py:46-56): look-ahead pad, first norm and
+// the time-major copies raw [Tp,B,F] (unscaled) and scaled [Tp,B,F] (normalised); sums[b] = per-clip (sum, sum_f c_Ns[f]
+// * row sum), inv1[b] = 1 / (mean + eps).  cum: causal running mean instead, fs [B*Tp] frame sums, cum1 [Tp*B] scales
+// (fs / cum1 unused otherwise).
+static const float TRAIN_CUM_EPS = 1.1920928955078125e-07f;  // audio_zen/constant.py:9
+int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, bool cum, float2* sums, float* inv1,
+                       float* raw, float* scaled, float2* fs, float* cum1, cudaStream_t st);
+// output of a Linear(H -> 2F) head: y [Tp,B,2F] (channel c*F+f) -> out [B,2,F,Tp-la], dropping the first `la` frames
+int train_output_launch(const float* y, int B, int Tp, int F, int la, float* out, cudaStream_t st);
+// its backward: dY [Tp,B,2F] = dout [B,2,F,T] re-laid out, zero on the first `la` frames, times act'(y) (FSN_ACT_*) from
+// the kept post-activation output y (unread for FSN_ACT_NONE)
+int train_dy_launch(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
+                    cudaStream_t st);
 // fp32 SIMT GEMM C[M,N] (+)= op(A) B (op(A) = A^T when ta), split-K over `scratch` for long K (deterministic)
 int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
                  bool accumulate, float* scratch, cudaStream_t st);

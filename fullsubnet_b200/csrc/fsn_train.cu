@@ -756,6 +756,97 @@ int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih,
   return colsum_launch(L.s.G, (size_t)rows, H4, H4, g_b_ih, g_b_hh, w.colsum, st);
 }
 
+int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const float* dout, const float* fc_w, int O,
+              float* dh_mid0, float* dh_mid1, float* dx, cudaStream_t st) {
+  float* mid[2] = {dh_mid0, dh_mid1};
+  int rc;
+  for (int t = steps - 1; t >= 0; --t) {
+    for (int l = n - 1; l >= 0; --l) {
+      const LayerBwd& q = L[l];
+      const bool top = l == n - 1;
+      const float* dh = top ? (dh_above ? dh_above + (size_t)t * q.R * q.H : nullptr) : mid[(n - 2 - l) & 1];
+      const float* dl = top && dout ? dout + (size_t)t * q.R * O : nullptr;
+      float* dxl = l > 0 ? mid[(n - 1 - l) & 1] : (dx ? dx + (size_t)t * q.R * q.K0 : nullptr);
+      if ((rc = layer_bwd_step(q, t, steps, dh, dl, top ? fc_w : nullptr, top ? O : 0, dxl, st))) return rc;
+    }
+  }
+  return FSN_OK;
+}
+
+// ------------------------------------------------------------------------------------------ shared by the training steps
+int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, bool cum, float2* sums, float* inv1,
+                       float* raw, float* scaled, float2* fs, float* cum1, cudaStream_t st) {
+  train_mag_stats_kernel<<<B, 256, 0, st>>>(noisy_mag, F, T, Ns, sums);
+  FSN_CHECK_LAUNCH("train_mag_stats_kernel");
+  int rc;
+  if ((rc = norm_scales_launch(sums, sums, B, (float)F * Tp, 1.f, inv1, nullptr, st))) return rc;
+  train_transpose_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(noisy_mag, inv1, raw, scaled, B, F, T, Tp);
+  FSN_CHECK_LAUNCH("train_transpose_kernel");
+  if (cum) {  // causal running mean per clip instead of the clip mean (base_model.py:220-251)
+    train_frame_sum_kernel<<<cdiv(Tp * B, 8), 256, 0, st>>>(raw, B, F, Tp, fs);
+    FSN_CHECK_LAUNCH("train_frame_sum_kernel");
+    if ((rc = cum_clip_scale_launch(fs, B, Tp, F, TRAIN_CUM_EPS, cum1, st))) return rc;
+    train_scale_tm_kernel<<<132 * 8, 256, 0, st>>>(raw, cum1, F, (size_t)Tp * B * F, scaled);
+    FSN_CHECK_LAUNCH("train_scale_tm_kernel");
+  }
+  return FSN_OK;
+}
+
+// y [Tp,B,2F] (channel c*F+f) -> out [B,2,F,T], dropping the first `la` frames
+__global__ void train_output_kernel(const float* __restrict__ y, int B, int Tp, int F, int la, float* __restrict__ out) {
+  __shared__ float tile[32][33];
+  const int T = Tp - la;
+  const int b = blockIdx.z >> 1, c = blockIdx.z & 1;
+  const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  for (int i = ty; i < 32; i += 8) {
+    const int t = t0 + i, f = f0 + tx;
+    tile[i][tx] = (t < T && f < F) ? y[((size_t)(t + la) * B + b) * (2 * F) + c * F + f] : 0.f;
+  }
+  __syncthreads();
+  for (int i = ty; i < 32; i += 8) {
+    const int f = f0 + i, t = t0 + tx;
+    if (f < F && t < T) out[(((size_t)b * 2 + c) * F + f) * T + t] = tile[tx][i];
+  }
+}
+
+int train_output_launch(const float* y, int B, int Tp, int F, int la, float* out, cudaStream_t st) {
+  train_output_kernel<<<dim3(cdiv(Tp - la, 32), cdiv(F, 32), B * 2), dim3(32, 8), 0, st>>>(y, B, Tp, F, la, out);
+  FSN_CHECK_LAUNCH("train_output_kernel");
+  return FSN_OK;
+}
+
+// dY [Tp,B,2F] from dout [B,2,F,T], zero on the look-ahead frames, times act'(y) of the kept post-activation output
+__global__ void train_dy_kernel(const float* __restrict__ dout, const float* __restrict__ y, int act, int B, int F, int T,
+                                int Tp, int la, float* __restrict__ dY) {
+  const size_t n = (size_t)Tp * B * 2 * F;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int cf = (int)(i % (2 * F));
+    const size_t tb = i / (2 * F);
+    const int b = (int)(tb % B), t = (int)(tb / B);
+    float v = t >= la ? dout[((size_t)b * 2 * F + cf) * T + (t - la)] : 0.f;
+    if (act == FSN_ACT_RELU) {
+      v = y[i] > 0.f ? v : 0.f;
+    } else if (act == FSN_ACT_RELU6) {
+      const float a = y[i];
+      v = (a > 0.f && a < 6.f) ? v : 0.f;
+    } else if (act == FSN_ACT_TANH) {
+      const float a = y[i];
+      v *= 1.f - a * a;
+    }
+    dY[i] = v;
+  }
+}
+
+int train_dy_launch(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
+                    cudaStream_t st) {
+  size_t g = ((size_t)Tp * B * 2 * F + 255) / 256;
+  if (g > 132 * 16) g = 132 * 16;
+  train_dy_kernel<<<(int)g, 256, 0, st>>>(dout, y, act, B, F, T, Tp, la, dY);
+  FSN_CHECK_LAUNCH("train_dy_kernel");
+  return FSN_OK;
+}
+
 }  // namespace fsn
 
 using namespace fsn;
@@ -783,21 +874,10 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   cudaStream_t st = (cudaStream_t)stream;
   const int Tp = m.Tp, F = m.F, Hf = d->fb_hidden, Hs = d->sb_hidden;
   // first norm (model.py:92) and the time-major copies
-  train_mag_stats_kernel<<<B, 256, 0, st>>>(noisy_mag, F, T, d->sb_num_neighbors, w.sums_mag);
-  FSN_CHECK_LAUNCH("train_mag_stats_kernel");
-  if ((rc = norm_scales_launch(w.sums_mag, w.sums_mag, B, (float)F * Tp, 1.f, w.inv1, nullptr, st))) return rc;
-  train_transpose_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(noisy_mag, w.inv1, w.raw, w.xfb, B,
-                                                                                     F, T, Tp);
-  FSN_CHECK_LAUNCH("train_transpose_kernel");
   const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
-  const float cum_eps = 1.1920928955078125e-07f;  // audio_zen/constant.py:9
-  if (cum) {  // causal running mean per clip instead of the clip mean (base_model.py:220-251)
-    train_frame_sum_kernel<<<cdiv(Tp * B, 8), 256, 0, st>>>(w.raw, B, F, Tp, w.fs);
-    FSN_CHECK_LAUNCH("train_frame_sum_kernel");
-    if ((rc = cum_clip_scale_launch(w.fs, B, Tp, F, cum_eps, w.cum1, st))) return rc;
-    train_scale_tm_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.cum1, F, (size_t)Tp * B * F, w.xfb);
-    FSN_CHECK_LAUNCH("train_scale_tm_kernel");
-  }
+  if ((rc = train_input_launch(noisy_mag, B, F, T, Tp, d->sb_num_neighbors, cum, w.sums_mag, w.inv1, w.raw, w.xfb, w.fs,
+                               w.cum1, st)))
+    return rc;
   // full-band stack + Linear/activation (model.py:92-95)
   const bool tc_fb = tc_layer_ok(d, Hf), tc_sb = tc_layer_ok(d, Hs);
   // fp16 operand copies: layer 0's hidden states double as layer 1's input
@@ -817,7 +897,7 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   if ((rc = norm_scales_launch(w.sums_mag, w.sums_fb, B, 1.f, (float)F * m.Ksb * Tp, nullptr, w.inv2, st))) return rc;
   // sub-band units (unfold + concat + norm + drop_band as one gather), then the sub-band stack (model.py:98-128)
   RowMap map{B, F, m.Fsub, m.G};
-  if (cum && (rc = cum_unit_scale_launch(w.raw, w.fbz, map, m.R, Tp, d->sb_num_neighbors, d->fb_num_neighbors, cum_eps, w.cum2,
+  if (cum && (rc = cum_unit_scale_launch(w.raw, w.fbz, map, m.R, Tp, d->sb_num_neighbors, d->fb_num_neighbors, TRAIN_CUM_EPS, w.cum2,
                                          st, /*time_major=*/true)))
     return rc;
   train_gather_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.fbz, w.inv2, cum ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,

@@ -1,5 +1,5 @@
-"""Mirror of recipes/dns_interspeech_2020/fullsubnet/trainer.py:14-181 (and of fast_fullsubnet/trainer.py, the same loop
-without drop_band) on top of
+"""Mirror of recipes/dns_interspeech_2020/fullsubnet/trainer.py:14-181 (and of fast_fullsubnet/trainer.py and
+fullband_baseline/trainer.py:32-71, the same loop without drop_band) on top of
 audio_zen/trainer/base_trainer.py:28-218 - the parts of the trainer that are arithmetic on the hot path (SURVEY 8a row
 A11, 8f rank 4): STFT of noisy/clean, cIRM target + drop_band, Model.forward, MSE, backward, gradient mean over
 ranks, clip, Adam; and the B=1 validation loop (enhance + loss + SI-SDR, all on the device).

@@ -338,12 +338,35 @@ typedef struct fsn_fullband_desc {
   int32_t look_ahead;
   int32_t activation; /* FSN_ACT_* */
   int32_t norm_type;  /* FSN_NORM_* */
+  int32_t precision;  /* training only: FSN_PREC_FP32 (0) or FSN_PREC_TF32_TC */
+  int32_t cell_type;  /* training only: FSN_CELL_* (0 = LSTM; the training step is built for LSTM only) */
 } fsn_fullband_desc;
 
 size_t fsn_fullband_workspace_bytes(const fsn_fullband_desc* d, int B, int T);
 int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w, const float* fc_b,
                          const float* noisy_mag, int B, int T, float* out, void* workspace, size_t workspace_bytes,
                          fsn_stream_t stream);
+
+/* Training step of recipes/dns_interspeech_2020/fullband_baseline/trainer.py:32-71, same conventions as fsn_train_*: the
+ * caller allocates the workspace and passes the same untouched buffer from forward to backward; the gradients of all
+ * 4 * num_layers + 2 parameters are OVERWRITTEN; no host synchronisation; arguments are checked before any CUDA call;
+ * every sum runs in a fixed order (two runs give identical bits).
+ *   fsn_fullband_train_forward  = Model.forward with gradients enabled: out [B,2,F,T], keeping the activations
+ *                                 back-propagation through time needs (time-major [Tp, B, .])
+ *   fsn_fullband_train_backward = loss.backward() from dout = d loss / d out [B,2,F,T]; g->layer[l] for l < num_layers
+ * d->precision: FSN_PREC_FP32, or FSN_PREC_TF32_TC (the LSTM layers on the wgmma tf32 GEMMs when hidden % 4 == 0, as in
+ * fsn_train_*); any other precision, the GRU cell, num_layers outside 1..8 or another norm -> FSN_ERR_UNSUPPORTED. */
+typedef struct fsn_fullband_grads {
+  fsn_lstm_grads layer[8];
+  float *fc_w, *fc_b;
+} fsn_fullband_grads;
+size_t fsn_fullband_train_workspace_bytes(const fsn_fullband_desc* d, int B, int T);
+int fsn_fullband_train_forward(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,
+                               const float* fc_b, const float* noisy_mag, int B, int T, float* out, void* workspace,
+                               size_t workspace_bytes, fsn_stream_t stream);
+int fsn_fullband_train_backward(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,
+                                const float* fc_b, const float* dout, int B, int T, const fsn_fullband_grads* g,
+                                void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 /* audio_zen/inferencer/base_inferencer.py:181-182 (SURVEY 8f rank 2): out = int16(gain * wav / max|wav|) per clip,
  * gain = 0.8 * 32767 in the reference; float32 multiply, divide, truncation toward zero like numpy; all-zero clip -> 0 */
