@@ -107,16 +107,6 @@ static bool fast_lstm_tc(const fsn_fast_desc* d) {
          lstm_rec_tc_supported(d->dec_hidden, x3);
 }
 
-struct FCarver {
-  char* base; size_t off;
-  explicit FCarver(void* p) : base((char*)p), off(0) {}
-  template <class T> T* take(size_t n) {
-    T* r = base ? (T*)(base + off) : nullptr;
-    off = align_up(off + n * sizeof(T), 256);
-    return r;
-  }
-};
-
 int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m) {
   FSN_REQUIRE(d && d->num_freqs > 1 && d->num_mels > 1 && d->shrink_size >= 1 && d->look_ahead >= 0, FSN_ERR_SHAPE,
               "fast model: bad descriptor");
@@ -132,7 +122,7 @@ int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m) {
 }
 
 static void fast_carve(const fsn_fast_desc* d, const FastDims& m, void* base, FastWs& w) {
-  FCarver c(base);
+  Carver c(base);
   const size_t BT = (size_t)m.B * m.Tp, R = (size_t)m.B * m.M;
   w.magT = c.take<float>(BT * m.F);
   w.melT = c.take<float>(BT * m.M);
@@ -166,7 +156,7 @@ static void fast_carve(const fsn_fast_desc* d, const FastDims& m, void* base, Fa
     int Hm = d->enc1_hidden > d->enc2_hidden ? d->enc1_hidden : d->enc2_hidden;
     if (d->dec_hidden > Hm) Hm = d->dec_hidden;
     int Km = Hm > 2 * m.M ? Hm : 2 * m.M;
-    lstm_tc_carve(c.base, c.off, BT, Km, Hm, d->precision == FSN_PREC_F16X3_TC, w.tc);
+    lstm_tc_carve(c, BT, Km, Hm, d->precision == FSN_PREC_F16X3_TC, w.tc);
     w.tc_mid = c.take<float>(BT * (d->enc1_hidden > d->dec_hidden ? d->enc1_hidden : d->dec_hidden));
   }
   w.bytes = c.off;

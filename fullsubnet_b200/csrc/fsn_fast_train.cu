@@ -6,8 +6,6 @@
 // Everything is time-major ([Tp, rows, .], the bottleneck [Ts, B*M, .]) like fsn_train.cu, so the LSTM layers reuse its
 // activation-saving forward, its per-step backward and its weight-gradient GEMMs.  Every reduction runs in a fixed order:
 // two runs give identical bits.  oracle/fast_fullsubnet_oracle.py:fast_model_forward under CPU autograd is the reference.
-#include <string.h>
-
 #include "fsn_internal.cuh"
 
 namespace fsn {
@@ -156,16 +154,6 @@ struct FastTrainWs {
 
 struct LayerShape { int R, K0, H, steps; };
 
-struct FCarverT {
-  char* base; size_t off;
-  explicit FCarverT(void* p) : base((char*)p), off(0) {}
-  template <class T> T* take(size_t n) {
-    T* r = base ? (T*)(base + off) : nullptr;
-    off = align_up(off + n * sizeof(T), 256);
-    return r;
-  }
-};
-
 static void layer_shapes(const fsn_fast_desc* d, const FastDims& m, LayerShape* s) {
   const int R = m.B * m.M;
   s[L_ENC1] = {m.B, m.M, d->enc1_hidden, m.Tp};
@@ -176,16 +164,13 @@ static void layer_shapes(const fsn_fast_desc* d, const FastDims& m, LayerShape* 
   s[L_DEC2] = {m.B, d->dec_hidden, d->dec_hidden, m.Tp};
 }
 
-// the same per-layer choice as fsn_train_forward / fsn_train_backward
-static bool tc_layer(const fsn_fast_desc* d, int H) { return d->precision == FSN_PREC_TF32_TC && (H & 3) == 0; }
-
 // the encoder input (normalised mel spectrogram) needs no gradient: no dx GEMM, no transposed W_ih
 static bool dx_tf32(int l) { return l != L_ENC1; }
 
 static size_t smax(size_t a, size_t b) { return a > b ? a : b; }
 
 static void carve_fast_train(const fsn_fast_desc* d, const FastDims& m, void* base, FastTrainWs& w) {
-  FCarverT c(base);
+  Carver c(base);
   const size_t Tp = m.Tp, B = m.B, F = m.F, M = m.M, K = m.K, Ts = m.Ts, R = (size_t)m.B * m.M;
   LayerShape s[NL];
   layer_shapes(d, m, s);
@@ -206,7 +191,7 @@ static void carve_fast_train(const fsn_fast_desc* d, const FastDims& m, void* ba
     rh = smax(rh, (size_t)s[l].R * H);
     hmax = smax(hmax, H);
     wmax = smax(wmax, 4 * H * (H + s[l].K0));
-    if (tc_layer(d, s[l].H)) {
+    if (tf32_layer(d->precision, s[l].H)) {
       g_blk = smax(g_blk, tgemm_blocked_floats(rows, 4 * s[l].H));
       x_blk = smax(x_blk, tgemm_blocked_floats(rows, s[l].K0 > s[l].H ? s[l].K0 : s[l].H));
     }
@@ -226,7 +211,7 @@ static void carve_fast_train(const fsn_fast_desc* d, const FastDims& m, void* ba
   for (int l = 0; l < NL; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
   if (d->precision == FSN_PREC_TF32_TC) {
     for (int l = 0; l < NL; ++l) {
-      if (!tc_layer(d, s[l].H)) continue;
+      if (!tf32_layer(d->precision, s[l].H)) continue;
       const size_t H = s[l].H;
       w.whhT[l] = c.take<float>(H * 4 * H);
       if (dx_tf32(l)) w.wihT[l] = c.take<float>((size_t)s[l].K0 * 4 * H);
@@ -254,11 +239,6 @@ static int fast_train_check(const fsn_fast_desc* d, int B, int T, FastDims& m) {
   return FSN_OK;
 }
 
-static void seq_of(const fsn_lstm_layer& l, fsn_seq_weights& s) {
-  memset(&s, 0, sizeof(s));
-  s.w_ih[0] = l.w_ih; s.w_hh[0] = l.w_hh; s.b_ih[0] = l.b_ih; s.b_hh[0] = l.b_hh;
-}
-
 static const fsn_lstm_layer& layer_weights(const fsn_fast_weights* wt, int l) {
   switch (l) {
     case L_ENC1: return wt->enc1;
@@ -268,35 +248,6 @@ static const fsn_lstm_layer& layer_weights(const fsn_fast_weights* wt, int l) {
     case L_DEC1: return wt->dec1;
     default: return wt->dec2;
   }
-}
-
-// forward of layer l over its steps from X [steps, R, K0]; X16 = fp16 copy of X left by the layer below (or nullptr)
-static int fast_layer_forward(const fsn_fast_desc* d, const fsn_fast_weights* wt, const FastTrainWs& w, const LayerShape* s,
-                              int l, const float* X, const __half* X16, cudaStream_t st) {
-  fsn_seq_weights sw;
-  seq_of(layer_weights(wt, l), sw);
-  const LayerShape& q = s[l];
-  if (!tc_layer(d, q.H)) return layer_forward_save(&sw, 0, X, q.R, q.K0, q.H, q.steps, w.L[l], st);
-  const LayerHalf half{w.h16[l], X16, w.w16};
-  return layer_forward_save_tc(&sw, 0, X, q.R, q.K0, q.H, q.steps, w.L[l], w.rec, st, w.splitk, SPLITK_SCRATCH_FLOATS, &half);
-}
-
-static LayerBwd layer_bwd(const fsn_fast_desc* d, const fsn_fast_weights* wt, const FastTrainWs& w, const LayerShape* s,
-                          int l, int slot) {
-  const fsn_lstm_layer& lw = layer_weights(wt, l);
-  const bool tc = tc_layer(d, s[l].H);
-  return LayerBwd{lw.w_ih, lw.w_hh, w.L[l], s[l].R, s[l].K0, s[l].H, w.dh_rec[slot], w.dc[slot],
-                  tc ? w.whhT[l] : nullptr, tc ? w.wihT[l] : nullptr, w.splitk};
-}
-
-static int transpose_weights(const fsn_fast_desc* d, const fsn_fast_weights* wt, const FastTrainWs& w, const LayerShape* s,
-                             int l, cudaStream_t st) {
-  if (!tc_layer(d, s[l].H)) return FSN_OK;
-  const fsn_lstm_layer& lw = layer_weights(wt, l);
-  int rc;
-  if ((rc = transpose_launch(lw.w_hh, (size_t)4 * s[l].H, s[l].H, w.whhT[l], st))) return rc;
-  if (w.wihT[l] && (rc = transpose_launch(lw.w_ih, (size_t)4 * s[l].H, s[l].K0, w.wihT[l], st))) return rc;
-  return FSN_OK;
 }
 
 static int grid_for(size_t n) {
@@ -331,6 +282,12 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   const int Tp = m.Tp, F = m.F, M = m.M, K = m.K, Ts = m.Ts, R = B * M;
   LayerShape s[NL];
   layer_shapes(d, m, s);
+  // layer l over its steps from X [steps, R, K0]; X16 = fp16 copy of X left by the layer below (or nullptr)
+  auto layer = [&](int l, const float* X, const __half* X16) {
+    const LayerHalf half{w.h16[l], X16, w.w16};
+    return layer_forward(d->precision, layer_weights(wt, l), X, s[l].R, s[l].K0, s[l].H, s[l].steps, w.L[l], w.rec, w.splitk,
+                         &half, st);
+  };
   // look-ahead pad + time-major layout, Mel filtering (model.py:161-166)
   ftr_transpose_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(mix_mag, w.magT, B, F, T, Tp);
   FSN_CHECK_LAUNCH("ftr_transpose_kernel");
@@ -342,8 +299,8 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   ftr_scale_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.melT, w.inv1, (size_t)Tp * B * M, M, B, 1, w.xenc);
   FSN_CHECK_LAUNCH("ftr_scale_kernel");
   // encoder: LSTM(M->He1), LSTM(He1->He2) + Linear(M) + ReLU (model.py:35-54,171)
-  if ((rc = fast_layer_forward(d, wt, w, s, L_ENC1, w.xenc, nullptr, st))) return rc;
-  if ((rc = fast_layer_forward(d, wt, w, s, L_ENC2, w.L[L_ENC1].H, nullptr, st))) return rc;  // He1 != He2: no shared fp16 path
+  if ((rc = layer(L_ENC1, w.xenc, nullptr))) return rc;
+  if ((rc = layer(L_ENC2, w.L[L_ENC1].H, nullptr))) return rc;  // He1 != He2: no shared fp16 path
   if ((rc = fc_gemm_launch(w.L[L_ENC2].H, wt->enc_fc_w, wt->enc_fc_b, w.encT, Tp * B, d->enc2_hidden, M, FSN_ACT_RELU, st)))
     return rc;
   // bottleneck input: unfold + concat + down-sampling, its norm; the normalised input is kept (model.py:174-187)
@@ -355,15 +312,15 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   ftr_scale_kernel<<<grid_for((size_t)Ts * R * K), 256, 0, st>>>(w.xbn, w.inv2, (size_t)Ts * R * K, K, R, M, w.xbn);
   FSN_CHECK_LAUNCH("ftr_scale_kernel");
   // bottleneck 2xLSTM(K->Hb->Hb) + Linear(1) + ReLU over Ts steps (model.py:188-189)
-  if ((rc = fast_layer_forward(d, wt, w, s, L_BN0, w.xbn, nullptr, st))) return rc;
-  if ((rc = fast_layer_forward(d, wt, w, s, L_BN1, w.L[L_BN0].H, w.h16[L_BN0], st))) return rc;
+  if ((rc = layer(L_BN0, w.xbn, nullptr))) return rc;
+  if ((rc = layer(L_BN1, w.L[L_BN0].H, w.h16[L_BN0]))) return rc;
   if ((rc = rows_fc_launch(w.L[L_BN1].H, Ts * R, d->bn_hidden, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out, 1, 0, st)))
     return rc;
   // up-sampling + concat, decoder LSTM(2M->Hd), LSTM(Hd->Hd) + Linear(2F) (model.py:191-196)
   ftr_dec_input_kernel<<<grid_for((size_t)Tp * B * 2 * M), 256, 0, st>>>(w.encT, w.bn_out, B, Tp, M, m.S, Ts, w.dec_in);
   FSN_CHECK_LAUNCH("ftr_dec_input_kernel");
-  if ((rc = fast_layer_forward(d, wt, w, s, L_DEC1, w.dec_in, nullptr, st))) return rc;
-  if ((rc = fast_layer_forward(d, wt, w, s, L_DEC2, w.L[L_DEC1].H, w.h16[L_DEC1], st))) return rc;
+  if ((rc = layer(L_DEC1, w.dec_in, nullptr))) return rc;
+  if ((rc = layer(L_DEC2, w.L[L_DEC1].H, w.h16[L_DEC1]))) return rc;
   if ((rc = fc_gemm_launch(w.L[L_DEC2].H, wt->dec_fc_w, wt->dec_fc_b, w.dec_out, Tp * B, d->dec_hidden, 2 * F, FSN_ACT_NONE, st)))
     return rc;
   return train_output_launch(w.dec_out, B, Tp, F, d->look_ahead, out, st);
@@ -386,31 +343,37 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   LayerShape s[NL];
   layer_shapes(d, m, s);
   const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
-  for (int l = 0; l < NL; ++l)
-    if ((rc = transpose_weights(d, wt, w, s, l, st))) return rc;
-  // ---- decoder Linear(2F) (model.py:196-200 backwards): dW = dY^T H, db = colsum dY, dH = dY W
+  // the lower layer of each pair keeps its BPTT state in dh_rec[0] / dc[0], the upper one in dh_rec[1] / dc[1]
+  LayerBwd L[NL];
+  for (int l = 0; l < NL; ++l) {
+    const fsn_lstm_layer& lw = layer_weights(wt, l);
+    L[l] = LayerBwd{lw.w_ih, lw.w_hh, w.L[l], s[l].R, s[l].K0, s[l].H, w.dh_rec[l & 1], w.dc[l & 1], w.whhT[l], w.wihT[l],
+                    w.splitk};
+    if ((rc = layer_bwd_transpose_weights(L[l], st))) return rc;
+  }
+  // ---- decoder Linear(2F) (model.py:196-200 backwards)
   if ((rc = train_dy_launch(dout, nullptr, FSN_ACT_NONE, B, F, T, Tp, d->look_ahead, w.dY, st))) return rc;
-  if ((rc = sgemm_launch(true, w.dY, 2 * F, w.L[L_DEC2].H, Hd, g->dec_fc_w, Hd, 2 * F, Hd, Tp * B, false, w.splitk, st)))
+  if ((rc = linear_bwd(w.dY, w.L[L_DEC2].H, wt->dec_fc_w, Tp * B, 2 * F, Hd, g->dec_fc_w, g->dec_fc_b, w.dH, w.splitk,
+                       w.colsum, st)))
     return rc;
-  if ((rc = colsum_launch(w.dY, (size_t)Tp * B, 2 * F, 2 * F, g->dec_fc_b, nullptr, w.colsum, st))) return rc;
-  if ((rc = sgemm_launch(false, w.dY, 2 * F, wt->dec_fc_w, Hd, w.dH, Hd, Tp * B, Hd, 2 * F, false, nullptr, st))) return rc;
   // ---- decoder BPTT, d dec_in
-  const LayerBwd dec[2] = {layer_bwd(d, wt, w, s, L_DEC1, 0), layer_bwd(d, wt, w, s, L_DEC2, 1)};
-  const LayerBwd &d1 = dec[0], &d2 = dec[1];
-  if ((rc = stack_bwd(dec, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, w.ddec, st))) return rc;
-  if ((rc = layer_weight_grads(d2, Tp, w.L[L_DEC1].H, g->dec2.w_ih, g->dec2.w_hh, g->dec2.b_ih, g->dec2.b_hh, wg, st))) return rc;
-  if ((rc = layer_weight_grads(d1, Tp, w.dec_in, g->dec1.w_ih, g->dec1.w_hh, g->dec1.b_ih, g->dec1.b_hh, wg, st))) return rc;
+  if ((rc = stack_bwd(L + L_DEC1, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, w.ddec, st))) return rc;
+  if ((rc = layer_weight_grads(L[L_DEC2], Tp, w.L[L_DEC1].H, g->dec2.w_ih, g->dec2.w_hh, g->dec2.b_ih, g->dec2.b_hh, wg, st)))
+    return rc;
+  if ((rc = layer_weight_grads(L[L_DEC1], Tp, w.dec_in, g->dec1.w_ih, g->dec1.w_hh, g->dec1.b_ih, g->dec1.b_hh, wg, st)))
+    return rc;
   // ---- up-sampling transpose + ReLU' of the bottleneck output, its Linear(1)
   ftr_dbn_kernel<<<grid_for((size_t)Ts * R), 256, 0, st>>>(w.ddec, w.bn_out, B, Tp, M, m.S, Ts, w.dbn);
   FSN_CHECK_LAUNCH("ftr_dbn_kernel");
-  if ((rc = sgemm_launch(true, w.dbn, 1, w.L[L_BN1].H, Hb, g->bn_fc_w, Hb, 1, Hb, Ts * R, false, w.splitk, st))) return rc;
-  if ((rc = colsum_launch(w.dbn, (size_t)Ts * R, 1, 1, g->bn_fc_b, nullptr, w.colsum, st))) return rc;
+  if ((rc = linear_bwd(w.dbn, w.L[L_BN1].H, wt->bn_fc_w, Ts * R, 1, Hb, g->bn_fc_w, g->bn_fc_b, nullptr, w.splitk, w.colsum,
+                       st)))
+    return rc;
   // ---- bottleneck BPTT (the Linear(1) backward folded into layer 1's point kernel), d X_bn
-  const LayerBwd bn[2] = {layer_bwd(d, wt, w, s, L_BN0, 0), layer_bwd(d, wt, w, s, L_BN1, 1)};
-  const LayerBwd &b0 = bn[0], &b1 = bn[1];
-  if ((rc = stack_bwd(bn, 2, Ts, nullptr, w.dbn, wt->bn_fc_w, 1, w.dh_mid, nullptr, w.dxbn, st))) return rc;
-  if ((rc = layer_weight_grads(b1, Ts, w.L[L_BN0].H, g->bn[1].w_ih, g->bn[1].w_hh, g->bn[1].b_ih, g->bn[1].b_hh, wg, st))) return rc;
-  if ((rc = layer_weight_grads(b0, Ts, w.xbn, g->bn[0].w_ih, g->bn[0].w_hh, g->bn[0].b_ih, g->bn[0].b_hh, wg, st))) return rc;
+  if ((rc = stack_bwd(L + L_BN0, 2, Ts, nullptr, w.dbn, wt->bn_fc_w, 1, w.dh_mid, nullptr, w.dxbn, st))) return rc;
+  if ((rc = layer_weight_grads(L[L_BN1], Ts, w.L[L_BN0].H, g->bn[1].w_ih, g->bn[1].w_hh, g->bn[1].b_ih, g->bn[1].b_hh, wg, st)))
+    return rc;
+  if ((rc = layer_weight_grads(L[L_BN0], Ts, w.xbn, g->bn[0].w_ih, g->bn[0].w_hh, g->bn[0].b_ih, g->bn[0].b_hh, wg, st)))
+    return rc;
   // ---- second norm + down-sampling + unfold backward, ReLU' of the encoder output, its Linear(M)
   train_dot_kernel<<<B, 256, 0, st>>>(w.dxbn, w.xbn, Ts, R, M, K, w.dot);
   FSN_CHECK_LAUNCH("train_dot_kernel");
@@ -418,13 +381,12 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
                                                                 d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
                                                                 (float)M * K * Ts, w.denc);
   FSN_CHECK_LAUNCH("ftr_denc_kernel");
-  if ((rc = sgemm_launch(true, w.denc, M, w.L[L_ENC2].H, He2, g->enc_fc_w, He2, M, He2, Tp * B, false, w.splitk, st))) return rc;
-  if ((rc = colsum_launch(w.denc, (size_t)Tp * B, M, M, g->enc_fc_b, nullptr, w.colsum, st))) return rc;
-  if ((rc = sgemm_launch(false, w.denc, M, wt->enc_fc_w, He2, w.dH, He2, Tp * B, He2, M, false, nullptr, st))) return rc;
+  if ((rc = linear_bwd(w.denc, w.L[L_ENC2].H, wt->enc_fc_w, Tp * B, M, He2, g->enc_fc_w, g->enc_fc_b, w.dH, w.splitk, w.colsum,
+                       st)))
+    return rc;
   // ---- encoder BPTT (its input is the normalised mel spectrogram: no dx)
-  const LayerBwd enc[2] = {layer_bwd(d, wt, w, s, L_ENC1, 0), layer_bwd(d, wt, w, s, L_ENC2, 1)};
-  const LayerBwd &e1 = enc[0], &e2 = enc[1];
-  if ((rc = stack_bwd(enc, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st))) return rc;
-  if ((rc = layer_weight_grads(e2, Tp, w.L[L_ENC1].H, g->enc2.w_ih, g->enc2.w_hh, g->enc2.b_ih, g->enc2.b_hh, wg, st))) return rc;
-  return layer_weight_grads(e1, Tp, w.xenc, g->enc1.w_ih, g->enc1.w_hh, g->enc1.b_ih, g->enc1.b_hh, wg, st);
+  if ((rc = stack_bwd(L + L_ENC1, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st))) return rc;
+  if ((rc = layer_weight_grads(L[L_ENC2], Tp, w.L[L_ENC1].H, g->enc2.w_ih, g->enc2.w_hh, g->enc2.b_ih, g->enc2.b_hh, wg, st)))
+    return rc;
+  return layer_weight_grads(L[L_ENC1], Tp, w.xenc, g->enc1.w_ih, g->enc1.w_hh, g->enc1.b_ih, g->enc1.b_hh, wg, st);
 }

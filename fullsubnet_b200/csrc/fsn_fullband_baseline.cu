@@ -39,22 +39,20 @@ static int fbb_check(const fsn_fullband_desc* d, int B, int T) {
 }
 
 static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbWs& w) {
-  char* p = (char*)base;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { void* r = p ? p + off : nullptr; off = align_up(off + bytes, 256); return r; };
+  Carver c(base);
   const size_t Tp = (size_t)T + d->look_ahead, F = d->num_freqs, H = d->hidden;
-  w.magT = (float*)take(B * Tp * F * 4);
-  w.fs = (float2*)take(B * Tp * 8);
-  w.sums = (float2*)take((size_t)B * 8);
-  w.inv1 = (float*)take((size_t)B * 4);
-  w.cum1 = (float*)take(B * Tp * 4);
-  w.seq[0] = (float*)take(B * Tp * H * 4);
-  w.seq[1] = (float*)take(B * Tp * H * 4);
-  w.c = (float*)take((size_t)B * H * 4);
-  w.pp = (float*)take((size_t)2 * 256 * H * 4);
-  w.barrier = (unsigned int*)take(256);
-  w.y = (float*)take(B * Tp * 2 * F * 4);
-  w.bytes = off;
+  w.magT = c.take<float>(B * Tp * F);
+  w.fs = c.take<float2>(B * Tp);
+  w.sums = c.take<float2>(B);
+  w.inv1 = c.take<float>(B);
+  w.cum1 = c.take<float>(B * Tp);
+  w.seq[0] = c.take<float>(B * Tp * H);
+  w.seq[1] = c.take<float>(B * Tp * H);
+  w.c = c.take<float>((size_t)B * H);
+  w.pp = c.take<float>((size_t)2 * 256 * H);
+  w.barrier = c.take<unsigned int>(64);
+  w.y = c.take<float>(B * Tp * 2 * F);
+  w.bytes = c.off;
 }
 
 }  // namespace fsn

@@ -6,8 +6,6 @@
 // per-step backward and the weight-gradient GEMMs are the ones of the fullsubnet step.  The normalised input has no
 // parameter behind it, so the norm needs no backward.  Every reduction runs in a fixed order: two runs give identical bits.
 // oracle/fullband_baseline_oracle.py:fbb_forward under CPU autograd is the reference.
-#include <string.h>
-
 #include "fsn_internal.cuh"
 
 namespace fsn {
@@ -26,23 +24,10 @@ struct FbbTrainWs {
   size_t bytes;
 };
 
-struct FbbCarver {
-  char* base; size_t off;
-  explicit FbbCarver(void* p) : base((char*)p), off(0) {}
-  template <class T> T* take(size_t n) {
-    T* r = base ? (T*)(base + off) : nullptr;
-    off = align_up(off + n * sizeof(T), 256);
-    return r;
-  }
-};
-
-// the same per-layer choice as fsn_train_* / fsn_fast_train_*
-static bool fbb_tc(const fsn_fullband_desc* d) { return d->precision == FSN_PREC_TF32_TC && (d->hidden & 3) == 0; }
-
 static int fbb_in_width(const fsn_fullband_desc* d, int l) { return l == 0 ? d->num_freqs : d->hidden; }
 
 static void carve_fbb_train(const fsn_fullband_desc* d, int B, int T, void* base, FbbTrainWs& w) {
-  FbbCarver c(base);
+  Carver c(base);
   const size_t Tp = (size_t)T + d->look_ahead, F = d->num_freqs, H = d->hidden, NL = d->num_layers;
   const size_t rows = Tp * B, K0max = F > H ? F : H;
   w.raw = c.take<float>(rows * F);
@@ -68,7 +53,7 @@ static void carve_fbb_train(const fsn_fullband_desc* d, int B, int T, void* base
   w.gT = w.xT = w.rec = nullptr;
   w.w16 = nullptr;
   for (int l = 0; l < FBB_MAX_LAYERS; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
-  if (fbb_tc(d)) {
+  if (tf32_layer(d->precision, d->hidden)) {
     for (size_t l = 0; l < NL; ++l) {
       w.whhT[l] = c.take<float>(H * 4 * H);
       if (l > 0) w.wihT[l] = c.take<float>(H * 4 * H);  // layer 0 computes no dx
@@ -94,12 +79,6 @@ static int fbb_train_check(const fsn_fullband_desc* d, int B, int T) {
               "fullband training: offline_laplace_norm and cumulative_laplace_norm are built");
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "fullband training: empty input (B=%d, T=%d)", B, T);
   return FSN_OK;
-}
-
-static LayerBwd fbb_layer_bwd(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const FbbTrainWs& w, int B, int l) {
-  const bool tc = fbb_tc(d);
-  return LayerBwd{layers[l].w_ih, layers[l].w_hh, w.L[l], B, fbb_in_width(d, l), d->hidden, w.dh_rec[l], w.dc[l],
-                  tc ? w.whhT[l] : nullptr, tc ? w.wihT[l] : nullptr, w.splitk};
 }
 
 }  // namespace fsn
@@ -131,20 +110,11 @@ extern "C" int fsn_fullband_train_forward(const fsn_fullband_desc* d, const fsn_
                                w.xfb, w.fs, w.cum1, st)))
     return rc;
   // num_layers x LSTM (model.py:57); on tf32_tc layer l's fp16 hidden states are layer l+1's fp16 input
-  const bool tc = fbb_tc(d);
   for (int l = 0; l < NL; ++l) {
-    fsn_seq_weights sw;
-    memset(&sw, 0, sizeof(sw));
-    sw.w_ih[0] = layers[l].w_ih; sw.w_hh[0] = layers[l].w_hh; sw.b_ih[0] = layers[l].b_ih; sw.b_hh[0] = layers[l].b_hh;
-    const float* X = l == 0 ? w.xfb : w.L[l - 1].H;
-    const int K0 = fbb_in_width(d, l);
-    if (tc) {
-      const LayerHalf half{w.h16[l], l > 0 ? w.h16[l - 1] : nullptr, w.w16};
-      rc = layer_forward_save_tc(&sw, 0, X, B, K0, H, Tp, w.L[l], w.rec, st, w.splitk, SPLITK_SCRATCH_FLOATS, &half);
-    } else {
-      rc = layer_forward_save(&sw, 0, X, B, K0, H, Tp, w.L[l], st);
-    }
-    if (rc) return rc;
+    const LayerHalf half{w.h16[l], l > 0 ? w.h16[l - 1] : nullptr, w.w16};
+    if ((rc = layer_forward(d->precision, layers[l], l == 0 ? w.xfb : w.L[l - 1].H, B, fbb_in_width(d, l), H, Tp, w.L[l], w.rec,
+                            w.splitk, &half, st)))
+      return rc;
   }
   // Linear(H -> 2F) + activation into y, kept for act' (model.py:58-62), then [B,2,F,T] without the look-ahead frames
   if ((rc = fc_gemm_launch(w.L[NL - 1].H, fc_w, fc_b, w.y, Tp * B, H, 2 * F, d->activation, st))) return rc;
@@ -164,21 +134,16 @@ extern "C" int fsn_fullband_train_backward(const fsn_fullband_desc* d, const fsn
               w.bytes);
   cudaStream_t st = (cudaStream_t)stream;
   const int F = d->num_freqs, H = d->hidden, Tp = T + d->look_ahead, NL = d->num_layers;
-  if (fbb_tc(d)) {
-    for (int l = 0; l < NL; ++l) {
-      if ((rc = transpose_launch(layers[l].w_hh, (size_t)4 * H, H, w.whhT[l], st))) return rc;
-      if (l > 0 && (rc = transpose_launch(layers[l].w_ih, (size_t)4 * H, H, w.wihT[l], st))) return rc;
-    }
-  }
-  // ---- output re-layout + act', Linear(2F): dW = dY^T H, db = colsum dY, dH = dY W
-  const float* Htop = w.L[NL - 1].H;
-  if ((rc = train_dy_launch(dout, w.y, d->activation, B, F, T, Tp, d->look_ahead, w.dY, st))) return rc;
-  if ((rc = sgemm_launch(true, w.dY, 2 * F, Htop, H, g->fc_w, H, 2 * F, H, Tp * B, false, w.splitk, st))) return rc;
-  if ((rc = colsum_launch(w.dY, (size_t)Tp * B, 2 * F, 2 * F, g->fc_b, nullptr, w.colsum, st))) return rc;
-  if ((rc = sgemm_launch(false, w.dY, 2 * F, fc_w, H, w.dH, H, Tp * B, H, 2 * F, false, nullptr, st))) return rc;
-  // ---- BPTT of the stack from the top, one step at a time (the input is the normalised spectrogram: no dx)
   LayerBwd L[FBB_MAX_LAYERS];
-  for (int l = 0; l < NL; ++l) L[l] = fbb_layer_bwd(d, layers, w, B, l);
+  for (int l = 0; l < NL; ++l) {
+    L[l] = LayerBwd{layers[l].w_ih, layers[l].w_hh, w.L[l], B, fbb_in_width(d, l), H, w.dh_rec[l], w.dc[l], w.whhT[l], w.wihT[l],
+                    w.splitk};
+    if ((rc = layer_bwd_transpose_weights(L[l], st))) return rc;
+  }
+  // ---- output re-layout + act', Linear(2F)
+  if ((rc = train_dy_launch(dout, w.y, d->activation, B, F, T, Tp, d->look_ahead, w.dY, st))) return rc;
+  if ((rc = linear_bwd(w.dY, w.L[NL - 1].H, fc_w, Tp * B, 2 * F, H, g->fc_w, g->fc_b, w.dH, w.splitk, w.colsum, st))) return rc;
+  // ---- BPTT of the stack from the top, one step at a time (the input is the normalised spectrogram: no dx)
   if ((rc = stack_bwd(L, NL, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid[0], w.dh_mid[1], nullptr, st))) return rc;
   // ---- weight gradients: layer 0 reads the normalised input, layer l the hidden states of layer l-1
   const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};

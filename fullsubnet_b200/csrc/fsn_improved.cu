@@ -108,16 +108,6 @@ struct ImpWs {
   size_t bytes;
 };
 
-struct ICarver {
-  char* base; size_t off;
-  explicit ICarver(void* p) : base((char*)p), off(0) {}
-  template <class T> T* take(size_t n) {
-    T* r = base ? (T*)(base + off) : nullptr;
-    off = align_up(off + n * sizeof(T), 256);
-    return r;
-  }
-};
-
 static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 
 static int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
@@ -149,7 +139,7 @@ static int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
 }
 
 static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, ImpWs& w) {
-  ICarver c(base);
+  Carver c(base);
   const size_t BFT = (size_t)m.B * m.F * m.T, BT = (size_t)m.B * m.T;
   w.mag = c.take<float>(BFT); w.real = c.take<float>(BFT); w.imag = c.take<float>(BFT);
   w.crm = c.take<float>(2 * BFT);
@@ -179,7 +169,7 @@ static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, 
   memset(&w.fbtc, 0, sizeof(w.fbtc));
   w.fbtc_mid = nullptr;
   if (d->precision == FSN_PREC_TF32_TC && lstm_rec_tc_supported(d->fb_hidden, false)) {
-    lstm_tc_carve(c.base, c.off, BT, m.Fu > d->fb_hidden ? m.Fu : d->fb_hidden, d->fb_hidden, false, w.fbtc);
+    lstm_tc_carve(c, BT, m.Fu > d->fb_hidden ? m.Fu : d->fb_hidden, d->fb_hidden, false, w.fbtc);
     w.fbtc_mid = c.take<float>(BT * d->fb_hidden);
   }
   w.bytes = c.off;
@@ -226,10 +216,8 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
   const bool fb_tc = w.fbtc_mid != nullptr;
   if (fb_tc) {
     // tensor cores: per layer one hoisted input-projection GEMM (tf32) + the persistent wgmma recurrence, Linear likewise
-    fsn_lstm_layer L0{wt->fb.w_ih[0], wt->fb.w_hh[0], wt->fb.b_ih[0], wt->fb.b_hh[0]};
-    fsn_lstm_layer L1{wt->fb.w_ih[1], wt->fb.w_hh[1], wt->fb.b_ih[1], wt->fb.b_hh[1]};
-    if ((rc = lstm_layer_tc(L0, w.magc, (size_t)Fu, Fu, w.inv1, T, 0, B, T, Hf, false, w.fbtc, w.fbtc_mid, st))) return rc;
-    if ((rc = lstm_layer_tc(L1, w.fbtc_mid, (size_t)Hf, Hf, nullptr, 1, 0, B, T, Hf, false, w.fbtc, w.fb_h1all, st))) return rc;
+    if ((rc = lstm_layer_tc(seq_layer(wt->fb, 0), w.magc, (size_t)Fu, Fu, w.inv1, T, 0, B, T, Hf, false, w.fbtc, w.fbtc_mid, st))) return rc;
+    if ((rc = lstm_layer_tc(seq_layer(wt->fb, 1), w.fbtc_mid, (size_t)Hf, Hf, nullptr, 1, 0, B, T, Hf, false, w.fbtc, w.fb_h1all, st))) return rc;
     if ((rc = linear_tc(w.fb_h1all, (size_t)Hf, Hf, wt->fb.fc_w, wt->fb.fc_b, Fu, d->fb_activation, w.fbT, (size_t)Fu,
                         (size_t)B * T, false, w.fbtc, st)))
       return rc;
@@ -285,8 +273,8 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
         imp_scale_rows_kernel<<<blocks, 256, 0, st>>>(w.X, w.invs, n, (size_t)R * g.W, (size_t)g.N * g.W, B);
         FSN_CHECK_LAUNCH("imp_scale_rows_kernel");
       }
-      if ((rc = layer_forward_save_tc(&sw, 0, w.X, R, g.W, Hs, T, w.tc, w.tc_rec, st))) return rc;
-      if ((rc = layer_forward_save_tc(&sw, 1, w.tc.H, R, Hs, Hs, T, l1, w.tc_rec, st))) return rc;
+      if ((rc = layer_forward_save_tc(seq_layer(sw, 0), w.X, R, g.W, Hs, T, w.tc, w.tc_rec, st))) return rc;
+      if ((rc = layer_forward_save_tc(seq_layer(sw, 1), w.tc.H, R, Hs, Hs, T, l1, w.tc_rec, st))) return rc;
       for (int t = 0; t < T; ++t) {
         const size_t warps = (size_t)R * 2 * g.cs;
         imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(w.tc_h1 + (size_t)t * R * Hs, R, Hs, sw.fc_w, sw.fc_b,

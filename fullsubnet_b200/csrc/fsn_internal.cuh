@@ -6,6 +6,21 @@
 
 namespace fsn {
 
+// Bump allocator over a caller's workspace: every block starts on a 256-byte boundary.  With a null base it hands out
+// nullptr and only counts the bytes, which is how the *_workspace_bytes queries size the same layout.
+struct Carver {
+  char* base; size_t off;
+  explicit Carver(void* p) : base((char*)p), off(0) {}
+  template <class T> T* take(size_t n) {
+    T* r = base ? (T*)(base + off) : nullptr;
+    off = align_up(off + n * sizeof(T), 256);
+    return r;
+  }
+};
+
+// layer l of a two-layer stack
+inline fsn_lstm_layer seq_layer(const fsn_seq_weights& w, int l) { return {w.w_ih[l], w.w_hh[l], w.b_ih[l], w.b_hh[l]}; }
+
 // Sub-band row -> (clip, frequency) map.  Row r = b' * Fsub + f' of the sub-band batch.
 // G <= 1: identity (Fsub = F).  G > 1: drop_band (audio_zen/acoustics/feature.py:332-345):
 // output clip b' of group g is input clip g + G*i, frequency f' is input bin g + G*f'.
@@ -89,27 +104,37 @@ struct LayerSave { float *G, *C, *H; };
 // fp16 side buffers of one layer (all nullable): H16 [Tp,R,H] copy of the hidden states (written by the step kernel, the
 // next layer's X16), X16 [Tp,R,K0] copy of the layer input, w16: 4H*(H+K0) halfs for the weight copies
 struct LayerHalf { __half* H16; const __half* X16; __half* w16; };
-int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp,
-                          const LayerSave& s, float* rec, cudaStream_t st, float* splitk = nullptr, size_t splitk_floats = 0,
+int layer_forward_save_tc(const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+                          float* rec, cudaStream_t st, float* splitk = nullptr, size_t splitk_floats = 0,
                           const LayerHalf* half = nullptr);
 // fp32 variant: one SIMT step kernel per step (lstm_step_launch with save_gates)
-int layer_forward_save(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+int layer_forward_save(const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
                        cudaStream_t st);
 
-// ---- back-propagation through time of one LSTM layer (fsn_train.cu), shared by the fullsubnet and fast_fullsubnet steps
 static const size_t SPLITK_SCRATCH_FLOATS = (size_t)16 << 20;  // 64 MB of split-K partial sums
 static const int COLSUM_MAX_S = 512;                            // row slabs of a column sum
+
+// Per-layer precision of the training steps: a layer runs on the tf32 tensor cores when the step asks for FSN_PREC_TF32_TC
+// and its hidden size keeps the rows of its operands 16-byte aligned; otherwise on the fp32 kernels.
+inline bool tf32_layer(int precision, int H) { return precision == FSN_PREC_TF32_TC && (H & 3) == 0; }
+// forward of one layer of a training step, on the variant tf32_layer picks (the fp32 one ignores rec / splitk / half)
+int layer_forward(int precision, const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+                  float* rec, float* splitk, const LayerHalf* half, cudaStream_t st);
+
+// ---- back-propagation through time of one LSTM layer (fsn_train.cu), shared by the training steps
 struct LayerBwd {
   const float *w_ih, *w_hh;
   LayerSave s;
   int R, K0, H;
   float *dh_rec, *dc;
-  const float *w_hhT, *w_ihT;  // tensor-core path: [H,4H] / [K0,4H] transposed copies (else nullptr)
+  float *w_hhT, *w_ihT;        // tensor-core path: [H,4H] / [K0,4H] transposed copies (else nullptr)
   float* splitk;               // split-K space of the per-step GEMMs (used when the layer has only a few tiles)
 };
 // scratch of layer_weight_grads: K-major copies of dG / layer input (tensor-core path, tgemm_blocked_floats of the largest
 // layer), split-K space (SPLITK_SCRATCH_FLOATS) and column-sum partials (COLSUM_MAX_S x 4H)
 struct WgradScratch { float *gT, *xT, *splitk, *colsum; };
+// tensor-core path: writes L.w_hhT, and L.w_ihT when the layer has one (it computes a dx); nothing when L.w_hhT is null
+int layer_bwd_transpose_weights(const LayerBwd& L, cudaStream_t st);
 // step t of one layer: pointwise gate gradients (d h from above = dh_above + dout W_fc for an O-output Linear on top),
 // then dh_rec = dG W_hh and, when dx != nullptr, dx = dG W_ih
 int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, const float* dout, const float* fc_w, int O,
@@ -141,6 +166,10 @@ int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, size_t ld
                  bool accumulate, float* scratch, cudaStream_t st);
 // out[c] (and out2[c] when given) = sum_r X[r*ldx + c], fixed order
 int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch, cudaStream_t st);
+// backward of a Linear Y = X W^T + b over `rows` rows, dY [rows,N], X [rows,K], W [N,K]: dW = dY^T X (split-K over
+// `splitk`), db = colsum dY (partials in `colsum`) and, when dX != nullptr, dX = dY W
+int linear_bwd(const float* dY, const float* X, const float* W, int rows, int N, int K, float* dW, float* db, float* dX,
+               float* splitk, float* colsum, cudaStream_t st);
 // out [cols, rows] = in [rows, cols]^T
 int transpose_launch(const float* in, size_t rows, int cols, float* out, cudaStream_t st);
 // per-clip (sum, sum_f c_N[f] * row sum) of a time-major x [Tp,B,F], one CTA per clip
@@ -213,7 +242,7 @@ int bias_act_launch(float* x, size_t rows, int N, size_t ld, const float* bias, 
 // workspace of lstm_layer_tc / linear_tc: prepared A operand [rows_T, Kmax (x3: 3 Kmax)], prepared weights
 // [4 Hmax, same], hoisted projection P [rows_T, 4 Hmax], recurrence scratch
 struct LstmTcWs { float *a, *w, *P; void* rec; };
-void lstm_tc_carve(char* base, size_t& off, size_t rows_T, int Kmax, int Hmax, bool x3, LstmTcWs& ws);
+void lstm_tc_carve(Carver& c, size_t rows_T, int Kmax, int Hmax, bool x3, LstmTcWs& ws);
 int lstm_layer_tc(const fsn_lstm_layer& L, const float* x, size_t ldx, int K, const float* row_scale, int rows_per_scale,
                   int scale_B, int R, int T, int H, bool x3, const LstmTcWs& ws, float* hall, cudaStream_t st);
 int linear_tc(const float* x, size_t ldx, int K, const float* W, const float* bias, int N, int act, float* out, size_t ldo,

@@ -468,13 +468,12 @@ int gemm_tc_split_launch(const float* a, size_t lda, const float* W, int N, int 
 
 // ---------------------------------------------------------------------------------------------------------------
 // One full LSTM layer and one Linear layer on top of the pieces above (what the model files call).
-void lstm_tc_carve(char* base, size_t& off, size_t rows_T, int Kmax, int Hmax, bool x3, LstmTcWs& ws) {
-  auto take = [&](size_t bytes) { char* r = base ? base + off : nullptr; off = align_up(off + bytes, 256); return r; };
+void lstm_tc_carve(Carver& c, size_t rows_T, int Kmax, int Hmax, bool x3, LstmTcWs& ws) {
   const size_t wa = (size_t)((Kmax + 3) & ~3) * (x3 ? 3 : 1);
-  ws.a = (float*)take(rows_T * wa * sizeof(float));
-  ws.w = (float*)take((size_t)4 * Hmax * wa * sizeof(float));
-  ws.P = (float*)take(rows_T * 4 * Hmax * sizeof(float));
-  ws.rec = take(lstm_rec_tc_scratch_bytes(Hmax, x3));
+  ws.a = c.take<float>(rows_T * wa);
+  ws.w = c.take<float>((size_t)4 * Hmax * wa);
+  ws.P = c.take<float>(rows_T * 4 * Hmax);
+  ws.rec = c.take<char>(lstm_rec_tc_scratch_bytes(Hmax, x3));
 }
 
 // operand A of a GEMM: x [rows, K] (row stride ldx) -> 16-byte aligned rows, scaled; x3: the [hi | lo | hi] layout
@@ -518,28 +517,28 @@ int linear_tc(const float* x, size_t ldx, int K, const float* W, const float* bi
 
 // unit-test hooks (tests/test_gpu_rec_tc.py): one LSTM layer / one Linear layer on the tensor-core path
 extern "C" size_t fsn_debug_lstm_tc_workspace_bytes(int R, int T, int K, int H, int x3) {
-  size_t off = 0;
+  fsn::Carver c(nullptr);
   fsn::LstmTcWs ws;
-  fsn::lstm_tc_carve(nullptr, off, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
-  return off;
+  fsn::lstm_tc_carve(c, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
+  return c.off;
 }
 extern "C" int fsn_debug_lstm_layer_tc(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                                        const float* x, int R, int T, int K, int H, int x3, float* hall, void* workspace,
                                        size_t workspace_bytes, fsn_stream_t stream) {
   FSN_REQUIRE(fsn::lstm_rec_tc_supported(H, x3 != 0), FSN_ERR_UNSUPPORTED, "lstm_layer_tc: hidden size %d not supported", H);
-  size_t off = 0;
+  fsn::Carver c(workspace);
   fsn::LstmTcWs ws;
-  fsn::lstm_tc_carve((char*)workspace, off, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
-  FSN_REQUIRE(workspace && workspace_bytes >= off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, off);
+  fsn::lstm_tc_carve(c, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
+  FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, c.off);
   fsn_lstm_layer L{w_ih, w_hh, b_ih, b_hh};
   return fsn::lstm_layer_tc(L, x, (size_t)K, K, nullptr, 1, 0, R, T, H, x3 != 0, ws, hall, (cudaStream_t)stream);
 }
 extern "C" int fsn_debug_linear_tc(const float* x, int rows, int K, const float* W, const float* bias, int N, int act, int x3,
                                    float* out, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
-  size_t off = 0;
+  fsn::Carver c(workspace);
   fsn::LstmTcWs ws;
   const int Hm = (N + 3) / 4 > 8 ? (N + 3) / 4 : 8;
-  fsn::lstm_tc_carve((char*)workspace, off, (size_t)rows, K, Hm, x3 != 0, ws);
-  FSN_REQUIRE(workspace && workspace_bytes >= off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, off);
+  fsn::lstm_tc_carve(c, (size_t)rows, K, Hm, x3 != 0, ws);
+  FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, c.off);
   return fsn::linear_tc(x, (size_t)K, K, W, bias, N, act, out, (size_t)N, (size_t)rows, x3 != 0, ws, (cudaStream_t)stream);
 }

@@ -36,16 +36,6 @@ static void prof_mark(int i, cudaStream_t st) {
 }
 static void prof_reset() { for (int i = 0; i < 5; ++i) g_ev_valid[i] = false; }
 
-struct Carver {
-  char* base; size_t off;
-  explicit Carver(void* p) : base((char*)p), off(0) {}
-  template <class T> T* take(size_t n) {
-    T* r = base ? (T*)(base + off) : nullptr;
-    off = align_up(off + n * sizeof(T), 256);
-    return r;
-  }
-};
-
 struct ModelWs {
   float *magT, *fbT, *inv1, *inv2;
   float2 *fs, *sums_mag, *sums_fb;
@@ -122,7 +112,7 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
   if (fb_tc_enabled(d, m.B)) {
     const int Hf = d->fb_hidden;
     const size_t rows = (size_t)m.B * m.Tp;
-    lstm_tc_carve(c.base, c.off, rows, m.F > Hf ? m.F : Hf, Hf, d->precision == FSN_PREC_F16X3_TC, w.tc);
+    lstm_tc_carve(c, rows, m.F > Hf ? m.F : Hf, Hf, d->precision == FSN_PREC_F16X3_TC, w.tc);
     w.tc_h0all = c.take<float>(rows * Hf);
   }
   w.cum1 = w.cum2 = nullptr;

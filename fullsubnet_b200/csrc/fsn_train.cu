@@ -508,63 +508,53 @@ struct TrainWs {
   size_t bytes;
 };
 
-struct TCarver {
-  char* base; size_t off;
-  explicit TCarver(void* p) : base((char*)p), off(0) {}
-  float* take(size_t n) {
-    float* r = base ? (float*)(base + off) : nullptr;
-    off = align_up(off + n * sizeof(float), 256);
-    return r;
-  }
-};
-
 static void carve_train(const fsn_model_desc* d, const Dims& m, void* base, TrainWs& w) {
-  TCarver c(base);
+  Carver c(base);
   const size_t Tp = m.Tp, B = m.B, F = m.F, R = m.R, Hf = d->fb_hidden, Hs = d->sb_hidden;
-  w.raw = c.take(Tp * B * F); w.xfb = c.take(Tp * B * F); w.fbz = c.take(Tp * B * F);
-  w.inv1 = c.take(B); w.inv2 = c.take(B);
-  w.sums_mag = (float2*)c.take(2 * B); w.sums_fb = (float2*)c.take(2 * B);
+  w.raw = c.take<float>(Tp * B * F); w.xfb = c.take<float>(Tp * B * F); w.fbz = c.take<float>(Tp * B * F);
+  w.inv1 = c.take<float>(B); w.inv2 = c.take<float>(B);
+  w.sums_mag = c.take<float2>(B); w.sums_fb = c.take<float2>(B);
   for (int l = 0; l < 2; ++l) {
-    w.fb[l].G = c.take(Tp * B * 4 * Hf); w.fb[l].C = c.take(Tp * B * Hf); w.fb[l].H = c.take(Tp * B * Hf);
-    w.sb[l].G = c.take(Tp * R * 4 * Hs); w.sb[l].C = c.take(Tp * R * Hs); w.sb[l].H = c.take(Tp * R * Hs);
+    w.fb[l].G = c.take<float>(Tp * B * 4 * Hf); w.fb[l].C = c.take<float>(Tp * B * Hf); w.fb[l].H = c.take<float>(Tp * B * Hf);
+    w.sb[l].G = c.take<float>(Tp * R * 4 * Hs); w.sb[l].C = c.take<float>(Tp * R * Hs); w.sb[l].H = c.take<float>(Tp * R * Hs);
   }
-  w.xsb = c.take(Tp * R * m.Ksb); w.dxsb = c.take(Tp * R * m.Ksb);
-  w.dout = c.take(Tp * R * 2);
-  w.dz = c.take(Tp * B * F); w.dfh1 = c.take(Tp * B * Hf);
+  w.xsb = c.take<float>(Tp * R * m.Ksb); w.dxsb = c.take<float>(Tp * R * m.Ksb);
+  w.dout = c.take<float>(Tp * R * 2);
+  w.dz = c.take<float>(Tp * B * F); w.dfh1 = c.take<float>(Tp * B * Hf);
   const size_t RH = (R * Hs > B * Hf) ? R * Hs : B * Hf;
-  for (int i = 0; i < 2; ++i) { w.dh_rec[i] = c.take(RH); w.dc[i] = c.take(RH); }
-  w.dh_mid = c.take(RH);
-  w.dot = c.take(B);
+  for (int i = 0; i < 2; ++i) { w.dh_rec[i] = c.take<float>(RH); w.dc[i] = c.take<float>(RH); }
+  w.dh_mid = c.take<float>(RH);
+  w.dot = c.take<float>(B);
   w.cum1 = w.cum2 = w.dunit = nullptr; w.fs = nullptr;
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
-    w.cum1 = c.take(Tp * B); w.cum2 = c.take(Tp * R); w.dunit = c.take(Tp * R);
-    w.fs = (float2*)c.take(2 * Tp * B);
+    w.cum1 = c.take<float>(Tp * B); w.cum2 = c.take<float>(Tp * R); w.dunit = c.take<float>(Tp * R);
+    w.fs = c.take<float2>(Tp * B);
   }
-  w.splitk = c.take(SPLITK_SCRATCH_FLOATS);
+  w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
   const size_t maxcols = 4 * (Hf > Hs ? Hf : Hs) > F ? 4 * (Hf > Hs ? Hf : Hs) : F;
-  w.colsum = c.take((size_t)COLSUM_MAX_S * maxcols);
-  w.splitk2 = c.take(SPLITK_SCRATCH_FLOATS);
-  w.colsum2 = c.take((size_t)COLSUM_MAX_S * maxcols);
+  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * maxcols);
+  w.splitk2 = c.take<float>(SPLITK_SCRATCH_FLOATS);
+  w.colsum2 = c.take<float>((size_t)COLSUM_MAX_S * maxcols);
   if (d->precision == FSN_PREC_TF32_TC) {
     for (int l = 0; l < 2; ++l) {
-      w.sb_whhT[l] = c.take(Hs * 4 * Hs);
-      w.sb_wihT[l] = c.take((l == 0 ? (size_t)m.Ksb : Hs) * 4 * Hs);
-      w.fb_whhT[l] = c.take(Hf * 4 * Hf);
+      w.sb_whhT[l] = c.take<float>(Hs * 4 * Hs);
+      w.sb_wihT[l] = c.take<float>((l == 0 ? (size_t)m.Ksb : Hs) * 4 * Hs);
+      w.fb_whhT[l] = c.take<float>(Hf * 4 * Hf);
     }
-    w.fb_wihT1 = c.take(Hf * 4 * Hf);
+    w.fb_wihT1 = c.take<float>(Hf * 4 * Hf);
     // K-major (block-tiled, zero padded: tgemm_blocked_floats) copies of dG and of the layer input / hidden states
     const size_t g_sb = tgemm_blocked_floats(Tp * R, 4 * (int)Hs), g_fb = tgemm_blocked_floats(Tp * B, 4 * (int)Hf);
-    w.gT = c.take(g_sb > g_fb ? g_sb : g_fb);
+    w.gT = c.take<float>(g_sb > g_fb ? g_sb : g_fb);
     const size_t x_sb = tgemm_blocked_floats(Tp * R, Hs > (size_t)m.Ksb ? (int)Hs : m.Ksb),
                  x_fb = tgemm_blocked_floats(Tp * B, Hf > F ? (int)Hf : (int)F);
-    w.xT = c.take(x_sb > x_fb ? x_sb : x_fb);
-    w.rec = c.take(4 * RH);
+    w.xT = c.take<float>(x_sb > x_fb ? x_sb : x_fb);
+    w.rec = c.take<float>(4 * RH);
     for (int l = 0; l < 2; ++l) {
-      w.fb_h16[l] = (__half*)c.take((Tp * B * Hf + 1) / 2);
-      w.sb_h16[l] = (__half*)c.take((Tp * R * Hs + 1) / 2);
+      w.fb_h16[l] = c.take<__half>(Tp * B * Hf);
+      w.sb_h16[l] = c.take<__half>(Tp * R * Hs);
     }
     const size_t wmax = Hf > Hs ? Hf : Hs;
-    w.w16 = (__half*)c.take((4 * wmax * 2 * wmax + 1) / 2);
+    w.w16 = c.take<__half>(4 * wmax * 2 * wmax);
   } else {
     w.fb_h16[0] = w.fb_h16[1] = w.sb_h16[0] = w.sb_h16[1] = w.w16 = nullptr;
   }
@@ -581,13 +571,13 @@ static int train_check(const fsn_model_desc* d) {
 }
 
 // one layer forward over all steps, saving gates / cell / hidden:  X [Tp,R,K0] (row_scale == nullptr)
-int layer_forward_save(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+int layer_forward_save(const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
                        cudaStream_t st) {
   for (int t = 0; t < Tp; ++t) {
     StepParams p;
     memset(&p, 0, sizeof(p));
     p.R = R; p.K0 = K0; p.H = H; p.first = (t == 0);
-    p.w_ih = w->w_ih[l]; p.w_hh = w->w_hh[l]; p.b_ih = w->b_ih[l]; p.b_hh = w->b_hh[l];
+    p.w_ih = w.w_ih; p.w_hh = w.w_hh; p.b_ih = w.b_ih; p.b_hh = w.b_hh;
     p.x0 = X + (size_t)t * R * K0; p.x0_row_stride = K0;
     p.h_prev = s.H + (size_t)(t > 0 ? t - 1 : 0) * R * H; p.h_prev_stride = H;
     p.h_out = s.H + (size_t)t * R * H; p.h_out_stride = H;
@@ -604,28 +594,27 @@ int layer_forward_save(const fsn_seq_weights* w, int l, const float* X, int R, i
 // wgmma and the cell on its accumulators, gates / cell / hidden saved.  Fallbacks, step by step: a layer input whose rows
 // are not 16-byte aligned keeps a hoisted projection of all steps (one GEMM into the gate buffer) that the step kernel
 // adds; with the fused kernel switched off (or H % 32 != 0) every step is a recurrent GEMM into `rec` + lstm_cell_fwd_kernel
-int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R, int K0, int H, int Tp,
-                                 const LayerSave& s, float* rec, cudaStream_t st, float* splitk, size_t splitk_floats,
-                                 const LayerHalf* half) {
+int layer_forward_save_tc(const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+                          float* rec, cudaStream_t st, float* splitk, size_t splitk_floats, const LayerHalf* half) {
   int rc;
   const int rows = Tp * R;
   static const int fused_min_rows = getenv("FSN_TRAIN_FUSED_MIN_ROWS") ? atoi(getenv("FSN_TRAIN_FUSED_MIN_ROWS")) : 1;
-  const bool fused = R >= fused_min_rows && lstm_fwd_step_supported(s.H, w->w_hh[l], H);
+  const bool fused = R >= fused_min_rows && lstm_fwd_step_supported(s.H, w.w_hh, H);
   // x_t W_ih^T as leading k blocks of the step kernel - no hoisted projection, G is written once and never read in the
   // forward pass (FSN_TRAIN_FOLD_K bounds the input width this is done for)
-  const bool fold = fused && lstm_fwd_step_folds_input(X, w->w_ih[l], K0);
+  const bool fold = fused && lstm_fwd_step_folds_input(X, w.w_ih, K0);
   // fp16 MMA operands: h_t (written by the step kernel next to the fp32 copy) and the weights; the folded layer input too
   // when the layer below left an fp16 copy (K0 % 8: 16-byte rows)
   const bool h16 = fused && half && half->H16 && half->w16 && lstm_fwd_step_half_enabled(H);
   const bool x16 = h16 && fold && half->X16 && (K0 % 8) == 0;
   __half* w_hh16 = h16 ? half->w16 : nullptr;
   __half* w_ih16 = x16 ? half->w16 + (size_t)4 * H * H : nullptr;
-  if (h16 && (rc = to_half_launch(w->w_hh[l], (size_t)4 * H * H, w_hh16, st))) return rc;
-  if (x16 && (rc = to_half_launch(w->w_ih[l], (size_t)4 * H * K0, w_ih16, st))) return rc;
+  if (h16 && (rc = to_half_launch(w.w_hh, (size_t)4 * H * H, w_hh16, st))) return rc;
+  if (x16 && (rc = to_half_launch(w.w_ih, (size_t)4 * H * K0, w_ih16, st))) return rc;
   if (fold) {
-  } else if (tgemm_supported(X, K0, w->w_ih[l], K0, K0)) {
-    if ((rc = tgemm_launch(X, K0, w->w_ih[l], K0, s.G, 4 * H, rows, 4 * H, K0, false, nullptr, 0, st))) return rc;
-  } else if ((rc = fc_gemm_launch(X, w->w_ih[l], nullptr, s.G, rows, K0, 4 * H, FSN_ACT_NONE, st))) {
+  } else if (tgemm_supported(X, K0, w.w_ih, K0, K0)) {
+    if ((rc = tgemm_launch(X, K0, w.w_ih, K0, s.G, 4 * H, rows, 4 * H, K0, false, nullptr, 0, st))) return rc;
+  } else if ((rc = fc_gemm_launch(X, w.w_ih, nullptr, s.G, rows, K0, 4 * H, FSN_ACT_NONE, st))) {
     return rc;  // rows of X not 16-byte aligned (K0 % 4 != 0): fp32 SIMT GEMM
   }
   const size_t n = (size_t)R * H;
@@ -641,8 +630,8 @@ int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R
         hs.H16_out = half->H16 + (size_t)t * R * H;
         if (x16) { hs.Xt16 = half->X16 + (size_t)t * R * K0; hs.w_ih16 = w_ih16; }
       }
-      if ((rc = lstm_fwd_step_launch(t > 0 ? s.H + (size_t)(t - 1) * R * H : nullptr, w->w_hh[l],
-                                     fold ? X + (size_t)t * R * K0 : nullptr, w->w_ih[l], K0, Gt, w->b_ih[l], w->b_hh[l],
+      if ((rc = lstm_fwd_step_launch(t > 0 ? s.H + (size_t)(t - 1) * R * H : nullptr, w.w_hh,
+                                     fold ? X + (size_t)t * R * K0 : nullptr, w.w_ih, K0, Gt, w.b_ih, w.b_hh,
                                      t > 0 ? s.C + (size_t)(t - 1) * R * H : nullptr, s.C + (size_t)t * R * H,
                                      s.H + (size_t)t * R * H, R, H, st, h16 ? &hs : nullptr)))
         return rc;
@@ -651,9 +640,9 @@ int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R
     // (first step of a layer with a hoisted projection: no product at all, the plain cell kernel; its h_0 also goes out
     // in fp16 below)
     if (t > 0)
-      if ((rc = tgemm_launch(s.H + (size_t)(t - 1) * R * H, H, w->w_hh[l], H, rec, 4 * H, R, 4 * H, H, false, splitk, splitk_floats, st)))
+      if ((rc = tgemm_launch(s.H + (size_t)(t - 1) * R * H, H, w.w_hh, H, rec, 4 * H, R, 4 * H, H, false, splitk, splitk_floats, st)))
         return rc;
-    lstm_cell_fwd_kernel<<<blocks, 256, 0, st>>>(Gt, t > 0 ? rec : nullptr, w->b_ih[l], w->b_hh[l],
+    lstm_cell_fwd_kernel<<<blocks, 256, 0, st>>>(Gt, t > 0 ? rec : nullptr, w.b_ih, w.b_hh,
                                                  t > 0 ? s.C + (size_t)(t - 1) * R * H : nullptr,
                                                  s.C + (size_t)t * R * H, s.H + (size_t)t * R * H, R, H);
     FSN_CHECK_LAUNCH("lstm_cell_fwd_kernel");
@@ -662,7 +651,28 @@ int layer_forward_save_tc(const fsn_seq_weights* w, int l, const float* X, int R
   return FSN_OK;
 }
 
-static bool tc_layer_ok(const fsn_model_desc* d, int H) { return d->precision == FSN_PREC_TF32_TC && (H & 3) == 0; }
+int layer_forward(int precision, const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
+                  float* rec, float* splitk, const LayerHalf* half, cudaStream_t st) {
+  if (!tf32_layer(precision, H)) return layer_forward_save(w, X, R, K0, H, Tp, s, st);
+  return layer_forward_save_tc(w, X, R, K0, H, Tp, s, rec, st, splitk, SPLITK_SCRATCH_FLOATS, half);
+}
+
+int layer_bwd_transpose_weights(const LayerBwd& L, cudaStream_t st) {
+  if (!L.w_hhT) return FSN_OK;
+  int rc;
+  if ((rc = transpose_launch(L.w_hh, (size_t)4 * L.H, L.H, L.w_hhT, st))) return rc;
+  if (L.w_ihT && (rc = transpose_launch(L.w_ih, (size_t)4 * L.H, L.K0, L.w_ihT, st))) return rc;
+  return FSN_OK;
+}
+
+int linear_bwd(const float* dY, const float* X, const float* W, int rows, int N, int K, float* dW, float* db, float* dX,
+               float* splitk, float* colsum, cudaStream_t st) {
+  int rc;
+  if ((rc = sgemm_launch(true, dY, N, X, K, dW, K, N, K, rows, false, splitk, st))) return rc;
+  if ((rc = colsum_launch(dY, (size_t)rows, N, N, db, nullptr, colsum, st))) return rc;
+  if (dX && (rc = sgemm_launch(false, dY, N, W, K, dX, K, rows, K, N, false, nullptr, st))) return rc;
+  return FSN_OK;
+}
 
 // step t of one layer: pointwise gate gradients, then dh_rec = dG W_hh and (optionally) dx = dG W_ih
 int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, const float* dout, const float* fc_w,
@@ -879,17 +889,12 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
                                w.cum1, st)))
     return rc;
   // full-band stack + Linear/activation (model.py:92-95)
-  const bool tc_fb = tc_layer_ok(d, Hf), tc_sb = tc_layer_ok(d, Hs);
   // fp16 operand copies: layer 0's hidden states double as layer 1's input
   const LayerHalf hf0{w.fb_h16[0], nullptr, w.w16}, hf1{w.fb_h16[1], w.fb_h16[0], w.w16};
   const LayerHalf hs0{w.sb_h16[0], nullptr, w.w16}, hs1{w.sb_h16[1], w.sb_h16[0], w.w16};
-  if (tc_fb) {
-    if ((rc = layer_forward_save_tc(fb, 0, w.xfb, B, F, Hf, Tp, w.fb[0], w.rec, st, w.splitk, SPLITK_SCRATCH_FLOATS, &hf0))) return rc;
-    if ((rc = layer_forward_save_tc(fb, 1, w.fb[0].H, B, Hf, Hf, Tp, w.fb[1], w.rec, st, w.splitk, SPLITK_SCRATCH_FLOATS, &hf1))) return rc;
-  } else {
-    if ((rc = layer_forward_save(fb, 0, w.xfb, B, F, Hf, Tp, w.fb[0], st))) return rc;
-    if ((rc = layer_forward_save(fb, 1, w.fb[0].H, B, Hf, Hf, Tp, w.fb[1], st))) return rc;
-  }
+  const int prec = d->precision;
+  if ((rc = layer_forward(prec, seq_layer(*fb, 0), w.xfb, B, F, Hf, Tp, w.fb[0], w.rec, w.splitk, &hf0, st))) return rc;
+  if ((rc = layer_forward(prec, seq_layer(*fb, 1), w.fb[0].H, B, Hf, Hf, Tp, w.fb[1], w.rec, w.splitk, &hf1, st))) return rc;
   if ((rc = fc_gemm_launch(w.fb[1].H, fb->fc_w, fb->fc_b, w.fbz, Tp * B, Hf, F, d->fb_activation, st))) return rc;
   // second norm in closed form (model.py:110-111)
   train_tm_stats_kernel<<<B, 256, 0, st>>>(w.fbz, B, F, Tp, d->fb_num_neighbors, w.sums_fb);
@@ -903,13 +908,8 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   train_gather_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.fbz, w.inv2, cum ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,
                                                d->sb_num_neighbors, d->fb_num_neighbors);
   FSN_CHECK_LAUNCH("train_gather_kernel");
-  if (tc_sb) {
-    if ((rc = layer_forward_save_tc(sb, 0, w.xsb, m.R, m.Ksb, Hs, Tp, w.sb[0], w.rec, st, w.splitk, SPLITK_SCRATCH_FLOATS, &hs0))) return rc;
-    if ((rc = layer_forward_save_tc(sb, 1, w.sb[0].H, m.R, Hs, Hs, Tp, w.sb[1], w.rec, st, w.splitk, SPLITK_SCRATCH_FLOATS, &hs1))) return rc;
-  } else {
-    if ((rc = layer_forward_save(sb, 0, w.xsb, m.R, m.Ksb, Hs, Tp, w.sb[0], st))) return rc;
-    if ((rc = layer_forward_save(sb, 1, w.sb[0].H, m.R, Hs, Hs, Tp, w.sb[1], st))) return rc;
-  }
+  if ((rc = layer_forward(prec, seq_layer(*sb, 0), w.xsb, m.R, m.Ksb, Hs, Tp, w.sb[0], w.rec, w.splitk, &hs0, st))) return rc;
+  if ((rc = layer_forward(prec, seq_layer(*sb, 1), w.sb[0].H, m.R, Hs, Hs, Tp, w.sb[1], w.rec, w.splitk, &hs1, st))) return rc;
   // sub-band Linear of every output frame in one launch (model.py:129-135; the first look_ahead steps have no frame)
   return sb_fc_steps_launch(w.sb[1].H + (size_t)d->look_ahead * m.R * Hs, m.R, Hs, Tp - d->look_ahead, sb->fc_w, sb->fc_b, 2,
                             d->sb_activation, crm, m.Fsub, m.T, 0, st);
@@ -974,41 +974,36 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
     FSN_CHECK_LAUNCH("colsum_final_kernel");
   }
   if ((rc = colsum_launch(w.dout, (size_t)Tp * R, 2, 2, gsb->fc_b, nullptr, w.colsum, st))) return rc;
-  // ---- sub-band stack, both layers one step apart
-  const bool tc_fb = tc_layer_ok(d, Hf), tc_sb = tc_layer_ok(d, Hs);
-  if (tc_sb) {
-    for (int l = 0; l < 2; ++l) {
-      if ((rc = transpose_launch(sb->w_hh[l], (size_t)4 * Hs, Hs, w.sb_whhT[l], st))) return rc;
-      if ((rc = transpose_launch(sb->w_ih[l], (size_t)4 * Hs, l == 0 ? K : Hs, w.sb_wihT[l], st))) return rc;
-    }
-  }
-  if (tc_fb) {
-    for (int l = 0; l < 2; ++l)
-      if ((rc = transpose_launch(fb->w_hh[l], (size_t)4 * Hf, Hf, w.fb_whhT[l], st))) return rc;
-    if ((rc = transpose_launch(fb->w_ih[1], (size_t)4 * Hf, Hf, w.fb_wihT1, st))) return rc;
-  }
-  LayerBwd s1{sb->w_ih[1], sb->w_hh[1], w.sb[1], R, Hs, Hs, w.dh_rec[1], w.dc[1], tc_sb ? w.sb_whhT[1] : nullptr,
-              tc_sb ? w.sb_wihT[1] : nullptr, w.splitk};
-  LayerBwd s0{sb->w_ih[0], sb->w_hh[0], w.sb[0], R, K, Hs, w.dh_rec[0], w.dc[0], tc_sb ? w.sb_whhT[0] : nullptr,
-              tc_sb ? w.sb_wihT[0] : nullptr, w.splitk};
-  for (int t = Tp - 1; t >= 0; --t) {
-    if ((rc = layer_bwd_step(s1, t, Tp, nullptr, w.dout + (size_t)t * R * 2, sb->fc_w, 2, w.dh_mid, st))) return rc;
-    if ((rc = layer_bwd_step(s0, t, Tp, w.dh_mid, nullptr, nullptr, 0, w.dxsb + (size_t)t * R * K, st))) return rc;
-  }
-  // ---- fork: sub-band weight gradients on the caller's stream, the rest of the chain (second norm, full-band Linear, full-band
-  // BPTT) on the side stream with its own split-K / column-sum scratch
+  const bool tc_fb = tf32_layer(d->precision, Hf), tc_sb = tf32_layer(d->precision, Hs);
+  // the full-band chain (second norm, full-band Linear, full-band BPTT) runs on the side stream when there is one, with its
+  // own split-K / column-sum scratch
   SideStream* side = side_stream();
-  cudaStream_t st2 = st;
-  float *splitk2 = w.splitk, *colsum2 = w.colsum;
+  cudaStream_t st2 = side ? side->s : st;
+  float* splitk2 = side ? w.splitk2 : w.splitk;
+  float* colsum2 = side ? w.colsum2 : w.colsum;
+  // sub-band layers 0, 1, full-band layers 0, 1 (full-band layer 0 computes no dx)
+  const LayerBwd L[4] = {
+      {sb->w_ih[0], sb->w_hh[0], w.sb[0], R, K, Hs, w.dh_rec[0], w.dc[0], tc_sb ? w.sb_whhT[0] : nullptr,
+       tc_sb ? w.sb_wihT[0] : nullptr, w.splitk},
+      {sb->w_ih[1], sb->w_hh[1], w.sb[1], R, Hs, Hs, w.dh_rec[1], w.dc[1], tc_sb ? w.sb_whhT[1] : nullptr,
+       tc_sb ? w.sb_wihT[1] : nullptr, w.splitk},
+      {fb->w_ih[0], fb->w_hh[0], w.fb[0], B, F, Hf, w.dh_rec[0], w.dc[0], tc_fb ? w.fb_whhT[0] : nullptr, nullptr, splitk2},
+      {fb->w_ih[1], fb->w_hh[1], w.fb[1], B, Hf, Hf, w.dh_rec[1], w.dc[1], tc_fb ? w.fb_whhT[1] : nullptr,
+       tc_fb ? w.fb_wihT1 : nullptr, splitk2}};
+  const LayerBwd *sbL = L, *fbL = L + 2;
+  for (int l = 0; l < 4; ++l)
+    if ((rc = layer_bwd_transpose_weights(L[l], st))) return rc;
+  // ---- sub-band stack, both layers one step apart
+  if ((rc = stack_bwd(sbL, 2, Tp, nullptr, w.dout, sb->fc_w, 2, w.dh_mid, nullptr, w.dxsb, st))) return rc;
+  // ---- fork: sub-band weight gradients on the caller's stream, the rest of the chain on st2
   if (side) {
     if ((rc = check_cuda(cudaEventRecord(side->fork, st), "event record"))) return rc;
     if ((rc = check_cuda(cudaStreamWaitEvent(side->s, side->fork, 0), "stream wait"))) return rc;
-    st2 = side->s; splitk2 = w.splitk2; colsum2 = w.colsum2;
   }
   const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
-  if ((rc = layer_weight_grads(s1, Tp, w.sb[0].H, gsb->w_ih[1], gsb->w_hh[1], gsb->b_ih[1], gsb->b_hh[1], wg, st)))
+  if ((rc = layer_weight_grads(sbL[1], Tp, w.sb[0].H, gsb->w_ih[1], gsb->w_hh[1], gsb->b_ih[1], gsb->b_hh[1], wg, st)))
     return rc;
-  if ((rc = layer_weight_grads(s0, Tp, w.xsb, gsb->w_ih[0], gsb->w_hh[0], gsb->b_ih[0], gsb->b_hh[0], wg, st))) return rc;
+  if ((rc = layer_weight_grads(sbL[0], Tp, w.xsb, gsb->w_ih[0], gsb->w_hh[0], gsb->b_ih[0], gsb->b_hh[0], wg, st))) return rc;
   // ---- second norm + drop_band + full-band Linear/activation
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
     train_cum_unit_bwd_kernel<<<cdiv(R, 128), 128, 0, st2>>>(w.dxsb, w.xsb, w.cum2, Tp, R, K, w.dunit);
@@ -1022,24 +1017,17 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
                                                 d->fb_activation, w.dz);
     FSN_CHECK_LAUNCH("train_dfbz_kernel");
   }
-  if ((rc = sgemm_launch(true, w.dz, F, w.fb[1].H, Hf, gfb->fc_w, Hf, F, Hf, Tp * B, false, splitk2, st2))) return rc;
-  if ((rc = colsum_launch(w.dz, (size_t)Tp * B, F, F, gfb->fc_b, nullptr, colsum2, st2))) return rc;
-  if ((rc = sgemm_launch(false, w.dz, F, fb->fc_w, Hf, w.dfh1, Hf, Tp * B, Hf, F, false, nullptr, st2))) return rc;
+  if ((rc = linear_bwd(w.dz, w.fb[1].H, fb->fc_w, Tp * B, F, Hf, gfb->fc_w, gfb->fc_b, w.dfh1, splitk2, colsum2, st2)))
+    return rc;
   // ---- full-band stack
-  LayerBwd f1{fb->w_ih[1], fb->w_hh[1], w.fb[1], B, Hf, Hf, w.dh_rec[1], w.dc[1], tc_fb ? w.fb_whhT[1] : nullptr,
-              tc_fb ? w.fb_wihT1 : nullptr, splitk2};
-  LayerBwd f0{fb->w_ih[0], fb->w_hh[0], w.fb[0], B, F, Hf, w.dh_rec[0], w.dc[0], tc_fb ? w.fb_whhT[0] : nullptr, nullptr, splitk2};
-  for (int t = Tp - 1; t >= 0; --t) {
-    if ((rc = layer_bwd_step(f1, t, Tp, w.dfh1 + (size_t)t * B * Hf, nullptr, nullptr, 0, w.dh_mid, st2))) return rc;
-    if ((rc = layer_bwd_step(f0, t, Tp, w.dh_mid, nullptr, nullptr, 0, nullptr, st2))) return rc;
-  }
+  if ((rc = stack_bwd(fbL, 2, Tp, w.dfh1, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st2))) return rc;
   if (side) {  // join: the full-band weight gradients share gT / xT / splitk / colsum with the sub-band ones
     if ((rc = check_cuda(cudaEventRecord(side->join, side->s), "event record"))) return rc;
     if ((rc = check_cuda(cudaStreamWaitEvent(st, side->join, 0), "stream wait"))) return rc;
   }
-  if ((rc = layer_weight_grads(f1, Tp, w.fb[0].H, gfb->w_ih[1], gfb->w_hh[1], gfb->b_ih[1], gfb->b_hh[1], wg, st)))
+  if ((rc = layer_weight_grads(fbL[1], Tp, w.fb[0].H, gfb->w_ih[1], gfb->w_hh[1], gfb->b_ih[1], gfb->b_hh[1], wg, st)))
     return rc;
-  return layer_weight_grads(f0, Tp, w.xfb, gfb->w_ih[0], gfb->w_hh[0], gfb->b_ih[0], gfb->b_hh[0], wg, st);
+  return layer_weight_grads(fbL[0], Tp, w.xfb, gfb->w_ih[0], gfb->w_hh[0], gfb->b_ih[0], gfb->b_hh[0], wg, st);
 }
 
 // ------------------------------------------------------------------------------------------ loss

@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..model.base_model import BaseModel
+from ..model.base_model import BaseModel, TrainStep
 from ..model.module.sequence_model import SequenceModel
 
 
@@ -36,66 +36,16 @@ _LAYERS = (("enc1", "encoder.0.", 0), ("enc2", "encoder.1.", 0), ("dec1", "decod
 _LINEARS = (("enc_fc", "encoder.1."), ("bn_fc", "bottleneck."), ("dec_fc", "decoder_lstm.1."))
 
 
-def _lstm_grads(grads: dict, prefix: str, l: int) -> "_lib.LstmGrads":
-    return _lib.LstmGrads(*(grads[f"{prefix}sequence_model.{n}_l{l}"].data_ptr()
-                            for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")))
-
-
 def _grad_struct(grads: dict) -> "_lib.FastGrads":
     g = _lib.FastGrads()
     for field, prefix, l in _LAYERS:
-        setattr(g, field, _lstm_grads(grads, prefix, l))
+        setattr(g, field, SequenceModel.grads_struct(grads, prefix, l))
     for l in range(2):
-        g.bn[l] = _lstm_grads(grads, "bottleneck.", l)
+        g.bn[l] = SequenceModel.grads_struct(grads, "bottleneck.", l)
     for field, prefix in _LINEARS:
         setattr(g, field + "_w", grads[f"{prefix}fc_output_layer.weight"].data_ptr())
         setattr(g, field + "_b", grads[f"{prefix}fc_output_layer.bias"].data_ptr())
     return g
-
-
-class _TrainForward(torch.autograd.Function):
-    """Model.forward in train mode with back-propagation through time in libfsn_b200 (fsn_fast_train_forward /
-    fsn_fast_train_backward).  The parameters are passed as inputs so autograd (and DDP's hooks) route the gradients to
-    them exactly as for the reference's nn.LSTM / nn.Linear modules."""
-
-    @staticmethod
-    def forward(ctx, model, x, *params):
-        B, _, F, T = x.shape
-        device = x.device
-        lib = _lib.load()
-        with torch.cuda.device(device):
-            d = model._desc(_lib.PREC[model._resolve_train_precision()])
-            w = model._weight_struct()
-            n = lib.fsn_fast_train_workspace_bytes(C.byref(d), B, T)
-            if n == 0:
-                _lib.check_workspace(n)
-            ws = torch.empty(n, dtype=torch.uint8, device=device)
-            out = torch.empty(B, 2, F, T, dtype=torch.float32, device=device)
-            _lib.check(lib.fsn_fast_train_forward(C.byref(d), C.byref(w), x.data_ptr(), B, T, out.data_ptr(),
-                                                  ws.data_ptr(), n, _lib.stream_ptr(device)))
-        ctx.model, ctx.ws, ctx.dims, ctx.desc = model, ws, (B, T), d
-        ctx.versions = model._version_key()
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        model, (B, T) = ctx.model, ctx.dims
-        if ctx.versions != model._version_key():
-            raise RuntimeError("fullsubnet_b200: a parameter was modified in place between forward and backward")
-        if ctx.ws is None:
-            raise RuntimeError("fullsubnet_b200: backward through the same forward twice (activations were released)")
-        dout = dout.contiguous().float()
-        device = dout.device
-        lib = _lib.load()
-        names = [k for k, _ in model.named_parameters()]
-        _, grads = model._new_flat_grads(device)
-        with torch.cuda.device(device):
-            w = model._weight_struct()
-            g = _grad_struct(grads)
-            _lib.check(lib.fsn_fast_train_backward(C.byref(ctx.desc), C.byref(w), dout.data_ptr(), B, T, C.byref(g),
-                                                   ctx.ws.data_ptr(), ctx.ws.numel(), _lib.stream_ptr(device)))
-        ctx.ws = None
-        return (None, None) + tuple(grads[k] for k in names)
 
 
 class _MelScale(nn.Module):
@@ -107,6 +57,11 @@ class _MelScale(nn.Module):
 
 
 class Model(BaseModel):
+    # training step (fast_fullsubnet/trainer.py:45-56): fsn_fast_train_forward keeps the activations,
+    # fsn_fast_train_backward runs BPTT
+    TRAIN_ENTRY_POINTS = ("fsn_fast_train_workspace_bytes", "fsn_fast_train_forward", "fsn_fast_train_backward")
+    TRAIN_TF32_STACKS = ("bottleneck",)
+
     def __init__(self, look_ahead, shrink_size, sequence_model, num_mels, encoder_input_size, bottleneck_hidden_size,
                  bottleneck_num_layers, noisy_input_num_neighbors, encoder_output_num_neighbors,
                  norm_type="offline_laplace_norm", weight_init=False, precision=None):
@@ -163,15 +118,14 @@ class Model(BaseModel):
             raise NotImplementedError("the tensor-core precisions need bottleneck_hidden_size = 384, 2 layers and input width <= 32")
         return self.precision
 
-    def _resolve_train_precision(self) -> str:
-        if self.train_precision == "auto":
-            return "tf32_tc" if self.bottleneck.hidden_size % 4 == 0 else "fp32"
-        if self.train_precision not in ("fp32", "tf32_tc"):
-            raise ValueError("train_precision must be 'fp32', 'tf32_tc' or 'auto'")
-        return self.train_precision
+    def _train_desc(self):
+        return self._desc(_lib.PREC[self._resolve_train_precision()])
 
-    def _version_key(self):
-        return tuple((p.data_ptr(), p._version) for p in self.parameters())
+    def _train_weights(self):
+        return (C.byref(self._weight_struct()),)
+
+    def _train_grads(self, grads):
+        return (C.byref(_grad_struct(grads)),)
 
     def _desc(self, prec: int):
         return _lib.FastDesc(num_freqs=self.encoder_input_size, look_ahead=self.look_ahead, shrink_size=self.shrink_size,
@@ -219,11 +173,8 @@ class Model(BaseModel):
         assert num_channels == 1, f"{self.__class__.__name__} takes a magnitude feature as the input."
         assert num_freqs == self.encoder_input_size
         x = _lib.require_cuda(mix_mag, "mix_mag")
-        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            # training step (fast_fullsubnet/trainer.py:45-56): kernels that keep the activations for BPTT
-            if not all(p.requires_grad for p in self.parameters()):
-                raise NotImplementedError("fullsubnet_b200: partially frozen models are not built")
-            return _TrainForward.apply(self, x, *self.parameters())
+        if self.training and self._records_grad():
+            return TrainStep.apply(self, x, *self.parameters())
         lib = _lib.load()
         with torch.cuda.device(x.device):
             d, w = self._structs(x.device)

@@ -13,68 +13,26 @@ import os
 import torch
 
 from .. import _lib
-from ..model.base_model import BaseModel
+from ..model.base_model import BaseModel, TrainStep
 from ..model.module.sequence_model import SequenceModel
 
 
-def _grad_struct(seq: SequenceModel, grads: dict, prefix: str) -> "_lib.SeqGrads":
+def _grad_struct(grads: dict, prefix: str) -> "_lib.SeqGrads":
     g = _lib.SeqGrads()
     for l in range(2):
-        for field, name in (("w_ih", "weight_ih"), ("w_hh", "weight_hh"), ("b_ih", "bias_ih"), ("b_hh", "bias_hh")):
-            getattr(g, field)[l] = grads[f"{prefix}sequence_model.{name}_l{l}"].data_ptr()
+        lg = SequenceModel.grads_struct(grads, prefix, l)
+        for field in ("w_ih", "w_hh", "b_ih", "b_hh"):
+            getattr(g, field)[l] = getattr(lg, field)
     g.fc_w = grads[f"{prefix}fc_output_layer.weight"].data_ptr()
     g.fc_b = grads[f"{prefix}fc_output_layer.bias"].data_ptr()
     return g
 
 
-class _TrainForward(torch.autograd.Function):
-    """Model.forward in train mode with back-propagation through time in libfsn_b200 (fsn_train_forward /
-    fsn_train_backward).  The parameters are passed as inputs so autograd (and DDP's hooks) route the gradients to
-    them exactly as for the reference's nn.LSTM / nn.Linear modules (trainer.py:63)."""
-
-    @staticmethod
-    def forward(ctx, model, x, *params):
-        B, _, F, T = x.shape
-        device = x.device
-        lib = _lib.load()
-        with torch.cuda.device(device):
-            desc = model._desc(model._resolve_train_precision(), int(model.num_groups_in_drop_band))
-            fb_w, sb_w = model.fb_model.weight_struct(), model.sb_model.weight_struct()
-            n = lib.fsn_train_workspace_bytes(C.byref(desc), B, T)
-            if n == 0:
-                _lib.check_workspace(n)
-            ws = torch.empty(n, dtype=torch.uint8, device=device)
-            G = desc.num_groups_in_drop_band if B > 1 and desc.num_groups_in_drop_band > 1 else 1
-            out = torch.empty(B, 2, F // G if G > 1 else F, T, dtype=torch.float32, device=device)
-            _lib.check(lib.fsn_train_forward(C.byref(desc), C.byref(fb_w), C.byref(sb_w), x.data_ptr(), B, T,
-                                             out.data_ptr(), ws.data_ptr(), n, _lib.stream_ptr(device)))
-        ctx.model, ctx.ws, ctx.dims, ctx.desc = model, ws, (B, T), desc
-        ctx.versions = model.fb_model.version_key() + model.sb_model.version_key()
-        return out
-
-    @staticmethod
-    def backward(ctx, dcrm):
-        model, (B, T) = ctx.model, ctx.dims
-        if ctx.versions != model.fb_model.version_key() + model.sb_model.version_key():
-            raise RuntimeError("fullsubnet_b200: a parameter was modified in place between forward and backward")
-        if ctx.ws is None:
-            raise RuntimeError("fullsubnet_b200: backward through the same forward twice (activations were released)")
-        dcrm = dcrm.contiguous().float()
-        device = dcrm.device
-        lib = _lib.load()
-        names = [k for k, _ in model.named_parameters()]
-        flat, grads = model._new_flat_grads(device)
-        with torch.cuda.device(device):
-            fb_w, sb_w = model.fb_model.weight_struct(), model.sb_model.weight_struct()
-            gfb, gsb = _grad_struct(model.fb_model, grads, "fb_model."), _grad_struct(model.sb_model, grads, "sb_model.")
-            _lib.check(lib.fsn_train_backward(C.byref(ctx.desc), C.byref(fb_w), C.byref(sb_w), dcrm.data_ptr(), B, T,
-                                              C.byref(gfb), C.byref(gsb), ctx.ws.data_ptr(), ctx.ws.numel(),
-                                              _lib.stream_ptr(device)))
-        ctx.ws = None
-        return (None, None) + tuple(grads[k] for k in names)
-
-
 class Model(BaseModel):
+    # training step (trainer.py:56-63): fsn_train_forward keeps the activations, fsn_train_backward runs BPTT
+    TRAIN_ENTRY_POINTS = ("fsn_train_workspace_bytes", "fsn_train_forward", "fsn_train_backward")
+    TRAIN_TF32_STACKS = ("fb_model", "sb_model")
+
     def __init__(self, num_freqs, look_ahead, sequence_model, fb_num_neighbors, sb_num_neighbors,
                  fb_output_activate_function, sb_output_activate_function, fb_model_hidden_size,
                  sb_model_hidden_size, norm_type="offline_laplace_norm", num_groups_in_drop_band=2,
@@ -122,13 +80,18 @@ class Model(BaseModel):
         d = self._desc("f16x3_tc", 1)
         return "f16x3_tc" if _lib.load().fsn_sb_packed_bytes(C.byref(d)) > 0 else "fp32"
 
-    def _resolve_train_precision(self) -> str:
-        if self.train_precision == "auto":
-            ok = self.fb_model.hidden_size % 4 == 0 and self.sb_model.hidden_size % 4 == 0
-            return "tf32_tc" if ok else "fp32"
-        if self.train_precision not in ("fp32", "tf32_tc"):
-            raise ValueError("train_precision must be 'fp32', 'tf32_tc' or 'auto'")
-        return self.train_precision
+    def _train_desc(self):
+        return self._desc(self._resolve_train_precision(), int(self.num_groups_in_drop_band))
+
+    def _train_weights(self):
+        return C.byref(self.fb_model.weight_struct()), C.byref(self.sb_model.weight_struct())
+
+    def _train_grads(self, grads):
+        return C.byref(_grad_struct(grads, "fb_model.")), C.byref(_grad_struct(grads, "sb_model."))
+
+    def _train_out_shape(self, desc, B, F, T):
+        G = desc.num_groups_in_drop_band if B > 1 and desc.num_groups_in_drop_band > 1 else 1
+        return (B, 2, F // G, T)
 
     def _desc(self, precision: str, num_groups: int) -> "_lib.ModelDesc":
         return _lib.ModelDesc(
@@ -164,11 +127,8 @@ class Model(BaseModel):
         assert num_channels == 1, f"{self.__class__.__name__} takes the mag feature as inputs."
         assert num_freqs == self.num_freqs, f"num_freqs {num_freqs} != {self.num_freqs}"
         x = _lib.require_cuda(noisy_mag, "noisy_mag")
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            # training step (trainer.py:56-63): fp32 kernels that keep the activations for BPTT
-            if not all(p.requires_grad for p in self.parameters()):
-                raise NotImplementedError("fullsubnet_b200: partially frozen models are not built")
-            return _TrainForward.apply(self, x, *self.parameters())
+        if self._records_grad():
+            return TrainStep.apply(self, x, *self.parameters())
         device = x.device
         lib = _lib.load()
         with torch.cuda.device(device):

@@ -1,11 +1,62 @@
 """Host-side pieces of audio_zen/model/base_model.py that the drop-in Model needs:
-norm_wrapper (:356-372) name checking and weight_init (:374-439, CPU-side initialisation); plus the flat-gradient
-buffers the training steps of fullsubnet and fast_fullsubnet share."""
+norm_wrapper (:356-372) name checking and weight_init (:374-439, CPU-side initialisation); plus the training step
+that fullsubnet, fast_fullsubnet and fullband_baseline share (autograd Function, precision choice, flat gradients)."""
 from __future__ import annotations
+
+import ctypes as C
 
 import torch
 import torch.nn as nn
 import torch.nn.init as init
+
+from .. import _lib
+
+
+class TrainStep(torch.autograd.Function):
+    """Model.forward with back-propagation through time in libfsn_b200.  The parameters are passed as inputs so
+    autograd (and DDP's hooks) route the gradients to them exactly as for the reference's nn.LSTM / nn.Linear modules.
+    The model names its library entry points and supplies the descriptor, the weight / gradient arguments and the
+    output shape (BaseModel's training-step hooks)."""
+
+    @staticmethod
+    def forward(ctx, model, x, *params):
+        B, _, F, T = x.shape
+        device = x.device
+        lib = _lib.load()
+        query, fwd, _ = (getattr(lib, name) for name in model.TRAIN_ENTRY_POINTS)
+        with torch.cuda.device(device):
+            desc = model._train_desc()
+            weights = model._train_weights()
+            n = query(C.byref(desc), B, T)
+            if n == 0:
+                _lib.check_workspace(n)
+            ws = torch.empty(n, dtype=torch.uint8, device=device)
+            out = torch.empty(model._train_out_shape(desc, B, F, T), dtype=torch.float32, device=device)
+            _lib.check(fwd(C.byref(desc), *weights, x.data_ptr(), B, T, out.data_ptr(), ws.data_ptr(), n,
+                           _lib.stream_ptr(device)))
+        ctx.model, ctx.ws, ctx.dims, ctx.desc = model, ws, (B, T), desc
+        ctx.versions = model._version_key()
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        model, (B, T) = ctx.model, ctx.dims
+        if ctx.versions != model._version_key():
+            raise RuntimeError("fullsubnet_b200: a parameter was modified in place between forward and backward")
+        if ctx.ws is None:
+            raise RuntimeError("fullsubnet_b200: backward through the same forward twice (activations were released)")
+        dy = dy.contiguous().float()
+        device = dy.device
+        bwd = getattr(_lib.load(), model.TRAIN_ENTRY_POINTS[2])
+        names = [k for k, _ in model.named_parameters()]
+        _, grads = model._new_flat_grads(device)
+        with torch.cuda.device(device):
+            weights = model._train_weights()
+            g = model._train_grads(grads)
+            _lib.check(bwd(C.byref(ctx.desc), *weights, dy.data_ptr(), B, T, *g, ctx.ws.data_ptr(), ctx.ws.numel(),
+                           _lib.stream_ptr(device)))
+        ctx.ws = None
+        return (None, None) + tuple(grads[k] for k in names)
 
 
 class BaseModel(nn.Module):
@@ -35,6 +86,38 @@ class BaseModel(nn.Module):
                     init.orthogonal_(param.data)
                 else:
                     init.normal_(param.data)
+
+    # ---------------------------------------------------------------- training step (TrainStep)
+    # Each trainable model sets TRAIN_ENTRY_POINTS (library workspace query, forward, backward), TRAIN_TF32_STACKS (the
+    # SequenceModel attributes whose hidden sizes decide train_precision="auto") and implements _train_desc(),
+    # _train_weights() and _train_grads(grads): the descriptor and the ctypes arguments of the weights / gradients.
+    TRAIN_ENTRY_POINTS: tuple = ()
+    TRAIN_TF32_STACKS: tuple = ()
+
+    def _resolve_train_precision(self) -> str:
+        """"fp32" (FMA) or "tf32_tc" (wgmma tf32); "auto" = tf32_tc when the TRAIN_TF32_STACKS hidden sizes are
+        multiples of 4."""
+        if self.train_precision == "auto":
+            ok = all(getattr(self, s).hidden_size % 4 == 0 for s in self.TRAIN_TF32_STACKS)
+            return "tf32_tc" if ok else "fp32"
+        if self.train_precision not in ("fp32", "tf32_tc"):
+            raise ValueError("train_precision must be 'fp32', 'tf32_tc' or 'auto'")
+        return self.train_precision
+
+    def _records_grad(self) -> bool:
+        """True when this forward is a training step: gradients are enabled and the parameters require them.  A
+        partially frozen model raises."""
+        if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
+            return False
+        if not all(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("fullsubnet_b200: partially frozen models are not built")
+        return True
+
+    def _train_out_shape(self, desc, B, F, T):
+        return (B, 2, F, T)
+
+    def _version_key(self):
+        return tuple((p.data_ptr(), p._version) for p in self.parameters())
 
     def flat_grad(self):
         """Makes every ``p.grad`` a view into one persistent flat fp32 buffer (keeping current values) and returns

@@ -13,6 +13,8 @@ import torch.nn as nn
 
 from ... import _lib
 
+LSTM_PARAMS = ("weight_ih", "weight_hh", "bias_ih", "bias_hh")  # in the field order of fsn_lstm_layer / fsn_lstm_grads
+
 
 class SequenceModel(nn.Module):
     def __init__(self, input_size, output_size, hidden_size, num_layers, bidirectional,
@@ -49,8 +51,13 @@ class SequenceModel(nn.Module):
     def layer_struct(self, l: int = 0) -> "_lib.LstmLayer":
         """Raw device pointers of LSTM layer ``l`` (fsn_lstm_layer)."""
         lstm = self.sequence_model
-        return _lib.LstmLayer(*(self._check(getattr(lstm, f"{n}_l{l}"), f"{n}_l{l}")
-                                for n in ("weight_ih", "weight_hh", "bias_ih", "bias_hh")))
+        return _lib.LstmLayer(*(self._check(getattr(lstm, f"{n}_l{l}"), f"{n}_l{l}") for n in LSTM_PARAMS))
+
+    @staticmethod
+    def grads_struct(grads: dict, prefix: str, l: int) -> "_lib.LstmGrads":
+        """Pointers of the gradients of LSTM layer ``l`` (fsn_lstm_grads), from named gradient tensors; ``prefix`` is
+        the SequenceModel's name in the model followed by a dot."""
+        return _lib.LstmGrads(*(grads[f"{prefix}sequence_model.{n}_l{l}"].data_ptr() for n in LSTM_PARAMS))
 
     def fc_ptrs(self):
         return (self._check(self.fc_output_layer.weight, "fc_output_layer.weight"),
@@ -60,18 +67,11 @@ class SequenceModel(nn.Module):
         """Raw device pointers into the parameter storage (fsn_seq_weights)."""
         assert self.num_layers == 2 and hasattr(self, "fc_output_layer")
         w = _lib.SeqWeights()
-        lstm = self.sequence_model
         for l in range(2):
-            for field, name in (("w_ih", "weight_ih"), ("w_hh", "weight_hh"), ("b_ih", "bias_ih"), ("b_hh", "bias_hh")):
-                p = getattr(lstm, f"{name}_l{l}")
-                if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous():
-                    raise RuntimeError(f"fullsubnet_b200: parameter {name}_l{l} must be a contiguous fp32 CUDA tensor "
-                                       f"(got {p.device}, {p.dtype}); call model.cuda() first - there is no CPU path.")
-                getattr(w, field)[l] = p.data_ptr()
-        for field, p in (("fc_w", self.fc_output_layer.weight), ("fc_b", self.fc_output_layer.bias)):
-            if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous():
-                raise RuntimeError("fullsubnet_b200: fc_output_layer parameters must be contiguous fp32 CUDA tensors")
-            setattr(w, field, p.data_ptr())
+            layer = self.layer_struct(l)
+            for field in ("w_ih", "w_hh", "b_ih", "b_hh"):
+                getattr(w, field)[l] = getattr(layer, field)
+        w.fc_w, w.fc_b = self.fc_ptrs()
         return w
 
     def version_key(self):
