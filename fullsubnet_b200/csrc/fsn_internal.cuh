@@ -71,7 +71,9 @@ int cum_clip_scale_launch(const float2* fs, int B, int Tp, int F, float eps, flo
 int cum_unit_scale_launch(const float* magT, const float* fbT, RowMap map, int R, int Tp, int Ns, int Nf, float eps,
                           float* scaleT, cudaStream_t st, bool time_major = false);
 
-// tf32 wgmma GEMM (fsn_tgemm.cu): C[M,N] (+)= A[M,K] B[N,K]^T, fp32 row-major operands with 16-byte aligned rows
+// tf32 wgmma GEMM (fsn_tgemm.cu): C[M,N] (+)= A[M,K] B[N,K]^T, fp32 row-major operands with 16-byte aligned rows.
+// tgemm_available: the device can run it (sm_90, opt-in shared memory) and FSN_NO_TGEMM is unset; asks the CUDA runtime
+bool tgemm_available();
 bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, int K);
 int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
                  bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st);
@@ -115,9 +117,12 @@ static const size_t SPLITK_SCRATCH_FLOATS = (size_t)16 << 20;  // 64 MB of split
 static const int COLSUM_MAX_S = 512;                            // row slabs of a column sum
 
 // Per-layer precision of the training steps: a layer runs on the tf32 tensor cores when the step asks for FSN_PREC_TF32_TC
-// and its hidden size keeps the rows of its operands 16-byte aligned; otherwise on the fp32 kernels.
+// and its hidden size keeps the rows of its operands 16-byte aligned; otherwise on the fp32 kernels.  tf32_layer sizes the
+// workspaces (no GPU needed); the layers themselves also need tgemm_available(), else the whole layer - forward, BPTT and
+// weight gradients alike - runs the fp32 kernels in the tensor-core layout of the workspace.
 inline bool tf32_layer(int precision, int H) { return precision == FSN_PREC_TF32_TC && (H & 3) == 0; }
-// forward of one layer of a training step, on the variant tf32_layer picks (the fp32 one ignores rec / splitk / half)
+// forward of one layer of a training step, on the variant tf32_layer and tgemm_available pick (the fp32 one ignores rec /
+// splitk / half)
 int layer_forward(int precision, const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
                   float* rec, float* splitk, const LayerHalf* half, cudaStream_t st);
 
@@ -127,7 +132,8 @@ struct LayerBwd {
   LayerSave s;
   int R, K0, H;
   float *dh_rec, *dc;
-  float *w_hhT, *w_ihT;        // tensor-core path: [H,4H] / [K0,4H] transposed copies (else nullptr)
+  float *w_hhT, *w_ihT;        // tensor-core path: [H,4H] / [K0,4H] transposed copies (else nullptr; unused when
+                               // !tgemm_available())
   float* splitk;               // split-K space of the per-step GEMMs (used when the layer has only a few tiles)
 };
 // scratch of layer_weight_grads: K-major copies of dG / layer input (tensor-core path, tgemm_blocked_floats of the largest

@@ -38,7 +38,10 @@ template <int BN> struct Cfg {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   // BN = 128: 3 stages (96 KB) so two CTAs share an SM - one writes its tile while the other runs its main loop
   static constexpr int STAGES = (BN == 128) ? 3 : 4;
-  static constexpr int LAG = (BN == 128) ? 2 : 3;      // cp.async groups in flight per producer thread
+  // cp.async groups in flight per producer thread.  At most STAGES - 2: the producer waits for stage i - STAGES to be
+  // released before it marks stage i - LAG full, and the consumers release stage i - STAGES only once stage
+  // i - STAGES + 1 is full, so LAG = STAGES - 1 deadlocks as soon as a tile has more than STAGES k blocks
+  static constexpr int LAG = STAGES - 2;
   static constexpr int MIN_CTAS = (BN == 128) ? 2 : 1;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
@@ -416,7 +419,7 @@ static int tgemm_sm_count() {
 // fixed-order sum of split-K slabs (fsn_train.cu)
 int splitk_reduce_launch(const float* part, int S, int M, int N, float* C, size_t ldc, bool accumulate, cudaStream_t st);
 
-bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, int K) {
+bool tgemm_available() {
   static int ok = -1;
   if (ok < 0) {
     int dev = 0, major = 0, smem = 0;
@@ -425,7 +428,11 @@ bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, in
     cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     ok = (major == 9 && smem >= tg::Cfg<128>::SMEM && getenv("FSN_NO_TGEMM") == nullptr) ? 1 : 0;
   }
-  return ok == 1 && K >= 4 && (lda & 3) == 0 && (ldb & 3) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
+  return ok == 1;
+}
+
+bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, int K) {
+  return tgemm_available() && K >= 4 && (lda & 3) == 0 && (ldb & 3) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
          (reinterpret_cast<uintptr_t>(Bm) & 15) == 0;
 }
 

@@ -653,12 +653,15 @@ int layer_forward_save_tc(const fsn_lstm_layer& w, const float* X, int R, int K0
 
 int layer_forward(int precision, const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
                   float* rec, float* splitk, const LayerHalf* half, cudaStream_t st) {
-  if (!tf32_layer(precision, H)) return layer_forward_save(w, X, R, K0, H, Tp, s, st);
+  if (!tf32_layer(precision, H) || !tgemm_available()) return layer_forward_save(w, X, R, K0, H, Tp, s, st);
   return layer_forward_save_tc(w, X, R, K0, H, Tp, s, rec, st, splitk, SPLITK_SCRATCH_FLOATS, half);
 }
 
+// the backward half of the rule of layer_forward: the transposed weights mark a tf32 layer
+static bool tc_bwd(const LayerBwd& L) { return L.w_hhT && tgemm_available(); }
+
 int layer_bwd_transpose_weights(const LayerBwd& L, cudaStream_t st) {
-  if (!L.w_hhT) return FSN_OK;
+  if (!tc_bwd(L)) return FSN_OK;
   int rc;
   if ((rc = transpose_launch(L.w_hh, (size_t)4 * L.H, L.H, L.w_hhT, st))) return rc;
   if (L.w_ihT && (rc = transpose_launch(L.w_ih, (size_t)4 * L.H, L.K0, L.w_ihT, st))) return rc;
@@ -693,13 +696,14 @@ int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, cons
   lstm_bwd_point_kernel<<<blocks, 256, 0, st>>>(p);
   FSN_CHECK_LAUNCH("lstm_bwd_point_kernel");
   int rc;
+  const bool tc = tc_bwd(L);
   if (t > 0) {
-    if (L.w_hhT) rc = tgemm_launch(p.G, 4 * L.H, L.w_hhT, 4 * L.H, L.dh_rec, L.H, L.R, L.H, 4 * L.H, false, L.splitk, SPLITK_SCRATCH_FLOATS, st);
+    if (tc) rc = tgemm_launch(p.G, 4 * L.H, L.w_hhT, 4 * L.H, L.dh_rec, L.H, L.R, L.H, 4 * L.H, false, L.splitk, SPLITK_SCRATCH_FLOATS, st);
     else         rc = sgemm_launch(false, p.G, 4 * L.H, L.w_hh, L.H, L.dh_rec, L.H, L.R, L.H, 4 * L.H, false, nullptr, st);
     if (rc) return rc;
   }
   if (dx) {
-    if (L.w_ihT) rc = tgemm_launch(p.G, 4 * L.H, L.w_ihT, 4 * L.H, dx, L.K0, L.R, L.K0, 4 * L.H, false, L.splitk, SPLITK_SCRATCH_FLOATS, st);
+    if (tc && L.w_ihT) rc = tgemm_launch(p.G, 4 * L.H, L.w_ihT, 4 * L.H, dx, L.K0, L.R, L.K0, 4 * L.H, false, L.splitk, SPLITK_SCRATCH_FLOATS, st);
     else         rc = sgemm_launch(false, p.G, 4 * L.H, L.w_ih, L.K0, dx, L.K0, L.R, L.K0, 4 * L.H, false, nullptr, st);
     if (rc) return rc;
   }
@@ -711,8 +715,9 @@ int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih,
                        float* g_b_hh, const WgradScratch& w, cudaStream_t st) {
   const int H4 = 4 * L.H;
   const int rows = Tp * L.R;
+  const bool tc = tc_bwd(L);
   int rc;
-  if (L.w_hhT && tgemm_blocked_enabled()) {
+  if (tc && tgemm_blocked_enabled()) {
     // tensor-core path, block-tiled K-major copies (one contiguous 16 KB burst per TMA box instead of 128 rows with a
     // pitch of `rows` floats): dW_ih = dG^T X, dW_hh = dG[1:]^T H[:-1]
     const int nkb = (rows + 31) / 32;
@@ -739,7 +744,7 @@ int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih,
     }
     return FSN_OK;
   }
-  if (L.w_hhT && (L.R & 3) == 0) {
+  if (tc && (L.R & 3) == 0) {
     // tensor-core path: K-major operands = transposed copies dG^T [4H, rows], X^T [K0, rows], H^T [H, rows]
     if ((rc = transpose_launch(L.s.G, (size_t)rows, H4, w.gT, st))) return rc;
     if ((rc = transpose_launch(X, (size_t)rows, L.K0, w.xT, st))) return rc;
@@ -1028,6 +1033,121 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   if ((rc = layer_weight_grads(fbL[1], Tp, w.fb[0].H, gfb->w_ih[1], gfb->w_hh[1], gfb->b_ih[1], gfb->b_hh[1], wg, st)))
     return rc;
   return layer_weight_grads(fbL[0], Tp, w.xfb, gfb->w_ih[0], gfb->w_hh[0], gfb->b_ih[0], gfb->b_hh[0], wg, st);
+}
+
+// ------------------------------------------------------------------------------------------ unit-test hook
+// An n-layer LSTM stack through the shared training pieces alone (layer_forward, layer_bwd_transpose_weights, stack_bwd,
+// layer_weight_grads), wired like fsn_fullband_train_*: per-layer saves and BPTT slots, layer l's fp16 hidden states are
+// layer l+1's fp16 input, one split-K / column-sum / K-major scratch for all layers.
+namespace fsn {
+static const int DBG_MAX_LAYERS = 8;
+
+struct DbgLstmWs {
+  LayerSave L[DBG_MAX_LAYERS];
+  float *dh_rec[DBG_MAX_LAYERS], *dc[DBG_MAX_LAYERS], *dh_mid[2];
+  float *splitk, *colsum, *gT, *xT, *rec;
+  float *whhT[DBG_MAX_LAYERS], *wihT[DBG_MAX_LAYERS];
+  __half *h16[DBG_MAX_LAYERS], *w16;
+  size_t bytes;
+};
+
+static void carve_dbg_lstm(int n, int R, int T, int K0, int H, int precision, void* base, DbgLstmWs& w) {
+  Carver c(base);
+  const size_t rows = (size_t)T * R, Hs = H, RH = (size_t)R * H, K0max = K0 > H ? K0 : H;
+  for (int l = 0; l < n; ++l) {
+    w.L[l].G = c.take<float>(rows * 4 * Hs); w.L[l].C = c.take<float>(rows * Hs); w.L[l].H = c.take<float>(rows * Hs);
+  }
+  for (int l = 0; l < n; ++l) { w.dh_rec[l] = c.take<float>(RH); w.dc[l] = c.take<float>(RH); }
+  w.dh_mid[0] = c.take<float>(RH);
+  w.dh_mid[1] = c.take<float>(RH);
+  w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
+  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * 4 * Hs);
+  w.gT = w.xT = w.rec = nullptr;
+  w.w16 = nullptr;
+  for (int l = 0; l < DBG_MAX_LAYERS; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
+  if (tf32_layer(precision, H)) {
+    for (int l = 0; l < n; ++l) {
+      w.whhT[l] = c.take<float>(Hs * 4 * Hs);
+      w.wihT[l] = c.take<float>((l == 0 ? (size_t)K0 : Hs) * 4 * Hs);  // layer 0's is used only when dx is asked for
+      w.h16[l] = c.take<__half>(rows * Hs);
+    }
+    w.gT = c.take<float>(tgemm_blocked_floats(rows, 4 * H));
+    w.xT = c.take<float>(tgemm_blocked_floats(rows, (int)K0max));
+    w.rec = c.take<float>(4 * RH);
+    w.w16 = c.take<__half>(4 * Hs * (Hs + K0max));
+  }
+  w.bytes = c.off;
+}
+
+static int dbg_lstm_check(int n, int R, int T, int K0, int H, int precision) {
+  FSN_REQUIRE(precision == FSN_PREC_FP32 || precision == FSN_PREC_TF32_TC, FSN_ERR_UNSUPPORTED,
+              "lstm_train hook: precision must be fp32 or tf32_tc");
+  FSN_REQUIRE(n >= 1 && n <= DBG_MAX_LAYERS, FSN_ERR_UNSUPPORTED, "lstm_train hook: 1..%d layers (got %d)", DBG_MAX_LAYERS, n);
+  FSN_REQUIRE(R > 0 && T > 0 && K0 > 0 && H > 0, FSN_ERR_SHAPE, "lstm_train hook: bad dims R=%d T=%d K0=%d H=%d", R, T, K0, H);
+  const size_t K0max = K0 > H ? K0 : H;
+  FSN_REQUIRE((size_t)T * R * 4 * ((size_t)H > K0max ? (size_t)H : K0max) < ((size_t)1 << 31), FSN_ERR_SHAPE,
+              "lstm_train hook: T*R*4*max(H,K0) must stay below 2^31");
+  return FSN_OK;
+}
+}  // namespace fsn
+
+extern "C" size_t fsn_debug_lstm_train_workspace_bytes(int n_layers, int R, int T, int K0, int H, int precision) {
+  if (dbg_lstm_check(n_layers, R, T, K0, H, precision)) return 0;
+  DbgLstmWs w;
+  carve_dbg_lstm(n_layers, R, T, K0, H, precision, nullptr, w);
+  return w.bytes;
+}
+
+extern "C" int fsn_debug_lstm_train(const fsn_lstm_layer* layers, int n_layers, int R, int T, int K0, int H, int precision,
+                                    const float* x, const float* dh_top, const float* dout, const float* fc_w, int O,
+                                    float* h_top, float* dx, const fsn_lstm_grads* g, float* trace, void* workspace,
+                                    size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  const int n = n_layers;
+  int rc = dbg_lstm_check(n, R, T, K0, H, precision);
+  if (rc) return rc;
+  FSN_REQUIRE(layers && x && h_top && g, FSN_ERR_SHAPE, "lstm_train hook: null argument");
+  FSN_REQUIRE(dh_top || dout, FSN_ERR_SHAPE, "lstm_train hook: no gradient on top (dh_top and dout both null)");
+  FSN_REQUIRE(dout ? (fc_w && O >= 1) : (!fc_w && O == 0), FSN_ERR_SHAPE,
+              "lstm_train hook: dout, fc_w and O >= 1 come together (O=%d)", O);
+  for (int l = 0; l < n; ++l)
+    FSN_REQUIRE(layers[l].w_ih && layers[l].w_hh && layers[l].b_ih && layers[l].b_hh && g[l].w_ih && g[l].w_hh && g[l].b_ih &&
+                    g[l].b_hh,
+                FSN_ERR_SHAPE, "lstm_train hook: null weight or gradient of layer %d", l);
+  DbgLstmWs w;
+  carve_dbg_lstm(n, R, T, K0, H, precision, workspace, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes,
+              w.bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t TRH = (size_t)T * R * H;
+  auto in_width = [&](int l) { return l == 0 ? K0 : H; };
+  for (int l = 0; l < n; ++l) {
+    const LayerHalf half{w.h16[l], l > 0 ? w.h16[l - 1] : nullptr, w.w16};
+    if ((rc = layer_forward(precision, layers[l], l == 0 ? x : w.L[l - 1].H, R, in_width(l), H, T, w.L[l], w.rec, w.splitk,
+                            &half, st)))
+      return rc;
+  }
+  if ((rc = check_cuda(cudaMemcpyAsync(h_top, w.L[n - 1].H, TRH * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy")))
+    return rc;
+  LayerBwd L[DBG_MAX_LAYERS];
+  for (int l = 0; l < n; ++l) {
+    L[l] = LayerBwd{layers[l].w_ih, layers[l].w_hh, w.L[l], R, in_width(l), H, w.dh_rec[l], w.dc[l], w.whhT[l],
+                    (l > 0 || dx) ? w.wihT[l] : nullptr, w.splitk};
+    if ((rc = layer_bwd_transpose_weights(L[l], st))) return rc;
+  }
+  if ((rc = stack_bwd(L, n, T, dh_top, dout, fc_w, O, w.dh_mid[0], w.dh_mid[1], dx, st))) return rc;
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  for (int l = n - 1; l >= 0; --l)
+    if ((rc = layer_weight_grads(L[l], T, l == 0 ? x : w.L[l - 1].H, g[l].w_ih, g[l].w_hh, g[l].b_ih, g[l].b_hh, wg, st)))
+      return rc;
+  if (trace)  // per layer: the saved hidden states [T,R,H], then dG [T,R,4H] (the gate buffer after BPTT)
+    for (int l = 0; l < n; ++l) {
+      float* dst = trace + (size_t)l * 5 * TRH;
+      if ((rc = check_cuda(cudaMemcpyAsync(dst, w.L[l].H, TRH * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy")) ||
+          (rc = check_cuda(cudaMemcpyAsync(dst + TRH, w.L[l].G, 4 * TRH * sizeof(float), cudaMemcpyDeviceToDevice, st), "copy")))
+        return rc;
+    }
+  return FSN_OK;
 }
 
 // ------------------------------------------------------------------------------------------ loss

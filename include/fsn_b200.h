@@ -442,6 +442,21 @@ int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int f
                          const float* inv2, const float* unit_scale, int la, int steps, int shrink,
                          int stages, int cluster, void* packed, float* crm, fsn_stream_t stream);
 
+/* unit-test hook for the LSTM layer shared by the training steps (fsn_train.cu): torch.nn.LSTM(K0, H, num_layers =
+ * n_layers) over x [T,R,K0] (time-major) through the same activation-saving forward, BPTT and weight-gradient pieces
+ * as fsn_train_* / fsn_fast_train_* / fsn_fullband_train_*, wired like fsn_fullband_train_*.  Layer 0 maps K0 -> H, the
+ * others H -> H.  Gradient on top: dh_top [T,R,H] and / or a Linear(H -> O) folded into the top layer, dout [T,R,O] with
+ * fc_w [O,H] (dout, fc_w and O >= 1 together, else NULL, NULL, 0).  Outputs: h_top [T,R,H]; dx [T,R,K0] when not NULL;
+ * g[l] = the gradients of layer l (overwritten, not accumulated); trace (nullable, n_layers * 5*T*R*H floats): per layer
+ * its hidden states [T,R,H] then dG [T,R,4H], the pre-activation gate gradients the weight gradients are built from.
+ * precision FSN_PREC_FP32 or FSN_PREC_TF32_TC (per layer as in the training steps), else FSN_ERR_UNSUPPORTED, as are
+ * n_layers outside 1..8.  Arguments are checked before any CUDA call; the workspace query needs no GPU. */
+size_t fsn_debug_lstm_train_workspace_bytes(int n_layers, int R, int T, int K0, int H, int precision);
+int fsn_debug_lstm_train(const fsn_lstm_layer* layers, int n_layers, int R, int T, int K0, int H, int precision,
+                         const float* x, const float* dh_top, const float* dout, const float* fc_w, int O, float* h_top,
+                         float* dx, const fsn_lstm_grads* g, float* trace, void* workspace, size_t workspace_bytes,
+                         fsn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -242,6 +242,64 @@ def test_c_abi_argument_validation_without_gpu():
         _lib.check(_lib.FSN_ERR_CUDA)
 
 
+def test_lstm_train_hook_checks_arguments_without_gpu():
+    """fsn_debug_lstm_train (the shared training LSTM layer alone) rejects every bad argument with its error class before
+    any CUDA call, and its workspace query needs no GPU: non-zero, growing with the layer count, the rows and the steps."""
+    import ctypes as C
+    from fullsubnet_b200 import _lib
+    lib = _lib.load()
+    q = lib.fsn_debug_lstm_train_workspace_bytes
+    fp32, tf32 = _lib.PREC["fp32"], _lib.PREC["tf32_tc"]
+    for prec in (fp32, tf32):
+        n = q(2, 31, 6, 20, 64, prec)
+        assert n > 0
+        assert q(3, 31, 6, 20, 64, prec) > n and q(2, 32, 6, 20, 64, prec) > n and q(2, 31, 7, 20, 64, prec) > n
+        assert q(8, 31, 6, 20, 64, prec) > q(3, 31, 6, 20, 64, prec)
+    assert q(2, 31, 6, 20, 64, tf32) > q(2, 31, 6, 20, 64, fp32)  # transposed weights, K-major and fp16 copies
+    assert q(2, 31, 6, 20, 257, tf32) == q(2, 31, 6, 20, 257, fp32)  # H % 4 != 0: the fp32 kernels and layout
+    for args, code in (((0, 4, 5, 8, 32, fp32), _lib.FSN_ERR_UNSUPPORTED), ((9, 4, 5, 8, 32, fp32), _lib.FSN_ERR_UNSUPPORTED),
+                       ((2, 4, 5, 8, 32, _lib.PREC["f16_tc"]), _lib.FSN_ERR_UNSUPPORTED),
+                       ((2, 0, 5, 8, 32, fp32), _lib.FSN_ERR_SHAPE), ((2, 4, 0, 8, 32, fp32), _lib.FSN_ERR_SHAPE),
+                       ((2, 4, 5, 0, 32, fp32), _lib.FSN_ERR_SHAPE), ((2, 4, 5, 8, 0, fp32), _lib.FSN_ERR_SHAPE),
+                       ((1, 1 << 16, 1 << 10, 8, 32, fp32), _lib.FSN_ERR_SHAPE)):  # 2^31 floats in one gate buffer
+        assert q(*args) == 0, args
+        assert lib.fsn_last_error_code() == code, (args, lib.fsn_last_error())
+
+    # the hook itself: stand-in device pointers, never dereferenced because every check fails before the first launch
+    n, R, T, K0, H = 2, 4, 5, 8, 32
+    p = 1 << 20
+
+    def layers():
+        return (_lib.LstmLayer * n)(*[_lib.LstmLayer(p, p, p, p) for _ in range(n)])
+
+    def grads():
+        return (_lib.LstmGrads * n)(*[_lib.LstmGrads(p, p, p, p) for _ in range(n)])
+
+    need = q(n, R, T, K0, H, fp32)
+
+    def call(n=n, R=R, prec=fp32, x=p, dh=p, dout=None, fc_w=None, O=0, L=None, g=None, ws=p, nbytes=need):
+        return lib.fsn_debug_lstm_train(L if L is not None else layers(), n, R, T, K0, H, prec, x, dh, dout, fc_w, O, p, p,
+                                        g if g is not None else grads(), None, ws, nbytes, None)
+
+    assert call(n=0) == _lib.FSN_ERR_UNSUPPORTED and call(n=9) == _lib.FSN_ERR_UNSUPPORTED
+    assert call(prec=_lib.PREC["f16x3_tc"]) == _lib.FSN_ERR_UNSUPPORTED
+    assert call(R=-1) == _lib.FSN_ERR_SHAPE
+    assert call(x=None) == _lib.FSN_ERR_SHAPE
+    assert call(dh=None) == _lib.FSN_ERR_SHAPE and b"no gradient on top" in lib.fsn_last_error()
+    assert call(dout=p, O=2) == _lib.FSN_ERR_SHAPE  # a Linear on top without its weight
+    assert call(dout=p, fc_w=p, O=0) == _lib.FSN_ERR_SHAPE
+    assert call(O=1) == _lib.FSN_ERR_SHAPE  # O with no fc_w
+    bad = grads()
+    bad[1].b_hh = None
+    assert call(g=bad) == _lib.FSN_ERR_SHAPE and b"layer 1" in lib.fsn_last_error()
+    bad = layers()
+    bad[0].w_ih = None
+    assert call(L=bad) == _lib.FSN_ERR_SHAPE
+    assert call(nbytes=need - 1) == _lib.FSN_ERR_WORKSPACE
+    assert call(ws=None) == _lib.FSN_ERR_WORKSPACE
+    assert call(prec=tf32, nbytes=need) == _lib.FSN_ERR_WORKSPACE  # the tensor-core layout is larger
+
+
 def test_row_map_and_reflect_count_match_oracle():
     """The drop_band row map (feature.py:332-345) and its inverse as compiled into the library vs the oracle's index
     form; reflect multiplicity c[r] of the closed-form second norm (SURVEY A6) vs the oracle and its closed values."""
