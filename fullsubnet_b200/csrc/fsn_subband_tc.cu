@@ -191,6 +191,19 @@ __device__ __forceinline__ float act_apply(float v, int act) {
 template <bool X3> __device__ __forceinline__ float sg(float x) { return X3 ? 1.0f / (1.0f + expf(-x)) : fast_sigmoid(x); }
 template <bool X3> __device__ __forceinline__ float th(float x) { return X3 ? 1.0f - 2.0f / (1.0f + expf(2.0f * x)) : fast_tanh(x); }
 
+// Consumer warpgroup releases weight stage `bar` to the producers of the CL CTAs that share the stream: one arrive per
+// warpgroup and destination CTA (w_empty counts CL), warp q signalling CTA q so that the remote arrives go out in
+// parallel.  No fence is needed: the stage is read only by this warpgroup's wgmma (async proxy), the wgmma.wait_group
+// before this call has retired those reads, and the producers overwrite the stage with TMA (async proxy) only after
+// the w_empty phase completes - the barrier phase alone orders the overwrite after the reads, so the arrive keeps its
+// default .release.cta semantics (the hand-off of CUTLASS's TMA pipelines for the same hazard).  Every warp of the
+// warpgroup has passed the w_full wait of the stage: the MMAs that read it are warpgroup-collective.
+__device__ __forceinline__ void release_stage(uint64_t* bar, int CL, int q, int lane) {
+  if (lane != 0 || q >= CL) return;
+  if (CL == 1) mbar_arrive(bar);
+  else mbar_arrive_remote(bar, (uint32_t)q);
+}
+
 template <bool X3>
 __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) {
   constexpr int PARTS = X3 ? 2 : 1;
@@ -217,7 +230,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
 
   // ---------------- one-time setup
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.w_full[s], 1); mbar_init(&bars.w_empty[s], 4 * CL); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.w_full[s], 1); mbar_init(&bars.w_empty[s], CL); }
     for (int i = 0; i < 2; ++i) { mbar_init(&bars.x_full[i], 1); mbar_init(&bars.x_empty[i], 4 * MT); }
     mbar_init(&bars.h0_ready, 4 * MT);
     mbar_init(&bars.h1_ready, 4 * MT);
@@ -243,7 +256,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
     const int n16 = (sp.fcw - sp.x) / 16;
     for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
   }
-  fence_proxy_async();
+  fence_proxy_async_smem();
   __syncthreads();
   if (CL > 1) cluster_sync_all();  // peers' barriers are initialised before any multicast reaches them
 
@@ -258,7 +271,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
       const size_t t_end = (it >= 1) ? PL.tiles0 + PL.tiles1 : PL.tiles0;
       const uint8_t* src = a.packed + t_begin * W_TILE;
       for (size_t tile = t_begin; tile < t_end; ++tile, src += W_TILE) {
-        mbar_wait<true>(&bars.w_empty[stage], phase ^ 1);  // all CL CTAs' consumers have drained this stage
+        // all CL CTAs' consumers have drained this stage (on the critical path: no back-off)
+        mbar_wait_cta<false>(&bars.w_empty[stage], phase ^ 1);
         if (elect_one()) {
           mbar_expect_tx(&bars.w_full[stage], W_TILE);
           if (CL == 1) {
@@ -277,7 +291,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
     // scaled by 1/(mu'+1e-5)  (base_model.py:35-44, model.py:98-111), fp16 (X3: + lo), B-operand layout
     const int nmag = 2 * a.Ns + 1;
     for (int t = 0; t < Tp; ++t) {
-      mbar_wait<true>(&bars.x_empty[t & 1], ((t >> 1) & 1) ^ 1);
+      mbar_wait_cta<true>(&bars.x_empty[t & 1], ((t >> 1) & 1) ^ 1);
       uint8_t* xb = smem + sp.x + (t & 1) * S_KBLK;
       // source frames of step t: itself, or (fast_fullsubnet/model.py:108-129) frame 0 alone, then blocks of
       // `shrink` frames, the last one over its own length
@@ -304,7 +318,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
         *reinterpret_cast<__half*>(xb + swz128_off(n, lane)) = hi;
         if (X3) *reinterpret_cast<__half*>(xb + LO + swz128_off(n, lane)) = __float2half_rn(v - __half2float(hi));
       }
-      fence_proxy_async();
+      fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars.x_full[t & 1]);
     }
@@ -317,7 +331,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
     const RowInfo ri = rows[ln];
     int staged = 0, t_stage0 = 0;
     for (int t = 0; t < Tp; ++t) {
-      mbar_wait<true>(&bars.h1_ready, t & 1);
+      mbar_wait_cta<true>(&bars.h1_ready, t & 1);
       if (t >= a.la) {
         float s0 = fcb0, s1 = fcb1;
         for (int w = 0; w < 4 * MT; ++w) {
@@ -366,12 +380,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
           const int t = it - layer;
           if (t < 0 || t >= Tp) continue;
           // operands of this step complete in shared memory (every phase waited on once, in order)
+          // (all of this kernel's barriers guard data written by this CTA or by TMA: CTA-scope waits)
           if (layer == 0) {
-            mbar_wait_mma(&bars.x_full[t & 1], (t >> 1) & 1);
-            for (; h0_seen < t; ++h0_seen) mbar_wait_mma(&bars.h0_ready, h0_seen & 1);      // h0_{t-1}
+            mbar_wait_cta<false>(&bars.x_full[t & 1], (t >> 1) & 1);
+            for (; h0_seen < t; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready, h0_seen & 1);      // h0_{t-1}
           } else {
-            for (; h0_seen < t + 1; ++h0_seen) mbar_wait_mma(&bars.h0_ready, h0_seen & 1);  // h0_t
-            for (; h1_seen < t; ++h1_seen) mbar_wait_mma(&bars.h1_ready, h1_seen & 1);      // h1_{t-1}
+            for (; h0_seen < t + 1; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready, h0_seen & 1);  // h0_t
+            for (; h1_seen < t; ++h1_seen) mbar_wait_cta<false>(&bars.h1_ready, h1_seen & 1);      // h1_{t-1}
           }
           const uint32_t x_addr = smem_u32(smem + sp.x + (t & 1) * S_KBLK);
           const uint32_t h0_cur = smem_u32(smem + sp.h0 + (t & 1) * nkh * S_KBLK);        // h0_t
@@ -390,8 +405,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
               wg::fence_operand(acc[g][hf]);
             }
           int prev_stage = -1;
-          if (m > 0 || !first_block) { mbar_wait_mma(&bars.turn[m], turns & 1); ++turns; }
+          if (m > 0 || !first_block) { mbar_wait_cta<false>(&bars.turn[m], turns & 1); ++turns; }
           first_block = false;
+          // ring slot and fill parity of stream stage `first`, then advanced stage by stage
+          int stage = (int)(first % (size_t)STAGES);
+          uint32_t wphase = (uint32_t)((first / (size_t)STAGES) & 1);
           for (int j = 0; j < nkb; ++j) {
             uint32_t sb;  // state address of k range j
             if (layer == 0) sb = (j == 0) ? x_addr : h0_prev + ((j - 1) >> 1) * S_KBLK + ((j - 1) & 1) * 64;
@@ -399,9 +417,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
                                    : h1_prev + ((j - H / KS) >> 1) * S_KBLK + ((j - H / KS) & 1) * 64;
 #pragma unroll
             for (int part = 0; part < PARTS; ++part) {
-              const size_t gi = first + (size_t)j * PARTS + part;
-              const int stage = (int)(gi % (size_t)STAGES);
-              mbar_wait_mma(&bars.w_full[stage], (uint32_t)((gi / (size_t)STAGES) & 1));
+              mbar_wait_cta<false>(&bars.w_full[stage], wphase);
               if (j == nkb - 1 && part == PARTS - 1 && lane == 0) mbar_arrive(&bars.turn[m + 1 < MT ? m + 1 : 0]);
               wg::fence();
               const uint32_t wa = wbase + stage * W_TILE;
@@ -419,11 +435,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
               }
               wg::commit();
               wg::wait<1>();  // the MMAs of the previous stage have read it
-              if (prev_stage >= 0 && lane == 0) {
-                if (CL == 1) mbar_arrive(&bars.w_empty[prev_stage]);
-                else for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&bars.w_empty[prev_stage], (uint32_t)r);
-              }
+              if (prev_stage >= 0) release_stage(&bars.w_empty[prev_stage], CL, q, lane);
               prev_stage = stage;
+              if (++stage == STAGES) { stage = 0; wphase ^= 1; }
             }
           }
           wg::wait<0>();
@@ -431,13 +445,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
           for (int g = 0; g < 4; ++g)
 #pragma unroll
             for (int hf = 0; hf < 2; ++hf) wg::fence_operand(acc[g][hf]);
-          if (lane == 0) {
-            if (CL == 1) mbar_arrive(&bars.w_empty[prev_stage]);
-            else for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&bars.w_empty[prev_stage], (uint32_t)r);
-            // this warpgroup's MMAs of the step have consumed x_t / h1_{t-1}
-            mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
-          }
-          if (layer == 1 && t >= 1) mbar_wait_mma(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
+          release_stage(&bars.w_empty[prev_stage], CL, q, lane);
+          // this warpgroup's MMAs of the step have consumed x_t / h1_{t-1}
+          if (lane == 0) mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
+          if (layer == 1 && t >= 1) mbar_wait_cta<false>(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
           float fsum[2][4];  // Linear partials [o][row slot j*2+e]
 #pragma unroll
           for (int i = 0; i < 8; ++i) fsum[i >> 2][i & 3] = 0.f;
@@ -487,7 +498,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
                 for (int s = 0; s < 4; ++s) my_part[o * NB + 8 * (s >> 1) + 2 * lane + (s & 1)] = fsum[o][s];
             }
             // every layer-1 MMA of this step (all warpgroups) has consumed h1_{t-1}: overwrite it with h1_t
-            mbar_wait_mma(&bars.l1_done, t & 1);
+            mbar_wait_cta<false>(&bars.l1_done, t & 1);
           }
 #pragma unroll
           for (int hf = 0; hf < 2; ++hf)
@@ -506,7 +517,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
                   if (X3) *reinterpret_cast<__half*>(p + LO) = lv[hf][hh][j * 2 + e];
                 }
             }
-          fence_proxy_async();
+          fence_proxy_async_smem();
           __syncwarp();
           if (lane == 0) mbar_arrive(layer ? &bars.h1_ready : &bars.h0_ready);
         }
@@ -557,27 +568,36 @@ int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed,
   return sb_tc_pack_raw(sb, d->sb_hidden, sb_ksb(d), 2, packed, st, d->precision == FSN_PREC_F16X3_TC);
 }
 
+// launch configuration of `tiles` CTAs (the caller keeps `attr` alive while cfg is used)
 template <bool X3>
-static int sb_tc_launch(const tc::KArgs& a, int H, cudaStream_t st) {
-  const tc::Smem sp = tc::smem_plan(H, a.stages, X3);
+static int sb_tc_config(int H, int stages, int cluster, int tiles, cudaStream_t st, cudaLaunchConfig_t& cfg,
+                        cudaLaunchAttribute* attr) {
+  const tc::Smem sp = tc::smem_plan(H, stages, X3);
   const size_t smem = sp.total + 1024;  // slack for the 1024-byte alignment of the dynamic segment
   int rc = check_cuda(cudaFuncSetAttribute(tc::sb_lstm_tc_kernel<X3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)smem), "sb_lstm_tc smem attr");
   if (rc) return rc;
-  const int tiles = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;  // padding CTAs own no valid row
-  cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(tiles);
   cfg.blockDim = dim3(128 + 128 * (H / 128));
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = a.cluster;
+  attr[0].val.clusterDim.x = cluster;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  return FSN_OK;
+}
+
+template <bool X3>
+static int sb_tc_launch(const tc::KArgs& a, int H, cudaStream_t st) {
+  const int tiles = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;  // padding CTAs own no valid row
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  int rc = sb_tc_config<X3>(H, a.stages, a.cluster, tiles, st, cfg, attr);
+  if (rc) return rc;
   rc = check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_lstm_tc_kernel<X3>, a), "sb_lstm_tc_kernel launch");
   if (rc) return rc;
   FSN_CHECK_LAUNCH("sb_lstm_tc_kernel");
@@ -618,6 +638,23 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
 // unit-test hook (tests/test_gpu_subband_tc.py): the sub-band stack on caller-provided inputs and launch configuration
 extern "C" size_t fsn_debug_sb_lstm_tc_packed_bytes(int H, int x3) {
   return fsn::sb_tc_shape_ok(H, 0) ? fsn::sb_tc_packed_bytes_raw(H, x3 != 0) : 0;
+}
+
+extern "C" int fsn_debug_sb_lstm_tc_max_clusters(int H, int x3, int stages, int cluster, int* clusters) {
+  using namespace fsn;
+  FSN_REQUIRE(cluster == 1 || cluster == 2 || cluster == 4, FSN_ERR_UNSUPPORTED,
+              "sb_lstm_tc: cluster size %d (1, 2 or 4)", cluster);
+  FSN_REQUIRE(stages >= 2 && stages <= tc::MAX_STAGES, FSN_ERR_UNSUPPORTED, "sb_lstm_tc: ring depth %d (2, 3 or 4)",
+              stages);
+  FSN_REQUIRE(sb_tc_shape_ok(H, 0), FSN_ERR_UNSUPPORTED, "sb_lstm_tc: unsupported hidden size %d", H);
+  FSN_REQUIRE(clusters, FSN_ERR_SHAPE, "sb_lstm_tc: missing output");
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  int rc = x3 ? sb_tc_config<true>(H, stages, cluster, cluster, nullptr, cfg, attr)
+              : sb_tc_config<false>(H, stages, cluster, cluster, nullptr, cfg, attr);
+  if (rc) return rc;
+  return x3 ? check_cuda(cudaOccupancyMaxActiveClusters(clusters, tc::sb_lstm_tc_kernel<true>, &cfg), "sb_lstm_tc occupancy")
+            : check_cuda(cudaOccupancyMaxActiveClusters(clusters, tc::sb_lstm_tc_kernel<false>, &cfg), "sb_lstm_tc occupancy");
 }
 
 extern "C" int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,

@@ -94,6 +94,38 @@ __device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
     if (++spins > (1u << 27)) asm volatile("trap;");
 }
 
+// ---- CTA-scope hand-offs.  A wait with .acquire.cluster makes every successful wait invalidate L1 (CCTL.IVALL) and
+// an arrive with .release.cluster fences at GPU scope (MEMBAR.ALL.GPU, ~1000 issue cycles) - neither is needed where
+// the data behind the barrier is written by this CTA, or by the TMA engine (async proxy, complete_tx)
+__device__ __forceinline__ bool mbar_try_wait_cta(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.acquire.cta.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.b32 %0, 1, 0, p;\n\t}"
+      : "=r"(ok)
+      : "r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
+// spin with a watchdog (trap, see mbar_wait); SLEEP = back off between polls, for waits off the critical path
+template <bool SLEEP>
+__device__ __forceinline__ void mbar_wait_cta(uint64_t* bar, uint32_t parity) {
+  uint32_t spins = 0;
+  while (!mbar_try_wait_cta(bar, parity)) {
+    if (SLEEP) __nanosleep(64);
+    if (++spins > (SLEEP ? (1u << 24) : (1u << 27))) asm volatile("trap;");
+  }
+}
+// generic-proxy writes to this CTA's shared memory -> later async-proxy reads (wgmma operands).  fence.proxy.async
+// without a state space also covers global memory and costs a GPU-scope MEMBAR
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// arrive on the barrier at the same offset in CTA `rank` of the cluster with the default .release.cta semantics: orders
+// nothing beyond the arriving thread's own CTA, so it publishes no generic-proxy data to the peer - an event signal
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa(smem_u32(bar), rank)) : "memory");
+}
+
 // ---- TMA engine (non-tensor bulk copy) and proxy fence
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(

@@ -437,6 +437,9 @@ int fsn_debug_linear_tc(const float* x, int rows, int K, const float* W, const f
  * (outputs beyond fc_out are act(0)).  stages (2..4) and cluster (1, 2, 4) choose the launch configuration, 0 = the
  * FSN_TC_STAGES / FSN_TC_CLUSTER default.  Arguments are checked before any CUDA call. */
 size_t fsn_debug_sb_lstm_tc_packed_bytes(int H, int x3);
+/* *clusters = how many clusters of the sub-band kernel can be resident at once on the current device for that launch
+ * configuration (cudaOccupancyMaxActiveClusters) */
+int fsn_debug_sb_lstm_tc_max_clusters(int H, int x3, int stages, int cluster, int* clusters);
 int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
                          const float* magT, const float* fbT, int B, int F, int src_T, int G,
                          const float* inv2, const float* unit_scale, int la, int steps, int shrink,
