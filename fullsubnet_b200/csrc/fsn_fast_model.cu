@@ -1,7 +1,6 @@
 // fast_fullsubnet (recipes/dns_interspeech_2020/fast_fullsubnet/model.py:11-202, BASELINE config 4): host
 // orchestration and the few extra kernels on top of the shared fp32 building blocks (mel filtering, real-time
 // down/up-sampling, bottleneck input, decoder re-layout).
-#include <stdlib.h>
 #include <string.h>
 
 #include "fsn_internal.cuh"
@@ -80,37 +79,40 @@ __global__ void fast_output_kernel(const float* __restrict__ dec, int B, int Tp,
   }
 }
 
+// GRU: the inference kernels of this model are built for LSTM only
 static bool fast_tc_ok(const fsn_fast_desc* d) {
   const int K = (2 * d->noisy_num_neighbors + 1) + (2 * d->enc_num_neighbors + 1);
-  return d->bn_hidden == 384 && d->bn_layers == 2 && K <= 32;
+  return d->cell_type == FSN_CELL_LSTM && d->bn_hidden == 384 && d->bn_layers == 2 && K <= 32;
 }
 static bool fast_x3(const fsn_fast_desc* d) { return d->precision == FSN_PREC_F16X3_TC; }
 
 struct FastWs {
   float *magT, *melT, *encT, *bn, *bn_out, *dec_in, *dec_out, *inv1, *inv2;
   float2 *fs, *sums;
-  float *e1_h[2], *e1_c, *e2_hall, *e2_c;
   float *bn_h0[2], *bn_h1[2], *bn_c0, *bn_c1;
-  float *d1_h[2], *d1_c, *d2_hall, *d2_c;
-  float* pp;               // h0 ping-pong of the persistent LSTM kernel [2][256][max H0]
-  unsigned int* barrier;
-  LstmTcWs tc;             // tensor-core LSTM layers of the encoder / decoder (fsn_lstm_rec_tc.cu)
-  float* tc_mid;           // first layer's output for every step [B*Tp, max(He1, Hd)]
+  SeqStackWs seq;          // encoder and decoder LSTM pairs, one after the other
   size_t bytes;
 };
 
 static bool fast_is_tc(const fsn_fast_desc* d) { return d->precision == FSN_PREC_F16_TC || d->precision == FSN_PREC_F16X3_TC; }
-// encoder / decoder LSTM pairs on the tensor cores?
-static bool fast_lstm_tc(const fsn_fast_desc* d) {
-  const bool x3 = d->precision == FSN_PREC_F16X3_TC;
-  return fast_is_tc(d) && lstm_rec_tc_supported(d->enc1_hidden, x3) && lstm_rec_tc_supported(d->enc2_hidden, x3) &&
-         lstm_rec_tc_supported(d->dec_hidden, x3);
+
+// encoder / decoder pair: LSTM(K0 -> H0), LSTM(H0 -> H1) + Linear(O) over B rows of Tp steps; on the tensor cores with
+// the tensor-core precisions when all three encoder / decoder hidden sizes are supported there
+static SeqStack fast_pair(const fsn_fast_desc* d, const FastDims& m, int K0, int H0, int H1, int O, int act) {
+  SeqStack s;
+  memset(&s, 0, sizeof(s));
+  s.R = m.B; s.Tp = m.Tp; s.K0 = K0; s.n = 2; s.H[0] = H0; s.H[1] = H1; s.O = O; s.act = act;
+  s.x3 = fast_x3(d);
+  s.tc = fast_is_tc(d) && lstm_rec_tc_supported(d->enc1_hidden, s.x3) && lstm_rec_tc_supported(d->enc2_hidden, s.x3) &&
+         lstm_rec_tc_supported(d->dec_hidden, s.x3);
+  return s;
 }
 
 int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m) {
   FSN_REQUIRE(d && d->num_freqs > 1 && d->num_mels > 1 && d->shrink_size >= 1 && d->look_ahead >= 0, FSN_ERR_SHAPE,
               "fast model: bad descriptor");
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "fast model: empty input (B=%d, T=%d)", B, T);
+  FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "fast model: the GRU cell is not built");
   FSN_REQUIRE(d->bn_layers == 2, FSN_ERR_UNSUPPORTED, "fast model: bottleneck_num_layers must be 2 in this build");
   FSN_REQUIRE(d->noisy_num_neighbors < d->num_mels && d->enc_num_neighbors < d->num_mels, FSN_ERR_SHAPE,
               "fast model: reflect padding needs num_neighbors < num_mels");
@@ -135,80 +137,15 @@ static void fast_carve(const fsn_fast_desc* d, const FastDims& m, void* base, Fa
   w.inv2 = c.take<float>(m.B);
   w.fs = c.take<float2>(BT);
   w.sums = c.take<float2>(m.B);
-  for (int i = 0; i < 2; ++i) w.e1_h[i] = c.take<float>((size_t)m.B * d->enc1_hidden);
-  w.e1_c = c.take<float>((size_t)m.B * d->enc1_hidden);
-  w.e2_hall = c.take<float>(BT * d->enc2_hidden);
-  w.e2_c = c.take<float>((size_t)m.B * d->enc2_hidden);
   if (!fast_is_tc(d)) {
     for (int i = 0; i < 2; ++i) { w.bn_h0[i] = c.take<float>(R * d->bn_hidden); w.bn_h1[i] = c.take<float>(R * d->bn_hidden); }
     w.bn_c0 = c.take<float>(R * d->bn_hidden);
     w.bn_c1 = c.take<float>(R * d->bn_hidden);
   }
-  for (int i = 0; i < 2; ++i) w.d1_h[i] = c.take<float>((size_t)m.B * d->dec_hidden);
-  w.d1_c = c.take<float>((size_t)m.B * d->dec_hidden);
-  w.d2_hall = c.take<float>(BT * d->dec_hidden);
-  w.d2_c = c.take<float>((size_t)m.B * d->dec_hidden);
-  w.pp = c.take<float>((size_t)2 * 256 * (d->dec_hidden > d->enc1_hidden ? d->dec_hidden : d->enc1_hidden));
-  w.barrier = c.take<unsigned int>(64);
-  memset(&w.tc, 0, sizeof(w.tc));
-  w.tc_mid = nullptr;
-  if (fast_lstm_tc(d)) {
-    int Hm = d->enc1_hidden > d->enc2_hidden ? d->enc1_hidden : d->enc2_hidden;
-    if (d->dec_hidden > Hm) Hm = d->dec_hidden;
-    int Km = Hm > 2 * m.M ? Hm : 2 * m.M;
-    lstm_tc_carve(c, BT, Km, Hm, d->precision == FSN_PREC_F16X3_TC, w.tc);
-    w.tc_mid = c.take<float>(BT * (d->enc1_hidden > d->dec_hidden ? d->enc1_hidden : d->dec_hidden));
-  }
+  auto mx = [](int a, int b) { return a > b ? a : b; };
+  seq_stack_carve(c, fast_pair(d, m, 2 * m.M, mx(d->enc1_hidden, d->dec_hidden), mx(d->enc2_hidden, d->dec_hidden),
+                               mx(m.M, 2 * m.F), 0), w.seq);
   w.bytes = c.off;
-}
-
-// two chained single-layer LSTMs over the same rows: layer a (x -> Ha, state ping-pong) feeds layer b
-// (Ha -> Hb, output kept for every step for the Linear layer that follows)
-static int run_lstm_pair(const fsn_lstm_layer& la, int Ka, int Ha, const fsn_lstm_layer& lb, int Hb, int R, int steps,
-                         const float* x, size_t x_row_stride, size_t x_step_stride, const float* row_scale,
-                         float* ha[2], float* ca, float* hb_all, float* cb, float* pp, unsigned int* barrier,
-                         cudaStream_t st, const LstmTcWs* tc = nullptr, float* tc_mid = nullptr, bool x3 = false) {
-  int rc;
-  static const bool stepwise = getenv("FSN_FB_STEPWISE") != nullptr;
-  if (!stepwise && tc && tc_mid && x_step_stride == (size_t)Ka && x_row_stride == (size_t)steps * Ka) {
-    // tensor cores: per layer one hoisted input-projection GEMM + the persistent wgmma recurrence
-    if ((rc = lstm_layer_tc(la, x, (size_t)Ka, Ka, row_scale, steps, 0, R, steps, Ha, x3, *tc, tc_mid, st))) return rc;
-    return lstm_layer_tc(lb, tc_mid, (size_t)Ha, Ha, nullptr, 1, 0, R, steps, Hb, x3, *tc, hb_all, st);
-  }
-  if (!stepwise && x_step_stride == (size_t)Ka && x_row_stride == (size_t)steps * Ka && fb_persistent_supported(Ka, Ha, Hb)) {
-    // persistent cooperative wavefront kernel (fsn_fullband.cu), chunks of <= 256 rows
-    fsn_seq_weights w2;
-    memset(&w2, 0, sizeof(w2));
-    w2.w_ih[0] = la.w_ih; w2.w_hh[0] = la.w_hh; w2.b_ih[0] = la.b_ih; w2.b_hh[0] = la.b_hh;
-    w2.w_ih[1] = lb.w_ih; w2.w_hh[1] = lb.w_hh; w2.b_ih[1] = lb.b_ih; w2.b_hh[1] = lb.b_hh;
-    for (int r0 = 0; r0 < R; r0 += 256) {
-      const int nb = (R - r0 < 256) ? R - r0 : 256;
-      if ((rc = fb_persistent_launch(&w2, x + (size_t)r0 * x_row_stride, row_scale ? row_scale + r0 : nullptr, pp,
-                                     hb_all + (size_t)r0 * steps * Hb, barrier, nb, Ka, Ha, Hb, steps, st)))
-        return rc;
-    }
-    return FSN_OK;
-  }
-  for (int t = 0; t < steps; ++t) {
-    StepParams p;
-    memset(&p, 0, sizeof(p));
-    p.R = R; p.first = (t == 0);
-    p.K0 = Ka; p.H = Ha;
-    p.w_ih = la.w_ih; p.w_hh = la.w_hh; p.b_ih = la.b_ih; p.b_hh = la.b_hh;
-    p.h_prev = ha[(t + 1) & 1]; p.h_prev_stride = Ha;
-    p.h_out = ha[t & 1]; p.h_out_stride = Ha;
-    p.c = ca;
-    p.x0 = x + (size_t)t * x_step_stride; p.x0_row_stride = x_row_stride; p.row_scale = row_scale;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-    p.K0 = Ha; p.H = Hb;
-    p.w_ih = lb.w_ih; p.w_hh = lb.w_hh; p.b_ih = lb.b_ih; p.b_hh = lb.b_hh;
-    p.x0 = ha[t & 1]; p.x0_row_stride = Ha; p.row_scale = nullptr;
-    p.h_prev = hb_all + (size_t)(t > 0 ? t - 1 : 0) * Hb; p.h_prev_stride = (size_t)steps * Hb;
-    p.h_out = hb_all + (size_t)t * Hb; p.h_out_stride = (size_t)steps * Hb;
-    p.c = cb;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-  }
-  return FSN_OK;
 }
 
 }  // namespace fsn
@@ -247,8 +184,6 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
               workspace_bytes, w.bytes);
   cudaStream_t st = (cudaStream_t)stream;
   const int Tp = m.Tp, M = m.M, F = m.F, R = B * M;
-  const bool lstm_tc = fast_lstm_tc(d);
-  static const int tc_mask = getenv("FSN_FAST_TC_MASK") ? atoi(getenv("FSN_FAST_TC_MASK")) : 15;  // debug: 1 enc LSTMs, 2 enc fc, 4 dec LSTMs, 8 dec fc
   // look-ahead pad + time-major layout, Mel filtering (model.py:161-166)
   if ((rc = transpose_mag_launch(mix_mag, w.magT, B, F, T, Tp, st))) return rc;
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, B * Tp, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true)))
@@ -257,17 +192,10 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   if ((rc = clip_stats_launch(w.melT, B, Tp, M, 0, w.fs, w.sums, st))) return rc;
   if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) return rc;
   // F_l2m: LSTM(M->He1), LSTM(He1->He2) + Linear(M) + ReLU (model.py:35-54,171)
-  if ((rc = run_lstm_pair(wt->enc1, M, d->enc1_hidden, wt->enc2, d->enc2_hidden, B, Tp, w.melT, (size_t)Tp * M, M,
-                          w.inv1, w.e1_h, w.e1_c, w.e2_hall, w.e2_c, w.pp, w.barrier, st, (lstm_tc && (tc_mask & 1)) ? &w.tc : nullptr, w.tc_mid,
-                          fast_x3(d))))
-    return rc;
-  if (lstm_tc && (tc_mask & 2)) {
-    if ((rc = linear_tc(w.e2_hall, (size_t)d->enc2_hidden, d->enc2_hidden, wt->enc_fc_w, wt->enc_fc_b, M, FSN_ACT_RELU, w.encT,
-                        (size_t)M, (size_t)B * Tp, fast_x3(d), w.tc, st)))
-      return rc;
-  } else if ((rc = fc_gemm_launch(w.e2_hall, wt->enc_fc_w, wt->enc_fc_b, w.encT, B * Tp, d->enc2_hidden, M, FSN_ACT_RELU, st))) {
-    return rc;
-  }
+  SeqStack enc = fast_pair(d, m, M, d->enc1_hidden, d->enc2_hidden, M, FSN_ACT_RELU);
+  enc.L[0] = wt->enc1; enc.L[1] = wt->enc2;
+  enc.x = w.melT; enc.scale = w.inv1; enc.fc_w = wt->enc_fc_w; enc.fc_b = wt->enc_fc_b; enc.out = w.encT;
+  if ((rc = seq_stack_forward(enc, w.seq, st))) return rc;
   // bottleneck input: unfold + concat + real-time down-sampling, then its norm (model.py:174-187)
   fast_bn_input_kernel<<<B * m.Ts, 256, 0, st>>>(w.melT, w.encT, B, Tp, M, d->noisy_num_neighbors,
                                                  d->enc_num_neighbors, m.S, m.Ts, w.bn, w.fs);
@@ -292,28 +220,18 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
     if ((rc = sb_tc_forward(a, st))) return rc;
     bn_bstride = 2 * M;
   } else {
-  for (int t = 0; t < m.Ts; ++t) {
-    StepParams p;
-    memset(&p, 0, sizeof(p));
-    p.R = R; p.first = (t == 0);
-    p.K0 = m.K; p.H = Hb;
-    p.w_ih = wt->bn[0].w_ih; p.w_hh = wt->bn[0].w_hh; p.b_ih = wt->bn[0].b_ih; p.b_hh = wt->bn[0].b_hh;
-    p.h_prev = w.bn_h0[(t + 1) & 1]; p.h_prev_stride = Hb;
-    p.h_out = w.bn_h0[t & 1]; p.h_out_stride = Hb;
-    p.c = w.bn_c0;
-    p.x0 = w.bn + (size_t)t * R * m.K; p.x0_row_stride = m.K; p.row_scale = w.inv2; p.row_scale_div = M;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-    p.K0 = Hb;
-    p.w_ih = wt->bn[1].w_ih; p.w_hh = wt->bn[1].w_hh; p.b_ih = wt->bn[1].b_ih; p.b_hh = wt->bn[1].b_hh;
-    p.x0 = w.bn_h0[t & 1]; p.x0_row_stride = Hb; p.row_scale = nullptr; p.row_scale_div = 0;
-    p.h_prev = w.bn_h1[(t + 1) & 1]; p.h_prev_stride = Hb;
-    p.h_out = w.bn_h1[t & 1]; p.h_out_stride = Hb;
-    p.c = w.bn_c1;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-    if ((rc = rows_fc_launch(w.bn_h1[t & 1], R, Hb, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out + t,
-                             (size_t)m.Ts, 0, st)))
-      return rc;
-  }
+    const Step2State s2{{w.bn_h0[0], w.bn_h0[1]}, w.bn_c0, {w.bn_h1[0], w.bn_h1[1]}, w.bn_c1, Hb, 0};
+    for (int t = 0; t < m.Ts; ++t) {
+      StepParams p;
+      memset(&p, 0, sizeof(p));
+      p.R = R; p.K0 = m.K; p.H = Hb;
+      p.w_ih = wt->bn[0].w_ih; p.w_hh = wt->bn[0].w_hh; p.b_ih = wt->bn[0].b_ih; p.b_hh = wt->bn[0].b_hh;
+      p.x0 = w.bn + (size_t)t * R * m.K; p.x0_row_stride = m.K; p.row_scale = w.inv2; p.row_scale_div = M;
+      if ((rc = lstm_step2_launch(p, SEG0_DENSE, t, wt->bn[1], s2, st))) return rc;
+      if ((rc = rows_fc_launch(s2.h1_at(t), R, Hb, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out + t, (size_t)m.Ts, 0,
+                               st)))
+        return rc;
+    }
   }
   // up-sampling + concat with the encoder output (model.py:191-194)
   {
@@ -324,18 +242,10 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
     FSN_CHECK_LAUNCH("fast_dec_input_kernel");
   }
   // F_m2l: LSTM(2M->Hd), LSTM(Hd->Hd) + Linear(2F) (model.py:77-96,196)
-  if ((rc = run_lstm_pair(wt->dec1, 2 * M, d->dec_hidden, wt->dec2, d->dec_hidden, B, Tp, w.dec_in, (size_t)Tp * 2 * M,
-                          2 * M, nullptr, w.d1_h, w.d1_c, w.d2_hall, w.d2_c, w.pp, w.barrier, st, (lstm_tc && (tc_mask & 4)) ? &w.tc : nullptr,
-                          w.tc_mid, fast_x3(d))))
-    return rc;
-  if (lstm_tc && (tc_mask & 8)) {
-    if ((rc = linear_tc(w.d2_hall, (size_t)d->dec_hidden, d->dec_hidden, wt->dec_fc_w, wt->dec_fc_b, 2 * F, FSN_ACT_NONE,
-                        w.dec_out, (size_t)2 * F, (size_t)B * Tp, fast_x3(d), w.tc, st)))
-      return rc;
-  } else if ((rc = fc_gemm_launch(w.d2_hall, wt->dec_fc_w, wt->dec_fc_b, w.dec_out, B * Tp, d->dec_hidden, 2 * F, FSN_ACT_NONE,
-                                  st))) {
-    return rc;
-  }
+  SeqStack dec = fast_pair(d, m, 2 * M, d->dec_hidden, d->dec_hidden, 2 * F, FSN_ACT_NONE);
+  dec.L[0] = wt->dec1; dec.L[1] = wt->dec2;
+  dec.x = w.dec_in; dec.fc_w = wt->dec_fc_w; dec.fc_b = wt->dec_fc_b; dec.out = w.dec_out;
+  if ((rc = seq_stack_forward(dec, w.seq, st))) return rc;
   dim3 grid(cdiv(T, 32), cdiv(F, 32), B * 2);
   fast_output_kernel<<<grid, dim3(32, 8), 0, st>>>(w.dec_out, B, Tp, F, d->look_ahead, out);
   FSN_CHECK_LAUNCH("fast_output_kernel");

@@ -14,7 +14,12 @@
 //
 // Thread mapping (512 threads): row = tid/2 (clip), half = tid%2 -> gate columns [8*half, 8*half+8)
 // of the CTA's 16 (= 2 complete hidden units), for both layers: 32 accumulators per thread.
+//
+// Below the kernel: seq_stack_forward, the SequenceModel every inference forward runs its clip-major LSTM stacks through
+// (this kernel, the per-step kernels or the tensor-core layers of fsn_lstm_rec_tc.cu).
 #include <cooperative_groups.h>
+#include <stdlib.h>
+#include <string.h>
 #include <type_traits>
 
 #include "fsn_internal.cuh"
@@ -264,15 +269,13 @@ bool fb_persistent_supported(int F, int H0, int H1) {
   return coop == 1 && fb_persistent_smem(F, H0, H1) <= (size_t)max_smem && cdiv(Hm, fb::MAX_UPC) <= sms;
 }
 
-// One persistent launch of a 2-layer LSTM wavefront (layer 0: F -> H0 with optional per-row input scale `inv1`,
-// layer 1: H0 -> H1) for rows [0, nb), nb <= 256; h0buf [2][nb][H0] scratch, h1all [nb][Tp][H1] output.
-int fb_persistent_launch(const fsn_seq_weights* w, const float* x_chunk, const float* inv1_chunk, float* h0buf,
-                         float* h1all_chunk, unsigned int* barrier, int nb, int F, int H0, int H1, int Tp,
-                         cudaStream_t st) {
+// The 2-layer LSTM wavefront, one persistent launch per chunk of <= 256 rows (fb::ROWS).
+int fb_persistent_launch(const fsn_lstm_layer* L, const float* x, const float* inv1, float* h0buf, float* h1all,
+                         unsigned int* barrier, int R, int F, int H0, int H1, int Tp, cudaStream_t st) {
   fb::Args a;
-  for (int l = 0; l < 2; ++l) { a.w_ih[l] = w->w_ih[l]; a.w_hh[l] = w->w_hh[l]; a.b_ih[l] = w->b_ih[l]; a.b_hh[l] = w->b_hh[l]; }
-  a.x = x_chunk; a.inv1 = inv1_chunk; a.h0buf = h0buf; a.h1all = h1all_chunk; a.barrier = barrier;
-  a.B = nb; a.F = F; a.H0 = H0; a.H1 = H1; a.Tp = Tp;
+  for (int l = 0; l < 2; ++l) { a.w_ih[l] = L[l].w_ih; a.w_hh[l] = L[l].w_hh; a.b_ih[l] = L[l].b_ih; a.b_hh[l] = L[l].b_hh; }
+  a.h0buf = h0buf; a.barrier = barrier;
+  a.F = F; a.H0 = H0; a.H1 = H1; a.Tp = Tp;
   int sms = 132;
   { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
   const int Hm = H0 > H1 ? H0 : H1;
@@ -284,14 +287,95 @@ int fb_persistent_launch(const fsn_seq_weights* w, const float* x_chunk, const f
   int rc = check_cuda(cudaFuncSetAttribute(fb::fb_lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
                       "fb_lstm smem attr");
   if (rc) return rc;
-  rc = check_cuda(cudaMemsetAsync(barrier, 0, sizeof(unsigned int), st), "fb barrier memset");
-  if (rc) return rc;
-  void* params[] = {(void*)&a};
-  rc = check_cuda(cudaLaunchCooperativeKernel((const void*)fb::fb_lstm_kernel, dim3(a.G), dim3(fb::THREADS), params,
-                                              smem, st), "fb_lstm cooperative launch");
-  if (rc) return rc;
-  FSN_CHECK_LAUNCH("fb_lstm_kernel");
+  for (int r0 = 0; r0 < R; r0 += fb::ROWS) {
+    a.B = (R - r0 < fb::ROWS) ? R - r0 : fb::ROWS;
+    a.x = x + (size_t)r0 * Tp * F; a.inv1 = inv1 ? inv1 + r0 : nullptr; a.h1all = h1all + (size_t)r0 * Tp * H1;
+    rc = check_cuda(cudaMemsetAsync(barrier, 0, sizeof(unsigned int), st), "fb barrier memset");
+    if (rc) return rc;
+    void* params[] = {(void*)&a};
+    rc = check_cuda(cudaLaunchCooperativeKernel((const void*)fb::fb_lstm_kernel, dim3(a.G), dim3(fb::THREADS), params,
+                                                smem, st), "fb_lstm cooperative launch");
+    if (rc) return rc;
+    FSN_CHECK_LAUNCH("fb_lstm_kernel");
+  }
   return FSN_OK;
+}
+
+void seq_stack_carve(Carver& c, const SeqStack& s, SeqStackWs& w) {
+  int Hm = 0;
+  for (int l = 0; l < s.n; ++l) Hm = s.H[l] > Hm ? s.H[l] : Hm;
+  const size_t rows = (size_t)s.R * s.Tp;
+  w.hall[0] = c.take<float>(rows * Hm);
+  w.hall[1] = (s.n > 2 || s.tc) ? c.take<float>(rows * Hm) : nullptr;
+  w.h0[0] = w.h0[1] = w.c1 = w.pp = nullptr;
+  w.barrier = nullptr;
+  if (s.n >= 2) {
+    w.h0[0] = c.take<float>((size_t)s.R * s.H[0]);
+    w.h0[1] = c.take<float>((size_t)s.R * s.H[0]);
+    w.c1 = c.take<float>((size_t)s.R * s.H[1]);
+  }
+  w.c0 = c.take<float>((size_t)s.R * Hm);  // layer 0's cell, then that of every layer past the first two
+  if (s.n >= 2 && !s.gru && !s.step_scale) {
+    w.pp = c.take<float>((size_t)2 * fb::ROWS * s.H[0]);
+    w.barrier = c.take<unsigned int>(64);
+  }
+  memset(&w.tc, 0, sizeof(w.tc));
+  if (s.tc) {
+    const int Hw = Hm > cdiv(s.O, 4) ? Hm : cdiv(s.O, 4);  // the prepared weights of the Linear share the [4 Hmax] rows
+    lstm_tc_carve(c, rows, s.K0 > Hm ? s.K0 : Hm, Hw, s.x3, w.tc);
+  }
+}
+
+int seq_stack_forward(const SeqStack& s, const SeqStackWs& w, cudaStream_t st) {
+  static const bool stepwise = getenv("FSN_FB_STEPWISE") != nullptr;  // debug: force the per-step kernels
+  const int R = s.R, Tp = s.Tp, n = s.n, Ht = s.H[n - 1];
+  auto hall = [&](int l) { return w.hall[(n - 1 - l) & 1]; };  // output of layer l, [R, Tp, H[l]]; the top one in hall[0]
+  int rc;
+  if (s.tc && !stepwise) {
+    // per layer one hoisted input-projection GEMM + the persistent wgmma recurrence; the Linear on the same GEMM
+    for (int l = 0; l < n; ++l) {
+      const int K = l ? s.H[l - 1] : s.K0;
+      const float* x = l ? hall(l - 1) : s.x;
+      if ((rc = lstm_layer_tc(s.L[l], x, (size_t)K, K, l ? nullptr : s.scale, Tp, (!l && s.step_scale) ? R : 0, R, Tp,
+                              s.H[l], s.x3, w.tc, hall(l), st)))
+        return rc;
+    }
+    return linear_tc(hall(n - 1), (size_t)Ht, Ht, s.fc_w, s.fc_b, s.O, s.act, s.out, (size_t)s.O, (size_t)R * Tp, s.x3, w.tc,
+                     st);
+  }
+  // one per-step kernel launch of layer l at step t: input x (layer 0) or layer l-1's output, h / c state set by the caller
+  auto step = [&](int l, int t) {
+    StepParams p;
+    memset(&p, 0, sizeof(p));
+    p.R = R; p.H = s.H[l]; p.first = (t == 0); p.gru = s.gru;
+    p.w_ih = s.L[l].w_ih; p.w_hh = s.L[l].w_hh; p.b_ih = s.L[l].b_ih; p.b_hh = s.L[l].b_hh;
+    p.K0 = l ? s.H[l - 1] : s.K0;
+    p.x0 = (l ? hall(l - 1) : s.x) + (size_t)t * p.K0; p.x0_row_stride = (size_t)Tp * p.K0;
+    if (!l) p.row_scale = (s.scale && s.step_scale) ? s.scale + (size_t)t * R : s.scale;
+    return p;
+  };
+  int l = 0;  // first layer left for the single-layer loop
+  if (!stepwise && n >= 2 && !s.gru && !s.step_scale && fb_persistent_supported(s.K0, s.H[0], s.H[1])) {
+    // weights resident in shared memory, layer wavefront, one grid barrier per time step
+    if ((rc = fb_persistent_launch(s.L, s.x, s.scale, w.pp, hall(1), w.barrier, R, s.K0, s.H[0], s.H[1], Tp, st))) return rc;
+    l = 2;
+  } else if (n >= 2) {
+    const Step2State s2{{w.h0[0], w.h0[1]}, w.c0, {hall(1), nullptr}, w.c1, s.H[1], Tp};
+    for (int t = 0; t < Tp; ++t)
+      if ((rc = lstm_step2_launch(step(0, t), SEG0_DENSE, t, s.L[1], s2, st))) return rc;
+    l = 2;
+  }
+  for (; l < n; ++l) {
+    const size_t ld = (size_t)Tp * s.H[l];
+    for (int t = 0; t < Tp; ++t) {
+      StepParams p = step(l, t);
+      p.h_prev = hall(l) + (size_t)(t > 0 ? t - 1 : 0) * s.H[l]; p.h_prev_stride = ld;
+      p.h_out = hall(l) + (size_t)t * s.H[l]; p.h_out_stride = ld;
+      p.c = w.c0;
+      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+    }
+  }
+  return fc_gemm_launch(hall(n - 1), s.fc_w, s.fc_b, s.out, R * Tp, Ht, s.O, s.act, st);
 }
 
 }  // namespace fsn

@@ -97,16 +97,22 @@ struct ImpDims { int B, L, T, F, Fu, S; SecGeom sec[FSN_IMP_MAX_SECTIONS]; int m
 struct ImpWs {
   float *mag, *real, *imag, *crm, *magc, *fbT, *X, *inv1, *invs;
   float2 *fs, *sums;
-  float *fb_pp, *fb_h1all;
-  unsigned int* barrier;
+  SeqStackWs fb;
   float *h0[2], *h1[2], *c0, *c1;
-  float *fbs_h0[2], *fbs_c0, *fbs_c1;  // per-step full-band fallback
   LayerSave tc;                        // FSN_PREC_TF32_TC: gates / cell / hidden of every step of one layer
   float *tc_h1, *tc_rec;
-  LstmTcWs fbtc;                       // FSN_PREC_TF32_TC: full band on the hoisted-GEMM + persistent-recurrence kernels
-  float* fbtc_mid;
   size_t bytes;
 };
+
+// full band (model.py:567): 2 x LSTM(Fu -> Hf -> Hf) + Linear(Hf -> Fu), rows = clips; FSN_PREC_TF32_TC runs it on the
+// single-pass tensor-core layers
+static SeqStack imp_fb_stack(const fsn_improved_desc* d, const ImpDims& m) {
+  SeqStack s;
+  memset(&s, 0, sizeof(s));
+  s.R = m.B; s.Tp = m.T; s.K0 = m.Fu; s.n = 2; s.H[0] = s.H[1] = d->fb_hidden; s.O = m.Fu; s.act = d->fb_activation;
+  s.tc = d->precision == FSN_PREC_TF32_TC && lstm_rec_tc_supported(d->fb_hidden, false);
+  return s;
+}
 
 static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 
@@ -148,15 +154,10 @@ static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, 
   w.X = c.take<float>(BT * m.maxRW);
   w.inv1 = c.take<float>(m.B); w.invs = c.take<float>(m.B);
   w.fs = c.take<float2>(BT); w.sums = c.take<float2>(m.B);
-  w.fb_pp = c.take<float>((size_t)2 * 256 * d->fb_hidden);
-  w.fb_h1all = c.take<float>(BT * d->fb_hidden);
-  w.barrier = c.take<unsigned int>(64);
+  seq_stack_carve(c, imp_fb_stack(d, m), w.fb);
   const size_t RH = (size_t)m.B * m.maxR * d->sb_hidden;
   for (int i = 0; i < 2; ++i) { w.h0[i] = c.take<float>(RH); w.h1[i] = c.take<float>(RH); }
   w.c0 = c.take<float>(RH); w.c1 = c.take<float>(RH);
-  const size_t BH = (size_t)m.B * d->fb_hidden;
-  w.fbs_h0[0] = c.take<float>(BH); w.fbs_h0[1] = c.take<float>(BH);
-  w.fbs_c0 = c.take<float>(BH); w.fbs_c1 = c.take<float>(BH);
   w.tc.G = w.tc.C = w.tc.H = w.tc_h1 = w.tc_rec = nullptr;
   if (d->precision == FSN_PREC_TF32_TC) {
     const size_t TR = (size_t)m.T * m.B * m.maxR;
@@ -165,12 +166,6 @@ static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, 
     w.tc.H = c.take<float>(TR * d->sb_hidden);
     w.tc_h1 = c.take<float>(TR * d->sb_hidden);
     w.tc_rec = c.take<float>(4 * RH);
-  }
-  memset(&w.fbtc, 0, sizeof(w.fbtc));
-  w.fbtc_mid = nullptr;
-  if (d->precision == FSN_PREC_TF32_TC && lstm_rec_tc_supported(d->fb_hidden, false)) {
-    lstm_tc_carve(c, BT, m.Fu > d->fb_hidden ? m.Fu : d->fb_hidden, d->fb_hidden, false, w.fbtc);
-    w.fbtc_mid = c.take<float>(BT * d->fb_hidden);
   }
   w.bytes = c.off;
 }
@@ -199,7 +194,7 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, w.bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  const int T = m.T, F = m.F, Fu = m.Fu, Hf = d->fb_hidden, Hs = d->sb_hidden;
+  const int T = m.T, F = m.F, Fu = m.Fu, Hs = d->sb_hidden;
   const float eps = 1.1920928955078125e-07f;  // np.finfo(np.float32).eps (model.py:23,148)
   float* crm = crm_out ? crm_out : w.crm;
   // STFT (model.py:550-557), |X|^fdrc without the Nyquist bin (564-565)
@@ -213,45 +208,10 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
   // full band: norm (566) -> 2xLSTM + Linear (567)
   if ((rc = clip_stats_launch(w.magc, B, T, Fu, 0, w.fs, w.sums, st))) return rc;
   if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)Fu * T, 1.f, w.inv1, nullptr, st, eps))) return rc;
-  const bool fb_tc = w.fbtc_mid != nullptr;
-  if (fb_tc) {
-    // tensor cores: per layer one hoisted input-projection GEMM (tf32) + the persistent wgmma recurrence, Linear likewise
-    if ((rc = lstm_layer_tc(seq_layer(wt->fb, 0), w.magc, (size_t)Fu, Fu, w.inv1, T, 0, B, T, Hf, false, w.fbtc, w.fbtc_mid, st))) return rc;
-    if ((rc = lstm_layer_tc(seq_layer(wt->fb, 1), w.fbtc_mid, (size_t)Hf, Hf, nullptr, 1, 0, B, T, Hf, false, w.fbtc, w.fb_h1all, st))) return rc;
-    if ((rc = linear_tc(w.fb_h1all, (size_t)Hf, Hf, wt->fb.fc_w, wt->fb.fc_b, Fu, d->fb_activation, w.fbT, (size_t)Fu,
-                        (size_t)B * T, false, w.fbtc, st)))
-      return rc;
-  } else if (fb_persistent_supported(Fu, Hf, Hf)) {
-    for (int b0 = 0; b0 < B; b0 += 256) {
-      const int nb = (B - b0 < 256) ? B - b0 : 256;
-      if ((rc = fb_persistent_launch(&wt->fb, w.magc + (size_t)b0 * T * Fu, w.inv1 + b0, w.fb_pp,
-                                     w.fb_h1all + (size_t)b0 * T * Hf, w.barrier, nb, Fu, Hf, Hf, T, st)))
-        return rc;
-    }
-  } else {
-    // weights of a (Fu + 3 Hf) x 16 slice exceed one SM's shared memory (n_fft = 1024): per-step kernels
-    for (int t = 0; t < T; ++t) {
-      StepParams p;
-      memset(&p, 0, sizeof(p));
-      p.R = B; p.H = Hf; p.first = (t == 0);
-      p.K0 = Fu;
-      p.w_ih = wt->fb.w_ih[0]; p.w_hh = wt->fb.w_hh[0]; p.b_ih = wt->fb.b_ih[0]; p.b_hh = wt->fb.b_hh[0];
-      p.h_prev = w.fbs_h0[(t + 1) & 1]; p.h_prev_stride = Hf;
-      p.h_out = w.fbs_h0[t & 1]; p.h_out_stride = Hf;
-      p.c = w.fbs_c0;
-      p.x0 = w.magc + (size_t)t * Fu; p.x0_row_stride = (size_t)T * Fu; p.row_scale = w.inv1;
-      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-      p.K0 = Hf;
-      p.w_ih = wt->fb.w_ih[1]; p.w_hh = wt->fb.w_hh[1]; p.b_ih = wt->fb.b_ih[1]; p.b_hh = wt->fb.b_hh[1];
-      p.x0 = w.fbs_h0[t & 1]; p.x0_row_stride = Hf; p.row_scale = nullptr;
-      p.h_prev = w.fb_h1all + (size_t)(t > 0 ? t - 1 : 0) * Hf; p.h_prev_stride = (size_t)T * Hf;
-      p.h_out = w.fb_h1all + (size_t)t * Hf; p.h_out_stride = (size_t)T * Hf;
-      p.c = w.fbs_c1;
-      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-    }
-  }
-  if (!fb_tc && (rc = fc_gemm_launch(w.fb_h1all, wt->fb.fc_w, wt->fb.fc_b, w.fbT, B * T, Hf, Fu, d->fb_activation, st)))
-    return rc;
+  SeqStack s = imp_fb_stack(d, m);
+  s.L[0] = seq_layer(wt->fb, 0); s.L[1] = seq_layer(wt->fb, 1);
+  s.x = w.magc; s.scale = w.inv1; s.fc_w = wt->fb.fc_w; s.fc_b = wt->fb.fc_b; s.out = w.fbT;
+  if ((rc = seq_stack_forward(s, w.fb, st))) return rc;
   // cRM, Nyquist row = 0 (572)
   if ((rc = check_cuda(cudaMemsetAsync(crm, 0, (size_t)2 * B * F * T * sizeof(float), st), "crm memset"))) return rc;
   // sub-band sections (408-447)
@@ -283,26 +243,16 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
       }
       continue;
     }
+    const Step2State s2{{w.h0[0], w.h0[1]}, w.c0, {w.h1[0], w.h1[1]}, w.c1, Hs, 0};
     for (int t = 0; t < T; ++t) {
       StepParams p;
       memset(&p, 0, sizeof(p));
-      p.R = R; p.first = (t == 0);
-      p.K0 = g.W; p.H = Hs;
+      p.R = R; p.K0 = g.W; p.H = Hs;
       p.w_ih = sw.w_ih[0]; p.w_hh = sw.w_hh[0]; p.b_ih = sw.b_ih[0]; p.b_hh = sw.b_hh[0];
-      p.h_prev = w.h0[(t + 1) & 1]; p.h_prev_stride = Hs;
-      p.h_out = w.h0[t & 1]; p.h_out_stride = Hs;
-      p.c = w.c0;
       p.x0 = w.X + (size_t)t * R * g.W; p.x0_row_stride = g.W; p.row_scale = w.invs; p.row_scale_div = g.N;
-      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-      p.K0 = Hs;
-      p.w_ih = sw.w_ih[1]; p.w_hh = sw.w_hh[1]; p.b_ih = sw.b_ih[1]; p.b_hh = sw.b_hh[1];
-      p.x0 = w.h0[t & 1]; p.x0_row_stride = Hs; p.row_scale = nullptr; p.row_scale_div = 0;
-      p.h_prev = w.h1[(t + 1) & 1]; p.h_prev_stride = Hs;
-      p.h_out = w.h1[t & 1]; p.h_out_stride = Hs;
-      p.c = w.c1;
-      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+      if ((rc = lstm_step2_launch(p, SEG0_DENSE, t, seq_layer(sw, 1), s2, st))) return rc;
       const size_t warps = (size_t)R * 2 * g.cs;
-      imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(w.h1[t & 1], R, Hs, sw.fc_w, sw.fc_b, g.cs, g.N, g.lo,
+      imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(s2.h1_at(t), R, Hs, sw.fc_w, sw.fc_b, g.cs, g.N, g.lo,
                                                                   d->sb_activation, crm, F, T, t);
       FSN_CHECK_LAUNCH("imp_fc_step_kernel");
     }

@@ -65,6 +65,18 @@ struct StepParams {
 };
 
 int lstm_step_launch(const StepParams& p, int mode, cudaStream_t st);
+// per-step state of a two-layer stack: layer 0's h ping-pong h0[2] [R,H0] and cell c0; layer 1's cell c1 and its h, either
+// a ping-pong h1[2] [R,H1] (keep_steps = 0) or one [R, keep_steps, H1] tensor h1[0] that keeps every step
+struct Step2State {
+  float *h0[2], *c0, *h1[2], *c1;
+  int H1, keep_steps;
+  float* h1_at(int t) const { return keep_steps ? h1[0] + (size_t)(t > 0 ? t : 0) * H1 : h1[t & 1]; }
+  size_t h1_stride() const { return (size_t)(keep_steps ? keep_steps : 1) * H1; }
+};
+// step t of a two-layer stack on the per-step kernels.  p: layer 0 of step t with R, H, gru, its weights and its input
+// (K0 and the SEG0_DENSE / SEG0_GATHER fields of `mode`) filled in; the helper sets the step and state fields, then runs
+// layer 1 (weights w1) on layer 0's h_t.  Layer 1's h_t is then at s.h1_at(t).
+int lstm_step2_launch(StepParams p, int mode, int t, const fsn_lstm_layer& w1, const Step2State& s, cudaStream_t st);
 // cumulative_laplace_norm (base_model.py:220-251): scale1T[t*B+b] from the frame sums fs[b*Tp+t].x, and
 // scaleT[t*R+r] of every sub-band unit (running mean over its K rows and the frames so far)
 int cum_clip_scale_launch(const float2* fs, int B, int Tp, int F, float eps, float* scale1T, cudaStream_t st);
@@ -228,11 +240,11 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
 // it into the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:181-182)
 int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st);
 
-// persistent cooperative full-band LSTM (fsn_fullband.cu)
+// persistent cooperative full-band LSTM (fsn_fullband.cu): layers L[0] (F -> H0, input x [R,Tp,F] times inv1[r] when
+// given) and L[1] (H0 -> H1) of R rows into h1all [R,Tp,H1]; h0buf [2][256][H0] scratch
 bool fb_persistent_supported(int F, int H0, int H1);
-int fb_persistent_launch(const fsn_seq_weights* w, const float* x_chunk, const float* inv1_chunk, float* h0buf,
-                         float* h1all_chunk, unsigned int* barrier, int nb, int F, int H0, int H1, int Tp,
-                         cudaStream_t st);
+int fb_persistent_launch(const fsn_lstm_layer* L, const float* x, const float* inv1, float* h0buf, float* h1all,
+                         unsigned int* barrier, int R, int F, int H0, int H1, int Tp, cudaStream_t st);
 
 // tensor-core LSTM layer for a small batch of sequences (fsn_lstm_rec_tc.cu): hoisted input projection on the tf32
 // GEMM (x3: three passes on tf32 hi/lo splits) + persistent cooperative wgmma recurrence (x3: fp16 hi/lo splits)
@@ -255,6 +267,31 @@ int linear_tc(const float* x, size_t ldx, int K, const float* W, const float* bi
               size_t rows, bool x3, const LstmTcWs& ws, cudaStream_t st);
 int gemm_tc_split_launch(const float* a, size_t lda, const float* W, int N, int K, float* w, float* C, size_t ldc, size_t M,
                          bool x3, cudaStream_t st);
+
+// One SequenceModel of the inference forwards over clip-major rows (sequence_model.py:106-125, fsn_fullband.cu): n LSTM
+// (or GRU) layers over x [R, Tp, K0] (contiguous; times scale[r], or scale[t*R + r] with step_scale), then Linear(H[n-1]
+// -> O) + act into out [R*Tp, O].  tc / x3 are the caller's rule for running the stack on the tensor cores
+// (lstm_layer_tc + linear_tc, x3: hi+lo compensated).  Otherwise, or under FSN_FB_STEPWISE, layers 0-1 run on the
+// persistent kernel when it fits (LSTM, no per-step scale), everything else on the per-step kernels, then fc_gemm.
+static const int SEQ_MAX_LAYERS = 8;
+struct SeqStack {
+  int R, Tp, K0, n, O, act;
+  int H[SEQ_MAX_LAYERS];
+  fsn_lstm_layer L[SEQ_MAX_LAYERS];
+  bool gru, step_scale, tc, x3;
+  const float *x, *scale, *fc_w, *fc_b;
+  float* out;
+};
+// layer outputs for every step (hall[0]: top layer), per-step state, persistent-kernel scratch, tensor-core workspace
+struct SeqStackWs {
+  float *hall[2], *h0[2], *c0, *c1, *pp;
+  unsigned int* barrier;
+  LstmTcWs tc;
+};
+// sizes the state of every path the stack's shape, cell, scale and tc flag allow (only those fields are read); a stack
+// no larger in any of K0, H[l], O (same R, Tp, n, flags) runs on the same workspace
+void seq_stack_carve(Carver& c, const SeqStack& s, SeqStackWs& w);
+int seq_stack_forward(const SeqStack& s, const SeqStackWs& w, cudaStream_t st);
 
 // tensor-core sub-band stack (fsn_subband_tc.cu)
 struct SbTcArgs {

@@ -262,6 +262,22 @@ int lstm_step_launch(const StepParams& p, int mode, cudaStream_t st) {
   return FSN_OK;
 }
 
+int lstm_step2_launch(StepParams p, int mode, int t, const fsn_lstm_layer& w1, const Step2State& s, cudaStream_t st) {
+  const int H0 = p.H;
+  p.first = (t == 0);
+  p.h_prev = s.h0[(t + 1) & 1]; p.h_prev_stride = H0;
+  p.h_out = s.h0[t & 1]; p.h_out_stride = H0;
+  p.c = s.c0;
+  int rc = lstm_step_launch(p, mode, st);
+  if (rc) return rc;
+  p.K0 = H0; p.H = s.H1;
+  p.w_ih = w1.w_ih; p.w_hh = w1.w_hh; p.b_ih = w1.b_ih; p.b_hh = w1.b_hh;
+  p.x0 = s.h0[t & 1]; p.x0_row_stride = H0; p.row_scale = nullptr; p.row_scale_div = 0;
+  p.h_prev = s.h1_at(t - 1); p.h_out = s.h1_at(t); p.h_prev_stride = p.h_out_stride = s.h1_stride();
+  p.c = s.c1;
+  return lstm_step_launch(p, SEG0_DENSE, st);
+}
+
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float apply_act(float v, int act) {
   switch (act) {

@@ -3,7 +3,6 @@
 //
 // Reference: recipes/dns_interspeech_2020/fullsubnet/model.py:72-136 (Model.forward),
 //            recipes/dns_interspeech_2020/inferencer.py:130-145 (full_band_crm_mask).
-#include <stdlib.h>
 #include <string.h>
 
 #include "fsn_internal.cuh"
@@ -39,24 +38,24 @@ static void prof_reset() { for (int i = 0; i < 5; ++i) g_ev_valid[i] = false; }
 struct ModelWs {
   float *magT, *fbT, *inv1, *inv2;
   float2 *fs, *sums_mag, *sums_fb;
-  float *fb_h0[2], *fb_c0, *fb_c1, *fb_h1all, *fb_pp;
   float *cum1, *cum2;  // cumulative norm: per-(step, clip) and per-(step, unit) scales
-  unsigned int* fb_barrier;
+  SeqStackWs fb;
   float *sb_h0[2], *sb_h1[2], *sb_c0, *sb_c1;
-  // tensor-core full-band path (fb_tc_forward): split operands, hoisted projection, layer-0 output, scratch
-  LstmTcWs tc;
-  float* tc_h0all;
   size_t bytes;
 };
 
-// full-band stack on the tensor cores?  (tensor-core precisions, offline norm, enough clips to fill an MMA tile)
-static bool fb_tc_enabled(const fsn_model_desc* d, int B) {
-  // every batch size takes the same path, so a clip's result does not depend on the batch it is enhanced in
-  static const int min_b = getenv("FSN_FB_TC_MIN_B") ? atoi(getenv("FSN_FB_TC_MIN_B")) : 1;
-  if (d->precision != FSN_PREC_F16_TC && d->precision != FSN_PREC_F16X3_TC) return false;
-  if (d->cell_type != FSN_CELL_LSTM) return false;
-  if (B < min_b) return false;
-  return lstm_rec_tc_supported(d->fb_hidden, d->precision == FSN_PREC_F16X3_TC);
+// full-band stack (model.py:92-95): 2-layer LSTM / GRU (F -> Hf -> Hf) + Linear(Hf -> F), rows = clips.  On the tensor
+// cores with the tensor-core precisions and LSTM, for every batch size, so a clip's result does not depend on the batch
+// it is enhanced in.
+static SeqStack fb_stack(const fsn_model_desc* d, const Dims& m) {
+  SeqStack s;
+  memset(&s, 0, sizeof(s));
+  s.R = m.B; s.Tp = m.Tp; s.K0 = m.F; s.n = 2; s.H[0] = s.H[1] = d->fb_hidden; s.O = m.F; s.act = d->fb_activation;
+  s.gru = d->cell_type == FSN_CELL_GRU;
+  s.step_scale = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
+  s.x3 = d->precision == FSN_PREC_F16X3_TC;
+  s.tc = (s.x3 || d->precision == FSN_PREC_F16_TC) && !s.gru && lstm_rec_tc_supported(d->fb_hidden, s.x3);
+  return s;
 }
 
 int make_dims(const fsn_model_desc* d, int B, int T, Dims& m) {
@@ -93,27 +92,12 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
   w.sums_fb = c.take<float2>(m.B);
   w.inv1 = c.take<float>(m.B);
   w.inv2 = c.take<float>(m.B);
-  const size_t BH = (size_t)m.B * d->fb_hidden;
-  w.fb_h0[0] = c.take<float>(BH);
-  w.fb_h0[1] = c.take<float>(BH);
-  w.fb_c0 = c.take<float>(BH);
-  w.fb_c1 = c.take<float>(BH);
-  w.fb_h1all = c.take<float>(BH * m.Tp);
-  w.fb_pp = c.take<float>((size_t)2 * 256 * d->fb_hidden);  // h0 ping-pong of the persistent kernel
-  w.fb_barrier = c.take<unsigned int>(64);
+  seq_stack_carve(c, fb_stack(d, m), w.fb);
   if (d->precision == FSN_PREC_FP32) {
     const size_t RH = (size_t)m.R * d->sb_hidden;
     for (int i = 0; i < 2; ++i) { w.sb_h0[i] = c.take<float>(RH); w.sb_h1[i] = c.take<float>(RH); }
     w.sb_c0 = c.take<float>(RH);
     w.sb_c1 = c.take<float>(RH);
-  }
-  memset(&w.tc, 0, sizeof(w.tc));
-  w.tc_h0all = nullptr;
-  if (fb_tc_enabled(d, m.B)) {
-    const int Hf = d->fb_hidden;
-    const size_t rows = (size_t)m.B * m.Tp;
-    lstm_tc_carve(c, rows, m.F > Hf ? m.F : Hf, Hf, d->precision == FSN_PREC_F16X3_TC, w.tc);
-    w.tc_h0all = c.take<float>(rows * Hf);
   }
   w.cum1 = w.cum2 = nullptr;
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
@@ -123,30 +107,11 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
   w.bytes = c.off;
 }
 
-// Full-band stack on the tensor cores (model.py:92-95; sequence_model.py:106-125): per layer the input projection of
-// all steps as one tf32 GEMM (three passes on hi/lo splits when x3) and the recurrence in the persistent wgmma
-// kernel; Linear(Hf -> F) + activation as the same GEMM + a bias/activation pass.  x3 keeps the fp32 error class.
-static int fb_tc_forward(const fsn_model_desc* d, const fsn_seq_weights* fb, const Dims& m, const ModelWs& w, cudaStream_t st) {
-  const int F = m.F, Tp = m.Tp, B = m.B, Hf = d->fb_hidden;
-  const bool x3 = d->precision == FSN_PREC_F16X3_TC;
-  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
-  int rc;
-  fsn_lstm_layer L0{fb->w_ih[0], fb->w_hh[0], fb->b_ih[0], fb->b_hh[0]}, L1{fb->w_ih[1], fb->w_hh[1], fb->b_ih[1], fb->b_hh[1]};
-  // layer 0: x = magT * 1/(mu + 1e-5) of the clip (model.py:92); cumulative norm: the scale of (clip, step) from the
-  // time-major table cum1[t*B + b] (base_model.py:220-251)
-  if ((rc = lstm_layer_tc(L0, w.magT, (size_t)F, F, cum ? w.cum1 : w.inv1, Tp, cum ? B : 0, B, Tp, Hf, x3, w.tc, w.tc_h0all, st)))
-    return rc;
-  if ((rc = lstm_layer_tc(L1, w.tc_h0all, (size_t)Hf, Hf, nullptr, 1, 0, B, Tp, Hf, x3, w.tc, w.fb_h1all, st))) return rc;
-  // Linear(Hf -> F) + activation (sequence_model.py:119-123) -> fbT [B, Tp, F]
-  return linear_tc(w.fb_h1all, (size_t)Hf, Hf, fb->fc_w, fb->fc_b, F, d->fb_activation, w.fbT, (size_t)F, (size_t)B * Tp, x3,
-                   w.tc, st);
-}
-
 // everything after the time-major magnitude exists: norms, full-band stack, sub-band stack
 static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
                       const void* sb_packed, const Dims& m, const ModelWs& w, float* crm, cudaStream_t st) {
   int rc;
-  const int F = m.F, Tp = m.Tp, B = m.B, Hf = d->fb_hidden, Hs = d->sb_hidden;
+  const int F = m.F, Tp = m.Tp, B = m.B, Hs = d->sb_hidden;
   // per-clip statistics of the look-ahead-padded magnitude (model.py:92, :111)
   if ((rc = clip_stats_launch(w.magT, B, Tp, F, d->sb_num_neighbors, w.fs, w.sums_mag, st))) return rc;
   if ((rc = norm_scales_launch(w.sums_mag, w.sums_mag, B, (float)F * Tp, 1.f, w.inv1, nullptr, st))) return rc;
@@ -154,46 +119,12 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
   const float cum_eps = 1.1920928955078125e-07f;  // audio_zen/constant.py:9 (np.finfo(np.float32).eps)
   if (cum && (rc = cum_clip_scale_launch(w.fs, B, Tp, F, cum_eps, w.cum1, st))) return rc;
 
-  // ---- full-band stack (model.py:92-95): 2-layer LSTM(F -> Hf -> Hf), rows = clips
-  static const bool fb_stepwise = getenv("FSN_FB_STEPWISE") != nullptr;  // debug: force the per-step kernels
-  const bool fb_tc = !fb_stepwise && fb_tc_enabled(d, B);
-  if (fb_tc) {
-    if ((rc = fb_tc_forward(d, fb, m, w, st))) return rc;
-  } else if (!fb_stepwise && !cum && d->cell_type == FSN_CELL_LSTM && fb_persistent_supported(F, Hf, Hf)) {
-    // one persistent cooperative kernel per chunk of <= 256 clips: weights resident in shared memory,
-    // layer wavefront, one grid barrier per time step
-    for (int b0 = 0; b0 < B; b0 += 256) {
-      const int nb = (B - b0 < 256) ? B - b0 : 256;
-      if ((rc = fb_persistent_launch(fb, w.magT + (size_t)b0 * Tp * F, w.inv1 + b0, w.fb_pp,
-                                     w.fb_h1all + (size_t)b0 * Tp * Hf, w.fb_barrier, nb, F, Hf, Hf, Tp, st)))
-        return rc;
-    }
-  } else {
-  for (int t = 0; t < Tp; ++t) {
-    StepParams p;
-    memset(&p, 0, sizeof(p));
-    p.R = B; p.H = Hf; p.first = (t == 0); p.gru = d->cell_type == FSN_CELL_GRU;
-    // layer 0: x_t = magT[b,t,:] * inv1[b]
-    p.K0 = F;
-    p.w_ih = fb->w_ih[0]; p.w_hh = fb->w_hh[0]; p.b_ih = fb->b_ih[0]; p.b_hh = fb->b_hh[0];
-    p.h_prev = w.fb_h0[(t + 1) & 1]; p.h_prev_stride = Hf;
-    p.h_out = w.fb_h0[t & 1]; p.h_out_stride = Hf;
-    p.c = w.fb_c0;
-    p.x0 = w.magT + (size_t)t * F; p.x0_row_stride = (size_t)Tp * F;
-    p.row_scale = cum ? w.cum1 + (size_t)t * B : w.inv1;  // cumulative: scale of (step t, clip b)
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-    // layer 1: x_t = h0_t, output kept for every t (input of the Linear layer)
-    p.K0 = Hf;
-    p.w_ih = fb->w_ih[1]; p.w_hh = fb->w_hh[1]; p.b_ih = fb->b_ih[1]; p.b_hh = fb->b_hh[1];
-    p.x0 = w.fb_h0[t & 1]; p.x0_row_stride = Hf; p.row_scale = nullptr;
-    p.h_prev = w.fb_h1all + (size_t)(t > 0 ? t - 1 : 0) * Hf; p.h_prev_stride = (size_t)Tp * Hf;
-    p.h_out = w.fb_h1all + (size_t)t * Hf; p.h_out_stride = (size_t)Tp * Hf;
-    p.c = w.fb_c1;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-  }
-  }
-  // Linear(Hf -> F) + activation over all (b,t): fbT[b,t,f]  (sequence_model.py:119-123)
-  if (!fb_tc && (rc = fc_gemm_launch(w.fb_h1all, fb->fc_w, fb->fc_b, w.fbT, B * Tp, Hf, F, d->fb_activation, st))) return rc;
+  // ---- full-band stack -> fbT [B, Tp, F]; x = magT * 1/(mu + 1e-5) of the clip (model.py:92) or, cumulative norm, the
+  // scale of (step, clip) from the time-major table cum1[t*B + b] (base_model.py:220-251)
+  SeqStack s = fb_stack(d, m);
+  s.L[0] = seq_layer(*fb, 0); s.L[1] = seq_layer(*fb, 1);
+  s.x = w.magT; s.scale = cum ? w.cum1 : w.inv1; s.fc_w = fb->fc_w; s.fc_b = fb->fc_b; s.out = w.fbT;
+  if ((rc = seq_stack_forward(s, w.fb, st))) return rc;
 
   // ---- second norm (model.py:110-111) in closed form: never materialise [B,F,Ksb,T']
   if ((rc = clip_stats_launch(w.fbT, B, Tp, F, d->fb_num_neighbors, w.fs, w.sums_fb, st))) return rc;
@@ -219,28 +150,19 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
   }
 
   // ---- sub-band stack, fp32 path (model.py:121-135): rows = (clip, frequency) units
+  const Step2State s2{{w.sb_h0[0], w.sb_h0[1]}, w.sb_c0, {w.sb_h1[0], w.sb_h1[1]}, w.sb_c1, Hs, 0};
   for (int t = 0; t < Tp; ++t) {
     StepParams p;
     memset(&p, 0, sizeof(p));
-    p.R = m.R; p.H = Hs; p.first = (t == 0); p.gru = d->cell_type == FSN_CELL_GRU;
+    p.R = m.R; p.H = Hs; p.gru = d->cell_type == FSN_CELL_GRU;
     p.K0 = m.Ksb;
     p.w_ih = sb->w_ih[0]; p.w_hh = sb->w_hh[0]; p.b_ih = sb->b_ih[0]; p.b_hh = sb->b_hh[0];
-    p.h_prev = w.sb_h0[(t + 1) & 1]; p.h_prev_stride = Hs;
-    p.h_out = w.sb_h0[t & 1]; p.h_out_stride = Hs;
-    p.c = w.sb_c0;
     p.magT = w.magT; p.fbT = w.fbT; p.inv2 = w.inv2;
     p.unit_scale = cum ? w.cum2 + (size_t)t * m.R : nullptr;
     p.F = F; p.Tp = Tp; p.t = t; p.Ns = d->sb_num_neighbors; p.Nf = d->fb_num_neighbors; p.map = map;
-    if ((rc = lstm_step_launch(p, SEG0_GATHER, st))) return rc;
-    p.K0 = Hs;
-    p.w_ih = sb->w_ih[1]; p.w_hh = sb->w_hh[1]; p.b_ih = sb->b_ih[1]; p.b_hh = sb->b_hh[1];
-    p.x0 = w.sb_h0[t & 1]; p.x0_row_stride = Hs; p.row_scale = nullptr;
-    p.h_prev = w.sb_h1[(t + 1) & 1]; p.h_prev_stride = Hs;
-    p.h_out = w.sb_h1[t & 1]; p.h_out_stride = Hs;
-    p.c = w.sb_c1;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+    if ((rc = lstm_step2_launch(p, SEG0_GATHER, t, seq_layer(*sb, 1), s2, st))) return rc;
     if (t >= d->look_ahead)
-      if ((rc = sb_fc_step_launch(w.sb_h1[t & 1], m.R, Hs, sb->fc_w, sb->fc_b, 2, d->sb_activation, crm, m.Fsub,
+      if ((rc = sb_fc_step_launch(s2.h1_at(t), m.R, Hs, sb->fc_w, sb->fc_b, 2, d->sb_activation, crm, m.Fsub,
                                   m.T, t - d->look_ahead, st)))
         return rc;
   }

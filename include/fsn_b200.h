@@ -193,7 +193,7 @@ typedef struct fsn_fast_desc {
   int32_t noisy_num_neighbors; /* noisy_input_num_neighbors */
   int32_t enc_num_neighbors;   /* encoder_output_num_neighbors */
   int32_t precision;           /* FSN_PREC_* for the bottleneck stack (the tensor-core path needs bn_hidden = 384) */
-  int32_t cell_type;           /* FSN_CELL_* (`sequence_model`); the training step is built for LSTM only */
+  int32_t cell_type;           /* FSN_CELL_* (`sequence_model`); inference and training are built for LSTM only */
 } fsn_fast_desc;
 
 typedef struct fsn_fast_weights {
@@ -339,7 +339,7 @@ typedef struct fsn_fullband_desc {
   int32_t activation; /* FSN_ACT_* */
   int32_t norm_type;  /* FSN_NORM_* */
   int32_t precision;  /* training only: FSN_PREC_FP32 (0) or FSN_PREC_TF32_TC */
-  int32_t cell_type;  /* training only: FSN_CELL_* (0 = LSTM; the training step is built for LSTM only) */
+  int32_t cell_type;  /* FSN_CELL_* (0 = LSTM; inference and training are built for LSTM only) */
 } fsn_fullband_desc;
 
 size_t fsn_fullband_workspace_bytes(const fsn_fullband_desc* d, int B, int T);

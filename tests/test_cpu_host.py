@@ -191,6 +191,16 @@ def test_workspace_queries_report_error_class_without_gpu():
     assert lib.fsn_fullband_workspace_bytes(C.byref(f), 4, 100) > 0
     f.num_layers = 9
     assert lib.fsn_fullband_workspace_bytes(C.byref(f), 4, 100) == 0 and lib.fsn_last_error_code() == _lib.FSN_ERR_UNSUPPORTED
+    # GRU: the fullband_baseline and fast_fullsubnet forwards have LSTM kernels only
+    f.num_layers, f.cell_type = 3, 1
+    assert lib.fsn_fullband_workspace_bytes(C.byref(f), 4, 100) == 0 and lib.fsn_last_error_code() == _lib.FSN_ERR_UNSUPPORTED
+    fd = _lib.FastDesc(num_freqs=257, look_ahead=2, shrink_size=2, num_mels=64, enc1_hidden=384, enc2_hidden=257,
+                       bn_hidden=384, bn_layers=2, dec_hidden=512, noisy_num_neighbors=5, enc_num_neighbors=0, precision=0,
+                       cell_type=0)
+    assert lib.fsn_fast_workspace_bytes(C.byref(fd), 4, 100) > 0 and lib.fsn_fast_packed_bytes(C.byref(fd)) > 0
+    fd.cell_type = 1
+    assert lib.fsn_fast_workspace_bytes(C.byref(fd), 4, 100) == 0 and lib.fsn_last_error_code() == _lib.FSN_ERR_UNSUPPORTED
+    assert lib.fsn_fast_packed_bytes(C.byref(fd)) == 0
 
 
 def test_write_wav_roundtrip(tmp_path):

@@ -261,6 +261,10 @@ def test_fast_fullsubnet_matches_reference(golden, dev, precision, tol):
         with torch.no_grad():
             got = m(x.to(dev))
         assert rel_max(got.cpu(), ref) < tol, Tn
+    # the inference kernels are built for LSTM only: a GRU model is refused before any kernel reads its [3H, K] weights
+    gru = Model(**dict(FO.DEFAULT_FAST_ARGS, sequence_model="GRU"), precision=precision).to(dev).eval()
+    with pytest.raises(NotImplementedError), torch.no_grad():
+        gru(mag[:1])
 
 
 # ------------------------------------------------------------------ improved_fullsubnet (config 5, A14)
@@ -368,6 +372,9 @@ def test_fullband_baseline_matches_reference(golden, dev):
         assert out.shape == g[tag + "_out"].shape
         assert rel_max(out.cpu(), g[tag + "_out"]) < 2e-5, tag
         assert rel_max(one.cpu(), g[tag + "_out"][1:2]) < 2e-5, tag
+    gru = Model(**dict(small, sequence_model="GRU")).to(dev).eval()  # LSTM inference kernels only
+    with pytest.raises(NotImplementedError), torch.no_grad():
+        gru(T(g["small_mag"], dev))
 
 
 # ------------------------------------------------------------------ host loop: int16 scaling (SURVEY 8f rank 2)
