@@ -6,30 +6,33 @@
 // The same stack shape is the fast_fullsubnet bottleneck (fsn_fast_model.cu): there the gather also down-samples
 // time (`shrink`) and the Linear layer has one output (the packer zero-pads the second).
 //
-// Formulation ("weights as the M operand").  A CTA owns NB sub-band units (rows of the
-// [B*F', .] batch) for all T' steps and both layers.  Per step and layer it needs
+// Formulation ("weights as the M operand", hidden units split over a CTA pair).  A PAIR of CTAs owns NB = 32 sub-band
+// units (rows of the [B*F', .] batch) for all T' steps and both layers; CTA `half` of the pair owns hidden units
+// [H/2 half, H/2 (half+1)).  Per step and layer the pair needs
 //     gates^T [4H, NB] = W [4H, K] . S^T [K, NB],      S = [x_t | h_{t-1}]  (layer 0)
 //                                                      S = [h0_t | h1_{t-1}] (layer 1)
-// which runs as wgmma m64nNBk16 (fp16 operands, fp32 accumulate), two m64 halves per gate of a
-// 128-unit slice m:
-//   * A operand  = 32 KB fp16 weight stages [4 gates x 128 x 32 k], pre-swizzled (64B) by the packer and
-//                  streamed from L2 with cp.async.bulk (TMA engine) through a ring; a cluster of CL CTAs
-//                  consumes the same stream, each loads 1/CL of a stage and multicasts it to all;
-//   * B operand  = the recurrent state S, fp16, resident in shared memory (K-major, 128B-swizzled),
-//                  written in place by the consumers (h) and the gather warp (x);
-//   * D          = fp32 accumulators in the registers of consumer warpgroup m, which owns hidden units
-//                  [128m, 128m+128): it issues the MMAs of its slice, keeps that slice's cell state c for all NB
-//                  rows and both layers in registers, applies the gate non-linearities in fp32 and writes h (fp16)
-//                  straight back into the B-operand layout.  While one warpgroup runs its cell, the next one's
-//                  MMAs consume the weight stream.
+// which runs as wgmma m64n32k16 (fp16 operands, fp32 accumulate), one m64 tile per gate of a 64-unit slice s:
+//   * A operand  = 16 KB fp16 weight stages [4 gates x 64 x 32 k], pre-swizzled (64B) by the packer and streamed
+//                  from L2 with cp.async.bulk (TMA engine) through a ring; each half has its own stream.  The CTAs
+//                  that hold the same half in the CL pairs of a cluster consume the same stream: each loads 1/CL of
+//                  a stage and multicasts it to all;
+//   * B operand  = the recurrent state S of all H units, fp16, resident in shared memory (K-major, 128B-swizzled;
+//                  x_t 64B-swizzled), written in place by the consumers (h: the own half directly, the peer's half
+//                  by a DSMEM bulk copy from the peer) and the gather warp (x);
+//   * D          = fp32 accumulators in the registers of consumer warpgroup m, which owns slice s = MT half + m, hidden
+//                  units [64s, 64s+64): it issues the MMAs of its slice, keeps that slice's cell state c for all NB
+//                  rows and both layers in registers, applies the gate non-linearities in fp32, writes h (fp16)
+//                  straight back into the B-operand layout and copies that k-block into the peer CTA.  While one
+//                  warpgroup runs its cell, the next one's MMAs consume the weight stream.
+// Each streamed weight byte thus meets 32 rows, twice the rows one CTA's registers could hold for all H units.
 // X3 (FSN_PREC_F16X3_TC) is the ERROR-COMPENSATED variant: weights and state are each split into two fp16 terms
 // (hi = rn(v), lo = rn(v - hi)) and every product is issued as W_hi.S_hi + W_hi.S_lo + W_lo.S_hi into the same fp32
 // accumulator (the dropped W_lo.S_lo term is 2^-22 relative); the stream carries a hi and a lo stage per k range and
 // the gate non-linearities use expf / IEEE division.
-// Nothing but the NB x 2 mask values per step ever leaves the SM.
+// Nothing but the NB x 2 mask values per step (and the pair's h / Linear exchange over DSMEM) ever leaves the SM.
 //
 // Warp roles (128 + 128 MT threads): 0 = weight-stage producer, 1 = idle, 2 = x_t gather, 3 = Linear(H->2) + output
-// staging, 4.. = consumer warpgroups (one per 128-unit slice m).
+// staging (half 0) or the half's Linear partial sums sent to half 0 (half 1), 4.. = consumer warpgroups.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -43,31 +46,34 @@ namespace tc {
 
 using namespace ptx;
 
-constexpr int NB = 16;                 // sub-band units per CTA (MMA N)
+constexpr int NB = 32;                 // sub-band units per CTA pair (MMA N)
 constexpr int KB = 64;                 // fp16 elements per 128-byte swizzle row
 constexpr int KS = 32;                 // k elements per weight stage
-constexpr int W_SUB = 128 * KS * 2;    // 8192 B: [128 gate rows x 32 k] of one gate, 64B-swizzled
-constexpr int W_TILE = 4 * W_SUB;      // 32768 B: one ring stage = the 4 gates (i,f,g,o) of one (slice m, k range, part)
-constexpr int S_KBLK = NB * KB * 2;    // 2048 B: one k-block of the state operand
+constexpr int US = 64;                 // hidden units per slice (MMA M): one consumer warpgroup, one k-block of h
+constexpr int W_SUB = US * KS * 2;     // 4096 B: [64 gate rows x 32 k] of one gate, 64B-swizzled
+constexpr int W_TILE = 4 * W_SUB;      // 16384 B: one ring stage = the 4 gates (i,f,g,o) of one (slice, k range, part)
+constexpr int S_KBLK = NB * KB * 2;    // 4096 B: one k-block of the state operand (= h of one slice)
+constexpr int X_BLK = NB * KS * 2;     // 2048 B: x_t, 64B-swizzled
 constexpr int MAX_STAGES = 4;          // weight ring depth (FSN_TC_STAGES, default 4)
-constexpr int MAX_MT = 3;
+constexpr int MAX_MT = 3;              // slices per CTA (H / 128)
 constexpr int OUT_T = 8;               // output frames staged before a store
 constexpr int NTHREADS = 128 + 128 * MAX_MT;
 
+// one stream per half: stage order = consumption order of that half's CTA; half 1's stream follows half 0's
 struct PackedLayout {
   int H, MT, nkb0, nkb1, parts;
-  size_t tiles0, tiles1;  // stages per step, per layer
+  size_t tiles0, tiles1;  // stages per step and half, per layer
   size_t off_bias, off_fcw, off_fcb, bytes;
 };
 
 __host__ __device__ inline PackedLayout packed_layout(int H, bool x3) {
   PackedLayout L;
   L.H = H; L.MT = H / 128;
-  L.nkb0 = 1 + H / KS; L.nkb1 = 2 * H / KS;  // k ranges of 32 per slice m
+  L.nkb0 = 1 + H / KS; L.nkb1 = 2 * H / KS;  // k ranges of 32 per slice
   L.parts = x3 ? 2 : 1;
   L.tiles0 = (size_t)L.MT * L.nkb0 * L.parts;
   L.tiles1 = (size_t)L.MT * L.nkb1 * L.parts;
-  L.off_bias = (L.tiles0 + L.tiles1) * W_TILE;
+  L.off_bias = 2 * (L.tiles0 + L.tiles1) * W_TILE;
   L.off_fcw = L.off_bias + (size_t)2 * 4 * H * sizeof(float);
   L.off_fcb = L.off_fcw + (size_t)2 * H * sizeof(float);
   L.bytes = L.off_fcb + 256;
@@ -75,7 +81,8 @@ __host__ __device__ inline PackedLayout packed_layout(int H, bool x3) {
 }
 
 // ---------------------------------------------------------------- weight packer
-// stage order = consumption order: layer, m (128-unit slice), k range of 32, part (hi, lo); 4 gate sub-tiles per stage
+// stage order = consumption order: half, layer, m (64-unit slice MT half + m), k range of 32, part (hi, lo);
+// 4 gate sub-tiles per stage
 __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restrict__ whh0,
                             const float* __restrict__ wih1, const float* __restrict__ whh1,
                             const float* __restrict__ bih0, const float* __restrict__ bhh0,
@@ -83,14 +90,15 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
                             const float* __restrict__ fcw, const float* __restrict__ fcb, int H, int Ksb, int x3,
                             int fc_out, uint8_t* __restrict__ out) {
   const PackedLayout L = packed_layout(H, x3 != 0);
-  const size_t nstages = L.tiles0 + L.tiles1;
-  const size_t total = nstages * 4 * 128 * 4;  // one thread per (stage, gate, row, 16-byte chunk)
+  const size_t per_half = L.tiles0 + L.tiles1;
+  const size_t total = 2 * per_half * 4 * US * 4;  // one thread per (stage, gate, row, 16-byte chunk)
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(i & 3);
-    const int r = (int)((i >> 2) & 127);
-    const int g = (int)((i >> 9) & 3);
-    const size_t st_abs = i >> 11;
-    size_t st = st_abs;
+    const int r = (int)((i >> 2) & (US - 1));
+    const int g = (int)((i >> 8) & 3);
+    const size_t st_abs = i >> 10;
+    const int half = (int)(st_abs / per_half);
+    size_t st = st_abs - half * per_half;
     const int layer = st >= L.tiles0;
     if (layer) st -= L.tiles0;
     const int part = (int)(st % L.parts);
@@ -98,7 +106,7 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
     const int nkb = layer ? L.nkb1 : L.nkb0;
     const int kb = (int)(st % nkb);
     const int m = (int)(st / nkb);
-    const int wrow = g * H + m * 128 + r;
+    const int wrow = g * H + (half * L.MT + m) * US + r;
     __half v[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
@@ -132,18 +140,19 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
 
 // ---------------------------------------------------------------- shared-memory plan
 struct Smem {
-  uint32_t w, x, h0, h1, lo, fcw, outst, rows, bars, total;
+  uint32_t w, x, h0, h1, lo, fcw, fcp, outst, rows, bars, total;
 };
 __host__ __device__ inline Smem smem_plan(int H, int stages, bool x3) {
   Smem s;
   const int nkh = H / KB;
   uint32_t o = 0;
   s.w = o; o += stages * W_TILE;
-  s.x = o; o += 2 * S_KBLK;
+  s.x = o; o += 2 * X_BLK;
   s.h0 = o; o += 2 * nkh * S_KBLK;
   s.h1 = o; o += nkh * S_KBLK;  // single buffer: h1_t overwrites h1_{t-1} once every layer-1 MMA of step t is done
   s.lo = o; o += x3 ? (o - s.x) : 0;  // X3: lo copies of x, h0, h1 at offset (lo - x) from the hi copies
   s.fcw = o; o += 4 * MAX_MT * 2 * NB * 4;  // Linear partial sums [consumer warp][o][row]
+  s.fcp = o; o += 2 * 2 * NB * 4;           // half 0: half 1's Linear sums [buffer][o][row]
   s.outst = o; o += NB * 2 * OUT_T * 4;
   s.rows = o; o += NB * 16;
   s.bars = o; o += 256;
@@ -154,8 +163,12 @@ __host__ __device__ inline Smem smem_plan(int H, int stages, bool x3) {
 struct Bars {
   uint64_t w_full[MAX_STAGES], w_empty[MAX_STAGES];
   uint64_t x_full[2], x_empty[2];
-  uint64_t h0_ready, h1_ready, fc_done;
+  // h0_ready[b]: h0_t (t & 1 = b) complete in buffer b, this half written here and the peer's half landed (complete_tx)
+  // h0_empty[b]: the peer's consumers have read h0 buffer b (their layer-1 MMAs of step t) - this CTA may copy into it
+  uint64_t h0_ready[2], h0_empty[2];
+  uint64_t h1_ready, h1_empty, fc_done;
   uint64_t l1_done;   // all layer-1 MMAs of a step have completed (h1 may be overwritten)
+  uint64_t fcp_full[2], fcp_empty[2];  // half 1 -> half 0 Linear sums
   // turn[m]: warpgroup m may wait on the weight ring - its predecessor in the stream has seen all of its own
   // stages land.  The ring's parity waits are only sound one phase ahead, so the warpgroups take the ring in turn
   uint64_t turn[MAX_MT];
@@ -191,17 +204,18 @@ __device__ __forceinline__ float act_apply(float v, int act) {
 template <bool X3> __device__ __forceinline__ float sg(float x) { return X3 ? 1.0f / (1.0f + expf(-x)) : fast_sigmoid(x); }
 template <bool X3> __device__ __forceinline__ float th(float x) { return X3 ? 1.0f - 2.0f / (1.0f + expf(2.0f * x)) : fast_tanh(x); }
 
-// Consumer warpgroup releases weight stage `bar` to the producers of the CL CTAs that share the stream: one arrive per
-// warpgroup and destination CTA (w_empty counts CL), warp q signalling CTA q so that the remote arrives go out in
-// parallel.  No fence is needed: the stage is read only by this warpgroup's wgmma (async proxy), the wgmma.wait_group
-// before this call has retired those reads, and the producers overwrite the stage with TMA (async proxy) only after
-// the w_empty phase completes - the barrier phase alone orders the overwrite after the reads, so the arrive keeps its
-// default .release.cta semantics (the hand-off of CUTLASS's TMA pipelines for the same hazard).  Every warp of the
-// warpgroup has passed the w_full wait of the stage: the MMAs that read it are warpgroup-collective.
-__device__ __forceinline__ void release_stage(uint64_t* bar, int CL, int q, int lane) {
+// Consumer warpgroup releases weight stage `bar` to the producers of the CL CTAs that share the stream (the CTAs of
+// the same half, ranks 2 q + half): one arrive per warpgroup and destination CTA (w_empty counts CL), warp q
+// signalling pair q so that the remote arrives go out in parallel.  No fence is needed: the stage is read only by
+// this warpgroup's wgmma (async proxy), the wgmma.wait_group before this call has retired those reads, and the
+// producers overwrite the stage with TMA (async proxy) only after the w_empty phase completes - the barrier phase
+// alone orders the overwrite after the reads, so the arrive keeps its default .release.cta semantics (the hand-off of
+// CUTLASS's TMA pipelines for the same hazard).  Every warp of the warpgroup has passed the w_full wait of the stage:
+// the MMAs that read it are warpgroup-collective.
+__device__ __forceinline__ void release_stage(uint64_t* bar, int CL, int half, int q, int lane) {
   if (lane != 0 || q >= CL) return;
   if (CL == 1) mbar_arrive(bar);
-  else mbar_arrive_remote(bar, (uint32_t)q);
+  else mbar_arrive_remote(bar, (uint32_t)(2 * q + half));
 }
 
 template <bool X3>
@@ -215,25 +229,34 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
   const int nkh = H / KB;
   const int STAGES = a.stages;
   const int CL = a.cluster;
-  const uint16_t cl_mask = (uint16_t)((1u << CL) - 1u);
-  const uint32_t cl_rank = (CL > 1) ? cluster_ctarank() : 0u;
+  // the cluster is CL pairs: rank 2 i + half, pair i; the CTAs of one half multicast that half's stream
+  const uint32_t cl_rank = cluster_ctarank();
+  const int half = (int)(cl_rank & 1u);
+  const uint32_t peer = cl_rank ^ 1u;
+  const uint16_t cl_mask = (uint16_t)((0x55u & ((1u << (2 * CL)) - 1u)) << half);
   const Smem sp = smem_plan(H, STAGES, X3);
   const uint32_t LO = sp.lo - sp.x;  // byte offset of a lo copy from its hi copy
   const PackedLayout PL = packed_layout(H, X3);
   Bars& bars = *reinterpret_cast<Bars*>(smem + sp.bars);
   RowInfo* rows = reinterpret_cast<RowInfo*>(smem + sp.rows);
   float* fc_part = reinterpret_cast<float*>(smem + sp.fcw);
+  float* fcp = reinterpret_cast<float*>(smem + sp.fcp);
   float* outst = reinterpret_cast<float*>(smem + sp.outst);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row0 = blockIdx.x * NB;
+  const int row0 = (blockIdx.x >> 1) * NB;
   const int Tp = a.Tp;
 
   // ---------------- one-time setup
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.w_full[s], 1); mbar_init(&bars.w_empty[s], CL); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&bars.x_full[i], 1); mbar_init(&bars.x_empty[i], 4 * MT); }
-    mbar_init(&bars.h0_ready, 4 * MT);
-    mbar_init(&bars.h1_ready, 4 * MT);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&bars.x_full[i], 1); mbar_init(&bars.x_empty[i], 4 * MT);
+      mbar_init(&bars.h0_ready[i], 5 * MT);  // 4 MT local warps + MT peer copies
+      mbar_init(&bars.h0_empty[i], MT);
+      mbar_init(&bars.fcp_full[i], 1); mbar_init(&bars.fcp_empty[i], 1);
+    }
+    mbar_init(&bars.h1_ready, 5 * MT);
+    mbar_init(&bars.h1_empty, MT);
     mbar_init(&bars.fc_done, 1);
     mbar_init(&bars.l1_done, 4 * MT);
     for (int m = 0; m < MAX_MT; ++m) mbar_init(&bars.turn[m], 4);
@@ -258,18 +281,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
   }
   fence_proxy_async_smem();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();  // peers' barriers are initialised before any multicast reaches them
+  cluster_sync_all();  // peers' barriers are initialised before any multicast, copy or remote arrive reaches them
 
   if (warp < 4) {
     // warpgroup 0 (producer / gather / Linear) needs few registers: hand the rest to the consumers
     asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
   if (warp == 0) {
-    // ================= weight-stage producer: the same (layer 0, layer 1) stream every step
+    // ================= weight-stage producer: this half's (layer 0, layer 1) stream, the same every step
+    const uint8_t* stream = a.packed + (size_t)half * (PL.tiles0 + PL.tiles1) * W_TILE;
     uint32_t stage = 0, phase = 0;
     for (int it = 0; it <= Tp; ++it) {
       const size_t t_begin = (it < Tp) ? 0 : PL.tiles0;
       const size_t t_end = (it >= 1) ? PL.tiles0 + PL.tiles1 : PL.tiles0;
-      const uint8_t* src = a.packed + t_begin * W_TILE;
+      const uint8_t* src = stream + t_begin * W_TILE;
       for (size_t tile = t_begin; tile < t_end; ++tile, src += W_TILE) {
         // all CL CTAs' consumers have drained this stage (on the critical path: no back-off)
         mbar_wait_cta<false>(&bars.w_empty[stage], phase ^ 1);
@@ -278,7 +302,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
           if (CL == 1) {
             bulk_g2s(smem + sp.w + stage * W_TILE, src, W_TILE, &bars.w_full[stage]);
           } else {
-            const uint32_t slice = W_TILE / CL, off = cl_rank * slice;
+            const uint32_t slice = W_TILE / CL, off = (cl_rank >> 1) * slice;
             bulk_g2s_mc(smem + sp.w + stage * W_TILE + off, src + off, slice, &bars.w_full[stage], cl_mask);
           }
         }
@@ -288,11 +312,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
     }
   } else if (warp == 2) {
     // ================= x_t gather: sub-band unit = 2Ns+1 reflected magnitude rows + 2Nf+1 full-band rows,
-    // scaled by 1/(mu'+1e-5)  (base_model.py:35-44, model.py:98-111), fp16 (X3: + lo), B-operand layout
+    // scaled by 1/(mu'+1e-5)  (base_model.py:35-44, model.py:98-111), fp16 (X3: + lo), B-operand layout.
+    // Both CTAs of a pair gather all NB rows (a duplicated L2 read is cheaper than an exchange)
     const int nmag = 2 * a.Ns + 1;
     for (int t = 0; t < Tp; ++t) {
       mbar_wait_cta<true>(&bars.x_empty[t & 1], ((t >> 1) & 1) ^ 1);
-      uint8_t* xb = smem + sp.x + (t & 1) * S_KBLK;
+      uint8_t* xb = smem + sp.x + (t & 1) * X_BLK;
       // source frames of step t: itself, or (fast_fullsubnet/model.py:108-129) frame 0 alone, then blocks of
       // `shrink` frames, the last one over its own length
       int f0 = t, f1 = t + 1;
@@ -315,38 +340,55 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
           }
         }
         const __half hi = __float2half_rn(v);
-        *reinterpret_cast<__half*>(xb + swz128_off(n, lane)) = hi;
-        if (X3) *reinterpret_cast<__half*>(xb + LO + swz128_off(n, lane)) = __float2half_rn(v - __half2float(hi));
+        *reinterpret_cast<__half*>(xb + swz64_off(n, lane)) = hi;
+        if (X3) *reinterpret_cast<__half*>(xb + LO + swz64_off(n, lane)) = __float2half_rn(v - __half2float(hi));
       }
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars.x_full[t & 1]);
     }
   } else if (warp == 3) {
-    // ================= Linear(H -> 2): sums the fp32 partial dot products of the consumer warps, adds
-    // the bias, stages OUT_T frames and stores crm[b', o, f', t - la]  (model.py:129-135 fused)
-    const float fcb0 = reinterpret_cast<const float*>(a.packed + PL.off_fcb)[0];
-    const float fcb1 = reinterpret_cast<const float*>(a.packed + PL.off_fcb)[1];
-    const int ln = lane < NB ? lane : 0;
-    const RowInfo ri = rows[ln];
+    // ================= Linear(H -> 2), one row per lane: sums the fp32 partial dot products of the consumer warps.
+    // Half 1 sends its sums to half 0; half 0 adds the bias, its own sums and half 1's (one fixed association
+    // order), stages OUT_T frames and stores crm[b', o, f', t - la]  (model.py:129-135 fused)
+    const float fcb0 = half ? 0.f : reinterpret_cast<const float*>(a.packed + PL.off_fcb)[0];
+    const float fcb1 = half ? 0.f : reinterpret_cast<const float*>(a.packed + PL.off_fcb)[1];
+    const RowInfo ri = rows[lane];
     int staged = 0, t_stage0 = 0;
     for (int t = 0; t < Tp; ++t) {
       mbar_wait_cta<true>(&bars.h1_ready, t & 1);
+      float s0 = fcb0, s1 = fcb1;
       if (t >= a.la) {
-        float s0 = fcb0, s1 = fcb1;
         for (int w = 0; w < 4 * MT; ++w) {
-          s0 += fc_part[(w * 2 + 0) * NB + ln];
-          s1 += fc_part[(w * 2 + 1) * NB + ln];
+          s0 += fc_part[(w * 2 + 0) * NB + lane];
+          s1 += fc_part[(w * 2 + 1) * NB + lane];
         }
-        if (staged == 0) t_stage0 = t - a.la;
-        outst[(ln * 2 + 0) * OUT_T + staged] = act_apply(s0, a.act);
-        outst[(ln * 2 + 1) * OUT_T + staged] = act_apply(s1, a.act);
-        ++staged;
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars.fc_done);
-      if (staged == OUT_T || (t == Tp - 1 && staged > 0)) {
-        if (lane < NB && ri.src_b >= 0) {
+      if (t < a.la) continue;
+      const int u = t - a.la, b = u & 1;
+      float* pb = fcp + b * 2 * NB;
+      if (half) {
+        // half 0 has read this buffer's previous sums (generic stores to another CTA: cluster-scope release/acquire)
+        mbar_wait<true>(&bars.fcp_empty[b], ((u >> 1) & 1) ^ 1);
+        st_remote_f32(pb + lane, peer, s0);
+        st_remote_f32(pb + NB + lane, peer, s1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive_cluster(&bars.fcp_full[b], peer);
+        continue;
+      }
+      mbar_wait<true>(&bars.fcp_full[b], (u >> 1) & 1);
+      s0 += pb[lane];
+      s1 += pb[NB + lane];
+      __syncwarp();
+      if (lane == 0) mbar_arrive_cluster(&bars.fcp_empty[b], peer);
+      if (staged == 0) t_stage0 = u;
+      outst[(lane * 2 + 0) * OUT_T + staged] = act_apply(s0, a.act);
+      outst[(lane * 2 + 1) * OUT_T + staged] = act_apply(s1, a.act);
+      ++staged;
+      if (staged == OUT_T || t == Tp - 1) {
+        if (ri.src_b >= 0) {
 #pragma unroll
           for (int o = 0; o < 2; ++o) {
             float* dst = a.crm + ((size_t)ri.out_idx + (size_t)o * a.Fsub) * a.T + t_stage0;
@@ -358,12 +400,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
     }
   }
   } else {
-    // ================= consumer warpgroup m: MMAs and cells of hidden units [128m, 128m+128) of both layers.
-    // Fragment of thread (warp q, lane l): unit 128 m + 64 hf + 16 q + l/4 + 8 hh, row n = 8 j + 2 (l%4) + e,
-    // register acc[g][hf][4 j + 2 hh + e]
+    // ================= consumer warpgroup m: MMAs and cells of slice s = MT half + m, hidden units [64s, 64s+64), of
+    // both layers.  Fragment of thread (warp q, lane l): unit 64 s + 16 q + l/4 + 8 hh, row n = 8 j + 2 (l%4) + e,
+    // register acc[g][4 j + 2 hh + e]
     asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
     const int m = (warp - 4) >> 2;
     const int q = warp & 3;
+    const int s = half * MT + m;
     if (m < MT) {
       const float* bias_g = reinterpret_cast<const float*>(a.packed + PL.off_bias);
       const float* fcw = reinterpret_cast<const float*>(a.packed + PL.off_fcw);
@@ -374,36 +417,35 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
       const uint32_t wbase = smem_u32(smem + sp.w);
       int h0_seen = 0, h1_seen = 0, turns = 0;
       bool first_block = true;
-      size_t tile_base = 0;  // global index (in the producer's stream) of this iteration's first stage
+      size_t tile_base = 0;  // index (in this half's stream) of this iteration's first stage
       for (int it = 0; it <= Tp; ++it) {
         for (int layer = 0; layer < 2; ++layer) {
           const int t = it - layer;
           if (t < 0 || t >= Tp) continue;
-          // operands of this step complete in shared memory (every phase waited on once, in order)
-          // (all of this kernel's barriers guard data written by this CTA or by TMA: CTA-scope waits)
+          // operands of this step complete in shared memory (every phase waited on once, in order).  All of this
+          // kernel's waits on the weight ring and the state are CTA-scope: each of those barriers guards data written
+          // by this CTA or by an async-proxy copy with complete_tx (TMA from L2, the peer's DSMEM bulk copy)
           if (layer == 0) {
             mbar_wait_cta<false>(&bars.x_full[t & 1], (t >> 1) & 1);
-            for (; h0_seen < t; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready, h0_seen & 1);      // h0_{t-1}
+            for (; h0_seen < t; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready[h0_seen & 1], (h0_seen >> 1) & 1);      // h0_{t-1}
           } else {
-            for (; h0_seen < t + 1; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready, h0_seen & 1);  // h0_t
-            for (; h1_seen < t; ++h1_seen) mbar_wait_cta<false>(&bars.h1_ready, h1_seen & 1);      // h1_{t-1}
+            for (; h0_seen < t + 1; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready[h0_seen & 1], (h0_seen >> 1) & 1);  // h0_t
+            for (; h1_seen < t; ++h1_seen) mbar_wait_cta<false>(&bars.h1_ready, h1_seen & 1);                          // h1_{t-1}
           }
-          const uint32_t x_addr = smem_u32(smem + sp.x + (t & 1) * S_KBLK);
+          const uint32_t x_addr = smem_u32(smem + sp.x + (t & 1) * X_BLK);
           const uint32_t h0_cur = smem_u32(smem + sp.h0 + (t & 1) * nkh * S_KBLK);        // h0_t
           const uint32_t h0_prev = smem_u32(smem + sp.h0 + ((t + 1) & 1) * nkh * S_KBLK);  // h0_{t-1}
           const uint32_t h1_prev = smem_u32(smem + sp.h1);                                    // h1_{t-1}
           // B operand k ranges: layer 0: [x_t (32 k)] [h0_{t-1} (H)]; layer 1: [h0_t (H)] [h1_{t-1} (H)]
           const int nkb = layer ? PL.nkb1 : PL.nkb0;
           const size_t first = tile_base + (layer ? ((it < Tp) ? PL.tiles0 : 0) : 0) + (size_t)m * nkb * PARTS;
-          float acc[4][2][8];
+          float acc[4][16];
 #pragma unroll
-          for (int g = 0; g < 4; ++g)
+          for (int g = 0; g < 4; ++g) {
 #pragma unroll
-            for (int hf = 0; hf < 2; ++hf) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) acc[g][hf][i] = 0.f;
-              wg::fence_operand(acc[g][hf]);
-            }
+            for (int i = 0; i < 16; ++i) acc[g][i] = 0.f;
+            wg::fence_operand(acc[g]);
+          }
           int prev_stage = -1;
           if (m > 0 || !first_block) { mbar_wait_cta<false>(&bars.turn[m], turns & 1); ++turns; }
           first_block = false;
@@ -411,8 +453,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
           int stage = (int)(first % (size_t)STAGES);
           uint32_t wphase = (uint32_t)((first / (size_t)STAGES) & 1);
           for (int j = 0; j < nkb; ++j) {
-            uint32_t sb;  // state address of k range j
-            if (layer == 0) sb = (j == 0) ? x_addr : h0_prev + ((j - 1) >> 1) * S_KBLK + ((j - 1) & 1) * 64;
+            // state descriptors of k range j: x_t is one 64B-swizzled block of 32 k, h the 128B-swizzled k-blocks
+            const bool xr = layer == 0 && j == 0;
+            uint32_t sb;
+            if (layer == 0) sb = xr ? x_addr : h0_prev + ((j - 1) >> 1) * S_KBLK + ((j - 1) & 1) * 64;
             else sb = (j < H / KS) ? h0_cur + (j >> 1) * S_KBLK + (j & 1) * 64
                                    : h1_prev + ((j - H / KS) >> 1) * S_KBLK + ((j - H / KS) & 1) * 64;
 #pragma unroll
@@ -423,103 +467,115 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
               const uint32_t wa = wbase + stage * W_TILE;
 #pragma unroll
               for (int kk = 0; kk < 2; ++kk) {
-                const uint64_t bd = wg::desc_sw128(sb + kk * 32);
+                const uint64_t bd = xr ? wg::desc_sw64(sb + kk * 32) : wg::desc_sw128(sb + kk * 32);
+                const uint64_t bl = xr ? wg::desc_sw64(sb + LO + kk * 32) : wg::desc_sw128(sb + LO + kk * 32);
 #pragma unroll
-                for (int g = 0; g < 4; ++g)
-#pragma unroll
-                  for (int hf = 0; hf < 2; ++hf) {
-                    const uint64_t ad = wg::desc_sw64(wa + g * W_SUB + hf * (64 * 64) + kk * 32);
-                    wg::mma_f16_n16(acc[g][hf], ad, bd, 1u);
-                    if (X3 && part == 0) wg::mma_f16_n16(acc[g][hf], ad, wg::desc_sw128(sb + LO + kk * 32), 1u);
-                  }
+                for (int g = 0; g < 4; ++g) {
+                  const uint64_t ad = wg::desc_sw64(wa + g * W_SUB + kk * 32);
+                  wg::mma_f16_n32(acc[g], ad, bd, 1u);
+                  if (X3 && part == 0) wg::mma_f16_n32(acc[g], ad, bl, 1u);
+                }
               }
               wg::commit();
               wg::wait<1>();  // the MMAs of the previous stage have read it
-              if (prev_stage >= 0) release_stage(&bars.w_empty[prev_stage], CL, q, lane);
+              if (prev_stage >= 0) release_stage(&bars.w_empty[prev_stage], CL, half, q, lane);
               prev_stage = stage;
               if (++stage == STAGES) { stage = 0; wphase ^= 1; }
             }
           }
           wg::wait<0>();
 #pragma unroll
-          for (int g = 0; g < 4; ++g)
-#pragma unroll
-            for (int hf = 0; hf < 2; ++hf) wg::fence_operand(acc[g][hf]);
-          release_stage(&bars.w_empty[prev_stage], CL, q, lane);
+          for (int g = 0; g < 4; ++g) wg::fence_operand(acc[g]);
+          release_stage(&bars.w_empty[prev_stage], CL, half, q, lane);
           // this warpgroup's MMAs of the step have consumed x_t / h1_{t-1}
           if (lane == 0) mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
+          if (layer == 1 && lane == 0) {
+            // ... and h0_t / h1_{t-1}, including the peer's half that the peer copied in: the peer may copy again
+            if (q == 2) mbar_arrive_remote(&bars.h0_empty[t & 1], peer);
+            if (q == 3) mbar_arrive_remote(&bars.h1_empty, peer);
+          }
           if (layer == 1 && t >= 1) mbar_wait_cta<false>(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
-          float fsum[2][4];  // Linear partials [o][row slot j*2+e]
+          float fsum[2][8];  // Linear partials [o][row slot j*2+e]
 #pragma unroll
-          for (int i = 0; i < 8; ++i) fsum[i >> 2][i & 3] = 0.f;
-          __half hv[2][2][4];  // h (fp16 hi) [hf][hh][row slot], held back for layer 1
-          __half lv[2][2][4];
-          uint8_t* hb = smem + (layer ? sp.h1 : sp.h0 + (t & 1) * nkh * S_KBLK);
+          for (int i = 0; i < 16; ++i) fsum[i >> 3][i & 7] = 0.f;
+          __half hv[2][8];  // h (fp16 hi) [hh][row slot], held back for layer 1
+          __half lv[2][8];
+          uint8_t* hb = smem + (layer ? sp.h1 : sp.h0 + (t & 1) * nkh * S_KBLK) + s * S_KBLK;  // this slice's k-block
 #pragma unroll
-          for (int hf = 0; hf < 2; ++hf)
+          for (int hh = 0; hh < 2; ++hh) {
+            const int u = s * US + 16 * q + (lane >> 2) + 8 * hh;
+            const float* bl = bias_g + (layer ? 4 * H : 0);
+            const float bi = bl[u], bff = bl[H + u], bg = bl[2 * H + u], bo = bl[3 * H + u];
+            const float w0 = fcw[u], w1 = fcw[H + u];
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              const int u = m * 128 + 64 * hf + 16 * q + (lane >> 2) + 8 * hh;
-              const float* bl = bias_g + (layer ? 4 * H : 0);
-              const float bi = bl[u], bff = bl[H + u], bg = bl[2 * H + u], bo = bl[3 * H + u];
-              const float w0 = fcw[u], w1 = fcw[H + u];
+            for (int j = 0; j < 4; ++j)
 #pragma unroll
-              for (int j = 0; j < 2; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const int ri = 4 * j + 2 * hh + e;
-                  const int ci = hf * 8 + hh * 4 + j * 2 + e;
-                  const float cp = layer ? c1[ci] : c0[ci];
-                  const float cn = sg<X3>(acc[1][hf][ri] + bff) * cp + sg<X3>(acc[0][hf][ri] + bi) * th<X3>(acc[2][hf][ri] + bg);
-                  if (layer) c1[ci] = cn; else c0[ci] = cn;
-                  const float h = sg<X3>(acc[3][hf][ri] + bo) * th<X3>(cn);
-                  const __half hi = __float2half_rn(h);
-                  hv[hf][hh][j * 2 + e] = hi;
-                  lv[hf][hh][j * 2 + e] = __float2half_rn(h - __half2float(hi));
-                  if (layer) { fsum[0][j * 2 + e] += h * w0; fsum[1][j * 2 + e] += h * w1; }
-                }
-            }
+              for (int e = 0; e < 2; ++e) {
+                const int ri = 4 * j + 2 * hh + e;
+                const int ci = hh * 8 + j * 2 + e;
+                const float cp = layer ? c1[ci] : c0[ci];
+                const float cn = sg<X3>(acc[1][ri] + bff) * cp + sg<X3>(acc[0][ri] + bi) * th<X3>(acc[2][ri] + bg);
+                if (layer) c1[ci] = cn; else c0[ci] = cn;
+                const float h = sg<X3>(acc[3][ri] + bo) * th<X3>(cn);
+                const __half hi = __float2half_rn(h);
+                hv[hh][j * 2 + e] = hi;
+                lv[hh][j * 2 + e] = __float2half_rn(h - __half2float(hi));
+                if (layer) { fsum[0][j * 2 + e] += h * w0; fsum[1][j * 2 + e] += h * w1; }
+              }
+          }
           if (layer == 1) {
             // Linear(H->2) in fp32: sum over the warp's units (lanes with equal lane % 4 hold the same rows)
 #pragma unroll
             for (int o = 0; o < 2; ++o)
 #pragma unroll
-              for (int s = 0; s < 4; ++s) {
-                float v = fsum[o][s];
+              for (int r = 0; r < 8; ++r) {
+                float v = fsum[o][r];
                 v += __shfl_xor_sync(0xffffffffu, v, 4);
                 v += __shfl_xor_sync(0xffffffffu, v, 8);
                 v += __shfl_xor_sync(0xffffffffu, v, 16);
-                fsum[o][s] = v;
+                fsum[o][r] = v;
               }
             if (lane < 4) {
 #pragma unroll
               for (int o = 0; o < 2; ++o)
 #pragma unroll
-                for (int s = 0; s < 4; ++s) my_part[o * NB + 8 * (s >> 1) + 2 * lane + (s & 1)] = fsum[o][s];
+                for (int r = 0; r < 8; ++r) my_part[o * NB + 8 * (r >> 1) + 2 * lane + (r & 1)] = fsum[o][r];
             }
-            // every layer-1 MMA of this step (all warpgroups) has consumed h1_{t-1}: overwrite it with h1_t
+            // every layer-1 MMA of this step in this CTA has consumed h1_{t-1}: overwrite it with h1_t
             mbar_wait_cta<false>(&bars.l1_done, t & 1);
+            // ... and in the peer, which also means the peer holds this slice's h1_{t-1} copy: its source may go
+            mbar_wait_cta<false>(&bars.h1_empty, t & 1);
+          } else if (t >= 2) {
+            // the peer's layer-1 MMAs of step t-2 have read h0_{t-2} in buffer t & 1 (and so this slice's copy of it
+            // has landed there); this CTA's own readers of the buffer are ordered by the ring turn (DESIGN 4.1)
+            mbar_wait_cta<false>(&bars.h0_empty[t & 1], ((t - 2) >> 1) & 1);
           }
 #pragma unroll
-          for (int hf = 0; hf < 2; ++hf)
+          for (int hh = 0; hh < 2; ++hh) {
+            const int u = 16 * q + (lane >> 2) + 8 * hh;  // unit within the slice
+            uint8_t* ub = hb + (u & 7) * 2;
+            const int chunk = u >> 3;
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              const int u = m * 128 + 64 * hf + 16 * q + (lane >> 2) + 8 * hh;
-              uint8_t* ub = hb + (u >> 6) * S_KBLK + (u & 7) * 2;
-              const int chunk = (u & 63) >> 3;
+            for (int j = 0; j < 4; ++j)
 #pragma unroll
-              for (int j = 0; j < 2; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const int n = 8 * j + 2 * (lane & 3) + e;
-                  uint8_t* p = ub + (n >> 3) * 1024 + (n & 7) * 128 + ((chunk ^ (n & 7)) << 4);
-                  *reinterpret_cast<__half*>(p) = hv[hf][hh][j * 2 + e];
-                  if (X3) *reinterpret_cast<__half*>(p + LO) = lv[hf][hh][j * 2 + e];
-                }
-            }
+              for (int e = 0; e < 2; ++e) {
+                const int n = 8 * j + 2 * (lane & 3) + e;
+                uint8_t* p = ub + (n >> 3) * 1024 + (n & 7) * 128 + ((chunk ^ (n & 7)) << 4);
+                *reinterpret_cast<__half*>(p) = hv[hh][j * 2 + e];
+                if (X3) *reinterpret_cast<__half*>(p + LO) = lv[hh][j * 2 + e];
+              }
+          }
           fence_proxy_async_smem();
           __syncwarp();
-          if (lane == 0) mbar_arrive(layer ? &bars.h1_ready : &bars.h0_ready);
+          uint64_t* ready = layer ? &bars.h1_ready : &bars.h0_ready[t & 1];
+          if (lane == 0) mbar_arrive(ready);
+          // the slice's k-block (hi, lo) into the same place of the peer, completing on the peer's ready barrier
+          named_sync(1 + m, 128);
+          if (q == 0 && lane == 0) {
+            mbar_arrive_expect_tx_remote(ready, peer, PARTS * S_KBLK);
+            bulk_s2s_remote(hb, S_KBLK, ready, peer);
+            if (X3) bulk_s2s_remote(hb + LO, S_KBLK, ready, peer);
+          }
         }
         tile_base += ((it < Tp) ? PL.tiles0 : 0) + ((it >= 1) ? PL.tiles1 : 0);
       }
@@ -528,7 +584,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
 
   // ---------------- teardown
   __syncthreads();
-  if (CL > 1) cluster_sync_all();  // no CTA leaves while a peer may still signal its barriers
+  cluster_sync_all();  // no CTA leaves while a peer may still signal its barriers or copy into it
 }
 
 }  // namespace tc
@@ -568,9 +624,10 @@ int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed,
   return sb_tc_pack_raw(sb, d->sb_hidden, sb_ksb(d), 2, packed, st, d->precision == FSN_PREC_F16X3_TC);
 }
 
-// launch configuration of `tiles` CTAs (the caller keeps `attr` alive while cfg is used)
+// launch configuration of `pairs` CTA pairs in clusters of `cluster` pairs (2 x cluster CTAs; the caller keeps `attr`
+// alive while cfg is used)
 template <bool X3>
-static int sb_tc_config(int H, int stages, int cluster, int tiles, cudaStream_t st, cudaLaunchConfig_t& cfg,
+static int sb_tc_config(int H, int stages, int cluster, int pairs, cudaStream_t st, cudaLaunchConfig_t& cfg,
                         cudaLaunchAttribute* attr) {
   const tc::Smem sp = tc::smem_plan(H, stages, X3);
   const size_t smem = sp.total + 1024;  // slack for the 1024-byte alignment of the dynamic segment
@@ -578,12 +635,12 @@ static int sb_tc_config(int H, int stages, int cluster, int tiles, cudaStream_t 
                                            (int)smem), "sb_lstm_tc smem attr");
   if (rc) return rc;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(tiles);
+  cfg.gridDim = dim3(2 * pairs);
   cfg.blockDim = dim3(128 + 128 * (H / 128));
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.x = 2 * cluster;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
@@ -593,10 +650,10 @@ static int sb_tc_config(int H, int stages, int cluster, int tiles, cudaStream_t 
 
 template <bool X3>
 static int sb_tc_launch(const tc::KArgs& a, int H, cudaStream_t st) {
-  const int tiles = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;  // padding CTAs own no valid row
+  const int pairs = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;  // padding pairs own no valid row
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
-  int rc = sb_tc_config<X3>(H, a.stages, a.cluster, tiles, st, cfg, attr);
+  int rc = sb_tc_config<X3>(H, a.stages, a.cluster, pairs, st, cfg, attr);
   if (rc) return rc;
   rc = check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_lstm_tc_kernel<X3>, a), "sb_lstm_tc_kernel launch");
   if (rc) return rc;
@@ -624,8 +681,10 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
   static int cluster_env = -1;
   if (cluster_env < 0) {
     const char* e = getenv("FSN_TC_CLUSTER");
-    cluster_env = e ? atoi(e) : 2;
-    if (cluster_env != 1 && cluster_env != 2 && cluster_env != 4) cluster_env = 2;
+    // default: pairs alone (clusters of 2 CTAs): all 66 clusters resident; multicast over 2 or 4 pairs costs residency
+    // (30 / 15 clusters) and measured slower (DESIGN 4.1)
+    cluster_env = e ? atoi(e) : 1;
+    if (cluster_env != 1 && cluster_env != 2 && cluster_env != 4) cluster_env = 1;
   }
   // an explicit launch configuration (the unit-test hook) overrides the environment
   a.stages = s.stages ? s.stages : stages_env;

@@ -125,6 +125,29 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
   asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa(smem_u32(bar), rank)) : "memory");
 }
+// same, also announcing `bytes` of asynchronous writes (complete_tx) that the current phase must wait for
+__device__ __forceinline__ void mbar_arrive_expect_tx_remote(uint64_t* bar, uint32_t rank, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;" ::"r"(mapa(smem_u32(bar), rank)), "r"(bytes)
+               : "memory");
+}
+// bulk copy (async proxy) of `bytes` of this CTA's shared memory to the same offset in CTA `rank`, completing on the
+// barrier at the same offset in that CTA.  The source must have been published to the async proxy
+// (fence.proxy.async.shared::cta by its writers, then a barrier that orders them before this thread)
+__device__ __forceinline__ void bulk_s2s_remote(const void* src, uint32_t bytes, uint64_t* bar, uint32_t rank) {
+  const uint32_t s = smem_u32(src);
+  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   mapa(s, rank)),
+               "r"(s), "r"(bytes), "r"(mapa(smem_u32(bar), rank))
+               : "memory");
+}
+// generic store to the same offset in CTA `rank` (publish with a .release.cluster arrive)
+__device__ __forceinline__ void st_remote_f32(float* p, uint32_t rank, float v) {
+  asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(mapa(smem_u32(p), rank)), "f"(v) : "memory");
+}
+// named barrier of `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // ---- TMA engine (non-tensor bulk copy) and proxy fence
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {

@@ -434,11 +434,12 @@ int fsn_debug_linear_tc(const float* x, int rows, int K, const float* W, const f
  * unit (b', f') of the drop_band map (G groups, as Model.forward applies them) gathers the reflected rows of its source
  * clip, scaled by inv2[clip] or, when unit_scale [steps, B*Fsub] is given, by unit_scale[t*R + r]; shrink > 1
  * down-samples time like fast_fullsubnet.  crm [B, 2, Fsub, steps - la] receives act(Linear) of steps la..steps-1
- * (outputs beyond fc_out are act(0)).  stages (2..4) and cluster (1, 2, 4) choose the launch configuration, 0 = the
- * FSN_TC_STAGES / FSN_TC_CLUSTER default.  Arguments are checked before any CUDA call. */
+ * (outputs beyond fc_out are act(0)).  stages (2..4) and cluster (1, 2, 4 CTA pairs that share each half's weight
+ * stream; a hardware cluster is 2 x cluster CTAs) choose the launch configuration, 0 = the FSN_TC_STAGES /
+ * FSN_TC_CLUSTER default.  Arguments are checked before any CUDA call. */
 size_t fsn_debug_sb_lstm_tc_packed_bytes(int H, int x3);
-/* *clusters = how many clusters of the sub-band kernel can be resident at once on the current device for that launch
- * configuration (cudaOccupancyMaxActiveClusters) */
+/* *clusters = how many clusters of the sub-band kernel (2 x cluster CTAs each) can be resident at once on the current
+ * device for that launch configuration (cudaOccupancyMaxActiveClusters) */
 int fsn_debug_sb_lstm_tc_max_clusters(int H, int x3, int stages, int cluster, int* clusters);
 int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
                          const float* magT, const float* fbT, int B, int F, int src_T, int G,

@@ -3,10 +3,12 @@ H = 384, precisions f16x3_tc and f16_tc, x FSN_TC_CLUSTER 1 / 2 / 4, x FSN_TC_ST
 
   python tools/tc_sweep.py [--precisions f16x3_tc,f16_tc] [--clusters 1,2,4] [--stages 2,3,4] [--batch 256] [--runs 2]
 
-The switches are read once per process, so every setting runs in a subprocess of its own.  Each setting prints the
-stage time from the library's stage events (fsn_set_profiling / fsn_last_stage_ms(2)), the time per ring stage in SM
-cycles next to the shared-memory budget of DESIGN 4.1, the resident clusters (cudaOccupancyMaxActiveClusters) and the
-waves they give, and the median SM clock sampled during the timed calls.  Card name and power limit are read once.
+The switches are read once per process, so every setting runs in a subprocess of its own.  FSN_TC_CLUSTER = CL is
+the number of CTA pairs that share each half's weight stream by multicast: a hardware cluster is 2 CL CTAs.  Each
+setting prints the stage time from the library's stage events (fsn_set_profiling / fsn_last_stage_ms(2)), the time per
+ring stage in SM cycles next to the shared-memory budget of DESIGN 4.1, the resident clusters
+(cudaOccupancyMaxActiveClusters) and the waves they give, and the median SM clock sampled during the timed calls.
+Card name and power limit are read once.
 """
 from __future__ import annotations
 
@@ -19,17 +21,18 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SR, HOP, CLIP_SECONDS, LA = 16000, 256, 4, 2
-H, NB, KS, W_TILE = 384, 16, 32, 32768
-A_BYTES = 64 * 16 * 2  # A operand of one m64n16k16 (weights), read from shared memory
-B_BYTES = 16 * 16 * 2  # B operand (state)
+H, NB, KS, W_TILE = 384, 32, 32, 16384  # NB rows per CTA pair; a stage is 4 gates x 64 units x 32 k of fp16
+A_BYTES = 64 * 16 * 2  # A operand of one m64n32k16 (weights), read from shared memory
+B_BYTES = 32 * 16 * 2  # B operand (state)
 SMEM_BYTES_PER_CLK = 128
 
 
 def shape(x3: bool):
-    """Ring stages, MMAs and shared-memory bytes per CTA and LSTM step (both layers, all 128-unit slices)."""
+    """Ring stages, MMAs and shared-memory bytes per CTA and LSTM step (both layers, the CTA's H / 128 slices of 64
+    hidden units: half of the units of its pair)."""
     mt, nkb = H // 128, (1 + H // KS) + 2 * H // KS
     stages = mt * nkb * (2 if x3 else 1)
-    mmas = mt * nkb * 16 * (3 if x3 else 1)  # 4 gates x 2 halves x 2 k16 per k range; X3: hi.hi, hi.lo, lo.hi
+    mmas = mt * nkb * 8 * (3 if x3 else 1)  # 4 gates x 2 k16 per k range; X3: hi.hi, hi.lo, lo.hi
     smem = stages * W_TILE + mmas * (A_BYTES + B_BYTES)
     return stages, mmas, smem
 
@@ -87,8 +90,8 @@ def main() -> None:
     print(f"# {name}, power limit {plimit} W, max SM clock {maxclk} MHz", flush=True)
     T = 1 + SR * CLIP_SECONDS // HOP
     steps = T + LA
-    ctas = -(-args.batch * 257 // NB)
-    print(f"# B = {args.batch} x {CLIP_SECONDS} s, {steps} LSTM steps, {ctas} CTAs of {NB} rows", flush=True)
+    pairs = -(-args.batch * 257 // NB)
+    print(f"# B = {args.batch} x {CLIP_SECONDS} s, {steps} LSTM steps, {pairs} CTA pairs of {NB} rows", flush=True)
     for prec in args.precisions.split(","):
         x3 = prec == "f16x3_tc"
         n_st, mmas, smem = shape(x3)
@@ -105,7 +108,7 @@ def main() -> None:
                     continue
                 r = json.loads(p.stdout.strip().splitlines()[-1])
                 ms = min(r["ms"])
-                clusters = -(-ctas // cl)
+                clusters = -(-pairs // cl)
                 waves = -(-clusters // r["resident_clusters"]) if r["resident_clusters"] > 0 else None
                 mhz = r["sm_mhz"] or float(maxclk)
                 cyc = ms * 1e-3 * mhz * 1e6 / (waves * steps * n_st) if waves else float("nan")
