@@ -61,6 +61,7 @@ class FastGrads(C.Structure):
 
 
 MAX_PARAM_TENSORS = 64
+SB_PROBE_FIELDS, SB_PROBE_SLOTS = 16, 4  # fsn_debug_sb_lstm_tc_probe records (FSN_SB_PROBE_FIELDS / _SLOTS)
 
 
 class ParamList(C.Structure):
@@ -155,6 +156,8 @@ _SIGNATURES = {
     "fsn_debug_sb_lstm_tc_max_clusters": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int)]),
     "fsn_debug_sb_lstm_tc": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _I,
                                        _I, _I, _I, _I, _P, _P, _P]),
+    "fsn_debug_sb_lstm_tc_probe": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P,
+                                             _I, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P]),
     "fsn_debug_tgemm": (C.c_int, [_P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _P, _L, _P]),
     "fsn_debug_tgemm_blocked": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _L, _P]),
     "fsn_debug_lstm_fwd_step": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _L, _P]),

@@ -304,6 +304,10 @@ struct SbTcArgs {
   bool x3;                // error-compensated variant (FSN_PREC_F16X3_TC image)
   RowMap map;
   int stages, cluster;    // weight ring depth (2..4) and CTAs per cluster (1, 2, 4); 0 = FSN_TC_STAGES / FSN_TC_CLUSTER
+  // non-null: run the cycle-stamp instantiation (fsn_debug_sb_lstm_tc_probe) for CTAs [0, stamp_ctas) and loop
+  // iterations [0, stamp_its); the production launches leave it null
+  long long* stamps;
+  int stamp_ctas, stamp_its;
 };
 size_t sb_tc_packed_bytes(const fsn_model_desc* d);
 size_t sb_tc_packed_bytes_raw(int H, bool x3);

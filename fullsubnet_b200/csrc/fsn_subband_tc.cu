@@ -181,6 +181,12 @@ struct RowInfo {
   int out_idx;        // crm index of (b', o=0, f', t=0) divided by T  (= (b'*2)*Fsub + f')
 };
 
+// The kernel takes KArgs as a __grid_constant__ parameter: its fields stay in parameter (constant-bank) space and are
+// read where they are used.  Passed as a plain by-value struct of at most 128 bytes, the front end instead loads every
+// field into a register at kernel entry and keeps it live through the whole kernel; in the x3 kernel, whose consumers
+// already need nearly all of their 152 registers, that costs 248 / 434 bytes of spill stores / loads (184-byte stack
+// frame) against 64 / 84 (48-byte frame), and 8 / 12 against 0 in the single pass - about 17 % of the headline step
+// (DESIGN 4.1).  tests/test_cpu_subband_resources.py checks the frames of the built library.
 struct KArgs {
   const uint8_t* packed;
   const float* magT; const float* fbT; const float* inv2;
@@ -189,7 +195,44 @@ struct KArgs {
   int R, F, Tp, la, T, Ns, Nf, H, Ksb, act, Fsub, stages, cluster;
   int src_T, shrink;  // frames in magT/fbT; x_t = mean of `shrink` source frames (fast_fullsubnet down-sampling), 1 = none
   RowMap map;
+  long long* stamps;  // PROBE instantiation only: records of CTAs [0, stamp_ctas), iterations [0, stamp_its)
+  int stamp_ctas, stamp_its;
 };
+
+// ---------------------------------------------------------------- cycle stamps (PROBE instantiation)
+// One record of PROBE_FIELDS int64 per (CTA, loop iteration it, layer, slot): slots 0 .. MAX_MT-1 are the consumer
+// warpgroups (block = that warpgroup's MMAs and cell of one layer; layer 1 of iteration it is step it - 1), slot MAX_MT
+// is the weight producer (layer-0 record of each iteration, the stages it streams in that iteration).  Durations are
+// SM cycles (clock64) summed over the block, as seen by thread 0 of the warpgroup / warp.
+enum ProbeField {
+  PF_T_BEGIN = 0,   // clock64 at block start, before the operand waits
+  PF_T_MMA0 = 1,    // first stage may be waited on (operand and turn waits done)
+  PF_T_MMA1 = 2,    // every MMA of the block retired (wait_group 0)
+  PF_T_END = 3,     // h written and the copy to the peer issued
+  PF_OPERAND = 4,   // waits on x_full / h0_ready / h1_ready (producer: w_empty waits)
+  PF_TURN = 5,      // wait on turn[m]
+  PF_W_FULL = 6,    // waits on w_full (stages landing)
+  PF_WAIT_GROUP = 7,// wgmma.wait_group
+  PF_GROUP_LAT = 8, // sum over the stage groups of commit -> return of the wait_group that retires the group
+                    // (after the NEXT stage's w_full wait and MMA issue: an upper bound on the retire latency)
+  PF_STAGES = 9,    // ring stages of the block
+  PF_CELL = 10,     // cell math, h stores, exchange issue (waits excluded)
+  PF_L1_DONE = 11,  // wait on l1_done
+  PF_H1_EMPTY = 12, // wait on h1_empty
+  PF_H0_EMPTY = 13, // wait on h0_empty
+  PF_FC_DONE = 14,  // wait on fc_done
+  PF_GT_BEGIN = 15, // globaltimer (ns) at block start
+  PROBE_FIELDS = 16
+};
+constexpr int PROBE_SLOTS = MAX_MT + 1;
+static_assert(PROBE_FIELDS == FSN_SB_PROBE_FIELDS && PROBE_SLOTS == FSN_SB_PROBE_SLOTS,
+              "probe record layout differs from fsn_b200.h (and fullsubnet_b200/_lib.py)");
+
+__device__ __forceinline__ long long globaltimer() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return (long long)t;
+}
 
 __device__ __forceinline__ float act_apply(float v, int act) {
   switch (act) {
@@ -218,9 +261,27 @@ __device__ __forceinline__ void release_stage(uint64_t* bar, int CL, int half, i
   else mbar_arrive_remote(bar, (uint32_t)(2 * q + half));
 }
 
-template <bool X3>
-__global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) {
+// PROBE: the same kernel with cycle stamps (ProbeField) written to a.stamps; the production launches use PROBE = false,
+// where every stamp below compiles away
+template <bool X3, bool PROBE>
+__global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_constant__ KArgs a) {
   constexpr int PARTS = X3 ? 2 : 1;
+  // probe clock: cycles since the previous mark (0 and no code without PROBE)
+  long long pt = 0;
+  auto mark = [&]() -> uint32_t {
+    if constexpr (PROBE) {
+      const long long n = clock64();
+      const uint32_t d = (uint32_t)(n - pt);
+      pt = n;
+      return d;
+    } else {
+      return 0u;
+    }
+  };
+  auto record = [&](int it, int layer, int slot) -> long long* {
+    return a.stamps + ((((size_t)blockIdx.x * a.stamp_its + it) * 2 + layer) * PROBE_SLOTS + slot) * PROBE_FIELDS;
+  };
+  const bool probe_cta = PROBE && (int)blockIdx.x < a.stamp_ctas;
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzle atoms need 1024-byte alignment in the shared window
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -294,9 +355,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
       const size_t t_begin = (it < Tp) ? 0 : PL.tiles0;
       const size_t t_end = (it >= 1) ? PL.tiles0 + PL.tiles1 : PL.tiles0;
       const uint8_t* src = stream + t_begin * W_TILE;
+      long long p_t0 = 0, p_g0 = 0;
+      uint32_t p_empty = 0;
+      if constexpr (PROBE) { p_g0 = globaltimer(); p_t0 = clock64(); pt = p_t0; }
       for (size_t tile = t_begin; tile < t_end; ++tile, src += W_TILE) {
         // all CL CTAs' consumers have drained this stage (on the critical path: no back-off)
+        mark();
         mbar_wait_cta<false>(&bars.w_empty[stage], phase ^ 1);
+        p_empty += mark();
         if (elect_one()) {
           mbar_expect_tx(&bars.w_full[stage], W_TILE);
           if (CL == 1) {
@@ -308,6 +374,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
         }
         __syncwarp();
         if (++stage == (uint32_t)STAGES) { stage = 0; phase ^= 1; }
+      }
+      if (probe_cta && it < a.stamp_its && lane == 0) {
+        long long* r = record(it, 0, MAX_MT);
+        r[PF_T_BEGIN] = p_t0; r[PF_T_END] = clock64(); r[PF_OPERAND] = p_empty;
+        r[PF_STAGES] = (long long)(t_end - t_begin); r[PF_GT_BEGIN] = p_g0;
       }
     }
   } else if (warp == 2) {
@@ -422,6 +493,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
         for (int layer = 0; layer < 2; ++layer) {
           const int t = it - layer;
           if (t < 0 || t >= Tp) continue;
+          // probe: block start, then the waits and phases of the block (ProbeField)
+          long long p_t0 = 0, p_g0 = 0, p_mma0 = 0, p_mma1 = 0, p_commit = 0, p_commit_prev = 0;
+          uint32_t p_opnd = 0, p_turn = 0, p_wfull = 0, p_wgw = 0, p_lat = 0, p_cell = 0, p_l1 = 0, p_h1e = 0, p_h0e = 0,
+                   p_fc = 0;
+          if constexpr (PROBE) { p_g0 = globaltimer(); p_t0 = clock64(); pt = p_t0; }
           // operands of this step complete in shared memory (every phase waited on once, in order).  All of this
           // kernel's waits on the weight ring and the state are CTA-scope: each of those barriers guards data written
           // by this CTA or by an async-proxy copy with complete_tx (TMA from L2, the peer's DSMEM bulk copy)
@@ -432,6 +508,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
             for (; h0_seen < t + 1; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready[h0_seen & 1], (h0_seen >> 1) & 1);  // h0_t
             for (; h1_seen < t; ++h1_seen) mbar_wait_cta<false>(&bars.h1_ready, h1_seen & 1);                          // h1_{t-1}
           }
+          p_opnd += mark();
           const uint32_t x_addr = smem_u32(smem + sp.x + (t & 1) * X_BLK);
           const uint32_t h0_cur = smem_u32(smem + sp.h0 + (t & 1) * nkh * S_KBLK);        // h0_t
           const uint32_t h0_prev = smem_u32(smem + sp.h0 + ((t + 1) & 1) * nkh * S_KBLK);  // h0_{t-1}
@@ -449,6 +526,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
           int prev_stage = -1;
           if (m > 0 || !first_block) { mbar_wait_cta<false>(&bars.turn[m], turns & 1); ++turns; }
           first_block = false;
+          p_turn += mark();
+          p_mma0 = pt;
           // ring slot and fill parity of stream stage `first`, then advanced stage by stage
           int stage = (int)(first % (size_t)STAGES);
           uint32_t wphase = (uint32_t)((first / (size_t)STAGES) & 1);
@@ -461,7 +540,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
                                    : h1_prev + ((j - H / KS) >> 1) * S_KBLK + ((j - H / KS) & 1) * 64;
 #pragma unroll
             for (int part = 0; part < PARTS; ++part) {
+              mark();
               mbar_wait_cta<false>(&bars.w_full[stage], wphase);
+              p_wfull += mark();
               if (j == nkb - 1 && part == PARTS - 1 && lane == 0) mbar_arrive(&bars.turn[m + 1 < MT ? m + 1 : 0]);
               wg::fence();
               const uint32_t wa = wbase + stage * W_TILE;
@@ -477,15 +558,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
                 }
               }
               wg::commit();
+              if constexpr (PROBE) p_commit = clock64();
+              mark();
               wg::wait<1>();  // the MMAs of the previous stage have read it
+              p_wgw += mark();
+              if constexpr (PROBE) {
+                if (prev_stage >= 0) p_lat += (uint32_t)(pt - p_commit_prev);
+                p_commit_prev = p_commit;
+              }
               if (prev_stage >= 0) release_stage(&bars.w_empty[prev_stage], CL, half, q, lane);
               prev_stage = stage;
               if (++stage == STAGES) { stage = 0; wphase ^= 1; }
             }
           }
+          mark();
           wg::wait<0>();
 #pragma unroll
           for (int g = 0; g < 4; ++g) wg::fence_operand(acc[g]);
+          p_wgw += mark();
+          if constexpr (PROBE) { p_lat += (uint32_t)(pt - p_commit_prev); p_mma1 = pt; }
           release_stage(&bars.w_empty[prev_stage], CL, half, q, lane);
           // this warpgroup's MMAs of the step have consumed x_t / h1_{t-1}
           if (lane == 0) mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
@@ -494,7 +585,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
             if (q == 2) mbar_arrive_remote(&bars.h0_empty[t & 1], peer);
             if (q == 3) mbar_arrive_remote(&bars.h1_empty, peer);
           }
+          p_cell += mark();
           if (layer == 1 && t >= 1) mbar_wait_cta<false>(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
+          p_fc += mark();
           float fsum[2][8];  // Linear partials [o][row slot j*2+e]
 #pragma unroll
           for (int i = 0; i < 16; ++i) fsum[i >> 3][i & 7] = 0.f;
@@ -541,14 +634,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
 #pragma unroll
                 for (int r = 0; r < 8; ++r) my_part[o * NB + 8 * (r >> 1) + 2 * lane + (r & 1)] = fsum[o][r];
             }
+            p_cell += mark();
             // every layer-1 MMA of this step in this CTA has consumed h1_{t-1}: overwrite it with h1_t
             mbar_wait_cta<false>(&bars.l1_done, t & 1);
+            p_l1 += mark();
             // ... and in the peer, which also means the peer holds this slice's h1_{t-1} copy: its source may go
             mbar_wait_cta<false>(&bars.h1_empty, t & 1);
+            p_h1e += mark();
           } else if (t >= 2) {
+            p_cell += mark();
             // the peer's layer-1 MMAs of step t-2 have read h0_{t-2} in buffer t & 1 (and so this slice's copy of it
             // has landed there); this CTA's own readers of the buffer are ordered by the ring turn (DESIGN 4.1)
             mbar_wait_cta<false>(&bars.h0_empty[t & 1], ((t - 2) >> 1) & 1);
+            p_h0e += mark();
           }
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
@@ -575,6 +673,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const KArgs a) 
             mbar_arrive_expect_tx_remote(ready, peer, PARTS * S_KBLK);
             bulk_s2s_remote(hb, S_KBLK, ready, peer);
             if (X3) bulk_s2s_remote(hb + LO, S_KBLK, ready, peer);
+          }
+          if constexpr (PROBE) {
+            p_cell += mark();
+            if (probe_cta && it < a.stamp_its && q == 0 && lane == 0) {
+              long long* r = record(it, layer, m);
+              r[PF_T_BEGIN] = p_t0; r[PF_T_MMA0] = p_mma0; r[PF_T_MMA1] = p_mma1; r[PF_T_END] = pt;
+              r[PF_OPERAND] = p_opnd; r[PF_TURN] = p_turn; r[PF_W_FULL] = p_wfull; r[PF_WAIT_GROUP] = p_wgw;
+              r[PF_GROUP_LAT] = p_lat; r[PF_STAGES] = nkb * PARTS; r[PF_CELL] = p_cell; r[PF_L1_DONE] = p_l1;
+              r[PF_H1_EMPTY] = p_h1e; r[PF_H0_EMPTY] = p_h0e; r[PF_FC_DONE] = p_fc; r[PF_GT_BEGIN] = p_g0;
+            }
           }
         }
         tile_base += ((it < Tp) ? PL.tiles0 : 0) + ((it >= 1) ? PL.tiles1 : 0);
@@ -626,12 +734,12 @@ int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed,
 
 // launch configuration of `pairs` CTA pairs in clusters of `cluster` pairs (2 x cluster CTAs; the caller keeps `attr`
 // alive while cfg is used)
-template <bool X3>
+template <bool X3, bool PROBE = false>
 static int sb_tc_config(int H, int stages, int cluster, int pairs, cudaStream_t st, cudaLaunchConfig_t& cfg,
                         cudaLaunchAttribute* attr) {
   const tc::Smem sp = tc::smem_plan(H, stages, X3);
   const size_t smem = sp.total + 1024;  // slack for the 1024-byte alignment of the dynamic segment
-  int rc = check_cuda(cudaFuncSetAttribute(tc::sb_lstm_tc_kernel<X3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  int rc = check_cuda(cudaFuncSetAttribute(tc::sb_lstm_tc_kernel<X3, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)smem), "sb_lstm_tc smem attr");
   if (rc) return rc;
   memset(&cfg, 0, sizeof(cfg));
@@ -648,14 +756,14 @@ static int sb_tc_config(int H, int stages, int cluster, int pairs, cudaStream_t 
   return FSN_OK;
 }
 
-template <bool X3>
+template <bool X3, bool PROBE>
 static int sb_tc_launch(const tc::KArgs& a, int H, cudaStream_t st) {
   const int pairs = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;  // padding pairs own no valid row
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
-  int rc = sb_tc_config<X3>(H, a.stages, a.cluster, pairs, st, cfg, attr);
+  int rc = sb_tc_config<X3, PROBE>(H, a.stages, a.cluster, pairs, st, cfg, attr);
   if (rc) return rc;
-  rc = check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_lstm_tc_kernel<X3>, a), "sb_lstm_tc_kernel launch");
+  rc = check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_lstm_tc_kernel<X3, PROBE>, a), "sb_lstm_tc_kernel launch");
   if (rc) return rc;
   FSN_CHECK_LAUNCH("sb_lstm_tc_kernel");
   return FSN_OK;
@@ -669,6 +777,7 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
   a.src_T = s.Tp; a.shrink = s.shrink > 1 ? s.shrink : 1;
   a.Ns = s.Ns; a.Nf = s.Nf; a.H = s.H; a.Ksb = (2 * s.Ns + 1) + (2 * s.Nf + 1); a.act = s.act;
   a.Fsub = s.map.Fsub; a.map = s.map;
+  a.stamps = s.stamps; a.stamp_ctas = s.stamp_ctas; a.stamp_its = s.stamp_its;
   FSN_REQUIRE(sb_tc_shape_ok(a.H, a.Ksb), FSN_ERR_UNSUPPORTED, "sb_lstm_tc: unsupported hidden size %d / input width %d",
               a.H, a.Ksb);
   static int stages_env = -1;
@@ -689,7 +798,8 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
   // an explicit launch configuration (the unit-test hook) overrides the environment
   a.stages = s.stages ? s.stages : stages_env;
   a.cluster = s.cluster ? s.cluster : cluster_env;
-  return s.x3 ? sb_tc_launch<true>(a, s.H, st) : sb_tc_launch<false>(a, s.H, st);
+  if (s.stamps) return s.x3 ? sb_tc_launch<true, true>(a, s.H, st) : sb_tc_launch<false, true>(a, s.H, st);
+  return s.x3 ? sb_tc_launch<true, false>(a, s.H, st) : sb_tc_launch<false, false>(a, s.H, st);
 }
 
 }  // namespace fsn
@@ -712,14 +822,14 @@ extern "C" int fsn_debug_sb_lstm_tc_max_clusters(int H, int x3, int stages, int 
   int rc = x3 ? sb_tc_config<true>(H, stages, cluster, cluster, nullptr, cfg, attr)
               : sb_tc_config<false>(H, stages, cluster, cluster, nullptr, cfg, attr);
   if (rc) return rc;
-  return x3 ? check_cuda(cudaOccupancyMaxActiveClusters(clusters, tc::sb_lstm_tc_kernel<true>, &cfg), "sb_lstm_tc occupancy")
-            : check_cuda(cudaOccupancyMaxActiveClusters(clusters, tc::sb_lstm_tc_kernel<false>, &cfg), "sb_lstm_tc occupancy");
+  return x3 ? check_cuda(cudaOccupancyMaxActiveClusters(clusters, tc::sb_lstm_tc_kernel<true, false>, &cfg), "sb_lstm_tc occupancy")
+            : check_cuda(cudaOccupancyMaxActiveClusters(clusters, tc::sb_lstm_tc_kernel<false, false>, &cfg), "sb_lstm_tc occupancy");
 }
 
-extern "C" int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
-                                    const float* magT, const float* fbT, int B, int F, int src_T, int G,
-                                    const float* inv2, const float* unit_scale, int la, int steps, int shrink, int stages,
-                                    int cluster, void* packed, float* crm, fsn_stream_t stream) {
+static int sb_lstm_tc_hook(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
+                           const float* magT, const float* fbT, int B, int F, int src_T, int G, const float* inv2,
+                           const float* unit_scale, int la, int steps, int shrink, int stages, int cluster, void* packed,
+                           float* crm, long long* stamps, int stamp_ctas, int stamp_steps, fsn_stream_t stream) {
   using namespace fsn;
   // every check precedes the first CUDA call
   FSN_REQUIRE(cluster == 0 || cluster == 1 || cluster == 2 || cluster == 4, FSN_ERR_UNSUPPORTED,
@@ -744,6 +854,14 @@ extern "C" int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, in
   FSN_REQUIRE(!(unit_scale && shrink > 1), FSN_ERR_UNSUPPORTED, "sb_lstm_tc: per-step scales with time down-sampling");
   FSN_REQUIRE(sb_tc_shape_ok(H, (2 * Ns + 1) + (2 * Nf + 1)), FSN_ERR_UNSUPPORTED,
               "sb_lstm_tc: unsupported hidden size %d / input width %d", H, (2 * Ns + 1) + (2 * Nf + 1));
+  if (stamps) {
+    // records exist for CTAs that own rows and for the loop iterations 0 .. steps (layer 1 runs one behind)
+    const int ctas = 2 * cdiv(B * Fsub, tc::NB);
+    FSN_REQUIRE(stamp_ctas >= 1 && stamp_ctas <= ctas, FSN_ERR_SHAPE, "sb_lstm_tc probe: %d sampled CTAs (1 .. %d)",
+                stamp_ctas, ctas);
+    FSN_REQUIRE(stamp_steps >= 1 && stamp_steps <= steps + 1, FSN_ERR_SHAPE,
+                "sb_lstm_tc probe: %d sampled iterations (1 .. steps + 1 = %d)", stamp_steps, steps + 1);
+  }
   cudaStream_t st = (cudaStream_t)stream;
   int rc = sb_tc_pack_raw(sb, H, (2 * Ns + 1) + (2 * Nf + 1), fc_out, packed, st, x3 != 0);
   if (rc) return rc;
@@ -754,5 +872,25 @@ extern "C" int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, in
   a.steps = steps; a.shrink = shrink; a.x3 = x3 != 0;
   a.map = RowMap{B, F, Fsub, g};
   a.stages = stages; a.cluster = cluster;
+  a.stamps = stamps; a.stamp_ctas = stamp_ctas; a.stamp_its = stamp_steps;
   return sb_tc_forward(a, st);
+}
+
+extern "C" int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
+                                    const float* magT, const float* fbT, int B, int F, int src_T, int G,
+                                    const float* inv2, const float* unit_scale, int la, int steps, int shrink, int stages,
+                                    int cluster, void* packed, float* crm, fsn_stream_t stream) {
+  return sb_lstm_tc_hook(sb, H, Ns, Nf, fc_out, act, x3, magT, fbT, B, F, src_T, G, inv2, unit_scale, la, steps, shrink,
+                         stages, cluster, packed, crm, nullptr, 0, 0, stream);
+}
+
+extern "C" int fsn_debug_sb_lstm_tc_probe(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
+                                          const float* magT, const float* fbT, int B, int F, int src_T, int G,
+                                          const float* inv2, const float* unit_scale, int la, int steps, int shrink,
+                                          int stages, int cluster, void* packed, float* crm, long long* stamps,
+                                          int stamp_ctas, int stamp_steps, fsn_stream_t stream) {
+  using namespace fsn;
+  FSN_REQUIRE(stamps, FSN_ERR_SHAPE, "sb_lstm_tc probe: missing stamp buffer");
+  return sb_lstm_tc_hook(sb, H, Ns, Nf, fc_out, act, x3, magT, fbT, B, F, src_T, G, inv2, unit_scale, la, steps, shrink,
+                         stages, cluster, packed, crm, stamps, stamp_ctas, stamp_steps, stream);
 }

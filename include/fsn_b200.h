@@ -445,6 +445,21 @@ int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int f
                          const float* magT, const float* fbT, int B, int F, int src_T, int G,
                          const float* inv2, const float* unit_scale, int la, int steps, int shrink,
                          int stages, int cluster, void* packed, float* crm, fsn_stream_t stream);
+/* the same run through the cycle-stamp instantiation of the kernel (same output bits): CTAs [0, stamp_ctas) (at most
+ * the 2 * ceil(B * Fsub / 32) CTAs that own rows) record, for the loop iterations [0, stamp_steps) (stamp_steps <=
+ * steps + 1: layer 1 runs one iteration behind layer 0), FSN_SB_PROBE_FIELDS int64 per (CTA, iteration, layer, slot)
+ * into stamps [stamp_ctas, stamp_steps, 2, FSN_SB_PROBE_SLOTS, FSN_SB_PROBE_FIELDS]: slots 0..2 are the consumer
+ * warpgroups (SM clock stamps of the block's start, MMA start, MMA end and end, then the cycles spent in each wait and
+ * in the cell; field order in fsn_subband_tc.cu, ProbeField), slot 3 the weight producer (layer-0 record of each
+ * iteration).  Records of blocks that do not exist (layer 1 of iteration 0, layer 0 of the last, slots beyond H / 128)
+ * are left as they were.  Arguments are checked before any CUDA call. */
+#define FSN_SB_PROBE_FIELDS 16
+#define FSN_SB_PROBE_SLOTS 4
+int fsn_debug_sb_lstm_tc_probe(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
+                               const float* magT, const float* fbT, int B, int F, int src_T, int G,
+                               const float* inv2, const float* unit_scale, int la, int steps, int shrink,
+                               int stages, int cluster, void* packed, float* crm, long long* stamps, int stamp_ctas,
+                               int stamp_steps, fsn_stream_t stream);
 
 /* unit-test hook for the LSTM layer shared by the training steps (fsn_train.cu): torch.nn.LSTM(K0, H, num_layers =
  * n_layers) over x [T,R,K0] (time-major) through the same activation-saving forward, BPTT and weight-gradient pieces

@@ -1,0 +1,133 @@
+// Stand-alone rate of the sub-band kernel's MMA sequence (DESIGN 4.1): m64n32k16 wgmma with both operands in shared
+// memory, issued per ring stage exactly as sb_lstm_tc_kernel issues them (x3: a hi stage of 16 MMAs - hi.hi, hi.lo per
+// gate and k16 - then a lo stage of 8; single pass: 8), one commit per stage, then wait_group<WAIT>.  1, 2 or 3
+// consumer warpgroups issue at once, each on its own 16 KB A block (same 64B swizzle as the weight stages) against one
+// shared 128B-swizzled B block (hi + lo); optionally warp 0 streams 16 KB bulk copies from L2 into a 4-slot ring of
+// its own at the same time.  No barriers between the consumers; operands are zero.  132 CTAs, one per SM.
+//
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o /tmp/mma_rate tools/mma_rate.cu && /tmp/mma_rate
+//
+// Prints per configuration the cycles per stage of one warpgroup and the per-SM cycles per MMA.
+#include <cuda_runtime.h>
+#include <stdio.h>
+
+#include "../fullsubnet_b200/csrc/fsn_tc_ptx.cuh"
+#include "../fullsubnet_b200/csrc/fsn_wgmma.cuh"
+using namespace fsn;
+using namespace fsn::ptx;
+
+constexpr int GRID = 132, ITERS = 2000, SMEM = 200 * 1024;
+
+// ORDER 0: per gate hi.hi then hi.lo (the kernel's order); 1: the four hi.hi before the four hi.lo
+template <bool X3, int ORDER, int WAIT>
+__global__ void __launch_bounds__(512, 1) mma_rate(int nwg, int prod, long long* out, const uint8_t* gsrc) {
+  extern __shared__ uint8_t raw[];
+  uint8_t* sm = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + 120 * 1024);
+  for (int i = threadIdx.x; i < 120 * 1024 / 16; i += blockDim.x) reinterpret_cast<uint4*>(sm)[i] = make_uint4(0, 0, 0, 0);
+  if (threadIdx.x == 0)
+    for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
+  fence_proxy_async_smem();
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp < 4) {
+    if (warp == 0 && prod) {  // one 16 KB bulk copy per stage the consumers run, 4 in flight
+      const int n = nwg * ITERS * (X3 ? 2 : 1);
+      const long long t0 = clock64();
+      for (int i = 0; i < n + 4; ++i) {
+        const int s = i & 3;
+        if (i >= 4) mbar_wait_cta<false>(&bars[s], ((i >> 2) - 1) & 1);
+        if (i < n && elect_one()) {
+          mbar_expect_tx(&bars[s], 16384);
+          bulk_g2s(sm + 56 * 1024 + s * 16384, gsrc + (size_t)(i % 64) * 16384, 16384, &bars[s]);
+        }
+        __syncwarp();
+      }
+      if (lane == 0) out[blockIdx.x * 8 + 7] = clock64() - t0;
+    }
+    return;
+  }
+  const int m = (warp - 4) >> 2;
+  if (m >= nwg) return;
+  const uint32_t wa = smem_u32(sm + m * 16384), sb = smem_u32(sm + 48 * 1024);
+  float acc[4][16];
+#pragma unroll
+  for (int g = 0; g < 4; ++g) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[g][i] = 0.f;
+    wg::fence_operand(acc[g]);
+  }
+  named_sync(1 + m, 128);
+  const long long t0 = clock64();
+  for (int it = 0; it < ITERS; ++it) {
+#pragma unroll
+    for (int part = 0; part < (X3 ? 2 : 1); ++part) {
+      wg::fence();
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) {
+        const uint64_t bd = wg::desc_sw128(sb + kk * 32), bl = wg::desc_sw128(sb + 4096 + kk * 32);
+        if (ORDER == 0 || !X3 || part == 1) {
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {
+            const uint64_t ad = wg::desc_sw64(wa + g * 4096 + kk * 32);
+            wg::mma_f16_n32(acc[g], ad, bd, 1u);
+            if (X3 && part == 0) wg::mma_f16_n32(acc[g], ad, bl, 1u);
+          }
+        } else {
+#pragma unroll
+          for (int g = 0; g < 4; ++g) wg::mma_f16_n32(acc[g], wg::desc_sw64(wa + g * 4096 + kk * 32), bd, 1u);
+#pragma unroll
+          for (int g = 0; g < 4; ++g) wg::mma_f16_n32(acc[g], wg::desc_sw64(wa + g * 4096 + kk * 32), bl, 1u);
+        }
+      }
+      wg::commit();
+      wg::wait<WAIT>();
+    }
+  }
+  wg::wait<0>();
+#pragma unroll
+  for (int g = 0; g < 4; ++g) wg::fence_operand(acc[g]);
+  const long long t1 = clock64();
+  float s = 0.f;
+#pragma unroll
+  for (int g = 0; g < 4; ++g)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) s += acc[g][i];
+  if ((threadIdx.x & 127) == 0) out[blockIdx.x * 8 + m] = (t1 - t0) + (s != 0.f ? 1 : 0);
+}
+
+template <bool X3, int ORDER, int WAIT>
+static void run(const char* name, long long* d_out, const uint8_t* gsrc) {
+  cudaFuncSetAttribute(mma_rate<X3, ORDER, WAIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+  for (int prod = 0; prod < 2; ++prod)
+    for (int nwg = 1; nwg <= 3; ++nwg) {
+      cudaMemset(d_out, 0, GRID * 8 * sizeof(long long));
+      mma_rate<X3, ORDER, WAIT><<<GRID, 512, SMEM>>>(nwg, prod, d_out, gsrc);
+      const cudaError_t e = cudaDeviceSynchronize();
+      long long h[GRID * 8];
+      cudaMemcpy(h, d_out, sizeof(h), cudaMemcpyDeviceToHost);
+      double cyc = 0;
+      for (int b = 0; b < GRID; ++b)
+        for (int m = 0; m < nwg; ++m) cyc += (double)h[b * 8 + m] / (GRID * nwg);
+      const int stages = ITERS * (X3 ? 2 : 1), mmas = ITERS * (X3 ? 24 : 8);
+      printf("%-12s TMA stream %d, %d warpgroup(s): %s  %6.1f cycles per stage and warpgroup, %5.1f cycles per MMA per SM\n",
+             name, prod, nwg, cudaGetErrorString(e), cyc / stages, cyc / ((double)mmas * nwg));
+    }
+}
+
+int main() {
+  long long* d_out;
+  uint8_t* gsrc;
+  cudaMalloc(&d_out, GRID * 8 * sizeof(long long));
+  cudaMalloc(&gsrc, 64 * 16384);
+  cudaMemset(gsrc, 0, 64 * 16384);
+  run<true, 0, 1>("x3 wait<1>", d_out, gsrc);
+  run<true, 1, 1>("x3 hh-first", d_out, gsrc);
+  run<true, 1, 2>("x3 wait<2>", d_out, gsrc);
+  run<true, 0, 0>("x3 wait<0>", d_out, gsrc);
+  run<false, 0, 1>("f16 wait<1>", d_out, gsrc);
+  run<false, 0, 0>("f16 wait<0>", d_out, gsrc);
+  cudaFree(d_out);
+  cudaFree(gsrc);
+  return 0;
+}
