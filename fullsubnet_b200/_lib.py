@@ -88,11 +88,15 @@ class ImprovedDesc(C.Structure):
                 ("sb_num_center", C.c_int32 * IMP_MAX_SECTIONS), ("sb_num_neighbor", C.c_int32 * IMP_MAX_SECTIONS),
                 ("fb_num_center", C.c_int32 * IMP_MAX_SECTIONS), ("fb_num_neighbor", C.c_int32 * IMP_MAX_SECTIONS),
                 ("fb_hidden", C.c_int32), ("sb_hidden", C.c_int32), ("fb_activation", C.c_int32),
-                ("sb_activation", C.c_int32), ("precision", C.c_int32)]
+                ("sb_activation", C.c_int32), ("precision", C.c_int32), ("cell_type", C.c_int32)]
 
 
 class ImprovedWeights(C.Structure):
     _fields_ = [("fb", SeqWeights), ("sb", SeqWeights * IMP_MAX_SECTIONS)]
+
+
+class ImprovedGrads(C.Structure):
+    _fields_ = [("fb", SeqGrads), ("sb", SeqGrads * IMP_MAX_SECTIONS)]
 
 
 _P, _I, _L, _F, _S = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
@@ -123,6 +127,11 @@ _SIGNATURES = {
     "fsn_improved_workspace_bytes": (_S, [C.POINTER(ImprovedDesc), _I, _I]),
     "fsn_improved_forward": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _I, _I, _P, _P, _P, _S,
                                        _P]),
+    "fsn_improved_train_workspace_bytes": (_S, [C.POINTER(ImprovedDesc), _I, _I]),
+    "fsn_improved_train_forward": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _I, _I, _P, _P, _S,
+                                             _P]),
+    "fsn_improved_train_backward": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _I, _I,
+                                              C.POINTER(ImprovedGrads), _P, _S, _P]),
     "fsn_train_workspace_bytes": (_S, [C.POINTER(ModelDesc), _I, _I]),
     "fsn_train_forward": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _I, _I, _P,
                                     _P, _S, _P]),

@@ -218,6 +218,57 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
   }
 }
 
+// Adjoint of (element-wise mask, irfft, window, overlap-add, envelope, crop) with respect to the mask, same tiling as
+// stft_kernel (kFR frames per CTA, two real frames per complex transform): frame t's samples g(t*hop + i) * win[i] go
+// through the forward real DFT; irfft's adjoint scales bin k by c_k/n (c = 1 at DC, 2 at bins 1 .. n/2-1, the
+// Im of DC gets no gradient), and the product with the kept spectrum gives dcrm[b,0,k,t] = dRe * real,
+// dcrm[b,1,k,t] = dIm * imag for k < F-1.
+__global__ void __launch_bounds__(kDspThreads)
+istft_mask_adjoint_kernel(const float* __restrict__ dwav, const float* __restrict__ real, const float* __restrict__ imag,
+                          int L, int n, int hop, int win_length, int T, float* __restrict__ dcrm) {
+  extern __shared__ float2 smem2[];
+  const int log2n = ilog2(n);
+  const int zstride = n + 1;
+  constexpr int NP = kFR / 2;
+  float2* z = smem2;
+  float2* tw = z + NP * zstride;
+  float* win = reinterpret_cast<float*>(tw + n / 2);
+  const int b = blockIdx.y;
+  const int t0 = blockIdx.x * kFR;
+  const int F = n / 2 + 1;
+  init_tables(tw, win, n, win_length);
+  __syncthreads();
+  const float* g = dwav + (size_t)b * L;
+  for (int idx = threadIdx.x; idx < NP * n; idx += blockDim.x) {
+    const int p = idx >> log2n;
+    const int i = idx & (n - 1);
+    const int ta = t0 + 2 * p, tb = ta + 1;
+    const float w = win[i];
+    float va = 0.f, vb = 0.f;
+    if (ta < T) va = istft_adjoint_sample(g, win, ta * hop + i, n, hop, T, L) * w;
+    if (tb < T) vb = istft_adjoint_sample(g, win, tb * hop + i, n, hop, T, L) * w;
+    z[p * zstride + (int)(__brev((unsigned)i) >> (32 - log2n))] = make_float2(va, vb);
+  }
+  __syncthreads();
+  fft_radix2_smem<false>(z, zstride, NP, n, log2n, tw);
+  const size_t plane = (size_t)F * T;
+  for (int idx = threadIdx.x; idx < (F - 1) * kFR; idx += blockDim.x) {
+    const int k = idx / kFR;
+    const int j = idx - k * kFR;
+    const int t = t0 + j;
+    if (t >= T) continue;
+    const float2 zk = z[(j >> 1) * zstride + k];
+    const float2 zn = z[(j >> 1) * zstride + ((n - k) & (n - 1))];
+    float re, im;
+    if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
+    else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+    const float sc = (k == 0 ? 1.f : 2.f) / (float)n;
+    const size_t o = (size_t)b * plane + (size_t)k * T + t;
+    dcrm[(size_t)b * plane + o] = sc * re * real[o];
+    dcrm[(size_t)b * plane + plane + o] = k == 0 ? 0.f : sc * im * imag[o];
+  }
+}
+
 // out = int16(gain * wav / peak) per clip, peak from the iSTFT epilogue (float32 mul, div, truncation like numpy)
 __global__ void scale_int16_kernel(const float* __restrict__ wav, const unsigned int* __restrict__ peak_bits, int L, float gain,
                                    int16_t* __restrict__ out, size_t n) {
@@ -344,6 +395,8 @@ int stft_dft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_
                     float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st);
 int istft_dft_launch(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B, int T,
                      int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st);
+int istft_mask_adjoint_dft_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
+                                  int hop, int win_length, float* dcrm, cudaStream_t st);
 static bool dft_size_ok(int n) { return !is_pow2(n) && (n & 1) == 0 && n >= 16 && n <= 1200; }
 
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
@@ -374,6 +427,25 @@ int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_leng
   stft_kernel<<<grid, kDspThreads, smem, st>>>(wav, L, n_fft, hop, win_length, T, mag, phase, real, imag, magT,
                                                T_pad);
   FSN_CHECK_LAUNCH("stft_kernel");
+  return FSN_OK;
+}
+
+int istft_mask_adjoint_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
+                              int hop, int win_length, float* dcrm, cudaStream_t st) {
+  FSN_REQUIRE(B > 0 && L > 0 && T > 0 && hop > 0 && hop <= n_fft && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE,
+              "istft adjoint: bad shape");
+  if (dft_size_ok(n_fft)) return istft_mask_adjoint_dft_launch(dwav, real, imag, B, L, T, n_fft, hop, win_length, dcrm, st);
+  FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
+              "istft adjoint: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);
+  const size_t smem = (size_t)(kFR / 2) * (n_fft + 1) * 8 + (size_t)n_fft / 2 * 8 + (size_t)n_fft * 4;
+  if (smem > 48 * 1024) {
+    int rc = check_cuda(cudaFuncSetAttribute(istft_mask_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                        "istft adjoint smem attr");
+    if (rc) return rc;
+  }
+  istft_mask_adjoint_kernel<<<dim3(cdiv(T, kFR), B), kDspThreads, smem, st>>>(dwav, real, imag, L, n_fft, hop, win_length, T,
+                                                                               dcrm);
+  FSN_CHECK_LAUNCH("istft_mask_adjoint_kernel");
   return FSN_OK;
 }
 

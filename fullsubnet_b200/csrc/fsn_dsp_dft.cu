@@ -191,6 +191,65 @@ istft_dft_kernel(const float* __restrict__ real, const float* __restrict__ imag,
   }
 }
 
+// adjoint of the element-wise mask + iSTFT with respect to the mask (istft_mask_adjoint_kernel of fsn_dsp.cu on the
+// direct DFT): frame t's samples g(t*hop + i) * win[i] -> forward DFT -> c_k/n scaling -> times the kept spectrum
+__global__ void __launch_bounds__(kDftThreads)
+istft_mask_adjoint_dft_kernel(const float* __restrict__ dwav, const float* __restrict__ real, const float* __restrict__ imag,
+                              int L, int n, int hop, int win_length, int T, float* __restrict__ dcrm) {
+  extern __shared__ float2 smem2[];
+  constexpr int NP = kDftFR / 2;
+  float2* zin = smem2;
+  float2* z = zin + NP * n;
+  float2* tw = z + NP * n;
+  float* win = reinterpret_cast<float*>(tw + n);
+  const int b = blockIdx.y;
+  const int t0 = blockIdx.x * kDftFR;
+  const int F = n / 2 + 1;
+  dft_tables(tw, win, n, win_length);
+  __syncthreads();
+  const float* g = dwav + (size_t)b * L;
+  for (int idx = threadIdx.x; idx < NP * n; idx += blockDim.x) {
+    const int p = idx / n;
+    const int i = idx - p * n;
+    const int ta = t0 + 2 * p, tb = ta + 1;
+    const float w = win[i];
+    float va = 0.f, vb = 0.f;
+    if (ta < T) va = istft_adjoint_sample(g, win, ta * hop + i, n, hop, T, L) * w;
+    if (tb < T) vb = istft_adjoint_sample(g, win, tb * hop + i, n, hop, T, L) * w;
+    zin[p * n + i] = make_float2(va, vb);
+  }
+  __syncthreads();
+  dft_smem<false>(zin, z, NP, n, tw);
+  const size_t plane = (size_t)F * T;
+  for (int idx = threadIdx.x; idx < (F - 1) * kDftFR; idx += blockDim.x) {
+    const int k = idx / kDftFR;
+    const int j = idx - k * kDftFR;
+    const int t = t0 + j;
+    if (t >= T) continue;
+    const float2 zk = z[(j >> 1) * n + k];
+    const float2 zn = z[(j >> 1) * n + (k == 0 ? 0 : n - k)];
+    float re, im;
+    if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
+    else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+    const float sc = (k == 0 ? 1.f : 2.f) / (float)n;
+    const size_t o = (size_t)b * plane + (size_t)k * T + t;
+    dcrm[(size_t)b * plane + o] = sc * re * real[o];
+    dcrm[(size_t)b * plane + plane + o] = k == 0 ? 0.f : sc * im * imag[o];
+  }
+}
+
+int istft_mask_adjoint_dft_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
+                                  int hop, int win_length, float* dcrm, cudaStream_t st) {
+  const size_t smem = (size_t)kDftFR * n_fft * 8 + (size_t)n_fft * 8 + (size_t)n_fft * 4;
+  int rc = check_cuda(cudaFuncSetAttribute(istft_mask_adjoint_dft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                      "istft adjoint smem attr");
+  if (rc) return rc;
+  istft_mask_adjoint_dft_kernel<<<dim3(cdiv(T, kDftFR), B), kDftThreads, smem, st>>>(dwav, real, imag, L, n_fft, hop,
+                                                                                      win_length, T, dcrm);
+  FSN_CHECK_LAUNCH("istft_mask_adjoint_dft_kernel");
+  return FSN_OK;
+}
+
 int stft_dft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, int T, int Tg, float* mag,
                     float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st) {
   const size_t smem = (size_t)kDftFR * n_fft * 8 + (size_t)n_fft * 8 + (size_t)n_fft * 4;

@@ -7,8 +7,8 @@
 
 namespace fsn {
 
-// |X|^fdrc with the Nyquist bin dropped, time-major: mag [B,F,T] -> out [B,T,F-1]  (model.py:564-565)
-__global__ void imp_compress_kernel(const float* __restrict__ mag, float* __restrict__ out, int F, int T, float fdrc) {
+// |X|^fdrc with the Nyquist bin dropped: mag [B,F,T] -> out [B,T,F-1], or [T,B,F-1] when tm  (model.py:564-565)
+__global__ void imp_compress_kernel(const float* __restrict__ mag, float* __restrict__ out, int F, int T, float fdrc, bool tm) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z, Fu = F - 1;
   const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
@@ -25,21 +25,19 @@ __global__ void imp_compress_kernel(const float* __restrict__ mag, float* __rest
   __syncthreads();
   for (int i = ty; i < 32; i += 8) {
     const int t = t0 + i, f = f0 + tx;
-    if (t < T && f < Fu) out[((size_t)b * T + t) * Fu + f] = tile[tx][i];
+    if (t < T && f < Fu) out[(tm ? (size_t)t * gridDim.z + b : (size_t)b * T + t) * Fu + f] = tile[tx][i];
   }
 }
 
-struct SecGeom { int lo, N, cs, ns, cf, nf, W; };
-
 // section input (model.py:321-405, 425-442): unit n of clip b at frame t = noisy rows lo+n*cs-ns .. (+cs+2ns) and
 // full-band rows lo+n*cf-nf .. (+cf+2nf), reflected (no edge repeat) at row 0 / row Fu-1.  One CTA per (b,t):
-// writes X[t][b*N+n][w] and the per-(b,t) sum (for the section norm).
+// writes X[t][b*N+n][w] and the per-(b,t) sum (for the section norm).  magc / fbT are [B,T,Fu], or [T,B,Fu] when tm.
 __global__ void imp_section_input_kernel(const float* __restrict__ magc, const float* __restrict__ fbT, int B, int T,
-                                         int Fu, SecGeom g, float* __restrict__ X, float2* __restrict__ fs) {
+                                         int Fu, SecGeom g, float* __restrict__ X, float2* __restrict__ fs, bool tm) {
   __shared__ float red[256];
   const int b = blockIdx.x / T, t = blockIdx.x % T;
   const int Wn = g.cs + 2 * g.ns;
-  const size_t base = ((size_t)b * T + t) * Fu;
+  const size_t base = (tm ? (size_t)t * B + b : (size_t)b * T + t) * Fu;
   float local = 0.f;
   for (int i = threadIdx.x; i < g.N * g.W; i += blockDim.x) {
     const int n = i / g.W, w = i - n * g.W;
@@ -62,16 +60,18 @@ __global__ void imp_section_input_kernel(const float* __restrict__ magc, const f
 }
 
 // Linear(H -> 2c) of one section for one frame, written into crm[b, ch, lo + n*c + j, t] with o = ch*c + j
-// (SubBandSequenceWrapper.forward, model.py:239-247); one warp per (row, output)
+// (SubBandSequenceWrapper.forward, model.py:239-247); one warp per (row, output).  `steps` consecutive frames from t0:
+// h [steps, R, H]
 __global__ void imp_fc_step_kernel(const float* __restrict__ h, int R, int H, const float* __restrict__ W,
                                    const float* __restrict__ bias, int c, int N, int lo, int act, float* __restrict__ crm,
-                                   int F, int T, int t) {
+                                   int F, int T, int t0, int steps) {
   const int O = 2 * c;
   const size_t wid = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (wid >= (size_t)R * O) return;
-  const int row = (int)(wid / O), o = (int)(wid % O);
-  const float* hp = h + (size_t)row * H;
+  if (wid >= (size_t)steps * R * O) return;
+  const size_t step_row = wid / O;
+  const int o = (int)(wid % O), t = t0 + (int)(step_row / R), row = (int)(step_row % R);
+  const float* hp = h + step_row * H;
   float s = 0.f;
   for (int k = lane; k < H; k += 32) s = fmaf(hp[k], W[(size_t)o * H + k], s);
   s = warp_sum(s);
@@ -83,16 +83,15 @@ __global__ void imp_fc_step_kernel(const float* __restrict__ h, int R, int H, co
   }
 }
 
-// X[t][r][w] *= inv[b(r)] with r = b*N + n: element i of the [T, R*W] tensor belongs to clip (i % (R*W)) / (N*W)
-__global__ void imp_scale_rows_kernel(float* __restrict__ X, const float* __restrict__ inv, size_t n, size_t per_t,
+// X[t][r][w] = src[t][r][w] * inv[b(r)] with r = b*N + n (src may be X): element i of the [T, R*W] tensor belongs to
+// clip (i % (R*W)) / (N*W)
+__global__ void imp_scale_rows_kernel(const float* src, float* X, const float* __restrict__ inv, size_t n, size_t per_t,
                                       size_t per_clip, int B) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const size_t b = (i % per_t) / per_clip;
-    X[i] *= inv[b < (size_t)B ? b : 0];
+    X[i] = src[i] * inv[b < (size_t)B ? b : 0];
   }
 }
-
-struct ImpDims { int B, L, T, F, Fu, S; SecGeom sec[FSN_IMP_MAX_SECTIONS]; int maxRW, maxR; };
 
 struct ImpWs {
   float *mag, *real, *imag, *crm, *magc, *fbT, *X, *inv1, *invs;
@@ -116,7 +115,7 @@ static SeqStack imp_fb_stack(const fsn_improved_desc* d, const ImpDims& m) {
 
 static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 
-static int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
+int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
   FSN_REQUIRE(d && B > 0 && L > 0, FSN_ERR_SHAPE, "improved model: empty input");
   FSN_REQUIRE((is_pow2(d->n_fft) && d->n_fft <= 2048) || (d->n_fft % 2 == 0 && d->n_fft >= 16 && d->n_fft <= 1200),
               FSN_ERR_UNSUPPORTED, "improved model: n_fft=%d unsupported (power of two <= 2048, or even and <= 1200)",
@@ -202,7 +201,7 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
     return rc;
   {
     dim3 grid(cdiv(T, 32), cdiv(Fu, 32), B);
-    imp_compress_kernel<<<grid, dim3(32, 8), 0, st>>>(w.mag, w.magc, F, T, d->fdrc);
+    imp_compress_kernel<<<grid, dim3(32, 8), 0, st>>>(w.mag, w.magc, F, T, d->fdrc, false);
     FSN_CHECK_LAUNCH("imp_compress_kernel");
   }
   // full band: norm (566) -> 2xLSTM + Linear (567)
@@ -218,7 +217,7 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
   for (int s = 0; s < m.S; ++s) {
     const SecGeom& g = m.sec[s];
     const int R = B * g.N;
-    imp_section_input_kernel<<<B * T, 256, 0, st>>>(w.magc, w.fbT, B, T, Fu, g, w.X, w.fs);
+    imp_section_input_kernel<<<B * T, 256, 0, st>>>(w.magc, w.fbT, B, T, Fu, g, w.X, w.fs, false);
     FSN_CHECK_LAUNCH("imp_section_input_kernel");
     if ((rc = clip_reduce_only_launch(w.fs, B, T, w.sums, st))) return rc;
     if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)g.N * g.W * T, 1.f, w.invs, nullptr, st, eps))) return rc;
@@ -230,7 +229,7 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
         const size_t n = (size_t)T * R * g.W;
         int blocks = (int)((n + 255) / 256);
         if (blocks > 132 * 16) blocks = 132 * 16;
-        imp_scale_rows_kernel<<<blocks, 256, 0, st>>>(w.X, w.invs, n, (size_t)R * g.W, (size_t)g.N * g.W, B);
+        imp_scale_rows_kernel<<<blocks, 256, 0, st>>>(w.X, w.X, w.invs, n, (size_t)R * g.W, (size_t)g.N * g.W, B);
         FSN_CHECK_LAUNCH("imp_scale_rows_kernel");
       }
       if ((rc = layer_forward_save_tc(seq_layer(sw, 0), w.X, R, g.W, Hs, T, w.tc, w.tc_rec, st))) return rc;
@@ -238,7 +237,7 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
       for (int t = 0; t < T; ++t) {
         const size_t warps = (size_t)R * 2 * g.cs;
         imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(w.tc_h1 + (size_t)t * R * Hs, R, Hs, sw.fc_w, sw.fc_b,
-                                                                    g.cs, g.N, g.lo, d->sb_activation, crm, F, T, t);
+                                                                    g.cs, g.N, g.lo, d->sb_activation, crm, F, T, t, 1);
         FSN_CHECK_LAUNCH("imp_fc_step_kernel");
       }
       continue;
@@ -253,7 +252,7 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
       if ((rc = lstm_step2_launch(p, SEG0_DENSE, t, seq_layer(sw, 1), s2, st))) return rc;
       const size_t warps = (size_t)R * 2 * g.cs;
       imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(s2.h1_at(t), R, Hs, sw.fc_w, sw.fc_b, g.cs, g.N, g.lo,
-                                                                  d->sb_activation, crm, F, T, t);
+                                                                  d->sb_activation, crm, F, T, t, 1);
       FSN_CHECK_LAUNCH("imp_fc_step_kernel");
     }
   }

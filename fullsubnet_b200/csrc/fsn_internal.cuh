@@ -240,6 +240,24 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
 // it into the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:181-182)
 int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st);
 
+// adjoint of the element-wise mask + iSTFT of improved_fullsubnet (istft_launch mask_mode 2) with respect to the mask:
+// dwav [B,L] -> dcrm [B,2,F,T] for the rows f < F-1 (the Nyquist row of the cRM is a constant; it is not written)
+int istft_mask_adjoint_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
+                              int hop, int win_length, float* dcrm, cudaStream_t st);
+
+// improved_fullsubnet (fsn_improved.cu), shared by its inference forward and its training step
+struct SecGeom { int lo, N, cs, ns, cf, nf, W; };  // section rows [lo, lo + N*cs), unit width W
+struct ImpDims { int B, L, T, F, Fu, S; SecGeom sec[FSN_IMP_MAX_SECTIONS]; int maxRW, maxR; };
+int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m);
+__global__ void imp_compress_kernel(const float* __restrict__ mag, float* __restrict__ out, int F, int T, float fdrc, bool tm);
+__global__ void imp_section_input_kernel(const float* __restrict__ magc, const float* __restrict__ fbT, int B, int T,
+                                         int Fu, SecGeom g, float* __restrict__ X, float2* __restrict__ fs, bool tm);
+__global__ void imp_fc_step_kernel(const float* __restrict__ h, int R, int H, const float* __restrict__ W,
+                                   const float* __restrict__ bias, int c, int N, int lo, int act, float* __restrict__ crm,
+                                   int F, int T, int t0, int steps);
+__global__ void imp_scale_rows_kernel(const float* src, float* X, const float* __restrict__ inv, size_t n, size_t per_t,
+                                      size_t per_clip, int B);
+
 // persistent cooperative full-band LSTM (fsn_fullband.cu): layers L[0] (F -> H0, input x [R,Tp,F] times inv1[r] when
 // given) and L[1] (H0 -> H1) of R rows into h1all [R,Tp,H1]; h0buf [2][256][H0] scratch
 bool fb_persistent_supported(int F, int H0, int H1);

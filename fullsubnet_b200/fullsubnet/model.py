@@ -17,17 +17,6 @@ from ..model.base_model import BaseModel, TrainStep
 from ..model.module.sequence_model import SequenceModel
 
 
-def _grad_struct(grads: dict, prefix: str) -> "_lib.SeqGrads":
-    g = _lib.SeqGrads()
-    for l in range(2):
-        lg = SequenceModel.grads_struct(grads, prefix, l)
-        for field in ("w_ih", "w_hh", "b_ih", "b_hh"):
-            getattr(g, field)[l] = getattr(lg, field)
-    g.fc_w = grads[f"{prefix}fc_output_layer.weight"].data_ptr()
-    g.fc_b = grads[f"{prefix}fc_output_layer.bias"].data_ptr()
-    return g
-
-
 class Model(BaseModel):
     # training step (trainer.py:56-63): fsn_train_forward keeps the activations, fsn_train_backward runs BPTT
     TRAIN_ENTRY_POINTS = ("fsn_train_workspace_bytes", "fsn_train_forward", "fsn_train_backward")
@@ -87,7 +76,8 @@ class Model(BaseModel):
         return C.byref(self.fb_model.weight_struct()), C.byref(self.sb_model.weight_struct())
 
     def _train_grads(self, grads):
-        return C.byref(_grad_struct(grads, "fb_model.")), C.byref(_grad_struct(grads, "sb_model."))
+        return (C.byref(SequenceModel.seq_grads_struct(grads, "fb_model.")),
+                C.byref(SequenceModel.seq_grads_struct(grads, "sb_model.")))
 
     def _train_out_shape(self, desc, B, F, T):
         G = desc.num_groups_in_drop_band if B > 1 and desc.num_groups_in_drop_band > 1 else 1

@@ -2,7 +2,10 @@
 
 Same constructor kwargs and ``state_dict`` keys (``fb_model.*``, ``sb_model.sb_models.{s}.*``);
 ``forward(y [B,L] | [B,1,L]) -> [B,1,L]`` (waveform in, enhanced waveform out) is one call into libfsn_b200
-(``fsn_improved_forward``: STFT -> |X|^fdrc -> full band -> per-section sub bands -> element-wise mask -> iSTFT)."""
+(``fsn_improved_forward``: STFT -> |X|^fdrc -> full band -> per-section sub bands -> element-wise mask -> iSTFT).  With
+gradients enabled the output is differentiable like the reference module's: the forward keeps its activations
+(``fsn_improved_train_forward``) and ``loss.backward()`` runs the iSTFT adjoint and back-propagation through time in the
+library (``fsn_improved_train_backward``), so any loss on the enhanced waveform trains the model."""
 from __future__ import annotations
 
 import ctypes as C
@@ -12,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from ..model.base_model import BaseModel
+from ..model.base_model import BaseModel, TrainStep
 from ..model.module.sequence_model import SequenceModel
 
 
@@ -24,6 +27,7 @@ class SubbandModel(nn.Module):
         super().__init__()
         assert len(freq_cutoffs) + 1 == len(sb_num_center_freqs) == len(sb_num_neighbor_freqs) \
             == len(fb_num_center_freqs) == len(fb_num_neighbor_freqs)
+        self.hidden_size = hidden_size
         self.sb_models = nn.ModuleList([
             SequenceModel(input_size=(sb_num_center_freqs[s] + sb_num_neighbor_freqs[s] * 2)
                           + (fb_num_center_freqs[s] + fb_num_neighbor_freqs[s] * 2),
@@ -38,6 +42,11 @@ class SubbandModel(nn.Module):
 
 
 class Model(BaseModel):
+    # training step (wav in, wav out; upstream ships no trainer): fsn_improved_train_forward keeps the activations,
+    # fsn_improved_train_backward runs the iSTFT adjoint and BPTT
+    TRAIN_ENTRY_POINTS = ("fsn_improved_train_workspace_bytes", "fsn_improved_train_forward", "fsn_improved_train_backward")
+    TRAIN_TF32_STACKS = ("fb_model", "sb_model")
+
     def __init__(self, n_fft=512, hop_length=128, win_length=512, fdrc=0.5, num_freqs=257, freq_cutoffs=[20, 80],
                  sb_num_center_freqs=[1, 4, 8], sb_num_neighbor_freqs=[15, 15, 15], fb_num_center_freqs=[1, 4, 8],
                  fb_num_neighbor_freqs=[15, 15, 15], fb_hidden_size=512, sb_hidden_size=384, sequence_model="LSTM",
@@ -60,6 +69,9 @@ class Model(BaseModel):
         # arithmetic of the sub-band sections (98 % of the FLOPs): "fp32" (FMA kernels), "tf32_tc" (wgmma tf32
         # GEMMs, fp32 accumulate; waveform within 1e-4 of the reference) or "auto" (= tf32_tc when sb_hidden % 4 == 0)
         self.precision = os.environ.get("FSN_IMPROVED_PRECISION", "auto")
+        # arithmetic of the training step's GEMMs: "fp32" (FMA) | "tf32_tc" (wgmma tf32 for the LSTM layers) | "auto" =
+        # tf32_tc when fb_hidden_size and sb_hidden_size are multiples of 4
+        self.train_precision = os.environ.get("FSN_TRAIN_PRECISION", "auto")
 
     def _resolve_precision(self) -> str:
         ok = self.sb_model.sb_models[0].hidden_size % 4 == 0
@@ -70,23 +82,48 @@ class Model(BaseModel):
         return self.precision
 
     def _structs(self):
+        return self._desc(self._resolve_precision()), self._weights()
+
+    def _desc(self, precision: str) -> "_lib.ImprovedDesc":
         sb = self.sb_model
         d = _lib.ImprovedDesc(n_fft=self.n_fft, hop_length=self.hop_length, win_length=self.win_length,
                               num_freqs=self.num_freqs, fdrc=float(self.fdrc), num_sections=len(sb.sb_models),
                               fb_hidden=self.fb_model.hidden_size, sb_hidden=sb.sb_models[0].hidden_size,
                               fb_activation=_lib.ACT[self.fb_model.output_activate_function],
                               sb_activation=_lib.ACT[sb.sb_models[0].output_activate_function],
-                              precision=_lib.PREC[self._resolve_precision()])
+                              precision=_lib.PREC[precision],
+                              cell_type=_lib.CELL[self.fb_model.cell])
         for s in range(len(sb.sb_models)):
             if s < len(sb.freq_cutoffs):
                 d.freq_cutoffs[s] = sb.freq_cutoffs[s]
             d.sb_num_center[s], d.sb_num_neighbor[s] = sb.sb_num_center_freqs[s], sb.sb_num_neighbor_freqs[s]
             d.fb_num_center[s], d.fb_num_neighbor[s] = sb.fb_num_center_freqs[s], sb.fb_num_neighbor_freqs[s]
+        return d
+
+    def _weights(self) -> "_lib.ImprovedWeights":
+        sb = self.sb_model
         w = _lib.ImprovedWeights()
         w.fb = self.fb_model.weight_struct()
         for s, m in enumerate(sb.sb_models):
             w.sb[s] = m.weight_struct()
-        return d, w
+        return w
+
+    def _train_desc(self):
+        return self._desc(self._resolve_train_precision())
+
+    def _train_weights(self):
+        return (C.byref(self._weights()),)
+
+    def _train_grads(self, grads):
+        g = _lib.ImprovedGrads()
+        g.fb = SequenceModel.seq_grads_struct(grads, "fb_model.")
+        for s in range(len(self.sb_model.sb_models)):
+            g.sb[s] = SequenceModel.seq_grads_struct(grads, f"sb_model.sb_models.{s}.")
+        return (C.byref(g),)
+
+    def _train_io(self, x, desc):
+        B, L = x.shape
+        return (B, L), (B, 1, L)
 
     def forward(self, y, return_crm: bool = False):
         """y [B,L] or [B,1,L] -> enhanced [B,1,L]  (model.py:541-591).  ``return_crm`` additionally returns the
@@ -96,8 +133,6 @@ class Model(BaseModel):
         if ndim == 3:
             assert y.size(1) == 1, "Input must be 2D (B, T) or 3D tensor (B, 1, T)"
             y = y.squeeze(1)
-        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("fullsubnet_b200: backward kernels are not built yet; use torch.no_grad()/eval().")
         x = _lib.require_cuda(y, "y")
         B, L = x.shape
         sb = self.sb_model
@@ -108,6 +143,14 @@ class Model(BaseModel):
                 raise ValueError(
                     "The number of center frequencies should be divisible by the subband freqency interval. "
                     f"Got {sb.sb_num_center_freqs[s]} and {bounds[s + 1] - bounds[s]}.")
+        if self._records_grad():
+            if return_crm:
+                raise NotImplementedError("fullsubnet_b200: return_crm is built for inference only (use torch.no_grad())")
+            if y.requires_grad:  # the library computes no input gradient; returning None would silently zero it
+                raise NotImplementedError("fullsubnet_b200: improved_fullsubnet training computes no gradient for the input")
+            if self.fb_model.cell != "LSTM":
+                raise NotImplementedError("fullsubnet_b200: improved_fullsubnet training is built for LSTM only")
+            return TrainStep.apply(self, x, *self.parameters())
         lib = _lib.load()
         with torch.cuda.device(x.device):
             d, w = self._structs()

@@ -20,27 +20,27 @@ class TrainStep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, x, *params):
-        B, _, F, T = x.shape
         device = x.device
         lib = _lib.load()
         query, fwd, _ = (getattr(lib, name) for name in model.TRAIN_ENTRY_POINTS)
         with torch.cuda.device(device):
             desc = model._train_desc()
             weights = model._train_weights()
-            n = query(C.byref(desc), B, T)
+            dims, out_shape = model._train_io(x, desc)
+            n = query(C.byref(desc), *dims)
             if n == 0:
                 _lib.check_workspace(n)
             ws = torch.empty(n, dtype=torch.uint8, device=device)
-            out = torch.empty(model._train_out_shape(desc, B, F, T), dtype=torch.float32, device=device)
-            _lib.check(fwd(C.byref(desc), *weights, x.data_ptr(), B, T, out.data_ptr(), ws.data_ptr(), n,
+            out = torch.empty(out_shape, dtype=torch.float32, device=device)
+            _lib.check(fwd(C.byref(desc), *weights, x.data_ptr(), *dims, out.data_ptr(), ws.data_ptr(), n,
                            _lib.stream_ptr(device)))
-        ctx.model, ctx.ws, ctx.dims, ctx.desc = model, ws, (B, T), desc
+        ctx.model, ctx.ws, ctx.dims, ctx.desc = model, ws, dims, desc
         ctx.versions = model._version_key()
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        model, (B, T) = ctx.model, ctx.dims
+        model = ctx.model
         if ctx.versions != model._version_key():
             raise RuntimeError("fullsubnet_b200: a parameter was modified in place between forward and backward")
         if ctx.ws is None:
@@ -53,7 +53,7 @@ class TrainStep(torch.autograd.Function):
         with torch.cuda.device(device):
             weights = model._train_weights()
             g = model._train_grads(grads)
-            _lib.check(bwd(C.byref(ctx.desc), *weights, dy.data_ptr(), B, T, *g, ctx.ws.data_ptr(), ctx.ws.numel(),
+            _lib.check(bwd(C.byref(ctx.desc), *weights, dy.data_ptr(), *ctx.dims, *g, ctx.ws.data_ptr(), ctx.ws.numel(),
                            _lib.stream_ptr(device)))
         ctx.ws = None
         return (None, None) + tuple(grads[k] for k in names)
@@ -91,6 +91,7 @@ class BaseModel(nn.Module):
     # Each trainable model sets TRAIN_ENTRY_POINTS (library workspace query, forward, backward), TRAIN_TF32_STACKS (the
     # SequenceModel attributes whose hidden sizes decide train_precision="auto") and implements _train_desc(),
     # _train_weights() and _train_grads(grads): the descriptor and the ctypes arguments of the weights / gradients.
+    # _train_io / _train_out_shape give the size arguments of the entry points and the output shape.
     TRAIN_ENTRY_POINTS: tuple = ()
     TRAIN_TF32_STACKS: tuple = ()
 
@@ -112,6 +113,12 @@ class BaseModel(nn.Module):
         if not all(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("fullsubnet_b200: partially frozen models are not built")
         return True
+
+    def _train_io(self, x, desc):
+        """(the size arguments of the training entry points, the output shape) for the input x: (B, T) and
+        _train_out_shape for a spectrogram [B,1,F,T]."""
+        B, _, F, T = x.shape
+        return (B, T), self._train_out_shape(desc, B, F, T)
 
     def _train_out_shape(self, desc, B, F, T):
         return (B, 2, F, T)

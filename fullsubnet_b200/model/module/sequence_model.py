@@ -59,6 +59,19 @@ class SequenceModel(nn.Module):
         the SequenceModel's name in the model followed by a dot."""
         return _lib.LstmGrads(*(grads[f"{prefix}sequence_model.{n}_l{l}"].data_ptr() for n in LSTM_PARAMS))
 
+    @staticmethod
+    def seq_grads_struct(grads: dict, prefix: str) -> "_lib.SeqGrads":
+        """Pointers of the gradients of a 2-layer stack with its Linear (fsn_seq_grads), from named gradient tensors;
+        ``prefix`` is the SequenceModel's name in the model followed by a dot."""
+        g = _lib.SeqGrads()
+        for l in range(2):
+            lg = SequenceModel.grads_struct(grads, prefix, l)
+            for field in ("w_ih", "w_hh", "b_ih", "b_hh"):
+                getattr(g, field)[l] = getattr(lg, field)
+        g.fc_w = grads[f"{prefix}fc_output_layer.weight"].data_ptr()
+        g.fc_b = grads[f"{prefix}fc_output_layer.bias"].data_ptr()
+        return g
+
     def fc_ptrs(self):
         return (self._check(self.fc_output_layer.weight, "fc_output_layer.weight"),
                 self._check(self.fc_output_layer.bias, "fc_output_layer.bias"))

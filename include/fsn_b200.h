@@ -219,8 +219,8 @@ int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_weights* w, co
  * recipes/dns_interspeech_2020/improved_fullsubnet/model.py:452-591  Model (BASELINE config 5, SURVEY 8a row A14)
  *   wav -> STFT -> |X|^fdrc, Nyquist bin dropped -> norm -> full-band 2xLSTM + Linear -> per sub-band section:
  *   strided unfold (centre/neighbour widths) of noisy and full-band output, concat, per-section norm, 2xLSTM +
- *   Linear(2*centre) -> cRM (Nyquist row 0) -> element-wise mask on (re, im) -> iSTFT -> wav.  fp32 kernels;
- *   n_fft must be a power of two (the reference's n_fft=960 example needs a mixed-radix FFT: not built).
+ *   Linear(2*centre) -> cRM (Nyquist row 0) -> element-wise mask on (re, im) -> iSTFT -> wav.  n_fft: a power of two
+ *   <= 2048 (radix-2 FFT), or even and <= 1200 (direct DFT; the reference's 48 kHz example uses n_fft = 960).
  * ---------------------------------------------------------------------------------------- */
 #define FSN_IMP_MAX_SECTIONS 8
 typedef struct fsn_improved_desc {
@@ -232,6 +232,7 @@ typedef struct fsn_improved_desc {
   int32_t fb_num_center[FSN_IMP_MAX_SECTIONS], fb_num_neighbor[FSN_IMP_MAX_SECTIONS];
   int32_t fb_hidden, sb_hidden, fb_activation, sb_activation;
   int32_t precision; /* FSN_PREC_FP32, or FSN_PREC_TF32_TC: the sub-band sections' GEMMs on wgmma tf32 */
+  int32_t cell_type; /* FSN_CELL_* (`sequence_model`); read by the training step only, which is built for LSTM */
 } fsn_improved_desc;
 
 typedef struct fsn_improved_weights {
@@ -367,6 +368,29 @@ int fsn_fullband_train_forward(const fsn_fullband_desc* d, const fsn_lstm_layer*
 int fsn_fullband_train_backward(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,
                                 const float* fc_b, const float* dout, int B, int T, const fsn_fullband_grads* g,
                                 void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+
+/* Training step of improved_fullsubnet (improved_fullsubnet/model.py:452-591 is a differentiable module, wav in and wav
+ * out; upstream ships no trainer, so any loss on the enhanced waveform drives it), same conventions as fsn_train_*: the
+ * caller allocates the workspace and passes the same untouched buffer from forward to backward; every gradient is
+ * OVERWRITTEN; no host synchronisation; arguments are checked before any CUDA call; every sum runs in a fixed order (two
+ * runs give identical bits).
+ *   fsn_improved_train_forward  = Model.forward with gradients enabled: wav [B,L] -> enhanced [B,L], keeping the noisy
+ *                                 spectrum, the normalised section inputs and their scales, the gates / cells / hidden
+ *                                 states of every LSTM layer and the post-activation outputs (time-major [T, rows, .])
+ *   fsn_improved_train_backward = loss.backward() from d_enhanced = d loss / d enhanced [B,L]; no input gradient
+ * d->precision: FSN_PREC_FP32, or FSN_PREC_TF32_TC (every LSTM layer with H % 4 == 0 on the wgmma tf32 GEMMs, as in
+ * fsn_train_*).  The GRU cell, another precision, fb_activation / sb_activation other than none or ReLU -> FSN_ERR_UNSUPPORTED;
+ * shapes as fsn_improved_forward. */
+typedef struct fsn_improved_grads {
+  fsn_seq_grads fb;                          /* fb_model */
+  fsn_seq_grads sb[FSN_IMP_MAX_SECTIONS];    /* sb_model.sb_models[s] */
+} fsn_improved_grads;
+size_t fsn_improved_train_workspace_bytes(const fsn_improved_desc* d, int B, int L);
+int fsn_improved_train_forward(const fsn_improved_desc* d, const fsn_improved_weights* w, const float* wav, int B, int L,
+                               float* enhanced, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn_improved_weights* w, const float* d_enhanced, int B,
+                                int L, const fsn_improved_grads* g, void* workspace, size_t workspace_bytes,
+                                fsn_stream_t stream);
 
 /* audio_zen/inferencer/base_inferencer.py:181-182 (SURVEY 8f rank 2): out = int16(gain * wav / max|wav|) per clip,
  * gain = 0.8 * 32767 in the reference; float32 multiply, divide, truncation toward zero like numpy; all-zero clip -> 0 */
