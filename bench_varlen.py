@@ -1,0 +1,155 @@
+"""bench_varlen.py - fullsubnet inference over clips of DIFFERENT lengths on one GPU.  Prints one JSON line.
+
+Workload: a seeded set of --clips clips (default 1024) whose lengths are distinct and uniform in 1 - 10 s at 16 kHz,
+the inference.toml model with weights W-a, the default precision ("auto": f16x3_tc), wav -> enhanced wav + int16 PCM
+(what the file loop writes).  Two schedules of the same clips:
+
+  exact       equal-length batches (``plan_batches(lengths, 256, 0)``): every length is distinct, so B = 1 per call
+              (fsn_enhance_pcm), which is what the file loop does on real recordings by default;
+  pad<x>      ``plan_batches(lengths, 256, x)``: length-sorted runs of <= 256 clips padded to their longest clip by at
+              most a fraction x of the batch's samples, one fsn_enhance_varlen call per batch.
+
+Each schedule is timed twice with CUDA events around the whole schedule: "resident" (inputs already in HBM, outputs left
+there) and "e2e" (pinned host float32 -> H2D -> call -> int16 D2H into pinned host memory, the file loop minus the wav
+I/O).  Every clip's PCM of every schedule is compared with the exact schedule's, bit for bit.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+
+SR = 16000
+GAIN = 0.8 * 32767.0
+
+
+def power_limit_w(index: int):
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30)
+        return float(out.stdout.strip().splitlines()[0])
+    except Exception:  # noqa: BLE001 - reported as unknown
+        return None
+
+
+def clip_lengths(n: int, seed: int):
+    rng = np.random.default_rng(seed)
+    return (rng.permutation(9 * SR + 1)[:n] + SR).tolist()  # distinct, uniform in [1 s, 10 s]
+
+
+class Schedule:
+    """The batches of one schedule with their staging buffers (device and pinned host), built outside the timing."""
+
+    def __init__(self, name, plan, lens, clips, dev):
+        self.name, self.plan, self.lens = name, plan, lens
+        self.batches = []
+        for idx in plan:
+            L = max(lens[i] for i in idx)
+            host = torch.zeros(len(idx), L, dtype=torch.float32).pin_memory()
+            for r, i in enumerate(idx):
+                host[r, :lens[i]] = clips[i]
+            mixed = any(lens[i] != L for i in idx)
+            self.batches.append(dict(idx=idx, L=L, lengths=[lens[i] for i in idx] if mixed else None, host=host,
+                                     dev=host.to(dev), pcm_host=torch.empty(len(idx), L, dtype=torch.int16).pin_memory()))
+        self.samples = sum(lens[i] for idx in plan for i in idx)
+        self.padded = sum(len(b["idx"]) * b["L"] for b in self.batches)
+
+    def run(self, m, e2e):
+        outs = []
+        for b in self.batches:
+            x = b["host"].to(b["dev"].device, non_blocking=True) if e2e else b["dev"]
+            pcm = m.enhance_pcm(x, gain=GAIN, lengths=b["lengths"])[1]
+            if e2e:
+                b["pcm_host"].copy_(pcm, non_blocking=True)
+            outs.append(pcm)
+        return outs
+
+
+def time_schedule(m, s, e2e, reps):
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    ms = []
+    for _ in range(reps):
+        ev0.record()
+        s.run(m, e2e)
+        ev1.record()
+        torch.cuda.synchronize()
+        ms.append(ev0.elapsed_time(ev1))
+    return ms
+
+
+def main():
+    from fullsubnet_b200 import _lib
+    from fullsubnet_b200.fullsubnet.model import Model
+    from fullsubnet_b200.inferencer import plan_batches
+    from oracle import fullsubnet_oracle as O  # weights / inputs generator only
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--gpus", type=int, default=1)
+    ap.add_argument("--clips", type=int, default=1024)
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--max-padding", type=float, nargs="+", default=[0.05, 0.1, 0.25])
+    ap.add_argument("--steps", type=int, default=1, help="timed repetitions of every schedule")
+    ap.add_argument("--warmup", type=int, default=1, help="untimed repetitions of every schedule")
+    ap.add_argument("--seed", type=int, default=0)
+    a = ap.parse_args()
+    assert a.gpus == 1, "bench_varlen.py measures one GPU"
+    assert torch.cuda.is_available(), "bench_varlen.py needs a CUDA device"
+    dev = torch.device("cuda", torch.cuda.current_device())
+    lib = _lib.load()
+    m = Model(**O.DEFAULT_MODEL_ARGS)
+    m.load_state_dict(O.make_state_dict(seed=0), strict=True)
+    m = m.to(dev).eval()
+    lens = clip_lengths(a.clips, a.seed)
+    noise = O.make_noisy(1, max(lens), seed=a.seed + 1, speechlike=True)[0]
+    rng = np.random.default_rng(a.seed + 2)
+    clips = [noise[int(rng.integers(0, max(lens) - L + 1)):][:L] * float(rng.uniform(0.3, 1.0)) for L in lens]
+
+    schedules = [Schedule("exact", plan_batches(lens, a.batch, 0.0), lens, clips, dev)]
+    for mp in a.max_padding:
+        schedules.append(Schedule(f"pad{mp:g}", plan_batches(lens, a.batch, mp), lens, clips, dev))
+    audio_s = sum(lens) / SR
+    res, ref = {}, None
+    for s in schedules:
+        for _ in range(a.warmup):
+            s.run(m, False)
+        n0 = lib.fsn_total_launch_count()
+        outs = s.run(m, False)
+        torch.cuda.synchronize()
+        launches = int(lib.fsn_total_launch_count() - n0)
+        per_clip = {i: pcm[r, :lens[i]] for b, pcm in zip(s.batches, outs) for r, i in enumerate(b["idx"])}
+        if ref is None:
+            ref = per_clip
+        identical = all(torch.equal(per_clip[i], ref[i]) for i in range(len(lens)))
+        r = {"calls": len(s.batches), "max_batch": max(len(b["idx"]) for b in s.batches), "gpu_launches": launches,
+             "padded_fraction": 1.0 - s.samples / s.padded, "pcm_identical_to_exact": identical}
+        for mode in ("resident", "e2e"):
+            ms = time_schedule(m, s, mode == "e2e", a.steps)
+            best = min(ms)
+            r[mode] = {"ms": best, "ms_all": ms, "clips_per_sec": len(lens) / (best * 1e-3),
+                       "xRT": audio_s / (best * 1e-3)}
+        res[s.name] = r
+        del outs, per_clip
+    best_name = max((n for n in res if n != "exact"), key=lambda n: res[n]["e2e"]["clips_per_sec"])
+    best = res[best_name]
+    print(json.dumps({
+        "metric": "clips_per_sec", "value": best["e2e"]["clips_per_sec"], "unit": "clips/s", "n_gpus": 1,
+        "steps": a.steps, "warmup": a.warmup, "higher_is_better": True, "best_schedule": best_name,
+        "speedup_vs_exact_e2e": best["e2e"]["clips_per_sec"] / res["exact"]["e2e"]["clips_per_sec"],
+        "speedup_vs_exact_resident": best["resident"]["clips_per_sec"] / res["exact"]["resident"]["clips_per_sec"],
+        "config": {"workload": f"{a.clips} clips, distinct lengths uniform in 1-10 s at 16 kHz ({audio_s:.0f} s of audio), "
+                               "fullsubnet inference.toml, W-a, wav -> enhanced + int16 PCM",
+                   "precision": m._resolve_precision(), "batch": a.batch, "seed": a.seed},
+        "schedules": res,
+        "device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(dev.index or 0)}))
+
+
+if __name__ == "__main__":
+    main()

@@ -6,6 +6,8 @@
 // FFT: shared-memory radix-2 DIT, two real frames packed into one complex transform
 // (frame A -> real lane, frame B -> imaginary lane), FR frames per CTA so that the [B,F,T]
 // (T-contiguous) stores / loads of the reference layout are FR*4-byte segments.
+#include <string.h>
+
 #include "fsn_common.cuh"
 
 namespace fsn {
@@ -58,10 +60,13 @@ __device__ __forceinline__ void init_tables(float2* tw, float* win, int n, int w
 }
 
 // ------------------------------------------------------------------------------------------
+// lens (nullable, device [B]): clip b holds lens[b] <= L samples of its row (stride L), so it reflects at lens[b] and has
+// T_b = 1 + lens[b]/hop frames; frames T_b .. T-1 are written as zeros and frame T_b enters its pair's transform as
+// zeros, exactly as in a call on that clip alone.  Null: every clip has L samples.
 __global__ void __launch_bounds__(kDspThreads)
 stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length, int T,
             float* __restrict__ mag, float* __restrict__ phase, float* __restrict__ real,
-            float* __restrict__ imag, float* __restrict__ magT, int T_pad) {
+            float* __restrict__ imag, float* __restrict__ magT, int T_pad, const int* __restrict__ lens) {
   extern __shared__ float2 smem2[];
   const int log2n = ilog2(n);
   const int zstride = n + 1;
@@ -72,6 +77,8 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
   const int b = blockIdx.y;
   const int t0 = blockIdx.x * kFR;
   const int F = n / 2 + 1;
+  const int Lb = lens ? lens[b] : L;
+  const int Tb = lens ? 1 + Lb / hop : T;
   init_tables(tw, win, n, win_length);
   __syncthreads();
   const float* x = wav + (size_t)b * L;
@@ -81,8 +88,8 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
     const int ta = t0 + 2 * p, tb = ta + 1;
     const float w = win[i];
     float va = 0.f, vb = 0.f;
-    if (ta < T) va = x[reflect_idx(ta * hop + i - n / 2, L)] * w;
-    if (tb < T) vb = x[reflect_idx(tb * hop + i - n / 2, L)] * w;
+    if (ta < Tb) va = x[reflect_idx(ta * hop + i - n / 2, Lb)] * w;
+    if (tb < Tb) vb = x[reflect_idx(tb * hop + i - n / 2, Lb)] * w;
     z[p * zstride + (int)(__brev((unsigned)i) >> (32 - log2n))] = make_float2(va, vb);
   }
   __syncthreads();
@@ -100,6 +107,7 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
     float re, im;
     if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
     else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+    if (t >= Tb) re = im = 0.f;
     const size_t o = (size_t)b * plane + (size_t)k * T + t;
     if (real) real[o] = re;
     if (imag) imag[o] = im;
@@ -113,7 +121,7 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
       const int t = t0 + j;
       if (t >= T_pad) continue;
       float m = 0.f;
-      if (t < T) {
+      if (t < Tb) {
         const float2 zk = z[(j >> 1) * zstride + k];
         const float2 zn = z[(j >> 1) * zstride + ((n - k) & (n - 1))];
         float re, im;
@@ -130,7 +138,8 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
 __global__ void __launch_bounds__(kDspThreads)
 istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int cstride,
              const float* __restrict__ crm, int mask_mode, int T, int n, int hop, int win_length, int out_len,
-             int seg, int np_max, float* __restrict__ wav, unsigned int* __restrict__ peak_bits) {
+             int seg, int np_max, float* __restrict__ wav, unsigned int* __restrict__ peak_bits,
+             const int* __restrict__ lens) {
   extern __shared__ float2 smem2[];
   const int log2n = ilog2(n);
   const int zstride = n + 1;
@@ -139,10 +148,15 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
   float* win = reinterpret_cast<float*>(tw + n / 2);
   const int b = blockIdx.y;
   const int F = n / 2 + 1;
+  // lens (nullable): clip b has T_b = 1 + lens[b]/hop of the T frames (row stride T) and lens[b] of the out_len output
+  // samples (row stride out_len); samples lens[b] .. out_len-1 are written as 0.  The segment tiling is absolute, so
+  // each CTA pairs the same frames as a call on that clip alone.
+  const int Lb = lens ? lens[b] : out_len;
+  const int Tb = lens ? 1 + Lb / hop : T;
   const int s_begin = n / 2 + blockIdx.x * seg;
-  const int s_end = min(s_begin + seg, n / 2 + out_len);
+  const int s_end = min(s_begin + seg, n / 2 + Lb);
   const int t_min = (s_begin >= n) ? (s_begin - n) / hop + 1 : 0;
-  const int t_max = min(T - 1, (s_end - 1) / hop);
+  const int t_max = min(Tb - 1, (s_end - 1) / hop);
   const int nframes = t_max - t_min + 1;
   const int np = nframes > 0 ? (nframes + 1) / 2 : 0;
   init_tables(tw, win, n, win_length);
@@ -187,7 +201,7 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
   __syncthreads();
   fft_radix2_smem<true>(z, zstride, np, n, log2n, tw);
 
-  const int full = n + hop * (T - 1);
+  const int full = n + hop * (Tb - 1);
   const float inv_n = 1.0f / (float)n;
   float* out = wav + (size_t)b * out_len;
   float peak = 0.f;
@@ -209,6 +223,9 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
     out[s - n / 2] = y;
     peak = fmaxf(peak, fabsf(y));
   }
+  if (lens)
+    for (int s = max(s_begin, n / 2 + Lb) + threadIdx.x; s < min(s_begin + seg, n / 2 + out_len); s += blockDim.x)
+      out[s - n / 2] = 0.f;
   if (peak_bits) {
     // max|y| of the clip for the int16 scaling of the host loop (base_inferencer.py:181-182): non-negative floats
     // order like their bit patterns, and max is order-independent, so the atomic is deterministic
@@ -269,12 +286,33 @@ istft_mask_adjoint_kernel(const float* __restrict__ dwav, const float* __restric
   }
 }
 
-// out = int16(gain * wav / peak) per clip, peak from the iSTFT epilogue (float32 mul, div, truncation like numpy)
+// out = int16(gain * wav / peak) per clip, peak from the iSTFT epilogue (float32 mul, div, truncation like numpy);
+// lens (nullable): 0 past the clip's own lens[b] samples of its row
 __global__ void scale_int16_kernel(const float* __restrict__ wav, const unsigned int* __restrict__ peak_bits, int L, float gain,
-                                   int16_t* __restrict__ out, size_t n) {
+                                   int16_t* __restrict__ out, size_t n, const int* __restrict__ lens) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float m = __uint_as_float(peak_bits[i / L]);
-    out[i] = (m > 0.f) ? (int16_t)__fdiv_rn(__fmul_rn(gain, wav[i]), m) : (int16_t)0;
+    const size_t b = i / L;
+    const float m = __uint_as_float(peak_bits[b]);
+    const bool keep = !lens || (int)(i - b * L) < lens[b];
+    out[i] = (keep && m > 0.f) ? (int16_t)__fdiv_rn(__fmul_rn(gain, wav[i]), m) : (int16_t)0;
+  }
+}
+
+// per-clip length table: lengths[off + i] = v[i], the values travelling in the parameter block (no host buffer is read
+// after the launch, and no copy from pageable memory can synchronise the stream)
+constexpr int kLenChunk = 1000;  // 4 KB parameter block with the two counts
+struct LenChunk { int off, n; int v[kLenChunk]; };
+__global__ void lengths_table_kernel(const __grid_constant__ LenChunk c, int* __restrict__ lengths) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < c.n) lengths[c.off + i] = c.v[i];
+}
+
+// crm [B, C, T]: frames t >= 1 + lengths[b]/hop of clip b set to 0
+__global__ void zero_frames_past_kernel(float* __restrict__ crm, const int* __restrict__ lengths, int C, int T, int hop,
+                                        size_t n) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int b = (int)(i / ((size_t)C * T));
+    if ((int)(i % T) >= 1 + lengths[b] / hop) crm[i] = 0.f;
   }
 }
 
@@ -400,8 +438,9 @@ int istft_mask_adjoint_dft_launch(const float* dwav, const float* real, const fl
 static bool dft_size_ok(int n) { return !is_pow2(n) && (n & 1) == 0 && n >= 16 && n <= 1200; }
 
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
-                float* real, float* imag, float* magT, int T_pad, cudaStream_t st) {
+                float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens) {
   FSN_REQUIRE(B > 0 && L > 0, FSN_ERR_SHAPE, "stft: empty input (B=%d, L=%d)", B, L);
+  FSN_REQUIRE(!lens || is_pow2(n_fft), FSN_ERR_UNSUPPORTED, "stft: per-clip lengths need a power-of-two n_fft");
   if (dft_size_ok(n_fft)) {
     FSN_REQUIRE(hop > 0 && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE, "stft: bad hop/win_length");
     FSN_REQUIRE(n_fft / 2 < L, FSN_ERR_SHAPE, "stft: reflect padding %d needs L > pad (L=%d)", n_fft / 2, L);
@@ -425,7 +464,7 @@ int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_leng
   }
   dim3 grid(cdiv(Tg, kFR), B);
   stft_kernel<<<grid, kDspThreads, smem, st>>>(wav, L, n_fft, hop, win_length, T, mag, phase, real, imag, magT,
-                                               T_pad);
+                                               T_pad, lens);
   FSN_CHECK_LAUNCH("stft_kernel");
   return FSN_OK;
 }
@@ -450,8 +489,11 @@ int istft_mask_adjoint_launch(const float* dwav, const float* real, const float*
 }
 
 int istft_launch(const float* real, const float* imag, int cstride, const float* crm, int B, int T, int n_fft,
-                 int hop, int win_length, int length, float* wav, cudaStream_t st, int mask_mode, unsigned int* peak_bits) {
+                 int hop, int win_length, int length, float* wav, cudaStream_t st, int mask_mode, unsigned int* peak_bits,
+                 const int* lens) {
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "istft: empty input");
+  FSN_REQUIRE(!lens || (is_pow2(n_fft) && length > 0), FSN_ERR_UNSUPPORTED,
+              "istft: per-clip lengths need a power-of-two n_fft and an output length");
   if (peak_bits) {
     FSN_REQUIRE(!dft_size_ok(n_fft), FSN_ERR_UNSUPPORTED, "istft: the fused peak is built for the power-of-two transform");
     int rc = check_cuda(cudaMemsetAsync(peak_bits, 0, (size_t)B * sizeof(unsigned int), st), "istft peak memset");
@@ -482,7 +524,7 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
   }
   dim3 grid(cdiv(out_len, seg), B);
   istft_kernel<<<grid, kDspThreads, smem, st>>>(real, imag, cstride, crm, mask_mode, T, n_fft, hop, win_length, out_len,
-                                                seg, np_max, wav, peak_bits);
+                                                seg, np_max, wav, peak_bits, lens);
   FSN_CHECK_LAUNCH("istft_kernel");
   return FSN_OK;
 }
@@ -493,12 +535,13 @@ using namespace fsn;
 
 extern "C" int fsn_stft(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag,
                         float* phase, float* real, float* imag, float* magT, int T_pad, fsn_stream_t stream) {
-  return stft_launch(wav, B, L, n_fft, hop, win_length, mag, phase, real, imag, magT, T_pad, (cudaStream_t)stream);
+  return stft_launch(wav, B, L, n_fft, hop, win_length, mag, phase, real, imag, magT, T_pad, (cudaStream_t)stream, nullptr);
 }
 
 extern "C" int fsn_istft(const float* real, const float* imag, int cstride, const float* crm, int B, int T,
                          int n_fft, int hop, int win_length, int length, float* wav, fsn_stream_t stream) {
-  return istft_launch(real, imag, cstride, crm, B, T, n_fft, hop, win_length, length, wav, (cudaStream_t)stream, 1, nullptr);
+  return istft_launch(real, imag, cstride, crm, B, T, n_fft, hop, win_length, length, wav, (cudaStream_t)stream, 1, nullptr,
+                      nullptr);
 }
 
 extern "C" int fsn_peak_normalize_int16(const float* wav, int B, int L, float gain, int16_t* out, fsn_stream_t stream) {
@@ -517,10 +560,30 @@ extern "C" int fsn_si_sdr(const float* reference, const float* estimation, int B
 
 // int16 scaling with the per-clip peak the iSTFT epilogue produced (fsn_enhance_pcm)
 namespace fsn {
-int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st) {
+int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st,
+                       const int* lens) {
   const size_t n = (size_t)B * L;
-  scale_int16_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(wav, peak_bits, L, gain, out, n);
+  scale_int16_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(wav, peak_bits, L, gain, out, n, lens);
   FSN_CHECK_LAUNCH("scale_int16_kernel");
+  return FSN_OK;
+}
+
+int lengths_table_launch(const int32_t* host_lengths, int B, int* lengths, cudaStream_t st) {
+  LenChunk c;
+  for (int off = 0; off < B; off += kLenChunk) {
+    c.off = off;
+    c.n = B - off < kLenChunk ? B - off : kLenChunk;
+    memcpy(c.v, host_lengths + off, (size_t)c.n * sizeof(int));
+    lengths_table_kernel<<<cdiv(c.n, 256), 256, 0, st>>>(c, lengths);
+    FSN_CHECK_LAUNCH("lengths_table_kernel");
+  }
+  return FSN_OK;
+}
+
+int zero_frames_past_launch(float* crm, const int* lengths, int B, int C, int T, int hop, cudaStream_t st) {
+  const size_t n = (size_t)B * C * T;
+  zero_frames_past_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(crm, lengths, C, T, hop, n);
+  FSN_CHECK_LAUNCH("zero_frames_past_kernel");
   return FSN_OK;
 }
 }  // namespace fsn

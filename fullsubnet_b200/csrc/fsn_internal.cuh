@@ -225,20 +225,31 @@ int sb_fc_step_launch(const float* h, int R, int H, const float* W, const float*
 int sb_fc_steps_launch(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act, float* crm,
                        int Fsub, int T_out, int t_out0, cudaStream_t st);
 int transpose_mag_launch(const float* in, float* out, int B, int F, int T, int T_pad, cudaStream_t st);
-int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs, float2* sums, cudaStream_t st);
+// Per-clip lengths (lens non-null, device [B] samples): clip b sums only its own Tp_b = 1 + lens[b]/hop + la frames of
+// the T_pad-strided partials, with the same per-thread stride and tree as a call with T_pad = Tp_b; norm_scales_launch
+// then takes cnt1 / cnt2 per frame and multiplies them by Tp_b.
+int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs, float2* sums, cudaStream_t st,
+                      const int* lens = nullptr, int hop = 0, int la = 0);
 int clip_reduce_only_launch(const float2* fs, int B, int T_pad, float2* sums, cudaStream_t st);
 int norm_scales_launch(const float2* mag_sums, const float2* fb_sums, int B, float cnt1, float cnt2, float* inv1,
-                       float* inv2, cudaStream_t st, float eps = 1e-5f);
+                       float* inv2, cudaStream_t st, float eps = 1e-5f, const int* lens = nullptr, int hop = 0,
+                       int la = 0);
 
+// lens (nullable, device [B]): clip b has lens[b] of the L samples of its row (fsn_enhance_varlen); power-of-two n_fft
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
-                float* real, float* imag, float* magT, int T_pad, cudaStream_t st);
+                float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens = nullptr);
 // mask_mode: 1 = decompress_cIRM + complex product (fullsubnet), 2 = element-wise re*crm0, im*crm1 (improved_fullsubnet)
 int istft_launch(const float* real, const float* imag, int cstride, const float* crm, int B, int T, int n_fft,
                  int hop, int win_length, int length, float* wav, cudaStream_t st, int mask_mode = 1,
-                 unsigned int* peak_bits = nullptr);
+                 unsigned int* peak_bits = nullptr, const int* lens = nullptr);
 // peak_bits (optional, [B]): max|wav| per clip as float bits, reduced in the iSTFT epilogue; scale_int16_launch turns
 // it into the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:181-182)
-int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st);
+int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st,
+                       const int* lens = nullptr);
+// device int32 table lengths[B] <- host_lengths, through kernel parameters (the host array is not read after the call)
+int lengths_table_launch(const int32_t* host_lengths, int B, int* lengths, cudaStream_t st);
+// crm [B, C, T]: frames t >= 1 + lengths[b]/hop of clip b set to 0
+int zero_frames_past_launch(float* crm, const int* lengths, int B, int C, int T, int hop, cudaStream_t st);
 
 // adjoint of the element-wise mask + iSTFT of improved_fullsubnet (istft_launch mask_mode 2) with respect to the mask:
 // dwav [B,L] -> dcrm [B,2,F,T] for the rows f < F-1 (the Nyquist row of the cRM is a constant; it is not written)

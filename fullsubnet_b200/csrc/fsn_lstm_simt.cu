@@ -46,12 +46,15 @@ __global__ void frame_stats_kernel(const float* __restrict__ x, int rows, int F,
   if (lane == 0) fs[row] = make_float2(s0, s1);
 }
 
-// one CTA per clip: fixed-order tree sum over its T_pad frame partials (deterministic)
-__global__ void clip_reduce_kernel(const float2* __restrict__ fs, int T_pad, float2* __restrict__ sums) {
+// one CTA per clip: fixed-order tree sum over its T_pad frame partials (deterministic); lens (nullable): only the
+// clip's own 1 + lens[b]/hop + la frames
+__global__ void clip_reduce_kernel(const float2* __restrict__ fs, int T_pad, float2* __restrict__ sums,
+                                   const int* __restrict__ lens, int hop, int la) {
   __shared__ float2 sh[256];
   const int b = blockIdx.x;
+  const int Tn = lens ? 1 + lens[b] / hop + la : T_pad;
   float2 a = make_float2(0.f, 0.f);
-  for (int t = threadIdx.x; t < T_pad; t += 256) {
+  for (int t = threadIdx.x; t < Tn; t += 256) {
     const float2 v = fs[(size_t)b * T_pad + t];
     a.x += v.x; a.y += v.y;
   }
@@ -66,10 +69,18 @@ __global__ void clip_reduce_kernel(const float2* __restrict__ fs, int T_pad, flo
 
 // inv1[b] = 1/(mean(mag_pad)+1e-5)              (model.py:92)
 // inv2[b] = 1/(mean(cat(unfold(mag), unfold(fb)))+1e-5) via the closed form   (model.py:110-111)
+// lens (nullable): cnt1 / cnt2 are per frame, times the clip's 1 + lens[b]/hop + la frames (the float product the host
+// forms for a call on that clip alone)
 __global__ void norm_scales_kernel(const float2* __restrict__ mag_sums, const float2* __restrict__ fb_sums, int B,
-                                   float cnt1, float cnt2, float* __restrict__ inv1, float* __restrict__ inv2, float eps) {
+                                   float cnt1, float cnt2, float* __restrict__ inv1, float* __restrict__ inv2, float eps,
+                                   const int* __restrict__ lens, int hop, int la) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
+  if (lens) {
+    const float tp = (float)(1 + lens[b] / hop + la);
+    cnt1 = __fmul_rn(cnt1, tp);
+    cnt2 = __fmul_rn(cnt2, tp);
+  }
   if (inv1) inv1[b] = 1.0f / (mag_sums[b].x / cnt1 + eps);
   if (inv2) inv2[b] = 1.0f / ((mag_sums[b].y + fb_sums[b].y) / cnt2 + eps);
 }
@@ -409,24 +420,25 @@ int transpose_mag_launch(const float* in, float* out, int B, int F, int T, int T
   return FSN_OK;
 }
 
-int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs, float2* sums, cudaStream_t st) {
+int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs, float2* sums, cudaStream_t st,
+                      const int* lens, int hop, int la) {
   const int rows = B * T_pad;
   frame_stats_kernel<<<cdiv(rows, 8), 256, 0, st>>>(x, rows, F, N, fs);
   FSN_CHECK_LAUNCH("frame_stats_kernel");
-  clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums);
+  clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums, lens, hop, la);
   FSN_CHECK_LAUNCH("clip_reduce_kernel");
   return FSN_OK;
 }
 
 int clip_reduce_only_launch(const float2* fs, int B, int T_pad, float2* sums, cudaStream_t st) {
-  clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums);
+  clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums, nullptr, 0, 0);
   FSN_CHECK_LAUNCH("clip_reduce_kernel");
   return FSN_OK;
 }
 
 int norm_scales_launch(const float2* mag_sums, const float2* fb_sums, int B, float cnt1, float cnt2, float* inv1,
-                       float* inv2, cudaStream_t st, float eps) {
-  norm_scales_kernel<<<cdiv(B, 128), 128, 0, st>>>(mag_sums, fb_sums, B, cnt1, cnt2, inv1, inv2, eps);
+                       float* inv2, cudaStream_t st, float eps, const int* lens, int hop, int la) {
+  norm_scales_kernel<<<cdiv(B, 128), 128, 0, st>>>(mag_sums, fb_sums, B, cnt1, cnt2, inv1, inv2, eps, lens, hop, la);
   FSN_CHECK_LAUNCH("norm_scales_kernel");
   return FSN_OK;
 }

@@ -107,14 +107,21 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
   w.bytes = c.off;
 }
 
-// everything after the time-major magnitude exists: norms, full-band stack, sub-band stack
+// everything after the time-major magnitude exists: norms, full-band stack, sub-band stack.  lens (nullable, device
+// [B] samples, fsn_enhance_varlen): the offline norms of clip b cover only its own Tp_b = 1 + lens[b]/hop + look_ahead
+// frames; every other stage is causal and runs unchanged over all Tp steps (frames past Tp_b never reach earlier ones).
 static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                      const void* sb_packed, const Dims& m, const ModelWs& w, float* crm, cudaStream_t st) {
+                      const void* sb_packed, const Dims& m, const ModelWs& w, float* crm, cudaStream_t st,
+                      const int* lens = nullptr, int hop = 0) {
   int rc;
-  const int F = m.F, Tp = m.Tp, B = m.B, Hs = d->sb_hidden;
+  const int F = m.F, Tp = m.Tp, B = m.B, Hs = d->sb_hidden, la = d->look_ahead;
+  // with per-clip lengths the counts are per frame (norm_scales_launch multiplies by the clip's own frame count)
+  const int tp_cnt = lens ? 1 : Tp;
   // per-clip statistics of the look-ahead-padded magnitude (model.py:92, :111)
-  if ((rc = clip_stats_launch(w.magT, B, Tp, F, d->sb_num_neighbors, w.fs, w.sums_mag, st))) return rc;
-  if ((rc = norm_scales_launch(w.sums_mag, w.sums_mag, B, (float)F * Tp, 1.f, w.inv1, nullptr, st))) return rc;
+  if ((rc = clip_stats_launch(w.magT, B, Tp, F, d->sb_num_neighbors, w.fs, w.sums_mag, st, lens, hop, la))) return rc;
+  if ((rc = norm_scales_launch(w.sums_mag, w.sums_mag, B, (float)F * tp_cnt, 1.f, w.inv1, nullptr, st, 1e-5f, lens, hop,
+                               la)))
+    return rc;
   const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
   const float cum_eps = 1.1920928955078125e-07f;  // audio_zen/constant.py:9 (np.finfo(np.float32).eps)
   if (cum && (rc = cum_clip_scale_launch(w.fs, B, Tp, F, cum_eps, w.cum1, st))) return rc;
@@ -127,8 +134,9 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
   if ((rc = seq_stack_forward(s, w.fb, st))) return rc;
 
   // ---- second norm (model.py:110-111) in closed form: never materialise [B,F,Ksb,T']
-  if ((rc = clip_stats_launch(w.fbT, B, Tp, F, d->fb_num_neighbors, w.fs, w.sums_fb, st))) return rc;
-  if ((rc = norm_scales_launch(w.sums_mag, w.sums_fb, B, 1.f, (float)F * m.Ksb * Tp, nullptr, w.inv2, st)))
+  if ((rc = clip_stats_launch(w.fbT, B, Tp, F, d->fb_num_neighbors, w.fs, w.sums_fb, st, lens, hop, la))) return rc;
+  if ((rc = norm_scales_launch(w.sums_mag, w.sums_fb, B, 1.f, (float)F * m.Ksb * tp_cnt, nullptr, w.inv2, st, 1e-5f, lens,
+                               hop, la)))
     return rc;
 
   prof_mark(2, st);
@@ -248,13 +256,16 @@ extern "C" int fsn_model_forward(const fsn_model_desc* d, const fsn_seq_weights*
 struct EnhanceWs {
   float *real, *imag, *crm;
   unsigned int* peak;
+  int* lens;  // fsn_enhance_varlen: device copy of the per-clip lengths
   void* model;
   size_t bytes;
 };
 
 static int carve_enhance(const fsn_model_desc* d, int B, int L, int n_fft, int hop, void* base, EnhanceWs& e,
-                         Dims& m) {
+                         Dims& m, bool varlen = false) {
   FSN_REQUIRE(hop > 0 && n_fft > 0, FSN_ERR_SHAPE, "enhance: bad n_fft/hop");
+  FSN_REQUIRE(!varlen || (n_fft & (n_fft - 1)) == 0, FSN_ERR_UNSUPPORTED,
+              "enhance_varlen: n_fft=%d: per-clip lengths are built for the power-of-two (radix-2) transform", n_fft);
   const int T = 1 + L / hop;
   int rc = make_dims(d, B, T, m);
   if (rc) return rc;
@@ -266,6 +277,7 @@ static int carve_enhance(const fsn_model_desc* d, int B, int L, int n_fft, int h
   e.imag = c.take<float>(BFT);
   e.crm = c.take<float>(2 * BFT);
   e.peak = c.take<unsigned int>(B);
+  e.lens = varlen ? c.take<int>(B) : nullptr;
   ModelWs w;
   carve_model(d, m, nullptr, w);
   e.model = base ? (char*)base + c.off : nullptr;
@@ -273,18 +285,42 @@ static int carve_enhance(const fsn_model_desc* d, int B, int L, int n_fft, int h
   return FSN_OK;
 }
 
-extern "C" size_t fsn_enhance_workspace_bytes(const fsn_model_desc* d, int B, int L, int n_fft, int hop) {
+static size_t enhance_workspace_bytes(const fsn_model_desc* d, int B, int L, int n_fft, int hop, bool varlen) {
   EnhanceWs e;
   Dims m;
   fsn_model_desc dd = *d;
   dd.num_groups_in_drop_band = 1;
-  if (carve_enhance(&dd, B, L, n_fft, hop, nullptr, e, m)) return 0;
+  if (carve_enhance(&dd, B, L, n_fft, hop, nullptr, e, m, varlen)) return 0;
   return e.bytes;
 }
 
+extern "C" size_t fsn_enhance_workspace_bytes(const fsn_model_desc* d, int B, int L, int n_fft, int hop) {
+  return enhance_workspace_bytes(d, B, L, n_fft, hop, false);
+}
+
+// ---- clips of different lengths in one call (lengths non-null: host [B]): buffers laid out for the longest clip
+// (L = L_max samples, T_max frames), the length-dependent kernels (STFT, offline norms, iSTFT, int16 scaling) bounded
+// per clip by the device copy of the table
+extern "C" size_t fsn_enhance_varlen_workspace_bytes(const fsn_model_desc* d, int B, int L_max, int n_fft, int hop) {
+  return enhance_workspace_bytes(d, B, L_max, n_fft, hop, true);
+}
+
+static int check_lengths(const int32_t* lengths, int B, int L_max, int n_fft) {
+  int longest = 0;
+  for (int b = 0; b < B; ++b) {
+    FSN_REQUIRE(lengths[b] > n_fft / 2 && lengths[b] <= L_max, FSN_ERR_SHAPE,
+                "enhance_varlen: clip %d has length %d, outside (n_fft/2, L_max] = (%d, %d]", b, lengths[b], n_fft / 2,
+                L_max);
+    longest = lengths[b] > longest ? lengths[b] : longest;
+  }
+  FSN_REQUIRE(longest == L_max, FSN_ERR_SHAPE, "enhance_varlen: the longest clip has %d samples, L_max = %d", longest,
+              L_max);
+  return FSN_OK;
+}
+
 static int enhance_impl(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                        const void* sb_packed, const float* wav, int B, int L, int n_fft, int hop, int win_length,
-                        float* enhanced, float* crm_out, int16_t* pcm, float pcm_gain, void* workspace,
+                        const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L, int n_fft, int hop,
+                        int win_length, float* enhanced, float* crm_out, int16_t* pcm, float pcm_gain, void* workspace,
                         size_t workspace_bytes, fsn_stream_t stream) {
   g_launches = 0;
   // batched inference == loop of B=1 calls of the reference inferencer: drop_band off
@@ -293,10 +329,11 @@ static int enhance_impl(const fsn_model_desc* d, const fsn_seq_weights* fb, cons
   dd.num_groups_in_drop_band = 1;
   EnhanceWs e;
   Dims m;
-  int rc = carve_enhance(&dd, B, L, n_fft, hop, workspace, e, m);
+  int rc = carve_enhance(&dd, B, L, n_fft, hop, workspace, e, m, lengths != nullptr);
   if (rc) return rc;
   FSN_REQUIRE(dd.precision == FSN_PREC_FP32 || sb_tc_supported(&dd), FSN_ERR_UNSUPPORTED,
               "FSN_PREC_F16_TC / FSN_PREC_F16X3_TC need sb_hidden in {128,256,384} and sub-band input width <= 32");
+  if (lengths && (rc = check_lengths(lengths, B, L, n_fft))) return rc;
   FSN_REQUIRE(workspace && workspace_bytes >= e.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, e.bytes);
   ModelWs w;
@@ -305,12 +342,15 @@ static int enhance_impl(const fsn_model_desc* d, const fsn_seq_weights* fb, cons
   float* crm = crm_out ? crm_out : e.crm;
   prof_reset();
   prof_mark(0, st);
-  if ((rc = stft_launch(wav, B, L, n_fft, hop, win_length, nullptr, nullptr, e.real, e.imag, w.magT, m.Tp, st)))
+  if (lengths && (rc = lengths_table_launch(lengths, B, e.lens, st))) return rc;
+  if ((rc = stft_launch(wav, B, L, n_fft, hop, win_length, nullptr, nullptr, e.real, e.imag, w.magT, m.Tp, st, e.lens)))
     return rc;
   prof_mark(1, st);
-  if ((rc = model_core(&dd, fb, sb, sb_packed, m, w, crm, st))) return rc;
-  rc = istft_launch(e.real, e.imag, 1, crm, B, m.T, n_fft, hop, win_length, L, enhanced, st, 1, pcm ? e.peak : nullptr);
-  if (!rc && pcm) rc = scale_int16_launch(enhanced, e.peak, B, L, pcm_gain, pcm, st);
+  if ((rc = model_core(&dd, fb, sb, sb_packed, m, w, crm, st, e.lens, hop))) return rc;
+  rc = istft_launch(e.real, e.imag, 1, crm, B, m.T, n_fft, hop, win_length, L, enhanced, st, 1, pcm ? e.peak : nullptr,
+                    e.lens);
+  if (!rc && pcm) rc = scale_int16_launch(enhanced, e.peak, B, L, pcm_gain, pcm, st, e.lens);
+  if (!rc && lengths && crm_out) rc = zero_frames_past_launch(crm_out, e.lens, B, 2 * m.F, m.T, hop, st);
   prof_mark(4, st);
   return rc;
 }
@@ -319,8 +359,8 @@ extern "C" int fsn_enhance(const fsn_model_desc* d, const fsn_seq_weights* fb, c
                            const void* sb_packed, const float* wav, int B, int L, int n_fft, int hop,
                            int win_length, float* enhanced, float* crm_out, void* workspace,
                            size_t workspace_bytes, fsn_stream_t stream) {
-  return enhance_impl(d, fb, sb, sb_packed, wav, B, L, n_fft, hop, win_length, enhanced, crm_out, nullptr, 0.f, workspace,
-                      workspace_bytes, stream);
+  return enhance_impl(d, fb, sb, sb_packed, wav, nullptr, B, L, n_fft, hop, win_length, enhanced, crm_out, nullptr, 0.f,
+                      workspace, workspace_bytes, stream);
 }
 
 extern "C" int fsn_enhance_pcm(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
@@ -328,6 +368,15 @@ extern "C" int fsn_enhance_pcm(const fsn_model_desc* d, const fsn_seq_weights* f
                                int win_length, float* enhanced, int16_t* pcm, float gain, void* workspace,
                                size_t workspace_bytes, fsn_stream_t stream) {
   FSN_REQUIRE(pcm && enhanced, FSN_ERR_SHAPE, "enhance_pcm: output buffers missing");
-  return enhance_impl(d, fb, sb, sb_packed, wav, B, L, n_fft, hop, win_length, enhanced, nullptr, pcm, gain, workspace,
-                      workspace_bytes, stream);
+  return enhance_impl(d, fb, sb, sb_packed, wav, nullptr, B, L, n_fft, hop, win_length, enhanced, nullptr, pcm, gain,
+                      workspace, workspace_bytes, stream);
+}
+
+extern "C" int fsn_enhance_varlen(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                                  const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L_max,
+                                  int n_fft, int hop, int win_length, float* enhanced, float* crm_out, int16_t* pcm,
+                                  float gain, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  FSN_REQUIRE(lengths, FSN_ERR_SHAPE, "enhance_varlen: lengths missing");
+  return enhance_impl(d, fb, sb, sb_packed, wav, lengths, B, L_max, n_fft, hop, win_length, enhanced, crm_out, pcm, gain,
+                      workspace, workspace_bytes, stream);
 }

@@ -10,6 +10,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
 import torch
 
 from .. import _lib
@@ -135,14 +136,56 @@ class Model(BaseModel):
                                              ws_bytes, _lib.stream_ptr(device)))
         return out
 
+    @staticmethod
+    def _lengths_table(lengths, B, L):
+        """Per-clip lengths (sequence of B ints or a CPU integer tensor) -> contiguous int32 host array."""
+        if isinstance(lengths, torch.Tensor):
+            if lengths.is_cuda or lengths.is_floating_point() or lengths.is_complex() or lengths.dim() != 1:
+                raise ValueError("lengths must be a 1-D CPU integer tensor or a sequence of ints")
+            lengths = lengths.tolist()
+        lens = np.ascontiguousarray([int(v) for v in lengths], dtype=np.int32)
+        if lens.shape != (B,):
+            raise ValueError(f"lengths has {lens.size} entries for a batch of {B} clips")
+        if lens.size and int(lens.max()) > L:
+            b = int(lens.argmax())
+            raise ValueError(f"lengths[{b}] = {int(lens[b])} exceeds the {L} samples of a row")
+        return lens
+
+    def _enhance_varlen(self, x, lens, n_fft, hop_length, win_length, crm, pcm, gain):
+        """One fsn_enhance_varlen call: clip b is row b's first lens[b] samples; out [B,L] is 0 past them."""
+        B, L = x.shape
+        device = x.device
+        lib = _lib.load()
+        with torch.cuda.device(device):
+            desc, fb_w, sb_w, packed = self._prepare(device, 1)
+            ws_bytes = _lib.check_workspace(lib.fsn_enhance_varlen_workspace_bytes(C.byref(desc), B, L, n_fft, hop_length))
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+            out = torch.empty(B, L, dtype=torch.float32, device=device)
+            _lib.check(lib.fsn_enhance_varlen(C.byref(desc), C.byref(fb_w), C.byref(sb_w), _lib.ptr(packed), x.data_ptr(),
+                                              lens.ctypes.data, B, L, n_fft, hop_length, win_length, out.data_ptr(),
+                                              _lib.ptr(crm), _lib.ptr(pcm), float(gain), ws.data_ptr(), ws_bytes,
+                                              _lib.stream_ptr(device)))
+        return out
+
     @torch.no_grad()
-    def enhance(self, noisy, n_fft=512, hop_length=256, win_length=512, return_crm=False):
+    def enhance(self, noisy, n_fft=512, hop_length=256, win_length=512, return_crm=False, lengths=None):
         """Fused wav -> wav path of Inferencer.full_band_crm_mask (recipes/.../inferencer.py:130-145),
-        batched over independent clips: noisy [B,L] -> enhanced [B,L]."""
+        batched over independent clips: noisy [B,L] -> enhanced [B,L].
+
+        ``lengths`` (B ints, or a CPU integer tensor; max must be L): clips of different lengths in one call
+        (fsn_enhance_varlen).  Clip b is ``noisy[b, :lengths[b]]``; the rest of the row is never read.  Its outputs
+        equal the call on that clip alone, bit for bit; ``enhanced[b, lengths[b]:]`` and the cRM frames
+        ``t >= 1 + lengths[b] // hop_length`` are 0."""
         assert noisy.dim() == 2, "noisy must be [B, L]"
+        lens = None if lengths is None else self._lengths_table(lengths, *noisy.shape)
         x = _lib.require_cuda(noisy, "noisy")
         B, L = x.shape
         device = x.device
+        if lens is not None:
+            crm = torch.empty(B, 2, n_fft // 2 + 1, 1 + L // hop_length, dtype=torch.float32,
+                              device=device) if return_crm else None
+            out = self._enhance_varlen(x, lens, n_fft, hop_length, win_length, crm, None, 0.0)
+            return (out, crm) if return_crm else out
         lib = _lib.load()
         with torch.cuda.device(device):
             desc, fb_w, sb_w, packed = self._prepare(device, 1)
@@ -159,14 +202,19 @@ class Model(BaseModel):
         return (out, crm) if return_crm else out
 
     @torch.no_grad()
-    def enhance_pcm(self, noisy, n_fft=512, hop_length=256, win_length=512, gain=0.8 * 32767.0):
+    def enhance_pcm(self, noisy, n_fft=512, hop_length=256, win_length=512, gain=0.8 * 32767.0, lengths=None):
         """``enhance`` plus the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:
         181-182) in the same library call (fsn_enhance_pcm: per-clip max|y| reduced in the iSTFT epilogue):
-        noisy [B,L] -> (enhanced float32 [B,L], pcm int16 [B,L])."""
+        noisy [B,L] -> (enhanced float32 [B,L], pcm int16 [B,L]).  ``lengths``: as in ``enhance``; each clip is
+        scaled by the peak of its own samples and its pcm row is 0 past them."""
         assert noisy.dim() == 2, "noisy must be [B, L]"
+        lens = None if lengths is None else self._lengths_table(lengths, *noisy.shape)
         x = _lib.require_cuda(noisy, "noisy")
         B, L = x.shape
         device = x.device
+        if lens is not None:
+            pcm = torch.empty(B, L, dtype=torch.int16, device=device)
+            return self._enhance_varlen(x, lens, n_fft, hop_length, win_length, None, pcm, gain), pcm
         lib = _lib.load()
         with torch.cuda.device(device):
             desc, fb_w, sb_w, packed = self._prepare(device, 1)

@@ -18,6 +18,34 @@ from .acoustics.mask import decompress_cIRM
 from .utils import initialize_module, prepare_device
 
 
+def plan_batches(lengths, batch_size: int, max_padding: float = 0.0):
+    """Batches of clip indices for the file loop.  ``max_padding == 0``: clips of exactly equal length, at most
+    ``batch_size`` per batch (shortest length first, file order within a length).  ``max_padding > 0``: the clips sorted
+    by length are cut into consecutive runs of at most ``batch_size`` clips whose padding -- B * L_max minus the samples
+    of the B clips -- stays within ``max_padding * B * L_max``; one such batch is one library call with per-clip
+    lengths."""
+    if batch_size < 1:
+        raise ValueError("batch_size must be >= 1")
+    if not 0.0 <= max_padding < 1.0:
+        raise ValueError("max_padding must be in [0, 1)")
+    lens = [int(v) for v in lengths]
+    order = sorted(range(len(lens)), key=lambda i: (lens[i], i))
+    batches, cur, total = [], [], 0
+    for i in order:
+        L = lens[i]  # the longest of cur + [i]: ascending order
+        n = len(cur) + 1
+        fits = len(cur) < batch_size and (n * L - (total + L) <= max_padding * n * L if max_padding > 0 else
+                                          (not cur or lens[cur[0]] == L))
+        if cur and not fits:
+            batches.append(cur)
+            cur, total = [], 0
+        cur.append(i)
+        total += L
+    if cur:
+        batches.append(cur)
+    return batches
+
+
 class Inferencer:
     def __init__(self, config: Optional[dict] = None, checkpoint_path=None, output_dir=None, model=None,
                  device=None):
@@ -60,13 +88,23 @@ class Inferencer:
         enhanced = enhanced.detach().squeeze(0).cpu().numpy()
         return enhanced
 
+    def supports_lengths(self) -> bool:
+        """Whether clips of different lengths can share one call (fullsubnet with a power-of-two n_fft)."""
+        return hasattr(self.model, "enhance") and self.n_fft & (self.n_fft - 1) == 0
+
+    def _check_lengths(self, lengths) -> None:
+        if lengths is not None and not hasattr(self.model, "enhance"):
+            raise NotImplementedError(f"{type(self.model).__module__}: per-clip lengths are built for fullsubnet only")
+
     @torch.no_grad()
-    def enhance_batch(self, noisy: torch.Tensor) -> torch.Tensor:
+    def enhance_batch(self, noisy: torch.Tensor, lengths=None) -> torch.Tensor:
         """The same path for B independent clips in ONE library call (fsn_enhance): pinned/host or device
-        ``noisy`` [B,L] -> device tensor [B,L].  Equivalent to looping full_band_crm_mask over the clips."""
+        ``noisy`` [B,L] -> device tensor [B,L].  Equivalent to looping full_band_crm_mask over the clips.
+        ``lengths`` (fullsubnet only): clip b is ``noisy[b, :lengths[b]]`` (fsn_enhance_varlen), its row 0 past it."""
+        self._check_lengths(lengths)
         x = noisy.to(self.device, non_blocking=True)
         if hasattr(self.model, "enhance"):  # fullsubnet: one fused library call
-            return self.model.enhance(x, self.n_fft, self.hop_length, self.win_length)
+            return self.model.enhance(x, self.n_fft, self.hop_length, self.win_length, lengths=lengths)
         # other models (fast_fullsubnet): same flow, three library calls (stft -> model -> mask + istft)
         import ctypes as C  # noqa: F401
         from . import _lib
@@ -86,14 +124,16 @@ class Inferencer:
         return out
 
     @torch.no_grad()
-    def enhance_to_pcm(self, noisy: torch.Tensor) -> torch.Tensor:
+    def enhance_to_pcm(self, noisy: torch.Tensor, lengths=None) -> torch.Tensor:
         """enhance_batch + the int16 scaling of base_inferencer.py:181-182 on the device: noisy [B,L] -> int16 [B,L]
-        (what the reference hands to ``sf.write``); only B*L*2 bytes come back to the host."""
+        (what the reference hands to ``sf.write``); only B*L*2 bytes come back to the host.  ``lengths``: as in
+        ``enhance_batch``; each clip is scaled by its own peak."""
         from . import _lib
-        if hasattr(self.model, "enhance_pcm") and self.n_fft & (self.n_fft - 1) == 0:
+        self._check_lengths(lengths)
+        if lengths is not None or (hasattr(self.model, "enhance_pcm") and self.n_fft & (self.n_fft - 1) == 0):
             x = noisy.to(self.device, non_blocking=True)  # fused: peak in the iSTFT epilogue, one scaling pass
             return self.model.enhance_pcm(x, self.n_fft, self.hop_length, self.win_length,
-                                          gain=0.8 * float(np.iinfo(np.int16).max))[1]
+                                          gain=0.8 * float(np.iinfo(np.int16).max), lengths=lengths)[1]
         enhanced = self.enhance_batch(noisy)
         B, L = enhanced.shape
         pcm = torch.empty(B, L, dtype=torch.int16, device=enhanced.device)
@@ -162,32 +202,33 @@ class Inferencer:
         return (vals * w).sum(axis=1).astype(np.float32)
 
     @torch.no_grad()
-    def enhance_files(self, paths, output_dir, batch_size: int = 64, sr=None):
-        """Batched form of the host loop of base_inferencer.py:163-195: files are grouped by length (a clip's result
-        depends on its own length through the per-clip norms, so clips are never padded), each group goes through ONE
-        fused library call per ``batch_size`` clips (pinned staging buffer -> H2D -> fsn_enhance_pcm -> int16 D2H), and
-        ``<output_dir>/<stem>.wav`` is written as 16-bit PCM like the reference.  Returns the written paths."""
-        from collections import defaultdict
+    def enhance_files(self, paths, output_dir, batch_size: int = 64, sr=None, max_padding: float = 0.0):
+        """Batched form of the host loop of base_inferencer.py:163-195: ``plan_batches`` groups the files, each batch
+        goes through ONE fused library call (pinned staging buffer -> H2D -> fsn_enhance_pcm -> int16 D2H), and
+        ``<output_dir>/<stem>.wav`` is written as 16-bit PCM like the reference.  Returns the written paths.
+
+        ``max_padding == 0`` (default): batches of equal-length clips only.  ``max_padding > 0`` (fullsubnet with a
+        power-of-two n_fft; other models keep equal-length batches): clips of different lengths share a batch, padded
+        to its longest clip by at most that fraction of the batch's samples, through fsn_enhance_varlen.  Every file
+        is bit-identical either way: each clip is bounded by its own length in the length-dependent kernels."""
         from pathlib import Path
         sr = int(sr or self.sr)
         out_dir = Path(output_dir)
         out_dir.mkdir(parents=True, exist_ok=True)
         clips = [(Path(p), self.load_wav(p, sr)) for p in paths]
-        groups = defaultdict(list)
-        for i, (_, y) in enumerate(clips):
-            groups[len(y)].append(i)
+        lens = [len(y) for _, y in clips]
         written = [None] * len(clips)
-        for L, idxs in sorted(groups.items()):
-            for s0 in range(0, len(idxs), batch_size):
-                chunk = idxs[s0:s0 + batch_size]
-                stage = torch.empty(len(chunk), L, dtype=torch.float32).pin_memory()
-                for r, i in enumerate(chunk):
-                    stage[r] = torch.from_numpy(clips[i][1])
-                pcm = self.enhance_to_pcm(stage).cpu().numpy()
-                for r, i in enumerate(chunk):
-                    dst = out_dir / f"{clips[i][0].stem}.wav"
-                    self.write_wav(dst, pcm[r], sr)
-                    written[i] = dst
+        for chunk in plan_batches(lens, batch_size, max_padding if self.supports_lengths() else 0.0):
+            L = max(lens[i] for i in chunk)
+            mixed = any(lens[i] != L for i in chunk)
+            stage = (torch.zeros if mixed else torch.empty)(len(chunk), L, dtype=torch.float32).pin_memory()
+            for r, i in enumerate(chunk):
+                stage[r, :lens[i]] = torch.from_numpy(clips[i][1])
+            pcm = self.enhance_to_pcm(stage, lengths=[lens[i] for i in chunk] if mixed else None).cpu().numpy()
+            for r, i in enumerate(chunk):
+                dst = out_dir / f"{clips[i][0].stem}.wav"
+                self.write_wav(dst, pcm[r, :lens[i]], sr)
+                written[i] = dst
         return written
 
     @torch.no_grad()

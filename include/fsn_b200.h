@@ -166,6 +166,22 @@ int fsn_enhance_pcm(const fsn_model_desc* d, const fsn_seq_weights* fb, const fs
                     const void* sb_packed, const float* wav, int B, int L, int n_fft, int hop, int win_length,
                     float* enhanced, int16_t* pcm, float gain, void* workspace, size_t workspace_bytes,
                     fsn_stream_t stream);
+/* Clips of different lengths in one call.  Row b of wav [B, L_max] holds clip b's lengths[b] samples; samples at index
+ * >= lengths[b] are never read.  lengths: HOST int32 [B], n_fft/2 < lengths[b] <= L_max and max(lengths) == L_max
+ * (else FSN_ERR_SHAPE naming the clip); it is copied into the workspace through kernel parameters during the call and
+ * not retained, so it may be pageable and may be reused as soon as the call returns.  Outputs, T_max = 1 + L_max/hop:
+ *   enhanced [B, L_max]           0 past lengths[b]
+ *   crm_out  [B, 2, F, T_max]     nullable; 0 for frames t >= T_b = 1 + lengths[b]/hop
+ *   pcm      [B, L_max] int16     nullable; int16(gain * y / max|y|) over the clip's own samples, 0 past lengths[b]
+ * Every clip's outputs are bit-identical to fsn_enhance / fsn_enhance_pcm on that clip alone with L = lengths[b]: the
+ * recurrent stages are causal, so they run over T_max + look_ahead steps for every clip, and only the STFT, the offline
+ * norms, the iSTFT and the int16 scaling are bounded per clip.  Same precisions, cells and norms as fsn_enhance
+ * (drop_band off); n_fft must be a power of two (else FSN_ERR_UNSUPPORTED).  Never synchronises the host. */
+size_t fsn_enhance_varlen_workspace_bytes(const fsn_model_desc* d, int B, int L_max, int n_fft, int hop);
+int fsn_enhance_varlen(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                       const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L_max, int n_fft,
+                       int hop, int win_length, float* enhanced, float* crm_out, int16_t* pcm, float gain,
+                       void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * recipes/dns_interspeech_2020/fast_fullsubnet/model.py:11-202  Model (BASELINE config 4, SURVEY 8a row A13)
@@ -254,7 +270,7 @@ int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improved_weights*
 int fsn_set_profiling(int enable);
 float fsn_last_stage_ms(int stage);
 
-/* number of kernel launches issued by the last fsn_model_forward / fsn_enhance on this thread
+/* number of kernel launches issued by the last fsn_model_forward / fsn_enhance (/ _pcm / _varlen) on this thread
  * (bench.py reports it as gpu_launches) */
 int64_t fsn_last_launch_count(void);
 /* kernels launched by this library since it was loaded (never reset): difference two readings */
