@@ -249,16 +249,18 @@ template <bool X3> __device__ __forceinline__ float th(float x) { return X3 ? 1.
 
 // Consumer warpgroup releases weight stage `bar` to the producers of the CL CTAs that share the stream (the CTAs of
 // the same half, ranks 2 q + half): one arrive per warpgroup and destination CTA (w_empty counts CL), warp q
-// signalling pair q so that the remote arrives go out in parallel.  No fence is needed: the stage is read only by
+// signalling pair q so that the remote arrives go out in parallel (`local`: CL = 1 and q = 0; `remote`: CL > 1 and
+// q < CL; both warp-uniform, so the arrives are predicated instructions of one elected lane and the stage loop has no
+// divergent region).  `pred`: there is a stage to release.  No fence is needed: the stage is read only by
 // this warpgroup's wgmma (async proxy), the wgmma.wait_group before this call has retired those reads, and the
 // producers overwrite the stage with TMA (async proxy) only after the w_empty phase completes - the barrier phase
 // alone orders the overwrite after the reads, so the arrive keeps its default .release.cta semantics (the hand-off of
 // CUTLASS's TMA pipelines for the same hazard).  Every warp of the warpgroup has passed the w_full wait of the stage:
 // the MMAs that read it are warpgroup-collective.
-__device__ __forceinline__ void release_stage(uint64_t* bar, int CL, int half, int q, int lane) {
-  if (lane != 0 || q >= CL) return;
-  if (CL == 1) mbar_arrive(bar);
-  else mbar_arrive_remote(bar, (uint32_t)(2 * q + half));
+__device__ __forceinline__ void release_stage(uint32_t bar, uint32_t pred, uint32_t local, uint32_t remote,
+                                              uint32_t rank) {
+  mbar_arrive_elect_if(bar, pred & local);
+  mbar_arrive_remote_elect_if(bar, rank, pred & remote);
 }
 
 // PROBE: the same kernel with cycle stamps (ProbeField) written to a.stamps; the production launches use PROBE = false,
@@ -475,8 +477,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
     // both layers.  Fragment of thread (warp q, lane l): unit 64 s + 16 q + l/4 + 8 hh, row n = 8 j + 2 (l%4) + e,
     // register acc[g][4 j + 2 hh + e]
     asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
-    const int m = (warp - 4) >> 2;
-    const int q = warp & 3;
+    // warpgroup and warp index broadcast from lane 0, so that the compiler knows them warp-uniform: the barrier
+    // addresses and MMA descriptor words of the stage loop can then live in uniform registers
+    const int m = __shfl_sync(0xffffffffu, (warp - 4) >> 2, 0);
+    const int q = __shfl_sync(0xffffffffu, warp & 3, 0);
     const int s = half * MT + m;
     if (m < MT) {
       const float* bias_g = reinterpret_cast<const float*>(a.packed + PL.off_bias);
@@ -485,7 +489,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
       float c0[16], c1[16];
 #pragma unroll
       for (int i = 0; i < 16; ++i) c0[i] = c1[i] = 0.f;
-      const uint32_t wbase = smem_u32(smem + sp.w);
+      // per-kernel constants of the stage loop: the A descriptor of ring slot 0 (a slot is W_TILE >> 4 further), the
+      // barriers, and which warps release a stage where (see release_stage)
+      const uint32_t a_lo0 = wg::desc_lo(smem_u32(smem + sp.w));
+      const uint32_t w_full0 = smem_u32(&bars.w_full[0]), w_empty0 = smem_u32(&bars.w_empty[0]);
+      const uint32_t turn_next = smem_u32(&bars.turn[m + 1 < MT ? m + 1 : 0]);
+      const uint32_t rel_local = CL == 1 && q == 0, rel_remote = CL > 1 && q < CL;
+      const uint32_t rel_rank = 2 * q + half;
       int h0_seen = 0, h1_seen = 0, turns = 0;
       bool first_block = true;
       size_t tile_base = 0;  // index (in this half's stream) of this iteration's first stage
@@ -513,7 +523,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
           const uint32_t h0_cur = smem_u32(smem + sp.h0 + (t & 1) * nkh * S_KBLK);        // h0_t
           const uint32_t h0_prev = smem_u32(smem + sp.h0 + ((t + 1) & 1) * nkh * S_KBLK);  // h0_{t-1}
           const uint32_t h1_prev = smem_u32(smem + sp.h1);                                    // h1_{t-1}
-          // B operand k ranges: layer 0: [x_t (32 k)] [h0_{t-1} (H)]; layer 1: [h0_t (H)] [h1_{t-1} (H)]
           const int nkb = layer ? PL.nkb1 : PL.nkb0;
           const size_t first = tile_base + (layer ? ((it < Tp) ? PL.tiles0 : 0) : 0) + (size_t)m * nkb * PARTS;
           float acc[4][16];
@@ -529,55 +538,70 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
           p_turn += mark();
           p_mma0 = pt;
           // ring slot and fill parity of stream stage `first`, then advanced stage by stage
-          int stage = (int)(first % (size_t)STAGES);
-          uint32_t wphase = (uint32_t)((first / (size_t)STAGES) & 1);
-          for (int j = 0; j < nkb; ++j) {
-            // state descriptors of k range j: x_t is one 64B-swizzled block of 32 k, h the 128B-swizzled k-blocks
-            const bool xr = layer == 0 && j == 0;
-            uint32_t sb;
-            if (layer == 0) sb = xr ? x_addr : h0_prev + ((j - 1) >> 1) * S_KBLK + ((j - 1) & 1) * 64;
-            else sb = (j < H / KS) ? h0_cur + (j >> 1) * S_KBLK + (j & 1) * 64
-                                   : h1_prev + ((j - H / KS) >> 1) * S_KBLK + ((j - H / KS) & 1) * 64;
+          // (broadcast from lane 0 like m and q: warp-uniform by construction)
+          int stage = __shfl_sync(0xffffffffu, (int)(first % (size_t)STAGES), 0);
+          uint32_t wphase = __shfl_sync(0xffffffffu, (uint32_t)((first / (size_t)STAGES) & 1), 0);
+          // one ring stage against the state k range of descriptor `bd` (lo copy LO bytes further): wait for it to
+          // land, issue its MMAs (x3 hi part: hi.hi and hi.lo per gate and k16; lo part and single pass: one per gate
+          // and k16), commit, retire the previous stage's group and release that stage.  `ends_block`: the block's
+          // last stage, after whose landing the next warpgroup in the stream may take the ring
+          auto issue_stage = [&](int part, uint32_t bd, uint32_t b_hi, uint32_t ends_block) {
+            mark();
+            mbar_wait_cta_warp(w_full0 + 8 * stage, wphase);
+            p_wfull += mark();
+            mbar_arrive_elect_if(turn_next, ends_block);
+            wg::fence();
+            const uint32_t ad = a_lo0 + stage * (W_TILE >> 4);
 #pragma unroll
-            for (int part = 0; part < PARTS; ++part) {
-              mark();
-              mbar_wait_cta<false>(&bars.w_full[stage], wphase);
-              p_wfull += mark();
-              if (j == nkb - 1 && part == PARTS - 1 && lane == 0) mbar_arrive(&bars.turn[m + 1 < MT ? m + 1 : 0]);
-              wg::fence();
-              const uint32_t wa = wbase + stage * W_TILE;
+            for (int kk = 0; kk < 2; ++kk)
 #pragma unroll
-              for (int kk = 0; kk < 2; ++kk) {
-                const uint64_t bd = xr ? wg::desc_sw64(sb + kk * 32) : wg::desc_sw128(sb + kk * 32);
-                const uint64_t bl = xr ? wg::desc_sw64(sb + LO + kk * 32) : wg::desc_sw128(sb + LO + kk * 32);
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                  const uint64_t ad = wg::desc_sw64(wa + g * W_SUB + kk * 32);
-                  wg::mma_f16_n32(acc[g], ad, bd, 1u);
-                  if (X3 && part == 0) wg::mma_f16_n32(acc[g], ad, bl, 1u);
-                }
+              for (int g = 0; g < 4; ++g) {
+                const uint32_t a_off = g * (W_SUB >> 4) + kk * 2;
+                wg::mma_f16_n32_w(acc[g], ad, a_off, wg::DESC_SW64_HI, bd, kk * 2, b_hi);
+                if (X3 && part == 0) wg::mma_f16_n32_w(acc[g], ad, a_off, wg::DESC_SW64_HI, bd, (LO >> 4) + kk * 2, b_hi);
               }
-              wg::commit();
-              if constexpr (PROBE) p_commit = clock64();
-              mark();
-              wg::wait<1>();  // the MMAs of the previous stage have read it
-              p_wgw += mark();
-              if constexpr (PROBE) {
-                if (prev_stage >= 0) p_lat += (uint32_t)(pt - p_commit_prev);
-                p_commit_prev = p_commit;
-              }
-              if (prev_stage >= 0) release_stage(&bars.w_empty[prev_stage], CL, half, q, lane);
-              prev_stage = stage;
-              if (++stage == STAGES) { stage = 0; wphase ^= 1; }
+            wg::commit();
+            if constexpr (PROBE) p_commit = clock64();
+            mark();
+            wg::wait<1>();  // the MMAs of the previous stage have read it
+            p_wgw += mark();
+            if constexpr (PROBE) {
+              if (prev_stage >= 0) p_lat += (uint32_t)(pt - p_commit_prev);
+              p_commit_prev = p_commit;
             }
+            release_stage(w_empty0 + 8 * prev_stage, prev_stage >= 0, rel_local, rel_remote, rel_rank);
+            prev_stage = stage;
+            if (++stage == STAGES) { stage = 0; wphase ^= 1; }
+          };
+          // B operand k ranges: layer 0: [x_t (32 k, one 64B-swizzled block)] [h0_{t-1} (H)]; layer 1: [h0_t (H)]
+          // [h1_{t-1} (H)].  A k-block of h (64 k, 128B-swizzled) is two k ranges, 64 B apart in the swizzle row
+          if (layer == 0) {
+#pragma unroll
+            for (int part = 0; part < PARTS; ++part) issue_stage(part, wg::desc_lo(x_addr), wg::DESC_SW64_HI, 0u);
           }
+          // (do-while: H >= 128, so every segment has k-blocks and the loops need no entry test)
+          const int nseg = layer ? 2 : 1;
+          int seg = 0;
+          do {
+            uint32_t bd = wg::desc_lo(layer == 0 ? h0_prev : seg == 0 ? h0_cur : h1_prev);
+            int kb = 0;
+            do {
+              const uint32_t ends_block = seg == nseg - 1 && kb == nkh - 1;
+#pragma unroll
+              for (int part = 0; part < PARTS; ++part) issue_stage(part, bd, wg::DESC_SW128_HI, 0u);
+#pragma unroll
+              for (int part = 0; part < PARTS; ++part)
+                issue_stage(part, bd + (64 >> 4), wg::DESC_SW128_HI, part == PARTS - 1 ? ends_block : 0u);
+              bd += S_KBLK >> 4;
+            } while (++kb < nkh);
+          } while (++seg < nseg);
           mark();
           wg::wait<0>();
 #pragma unroll
           for (int g = 0; g < 4; ++g) wg::fence_operand(acc[g]);
           p_wgw += mark();
           if constexpr (PROBE) { p_lat += (uint32_t)(pt - p_commit_prev); p_mma1 = pt; }
-          release_stage(&bars.w_empty[prev_stage], CL, half, q, lane);
+          release_stage(w_empty0 + 8 * prev_stage, 1u, rel_local, rel_remote, rel_rank);
           // this warpgroup's MMAs of the step have consumed x_t / h1_{t-1}
           if (lane == 0) mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
           if (layer == 1 && lane == 0) {

@@ -117,6 +117,46 @@ __device__ __forceinline__ void mbar_wait_cta(uint64_t* bar, uint32_t parity) {
     if (++spins > (SLEEP ? (1u << 24) : (1u << 27))) asm volatile("trap;");
   }
 }
+// the wait of mbar_wait_cta<false> for a whole warp at once, with the poll loop inside one asm block: the warp leaves
+// the loop together (vote.all), so the compiler sees no divergent region to reconverge and can keep a warp-uniform
+// barrier address and parity in uniform registers.  Same watchdog (trap after 2^27 polls)
+__device__ __forceinline__ void mbar_wait_cta_warp(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b32 n;\n\t"
+      "mov.b32 n, 0;\n"
+      "WAIT:\n\t"
+      "mbarrier.try_wait.parity.acquire.cta.shared::cta.b64 p, [%0], %1;\n\t"
+      "vote.sync.all.pred p, p, 0xffffffff;\n\t"
+      "@p bra.uni DONE;\n\t"
+      "add.u32 n, n, 1;\n\t"
+      "setp.gt.u32 p, n, 134217728;\n\t"
+      "@p trap;\n\t"
+      "bra.uni WAIT;\n"
+      "DONE:\n\t}"
+      ::"r"(bar), "r"(parity)
+      : "memory");
+}
+// arrive by one elected lane of the warp if `pred` (warp-uniform): a predicated instruction, no divergent region
+__device__ __forceinline__ void mbar_arrive_elect_if(uint32_t bar, uint32_t pred) {
+  asm volatile(
+      "{\n\t.reg .pred e, p;\n\t"
+      "elect.sync _|e, 0xffffffff;\n\t"
+      "setp.ne.and.b32 p, %1, 0, e;\n\t"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+      ::"r"(bar), "r"(pred)
+      : "memory");
+}
+// same on the barrier at the same offset in CTA `rank` of the cluster (default .release.cta: an event signal)
+__device__ __forceinline__ void mbar_arrive_remote_elect_if(uint32_t bar, uint32_t rank, uint32_t pred) {
+  asm volatile(
+      "{\n\t.reg .pred e, p;\n\t.reg .b32 r;\n\t"
+      "elect.sync _|e, 0xffffffff;\n\t"
+      "setp.ne.and.b32 p, %2, 0, e;\n\t"
+      "@p mapa.shared::cluster.u32 r, %0, %1;\n\t"
+      "@p mbarrier.arrive.shared::cluster.b64 _, [r];\n\t}"
+      ::"r"(bar), "r"(rank), "r"(pred)
+      : "memory");
+}
 // generic-proxy writes to this CTA's shared memory -> later async-proxy reads (wgmma operands).  fence.proxy.async
 // without a state space also covers global memory and costs a GPU-scope MEMBAR
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }

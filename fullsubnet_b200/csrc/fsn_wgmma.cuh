@@ -48,6 +48,27 @@ __device__ __forceinline__ void mma_f16_n32(float (&d)[16], uint64_t a, uint64_t
       : "memory");
 }
 
+// Descriptor words: a descriptor is (hi << 32) | lo, and the start address field of lo moves by 1 per 16 bytes without
+// carrying out of it anywhere in the shared window, so a descriptor at `bytes` further is lo + bytes / 16.
+constexpr uint32_t DESC_SW128_HI = 64u | (1u << 30), DESC_SW64_HI = 32u | (2u << 30);
+__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFF) | (1u << 16); }
+
+// m64n32k16, f16 operands, accumulating, with the descriptors given as words: A = (a_hi, a_lo + a_off), B = (b_hi,
+// b_lo + b_off).  The offsets are added inside the asm so that the front end cannot re-associate them with a
+// loop-carried base and hoist one 64-bit descriptor per offset out of the loop: in a stage loop the base stays in a
+// uniform register and each MMA costs one uniform add
+__device__ __forceinline__ void mma_f16_n32_w(float (&d)[16], uint32_t a_lo, uint32_t a_off, uint32_t a_hi,
+                                              uint32_t b_lo, uint32_t b_off, uint32_t b_hi) {
+  asm volatile(
+      "{\n\t.reg .b32 al, bl;\n\t.reg .b64 a, b;\n\t"
+      "add.u32 al, %16, %17;\n\tadd.u32 bl, %19, %20;\n\t"
+      "mov.b64 a, {al, %18};\n\tmov.b64 b, {bl, %21};\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, a, b, 1, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a_lo), "r"(a_off), "r"(a_hi), "r"(b_lo), "r"(b_off), "r"(b_hi)
+      : "memory");
+}
+
 // m64n64k16, f16 operands; scale_d = 0 overwrites D
 __device__ __forceinline__ void mma_f16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(

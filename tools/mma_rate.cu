@@ -8,6 +8,17 @@
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o /tmp/mma_rate tools/mma_rate.cu && /tmp/mma_rate
 //
 // Prints per configuration the cycles per stage of one warpgroup and the per-SM cycles per MMA.
+//
+// The loop above has loop-invariant descriptors and no barriers, which the kernel's stage loop does not have.  The
+// `ctl` variants (one warpgroup, no TMA stream) put the kernel's per-stage pieces around the same MMAs, as the kernel
+// before and after its stage-loop rewrite issues them:
+//   (a) every descriptor built per MMA (desc_sw64 / desc_sw128) from a ring slot and a state k range that change every
+//       stage (runtime strides, 0 here, so the operands and their banks stay those of the plain loop);
+//   (b) a try-wait on an already completed mbarrier per stage and the release arrive of the stage before, by lane 0 of
+//       the warps q < CL (CL a kernel argument) in a divergent region, as release_stage did;
+//   (c) both: the former kernel's stage loop;
+//   (u) the rewritten loop: warp-uniform slot and phase, descriptor words stepped by constants (wg::mma_f16_n32_w), the
+//       warp-wide wait and elected, predicated arrives.
 #include <cuda_runtime.h>
 #include <stdio.h>
 
@@ -115,6 +126,102 @@ static void run(const char* name, long long* d_out, const uint8_t* gsrc) {
     }
 }
 
+// stage-loop controls (header): VAR 0 plain, 1 (a), 2 (b), 3 (c), 4 (u); one warpgroup (warps 4..7), nst ring slots
+template <bool X3, int VAR>
+__global__ void __launch_bounds__(512, 1) stage_ctl(int nst, uint32_t slot_stride, uint32_t k_stride, int CL,
+                                                    long long* out) {
+  constexpr int PARTS = X3 ? 2 : 1;
+  extern __shared__ uint8_t raw[];
+  uint8_t* sm = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + 120 * 1024);  // [0]: completed "w_full", [1]: "w_empty"
+  for (int i = threadIdx.x; i < 120 * 1024 / 16; i += blockDim.x) reinterpret_cast<uint4*>(sm)[i] = make_uint4(0, 0, 0, 0);
+  if (threadIdx.x == 0) {
+    mbar_init(&bars[0], 1);
+    mbar_init(&bars[1], (1u << 20) - 1);
+    mbar_arrive(&bars[0]);  // phase 0 complete: every parity-0 wait below succeeds at its first poll
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp < 4 || warp >= 8) return;
+  const int q = VAR == 4 ? __shfl_sync(0xffffffffu, warp & 3, 0) : warp & 3;
+  const uint32_t wbase = smem_u32(sm), sbase = smem_u32(sm + 48 * 1024), LO = 4096;
+  const uint32_t full = smem_u32(&bars[0]), empty = smem_u32(&bars[1]);
+  const uint32_t rel_local = CL == 1 && q == 0;
+  float acc[4][16];
+#pragma unroll
+  for (int g = 0; g < 4; ++g) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[g][i] = 0.f;
+    wg::fence_operand(acc[g]);
+  }
+  int stage = 0, prev = -1;
+  uint32_t j = 0;
+  named_sync(1, 128);
+  const long long t0 = clock64();
+  for (int it = 0; it < ITERS; ++it, ++j) {
+#pragma unroll
+    for (int part = 0; part < PARTS; ++part) {
+      if (VAR & 2) mbar_wait_cta<false>(&bars[0], 0);
+      if (VAR == 4) mbar_wait_cta_warp(full, 0);
+      wg::fence();
+      const uint32_t wa = (VAR & 1) || VAR == 4 ? wbase + stage * slot_stride : wbase;
+      const uint32_t sb = (VAR & 1) || VAR == 4 ? sbase + (j >> 1) * k_stride + (j & 1) * k_stride : sbase;
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) {
+        const uint64_t bd = wg::desc_sw128(sb + kk * 32), bl = wg::desc_sw128(sb + LO + kk * 32);
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          if (VAR == 4) {
+            const uint32_t a_lo = wg::desc_lo(wa), b_lo = wg::desc_lo(sb);
+            wg::mma_f16_n32_w(acc[g], a_lo, g * 256 + kk * 2, wg::DESC_SW64_HI, b_lo, kk * 2, wg::DESC_SW128_HI);
+            if (X3 && part == 0)
+              wg::mma_f16_n32_w(acc[g], a_lo, g * 256 + kk * 2, wg::DESC_SW64_HI, b_lo, LO / 16 + kk * 2, wg::DESC_SW128_HI);
+          } else {
+            const uint64_t ad = wg::desc_sw64(wa + g * 4096 + kk * 32);
+            wg::mma_f16_n32(acc[g], ad, bd, 1u);
+            if (X3 && part == 0) wg::mma_f16_n32(acc[g], ad, bl, 1u);
+          }
+        }
+      }
+      wg::commit();
+      wg::wait<1>();
+      if ((VAR & 2) && prev >= 0 && lane == 0 && q < CL) {
+        if (CL == 1) mbar_arrive(&bars[1]);
+        else mbar_arrive_remote(&bars[1], (uint32_t)(2 * q));
+      }
+      if (VAR == 4) mbar_arrive_elect_if(empty, (prev >= 0) & rel_local);
+      prev = stage;
+      if (++stage == nst) stage = 0;
+    }
+  }
+  wg::wait<0>();
+#pragma unroll
+  for (int g = 0; g < 4; ++g) wg::fence_operand(acc[g]);
+  const long long t1 = clock64();
+  float s = 0.f;
+#pragma unroll
+  for (int g = 0; g < 4; ++g)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) s += acc[g][i];
+  if (threadIdx.x == 128) out[blockIdx.x] = (t1 - t0) + (s != 0.f ? 1 : 0);
+}
+
+template <bool X3, int VAR>
+static void run_ctl(const char* name, long long* d_out) {
+  cudaFuncSetAttribute(stage_ctl<X3, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+  cudaMemset(d_out, 0, GRID * 8 * sizeof(long long));
+  stage_ctl<X3, VAR><<<GRID, 512, SMEM>>>(4, 0u, 0u, 1, d_out);
+  const cudaError_t e = cudaDeviceSynchronize();
+  long long h[GRID];
+  cudaMemcpy(h, d_out, sizeof(h), cudaMemcpyDeviceToHost);
+  double cyc = 0;
+  for (int b = 0; b < GRID; ++b) cyc += (double)h[b] / GRID;
+  const int stages = ITERS * (X3 ? 2 : 1), mmas = ITERS * (X3 ? 24 : 8);
+  printf("%-16s 1 warpgroup: %s  %6.1f cycles per stage, %5.1f cycles per MMA\n", name, cudaGetErrorString(e),
+         cyc / stages, cyc / mmas);
+}
+
 int main() {
   long long* d_out;
   uint8_t* gsrc;
@@ -127,6 +234,16 @@ int main() {
   run<true, 0, 0>("x3 wait<0>", d_out, gsrc);
   run<false, 0, 1>("f16 wait<1>", d_out, gsrc);
   run<false, 0, 0>("f16 wait<0>", d_out, gsrc);
+  run_ctl<true, 0>("x3 ctl plain", d_out);
+  run_ctl<true, 1>("x3 ctl (a) desc", d_out);
+  run_ctl<true, 2>("x3 ctl (b) bars", d_out);
+  run_ctl<true, 3>("x3 ctl (c) both", d_out);
+  run_ctl<true, 4>("x3 ctl (u) new", d_out);
+  run_ctl<false, 0>("f16 ctl plain", d_out);
+  run_ctl<false, 1>("f16 ctl (a) desc", d_out);
+  run_ctl<false, 2>("f16 ctl (b) bars", d_out);
+  run_ctl<false, 3>("f16 ctl (c) both", d_out);
+  run_ctl<false, 4>("f16 ctl (u) new", d_out);
   cudaFree(d_out);
   cudaFree(gsrc);
   return 0;
