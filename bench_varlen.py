@@ -1,13 +1,19 @@
-"""bench_varlen.py - fullsubnet inference over clips of DIFFERENT lengths on one GPU.  Prints one JSON line.
+"""bench_varlen.py - inference over clips of DIFFERENT lengths on one GPU.  Prints one JSON line.
 
-Workload: a seeded set of --clips clips (default 1024) whose lengths are distinct and uniform in 1 - 10 s at 16 kHz,
-the inference.toml model with weights W-a, the default precision ("auto": f16x3_tc), wav -> enhanced wav + int16 PCM
-(what the file loop writes).  Two schedules of the same clips:
+Workload (--model fullsubnet, the default): a seeded set of --clips clips (default 1024) whose lengths are distinct and
+uniform in 1 - 10 s at 16 kHz, the inference.toml model with weights W-a, the default precision ("auto": f16x3_tc),
+wav -> enhanced wav + int16 PCM (what the file loop writes).  Two schedules of the same clips:
 
   exact       equal-length batches (``plan_batches(lengths, 256, 0)``): every length is distinct, so B = 1 per call
               (fsn_enhance_pcm), which is what the file loop does on real recordings by default;
   pad<x>      ``plan_batches(lengths, 256, x)``: length-sorted runs of <= 256 clips padded to their longest clip by at
               most a fraction x of the batch's samples, one fsn_enhance_varlen call per batch.
+
+--model improved_fullsubnet --variant k16|k48|k48_960: the same schedules for improved_fullsubnet with bench.py's
+constructor arguments and weights of that variant, the default precision ("auto": tf32_tc), clip lengths distinct and
+uniform in 1 - 10 s at the variant's sample rate (16 or 48 kHz), fsn_improved_enhance for every call.  Its sections
+launch kernels once per frame, and one call on a 10 s clip keeps every step's gates, so the defaults are --clips 256
+and --batch 64.
 
 Each schedule is timed twice with CUDA events around the whole schedule: "resident" (inputs already in HBM, outputs left
 there) and "e2e" (pinned host float32 -> H2D -> call -> int16 D2H into pinned host memory, the file loop minus the wav
@@ -27,7 +33,7 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-SR = 16000
+SR = 16000  # fullsubnet; improved_fullsubnet: the variant's rate
 GAIN = 0.8 * 32767.0
 
 
@@ -40,9 +46,9 @@ def power_limit_w(index: int):
         return None
 
 
-def clip_lengths(n: int, seed: int):
+def clip_lengths(n: int, seed: int, sr: int = SR):
     rng = np.random.default_rng(seed)
-    return (rng.permutation(9 * SR + 1)[:n] + SR).tolist()  # distinct, uniform in [1 s, 10 s]
+    return (rng.permutation(9 * sr + 1)[:n] + sr).tolist()  # distinct, uniform in [1 s, 10 s]
 
 
 class Schedule:
@@ -86,36 +92,57 @@ def time_schedule(m, s, e2e, reps):
     return ms
 
 
+def make_model(a, dev):
+    """(model, sample rate, workload description) of --model / --variant"""
+    from oracle import fullsubnet_oracle as O  # weights / inputs generator only
+    if a.model == "fullsubnet":
+        from fullsubnet_b200.fullsubnet.model import Model
+        m = Model(**O.DEFAULT_MODEL_ARGS)
+        m.load_state_dict(O.make_state_dict(seed=0), strict=True)
+        return m.to(dev).eval(), SR, "fullsubnet inference.toml, W-a"
+    from fullsubnet_b200.improved_fullsubnet.model import Model as ImpModel
+    from oracle import improved_fullsubnet_oracle as IO
+    imp_args = {"k48": IO.ARGS_48K_1024, "k48_960": IO.ARGS_48K_960, "k16": IO.DEFAULT_IMPROVED_ARGS}[a.variant]
+    m = ImpModel(**imp_args)  # the constructor arguments and weights of bench.py --variant
+    m.load_state_dict(IO.make_improved_state_dict(seed=5, args=imp_args), strict=True)
+    sr = 16000 if a.variant == "k16" else 48000
+    return m.to(dev).eval(), sr, (f"improved_fullsubnet {a.variant} (n_fft={imp_args['n_fft']}, "
+                                  f"hop={imp_args['hop_length']})")
+
+
 def main():
     from fullsubnet_b200 import _lib
-    from fullsubnet_b200.fullsubnet.model import Model
     from fullsubnet_b200.inferencer import plan_batches
     from oracle import fullsubnet_oracle as O  # weights / inputs generator only
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--clips", type=int, default=1024)
-    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--model", default="fullsubnet", choices=["fullsubnet", "improved_fullsubnet"])
+    ap.add_argument("--variant", default="k48", choices=["k48", "k48_960", "k16"],
+                    help="improved_fullsubnet constructor args (as bench.py --variant)")
+    ap.add_argument("--clips", type=int, default=None, help="default 1024 (fullsubnet), 256 (improved_fullsubnet)")
+    ap.add_argument("--batch", type=int, default=None, help="default 256 (fullsubnet), 64 (improved_fullsubnet)")
     ap.add_argument("--max-padding", type=float, nargs="+", default=[0.05, 0.1, 0.25])
     ap.add_argument("--steps", type=int, default=1, help="timed repetitions of every schedule")
     ap.add_argument("--warmup", type=int, default=1, help="untimed repetitions of every schedule")
     ap.add_argument("--seed", type=int, default=0)
     a = ap.parse_args()
+    improved = a.model == "improved_fullsubnet"
+    a.clips = a.clips or (256 if improved else 1024)
+    a.batch = a.batch or (64 if improved else 256)
     assert a.gpus == 1, "bench_varlen.py measures one GPU"
     assert torch.cuda.is_available(), "bench_varlen.py needs a CUDA device"
     dev = torch.device("cuda", torch.cuda.current_device())
     lib = _lib.load()
-    m = Model(**O.DEFAULT_MODEL_ARGS)
-    m.load_state_dict(O.make_state_dict(seed=0), strict=True)
-    m = m.to(dev).eval()
-    lens = clip_lengths(a.clips, a.seed)
-    noise = O.make_noisy(1, max(lens), seed=a.seed + 1, speechlike=True)[0]
+    m, sr, what = make_model(a, dev)
+    lens = clip_lengths(a.clips, a.seed, sr)
+    noise = O.make_noisy(1, max(lens), seed=a.seed + 1, speechlike=True, sr=sr)[0]
     rng = np.random.default_rng(a.seed + 2)
     clips = [noise[int(rng.integers(0, max(lens) - L + 1)):][:L] * float(rng.uniform(0.3, 1.0)) for L in lens]
 
     schedules = [Schedule("exact", plan_batches(lens, a.batch, 0.0), lens, clips, dev)]
     for mp in a.max_padding:
         schedules.append(Schedule(f"pad{mp:g}", plan_batches(lens, a.batch, mp), lens, clips, dev))
-    audio_s = sum(lens) / SR
+    audio_s = sum(lens) / sr
     res, ref = {}, None
     for s in schedules:
         for _ in range(a.warmup):
@@ -139,14 +166,17 @@ def main():
         del outs, per_clip
     best_name = max((n for n in res if n != "exact"), key=lambda n: res[n]["e2e"]["clips_per_sec"])
     best = res[best_name]
+    config = {"workload": f"{a.clips} clips, distinct lengths uniform in 1-10 s at {sr // 1000} kHz ({audio_s:.0f} s of "
+                          f"audio), {what}, wav -> enhanced + int16 PCM",
+              "precision": m._resolve_precision(), "batch": a.batch, "seed": a.seed}
+    if improved:
+        config.update(model=a.model, variant=a.variant)
     print(json.dumps({
         "metric": "clips_per_sec", "value": best["e2e"]["clips_per_sec"], "unit": "clips/s", "n_gpus": 1,
         "steps": a.steps, "warmup": a.warmup, "higher_is_better": True, "best_schedule": best_name,
         "speedup_vs_exact_e2e": best["e2e"]["clips_per_sec"] / res["exact"]["e2e"]["clips_per_sec"],
         "speedup_vs_exact_resident": best["resident"]["clips_per_sec"] / res["exact"]["resident"]["clips_per_sec"],
-        "config": {"workload": f"{a.clips} clips, distinct lengths uniform in 1-10 s at 16 kHz ({audio_s:.0f} s of audio), "
-                               "fullsubnet inference.toml, W-a, wav -> enhanced + int16 PCM",
-                   "precision": m._resolve_precision(), "batch": a.batch, "seed": a.seed},
+        "config": config,
         "schedules": res,
         "device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(dev.index or 0)}))
 

@@ -6,6 +6,7 @@ import ctypes as C
 import os
 from typing import Optional
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -130,6 +131,9 @@ _SIGNATURES = {
     "fsn_improved_workspace_bytes": (_S, [C.POINTER(ImprovedDesc), _I, _I]),
     "fsn_improved_forward": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _I, _I, _P, _P, _P, _S,
                                        _P]),
+    "fsn_improved_enhance_workspace_bytes": (_S, [C.POINTER(ImprovedDesc), _I, _I]),
+    "fsn_improved_enhance": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _P, _I, _I, _P, _P, _P, _F,
+                                       _P, _S, _P]),
     "fsn_improved_train_workspace_bytes": (_S, [C.POINTER(ImprovedDesc), _I, _I]),
     "fsn_improved_train_forward": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _I, _I, _P, _P, _S,
                                              _P]),
@@ -229,6 +233,22 @@ def require_cuda(t: torch.Tensor, what: str) -> torch.Tensor:
     if t.dtype != torch.float32:
         t = t.float()
     return t.contiguous()
+
+
+def lengths_table(lengths, B: int, L: int) -> np.ndarray:
+    """Per-clip lengths (sequence of B ints or a CPU integer tensor) -> contiguous int32 host array; the library checks
+    the rest (n_fft/2 < length, max == L) before any CUDA call."""
+    if isinstance(lengths, torch.Tensor):
+        if lengths.is_cuda or lengths.is_floating_point() or lengths.is_complex() or lengths.dim() != 1:
+            raise ValueError("lengths must be a 1-D CPU integer tensor or a sequence of ints")
+        lengths = lengths.tolist()
+    lens = np.ascontiguousarray([int(v) for v in lengths], dtype=np.int32)
+    if lens.shape != (B,):
+        raise ValueError(f"lengths has {lens.size} entries for a batch of {B} clips")
+    if lens.size and int(lens.max()) > L:
+        b = int(lens.argmax())
+        raise ValueError(f"lengths[{b}] = {int(lens[b])} exceeds the {L} samples of a row")
+    return lens
 
 
 def stream_ptr(device) -> int:

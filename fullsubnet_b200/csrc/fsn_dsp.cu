@@ -430,9 +430,10 @@ static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 
 // fsn_dsp_dft.cu: direct-DFT variants for even transform sizes that are not a power of two (e.g. 960)
 int stft_dft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, int T, int Tg, float* mag,
-                    float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st);
+                    float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens);
 int istft_dft_launch(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B, int T,
-                     int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st);
+                     int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st, unsigned int* peak_bits,
+                     const int* lens);
 int istft_mask_adjoint_dft_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
                                   int hop, int win_length, float* dcrm, cudaStream_t st);
 static bool dft_size_ok(int n) { return !is_pow2(n) && (n & 1) == 0 && n >= 16 && n <= 1200; }
@@ -440,14 +441,13 @@ static bool dft_size_ok(int n) { return !is_pow2(n) && (n & 1) == 0 && n >= 16 &
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
                 float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens) {
   FSN_REQUIRE(B > 0 && L > 0, FSN_ERR_SHAPE, "stft: empty input (B=%d, L=%d)", B, L);
-  FSN_REQUIRE(!lens || is_pow2(n_fft), FSN_ERR_UNSUPPORTED, "stft: per-clip lengths need a power-of-two n_fft");
   if (dft_size_ok(n_fft)) {
     FSN_REQUIRE(hop > 0 && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE, "stft: bad hop/win_length");
     FSN_REQUIRE(n_fft / 2 < L, FSN_ERR_SHAPE, "stft: reflect padding %d needs L > pad (L=%d)", n_fft / 2, L);
     FSN_REQUIRE(!magT || T_pad >= 1 + L / hop, FSN_ERR_SHAPE, "stft: T_pad < T");
     const int Td = 1 + L / hop;
     return stft_dft_launch(wav, B, L, n_fft, hop, win_length, Td, magT ? (T_pad > Td ? T_pad : Td) : Td, mag, phase, real,
-                           imag, magT, T_pad, st);
+                           imag, magT, T_pad, st, lens);
   }
   FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
               "stft: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);
@@ -492,10 +492,8 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
                  int hop, int win_length, int length, float* wav, cudaStream_t st, int mask_mode, unsigned int* peak_bits,
                  const int* lens) {
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "istft: empty input");
-  FSN_REQUIRE(!lens || (is_pow2(n_fft) && length > 0), FSN_ERR_UNSUPPORTED,
-              "istft: per-clip lengths need a power-of-two n_fft and an output length");
+  FSN_REQUIRE(!lens || length > 0, FSN_ERR_UNSUPPORTED, "istft: per-clip lengths need an output length");
   if (peak_bits) {
-    FSN_REQUIRE(!dft_size_ok(n_fft), FSN_ERR_UNSUPPORTED, "istft: the fused peak is built for the power-of-two transform");
     int rc = check_cuda(cudaMemsetAsync(peak_bits, 0, (size_t)B * sizeof(unsigned int), st), "istft peak memset");
     if (rc) return rc;
   }
@@ -505,7 +503,8 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
     FSN_REQUIRE(cstride == 1 || cstride == 2, FSN_ERR_SHAPE, "istft: cstride must be 1 or 2");
     const int olen = length > 0 ? length : hop * (T - 1);
     FSN_REQUIRE(olen > 0, FSN_ERR_SHAPE, "istft: output length %d", olen);
-    return istft_dft_launch(real, imag, cstride, crm, mask_mode, B, T, n_fft, hop, win_length, olen, wav, st);
+    return istft_dft_launch(real, imag, cstride, crm, mask_mode, B, T, n_fft, hop, win_length, olen, wav, st, peak_bits,
+                            lens);
   }
   FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
               "istft: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);

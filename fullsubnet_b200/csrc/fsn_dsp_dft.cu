@@ -4,7 +4,8 @@
 // Same data flow as fsn_dsp.cu (two real frames packed into one complex transform, FR frames per CTA, fused mask and
 // overlap-add), but the transform itself is a direct O(n^2) DFT in shared memory against a full-circle twiddle
 // table: at n = 960 that is 3.7 MFLOP per frame, i.e. < 1 % of the model's 217 MFLOP per frame, so a mixed-radix
-// FFT would not move the step time.  The power-of-two kernels are untouched.
+// FFT would not move the step time.  The power-of-two kernels are untouched.  Per-clip lengths (lens, nullable) follow
+// the rules of the radix-2 kernels in fsn_dsp.cu.
 #include "fsn_common.cuh"
 
 namespace fsn {
@@ -51,7 +52,7 @@ __device__ __forceinline__ void dft_smem(const float2* in, float2* out, int np, 
 __global__ void __launch_bounds__(kDftThreads)
 stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length, int T, float* __restrict__ mag,
                 float* __restrict__ phase, float* __restrict__ real, float* __restrict__ imag,
-                float* __restrict__ magT, int T_pad) {
+                float* __restrict__ magT, int T_pad, const int* __restrict__ lens) {
   extern __shared__ float2 smem2[];
   constexpr int NP = kDftFR / 2;
   float2* zin = smem2;
@@ -61,6 +62,8 @@ stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_le
   const int b = blockIdx.y;
   const int t0 = blockIdx.x * kDftFR;
   const int F = n / 2 + 1;
+  const int Lb = lens ? lens[b] : L;
+  const int Tb = lens ? 1 + Lb / hop : T;
   dft_tables(tw, win, n, win_length);
   __syncthreads();
   const float* x = wav + (size_t)b * L;
@@ -70,8 +73,8 @@ stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_le
     const int ta = t0 + 2 * p, tb = ta + 1;
     const float w = win[i];
     float va = 0.f, vb = 0.f;
-    if (ta < T) va = x[reflect_idx(ta * hop + i - n / 2, L)] * w;
-    if (tb < T) vb = x[reflect_idx(tb * hop + i - n / 2, L)] * w;
+    if (ta < Tb) va = x[reflect_idx(ta * hop + i - n / 2, Lb)] * w;
+    if (tb < Tb) vb = x[reflect_idx(tb * hop + i - n / 2, Lb)] * w;
     zin[p * n + i] = make_float2(va, vb);  // frame A -> real lane, frame B -> imaginary lane
   }
   __syncthreads();
@@ -88,6 +91,7 @@ stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_le
     float re, im;
     if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
     else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+    if (t >= Tb) re = im = 0.f;
     const size_t o = (size_t)b * plane + (size_t)k * T + t;
     if (real) real[o] = re;
     if (imag) imag[o] = im;
@@ -101,7 +105,7 @@ stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_le
       const int t = t0 + j;
       if (t >= T_pad) continue;
       float m = 0.f;
-      if (t < T) {
+      if (t < Tb) {
         const float2 zk = z[(j >> 1) * n + k];
         const float2 zn = z[(j >> 1) * n + (k == 0 ? 0 : n - k)];
         float re, im;
@@ -117,7 +121,8 @@ stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_le
 __global__ void __launch_bounds__(kDftThreads)
 istft_dft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int cstride,
                  const float* __restrict__ crm, int mask_mode, int T, int n, int hop, int win_length, int out_len,
-                 int seg, int np_max, float* __restrict__ wav) {
+                 int seg, int np_max, float* __restrict__ wav, unsigned int* __restrict__ peak_bits,
+                 const int* __restrict__ lens) {
   extern __shared__ float2 smem2[];
   float2* zin = smem2;
   float2* z = zin + np_max * n;
@@ -125,10 +130,12 @@ istft_dft_kernel(const float* __restrict__ real, const float* __restrict__ imag,
   float* win = reinterpret_cast<float*>(tw + n);
   const int b = blockIdx.y;
   const int F = n / 2 + 1;
+  const int Lb = lens ? lens[b] : out_len;
+  const int Tb = lens ? 1 + Lb / hop : T;
   const int s_begin = n / 2 + blockIdx.x * seg;
-  const int s_end = min(s_begin + seg, n / 2 + out_len);
+  const int s_end = min(s_begin + seg, n / 2 + Lb);
   const int t_min = (s_begin >= n) ? (s_begin - n) / hop + 1 : 0;
-  const int t_max = min(T - 1, (s_end - 1) / hop);
+  const int t_max = min(Tb - 1, (s_end - 1) / hop);
   const int nframes = t_max - t_min + 1;
   const int np = nframes > 0 ? (nframes + 1) / 2 : 0;
   dft_tables(tw, win, n, win_length);
@@ -170,9 +177,10 @@ istft_dft_kernel(const float* __restrict__ real, const float* __restrict__ imag,
   __syncthreads();
   dft_smem<true>(zin, z, np, n, tw);
 
-  const int full = n + hop * (T - 1);
+  const int full = n + hop * (Tb - 1);
   const float inv_n = 1.0f / (float)n;
   float* out = wav + (size_t)b * out_len;
+  float peak = 0.f;
   for (int s = s_begin + threadIdx.x; s < s_end; s += blockDim.x) {
     float acc = 0.f, env = 0.f;
     if (s < full) {
@@ -187,7 +195,17 @@ istft_dft_kernel(const float* __restrict__ real, const float* __restrict__ imag,
         env += w * w;
       }
     }
-    out[s - n / 2] = (env > 1e-11f) ? acc / env : 0.f;
+    const float y = (env > 1e-11f) ? acc / env : 0.f;
+    out[s - n / 2] = y;
+    peak = fmaxf(peak, fabsf(y));
+  }
+  if (lens)
+    for (int s = max(s_begin, n / 2 + Lb) + threadIdx.x; s < min(s_begin + seg, n / 2 + out_len); s += blockDim.x)
+      out[s - n / 2] = 0.f;
+  if (peak_bits) {  // per-clip max|y| as in istft_kernel (order-independent, so the atomic is deterministic)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) peak = fmaxf(peak, __shfl_xor_sync(0xffffffffu, peak, o));
+    if ((threadIdx.x & 31) == 0 && peak > 0.f) atomicMax(peak_bits + b, __float_as_uint(peak));
   }
 }
 
@@ -251,20 +269,21 @@ int istft_mask_adjoint_dft_launch(const float* dwav, const float* real, const fl
 }
 
 int stft_dft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, int T, int Tg, float* mag,
-                    float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st) {
+                    float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens) {
   const size_t smem = (size_t)kDftFR * n_fft * 8 + (size_t)n_fft * 8 + (size_t)n_fft * 4;
   int rc = check_cuda(cudaFuncSetAttribute(stft_dft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
                       "stft smem attr");
   if (rc) return rc;
   dim3 grid(cdiv(Tg, kDftFR), B);
   stft_dft_kernel<<<grid, kDftThreads, smem, st>>>(wav, L, n_fft, hop, win_length, T, mag, phase, real, imag, magT,
-                                                   T_pad);
+                                                   T_pad, lens);
   FSN_CHECK_LAUNCH("stft_dft_kernel");
   return FSN_OK;
 }
 
 int istft_dft_launch(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B, int T,
-                     int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st) {
+                     int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st, unsigned int* peak_bits,
+                     const int* lens) {
   const int seg = kDftFR * hop;
   const int np_max = (kDftFR + cdiv(n_fft, hop) + 2) / 2;
   const size_t smem = (size_t)2 * np_max * n_fft * 8 + (size_t)n_fft * 8 + (size_t)n_fft * 4;
@@ -275,7 +294,7 @@ int istft_dft_launch(const float* real, const float* imag, int cstride, const fl
   if (rc) return rc;
   dim3 grid(cdiv(out_len, seg), B);
   istft_dft_kernel<<<grid, kDftThreads, smem, st>>>(real, imag, cstride, crm, mask_mode, T, n_fft, hop, win_length,
-                                                    out_len, seg, np_max, wav);
+                                                    out_len, seg, np_max, wav, peak_bits, lens);
   FSN_CHECK_LAUNCH("istft_dft_kernel");
   return FSN_OK;
 }

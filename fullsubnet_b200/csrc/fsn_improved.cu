@@ -100,6 +100,8 @@ struct ImpWs {
   float *h0[2], *h1[2], *c0, *c1;
   LayerSave tc;                        // FSN_PREC_TF32_TC: gates / cell / hidden of every step of one layer
   float *tc_h1, *tc_rec;
+  unsigned int* peak;                  // fsn_improved_enhance: per-clip max|y| of the int16 output
+  int* lens;                           // fsn_improved_enhance: device copy of the per-clip lengths
   size_t bytes;
 };
 
@@ -143,7 +145,8 @@ int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
   return FSN_OK;
 }
 
-static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, ImpWs& w) {
+// enhance: also the per-clip peak and length table of fsn_improved_enhance, after everything fsn_improved_forward uses
+static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, ImpWs& w, bool enhance = false) {
   Carver c(base);
   const size_t BFT = (size_t)m.B * m.F * m.T, BT = (size_t)m.B * m.T;
   w.mag = c.take<float>(BFT); w.real = c.take<float>(BFT); w.imag = c.take<float>(BFT);
@@ -166,47 +169,35 @@ static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, 
     w.tc_h1 = c.take<float>(TR * d->sb_hidden);
     w.tc_rec = c.take<float>(4 * RH);
   }
+  w.peak = enhance ? c.take<unsigned int>(m.B) : nullptr;
+  w.lens = enhance ? c.take<int>(m.B) : nullptr;
   w.bytes = c.off;
 }
 
-}  // namespace fsn
-
-using namespace fsn;
-
-extern "C" size_t fsn_improved_workspace_bytes(const fsn_improved_desc* d, int B, int L) {
-  ImpDims m;
-  if (imp_dims(d, B, L, m)) return 0;
-  ImpWs w;
-  imp_carve(d, m, nullptr, w);
-  return w.bytes;
-}
-
-extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improved_weights* wt, const float* wav, int B,
-                                    int L, float* enhanced, float* crm_out, void* workspace, size_t workspace_bytes,
-                                    fsn_stream_t stream) {
-  launch_counter() = 0;
-  ImpDims m;
-  int rc = imp_dims(d, B, L, m);
-  if (rc) return rc;
-  ImpWs w;
-  imp_carve(d, m, workspace, w);
-  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
-              workspace_bytes, w.bytes);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int T = m.T, F = m.F, Fu = m.Fu, Hs = d->sb_hidden;
+// The forward on a carved workspace, wav [B,L] -> enhanced [B,L] (+ crm [B,2,F,T]).  lens (nullable, device [B]): clip b
+// is the first lens[b] samples of its row.  Only the length-dependent kernels read it - the STFT, the full-band and
+// section norms and the iSTFT (with peak, when given) - so every clip gives the bits of a call on that clip alone; the
+// recurrent stacks and the section Linear are causal and run over all T steps.
+static int imp_forward(const fsn_improved_desc* d, const fsn_improved_weights* wt, const ImpDims& m, const ImpWs& w,
+                       const float* wav, float* enhanced, float* crm_out, unsigned int* peak, const int* lens,
+                       cudaStream_t st) {
+  const int B = m.B, L = m.L, T = m.T, F = m.F, Fu = m.Fu, Hs = d->sb_hidden, hop = d->hop_length;
+  int rc;
   const float eps = 1.1920928955078125e-07f;  // np.finfo(np.float32).eps (model.py:23,148)
   float* crm = crm_out ? crm_out : w.crm;
   // STFT (model.py:550-557), |X|^fdrc without the Nyquist bin (564-565)
-  if ((rc = stft_launch(wav, B, L, d->n_fft, d->hop_length, d->win_length, w.mag, nullptr, w.real, w.imag, nullptr, 0, st)))
+  if ((rc = stft_launch(wav, B, L, d->n_fft, hop, d->win_length, w.mag, nullptr, w.real, w.imag, nullptr, 0, st, lens)))
     return rc;
   {
     dim3 grid(cdiv(T, 32), cdiv(Fu, 32), B);
     imp_compress_kernel<<<grid, dim3(32, 8), 0, st>>>(w.mag, w.magc, F, T, d->fdrc, false);
     FSN_CHECK_LAUNCH("imp_compress_kernel");
   }
-  // full band: norm (566) -> 2xLSTM + Linear (567)
-  if ((rc = clip_stats_launch(w.magc, B, T, Fu, 0, w.fs, w.sums, st))) return rc;
-  if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)Fu * T, 1.f, w.inv1, nullptr, st, eps))) return rc;
+  // full band: norm (566) -> 2xLSTM + Linear (567); with lens the counts are per frame, times the clip's own frames
+  if ((rc = clip_stats_launch(w.magc, B, T, Fu, 0, w.fs, w.sums, st, lens, hop, 0))) return rc;
+  if ((rc = norm_scales_launch(w.sums, w.sums, B, lens ? (float)Fu : (float)Fu * T, 1.f, w.inv1, nullptr, st, eps, lens,
+                               hop, 0)))
+    return rc;
   SeqStack s = imp_fb_stack(d, m);
   s.L[0] = seq_layer(wt->fb, 0); s.L[1] = seq_layer(wt->fb, 1);
   s.x = w.magc; s.scale = w.inv1; s.fc_w = wt->fb.fc_w; s.fc_b = wt->fb.fc_b; s.out = w.fbT;
@@ -219,8 +210,10 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
     const int R = B * g.N;
     imp_section_input_kernel<<<B * T, 256, 0, st>>>(w.magc, w.fbT, B, T, Fu, g, w.X, w.fs, false);
     FSN_CHECK_LAUNCH("imp_section_input_kernel");
-    if ((rc = clip_reduce_only_launch(w.fs, B, T, w.sums, st))) return rc;
-    if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)g.N * g.W * T, 1.f, w.invs, nullptr, st, eps))) return rc;
+    if ((rc = clip_reduce_only_launch(w.fs, B, T, w.sums, st, lens, hop, 0))) return rc;
+    if ((rc = norm_scales_launch(w.sums, w.sums, B, lens ? (float)g.N * g.W : (float)g.N * g.W * T, 1.f, w.invs, nullptr,
+                                 st, eps, lens, hop, 0)))
+      return rc;
     const fsn_seq_weights& sw = wt->sb[s];
     if (d->precision == FSN_PREC_TF32_TC) {
       // layer by layer over all steps: hoisted input projection + per-step recurrent GEMM on wgmma (tf32), fused cell
@@ -257,5 +250,63 @@ extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improv
     }
   }
   // element-wise mask on (re, im) + iSTFT (575-589)
-  return istft_launch(w.real, w.imag, 1, crm, B, T, d->n_fft, d->hop_length, d->win_length, L, enhanced, st, 2);
+  return istft_launch(w.real, w.imag, 1, crm, B, T, d->n_fft, hop, d->win_length, L, enhanced, st, 2, peak, lens);
+}
+
+}  // namespace fsn
+
+using namespace fsn;
+
+extern "C" size_t fsn_improved_workspace_bytes(const fsn_improved_desc* d, int B, int L) {
+  ImpDims m;
+  if (imp_dims(d, B, L, m)) return 0;
+  ImpWs w;
+  imp_carve(d, m, nullptr, w);
+  return w.bytes;
+}
+
+extern "C" int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improved_weights* wt, const float* wav, int B,
+                                    int L, float* enhanced, float* crm_out, void* workspace, size_t workspace_bytes,
+                                    fsn_stream_t stream) {
+  launch_counter() = 0;
+  ImpDims m;
+  int rc = imp_dims(d, B, L, m);
+  if (rc) return rc;
+  ImpWs w;
+  imp_carve(d, m, workspace, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, w.bytes);
+  return imp_forward(d, wt, m, w, wav, enhanced, crm_out, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+// ---- clips of different lengths in one call (lengths non-null: host [B]), buffers laid out for the longest clip
+// (L_max samples, T_max frames); optional int16 output with the per-clip peak of the iSTFT epilogue
+extern "C" size_t fsn_improved_enhance_workspace_bytes(const fsn_improved_desc* d, int B, int L_max) {
+  ImpDims m;
+  if (imp_dims(d, B, L_max, m)) return 0;
+  ImpWs w;
+  imp_carve(d, m, nullptr, w, true);
+  return w.bytes;
+}
+
+extern "C" int fsn_improved_enhance(const fsn_improved_desc* d, const fsn_improved_weights* wt, const float* wav,
+                                    const int32_t* lengths, int B, int L_max, float* enhanced, float* crm_out,
+                                    int16_t* pcm, float gain, void* workspace, size_t workspace_bytes,
+                                    fsn_stream_t stream) {
+  launch_counter() = 0;
+  ImpDims m;
+  int rc = imp_dims(d, B, L_max, m);
+  if (rc) return rc;
+  if (lengths && (rc = check_lengths(lengths, B, L_max, d->n_fft, "improved_enhance"))) return rc;
+  ImpWs w;
+  imp_carve(d, m, workspace, w, true);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, w.bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int* lens = lengths ? w.lens : nullptr;
+  if (lengths && (rc = lengths_table_launch(lengths, B, w.lens, st))) return rc;
+  if ((rc = imp_forward(d, wt, m, w, wav, enhanced, crm_out, pcm ? w.peak : nullptr, lens, st))) return rc;
+  if (pcm && (rc = scale_int16_launch(enhanced, w.peak, B, L_max, gain, pcm, st, lens))) return rc;
+  if (lens && crm_out) rc = zero_frames_past_launch(crm_out, lens, B, 2 * m.F, m.T, d->hop_length, st);
+  return rc;
 }

@@ -230,19 +230,21 @@ int transpose_mag_launch(const float* in, float* out, int B, int F, int T, int T
 // then takes cnt1 / cnt2 per frame and multiplies them by Tp_b.
 int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs, float2* sums, cudaStream_t st,
                       const int* lens = nullptr, int hop = 0, int la = 0);
-int clip_reduce_only_launch(const float2* fs, int B, int T_pad, float2* sums, cudaStream_t st);
+int clip_reduce_only_launch(const float2* fs, int B, int T_pad, float2* sums, cudaStream_t st, const int* lens = nullptr,
+                            int hop = 0, int la = 0);
 int norm_scales_launch(const float2* mag_sums, const float2* fb_sums, int B, float cnt1, float cnt2, float* inv1,
                        float* inv2, cudaStream_t st, float eps = 1e-5f, const int* lens = nullptr, int hop = 0,
                        int la = 0);
 
-// lens (nullable, device [B]): clip b has lens[b] of the L samples of its row (fsn_enhance_varlen); power-of-two n_fft
+// lens (nullable, device [B]): clip b has lens[b] of the L samples of its row (fsn_enhance_varlen, fsn_improved_enhance)
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
                 float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens = nullptr);
 // mask_mode: 1 = decompress_cIRM + complex product (fullsubnet), 2 = element-wise re*crm0, im*crm1 (improved_fullsubnet)
 int istft_launch(const float* real, const float* imag, int cstride, const float* crm, int B, int T, int n_fft,
                  int hop, int win_length, int length, float* wav, cudaStream_t st, int mask_mode = 1,
                  unsigned int* peak_bits = nullptr, const int* lens = nullptr);
-// peak_bits (optional, [B]): max|wav| per clip as float bits, reduced in the iSTFT epilogue; scale_int16_launch turns
+// peak_bits (optional, [B]): max|wav| per clip as float bits, reduced in the iSTFT epilogue (radix-2 and direct DFT alike,
+// bounded by lens when given); scale_int16_launch turns
 // it into the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:181-182)
 int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st,
                        const int* lens = nullptr);
@@ -250,6 +252,9 @@ int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, i
 int lengths_table_launch(const int32_t* host_lengths, int B, int* lengths, cudaStream_t st);
 // crm [B, C, T]: frames t >= 1 + lengths[b]/hop of clip b set to 0
 int zero_frames_past_launch(float* crm, const int* lengths, int B, int C, int T, int hop, cudaStream_t st);
+// host checks of a per-clip length table before any CUDA call: n_fft/2 < lengths[b] <= L_max and max == L_max, else
+// FSN_ERR_SHAPE naming the clip (`who` prefixes the message)
+int check_lengths(const int32_t* lengths, int B, int L_max, int n_fft, const char* who);
 
 // adjoint of the element-wise mask + iSTFT of improved_fullsubnet (istft_launch mask_mode 2) with respect to the mask:
 // dwav [B,L] -> dcrm [B,2,F,T] for the rows f < F-1 (the Nyquist row of the cRM is a constant; it is not written)

@@ -430,8 +430,9 @@ int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs
   return FSN_OK;
 }
 
-int clip_reduce_only_launch(const float2* fs, int B, int T_pad, float2* sums, cudaStream_t st) {
-  clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums, nullptr, 0, 0);
+int clip_reduce_only_launch(const float2* fs, int B, int T_pad, float2* sums, cudaStream_t st, const int* lens, int hop,
+                            int la) {
+  clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums, lens, hop, la);
   FSN_CHECK_LAUNCH("clip_reduce_kernel");
   return FSN_OK;
 }

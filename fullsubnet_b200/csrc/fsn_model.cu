@@ -305,18 +305,18 @@ extern "C" size_t fsn_enhance_varlen_workspace_bytes(const fsn_model_desc* d, in
   return enhance_workspace_bytes(d, B, L_max, n_fft, hop, true);
 }
 
-static int check_lengths(const int32_t* lengths, int B, int L_max, int n_fft) {
+namespace fsn {
+int check_lengths(const int32_t* lengths, int B, int L_max, int n_fft, const char* who) {
   int longest = 0;
   for (int b = 0; b < B; ++b) {
     FSN_REQUIRE(lengths[b] > n_fft / 2 && lengths[b] <= L_max, FSN_ERR_SHAPE,
-                "enhance_varlen: clip %d has length %d, outside (n_fft/2, L_max] = (%d, %d]", b, lengths[b], n_fft / 2,
-                L_max);
+                "%s: clip %d has length %d, outside (n_fft/2, L_max] = (%d, %d]", who, b, lengths[b], n_fft / 2, L_max);
     longest = lengths[b] > longest ? lengths[b] : longest;
   }
-  FSN_REQUIRE(longest == L_max, FSN_ERR_SHAPE, "enhance_varlen: the longest clip has %d samples, L_max = %d", longest,
-              L_max);
+  FSN_REQUIRE(longest == L_max, FSN_ERR_SHAPE, "%s: the longest clip has %d samples, L_max = %d", who, longest, L_max);
   return FSN_OK;
 }
+}  // namespace fsn
 
 static int enhance_impl(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
                         const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L, int n_fft, int hop,
@@ -333,7 +333,7 @@ static int enhance_impl(const fsn_model_desc* d, const fsn_seq_weights* fb, cons
   if (rc) return rc;
   FSN_REQUIRE(dd.precision == FSN_PREC_FP32 || sb_tc_supported(&dd), FSN_ERR_UNSUPPORTED,
               "FSN_PREC_F16_TC / FSN_PREC_F16X3_TC need sb_hidden in {128,256,384} and sub-band input width <= 32");
-  if (lengths && (rc = check_lengths(lengths, B, L, n_fft))) return rc;
+  if (lengths && (rc = check_lengths(lengths, B, L, n_fft, "enhance_varlen"))) return rc;
   FSN_REQUIRE(workspace && workspace_bytes >= e.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, e.bytes);
   ModelWs w;

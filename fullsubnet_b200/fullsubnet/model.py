@@ -10,7 +10,6 @@ from __future__ import annotations
 import ctypes as C
 import os
 
-import numpy as np
 import torch
 
 from .. import _lib
@@ -139,17 +138,7 @@ class Model(BaseModel):
     @staticmethod
     def _lengths_table(lengths, B, L):
         """Per-clip lengths (sequence of B ints or a CPU integer tensor) -> contiguous int32 host array."""
-        if isinstance(lengths, torch.Tensor):
-            if lengths.is_cuda or lengths.is_floating_point() or lengths.is_complex() or lengths.dim() != 1:
-                raise ValueError("lengths must be a 1-D CPU integer tensor or a sequence of ints")
-            lengths = lengths.tolist()
-        lens = np.ascontiguousarray([int(v) for v in lengths], dtype=np.int32)
-        if lens.shape != (B,):
-            raise ValueError(f"lengths has {lens.size} entries for a batch of {B} clips")
-        if lens.size and int(lens.max()) > L:
-            b = int(lens.argmax())
-            raise ValueError(f"lengths[{b}] = {int(lens[b])} exceeds the {L} samples of a row")
-        return lens
+        return _lib.lengths_table(lengths, B, L)
 
     def _enhance_varlen(self, x, lens, n_fft, hop_length, win_length, crm, pcm, gain):
         """One fsn_enhance_varlen call: clip b is row b's first lens[b] samples; out [B,L] is 0 past them."""

@@ -46,6 +46,9 @@ class Model(BaseModel):
     # fsn_improved_train_backward runs the iSTFT adjoint and BPTT
     TRAIN_ENTRY_POINTS = ("fsn_improved_train_workspace_bytes", "fsn_improved_train_forward", "fsn_improved_train_backward")
     TRAIN_TF32_STACKS = ("fb_model", "sb_model")
+    # waveform in, waveform out with the model's own STFT: the Inferencer calls enhance / enhance_pcm instead of computing
+    # a magnitude spectrogram for it
+    WAVEFORM_INPUT = True
 
     def __init__(self, n_fft=512, hop_length=128, win_length=512, fdrc=0.5, num_freqs=257, freq_cutoffs=[20, 80],
                  sb_num_center_freqs=[1, 4, 8], sb_num_neighbor_freqs=[15, 15, 15], fb_num_center_freqs=[1, 4, 8],
@@ -125,6 +128,16 @@ class Model(BaseModel):
         B, L = x.shape
         return (B, L), (B, 1, L)
 
+    def _check_sections(self):
+        sb = self.sb_model
+        bounds = [0] + sb.freq_cutoffs + [self.num_freqs - 1]
+        for s in range(len(sb.sb_models)):  # model.py:341-345 (both the noisy and the full-band unfold)
+            if (bounds[s + 1] - bounds[s]) % sb.sb_num_center_freqs[s] or \
+                    (bounds[s + 1] - bounds[s]) % sb.fb_num_center_freqs[s]:
+                raise ValueError(
+                    "The number of center frequencies should be divisible by the subband freqency interval. "
+                    f"Got {sb.sb_num_center_freqs[s]} and {bounds[s + 1] - bounds[s]}.")
+
     def forward(self, y, return_crm: bool = False):
         """y [B,L] or [B,1,L] -> enhanced [B,1,L]  (model.py:541-591).  ``return_crm`` additionally returns the
         [B,2,F,T] mask (Nyquist row zero) - an extension used by the parity tests."""
@@ -135,14 +148,7 @@ class Model(BaseModel):
             y = y.squeeze(1)
         x = _lib.require_cuda(y, "y")
         B, L = x.shape
-        sb = self.sb_model
-        bounds = [0] + sb.freq_cutoffs + [self.num_freqs - 1]
-        for s in range(len(sb.sb_models)):  # model.py:341-345 (both the noisy and the full-band unfold)
-            if (bounds[s + 1] - bounds[s]) % sb.sb_num_center_freqs[s] or \
-                    (bounds[s + 1] - bounds[s]) % sb.fb_num_center_freqs[s]:
-                raise ValueError(
-                    "The number of center frequencies should be divisible by the subband freqency interval. "
-                    f"Got {sb.sb_num_center_freqs[s]} and {bounds[s + 1] - bounds[s]}.")
+        self._check_sections()
         if self._records_grad():
             if return_crm:
                 raise NotImplementedError("fullsubnet_b200: return_crm is built for inference only (use torch.no_grad())")
@@ -164,3 +170,45 @@ class Model(BaseModel):
             _lib.check(lib.fsn_improved_forward(C.byref(d), C.byref(w), x.data_ptr(), B, L, out.data_ptr(),
                                                 _lib.ptr(crm), ws.data_ptr(), n, _lib.stream_ptr(x.device)))
         return (out, crm) if return_crm else out
+
+    def _enhance_call(self, y, lengths, crm, pcm, gain):
+        """One fsn_improved_enhance call: y [B,L] (CUDA) -> enhanced [B,L]; clip b is row b's first lengths[b] samples
+        (all L when lengths is None), its outputs 0 past them."""
+        B, L = y.shape
+        lens = None if lengths is None else _lib.lengths_table(lengths, B, L)
+        x = _lib.require_cuda(y, "y")
+        self._check_sections()
+        lib = _lib.load()
+        with torch.cuda.device(x.device):
+            d, w = self._structs()
+            n = _lib.check_workspace(lib.fsn_improved_enhance_workspace_bytes(C.byref(d), B, L))
+            ws = torch.empty(n, dtype=torch.uint8, device=x.device)
+            out = torch.empty(B, L, dtype=torch.float32, device=x.device)
+            _lib.check(lib.fsn_improved_enhance(C.byref(d), C.byref(w), x.data_ptr(), None if lens is None else lens.ctypes.data,
+                                                B, L, out.data_ptr(), _lib.ptr(crm), _lib.ptr(pcm), float(gain),
+                                                ws.data_ptr(), n, _lib.stream_ptr(x.device)))
+        return out
+
+    @torch.no_grad()
+    def enhance(self, y, lengths=None, return_crm: bool = False):
+        """y [B,L] -> enhanced [B,L] in one library call (fsn_improved_enhance); with ``lengths=None`` the bits of
+        ``forward``.  ``lengths`` (B ints, or a CPU integer tensor; max must be L): clips of different lengths in one
+        call.  Clip b is ``y[b, :lengths[b]]``; the rest of the row is never read.  Its outputs equal the call on that
+        clip alone, bit for bit; ``enhanced[b, lengths[b]:]`` and the cRM frames ``t >= 1 + lengths[b] // hop_length``
+        are 0.  ``return_crm`` additionally returns the [B,2,F,T_max] mask."""
+        assert y.dim() == 2, "y must be [B, L]"
+        B, L = y.shape
+        crm = torch.empty(B, 2, self.num_freqs, 1 + L // self.hop_length, dtype=torch.float32,
+                          device=y.device) if return_crm else None
+        out = self._enhance_call(y, lengths, crm, None, 0.0)
+        return (out, crm) if return_crm else out
+
+    @torch.no_grad()
+    def enhance_pcm(self, y, gain=0.8 * 32767.0, lengths=None):
+        """``enhance`` plus the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:
+        181-182) in the same call, the per-clip max|y| reduced in the iSTFT epilogue: y [B,L] -> (enhanced float32
+        [B,L], pcm int16 [B,L]).  ``lengths``: as in ``enhance``; each clip is scaled by the peak of its own samples
+        and its pcm row is 0 past them."""
+        assert y.dim() == 2, "y must be [B, L]"
+        pcm = torch.empty(y.shape, dtype=torch.int16, device=y.device)
+        return self._enhance_call(y, lengths, None, pcm, gain), pcm

@@ -46,20 +46,35 @@ def plan_batches(lengths, batch_size: int, max_padding: float = 0.0):
     return batches
 
 
+def takes_waveform(model) -> bool:
+    """Whether ``model`` maps waveforms to waveforms with its own STFT (improved_fullsubnet) instead of taking the
+    Inferencer's magnitude spectrogram."""
+    return bool(getattr(type(model), "WAVEFORM_INPUT", False))
+
+
 class Inferencer:
     def __init__(self, config: Optional[dict] = None, checkpoint_path=None, output_dir=None, model=None,
                  device=None):
         self.device = torch.device(device) if device is not None else prepare_device(torch.cuda.device_count())
-        acoustics = (config or {}).get("acoustics", {"n_fft": 512, "hop_length": 256, "win_length": 512, "sr": 16000})
+        if model is not None:
+            self.model = model.to(self.device).eval()
+        else:
+            self.model, self.epoch = self._load_model(config["model"], checkpoint_path, self.device)
+        acoustics = (config or {}).get("acoustics")
+        if takes_waveform(self.model):
+            # the model computes its own STFT: n_fft / hop / window come from it, and a config must agree with it
+            own = {"n_fft": self.model.n_fft, "hop_length": self.model.hop_length, "win_length": self.model.win_length}
+            bad = {k: acoustics[k] for k in own if acoustics is not None and k in acoustics and acoustics[k] != own[k]}
+            if bad:
+                raise ValueError(f"acoustics {bad} disagree with the model's own STFT {own}")
+            acoustics = dict(acoustics or {"sr": 16000}, **own)
+        elif acoustics is None:
+            acoustics = {"n_fft": 512, "hop_length": 256, "win_length": 512, "sr": 16000}
         self.acoustic_config = acoustics
         self.n_fft, self.hop_length = acoustics["n_fft"], acoustics["hop_length"]
         self.win_length, self.sr = acoustics["win_length"], acoustics.get("sr", 16000)
         self.torch_stft = partial(stft, n_fft=self.n_fft, hop_length=self.hop_length, win_length=self.win_length)
         self.torch_istft = partial(istft, n_fft=self.n_fft, hop_length=self.hop_length, win_length=self.win_length)
-        if model is not None:
-            self.model = model.to(self.device).eval()
-        else:
-            self.model, self.epoch = self._load_model(config["model"], checkpoint_path, self.device)
         self.inference_config = (config or {}).get("inferencer", {"type": "full_band_crm_mask", "args": {}})
         self.config = config
 
@@ -76,7 +91,10 @@ class Inferencer:
 
     @torch.no_grad()
     def full_band_crm_mask(self, noisy, inference_args=None):
-        """inferencer.py:130-145, op by op through the drop-in functions: noisy [1,L] -> np.float32 [L]."""
+        """inferencer.py:130-145, op by op through the drop-in functions: noisy [1,L] -> np.float32 [L].  A model that
+        takes waveforms (improved_fullsubnet) is the whole path: its enhanced waveform."""
+        if takes_waveform(self.model):
+            return self.model(noisy.reshape(1, -1)).detach().reshape(-1).cpu().numpy()
         noisy_mag, _, noisy_real, noisy_imag = self.torch_stft(noisy)
         noisy_mag = noisy_mag.unsqueeze(1)
         pred_crm = self.model(noisy_mag)
@@ -89,12 +107,16 @@ class Inferencer:
         return enhanced
 
     def supports_lengths(self) -> bool:
-        """Whether clips of different lengths can share one call (fullsubnet with a power-of-two n_fft)."""
+        """Whether clips of different lengths can share one call: improved_fullsubnet (every n_fft it accepts), and
+        fullsubnet with a power-of-two n_fft."""
+        if takes_waveform(self.model):
+            return True
         return hasattr(self.model, "enhance") and self.n_fft & (self.n_fft - 1) == 0
 
     def _check_lengths(self, lengths) -> None:
-        if lengths is not None and not hasattr(self.model, "enhance"):
-            raise NotImplementedError(f"{type(self.model).__module__}: per-clip lengths are built for fullsubnet only")
+        if lengths is not None and not takes_waveform(self.model) and not hasattr(self.model, "enhance"):
+            raise NotImplementedError(f"{type(self.model).__module__}: per-clip lengths are built for fullsubnet and "
+                                      "improved_fullsubnet only")
 
     @torch.no_grad()
     def enhance_batch(self, noisy: torch.Tensor, lengths=None) -> torch.Tensor:
@@ -103,6 +125,8 @@ class Inferencer:
         ``lengths`` (fullsubnet only): clip b is ``noisy[b, :lengths[b]]`` (fsn_enhance_varlen), its row 0 past it."""
         self._check_lengths(lengths)
         x = noisy.to(self.device, non_blocking=True)
+        if takes_waveform(self.model):  # improved_fullsubnet: one library call with the model's own STFT
+            return self.model.enhance(x, lengths=lengths)
         if hasattr(self.model, "enhance"):  # fullsubnet: one fused library call
             return self.model.enhance(x, self.n_fft, self.hop_length, self.win_length, lengths=lengths)
         # other models (fast_fullsubnet): same flow, three library calls (stft -> model -> mask + istft)
@@ -130,6 +154,9 @@ class Inferencer:
         ``enhance_batch``; each clip is scaled by its own peak."""
         from . import _lib
         self._check_lengths(lengths)
+        if takes_waveform(self.model):
+            x = noisy.to(self.device, non_blocking=True)
+            return self.model.enhance_pcm(x, gain=0.8 * float(np.iinfo(np.int16).max), lengths=lengths)[1]
         if lengths is not None or (hasattr(self.model, "enhance_pcm") and self.n_fft & (self.n_fft - 1) == 0):
             x = noisy.to(self.device, non_blocking=True)  # fused: peak in the iSTFT epilogue, one scaling pass
             return self.model.enhance_pcm(x, self.n_fft, self.hop_length, self.win_length,
@@ -207,10 +234,11 @@ class Inferencer:
         goes through ONE fused library call (pinned staging buffer -> H2D -> fsn_enhance_pcm -> int16 D2H), and
         ``<output_dir>/<stem>.wav`` is written as 16-bit PCM like the reference.  Returns the written paths.
 
-        ``max_padding == 0`` (default): batches of equal-length clips only.  ``max_padding > 0`` (fullsubnet with a
-        power-of-two n_fft; other models keep equal-length batches): clips of different lengths share a batch, padded
-        to its longest clip by at most that fraction of the batch's samples, through fsn_enhance_varlen.  Every file
-        is bit-identical either way: each clip is bounded by its own length in the length-dependent kernels."""
+        ``max_padding == 0`` (default): batches of equal-length clips only.  ``max_padding > 0`` (improved_fullsubnet,
+        and fullsubnet with a power-of-two n_fft; other models keep equal-length batches): clips of different lengths
+        share a batch, padded to its longest clip by at most that fraction of the batch's samples, through
+        fsn_enhance_varlen / fsn_improved_enhance.  Every file is bit-identical either way: each clip is bounded by its
+        own length in the length-dependent kernels."""
         from pathlib import Path
         sr = int(sr or self.sr)
         out_dir = Path(output_dir)

@@ -262,6 +262,23 @@ size_t fsn_improved_workspace_bytes(const fsn_improved_desc* d, int B, int L);
 int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improved_weights* w, const float* wav, int B, int L,
                          float* enhanced, float* crm_out, void* workspace, size_t workspace_bytes,
                          fsn_stream_t stream);
+/* Clips of different lengths in one call, with the int16 output of the reference host loop.  Row b of wav [B, L_max]
+ * holds clip b's lengths[b] samples; samples at index >= lengths[b] are never read.  lengths: HOST int32 [B], nullable
+ * (= every clip L_max samples), n_fft/2 < lengths[b] <= L_max and max(lengths) == L_max (else FSN_ERR_SHAPE naming the
+ * clip); copied into the workspace through kernel parameters during the call and not retained.  Outputs, T_max = 1 +
+ * L_max/hop_length:
+ *   enhanced [B, L_max]           0 past lengths[b]
+ *   crm_out  [B, 2, F, T_max]     nullable; Nyquist row 0, and 0 for frames t >= T_b = 1 + lengths[b]/hop_length
+ *   pcm      [B, L_max] int16     nullable; int16(gain * y / max|y|) over the clip's own samples, 0 past lengths[b]
+ * Every clip's outputs are bit-identical to fsn_improved_forward on that clip alone with L = lengths[b] (and pcm to
+ * fsn_peak_normalize_int16 of that waveform): the full-band stack, the section LSTMs and their Linear are causal and run
+ * over T_max steps for every clip; only the STFT, the full-band and section norms, the iSTFT and the int16 scaling are
+ * bounded per clip.  Same precisions and n_fft sizes as fsn_improved_forward.  Never allocates, never synchronises the
+ * host. */
+size_t fsn_improved_enhance_workspace_bytes(const fsn_improved_desc* d, int B, int L_max);
+int fsn_improved_enhance(const fsn_improved_desc* d, const fsn_improved_weights* w, const float* wav,
+                         const int32_t* lengths, int B, int L_max, float* enhanced, float* crm_out, int16_t* pcm,
+                         float gain, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 /* Opt-in stage timing for bench.py: when enabled, fsn_model_forward / fsn_enhance bracket their
  * stages with CUDA events on `stream` (thread-local, created lazily).  After the caller has
