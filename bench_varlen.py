@@ -15,6 +15,10 @@ uniform in 1 - 10 s at the variant's sample rate (16 or 48 kHz), fsn_improved_en
 launch kernels once per frame, and one call on a 10 s clip keeps every step's gates, so the defaults are --clips 256
 and --batch 64.
 
+--model fullband_baseline: the same schedules and clips as fullsubnet for the paper's baseline (its full-size constructor
+arguments, seed-11 weights, fp32), fsn_fullband_enhance for every call.  The JSON line also carries "per_call_64x10s":
+the time of one call on 64 clips of 10 s (resident, null lengths).
+
 Each schedule is timed twice with CUDA events around the whole schedule: "resident" (inputs already in HBM, outputs left
 there) and "e2e" (pinned host float32 -> H2D -> call -> int16 D2H into pinned host memory, the file loop minus the wav
 I/O).  Every clip's PCM of every schedule is compared with the exact schedule's, bit for bit.
@@ -95,6 +99,12 @@ def time_schedule(m, s, e2e, reps):
 def make_model(a, dev):
     """(model, sample rate, workload description) of --model / --variant"""
     from oracle import fullsubnet_oracle as O  # weights / inputs generator only
+    if a.model == "fullband_baseline":
+        from fullsubnet_b200.fullband_baseline.model import Model as FbbModel
+        from oracle import fullband_baseline_oracle as BO
+        m = FbbModel(**BO.DEFAULT_FBB_ARGS)
+        m.load_state_dict(BO.make_fbb_state_dict(seed=11), strict=True)
+        return m.to(dev).eval(), SR, "fullband_baseline (F=257, H=512, 3 layers, offline norm), seed-11 weights"
     if a.model == "fullsubnet":
         from fullsubnet_b200.fullsubnet.model import Model
         m = Model(**O.DEFAULT_MODEL_ARGS)
@@ -110,13 +120,29 @@ def make_model(a, dev):
                                   f"hop={imp_args['hop_length']})")
 
 
+def per_call_ms(m, dev, reps):
+    """Best-of-reps time of one enhance_pcm call on 64 clips of 10 s (null lengths, inputs and outputs in HBM)."""
+    from oracle import fullsubnet_oracle as O  # inputs generator only
+    x = O.make_noisy(64, 10 * SR, seed=64, speechlike=True).to(dev)
+    m.enhance_pcm(x, gain=GAIN)
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ms = []
+    for _ in range(max(reps, 3)):
+        ev0.record()
+        m.enhance_pcm(x, gain=GAIN)
+        ev1.record()
+        torch.cuda.synchronize()
+        ms.append(ev0.elapsed_time(ev1))
+    return {"ms": min(ms), "ms_all": ms}
+
+
 def main():
     from fullsubnet_b200 import _lib
     from fullsubnet_b200.inferencer import plan_batches
     from oracle import fullsubnet_oracle as O  # weights / inputs generator only
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--model", default="fullsubnet", choices=["fullsubnet", "improved_fullsubnet"])
+    ap.add_argument("--model", default="fullsubnet", choices=["fullsubnet", "improved_fullsubnet", "fullband_baseline"])
     ap.add_argument("--variant", default="k48", choices=["k48", "k48_960", "k16"],
                     help="improved_fullsubnet constructor args (as bench.py --variant)")
     ap.add_argument("--clips", type=int, default=None, help="default 1024 (fullsubnet), 256 (improved_fullsubnet)")
@@ -169,15 +195,19 @@ def main():
     config = {"workload": f"{a.clips} clips, distinct lengths uniform in 1-10 s at {sr // 1000} kHz ({audio_s:.0f} s of "
                           f"audio), {what}, wav -> enhanced + int16 PCM",
               "precision": m._resolve_precision(), "batch": a.batch, "seed": a.seed}
+    extra = {}
     if improved:
         config.update(model=a.model, variant=a.variant)
+    if a.model == "fullband_baseline":
+        config.update(model=a.model)
+        extra["per_call_64x10s"] = per_call_ms(m, dev, a.steps)
     print(json.dumps({
         "metric": "clips_per_sec", "value": best["e2e"]["clips_per_sec"], "unit": "clips/s", "n_gpus": 1,
         "steps": a.steps, "warmup": a.warmup, "higher_is_better": True, "best_schedule": best_name,
         "speedup_vs_exact_e2e": best["e2e"]["clips_per_sec"] / res["exact"]["e2e"]["clips_per_sec"],
         "speedup_vs_exact_resident": best["resident"]["clips_per_sec"] / res["exact"]["resident"]["clips_per_sec"],
         "config": config,
-        "schedules": res,
+        "schedules": res, **extra,
         "device": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(dev.index or 0)}))
 
 

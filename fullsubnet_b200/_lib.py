@@ -154,6 +154,9 @@ _SIGNATURES = {
     "fsn_clip_adam": (C.c_int, [C.POINTER(ParamList), _F, _F, _F, _F, _F, _F, _I, _P, _P, _S, _P]),
     "fsn_fullband_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
     "fsn_fullband_forward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, _P, _P, _S, _P]),
+    "fsn_fullband_enhance_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I, _I, _I]),
+    "fsn_fullband_enhance": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _F, _P,
+                                       _S, _P]),
     "fsn_fullband_train_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
     "fsn_fullband_train_forward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, _P, _P, _S, _P]),
     "fsn_fullband_train_backward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, C.POINTER(FullbandGrads), _P,

@@ -1,6 +1,7 @@
 // fullband_baseline (recipes/dns_interspeech_2020/fullband_baseline/model.py:8-68; SURVEY 8f rank 3):
 // look-ahead pad -> norm -> num_layers x LSTM(F -> H) -> Linear(H -> 2F) [+ activation] -> [B,2,F,T].
-// Host orchestration: the norm, the fp32 SequenceModel of fsn_fullband.cu (seq_stack_forward) and one re-layout kernel.
+// Host orchestration: the norm, the SequenceModel of fsn_fullband.cu (seq_stack_forward) and one re-layout kernel;
+// fsn_fullband_enhance adds the STFT, the mask + iSTFT of Inferencer.full_band_crm_mask and the int16 output.
 #include <string.h>
 
 #include "fsn_internal.cuh"
@@ -25,6 +26,9 @@ struct FbbWs {
   float *magT, *inv1, *cum1, *y;
   float2 *fs, *sums;
   SeqStackWs seq;
+  float *real, *imag, *crm;  // fsn_fullband_enhance: spectrum of the input, cRM when the caller keeps none
+  unsigned int* peak;        // fsn_fullband_enhance: per-clip max|y| of the int16 output
+  int* lens;                 // fsn_fullband_enhance: device copy of the per-clip lengths
   size_t bytes;
 };
 
@@ -35,10 +39,15 @@ static int fbb_check(const fsn_fullband_desc* d, int B, int T) {
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "fullband: empty input (B=%d, T=%d)", B, T);
   FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE,
               FSN_ERR_UNSUPPORTED, "You must set up a type of Norm. (offline_laplace_norm / cumulative_laplace_norm are built)");
+  // the tensor-core stack misses the reference gates on this model (DESIGN 4.9): f16x3_tc 1.8e-4 waveform max-abs on
+  // the clipping weight set, f16_tc 1.6e-3 relative cRM
+  FSN_REQUIRE(d->precision != FSN_PREC_F16X3_TC && d->precision != FSN_PREC_F16_TC, FSN_ERR_UNSUPPORTED,
+              "fullband: the tensor-core precisions are not built for this model; use FSN_PREC_FP32");
   return FSN_OK;
 }
 
-// num_layers x LSTM(F -> H) + Linear(H -> 2F), rows = clips, fp32 kernels
+// num_layers x LSTM(F -> H) + Linear(H -> 2F), rows = clips, fp32 kernels (also for the training precision
+// FSN_PREC_TF32_TC).  The path does not depend on B, so a clip gets the same bits in any batch.
 static SeqStack fbb_stack(const fsn_fullband_desc* d, int B, int T) {
   SeqStack s;
   memset(&s, 0, sizeof(s));
@@ -48,7 +57,8 @@ static SeqStack fbb_stack(const fsn_fullband_desc* d, int B, int T) {
   return s;
 }
 
-static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbWs& w) {
+// enhance: also the spectrum, cRM, per-clip peak and length table of fsn_fullband_enhance (n_fft / 2 + 1 = num_freqs)
+static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbWs& w, bool enhance = false) {
   Carver c(base);
   const size_t Tp = (size_t)T + d->look_ahead, F = d->num_freqs;
   w.magT = c.take<float>(B * Tp * F);
@@ -58,7 +68,53 @@ static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbW
   w.cum1 = c.take<float>(B * Tp);
   seq_stack_carve(c, fbb_stack(d, B, T), w.seq);
   w.y = c.take<float>(B * Tp * 2 * F);
+  w.real = w.imag = w.crm = nullptr;
+  w.peak = nullptr;
+  w.lens = nullptr;
+  if (enhance) {
+    const size_t BFT = (size_t)B * F * T;
+    w.real = c.take<float>(BFT); w.imag = c.take<float>(BFT); w.crm = c.take<float>(2 * BFT);
+    w.peak = c.take<unsigned int>(B);
+    w.lens = c.take<int>(B);
+  }
   w.bytes = c.off;
+}
+
+// everything after the time-major, look-ahead-padded magnitude w.magT exists: norm -> stack -> out [B,2,F,T].  lens
+// (nullable, device [B] samples): the offline norm of clip b covers only its own Tp_b = 1 + lens[b]/hop + look_ahead
+// frames; the cumulative norm and the stack are causal and run over all Tp steps.
+static int fbb_core(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w, const float* fc_b, int B,
+                    int T, const FbbWs& w, float* out, cudaStream_t st, const int* lens = nullptr, int hop = 0) {
+  int rc;
+  const int F = d->num_freqs, Tp = T + d->look_ahead, la = d->look_ahead;
+  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
+  if ((rc = clip_stats_launch(w.magT, B, Tp, F, 0, w.fs, w.sums, st, lens, hop, la))) return rc;
+  if ((rc = norm_scales_launch(w.sums, w.sums, B, lens ? (float)F : (float)F * Tp, 1.f, w.inv1, nullptr, st, 1e-5f, lens,
+                               hop, la)))
+    return rc;
+  if (cum && (rc = cum_clip_scale_launch(w.fs, B, Tp, F, 1.1920928955078125e-07f, w.cum1, st))) return rc;
+  SeqStack s = fbb_stack(d, B, T);
+  for (int l = 0; l < s.n; ++l) s.L[l] = layers[l];
+  s.x = w.magT; s.scale = cum ? w.cum1 : w.inv1; s.fc_w = fc_w; s.fc_b = fc_b; s.out = w.y;
+  if ((rc = seq_stack_forward(s, w.seq, st))) return rc;
+  const size_t n = (size_t)B * 2 * F * T;
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  fbb_output_kernel<<<blocks, 256, 0, st>>>(w.y, out, B, F, T, Tp, la);
+  FSN_CHECK_LAUNCH("fbb_output_kernel");
+  return FSN_OK;
+}
+
+static int fbb_enhance_dims(const fsn_fullband_desc* d, int B, int L, int n_fft, int hop, bool varlen, int& T) {
+  FSN_REQUIRE(hop > 0 && n_fft > 0 && L > 0, FSN_ERR_SHAPE, "fullband_enhance: bad n_fft/hop/L");
+  FSN_REQUIRE(!varlen || (n_fft & (n_fft - 1)) == 0, FSN_ERR_UNSUPPORTED,
+              "fullband_enhance: n_fft=%d: per-clip lengths are built for the power-of-two (radix-2) transform", n_fft);
+  T = 1 + L / hop;
+  int rc = fbb_check(d, B, T);
+  if (rc) return rc;
+  FSN_REQUIRE(n_fft / 2 + 1 == d->num_freqs, FSN_ERR_SHAPE, "fullband_enhance: n_fft/2+1 = %d != num_freqs = %d",
+              n_fft / 2 + 1, d->num_freqs);
+  return FSN_OK;
 }
 
 }  // namespace fsn
@@ -83,20 +139,46 @@ extern "C" int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_l
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, w.bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  const int F = d->num_freqs, Tp = T + d->look_ahead;
-  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
-  if ((rc = transpose_mag_launch(noisy_mag, w.magT, B, F, T, Tp, st))) return rc;
-  if ((rc = clip_stats_launch(w.magT, B, Tp, F, 0, w.fs, w.sums, st))) return rc;
-  if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)F * Tp, 1.f, w.inv1, nullptr, st))) return rc;
-  if (cum && (rc = cum_clip_scale_launch(w.fs, B, Tp, F, 1.1920928955078125e-07f, w.cum1, st))) return rc;
-  SeqStack s = fbb_stack(d, B, T);
-  for (int l = 0; l < s.n; ++l) s.L[l] = layers[l];
-  s.x = w.magT; s.scale = cum ? w.cum1 : w.inv1; s.fc_w = fc_w; s.fc_b = fc_b; s.out = w.y;
-  if ((rc = seq_stack_forward(s, w.seq, st))) return rc;
-  const size_t n = (size_t)B * 2 * F * T;
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  fbb_output_kernel<<<blocks, 256, 0, st>>>(w.y, out, B, F, T, Tp, d->look_ahead);
-  FSN_CHECK_LAUNCH("fbb_output_kernel");
-  return FSN_OK;
+  if ((rc = transpose_mag_launch(noisy_mag, w.magT, B, d->num_freqs, T, T + d->look_ahead, st))) return rc;
+  return fbb_core(d, layers, fc_w, fc_b, B, T, w, out, st);
+}
+
+// ---- wav -> wav, clips of different lengths in one call (lengths non-null: host [B]), buffers laid out for the longest
+// clip (L_max samples, T_max frames); optional int16 output with the per-clip peak of the iSTFT epilogue
+extern "C" size_t fsn_fullband_enhance_workspace_bytes(const fsn_fullband_desc* d, int B, int L_max, int n_fft, int hop) {
+  int T;
+  if (fbb_enhance_dims(d, B, L_max, n_fft, hop, false, T)) return 0;
+  FbbWs w;
+  fbb_carve(d, B, T, nullptr, w, true);
+  return w.bytes;
+}
+
+extern "C" int fsn_fullband_enhance(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,
+                                    const float* fc_b, const float* wav, const int32_t* lengths, int B, int L_max,
+                                    int n_fft, int hop, int win_length, float* enhanced, float* crm_out, int16_t* pcm,
+                                    float gain, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  int T, rc = fbb_enhance_dims(d, B, L_max, n_fft, hop, lengths != nullptr, T);
+  if (rc) return rc;
+  if (lengths && (rc = check_lengths(lengths, B, L_max, n_fft, "fullband_enhance"))) return rc;
+  FbbWs w;
+  fbb_carve(d, B, T, workspace, w, true);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, w.bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int* lens = lengths ? w.lens : nullptr;
+  float* crm = crm_out ? crm_out : w.crm;
+  if (lengths && (rc = lengths_table_launch(lengths, B, w.lens, st))) return rc;
+  // STFT straight into the time-major magnitude with the look-ahead frames zeroed (model.py:46-49)
+  if ((rc = stft_launch(wav, B, L_max, n_fft, hop, win_length, nullptr, nullptr, w.real, w.imag, w.magT,
+                        T + d->look_ahead, st, lens)))
+    return rc;
+  if ((rc = fbb_core(d, layers, fc_w, fc_b, B, T, w, crm, st, lens, hop))) return rc;
+  // decompress_cIRM + complex product + iSTFT (inferencer.py:130-145)
+  if ((rc = istft_launch(w.real, w.imag, 1, crm, B, T, n_fft, hop, win_length, L_max, enhanced, st, 1,
+                         pcm ? w.peak : nullptr, lens)))
+    return rc;
+  if (pcm && (rc = scale_int16_launch(enhanced, w.peak, B, L_max, gain, pcm, st, lens))) return rc;
+  if (lens && crm_out) rc = zero_frames_past_launch(crm_out, lens, B, 2 * d->num_freqs, T, hop, st);
+  return rc;
 }

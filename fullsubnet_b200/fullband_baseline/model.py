@@ -2,7 +2,8 @@
 
 Same constructor kwargs and ``state_dict`` keys (``fullband_model.sequence_model.weight_ih_l{0,1,2}`` ...,
 ``fullband_model.fc_output_layer.*``); ``forward(noisy_mag [B,1,F,T]) -> [B,2,F,T]`` is one call into libfsn_b200
-(``fsn_fullband_forward``).  With gradients enabled the forward keeps its activations (``fsn_fullband_train_forward``)
+(``fsn_fullband_forward``).  ``enhance`` / ``enhance_pcm`` run the wav -> wav path of ``Inferencer.full_band_crm_mask``
+for a batch of clips, of equal or different lengths, in one call (``fsn_fullband_enhance``).  With gradients enabled the forward keeps its activations (``fsn_fullband_train_forward``)
 and ``loss.backward()`` runs back-propagation through time in the library (``fsn_fullband_train_backward``), the
 training step of fullband_baseline/trainer.py:32-71."""
 from __future__ import annotations
@@ -24,7 +25,7 @@ class Model(BaseModel):
     TRAIN_TF32_STACKS = ("fullband_model",)
 
     def __init__(self, num_freqs, hidden_size, sequence_model, output_activate_function, look_ahead,
-                 norm_type="offline_laplace_norm", weight_init=True):
+                 norm_type="offline_laplace_norm", weight_init=True, precision=None):
         super().__init__()
         self.fullband_model = SequenceModel(input_size=num_freqs, output_size=num_freqs * 2, hidden_size=hidden_size,
                                             num_layers=3, bidirectional=False, sequence_model=sequence_model,
@@ -32,11 +33,24 @@ class Model(BaseModel):
         self.num_freqs = num_freqs
         self.look_ahead = look_ahead
         self.norm = self.norm_wrapper(norm_type)
+        # inference arithmetic: "fp32" (= "auto") only.  The tensor-core stack misses the reference gates on this model
+        # (f16x3_tc: 1.8e-4 waveform max-abs on the clipping weight set; f16_tc: 1.6e-3 relative cRM), so it is not
+        # built, and the process-wide FSN_PRECISION of the other models is not read here.
+        self.precision = precision or "auto"
         # arithmetic of the training step's GEMMs: "fp32" (FMA) | "tf32_tc" (wgmma tf32 for the LSTM layers) | "auto" =
         # tf32_tc when hidden_size is a multiple of 4
         self.train_precision = os.environ.get("FSN_TRAIN_PRECISION", "auto")
         if weight_init:
             self.apply(self.weight_init)
+
+    def _resolve_precision(self) -> str:
+        if self.precision not in ("fp32", "auto"):
+            raise ValueError("fullband_baseline precision must be 'fp32' or 'auto': the tensor-core precisions are not "
+                             "built for this model")
+        return "fp32"
+
+    def _infer_desc(self):
+        return self._desc(_lib.PREC[self._resolve_precision()])
 
     def _train_desc(self):
         return self._desc(_lib.PREC[self._resolve_train_precision()])
@@ -76,7 +90,7 @@ class Model(BaseModel):
             return TrainStep.apply(self, x, *self.parameters())
         lib = _lib.load()
         with torch.cuda.device(x.device):
-            d = self._desc()
+            d = self._infer_desc()
             layers, fc_w, fc_b = self._weight_ptrs()
             n = _lib.check_workspace(lib.fsn_fullband_workspace_bytes(C.byref(d), batch_size, num_frames))
             ws = torch.empty(n, dtype=torch.uint8, device=x.device)
@@ -84,3 +98,48 @@ class Model(BaseModel):
             _lib.check(lib.fsn_fullband_forward(C.byref(d), layers, fc_w, fc_b, x.data_ptr(), batch_size, num_frames,
                                                 out.data_ptr(), ws.data_ptr(), n, _lib.stream_ptr(x.device)))
         return out
+
+    def _enhance_call(self, noisy, n_fft, hop_length, win_length, lengths, crm, pcm, gain):
+        """One fsn_fullband_enhance call: noisy [B,L] -> enhanced [B,L]; clip b is row b's first lengths[b] samples (all
+        L when lengths is None), its outputs 0 past them."""
+        B, L = noisy.shape
+        lens = None if lengths is None else _lib.lengths_table(lengths, B, L)
+        x = _lib.require_cuda(noisy, "noisy")
+        lib = _lib.load()
+        with torch.cuda.device(x.device):
+            d = self._infer_desc()
+            layers, fc_w, fc_b = self._weight_ptrs()
+            n = _lib.check_workspace(lib.fsn_fullband_enhance_workspace_bytes(C.byref(d), B, L, n_fft, hop_length))
+            ws = torch.empty(n, dtype=torch.uint8, device=x.device)
+            out = torch.empty(B, L, dtype=torch.float32, device=x.device)
+            _lib.check(lib.fsn_fullband_enhance(C.byref(d), layers, fc_w, fc_b, x.data_ptr(),
+                                                None if lens is None else lens.ctypes.data, B, L, n_fft, hop_length,
+                                                win_length, out.data_ptr(), _lib.ptr(crm), _lib.ptr(pcm), float(gain),
+                                                ws.data_ptr(), n, _lib.stream_ptr(x.device)))
+        return out
+
+    @torch.no_grad()
+    def enhance(self, noisy, n_fft=512, hop_length=256, win_length=512, return_crm=False, lengths=None):
+        """Fused wav -> wav path of Inferencer.full_band_crm_mask (recipes/.../inferencer.py:130-145), batched over
+        independent clips in one library call (fsn_fullband_enhance): noisy [B,L] -> enhanced [B,L].
+
+        ``lengths`` (B ints, or a CPU integer tensor; max must be L; power-of-two n_fft): clips of different lengths in
+        one call.  Clip b is ``noisy[b, :lengths[b]]``; the rest of the row is never read.  Its outputs equal the call on
+        that clip alone, bit for bit; ``enhanced[b, lengths[b]:]`` and the cRM frames ``t >= 1 + lengths[b] //
+        hop_length`` are 0.  ``return_crm`` additionally returns the [B,2,F,T_max] model output."""
+        assert noisy.dim() == 2, "noisy must be [B, L]"
+        B, L = noisy.shape
+        crm = torch.empty(B, 2, n_fft // 2 + 1, 1 + L // hop_length, dtype=torch.float32,
+                          device=noisy.device) if return_crm else None
+        out = self._enhance_call(noisy, n_fft, hop_length, win_length, lengths, crm, None, 0.0)
+        return (out, crm) if return_crm else out
+
+    @torch.no_grad()
+    def enhance_pcm(self, noisy, n_fft=512, hop_length=256, win_length=512, gain=0.8 * 32767.0, lengths=None):
+        """``enhance`` plus the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:
+        181-182) in the same call, the per-clip max|y| reduced in the iSTFT epilogue: noisy [B,L] -> (enhanced float32
+        [B,L], pcm int16 [B,L]).  ``lengths``: as in ``enhance``; each clip is scaled by the peak of its own samples and
+        its pcm row is 0 past them."""
+        assert noisy.dim() == 2, "noisy must be [B, L]"
+        pcm = torch.empty(noisy.shape, dtype=torch.int16, device=noisy.device)
+        return self._enhance_call(noisy, n_fft, hop_length, win_length, lengths, None, pcm, gain), pcm

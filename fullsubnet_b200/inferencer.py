@@ -108,26 +108,26 @@ class Inferencer:
 
     def supports_lengths(self) -> bool:
         """Whether clips of different lengths can share one call: improved_fullsubnet (every n_fft it accepts), and
-        fullsubnet with a power-of-two n_fft."""
+        fullsubnet and fullband_baseline with a power-of-two n_fft."""
         if takes_waveform(self.model):
             return True
         return hasattr(self.model, "enhance") and self.n_fft & (self.n_fft - 1) == 0
 
     def _check_lengths(self, lengths) -> None:
         if lengths is not None and not takes_waveform(self.model) and not hasattr(self.model, "enhance"):
-            raise NotImplementedError(f"{type(self.model).__module__}: per-clip lengths are built for fullsubnet and "
-                                      "improved_fullsubnet only")
+            raise NotImplementedError(f"{type(self.model).__module__}: per-clip lengths are built for fullsubnet, "
+                                      "improved_fullsubnet and fullband_baseline only")
 
     @torch.no_grad()
     def enhance_batch(self, noisy: torch.Tensor, lengths=None) -> torch.Tensor:
-        """The same path for B independent clips in ONE library call (fsn_enhance): pinned/host or device
-        ``noisy`` [B,L] -> device tensor [B,L].  Equivalent to looping full_band_crm_mask over the clips.
-        ``lengths`` (fullsubnet only): clip b is ``noisy[b, :lengths[b]]`` (fsn_enhance_varlen), its row 0 past it."""
+        """The same path for B independent clips in ONE library call (fsn_enhance, fsn_fullband_enhance): pinned/host or
+        device ``noisy`` [B,L] -> device tensor [B,L].  Equivalent to looping full_band_crm_mask over the clips.
+        ``lengths`` (models with a fused call): clip b is ``noisy[b, :lengths[b]]``, its row 0 past it."""
         self._check_lengths(lengths)
         x = noisy.to(self.device, non_blocking=True)
         if takes_waveform(self.model):  # improved_fullsubnet: one library call with the model's own STFT
             return self.model.enhance(x, lengths=lengths)
-        if hasattr(self.model, "enhance"):  # fullsubnet: one fused library call
+        if hasattr(self.model, "enhance"):  # fullsubnet, fullband_baseline: one fused library call
             return self.model.enhance(x, self.n_fft, self.hop_length, self.win_length, lengths=lengths)
         # other models (fast_fullsubnet): same flow, three library calls (stft -> model -> mask + istft)
         import ctypes as C  # noqa: F401
@@ -235,9 +235,9 @@ class Inferencer:
         ``<output_dir>/<stem>.wav`` is written as 16-bit PCM like the reference.  Returns the written paths.
 
         ``max_padding == 0`` (default): batches of equal-length clips only.  ``max_padding > 0`` (improved_fullsubnet,
-        and fullsubnet with a power-of-two n_fft; other models keep equal-length batches): clips of different lengths
-        share a batch, padded to its longest clip by at most that fraction of the batch's samples, through
-        fsn_enhance_varlen / fsn_improved_enhance.  Every file is bit-identical either way: each clip is bounded by its
+        and fullsubnet and fullband_baseline with a power-of-two n_fft; other models keep equal-length batches): clips of
+        different lengths share a batch, padded to its longest clip by at most that fraction of the batch's samples,
+        through fsn_enhance_varlen / fsn_improved_enhance / fsn_fullband_enhance.  Every file is bit-identical either way: each clip is bounded by its
         own length in the length-dependent kernels."""
         from pathlib import Path
         sr = int(sr or self.sr)

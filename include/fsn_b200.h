@@ -363,8 +363,11 @@ int fsn_clip_adam(const fsn_param_list* L, float max_norm, float grad_scale, flo
 
 /* ------------------------------------------------------------------------------------------
  * recipes/dns_interspeech_2020/fullband_baseline/model.py:8-68  Model (SURVEY 8f rank 3)
- *   look-ahead pad -> norm -> num_layers x LSTM(F -> H) -> Linear(H -> 2F) [+ activation] -> [B,2,F,T]; fp32 kernels.
- *   layers: num_layers entries (PyTorch parameter layout); fc_w [2F,H], fc_b [2F]. */
+ *   look-ahead pad -> norm -> num_layers x LSTM(F -> H) -> Linear(H -> 2F) [+ activation] -> [B,2,F,T].
+ *   layers: num_layers entries (PyTorch parameter layout); fc_w [2F,H], fc_b [2F].
+ * Inference (fsn_fullband_forward, fsn_fullband_enhance) runs the fp32 kernels for FSN_PREC_FP32 and FSN_PREC_TF32_TC;
+ * FSN_PREC_F16X3_TC / FSN_PREC_F16_TC -> FSN_ERR_UNSUPPORTED (the tensor-core stack misses the reference gates on
+ * this model). */
 typedef struct fsn_fullband_desc {
   int32_t num_freqs;
   int32_t hidden;
@@ -372,7 +375,7 @@ typedef struct fsn_fullband_desc {
   int32_t look_ahead;
   int32_t activation; /* FSN_ACT_* */
   int32_t norm_type;  /* FSN_NORM_* */
-  int32_t precision;  /* training only: FSN_PREC_FP32 (0) or FSN_PREC_TF32_TC */
+  int32_t precision;  /* FSN_PREC_FP32 (0) or FSN_PREC_TF32_TC (training: the tf32 GEMMs; inference: fp32 kernels) */
   int32_t cell_type;  /* FSN_CELL_* (0 = LSTM; inference and training are built for LSTM only) */
 } fsn_fullband_desc;
 
@@ -380,6 +383,26 @@ size_t fsn_fullband_workspace_bytes(const fsn_fullband_desc* d, int B, int T);
 int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w, const float* fc_b,
                          const float* noisy_mag, int B, int T, float* out, void* workspace, size_t workspace_bytes,
                          fsn_stream_t stream);
+/* wav -> wav: the fullband_baseline Model inside Inferencer.full_band_crm_mask (recipes/dns_interspeech_2020/
+ * inferencer.py:130-145: stft -> model -> decompress_cIRM -> complex product -> istft) for B clips in one call, with the
+ * int16 output of the reference host loop.  Row b of wav [B, L_max] holds clip b's lengths[b] samples; samples at index
+ * >= lengths[b] are never read.  lengths: HOST int32 [B], nullable (= every clip L_max samples), n_fft/2 < lengths[b] <=
+ * L_max and max(lengths) == L_max (else FSN_ERR_SHAPE naming the clip); copied into the workspace through kernel
+ * parameters during the call and not retained.  n_fft / 2 + 1 must equal num_freqs.  Outputs, T_max = 1 + L_max/hop:
+ *   enhanced [B, L_max]           0 past lengths[b]
+ *   crm_out  [B, 2, F, T_max]     nullable; the model's output, 0 for frames t >= T_b = 1 + lengths[b]/hop
+ *   pcm      [B, L_max] int16     nullable; int16(gain * y / max|y|) over the clip's own samples, 0 past lengths[b]
+ * With null lengths, enhanced equals fsn_stft -> fsn_fullband_forward -> fsn_istft bit for bit and crm_out equals
+ * fsn_fullband_forward; any n_fft fsn_stft / fsn_istft accept.  With lengths, every clip's outputs are bit-identical to
+ * a null-lengths call on that clip alone with L = lengths[b] (and pcm to fsn_peak_normalize_int16 of that waveform): the
+ * stack is causal and runs over T_max + look_ahead steps for every clip; only the STFT, the offline norm, the iSTFT and
+ * the int16 scaling are bounded per clip.  n_fft must then be a power of two (else FSN_ERR_UNSUPPORTED).  Same precisions,
+ * norms and cells as fsn_fullband_forward.  Never allocates, never synchronises the host. */
+size_t fsn_fullband_enhance_workspace_bytes(const fsn_fullband_desc* d, int B, int L_max, int n_fft, int hop);
+int fsn_fullband_enhance(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w, const float* fc_b,
+                         const float* wav, const int32_t* lengths, int B, int L_max, int n_fft, int hop, int win_length,
+                         float* enhanced, float* crm_out, int16_t* pcm, float gain, void* workspace,
+                         size_t workspace_bytes, fsn_stream_t stream);
 
 /* Training step of recipes/dns_interspeech_2020/fullband_baseline/trainer.py:32-71, same conventions as fsn_train_*: the
  * caller allocates the workspace and passes the same untouched buffer from forward to backward; the gradients of all
