@@ -5,9 +5,9 @@ uniform in 1 - 10 s at 16 kHz, the inference.toml model with weights W-a, the de
 wav -> enhanced wav + int16 PCM (what the file loop writes).  Two schedules of the same clips:
 
   exact       equal-length batches (``plan_batches(lengths, 256, 0)``): every length is distinct, so B = 1 per call
-              (fsn_enhance_pcm), which is what the file loop does on real recordings by default;
+              (fsn_enhance with the int16 output), which is what the file loop does on real recordings by default;
   pad<x>      ``plan_batches(lengths, 256, x)``: length-sorted runs of <= 256 clips padded to their longest clip by at
-              most a fraction x of the batch's samples, one fsn_enhance_varlen call per batch.
+              most a fraction x of the batch's samples, one fsn_enhance call with per-clip lengths per batch.
 
 --model improved_fullsubnet --variant k16|k48|k48_960: the same schedules for improved_fullsubnet with bench.py's
 constructor arguments and weights of that variant, the default precision ("auto": tf32_tc), clip lengths distinct and

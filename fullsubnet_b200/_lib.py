@@ -117,13 +117,8 @@ _SIGNATURES = {
     "fsn_model_forward": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P,
                                     _I, _I, _P, _P, _S, _P]),
     "fsn_enhance_workspace_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I, _I]),
-    "fsn_enhance": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P, _I, _I,
-                              _I, _I, _I, _P, _P, _P, _S, _P]),
-    "fsn_enhance_pcm": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P, _I, _I,
-                                  _I, _I, _I, _P, _P, _F, _P, _S, _P]),
-    "fsn_enhance_varlen_workspace_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I, _I]),
-    "fsn_enhance_varlen": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P, _P, _I,
-                                     _I, _I, _I, _I, _P, _P, _P, _F, _P, _S, _P]),
+    "fsn_enhance": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P, _P, _I, _I,
+                              _I, _I, _I, _P, _P, _P, _F, _P, _S, _P]),
     "fsn_fast_workspace_bytes": (_S, [C.POINTER(FastDesc), _I, _I]),
     "fsn_fast_packed_bytes": (_S, [C.POINTER(FastDesc)]),
     "fsn_fast_pack_bn_weights": (C.c_int, [C.POINTER(FastDesc), C.POINTER(FastWeights), _P, _P]),

@@ -8,7 +8,7 @@
 // (T-contiguous) stores / loads of the reference layout are FR*4-byte segments.
 #include <string.h>
 
-#include "fsn_common.cuh"
+#include "fsn_internal.cuh"
 
 namespace fsn {
 
@@ -557,32 +557,61 @@ extern "C" int fsn_si_sdr(const float* reference, const float* estimation, int B
   return FSN_OK;
 }
 
-// int16 scaling with the per-clip peak the iSTFT epilogue produced (fsn_enhance_pcm)
+// ---- the wav side of the wav -> wav entry points (fsn_internal.cuh)
 namespace fsn {
-int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st,
-                       const int* lens) {
-  const size_t n = (size_t)B * L;
-  scale_int16_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(wav, peak_bits, L, gain, out, n, lens);
-  FSN_CHECK_LAUNCH("scale_int16_kernel");
+void wav_carve(Carver& c, int B, int F, int T, WavWs& w) {
+  const size_t BFT = (size_t)B * F * T;
+  w.real = w.imag = w.crm = nullptr;
+  if (BFT) { w.real = c.take<float>(BFT); w.imag = c.take<float>(BFT); w.crm = c.take<float>(2 * BFT); }
+  w.peak = c.take<unsigned int>(B);
+  w.lens = c.take<int>(B);
+}
+
+int wav_check(const int32_t* lengths, int B, int L_max, int n_fft, bool pow2_lengths, const float* enhanced,
+              const char* who) {
+  if (lengths) {
+    FSN_REQUIRE(!pow2_lengths || (n_fft & (n_fft - 1)) == 0, FSN_ERR_UNSUPPORTED,
+                "%s: n_fft=%d: per-clip lengths are built for the power-of-two (radix-2) transform", who, n_fft);
+    int longest = 0;
+    for (int b = 0; b < B; ++b) {
+      FSN_REQUIRE(lengths[b] > n_fft / 2 && lengths[b] <= L_max, FSN_ERR_SHAPE,
+                  "%s: clip %d has length %d, outside (n_fft/2, L_max] = (%d, %d]", who, b, lengths[b], n_fft / 2, L_max);
+      longest = lengths[b] > longest ? lengths[b] : longest;
+    }
+    FSN_REQUIRE(longest == L_max, FSN_ERR_SHAPE, "%s: the longest clip has %d samples, L_max = %d", who, longest, L_max);
+  }
+  FSN_REQUIRE(enhanced, FSN_ERR_SHAPE, "%s: enhanced output buffer missing", who);
   return FSN_OK;
 }
 
-int lengths_table_launch(const int32_t* host_lengths, int B, int* lengths, cudaStream_t st) {
+int wav_prologue(const int32_t* lengths, int B, WavWs& w, cudaStream_t st) {
+  if (!lengths) {
+    w.lens = nullptr;
+    return FSN_OK;
+  }
   LenChunk c;
   for (int off = 0; off < B; off += kLenChunk) {
     c.off = off;
     c.n = B - off < kLenChunk ? B - off : kLenChunk;
-    memcpy(c.v, host_lengths + off, (size_t)c.n * sizeof(int));
-    lengths_table_kernel<<<cdiv(c.n, 256), 256, 0, st>>>(c, lengths);
+    memcpy(c.v, lengths + off, (size_t)c.n * sizeof(int));
+    lengths_table_kernel<<<cdiv(c.n, 256), 256, 0, st>>>(c, w.lens);
     FSN_CHECK_LAUNCH("lengths_table_kernel");
   }
   return FSN_OK;
 }
 
-int zero_frames_past_launch(float* crm, const int* lengths, int B, int C, int T, int hop, cudaStream_t st) {
-  const size_t n = (size_t)B * C * T;
-  zero_frames_past_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(crm, lengths, C, T, hop, n);
-  FSN_CHECK_LAUNCH("zero_frames_past_kernel");
+int wav_epilogue(const WavWs& w, const float* enhanced, int B, int L, int16_t* pcm, float gain, float* crm_out, int F, int T,
+                 int hop, cudaStream_t st) {
+  if (pcm) {
+    const size_t n = (size_t)B * L;
+    scale_int16_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(enhanced, w.peak, L, gain, pcm, n, w.lens);
+    FSN_CHECK_LAUNCH("scale_int16_kernel");
+  }
+  if (w.lens && crm_out) {
+    const size_t n = (size_t)B * 2 * F * T;
+    zero_frames_past_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(crm_out, w.lens, 2 * F, T, hop, n);
+    FSN_CHECK_LAUNCH("zero_frames_past_kernel");
+  }
   return FSN_OK;
 }
 }  // namespace fsn

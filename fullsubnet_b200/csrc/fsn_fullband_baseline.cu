@@ -26,9 +26,7 @@ struct FbbWs {
   float *magT, *inv1, *cum1, *y;
   float2 *fs, *sums;
   SeqStackWs seq;
-  float *real, *imag, *crm;  // fsn_fullband_enhance: spectrum of the input, cRM when the caller keeps none
-  unsigned int* peak;        // fsn_fullband_enhance: per-clip max|y| of the int16 output
-  int* lens;                 // fsn_fullband_enhance: device copy of the per-clip lengths
+  WavWs wav;  // fsn_fullband_enhance
   size_t bytes;
 };
 
@@ -57,7 +55,7 @@ static SeqStack fbb_stack(const fsn_fullband_desc* d, int B, int T) {
   return s;
 }
 
-// enhance: also the spectrum, cRM, per-clip peak and length table of fsn_fullband_enhance (n_fft / 2 + 1 = num_freqs)
+// enhance: also the wav-side buffers of fsn_fullband_enhance (n_fft / 2 + 1 = num_freqs)
 static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbWs& w, bool enhance = false) {
   Carver c(base);
   const size_t Tp = (size_t)T + d->look_ahead, F = d->num_freqs;
@@ -68,15 +66,7 @@ static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbW
   w.cum1 = c.take<float>(B * Tp);
   seq_stack_carve(c, fbb_stack(d, B, T), w.seq);
   w.y = c.take<float>(B * Tp * 2 * F);
-  w.real = w.imag = w.crm = nullptr;
-  w.peak = nullptr;
-  w.lens = nullptr;
-  if (enhance) {
-    const size_t BFT = (size_t)B * F * T;
-    w.real = c.take<float>(BFT); w.imag = c.take<float>(BFT); w.crm = c.take<float>(2 * BFT);
-    w.peak = c.take<unsigned int>(B);
-    w.lens = c.take<int>(B);
-  }
+  if (enhance) wav_carve(c, B, (int)F, T, w.wav);
   w.bytes = c.off;
 }
 
@@ -105,10 +95,8 @@ static int fbb_core(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, co
   return FSN_OK;
 }
 
-static int fbb_enhance_dims(const fsn_fullband_desc* d, int B, int L, int n_fft, int hop, bool varlen, int& T) {
+static int fbb_enhance_dims(const fsn_fullband_desc* d, int B, int L, int n_fft, int hop, int& T) {
   FSN_REQUIRE(hop > 0 && n_fft > 0 && L > 0, FSN_ERR_SHAPE, "fullband_enhance: bad n_fft/hop/L");
-  FSN_REQUIRE(!varlen || (n_fft & (n_fft - 1)) == 0, FSN_ERR_UNSUPPORTED,
-              "fullband_enhance: n_fft=%d: per-clip lengths are built for the power-of-two (radix-2) transform", n_fft);
   T = 1 + L / hop;
   int rc = fbb_check(d, B, T);
   if (rc) return rc;
@@ -147,7 +135,7 @@ extern "C" int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_l
 // clip (L_max samples, T_max frames); optional int16 output with the per-clip peak of the iSTFT epilogue
 extern "C" size_t fsn_fullband_enhance_workspace_bytes(const fsn_fullband_desc* d, int B, int L_max, int n_fft, int hop) {
   int T;
-  if (fbb_enhance_dims(d, B, L_max, n_fft, hop, false, T)) return 0;
+  if (fbb_enhance_dims(d, B, L_max, n_fft, hop, T)) return 0;
   FbbWs w;
   fbb_carve(d, B, T, nullptr, w, true);
   return w.bytes;
@@ -158,27 +146,25 @@ extern "C" int fsn_fullband_enhance(const fsn_fullband_desc* d, const fsn_lstm_l
                                     int n_fft, int hop, int win_length, float* enhanced, float* crm_out, int16_t* pcm,
                                     float gain, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
   launch_counter() = 0;
-  int T, rc = fbb_enhance_dims(d, B, L_max, n_fft, hop, lengths != nullptr, T);
+  int T, rc = fbb_enhance_dims(d, B, L_max, n_fft, hop, T);
   if (rc) return rc;
-  if (lengths && (rc = check_lengths(lengths, B, L_max, n_fft, "fullband_enhance"))) return rc;
+  if ((rc = wav_check(lengths, B, L_max, n_fft, true, enhanced, "fullband_enhance"))) return rc;
   FbbWs w;
   fbb_carve(d, B, T, workspace, w, true);
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, w.bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  const int* lens = lengths ? w.lens : nullptr;
-  float* crm = crm_out ? crm_out : w.crm;
-  if (lengths && (rc = lengths_table_launch(lengths, B, w.lens, st))) return rc;
+  WavWs& e = w.wav;
+  float* crm = crm_out ? crm_out : e.crm;
+  if ((rc = wav_prologue(lengths, B, e, st))) return rc;
   // STFT straight into the time-major magnitude with the look-ahead frames zeroed (model.py:46-49)
-  if ((rc = stft_launch(wav, B, L_max, n_fft, hop, win_length, nullptr, nullptr, w.real, w.imag, w.magT,
-                        T + d->look_ahead, st, lens)))
+  if ((rc = stft_launch(wav, B, L_max, n_fft, hop, win_length, nullptr, nullptr, e.real, e.imag, w.magT,
+                        T + d->look_ahead, st, e.lens)))
     return rc;
-  if ((rc = fbb_core(d, layers, fc_w, fc_b, B, T, w, crm, st, lens, hop))) return rc;
+  if ((rc = fbb_core(d, layers, fc_w, fc_b, B, T, w, crm, st, e.lens, hop))) return rc;
   // decompress_cIRM + complex product + iSTFT (inferencer.py:130-145)
-  if ((rc = istft_launch(w.real, w.imag, 1, crm, B, T, n_fft, hop, win_length, L_max, enhanced, st, 1,
-                         pcm ? w.peak : nullptr, lens)))
+  if ((rc = istft_launch(e.real, e.imag, 1, crm, B, T, n_fft, hop, win_length, L_max, enhanced, st, 1,
+                         pcm ? e.peak : nullptr, e.lens)))
     return rc;
-  if (pcm && (rc = scale_int16_launch(enhanced, w.peak, B, L_max, gain, pcm, st, lens))) return rc;
-  if (lens && crm_out) rc = zero_frames_past_launch(crm_out, lens, B, 2 * d->num_freqs, T, hop, st);
-  return rc;
+  return wav_epilogue(e, enhanced, B, L_max, pcm, gain, crm_out, d->num_freqs, T, hop, st);
 }

@@ -100,8 +100,7 @@ struct ImpWs {
   float *h0[2], *h1[2], *c0, *c1;
   LayerSave tc;                        // FSN_PREC_TF32_TC: gates / cell / hidden of every step of one layer
   float *tc_h1, *tc_rec;
-  unsigned int* peak;                  // fsn_improved_enhance: per-clip max|y| of the int16 output
-  int* lens;                           // fsn_improved_enhance: device copy of the per-clip lengths
+  WavWs wav;                           // fsn_improved_enhance: peak and length table (spectrum and cRM above)
   size_t bytes;
 };
 
@@ -169,8 +168,7 @@ static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, 
     w.tc_h1 = c.take<float>(TR * d->sb_hidden);
     w.tc_rec = c.take<float>(4 * RH);
   }
-  w.peak = enhance ? c.take<unsigned int>(m.B) : nullptr;
-  w.lens = enhance ? c.take<int>(m.B) : nullptr;
+  if (enhance) wav_carve(c, m.B, 0, m.T, w.wav);
   w.bytes = c.off;
 }
 
@@ -297,16 +295,13 @@ extern "C" int fsn_improved_enhance(const fsn_improved_desc* d, const fsn_improv
   ImpDims m;
   int rc = imp_dims(d, B, L_max, m);
   if (rc) return rc;
-  if (lengths && (rc = check_lengths(lengths, B, L_max, d->n_fft, "improved_enhance"))) return rc;
+  if ((rc = wav_check(lengths, B, L_max, d->n_fft, false, enhanced, "improved_enhance"))) return rc;
   ImpWs w;
   imp_carve(d, m, workspace, w, true);
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, w.bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  const int* lens = lengths ? w.lens : nullptr;
-  if (lengths && (rc = lengths_table_launch(lengths, B, w.lens, st))) return rc;
-  if ((rc = imp_forward(d, wt, m, w, wav, enhanced, crm_out, pcm ? w.peak : nullptr, lens, st))) return rc;
-  if (pcm && (rc = scale_int16_launch(enhanced, w.peak, B, L_max, gain, pcm, st, lens))) return rc;
-  if (lens && crm_out) rc = zero_frames_past_launch(crm_out, lens, B, 2 * m.F, m.T, d->hop_length, st);
-  return rc;
+  if ((rc = wav_prologue(lengths, B, w.wav, st))) return rc;
+  if ((rc = imp_forward(d, wt, m, w, wav, enhanced, crm_out, pcm ? w.wav.peak : nullptr, w.wav.lens, st))) return rc;
+  return wav_epilogue(w.wav, enhanced, B, L_max, pcm, gain, crm_out, m.F, m.T, d->hop_length, st);
 }

@@ -236,7 +236,7 @@ int norm_scales_launch(const float2* mag_sums, const float2* fb_sums, int B, flo
                        float* inv2, cudaStream_t st, float eps = 1e-5f, const int* lens = nullptr, int hop = 0,
                        int la = 0);
 
-// lens (nullable, device [B]): clip b has lens[b] of the L samples of its row (fsn_enhance_varlen, fsn_improved_enhance)
+// lens (nullable, device [B]): clip b has lens[b] of the L samples of its row (the *_enhance entry points)
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
                 float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens = nullptr);
 // mask_mode: 1 = decompress_cIRM + complex product (fullsubnet), 2 = element-wise re*crm0, im*crm1 (improved_fullsubnet)
@@ -244,17 +244,31 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
                  int hop, int win_length, int length, float* wav, cudaStream_t st, int mask_mode = 1,
                  unsigned int* peak_bits = nullptr, const int* lens = nullptr);
 // peak_bits (optional, [B]): max|wav| per clip as float bits, reduced in the iSTFT epilogue (radix-2 and direct DFT alike,
-// bounded by lens when given); scale_int16_launch turns
-// it into the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:181-182)
-int scale_int16_launch(const float* wav, const unsigned int* peak_bits, int B, int L, float gain, int16_t* out, cudaStream_t st,
-                       const int* lens = nullptr);
-// device int32 table lengths[B] <- host_lengths, through kernel parameters (the host array is not read after the call)
-int lengths_table_launch(const int32_t* host_lengths, int B, int* lengths, cudaStream_t st);
-// crm [B, C, T]: frames t >= 1 + lengths[b]/hop of clip b set to 0
-int zero_frames_past_launch(float* crm, const int* lengths, int B, int C, int T, int hop, cudaStream_t st);
-// host checks of a per-clip length table before any CUDA call: n_fft/2 < lengths[b] <= L_max and max == L_max, else
-// FSN_ERR_SHAPE naming the clip (`who` prefixes the message)
-int check_lengths(const int32_t* lengths, int B, int L_max, int n_fft, const char* who);
+// bounded by lens when given); wav_epilogue turns it into the int16 scaling of the reference host loop
+// (audio_zen/inferencer/base_inferencer.py:181-182)
+
+// ---- the wav side of the wav -> wav entry points (fsn_enhance, fsn_fullband_enhance, fsn_improved_enhance).  Each reads
+// dims -> wav_check -> carve -> workspace check -> wav_prologue -> its own STFT / model / iSTFT (peak when pcm is given,
+// lens) -> wav_epilogue.
+struct WavWs {
+  float *real, *imag, *crm;  // spectrum of the input [B,F,T]; cRM [B,2,F,T] when the caller keeps none
+  unsigned int* peak;        // per-clip max|y| of the int16 output
+  int* lens;                 // device copy of the per-clip lengths; nullptr after wav_prologue when the call has none
+};
+// F = 0: the peak and length table only (improved_fullsubnet carves its spectrum and cRM where its forward needs them)
+void wav_carve(Carver& c, int B, int F, int T, WavWs& w);
+// host checks before any CUDA call.  lengths (nullable, host [B]): n_fft/2 < lengths[b] <= L_max and max == L_max, else
+// FSN_ERR_SHAPE naming the clip; with pow2_lengths a non-power-of-two n_fft refuses them (FSN_ERR_UNSUPPORTED).
+// enhanced must be non-null.  `who` prefixes the messages.
+int wav_check(const int32_t* lengths, int B, int L_max, int n_fft, bool pow2_lengths, const float* enhanced,
+              const char* who);
+// device length table w.lens <- lengths through kernel parameters (the host array is not read after the call); no
+// lengths: w.lens = nullptr, so the kernels that take lens run their whole-row path
+int wav_prologue(const int32_t* lengths, int B, WavWs& w, cudaStream_t st);
+// pcm (nullable) <- int16 scaling of enhanced [B,L] by the peak; with lengths, the caller's crm_out [B,2,F,T] (nullable)
+// is zeroed for frames t >= 1 + lengths[b]/hop
+int wav_epilogue(const WavWs& w, const float* enhanced, int B, int L, int16_t* pcm, float gain, float* crm_out, int F, int T,
+                 int hop, cudaStream_t st);
 
 // adjoint of the element-wise mask + iSTFT of improved_fullsubnet (istft_launch mask_mode 2) with respect to the mask:
 // dwav [B,L] -> dcrm [B,2,F,T] for the rows f < F-1 (the Nyquist row of the cRM is a constant; it is not written)

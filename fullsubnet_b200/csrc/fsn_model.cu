@@ -108,7 +108,7 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
 }
 
 // everything after the time-major magnitude exists: norms, full-band stack, sub-band stack.  lens (nullable, device
-// [B] samples, fsn_enhance_varlen): the offline norms of clip b cover only its own Tp_b = 1 + lens[b]/hop + look_ahead
+// [B] samples, fsn_enhance): the offline norms of clip b cover only its own Tp_b = 1 + lens[b]/hop + look_ahead
 // frames; every other stage is causal and runs unchanged over all Tp steps (frames past Tp_b never reach earlier ones).
 static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
                       const void* sb_packed, const Dims& m, const ModelWs& w, float* crm, cudaStream_t st,
@@ -182,7 +182,7 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
 
 using namespace fsn;
 
-extern "C" int fsn_version(void) { return 100; }
+extern "C" int fsn_version(void) { return 101; }
 extern "C" const char* fsn_last_error(void) { return g_err; }
 extern "C" int fsn_last_error_code(void) { return g_err_code; }
 extern "C" int64_t fsn_last_launch_count(void) { return g_launches; }
@@ -253,130 +253,68 @@ extern "C" int fsn_model_forward(const fsn_model_desc* d, const fsn_seq_weights*
   return model_core(d, fb, sb, sb_packed, m, w, crm, st);
 }
 
-struct EnhanceWs {
-  float *real, *imag, *crm;
-  unsigned int* peak;
-  int* lens;  // fsn_enhance_varlen: device copy of the per-clip lengths
-  void* model;
-  size_t bytes;
-};
-
-static int carve_enhance(const fsn_model_desc* d, int B, int L, int n_fft, int hop, void* base, EnhanceWs& e,
-                         Dims& m, bool varlen = false) {
+// ---- wav -> wav (fsn_enhance).  Batched inference == loop of B=1 calls of the reference inferencer: drop_band off
+// (audio_zen/inferencer/base_inferencer.py:78,173; SURVEY fact 4).  Buffers are laid out for the longest clip (L_max
+// samples, T frames); with lengths, the length-dependent kernels (STFT, offline norms, iSTFT, int16 scaling) are bounded
+// per clip by the device copy of the table.
+static int enhance_dims(const fsn_model_desc* d, int B, int L, int n_fft, int hop, fsn_model_desc& dd, Dims& m) {
   FSN_REQUIRE(hop > 0 && n_fft > 0, FSN_ERR_SHAPE, "enhance: bad n_fft/hop");
-  FSN_REQUIRE(!varlen || (n_fft & (n_fft - 1)) == 0, FSN_ERR_UNSUPPORTED,
-              "enhance_varlen: n_fft=%d: per-clip lengths are built for the power-of-two (radix-2) transform", n_fft);
-  const int T = 1 + L / hop;
-  int rc = make_dims(d, B, T, m);
+  dd = *d;
+  dd.num_groups_in_drop_band = 1;
+  int rc = make_dims(&dd, B, 1 + L / hop, m);
   if (rc) return rc;
   FSN_REQUIRE(n_fft / 2 + 1 == d->num_freqs, FSN_ERR_SHAPE, "enhance: n_fft/2+1 = %d != num_freqs = %d",
               n_fft / 2 + 1, d->num_freqs);
+  return FSN_OK;
+}
+
+// the wav-side buffers, then the model's; returns the bytes
+static size_t carve_enhance(const fsn_model_desc* d, const Dims& m, void* base, WavWs& e, ModelWs& w) {
   Carver c(base);
-  const size_t BFT = (size_t)B * m.F * T;
-  e.real = c.take<float>(BFT);
-  e.imag = c.take<float>(BFT);
-  e.crm = c.take<float>(2 * BFT);
-  e.peak = c.take<unsigned int>(B);
-  e.lens = varlen ? c.take<int>(B) : nullptr;
+  wav_carve(c, m.B, m.F, m.T, e);
+  carve_model(d, m, base ? (char*)base + c.off : nullptr, w);
+  return c.off + w.bytes;
+}
+
+extern "C" size_t fsn_enhance_workspace_bytes(const fsn_model_desc* d, int B, int L_max, int n_fft, int hop) {
+  fsn_model_desc dd;
+  Dims m;
+  if (enhance_dims(d, B, L_max, n_fft, hop, dd, m)) return 0;
+  WavWs e;
   ModelWs w;
-  carve_model(d, m, nullptr, w);
-  e.model = base ? (char*)base + c.off : nullptr;
-  e.bytes = c.off + w.bytes;
-  return FSN_OK;
+  return carve_enhance(&dd, m, nullptr, e, w);
 }
 
-static size_t enhance_workspace_bytes(const fsn_model_desc* d, int B, int L, int n_fft, int hop, bool varlen) {
-  EnhanceWs e;
-  Dims m;
-  fsn_model_desc dd = *d;
-  dd.num_groups_in_drop_band = 1;
-  if (carve_enhance(&dd, B, L, n_fft, hop, nullptr, e, m, varlen)) return 0;
-  return e.bytes;
-}
-
-extern "C" size_t fsn_enhance_workspace_bytes(const fsn_model_desc* d, int B, int L, int n_fft, int hop) {
-  return enhance_workspace_bytes(d, B, L, n_fft, hop, false);
-}
-
-// ---- clips of different lengths in one call (lengths non-null: host [B]): buffers laid out for the longest clip
-// (L = L_max samples, T_max frames), the length-dependent kernels (STFT, offline norms, iSTFT, int16 scaling) bounded
-// per clip by the device copy of the table
-extern "C" size_t fsn_enhance_varlen_workspace_bytes(const fsn_model_desc* d, int B, int L_max, int n_fft, int hop) {
-  return enhance_workspace_bytes(d, B, L_max, n_fft, hop, true);
-}
-
-namespace fsn {
-int check_lengths(const int32_t* lengths, int B, int L_max, int n_fft, const char* who) {
-  int longest = 0;
-  for (int b = 0; b < B; ++b) {
-    FSN_REQUIRE(lengths[b] > n_fft / 2 && lengths[b] <= L_max, FSN_ERR_SHAPE,
-                "%s: clip %d has length %d, outside (n_fft/2, L_max] = (%d, %d]", who, b, lengths[b], n_fft / 2, L_max);
-    longest = lengths[b] > longest ? lengths[b] : longest;
-  }
-  FSN_REQUIRE(longest == L_max, FSN_ERR_SHAPE, "%s: the longest clip has %d samples, L_max = %d", who, longest, L_max);
-  return FSN_OK;
-}
-}  // namespace fsn
-
-static int enhance_impl(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                        const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L, int n_fft, int hop,
-                        int win_length, float* enhanced, float* crm_out, int16_t* pcm, float pcm_gain, void* workspace,
-                        size_t workspace_bytes, fsn_stream_t stream) {
+extern "C" int fsn_enhance(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                           const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L_max, int n_fft,
+                           int hop, int win_length, float* enhanced, float* crm_out, int16_t* pcm, float gain,
+                           void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
   g_launches = 0;
-  // batched inference == loop of B=1 calls of the reference inferencer: drop_band off
-  // (audio_zen/inferencer/base_inferencer.py:78,173; SURVEY fact 4)
-  fsn_model_desc dd = *d;
-  dd.num_groups_in_drop_band = 1;
-  EnhanceWs e;
+  fsn_model_desc dd;
   Dims m;
-  int rc = carve_enhance(&dd, B, L, n_fft, hop, workspace, e, m, lengths != nullptr);
+  int rc = enhance_dims(d, B, L_max, n_fft, hop, dd, m);
   if (rc) return rc;
   FSN_REQUIRE(dd.precision == FSN_PREC_FP32 || sb_tc_supported(&dd), FSN_ERR_UNSUPPORTED,
               "FSN_PREC_F16_TC / FSN_PREC_F16X3_TC need sb_hidden in {128,256,384} and sub-band input width <= 32");
-  if (lengths && (rc = check_lengths(lengths, B, L, n_fft, "enhance_varlen"))) return rc;
-  FSN_REQUIRE(workspace && workspace_bytes >= e.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
-              workspace_bytes, e.bytes);
+  if ((rc = wav_check(lengths, B, L_max, n_fft, true, enhanced, "enhance"))) return rc;
+  WavWs e;
   ModelWs w;
-  carve_model(&dd, m, e.model, w);
+  const size_t bytes = carve_enhance(&dd, m, workspace, e, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, bytes);
   cudaStream_t st = (cudaStream_t)stream;
   float* crm = crm_out ? crm_out : e.crm;
   prof_reset();
   prof_mark(0, st);
-  if (lengths && (rc = lengths_table_launch(lengths, B, e.lens, st))) return rc;
-  if ((rc = stft_launch(wav, B, L, n_fft, hop, win_length, nullptr, nullptr, e.real, e.imag, w.magT, m.Tp, st, e.lens)))
+  if ((rc = wav_prologue(lengths, B, e, st))) return rc;
+  if ((rc = stft_launch(wav, B, L_max, n_fft, hop, win_length, nullptr, nullptr, e.real, e.imag, w.magT, m.Tp, st,
+                        e.lens)))
     return rc;
   prof_mark(1, st);
   if ((rc = model_core(&dd, fb, sb, sb_packed, m, w, crm, st, e.lens, hop))) return rc;
-  rc = istft_launch(e.real, e.imag, 1, crm, B, m.T, n_fft, hop, win_length, L, enhanced, st, 1, pcm ? e.peak : nullptr,
+  rc = istft_launch(e.real, e.imag, 1, crm, B, m.T, n_fft, hop, win_length, L_max, enhanced, st, 1, pcm ? e.peak : nullptr,
                     e.lens);
-  if (!rc && pcm) rc = scale_int16_launch(enhanced, e.peak, B, L, pcm_gain, pcm, st, e.lens);
-  if (!rc && lengths && crm_out) rc = zero_frames_past_launch(crm_out, e.lens, B, 2 * m.F, m.T, hop, st);
+  if (!rc) rc = wav_epilogue(e, enhanced, B, L_max, pcm, gain, crm_out, m.F, m.T, hop, st);
   prof_mark(4, st);
   return rc;
-}
-
-extern "C" int fsn_enhance(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                           const void* sb_packed, const float* wav, int B, int L, int n_fft, int hop,
-                           int win_length, float* enhanced, float* crm_out, void* workspace,
-                           size_t workspace_bytes, fsn_stream_t stream) {
-  return enhance_impl(d, fb, sb, sb_packed, wav, nullptr, B, L, n_fft, hop, win_length, enhanced, crm_out, nullptr, 0.f,
-                      workspace, workspace_bytes, stream);
-}
-
-extern "C" int fsn_enhance_pcm(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                               const void* sb_packed, const float* wav, int B, int L, int n_fft, int hop,
-                               int win_length, float* enhanced, int16_t* pcm, float gain, void* workspace,
-                               size_t workspace_bytes, fsn_stream_t stream) {
-  FSN_REQUIRE(pcm && enhanced, FSN_ERR_SHAPE, "enhance_pcm: output buffers missing");
-  return enhance_impl(d, fb, sb, sb_packed, wav, nullptr, B, L, n_fft, hop, win_length, enhanced, nullptr, pcm, gain,
-                      workspace, workspace_bytes, stream);
-}
-
-extern "C" int fsn_enhance_varlen(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                                  const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L_max,
-                                  int n_fft, int hop, int win_length, float* enhanced, float* crm_out, int16_t* pcm,
-                                  float gain, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
-  FSN_REQUIRE(lengths, FSN_ERR_SHAPE, "enhance_varlen: lengths missing");
-  return enhance_impl(d, fb, sb, sb_packed, wav, lengths, B, L_max, n_fft, hop, win_length, enhanced, crm_out, pcm, gain,
-                      workspace, workspace_bytes, stream);
 }

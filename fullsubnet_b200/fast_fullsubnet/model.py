@@ -178,9 +178,7 @@ class Model(BaseModel):
         lib = _lib.load()
         with torch.cuda.device(x.device):
             d, w = self._structs(x.device)
-            n = lib.fsn_fast_workspace_bytes(C.byref(d), batch_size, num_frames)
-            if n == 0:
-                _lib.check_workspace(n)
+            n = _lib.check_workspace(lib.fsn_fast_workspace_bytes(C.byref(d), batch_size, num_frames))
             ws = torch.empty(n, dtype=torch.uint8, device=x.device)
             out = torch.empty(batch_size, 2, num_freqs, num_frames, dtype=torch.float32, device=x.device)
             _lib.check(lib.fsn_fast_model_forward(C.byref(d), C.byref(w), x.data_ptr(), batch_size, num_frames,

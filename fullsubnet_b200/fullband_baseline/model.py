@@ -14,11 +14,13 @@ import os
 import torch
 
 from .. import _lib
-from ..model.base_model import BaseModel, TrainStep
+from ..model.base_model import BaseModel, SpectrogramEnhance, TrainStep
 from ..model.module.sequence_model import SequenceModel
 
 
-class Model(BaseModel):
+class Model(SpectrogramEnhance, BaseModel):
+    # fused wav -> wav call (enhance / enhance_pcm): stft -> model -> mask + istft [-> int16] in one library call
+    ENHANCE_ENTRY_POINTS = ("fsn_fullband_enhance_workspace_bytes", "fsn_fullband_enhance")
     # training step (fullband_baseline/trainer.py:32-71): fsn_fullband_train_forward keeps the activations,
     # fsn_fullband_train_backward runs BPTT
     TRAIN_ENTRY_POINTS = ("fsn_fullband_train_workspace_bytes", "fsn_fullband_train_forward", "fsn_fullband_train_backward")
@@ -51,6 +53,9 @@ class Model(BaseModel):
 
     def _infer_desc(self):
         return self._desc(_lib.PREC[self._resolve_precision()])
+
+    def _enhance_args(self, device):
+        return self._infer_desc(), self._weight_ptrs()
 
     def _train_desc(self):
         return self._desc(_lib.PREC[self._resolve_train_precision()])
@@ -98,48 +103,3 @@ class Model(BaseModel):
             _lib.check(lib.fsn_fullband_forward(C.byref(d), layers, fc_w, fc_b, x.data_ptr(), batch_size, num_frames,
                                                 out.data_ptr(), ws.data_ptr(), n, _lib.stream_ptr(x.device)))
         return out
-
-    def _enhance_call(self, noisy, n_fft, hop_length, win_length, lengths, crm, pcm, gain):
-        """One fsn_fullband_enhance call: noisy [B,L] -> enhanced [B,L]; clip b is row b's first lengths[b] samples (all
-        L when lengths is None), its outputs 0 past them."""
-        B, L = noisy.shape
-        lens = None if lengths is None else _lib.lengths_table(lengths, B, L)
-        x = _lib.require_cuda(noisy, "noisy")
-        lib = _lib.load()
-        with torch.cuda.device(x.device):
-            d = self._infer_desc()
-            layers, fc_w, fc_b = self._weight_ptrs()
-            n = _lib.check_workspace(lib.fsn_fullband_enhance_workspace_bytes(C.byref(d), B, L, n_fft, hop_length))
-            ws = torch.empty(n, dtype=torch.uint8, device=x.device)
-            out = torch.empty(B, L, dtype=torch.float32, device=x.device)
-            _lib.check(lib.fsn_fullband_enhance(C.byref(d), layers, fc_w, fc_b, x.data_ptr(),
-                                                None if lens is None else lens.ctypes.data, B, L, n_fft, hop_length,
-                                                win_length, out.data_ptr(), _lib.ptr(crm), _lib.ptr(pcm), float(gain),
-                                                ws.data_ptr(), n, _lib.stream_ptr(x.device)))
-        return out
-
-    @torch.no_grad()
-    def enhance(self, noisy, n_fft=512, hop_length=256, win_length=512, return_crm=False, lengths=None):
-        """Fused wav -> wav path of Inferencer.full_band_crm_mask (recipes/.../inferencer.py:130-145), batched over
-        independent clips in one library call (fsn_fullband_enhance): noisy [B,L] -> enhanced [B,L].
-
-        ``lengths`` (B ints, or a CPU integer tensor; max must be L; power-of-two n_fft): clips of different lengths in
-        one call.  Clip b is ``noisy[b, :lengths[b]]``; the rest of the row is never read.  Its outputs equal the call on
-        that clip alone, bit for bit; ``enhanced[b, lengths[b]:]`` and the cRM frames ``t >= 1 + lengths[b] //
-        hop_length`` are 0.  ``return_crm`` additionally returns the [B,2,F,T_max] model output."""
-        assert noisy.dim() == 2, "noisy must be [B, L]"
-        B, L = noisy.shape
-        crm = torch.empty(B, 2, n_fft // 2 + 1, 1 + L // hop_length, dtype=torch.float32,
-                          device=noisy.device) if return_crm else None
-        out = self._enhance_call(noisy, n_fft, hop_length, win_length, lengths, crm, None, 0.0)
-        return (out, crm) if return_crm else out
-
-    @torch.no_grad()
-    def enhance_pcm(self, noisy, n_fft=512, hop_length=256, win_length=512, gain=0.8 * 32767.0, lengths=None):
-        """``enhance`` plus the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:
-        181-182) in the same call, the per-clip max|y| reduced in the iSTFT epilogue: noisy [B,L] -> (enhanced float32
-        [B,L], pcm int16 [B,L]).  ``lengths``: as in ``enhance``; each clip is scaled by the peak of its own samples and
-        its pcm row is 0 past them."""
-        assert noisy.dim() == 2, "noisy must be [B, L]"
-        pcm = torch.empty(noisy.shape, dtype=torch.int16, device=noisy.device)
-        return self._enhance_call(noisy, n_fft, hop_length, win_length, lengths, None, pcm, gain), pcm

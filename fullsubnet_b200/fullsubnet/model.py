@@ -4,7 +4,8 @@ Same constructor kwargs, same 20 ``state_dict`` entries, same ``forward`` contra
 (``noisy_mag [B,1,F,T] -> cRM [B,2,F',T]``, incl. drop_band when B > 1), but the whole forward
 is one call into libfsn_b200 (``fsn_model_forward``): look-ahead pad, both laplace norms (second
 in closed form), full-band 2xLSTM + Linear + ReLU, sub-band unfold (never materialised),
-sub-band 2xLSTM + Linear, output re-layout."""
+sub-band 2xLSTM + Linear, output re-layout.  ``enhance`` / ``enhance_pcm`` run the wav -> wav path of
+``Inferencer.full_band_crm_mask`` for a batch of clips, of equal or different lengths, in one call (``fsn_enhance``)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -13,11 +14,13 @@ import os
 import torch
 
 from .. import _lib
-from ..model.base_model import BaseModel, TrainStep
+from ..model.base_model import BaseModel, SpectrogramEnhance, TrainStep
 from ..model.module.sequence_model import SequenceModel
 
 
-class Model(BaseModel):
+class Model(SpectrogramEnhance, BaseModel):
+    # fused wav -> wav call (enhance / enhance_pcm): stft -> model -> mask + istft [-> int16] in one library call
+    ENHANCE_ENTRY_POINTS = ("fsn_enhance_workspace_bytes", "fsn_enhance")
     # training step (trainer.py:56-63): fsn_train_forward keeps the activations, fsn_train_backward runs BPTT
     TRAIN_ENTRY_POINTS = ("fsn_train_workspace_bytes", "fsn_train_forward", "fsn_train_backward")
     TRAIN_TF32_STACKS = ("fb_model", "sb_model")
@@ -109,6 +112,10 @@ class Model(BaseModel):
         packed = self._packed_sb(desc, sb_w, device) if prec in ("f16_tc", "f16x3_tc") else None
         return desc, fb_w, sb_w, packed
 
+    def _enhance_args(self, device):
+        desc, fb_w, sb_w, packed = self._prepare(device, 1)
+        return desc, (C.byref(fb_w), C.byref(sb_w), _lib.ptr(packed))
+
     # ---------------------------------------------------------------- reference API
     def forward(self, noisy_mag):
         """noisy_mag [B,1,F,T] -> [B,2,F,T]  (or [B,2,F//G,T], batch order 0,2,4,..,1,3,5,.. when B>1, G>1)."""
@@ -125,95 +132,10 @@ class Model(BaseModel):
             desc, fb_w, sb_w, packed = self._prepare(device, int(self.num_groups_in_drop_band))
             G = desc.num_groups_in_drop_band if batch_size > 1 and desc.num_groups_in_drop_band > 1 else 1
             f_out = num_freqs // G if G > 1 else num_freqs
-            ws_bytes = lib.fsn_model_workspace_bytes(C.byref(desc), batch_size, num_frames)
-            if ws_bytes == 0:
-                _lib.check_workspace(ws_bytes)
+            ws_bytes = _lib.check_workspace(lib.fsn_model_workspace_bytes(C.byref(desc), batch_size, num_frames))
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             out = torch.empty(batch_size, 2, f_out, num_frames, dtype=torch.float32, device=device)
             _lib.check(lib.fsn_model_forward(C.byref(desc), C.byref(fb_w), C.byref(sb_w), _lib.ptr(packed),
                                              x.data_ptr(), batch_size, num_frames, out.data_ptr(), ws.data_ptr(),
                                              ws_bytes, _lib.stream_ptr(device)))
         return out
-
-    @staticmethod
-    def _lengths_table(lengths, B, L):
-        """Per-clip lengths (sequence of B ints or a CPU integer tensor) -> contiguous int32 host array."""
-        return _lib.lengths_table(lengths, B, L)
-
-    def _enhance_varlen(self, x, lens, n_fft, hop_length, win_length, crm, pcm, gain):
-        """One fsn_enhance_varlen call: clip b is row b's first lens[b] samples; out [B,L] is 0 past them."""
-        B, L = x.shape
-        device = x.device
-        lib = _lib.load()
-        with torch.cuda.device(device):
-            desc, fb_w, sb_w, packed = self._prepare(device, 1)
-            ws_bytes = _lib.check_workspace(lib.fsn_enhance_varlen_workspace_bytes(C.byref(desc), B, L, n_fft, hop_length))
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            out = torch.empty(B, L, dtype=torch.float32, device=device)
-            _lib.check(lib.fsn_enhance_varlen(C.byref(desc), C.byref(fb_w), C.byref(sb_w), _lib.ptr(packed), x.data_ptr(),
-                                              lens.ctypes.data, B, L, n_fft, hop_length, win_length, out.data_ptr(),
-                                              _lib.ptr(crm), _lib.ptr(pcm), float(gain), ws.data_ptr(), ws_bytes,
-                                              _lib.stream_ptr(device)))
-        return out
-
-    @torch.no_grad()
-    def enhance(self, noisy, n_fft=512, hop_length=256, win_length=512, return_crm=False, lengths=None):
-        """Fused wav -> wav path of Inferencer.full_band_crm_mask (recipes/.../inferencer.py:130-145),
-        batched over independent clips: noisy [B,L] -> enhanced [B,L].
-
-        ``lengths`` (B ints, or a CPU integer tensor; max must be L): clips of different lengths in one call
-        (fsn_enhance_varlen).  Clip b is ``noisy[b, :lengths[b]]``; the rest of the row is never read.  Its outputs
-        equal the call on that clip alone, bit for bit; ``enhanced[b, lengths[b]:]`` and the cRM frames
-        ``t >= 1 + lengths[b] // hop_length`` are 0."""
-        assert noisy.dim() == 2, "noisy must be [B, L]"
-        lens = None if lengths is None else self._lengths_table(lengths, *noisy.shape)
-        x = _lib.require_cuda(noisy, "noisy")
-        B, L = x.shape
-        device = x.device
-        if lens is not None:
-            crm = torch.empty(B, 2, n_fft // 2 + 1, 1 + L // hop_length, dtype=torch.float32,
-                              device=device) if return_crm else None
-            out = self._enhance_varlen(x, lens, n_fft, hop_length, win_length, crm, None, 0.0)
-            return (out, crm) if return_crm else out
-        lib = _lib.load()
-        with torch.cuda.device(device):
-            desc, fb_w, sb_w, packed = self._prepare(device, 1)
-            ws_bytes = lib.fsn_enhance_workspace_bytes(C.byref(desc), B, L, n_fft, hop_length)
-            if ws_bytes == 0:
-                _lib.check_workspace(ws_bytes)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            out = torch.empty(B, L, dtype=torch.float32, device=device)
-            crm = torch.empty(B, 2, n_fft // 2 + 1, 1 + L // hop_length, dtype=torch.float32,
-                              device=device) if return_crm else None
-            _lib.check(lib.fsn_enhance(C.byref(desc), C.byref(fb_w), C.byref(sb_w), _lib.ptr(packed), x.data_ptr(),
-                                       B, L, n_fft, hop_length, win_length, out.data_ptr(), _lib.ptr(crm),
-                                       ws.data_ptr(), ws_bytes, _lib.stream_ptr(device)))
-        return (out, crm) if return_crm else out
-
-    @torch.no_grad()
-    def enhance_pcm(self, noisy, n_fft=512, hop_length=256, win_length=512, gain=0.8 * 32767.0, lengths=None):
-        """``enhance`` plus the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:
-        181-182) in the same library call (fsn_enhance_pcm: per-clip max|y| reduced in the iSTFT epilogue):
-        noisy [B,L] -> (enhanced float32 [B,L], pcm int16 [B,L]).  ``lengths``: as in ``enhance``; each clip is
-        scaled by the peak of its own samples and its pcm row is 0 past them."""
-        assert noisy.dim() == 2, "noisy must be [B, L]"
-        lens = None if lengths is None else self._lengths_table(lengths, *noisy.shape)
-        x = _lib.require_cuda(noisy, "noisy")
-        B, L = x.shape
-        device = x.device
-        if lens is not None:
-            pcm = torch.empty(B, L, dtype=torch.int16, device=device)
-            return self._enhance_varlen(x, lens, n_fft, hop_length, win_length, None, pcm, gain), pcm
-        lib = _lib.load()
-        with torch.cuda.device(device):
-            desc, fb_w, sb_w, packed = self._prepare(device, 1)
-            ws_bytes = lib.fsn_enhance_workspace_bytes(C.byref(desc), B, L, n_fft, hop_length)
-            if ws_bytes == 0:
-                _lib.check_workspace(ws_bytes)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            out = torch.empty(B, L, dtype=torch.float32, device=device)
-            pcm = torch.empty(B, L, dtype=torch.int16, device=device)
-            _lib.check(lib.fsn_enhance_pcm(C.byref(desc), C.byref(fb_w), C.byref(sb_w), _lib.ptr(packed), x.data_ptr(),
-                                           B, L, n_fft, hop_length, win_length, out.data_ptr(), pcm.data_ptr(),
-                                           float(gain), ws.data_ptr(), ws_bytes, _lib.stream_ptr(device)))
-        return out, pcm

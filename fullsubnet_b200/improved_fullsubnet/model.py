@@ -49,6 +49,8 @@ class Model(BaseModel):
     # waveform in, waveform out with the model's own STFT: the Inferencer calls enhance / enhance_pcm instead of computing
     # a magnitude spectrogram for it
     WAVEFORM_INPUT = True
+    # fused wav -> wav call (enhance / enhance_pcm); its STFT geometry is in the descriptor
+    ENHANCE_ENTRY_POINTS = ("fsn_improved_enhance_workspace_bytes", "fsn_improved_enhance")
 
     def __init__(self, n_fft=512, hop_length=128, win_length=512, fdrc=0.5, num_freqs=257, freq_cutoffs=[20, 80],
                  sb_num_center_freqs=[1, 4, 8], sb_num_neighbor_freqs=[15, 15, 15], fb_num_center_freqs=[1, 4, 8],
@@ -86,6 +88,11 @@ class Model(BaseModel):
 
     def _structs(self):
         return self._desc(self._resolve_precision()), self._weights()
+
+    def _enhance_args(self, device):
+        self._check_sections()
+        d, w = self._structs()
+        return d, (C.byref(w),)
 
     def _desc(self, precision: str) -> "_lib.ImprovedDesc":
         sb = self.sb_model
@@ -160,9 +167,7 @@ class Model(BaseModel):
         lib = _lib.load()
         with torch.cuda.device(x.device):
             d, w = self._structs()
-            n = lib.fsn_improved_workspace_bytes(C.byref(d), B, L)
-            if n == 0:
-                _lib.check_workspace(n)
+            n = _lib.check_workspace(lib.fsn_improved_workspace_bytes(C.byref(d), B, L))
             ws = torch.empty(n, dtype=torch.uint8, device=x.device)
             out = torch.empty(B, 1, L, dtype=torch.float32, device=x.device)
             crm = torch.empty(B, 2, self.num_freqs, 1 + L // self.hop_length, dtype=torch.float32,
@@ -170,24 +175,6 @@ class Model(BaseModel):
             _lib.check(lib.fsn_improved_forward(C.byref(d), C.byref(w), x.data_ptr(), B, L, out.data_ptr(),
                                                 _lib.ptr(crm), ws.data_ptr(), n, _lib.stream_ptr(x.device)))
         return (out, crm) if return_crm else out
-
-    def _enhance_call(self, y, lengths, crm, pcm, gain):
-        """One fsn_improved_enhance call: y [B,L] (CUDA) -> enhanced [B,L]; clip b is row b's first lengths[b] samples
-        (all L when lengths is None), its outputs 0 past them."""
-        B, L = y.shape
-        lens = None if lengths is None else _lib.lengths_table(lengths, B, L)
-        x = _lib.require_cuda(y, "y")
-        self._check_sections()
-        lib = _lib.load()
-        with torch.cuda.device(x.device):
-            d, w = self._structs()
-            n = _lib.check_workspace(lib.fsn_improved_enhance_workspace_bytes(C.byref(d), B, L))
-            ws = torch.empty(n, dtype=torch.uint8, device=x.device)
-            out = torch.empty(B, L, dtype=torch.float32, device=x.device)
-            _lib.check(lib.fsn_improved_enhance(C.byref(d), C.byref(w), x.data_ptr(), None if lens is None else lens.ctypes.data,
-                                                B, L, out.data_ptr(), _lib.ptr(crm), _lib.ptr(pcm), float(gain),
-                                                ws.data_ptr(), n, _lib.stream_ptr(x.device)))
-        return out
 
     @torch.no_grad()
     def enhance(self, y, lengths=None, return_crm: bool = False):
@@ -197,10 +184,7 @@ class Model(BaseModel):
         clip alone, bit for bit; ``enhanced[b, lengths[b]:]`` and the cRM frames ``t >= 1 + lengths[b] // hop_length``
         are 0.  ``return_crm`` additionally returns the [B,2,F,T_max] mask."""
         assert y.dim() == 2, "y must be [B, L]"
-        B, L = y.shape
-        crm = torch.empty(B, 2, self.num_freqs, 1 + L // self.hop_length, dtype=torch.float32,
-                          device=y.device) if return_crm else None
-        out = self._enhance_call(y, lengths, crm, None, 0.0)
+        out, crm, _ = self._enhance_call(y, lengths, return_crm, None)
         return (out, crm) if return_crm else out
 
     @torch.no_grad()
@@ -210,5 +194,5 @@ class Model(BaseModel):
         [B,L], pcm int16 [B,L]).  ``lengths``: as in ``enhance``; each clip is scaled by the peak of its own samples
         and its pcm row is 0 past them."""
         assert y.dim() == 2, "y must be [B, L]"
-        pcm = torch.empty(y.shape, dtype=torch.int16, device=y.device)
-        return self._enhance_call(y, lengths, None, pcm, gain), pcm
+        out, _, pcm = self._enhance_call(y, lengths, False, gain)
+        return out, pcm

@@ -52,6 +52,12 @@ def takes_waveform(model) -> bool:
     return bool(getattr(type(model), "WAVEFORM_INPUT", False))
 
 
+def has_fused_call(model) -> bool:
+    """Whether ``model`` runs wav -> wav (STFT, model, mask + iSTFT, int16) in one library call with per-clip lengths
+    (``enhance`` / ``enhance_pcm``): the models that set ENHANCE_ENTRY_POINTS."""
+    return bool(getattr(type(model), "ENHANCE_ENTRY_POINTS", ()))
+
+
 class Inferencer:
     def __init__(self, config: Optional[dict] = None, checkpoint_path=None, output_dir=None, model=None,
                  device=None):
@@ -111,24 +117,26 @@ class Inferencer:
         fullsubnet and fullband_baseline with a power-of-two n_fft."""
         if takes_waveform(self.model):
             return True
-        return hasattr(self.model, "enhance") and self.n_fft & (self.n_fft - 1) == 0
+        return has_fused_call(self.model) and self.n_fft & (self.n_fft - 1) == 0
+
+    def _stft_args(self) -> tuple:
+        """The STFT geometry a fused call takes: none for a model with its own (improved_fullsubnet)."""
+        return () if takes_waveform(self.model) else (self.n_fft, self.hop_length, self.win_length)
 
     def _check_lengths(self, lengths) -> None:
-        if lengths is not None and not takes_waveform(self.model) and not hasattr(self.model, "enhance"):
+        if lengths is not None and not has_fused_call(self.model):
             raise NotImplementedError(f"{type(self.model).__module__}: per-clip lengths are built for fullsubnet, "
                                       "improved_fullsubnet and fullband_baseline only")
 
     @torch.no_grad()
     def enhance_batch(self, noisy: torch.Tensor, lengths=None) -> torch.Tensor:
-        """The same path for B independent clips in ONE library call (fsn_enhance, fsn_fullband_enhance): pinned/host or
-        device ``noisy`` [B,L] -> device tensor [B,L].  Equivalent to looping full_band_crm_mask over the clips.
+        """The same path for B independent clips in ONE library call (the model's fused call): pinned/host or device
+        ``noisy`` [B,L] -> device tensor [B,L].  Equivalent to looping full_band_crm_mask over the clips.
         ``lengths`` (models with a fused call): clip b is ``noisy[b, :lengths[b]]``, its row 0 past it."""
         self._check_lengths(lengths)
         x = noisy.to(self.device, non_blocking=True)
-        if takes_waveform(self.model):  # improved_fullsubnet: one library call with the model's own STFT
-            return self.model.enhance(x, lengths=lengths)
-        if hasattr(self.model, "enhance"):  # fullsubnet, fullband_baseline: one fused library call
-            return self.model.enhance(x, self.n_fft, self.hop_length, self.win_length, lengths=lengths)
+        if has_fused_call(self.model):
+            return self.model.enhance(x, *self._stft_args(), lengths=lengths)
         # other models (fast_fullsubnet): same flow, three library calls (stft -> model -> mask + istft)
         import ctypes as C  # noqa: F401
         from . import _lib
@@ -154,13 +162,11 @@ class Inferencer:
         ``enhance_batch``; each clip is scaled by its own peak."""
         from . import _lib
         self._check_lengths(lengths)
-        if takes_waveform(self.model):
+        if has_fused_call(self.model):  # peak in the iSTFT epilogue, one scaling pass
             x = noisy.to(self.device, non_blocking=True)
-            return self.model.enhance_pcm(x, gain=0.8 * float(np.iinfo(np.int16).max), lengths=lengths)[1]
-        if lengths is not None or (hasattr(self.model, "enhance_pcm") and self.n_fft & (self.n_fft - 1) == 0):
-            x = noisy.to(self.device, non_blocking=True)  # fused: peak in the iSTFT epilogue, one scaling pass
-            return self.model.enhance_pcm(x, self.n_fft, self.hop_length, self.win_length,
-                                          gain=0.8 * float(np.iinfo(np.int16).max), lengths=lengths)[1]
+            return self.model.enhance_pcm(x, *self._stft_args(), gain=0.8 * float(np.iinfo(np.int16).max),
+                                          lengths=lengths)[1]
+        # models without a fused call (fast_fullsubnet): enhance_batch, then the two-pass int16 kernel
         enhanced = self.enhance_batch(noisy)
         B, L = enhanced.shape
         pcm = torch.empty(B, L, dtype=torch.int16, device=enhanced.device)
@@ -231,14 +237,14 @@ class Inferencer:
     @torch.no_grad()
     def enhance_files(self, paths, output_dir, batch_size: int = 64, sr=None, max_padding: float = 0.0):
         """Batched form of the host loop of base_inferencer.py:163-195: ``plan_batches`` groups the files, each batch
-        goes through ONE fused library call (pinned staging buffer -> H2D -> fsn_enhance_pcm -> int16 D2H), and
+        goes through ONE fused library call (pinned staging buffer -> H2D -> the model's enhance_pcm -> int16 D2H), and
         ``<output_dir>/<stem>.wav`` is written as 16-bit PCM like the reference.  Returns the written paths.
 
         ``max_padding == 0`` (default): batches of equal-length clips only.  ``max_padding > 0`` (improved_fullsubnet,
         and fullsubnet and fullband_baseline with a power-of-two n_fft; other models keep equal-length batches): clips of
         different lengths share a batch, padded to its longest clip by at most that fraction of the batch's samples,
-        through fsn_enhance_varlen / fsn_improved_enhance / fsn_fullband_enhance.  Every file is bit-identical either way: each clip is bounded by its
-        own length in the length-dependent kernels."""
+        through fsn_enhance / fsn_improved_enhance / fsn_fullband_enhance.  Every file is bit-identical either way: each
+        clip is bounded by its own length in the length-dependent kernels."""
         from pathlib import Path
         sr = int(sr or self.sr)
         out_dir = Path(output_dir)

@@ -1,6 +1,7 @@
 """Host-side pieces of audio_zen/model/base_model.py that the drop-in Model needs:
 norm_wrapper (:356-372) name checking and weight_init (:374-439, CPU-side initialisation); plus the training step
-that fullsubnet, fast_fullsubnet and fullband_baseline share (autograd Function, precision choice, flat gradients)."""
+that fullsubnet, fast_fullsubnet and fullband_baseline share (autograd Function, precision choice, flat gradients),
+and the fused wav -> wav call of the models that have one."""
 from __future__ import annotations
 
 import ctypes as C
@@ -27,9 +28,7 @@ class TrainStep(torch.autograd.Function):
             desc = model._train_desc()
             weights = model._train_weights()
             dims, out_shape = model._train_io(x, desc)
-            n = query(C.byref(desc), *dims)
-            if n == 0:
-                _lib.check_workspace(n)
+            n = _lib.check_workspace(query(C.byref(desc), *dims))
             ws = torch.empty(n, dtype=torch.uint8, device=device)
             out = torch.empty(out_shape, dtype=torch.float32, device=device)
             _lib.check(fwd(C.byref(desc), *weights, x.data_ptr(), *dims, out.data_ptr(), ws.data_ptr(), n,
@@ -123,6 +122,37 @@ class BaseModel(nn.Module):
     def _train_out_shape(self, desc, B, F, T):
         return (B, 2, F, T)
 
+    # ---------------------------------------------------------------- fused wav -> wav call (_enhance_call)
+    # Each model with one sets ENHANCE_ENTRY_POINTS (library workspace query, call) and implements _enhance_args(device):
+    # the descriptor and the ctypes arguments of the weights.
+    ENHANCE_ENTRY_POINTS: tuple = ()
+
+    def _enhance_call(self, noisy, *args):
+        """One fused library call: noisy [B,L] -> (enhanced [B,L], crm [B,2,F,T] or None, pcm int16 [B,L] or None).
+        ``args`` = (*stft, lengths, return_crm, gain): ``stft`` is (n_fft, hop_length, win_length) for the models that
+        take the Inferencer's STFT geometry and empty for one whose descriptor holds its own; clip b is row b's first
+        lengths[b] samples (all L when lengths is None), its outputs 0 past them; ``gain`` None: no int16 output."""
+        *stft, lengths, return_crm, gain = args
+        B, L = noisy.shape
+        lens = None if lengths is None else _lib.lengths_table(lengths, B, L)
+        x = _lib.require_cuda(noisy, "noisy")
+        n_fft, hop = stft[:2] if stft else (self.n_fft, self.hop_length)
+        F, T = n_fft // 2 + 1, 1 + L // hop
+        device = x.device
+        lib = _lib.load()
+        query, call = (getattr(lib, name) for name in self.ENHANCE_ENTRY_POINTS)
+        with torch.cuda.device(device):
+            desc, weights = self._enhance_args(device)
+            n = _lib.check_workspace(query(C.byref(desc), B, L, *stft[:2]))
+            crm = torch.empty(B, 2, F, T, dtype=torch.float32, device=device) if return_crm else None
+            pcm = None if gain is None else torch.empty(B, L, dtype=torch.int16, device=device)
+            ws = torch.empty(n, dtype=torch.uint8, device=device)
+            out = torch.empty(B, L, dtype=torch.float32, device=device)
+            _lib.check(call(C.byref(desc), *weights, x.data_ptr(), None if lens is None else lens.ctypes.data, B, L,
+                            *stft, out.data_ptr(), _lib.ptr(crm), _lib.ptr(pcm), 0.0 if gain is None else float(gain),
+                            ws.data_ptr(), n, _lib.stream_ptr(device)))
+        return out, crm, pcm
+
     def _version_key(self):
         return tuple((p.data_ptr(), p._version) for p in self.parameters())
 
@@ -157,3 +187,30 @@ class BaseModel(nn.Module):
             views[k] = flat[off:off + p.numel()].view_as(p)
             off += p.numel()
         return flat, views
+
+
+class SpectrogramEnhance:
+    """enhance / enhance_pcm of the models that take the Inferencer's STFT geometry (fullsubnet, fullband_baseline)."""
+
+    @torch.no_grad()
+    def enhance(self, noisy, n_fft=512, hop_length=256, win_length=512, return_crm=False, lengths=None):
+        """Fused wav -> wav path of Inferencer.full_band_crm_mask (recipes/.../inferencer.py:130-145), batched over
+        independent clips in one library call: noisy [B,L] -> enhanced [B,L].
+
+        ``lengths`` (B ints, or a CPU integer tensor; max must be L; power-of-two n_fft): clips of different lengths in
+        one call.  Clip b is ``noisy[b, :lengths[b]]``; the rest of the row is never read.  Its outputs equal the call on
+        that clip alone, bit for bit; ``enhanced[b, lengths[b]:]`` and the cRM frames ``t >= 1 + lengths[b] //
+        hop_length`` are 0.  ``return_crm`` additionally returns the [B,2,F,T_max] model output."""
+        assert noisy.dim() == 2, "noisy must be [B, L]"
+        out, crm, _ = self._enhance_call(noisy, n_fft, hop_length, win_length, lengths, return_crm, None)
+        return (out, crm) if return_crm else out
+
+    @torch.no_grad()
+    def enhance_pcm(self, noisy, n_fft=512, hop_length=256, win_length=512, gain=0.8 * 32767.0, lengths=None):
+        """``enhance`` plus the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:
+        181-182) in the same call, the per-clip max|y| reduced in the iSTFT epilogue: noisy [B,L] -> (enhanced float32
+        [B,L], pcm int16 [B,L]).  ``lengths``: as in ``enhance``; each clip is scaled by the peak of its own samples and
+        its pcm row is 0 past them."""
+        assert noisy.dim() == 2, "noisy must be [B, L]"
+        out, _, pcm = self._enhance_call(noisy, n_fft, hop_length, win_length, lengths, False, gain)
+        return out, pcm

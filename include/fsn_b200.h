@@ -150,38 +150,28 @@ int fsn_model_forward(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
                       const void* sb_packed, const float* noisy_mag, int B, int T, float* crm,
                       void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
-/* recipes/dns_interspeech_2020/inferencer.py:130-145  Inferencer.full_band_crm_mask, batched
- * over independent clips (drop_band off): wav [B,L] -> enhanced [B,L]; crm_out (optional,
- * [B,2,F,T]) receives the mask.  One call = stft -> model -> decompress/mask -> istft. */
-size_t fsn_enhance_workspace_bytes(const fsn_model_desc* d, int B, int L, int n_fft, int hop);
-int fsn_enhance(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                const void* sb_packed, const float* wav, int B, int L, int n_fft, int hop, int win_length,
-                float* enhanced, float* crm_out, void* workspace, size_t workspace_bytes,
-                fsn_stream_t stream);
-/* The same call followed by the int16 scaling of the reference host loop (audio_zen/inferencer/base_inferencer.py:
- * 181-182: int16(gain * y / max|y|), gain = 0.8 * 32767): max|y| per clip is reduced in the iSTFT epilogue, so the
- * float waveform is read once more and only 2 bytes per sample have to go back to the host.  `enhanced` (float,
- * [B,L]) is still written; pcm [B,L] int16. */
-int fsn_enhance_pcm(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                    const void* sb_packed, const float* wav, int B, int L, int n_fft, int hop, int win_length,
-                    float* enhanced, int16_t* pcm, float gain, void* workspace, size_t workspace_bytes,
-                    fsn_stream_t stream);
-/* Clips of different lengths in one call.  Row b of wav [B, L_max] holds clip b's lengths[b] samples; samples at index
- * >= lengths[b] are never read.  lengths: HOST int32 [B], n_fft/2 < lengths[b] <= L_max and max(lengths) == L_max
- * (else FSN_ERR_SHAPE naming the clip); it is copied into the workspace through kernel parameters during the call and
- * not retained, so it may be pageable and may be reused as soon as the call returns.  Outputs, T_max = 1 + L_max/hop:
- *   enhanced [B, L_max]           0 past lengths[b]
- *   crm_out  [B, 2, F, T_max]     nullable; 0 for frames t >= T_b = 1 + lengths[b]/hop
+/* recipes/dns_interspeech_2020/inferencer.py:130-145  Inferencer.full_band_crm_mask, batched over independent clips
+ * (drop_band off), with the int16 output of the reference host loop: one call = stft -> model -> decompress/mask ->
+ * istft [-> int16].  ABI version 101 changed this entry point: it now takes the argument list of fsn_fullband_enhance
+ * (lengths, pcm and gain), and version 100's separate int16 and per-clip-length entry points are gone.  Row b of wav
+ * [B, L_max] holds clip b's lengths[b] samples; samples at index >= lengths[b] are never read.  lengths: HOST int32 [B],
+ * nullable (= every clip L_max samples), n_fft/2 < lengths[b] <= L_max and max(lengths) == L_max (else FSN_ERR_SHAPE
+ * naming the clip); copied into the workspace through kernel parameters during the call and not retained, so it may be
+ * pageable and may be reused as soon as the call returns.  Outputs, T_max = 1 + L_max/hop:
+ *   enhanced [B, L_max]           required (NULL: FSN_ERR_SHAPE); 0 past lengths[b]
+ *   crm_out  [B, 2, F, T_max]     nullable; the model's output, 0 for frames t >= T_b = 1 + lengths[b]/hop
  *   pcm      [B, L_max] int16     nullable; int16(gain * y / max|y|) over the clip's own samples, 0 past lengths[b]
- * Every clip's outputs are bit-identical to fsn_enhance / fsn_enhance_pcm on that clip alone with L = lengths[b]: the
+ *                                 (audio_zen/inferencer/base_inferencer.py:181-182, gain = 0.8 * 32767; max|y| per
+ *                                 clip is reduced in the iSTFT epilogue, so only 2 bytes per sample go back to the host)
+ * With lengths, every clip's outputs are bit-identical to a null-lengths call on that clip alone with L = lengths[b]: the
  * recurrent stages are causal, so they run over T_max + look_ahead steps for every clip, and only the STFT, the offline
- * norms, the iSTFT and the int16 scaling are bounded per clip.  Same precisions, cells and norms as fsn_enhance
- * (drop_band off); n_fft must be a power of two (else FSN_ERR_UNSUPPORTED).  Never synchronises the host. */
-size_t fsn_enhance_varlen_workspace_bytes(const fsn_model_desc* d, int B, int L_max, int n_fft, int hop);
-int fsn_enhance_varlen(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                       const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L_max, int n_fft,
-                       int hop, int win_length, float* enhanced, float* crm_out, int16_t* pcm, float gain,
-                       void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+ * norms, the iSTFT and the int16 scaling are bounded per clip; n_fft must then be a power of two (else
+ * FSN_ERR_UNSUPPORTED).  Never allocates, never synchronises the host. */
+size_t fsn_enhance_workspace_bytes(const fsn_model_desc* d, int B, int L_max, int n_fft, int hop);
+int fsn_enhance(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                const void* sb_packed, const float* wav, const int32_t* lengths, int B, int L_max, int n_fft, int hop,
+                int win_length, float* enhanced, float* crm_out, int16_t* pcm, float gain, void* workspace,
+                size_t workspace_bytes, fsn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * recipes/dns_interspeech_2020/fast_fullsubnet/model.py:11-202  Model (BASELINE config 4, SURVEY 8a row A13)
@@ -267,7 +257,7 @@ int fsn_improved_forward(const fsn_improved_desc* d, const fsn_improved_weights*
  * (= every clip L_max samples), n_fft/2 < lengths[b] <= L_max and max(lengths) == L_max (else FSN_ERR_SHAPE naming the
  * clip); copied into the workspace through kernel parameters during the call and not retained.  Outputs, T_max = 1 +
  * L_max/hop_length:
- *   enhanced [B, L_max]           0 past lengths[b]
+ *   enhanced [B, L_max]           required (NULL: FSN_ERR_SHAPE); 0 past lengths[b]
  *   crm_out  [B, 2, F, T_max]     nullable; Nyquist row 0, and 0 for frames t >= T_b = 1 + lengths[b]/hop_length
  *   pcm      [B, L_max] int16     nullable; int16(gain * y / max|y|) over the clip's own samples, 0 past lengths[b]
  * Every clip's outputs are bit-identical to fsn_improved_forward on that clip alone with L = lengths[b] (and pcm to
@@ -287,7 +277,7 @@ int fsn_improved_enhance(const fsn_improved_desc* d, const fsn_improved_weights*
 int fsn_set_profiling(int enable);
 float fsn_last_stage_ms(int stage);
 
-/* number of kernel launches issued by the last fsn_model_forward / fsn_enhance (/ _pcm / _varlen) on this thread
+/* number of kernel launches issued by the last fsn_model_forward / fsn_enhance on this thread
  * (bench.py reports it as gpu_launches) */
 int64_t fsn_last_launch_count(void);
 /* kernels launched by this library since it was loaded (never reset): difference two readings */
@@ -389,7 +379,7 @@ int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_layer* layer
  * >= lengths[b] are never read.  lengths: HOST int32 [B], nullable (= every clip L_max samples), n_fft/2 < lengths[b] <=
  * L_max and max(lengths) == L_max (else FSN_ERR_SHAPE naming the clip); copied into the workspace through kernel
  * parameters during the call and not retained.  n_fft / 2 + 1 must equal num_freqs.  Outputs, T_max = 1 + L_max/hop:
- *   enhanced [B, L_max]           0 past lengths[b]
+ *   enhanced [B, L_max]           required (NULL: FSN_ERR_SHAPE); 0 past lengths[b]
  *   crm_out  [B, 2, F, T_max]     nullable; the model's output, 0 for frames t >= T_b = 1 + lengths[b]/hop
  *   pcm      [B, L_max] int16     nullable; int16(gain * y / max|y|) over the clip's own samples, 0 past lengths[b]
  * With null lengths, enhanced equals fsn_stft -> fsn_fullband_forward -> fsn_istft bit for bit and crm_out equals

@@ -24,11 +24,11 @@ def _desc(prec="fp32", **kw):
     return _lib.FullbandDesc(**a)
 
 
-def _call(lib, d, lengths, L_max, n_fft=512):
+def _call(lib, d, lengths, L_max, n_fft=512, enhanced=None):
     arr = None if lengths is None else (C.c_int32 * len(lengths))(*lengths)
     B = 2 if lengths is None else len(lengths)
-    return lib.fsn_fullband_enhance(C.byref(d), None, None, None, None, arr, B, L_max, n_fft, n_fft // 2, n_fft, None, None,
-                                    None, 1.0, None, 0, None)
+    return lib.fsn_fullband_enhance(C.byref(d), None, None, None, None, arr, B, L_max, n_fft, n_fft // 2, n_fft, enhanced,
+                                    None, None, 1.0, None, 0, None)
 
 
 def test_fbb_workspace_queries_need_no_gpu():
@@ -52,7 +52,7 @@ def test_fbb_workspace_queries_need_no_gpu():
     assert lib.fsn_last_error_code() == _lib.FSN_ERR_SHAPE
 
 
-def test_fbb_enhance_rejects_bad_arguments_before_any_cuda_call():
+def test_fbb_enhance_checks_arguments_before_any_cuda_call():
     """No workspace, no weights, no device: every one of these fails on its argument check."""
     from fullsubnet_b200 import _lib
     lib = _lib.load()
@@ -63,13 +63,14 @@ def test_fbb_enhance_rejects_bad_arguments_before_any_cuda_call():
     assert b"clip 1" in lib.fsn_last_error()
     assert _call(lib, d, [15000, 257, 3000], 16000) == _lib.FSN_ERR_SHAPE  # max(lengths) != L_max
     assert b"15000" in lib.fsn_last_error()
-    # valid lengths reach the workspace check, the last one before the first launch
-    assert _call(lib, d, [16000, 257, 3000], 16000) == _lib.FSN_ERR_WORKSPACE
-    assert _call(lib, d, None, 16000) == _lib.FSN_ERR_WORKSPACE
+    # valid lengths reach the workspace check, the last one before the first launch (a stand-in output pointer, never
+    # written: the call returns before any CUDA call)
+    assert _call(lib, d, [16000, 257, 3000], 16000, enhanced=16) == _lib.FSN_ERR_WORKSPACE
+    assert _call(lib, d, None, 16000, enhanced=16) == _lib.FSN_ERR_WORKSPACE
     # per-clip lengths are built for the power-of-two transform; null lengths take every n_fft
     d960 = _desc(num_freqs=481)
     assert _call(lib, d960, [48000, 30000], 48000, 960) == _lib.FSN_ERR_UNSUPPORTED
-    assert _call(lib, d960, None, 48000, 960) == _lib.FSN_ERR_WORKSPACE
+    assert _call(lib, d960, None, 48000, 960, enhanced=16) == _lib.FSN_ERR_WORKSPACE
     # the tensor-core precisions and the GRU cell are refused, as by fsn_fullband_forward
     for prec in ("f16x3_tc", "f16_tc"):
         assert _call(lib, _desc(prec), None, 16000) == _lib.FSN_ERR_UNSUPPORTED

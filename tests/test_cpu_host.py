@@ -213,7 +213,7 @@ def test_write_wav_roundtrip(tmp_path):
         assert np.array_equal(np.frombuffer(f.readframes(1000), dtype="<i2"), pcm)
 
 
-def test_c_abi_argument_validation_without_gpu():
+def test_c_abi_arguments_are_validated_without_gpu():
     """Every entry point validates its arguments before touching CUDA: the error classes of the reference's asserts can
     be checked on the CPU box (no kernel is launched by these calls)."""
     import ctypes as C
@@ -238,8 +238,21 @@ def test_c_abi_argument_validation_without_gpu():
     assert lib.fsn_rir_convolve(None, None, None, 2, 100, 0, None, None) == _lib.FSN_ERR_SHAPE
     d = _lib.ModelDesc(num_freqs=257, look_ahead=2, fb_num_neighbors=0, sb_num_neighbors=15, fb_hidden=512, sb_hidden=384,
                        fb_activation=1, sb_activation=0, norm_type=0, num_groups_in_drop_band=1, precision=3, cell_type=0)
-    assert lib.fsn_enhance_pcm(C.byref(d), None, None, None, None, 2, 4000, 512, 256, 512, None, None, 1.0, None, 0, None) \
-        == _lib.FSN_ERR_SHAPE  # output buffers missing
+    # the float output is required, also when only the int16 one is wanted (a stand-in pcm pointer, never written: each
+    # call returns before any CUDA call)
+    assert lib.fsn_enhance(C.byref(d), None, None, None, None, None, 2, 4000, 512, 256, 512, None, None, 16, 1.0, None, 0,
+                           None) == _lib.FSN_ERR_SHAPE
+    assert b"enhanced" in lib.fsn_last_error()
+    fbb = _lib.FullbandDesc(num_freqs=257, hidden=512, num_layers=3, look_ahead=2, activation=0, norm_type=0, precision=0,
+                            cell_type=0)
+    assert lib.fsn_fullband_enhance(C.byref(fbb), None, None, None, None, None, 2, 4000, 512, 256, 512, None, None, 16, 1.0,
+                                    None, 0, None) == _lib.FSN_ERR_SHAPE
+    assert b"enhanced" in lib.fsn_last_error()
+    from fullsubnet_b200.improved_fullsubnet.model import Model as Improved
+    imp = Improved()._desc("fp32")
+    assert lib.fsn_improved_enhance(C.byref(imp), None, None, None, 2, 4000, None, None, 16, 1.0, None, 0, None) \
+        == _lib.FSN_ERR_SHAPE
+    assert b"enhanced" in lib.fsn_last_error()
     assert lib.fsn_enhance_workspace_bytes(C.byref(d), 2, 4000, 512, 256) > 0
     d.cell_type = 1  # GRU with a tensor-core precision
     assert lib.fsn_enhance_workspace_bytes(C.byref(d), 2, 4000, 512, 256) == 0

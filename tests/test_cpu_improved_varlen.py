@@ -13,9 +13,10 @@ def _model(args=None):
     return Model(**(args or IO.DEFAULT_IMPROVED_ARGS))
 
 
-def _call(lib, d, lengths, L_max):
+def _call(lib, d, lengths, L_max, enhanced=None):
     arr = (C.c_int32 * len(lengths))(*lengths)
-    return lib.fsn_improved_enhance(C.byref(d), None, None, arr, len(lengths), L_max, None, None, None, 1.0, None, 0, None)
+    return lib.fsn_improved_enhance(C.byref(d), None, None, arr, len(lengths), L_max, enhanced, None, None, 1.0, None, 0,
+                                    None)
 
 
 def test_improved_enhance_workspace_query_needs_no_gpu():
@@ -35,7 +36,7 @@ def test_improved_enhance_workspace_query_needs_no_gpu():
     assert lib.fsn_last_error_code() == _lib.FSN_ERR_UNSUPPORTED
 
 
-def test_improved_enhance_rejects_bad_lengths_before_any_cuda_call():
+def test_improved_enhance_checks_arguments_before_any_cuda_call():
     """No workspace, no weights, no device: every one of these fails on its argument check."""
     from fullsubnet_b200 import _lib
     from oracle import improved_fullsubnet_oracle as IO
@@ -47,14 +48,15 @@ def test_improved_enhance_rejects_bad_lengths_before_any_cuda_call():
     assert b"clip 1" in lib.fsn_last_error()
     assert _call(lib, d, [15000, 257, 3000], 16000) == _lib.FSN_ERR_SHAPE  # max(lengths) != L_max
     assert b"15000" in lib.fsn_last_error()
-    # valid lengths reach the workspace check, the last one before the first launch; n_fft 960 included
-    assert _call(lib, d, [16000, 257, 3000], 16000) == _lib.FSN_ERR_WORKSPACE
+    # valid lengths reach the workspace check, the last one before the first launch; n_fft 960 included (a stand-in
+    # output pointer, never written: the call returns before any CUDA call)
+    assert _call(lib, d, [16000, 257, 3000], 16000, enhanced=16) == _lib.FSN_ERR_WORKSPACE
     d960 = _model(IO.ARGS_48K_960)._desc("fp32")
     assert _call(lib, d960, [48000, 480], 48000) == _lib.FSN_ERR_SHAPE
     assert b"clip 1" in lib.fsn_last_error()
-    assert _call(lib, d960, [48000, 481], 48000) == _lib.FSN_ERR_WORKSPACE
+    assert _call(lib, d960, [48000, 481], 48000, enhanced=16) == _lib.FSN_ERR_WORKSPACE
     # null lengths: every clip L_max samples
-    assert lib.fsn_improved_enhance(C.byref(d960), None, None, None, 2, 48000, None, None, None, 1.0, None, 0,
+    assert lib.fsn_improved_enhance(C.byref(d960), None, None, None, 2, 48000, 16, None, None, 1.0, None, 0,
                                     None) == _lib.FSN_ERR_WORKSPACE
 
 

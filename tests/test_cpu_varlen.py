@@ -1,4 +1,4 @@
-"""CPU-only checks of the clips-of-different-lengths path: fsn_enhance_varlen's workspace query and argument checks
+"""CPU-only checks of the clips-of-different-lengths path: fsn_enhance's workspace query and argument checks
 (both answer before any CUDA call), the file loop's batch planner, and the Python ``lengths`` argument."""
 import ctypes as C
 import random
@@ -16,26 +16,24 @@ def _desc(**kw):
     return _lib.ModelDesc(**a)
 
 
-def _call(lib, d, lengths, L_max, n_fft=512, hop=256):
+def _call(lib, d, lengths, L_max, n_fft=512, hop=256, enhanced=None):
     arr = (C.c_int32 * len(lengths))(*lengths)
-    return lib.fsn_enhance_varlen(C.byref(d), None, None, None, None, arr, len(lengths), L_max, n_fft, hop, n_fft, None,
-                                  None, None, 1.0, None, 0, None)
+    return lib.fsn_enhance(C.byref(d), None, None, None, None, arr, len(lengths), L_max, n_fft, hop, n_fft, enhanced, None,
+                           None, 1.0, None, 0, None)
 
 
-def test_varlen_workspace_query_needs_no_gpu():
+def test_enhance_workspace_query_needs_no_gpu():
     from fullsubnet_b200 import _lib
     lib = _lib.load()
     d = _desc()
-    n = lib.fsn_enhance_varlen_workspace_bytes(C.byref(d), 4, 64000, 512, 256)
-    # the enhance workspace plus the per-clip length table
-    assert n > lib.fsn_enhance_workspace_bytes(C.byref(d), 4, 64000, 512, 256) > 0
-    assert lib.fsn_enhance_varlen_workspace_bytes(C.byref(d), 8, 64000, 512, 256) > n
-    d960 = _desc(num_freqs=481)
-    assert lib.fsn_enhance_varlen_workspace_bytes(C.byref(d960), 4, 48000, 960, 480) == 0
-    assert lib.fsn_last_error_code() == _lib.FSN_ERR_UNSUPPORTED
+    n = lib.fsn_enhance_workspace_bytes(C.byref(d), 4, 64000, 512, 256)
+    assert n > 0
+    assert lib.fsn_enhance_workspace_bytes(C.byref(d), 8, 64000, 512, 256) > n
+    # the query takes no lengths: at n_fft 960 it sizes the null-lengths call (lengths are refused at the call)
+    assert lib.fsn_enhance_workspace_bytes(C.byref(_desc(num_freqs=481)), 4, 48000, 960, 480) > 0
 
 
-def test_varlen_rejects_bad_lengths_before_any_cuda_call():
+def test_enhance_rejects_bad_lengths_before_any_cuda_call():
     """No workspace, no weights, no device: every one of these fails on its argument check."""
     from fullsubnet_b200 import _lib
     lib = _lib.load()
@@ -48,8 +46,9 @@ def test_varlen_rejects_bad_lengths_before_any_cuda_call():
     assert b"3900" in lib.fsn_last_error()
     assert _call(lib, _desc(num_freqs=481), [4800, 4000], 4800, 960, 480) == _lib.FSN_ERR_UNSUPPORTED
     assert b"n_fft=960" in lib.fsn_last_error()
-    # valid lengths reach the workspace check, the last one before the first launch
-    assert _call(lib, d, [4000, 257, 3000], 4000) == _lib.FSN_ERR_WORKSPACE
+    # valid lengths reach the workspace check, the last one before the first launch (a stand-in output pointer, never
+    # written: the call returns before any CUDA call)
+    assert _call(lib, d, [4000, 257, 3000], 4000, enhanced=16) == _lib.FSN_ERR_WORKSPACE
 
 
 def _check_plan(lens, bs, mp):
@@ -92,7 +91,8 @@ def test_plan_batches_exact_groups_at_zero_padding():
         plan_batches(lens, 4, 1.0)
 
 
-def test_python_lengths_argument_is_checked():
+def test_python_lengths_argument_and_table_are_checked():
+    from fullsubnet_b200 import _lib
     from fullsubnet_b200.fullsubnet.model import Model
     from oracle import fullsubnet_oracle as O
     m = Model(**O.DEFAULT_MODEL_ARGS)
@@ -104,7 +104,7 @@ def test_python_lengths_argument_is_checked():
             fn(y, lengths=[4000, 4001, 300])
         with pytest.raises(ValueError):
             fn(y, lengths=torch.tensor([4000.0, 3000.0, 300.0]))
-    lens = Model._lengths_table(torch.tensor([4000, 3000, 300]), 3, 4000)
+    lens = _lib.lengths_table(torch.tensor([4000, 3000, 300]), 3, 4000)
     assert lens.dtype == np.int32 and lens.tolist() == [4000, 3000, 300] and lens.flags["C_CONTIGUOUS"]
 
 

@@ -423,9 +423,9 @@ def test_gru_model_matches_reference(golden, dev):
 
 
 def test_batched_file_loop_matches_reference_host_loop(dev, tmp_path):
-    """Inferencer.enhance_files: wav files of two different lengths -> grouped batches -> fsn_enhance_pcm (int16 scaling
-    fused behind the iSTFT) -> wav files; every file equals the reference's per-file flow (base_inferencer.py:172-187:
-    full_band_crm_mask on that clip alone, int16(0.8 * 32767 * y / max|y|))."""
+    """Inferencer.enhance_files: wav files of two different lengths -> grouped batches -> fsn_enhance with pcm (int16
+    scaling fused behind the iSTFT) -> wav files; every file equals the reference's per-file flow
+    (base_inferencer.py:172-187: full_band_crm_mask on that clip alone, int16(0.8 * 32767 * y / max|y|))."""
     import wave
     from fullsubnet_b200.inferencer import Inferencer
     from oracle import fullsubnet_oracle as O

@@ -1,6 +1,7 @@
-"""Clips of different lengths in one fullsubnet call (fsn_enhance_varlen): every clip of a mixed batch is bit-identical
-to the same clip enhanced alone, whatever its length, its neighbours or the samples past its end; the file loop's
-mixed-length batches write the same files as equal-length batches."""
+"""Clips of different lengths in one fullsubnet call (fsn_enhance with lengths): every clip of a mixed batch is
+bit-identical to the same clip enhanced alone, whatever its length, its neighbours or the samples past its end; the file
+loop's mixed-length batches write the same files as equal-length batches; and the Inferencer's int16 output takes the
+fused call at every n_fft."""
 import numpy as np
 import pytest
 import torch
@@ -172,3 +173,34 @@ def test_file_loop_mixed_length_batches(dev, tmp_path, monkeypatch):
             got = np.frombuffer(f.readframes(f.getnframes()), dtype="<i2")
         assert got.shape == ref.shape
         assert np.abs(got.astype(np.int32) - ref).max() <= 1
+
+
+@pytest.mark.parametrize("which", ["fullsubnet", "fullband_baseline"])
+def test_inferencer_pcm_at_n_fft_960_equals_the_two_pass_path(dev, which):
+    """n_fft 960 (direct DFT): Inferencer.enhance_to_pcm takes the model's fused enhance_pcm, and its int16 output is
+    enhance_batch followed by the two-pass fsn_peak_normalize_int16, bit for bit."""
+    from fullsubnet_b200 import _lib
+    from fullsubnet_b200.inferencer import Inferencer
+    from oracle import fullsubnet_oracle as O
+    if which == "fullsubnet":
+        args = dict(O.DEFAULT_MODEL_ARGS, num_freqs=481)
+        m = _model(args, O.make_state_dict(seed=0, args=args), dev, "auto")
+    else:
+        from fullsubnet_b200.fullband_baseline.model import Model
+        from oracle import fullband_baseline_oracle as BO
+        args = dict(BO.DEFAULT_FBB_ARGS, num_freqs=481)
+        m = Model(**args)
+        m.load_state_dict(BO.make_fbb_state_dict(seed=11, args=args), strict=True)
+        m = m.to(dev).eval()
+    cfg = {"acoustics": {"n_fft": 960, "hop_length": 480, "win_length": 960, "sr": 48000}}
+    inf = Inferencer(config=cfg, model=m, device=dev)
+    B, L = 3, 48000 + 123
+    y = O.make_noisy(B, L, seed=21, speechlike=True, sr=48000)
+    pcm = inf.enhance_to_pcm(y)
+    enhanced = inf.enhance_batch(y)
+    ref = torch.empty_like(pcm)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().fsn_peak_normalize_int16(enhanced.data_ptr(), B, L, 0.8 * float(np.iinfo(np.int16).max),
+                                                      ref.data_ptr(), _lib.stream_ptr(dev)))
+    assert pcm.dtype == torch.int16 and pcm.shape == (B, L)
+    assert torch.equal(pcm, ref)
