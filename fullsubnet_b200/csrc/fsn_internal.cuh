@@ -1,5 +1,6 @@
 // Internal (non-ABI) declarations shared by the translation units of libfsn_b200.
 #pragma once
+#include <cudaTypedefs.h>
 #include <cuda_fp16.h>
 
 #include "fsn_common.cuh"
@@ -83,8 +84,17 @@ int cum_clip_scale_launch(const float2* fs, int B, int Tp, int F, float eps, flo
 int cum_unit_scale_launch(const float* magT, const float* fbT, RowMap map, int R, int Tp, int Ns, int Nf, float eps,
                           float* scaleT, cudaStream_t st, bool time_major = false);
 
+// TMA tensor maps (fsn_tgemm.cu).  tmap_encoder: cuTensorMapEncodeTiled through the runtime's driver entry point (no link
+// against libcuda), nullptr when the driver lacks it.  encode_tmap_2d: a row-major 2-D array of `inner` elements per row,
+// `rows` rows pitch_bytes apart, read in boxes of box_inner x box_rows with 128B swizzle, zero fill outside; false when
+// the encoder is missing or refuses the layout
+PFN_cuTensorMapEncodeTiled_v12000 tmap_encoder();
+bool encode_tmap_2d(CUtensorMap* m, CUtensorMapDataType dtype, const void* base, cuuint64_t inner, cuuint64_t rows,
+                    cuuint64_t pitch_bytes, cuuint32_t box_inner, cuuint32_t box_rows);
+
 // tf32 wgmma GEMM (fsn_tgemm.cu): C[M,N] (+)= A[M,K] B[N,K]^T, fp32 row-major operands with 16-byte aligned rows.
-// tgemm_available: the device can run it (sm_90, opt-in shared memory) and FSN_NO_TGEMM is unset; asks the CUDA runtime
+// tgemm_available: the device can run it (sm_90, opt-in shared memory) and the driver has the tensor-map encoder; asks
+// the CUDA runtime
 bool tgemm_available();
 bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, int K);
 int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
@@ -94,7 +104,6 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
 size_t tgemm_blocked_floats(size_t K, int M);
 int transpose_blocked_launch(const float* in, size_t K, int M, size_t ld, float* out, cudaStream_t st, float* colsum_part,
                              int max_slabs, int* slabs);
-bool tgemm_blocked_enabled();
 int tgemm_blocked_launch(const float* Ablk, int nkb_a, int a_kb0, const float* Bblk, int nkb_b, int b_kb0, float* C, size_t ldc,
                          int M, int N, int K, bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st);
 
@@ -105,15 +114,15 @@ struct LstmStepHalf {
   const __half *Hprev16, *w_hh16, *Xt16, *w_ih16;
   __half* H16_out;
 };
-bool lstm_fwd_step_half_enabled(int H);
 int to_half_launch(const float* in, size_t n, __half* out, cudaStream_t st);
 int lstm_fwd_step_launch(const float* Hprev, const float* w_hh, const float* Xt, const float* w_ih, int K0, float* Gt,
                          const float* b_ih, const float* b_hh, const float* C_prev, float* C_out, float* H_out, int R, int H,
                          cudaStream_t st, const LstmStepHalf* h = nullptr);
 
-// one LSTM layer over all steps on the tf32 tensor-core path (fsn_train.cu): input projection of all steps hoisted
-// into one GEMM, then per step the recurrent GEMM into `rec` [R,4H] and the fused cell kernel.  G [Tp,R,4H]
-// (post-activation gates), C, H [Tp,R,H] receive every step.  X [Tp,R,K0] contiguous.
+// one LSTM layer over all steps on the tf32 tensor-core path (fsn_train.cu): one lstm_fwd_step_kernel per step when
+// H % 32 == 0 (the layer input folded in up to 512 wide, else one hoisted projection GEMM of all steps), otherwise per
+// step the recurrent GEMM into `rec` [R,4H] and the cell kernel.  G [Tp,R,4H] (post-activation gates), C, H [Tp,R,H]
+// receive every step.  X [Tp,R,K0] contiguous.
 struct LayerSave { float *G, *C, *H; };
 // fp16 side buffers of one layer (all nullable): H16 [Tp,R,H] copy of the hidden states (written by the step kernel, the
 // next layer's X16), X16 [Tp,R,K0] copy of the layer input, w16: 4H*(H+K0) halfs for the weight copies

@@ -17,8 +17,6 @@
 // Column block j (8 columns) of D is gate j % 4, so the thread that holds a row's fragment holds all four gates of
 // the same two units: c stays in 8 registers (4 rows x 2 units), no exchange.  Groups of 64 CTAs cover 128 clips
 // each with H = 512.
-#include <cuda.h>
-#include <cudaTypedefs.h>
 #include <string.h>
 #include <stdlib.h>
 
@@ -317,21 +315,6 @@ __global__ void bias_act_kernel(float* __restrict__ x, size_t rows, int N, size_
   }
 }
 
-static PFN_cuTensorMapEncodeTiled_v12000 encoder() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
-    cudaGetLastError();
-  }
-  return fn;
-}
-
 static size_t smem_bytes(int Kp, bool x3, int stages) {
   const int parts = x3 ? 2 : 1;
   return (size_t)stages * parts * A_TILE + (size_t)(Kp / KB) * parts * NG * 128 + sizeof(Bars) + 1024;
@@ -349,7 +332,7 @@ static int rec_sm_count() {
 // tensor-core recurrence available for hidden size H on this device?
 bool lstm_rec_tc_supported(int H, bool x3) {
   static const bool off = getenv("FSN_NO_REC_TC") != nullptr;
-  if (off || H < 64 || !rec::encoder()) return false;  // H >= 64: see lstm_rec_tc_scratch_bytes
+  if (off || H < 64 || !tmap_encoder()) return false;  // H >= 64: see lstm_rec_tc_scratch_bytes
   int dev = 0, coop = 0, max_smem = 0, major = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
@@ -408,13 +391,8 @@ int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, 
     if ((rc = check_cuda(cudaMemsetAsync(scratch, 0, state_bytes, st), "lstm_rec_tc memset"))) return rc;
     if ((rc = check_cuda(cudaMemsetAsync(barrier, 0, 64 * 32 * sizeof(unsigned int), st), "lstm_rec_tc memset"))) return rc;
     CUtensorMap tm;
-    cuuint64_t gdim[2] = {(cuuint64_t)Kp, (cuuint64_t)(2 * parts * Rpad)};
-    cuuint64_t gstr[1] = {(cuuint64_t)Kp * sizeof(__half)};
-    cuuint32_t box[2] = {(cuuint32_t)rec::KB, (cuuint32_t)rec::MR};
-    cuuint32_t estr[2] = {1, 1};
-    FSN_REQUIRE(rec::encoder()(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)state, gdim, gstr, box, estr,
-                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS,
+    FSN_REQUIRE(encode_tmap_2d(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, state, Kp, 2 * parts * Rpad, Kp * sizeof(__half), rec::KB,
+                               rec::MR),
                 FSN_ERR_CUDA, "lstm_rec_tc: cuTensorMapEncodeTiled failed");
     rec::Args a;
     a.w_hh = w_hh; a.b_ih = b_ih; a.b_hh = b_hh;

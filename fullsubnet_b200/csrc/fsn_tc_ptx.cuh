@@ -1,4 +1,4 @@
-// PTX helpers shared by the tensor-core kernels (mbarrier, bulk copy / TMA, cp.async, cluster / DSMEM).
+// PTX helpers shared by the tensor-core kernels (mbarrier, bulk copy / TMA, cluster / DSMEM).
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -217,14 +217,6 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// 16-byte asynchronous copy global -> shared; bytes beyond src_bytes (0..16) are zero-filled
-__device__ __forceinline__ void cp_async16_zfill(uint32_t dst_smem, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_smem), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // byte offset of element (row, k) in a K-major 128B-swizzled block of 64 k (rows of 128 B)
 __host__ __device__ __forceinline__ int swz128_off(int row, int k) {
   return (row >> 3) * 1024 + (row & 7) * 128 + ((((k >> 3) ^ (row & 7)) & 7) << 4) + (k & 7) * 2;

@@ -5,9 +5,8 @@
 //   warpgroups 0-1  consumers: warpgroup h multiplies rows 64h..64h+63 of the tile (m64nBNk8, 4 per stage), releases each
 //                   stage once the wgmma that read it has retired (wait_group 1), and writes its accumulator fragment
 //                   straight from registers after the last stage.
-//   producers       tgemm_tma_kernel: one warp, one elected lane issues the TMA tiled loads (128B swizzle, rows / k beyond
-//                   the matrix zero-filled by the tensor map) of a stage.  tgemm_kernel: a third warpgroup whose threads
-//                   copy 16-byte chunks with cp.async straight into the same 128B-swizzled K-major layout (chunk ^= row & 7).
+//   producer        one warp, one elected lane issues the TMA tiled loads (128B swizzle, rows / k beyond the matrix
+//                   zero-filled by the tensor map) of a stage.
 // No operand conversion pass: the tensor core reads fp32 bits as tf32 (10-bit mantissa, truncation).
 //
 // Also in this file, built from the same pieces (DESIGN.md 4.2):
@@ -15,10 +14,6 @@
 //                           weight-gradient GEMMs dW = dG^T X
 //   lstm_fwd_step_kernel    one LSTM step of the training forward: [x_t | h_{t-1}] [W_ih | W_hh]^T (fp16 / tf32 operands)
 //                           and the cell in one launch; tile = 128 rows x (4 gates x 32 hidden units)
-#include <cuda.h>
-#include <cudaTypedefs.h>
-#include <string.h>
-
 #include "fsn_internal.cuh"
 #include "fsn_tc_ptx.cuh"
 #include "fsn_wgmma.cuh"
@@ -38,10 +33,6 @@ template <int BN> struct Cfg {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   // BN = 128: 3 stages (96 KB) so two CTAs share an SM - one writes its tile while the other runs its main loop
   static constexpr int STAGES = (BN == 128) ? 3 : 4;
-  // cp.async groups in flight per producer thread.  At most STAGES - 2: the producer waits for stage i - STAGES to be
-  // released before it marks stage i - LAG full, and the consumers release stage i - STAGES only once stage
-  // i - STAGES + 1 is full, so LAG = STAGES - 1 deadlocks as soon as a tile has more than STAGES k blocks
-  static constexpr int LAG = STAGES - 2;
   static constexpr int MIN_CTAS = (BN == 128) ? 2 : 1;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
@@ -110,80 +101,14 @@ __device__ __forceinline__ void epilogue(const float (&acc)[BN / 2], float* __re
   }
 }
 
-template <int BN>
-__global__ void __launch_bounds__(CONSUMERS + 128, 1)
-tgemm_kernel(const float* __restrict__ A, size_t lda, const float* __restrict__ Bm, size_t ldb, float* __restrict__ C,
-             size_t ldc, int M, int N, int K, int k_per_split, int accumulate, size_t split_stride) {
-  using CF = Cfg<BN>;
-  constexpr int STAGES = CF::STAGES, LAG = CF::LAG;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  Bars& bars = *reinterpret_cast<Bars*>(smem + STAGES * CF::STAGE_BYTES);
-  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-  const int kb = blockIdx.z * k_per_split;
-  const int ke = (kb + k_per_split < K) ? kb + k_per_split : K;
-  const int nk = (ke - kb + BK - 1) / BK;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 128); mbar_init(&bars.empty[s], CONSUMERS / 32); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  if (threadIdx.x >= CONSUMERS) {
-    // ------------------------------------------------------------------ producers
-    // thread -> (16-byte chunk c = tid & 7 of a 128-byte row, rows (tid >> 3) + 16 j): 8 threads read one full line
-    const int tid = threadIdx.x - CONSUMERS;
-    const int c = tid & 7, rbase = tid >> 3;
-    const uint32_t sw = (uint32_t)(rbase & 7);  // (rbase + 16 j) & 7
-    const uint32_t dst_off = (uint32_t)((rbase >> 3) * 1024 + (rbase & 7) * 128) + (((uint32_t)c ^ sw) << 4);
-    const uint32_t smem_base = smem_u32(smem);
-    const float* a_row = A + (size_t)(m0 + rbase) * lda + c * 4;
-    const float* b_row = Bm + (size_t)(n0 + rbase) * ldb + c * 4;
-    for (int i = 0; i < nk + LAG; ++i) {
-      if (i < nk) {
-        const int s = i % STAGES;
-        if (i >= STAGES) mbar_wait<true>(&bars.empty[s], (uint32_t)(((i / STAGES) - 1) & 1));
-        const int k0 = kb + i * BK;
-        int rem = (ke - (k0 + c * 4)) * 4;
-        rem = rem < 0 ? 0 : (rem > 16 ? 16 : rem);
-        const uint32_t sa = smem_base + s * CF::STAGE_BYTES + dst_off;
-#pragma unroll
-        for (int j = 0; j < BM / 16; ++j) {
-          const uint32_t nb = (m0 + rbase + 16 * j < M) ? (uint32_t)rem : 0u;
-          cp_async16_zfill(sa + j * 2048, nb ? (const void*)(a_row + (size_t)(16 * j) * lda + k0) : (const void*)A, nb);
-        }
-#pragma unroll
-        for (int j = 0; j < BN / 16; ++j) {
-          const uint32_t nb = (n0 + rbase + 16 * j < N) ? (uint32_t)rem : 0u;
-          cp_async16_zfill(sa + A_BYTES + j * 2048, nb ? (const void*)(b_row + (size_t)(16 * j) * ldb + k0) : (const void*)Bm,
-                           nb);
-        }
-      }
-      cp_async_commit();
-      if (i >= LAG) {
-        cp_async_wait<LAG>();   // group i-LAG (k-step i-LAG) has landed
-        fence_proxy_async();    // generic-proxy writes -> visible to the tensor core (async proxy)
-        mbar_arrive(&bars.full[(i - LAG) % STAGES]);
-      }
-    }
-  } else {
-    float acc[BN / 2];
-    mma_loop<BN>(smem, bars, nk, acc);
-    epilogue<BN>(acc, C, ldc, M, N, m0, n0, accumulate, split_stride);
-  }
-}
-
-// Same tile, operands fed by TMA: one elected lane issues the tiled loads of a stage (128B hardware swizzle, rows / k
-// beyond the matrix zero-filled by the tensor map), the full barrier counts the transaction bytes.
+// One elected lane of the producer warp issues the tiled loads of a stage (128B hardware swizzle, rows / k beyond the
+// matrix zero-filled by the tensor map), the full barrier counts the transaction bytes.
 template <int BN>
 __global__ void __launch_bounds__(CONSUMERS + 32, Cfg<BN>::MIN_CTAS)
-tgemm_tma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmB2, float* __restrict__ C, size_t ldc, int M, int N, int K,
-                 int k_per_split, int accumulate, size_t split_stride, BlockedOps bo) {
+tgemm_tma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, float* __restrict__ C,
+                 size_t ldc, int M, int N, int K, int k_per_split, int accumulate, size_t split_stride, BlockedOps bo) {
   using CF = Cfg<BN>;
   constexpr int STAGES = CF::STAGES;
-  (void)tmB2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   Bars& bars = *reinterpret_cast<Bars*>(smem + STAGES * CF::STAGE_BYTES);
@@ -249,13 +174,14 @@ __device__ __forceinline__ float tanh_mufu(float x) {
   return fmaf(2.0f, r, -1.0f);
 }
 
-// HT: hidden size known at compile time (0: runtime) - the strides of the cell become immediate offsets
-// ST: TMA stages
-template <int ST> struct StepCfg {
-  static constexpr int MAIN = ST * Cfg<128>::STAGE_BYTES;
+// shared memory of the step kernel: two TMA stages of the 128 x 128 tile
+struct StepCfg {
+  static constexpr int STAGES = 2;
+  static constexpr int MAIN = STAGES * Cfg<128>::STAGE_BYTES;
   static constexpr int SMEM = MAIN + 1024 /*align*/ + 256 /*barriers*/;
 };
-template <bool FOLD, int HT, int ST>
+// HT: hidden size known at compile time (0: runtime) - the strides of the cell become immediate offsets
+template <bool FOLD, int HT>
 __global__ void __launch_bounds__(CONSUMERS + 32, 2)
 lstm_fwd_step_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmWx, float* __restrict__ G,
@@ -264,10 +190,10 @@ lstm_fwd_step_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
                      int nkh, int x16, int h16) {
   const int H = HT ? HT : H_rt;
   using CF = Cfg<128>;
-  constexpr int STAGES = ST;
+  constexpr int STAGES = StepCfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  Bars& bars = *reinterpret_cast<Bars*>(smem + StepCfg<ST>::MAIN);
+  Bars& bars = *reinterpret_cast<Bars*>(smem + StepCfg::MAIN);
   const int m0 = blockIdx.x * BM, u0 = blockIdx.y * 32;
   // k blocks: first nkx of x_t W_ih^T (a narrow layer input is folded in here instead of a hoisted projection: G then
   // carries no P and is only written), then nkh of h_{t-1} W_hh^T (0 at the first step)
@@ -343,8 +269,7 @@ lstm_fwd_step_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
           const float b = b_ih[g * H + u] + b_hh[g * H + u];
           z[g] = FOLD ? a + b : (gr[g * H + u] + b) + a;
         }
-        // ex2 + rcp forms (2 ulp class; the tf32 / fp16 products around them are 1e-3 class).  FSN_TRAIN_FAST_ACT=0
-        // selects the unfused GEMM + lstm_cell_fwd_kernel path with expf / IEEE division instead
+        // ex2 + rcp forms (2 ulp class; the tf32 / fp16 products around them are 1e-3 class)
         const float gi = sigmoid_mufu(z[0]), gf = sigmoid_mufu(z[1]), gg = tanh_mufu(z[2]), go = sigmoid_mufu(z[3]);
         const float cp = C_prev ? C_prev[(size_t)row * H + u] : 0.f;
         const float cn = fmaf(gf, cp, gi * gg);
@@ -361,50 +286,44 @@ lstm_fwd_step_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
 }  // namespace tg
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda)
-static PFN_cuTensorMapEncodeTiled_v12000 tmap_encoder() {
+PFN_cuTensorMapEncodeTiled_v12000 tmap_encoder() {
   static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
   static bool tried = false;
   if (!tried) {
     tried = true;
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
-    if (getenv("FSN_TGEMM_FEED") == nullptr || strcmp(getenv("FSN_TGEMM_FEED"), "cpasync") != 0)
-      if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-          q == cudaDriverEntryPointSuccess)
-        fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
     cudaGetLastError();
   }
   return fn;
 }
 
-// fp32 [rows, K] row-major (ld floats) -> boxes of box_rows x 32 floats, 128B swizzle, zero fill outside
+bool encode_tmap_2d(CUtensorMap* m, CUtensorMapDataType dtype, const void* base, cuuint64_t inner, cuuint64_t rows,
+                    cuuint64_t pitch_bytes, cuuint32_t box_inner, cuuint32_t box_rows) {
+  PFN_cuTensorMapEncodeTiled_v12000 fn = tmap_encoder();
+  if (!fn) return false;
+  cuuint64_t gdim[2] = {inner, rows};
+  cuuint64_t gstr[1] = {pitch_bytes};
+  cuuint32_t box[2] = {box_inner, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  return fn(m, dtype, 2, (void*)base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// fp32 [rows, K] row-major (ld floats) -> boxes of box_rows x 32 floats
 static bool make_tmap(CUtensorMap* m, const float* base, int K, int rows, size_t ld, int box_rows) {
-  PFN_cuTensorMapEncodeTiled_v12000 fn = tmap_encoder();
-  if (!fn) return false;
-  cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)ld * sizeof(float)};
-  cuuint32_t box[2] = {(cuuint32_t)tg::BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) ==
-         CUDA_SUCCESS;
+  return encode_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, K, rows, ld * sizeof(float), tg::BK, box_rows);
 }
 
-// fp16 [rows, K] row-major (ld halfs) -> boxes of box_rows x 64 halfs (128 bytes), 128B swizzle, zero fill outside
+// fp16 [rows, K] row-major (ld halfs) -> boxes of box_rows x 64 halfs (128 bytes)
 static bool make_tmap16(CUtensorMap* m, const __half* base, int K, int rows, size_t ld, int box_rows) {
-  PFN_cuTensorMapEncodeTiled_v12000 fn = tmap_encoder();
-  if (!fn) return false;
-  cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)ld * sizeof(__half)};
-  cuuint32_t box[2] = {(cuuint32_t)(2 * tg::BK), (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) ==
-         CUDA_SUCCESS;
+  return encode_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, base, K, rows, ld * sizeof(__half), 2 * tg::BK, box_rows);
 }
 
-constexpr int TGEMM_THREADS = tg::CONSUMERS + 32;      // TMA-fed kernels: two consumer warpgroups + producer warp
-constexpr int TGEMM_CP_THREADS = tg::CONSUMERS + 128;  // cp.async-fed kernel: producer warpgroup
+constexpr int TGEMM_THREADS = tg::CONSUMERS + 32;  // two consumer warpgroups + producer warp
 
 static int tgemm_sm_count() {
   static int sms = 0;
@@ -426,7 +345,7 @@ bool tgemm_available() {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    ok = (major == 9 && smem >= tg::Cfg<128>::SMEM && getenv("FSN_NO_TGEMM") == nullptr) ? 1 : 0;
+    ok = (major == 9 && smem >= tg::Cfg<128>::SMEM && tmap_encoder() != nullptr) ? 1 : 0;
   }
   return ok == 1;
 }
@@ -436,25 +355,12 @@ bool tgemm_supported(const float* A, size_t lda, const float* Bm, size_t ldb, in
          (reinterpret_cast<uintptr_t>(Bm) & 15) == 0;
 }
 
-// C[M,N] (+)= A[M,K] B[N,K]^T; `scratch` (>= scratch_floats) enables split-K for long-K / few-tile problems
-int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
-                 bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st) {
-  if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
-  FSN_REQUIRE(tgemm_supported(A, lda, Bm, ldb, K), FSN_ERR_UNSUPPORTED, "tgemm: operands must be 16-byte aligned rows");
-  static const int force_bn = getenv("FSN_TGEMM_BN") && atoi(getenv("FSN_TGEMM_BN")) == 128 ? 128 : 0;
-  int BN = force_bn ? force_bn : ((N >= 256 && N % 256 == 0) ? 256 : 128);
-  // a handful of tiles (per-step GEMMs of the full-band stack, 64 rows): narrow tiles + split-K so that the weight
-  // matrix is streamed by ~64 CTAs instead of 2-8
-  const bool few = scratch && K < 8192 && cdiv(M, tg::BM) * cdiv(N, 128) <= 32;
-  if (few && !force_bn) BN = 128;
-  // short K, many tiles (hoisted input projections: output-write bound): 128-wide tiles, two CTAs per SM, so one CTA's
-  // epilogue overlaps the other's main loop (measured 1081 -> 945 us at K = 384, 778 -> 522 us at K = 32 per 195 k rows)
-  static const int smallk_bn = getenv("FSN_TGEMM_SMALLK_BN") ? atoi(getenv("FSN_TGEMM_SMALLK_BN")) : 128;
-  if (!force_bn && K <= 512 && BN == 256 && cdiv(M, tg::BM) >= 1024) BN = smallk_bn == 256 ? 256 : 128;
+// split-K slices of a long-K GEMM with few tiles: minimise waves(tiles * S) / S over the SM slots (1 or 2 resident CTAs
+// per SM), slices of >= 2048 k, S * M * N partial sums within the scratch
+static int splitk_slices(int M, int N, int K, int BN, const float* scratch, size_t scratch_floats) {
   const int tiles = cdiv(M, tg::BM) * cdiv(N, BN);
   int S = 1;
   if (scratch && K >= 8192 && tiles < 296) {
-    // minimise waves(tiles * S) / S over the SM slots (1 or 2 resident CTAs per SM), slices of >= 2048 k
     const int slots = tgemm_sm_count() * (BN == 128 ? 2 : 1);  // resident CTAs
     double best = 1e30;
     for (int s = 1; s <= 64 && s <= cdiv(K, 2048); ++s) {
@@ -463,8 +369,41 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
       if (cost < best) { best = cost; S = s; }
     }
   }
+  return S;
+}
+
+// dynamic shared memory opt-in of both tile widths of tgemm_tma_kernel (per device)
+static int tgemm_smem_optin() {
+  static bool done_by_dev[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  bool& done = done_by_dev[dev & 63];
+  if (done) return FSN_OK;
+  int rc;
+  if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            tg::Cfg<256>::SMEM), "tgemm smem attr")) ||
+      (rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            tg::Cfg<128>::SMEM), "tgemm smem attr")))
+    return rc;
+  done = true;
+  return FSN_OK;
+}
+
+// C[M,N] (+)= A[M,K] B[N,K]^T; `scratch` (>= scratch_floats) enables split-K for long-K / few-tile problems
+int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
+                 bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st) {
+  if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
+  FSN_REQUIRE(tgemm_supported(A, lda, Bm, ldb, K), FSN_ERR_UNSUPPORTED, "tgemm: operands must be 16-byte aligned rows");
+  // a handful of tiles (per-step GEMMs of the full-band stack, 64 rows): narrow tiles + split-K so that the weight
+  // matrix is streamed by ~64 CTAs instead of 2-8
+  const bool few = scratch && K < 8192 && cdiv(M, tg::BM) * cdiv(N, 128) <= 32;
+  // short K, many tiles (hoisted input projections: output-write bound): 128-wide tiles, two CTAs per SM, so one CTA's
+  // epilogue overlaps the other's main loop (measured 1081 -> 945 us at K = 384, 778 -> 522 us at K = 32 per 195 k rows)
+  const bool short_k_many_tiles = K <= 512 && cdiv(M, tg::BM) >= 1024;
+  const int BN = (N >= 256 && N % 256 == 0 && !few && !short_k_many_tiles) ? 256 : 128;
+  int S = splitk_slices(M, N, K, BN, scratch, scratch_floats);
   if (few && K >= 256) {
-    S = 64 / tiles;
+    S = 64 / (cdiv(M, tg::BM) * cdiv(N, BN));
     if (S > K / 128) S = K / 128;
     while (S > 1 && (size_t)S * M * N > scratch_floats) --S;
     if (S < 1) S = 1;
@@ -475,56 +414,17 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
   float* dst = S > 1 ? scratch : C;
   const size_t ldd = S > 1 ? (size_t)N : ldc;
   const int acc = (S > 1) ? 0 : (accumulate ? 1 : 0);
-  int rc;
   CUtensorMap tmA, tmB;
-  CUtensorMap tmB2;
-  if (make_tmap(&tmA, A, K, M, lda, tg::BM) && make_tmap(&tmB, Bm, K, N, ldb, BN > 256 ? 256 : BN) &&
-      make_tmap(&tmB2, Bm, K, N, ldb, BN > 256 ? BN - 256 : 128)) {
-    static bool attr_by_dev[64] = {};  // the opt-in is per device
-    int cur_dev_ = 0; cudaGetDevice(&cur_dev_); bool& attr = attr_by_dev[cur_dev_ & 63];
-    if (!attr) {
-      if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                tg::Cfg<256>::SMEM), "tgemm smem attr")))
-        return rc;
-      if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                tg::Cfg<128>::SMEM), "tgemm smem attr")))
-        return rc;
-      attr = true;
-    }
-    if (BN == 256)
-      tg::tgemm_tma_kernel<256><<<grid, TGEMM_THREADS, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, tmB2, dst, ldd, M, N, K, kps, acc,
-                                                                       (size_t)M * N, tg::BlockedOps{0, 0, 0, 0, 0});
-    else
-      tg::tgemm_tma_kernel<128><<<grid, TGEMM_THREADS, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, tmB2, dst, ldd, M, N, K, kps, acc,
-                                                                       (size_t)M * N, tg::BlockedOps{0, 0, 0, 0, 0});
-    FSN_CHECK_LAUNCH("tgemm_tma_kernel");
-    if (S > 1) return splitk_reduce_launch(scratch, S, M, N, C, ldc, accumulate, st);
-    return FSN_OK;
-  }
-  if (BN == 256) {
-    static bool attr_by_dev[64] = {};  // the opt-in is per device
-    int cur_dev_ = 0; cudaGetDevice(&cur_dev_); bool& attr = attr_by_dev[cur_dev_ & 63];
-    if (!attr) {
-      if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                tg::Cfg<256>::SMEM), "tgemm smem attr")))
-        return rc;
-      attr = true;
-    }
-    tg::tgemm_kernel<256><<<grid, TGEMM_CP_THREADS, tg::Cfg<256>::SMEM, st>>>(A, lda, Bm, ldb, dst, ldd, M, N, K, kps, acc,
-                                                                 (size_t)M * N);
-  } else {
-    static bool attr_by_dev[64] = {};  // the opt-in is per device
-    int cur_dev_ = 0; cudaGetDevice(&cur_dev_); bool& attr = attr_by_dev[cur_dev_ & 63];
-    if (!attr) {
-      if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                tg::Cfg<128>::SMEM), "tgemm smem attr")))
-        return rc;
-      attr = true;
-    }
-    tg::tgemm_kernel<128><<<grid, TGEMM_CP_THREADS, tg::Cfg<128>::SMEM, st>>>(A, lda, Bm, ldb, dst, ldd, M, N, K, kps, acc,
-                                                                 (size_t)M * N);
-  }
-  FSN_CHECK_LAUNCH("tgemm_kernel");
+  FSN_REQUIRE(make_tmap(&tmA, A, K, M, lda, tg::BM) && make_tmap(&tmB, Bm, K, N, ldb, BN), FSN_ERR_CUDA,
+              "tgemm: tensor-map encoding failed");
+  int rc;
+  if ((rc = tgemm_smem_optin())) return rc;
+  const tg::BlockedOps plain{0, 0, 0, 0, 0};
+  if (BN == 256)
+    tg::tgemm_tma_kernel<256><<<grid, TGEMM_THREADS, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, plain);
+  else
+    tg::tgemm_tma_kernel<128><<<grid, TGEMM_THREADS, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, plain);
+  FSN_CHECK_LAUNCH("tgemm_tma_kernel");
   if (S > 1) return splitk_reduce_launch(scratch, S, M, N, C, ldc, accumulate, st);
   return FSN_OK;
 }
@@ -533,21 +433,13 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
 // fused recurrent GEMM + LSTM cell of one training-forward step (tg::lstm_fwd_step_kernel); G_t [R,4H] holds the hoisted
 // input projection and receives the post-activation gates
 bool lstm_fwd_step_supported(const float* Hbuf, const float* w_hh, int H) {
-  static const int mode = getenv("FSN_TRAIN_FUSED_FWD") ? atoi(getenv("FSN_TRAIN_FUSED_FWD")) : 1;
-  static const int fast_act = getenv("FSN_TRAIN_FAST_ACT") ? atoi(getenv("FSN_TRAIN_FAST_ACT")) : 1;
-  return mode != 0 && fast_act != 0 && (H % 32) == 0 && tmap_encoder() != nullptr && tgemm_supported(Hbuf, H, w_hh, H, H);
+  return (H % 32) == 0 && tgemm_supported(Hbuf, H, w_hh, H, H);
 }
 // the layer input is multiplied inside the step kernel (no hoisted projection, no P round trip through HBM: 2 x 9.6 GB per
 // sub-band layer at config 3).  Measured per training step: no fold 110.5 ms, fold K0 <= 64 105.6 ms, all layers 99.1 ms
+static constexpr int STEP_FOLD_MAX_K = 512;  // widest layer input folded in
 bool lstm_fwd_step_folds_input(const float* X, const float* w_ih, int K0) {
-  static const int maxk = getenv("FSN_TRAIN_FOLD_K") ? atoi(getenv("FSN_TRAIN_FOLD_K")) : 512;
-  return K0 <= maxk && tgemm_supported(X, K0, w_ih, K0, K0);
-}
-// fp16 copies of the MMA operands (h and the weights rounded to nearest: the same 11-bit significand as tf32 reads, half the
-// bytes through L2 and twice the tensor rate); the fp32 state, the saved activations and the backward pass are unchanged
-bool lstm_fwd_step_half_enabled(int H) {
-  static const int on = getenv("FSN_TRAIN_F16_FWD") ? atoi(getenv("FSN_TRAIN_F16_FWD")) : 1;
-  return on != 0 && (H % 8) == 0;
+  return K0 <= STEP_FOLD_MAX_K && tgemm_supported(X, K0, w_ih, K0, K0);
 }
 // Hprev == nullptr: first step (no recurrent term).  Xt / w_ih (nullable together): fold x_t W_ih^T in, G_t is then
 // write-only; otherwise G_t holds the hoisted projection P_t.  h: optional fp16 operands (see LstmStepHalf)
@@ -572,12 +464,9 @@ int lstm_fwd_step_launch(const float* Hprev, const float* w_hh, const float* Xt,
   int dev = 0; cudaGetDevice(&dev); bool& attr = attr_by_dev[dev & 63];
   if (!attr) {
     int rc;
-#define FSN_STEP_ATTR(FOLD, HT)                                                                                               \
-  if ((rc = check_cuda(cudaFuncSetAttribute(tg::lstm_fwd_step_kernel<FOLD, HT, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                            tg::StepCfg<2>::SMEM), "lstm_fwd_step smem attr")))                             \
-    return rc;                                                                                                                \
-  if ((rc = check_cuda(cudaFuncSetAttribute(tg::lstm_fwd_step_kernel<FOLD, HT, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                            tg::StepCfg<3>::SMEM), "lstm_fwd_step smem attr")))                             \
+#define FSN_STEP_ATTR(FOLD, HT)                                                                                            \
+  if ((rc = check_cuda(cudaFuncSetAttribute(tg::lstm_fwd_step_kernel<FOLD, HT>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                            tg::StepCfg::SMEM), "lstm_fwd_step smem attr")))                               \
     return rc
     FSN_STEP_ATTR(true, 384); FSN_STEP_ATTR(true, 512); FSN_STEP_ATTR(true, 0);
     FSN_STEP_ATTR(false, 384); FSN_STEP_ATTR(false, 512); FSN_STEP_ATTR(false, 0);
@@ -587,24 +476,15 @@ int lstm_fwd_step_launch(const float* Hprev, const float* w_hh, const float* Xt,
   const int nkx = Xt ? cdiv(K0, x16 ? 2 * tg::BK : tg::BK) : 0, nkh = Hprev ? cdiv(H, h16 ? 2 * tg::BK : tg::BK) : 0;
   FSN_REQUIRE(nkx + nkh > 0, FSN_ERR_SHAPE, "lstm_fwd_step: nothing to multiply");
   const dim3 grid(cdiv(R, tg::BM), H / 32);
-  static const int stages = getenv("FSN_TRAIN_STEP_STAGES") ? atoi(getenv("FSN_TRAIN_STEP_STAGES")) : 2;
-#define FSN_STEP_LAUNCH(FOLD, HT)                                                                                              \
-  do {                                                                                                                         \
-    if (stages == 2)                                                                                                           \
-      tg::lstm_fwd_step_kernel<FOLD, HT, 2><<<grid, TGEMM_THREADS, tg::StepCfg<2>::SMEM, st>>>(                                          \
-          tmA, tmB, tmX, tmWx, Gt, b_ih, b_hh, C_prev, C_out, H_out, h16 ? h->H16_out : nullptr, R, H, nkx, nkh, x16 ? 1 : 0,  \
-          h16 ? 1 : 0);                                                                                                        \
-    else                                                                                                                       \
-      tg::lstm_fwd_step_kernel<FOLD, HT, 3><<<grid, TGEMM_THREADS, tg::StepCfg<3>::SMEM, st>>>(                                          \
-          tmA, tmB, tmX, tmWx, Gt, b_ih, b_hh, C_prev, C_out, H_out, h16 ? h->H16_out : nullptr, R, H, nkx, nkh, x16 ? 1 : 0,  \
-          h16 ? 1 : 0);                                                                                                        \
-  } while (0)
+#define FSN_STEP_LAUNCH(FOLD, HT)                                                                                          \
+  tg::lstm_fwd_step_kernel<FOLD, HT><<<grid, TGEMM_THREADS, tg::StepCfg::SMEM, st>>>(                                      \
+      tmA, tmB, tmX, tmWx, Gt, b_ih, b_hh, C_prev, C_out, H_out, h16 ? h->H16_out : nullptr, R, H, nkx, nkh, x16 ? 1 : 0, \
+      h16 ? 1 : 0)
   if (Xt) {
     if (H == 384) FSN_STEP_LAUNCH(true, 384); else if (H == 512) FSN_STEP_LAUNCH(true, 512); else FSN_STEP_LAUNCH(true, 0);
   } else {
     if (H == 384) FSN_STEP_LAUNCH(false, 384); else if (H == 512) FSN_STEP_LAUNCH(false, 512); else FSN_STEP_LAUNCH(false, 0);
   }
-  (void)0;
 #undef FSN_STEP_LAUNCH
   FSN_CHECK_LAUNCH("lstm_fwd_step_kernel");
   return FSN_OK;
@@ -689,54 +569,32 @@ int transpose_blocked_launch(const float* in, size_t K, int M, size_t ld, float*
   return FSN_OK;
 }
 
-bool tgemm_blocked_enabled() {
-  static const bool on = getenv("FSN_TGEMM_BLOCKED") == nullptr || atoi(getenv("FSN_TGEMM_BLOCKED")) != 0;
-  return on && tmap_encoder() != nullptr;
-}
-
 // C[M,N] (+)= A^T B over K, operands block-tiled (transpose_blocked_launch) with nkb_a / nkb_b k blocks per tile row;
 // a_kb0 / b_kb0: first k block of each operand (lets dW_hh pair dG[1:] with H[:-1])
 int tgemm_blocked_launch(const float* Ablk, int nkb_a, int a_kb0, const float* Bblk, int nkb_b, int b_kb0, float* C, size_t ldc,
                          int M, int N, int K, bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st) {
   if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
-  PFN_cuTensorMapEncodeTiled_v12000 fn = tmap_encoder();
-  FSN_REQUIRE(fn, FSN_ERR_UNSUPPORTED, "tgemm_blocked: cuTensorMapEncodeTiled unavailable");
-  int BN = (N > 128) ? 256 : 128;
-  const int tiles = cdiv(M, tg::BM) * cdiv(N, BN);
-  int S = 1;
-  if (scratch && K >= 8192 && tiles < 296) {
-    const int slots = tgemm_sm_count() * (BN == 128 ? 2 : 1);
-    double best = 1e30;
-    for (int s = 1; s <= 64 && s <= cdiv(K, 2048); ++s) {
-      if ((size_t)s * M * N > scratch_floats) break;
-      const double cost = (double)cdiv(tiles * s, slots) / s + 1e-4 * s;
-      if (cost < best) { best = cost; S = s; }
-    }
-  }
+  FSN_REQUIRE(tmap_encoder(), FSN_ERR_UNSUPPORTED, "tgemm_blocked: cuTensorMapEncodeTiled unavailable");
+  const int BN = (N > 128) ? 256 : 128;
+  int S = splitk_slices(M, N, K, BN, scratch, scratch_floats);
   const int kps = cdiv(cdiv(K, S), tg::BK) * tg::BK;
   S = cdiv(K, kps);
   dim3 grid(cdiv(M, tg::BM), cdiv(N, BN), S);
   float* dst = S > 1 ? scratch : C;
   const size_t ldd = S > 1 ? (size_t)N : ldc;
   const int acc = (S > 1) ? 0 : (accumulate ? 1 : 0);
+  // each operand viewed as [tile rows, 32] floats, one 128-row box per tile; tiles past it: zero fill
   CUtensorMap tmA, tmB;
-  cuuint64_t gstr[1] = {128};
-  cuuint32_t box[2] = {32, 128}, estr[2] = {1, 1};
-  cuuint64_t gA[2] = {32, (cuuint64_t)cdiv(M, 128) * 128 * (cuuint64_t)nkb_a};
-  cuuint64_t gB[2] = {32, (cuuint64_t)cdiv(N, 128) * 128 * (cuuint64_t)nkb_b};  // tiles past it: zero fill
-  FSN_REQUIRE(fn(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)Ablk, gA, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS &&
-                  fn(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)Bblk, gB, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS,
+  FSN_REQUIRE(make_tmap(&tmA, Ablk, tg::BK, cdiv(M, 128) * 128 * nkb_a, tg::BK, 128) &&
+                  make_tmap(&tmB, Bblk, tg::BK, cdiv(N, 128) * 128 * nkb_b, tg::BK, 128),
               FSN_ERR_CUDA, "tgemm_blocked: tensor-map encoding failed");
   int rc;
-  if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, tg::Cfg<256>::SMEM), "tgemm smem attr"))) return rc;
-  if ((rc = check_cuda(cudaFuncSetAttribute(tg::tgemm_tma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, tg::Cfg<128>::SMEM), "tgemm smem attr"))) return rc;
+  if ((rc = tgemm_smem_optin())) return rc;
   const tg::BlockedOps bo{1, nkb_a, nkb_b, a_kb0, b_kb0};
   if (BN == 256)
-    tg::tgemm_tma_kernel<256><<<grid, TGEMM_THREADS, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
+    tg::tgemm_tma_kernel<256><<<grid, TGEMM_THREADS, tg::Cfg<256>::SMEM, st>>>(tmA, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
   else
-    tg::tgemm_tma_kernel<128><<<grid, TGEMM_THREADS, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
+    tg::tgemm_tma_kernel<128><<<grid, TGEMM_THREADS, tg::Cfg<128>::SMEM, st>>>(tmA, tmB, dst, ldd, M, N, K, kps, acc, (size_t)M * N, bo);
   FSN_CHECK_LAUNCH("tgemm_tma_kernel");
   if (S > 1) return splitk_reduce_launch(scratch, S, M, N, C, ldc, accumulate, st);
   return FSN_OK;

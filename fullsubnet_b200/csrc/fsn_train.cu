@@ -590,22 +590,23 @@ int layer_forward_save(const fsn_lstm_layer& w, const float* X, int R, int K0, i
   return FSN_OK;
 }
 
-// tensor-core variant.  Default: ONE kernel per step (lstm_fwd_step_kernel, fsn_tgemm.cu): [x_t | h_{t-1}] [W_ih | W_hh]^T on
-// wgmma and the cell on its accumulators, gates / cell / hidden saved.  Fallbacks, step by step: a layer input whose rows
-// are not 16-byte aligned keeps a hoisted projection of all steps (one GEMM into the gate buffer) that the step kernel
-// adds; with the fused kernel switched off (or H % 32 != 0) every step is a recurrent GEMM into `rec` + lstm_cell_fwd_kernel
+// tensor-core variant.  H % 32 == 0: ONE kernel per step (lstm_fwd_step_kernel, fsn_tgemm.cu): [x_t | h_{t-1}] [W_ih | W_hh]^T
+// on wgmma and the cell on its accumulators, gates / cell / hidden saved.  A layer input wider than 512 or whose rows are
+// not 16-byte aligned keeps a hoisted projection of all steps (one GEMM into the gate buffer) that the step kernel adds.
+// H % 32 != 0: every step is a recurrent GEMM into `rec` + lstm_cell_fwd_kernel
 int layer_forward_save_tc(const fsn_lstm_layer& w, const float* X, int R, int K0, int H, int Tp, const LayerSave& s,
                           float* rec, cudaStream_t st, float* splitk, size_t splitk_floats, const LayerHalf* half) {
   int rc;
   const int rows = Tp * R;
-  static const int fused_min_rows = getenv("FSN_TRAIN_FUSED_MIN_ROWS") ? atoi(getenv("FSN_TRAIN_FUSED_MIN_ROWS")) : 1;
-  const bool fused = R >= fused_min_rows && lstm_fwd_step_supported(s.H, w.w_hh, H);
+  const bool fused = lstm_fwd_step_supported(s.H, w.w_hh, H);
   // x_t W_ih^T as leading k blocks of the step kernel - no hoisted projection, G is written once and never read in the
-  // forward pass (FSN_TRAIN_FOLD_K bounds the input width this is done for)
+  // forward pass
   const bool fold = fused && lstm_fwd_step_folds_input(X, w.w_ih, K0);
-  // fp16 MMA operands: h_t (written by the step kernel next to the fp32 copy) and the weights; the folded layer input too
-  // when the layer below left an fp16 copy (K0 % 8: 16-byte rows)
-  const bool h16 = fused && half && half->H16 && half->w16 && lstm_fwd_step_half_enabled(H);
+  // fp16 MMA operands when the caller passes the buffers: h_t (written by the step kernel next to the fp32 copy) and the
+  // weights, rounded to nearest (the same 11-bit significand as a tf32 read, half the bytes through L2 and twice the
+  // tensor rate); the folded layer input too when the layer below left an fp16 copy (K0 % 8: 16-byte rows).  The fp32
+  // state, the saved activations and the backward pass are unchanged
+  const bool h16 = fused && half && half->H16 && half->w16;
   const bool x16 = h16 && fold && half->X16 && (K0 % 8) == 0;
   __half* w_hh16 = h16 ? half->w16 : nullptr;
   __half* w_ih16 = x16 ? half->w16 + (size_t)4 * H * H : nullptr;
@@ -715,9 +716,8 @@ int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih,
                        float* g_b_hh, const WgradScratch& w, cudaStream_t st) {
   const int H4 = 4 * L.H;
   const int rows = Tp * L.R;
-  const bool tc = tc_bwd(L);
   int rc;
-  if (tc && tgemm_blocked_enabled()) {
+  if (tc_bwd(L)) {
     // tensor-core path, block-tiled K-major copies (one contiguous 16 KB burst per TMA box instead of 128 rows with a
     // pitch of `rows` floats): dW_ih = dG^T X, dW_hh = dG[1:]^T H[:-1]
     const int nkb = (rows + 31) / 32;
@@ -743,22 +743,6 @@ int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih,
       return rc;
     }
     return FSN_OK;
-  }
-  if (tc && (L.R & 3) == 0) {
-    // tensor-core path: K-major operands = transposed copies dG^T [4H, rows], X^T [K0, rows], H^T [H, rows]
-    if ((rc = transpose_launch(L.s.G, (size_t)rows, H4, w.gT, st))) return rc;
-    if ((rc = transpose_launch(X, (size_t)rows, L.K0, w.xT, st))) return rc;
-    if ((rc = tgemm_launch(w.gT, rows, w.xT, rows, g_w_ih, L.K0, H4, L.K0, rows, false, w.splitk, SPLITK_SCRATCH_FLOATS, st)))
-      return rc;
-    if (Tp > 1) {
-      if ((rc = transpose_launch(L.s.H, (size_t)rows, L.H, w.xT, st))) return rc;
-      if ((rc = tgemm_launch(w.gT + L.R, rows, w.xT, rows, g_w_hh, L.H, H4, L.H, rows - L.R, false, w.splitk,
-                             SPLITK_SCRATCH_FLOATS, st)))
-        return rc;
-    } else if ((rc = check_cuda(cudaMemsetAsync(g_w_hh, 0, (size_t)H4 * L.H * sizeof(float), st), "memset"))) {
-      return rc;
-    }
-    return colsum_launch(L.s.G, (size_t)rows, H4, H4, g_b_ih, g_b_hh, w.colsum, st);
   }
   if ((rc = sgemm_launch(true, L.s.G, H4, X, L.K0, g_w_ih, L.K0, H4, L.K0, rows, false, w.splitk, st))) return rc;
   if (Tp > 1) {
@@ -925,25 +909,22 @@ namespace fsn {
 // gradients are a dozen HBM-bound kernels with no dependency on it - they run side by side.  One high-priority
 // non-blocking stream and two events per device, created on first use; fork / join through events only, so the pattern
 // is also legal inside a stream capture.
-struct SideStream { cudaStream_t s; cudaEvent_t fork, join; bool ok; };
-static SideStream* side_stream() {
+struct SideStream { cudaStream_t s; cudaEvent_t fork, join; };
+static int side_stream(SideStream** out) {
   static SideStream per_dev[64] = {};
-  static bool tried[64] = {};
-  static const bool enabled = getenv("FSN_TRAIN_OVERLAP") == nullptr || atoi(getenv("FSN_TRAIN_OVERLAP")) != 0;
-  if (!enabled) return nullptr;
   int dev = 0;
   cudaGetDevice(&dev);
   SideStream& x = per_dev[dev & 63];
-  if (!tried[dev & 63]) {
-    tried[dev & 63] = true;
+  int rc;
+  if (!x.s) {  // a failed creation is retried by the next call, keeping what it did create
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    x.ok = cudaStreamCreateWithPriority(&x.s, cudaStreamNonBlocking, hi) == cudaSuccess &&
-           cudaEventCreateWithFlags(&x.fork, cudaEventDisableTiming) == cudaSuccess &&
-           cudaEventCreateWithFlags(&x.join, cudaEventDisableTiming) == cudaSuccess;
-    if (!x.ok) cudaGetLastError();
+    if ((rc = check_cuda(cudaStreamCreateWithPriority(&x.s, cudaStreamNonBlocking, hi), "side stream"))) return rc;
   }
-  return x.ok ? &x : nullptr;
+  if (!x.fork && (rc = check_cuda(cudaEventCreateWithFlags(&x.fork, cudaEventDisableTiming), "side stream event"))) return rc;
+  if (!x.join && (rc = check_cuda(cudaEventCreateWithFlags(&x.join, cudaEventDisableTiming), "side stream event"))) return rc;
+  *out = &x;
+  return FSN_OK;
 }
 }  // namespace fsn
 
@@ -980,31 +961,28 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   }
   if ((rc = colsum_launch(w.dout, (size_t)Tp * R, 2, 2, gsb->fc_b, nullptr, w.colsum, st))) return rc;
   const bool tc_fb = tf32_layer(d->precision, Hf), tc_sb = tf32_layer(d->precision, Hs);
-  // the full-band chain (second norm, full-band Linear, full-band BPTT) runs on the side stream when there is one, with its
-  // own split-K / column-sum scratch
-  SideStream* side = side_stream();
-  cudaStream_t st2 = side ? side->s : st;
-  float* splitk2 = side ? w.splitk2 : w.splitk;
-  float* colsum2 = side ? w.colsum2 : w.colsum;
+  // the full-band chain (second norm, full-band Linear, full-band BPTT) runs on the side stream st2, with its own split-K /
+  // column-sum scratch
+  SideStream* side = nullptr;
+  if ((rc = side_stream(&side))) return rc;
+  cudaStream_t st2 = side->s;
   // sub-band layers 0, 1, full-band layers 0, 1 (full-band layer 0 computes no dx)
   const LayerBwd L[4] = {
       {sb->w_ih[0], sb->w_hh[0], w.sb[0], R, K, Hs, w.dh_rec[0], w.dc[0], tc_sb ? w.sb_whhT[0] : nullptr,
        tc_sb ? w.sb_wihT[0] : nullptr, w.splitk},
       {sb->w_ih[1], sb->w_hh[1], w.sb[1], R, Hs, Hs, w.dh_rec[1], w.dc[1], tc_sb ? w.sb_whhT[1] : nullptr,
        tc_sb ? w.sb_wihT[1] : nullptr, w.splitk},
-      {fb->w_ih[0], fb->w_hh[0], w.fb[0], B, F, Hf, w.dh_rec[0], w.dc[0], tc_fb ? w.fb_whhT[0] : nullptr, nullptr, splitk2},
+      {fb->w_ih[0], fb->w_hh[0], w.fb[0], B, F, Hf, w.dh_rec[0], w.dc[0], tc_fb ? w.fb_whhT[0] : nullptr, nullptr, w.splitk2},
       {fb->w_ih[1], fb->w_hh[1], w.fb[1], B, Hf, Hf, w.dh_rec[1], w.dc[1], tc_fb ? w.fb_whhT[1] : nullptr,
-       tc_fb ? w.fb_wihT1 : nullptr, splitk2}};
+       tc_fb ? w.fb_wihT1 : nullptr, w.splitk2}};
   const LayerBwd *sbL = L, *fbL = L + 2;
   for (int l = 0; l < 4; ++l)
     if ((rc = layer_bwd_transpose_weights(L[l], st))) return rc;
   // ---- sub-band stack, both layers one step apart
   if ((rc = stack_bwd(sbL, 2, Tp, nullptr, w.dout, sb->fc_w, 2, w.dh_mid, nullptr, w.dxsb, st))) return rc;
   // ---- fork: sub-band weight gradients on the caller's stream, the rest of the chain on st2
-  if (side) {
-    if ((rc = check_cuda(cudaEventRecord(side->fork, st), "event record"))) return rc;
-    if ((rc = check_cuda(cudaStreamWaitEvent(side->s, side->fork, 0), "stream wait"))) return rc;
-  }
+  if ((rc = check_cuda(cudaEventRecord(side->fork, st), "event record"))) return rc;
+  if ((rc = check_cuda(cudaStreamWaitEvent(st2, side->fork, 0), "stream wait"))) return rc;
   const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
   if ((rc = layer_weight_grads(sbL[1], Tp, w.sb[0].H, gsb->w_ih[1], gsb->w_hh[1], gsb->b_ih[1], gsb->b_hh[1], wg, st)))
     return rc;
@@ -1022,14 +1000,13 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
                                                 d->fb_activation, w.dz);
     FSN_CHECK_LAUNCH("train_dfbz_kernel");
   }
-  if ((rc = linear_bwd(w.dz, w.fb[1].H, fb->fc_w, Tp * B, F, Hf, gfb->fc_w, gfb->fc_b, w.dfh1, splitk2, colsum2, st2)))
+  if ((rc = linear_bwd(w.dz, w.fb[1].H, fb->fc_w, Tp * B, F, Hf, gfb->fc_w, gfb->fc_b, w.dfh1, w.splitk2, w.colsum2, st2)))
     return rc;
   // ---- full-band stack
   if ((rc = stack_bwd(fbL, 2, Tp, w.dfh1, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st2))) return rc;
-  if (side) {  // join: the full-band weight gradients share gT / xT / splitk / colsum with the sub-band ones
-    if ((rc = check_cuda(cudaEventRecord(side->join, side->s), "event record"))) return rc;
-    if ((rc = check_cuda(cudaStreamWaitEvent(st, side->join, 0), "stream wait"))) return rc;
-  }
+  // join: the full-band weight gradients share gT / xT / splitk / colsum with the sub-band ones
+  if ((rc = check_cuda(cudaEventRecord(side->join, st2), "event record"))) return rc;
+  if ((rc = check_cuda(cudaStreamWaitEvent(st, side->join, 0), "stream wait"))) return rc;
   if ((rc = layer_weight_grads(fbL[1], Tp, w.fb[0].H, gfb->w_ih[1], gfb->w_hh[1], gfb->b_ih[1], gfb->b_hh[1], wg, st)))
     return rc;
   return layer_weight_grads(fbL[0], Tp, w.xfb, gfb->w_ih[0], gfb->w_hh[0], gfb->b_ih[0], gfb->b_hh[0], wg, st);

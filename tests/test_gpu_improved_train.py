@@ -189,18 +189,3 @@ def test_error_behaviour(dev):
     gru = Model(**dict(IO.DEFAULT_IMPROVED_ARGS, **SMALL_256, sequence_model="GRU")).to(dev).train()
     with pytest.raises(NotImplementedError):
         gru(y)
-
-
-def test_unfused_training_paths_in_a_subprocess():
-    """The fallbacks behind the fused step kernel and the block-tiled weight-gradient operands (environment switches, read
-    once per process): the tf32 golden steps of the unmodified reference still pass."""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, FSN_TRAIN_FUSED_FWD="0", FSN_TGEMM_BLOCKED="0")
-    out = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_gpu_improved_train.py"), "-m", "gpu",
-                          "-x", "-q", "-k", "two_golden_steps_match_reference and True-tf32_tc"],
-                         env=env, capture_output=True, text=True, timeout=900, cwd=root)
-    assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-1000:]
-    assert " passed" in out.stdout and "failed" not in out.stdout, out.stdout[-1000:]

@@ -1,5 +1,5 @@
-"""Times the tf32 wgmma GEMM on the shapes of the training step (config 3): python tools/tgemm_shapes.py
-(FSN_TGEMM_BN / FSN_TGEMM_SMALLK_BN select tile widths per process)."""
+"""Times the tf32 wgmma GEMM on the shapes of the training step (config 3), with the tile width and split-K count
+tgemm_launch picks for each shape: python tools/tgemm_shapes.py"""
 import sys
 
 import torch
