@@ -178,6 +178,9 @@ _SIGNATURES = {
     "fsn_debug_lstm_train_workspace_bytes": (_S, [_I, _I, _I, _I, _I, _I]),
     "fsn_debug_lstm_train": (C.c_int, [C.POINTER(LstmLayer), _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P,
                                        C.POINTER(LstmGrads), _P, _P, _S, _P]),
+    "fsn_debug_seq_stack_workspace_bytes": (_S, [_I, C.POINTER(C.c_int), _I, _I, _I, _I, _I, _I, _I, _I]),
+    "fsn_debug_seq_stack": (C.c_int, [C.POINTER(LstmLayer), _I, C.POINTER(C.c_int), _I, _I, _I, _I, _I, _I, _I, _I, _P, _P,
+                                      _P, _P, _I, _I, _P, _P, _S, C.POINTER(C.c_int), _P]),
     "fsn_last_error_code": (C.c_int, []),
     "fsn_last_launch_count": (C.c_int64, []),
     "fsn_total_launch_count": (C.c_int64, []),

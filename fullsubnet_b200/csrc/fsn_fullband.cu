@@ -110,6 +110,11 @@ __global__ void __launch_bounds__(THREADS, 1) fb_lstm_kernel(const Args a) {
     }
     W1[idx] = w;
   }
+  // the A tiles' padding columns [KC, RS) are never loaded.  When H1 % KC != 0 the last chunk of the h1 segment reads
+  // weight rows past W1, i.e. the start of the first tile, and multiplies them by zero-filled A: zero the padding once so
+  // that stale shared memory (an Inf or NaN) cannot turn those products into NaN
+  for (int idx = tid; idx < NSTAGE * ROWS; idx += THREADS)
+    *reinterpret_cast<float4*>(At + (size_t)idx * RS + KC) = make_float4(0.f, 0.f, 0.f, 0.f);
   float bias0[4], bias1[4];
 #pragma unroll
   for (int g = 0; g < 4; ++g) {
@@ -326,12 +331,21 @@ void seq_stack_carve(Carver& c, const SeqStack& s, SeqStackWs& w) {
   }
 }
 
+SeqPath seq_stack_path(const SeqStack& s) {
+  static const bool env_stepwise = getenv("FSN_FB_STEPWISE") != nullptr;  // debug: force the per-step kernels
+  const bool stepwise = env_stepwise || s.force_stepwise;
+  if (s.tc && !stepwise) return SEQ_PATH_TC;
+  if (s.n < 2) return SEQ_PATH_ONE_LAYER;
+  if (!stepwise && !s.gru && !s.step_scale && fb_persistent_supported(s.K0, s.H[0], s.H[1])) return SEQ_PATH_PERSISTENT;
+  return SEQ_PATH_STEP2;
+}
+
 int seq_stack_forward(const SeqStack& s, const SeqStackWs& w, cudaStream_t st) {
-  static const bool stepwise = getenv("FSN_FB_STEPWISE") != nullptr;  // debug: force the per-step kernels
+  const SeqPath path = seq_stack_path(s);
   const int R = s.R, Tp = s.Tp, n = s.n, Ht = s.H[n - 1];
   auto hall = [&](int l) { return w.hall[(n - 1 - l) & 1]; };  // output of layer l, [R, Tp, H[l]]; the top one in hall[0]
   int rc;
-  if (s.tc && !stepwise) {
+  if (path == SEQ_PATH_TC) {
     // per layer one hoisted input-projection GEMM + the persistent wgmma recurrence; the Linear on the same GEMM
     for (int l = 0; l < n; ++l) {
       const int K = l ? s.H[l - 1] : s.K0;
@@ -355,11 +369,11 @@ int seq_stack_forward(const SeqStack& s, const SeqStackWs& w, cudaStream_t st) {
     return p;
   };
   int l = 0;  // first layer left for the single-layer loop
-  if (!stepwise && n >= 2 && !s.gru && !s.step_scale && fb_persistent_supported(s.K0, s.H[0], s.H[1])) {
+  if (path == SEQ_PATH_PERSISTENT) {
     // weights resident in shared memory, layer wavefront, one grid barrier per time step
     if ((rc = fb_persistent_launch(s.L, s.x, s.scale, w.pp, hall(1), w.barrier, R, s.K0, s.H[0], s.H[1], Tp, st))) return rc;
     l = 2;
-  } else if (n >= 2) {
+  } else if (path == SEQ_PATH_STEP2) {
     const Step2State s2{{w.h0[0], w.h0[1]}, w.c0, {hall(1), nullptr}, w.c1, s.H[1], Tp};
     for (int t = 0; t < Tp; ++t)
       if ((rc = lstm_step2_launch(step(0, t), SEG0_DENSE, t, s.L[1], s2, st))) return rc;
@@ -378,4 +392,64 @@ int seq_stack_forward(const SeqStack& s, const SeqStackWs& w, cudaStream_t st) {
   return fc_gemm_launch(hall(n - 1), s.fc_w, s.fc_b, s.out, R * Tp, Ht, s.O, s.act, st);
 }
 
+// shape checks of the unit-test hook (host only) and its SeqStack; pointers and the tensor-core rule are the hook's
+static int dbg_seq_stack(int n, const int* H, int R, int Tp, int K0, int gru, int step_scale, int tc, int x3, int O,
+                         SeqStack& s) {
+  FSN_REQUIRE(n >= 1 && n <= SEQ_MAX_LAYERS, FSN_ERR_UNSUPPORTED, "seq_stack hook: 1..%d layers (got %d)", SEQ_MAX_LAYERS, n);
+  FSN_REQUIRE(H, FSN_ERR_SHAPE, "seq_stack hook: null hidden sizes");
+  FSN_REQUIRE(R > 0 && Tp > 0 && K0 > 0 && O > 0, FSN_ERR_SHAPE, "seq_stack hook: bad dims R=%d Tp=%d K0=%d O=%d", R, Tp, K0, O);
+  int Hm = K0 > O ? K0 : O;
+  for (int l = 0; l < n; ++l) {
+    FSN_REQUIRE(H[l] > 0, FSN_ERR_SHAPE, "seq_stack hook: hidden size of layer %d is %d", l, H[l]);
+    Hm = H[l] > Hm ? H[l] : Hm;
+  }
+  FSN_REQUIRE((size_t)R * Tp * 4 * Hm < ((size_t)1 << 31), FSN_ERR_SHAPE, "seq_stack hook: R*Tp*4*max(K0,H,O) must stay below 2^31");
+  FSN_REQUIRE(!(tc && gru), FSN_ERR_UNSUPPORTED, "seq_stack hook: the tensor-core stack has no GRU cell");
+  memset(&s, 0, sizeof(s));
+  s.R = R; s.Tp = Tp; s.K0 = K0; s.n = n; s.O = O;
+  for (int l = 0; l < n; ++l) s.H[l] = H[l];
+  s.gru = gru != 0; s.step_scale = step_scale != 0; s.tc = tc != 0; s.x3 = x3 != 0;
+  return FSN_OK;
+}
+
 }  // namespace fsn
+
+using namespace fsn;
+
+extern "C" size_t fsn_debug_seq_stack_workspace_bytes(int n, const int* H, int R, int Tp, int K0, int gru, int step_scale, int tc,
+                                                      int x3, int O) {
+  SeqStack s;
+  if (dbg_seq_stack(n, H, R, Tp, K0, gru, step_scale, tc, x3, O, s)) return 0;
+  Carver c(nullptr);
+  SeqStackWs w;
+  seq_stack_carve(c, s, w);
+  return c.off;
+}
+
+extern "C" int fsn_debug_seq_stack(const fsn_lstm_layer* layers, int n, const int* H, int R, int Tp, int K0, int gru,
+                                   int step_scale, int tc, int x3, int force_stepwise, const float* x, const float* scale,
+                                   const float* fc_w, const float* fc_b, int O, int act, float* out, void* workspace,
+                                   size_t workspace_bytes, int* path, fsn_stream_t stream) {
+  launch_counter() = 0;
+  SeqStack s;
+  int rc = dbg_seq_stack(n, H, R, Tp, K0, gru, step_scale, tc, x3, O, s);
+  if (rc) return rc;
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "seq_stack hook: unknown activation %d", act);
+  FSN_REQUIRE(layers && x && fc_w && fc_b && out, FSN_ERR_SHAPE, "seq_stack hook: null argument");
+  for (int l = 0; l < n; ++l) {
+    FSN_REQUIRE(layers[l].w_ih && layers[l].w_hh && layers[l].b_ih && layers[l].b_hh, FSN_ERR_SHAPE,
+                "seq_stack hook: null weight of layer %d", l);
+    FSN_REQUIRE(!tc || lstm_rec_tc_supported(H[l], x3 != 0), FSN_ERR_UNSUPPORTED,
+                "seq_stack hook: hidden size %d of layer %d is not supported on the tensor cores", H[l], l);
+    s.L[l] = layers[l];
+  }
+  SeqStackWs w;
+  Carver c(workspace);
+  seq_stack_carve(c, s, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes,
+              c.off);
+  s.act = act; s.force_stepwise = force_stepwise != 0;
+  s.x = x; s.scale = scale; s.fc_w = fc_w; s.fc_b = fc_b; s.out = out;
+  if (path) *path = seq_stack_path(s);
+  return seq_stack_forward(s, w, (cudaStream_t)stream);
+}

@@ -328,17 +328,29 @@ int gemm_tc_split_launch(const float* a, size_t lda, const float* W, int N, int 
 // One SequenceModel of the inference forwards over clip-major rows (sequence_model.py:106-125, fsn_fullband.cu): n LSTM
 // (or GRU) layers over x [R, Tp, K0] (contiguous; times scale[r], or scale[t*R + r] with step_scale), then Linear(H[n-1]
 // -> O) + act into out [R*Tp, O].  tc / x3 are the caller's rule for running the stack on the tensor cores
-// (lstm_layer_tc + linear_tc, x3: hi+lo compensated).  Otherwise, or under FSN_FB_STEPWISE, layers 0-1 run on the
-// persistent kernel when it fits (LSTM, no per-step scale), everything else on the per-step kernels, then fc_gemm.
+// (lstm_layer_tc + linear_tc, x3: hi+lo compensated).  Otherwise, or under FSN_FB_STEPWISE / force_stepwise, layers 0-1
+// run on the persistent kernel when it fits (LSTM, no per-step scale, not forced per-step), everything else on the
+// per-step kernels, then fc_gemm.
 static const int SEQ_MAX_LAYERS = 8;
 struct SeqStack {
   int R, Tp, K0, n, O, act;
   int H[SEQ_MAX_LAYERS];
   fsn_lstm_layer L[SEQ_MAX_LAYERS];
   bool gru, step_scale, tc, x3;
+  bool force_stepwise;  // the per-step kernels for every layer, as FSN_FB_STEPWISE (the unit-test hook sets it)
   const float *x, *scale, *fc_w, *fc_b;
   float* out;
 };
+// the path seq_stack_forward takes for a stack (values of fsn_debug_seq_stack's *path): tensor cores; layers 0-1 on the
+// persistent kernel; layers 0-1 two per-step launches per step (lstm_step2_launch); one layer on the per-step kernel.
+// Layers past the first two run the per-step kernel on every path but the tensor-core one.
+enum SeqPath {
+  SEQ_PATH_TC = FSN_SEQ_PATH_TC,
+  SEQ_PATH_PERSISTENT = FSN_SEQ_PATH_PERSISTENT,
+  SEQ_PATH_STEP2 = FSN_SEQ_PATH_STEP2,
+  SEQ_PATH_ONE_LAYER = FSN_SEQ_PATH_ONE_LAYER
+};
+SeqPath seq_stack_path(const SeqStack& s);
 // layer outputs for every step (hall[0]: top layer), per-step state, persistent-kernel scratch, tensor-core workspace
 struct SeqStackWs {
   float *hall[2], *h0[2], *c0, *c1, *pp;

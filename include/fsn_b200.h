@@ -546,6 +546,22 @@ int fsn_debug_lstm_train(const fsn_lstm_layer* layers, int n_layers, int R, int 
                          float* dx, const fsn_lstm_grads* g, float* trace, void* workspace, size_t workspace_bytes,
                          fsn_stream_t stream);
 
+/* unit-test hook for the SequenceModel every inference forward runs its clip-major LSTM stacks through (seq_stack_forward,
+ * fsn_fullband.cu; audio_zen/model/module/sequence_model.py:106-125): n layers (1..8; LSTM, or GRU with gru != 0) of hidden
+ * sizes H[0..n-1] over x [R, Tp, K0] (layer l maps H[l-1] -> H[l]), the layer-0 input times scale[r] (scale [R]) or, with
+ * step_scale, scale[t*R + r] (scale [Tp, R]); scale nullable.  Then Linear(H[n-1] -> O) + act (FSN_ACT_*) into
+ * out [R, Tp, O].  tc != 0 asks for the tensor-core stack (x3 != 0: compensated) as the model files do: LSTM only, and every
+ * H must be supported there (else FSN_ERR_UNSUPPORTED).  force_stepwise != 0 runs the per-step kernels as
+ * FSN_FB_STEPWISE does.  *path (nullable) receives the FSN_SEQ_PATH_* the stack ran on.  Arguments are checked before any
+ * CUDA call; the workspace query needs no GPU. */
+enum { FSN_SEQ_PATH_TC = 0, FSN_SEQ_PATH_PERSISTENT = 1, FSN_SEQ_PATH_STEP2 = 2, FSN_SEQ_PATH_ONE_LAYER = 3 };
+size_t fsn_debug_seq_stack_workspace_bytes(int n, const int* H, int R, int Tp, int K0, int gru, int step_scale, int tc, int x3,
+                                           int O);
+int fsn_debug_seq_stack(const fsn_lstm_layer* layers, int n, const int* H, int R, int Tp, int K0, int gru, int step_scale,
+                        int tc, int x3, int force_stepwise, const float* x, const float* scale, const float* fc_w,
+                        const float* fc_b, int O, int act, float* out, void* workspace, size_t workspace_bytes, int* path,
+                        fsn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
