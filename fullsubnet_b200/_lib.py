@@ -36,7 +36,7 @@ class LstmLayer(C.Structure):
 class FastDesc(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "num_freqs", "look_ahead", "shrink_size", "num_mels", "enc1_hidden", "enc2_hidden", "bn_hidden", "bn_layers",
-        "dec_hidden", "noisy_num_neighbors", "enc_num_neighbors", "precision", "cell_type")]
+        "dec_hidden", "noisy_num_neighbors", "enc_num_neighbors", "precision", "cell_type", "norm_type")]
 
 
 class FastWeights(C.Structure):

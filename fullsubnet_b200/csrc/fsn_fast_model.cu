@@ -42,6 +42,29 @@ __global__ void fast_bn_input_kernel(const float* __restrict__ melT, const float
   if (threadIdx.x == 0) fs[(size_t)b * Ts + ts] = make_float2(red[0], red[0]);
 }
 
+// second cumulative norm (model.py:186-187 -> base_model.py:220-251 on [B*M, K, Ts]): one thread per row (b,m), sequential
+// over the shrunk steps; the row sum of each step runs over the K block means fast_bn_input_kernel / ftr_bn_input_kernel
+// wrote, so inference and training share the scales
+__global__ void fast_cum_bn_scale_kernel(const float* __restrict__ bn, int R, int K, int Ts, float eps,
+                                         float* __restrict__ scaleT) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  float run = 0.f;
+  for (int ts = 0; ts < Ts; ++ts) {
+    const float* x = bn + ((size_t)ts * R + r) * K;
+    float s = 0.f;
+    for (int k = 0; k < K; ++k) s += x[k];
+    run += s;
+    scaleT[(size_t)ts * R + r] = 1.0f / (run / ((float)K * (float)(ts + 1)) + eps);
+  }
+}
+
+int fast_cum_bn_scale_launch(const float* bn, int R, int K, int Ts, float eps, float* scaleT, cudaStream_t st) {
+  fast_cum_bn_scale_kernel<<<cdiv(R, 128), 128, 0, st>>>(bn, R, K, Ts, eps, scaleT);
+  FSN_CHECK_LAUNCH("fast_cum_bn_scale_kernel");
+  return FSN_OK;
+}
+
 // decoder input (model.py:194): [enc_out (M) | up-sampled bottleneck output (M)] per (b,t); frame t of the
 // up-sampled signal is shrunk frame t / S (model.py:131-140)
 // bn_out element (b, m, ts) lives at bn_out[(b*bn_bstride + m) * Ts + ts]: bn_bstride = M for the fp32 path
@@ -88,6 +111,7 @@ static bool fast_x3(const fsn_fast_desc* d) { return d->precision == FSN_PREC_F1
 
 struct FastWs {
   float *magT, *melT, *encT, *bn, *bn_out, *dec_in, *dec_out, *inv1, *inv2;
+  float *cum1, *cum2;  // cumulative norm: scales of (frame, clip) [Tp, B] and of (shrunk step, row) [Ts, B*M]
   float2 *fs, *sums;
   float *bn_h0[2], *bn_h1[2], *bn_c0, *bn_c1;
   SeqStackWs seq;          // encoder and decoder LSTM pairs, one after the other
@@ -113,6 +137,8 @@ int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m) {
               "fast model: bad descriptor");
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "fast model: empty input (B=%d, T=%d)", B, T);
   FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "fast model: the GRU cell is not built");
+  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, FSN_ERR_UNSUPPORTED,
+              "fast model: norm_type %d is not built", d->norm_type);
   FSN_REQUIRE(d->bn_layers == 2, FSN_ERR_UNSUPPORTED, "fast model: bottleneck_num_layers must be 2 in this build");
   FSN_REQUIRE(d->noisy_num_neighbors < d->num_mels && d->enc_num_neighbors < d->num_mels, FSN_ERR_SHAPE,
               "fast model: reflect padding needs num_neighbors < num_mels");
@@ -120,6 +146,7 @@ int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m) {
   m.K = (2 * d->noisy_num_neighbors + 1) + (2 * d->enc_num_neighbors + 1);
   FSN_REQUIRE(m.Tp >= 2, FSN_ERR_SHAPE, "fast model: needs at least 2 frames incl. look-ahead");
   m.Ts = 1 + cdiv(m.Tp - 1, m.S);
+  m.cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
   return FSN_OK;
 }
 
@@ -137,6 +164,11 @@ static void fast_carve(const fsn_fast_desc* d, const FastDims& m, void* base, Fa
   w.inv2 = c.take<float>(m.B);
   w.fs = c.take<float2>(BT);
   w.sums = c.take<float2>(m.B);
+  w.cum1 = w.cum2 = nullptr;
+  if (m.cum) {
+    w.cum1 = c.take<float>(BT);
+    w.cum2 = c.take<float>((size_t)m.Ts * R);
+  }
   if (!fast_is_tc(d)) {
     for (int i = 0; i < 2; ++i) { w.bn_h0[i] = c.take<float>(R * d->bn_hidden); w.bn_h1[i] = c.take<float>(R * d->bn_hidden); }
     w.bn_c0 = c.take<float>(R * d->bn_hidden);
@@ -188,21 +220,32 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   if ((rc = transpose_mag_launch(mix_mag, w.magT, B, F, T, Tp, st))) return rc;
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, B * Tp, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true)))
     return rc;
-  // encoder input norm (model.py:170): per-clip mean of the mel spectrogram incl. the look-ahead frames
+  // encoder input norm (model.py:170): per-clip mean of the mel spectrogram incl. the look-ahead frames, or (cumulative
+  // norm) the running mean over the mel bins of the frames so far, time-major cum1[t*B + b] (base_model.py:220-251)
   if ((rc = clip_stats_launch(w.melT, B, Tp, M, 0, w.fs, w.sums, st))) return rc;
-  if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) return rc;
+  if (m.cum) {
+    if ((rc = cum_clip_scale_launch(w.fs, B, Tp, M, TRAIN_CUM_EPS, w.cum1, st))) return rc;
+  } else if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) {
+    return rc;
+  }
   // F_l2m: LSTM(M->He1), LSTM(He1->He2) + Linear(M) + ReLU (model.py:35-54,171)
   SeqStack enc = fast_pair(d, m, M, d->enc1_hidden, d->enc2_hidden, M, FSN_ACT_RELU);
   enc.L[0] = wt->enc1; enc.L[1] = wt->enc2;
-  enc.x = w.melT; enc.scale = w.inv1; enc.fc_w = wt->enc_fc_w; enc.fc_b = wt->enc_fc_b; enc.out = w.encT;
+  enc.x = w.melT; enc.scale = m.cum ? w.cum1 : w.inv1; enc.step_scale = m.cum;
+  enc.fc_w = wt->enc_fc_w; enc.fc_b = wt->enc_fc_b; enc.out = w.encT;
   if ((rc = seq_stack_forward(enc, w.seq, st))) return rc;
   // bottleneck input: unfold + concat + real-time down-sampling, then its norm (model.py:174-187)
   fast_bn_input_kernel<<<B * m.Ts, 256, 0, st>>>(w.melT, w.encT, B, Tp, M, d->noisy_num_neighbors,
                                                  d->enc_num_neighbors, m.S, m.Ts, w.bn, w.fs);
   FSN_CHECK_LAUNCH("fast_bn_input_kernel");
-  // per-clip sum of the per-(b,ts) partials (fixed order), then 1/(mean+1e-5)
-  if ((rc = clip_reduce_only_launch(w.fs, B, m.Ts, w.sums, st))) return rc;
-  if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)M * m.K * m.Ts, 1.f, w.inv2, nullptr, st))) return rc;
+  if (m.cum) {
+    // per-(shrunk step, row) running mean over the K block means, time-major cum2[ts*R + r]
+    if ((rc = fast_cum_bn_scale_launch(w.bn, R, m.K, m.Ts, TRAIN_CUM_EPS, w.cum2, st))) return rc;
+  } else {
+    // per-clip sum of the per-(b,ts) partials (fixed order), then 1/(mean+1e-5)
+    if ((rc = clip_reduce_only_launch(w.fs, B, m.Ts, w.sums, st))) return rc;
+    if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)M * m.K * m.Ts, 1.f, w.inv2, nullptr, st))) return rc;
+  }
   // S: 2xLSTM(K->Hb->Hb) + Linear(1) + ReLU on B*M rows over Ts steps (model.py:188-189)
   const int Hb = d->bn_hidden;
   int bn_bstride = M;
@@ -213,7 +256,9 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
                 "fast model: the tensor-core precisions need packed bottleneck weights, bn_hidden = 384 and input width <= 32");
     SbTcArgs a;
     memset(&a, 0, sizeof(a));
+    // cumulative norm: unit_scale replaces inv2[clip] (which the kernel still loads, unwritten and unused)
     a.packed = wt->bn_packed; a.magT = w.melT; a.fbT = w.encT; a.inv2 = w.inv2; a.crm = w.bn_out;
+    a.unit_scale = m.cum ? w.cum2 : nullptr;
     a.B = B; a.F = M; a.Tp = Tp; a.la = 0; a.Ns = d->noisy_num_neighbors; a.Nf = d->enc_num_neighbors;
     a.H = Hb; a.act = FSN_ACT_RELU; a.steps = m.Ts; a.shrink = m.S; a.x3 = fast_x3(d);
     a.map = RowMap{B, M, M, 1};
@@ -226,7 +271,9 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
       memset(&p, 0, sizeof(p));
       p.R = R; p.K0 = m.K; p.H = Hb;
       p.w_ih = wt->bn[0].w_ih; p.w_hh = wt->bn[0].w_hh; p.b_ih = wt->bn[0].b_ih; p.b_hh = wt->bn[0].b_hh;
-      p.x0 = w.bn + (size_t)t * R * m.K; p.x0_row_stride = m.K; p.row_scale = w.inv2; p.row_scale_div = M;
+      p.x0 = w.bn + (size_t)t * R * m.K; p.x0_row_stride = m.K;
+      if (m.cum) { p.row_scale = w.cum2 + (size_t)t * R; p.row_scale_div = 1; }
+      else       { p.row_scale = w.inv2; p.row_scale_div = M; }
       if ((rc = lstm_step2_launch(p, SEG0_DENSE, t, wt->bn[1], s2, st))) return rc;
       if ((rc = rows_fc_launch(s2.h1_at(t), R, Hb, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out + t, (size_t)m.Ts, 0,
                                st)))

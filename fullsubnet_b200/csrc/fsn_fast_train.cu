@@ -1,7 +1,8 @@
 // Training step of fast_fullsubnet (recipes/dns_interspeech_2020/fast_fullsubnet/trainer.py:45-56, model.py:143-202):
 //   fsn_fast_train_forward   Model.forward in train mode, keeping what back-propagation through time needs
 //   fsn_fast_train_backward  Linear(2F) -> decoder BPTT -> up-sampling transpose -> ReLU' -> bottleneck BPTT -> second
-//                            norm + down-sampling + unfold (closed form, gather) -> ReLU' -> Linear(M) -> encoder BPTT;
+//                            norm + down-sampling + unfold (closed form, gather; cumulative norm: per-row suffix sums
+//                            over the shrunk steps) -> ReLU' -> Linear(M) -> encoder BPTT;
 //                            weight gradients of every LSTM layer through layer_weight_grads (fsn_train.cu)
 // Everything is time-major ([Tp, rows, .], the bottleneck [Ts, B*M, .]) like fsn_train.cu, so the LSTM layers reuse its
 // activation-saving forward, its per-step backward and its weight-gradient GEMMs.  Every reduction runs in a fixed order:
@@ -106,10 +107,14 @@ __global__ void ftr_dbn_kernel(const float* __restrict__ ddec, const float* __re
 // d encT [Tp,B,M] = ReLU'(encT) * ( ddec[t,b,m] (decoder input, columns < M)
 //   + inv2[b] * sum_{(m',k) : reflect(m' + k - Ne) = m} dX[ts(t), b*M+m', 2Nn+1+k] / len(ts)    (unfold^T . down-sampling^T)
 //   - inv2[b] * dot[b] * c_Ne[m] / (M K Ts len(ts)) )                                           (second-norm backward)
-// gather form: the (m', k) pairs of m are the direct, left-reflected and right-reflected sources of each offset k - Ne
+// gather form: the (m', k) pairs of m are the direct, left-reflected and right-reflected sources of each offset k - Ne.
+// CUM (cumulative norm, scaleT / suffix [Ts, B*M]): each source term is the gradient of the block mean u[ts, r', k],
+//   dX[ts, r', k] s[ts, r'] + suffix[ts, r'], divided by len(ts), and there is no per-clip term
+template <bool CUM>
 __global__ void ftr_denc_kernel(const float* __restrict__ ddec, const float* __restrict__ dX, const float* __restrict__ encT,
-                                const float* __restrict__ inv2, const float* __restrict__ dot, int B, int Tp, int M, int Nn,
-                                int Ne, int S, float cnt2, float* __restrict__ denc) {
+                                const float* __restrict__ inv2, const float* __restrict__ dot, const float* __restrict__ scaleT,
+                                const float* __restrict__ suffix, int B, int Tp, int M, int Nn, int Ne, int S, float cnt2,
+                                float* __restrict__ denc) {
   const int K = (2 * Nn + 1) + (2 * Ne + 1);
   const size_t n = (size_t)Tp * B * M;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -120,19 +125,45 @@ __global__ void ftr_denc_kernel(const float* __restrict__ ddec, const float* __r
     int t0, len;
     shrink_block(ts, S, Tp, t0, len);
     const float* dx = dX + ((size_t)ts * B * M + (size_t)b * M) * K + (2 * Nn + 1);
+    const size_t row0 = (size_t)ts * B * M + (size_t)b * M;  // scaleT / suffix index of (ts, row b*M)
+    auto term = [&](int src, int k) {
+      return CUM ? fmaf(dx[(size_t)src * K + k], scaleT[row0 + src], suffix[row0 + src]) : dx[(size_t)src * K + k];
+    };
     float acc = 0.f;
     for (int k = 0; k <= 2 * Ne; ++k) {
       const int o = k - Ne;
       int src = m - o;                                        // m' + o = m
-      if (src >= 0 && src < M) acc += dx[(size_t)src * K + k];
+      if (src >= 0 && src < M) acc += term(src, k);
       src = -m - o;                                           // m' + o = -m < 0
-      if (m > 0 && src >= 0 && src < M) acc += dx[(size_t)src * K + k];
+      if (m > 0 && src >= 0 && src < M) acc += term(src, k);
       src = 2 * (M - 1) - m - o;                              // m' + o = 2(M-1) - m >= M
-      if (m < M - 1 && src >= 0 && src < M) acc += dx[(size_t)src * K + k];
+      if (m < M - 1 && src >= 0 && src < M) acc += term(src, k);
+    }
+    if (CUM) {
+      const float v = ddec[tb * 2 * M + m] + acc / (float)len;
+      denc[i] = encT[i] > 0.f ? v : 0.f;
+      continue;
     }
     const float s = inv2[b], fl = (float)len;
     float v = ddec[tb * 2 * M + m] + s * acc / fl - s * dot[b] * (float)reflect_count(m, M, Ne) / (cnt2 * fl);
     denc[i] = encT[i] > 0.f ? v : 0.f;
+  }
+}
+
+// backward of the second cumulative norm X[ts,r,k] = u[ts,r,k] s[ts,r] (fast_cum_bn_scale_launch):
+//   d u[ts,r,k] = dX[ts,r,k] s[ts,r] + suffix[ts,r],  suffix[ts,r] = sum_{ts'' >= ts} -s[ts'',r] <dX[ts'',r,:], X[ts'',r,:]> /
+//   (K (ts''+1)).  One thread per row, sequential in ts (fixed order); ftr_denc_kernel<true> maps d u back to the encoder
+__global__ void ftr_cum_suffix_kernel(const float* __restrict__ dX, const float* __restrict__ X, const float* __restrict__ scaleT,
+                                      int Ts, int R, int K, float* __restrict__ suffix) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  float acc = 0.f;
+  for (int ts = Ts - 1; ts >= 0; --ts) {
+    const size_t o = ((size_t)ts * R + r) * K;
+    float dot = 0.f;
+    for (int k = 0; k < K; ++k) dot = fmaf(dX[o + k], X[o + k], dot);
+    acc += -scaleT[(size_t)ts * R + r] * dot / ((float)K * (float)(ts + 1));
+    suffix[(size_t)ts * R + r] = acc;
   }
 }
 
@@ -143,6 +174,10 @@ struct FastTrainWs {
   float *magT, *melT, *xenc, *encT, *xbn, *bn_out, *dec_in, *dec_out;
   float *inv1, *inv2, *dot;
   float2 *sums1, *sums2, *fs;
+  // cumulative norm: frame sums of the mel spectrogram [B*Tp], scales of (frame, clip) [Tp, B] and of (shrunk step, row)
+  // [Ts, B*M] (kept for the backward), suffix sums of the second norm's backward [Ts, B*M]
+  float2* fs1;
+  float *cum1, *cum2, *suffix;
   LayerSave L[NL];
   float *dY, *dH, *ddec, *dbn, *dxbn, *denc;
   float *dh_rec[2], *dc[2], *dh_mid;
@@ -222,6 +257,14 @@ static void carve_fast_train(const fsn_fast_desc* d, const FastDims& m, void* ba
     w.rec = c.take<float>(4 * rh);
     w.w16 = c.take<__half>(wmax);
   }
+  w.fs1 = nullptr;
+  w.cum1 = w.cum2 = w.suffix = nullptr;
+  if (m.cum) {
+    w.fs1 = c.take<float2>(B * Tp);
+    w.cum1 = c.take<float>(Tp * B);
+    w.cum2 = c.take<float>(Ts * R);
+    w.suffix = c.take<float>(Ts * R);
+  }
   w.bytes = c.off;
 }
 
@@ -292,12 +335,21 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   ftr_transpose_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(mix_mag, w.magT, B, F, T, Tp);
   FSN_CHECK_LAUNCH("ftr_transpose_kernel");
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, Tp * B, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true))) return rc;
-  // first norm (model.py:170): the mel spectrogram has no parameter behind it, only the normalised copy is kept
-  train_tm_stats_kernel<<<B, 256, 0, st>>>(w.melT, B, M, Tp, 0, w.sums1);
-  FSN_CHECK_LAUNCH("train_tm_stats_kernel");
-  if ((rc = norm_scales_launch(w.sums1, w.sums1, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) return rc;
-  ftr_scale_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.melT, w.inv1, (size_t)Tp * B * M, M, B, 1, w.xenc);
-  FSN_CHECK_LAUNCH("ftr_scale_kernel");
+  // first norm (model.py:170): the mel spectrogram has no parameter behind it, only the normalised copy is kept;
+  // cumulative norm: one scale per (frame, clip) from the running mean over the mel bins
+  if (m.cum) {
+    train_frame_sum_kernel<<<cdiv(Tp * B, 8), 256, 0, st>>>(w.melT, B, M, Tp, w.fs1);
+    FSN_CHECK_LAUNCH("train_frame_sum_kernel");
+    if ((rc = cum_clip_scale_launch(w.fs1, B, Tp, M, TRAIN_CUM_EPS, w.cum1, st))) return rc;
+    train_scale_tm_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.melT, w.cum1, M, (size_t)Tp * B * M, w.xenc);
+    FSN_CHECK_LAUNCH("train_scale_tm_kernel");
+  } else {
+    train_tm_stats_kernel<<<B, 256, 0, st>>>(w.melT, B, M, Tp, 0, w.sums1);
+    FSN_CHECK_LAUNCH("train_tm_stats_kernel");
+    if ((rc = norm_scales_launch(w.sums1, w.sums1, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) return rc;
+    ftr_scale_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.melT, w.inv1, (size_t)Tp * B * M, M, B, 1, w.xenc);
+    FSN_CHECK_LAUNCH("ftr_scale_kernel");
+  }
   // encoder: LSTM(M->He1), LSTM(He1->He2) + Linear(M) + ReLU (model.py:35-54,171)
   if ((rc = layer(L_ENC1, w.xenc, nullptr))) return rc;
   if ((rc = layer(L_ENC2, w.L[L_ENC1].H, nullptr))) return rc;  // He1 != He2: no shared fp16 path
@@ -307,10 +359,16 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   ftr_bn_input_kernel<<<B * Ts, 256, 0, st>>>(w.melT, w.encT, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
                                               Ts, w.xbn, w.fs);
   FSN_CHECK_LAUNCH("ftr_bn_input_kernel");
-  if ((rc = clip_reduce_only_launch(w.fs, B, Ts, w.sums2, st))) return rc;
-  if ((rc = norm_scales_launch(w.sums2, w.sums2, B, (float)M * K * Ts, 1.f, w.inv2, nullptr, st))) return rc;
-  ftr_scale_kernel<<<grid_for((size_t)Ts * R * K), 256, 0, st>>>(w.xbn, w.inv2, (size_t)Ts * R * K, K, R, M, w.xbn);
-  FSN_CHECK_LAUNCH("ftr_scale_kernel");
+  if (m.cum) {  // per-(shrunk step, row) scales, kept in cum2 for the backward
+    if ((rc = fast_cum_bn_scale_launch(w.xbn, R, K, Ts, TRAIN_CUM_EPS, w.cum2, st))) return rc;
+    train_scale_tm_kernel<<<grid_for((size_t)Ts * R * K), 256, 0, st>>>(w.xbn, w.cum2, K, (size_t)Ts * R * K, w.xbn);
+    FSN_CHECK_LAUNCH("train_scale_tm_kernel");
+  } else {
+    if ((rc = clip_reduce_only_launch(w.fs, B, Ts, w.sums2, st))) return rc;
+    if ((rc = norm_scales_launch(w.sums2, w.sums2, B, (float)M * K * Ts, 1.f, w.inv2, nullptr, st))) return rc;
+    ftr_scale_kernel<<<grid_for((size_t)Ts * R * K), 256, 0, st>>>(w.xbn, w.inv2, (size_t)Ts * R * K, K, R, M, w.xbn);
+    FSN_CHECK_LAUNCH("ftr_scale_kernel");
+  }
   // bottleneck 2xLSTM(K->Hb->Hb) + Linear(1) + ReLU over Ts steps (model.py:188-189)
   if ((rc = layer(L_BN0, w.xbn, nullptr))) return rc;
   if ((rc = layer(L_BN1, w.L[L_BN0].H, w.h16[L_BN0]))) return rc;
@@ -375,11 +433,19 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   if ((rc = layer_weight_grads(L[L_BN0], Ts, w.xbn, g->bn[0].w_ih, g->bn[0].w_hh, g->bn[0].b_ih, g->bn[0].b_hh, wg, st)))
     return rc;
   // ---- second norm + down-sampling + unfold backward, ReLU' of the encoder output, its Linear(M)
-  train_dot_kernel<<<B, 256, 0, st>>>(w.dxbn, w.xbn, Ts, R, M, K, w.dot);
-  FSN_CHECK_LAUNCH("train_dot_kernel");
-  ftr_denc_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.ddec, w.dxbn, w.encT, w.inv2, w.dot, B, Tp, M,
-                                                                d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
-                                                                (float)M * K * Ts, w.denc);
+  if (m.cum) {
+    ftr_cum_suffix_kernel<<<cdiv(R, 128), 128, 0, st>>>(w.dxbn, w.xbn, w.cum2, Ts, R, K, w.suffix);
+    FSN_CHECK_LAUNCH("ftr_cum_suffix_kernel");
+    ftr_denc_kernel<true><<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(
+        w.ddec, w.dxbn, w.encT, nullptr, nullptr, w.cum2, w.suffix, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors,
+        m.S, 0.f, w.denc);
+  } else {
+    train_dot_kernel<<<B, 256, 0, st>>>(w.dxbn, w.xbn, Ts, R, M, K, w.dot);
+    FSN_CHECK_LAUNCH("train_dot_kernel");
+    ftr_denc_kernel<false><<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(
+        w.ddec, w.dxbn, w.encT, w.inv2, w.dot, nullptr, nullptr, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
+        (float)M * K * Ts, w.denc);
+  }
   FSN_CHECK_LAUNCH("ftr_denc_kernel");
   if ((rc = linear_bwd(w.denc, w.L[L_ENC2].H, wt->enc_fc_w, Tp * B, M, He2, g->enc_fc_w, g->enc_fc_b, w.dH, w.splitk, w.colsum,
                        st)))

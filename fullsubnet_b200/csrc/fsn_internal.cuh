@@ -205,9 +205,19 @@ __global__ void train_tm_stats_kernel(const float* __restrict__ x, int B, int F,
 __global__ void train_dot_kernel(const float* __restrict__ dX, const float* __restrict__ X, int Tp, int R, int Fsub, int K,
                                  float* __restrict__ dot);
 
-// shapes of one fast_fullsubnet Model.forward call (fsn_fast_model.cu): Ts = shrunk steps of the bottleneck
-struct FastDims { int B, T, Tp, F, M, K, Ts, S; };
+// shapes of one fast_fullsubnet Model.forward call (fsn_fast_model.cu): Ts = shrunk steps of the bottleneck; cum: the
+// descriptor asks for the cumulative norm
+struct FastDims { int B, T, Tp, F, M, K, Ts, S; bool cum; };
 int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m);
+// fast_fullsubnet's second cumulative norm (model.py:186-187, base_model.py:220-251) on the down-sampled bottleneck
+// input bn [Ts, R, K] (time-major, before the norm): scaleT[ts*R + r] = 1 / (mean of row r over its K features and the
+// shrunk steps <= ts + eps)
+int fast_cum_bn_scale_launch(const float* bn, int R, int K, int Ts, float eps, float* scaleT, cudaStream_t st);
+// frame sums of a time-major raw [Tp,B,F] into fs[b*Tp + t].x (the layout cum_clip_scale_launch reads), and
+// out[i] = raw[i] * scale[i / F] (per-(step, clip) scales of a [Tp*B] table, or per-(step, row) ones with F = row width)
+__global__ void train_frame_sum_kernel(const float* __restrict__ raw, int B, int F, int Tp, float2* __restrict__ fs);
+__global__ void train_scale_tm_kernel(const float* __restrict__ raw, const float* __restrict__ scale1T, int F, size_t n,
+                                      float* __restrict__ out);
 
 // shapes of one Model.forward call (fsn_model.cu)
 struct Dims {

@@ -182,7 +182,7 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
 
 using namespace fsn;
 
-extern "C" int fsn_version(void) { return 101; }
+extern "C" int fsn_version(void) { return 102; }
 extern "C" const char* fsn_last_error(void) { return g_err; }
 extern "C" int fsn_last_error_code(void) { return g_err_code; }
 extern "C" int64_t fsn_last_launch_count(void) { return g_launches; }

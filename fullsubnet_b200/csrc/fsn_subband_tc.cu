@@ -409,7 +409,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
             v *= a.unit_scale ? a.unit_scale[(size_t)t * a.R + row0 + n] : ri.scale;
           } else {
             for (int fr = f0; fr < f1; ++fr) v += src[((size_t)ri.src_b * a.src_T + fr) * a.F + col];
-            v *= wmean * ri.scale;
+            v *= wmean * (a.unit_scale ? a.unit_scale[(size_t)t * a.R + row0 + n] : ri.scale);
           }
         }
         const __half hi = __float2half_rn(v);
@@ -796,7 +796,7 @@ static int sb_tc_launch(const tc::KArgs& a, int H, cudaStream_t st) {
 int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
   tc::KArgs a;
   a.packed = (const uint8_t*)s.packed;
-  a.magT = s.magT; a.fbT = s.fbT; a.inv2 = s.inv2; a.unit_scale = s.shrink > 1 ? nullptr : s.unit_scale; a.crm = s.crm;
+  a.magT = s.magT; a.fbT = s.fbT; a.inv2 = s.inv2; a.unit_scale = s.unit_scale; a.crm = s.crm;
   a.R = s.map.B * s.map.Fsub; a.F = s.F; a.Tp = s.steps > 0 ? s.steps : s.Tp; a.la = s.la; a.T = a.Tp - s.la;
   a.src_T = s.Tp; a.shrink = s.shrink > 1 ? s.shrink : 1;
   a.Ns = s.Ns; a.Nf = s.Nf; a.H = s.H; a.Ksb = (2 * s.Ns + 1) + (2 * s.Nf + 1); a.act = s.act;

@@ -88,8 +88,8 @@ class Model(BaseModel):
         self.encoder_input_size = encoder_input_size
         self.noisy_input_num_neighbors = noisy_input_num_neighbors
         self.enc_output_num_neighbors = encoder_output_num_neighbors
-        if norm_type != "offline_laplace_norm":
-            raise NotImplementedError(f"norm_type {norm_type!r} is not built for fast_fullsubnet (SURVEY 8f)")
+        # offline_laplace_norm or cumulative_laplace_norm (both norms, every precision, inference and training); the
+        # other upstream norms raise NotImplementedError
         self.norm = self.norm_wrapper(norm_type)
         # arithmetic: 'fp32' (FMA kernels) | 'f16x3_tc' (tensor cores, hi+lo split operands, the fp32 error class) |
         # 'f16_tc' (tensor cores, single pass, ~1e-4) | 'auto' = f16x3_tc when the shape allows, else fp32.  The
@@ -133,7 +133,7 @@ class Model(BaseModel):
                           bn_hidden=self.bottleneck.hidden_size, bn_layers=self.bottleneck.num_layers, dec_hidden=512,
                           noisy_num_neighbors=self.noisy_input_num_neighbors,
                           enc_num_neighbors=self.enc_output_num_neighbors, precision=prec,
-                          cell_type=_lib.CELL[self.sequence_model_type])
+                          cell_type=_lib.CELL[self.sequence_model_type], norm_type=self.norm)
 
     def _weight_struct(self):
         """Raw device pointers of every parameter (fsn_fast_weights, no packed bottleneck image)."""

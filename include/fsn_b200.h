@@ -43,7 +43,8 @@ enum {
 
 enum { FSN_ACT_NONE = 0, FSN_ACT_RELU = 1, FSN_ACT_TANH = 2, FSN_ACT_RELU6 = 3 };
 /* FSN_NORM_CUMULATIVE_LAPLACE (audio_zen/model/base_model.py:220-251): causal running mean per clip (first norm) and
- * per sub-band unit (second norm); built for the fp32 inference path of fsn_model_forward / fsn_enhance */
+ * per sub-band unit (second norm); built for the fp32 inference path of fsn_model_forward / fsn_enhance, and for
+ * fast_fullsubnet (fsn_fast_desc.norm_type) on every precision of inference and training */
 enum { FSN_NORM_OFFLINE_LAPLACE = 0, FSN_NORM_CUMULATIVE_LAPLACE = 1 };
 enum { FSN_CELL_LSTM = 0, FSN_CELL_GRU = 1 };
 /* arithmetic of the sub-band LSTM stack (99 % of the FLOPs):
@@ -59,6 +60,7 @@ enum { FSN_CELL_LSTM = 0, FSN_CELL_GRU = 1 };
  *                       rel), needed where decompress_cIRM amplifies mask errors x100 (|cRM| near the 9.9 clip) */
 enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F16X3_TC = 3 };
 
+/* ABI version: 101 changed fsn_enhance's argument list; 102 appended norm_type to fsn_fast_desc, so that struct grew */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -200,6 +202,10 @@ typedef struct fsn_fast_desc {
   int32_t enc_num_neighbors;   /* encoder_output_num_neighbors */
   int32_t precision;           /* FSN_PREC_* for the bottleneck stack (the tensor-core path needs bn_hidden = 384) */
   int32_t cell_type;           /* FSN_CELL_* (`sequence_model`); inference and training are built for LSTM only */
+  int32_t norm_type;           /* FSN_NORM_* of both norms (model.py:170,187); every precision, inference and training.
+                                * FSN_NORM_CUMULATIVE_LAPLACE: one scale per (clip, frame) over the mel bins for the
+                                * encoder, one per (clip, mel row, shrunk step) over the K features for the bottleneck.
+                                * Other values -> FSN_ERR_UNSUPPORTED before any CUDA call.  Appended in ABI version 102. */
 } fsn_fast_desc;
 
 typedef struct fsn_fast_weights {
