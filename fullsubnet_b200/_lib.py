@@ -181,6 +181,10 @@ _SIGNATURES = {
     "fsn_debug_seq_stack_workspace_bytes": (_S, [_I, C.POINTER(C.c_int), _I, _I, _I, _I, _I, _I, _I, _I]),
     "fsn_debug_seq_stack": (C.c_int, [C.POINTER(LstmLayer), _I, C.POINTER(C.c_int), _I, _I, _I, _I, _I, _I, _I, _I, _P, _P,
                                       _P, _P, _I, _I, _P, _P, _S, C.POINTER(C.c_int), _P]),
+    "fsn_debug_stft": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "fsn_debug_istft": (C.c_int, [_P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P]),
+    "fsn_debug_istft_mask_adjoint": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "fsn_debug_wav_epilogue": (C.c_int, [_P, _P, _I, _I, _P, _P, _F, _P, _P, _I, _I, _I, _P]),
     "fsn_last_error_code": (C.c_int, []),
     "fsn_last_launch_count": (C.c_int64, []),
     "fsn_total_launch_count": (C.c_int64, []),

@@ -55,7 +55,9 @@ __device__ __forceinline__ void init_tables(float2* tw, float* win, int n, int w
   const int left = (n - win_length) / 2;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const int m = i - left;
-    win[i] = (m >= 0 && m < win_length) ? 0.5f - 0.5f * cospif(2.0f * (float)m / (float)win_length) : 0.0f;
+    // torch.hann_window(1) is [1], not the 0 of the periodic formula
+    const float h = win_length == 1 ? 1.0f : 0.5f - 0.5f * cospif(2.0f * (float)m / (float)win_length);
+    win[i] = (m >= 0 && m < win_length) ? h : 0.0f;
   }
 }
 
@@ -105,8 +107,9 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
     const float2 zk = z[(j >> 1) * zstride + k];
     const float2 zn = z[(j >> 1) * zstride + ((n - k) & (n - 1))];
     float re, im;
+    // at DC and Nyquist zk == zn, so both Im are +0 and a negative Re has phase +pi, as torch.angle gives
     if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
-    else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+    else              { re = 0.5f * (zk.y + zn.y); im = 0.5f * (zn.x - zk.x); }
     if (t >= Tb) re = im = 0.f;
     const size_t o = (size_t)b * plane + (size_t)k * T + t;
     if (real) real[o] = re;
@@ -126,7 +129,7 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
         const float2 zn = z[(j >> 1) * zstride + ((n - k) & (n - 1))];
         float re, im;
         if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
-        else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+        else              { re = 0.5f * (zk.y + zn.y); im = 0.5f * (zn.x - zk.x); }
         m = hypotf(re, im);
       }
       magT[((size_t)b * T_pad + t) * F + k] = m;
@@ -431,35 +434,69 @@ static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 // fsn_dsp_dft.cu: direct-DFT variants for even transform sizes that are not a power of two (e.g. 960)
 int stft_dft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, int T, int Tg, float* mag,
                     float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens);
+size_t istft_dft_smem_bytes(int n_fft, int hop);
 int istft_dft_launch(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B, int T,
                      int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st, unsigned int* peak_bits,
                      const int* lens);
 int istft_mask_adjoint_dft_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
                                   int hop, int win_length, float* dcrm, cudaStream_t st);
 static bool dft_size_ok(int n) { return !is_pow2(n) && (n & 1) == 0 && n >= 16 && n <= 1200; }
+static bool dsp_size_ok(int n) { return dft_size_ok(n) || (is_pow2(n) && n >= 16 && n <= 2048); }
 
-int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
-                float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens) {
+constexpr int kMaxGridY = 65535;            // the three DSP grids put the clip in gridDim.y
+constexpr size_t kSmemOptin = 227 * 1024;  // opt-in dynamic shared memory per block on sm_90
+
+static size_t istft_smem_bytes(int n_fft, int hop) {
+  if (dft_size_ok(n_fft)) return istft_dft_smem_bytes(n_fft, hop);
+  const int np_max = (kFR + cdiv(n_fft, hop) + 2) / 2;
+  return (size_t)np_max * (n_fft + 1) * 8 + (size_t)n_fft / 2 * 8 + (size_t)n_fft * 4;
+}
+
+// host checks of stft_launch, before any CUDA call
+static int stft_check(int B, int L, int n_fft, int hop, int win_length, const float* magT, int T_pad) {
   FSN_REQUIRE(B > 0 && L > 0, FSN_ERR_SHAPE, "stft: empty input (B=%d, L=%d)", B, L);
-  if (dft_size_ok(n_fft)) {
-    FSN_REQUIRE(hop > 0 && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE, "stft: bad hop/win_length");
-    FSN_REQUIRE(n_fft / 2 < L, FSN_ERR_SHAPE, "stft: reflect padding %d needs L > pad (L=%d)", n_fft / 2, L);
-    FSN_REQUIRE(!magT || T_pad >= 1 + L / hop, FSN_ERR_SHAPE, "stft: T_pad < T");
-    const int Td = 1 + L / hop;
-    return stft_dft_launch(wav, B, L, n_fft, hop, win_length, Td, magT ? (T_pad > Td ? T_pad : Td) : Td, mag, phase, real,
-                           imag, magT, T_pad, st, lens);
-  }
-  FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
+  FSN_REQUIRE(B <= kMaxGridY, FSN_ERR_UNSUPPORTED, "stft: B=%d clips, at most %d", B, kMaxGridY);
+  FSN_REQUIRE(dsp_size_ok(n_fft), FSN_ERR_UNSUPPORTED,
               "stft: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);
   FSN_REQUIRE(hop > 0 && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE, "stft: bad hop/win_length");
   FSN_REQUIRE(n_fft / 2 < L, FSN_ERR_SHAPE, "stft: reflect padding %d needs L > pad (L=%d)", n_fft / 2, L);
+  FSN_REQUIRE(!magT || T_pad >= 1 + L / hop, FSN_ERR_SHAPE, "stft: T_pad < T");
+  return FSN_OK;
+}
+
+// host checks of istft_launch, before any CUDA call (the peak memset included)
+static int istft_check(int B, int T, int n_fft, int hop, int win_length, int cstride, int length, bool lens) {
+  FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "istft: empty input");
+  FSN_REQUIRE(B <= kMaxGridY, FSN_ERR_UNSUPPORTED, "istft: B=%d clips, at most %d", B, kMaxGridY);
+  FSN_REQUIRE(!lens || length > 0, FSN_ERR_UNSUPPORTED, "istft: per-clip lengths need an output length");
+  FSN_REQUIRE(dsp_size_ok(n_fft), FSN_ERR_UNSUPPORTED,
+              "istft: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);
+  FSN_REQUIRE(hop > 0 && hop <= n_fft && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE,
+              "istft: bad hop/win_length");
+  FSN_REQUIRE(cstride == 1 || cstride == 2, FSN_ERR_SHAPE, "istft: cstride must be 1 or 2");
+  const int out_len = length > 0 ? length : hop * (T - 1);
+  FSN_REQUIRE(out_len > 0, FSN_ERR_SHAPE, "istft: output length %d", out_len);
+  // a clip of lens[b] <= length samples reads frames up to lens[b]/hop
+  FSN_REQUIRE(!lens || length / hop < T, FSN_ERR_SHAPE, "istft: %d frames, per-clip lengths up to %d need %d", T, length,
+              1 + length / hop);
+  const size_t smem = istft_smem_bytes(n_fft, hop);
+  FSN_REQUIRE(smem <= kSmemOptin, FSN_ERR_UNSUPPORTED,
+              "istft: n_fft=%d with hop=%d needs %zu bytes of shared memory, at most %zu", n_fft, hop, smem, kSmemOptin);
+  return FSN_OK;
+}
+
+int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
+                float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens) {
+  int rc = stft_check(B, L, n_fft, hop, win_length, magT, T_pad);
+  if (rc) return rc;
   const int T = 1 + L / hop;
   const int Tg = magT ? (T_pad > T ? T_pad : T) : T;
-  FSN_REQUIRE(!magT || T_pad >= T, FSN_ERR_SHAPE, "stft: T_pad < T");
+  if (dft_size_ok(n_fft))
+    return stft_dft_launch(wav, B, L, n_fft, hop, win_length, T, Tg, mag, phase, real, imag, magT, T_pad, st, lens);
   const size_t smem = (size_t)(kFR / 2) * (n_fft + 1) * 8 + (size_t)n_fft / 2 * 8 + (size_t)n_fft * 4;
   if (smem > 48 * 1024) {
-    int rc = check_cuda(cudaFuncSetAttribute(stft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                        "stft smem attr");
+    rc = check_cuda(cudaFuncSetAttribute(stft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                    "stft smem attr");
     if (rc) return rc;
   }
   dim3 grid(cdiv(Tg, kFR), B);
@@ -473,6 +510,7 @@ int istft_mask_adjoint_launch(const float* dwav, const float* real, const float*
                               int hop, int win_length, float* dcrm, cudaStream_t st) {
   FSN_REQUIRE(B > 0 && L > 0 && T > 0 && hop > 0 && hop <= n_fft && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE,
               "istft adjoint: bad shape");
+  FSN_REQUIRE(B <= kMaxGridY, FSN_ERR_UNSUPPORTED, "istft adjoint: B=%d clips, at most %d", B, kMaxGridY);
   if (dft_size_ok(n_fft)) return istft_mask_adjoint_dft_launch(dwav, real, imag, B, L, T, n_fft, hop, win_length, dcrm, st);
   FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
               "istft adjoint: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);
@@ -491,34 +529,22 @@ int istft_mask_adjoint_launch(const float* dwav, const float* real, const float*
 int istft_launch(const float* real, const float* imag, int cstride, const float* crm, int B, int T, int n_fft,
                  int hop, int win_length, int length, float* wav, cudaStream_t st, int mask_mode, unsigned int* peak_bits,
                  const int* lens) {
-  FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "istft: empty input");
-  FSN_REQUIRE(!lens || length > 0, FSN_ERR_UNSUPPORTED, "istft: per-clip lengths need an output length");
+  int rc = istft_check(B, T, n_fft, hop, win_length, cstride, length, lens != nullptr);
+  if (rc) return rc;
   if (peak_bits) {
-    int rc = check_cuda(cudaMemsetAsync(peak_bits, 0, (size_t)B * sizeof(unsigned int), st), "istft peak memset");
+    rc = check_cuda(cudaMemsetAsync(peak_bits, 0, (size_t)B * sizeof(unsigned int), st), "istft peak memset");
     if (rc) return rc;
   }
-  if (dft_size_ok(n_fft)) {
-    FSN_REQUIRE(hop > 0 && hop <= n_fft && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE,
-                "istft: bad hop/win_length");
-    FSN_REQUIRE(cstride == 1 || cstride == 2, FSN_ERR_SHAPE, "istft: cstride must be 1 or 2");
-    const int olen = length > 0 ? length : hop * (T - 1);
-    FSN_REQUIRE(olen > 0, FSN_ERR_SHAPE, "istft: output length %d", olen);
-    return istft_dft_launch(real, imag, cstride, crm, mask_mode, B, T, n_fft, hop, win_length, olen, wav, st, peak_bits,
-                            lens);
-  }
-  FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
-              "istft: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);
-  FSN_REQUIRE(hop > 0 && hop <= n_fft && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE,
-              "istft: bad hop/win_length");
-  FSN_REQUIRE(cstride == 1 || cstride == 2, FSN_ERR_SHAPE, "istft: cstride must be 1 or 2");
   const int out_len = length > 0 ? length : hop * (T - 1);
-  FSN_REQUIRE(out_len > 0, FSN_ERR_SHAPE, "istft: output length %d", out_len);
+  if (dft_size_ok(n_fft))
+    return istft_dft_launch(real, imag, cstride, crm, mask_mode, B, T, n_fft, hop, win_length, out_len, wav, st, peak_bits,
+                            lens);
   const int seg = kFR * hop;
   const int np_max = (kFR + cdiv(n_fft, hop) + 2) / 2;
-  const size_t smem = (size_t)np_max * (n_fft + 1) * 8 + (size_t)n_fft / 2 * 8 + (size_t)n_fft * 4;
+  const size_t smem = istft_smem_bytes(n_fft, hop);
   if (smem > 48 * 1024) {
-    int rc = check_cuda(cudaFuncSetAttribute(istft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                        "istft smem attr");
+    rc = check_cuda(cudaFuncSetAttribute(istft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                    "istft smem attr");
     if (rc) return rc;
   }
   dim3 grid(cdiv(out_len, seg), B);
@@ -615,6 +641,71 @@ int wav_epilogue(const WavWs& w, const float* enhanced, int B, int L, int16_t* p
   return FSN_OK;
 }
 }  // namespace fsn
+
+// ---- unit-test hooks of the signal layer (include/fsn_b200.h): the internal launchers called directly, every argument
+// checked before any CUDA call; host lengths go to lens_dev through wav_prologue as in the wav -> wav entry points
+extern "C" int fsn_debug_stft(const float* wav, int B, int L, int n_fft, int hop, int win_length, const int32_t* lengths,
+                              int* lens_dev, float* mag, float* phase, float* real, float* imag, float* magT, int T_pad,
+                              fsn_stream_t stream) {
+  launch_counter() = 0;
+  int rc = stft_check(B, L, n_fft, hop, win_length, magT, T_pad);
+  if (rc) return rc;
+  FSN_REQUIRE(!lengths || lens_dev, FSN_ERR_SHAPE, "stft hook: lengths need a device length table");
+  if ((rc = wav_check(lengths, B, L, n_fft, false, wav, "stft hook"))) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  WavWs w = {nullptr, nullptr, nullptr, nullptr, lens_dev};
+  if ((rc = wav_prologue(lengths, B, w, st))) return rc;
+  return stft_launch(wav, B, L, n_fft, hop, win_length, mag, phase, real, imag, magT, T_pad, st, w.lens);
+}
+
+extern "C" int fsn_debug_istft(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B,
+                               int T, int n_fft, int hop, int win_length, int length, const int32_t* lengths, int* lens_dev,
+                               float* wav, unsigned int* peak_bits, int16_t* pcm, float gain, float* crm_out,
+                               fsn_stream_t stream) {
+  launch_counter() = 0;
+  int rc = istft_check(B, T, n_fft, hop, win_length, cstride, length, lengths != nullptr);
+  if (rc) return rc;
+  FSN_REQUIRE(mask_mode >= 0 && mask_mode <= 2, FSN_ERR_SHAPE, "istft hook: unknown mask mode %d", mask_mode);
+  FSN_REQUIRE((crm != nullptr) == (mask_mode != 0), FSN_ERR_SHAPE, "istft hook: mask mode %d with%s a mask", mask_mode,
+              crm ? "" : "out");
+  FSN_REQUIRE(real && imag, FSN_ERR_SHAPE, "istft hook: null spectrum");
+  FSN_REQUIRE(!pcm || peak_bits, FSN_ERR_SHAPE, "istft hook: the int16 output needs the peak");
+  FSN_REQUIRE(!crm_out || lengths, FSN_ERR_SHAPE, "istft hook: zeroing frames past each clip needs lengths");
+  FSN_REQUIRE(!lengths || lens_dev, FSN_ERR_SHAPE, "istft hook: lengths need a device length table");
+  const int out_len = length > 0 ? length : hop * (T - 1);
+  if ((rc = wav_check(lengths, B, out_len, n_fft, false, wav, "istft hook"))) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  WavWs w = {nullptr, nullptr, nullptr, peak_bits, lens_dev};
+  if ((rc = wav_prologue(lengths, B, w, st))) return rc;
+  if ((rc = istft_launch(real, imag, cstride, crm, B, T, n_fft, hop, win_length, length, wav, st, mask_mode, peak_bits,
+                         w.lens)))
+    return rc;
+  if (!pcm && !crm_out) return FSN_OK;
+  return wav_epilogue(w, wav, B, out_len, pcm, gain, crm_out, n_fft / 2 + 1, T, hop, st);
+}
+
+extern "C" int fsn_debug_istft_mask_adjoint(const float* dwav, const float* real, const float* imag, int B, int L, int T,
+                                            int n_fft, int hop, int win_length, float* dcrm, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(dwav && real && imag && dcrm, FSN_ERR_SHAPE, "istft adjoint hook: null argument");
+  return istft_mask_adjoint_launch(dwav, real, imag, B, L, T, n_fft, hop, win_length, dcrm, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_wav_epilogue(const float* enhanced, const unsigned int* peak_bits, int B, int L,
+                                      const int32_t* lengths, int* lens_dev, float gain, int16_t* pcm, float* crm_out, int F,
+                                      int T, int hop, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(B > 0 && L > 0 && F >= 2 && T > 0 && hop > 0, FSN_ERR_SHAPE, "wav epilogue hook: bad shape");
+  FSN_REQUIRE(!pcm || peak_bits, FSN_ERR_SHAPE, "wav epilogue hook: the int16 output needs the peak");
+  FSN_REQUIRE(!crm_out || lengths, FSN_ERR_SHAPE, "wav epilogue hook: zeroing frames past each clip needs lengths");
+  FSN_REQUIRE(!lengths || lens_dev, FSN_ERR_SHAPE, "wav epilogue hook: lengths need a device length table");
+  int rc = wav_check(lengths, B, L, 2 * (F - 1), false, enhanced, "wav epilogue hook");
+  if (rc) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  WavWs w = {nullptr, nullptr, nullptr, const_cast<unsigned int*>(peak_bits), lens_dev};
+  if ((rc = wav_prologue(lengths, B, w, st))) return rc;
+  return wav_epilogue(w, enhanced, B, L, pcm, gain, crm_out, F, T, hop, st);
+}
 
 extern "C" int fsn_decompress_cirm(const float* in, float* out, int64_t n, float K, float limit,
                                    fsn_stream_t stream) {

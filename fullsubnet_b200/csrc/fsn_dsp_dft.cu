@@ -22,7 +22,8 @@ __device__ __forceinline__ void dft_tables(float2* tw, float* win, int n, int wi
   const int left = (n - win_length) / 2;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const int m = i - left;
-    win[i] = (m >= 0 && m < win_length) ? 0.5f - 0.5f * cospif(2.0f * (float)m / (float)win_length) : 0.0f;
+    const float h = win_length == 1 ? 1.0f : 0.5f - 0.5f * cospif(2.0f * (float)m / (float)win_length);  // hann_window(1) = [1]
+    win[i] = (m >= 0 && m < win_length) ? h : 0.0f;
   }
 }
 
@@ -90,7 +91,7 @@ stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_le
     const float2 zn = z[(j >> 1) * n + (k == 0 ? 0 : n - k)];
     float re, im;
     if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
-    else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+    else              { re = 0.5f * (zk.y + zn.y); im = 0.5f * (zn.x - zk.x); }
     if (t >= Tb) re = im = 0.f;
     const size_t o = (size_t)b * plane + (size_t)k * T + t;
     if (real) real[o] = re;
@@ -110,7 +111,7 @@ stft_dft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_le
         const float2 zn = z[(j >> 1) * n + (k == 0 ? 0 : n - k)];
         float re, im;
         if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
-        else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+        else              { re = 0.5f * (zk.y + zn.y); im = 0.5f * (zn.x - zk.x); }
         m = hypotf(re, im);
       }
       magT[((size_t)b * T_pad + t) * F + k] = m;
@@ -281,14 +282,18 @@ int stft_dft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_
   return FSN_OK;
 }
 
+static int istft_dft_np_max(int n_fft, int hop) { return (kDftFR + cdiv(n_fft, hop) + 2) / 2; }
+
+size_t istft_dft_smem_bytes(int n_fft, int hop) {
+  return (size_t)2 * istft_dft_np_max(n_fft, hop) * n_fft * 8 + (size_t)n_fft * 8 + (size_t)n_fft * 4;
+}
+
 int istft_dft_launch(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B, int T,
                      int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st, unsigned int* peak_bits,
                      const int* lens) {
   const int seg = kDftFR * hop;
-  const int np_max = (kDftFR + cdiv(n_fft, hop) + 2) / 2;
-  const size_t smem = (size_t)2 * np_max * n_fft * 8 + (size_t)n_fft * 8 + (size_t)n_fft * 4;
-  FSN_REQUIRE(smem <= 227 * 1024, FSN_ERR_UNSUPPORTED, "istft: n_fft=%d with hop=%d needs %zu bytes of shared memory",
-              n_fft, hop, smem);
+  const int np_max = istft_dft_np_max(n_fft, hop);
+  const size_t smem = istft_dft_smem_bytes(n_fft, hop);  // istft_launch refused it above the opt-in limit
   int rc = check_cuda(cudaFuncSetAttribute(istft_dft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
                       "istft smem attr");
   if (rc) return rc;

@@ -568,6 +568,34 @@ int fsn_debug_seq_stack(const fsn_lstm_layer* layers, int n, const int* H, int R
                         const float* fc_b, int O, int act, float* out, void* workspace, size_t workspace_bytes, int* path,
                         fsn_stream_t stream);
 
+/* unit-test hooks for the signal layer (fsn_dsp.cu, fsn_dsp_dft.cu; torch.stft / torch.istft with center=True, reflect
+ * padding and a periodic Hann window of win_length centred in n_fft): the internal launchers behind fsn_stft, fsn_istft and
+ * the wav -> wav entry points, called directly.  n_fft a power of two in [16, 2048] (radix-2 kernels) or even in [16, 1200]
+ * (direct DFT); B <= 65535; the iSTFT refuses a hop whose frames would not fit in shared memory (FSN_ERR_UNSUPPORTED).
+ * lengths (nullable, host [B]): per-clip lengths n_fft/2 < lengths[b] <= L (iSTFT: <= its output length), max == L, copied
+ * to lens_dev (device [B]) through the kernel parameters.
+ *   fsn_debug_stft: wav [B,L] -> any of mag, phase, real, imag [B,F,T] (F = n_fft/2+1, T = 1+L/hop) and magT [B,T_pad,F]
+ *     (nullable each); clip b has 1 + lengths[b]/hop frames, the rest are 0.
+ *   fsn_debug_istft: [B,F,T] spectrum (real / imag cstride floats apart: 2 for interleaved complex) times crm [B,2,F,T]
+ *     (mask_mode 0: none, crm NULL; 1: decompressed cIRM, complex product; 2: element-wise) -> wav [B,length]
+ *     (length <= 0: hop*(T-1)); peak_bits (nullable, [B]) <- max|wav| per clip as float bits; pcm (nullable, [B,length],
+ *     needs peak_bits) <- int16(gain * wav / peak); crm_out (nullable, [B,2,F,T], needs lengths) zeroed for frames
+ *     t >= 1 + lengths[b]/hop.
+ *   fsn_debug_istft_mask_adjoint: d loss / d crm [B,2,F,T] of mask_mode 2 with wav length L, for dwav [B,L]; rows f < F-1
+ *     (the Nyquist row is not written).
+ *   fsn_debug_wav_epilogue: the int16 output and crm_out zeroing of fsn_debug_istft on a caller's enhanced [B,L] and peak.
+ * Arguments are checked before any CUDA call. */
+int fsn_debug_stft(const float* wav, int B, int L, int n_fft, int hop, int win_length, const int32_t* lengths, int* lens_dev,
+                   float* mag, float* phase, float* real, float* imag, float* magT, int T_pad, fsn_stream_t stream);
+int fsn_debug_istft(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B, int T,
+                    int n_fft, int hop, int win_length, int length, const int32_t* lengths, int* lens_dev, float* wav,
+                    unsigned int* peak_bits, int16_t* pcm, float gain, float* crm_out, fsn_stream_t stream);
+int fsn_debug_istft_mask_adjoint(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
+                                 int hop, int win_length, float* dcrm, fsn_stream_t stream);
+int fsn_debug_wav_epilogue(const float* enhanced, const unsigned int* peak_bits, int B, int L, const int32_t* lengths,
+                           int* lens_dev, float gain, int16_t* pcm, float* crm_out, int F, int T, int hop,
+                           fsn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -48,8 +48,11 @@ def test_stft_matches_reference(golden, dev):
     assert rel_max(real.cpu(), g["real"]) < 5e-6 and rel_max(imag.cpu(), g["imag"]) < 5e-6
     assert rel_max(mag.cpu(), g["mag"]) < 5e-6
     sel = g["mag"] > 1e-2 * g["mag"].max()
-    d = np.angle(np.exp(1j * (phase.cpu().numpy() - g["phase"])))
-    assert np.abs(d[sel]).max() < 1e-4
+    # phase compared directly, not modulo 2 pi: a negative Re with Im exactly 0 (DC, Nyquist) is +pi in both.  Only bins
+    # whose non-zero Im is too small for its float32 sign to be certain sit on the branch cut and are left out.
+    cut = (g["real"] < 0) & (g["imag"] != 0) & (np.abs(g["imag"]) < 1e-5 * g["mag"].max())
+    d = phase.cpu().numpy() - g["phase"]
+    assert np.abs(d[sel & ~cut]).max() < 1e-4
     mag3 = stft(T(g["y3"], dev), 512, 256, 512)[0]  # [B,C,T] input (feature.py:30-31,43-44)
     assert mag3.shape == g["mag3"].shape and rel_max(mag3.cpu(), g["mag3"]) < 5e-6
     _, _, rs, is_ = stft(T(g["y"], dev), 64, 32, 64)
