@@ -82,19 +82,4 @@ __device__ __forceinline__ float decompress_cirm_f(float m, float K, float limit
   return -K * logf((K - m) / (K + m));
 }
 
-// g(s) = d loss / d (overlap-added sample s) of the iSTFT: dwav at the sample the forward wrote (s - n/2 in [0, L), s
-// inside the frames) over the window-square envelope, with the same frames in the same order as the iSTFT kernels; else 0
-__device__ __forceinline__ float istft_adjoint_sample(const float* __restrict__ dwav, const float* __restrict__ win, int s,
-                                                      int n, int hop, int T, int L) {
-  if (s < n / 2 || s >= n / 2 + L || s >= n + hop * (T - 1)) return 0.f;
-  const int tl = (s >= n) ? (s - n) / hop + 1 : 0;
-  const int th = min(T - 1, s / hop);
-  float env = 0.f;
-  for (int t = tl; t <= th; ++t) {
-    const float w = win[s - t * hop];
-    env += w * w;
-  }
-  return (env > 1e-11f) ? dwav[s - n / 2] / env : 0.f;
-}
-
 }  // namespace fsn

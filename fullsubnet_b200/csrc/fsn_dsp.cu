@@ -1,11 +1,16 @@
-// STFT / iSTFT (+ fused cIRM decompress & complex mask) and the elementwise mask ops.
+// STFT / iSTFT (+ fused cIRM decompress & complex mask), the iSTFT's mask adjoint, and the elementwise mask ops.
 //
 // Reference semantics: audio_zen/acoustics/feature.py:9-91 (-> torch.stft / torch.istft),
 // audio_zen/acoustics/mask.py:7-64, recipes/dns_interspeech_2020/inferencer.py:136-143.
 //
-// FFT: shared-memory radix-2 DIT, two real frames packed into one complex transform
-// (frame A -> real lane, frame B -> imaginary lane), FR frames per CTA so that the [B,F,T]
-// (T-contiguous) stores / loads of the reference layout are FR*4-byte segments.
+// Two real frames packed into one complex transform (frame A -> real lane, frame B -> imaginary lane), kFR frames per
+// CTA so that the [B,F,T] (T-contiguous) stores / loads of the reference layout are kFR*4-byte segments.  The three
+// transform kernels are templates over the transform policy:
+//   Radix2     n a power of two: shared-memory radix-2 DIT, in place;
+//   DirectDft  n even and not a power of two (the reference's 48 kHz improved_fullsubnet example uses n_fft = 960,
+//              hop = 480: recipes/dns_interspeech_2020/improved_fullsubnet/model.py:603-620): a direct O(n^2) DFT in
+//              shared memory against a full-circle twiddle table.  At n = 960 that is 3.7 MFLOP per frame, i.e. < 1 %
+//              of the model's 217 MFLOP per frame, so a mixed-radix FFT would not move the step time.
 #include <string.h>
 
 #include "fsn_internal.cuh"
@@ -18,10 +23,10 @@ constexpr int kDspThreads = 256;
 __device__ __forceinline__ int ilog2(int n) { return 31 - __clz(n); }
 
 // in-place radix-2 DIT over `npairs` independent transforms whose inputs are already in
-// bit-reversed order; tw[k] = exp(-2*pi*i*k/n)
+// bit-reversed order; tw[k] = exp(-2*pi*i*k/n).  Returns z.
 template <bool INVERSE>
-__device__ __forceinline__ void fft_radix2_smem(float2* z, int zstride, int npairs, int n, int log2n,
-                                                const float2* tw) {
+__device__ __forceinline__ float2* fft_radix2_smem(float2* z, int zstride, int npairs, int n, int log2n,
+                                                   const float2* tw) {
   const int nb_log = log2n - 1;
   const int total = npairs << nb_log;
   for (int s = 1; s <= log2n; ++s) {
@@ -44,10 +49,72 @@ __device__ __forceinline__ void fft_radix2_smem(float2* z, int zstride, int npai
     }
     __syncthreads();
   }
+  return z;
 }
 
-__device__ __forceinline__ void init_tables(float2* tw, float* win, int n, int win_length) {
-  for (int k = threadIdx.x; k < n / 2; k += blockDim.x) {
+// out[p][k] = sum_i in[p][i] * tw[(i*k) mod n]   (INVERSE: conj(tw)); np transforms of length n, natural order.
+// Returns out.
+template <bool INVERSE>
+__device__ __forceinline__ float2* dft_smem(const float2* in, float2* out, int np, int n, const float2* tw) {
+  for (int idx = threadIdx.x; idx < np * n; idx += blockDim.x) {
+    const int p = idx / n;
+    const int k = idx - p * n;
+    const float2* a = in + (size_t)p * n;
+    float re = 0.f, im = 0.f;
+    int m = 0;
+    // at n = 960 (one CTA per SM) this loop is latency-bound, and the compiler's default 4-way schedule of it shifts
+    // with the code of the calling kernel, by up to 13 % on an H100; unrolled by 8 it is faster in all three kernels
+#pragma unroll 8
+    for (int i = 0; i < n; ++i) {
+      float2 w = tw[m];
+      if (INVERSE) w.y = -w.y;
+      const float2 v = a[i];
+      re = fmaf(v.x, w.x, fmaf(-v.y, w.y, re));
+      im = fmaf(v.x, w.y, fmaf(v.y, w.x, im));
+      m += k;
+      if (m >= n) m -= n;
+    }
+    out[(size_t)p * n + k] = make_float2(re, im);
+  }
+  __syncthreads();
+  return out;
+}
+
+// A transform policy holds what differs between the two transforms, and nothing else: the dynamic shared memory of np
+// frame pairs (the transform's input rows `stride` apart, its result, tw_len twiddles, the window of n floats), the
+// input slot of sample i, the (pair, sample) of a flat fill index, and the transform, which returns the buffer that
+// holds the result (row j >> 1 has frame j).
+struct Radix2 {  // in place, bit-reversed input, twiddles for k < n/2
+  static size_t smem_bytes(int n, int np) { return (size_t)np * (n + 1) * 8 + (size_t)n / 2 * 8 + (size_t)n * 4; }
+  int n, log2n, stride, tw_len;
+  float2 *in, *tw;
+  float* win;
+  __device__ Radix2(float2* smem, int n_, int np)
+      : n(n_), log2n(ilog2(n_)), stride(n_ + 1), tw_len(n_ / 2), in(smem), tw(smem + np * stride),
+        win(reinterpret_cast<float*>(tw + n_ / 2)) {}
+  __device__ void split(int idx, int& p, int& i) const { p = idx >> log2n; i = idx & (n - 1); }
+  __device__ int slot(int i) const { return (int)(__brev((unsigned)i) >> (32 - log2n)); }
+  template <bool INVERSE>
+  __device__ const float2* transform(int np) const { return fft_radix2_smem<INVERSE>(in, stride, np, n, log2n, tw); }
+};
+
+struct DirectDft {  // out of place, natural-order input, twiddles for the full circle
+  static size_t smem_bytes(int n, int np) { return (size_t)2 * np * n * 8 + (size_t)n * 8 + (size_t)n * 4; }
+  int n, stride, tw_len;
+  float2 *in, *out, *tw;
+  float* win;
+  __device__ DirectDft(float2* smem, int n_, int np)
+      : n(n_), stride(n_), tw_len(n_), in(smem), out(smem + np * n_), tw(out + np * n_),
+        win(reinterpret_cast<float*>(tw + n_)) {}
+  __device__ void split(int idx, int& p, int& i) const { p = idx / n; i = idx - p * n; }
+  __device__ int slot(int i) const { return i; }
+  template <bool INVERSE>
+  __device__ const float2* transform(int np) const { return dft_smem<INVERSE>(in, out, np, n, tw); }
+};
+
+// tw[k] = exp(-2*pi*i*k/n) for k < tw_len; win = periodic Hann of win_length centred in n
+__device__ __forceinline__ void init_tables(float2* tw, int tw_len, float* win, int n, int win_length) {
+  for (int k = threadIdx.x; k < tw_len; k += blockDim.x) {
     float s, c;
     sincospif(-2.0f * (float)k / (float)n, &s, &c);
     tw[k] = make_float2(c, s);
@@ -61,41 +128,56 @@ __device__ __forceinline__ void init_tables(float2* tw, float* win, int n, int w
   }
 }
 
+// windowed frames t0 + 2p (real lane) and t0 + 2p + 1 (imaginary lane) of np pairs into the transform's input;
+// sample(t, i) is sample i of frame t < Tv, frames from Tv on enter as zeros
+template <class P, class Sample>
+__device__ __forceinline__ void fill_frame_pairs(const P& tr, int np, int t0, int Tv, Sample sample) {
+  for (int idx = threadIdx.x; idx < np * tr.n; idx += blockDim.x) {
+    int p, i;
+    tr.split(idx, p, i);
+    const int ta = t0 + 2 * p, tb = ta + 1;
+    const float w = tr.win[i];
+    float va = 0.f, vb = 0.f;
+    if (ta < Tv) va = sample(ta, i) * w;
+    if (tb < Tv) vb = sample(tb, i) * w;
+    tr.in[p * tr.stride + tr.slot(i)] = make_float2(va, vb);
+  }
+}
+
+// (Re, Im) of bin k of frame j from the packed transform result z.  At DC and Nyquist zk == zn, so both Im are +0 and
+// a negative Re has phase +pi, as torch.angle gives.
+__device__ __forceinline__ float2 unpack_bin(const float2* z, int stride, int n, int j, int k) {
+  const float2 zk = z[(j >> 1) * stride + k];
+  const float2 zn = z[(j >> 1) * stride + (k == 0 ? 0 : n - k)];
+  float re, im;
+  if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
+  else              { re = 0.5f * (zk.y + zn.y); im = 0.5f * (zn.x - zk.x); }
+  return make_float2(re, im);
+}
+
 // ------------------------------------------------------------------------------------------
 // lens (nullable, device [B]): clip b holds lens[b] <= L samples of its row (stride L), so it reflects at lens[b] and has
 // T_b = 1 + lens[b]/hop frames; frames T_b .. T-1 are written as zeros and frame T_b enters its pair's transform as
 // zeros, exactly as in a call on that clip alone.  Null: every clip has L samples.
+template <class P>
 __global__ void __launch_bounds__(kDspThreads)
 stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length, int T,
             float* __restrict__ mag, float* __restrict__ phase, float* __restrict__ real,
             float* __restrict__ imag, float* __restrict__ magT, int T_pad, const int* __restrict__ lens) {
   extern __shared__ float2 smem2[];
-  const int log2n = ilog2(n);
-  const int zstride = n + 1;
   constexpr int NP = kFR / 2;
-  float2* z = smem2;
-  float2* tw = z + NP * zstride;
-  float* win = reinterpret_cast<float*>(tw + n / 2);
+  const P tr(smem2, n, NP);
   const int b = blockIdx.y;
   const int t0 = blockIdx.x * kFR;
   const int F = n / 2 + 1;
   const int Lb = lens ? lens[b] : L;
   const int Tb = lens ? 1 + Lb / hop : T;
-  init_tables(tw, win, n, win_length);
+  init_tables(tr.tw, tr.tw_len, tr.win, n, win_length);
   __syncthreads();
   const float* x = wav + (size_t)b * L;
-  for (int idx = threadIdx.x; idx < NP * n; idx += blockDim.x) {
-    const int p = idx >> log2n;
-    const int i = idx & (n - 1);
-    const int ta = t0 + 2 * p, tb = ta + 1;
-    const float w = win[i];
-    float va = 0.f, vb = 0.f;
-    if (ta < Tb) va = x[reflect_idx(ta * hop + i - n / 2, Lb)] * w;
-    if (tb < Tb) vb = x[reflect_idx(tb * hop + i - n / 2, Lb)] * w;
-    z[p * zstride + (int)(__brev((unsigned)i) >> (32 - log2n))] = make_float2(va, vb);
-  }
+  fill_frame_pairs(tr, NP, t0, Tb, [&](int t, int i) { return x[reflect_idx(t * hop + i - n / 2, Lb)]; });
   __syncthreads();
-  fft_radix2_smem<false>(z, zstride, NP, n, log2n, tw);
+  const float2* z = tr.template transform<false>(NP);
 
   // un-pack the two real transforms and store in the reference layout [B,F,T]
   const size_t plane = (size_t)F * T;
@@ -104,18 +186,13 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
     const int j = idx - k * kFR;
     const int t = t0 + j;
     if (t >= T) continue;
-    const float2 zk = z[(j >> 1) * zstride + k];
-    const float2 zn = z[(j >> 1) * zstride + ((n - k) & (n - 1))];
-    float re, im;
-    // at DC and Nyquist zk == zn, so both Im are +0 and a negative Re has phase +pi, as torch.angle gives
-    if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
-    else              { re = 0.5f * (zk.y + zn.y); im = 0.5f * (zn.x - zk.x); }
-    if (t >= Tb) re = im = 0.f;
+    float2 c = unpack_bin(z, tr.stride, n, j, k);
+    if (t >= Tb) c = make_float2(0.f, 0.f);
     const size_t o = (size_t)b * plane + (size_t)k * T + t;
-    if (real) real[o] = re;
-    if (imag) imag[o] = im;
-    if (mag) mag[o] = hypotf(re, im);
-    if (phase) phase[o] = atan2f(im, re);
+    if (real) real[o] = c.x;
+    if (imag) imag[o] = c.y;
+    if (mag) mag[o] = hypotf(c.x, c.y);
+    if (phase) phase[o] = atan2f(c.y, c.x);
   }
   if (magT) {  // time-major copy with the look-ahead rows zeroed
     for (int idx = threadIdx.x; idx < F * kFR; idx += blockDim.x) {
@@ -125,12 +202,8 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
       if (t >= T_pad) continue;
       float m = 0.f;
       if (t < Tb) {
-        const float2 zk = z[(j >> 1) * zstride + k];
-        const float2 zn = z[(j >> 1) * zstride + ((n - k) & (n - 1))];
-        float re, im;
-        if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
-        else              { re = 0.5f * (zk.y + zn.y); im = 0.5f * (zn.x - zk.x); }
-        m = hypotf(re, im);
+        const float2 c = unpack_bin(z, tr.stride, n, j, k);
+        m = hypotf(c.x, c.y);
       }
       magT[((size_t)b * T_pad + t) * F + k] = m;
     }
@@ -138,17 +211,14 @@ stft_kernel(const float* __restrict__ wav, int L, int n, int hop, int win_length
 }
 
 // ------------------------------------------------------------------------------------------
+template <class P>
 __global__ void __launch_bounds__(kDspThreads)
 istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int cstride,
              const float* __restrict__ crm, int mask_mode, int T, int n, int hop, int win_length, int out_len,
              int seg, int np_max, float* __restrict__ wav, unsigned int* __restrict__ peak_bits,
              const int* __restrict__ lens) {
   extern __shared__ float2 smem2[];
-  const int log2n = ilog2(n);
-  const int zstride = n + 1;
-  float2* z = smem2;
-  float2* tw = z + np_max * zstride;
-  float* win = reinterpret_cast<float*>(tw + n / 2);
+  const P tr(smem2, n, np_max);
   const int b = blockIdx.y;
   const int F = n / 2 + 1;
   // lens (nullable): clip b has T_b = 1 + lens[b]/hop of the T frames (row stride T) and lens[b] of the out_len output
@@ -162,7 +232,7 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
   const int t_max = min(Tb - 1, (s_end - 1) / hop);
   const int nframes = t_max - t_min + 1;
   const int np = nframes > 0 ? (nframes + 1) / 2 : 0;
-  init_tables(tw, win, n, win_length);
+  init_tables(tr.tw, tr.tw_len, tr.win, n, win_length);
   const size_t plane = (size_t)F * T;
   const float* xr = real + (size_t)b * plane * cstride;
   const float* xi = imag + (size_t)b * plane * cstride;
@@ -195,14 +265,12 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
       e[q][1] = (k == 0 || k == n / 2) ? 0.f : i;  // irfft ignores Im of DC / Nyquist
     }
     // Z = Ea + i*Eb on the full circle (Hermitian extension of both)
-    z[p * zstride + (int)(__brev((unsigned)k) >> (32 - log2n))] =
-        make_float2(e[0][0] - e[1][1], e[0][1] + e[1][0]);
+    tr.in[p * tr.stride + tr.slot(k)] = make_float2(e[0][0] - e[1][1], e[0][1] + e[1][0]);
     if (k > 0 && k < n / 2)
-      z[p * zstride + (int)(__brev((unsigned)(n - k)) >> (32 - log2n))] =
-          make_float2(e[0][0] + e[1][1], -e[0][1] + e[1][0]);
+      tr.in[p * tr.stride + tr.slot(n - k)] = make_float2(e[0][0] + e[1][1], -e[0][1] + e[1][0]);
   }
   __syncthreads();
-  fft_radix2_smem<true>(z, zstride, np, n, log2n, tw);
+  const float2* z = tr.template transform<true>(np);
 
   const int full = n + hop * (Tb - 1);
   const float inv_n = 1.0f / (float)n;
@@ -216,8 +284,8 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
       for (int t = tl; t <= th; ++t) {
         const int i = s - t * hop;
         const int q = t - t_min;
-        const float2 v = z[(q >> 1) * zstride + i];
-        const float w = win[i];
+        const float2 v = z[(q >> 1) * tr.stride + i];
+        const float w = tr.win[i];
         acc += ((q & 1) ? v.y : v.x) * inv_n * w;
         env += w * w;
       }
@@ -238,54 +306,53 @@ istft_kernel(const float* __restrict__ real, const float* __restrict__ imag, int
   }
 }
 
+// g(s) = d loss / d (overlap-added sample s) of the iSTFT: dwav at the sample the forward wrote (s - n/2 in [0, L), s
+// inside the frames) over the window-square envelope, with the same frames in the same order as istft_kernel; else 0
+__device__ __forceinline__ float istft_adjoint_sample(const float* __restrict__ dwav, const float* __restrict__ win, int s,
+                                                      int n, int hop, int T, int L) {
+  if (s < n / 2 || s >= n / 2 + L || s >= n + hop * (T - 1)) return 0.f;
+  const int tl = (s >= n) ? (s - n) / hop + 1 : 0;
+  const int th = min(T - 1, s / hop);
+  float env = 0.f;
+  for (int t = tl; t <= th; ++t) {
+    const float w = win[s - t * hop];
+    env += w * w;
+  }
+  return (env > 1e-11f) ? dwav[s - n / 2] / env : 0.f;
+}
+
 // Adjoint of (element-wise mask, irfft, window, overlap-add, envelope, crop) with respect to the mask, same tiling as
 // stft_kernel (kFR frames per CTA, two real frames per complex transform): frame t's samples g(t*hop + i) * win[i] go
 // through the forward real DFT; irfft's adjoint scales bin k by c_k/n (c = 1 at DC, 2 at bins 1 .. n/2-1, the
 // Im of DC gets no gradient), and the product with the kept spectrum gives dcrm[b,0,k,t] = dRe * real,
 // dcrm[b,1,k,t] = dIm * imag for k < F-1.
+template <class P>
 __global__ void __launch_bounds__(kDspThreads)
 istft_mask_adjoint_kernel(const float* __restrict__ dwav, const float* __restrict__ real, const float* __restrict__ imag,
                           int L, int n, int hop, int win_length, int T, float* __restrict__ dcrm) {
   extern __shared__ float2 smem2[];
-  const int log2n = ilog2(n);
-  const int zstride = n + 1;
   constexpr int NP = kFR / 2;
-  float2* z = smem2;
-  float2* tw = z + NP * zstride;
-  float* win = reinterpret_cast<float*>(tw + n / 2);
+  const P tr(smem2, n, NP);
   const int b = blockIdx.y;
   const int t0 = blockIdx.x * kFR;
   const int F = n / 2 + 1;
-  init_tables(tw, win, n, win_length);
+  init_tables(tr.tw, tr.tw_len, tr.win, n, win_length);
   __syncthreads();
   const float* g = dwav + (size_t)b * L;
-  for (int idx = threadIdx.x; idx < NP * n; idx += blockDim.x) {
-    const int p = idx >> log2n;
-    const int i = idx & (n - 1);
-    const int ta = t0 + 2 * p, tb = ta + 1;
-    const float w = win[i];
-    float va = 0.f, vb = 0.f;
-    if (ta < T) va = istft_adjoint_sample(g, win, ta * hop + i, n, hop, T, L) * w;
-    if (tb < T) vb = istft_adjoint_sample(g, win, tb * hop + i, n, hop, T, L) * w;
-    z[p * zstride + (int)(__brev((unsigned)i) >> (32 - log2n))] = make_float2(va, vb);
-  }
+  fill_frame_pairs(tr, NP, t0, T, [&](int t, int i) { return istft_adjoint_sample(g, tr.win, t * hop + i, n, hop, T, L); });
   __syncthreads();
-  fft_radix2_smem<false>(z, zstride, NP, n, log2n, tw);
+  const float2* z = tr.template transform<false>(NP);
   const size_t plane = (size_t)F * T;
   for (int idx = threadIdx.x; idx < (F - 1) * kFR; idx += blockDim.x) {
     const int k = idx / kFR;
     const int j = idx - k * kFR;
     const int t = t0 + j;
     if (t >= T) continue;
-    const float2 zk = z[(j >> 1) * zstride + k];
-    const float2 zn = z[(j >> 1) * zstride + ((n - k) & (n - 1))];
-    float re, im;
-    if ((j & 1) == 0) { re = 0.5f * (zk.x + zn.x); im = 0.5f * (zk.y - zn.y); }
-    else              { re = 0.5f * (zk.y + zn.y); im = -0.5f * (zk.x - zn.x); }
+    const float2 c = unpack_bin(z, tr.stride, n, j, k);
     const float sc = (k == 0 ? 1.f : 2.f) / (float)n;
     const size_t o = (size_t)b * plane + (size_t)k * T + t;
-    dcrm[(size_t)b * plane + o] = sc * re * real[o];
-    dcrm[(size_t)b * plane + plane + o] = k == 0 ? 0.f : sc * im * imag[o];
+    dcrm[(size_t)b * plane + o] = sc * c.x * real[o];
+    dcrm[(size_t)b * plane + plane + o] = k == 0 ? 0.f : sc * c.y * imag[o];
   }
 }
 
@@ -431,25 +498,33 @@ static int ew_grid(int64_t n) {
 
 static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 
-// fsn_dsp_dft.cu: direct-DFT variants for even transform sizes that are not a power of two (e.g. 960)
-int stft_dft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, int T, int Tg, float* mag,
-                    float* phase, float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens);
-size_t istft_dft_smem_bytes(int n_fft, int hop);
-int istft_dft_launch(const float* real, const float* imag, int cstride, const float* crm, int mask_mode, int B, int T,
-                     int n_fft, int hop, int win_length, int out_len, float* wav, cudaStream_t st, unsigned int* peak_bits,
-                     const int* lens);
-int istft_mask_adjoint_dft_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
-                                  int hop, int win_length, float* dcrm, cudaStream_t st);
+// the transform policy: DirectDft for these sizes, Radix2 for the powers of two
 static bool dft_size_ok(int n) { return !is_pow2(n) && (n & 1) == 0 && n >= 16 && n <= 1200; }
-static bool dsp_size_ok(int n) { return dft_size_ok(n) || (is_pow2(n) && n >= 16 && n <= 2048); }
+bool dsp_size_ok(int n) { return dft_size_ok(n) || (is_pow2(n) && n >= 16 && n <= 2048); }
 
 constexpr int kMaxGridY = 65535;            // the three DSP grids put the clip in gridDim.y
 constexpr size_t kSmemOptin = 227 * 1024;  // opt-in dynamic shared memory per block on sm_90
 
-static size_t istft_smem_bytes(int n_fft, int hop) {
-  if (dft_size_ok(n_fft)) return istft_dft_smem_bytes(n_fft, hop);
-  const int np_max = (kFR + cdiv(n_fft, hop) + 2) / 2;
-  return (size_t)np_max * (n_fft + 1) * 8 + (size_t)n_fft / 2 * 8 + (size_t)n_fft * 4;
+// dynamic shared memory of np frame pairs under the policy that runs n_fft
+static size_t dsp_smem_bytes(int n_fft, int np) {
+  return dft_size_ok(n_fft) ? DirectDft::smem_bytes(n_fft, np) : Radix2::smem_bytes(n_fft, np);
+}
+
+// the most frame pairs one iSTFT CTA transforms: the frames overlapping its kFR * hop output samples
+static int istft_np_max(int n_fft, int hop) { return (kFR + cdiv(n_fft, hop) + 2) / 2; }
+static size_t istft_smem_bytes(int n_fft, int hop) { return dsp_smem_bytes(n_fft, istft_np_max(n_fft, hop)); }
+
+// launches a DSP kernel with smem bytes of dynamic shared memory, opting in to more than the default 48 KB
+template <typename... KArgs, typename... Args>
+static int dsp_launch(void (*kernel)(KArgs...), dim3 grid, size_t smem, cudaStream_t st, const char* name,
+                      Args... args) {
+  if (smem > 48 * 1024) {
+    const int rc = check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), name);
+    if (rc) return rc;
+  }
+  kernel<<<grid, kDspThreads, smem, st>>>(args...);
+  FSN_CHECK_LAUNCH(name);
+  return FSN_OK;
 }
 
 // host checks of stft_launch, before any CUDA call
@@ -487,23 +562,13 @@ static int istft_check(int B, int T, int n_fft, int hop, int win_length, int cst
 
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
                 float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens) {
-  int rc = stft_check(B, L, n_fft, hop, win_length, magT, T_pad);
+  const int rc = stft_check(B, L, n_fft, hop, win_length, magT, T_pad);
   if (rc) return rc;
   const int T = 1 + L / hop;
   const int Tg = magT ? (T_pad > T ? T_pad : T) : T;
-  if (dft_size_ok(n_fft))
-    return stft_dft_launch(wav, B, L, n_fft, hop, win_length, T, Tg, mag, phase, real, imag, magT, T_pad, st, lens);
-  const size_t smem = (size_t)(kFR / 2) * (n_fft + 1) * 8 + (size_t)n_fft / 2 * 8 + (size_t)n_fft * 4;
-  if (smem > 48 * 1024) {
-    rc = check_cuda(cudaFuncSetAttribute(stft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                    "stft smem attr");
-    if (rc) return rc;
-  }
-  dim3 grid(cdiv(Tg, kFR), B);
-  stft_kernel<<<grid, kDspThreads, smem, st>>>(wav, L, n_fft, hop, win_length, T, mag, phase, real, imag, magT,
-                                               T_pad, lens);
-  FSN_CHECK_LAUNCH("stft_kernel");
-  return FSN_OK;
+  return dsp_launch(dft_size_ok(n_fft) ? stft_kernel<DirectDft> : stft_kernel<Radix2>, dim3(cdiv(Tg, kFR), B),
+                    dsp_smem_bytes(n_fft, kFR / 2), st, "stft_kernel", wav, L, n_fft, hop, win_length, T, mag, phase,
+                    real, imag, magT, T_pad, lens);
 }
 
 int istft_mask_adjoint_launch(const float* dwav, const float* real, const float* imag, int B, int L, int T, int n_fft,
@@ -511,19 +576,11 @@ int istft_mask_adjoint_launch(const float* dwav, const float* real, const float*
   FSN_REQUIRE(B > 0 && L > 0 && T > 0 && hop > 0 && hop <= n_fft && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE,
               "istft adjoint: bad shape");
   FSN_REQUIRE(B <= kMaxGridY, FSN_ERR_UNSUPPORTED, "istft adjoint: B=%d clips, at most %d", B, kMaxGridY);
-  if (dft_size_ok(n_fft)) return istft_mask_adjoint_dft_launch(dwav, real, imag, B, L, T, n_fft, hop, win_length, dcrm, st);
-  FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
+  FSN_REQUIRE(dsp_size_ok(n_fft), FSN_ERR_UNSUPPORTED,
               "istft adjoint: n_fft=%d unsupported (power of two in [16,2048], or even and <= 1200)", n_fft);
-  const size_t smem = (size_t)(kFR / 2) * (n_fft + 1) * 8 + (size_t)n_fft / 2 * 8 + (size_t)n_fft * 4;
-  if (smem > 48 * 1024) {
-    int rc = check_cuda(cudaFuncSetAttribute(istft_mask_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                        "istft adjoint smem attr");
-    if (rc) return rc;
-  }
-  istft_mask_adjoint_kernel<<<dim3(cdiv(T, kFR), B), kDspThreads, smem, st>>>(dwav, real, imag, L, n_fft, hop, win_length, T,
-                                                                               dcrm);
-  FSN_CHECK_LAUNCH("istft_mask_adjoint_kernel");
-  return FSN_OK;
+  return dsp_launch(dft_size_ok(n_fft) ? istft_mask_adjoint_kernel<DirectDft> : istft_mask_adjoint_kernel<Radix2>,
+                    dim3(cdiv(T, kFR), B), dsp_smem_bytes(n_fft, kFR / 2), st, "istft_mask_adjoint_kernel", dwav, real,
+                    imag, L, n_fft, hop, win_length, T, dcrm);
 }
 
 int istft_launch(const float* real, const float* imag, int cstride, const float* crm, int B, int T, int n_fft,
@@ -536,22 +593,10 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
     if (rc) return rc;
   }
   const int out_len = length > 0 ? length : hop * (T - 1);
-  if (dft_size_ok(n_fft))
-    return istft_dft_launch(real, imag, cstride, crm, mask_mode, B, T, n_fft, hop, win_length, out_len, wav, st, peak_bits,
-                            lens);
   const int seg = kFR * hop;
-  const int np_max = (kFR + cdiv(n_fft, hop) + 2) / 2;
-  const size_t smem = istft_smem_bytes(n_fft, hop);
-  if (smem > 48 * 1024) {
-    rc = check_cuda(cudaFuncSetAttribute(istft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                    "istft smem attr");
-    if (rc) return rc;
-  }
-  dim3 grid(cdiv(out_len, seg), B);
-  istft_kernel<<<grid, kDspThreads, smem, st>>>(real, imag, cstride, crm, mask_mode, T, n_fft, hop, win_length, out_len,
-                                                seg, np_max, wav, peak_bits, lens);
-  FSN_CHECK_LAUNCH("istft_kernel");
-  return FSN_OK;
+  return dsp_launch(dft_size_ok(n_fft) ? istft_kernel<DirectDft> : istft_kernel<Radix2>, dim3(cdiv(out_len, seg), B),
+                    istft_smem_bytes(n_fft, hop), st, "istft_kernel", real, imag, cstride, crm, mask_mode, T, n_fft, hop,
+                    win_length, out_len, seg, istft_np_max(n_fft, hop), wav, peak_bits, lens);
 }
 
 }  // namespace fsn

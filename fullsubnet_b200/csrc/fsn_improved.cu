@@ -114,13 +114,10 @@ static SeqStack imp_fb_stack(const fsn_improved_desc* d, const ImpDims& m) {
   return s;
 }
 
-static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
-
 int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
   FSN_REQUIRE(d && B > 0 && L > 0, FSN_ERR_SHAPE, "improved model: empty input");
-  FSN_REQUIRE((is_pow2(d->n_fft) && d->n_fft <= 2048) || (d->n_fft % 2 == 0 && d->n_fft >= 16 && d->n_fft <= 1200),
-              FSN_ERR_UNSUPPORTED, "improved model: n_fft=%d unsupported (power of two <= 2048, or even and <= 1200)",
-              d->n_fft);
+  FSN_REQUIRE(dsp_size_ok(d->n_fft), FSN_ERR_UNSUPPORTED,
+              "improved model: n_fft=%d unsupported (power of two <= 2048, or even and <= 1200)", d->n_fft);
   FSN_REQUIRE(d->num_freqs == d->n_fft / 2 + 1, FSN_ERR_SHAPE, "improved model: num_freqs != n_fft/2+1");
   FSN_REQUIRE(d->num_sections >= 1 && d->num_sections <= FSN_IMP_MAX_SECTIONS, FSN_ERR_SHAPE, "improved model: sections");
   FSN_REQUIRE(d->precision == FSN_PREC_FP32 || (d->precision == FSN_PREC_TF32_TC && (d->sb_hidden & 3) == 0),

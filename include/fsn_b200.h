@@ -232,7 +232,7 @@ int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_weights* w, co
  *   wav -> STFT -> |X|^fdrc, Nyquist bin dropped -> norm -> full-band 2xLSTM + Linear -> per sub-band section:
  *   strided unfold (centre/neighbour widths) of noisy and full-band output, concat, per-section norm, 2xLSTM +
  *   Linear(2*centre) -> cRM (Nyquist row 0) -> element-wise mask on (re, im) -> iSTFT -> wav.  n_fft: a power of two
- *   <= 2048 (radix-2 FFT), or even and <= 1200 (direct DFT; the reference's 48 kHz example uses n_fft = 960).
+ *   in [16, 2048] (radix-2 FFT), or even in [16, 1200] (direct DFT; the reference's 48 kHz example uses n_fft = 960).
  * ---------------------------------------------------------------------------------------- */
 #define FSN_IMP_MAX_SECTIONS 8
 typedef struct fsn_improved_desc {
@@ -568,9 +568,9 @@ int fsn_debug_seq_stack(const fsn_lstm_layer* layers, int n, const int* H, int R
                         const float* fc_b, int O, int act, float* out, void* workspace, size_t workspace_bytes, int* path,
                         fsn_stream_t stream);
 
-/* unit-test hooks for the signal layer (fsn_dsp.cu, fsn_dsp_dft.cu; torch.stft / torch.istft with center=True, reflect
- * padding and a periodic Hann window of win_length centred in n_fft): the internal launchers behind fsn_stft, fsn_istft and
- * the wav -> wav entry points, called directly.  n_fft a power of two in [16, 2048] (radix-2 kernels) or even in [16, 1200]
+/* unit-test hooks for the signal layer (fsn_dsp.cu; torch.stft / torch.istft with center=True, reflect padding and a
+ * periodic Hann window of win_length centred in n_fft): the internal launchers behind fsn_stft, fsn_istft and the
+ * wav -> wav entry points, called directly.  n_fft a power of two in [16, 2048] (radix-2 FFT) or even in [16, 1200]
  * (direct DFT); B <= 65535; the iSTFT refuses a hop whose frames would not fit in shared memory (FSN_ERR_UNSUPPORTED).
  * lengths (nullable, host [B]): per-clip lengths n_fft/2 < lengths[b] <= L (iSTFT: <= its output length), max == L, copied
  * to lens_dev (device [B]) through the kernel parameters.

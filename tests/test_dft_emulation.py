@@ -1,6 +1,7 @@
-"""CPU emulation of the index arithmetic of fullsubnet_b200/csrc/fsn_dsp_dft.cu (two real frames packed into one
-complex direct DFT, un-packing, Hermitian extension, overlap-add segments) against the oracle STFT / iSTFT.
-It pins the ALGORITHM of the non-power-of-two kernels on the CPU; the kernels themselves are checked on the GPU
+"""CPU emulation of the index arithmetic of the STFT / iSTFT kernels of fullsubnet_b200/csrc/fsn_dsp.cu on their
+direct-DFT policy (the shared framing: two real frames packed into one complex direct DFT, un-packing, Hermitian
+extension, overlap-add segments) against the oracle STFT / iSTFT.
+It pins the ALGORITHM of the non-power-of-two path on the CPU; the kernels themselves are checked on the GPU
 (tests/test_gpu_parity.py::test_non_power_of_two_stft_istft)."""
 import numpy as np
 import pytest

@@ -1,6 +1,6 @@
-"""The signal layer alone against float64: the STFT, iSTFT and iSTFT-mask-adjoint kernels (radix-2, fsn_dsp.cu, and direct
-DFT, fsn_dsp_dft.cu) and the wav epilogue through their unit-test hooks, against the reference of tests/test_cpu_dsp.py
-(itself pinned to torch.stft / torch.istft / autograd in float64).
+"""The signal layer alone against float64: the STFT, iSTFT and iSTFT-mask-adjoint kernels of fsn_dsp.cu on both transform
+policies (radix-2 FFT and direct DFT) and the wav epilogue through their unit-test hooks, against the reference of
+tests/test_cpu_dsp.py (itself pinned to torch.stft / torch.istft / autograd in float64).
 
 Every call also checks: the guard floats past each output are untouched, every output element is written, two runs give
 the same bits, and a clip inside a batch gives the bits it gives alone.  Error bounds are about 4x the worst error

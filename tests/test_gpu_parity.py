@@ -329,7 +329,7 @@ def test_cumulative_laplace_norm_matches_reference(golden, dev):
             WAV_TOL if prec != "f16_tc" else 1e-2), prec
 
 
-# ------------------------------------------------------------------ n_fft = 960 (direct-DFT kernels, fsn_dsp_dft.cu)
+# ------------------------------------------------------------------ n_fft = 960 (the direct-DFT policy of fsn_dsp.cu)
 def test_non_power_of_two_stft_istft(golden, dev):
     from fullsubnet_b200.acoustics.feature import stft, istft
     g = golden("improved_960")
