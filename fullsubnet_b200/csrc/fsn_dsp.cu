@@ -491,11 +491,6 @@ __global__ void si_sdr_kernel(const float* __restrict__ ref, const float* __rest
   if (threadIdx.x == 0) out[blockIdx.x] = (float)(10.0 * log10(sa[0] / sb[0]));
 }
 
-static int ew_grid(int64_t n) {
-  int64_t g = (n + 255) / 256;
-  return (int)(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
-}
-
 static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
 
 // the transform policy: DirectDft for these sizes, Radix2 for the powers of two
@@ -675,12 +670,12 @@ int wav_epilogue(const WavWs& w, const float* enhanced, int B, int L, int16_t* p
                  int hop, cudaStream_t st) {
   if (pcm) {
     const size_t n = (size_t)B * L;
-    scale_int16_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(enhanced, w.peak, L, gain, pcm, n, w.lens);
+    scale_int16_kernel<<<ew_grid((size_t)n), 256, 0, st>>>(enhanced, w.peak, L, gain, pcm, n, w.lens);
     FSN_CHECK_LAUNCH("scale_int16_kernel");
   }
   if (w.lens && crm_out) {
     const size_t n = (size_t)B * 2 * F * T;
-    zero_frames_past_kernel<<<ew_grid((int64_t)n), 256, 0, st>>>(crm_out, w.lens, 2 * F, T, hop, n);
+    zero_frames_past_kernel<<<ew_grid((size_t)n), 256, 0, st>>>(crm_out, w.lens, 2 * F, T, hop, n);
     FSN_CHECK_LAUNCH("zero_frames_past_kernel");
   }
   return FSN_OK;
@@ -755,14 +750,14 @@ extern "C" int fsn_debug_wav_epilogue(const float* enhanced, const unsigned int*
 extern "C" int fsn_decompress_cirm(const float* in, float* out, int64_t n, float K, float limit,
                                    fsn_stream_t stream) {
   if (n <= 0) return FSN_OK;
-  decompress_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(in, out, n, K, limit);
+  decompress_kernel<<<ew_grid((size_t)n), 256, 0, (cudaStream_t)stream>>>(in, out, n, K, limit);
   FSN_CHECK_LAUNCH("decompress_kernel");
   return FSN_OK;
 }
 
 extern "C" int fsn_compress_cirm(const float* in, float* out, int64_t n, float K, float C, fsn_stream_t stream) {
   if (n <= 0) return FSN_OK;
-  compress_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(in, out, n, K, C);
+  compress_kernel<<<ew_grid((size_t)n), 256, 0, (cudaStream_t)stream>>>(in, out, n, K, C);
   FSN_CHECK_LAUNCH("compress_kernel");
   return FSN_OK;
 }
@@ -770,7 +765,7 @@ extern "C" int fsn_compress_cirm(const float* in, float* out, int64_t n, float K
 extern "C" int fsn_build_cirm(const float* nr, const float* ni, const float* cr, const float* ci, float* out,
                               int64_t n, fsn_stream_t stream) {
   if (n <= 0) return FSN_OK;
-  build_cirm_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(nr, ni, cr, ci, reinterpret_cast<float2*>(out), n);
+  build_cirm_kernel<<<ew_grid((size_t)n), 256, 0, (cudaStream_t)stream>>>(nr, ni, cr, ci, reinterpret_cast<float2*>(out), n);
   FSN_CHECK_LAUNCH("build_cirm_kernel");
   return FSN_OK;
 }
@@ -781,7 +776,7 @@ extern "C" int fsn_drop_band(const float* in, float* out, int B, int C, int F, i
   FSN_REQUIRE(G >= 2, FSN_ERR_SHAPE, "drop_band: G < 2 is the identity, handle on the host");
   const int64_t n = (int64_t)B * C * (F / G) * T;
   if (n <= 0) return FSN_OK;
-  drop_band_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(in, out, B, C, F, T, G);
+  drop_band_kernel<<<ew_grid((size_t)n), 256, 0, (cudaStream_t)stream>>>(in, out, B, C, F, T, G);
   FSN_CHECK_LAUNCH("drop_band_kernel");
   return FSN_OK;
 }

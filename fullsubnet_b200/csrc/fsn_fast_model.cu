@@ -1,49 +1,14 @@
 // fast_fullsubnet (recipes/dns_interspeech_2020/fast_fullsubnet/model.py:11-202, BASELINE config 4): host
-// orchestration and the few extra kernels on top of the shared fp32 building blocks (mel filtering, real-time
-// down/up-sampling, bottleneck input, decoder re-layout).
+// orchestration and the second cumulative norm on top of the shared fp32 building blocks (mel filtering as a GEMM, the
+// bottleneck input with its real-time down-sampling and the decoder input with its up-sampling in fsn_lstm_simt.cu).
 #include <string.h>
 
 #include "fsn_internal.cuh"
 
 namespace fsn {
 
-// bottleneck input (model.py:174-187 before the norm): row (b,m), feature k: 2Nn+1 reflected mel rows + 2Ne+1
-// encoder-output rows, down-sampled in time (first frame alone, then means of `S` frames; the last block over its
-// own length).  One CTA per (b, ts): writes bn[ts][b*M+m][k] and the deterministic per-(b,ts) sum.
-__global__ void fast_bn_input_kernel(const float* __restrict__ melT, const float* __restrict__ encT, int B, int Tp,
-                                     int M, int Nn, int Ne, int S, int Ts, float* __restrict__ bn,
-                                     float2* __restrict__ fs) {
-  __shared__ float red[256];
-  const int b = blockIdx.x / Ts, ts = blockIdx.x % Ts;
-  const int K = (2 * Nn + 1) + (2 * Ne + 1);
-  int t0, t1;  // frames [t0, t1) averaged into this shrunk frame
-  if (ts == 0) { t0 = 0; t1 = 1; }
-  else { t0 = 1 + (ts - 1) * S; t1 = min(t0 + S, Tp); }
-  const float inv = 1.0f / (float)(t1 - t0);
-  float local = 0.f;
-  for (int i = threadIdx.x; i < M * K; i += blockDim.x) {
-    const int m = i / K, k = i - m * K;
-    float acc = 0.f;
-    for (int t = t0; t < t1; ++t) {
-      const size_t base = ((size_t)b * Tp + t) * M;
-      acc += (k < 2 * Nn + 1) ? melT[base + reflect_idx(m + k - Nn, M)]
-                              : encT[base + reflect_idx(m + (k - (2 * Nn + 1)) - Ne, M)];
-    }
-    const float v = acc * inv;
-    bn[((size_t)ts * B * M + (size_t)b * M + m) * K + k] = v;
-    local += v;
-  }
-  red[threadIdx.x] = local;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) fs[(size_t)b * Ts + ts] = make_float2(red[0], red[0]);
-}
-
 // second cumulative norm (model.py:186-187 -> base_model.py:220-251 on [B*M, K, Ts]): one thread per row (b,m), sequential
-// over the shrunk steps; the row sum of each step runs over the K block means fast_bn_input_kernel / ftr_bn_input_kernel
+// over the shrunk steps; the row sum of each step runs over the K block means fast_bn_input_launch
 // wrote, so inference and training share the scales
 __global__ void fast_cum_bn_scale_kernel(const float* __restrict__ bn, int R, int K, int Ts, float eps,
                                          float* __restrict__ scaleT) {
@@ -63,43 +28,6 @@ int fast_cum_bn_scale_launch(const float* bn, int R, int K, int Ts, float eps, f
   fast_cum_bn_scale_kernel<<<cdiv(R, 128), 128, 0, st>>>(bn, R, K, Ts, eps, scaleT);
   FSN_CHECK_LAUNCH("fast_cum_bn_scale_kernel");
   return FSN_OK;
-}
-
-// decoder input (model.py:194): [enc_out (M) | up-sampled bottleneck output (M)] per (b,t); frame t of the
-// up-sampled signal is shrunk frame t / S (model.py:131-140)
-// bn_out element (b, m, ts) lives at bn_out[(b*bn_bstride + m) * Ts + ts]: bn_bstride = M for the fp32 path
-// ([B*M, Ts]) and 2*M for the tensor-core path, which writes a [B,2,M,Ts] tensor whose channel 0 is the output
-__global__ void fast_dec_input_kernel(const float* __restrict__ encT, const float* __restrict__ bn_out, int bn_bstride,
-                                      int B, int Tp, int M, int S, int Ts, float* __restrict__ dec_in) {
-  const size_t total = (size_t)B * Tp * 2 * M;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % (2 * M));
-    const size_t bt = i / (2 * M);
-    const int t = (int)(bt % Tp), b = (int)(bt / Tp);
-    float v;
-    if (c < M) v = encT[bt * M + c];
-    else       v = bn_out[((size_t)b * bn_bstride + (c - M)) * Ts + min(t / S, Ts - 1)];
-    dec_in[i] = v;
-  }
-}
-
-// dec [B,Tp,2F] (channel c*F+f) -> out [B,2,F,T], dropping the first `la` frames (model.py:197-200)
-__global__ void fast_output_kernel(const float* __restrict__ dec, int B, int Tp, int F, int la, float* __restrict__ out) {
-  __shared__ float tile[32][33];
-  const int T = Tp - la;
-  const int bc = blockIdx.z;                 // b*2 + c
-  const int b = bc >> 1, c = bc & 1;
-  const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  for (int i = ty; i < 32; i += 8) {         // read: f contiguous
-    const int t = t0 + i, f = f0 + tx;
-    tile[i][tx] = (t < T && f < F) ? dec[((size_t)b * Tp + t + la) * (2 * F) + c * F + f] : 0.f;
-  }
-  __syncthreads();
-  for (int i = ty; i < 32; i += 8) {         // write: t contiguous
-    const int f = f0 + i, t = t0 + tx;
-    if (f < F && t < T) out[(((size_t)b * 2 + c) * F + f) * T + t] = tile[tx][i];
-  }
 }
 
 // GRU: the inference kernels of this model are built for LSTM only
@@ -217,7 +145,7 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   cudaStream_t st = (cudaStream_t)stream;
   const int Tp = m.Tp, M = m.M, F = m.F, R = B * M;
   // look-ahead pad + time-major layout, Mel filtering (model.py:161-166)
-  if ((rc = transpose_mag_launch(mix_mag, w.magT, B, F, T, Tp, st))) return rc;
+  if ((rc = transpose_mag_launch(mix_mag, B, F, T, Tp, (size_t)Tp * F, F, w.magT, nullptr, nullptr, st))) return rc;
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, B * Tp, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true)))
     return rc;
   // encoder input norm (model.py:170): per-clip mean of the mel spectrogram incl. the look-ahead frames, or (cumulative
@@ -235,9 +163,9 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   enc.fc_w = wt->enc_fc_w; enc.fc_b = wt->enc_fc_b; enc.out = w.encT;
   if ((rc = seq_stack_forward(enc, w.seq, st))) return rc;
   // bottleneck input: unfold + concat + real-time down-sampling, then its norm (model.py:174-187)
-  fast_bn_input_kernel<<<B * m.Ts, 256, 0, st>>>(w.melT, w.encT, B, Tp, M, d->noisy_num_neighbors,
-                                                 d->enc_num_neighbors, m.S, m.Ts, w.bn, w.fs);
-  FSN_CHECK_LAUNCH("fast_bn_input_kernel");
+  if ((rc = fast_bn_input_launch(w.melT, w.encT, (size_t)Tp * M, M, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors,
+                                 m.S, m.Ts, w.bn, w.fs, st)))
+    return rc;
   if (m.cum) {
     // per-(shrunk step, row) running mean over the K block means, time-major cum2[ts*R + r]
     if ((rc = fast_cum_bn_scale_launch(w.bn, R, m.K, m.Ts, TRAIN_CUM_EPS, w.cum2, st))) return rc;
@@ -247,6 +175,7 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
     if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)M * m.K * m.Ts, 1.f, w.inv2, nullptr, st))) return rc;
   }
   // S: 2xLSTM(K->Hb->Hb) + Linear(1) + ReLU on B*M rows over Ts steps (model.py:188-189)
+  // bn_out element (b, m, ts): [B*M, Ts] from the fp32 path, channel 0 of the [B,2,M,Ts] the tensor-core kernel writes
   const int Hb = d->bn_hidden;
   int bn_bstride = M;
   if (fast_is_tc(d)) {
@@ -275,26 +204,19 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
       if (m.cum) { p.row_scale = w.cum2 + (size_t)t * R; p.row_scale_div = 1; }
       else       { p.row_scale = w.inv2; p.row_scale_div = M; }
       if ((rc = lstm_step2_launch(p, SEG0_DENSE, t, wt->bn[1], s2, st))) return rc;
-      if ((rc = rows_fc_launch(s2.h1_at(t), R, Hb, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out + t, (size_t)m.Ts, 0,
-                               st)))
+      if ((rc = sb_head_launch(s2.h1_at(t), R, Hb, 1, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out,
+                               HeadGeom{R, 1, 0, 0, (size_t)m.Ts}, t, st)))
         return rc;
     }
   }
   // up-sampling + concat with the encoder output (model.py:191-194)
-  {
-    const size_t n = (size_t)B * Tp * 2 * M;
-    int g = (int)((n + 255) / 256);
-    if (g > 132 * 16) g = 132 * 16;
-    fast_dec_input_kernel<<<g, 256, 0, st>>>(w.encT, w.bn_out, bn_bstride, B, Tp, M, m.S, m.Ts, w.dec_in);
-    FSN_CHECK_LAUNCH("fast_dec_input_kernel");
-  }
+  if ((rc = fast_dec_input_launch(w.encT, w.bn_out, (size_t)bn_bstride * m.Ts, m.Ts, 1, B, Tp, M, m.S, m.Ts, Tp, 1, w.dec_in,
+                                  st)))
+    return rc;
   // F_m2l: LSTM(2M->Hd), LSTM(Hd->Hd) + Linear(2F) (model.py:77-96,196)
   SeqStack dec = fast_pair(d, m, 2 * M, d->dec_hidden, d->dec_hidden, 2 * F, FSN_ACT_NONE);
   dec.L[0] = wt->dec1; dec.L[1] = wt->dec2;
   dec.x = w.dec_in; dec.fc_w = wt->dec_fc_w; dec.fc_b = wt->dec_fc_b; dec.out = w.dec_out;
   if ((rc = seq_stack_forward(dec, w.seq, st))) return rc;
-  dim3 grid(cdiv(T, 32), cdiv(F, 32), B * 2);
-  fast_output_kernel<<<grid, dim3(32, 8), 0, st>>>(w.dec_out, B, Tp, F, d->look_ahead, out);
-  FSN_CHECK_LAUNCH("fast_output_kernel");
-  return FSN_OK;
+  return crm_output_launch(w.dec_out, (size_t)Tp * 2 * F, 2 * F, B, Tp, F, d->look_ahead, out, st);
 }

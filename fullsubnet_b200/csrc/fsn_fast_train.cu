@@ -11,83 +11,6 @@
 
 namespace fsn {
 
-// ------------------------------------------------------------------------------------------ forward kernels
-// mag [B,F,T] -> magT [Tp,B,F], zero look-ahead frames (model.py:161)
-__global__ void ftr_transpose_kernel(const float* __restrict__ mag, float* __restrict__ magT, int B, int F, int T, int Tp) {
-  __shared__ float tile[32][33];
-  const int b = blockIdx.z, f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  for (int i = ty; i < 32; i += 8) {
-    const int f = f0 + i, t = t0 + tx;
-    tile[i][tx] = (f < F && t < T) ? mag[((size_t)b * F + f) * T + t] : 0.f;
-  }
-  __syncthreads();
-  for (int i = ty; i < 32; i += 8) {
-    const int t = t0 + i, f = f0 + tx;
-    if (t < Tp && f < F) magT[((size_t)t * B + b) * F + f] = tile[tx][i];
-  }
-}
-
-// out[i] = in[i] * scale[(i / cols) % B / div]  (rows of a [steps, B*div, cols] tensor scaled per clip)
-__global__ void ftr_scale_kernel(const float* __restrict__ in, const float* __restrict__ scale, size_t n, int cols, int rows,
-                                 int div, float* __restrict__ out) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    out[i] = in[i] * scale[(int)((i / cols) % rows) / div];
-}
-
-// first frame of shrunk step ts and the number of frames averaged into it (model.py:108-129)
-__device__ __forceinline__ void shrink_block(int ts, int S, int Tp, int& t0, int& len) {
-  if (ts == 0) { t0 = 0; len = 1; return; }
-  t0 = 1 + (ts - 1) * S;
-  len = min(t0 + S, Tp) - t0;
-}
-
-// bottleneck input before its norm (model.py:174-187), time-major sources melT / encT [Tp,B,M]: row (b,m) of shrunk step
-// ts, feature k = 2Nn+1 reflected noisy-mel rows || 2Ne+1 reflected encoder rows, averaged over the block of ts.  One CTA
-// per (b, ts): bn[ts][b*M+m][k] and the fixed-order sum fs[b*Ts+ts] (the layout clip_reduce_only_launch reads)
-__global__ void ftr_bn_input_kernel(const float* __restrict__ melT, const float* __restrict__ encT, int B, int Tp, int M,
-                                    int Nn, int Ne, int S, int Ts, float* __restrict__ bn, float2* __restrict__ fs) {
-  __shared__ float red[256];
-  const int b = blockIdx.x / Ts, ts = blockIdx.x % Ts;
-  const int K = (2 * Nn + 1) + (2 * Ne + 1);
-  int t0, len;
-  shrink_block(ts, S, Tp, t0, len);
-  const float inv = 1.0f / (float)len;
-  float local = 0.f;
-  for (int i = threadIdx.x; i < M * K; i += blockDim.x) {
-    const int m = i / K, k = i - m * K;
-    float acc = 0.f;
-    for (int t = t0; t < t0 + len; ++t) {
-      const size_t base = ((size_t)t * B + b) * M;
-      acc += (k < 2 * Nn + 1) ? melT[base + reflect_idx(m + k - Nn, M)]
-                              : encT[base + reflect_idx(m + (k - (2 * Nn + 1)) - Ne, M)];
-    }
-    const float v = acc * inv;
-    bn[((size_t)ts * B * M + (size_t)b * M + m) * K + k] = v;
-    local += v;
-  }
-  red[threadIdx.x] = local;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) fs[(size_t)b * Ts + ts] = make_float2(red[0], red[0]);
-}
-
-// decoder input dec_in [Tp,B,2M] = [encoder output | up-sampled bottleneck output] (model.py:191-194): frame t reads shrunk
-// step min(t/S, Ts-1) of bn_out [Ts, B*M]
-__global__ void ftr_dec_input_kernel(const float* __restrict__ encT, const float* __restrict__ bn_out, int B, int Tp, int M,
-                                     int S, int Ts, float* __restrict__ dec_in) {
-  const size_t n = (size_t)Tp * B * 2 * M;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int c = (int)(i % (2 * M));
-    const size_t tb = i / (2 * M);
-    const int b = (int)(tb % B), t = (int)(tb / B);
-    dec_in[i] = c < M ? encT[tb * M + c] : bn_out[(size_t)min(t / S, Ts - 1) * B * M + (size_t)b * M + (c - M)];
-  }
-}
-
 // ------------------------------------------------------------------------------------------ backward kernels
 // transpose of the up-sampling (frame t <- shrunk step min(t/S, Ts-1)) on the bottleneck half of d dec_in, times ReLU' of
 // the bottleneck output: dbn[ts, r] = [bn_out > 0] * sum over the frames that read ts (ascending t)
@@ -293,11 +216,6 @@ static const fsn_lstm_layer& layer_weights(const fsn_fast_weights* wt, int l) {
   }
 }
 
-static int grid_for(size_t n) {
-  size_t g = (n + 255) / 256;
-  return (int)(g > 132 * 16 ? 132 * 16 : (g ? g : 1));
-}
-
 }  // namespace fsn
 
 using namespace fsn;
@@ -332,23 +250,19 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
                          &half, st);
   };
   // look-ahead pad + time-major layout, Mel filtering (model.py:161-166)
-  ftr_transpose_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(mix_mag, w.magT, B, F, T, Tp);
-  FSN_CHECK_LAUNCH("ftr_transpose_kernel");
+  if ((rc = transpose_mag_launch(mix_mag, B, F, T, Tp, F, (size_t)B * F, w.magT, nullptr, nullptr, st))) return rc;
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, Tp * B, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true))) return rc;
   // first norm (model.py:170): the mel spectrogram has no parameter behind it, only the normalised copy is kept;
   // cumulative norm: one scale per (frame, clip) from the running mean over the mel bins
   if (m.cum) {
-    train_frame_sum_kernel<<<cdiv(Tp * B, 8), 256, 0, st>>>(w.melT, B, M, Tp, w.fs1);
-    FSN_CHECK_LAUNCH("train_frame_sum_kernel");
+    if ((rc = frame_stats_launch(w.melT, B, Tp, M, 0, M, (size_t)B * M, w.fs1, st))) return rc;
     if ((rc = cum_clip_scale_launch(w.fs1, B, Tp, M, TRAIN_CUM_EPS, w.cum1, st))) return rc;
-    train_scale_tm_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.melT, w.cum1, M, (size_t)Tp * B * M, w.xenc);
-    FSN_CHECK_LAUNCH("train_scale_tm_kernel");
+    if ((rc = scale_rows_launch(w.melT, w.cum1, (size_t)Tp * B * M, M, Tp * B, 1, w.xenc, st))) return rc;
   } else {
     train_tm_stats_kernel<<<B, 256, 0, st>>>(w.melT, B, M, Tp, 0, w.sums1);
     FSN_CHECK_LAUNCH("train_tm_stats_kernel");
     if ((rc = norm_scales_launch(w.sums1, w.sums1, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) return rc;
-    ftr_scale_kernel<<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(w.melT, w.inv1, (size_t)Tp * B * M, M, B, 1, w.xenc);
-    FSN_CHECK_LAUNCH("ftr_scale_kernel");
+    if ((rc = scale_rows_launch(w.melT, w.inv1, (size_t)Tp * B * M, M, B, 1, w.xenc, st))) return rc;
   }
   // encoder: LSTM(M->He1), LSTM(He1->He2) + Linear(M) + ReLU (model.py:35-54,171)
   if ((rc = layer(L_ENC1, w.xenc, nullptr))) return rc;
@@ -356,32 +270,30 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   if ((rc = fc_gemm_launch(w.L[L_ENC2].H, wt->enc_fc_w, wt->enc_fc_b, w.encT, Tp * B, d->enc2_hidden, M, FSN_ACT_RELU, st)))
     return rc;
   // bottleneck input: unfold + concat + down-sampling, its norm; the normalised input is kept (model.py:174-187)
-  ftr_bn_input_kernel<<<B * Ts, 256, 0, st>>>(w.melT, w.encT, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
-                                              Ts, w.xbn, w.fs);
-  FSN_CHECK_LAUNCH("ftr_bn_input_kernel");
+  if ((rc = fast_bn_input_launch(w.melT, w.encT, M, (size_t)B * M, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors,
+                                 m.S, Ts, w.xbn, w.fs, st)))
+    return rc;
   if (m.cum) {  // per-(shrunk step, row) scales, kept in cum2 for the backward
     if ((rc = fast_cum_bn_scale_launch(w.xbn, R, K, Ts, TRAIN_CUM_EPS, w.cum2, st))) return rc;
-    train_scale_tm_kernel<<<grid_for((size_t)Ts * R * K), 256, 0, st>>>(w.xbn, w.cum2, K, (size_t)Ts * R * K, w.xbn);
-    FSN_CHECK_LAUNCH("train_scale_tm_kernel");
+    if ((rc = scale_rows_launch(w.xbn, w.cum2, (size_t)Ts * R * K, K, Ts * R, 1, w.xbn, st))) return rc;
   } else {
     if ((rc = clip_reduce_only_launch(w.fs, B, Ts, w.sums2, st))) return rc;
     if ((rc = norm_scales_launch(w.sums2, w.sums2, B, (float)M * K * Ts, 1.f, w.inv2, nullptr, st))) return rc;
-    ftr_scale_kernel<<<grid_for((size_t)Ts * R * K), 256, 0, st>>>(w.xbn, w.inv2, (size_t)Ts * R * K, K, R, M, w.xbn);
-    FSN_CHECK_LAUNCH("ftr_scale_kernel");
+    if ((rc = scale_rows_launch(w.xbn, w.inv2, (size_t)Ts * R * K, K, R, M, w.xbn, st))) return rc;
   }
   // bottleneck 2xLSTM(K->Hb->Hb) + Linear(1) + ReLU over Ts steps (model.py:188-189)
   if ((rc = layer(L_BN0, w.xbn, nullptr))) return rc;
   if ((rc = layer(L_BN1, w.L[L_BN0].H, w.h16[L_BN0]))) return rc;
-  if ((rc = rows_fc_launch(w.L[L_BN1].H, Ts * R, d->bn_hidden, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out, 1, 0, st)))
+  if ((rc = sb_head_launch(w.L[L_BN1].H, Ts * R, d->bn_hidden, 1, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bn_out,
+                           HeadGeom{Ts * R, 1, 0, 0, 1}, 0, st)))
     return rc;
   // up-sampling + concat, decoder LSTM(2M->Hd), LSTM(Hd->Hd) + Linear(2F) (model.py:191-196)
-  ftr_dec_input_kernel<<<grid_for((size_t)Tp * B * 2 * M), 256, 0, st>>>(w.encT, w.bn_out, B, Tp, M, m.S, Ts, w.dec_in);
-  FSN_CHECK_LAUNCH("ftr_dec_input_kernel");
+  if ((rc = fast_dec_input_launch(w.encT, w.bn_out, M, 1, (size_t)B * M, B, Tp, M, m.S, Ts, 1, B, w.dec_in, st))) return rc;
   if ((rc = layer(L_DEC1, w.dec_in, nullptr))) return rc;
   if ((rc = layer(L_DEC2, w.L[L_DEC1].H, w.h16[L_DEC1]))) return rc;
   if ((rc = fc_gemm_launch(w.L[L_DEC2].H, wt->dec_fc_w, wt->dec_fc_b, w.dec_out, Tp * B, d->dec_hidden, 2 * F, FSN_ACT_NONE, st)))
     return rc;
-  return train_output_launch(w.dec_out, B, Tp, F, d->look_ahead, out, st);
+  return crm_output_launch(w.dec_out, 2 * F, (size_t)B * 2 * F, B, Tp, F, d->look_ahead, out, st);
 }
 
 extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* dout, int B, int T,
@@ -421,7 +333,7 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   if ((rc = layer_weight_grads(L[L_DEC1], Tp, w.dec_in, g->dec1.w_ih, g->dec1.w_hh, g->dec1.b_ih, g->dec1.b_hh, wg, st)))
     return rc;
   // ---- up-sampling transpose + ReLU' of the bottleneck output, its Linear(1)
-  ftr_dbn_kernel<<<grid_for((size_t)Ts * R), 256, 0, st>>>(w.ddec, w.bn_out, B, Tp, M, m.S, Ts, w.dbn);
+  ftr_dbn_kernel<<<ew_grid((size_t)Ts * R), 256, 0, st>>>(w.ddec, w.bn_out, B, Tp, M, m.S, Ts, w.dbn);
   FSN_CHECK_LAUNCH("ftr_dbn_kernel");
   if ((rc = linear_bwd(w.dbn, w.L[L_BN1].H, wt->bn_fc_w, Ts * R, 1, Hb, g->bn_fc_w, g->bn_fc_b, nullptr, w.splitk, w.colsum,
                        st)))
@@ -436,13 +348,13 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   if (m.cum) {
     ftr_cum_suffix_kernel<<<cdiv(R, 128), 128, 0, st>>>(w.dxbn, w.xbn, w.cum2, Ts, R, K, w.suffix);
     FSN_CHECK_LAUNCH("ftr_cum_suffix_kernel");
-    ftr_denc_kernel<true><<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(
+    ftr_denc_kernel<true><<<ew_grid((size_t)Tp * B * M), 256, 0, st>>>(
         w.ddec, w.dxbn, w.encT, nullptr, nullptr, w.cum2, w.suffix, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors,
         m.S, 0.f, w.denc);
   } else {
     train_dot_kernel<<<B, 256, 0, st>>>(w.dxbn, w.xbn, Ts, R, M, K, w.dot);
     FSN_CHECK_LAUNCH("train_dot_kernel");
-    ftr_denc_kernel<false><<<grid_for((size_t)Tp * B * M), 256, 0, st>>>(
+    ftr_denc_kernel<false><<<ew_grid((size_t)Tp * B * M), 256, 0, st>>>(
         w.ddec, w.dxbn, w.encT, w.inv2, w.dot, nullptr, nullptr, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
         (float)M * K * Ts, w.denc);
   }

@@ -1,26 +1,12 @@
 // fullband_baseline (recipes/dns_interspeech_2020/fullband_baseline/model.py:8-68; SURVEY 8f rank 3):
 // look-ahead pad -> norm -> num_layers x LSTM(F -> H) -> Linear(H -> 2F) [+ activation] -> [B,2,F,T].
-// Host orchestration: the norm, the SequenceModel of fsn_fullband.cu (seq_stack_forward) and one re-layout kernel;
+// Host orchestration: the norm, the SequenceModel of fsn_fullband.cu (seq_stack_forward) and the output re-layout;
 // fsn_fullband_enhance adds the STFT, the mask + iSTFT of Inferencer.full_band_crm_mask and the int16 output.
 #include <string.h>
 
 #include "fsn_internal.cuh"
 
 namespace fsn {
-
-// y [B, Tp, 2F] (row = clip-major, time) -> out [B, 2, F, T] dropping the first `la` steps (model.py:58-62)
-__global__ void fbb_output_kernel(const float* __restrict__ y, float* __restrict__ out, int B, int F, int T, int Tp,
-                                  int la) {
-  const size_t n = (size_t)B * 2 * F * T;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int t = (int)(i % T);
-    size_t q = i / T;
-    const int f = (int)(q % F); q /= F;
-    const int c = (int)(q & 1);
-    const size_t b = q >> 1;
-    out[i] = y[((b * Tp) + t + la) * (size_t)(2 * F) + (size_t)c * F + f];
-  }
-}
 
 struct FbbWs {
   float *magT, *inv1, *cum1, *y;
@@ -87,12 +73,7 @@ static int fbb_core(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, co
   for (int l = 0; l < s.n; ++l) s.L[l] = layers[l];
   s.x = w.magT; s.scale = cum ? w.cum1 : w.inv1; s.fc_w = fc_w; s.fc_b = fc_b; s.out = w.y;
   if ((rc = seq_stack_forward(s, w.seq, st))) return rc;
-  const size_t n = (size_t)B * 2 * F * T;
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  fbb_output_kernel<<<blocks, 256, 0, st>>>(w.y, out, B, F, T, Tp, la);
-  FSN_CHECK_LAUNCH("fbb_output_kernel");
-  return FSN_OK;
+  return crm_output_launch(w.y, (size_t)Tp * 2 * F, 2 * F, B, Tp, F, la, out, st);
 }
 
 static int fbb_enhance_dims(const fsn_fullband_desc* d, int B, int L, int n_fft, int hop, int& T) {
@@ -127,7 +108,8 @@ extern "C" int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_l
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, w.bytes);
   cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = transpose_mag_launch(noisy_mag, w.magT, B, d->num_freqs, T, T + d->look_ahead, st))) return rc;
+  const int F = d->num_freqs, Tp = T + d->look_ahead;
+  if ((rc = transpose_mag_launch(noisy_mag, B, F, T, Tp, (size_t)Tp * F, F, w.magT, nullptr, nullptr, st))) return rc;
   return fbb_core(d, layers, fc_w, fc_b, B, T, w, out, st);
 }
 

@@ -118,7 +118,7 @@ extern "C" int fsn_fullband_train_forward(const fsn_fullband_desc* d, const fsn_
   }
   // Linear(H -> 2F) + activation into y, kept for act' (model.py:58-62), then [B,2,F,T] without the look-ahead frames
   if ((rc = fc_gemm_launch(w.L[NL - 1].H, fc_w, fc_b, w.y, Tp * B, H, 2 * F, d->activation, st))) return rc;
-  return train_output_launch(w.y, B, Tp, F, d->look_ahead, out, st);
+  return crm_output_launch(w.y, 2 * F, (size_t)B * 2 * F, B, Tp, F, d->look_ahead, out, st);
 }
 
 extern "C" int fsn_fullband_train_backward(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,

@@ -59,40 +59,6 @@ __global__ void imp_section_input_kernel(const float* __restrict__ magc, const f
   if (threadIdx.x == 0) fs[(size_t)b * T + t] = make_float2(red[0], red[0]);
 }
 
-// Linear(H -> 2c) of one section for one frame, written into crm[b, ch, lo + n*c + j, t] with o = ch*c + j
-// (SubBandSequenceWrapper.forward, model.py:239-247); one warp per (row, output).  `steps` consecutive frames from t0:
-// h [steps, R, H]
-__global__ void imp_fc_step_kernel(const float* __restrict__ h, int R, int H, const float* __restrict__ W,
-                                   const float* __restrict__ bias, int c, int N, int lo, int act, float* __restrict__ crm,
-                                   int F, int T, int t0, int steps) {
-  const int O = 2 * c;
-  const size_t wid = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (wid >= (size_t)steps * R * O) return;
-  const size_t step_row = wid / O;
-  const int o = (int)(wid % O), t = t0 + (int)(step_row / R), row = (int)(step_row % R);
-  const float* hp = h + step_row * H;
-  float s = 0.f;
-  for (int k = lane; k < H; k += 32) s = fmaf(hp[k], W[(size_t)o * H + k], s);
-  s = warp_sum(s);
-  if (lane == 0) {
-    s += bias[o];
-    if (act == FSN_ACT_RELU) s = fmaxf(s, 0.f);
-    const int b = row / N, n = row - b * N, ch = o / c, j = o - ch * c;
-    crm[(((size_t)b * 2 + ch) * F + (lo + n * c + j)) * T + t] = s;
-  }
-}
-
-// X[t][r][w] = src[t][r][w] * inv[b(r)] with r = b*N + n (src may be X): element i of the [T, R*W] tensor belongs to
-// clip (i % (R*W)) / (N*W)
-__global__ void imp_scale_rows_kernel(const float* src, float* X, const float* __restrict__ inv, size_t n, size_t per_t,
-                                      size_t per_clip, int B) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const size_t b = (i % per_t) / per_clip;
-    X[i] = src[i] * inv[b < (size_t)B ? b : 0];
-  }
-}
-
 struct ImpWs {
   float *mag, *real, *imag, *crm, *magc, *fbT, *X, *inv1, *invs;
   float2 *fs, *sums;
@@ -213,21 +179,14 @@ static int imp_forward(const fsn_improved_desc* d, const fsn_improved_weights* w
     if (d->precision == FSN_PREC_TF32_TC) {
       // layer by layer over all steps: hoisted input projection + per-step recurrent GEMM on wgmma (tf32), fused cell
       LayerSave l1{w.tc.G, w.tc.C, w.tc_h1};
-      {  // scale X by the section norm in place (the tensor-core GEMM reads plain fp32 rows)
-        const size_t n = (size_t)T * R * g.W;
-        int blocks = (int)((n + 255) / 256);
-        if (blocks > 132 * 16) blocks = 132 * 16;
-        imp_scale_rows_kernel<<<blocks, 256, 0, st>>>(w.X, w.X, w.invs, n, (size_t)R * g.W, (size_t)g.N * g.W, B);
-        FSN_CHECK_LAUNCH("imp_scale_rows_kernel");
-      }
+      // scale X by the section norm in place (the tensor-core GEMM reads plain fp32 rows)
+      if ((rc = scale_rows_launch(w.X, w.invs, (size_t)T * R * g.W, g.W, R, g.N, w.X, st))) return rc;
       if ((rc = layer_forward_save_tc(seq_layer(sw, 0), w.X, R, g.W, Hs, T, w.tc, w.tc_rec, st))) return rc;
       if ((rc = layer_forward_save_tc(seq_layer(sw, 1), w.tc.H, R, Hs, Hs, T, l1, w.tc_rec, st))) return rc;
-      for (int t = 0; t < T; ++t) {
-        const size_t warps = (size_t)R * 2 * g.cs;
-        imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(w.tc_h1 + (size_t)t * R * Hs, R, Hs, sw.fc_w, sw.fc_b,
-                                                                    g.cs, g.N, g.lo, d->sb_activation, crm, F, T, t, 1);
-        FSN_CHECK_LAUNCH("imp_fc_step_kernel");
-      }
+      for (int t = 0; t < T; ++t)
+        if ((rc = sb_head_launch(w.tc_h1 + (size_t)t * R * Hs, R, Hs, 1, sw.fc_w, sw.fc_b, 2 * g.cs, d->sb_activation, crm,
+                                 imp_head_geom(g, F, T), t, st)))
+          return rc;
       continue;
     }
     const Step2State s2{{w.h0[0], w.h0[1]}, w.c0, {w.h1[0], w.h1[1]}, w.c1, Hs, 0};
@@ -238,10 +197,9 @@ static int imp_forward(const fsn_improved_desc* d, const fsn_improved_weights* w
       p.w_ih = sw.w_ih[0]; p.w_hh = sw.w_hh[0]; p.b_ih = sw.b_ih[0]; p.b_hh = sw.b_hh[0];
       p.x0 = w.X + (size_t)t * R * g.W; p.x0_row_stride = g.W; p.row_scale = w.invs; p.row_scale_div = g.N;
       if ((rc = lstm_step2_launch(p, SEG0_DENSE, t, seq_layer(sw, 1), s2, st))) return rc;
-      const size_t warps = (size_t)R * 2 * g.cs;
-      imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(s2.h1_at(t), R, Hs, sw.fc_w, sw.fc_b, g.cs, g.N, g.lo,
-                                                                  d->sb_activation, crm, F, T, t, 1);
-      FSN_CHECK_LAUNCH("imp_fc_step_kernel");
+      if ((rc = sb_head_launch(s2.h1_at(t), R, Hs, 1, sw.fc_w, sw.fc_b, 2 * g.cs, d->sb_activation, crm, imp_head_geom(g, F, T),
+                               t, st)))
+        return rc;
     }
   }
   // element-wise mask on (re, im) + iSTFT (575-589)

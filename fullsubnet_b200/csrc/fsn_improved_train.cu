@@ -108,29 +108,6 @@ static int imp_train_check(const fsn_improved_desc* d, int B, int L, ImpDims& m)
   return FSN_OK;
 }
 
-static unsigned ew_blocks(size_t n) {
-  const size_t g = (n + 255) / 256;
-  return (unsigned)(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
-}
-
-// dY [T, B*N, 2c] of one section's Linear from dcrm [B,2,F,T] (inverse of the scatter of imp_fc_step_kernel: output
-// o = ch*c + j of unit n is cRM row lo + n*c + j of channel ch), times ReLU' of the kept post-activation cRM
-__global__ void imp_dy_kernel(const float* __restrict__ dcrm, const float* __restrict__ crm, int B, int F, int T, int c,
-                              int N, int lo, int act, float* __restrict__ dY) {
-  const int O = 2 * c, R = B * N;
-  const size_t n = (size_t)T * R * O;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int o = (int)(i % O);
-    const size_t tr = i / O;
-    const int r = (int)(tr % R), t = (int)(tr / R);
-    const int b = r / N, u = r - b * N, ch = o / c, j = o - ch * c;
-    const size_t idx = (((size_t)b * 2 + ch) * F + lo + u * c + j) * T + t;
-    float v = dcrm[idx];
-    if (act == FSN_ACT_RELU && !(crm[idx] > 0.f)) v = 0.f;
-    dY[i] = v;
-  }
-}
-
 __device__ __forceinline__ int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
 // Backward of one section's norm and full-band unfold, gather form: for every full-band output element (t, b, r),
@@ -201,8 +178,7 @@ extern "C" int fsn_improved_train_forward(const fsn_improved_desc* d, const fsn_
   FSN_CHECK_LAUNCH("train_tm_stats_kernel");
   if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)Fu * T, 1.f, w.inv1, nullptr, st, IMP_EPS))) return rc;
   const size_t nfb = (size_t)T * B * Fu;
-  imp_scale_rows_kernel<<<ew_blocks(nfb), 256, 0, st>>>(w.raw, w.xfb, w.inv1, nfb, (size_t)B * Fu, (size_t)Fu, B);
-  FSN_CHECK_LAUNCH("imp_scale_rows_kernel");
+  if ((rc = scale_rows_launch(w.raw, w.inv1, nfb, Fu, B, 1, w.xfb, st))) return rc;
   // fp16 operand copies of the tf32 step kernel: layer 0's hidden states double as layer 1's input
   const LayerHalf h0{w.h16[0], nullptr, w.w16}, h1{w.h16[1], w.h16[0], w.w16};
   if ((rc = layer_forward(prec, seq_layer(wt->fb, 0), w.xfb, B, Fu, Hf, T, w.fb[0], w.rec, w.splitk, &h0, st))) return rc;
@@ -221,14 +197,12 @@ extern "C" int fsn_improved_train_forward(const fsn_improved_desc* d, const fsn_
     if ((rc = clip_reduce_only_launch(w.fs, B, T, w.sums, st))) return rc;
     if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)g.N * g.W * T, 1.f, q.invs, nullptr, st, IMP_EPS))) return rc;
     const size_t nx = (size_t)T * R * g.W;
-    imp_scale_rows_kernel<<<ew_blocks(nx), 256, 0, st>>>(q.Xn, q.Xn, q.invs, nx, (size_t)R * g.W, (size_t)g.N * g.W, B);
-    FSN_CHECK_LAUNCH("imp_scale_rows_kernel");
+    if ((rc = scale_rows_launch(q.Xn, q.invs, nx, g.W, R, g.N, q.Xn, st))) return rc;
     if ((rc = layer_forward(prec, seq_layer(sw, 0), q.Xn, R, g.W, Hs, T, q.L[0], w.rec, w.splitk, &h0, st))) return rc;
     if ((rc = layer_forward(prec, seq_layer(sw, 1), q.L[0].H, R, Hs, Hs, T, q.L[1], w.rec, w.splitk, &h1, st))) return rc;
-    const size_t warps = (size_t)T * R * 2 * g.cs;
-    imp_fc_step_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(q.L[1].H, R, Hs, sw.fc_w, sw.fc_b, g.cs, g.N, g.lo,
-                                                                    d->sb_activation, w.crm, F, T, 0, T);
-    FSN_CHECK_LAUNCH("imp_fc_step_kernel");
+    if ((rc = sb_head_launch(q.L[1].H, R, Hs, T, sw.fc_w, sw.fc_b, 2 * g.cs, d->sb_activation, w.crm, imp_head_geom(g, F, T), 0,
+                             st)))
+      return rc;
   }
   // element-wise mask on (re, im) + iSTFT (575-589)
   return istft_launch(w.real, w.imag, 1, w.crm, B, T, d->n_fft, d->hop_length, d->win_length, L, enhanced, st, 2);
@@ -267,14 +241,13 @@ extern "C" int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn
                  ts ? w.wihT[1] : nullptr, w.splitk}};
     for (int l = 0; l < 2; ++l)
       if ((rc = layer_bwd_transpose_weights(Ls[l], st))) return rc;
-    imp_dy_kernel<<<ew_blocks((size_t)T * R * O), 256, 0, st>>>(w.dcrm, w.crm, B, F, T, sg.cs, sg.N, sg.lo, d->sb_activation, w.dY);
-    FSN_CHECK_LAUNCH("imp_dy_kernel");
+    if ((rc = sb_head_bwd_launch(w.dcrm, w.crm, d->sb_activation, R, O, T, 0, imp_head_geom(sg, F, T), w.dY, st))) return rc;
     if ((rc = linear_bwd(w.dY, q.L[1].H, sw.fc_w, T * R, O, Hs, sgr.fc_w, sgr.fc_b, w.dH, w.splitk, w.colsum, st))) return rc;
     // BPTT down to the normalised section input
     if ((rc = stack_bwd(Ls, 2, T, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, w.dX, st))) return rc;
     train_dot_kernel<<<B, 256, 0, st>>>(w.dX, q.Xn, T, R, sg.N, sg.W, w.dot);
     FSN_CHECK_LAUNCH("train_dot_kernel");
-    imp_unfold_bwd_kernel<<<ew_blocks((size_t)T * B * Fu), 256, 0, st>>>(
+    imp_unfold_bwd_kernel<<<ew_grid((size_t)T * B * Fu), 256, 0, st>>>(
         w.dX, q.invs, w.dot, (float)sg.N * sg.W * T, sg, B, T, Fu, s == 0, s == m.S - 1 ? d->fb_activation : FSN_ACT_NONE,
         w.yfb, w.dfb);
     FSN_CHECK_LAUNCH("imp_unfold_bwd_kernel");

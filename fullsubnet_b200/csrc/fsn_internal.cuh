@@ -22,6 +22,22 @@ struct Carver {
 // layer l of a two-layer stack
 inline fsn_lstm_layer seq_layer(const fsn_seq_weights& w, int l) { return {w.w_ih[l], w.w_hh[l], w.b_ih[l], w.b_hh[l]}; }
 
+// grid of a grid-stride elementwise kernel of 256 threads over n elements: one element per thread up to 132 * 16 blocks
+// (16 per SM of an H100 SXM)
+inline unsigned ew_grid(size_t n) {
+  const size_t g = (n + 255) / 256;
+  return (unsigned)(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
+}
+
+// v (the gradient at the output of an activation, FSN_ACT_*) times its derivative, from the post-activation output y
+// (unread for FSN_ACT_NONE)
+__device__ __forceinline__ float act_grad(float v, const float* y, size_t i, int act) {
+  if (act == FSN_ACT_RELU) return y[i] > 0.f ? v : 0.f;
+  if (act == FSN_ACT_RELU6) { const float a = y[i]; return (a > 0.f && a < 6.f) ? v : 0.f; }
+  if (act == FSN_ACT_TANH) { const float a = y[i]; return v * (1.f - a * a); }
+  return v;
+}
+
 // Sub-band row -> (clip, frequency) map.  Row r = b' * Fsub + f' of the sub-band batch.
 // G <= 1: identity (Fsub = F).  G > 1: drop_band (audio_zen/acoustics/feature.py:332-345):
 // output clip b' of group g is input clip g + G*i, frequency f' is input bin g + G*f'.
@@ -182,8 +198,6 @@ int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const 
 static const float TRAIN_CUM_EPS = 1.1920928955078125e-07f;  // audio_zen/constant.py:9
 int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, bool cum, float2* sums, float* inv1,
                        float* raw, float* scaled, float2* fs, float* cum1, cudaStream_t st);
-// output of a Linear(H -> 2F) head: y [Tp,B,2F] (channel c*F+f) -> out [B,2,F,Tp-la], dropping the first `la` frames
-int train_output_launch(const float* y, int B, int Tp, int F, int la, float* out, cudaStream_t st);
 // its backward: dY [Tp,B,2F] = dout [B,2,F,T] re-laid out, zero on the first `la` frames, times act'(y) (FSN_ACT_*) from
 // the kept post-activation output y (unread for FSN_ACT_NONE)
 int train_dy_launch(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
@@ -213,11 +227,27 @@ int fast_dims(const fsn_fast_desc* d, int B, int T, FastDims& m);
 // input bn [Ts, R, K] (time-major, before the norm): scaleT[ts*R + r] = 1 / (mean of row r over its K features and the
 // shrunk steps <= ts + eps)
 int fast_cum_bn_scale_launch(const float* bn, int R, int K, int Ts, float eps, float* scaleT, cudaStream_t st);
-// frame sums of a time-major raw [Tp,B,F] into fs[b*Tp + t].x (the layout cum_clip_scale_launch reads), and
-// out[i] = raw[i] * scale[i / F] (per-(step, clip) scales of a [Tp*B] table, or per-(step, row) ones with F = row width)
-__global__ void train_frame_sum_kernel(const float* __restrict__ raw, int B, int F, int Tp, float2* __restrict__ fs);
-__global__ void train_scale_tm_kernel(const float* __restrict__ raw, const float* __restrict__ scale1T, int F, size_t n,
-                                      float* __restrict__ out);
+// first frame of shrunk step ts and the number of frames averaged into it (fast_fullsubnet/model.py:108-129)
+__device__ __forceinline__ void shrink_block(int ts, int S, int Tp, int& t0, int& len) {
+  if (ts == 0) { t0 = 0; len = 1; return; }
+  t0 = 1 + (ts - 1) * S;
+  len = min(t0 + S, Tp) - t0;
+}
+// fast_fullsubnet bottleneck input before its norm (model.py:174-187) from melT / encT, element (b, t, m) of both at
+// b*bs + t*ts + m: row (b,m) of shrunk step ts, feature k = 2Nn+1 reflected noisy-mel rows || 2Ne+1 reflected encoder
+// rows, averaged over the block of ts, into bn [Ts, B*M, K]; fs[b*Ts + ts] = fixed-order sum of the (b, ts) block (.x and
+// .y alike, the layout clip_reduce_only_launch reads)
+int fast_bn_input_launch(const float* melT, const float* encT, size_t bs, size_t ts, int B, int Tp, int M, int Nn, int Ne,
+                         int S, int Ts, float* bn, float2* fs, cudaStream_t st);
+// fast_fullsubnet decoder input (model.py:191-194): dec_in row (b,t) = [encoder output (M) | up-sampled bottleneck output
+// (M)].  Row (b,t) of encT [., M] and dec_in [., 2M] is b*rbs + t*rts (clip-major: Tp, 1; time-major: 1, B); frame t reads
+// shrunk step min(t/S, Ts-1) of bn_out, element (b, m, ts) at b*nbs + m*nms + ts*nts
+int fast_dec_input_launch(const float* encT, const float* bn_out, size_t nbs, size_t nms, size_t nts, int B, int Tp, int M,
+                          int S, int Ts, size_t rbs, size_t rts, float* dec_in, cudaStream_t st);
+// out[i] = in[i] * scale[((i / cols) % rows) / div] over n elements (in may be out): rows of `cols` elements, the scale
+// of a row shared by `div` consecutive rows and repeating every `rows` rows
+int scale_rows_launch(const float* in, const float* scale, size_t n, int cols, int rows, int div, float* out,
+                      cudaStream_t st);
 
 // shapes of one Model.forward call (fsn_model.cu)
 struct Dims {
@@ -236,14 +266,33 @@ __host__ __device__ inline int unit_to_row(const RowMap& m, int b, int f) {
 }
 int fc_gemm_launch(const float* A, const float* W, const float* bias, float* out, int M, int K, int O, int act,
                    cudaStream_t st, bool w_kmajor = false);
-// out[row*row_stride + o*o_stride] = act(h[row,:] . W[o,:] + b[o]), one warp per row (small O)
-int rows_fc_launch(const float* h, int R, int H, const float* W, const float* bias, int O, int act, float* out,
-                   size_t row_stride, size_t o_stride, cudaStream_t st);
-int sb_fc_step_launch(const float* h, int R, int H, const float* W, const float* bias, int O, int act, float* crm,
-                      int Fsub, int T_out, int t_out, cudaStream_t st);
-int sb_fc_steps_launch(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act, float* crm,
-                       int Fsub, int T_out, int t_out0, cudaStream_t st);
-int transpose_mag_launch(const float* in, float* out, int B, int F, int T, int T_pad, cudaStream_t st);
+// Where a sub-band head Linear(H -> O <= 2c) writes: row r = b*N + n of the sub-band batch, output o = ch*c + j goes to
+// out[((b*2 + ch)*rows + lo + n*c + j)*rs + t] at frame t, i.e. a [B, 2, rows, frames] cRM with rows rs apart and
+// contiguous frames (fullsubnet/model.py:129-135: c = 1; improved_fullsubnet/model.py:239-247: one section, c its centre
+// width; with N = R every row is clip 0 and channel 0 is a plain [rows, frames] table)
+struct HeadGeom {
+  int N, c, lo, rows;
+  size_t rs;
+};
+// out = act(h W^T + b) for `steps` frames of h [steps, R, H] into frames t0 .. t0+steps-1 of g; one warp per (step, row,
+// output): lane-strided fmaf over H, warp_sum, + bias, act (FSN_ACT_*)
+int sb_head_launch(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act, float* out,
+                   const HeadGeom& g, int t0, cudaStream_t st);
+// its backward: dY [steps, R, O] from the cRM gradient dcrm laid out by g, zero on the first `la` steps (step t reads
+// frame t - la), times act'(y) of the kept post-activation output y in the same layout (unread for FSN_ACT_NONE)
+int sb_head_bwd_launch(const float* dcrm, const float* y, int act, int R, int O, int steps, int la, const HeadGeom& g,
+                       float* dY, cudaStream_t st);
+// fullsubnet's sub-band Linear(H -> 2): row r = b'*Fsub + f' into crm [B', 2, Fsub, T]
+inline HeadGeom fsn_head_geom(int Fsub, int T) { return HeadGeom{Fsub, 1, 0, Fsub, (size_t)T}; }
+// output of a Linear(H -> 2F) head: y rows (b,t) of 2F (channel c*F+f), row (b,t) at b*bs + t*ts elements -> out
+// [B,2,F,Tp-la], dropping the first `la` frames
+int crm_output_launch(const float* y, size_t bs, size_t ts, int B, int Tp, int F, int la, float* out, cudaStream_t st);
+// mag [B,F,T] -> out, element (b,t,f) at b*bs + t*ts + f, for t < Tp with frames T..Tp-1 zero (look-ahead pad);
+// scaled (nullable) receives the same elements times scale[b]
+int transpose_mag_launch(const float* in, int B, int F, int T, int Tp, size_t bs, size_t ts, float* out,
+                         const float* scale, float* scaled, cudaStream_t st);
+// fs[b*Tp + t] = (sum_f x, sum_f c_N[f] x) of the frames of x, element (b,t,f) at b*bs + t*ts + f
+int frame_stats_launch(const float* x, int B, int Tp, int F, int N, size_t bs, size_t ts, float2* fs, cudaStream_t st);
 // Per-clip lengths (lens non-null, device [B] samples): clip b sums only its own Tp_b = 1 + lens[b]/hop + la frames of
 // the T_pad-strided partials, with the same per-thread stride and tree as a call with T_pad = Tp_b; norm_scales_launch
 // then takes cnt1 / cnt2 per frame and multiplies them by Tp_b.
@@ -303,11 +352,8 @@ int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m);
 __global__ void imp_compress_kernel(const float* __restrict__ mag, float* __restrict__ out, int F, int T, float fdrc, bool tm);
 __global__ void imp_section_input_kernel(const float* __restrict__ magc, const float* __restrict__ fbT, int B, int T,
                                          int Fu, SecGeom g, float* __restrict__ X, float2* __restrict__ fs, bool tm);
-__global__ void imp_fc_step_kernel(const float* __restrict__ h, int R, int H, const float* __restrict__ W,
-                                   const float* __restrict__ bias, int c, int N, int lo, int act, float* __restrict__ crm,
-                                   int F, int T, int t0, int steps);
-__global__ void imp_scale_rows_kernel(const float* src, float* X, const float* __restrict__ inv, size_t n, size_t per_t,
-                                      size_t per_clip, int B);
+// where section g's Linear(H -> 2c) writes in the cRM [B,2,F,T]
+inline HeadGeom imp_head_geom(const SecGeom& g, int F, int T) { return HeadGeom{g.N, g.cs, g.lo, F, (size_t)T}; }
 
 // persistent cooperative full-band LSTM (fsn_fullband.cu): layers L[0] (F -> H0, input x [R,Tp,F] times inv1[r] when
 // given) and L[1] (H0 -> H1) of R rows into h1all [R,Tp,H1]; h0buf [2][256][H0] scratch

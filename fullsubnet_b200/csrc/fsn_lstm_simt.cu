@@ -10,9 +10,14 @@
 
 namespace fsn {
 
-// ------------------------------------------------------------------------------------------
-// [B,F,T] -> [B,T_pad,F], rows T..T_pad-1 zero (model.py:85 look-ahead pad fused)
-__global__ void transpose_mag_kernel(const float* __restrict__ in, float* __restrict__ out, int F, int T, int T_pad) {
+// ------------------------------------------------------------------------------------------ layout
+// Clip-major inference tensors ([B, Tp, .]) and time-major training ones ([Tp, B, .]) share these kernels: each takes
+// the element strides of its (clip, frame) axes.
+
+// [B,F,T] -> out (b,t,f) at b*bs + t*ts + f, frames T..Tp-1 zero (model.py:85 look-ahead pad fused); scaled (nullable)
+// = the same times scale[b] (model.py:92)
+__global__ void transpose_mag_kernel(const float* __restrict__ in, int F, int T, int Tp, size_t bs, size_t ts,
+                                     float* __restrict__ out, const float* __restrict__ scale, float* __restrict__ scaled) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
@@ -22,19 +27,97 @@ __global__ void transpose_mag_kernel(const float* __restrict__ in, float* __rest
     tile[i][tx] = (f < F && t < T) ? in[((size_t)b * F + f) * T + t] : 0.f;
   }
   __syncthreads();
+  const float s = scaled ? scale[b] : 0.f;
   for (int i = ty; i < 32; i += 8) {
     const int t = t0 + i, f = f0 + tx;
-    if (t < T_pad && f < F) out[((size_t)b * T_pad + t) * F + f] = tile[tx][i];
+    if (t < Tp && f < F) {
+      const float v = tile[tx][i];
+      const size_t o = (size_t)b * bs + (size_t)t * ts + f;
+      out[o] = v;
+      if (scaled) scaled[o] = v * s;
+    }
   }
 }
 
+// y rows (b,t) of 2F at b*bs + t*ts (channel c*F+f) -> out [B,2,F,T], T = Tp - la, dropping the first `la` frames
+// (fullsubnet/model.py:129-135, fast_fullsubnet/model.py:197-200, fullband_baseline/model.py:58-62)
+__global__ void crm_output_kernel(const float* __restrict__ y, size_t bs, size_t ts, int Tp, int F, int la,
+                                  float* __restrict__ out) {
+  __shared__ float tile[32][33];
+  const int T = Tp - la;
+  const int b = blockIdx.z >> 1, c = blockIdx.z & 1;
+  const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  for (int i = ty; i < 32; i += 8) {  // read: f contiguous
+    const int t = t0 + i, f = f0 + tx;
+    tile[i][tx] = (t < T && f < F) ? y[(size_t)b * bs + (size_t)(t + la) * ts + c * F + f] : 0.f;
+  }
+  __syncthreads();
+  for (int i = ty; i < 32; i += 8) {  // write: t contiguous
+    const int f = f0 + i, t = t0 + tx;
+    if (f < F && t < T) out[(((size_t)b * 2 + c) * F + f) * T + t] = tile[tx][i];
+  }
+}
 
-// one warp per (b,t) row of a time-major [B,T_pad,F] tensor: fs[row] = (sum_f x, sum_f c_N[f] x)
-__global__ void frame_stats_kernel(const float* __restrict__ x, int rows, int F, int N, float2* __restrict__ fs) {
+// One CTA per (b, ts); see fast_bn_input_launch
+__global__ void fast_bn_input_kernel(const float* __restrict__ melT, const float* __restrict__ encT, size_t bs, size_t ts_,
+                                     int B, int Tp, int M, int Nn, int Ne, int S, int Ts, float* __restrict__ bn,
+                                     float2* __restrict__ fs) {
+  __shared__ float red[256];
+  const int b = blockIdx.x / Ts, ts = blockIdx.x % Ts;
+  const int K = (2 * Nn + 1) + (2 * Ne + 1);
+  int t0, len;
+  shrink_block(ts, S, Tp, t0, len);
+  const float inv = 1.0f / (float)len;
+  float local = 0.f;
+  for (int i = threadIdx.x; i < M * K; i += blockDim.x) {
+    const int m = i / K, k = i - m * K;
+    float acc = 0.f;
+    for (int t = t0; t < t0 + len; ++t) {
+      const size_t base = (size_t)b * bs + (size_t)t * ts_;
+      acc += (k < 2 * Nn + 1) ? melT[base + reflect_idx(m + k - Nn, M)]
+                              : encT[base + reflect_idx(m + (k - (2 * Nn + 1)) - Ne, M)];
+    }
+    const float v = acc * inv;
+    bn[((size_t)ts * B * M + (size_t)b * M + m) * K + k] = v;
+    local += v;
+  }
+  red[threadIdx.x] = local;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) fs[(size_t)b * Ts + ts] = make_float2(red[0], red[0]);
+}
+
+// see fast_dec_input_launch; element i of dec_in is column i % 2M of row i / 2M
+__global__ void fast_dec_input_kernel(const float* __restrict__ encT, const float* __restrict__ bn_out, size_t nbs,
+                                      size_t nms, size_t nts, int B, int Tp, int M, int S, int Ts, size_t rbs, size_t rts,
+                                      float* __restrict__ dec_in) {
+  const size_t n = (size_t)B * Tp * 2 * M;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % (2 * M));
+    const size_t q = i / (2 * M);
+    const int b = (int)((q / rbs) % B), t = (int)((q / rts) % Tp);
+    dec_in[i] = c < M ? encT[q * M + c] : bn_out[(size_t)b * nbs + (size_t)(c - M) * nms + (size_t)min(t / S, Ts - 1) * nts];
+  }
+}
+
+__global__ void scale_rows_kernel(const float* in, const float* __restrict__ scale, size_t n, int cols, int rows, int div,
+                                  float* out) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    out[i] = in[i] * scale[(int)((i / cols) % rows) / div];
+}
+
+// one warp per frame (b,t) of x, element (b,t,f) at b*bs + t*ts + f: fs[b*Tp + t] = (sum_f x, sum_f c_N[f] x)
+__global__ void frame_stats_kernel(const float* __restrict__ x, int B, int Tp, int F, int N, size_t bs, size_t ts,
+                                   float2* __restrict__ fs) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  const float* p = x + (size_t)row * F;
+  if (row >= B * Tp) return;
+  const int b = row / Tp, t = row - b * Tp;
+  const float* p = x + (size_t)b * bs + (size_t)t * ts;
   float s0 = 0.f, s1 = 0.f;
   for (int f = lane; f < F; f += 32) {
     const float v = p[f];
@@ -354,77 +437,113 @@ int fc_gemm_launch(const float* A, const float* W, const float* bias, float* out
   return FSN_OK;
 }
 
-// sub-band Linear(H -> O, O small) for one time step, one warp per row, written straight into
-// crm[b', o, f', t_out] (model.py:129-135: reshape/permute + look-ahead slice fused)
-__global__ void sb_fc_step_kernel(const float* __restrict__ h, int R, int H, const float* __restrict__ W,
-                                  const float* __restrict__ bias, int O, int act, float* __restrict__ crm, int Fsub,
-                                  int T_out, int t_out, size_t step_stride) {
-  // blockIdx.y: step (h of step y starts step_stride floats further and lands in frame t_out + y)
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+// sub-band head Linear(H -> O <= 2c) of `steps` frames, one warp per (step, row, output), written straight into the
+// cRM through g (model.py:129-135: reshape/permute + look-ahead slice fused).  The activation is a template argument: with
+// a runtime switch these short warps took 4.6 % longer on the improved_fullsubnet heads (H100 SXM, 700 W)
+template <int ACT>
+__global__ void sb_head_kernel(const float* __restrict__ h, int R, int H, int steps, const float* __restrict__ W,
+                               const float* __restrict__ bias, int O, float* __restrict__ out, HeadGeom g, int t0) {
+  const size_t wid = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (row >= R) return;
-  t_out += blockIdx.y;
-  const float* hp = h + (size_t)blockIdx.y * step_stride + (size_t)row * H;
-  const int bq = row / Fsub, fq = row - bq * Fsub;
-  for (int o = 0; o < O; ++o) {
-    float s = 0.f;
-    for (int k = lane; k < H; k += 32) s = fmaf(hp[k], W[(size_t)o * H + k], s);
-    s = warp_sum(s);
-    if (lane == 0) crm[(((size_t)bq * O + o) * Fsub + fq) * T_out + t_out] = apply_act(s + bias[o], act);
+  if (wid >= (size_t)steps * R * O) return;
+  const size_t step_row = wid / O;
+  const int o = (int)(wid % O), t = t0 + (int)(step_row / R), row = (int)(step_row % R);
+  const float* hp = h + step_row * H;
+  float s = 0.f;
+  for (int k = lane; k < H; k += 32) s = fmaf(hp[k], W[(size_t)o * H + k], s);
+  s = warp_sum(s);
+  if (lane == 0) {
+    const int b = row / g.N, n = row - b * g.N, ch = o / g.c, j = o - ch * g.c;
+    out[(((size_t)b * 2 + ch) * g.rows + g.lo + n * g.c + j) * g.rs + t] = apply_act(s + bias[o], ACT);
   }
 }
 
-__global__ void rows_fc_kernel(const float* __restrict__ h, int R, int H, const float* __restrict__ W,
-                               const float* __restrict__ bias, int O, int act, float* __restrict__ out, size_t row_stride,
-                               size_t o_stride) {
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (row >= R) return;
-  const float* hp = h + (size_t)row * H;
-  for (int o = 0; o < O; ++o) {
-    float s = 0.f;
-    for (int k = lane; k < H; k += 32) s = fmaf(hp[k], W[(size_t)o * H + k], s);
-    s = warp_sum(s);
-    if (lane == 0) out[(size_t)row * row_stride + (size_t)o * o_stride] = apply_act(s + bias[o], act);
+// the inverse gather of sb_head_kernel's scatter: dY[t, r, o] = act'(y) dcrm at frame t - la, 0 for t < la
+__global__ void sb_head_bwd_kernel(const float* __restrict__ dcrm, const float* __restrict__ y, int act, int R, int O,
+                                   int steps, int la, HeadGeom g, float* __restrict__ dY) {
+  const size_t n = (size_t)steps * R * O;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int o = (int)(i % O);
+    const size_t tr = i / O;
+    const int r = (int)(tr % R), t = (int)(tr / R);
+    float v = 0.f;
+    if (t >= la) {
+      const int b = r / g.N, u = r - b * g.N, ch = o / g.c, j = o - ch * g.c;
+      const size_t idx = (((size_t)b * 2 + ch) * g.rows + g.lo + u * g.c + j) * g.rs + (t - la);
+      v = act_grad(dcrm[idx], y, idx, act);
+    }
+    dY[i] = v;
   }
 }
 
-int rows_fc_launch(const float* h, int R, int H, const float* W, const float* bias, int O, int act, float* out,
-                   size_t row_stride, size_t o_stride, cudaStream_t st) {
-  rows_fc_kernel<<<cdiv(R, 8), 256, 0, st>>>(h, R, H, W, bias, O, act, out, row_stride, o_stride);
-  FSN_CHECK_LAUNCH("rows_fc_kernel");
+int sb_head_launch(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act, float* out,
+                   const HeadGeom& g, int t0, cudaStream_t st) {
+  const size_t blocks = ((size_t)steps * R * O + 7) / 8;
+  if (blocks == 0) return FSN_OK;
+  FSN_REQUIRE(blocks <= 0x7fffffff, FSN_ERR_SHAPE, "sub-band head: too many rows");
+  const unsigned grid = (unsigned)blocks;
+  switch (act) {
+    case FSN_ACT_RELU: sb_head_kernel<FSN_ACT_RELU><<<grid, 256, 0, st>>>(h, R, H, steps, W, bias, O, out, g, t0); break;
+    case FSN_ACT_TANH: sb_head_kernel<FSN_ACT_TANH><<<grid, 256, 0, st>>>(h, R, H, steps, W, bias, O, out, g, t0); break;
+    case FSN_ACT_RELU6: sb_head_kernel<FSN_ACT_RELU6><<<grid, 256, 0, st>>>(h, R, H, steps, W, bias, O, out, g, t0); break;
+    default: sb_head_kernel<FSN_ACT_NONE><<<grid, 256, 0, st>>>(h, R, H, steps, W, bias, O, out, g, t0); break;
+  }
+  FSN_CHECK_LAUNCH("sb_head_kernel");
   return FSN_OK;
 }
 
-int sb_fc_step_launch(const float* h, int R, int H, const float* W, const float* bias, int O, int act, float* crm,
-                      int Fsub, int T_out, int t_out, cudaStream_t st) {
-  sb_fc_step_kernel<<<cdiv(R, 8), 256, 0, st>>>(h, R, H, W, bias, O, act, crm, Fsub, T_out, t_out, 0);
-  FSN_CHECK_LAUNCH("sb_fc_step_kernel");
+int sb_head_bwd_launch(const float* dcrm, const float* y, int act, int R, int O, int steps, int la, const HeadGeom& g,
+                       float* dY, cudaStream_t st) {
+  sb_head_bwd_kernel<<<ew_grid((size_t)steps * R * O), 256, 0, st>>>(dcrm, y, act, R, O, steps, la, g, dY);
+  FSN_CHECK_LAUNCH("sb_head_bwd_kernel");
   return FSN_OK;
 }
 
-// the same Linear for `steps` consecutive steps of a time-major [steps, R, H] block in one launch (training forward)
-int sb_fc_steps_launch(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act, float* crm,
-                       int Fsub, int T_out, int t_out0, cudaStream_t st) {
-  if (steps <= 0) return FSN_OK;
-  FSN_REQUIRE(steps <= 65535, FSN_ERR_SHAPE, "sb_fc_steps: too many steps");
-  sb_fc_step_kernel<<<dim3(cdiv(R, 8), steps), 256, 0, st>>>(h, R, H, W, bias, O, act, crm, Fsub, T_out, t_out0, (size_t)R * H);
-  FSN_CHECK_LAUNCH("sb_fc_step_kernel");
+int crm_output_launch(const float* y, size_t bs, size_t ts, int B, int Tp, int F, int la, float* out, cudaStream_t st) {
+  crm_output_kernel<<<dim3(cdiv(Tp - la, 32), cdiv(F, 32), B * 2), dim3(32, 8), 0, st>>>(y, bs, ts, Tp, F, la, out);
+  FSN_CHECK_LAUNCH("crm_output_kernel");
   return FSN_OK;
 }
 
-int transpose_mag_launch(const float* in, float* out, int B, int F, int T, int T_pad, cudaStream_t st) {
-  dim3 grid(cdiv(T_pad, 32), cdiv(F, 32), B);
-  transpose_mag_kernel<<<grid, dim3(32, 8), 0, st>>>(in, out, F, T, T_pad);
+int transpose_mag_launch(const float* in, int B, int F, int T, int Tp, size_t bs, size_t ts, float* out,
+                         const float* scale, float* scaled, cudaStream_t st) {
+  transpose_mag_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(in, F, T, Tp, bs, ts, out, scale, scaled);
   FSN_CHECK_LAUNCH("transpose_mag_kernel");
+  return FSN_OK;
+}
+
+int fast_bn_input_launch(const float* melT, const float* encT, size_t bs, size_t ts, int B, int Tp, int M, int Nn, int Ne,
+                         int S, int Ts, float* bn, float2* fs, cudaStream_t st) {
+  fast_bn_input_kernel<<<B * Ts, 256, 0, st>>>(melT, encT, bs, ts, B, Tp, M, Nn, Ne, S, Ts, bn, fs);
+  FSN_CHECK_LAUNCH("fast_bn_input_kernel");
+  return FSN_OK;
+}
+
+int fast_dec_input_launch(const float* encT, const float* bn_out, size_t nbs, size_t nms, size_t nts, int B, int Tp, int M,
+                          int S, int Ts, size_t rbs, size_t rts, float* dec_in, cudaStream_t st) {
+  fast_dec_input_kernel<<<ew_grid((size_t)B * Tp * 2 * M), 256, 0, st>>>(encT, bn_out, nbs, nms, nts, B, Tp, M, S, Ts, rbs,
+                                                                          rts, dec_in);
+  FSN_CHECK_LAUNCH("fast_dec_input_kernel");
+  return FSN_OK;
+}
+
+int scale_rows_launch(const float* in, const float* scale, size_t n, int cols, int rows, int div, float* out,
+                      cudaStream_t st) {
+  scale_rows_kernel<<<ew_grid(n), 256, 0, st>>>(in, scale, n, cols, rows, div, out);
+  FSN_CHECK_LAUNCH("scale_rows_kernel");
+  return FSN_OK;
+}
+
+int frame_stats_launch(const float* x, int B, int Tp, int F, int N, size_t bs, size_t ts, float2* fs, cudaStream_t st) {
+  frame_stats_kernel<<<cdiv(B * Tp, 8), 256, 0, st>>>(x, B, Tp, F, N, bs, ts, fs);
+  FSN_CHECK_LAUNCH("frame_stats_kernel");
   return FSN_OK;
 }
 
 int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs, float2* sums, cudaStream_t st,
                       const int* lens, int hop, int la) {
-  const int rows = B * T_pad;
-  frame_stats_kernel<<<cdiv(rows, 8), 256, 0, st>>>(x, rows, F, N, fs);
-  FSN_CHECK_LAUNCH("frame_stats_kernel");
+  int rc;
+  if ((rc = frame_stats_launch(x, B, T_pad, F, N, (size_t)T_pad * F, F, fs, st))) return rc;
   clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums, lens, hop, la);
   FSN_CHECK_LAUNCH("clip_reduce_kernel");
   return FSN_OK;

@@ -170,8 +170,8 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
     p.F = F; p.Tp = Tp; p.t = t; p.Ns = d->sb_num_neighbors; p.Nf = d->fb_num_neighbors; p.map = map;
     if ((rc = lstm_step2_launch(p, SEG0_GATHER, t, seq_layer(*sb, 1), s2, st))) return rc;
     if (t >= d->look_ahead)
-      if ((rc = sb_fc_step_launch(s2.h1_at(t), m.R, Hs, sb->fc_w, sb->fc_b, 2, d->sb_activation, crm, m.Fsub,
-                                  m.T, t - d->look_ahead, st)))
+      if ((rc = sb_head_launch(s2.h1_at(t), m.R, Hs, 1, sb->fc_w, sb->fc_b, 2, d->sb_activation, crm,
+                               fsn_head_geom(m.Fsub, m.T), t - d->look_ahead, st)))
         return rc;
   }
   prof_mark(3, st);
@@ -248,7 +248,7 @@ extern "C" int fsn_model_forward(const fsn_model_desc* d, const fsn_seq_weights*
   cudaStream_t st = (cudaStream_t)stream;
   prof_reset();
   prof_mark(0, st);
-  if ((rc = transpose_mag_launch(noisy_mag, w.magT, B, m.F, T, m.Tp, st))) return rc;
+  if ((rc = transpose_mag_launch(noisy_mag, B, m.F, T, m.Tp, (size_t)m.Tp * m.F, m.F, w.magT, nullptr, nullptr, st))) return rc;
   prof_mark(1, st);
   return model_core(d, fb, sb, sb_packed, m, w, crm, st);
 }

@@ -244,29 +244,6 @@ __global__ void train_tm_stats_kernel(const float* __restrict__ x, int B, int F,
   if (threadIdx.x == 0) sums[b] = sh[0];
 }
 
-// mag [B,F,T] -> raw [Tp,B,F] (zero look-ahead frames, model.py:85) and scaled = raw * inv1[b] (model.py:92)
-__global__ void train_transpose_kernel(const float* __restrict__ mag, const float* __restrict__ inv1,
-                                       float* __restrict__ raw, float* __restrict__ scaled, int B, int F, int T, int Tp) {
-  __shared__ float tile[32][33];
-  const int b = blockIdx.z, f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  for (int i = ty; i < 32; i += 8) {
-    const int f = f0 + i, t = t0 + tx;
-    tile[i][tx] = (f < F && t < T) ? mag[((size_t)b * F + f) * T + t] : 0.f;
-  }
-  __syncthreads();
-  const float s = inv1[b];
-  for (int i = ty; i < 32; i += 8) {
-    const int t = t0 + i, f = f0 + tx;
-    if (t < Tp && f < F) {
-      const float v = tile[tx][i];
-      const size_t o = ((size_t)t * B + b) * F + f;
-      raw[o] = v;
-      scaled[o] = v * s;
-    }
-  }
-}
-
 // sub-band input X[t,r,k] (base_model.py:13-46 + model.py:98-119): unit (b,f) of row r, scaled by inv2[b]
 __global__ void train_gather_kernel(const float* __restrict__ raw, const float* __restrict__ fbz,
                                     const float* __restrict__ inv2, const float* __restrict__ unit_scale,
@@ -288,23 +265,6 @@ __global__ void train_gather_kernel(const float* __restrict__ raw, const float* 
 }
 
 // ---- cumulative_laplace_norm in the training step (audio_zen/model/base_model.py:220-251)
-// frame sums of a time-major tensor raw [Tp,B,F] in the layout cum_clip_scale_launch reads: fs[b*Tp + t].x
-__global__ void train_frame_sum_kernel(const float* __restrict__ raw, int B, int F, int Tp, float2* __restrict__ fs) {
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);  // row = t*B + b
-  const int lane = threadIdx.x & 31;
-  if (row >= Tp * B) return;
-  const float* p = raw + (size_t)row * F;
-  float a = 0.f;
-  for (int f = lane; f < F; f += 32) a += p[f];
-  a = warp_sum(a);
-  if (lane == 0) { const int t = row / B, b = row - t * B; fs[(size_t)b * Tp + t] = make_float2(a, a); }
-}
-// xfb[t,b,f] = raw[t,b,f] * scale1T[t*B + b]
-__global__ void train_scale_tm_kernel(const float* __restrict__ raw, const float* __restrict__ scale1T, int F, size_t n,
-                                      float* __restrict__ out) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    out[i] = raw[i] * scale1T[i / F];
-}
 // Backward of X[t,r,k] = u[t,r,k] * s[t,r], s = 1/(m + eps), m[t,r] = sum_{t'<=t} sum_k u[t',r,k] / (K (t+1)):
 //   d u[t,r,k] = dX[t,r,k] s[t,r] + sum_{t''>=t} q[t'',r],   q[t,r] = -s[t,r] <dX[t,r,:], X[t,r,:]> / (K (t+1)).
 // Only the full-band row k = K-1 has a parameter behind it (Nf = 0): dunit[t,r] = its gradient.  One thread per
@@ -332,12 +292,7 @@ __global__ void train_dfbz_cum_kernel(const float* __restrict__ dunit, const flo
     const size_t tb = i / map.F;
     const int b = (int)(tb % map.B), t = (int)(tb / map.B);
     const int r = unit_to_row(map, b, f);
-    float v = r >= 0 ? dunit[(size_t)t * R + r] : 0.f;
-    const float y = fbz[i];
-    if (act == FSN_ACT_RELU) v = y > 0.f ? v : 0.f;
-    else if (act == FSN_ACT_TANH) v *= 1.f - y * y;
-    else if (act == FSN_ACT_RELU6) v = (y > 0.f && y < 6.f) ? v : 0.f;
-    dz[i] = v;
+    dz[i] = act_grad(r >= 0 ? dunit[(size_t)t * R + r] : 0.f, fbz, i, act);
   }
 }
 
@@ -390,23 +345,6 @@ int transpose_launch(const float* in, size_t rows, int cols, float* out, cudaStr
 }
 
 // ------------------------------------------------------------------------------------------ backward kernels
-// dout[t,r,o] = dcrm[b',o,f',t-la] (0 for the look-ahead steps)  (model.py:129-135 backwards)
-__global__ void train_dout_kernel(const float* __restrict__ dcrm, float* __restrict__ dout, int R, int Fsub, int T,
-                                  int Tp, int la) {
-  const size_t n = (size_t)Tp * R * 2;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int o = (int)(i & 1);
-    const size_t tr = i >> 1;
-    const int r = (int)(tr % R), t = (int)(tr / R);
-    float v = 0.f;
-    if (t >= la) {
-      const int bq = r / Fsub, fq = r - bq * Fsub;
-      v = dcrm[(((size_t)bq * 2 + o) * Fsub + fq) * T + (t - la)];
-    }
-    dout[i] = v;
-  }
-}
-
 struct BwdPoint {
   int R, H;
   float* G;             // [R,4H] in: gates (post-activation), out: d(pre-activation)
@@ -618,9 +556,7 @@ int layer_forward_save_tc(const fsn_lstm_layer& w, const float* X, int R, int K0
   } else if ((rc = fc_gemm_launch(X, w.w_ih, nullptr, s.G, rows, K0, 4 * H, FSN_ACT_NONE, st))) {
     return rc;  // rows of X not 16-byte aligned (K0 % 4 != 0): fp32 SIMT GEMM
   }
-  const size_t n = (size_t)R * H;
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 16) blocks = 132 * 16;
+  const unsigned blocks = ew_grid((size_t)R * H);
   for (int t = 0; t < Tp; ++t) {
     float* Gt = s.G + (size_t)t * R * 4 * H;
     if (fused && (t > 0 || fold)) {  // GEMM + cell in one kernel, the recurrent product stays in registers
@@ -691,10 +627,7 @@ int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, cons
   p.dh_rec = (t == Tp - 1) ? nullptr : L.dh_rec;
   p.dc = L.dc; p.first_dc = (t == Tp - 1);
   p.dout = dout; p.fc_w = fc_w; p.O = O;
-  const size_t n = (size_t)L.R * L.H;
-  int blocks = (int)((n + 255) / 256);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  lstm_bwd_point_kernel<<<blocks, 256, 0, st>>>(p);
+  lstm_bwd_point_kernel<<<ew_grid((size_t)L.R * L.H), 256, 0, st>>>(p);
   FSN_CHECK_LAUNCH("lstm_bwd_point_kernel");
   int rc;
   const bool tc = tc_bwd(L);
@@ -779,39 +712,13 @@ int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int 
   FSN_CHECK_LAUNCH("train_mag_stats_kernel");
   int rc;
   if ((rc = norm_scales_launch(sums, sums, B, (float)F * Tp, 1.f, inv1, nullptr, st))) return rc;
-  train_transpose_kernel<<<dim3(cdiv(Tp, 32), cdiv(F, 32), B), dim3(32, 8), 0, st>>>(noisy_mag, inv1, raw, scaled, B, F, T, Tp);
-  FSN_CHECK_LAUNCH("train_transpose_kernel");
+  // raw [Tp,B,F] and scaled = raw * inv1[b]
+  if ((rc = transpose_mag_launch(noisy_mag, B, F, T, Tp, F, (size_t)B * F, raw, inv1, scaled, st))) return rc;
   if (cum) {  // causal running mean per clip instead of the clip mean (base_model.py:220-251)
-    train_frame_sum_kernel<<<cdiv(Tp * B, 8), 256, 0, st>>>(raw, B, F, Tp, fs);
-    FSN_CHECK_LAUNCH("train_frame_sum_kernel");
+    if ((rc = frame_stats_launch(raw, B, Tp, F, 0, F, (size_t)B * F, fs, st))) return rc;
     if ((rc = cum_clip_scale_launch(fs, B, Tp, F, TRAIN_CUM_EPS, cum1, st))) return rc;
-    train_scale_tm_kernel<<<132 * 8, 256, 0, st>>>(raw, cum1, F, (size_t)Tp * B * F, scaled);
-    FSN_CHECK_LAUNCH("train_scale_tm_kernel");
+    if ((rc = scale_rows_launch(raw, cum1, (size_t)Tp * B * F, F, Tp * B, 1, scaled, st))) return rc;  // scale of (t, b)
   }
-  return FSN_OK;
-}
-
-// y [Tp,B,2F] (channel c*F+f) -> out [B,2,F,T], dropping the first `la` frames
-__global__ void train_output_kernel(const float* __restrict__ y, int B, int Tp, int F, int la, float* __restrict__ out) {
-  __shared__ float tile[32][33];
-  const int T = Tp - la;
-  const int b = blockIdx.z >> 1, c = blockIdx.z & 1;
-  const int f0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  for (int i = ty; i < 32; i += 8) {
-    const int t = t0 + i, f = f0 + tx;
-    tile[i][tx] = (t < T && f < F) ? y[((size_t)(t + la) * B + b) * (2 * F) + c * F + f] : 0.f;
-  }
-  __syncthreads();
-  for (int i = ty; i < 32; i += 8) {
-    const int f = f0 + i, t = t0 + tx;
-    if (f < F && t < T) out[(((size_t)b * 2 + c) * F + f) * T + t] = tile[tx][i];
-  }
-}
-
-int train_output_launch(const float* y, int B, int Tp, int F, int la, float* out, cudaStream_t st) {
-  train_output_kernel<<<dim3(cdiv(Tp - la, 32), cdiv(F, 32), B * 2), dim3(32, 8), 0, st>>>(y, B, Tp, F, la, out);
-  FSN_CHECK_LAUNCH("train_output_kernel");
   return FSN_OK;
 }
 
@@ -823,25 +730,13 @@ __global__ void train_dy_kernel(const float* __restrict__ dout, const float* __r
     const int cf = (int)(i % (2 * F));
     const size_t tb = i / (2 * F);
     const int b = (int)(tb % B), t = (int)(tb / B);
-    float v = t >= la ? dout[((size_t)b * 2 * F + cf) * T + (t - la)] : 0.f;
-    if (act == FSN_ACT_RELU) {
-      v = y[i] > 0.f ? v : 0.f;
-    } else if (act == FSN_ACT_RELU6) {
-      const float a = y[i];
-      v = (a > 0.f && a < 6.f) ? v : 0.f;
-    } else if (act == FSN_ACT_TANH) {
-      const float a = y[i];
-      v *= 1.f - a * a;
-    }
-    dY[i] = v;
+    dY[i] = act_grad(t >= la ? dout[((size_t)b * 2 * F + cf) * T + (t - la)] : 0.f, y, i, act);
   }
 }
 
 int train_dy_launch(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
                     cudaStream_t st) {
-  size_t g = ((size_t)Tp * B * 2 * F + 255) / 256;
-  if (g > 132 * 16) g = 132 * 16;
-  train_dy_kernel<<<(int)g, 256, 0, st>>>(dout, y, act, B, F, T, Tp, la, dY);
+  train_dy_kernel<<<ew_grid((size_t)Tp * B * 2 * F), 256, 0, st>>>(dout, y, act, B, F, T, Tp, la, dY);
   FSN_CHECK_LAUNCH("train_dy_kernel");
   return FSN_OK;
 }
@@ -900,8 +795,8 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   if ((rc = layer_forward(prec, seq_layer(*sb, 0), w.xsb, m.R, m.Ksb, Hs, Tp, w.sb[0], w.rec, w.splitk, &hs0, st))) return rc;
   if ((rc = layer_forward(prec, seq_layer(*sb, 1), w.sb[0].H, m.R, Hs, Hs, Tp, w.sb[1], w.rec, w.splitk, &hs1, st))) return rc;
   // sub-band Linear of every output frame in one launch (model.py:129-135; the first look_ahead steps have no frame)
-  return sb_fc_steps_launch(w.sb[1].H + (size_t)d->look_ahead * m.R * Hs, m.R, Hs, Tp - d->look_ahead, sb->fc_w, sb->fc_b, 2,
-                            d->sb_activation, crm, m.Fsub, m.T, 0, st);
+  return sb_head_launch(w.sb[1].H + (size_t)d->look_ahead * m.R * Hs, m.R, Hs, Tp - d->look_ahead, sb->fc_w, sb->fc_b, 2,
+                        d->sb_activation, crm, fsn_head_geom(m.Fsub, m.T), 0, st);
 }
 
 namespace fsn {
@@ -946,8 +841,8 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   const int Tp = m.Tp, F = m.F, R = m.R, Hf = d->fb_hidden, Hs = d->sb_hidden, K = m.Ksb;
   RowMap map{B, F, m.Fsub, m.G};
   // ---- sub-band Linear (model.py:129-135 backwards)
-  train_dout_kernel<<<132 * 8, 256, 0, st>>>(dcrm, w.dout, R, m.Fsub, T, Tp, d->look_ahead);
-  FSN_CHECK_LAUNCH("train_dout_kernel");
+  if ((rc = sb_head_bwd_launch(dcrm, nullptr, FSN_ACT_NONE, R, 2, Tp, d->look_ahead, fsn_head_geom(m.Fsub, T), w.dout, st)))
+    return rc;
   {  // dW of the 2-output Linear: one streaming pass over h1 (2.4 GB at config 3)
     const size_t rows = (size_t)Tp * R;
     int S = (int)((rows + 2047) / 2048);

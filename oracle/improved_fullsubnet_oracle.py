@@ -67,6 +67,10 @@ def seq_time_major(x: torch.Tensor, sd, prefix: str, act) -> torch.Tensor:
     o = o @ sd[prefix + "fc_output_layer.weight"].t() + sd[prefix + "fc_output_layer.bias"]
     if act == "ReLU":
         o = torch.relu(o)
+    elif act == "Tanh":
+        o = torch.tanh(o)
+    elif act == "ReLU6":
+        o = torch.clamp(o, 0, 6)
     elif act:
         raise NotImplementedError(act)
     return o.permute(0, 2, 1)

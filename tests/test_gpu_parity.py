@@ -299,6 +299,31 @@ def test_improved_fullsubnet_matches_reference(golden, dev, tag, prec):
         bad(y)
 
 
+@pytest.mark.parametrize("prec", ["fp32", "tf32_tc"])
+def test_improved_fullsubnet_tanh_head_matches_oracle(golden, dev, prec):
+    """sb_output_activate_function="Tanh": the section heads apply it (improved_fullsubnet/model.py:69-74)."""
+    from fullsubnet_b200.improved_fullsubnet.model import Model
+    from oracle import improved_fullsubnet_oracle as IO
+    args = dict(IO.DEFAULT_IMPROVED_ARGS, sb_output_activate_function="Tanh")
+    sd = IO.make_improved_state_dict(seed=5, args=args)
+    for k in sd:  # heads 4x the init scale: the Tanh bends their outputs, a head without it misses by >> WAV_TOL
+        if k.startswith("sb_model.") and "fc_output_layer" in k:
+            sd[k] = sd[k] * 4.0
+    m = Model(**args)
+    m.load_state_dict(sd, strict=True)
+    m.precision = prec
+    m = m.to(dev).eval()
+    y = torch.from_numpy(np.asarray(golden("improved")["k16_y"]))
+    ref = IO.improved_forward(y, sd, args).numpy()
+    with torch.no_grad():
+        wav = m(y.to(dev))
+    err = np.abs(wav.cpu().numpy() - ref).max()
+    print(f"improved_fullsubnet Tanh head {prec}: waveform max-abs {err:.2e} (scale {np.abs(ref).max():.2e})")
+    if prec == "fp32":
+        assert err < 1e-6
+    assert err < WAV_TOL
+
+
 # ------------------------------------------------------------------ cumulative_laplace_norm (SURVEY 8f rank 1)
 def test_cumulative_laplace_norm_matches_reference(golden, dev):
     from fullsubnet_b200.fullsubnet.model import Model
