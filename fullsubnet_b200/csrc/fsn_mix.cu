@@ -33,38 +33,60 @@ __device__ __forceinline__ float block_max(float v, double* sh) {
 }
 
 // out[b, n] = sum_k x[b, n-k] rir[b, k], n < L (the first L samples of the full convolution); clips with
-// rir_len[b] == 0 are copied.  Direct form: 256 outputs per CTA, taps staged through shared memory in chunks.
-constexpr int CO = 256, CK = 1024;
-__global__ void __launch_bounds__(CO) rir_conv_kernel(const float* __restrict__ x, const float* __restrict__ rir,
+// rir_len[b] == 0 are copied.  Direct form, register-blocked: each thread computes CR consecutive outputs from one
+// broadcast tap load and one sample load per tap; the taps and a segment of the clip are staged through shared memory
+// as doubles in chunks of CK taps.  Each output is summed k ascending in one double accumulator.  A product of two
+// floats is exact in double, so every term and every partial sum is the one of the plain loop
+// "for k: acc += (double)rir[k] * (double)x[n-k]"; the zero terms it adds or skips (k >= rir_len, n - k < 0) cannot
+// change a sum that starts at +0.  CR is odd so the threads' sample loads (stride CR doubles) hit distinct banks.
+constexpr int CT = 128, CR = 9, CO = CT * CR, CK = 128 * CR;
+static_assert(CK % CR == 0, "a chunk is a whole number of register rotations");
+__global__ void __launch_bounds__(CT) rir_conv_kernel(const float* __restrict__ x, const float* __restrict__ rir,
                                                       const int* __restrict__ rir_len, int L, int Lr_max,
                                                       float* __restrict__ out) {
-  __shared__ float taps[CK];
-  __shared__ float seg[CK + CO];
-  const int b = blockIdx.y, n0 = blockIdx.x * CO, n = n0 + threadIdx.x;
+  __shared__ double taps[CK];
+  __shared__ double seg[CK + CO];  // seg[i] = x[n0 - k0 - CK + i]
+  const int b = blockIdx.y, n0 = blockIdx.x * CO, t0 = threadIdx.x * CR;
   const float* xb = x + (size_t)b * L;
+  float* ob = out + (size_t)b * L;
   const int lr = rir_len ? min(rir_len[b], Lr_max) : Lr_max;
   if (lr <= 0) {
-    if (n < L) out[(size_t)b * L + n] = xb[n];
+    for (int i = threadIdx.x; i < CO && n0 + i < L; i += CT) ob[n0 + i] = xb[n0 + i];
     return;
   }
   const float* rb = rir + (size_t)b * Lr_max;
-  double acc = 0.0;  // double accumulation: the reference's FFT convolution carries ~1e-7 relative error per output
+  double acc[CR];
+#pragma unroll
+  for (int r = 0; r < CR; ++r) acc[r] = 0.0;  // double accumulation: the reference's FFT convolution carries ~1e-7
+                                              // relative error per output
   for (int k0 = 0; k0 < lr && k0 <= n0 + CO - 1; k0 += CK) {
+    const int kn = min(CK, lr - k0);
     __syncthreads();
-    for (int i = threadIdx.x; i < CK; i += CO) taps[i] = (k0 + i < lr) ? rb[k0 + i] : 0.f;
-    // x[n0 - k0 - (CK-1) .. n0 - k0 + CO - 1]
-    const int base = n0 - k0 - (CK - 1);
-    for (int i = threadIdx.x; i < CK + CO; i += CO) {
+    for (int i = threadIdx.x; i < CK; i += CT) taps[i] = i < kn ? (double)rb[k0 + i] : 0.0;
+    const int base = n0 - k0 - CK;
+    for (int i = threadIdx.x; i < CK + CO; i += CT) {
       const int j = base + i;
-      seg[i] = (j >= 0 && j < L) ? xb[j] : 0.f;
+      seg[i] = (j >= 0 && j < L) ? (double)xb[j] : 0.0;
     }
     __syncthreads();
-    // x[n - (k0 + kk)] = seg[(n - n0) + (CK - 1) - kk]
-    const float* sp = seg + threadIdx.x + (CK - 1);
-#pragma unroll 8
-    for (int kk = 0; kk < CK; ++kk) acc += (double)taps[kk] * (double)sp[-kk];
+    // x[n0 + t0 + d - k0] = sp[d]; the window w holds offsets d = r - kk (r < CR) of step kk, offset d in slot d mod CR
+    const double* sp = seg + t0 + CK;
+    double w[CR];
+#pragma unroll
+    for (int r = 0; r < CR; ++r) w[r] = sp[r];
+    for (int kk = 0; kk < kn; kk += CR) {
+#pragma unroll
+      for (int j = 0; j < CR; ++j) {
+        const double h = taps[kk + j];
+#pragma unroll
+        for (int r = 0; r < CR; ++r) acc[r] = fma(h, w[(r - j + CR) % CR], acc[r]);
+        w[CR - 1 - j] = sp[-(kk + j + 1)];  // offset -(kk+j+1) replaces CR-1-(kk+j), which step kk+j+1 no longer needs
+      }
+    }
   }
-  if (n < L) out[(size_t)b * L + n] = (float)acc;
+#pragma unroll
+  for (int r = 0; r < CR; ++r)
+    if (n0 + t0 + r < L) ob[n0 + t0 + r] = (float)acc[r];
 }
 
 __global__ void __launch_bounds__(THREADS) snr_mix_kernel(const float* __restrict__ clean, const float* __restrict__ noise,
@@ -125,7 +147,7 @@ using namespace fsn;
 extern "C" int fsn_rir_convolve(const float* x, const float* rir, const int* rir_len, int B, int L, int Lr_max, float* out,
                                 fsn_stream_t stream) {
   FSN_REQUIRE(B > 0 && L > 0 && Lr_max > 0, FSN_ERR_SHAPE, "rir_convolve: empty input");
-  mix::rir_conv_kernel<<<dim3(cdiv(L, mix::CO), B), mix::CO, 0, (cudaStream_t)stream>>>(x, rir, rir_len, L, Lr_max, out);
+  mix::rir_conv_kernel<<<dim3(cdiv(L, mix::CO), B), mix::CT, 0, (cudaStream_t)stream>>>(x, rir, rir_len, L, Lr_max, out);
   FSN_CHECK_LAUNCH("rir_conv_kernel");
   return FSN_OK;
 }

@@ -15,7 +15,7 @@ import torch
 
 from .acoustics.feature import istft, stft
 from .acoustics.mask import decompress_cIRM
-from .utils import initialize_module, prepare_device
+from .utils import initialize_module, prepare_device, read_wav
 
 
 def plan_batches(lengths, batch_size: int, max_padding: float = 0.0):
@@ -193,24 +193,8 @@ class Inferencer:
         ``librosa.load(path, sr=sr)`` (dataset_inference.py:41): same int -> float scaling (1/32768 for 16-bit); when the
         file's rate differs, a windowed-sinc polyphase resampler stands in for librosa's soxr (not bit-identical to it -
         the hot-path parity contract starts at the 16 kHz waveform)."""
-        import wave
-        with wave.open(str(path), "rb") as f:
-            nch, width, rate, n = f.getnchannels(), f.getsampwidth(), f.getframerate(), f.getnframes()
-            raw = f.readframes(n)
-        if width == 2:
-            y = np.frombuffer(raw, dtype="<i2").astype(np.float32) / 32768.0
-        elif width == 1:
-            y = (np.frombuffer(raw, dtype=np.uint8).astype(np.float32) - 128.0) / 128.0
-        elif width == 4:
-            y = np.frombuffer(raw, dtype="<i4").astype(np.float32) / 2147483648.0
-        elif width == 3:
-            b = np.frombuffer(raw, dtype=np.uint8).reshape(-1, 3).astype(np.int32)
-            v = b[:, 0] | (b[:, 1] << 8) | (b[:, 2] << 16)
-            y = (np.where(v >= 1 << 23, v - (1 << 24), v)).astype(np.float32) / 8388608.0
-        else:
-            raise NotImplementedError(f"wav sample width {width}")
-        if nch > 1:  # librosa.load(mono=True): mean over the channels
-            y = y.reshape(-1, nch).mean(axis=1).astype(np.float32)
+        wav, rate = read_wav(path)
+        y = wav[0] if len(wav) == 1 else np.ascontiguousarray(wav.T).mean(axis=1).astype(np.float32)  # librosa(mono=True)
         if rate != sr:
             y = Inferencer.resample(y, rate, sr)
         return np.ascontiguousarray(y, dtype=np.float32)

@@ -1,8 +1,8 @@
 """Mirror of recipes/dns_interspeech_2020/fullsubnet/trainer.py:14-181 (and of fast_fullsubnet/trainer.py and
 fullband_baseline/trainer.py:32-71, the same loop without drop_band) on top of
 audio_zen/trainer/base_trainer.py:28-218 - the parts of the trainer that are arithmetic on the hot path (SURVEY 8a row
-A11, 8f rank 4): STFT of noisy/clean, cIRM target + drop_band, Model.forward, MSE, backward, gradient mean over
-ranks, clip, Adam; and the B=1 validation loop (enhance + loss + SI-SDR, all on the device).
+A11, 8f rank 4): mixing of a Dataset batch, STFT of noisy/clean, cIRM target + drop_band, Model.forward, MSE,
+backward, gradient mean over ranks, clip, Adam; and the B=1 validation loop (enhance + loss + SI-SDR, all on the device).
 
 Same constructor arguments and config keys as the reference, so `train.py:65-80` can construct it unchanged
 (``meta.use_amp`` is accepted: the kernels compute in fp32 / tf32, at least the precision of the reference's fp16
@@ -26,6 +26,7 @@ import torch
 from . import _lib
 from .acoustics.feature import drop_band, istft, stft
 from .acoustics.mask import build_complex_ideal_ratio_mask, decompress_cIRM
+from .dataset import mix_batch
 from .optim import FusedClipAdam
 
 
@@ -93,9 +94,14 @@ class Trainer:
             self._resume_checkpoint()
 
     # ------------------------------------------------------------------ one optimisation step (trainer.py:41-71)
-    def train_step(self, noisy, clean):
+    def train_step(self, noisy, clean=None):
+        """One step on ``(noisy, clean)`` [B,L], or on a batch of ``fullsubnet_b200.dataset.Dataset`` items passed as
+        ``noisy`` (a dict): moved to the device and mixed there (``dataset.mix_batch``) before the same step."""
         model, core = self.model, self.core
         self.optimizer.zero_grad(set_to_none=False)
+        if isinstance(noisy, dict):
+            assert clean is None, "a Dataset batch carries its own clean speech"
+            noisy, clean = mix_batch(noisy, self.device)
         noisy = noisy.to(self.device, non_blocking=True)
         clean = clean.to(self.device, non_blocking=True)
         noisy_mag, _, noisy_real, noisy_imag = self.torch_stft(noisy)
@@ -178,8 +184,8 @@ class Trainer:
 
     def _train_epoch(self, epoch):
         loss_total = torch.zeros((), device=self.device)
-        for noisy, clean in self.train_dataloader:
-            loss_total += self.train_step(noisy, clean)
+        for batch in self.train_dataloader:  # (noisy, clean), or a dict of Dataset items that train_step mixes
+            loss_total += self.train_step(batch) if isinstance(batch, dict) else self.train_step(*batch)
         return float(loss_total) / max(1, len(self.train_dataloader))  # the step loop itself never synchronises
 
     def train(self):
