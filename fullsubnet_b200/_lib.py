@@ -145,6 +145,8 @@ _SIGNATURES = {
                                           _S, _P]),
     "fsn_mse_loss_scratch_bytes": (_S, []),
     "fsn_mse_loss": (C.c_int, [_P, _P, _I, _I, _I, _P, _P, _P, _S, _P]),
+    "fsn_cirm_mse_per_clip_workspace_bytes": (_S, [_I, _I, _I, _I]),
+    "fsn_cirm_mse_per_clip": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _S, _P]),
     "fsn_clip_adam_scratch_bytes": (_S, []),
     "fsn_clip_adam": (C.c_int, [C.POINTER(ParamList), _F, _F, _F, _F, _F, _F, _I, _P, _P, _S, _P]),
     "fsn_fullband_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
@@ -158,6 +160,7 @@ _SIGNATURES = {
                                               _S, _P]),
     "fsn_peak_normalize_int16": (C.c_int, [_P, _I, _I, _F, _P, _P]),
     "fsn_si_sdr": (C.c_int, [_P, _P, _I, _I, _P, _P]),
+    "fsn_si_sdr_lengths": (C.c_int, [_P, _P, _P, _I, _I, _P, _P]),
     "fsn_rir_convolve": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P]),
     "fsn_snr_mix": (C.c_int, [_P, _P, _P, _P, _F, _F, _I, _I, _P, _P, _P]),
     "fsn_debug_row_to_unit": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -82,4 +82,30 @@ __device__ __forceinline__ float decompress_cirm_f(float m, float K, float limit
   return -K * logf((K - m) / (K + m));
 }
 
+// mask.py:38-40
+__device__ __forceinline__ float compress_cirm_f(float m, float K, float C) {
+  m = (m <= -100.f) ? -100.f : m;
+  const float e = expf(-C * m);
+  return K * (1.f - e) / (1.f + e);
+}
+
+// mask.py:22-29: the compressed cIRM (real, imag) of one bin from the noisy (a + ib) and clean (c + id) spectra
+__device__ __forceinline__ float2 cirm_f(float a, float b, float c, float d) {
+  const float eps = 1.1920928955078125e-07f;  // audio_zen/constant.py:9
+  const float den = a * a + b * b + eps;
+  return make_float2(compress_cirm_f((a * c + b * d) / den, 10.f, 0.1f), compress_cirm_f((a * d - b * c) / den, 10.f, 0.1f));
+}
+
+// fixed-order tree sum over the 256 threads of a CTA; the total reaches thread 0
+template <class V>
+__device__ __forceinline__ V cta_tree_sum256(V a, V* sh) {
+  sh[threadIdx.x] = a;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
+    __syncthreads();
+  }
+  return sh[0];
+}
+
 }  // namespace fsn

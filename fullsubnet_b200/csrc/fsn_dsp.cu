@@ -393,13 +393,6 @@ __global__ void decompress_kernel(const float* __restrict__ in, float* __restric
     out[i] = decompress_cirm_f(in[i], K, limit);
 }
 
-// mask.py:38-40
-__device__ __forceinline__ float compress_cirm_f(float m, float K, float C) {
-  m = (m <= -100.f) ? -100.f : m;
-  const float e = expf(-C * m);
-  return K * (1.f - e) / (1.f + e);
-}
-
 __global__ void compress_kernel(const float* __restrict__ in, float* __restrict__ out, int64_t n, float K, float C) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = compress_cirm_f(in[i], K, C);
@@ -409,13 +402,8 @@ __global__ void compress_kernel(const float* __restrict__ in, float* __restrict_
 __global__ void build_cirm_kernel(const float* __restrict__ nr, const float* __restrict__ ni,
                                   const float* __restrict__ cr, const float* __restrict__ ci,
                                   float2* __restrict__ out, int64_t n) {
-  const float eps = 1.1920928955078125e-07f;  // audio_zen/constant.py:9
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const float a = nr[i], b = ni[i], c = cr[i], d = ci[i];
-    const float den = a * a + b * b + eps;
-    out[i] = make_float2(compress_cirm_f((a * c + b * d) / den, 10.f, 0.1f),
-                         compress_cirm_f((a * d - b * c) / den, 10.f, 0.1f));
-  }
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = cirm_f(nr[i], ni[i], cr[i], ci[i]);
 }
 
 // feature.py:332-345: output clip b' of group g <- clip g + G*i, frequency f' <- g + G*f'
@@ -461,11 +449,11 @@ __global__ void peak_normalize_int16_kernel(const float* __restrict__ wav, int L
 
 // audio_zen/metrics.py:6-31 SI_SDR(reference, estimation) per clip: alpha = <ref,est>/<ref,ref>;
 // 10 log10(|alpha ref|^2 / |est - alpha ref|^2).  One CTA per clip, two passes, fixed-order tree reductions in
-// double (the reference sums in float32 pairwise; both agree to ~1e-5 dB on 4 s clips).
-__global__ void si_sdr_kernel(const float* __restrict__ ref, const float* __restrict__ est, int L, float* __restrict__ out) {
+// double (the reference sums in float32 pairwise; both agree to ~1e-5 dB on 4 s clips).  The CTA of 256 threads reduces
+// the L samples at r / e into *out.
+__device__ __forceinline__ void si_sdr_clip(const float* __restrict__ r, const float* __restrict__ e, int L,
+                                            float* __restrict__ out) {
   __shared__ double sa[256], sb[256];
-  const float* r = ref + (size_t)blockIdx.x * L;
-  const float* e = est + (size_t)blockIdx.x * L;
   double a = 0.0, b = 0.0;
   for (int i = threadIdx.x; i < L; i += blockDim.x) { a += (double)r[i] * r[i]; b += (double)r[i] * e[i]; }
   sa[threadIdx.x] = a; sb[threadIdx.x] = b;
@@ -488,7 +476,21 @@ __global__ void si_sdr_kernel(const float* __restrict__ ref, const float* __rest
     if (threadIdx.x < s) { sa[threadIdx.x] += sa[threadIdx.x + s]; sb[threadIdx.x] += sb[threadIdx.x + s]; }
     __syncthreads();
   }
-  if (threadIdx.x == 0) out[blockIdx.x] = (float)(10.0 * log10(sa[0] / sb[0]));
+  if (threadIdx.x == 0) *out = (float)(10.0 * log10(sa[0] / sb[0]));
+}
+
+// clip b: row b of [B, L]
+__global__ void si_sdr_kernel(const float* __restrict__ ref, const float* __restrict__ est, int L, float* __restrict__ out) {
+  const size_t o = (size_t)blockIdx.x * L;
+  si_sdr_clip(ref + o, est + o, L, out + blockIdx.x);
+}
+
+// clip c.off + i: the first c.v[i] samples of its row of [B, L_max]
+__global__ void si_sdr_lengths_kernel(const float* __restrict__ ref, const float* __restrict__ est, int L_max,
+                                      const __grid_constant__ LenChunk c, float* __restrict__ out) {
+  const int b = c.off + blockIdx.x;
+  const size_t o = (size_t)b * L_max;
+  si_sdr_clip(ref + o, est + o, c.v[blockIdx.x], out + b);
 }
 
 static bool is_pow2(int n) { return n > 0 && (n & (n - 1)) == 0; }
@@ -523,7 +525,7 @@ static int dsp_launch(void (*kernel)(KArgs...), dim3 grid, size_t smem, cudaStre
 }
 
 // host checks of stft_launch, before any CUDA call
-static int stft_check(int B, int L, int n_fft, int hop, int win_length, const float* magT, int T_pad) {
+int stft_check(int B, int L, int n_fft, int hop, int win_length, const float* magT, int T_pad) {
   FSN_REQUIRE(B > 0 && L > 0, FSN_ERR_SHAPE, "stft: empty input (B=%d, L=%d)", B, L);
   FSN_REQUIRE(B <= kMaxGridY, FSN_ERR_UNSUPPORTED, "stft: B=%d clips, at most %d", B, kMaxGridY);
   FSN_REQUIRE(dsp_size_ok(n_fft), FSN_ERR_UNSUPPORTED,
@@ -620,6 +622,24 @@ extern "C" int fsn_si_sdr(const float* reference, const float* estimation, int B
   FSN_REQUIRE(B > 0 && L > 0, FSN_ERR_SHAPE, "si_sdr: empty input");
   si_sdr_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(reference, estimation, L, out);
   FSN_CHECK_LAUNCH("si_sdr_kernel");
+  return FSN_OK;
+}
+
+extern "C" int fsn_si_sdr_lengths(const float* reference, const float* estimation, const int32_t* lengths, int B, int L_max,
+                                  float* out, fsn_stream_t stream) {
+  if (!lengths) return fsn_si_sdr(reference, estimation, B, L_max, out, stream);
+  FSN_REQUIRE(B > 0 && L_max > 0, FSN_ERR_SHAPE, "si_sdr_lengths: empty input");
+  for (int b = 0; b < B; ++b)
+    FSN_REQUIRE(lengths[b] > 0 && lengths[b] <= L_max, FSN_ERR_SHAPE,
+                "si_sdr_lengths: clip %d has length %d, outside (0, L_max] = (0, %d]", b, lengths[b], L_max);
+  LenChunk c;  // the lengths travel in the parameter block, like the length table of the wav -> wav entry points
+  for (int off = 0; off < B; off += kLenChunk) {
+    c.off = off;
+    c.n = B - off < kLenChunk ? B - off : kLenChunk;
+    memcpy(c.v, lengths + off, (size_t)c.n * sizeof(int));
+    si_sdr_lengths_kernel<<<c.n, 256, 0, (cudaStream_t)stream>>>(reference, estimation, L_max, c, out);
+    FSN_CHECK_LAUNCH("si_sdr_lengths_kernel");
+  }
   return FSN_OK;
 }
 

@@ -306,6 +306,8 @@ int norm_scales_launch(const float2* mag_sums, const float2* fb_sums, int B, flo
 
 // the n_fft the signal layer accepts: a power of two in [16, 2048] (radix-2 FFT) or even in [16, 1200] (direct DFT)
 bool dsp_size_ok(int n_fft);
+// the host checks stft_launch makes before any CUDA call, for entry points that must refuse before their own launches
+int stft_check(int B, int L, int n_fft, int hop, int win_length, const float* magT, int T_pad);
 // lens (nullable, device [B]): clip b has lens[b] of the L samples of its row (the *_enhance entry points)
 int stft_launch(const float* wav, int B, int L, int n_fft, int hop, int win_length, float* mag, float* phase,
                 float* real, float* imag, float* magT, int T_pad, cudaStream_t st, const int* lens = nullptr);

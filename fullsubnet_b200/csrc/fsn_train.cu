@@ -1024,6 +1024,14 @@ extern "C" int fsn_debug_lstm_train(const fsn_lstm_layer* layers, int n_layers, 
 
 // ------------------------------------------------------------------------------------------ loss
 namespace fsn {
+constexpr int MSE_BLOCKS = 1024;
+
+// the partition of an MSE over n elements: min(MSE_BLOCKS, ceil(n/256)) CTAs of 256 threads, grid-stride
+__host__ __device__ inline int mse_blocks(size_t n) {
+  const size_t nb = (n + 255) / 256;
+  return nb > MSE_BLOCKS ? MSE_BLOCKS : (int)nb;
+}
+
 // loss = mean((cirm - crm)^2) with cirm [B,Fs,T,2] (trainer.py:49-54) and crm [B,2,Fs,T] (Model.forward);
 // dcrm = 2 (crm - cirm) / n.  Stage 1: per-CTA partial sums; stage 2: fixed-order sum.
 __global__ void mse_part_kernel(const float* __restrict__ cirm, const float* __restrict__ crm, int Fs, int T, size_t n,
@@ -1042,27 +1050,72 @@ __global__ void mse_part_kernel(const float* __restrict__ cirm, const float* __r
     a = fmaf(dlt, dlt, a);
     if (dcrm) dcrm[i] = k * dlt;
   }
-  sh[threadIdx.x] = a;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) part[blockIdx.x] = sh[0];
+  a = cta_tree_sum256(a, sh);
+  if (threadIdx.x == 0) part[blockIdx.x] = a;
 }
-__global__ void mse_final_kernel(const float* __restrict__ part, int nb, size_t n, float* __restrict__ loss) {
+
+// stage 2 of one MSE: the nb partials summed in double in a fixed order, over n
+__device__ __forceinline__ float mse_final(const float* __restrict__ part, int nb, size_t n) {
   __shared__ double sh[256];
   double a = 0.0;
   for (int i = threadIdx.x; i < nb; i += 256) a += (double)part[i];
-  sh[threadIdx.x] = a;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *loss = (float)(sh[0] / (double)n);
+  return (float)(cta_tree_sum256(a, sh) / (double)n);
 }
-constexpr int MSE_BLOCKS = 1024;
+
+__global__ void mse_final_kernel(const float* __restrict__ part, int nb, size_t n, float* __restrict__ loss) {
+  const float v = mse_final(part, nb, n);
+  if (threadIdx.x == 0) *loss = v;
+}
+
+// Per-clip cIRM loss (grid (MSE_BLOCKS, B)): clip b = blockIdx.y has T_b = 1 + lens[b]/hop of the T frames (all T
+// without lens), n_b = 2 F T_b elements in crm's [o,f,t] order, and the partition of fsn_mse_loss at B = 1, T = T_b.
+// Each element builds its cIRM value from the four spectra [B,F,T] (fsn_build_cirm's arithmetic) and subtracts it
+// from crm [B,2,F,T] as mse_part_kernel does.  Partials at part[b * MSE_BLOCKS + CTA].
+__global__ void cirm_mse_part_kernel(const float* __restrict__ nr, const float* __restrict__ ni,
+                                     const float* __restrict__ cr, const float* __restrict__ ci,
+                                     const float* __restrict__ crm, int F, int T, int hop, const int* __restrict__ lens,
+                                     float* __restrict__ part) {
+  __shared__ float sh[256];
+  const int b = blockIdx.y;
+  const int Tb = lens ? 1 + lens[b] / hop : T;
+  const size_t n = (size_t)2 * F * Tb;
+  const int nb = mse_blocks(n);
+  if ((int)blockIdx.x >= nb) return;  // the whole CTA: no barrier is skipped
+  const size_t plane = (size_t)F * T;
+  const float* c = crm + (size_t)b * 2 * plane;
+  float a = 0.f;
+  for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)nb * 256) {
+    const int t = (int)(i % Tb);
+    const size_t q = i / Tb;
+    const int f = (int)(q % F);
+    const int o = (int)(q / F);
+    const size_t s = (size_t)b * plane + (size_t)f * T + t;
+    const float2 m = cirm_f(nr[s], ni[s], cr[s], ci[s]);
+    const float dlt = c[o * plane + (size_t)f * T + t] - (o ? m.y : m.x);
+    a = fmaf(dlt, dlt, a);
+  }
+  a = cta_tree_sum256(a, sh);
+  if (threadIdx.x == 0) part[(size_t)b * MSE_BLOCKS + blockIdx.x] = a;
+}
+
+__global__ void cirm_mse_final_kernel(const float* __restrict__ part, int F, int T, int hop, const int* __restrict__ lens,
+                                      float* __restrict__ loss) {
+  const int b = blockIdx.x;
+  const size_t n = (size_t)2 * F * (lens ? 1 + lens[b] / hop : T);
+  const float v = mse_final(part + (size_t)b * MSE_BLOCKS, mse_blocks(n), n);
+  if (threadIdx.x == 0) loss[b] = v;
+}
+
+// workspace of fsn_cirm_mse_per_clip: the noisy and clean spectra [B,F,T], the partials, the length table
+struct CirmMseWs { float *nr, *ni, *cr, *ci, *part; int* lens; };
+static size_t carve_cirm_mse(void* base, int B, int F, int T, CirmMseWs& w) {
+  Carver c(base);
+  const size_t BFT = (size_t)B * F * T;
+  w.nr = c.take<float>(BFT); w.ni = c.take<float>(BFT); w.cr = c.take<float>(BFT); w.ci = c.take<float>(BFT);
+  w.part = c.take<float>((size_t)B * MSE_BLOCKS);
+  w.lens = c.take<int>(B);
+  return c.off;
+}
 }  // namespace fsn
 
 extern "C" size_t fsn_mse_loss_scratch_bytes(void) { return MSE_BLOCKS * sizeof(float); }
@@ -1073,12 +1126,45 @@ extern "C" int fsn_mse_loss(const float* cirm, const float* crm, int B, int Fsub
   FSN_REQUIRE(scratch && scratch_bytes >= MSE_BLOCKS * sizeof(float), FSN_ERR_WORKSPACE, "mse_loss: scratch too small");
   cudaStream_t st = (cudaStream_t)stream;
   const size_t n = (size_t)B * 2 * Fsub * T;
-  int nb = (int)((n + 255) / 256);
-  if (nb > MSE_BLOCKS) nb = MSE_BLOCKS;
+  const int nb = mse_blocks(n);
   mse_part_kernel<<<nb, 256, 0, st>>>(cirm, crm, Fsub, T, n, dcrm, (float*)scratch);
   FSN_CHECK_LAUNCH("mse_part_kernel");
   mse_final_kernel<<<1, 256, 0, st>>>((const float*)scratch, nb, n, loss);
   FSN_CHECK_LAUNCH("mse_final_kernel");
+  return FSN_OK;
+}
+
+extern "C" size_t fsn_cirm_mse_per_clip_workspace_bytes(int B, int L_max, int n_fft, int hop) {
+  if (stft_check(B, L_max, n_fft, hop, n_fft, nullptr, 0)) return 0;  // the call's own checks, win_length aside
+  CirmMseWs w;
+  return carve_cirm_mse(nullptr, B, n_fft / 2 + 1, 1 + L_max / hop, w);
+}
+
+extern "C" int fsn_cirm_mse_per_clip(const float* noisy_wav, const float* clean_wav, const int32_t* lengths, int B,
+                                     int L_max, int n_fft, int hop, int win_length, const float* crm, float* loss,
+                                     void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  int rc = stft_check(B, L_max, n_fft, hop, win_length, nullptr, 0);
+  if (rc) return rc;
+  FSN_REQUIRE(noisy_wav && clean_wav && crm, FSN_ERR_SHAPE, "cirm_mse_per_clip: null input");
+  if ((rc = wav_check(lengths, B, L_max, n_fft, false, loss, "cirm_mse_per_clip"))) return rc;
+  const int F = n_fft / 2 + 1, T = 1 + L_max / hop;
+  CirmMseWs w;
+  const size_t bytes = carve_cirm_mse(workspace, B, F, T, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= bytes, FSN_ERR_WORKSPACE, "cirm_mse_per_clip: workspace too small: %zu < %zu",
+              workspace_bytes, bytes);
+  const cudaStream_t st = (cudaStream_t)stream;
+  WavWs lw = {nullptr, nullptr, nullptr, nullptr, w.lens};
+  if ((rc = wav_prologue(lengths, B, lw, st))) return rc;
+  if ((rc = stft_launch(noisy_wav, B, L_max, n_fft, hop, win_length, nullptr, nullptr, w.nr, w.ni, nullptr, 0, st,
+                        lw.lens)) ||
+      (rc = stft_launch(clean_wav, B, L_max, n_fft, hop, win_length, nullptr, nullptr, w.cr, w.ci, nullptr, 0, st,
+                        lw.lens)))
+    return rc;
+  cirm_mse_part_kernel<<<dim3(MSE_BLOCKS, B), 256, 0, st>>>(w.nr, w.ni, w.cr, w.ci, crm, F, T, hop, lw.lens, w.part);
+  FSN_CHECK_LAUNCH("cirm_mse_part_kernel");
+  cirm_mse_final_kernel<<<B, 256, 0, st>>>(w.part, F, T, hop, lw.lens, loss);
+  FSN_CHECK_LAUNCH("cirm_mse_final_kernel");
   return FSN_OK;
 }
 

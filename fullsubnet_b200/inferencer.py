@@ -129,14 +129,15 @@ class Inferencer:
                                       "improved_fullsubnet and fullband_baseline only")
 
     @torch.no_grad()
-    def enhance_batch(self, noisy: torch.Tensor, lengths=None) -> torch.Tensor:
+    def enhance_batch(self, noisy: torch.Tensor, lengths=None, return_crm: bool = False):
         """The same path for B independent clips in ONE library call (the model's fused call): pinned/host or device
         ``noisy`` [B,L] -> device tensor [B,L].  Equivalent to looping full_band_crm_mask over the clips.
-        ``lengths`` (models with a fused call): clip b is ``noisy[b, :lengths[b]]``, its row 0 past it."""
+        ``lengths`` (models with a fused call): clip b is ``noisy[b, :lengths[b]]``, its row 0 past it.
+        ``return_crm``: (enhanced, the model output [B,2,F,T] the mask was built from)."""
         self._check_lengths(lengths)
         x = noisy.to(self.device, non_blocking=True)
         if has_fused_call(self.model):
-            return self.model.enhance(x, *self._stft_args(), lengths=lengths)
+            return self.model.enhance(x, *self._stft_args(), lengths=lengths, return_crm=return_crm)
         # other models (fast_fullsubnet): same flow, three library calls (stft -> model -> mask + istft)
         import ctypes as C  # noqa: F401
         from . import _lib
@@ -153,7 +154,7 @@ class Inferencer:
             crm = self.model(buf[0].unsqueeze(1)).contiguous()
             _lib.check(lib.fsn_istft(buf[1].data_ptr(), buf[2].data_ptr(), 1, crm.data_ptr(), B, T, self.n_fft,
                                      self.hop_length, self.win_length, L, out.data_ptr(), st))
-        return out
+        return (out, crm) if return_crm else out
 
     @torch.no_grad()
     def enhance_to_pcm(self, noisy: torch.Tensor, lengths=None) -> torch.Tensor:

@@ -45,5 +45,28 @@ class MSELoss(torch.nn.Module):
         return _FusedMSE.apply(b.contiguous(), a.permute(0, 3, 1, 2).contiguous())
 
 
+def cirm_mse_per_clip(noisy, clean, crm, n_fft, hop_length, win_length, lengths=None) -> torch.Tensor:
+    """Validation loss of B clips in one call (fsn_cirm_mse_per_clip): noisy, clean [B,L] and the model output crm
+    [B,2,F,T] on them -> loss [B], where loss[b] equals ``MSELoss()(cIRM, cRM)`` of the trainer on clip b alone, bit
+    for bit.  ``lengths`` (B ints, max L): clip b is row b's first lengths[b] samples and its 1 + lengths[b] //
+    hop_length frames of crm."""
+    noisy = _lib.require_cuda(noisy, "noisy")
+    clean = _lib.require_cuda(clean, "clean")
+    crm = _lib.require_cuda(crm, "crm")
+    B, L = noisy.shape
+    assert clean.shape == (B, L) and crm.shape == (B, 2, n_fft // 2 + 1, 1 + L // hop_length), (clean.shape, crm.shape)
+    lens = None if lengths is None else _lib.lengths_table(lengths, B, L)
+    lib = _lib.load()
+    device = noisy.device
+    with torch.cuda.device(device):
+        n = _lib.check_workspace(lib.fsn_cirm_mse_per_clip_workspace_bytes(B, L, n_fft, hop_length))
+        ws = torch.empty(n, dtype=torch.uint8, device=device)
+        loss = torch.empty(B, dtype=torch.float32, device=device)
+        _lib.check(lib.fsn_cirm_mse_per_clip(noisy.data_ptr(), clean.data_ptr(), None if lens is None else lens.ctypes.data,
+                                             B, L, n_fft, hop_length, win_length, crm.data_ptr(), loss.data_ptr(),
+                                             ws.data_ptr(), n, _lib.stream_ptr(device)))
+    return loss
+
+
 mse_loss = MSELoss
 l1_loss = torch.nn.L1Loss

@@ -2,7 +2,8 @@
 fullband_baseline/trainer.py:32-71, the same loop without drop_band) on top of
 audio_zen/trainer/base_trainer.py:28-218 - the parts of the trainer that are arithmetic on the hot path (SURVEY 8a row
 A11, 8f rank 4): mixing of a Dataset batch, STFT of noisy/clean, cIRM target + drop_band, Model.forward, MSE,
-backward, gradient mean over ranks, clip, Adam; and the B=1 validation loop (enhance + loss + SI-SDR, all on the device).
+backward, gradient mean over ranks, clip, Adam; and the validation loop, its B=1 items enhanced in groups (enhance +
+per-clip loss + SI-SDR, all on the device).
 
 Same constructor arguments and config keys as the reference, so `train.py:65-80` can construct it unchanged
 (``meta.use_amp`` is accepted: the kernels compute in fp32 / tf32, at least the precision of the reference's fp16
@@ -21,12 +22,15 @@ from __future__ import annotations
 from functools import partial
 from pathlib import Path
 
+import numpy as np
 import torch
 
 from . import _lib
 from .acoustics.feature import drop_band, istft, stft
-from .acoustics.mask import build_complex_ideal_ratio_mask, decompress_cIRM
+from .acoustics.mask import build_complex_ideal_ratio_mask
 from .dataset import mix_batch
+from .inferencer import Inferencer, plan_batches
+from .loss import MSELoss, cirm_mse_per_clip
 from .optim import FusedClipAdam
 
 
@@ -42,16 +46,27 @@ def broadcast_parameters(model, dist, src: int = 0) -> None:
             dist.broadcast(t.data, src)
 
 
-def si_sdr(reference: torch.Tensor, estimation: torch.Tensor) -> torch.Tensor:
-    """audio_zen/metrics.py:6-31 on the device: [B,L] x [B,L] -> [B] dB (fsn_si_sdr)."""
+def si_sdr(reference: torch.Tensor, estimation: torch.Tensor, lengths=None) -> torch.Tensor:
+    """audio_zen/metrics.py:6-31 on the device: [B,L] x [B,L] -> [B] dB (fsn_si_sdr).  ``lengths`` (B ints, max L):
+    clip b is row b's first lengths[b] samples, and out[b] equals the call on it alone (fsn_si_sdr_lengths)."""
     reference = _lib.require_cuda(reference, "reference")
     estimation = _lib.require_cuda(estimation, "estimation")
     assert reference.shape == estimation.shape and reference.dim() == 2
-    out = torch.empty(reference.shape[0], dtype=torch.float32, device=reference.device)
+    B, L = reference.shape
+    lens = None if lengths is None else _lib.lengths_table(lengths, B, L)
+    out = torch.empty(B, dtype=torch.float32, device=reference.device)
     with torch.cuda.device(reference.device):
-        _lib.check(_lib.load().fsn_si_sdr(reference.data_ptr(), estimation.data_ptr(), reference.shape[0],
-                                          reference.shape[1], out.data_ptr(), _lib.stream_ptr(reference.device)))
+        _lib.check(_lib.load().fsn_si_sdr_lengths(reference.data_ptr(), estimation.data_ptr(),
+                                                  None if lens is None else lens.ctypes.data, B, L, out.data_ptr(),
+                                                  _lib.stream_ptr(reference.device)))
     return out
+
+
+def validation_groups(inferencer, lengths, batch_size: int, max_padding: float):
+    """The groups of validation items (indices into ``lengths``) that share one enhance call: ``plan_batches``, with
+    clips of different lengths together only where the model's fused call takes per-clip lengths
+    (``Inferencer.supports_lengths``); fast_fullsubnet gets equal-length groups, as in ``enhance_files``."""
+    return plan_batches(lengths, batch_size, max_padding if inferencer.supports_lengths() else 0.0)
 
 
 class Trainer:
@@ -71,6 +86,7 @@ class Trainer:
         ac = config["acoustics"]
         self.torch_stft = partial(stft, n_fft=ac["n_fft"], hop_length=ac["hop_length"], win_length=ac["win_length"])
         self.torch_istft = partial(istft, n_fft=ac["n_fft"], hop_length=ac["hop_length"], win_length=ac["win_length"])
+        self.acoustics = ac
         self.train_config = config["trainer"]["train"]
         self.epochs = self.train_config["epochs"]
         self.save_checkpoint_interval = self.train_config["save_checkpoint_interval"]
@@ -80,6 +96,10 @@ class Trainer:
         self.validation_config = config["trainer"].get("validation", {})
         self.validation_interval = self.validation_config.get("validation_interval", 1)
         self.save_max_metric_score = self.validation_config.get("save_max_metric_score", True)
+        # validation items per enhance call, and how much padding lets clips of different lengths share one
+        self.validation_batch_size = self.validation_config.get("batch_size", 32)
+        self.validation_max_padding = self.validation_config.get("max_padding", 0.25)
+        plan_batches([], self.validation_batch_size, self.validation_max_padding)  # refuses bad values here
         self.only_validation = only_validation
         self.start_epoch = 1
         self.best_score = float("-inf") if self.save_max_metric_score else float("inf")
@@ -127,44 +147,66 @@ class Trainer:
             self.optimizer.step()
         return loss.detach()
 
-    # ------------------------------------------------------------------ validation (trainer.py:78-181), B = 1 loop
+    # ------------------------------------------------------------------ validation (trainer.py:78-181), in groups
     @torch.no_grad()
+    def _validation_items(self):
+        """The validation dataloader's items (noisy [1,L], clean [1,L], name, speech_type) evaluated in groups
+        (``validation_groups``): one fused enhance call per group (the model's mask + iSTFT, as
+        Inferencer.enhance_batch), then ``cirm_mse_per_clip`` and ``si_sdr`` over each clip's own length.  Returns
+        (loss float32 [N], SI-SDR float32 [N], speech types) in dataloader order, after ONE device-to-host copy.  Each
+        loss equals the reference's B=1 ``loss_function(cIRM, cRM)`` on that item alone (no drop_band), bit for bit."""
+        if not isinstance(self.loss_function, (MSELoss, torch.nn.MSELoss)) or \
+                getattr(self.loss_function, "reduction", "mean") != "mean":
+            raise NotImplementedError("fullsubnet_b200: validation computes the recipes' mean-squared cIRM loss only")
+        ac = self.acoustics
+        n_fft, hop, win = ac["n_fft"], ac["hop_length"], ac["win_length"]
+        inferencer = Inferencer(config={"acoustics": ac}, model=self.core, device=self.device)
+        noisy_items, clean_items, item_types = [], [], []
+        for noisy, clean, name, speech_type in self.valid_dataloader:
+            assert len(name) == 1, "The batch size for the validation stage must be one."
+            assert noisy.shape == clean.shape and noisy.shape[0] == 1
+            noisy_items.append(noisy.to(self.device, non_blocking=True).reshape(-1))
+            clean_items.append(clean.to(self.device, non_blocking=True).reshape(-1))
+            item_types.append(speech_type[0])
+        lens = [x.numel() for x in noisy_items]
+        groups = validation_groups(inferencer, lens, self.validation_batch_size, self.validation_max_padding)
+        order = [i for g in groups for i in g]
+        values = torch.empty(2, len(order), dtype=torch.float32, device=self.device)  # loss, SI-SDR in group order
+        pos = 0
+        for g in groups:
+            g_lens = [lens[i] for i in g]
+            lengths = g_lens if min(g_lens) != max(g_lens) else None
+            noisy = torch.nn.utils.rnn.pad_sequence([noisy_items[i] for i in g], batch_first=True)
+            clean = torch.nn.utils.rnn.pad_sequence([clean_items[i] for i in g], batch_first=True)
+            enhanced, crm = inferencer.enhance_batch(noisy, lengths=lengths, return_crm=True)
+            values[0, pos:pos + len(g)] = cirm_mse_per_clip(noisy, clean, crm, n_fft, hop, win, lengths)
+            values[1, pos:pos + len(g)] = si_sdr(clean, enhanced, lengths)
+            pos += len(g)
+        per_item = np.empty((2, len(order)), dtype=np.float32)
+        per_item[:, order] = values.cpu().numpy()
+        return per_item[0], per_item[1], item_types
+
     def _validation_epoch(self, epoch):
-        """Per item (noisy [1,L], clean [1,L], name, speech_type): cIRM loss of the B=1 forward (no drop_band, like the
-        reference at B=1), enhanced waveform through decompress / complex product / iSTFT, SI-SDR on the device.
-        Returns the mean SI-SDR of the "With_reverb" items (the reference's score, trainer.py:181); per-type losses
-        and scores stay in ``self.last_validation``.  No host synchronisation inside the loop."""
+        """Loss and SI-SDR of every validation item (``_validation_items``), summed per speech type in float32 in
+        dataloader order like the reference's B=1 loop.  Returns the mean SI-SDR of the "With_reverb" items (the
+        reference's score, trainer.py:181); per-type losses and scores stay in ``self.last_validation``."""
         types = ("With_reverb", "No_reverb")
-        zero = lambda: torch.zeros((), device=self.device)  # noqa: E731
-        loss_total, n_items = zero(), 0
-        loss_list = {k: zero() for k in types}
-        score_list = {k: zero() for k in types}
-        count = {k: 0 for k in types}
         model = self.core
         was_training = model.training
         model.eval()
-        for noisy, clean, name, speech_type in self.valid_dataloader:
-            assert len(name) == 1, "The batch size for the validation stage must be one."
-            speech_type = speech_type[0]
-            noisy = noisy.to(self.device, non_blocking=True)
-            clean = clean.to(self.device, non_blocking=True)
-            noisy_mag, _, noisy_real, noisy_imag = self.torch_stft(noisy)
-            _, _, clean_real, clean_imag = self.torch_stft(clean)
-            cIRM = build_complex_ideal_ratio_mask(noisy_real, noisy_imag, clean_real, clean_imag)
-            cRM = model(noisy_mag.unsqueeze(1)).permute(0, 2, 3, 1)
-            loss = self.loss_function(cIRM, cRM)
-            cRM = decompress_cIRM(cRM)
-            enhanced_real = cRM[..., 0] * noisy_real - cRM[..., 1] * noisy_imag
-            enhanced_imag = cRM[..., 1] * noisy_real + cRM[..., 0] * noisy_imag
-            enhanced = self.torch_istft((enhanced_real, enhanced_imag), length=noisy.size(-1), input_type="real_imag")
-            assert noisy.shape == clean.shape == enhanced.shape
-            loss_total += loss
-            n_items += 1
-            loss_list[speech_type] += loss
-            score_list[speech_type] += si_sdr(clean, enhanced)[0]
+        try:
+            loss, score, item_types = self._validation_items()
+        finally:
+            model.train(was_training)
+        zero = np.float32(0.0)
+        loss_total, loss_list, score_list = zero, {k: zero for k in types}, {k: zero for k in types}
+        count = {k: 0 for k in types}
+        for i, speech_type in enumerate(item_types):
+            loss_total += loss[i]
+            loss_list[speech_type] += loss[i]
+            score_list[speech_type] += score[i]
             count[speech_type] += 1
-        model.train(was_training)
-        n = max(1, n_items)
+        n = max(1, len(item_types))
         self.last_validation = {
             "loss_total": float(loss_total) / n,
             "loss": {k: float(loss_list[k]) / n for k in types},  # divided by len(dataloader) like trainer.py:163-168

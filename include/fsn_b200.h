@@ -60,7 +60,10 @@ enum { FSN_CELL_LSTM = 0, FSN_CELL_GRU = 1 };
  *                       rel), needed where decompress_cIRM amplifies mask errors x100 (|cRM| near the 9.9 clip) */
 enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F16X3_TC = 3 };
 
-/* ABI version: 101 changed fsn_enhance's argument list; 102 appended norm_type to fsn_fast_desc, so that struct grew */
+/* ABI version: 101 changed fsn_enhance's argument list; 102 appended norm_type to fsn_fast_desc, so that struct grew.
+ * The version counts changes that break an existing caller.  Entry points added since 102 leave every earlier argument
+ * list and struct as it was, so the version stays 102; a caller finds them by symbol: fsn_cirm_mse_per_clip (+ its
+ * workspace query) and fsn_si_sdr_lengths (the grouped validation loss and SI-SDR). */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -343,6 +346,19 @@ size_t fsn_mse_loss_scratch_bytes(void);
 int fsn_mse_loss(const float* cirm, const float* crm, int B, int Fsub, int T, float* loss, float* dcrm,
                  void* scratch, size_t scratch_bytes, fsn_stream_t stream);
 
+/* Validation loss of recipes/dns_interspeech_2020/fullsubnet/trainer.py:78-181 for B clips at once (an addition at
+ * version 102, see fsn_version).  Clip b is the first lengths[b] samples of row b of noisy_wav / clean_wav [B,L_max] (lengths: host int32 [B], nullable = all
+ * L_max; n_fft/2 < lengths[b] <= L_max and max == L_max), and crm [B,2,F,T_max] (F = n_fft/2+1, T_max = 1 + L_max/hop)
+ * is the model output on it.  loss[b] (device [B]) = MSE between the compressed cIRM of the clip's two STFTs
+ * (fsn_build_cirm) and crm over its own T_b = 1 + lengths[b]/hop frames, reduced with the partition and tree of
+ * fsn_mse_loss at B = 1, T = T_b: bit-identical to fsn_stft + fsn_build_cirm + fsn_mse_loss on that clip alone.  No
+ * drop_band (the reference validates at B = 1).  Every argument is checked before any CUDA call; the workspace query
+ * needs no device and returns 0 for a refused shape. */
+size_t fsn_cirm_mse_per_clip_workspace_bytes(int B, int L_max, int n_fft, int hop);
+int fsn_cirm_mse_per_clip(const float* noisy_wav, const float* clean_wav, const int32_t* lengths, int B, int L_max,
+                          int n_fft, int hop, int win_length, const float* crm, float* loss, void* workspace,
+                          size_t workspace_bytes, fsn_stream_t stream);
+
 #define FSN_MAX_PARAM_TENSORS 64
 typedef struct fsn_param_list {
   int n;
@@ -452,6 +468,11 @@ int fsn_peak_normalize_int16(const float* wav, int B, int L, float gain, int16_t
  * fullsubnet/trainer.py:78-181 that is pure arithmetic; STOI / PESQ are third-party CPU packages and stay out).
  * reference, estimation [B,L] -> out[B] in dB; fixed-order reductions. */
 int fsn_si_sdr(const float* reference, const float* estimation, int B, int L, float* out, fsn_stream_t stream);
+/* fsn_si_sdr over the first lengths[b] samples of each row of [B,L_max] (lengths: host int32 [B], 0 < lengths[b] <=
+ * L_max, checked before any CUDA call; NULL = fsn_si_sdr).  out[b] is bit-identical to fsn_si_sdr on that clip alone.
+ * An addition at version 102 (see fsn_version). */
+int fsn_si_sdr_lengths(const float* reference, const float* estimation, const int32_t* lengths, int B, int L_max,
+                       float* out, fsn_stream_t stream);
 
 /* recipes/dns_interspeech_2020/dataset_train.py:136-199  Dataset.snr_mix for a batch (SURVEY 8f rank 4): the random
  * draws (snr, noisy target dBFS, which RIR) are made by the caller and passed in.
