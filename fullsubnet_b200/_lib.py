@@ -149,6 +149,7 @@ _SIGNATURES = {
     "fsn_cirm_mse_per_clip": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _S, _P]),
     "fsn_clip_adam_scratch_bytes": (_S, []),
     "fsn_clip_adam": (C.c_int, [C.POINTER(ParamList), _F, _F, _F, _F, _F, _F, _I, _P, _P, _S, _P]),
+    "fsn_clip_adam_steps": (C.c_int, [C.POINTER(ParamList), _F, _F, _F, _F, _F, _F, _P, _P, _P, _S, _P]),
     "fsn_fullband_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
     "fsn_fullband_forward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, _P, _P, _S, _P]),
     "fsn_fullband_enhance_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I, _I, _I]),

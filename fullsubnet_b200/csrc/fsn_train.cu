@@ -1209,9 +1209,15 @@ __global__ void gradnorm_final_kernel(const float* __restrict__ part, int n, flo
   }
 }
 
+// bias corrections of each tensor's own step: 1 - beta1^step and sqrt(1 - beta2^step), computed on the host in float
+struct AdamBias {
+  float bc1[FSN_MAX_PARAM_TENSORS];
+  float bc2_sqrt[FSN_MAX_PARAM_TENSORS];
+};
+
 // torch.optim.Adam single-tensor update (no weight decay / amsgrad); the clipped, scaled gradient is written back
-__global__ void adam_kernel(const fsn_param_list L, const float* __restrict__ coef_ptr, float lr, float b1, float b2,
-                            float eps, float bc1, float bc2_sqrt) {
+__global__ void adam_kernel(const fsn_param_list L, const AdamBias bias, const float* __restrict__ coef_ptr, float lr,
+                            float b1, float b2, float eps) {
   const int ti = blockIdx.y;
   float* p = L.param[ti];
   float* g = L.grad[ti];
@@ -1219,7 +1225,8 @@ __global__ void adam_kernel(const fsn_param_list L, const float* __restrict__ co
   float* v = L.exp_avg_sq[ti];
   const int64_t n = L.numel[ti];
   const float coef = coef_ptr[1];
-  const float step_size = lr / bc1;
+  const float step_size = lr / bias.bc1[ti];
+  const float bc2_sqrt = bias.bc2_sqrt[ti];
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) {
     const float gi = g[i] * coef;
     g[i] = gi;
@@ -1235,13 +1242,21 @@ __global__ void adam_kernel(const fsn_param_list L, const float* __restrict__ co
 
 extern "C" size_t fsn_clip_adam_scratch_bytes(void) { return (FSN_MAX_PARAM_TENSORS * ADAM_CHUNKS + 2) * sizeof(float); }
 
-extern "C" int fsn_clip_adam(const fsn_param_list* L, float max_norm, float grad_scale, float lr, float beta1,
-                             float beta2, float eps, int step, float* norm_out, void* scratch, size_t scratch_bytes,
-                             fsn_stream_t stream) {
+extern "C" int fsn_clip_adam_steps(const fsn_param_list* L, float max_norm, float grad_scale, float lr, float beta1,
+                                   float beta2, float eps, const int* steps, float* norm_out, void* scratch,
+                                   size_t scratch_bytes, fsn_stream_t stream) {
   FSN_REQUIRE(L && L->n > 0 && L->n <= FSN_MAX_PARAM_TENSORS, FSN_ERR_SHAPE, "clip_adam: 1..%d tensors",
               FSN_MAX_PARAM_TENSORS);
-  FSN_REQUIRE(step >= 1, FSN_ERR_SHAPE, "clip_adam: step starts at 1");
+  FSN_REQUIRE(steps, FSN_ERR_SHAPE, "clip_adam: no step table");
+  for (int i = 0; i < L->n; ++i)
+    FSN_REQUIRE(steps[i] >= 1, FSN_ERR_SHAPE, "clip_adam: step starts at 1 (tensor %d has step %d)", i, steps[i]);
   FSN_REQUIRE(scratch && scratch_bytes >= fsn_clip_adam_scratch_bytes(), FSN_ERR_WORKSPACE, "clip_adam: scratch too small");
+  AdamBias bias;
+  for (int i = 0; i < L->n; ++i) {
+    bias.bc1[i] = 1.f - powf(beta1, (float)steps[i]);
+    bias.bc2_sqrt[i] = sqrtf(1.f - powf(beta2, (float)steps[i]));
+  }
+  for (int i = L->n; i < FSN_MAX_PARAM_TENSORS; ++i) bias.bc1[i] = bias.bc2_sqrt[i] = 1.f;  // unread
   cudaStream_t st = (cudaStream_t)stream;
   float* part = (float*)scratch;
   float* res = norm_out ? norm_out : part + FSN_MAX_PARAM_TENSORS * ADAM_CHUNKS;
@@ -1249,9 +1264,20 @@ extern "C" int fsn_clip_adam(const fsn_param_list* L, float max_norm, float grad
   FSN_CHECK_LAUNCH("gradsq_part_kernel");
   gradnorm_final_kernel<<<1, 256, 0, st>>>(part, L->n * ADAM_CHUNKS, grad_scale, max_norm, res);
   FSN_CHECK_LAUNCH("gradnorm_final_kernel");
-  const float bc1 = 1.f - powf(beta1, (float)step);
-  const float bc2 = 1.f - powf(beta2, (float)step);
-  adam_kernel<<<dim3(ADAM_CHUNKS * 4, L->n), 256, 0, st>>>(*L, res, lr, beta1, beta2, eps, bc1, sqrtf(bc2));
+  adam_kernel<<<dim3(ADAM_CHUNKS * 4, L->n), 256, 0, st>>>(*L, bias, res, lr, beta1, beta2, eps);
   FSN_CHECK_LAUNCH("adam_kernel");
   return FSN_OK;
+}
+
+// every tensor at the same step: the bias corrections, and so every output bit, of the single-step launcher
+extern "C" int fsn_clip_adam(const fsn_param_list* L, float max_norm, float grad_scale, float lr, float beta1,
+                             float beta2, float eps, int step, float* norm_out, void* scratch, size_t scratch_bytes,
+                             fsn_stream_t stream) {
+  FSN_REQUIRE(L && L->n > 0 && L->n <= FSN_MAX_PARAM_TENSORS, FSN_ERR_SHAPE, "clip_adam: 1..%d tensors",
+              FSN_MAX_PARAM_TENSORS);
+  FSN_REQUIRE(step >= 1, FSN_ERR_SHAPE, "clip_adam: step starts at 1");
+  int steps[FSN_MAX_PARAM_TENSORS];
+  for (int i = 0; i < L->n; ++i) steps[i] = step;
+  return fsn_clip_adam_steps(L, max_norm, grad_scale, lr, beta1, beta2, eps, steps, norm_out, scratch, scratch_bytes,
+                             stream);
 }

@@ -1,6 +1,7 @@
 """``clip_grad_norm_`` + ``torch.optim.Adam.step`` (fullsubnet/trainer.py:65-68, train.py:55-59) as three kernel
-launches without a host synchronisation (fsn_clip_adam).  State keys (``step``, ``exp_avg``, ``exp_avg_sq``) and
-``param_groups`` follow torch.optim.Adam, so checkpoints written by either optimiser load into the other."""
+launches without a host synchronisation (fsn_clip_adam_steps).  State keys (``step``, ``exp_avg``, ``exp_avg_sq``) and
+``param_groups`` follow torch.optim.Adam, so checkpoints written by either optimiser load into the other.  Like
+torch.optim.Adam, each parameter counts its own steps: one whose grad is None is skipped and its count stays."""
 from __future__ import annotations
 
 import ctypes as C
@@ -46,7 +47,7 @@ class FusedClipAdam(torch.optim.Optimizer):
                 raise NotImplementedError(f"FusedClipAdam handles <= {_lib.MAX_PARAM_TENSORS} tensors per group")
             L = _lib.ParamList()
             L.n = len(ps)
-            step = None
+            steps = (C.c_int * len(ps))()
             for i, p in enumerate(ps):
                 _lib.require_cuda(p, "parameter")
                 st = self.state[p]
@@ -55,7 +56,7 @@ class FusedClipAdam(torch.optim.Optimizer):
                     st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                     st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                 st["step"] += 1
-                step = int(st["step"])
+                steps[i] = int(st["step"])
                 g = p.grad
                 if not g.is_contiguous() or g.dtype != torch.float32:
                     raise RuntimeError("FusedClipAdam needs contiguous fp32 gradients")
@@ -68,9 +69,10 @@ class FusedClipAdam(torch.optim.Optimizer):
                     self._scratch = torch.empty(lib.fsn_clip_adam_scratch_bytes(), dtype=torch.uint8, device=device)
                 self.last_norm = torch.empty(2, dtype=torch.float32, device=device)
                 b1, b2 = group["betas"]
-                _lib.check(lib.fsn_clip_adam(C.byref(L), float(self.max_norm or 0.0), float(grad_scale), group["lr"],
-                                             b1, b2, group["eps"], step, self.last_norm.data_ptr(),
-                                             self._scratch.data_ptr(), self._scratch.numel(), _lib.stream_ptr(device)))
+                _lib.check(lib.fsn_clip_adam_steps(C.byref(L), float(self.max_norm or 0.0), float(grad_scale),
+                                                   group["lr"], b1, b2, group["eps"], steps, self.last_norm.data_ptr(),
+                                                   self._scratch.data_ptr(), self._scratch.numel(),
+                                                   _lib.stream_ptr(device)))
             # the kernel wrote through raw pointers: tell autograd / the packed-weight caches (keyed on
             # (data_ptr, _version), fullsubnet/model.py:_packed_sb) that the parameters changed
             torch._C._increment_version(ps)

@@ -63,7 +63,8 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
 /* ABI version: 101 changed fsn_enhance's argument list; 102 appended norm_type to fsn_fast_desc, so that struct grew.
  * The version counts changes that break an existing caller.  Entry points added since 102 leave every earlier argument
  * list and struct as it was, so the version stays 102; a caller finds them by symbol: fsn_cirm_mse_per_clip (+ its
- * workspace query) and fsn_si_sdr_lengths (the grouped validation loss and SI-SDR). */
+ * workspace query), fsn_si_sdr_lengths (the grouped validation loss and SI-SDR) and fsn_clip_adam_steps (one Adam step
+ * count per tensor). */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -304,7 +305,13 @@ int64_t fsn_total_launch_count(void);
  *   fsn_clip_adam       = clip_grad_norm_(max_norm) + Adam step (trainer.py:65-68, train.py:55-59) over a list of
  *                         tensors, no host synchronisation.  grad_scale multiplies every gradient first (1/world
  *                         after a sum all-reduce).  norm_out (optional, 2 floats on the device) receives the total
- *                         norm and the applied coefficient; gradients are left clipped like the reference. */
+ *                         norm and the applied coefficient; gradients are left clipped like the reference.
+ *                         Every tensor is at the same step (>= 1).
+ *   fsn_clip_adam_steps = fsn_clip_adam with one step per tensor, as torch.optim.Adam keeps one per parameter (a
+ *                         parameter skipped while its grad was None, a resumed checkpoint): steps is a HOST array of
+ *                         L->n entries, each >= 1, read during the call and not retained.  Tensor i gets the bias
+ *                         corrections of steps[i]; with every entry equal the outputs are those of fsn_clip_adam bit
+ *                         for bit.  Arguments are checked before any CUDA call. */
 typedef struct fsn_seq_grads {
   float* w_ih[2];
   float* w_hh[2];
@@ -372,6 +379,9 @@ typedef struct fsn_param_list {
 size_t fsn_clip_adam_scratch_bytes(void);
 int fsn_clip_adam(const fsn_param_list* L, float max_norm, float grad_scale, float lr, float beta1, float beta2,
                   float eps, int step, float* norm_out, void* scratch, size_t scratch_bytes, fsn_stream_t stream);
+int fsn_clip_adam_steps(const fsn_param_list* L, float max_norm, float grad_scale, float lr, float beta1, float beta2,
+                        float eps, const int* steps, float* norm_out, void* scratch, size_t scratch_bytes,
+                        fsn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * recipes/dns_interspeech_2020/fullband_baseline/model.py:8-68  Model (SURVEY 8f rank 3)
