@@ -189,6 +189,12 @@ _SIGNATURES = {
     "fsn_debug_istft": (C.c_int, [_P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P]),
     "fsn_debug_istft_mask_adjoint": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
     "fsn_debug_wav_epilogue": (C.c_int, [_P, _P, _I, _I, _P, _P, _F, _P, _P, _I, _I, _I, _P]),
+    "fsn_debug_norm_unfold_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _P, _P, _P]),
+    "fsn_debug_fast_norm_unfold_bwd": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P, _P, _P, _P]),
+    "fsn_debug_imp_unfold_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "fsn_debug_imp_section_input": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "fsn_debug_norm_stats": (C.c_int, [_P, _I, _I, _I, _I, _L, _L, _P, _P, _I, _I, _P, _F, _F, _F, _P, _P, _P, _P, _P]),
+    "fsn_debug_train_stats": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P]),
     "fsn_last_error_code": (C.c_int, []),
     "fsn_last_launch_count": (C.c_int64, []),
     "fsn_total_launch_count": (C.c_int64, []),

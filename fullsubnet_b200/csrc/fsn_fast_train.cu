@@ -90,6 +90,31 @@ __global__ void ftr_cum_suffix_kernel(const float* __restrict__ dX, const float*
   }
 }
 
+int ftr_dbn_launch(const float* ddec, const float* bn_out, int B, int Tp, int M, int S, int Ts, float* dbn, cudaStream_t st) {
+  ftr_dbn_kernel<<<ew_grid((size_t)Ts * B * M), 256, 0, st>>>(ddec, bn_out, B, Tp, M, S, Ts, dbn);
+  FSN_CHECK_LAUNCH("ftr_dbn_kernel");
+  return FSN_OK;
+}
+
+int ftr_cum_suffix_launch(const float* dX, const float* X, const float* scaleT, int Ts, int R, int K, float* suffix,
+                          cudaStream_t st) {
+  ftr_cum_suffix_kernel<<<cdiv(R, 128), 128, 0, st>>>(dX, X, scaleT, Ts, R, K, suffix);
+  FSN_CHECK_LAUNCH("ftr_cum_suffix_kernel");
+  return FSN_OK;
+}
+
+int ftr_denc_launch(bool cum, const float* ddec, const float* dX, const float* encT, const float* inv2, const float* dot,
+                    const float* scaleT, const float* suffix, int B, int Tp, int M, int Nn, int Ne, int S, float cnt2,
+                    float* denc, cudaStream_t st) {
+  const unsigned grid = ew_grid((size_t)Tp * B * M);
+  if (cum)
+    ftr_denc_kernel<true><<<grid, 256, 0, st>>>(ddec, dX, encT, inv2, dot, scaleT, suffix, B, Tp, M, Nn, Ne, S, cnt2, denc);
+  else
+    ftr_denc_kernel<false><<<grid, 256, 0, st>>>(ddec, dX, encT, inv2, dot, scaleT, suffix, B, Tp, M, Nn, Ne, S, cnt2, denc);
+  FSN_CHECK_LAUNCH("ftr_denc_kernel");
+  return FSN_OK;
+}
+
 // ------------------------------------------------------------------------------------------ workspace
 enum { L_ENC1, L_ENC2, L_BN0, L_BN1, L_DEC1, L_DEC2, NL };
 
@@ -259,8 +284,7 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
     if ((rc = cum_clip_scale_launch(w.fs1, B, Tp, M, TRAIN_CUM_EPS, w.cum1, st))) return rc;
     if ((rc = scale_rows_launch(w.melT, w.cum1, (size_t)Tp * B * M, M, Tp * B, 1, w.xenc, st))) return rc;
   } else {
-    train_tm_stats_kernel<<<B, 256, 0, st>>>(w.melT, B, M, Tp, 0, w.sums1);
-    FSN_CHECK_LAUNCH("train_tm_stats_kernel");
+    if ((rc = train_tm_stats_launch(w.melT, B, M, Tp, 0, w.sums1, st))) return rc;
     if ((rc = norm_scales_launch(w.sums1, w.sums1, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) return rc;
     if ((rc = scale_rows_launch(w.melT, w.inv1, (size_t)Tp * B * M, M, B, 1, w.xenc, st))) return rc;
   }
@@ -333,8 +357,7 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   if ((rc = layer_weight_grads(L[L_DEC1], Tp, w.dec_in, g->dec1.w_ih, g->dec1.w_hh, g->dec1.b_ih, g->dec1.b_hh, wg, st)))
     return rc;
   // ---- up-sampling transpose + ReLU' of the bottleneck output, its Linear(1)
-  ftr_dbn_kernel<<<ew_grid((size_t)Ts * R), 256, 0, st>>>(w.ddec, w.bn_out, B, Tp, M, m.S, Ts, w.dbn);
-  FSN_CHECK_LAUNCH("ftr_dbn_kernel");
+  if ((rc = ftr_dbn_launch(w.ddec, w.bn_out, B, Tp, M, m.S, Ts, w.dbn, st))) return rc;
   if ((rc = linear_bwd(w.dbn, w.L[L_BN1].H, wt->bn_fc_w, Ts * R, 1, Hb, g->bn_fc_w, g->bn_fc_b, nullptr, w.splitk, w.colsum,
                        st)))
     return rc;
@@ -346,19 +369,16 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
     return rc;
   // ---- second norm + down-sampling + unfold backward, ReLU' of the encoder output, its Linear(M)
   if (m.cum) {
-    ftr_cum_suffix_kernel<<<cdiv(R, 128), 128, 0, st>>>(w.dxbn, w.xbn, w.cum2, Ts, R, K, w.suffix);
-    FSN_CHECK_LAUNCH("ftr_cum_suffix_kernel");
-    ftr_denc_kernel<true><<<ew_grid((size_t)Tp * B * M), 256, 0, st>>>(
-        w.ddec, w.dxbn, w.encT, nullptr, nullptr, w.cum2, w.suffix, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors,
-        m.S, 0.f, w.denc);
+    if ((rc = ftr_cum_suffix_launch(w.dxbn, w.xbn, w.cum2, Ts, R, K, w.suffix, st))) return rc;
+    if ((rc = ftr_denc_launch(true, w.ddec, w.dxbn, w.encT, nullptr, nullptr, w.cum2, w.suffix, B, Tp, M,
+                              d->noisy_num_neighbors, d->enc_num_neighbors, m.S, 0.f, w.denc, st)))
+      return rc;
   } else {
-    train_dot_kernel<<<B, 256, 0, st>>>(w.dxbn, w.xbn, Ts, R, M, K, w.dot);
-    FSN_CHECK_LAUNCH("train_dot_kernel");
-    ftr_denc_kernel<false><<<ew_grid((size_t)Tp * B * M), 256, 0, st>>>(
-        w.ddec, w.dxbn, w.encT, w.inv2, w.dot, nullptr, nullptr, B, Tp, M, d->noisy_num_neighbors, d->enc_num_neighbors, m.S,
-        (float)M * K * Ts, w.denc);
+    if ((rc = train_dot_launch(w.dxbn, w.xbn, Ts, R, M, K, B, w.dot, st))) return rc;
+    if ((rc = ftr_denc_launch(false, w.ddec, w.dxbn, w.encT, w.inv2, w.dot, nullptr, nullptr, B, Tp, M,
+                              d->noisy_num_neighbors, d->enc_num_neighbors, m.S, (float)M * K * Ts, w.denc, st)))
+      return rc;
   }
-  FSN_CHECK_LAUNCH("ftr_denc_kernel");
   if ((rc = linear_bwd(w.denc, w.L[L_ENC2].H, wt->enc_fc_w, Tp * B, M, He2, g->enc_fc_w, g->enc_fc_b, w.dH, w.splitk, w.colsum,
                        st)))
     return rc;
@@ -367,4 +387,32 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   if ((rc = layer_weight_grads(L[L_ENC2], Tp, w.L[L_ENC1].H, g->enc2.w_ih, g->enc2.w_hh, g->enc2.b_ih, g->enc2.b_hh, wg, st)))
     return rc;
   return layer_weight_grads(L[L_ENC1], Tp, w.xenc, g->enc1.w_ih, g->enc1.w_hh, g->enc1.b_ih, g->enc1.b_hh, wg, st);
+}
+
+// ---- unit-test hook of the bottleneck backward (include/fsn_b200.h): the launchers fsn_fast_train_backward runs, every
+// argument checked before any CUDA call
+extern "C" int fsn_debug_fast_norm_unfold_bwd(const float* ddec, const float* dX, const float* X, const float* encT,
+                                              const float* bn_out, const float* scale, int cum, int B, int Tp, int M, int Nn,
+                                              int Ne, int S, float cnt2, float* mid, float* denc, float* dbn,
+                                              fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(ddec && (!dbn || bn_out) && (!denc || (dX && X && encT && scale && mid)), FSN_ERR_SHAPE,
+              "fast backward hook: null argument");
+  FSN_REQUIRE(B > 0 && Tp > 0 && M > 0 && S > 0, FSN_ERR_SHAPE, "fast backward hook: bad shape B=%d Tp=%d M=%d S=%d", B, Tp,
+              M, S);
+  FSN_REQUIRE(Nn >= 0 && Ne >= 0 && Nn < M && Ne < M, FSN_ERR_SHAPE, "fast backward hook: reflect padding needs 0 <= Nn, Ne < M");
+  FSN_REQUIRE(cum || !denc || cnt2 > 0.f, FSN_ERR_SHAPE, "fast backward hook: cnt2 must be positive");
+  const int Ts = 1 + cdiv(Tp - 1, S), R = B * M, K = (2 * Nn + 1) + (2 * Ne + 1);
+  FSN_REQUIRE((size_t)Tp * B * 2 * M < ((size_t)1 << 31) && (size_t)Ts * R * K < ((size_t)1 << 31), FSN_ERR_SHAPE,
+              "fast backward hook: tensors must stay below 2^31 elements");
+  const cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (dbn && (rc = ftr_dbn_launch(ddec, bn_out, B, Tp, M, S, Ts, dbn, st))) return rc;
+  if (!denc) return FSN_OK;
+  if (cum) {
+    if ((rc = ftr_cum_suffix_launch(dX, X, scale, Ts, R, K, mid, st))) return rc;
+    return ftr_denc_launch(true, ddec, dX, encT, nullptr, nullptr, scale, mid, B, Tp, M, Nn, Ne, S, 0.f, denc, st);
+  }
+  if ((rc = train_dot_launch(dX, X, Ts, R, M, K, B, mid, st))) return rc;
+  return ftr_denc_launch(false, ddec, dX, encT, scale, mid, nullptr, nullptr, B, Tp, M, Nn, Ne, S, cnt2, denc, st);
 }

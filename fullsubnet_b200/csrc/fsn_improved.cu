@@ -59,6 +59,13 @@ __global__ void imp_section_input_kernel(const float* __restrict__ magc, const f
   if (threadIdx.x == 0) fs[(size_t)b * T + t] = make_float2(red[0], red[0]);
 }
 
+int imp_section_input_launch(const float* magc, const float* fbT, int B, int T, int Fu, const SecGeom& g, float* X, float2* fs,
+                             bool tm, cudaStream_t st) {
+  imp_section_input_kernel<<<B * T, 256, 0, st>>>(magc, fbT, B, T, Fu, g, X, fs, tm);
+  FSN_CHECK_LAUNCH("imp_section_input_kernel");
+  return FSN_OK;
+}
+
 struct ImpWs {
   float *mag, *real, *imag, *crm, *magc, *fbT, *X, *inv1, *invs;
   float2 *fs, *sums;
@@ -80,6 +87,17 @@ static SeqStack imp_fb_stack(const fsn_improved_desc* d, const ImpDims& m) {
   return s;
 }
 
+int sec_geom(int lo, int hi, int cs, int ns, int cf, int nf, int Fu, SecGeom& g) {
+  g.lo = lo; g.cs = cs; g.ns = ns; g.cf = cf; g.nf = nf;
+  FSN_REQUIRE(cs > 0 && cf > 0 && lo >= 0 && hi > lo && (hi - lo) % cs == 0 && (hi - lo) % cf == 0, FSN_ERR_SHAPE,
+              "The number of center frequencies should be divisible by the subband freqency interval.");
+  FSN_REQUIRE(cs == cf, FSN_ERR_UNSUPPORTED, "improved model: sb/fb centre widths of a section must match");
+  FSN_REQUIRE(ns >= 0 && nf >= 0 && ns < Fu && nf < Fu, FSN_ERR_SHAPE, "improved model: neighbours >= num_freqs");
+  g.N = (hi - lo) / cs;
+  g.W = (cs + 2 * ns) + (cf + 2 * nf);
+  return FSN_OK;
+}
+
 int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
   FSN_REQUIRE(d && B > 0 && L > 0, FSN_ERR_SHAPE, "improved model: empty input");
   FSN_REQUIRE(dsp_size_ok(d->n_fft), FSN_ERR_UNSUPPORTED,
@@ -92,15 +110,9 @@ int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
   m.maxRW = 0; m.maxR = 0;
   for (int s = 0; s < m.S; ++s) {
     SecGeom& g = m.sec[s];
-    g.lo = s == 0 ? 0 : d->freq_cutoffs[s - 1];
-    const int hi = s == m.S - 1 ? m.Fu : d->freq_cutoffs[s];
-    g.cs = d->sb_num_center[s]; g.ns = d->sb_num_neighbor[s]; g.cf = d->fb_num_center[s]; g.nf = d->fb_num_neighbor[s];
-    FSN_REQUIRE(g.cs > 0 && hi > g.lo && (hi - g.lo) % g.cs == 0 && (hi - g.lo) % g.cf == 0, FSN_ERR_SHAPE,
-                "The number of center frequencies should be divisible by the subband freqency interval.");
-    FSN_REQUIRE(g.cs == g.cf, FSN_ERR_UNSUPPORTED, "improved model: sb/fb centre widths of a section must match");
-    FSN_REQUIRE(g.ns < m.Fu && g.nf < m.Fu, FSN_ERR_SHAPE, "improved model: neighbours >= num_freqs");
-    g.N = (hi - g.lo) / g.cs;
-    g.W = (g.cs + 2 * g.ns) + (g.cf + 2 * g.nf);
+    const int rc = sec_geom(s == 0 ? 0 : d->freq_cutoffs[s - 1], s == m.S - 1 ? m.Fu : d->freq_cutoffs[s], d->sb_num_center[s],
+                            d->sb_num_neighbor[s], d->fb_num_center[s], d->fb_num_neighbor[s], m.Fu, g);
+    if (rc) return rc;
     if (g.N * g.W > m.maxRW) m.maxRW = g.N * g.W;
     if (g.N > m.maxR) m.maxR = g.N;
   }
@@ -169,8 +181,7 @@ static int imp_forward(const fsn_improved_desc* d, const fsn_improved_weights* w
   for (int s = 0; s < m.S; ++s) {
     const SecGeom& g = m.sec[s];
     const int R = B * g.N;
-    imp_section_input_kernel<<<B * T, 256, 0, st>>>(w.magc, w.fbT, B, T, Fu, g, w.X, w.fs, false);
-    FSN_CHECK_LAUNCH("imp_section_input_kernel");
+    if ((rc = imp_section_input_launch(w.magc, w.fbT, B, T, Fu, g, w.X, w.fs, false, st))) return rc;
     if ((rc = clip_reduce_only_launch(w.fs, B, T, w.sums, st, lens, hop, 0))) return rc;
     if ((rc = norm_scales_launch(w.sums, w.sums, B, lens ? (float)g.N * g.W : (float)g.N * g.W * T, 1.f, w.invs, nullptr,
                                  st, eps, lens, hop, 0)))
@@ -259,4 +270,20 @@ extern "C" int fsn_improved_enhance(const fsn_improved_desc* d, const fsn_improv
   if ((rc = wav_prologue(lengths, B, w.wav, st))) return rc;
   if ((rc = imp_forward(d, wt, m, w, wav, enhanced, crm_out, pcm ? w.wav.peak : nullptr, w.wav.lens, st))) return rc;
   return wav_epilogue(w.wav, enhanced, B, L_max, pcm, gain, crm_out, m.F, m.T, d->hop_length, st);
+}
+
+// ---- unit-test hook of the section input (include/fsn_b200.h): the launcher both improved forwards run, every argument
+// checked before any CUDA call
+extern "C" int fsn_debug_imp_section_input(const float* magc, const float* fbT, int B, int T, int Fu, int lo, int hi, int cs,
+                                           int ns, int cf, int nf, int tm, float* X, float* fs, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(magc && fbT && X && fs, FSN_ERR_SHAPE, "section input hook: null argument");
+  FSN_REQUIRE(B > 0 && T > 0 && Fu >= 2 && hi <= Fu, FSN_ERR_SHAPE, "section input hook: bad shape B=%d T=%d Fu=%d", B, T,
+              Fu);
+  SecGeom g;
+  const int rc = sec_geom(lo, hi, cs, ns, cf, nf, Fu, g);
+  if (rc) return rc;
+  FSN_REQUIRE((size_t)T * B * g.N * g.W < ((size_t)1 << 31) && (size_t)B * T < ((size_t)1 << 31), FSN_ERR_SHAPE,
+              "section input hook: tensors must stay below 2^31 elements");
+  return imp_section_input_launch(magc, fbT, B, T, Fu, g, X, reinterpret_cast<float2*>(fs), tm != 0, (cudaStream_t)stream);
 }

@@ -142,6 +142,13 @@ __global__ void imp_unfold_bwd_kernel(const float* __restrict__ dX, const float*
   }
 }
 
+int imp_unfold_bwd_launch(const float* dX, const float* invs, const float* dot, float cnt, const SecGeom& g, int B, int T,
+                          int Fu, bool first, int act, const float* y, float* dfb, cudaStream_t st) {
+  imp_unfold_bwd_kernel<<<ew_grid((size_t)T * B * Fu), 256, 0, st>>>(dX, invs, dot, cnt, g, B, T, Fu, first, act, y, dfb);
+  FSN_CHECK_LAUNCH("imp_unfold_bwd_kernel");
+  return FSN_OK;
+}
+
 }  // namespace fsn
 
 using namespace fsn;
@@ -174,8 +181,7 @@ extern "C" int fsn_improved_train_forward(const fsn_improved_desc* d, const fsn_
   imp_compress_kernel<<<dim3(cdiv(T, 32), cdiv(Fu, 32), B), dim3(32, 8), 0, st>>>(w.mag, w.raw, F, T, d->fdrc, true);
   FSN_CHECK_LAUNCH("imp_compress_kernel");
   // full band: norm (566) -> 2xLSTM + Linear + act (567), y kept for act'
-  train_tm_stats_kernel<<<B, 256, 0, st>>>(w.raw, B, Fu, T, 0, w.sums);
-  FSN_CHECK_LAUNCH("train_tm_stats_kernel");
+  if ((rc = train_tm_stats_launch(w.raw, B, Fu, T, 0, w.sums, st))) return rc;
   if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)Fu * T, 1.f, w.inv1, nullptr, st, IMP_EPS))) return rc;
   const size_t nfb = (size_t)T * B * Fu;
   if ((rc = scale_rows_launch(w.raw, w.inv1, nfb, Fu, B, 1, w.xfb, st))) return rc;
@@ -192,8 +198,7 @@ extern "C" int fsn_improved_train_forward(const fsn_improved_desc* d, const fsn_
     const ImpSecSave& q = w.sec[s];
     const int R = B * g.N;
     const fsn_seq_weights& sw = wt->sb[s];
-    imp_section_input_kernel<<<B * T, 256, 0, st>>>(w.raw, w.yfb, B, T, Fu, g, q.Xn, w.fs, true);
-    FSN_CHECK_LAUNCH("imp_section_input_kernel");
+    if ((rc = imp_section_input_launch(w.raw, w.yfb, B, T, Fu, g, q.Xn, w.fs, true, st))) return rc;
     if ((rc = clip_reduce_only_launch(w.fs, B, T, w.sums, st))) return rc;
     if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)g.N * g.W * T, 1.f, q.invs, nullptr, st, IMP_EPS))) return rc;
     const size_t nx = (size_t)T * R * g.W;
@@ -245,12 +250,10 @@ extern "C" int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn
     if ((rc = linear_bwd(w.dY, q.L[1].H, sw.fc_w, T * R, O, Hs, sgr.fc_w, sgr.fc_b, w.dH, w.splitk, w.colsum, st))) return rc;
     // BPTT down to the normalised section input
     if ((rc = stack_bwd(Ls, 2, T, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, w.dX, st))) return rc;
-    train_dot_kernel<<<B, 256, 0, st>>>(w.dX, q.Xn, T, R, sg.N, sg.W, w.dot);
-    FSN_CHECK_LAUNCH("train_dot_kernel");
-    imp_unfold_bwd_kernel<<<ew_grid((size_t)T * B * Fu), 256, 0, st>>>(
-        w.dX, q.invs, w.dot, (float)sg.N * sg.W * T, sg, B, T, Fu, s == 0, s == m.S - 1 ? d->fb_activation : FSN_ACT_NONE,
-        w.yfb, w.dfb);
-    FSN_CHECK_LAUNCH("imp_unfold_bwd_kernel");
+    if ((rc = train_dot_launch(w.dX, q.Xn, T, R, sg.N, sg.W, B, w.dot, st))) return rc;
+    if ((rc = imp_unfold_bwd_launch(w.dX, q.invs, w.dot, (float)sg.N * sg.W * T, sg, B, T, Fu, s == 0,
+                                    s == m.S - 1 ? d->fb_activation : FSN_ACT_NONE, w.yfb, w.dfb, st)))
+      return rc;
     if ((rc = layer_weight_grads(Ls[1], T, q.L[0].H, sgr.w_ih[1], sgr.w_hh[1], sgr.b_ih[1], sgr.b_hh[1], wg, st))) return rc;
     if ((rc = layer_weight_grads(Ls[0], T, q.Xn, sgr.w_ih[0], sgr.w_hh[0], sgr.b_ih[0], sgr.b_hh[0], wg, st))) return rc;
   }
@@ -267,4 +270,26 @@ extern "C" int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn
   if ((rc = stack_bwd(Lf, 2, T, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st))) return rc;
   if ((rc = layer_weight_grads(Lf[1], T, w.fb[0].H, fg.w_ih[1], fg.w_hh[1], fg.b_ih[1], fg.b_hh[1], wg, st))) return rc;
   return layer_weight_grads(Lf[0], T, w.xfb, fg.w_ih[0], fg.w_hh[0], fg.b_ih[0], fg.b_hh[0], wg, st);
+}
+
+// ---- unit-test hook of one section's norm + unfold backward (include/fsn_b200.h): the launchers
+// fsn_improved_train_backward runs per section, every argument checked before any CUDA call
+extern "C" int fsn_debug_imp_unfold_bwd(const float* dX, const float* Xn, const float* invs, const float* y, int B, int T,
+                                        int Fu, int lo, int hi, int cs, int ns, int cf, int nf, int first, int act,
+                                        float* dot, float* dfb, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(dX && Xn && invs && dot && dfb && (act == FSN_ACT_NONE || y), FSN_ERR_SHAPE,
+              "improved unfold backward hook: null argument");
+  FSN_REQUIRE(B > 0 && T > 0 && Fu >= 2 && hi <= Fu, FSN_ERR_SHAPE, "improved unfold backward hook: bad shape B=%d T=%d Fu=%d",
+              B, T, Fu);
+  FSN_REQUIRE(act == FSN_ACT_NONE || act == FSN_ACT_RELU, FSN_ERR_UNSUPPORTED,
+              "improved unfold backward hook: act none or ReLU are built");
+  SecGeom g;
+  int rc = sec_geom(lo, hi, cs, ns, cf, nf, Fu, g);
+  if (rc) return rc;
+  FSN_REQUIRE((size_t)T * B * g.N * g.W < ((size_t)1 << 31) && (size_t)T * B * Fu < ((size_t)1 << 31), FSN_ERR_SHAPE,
+              "improved unfold backward hook: tensors must stay below 2^31 elements");
+  const cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = train_dot_launch(dX, Xn, T, B * g.N, g.N, g.W, B, dot, st))) return rc;
+  return imp_unfold_bwd_launch(dX, invs, dot, (float)g.N * g.W * T, g, B, T, Fu, first != 0, act, y, dfb, st);
 }

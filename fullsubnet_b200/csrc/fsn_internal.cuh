@@ -213,11 +213,24 @@ int linear_bwd(const float* dY, const float* X, const float* W, int rows, int N,
                float* splitk, float* colsum, cudaStream_t st);
 // out [cols, rows] = in [rows, cols]^T
 int transpose_launch(const float* in, size_t rows, int cols, float* out, cudaStream_t st);
-// per-clip (sum, sum_f c_N[f] * row sum) of a time-major x [Tp,B,F], one CTA per clip
-__global__ void train_tm_stats_kernel(const float* __restrict__ x, int B, int F, int Tp, int N, float2* __restrict__ sums);
-// dot[b'] = sum over the rows [b'*Fsub, (b'+1)*Fsub) of every step of dX * X  (laplace-norm backward), one CTA per clip
-__global__ void train_dot_kernel(const float* __restrict__ dX, const float* __restrict__ X, int Tp, int R, int Fsub, int K,
-                                 float* __restrict__ dot);
+// per-clip (sum, sum_f c_N[f] * row sum) of a time-major x [Tp,B,F] (train_tm_stats) or of mag [B,F,T]
+// (train_mag_stats), one CTA per clip, fixed-order tree
+int train_tm_stats_launch(const float* x, int B, int F, int Tp, int N, float2* sums, cudaStream_t st);
+int train_mag_stats_launch(const float* mag, int B, int F, int T, int Ns, float2* sums, cudaStream_t st);
+// dot[b'] = sum over the rows [b'*Fsub, (b'+1)*Fsub) of every step of dX * X [Tp,R,K]  (laplace-norm backward), one CTA
+// per clip b' < clips
+int train_dot_launch(const float* dX, const float* X, int Tp, int R, int Fsub, int K, int clips, float* dot, cudaStream_t st);
+// backward of fullsubnet's second offline norm + drop_band with respect to the full-band output (Nf = 0, its column K-1
+// of the sub-band input X [Tp,R,K]): dz [Tp,B,F] = act'(fbz) * (dX[t, row(b,f), K-1] inv2[b] - inv2[b] dot[b'] / cnt2),
+// one grid-stride kernel; units drop_band removed keep the norm-mean term
+int train_dfbz_launch(const float* dX, const float* fbz, const float* inv2, const float* dot, RowMap map, int Tp, int R, int K,
+                      float cnt2, int act, float* dz, cudaStream_t st);
+// the same for the second cumulative norm (scaleT [Tp,R]): dunit [Tp,R] = gradient of the full-band column of every unit
+// (one thread per row, suffix sum over t), then dz = act'(fbz) * dunit of the unit's row (0 where drop_band removed it)
+int train_cum_unit_bwd_launch(const float* dX, const float* X, const float* scaleT, int Tp, int R, int K, float* dunit,
+                              cudaStream_t st);
+int train_dfbz_cum_launch(const float* dunit, const float* fbz, RowMap map, int Tp, int R, int act, float* dz,
+                          cudaStream_t st);
 
 // shapes of one fast_fullsubnet Model.forward call (fsn_fast_model.cu): Ts = shrunk steps of the bottleneck; cum: the
 // descriptor asks for the cumulative norm
@@ -239,6 +252,17 @@ __device__ __forceinline__ void shrink_block(int ts, int S, int Tp, int& t0, int
 // .y alike, the layout clip_reduce_only_launch reads)
 int fast_bn_input_launch(const float* melT, const float* encT, size_t bs, size_t ts, int B, int Tp, int M, int Nn, int Ne,
                          int S, int Ts, float* bn, float2* fs, cudaStream_t st);
+// fast_fullsubnet backward (fsn_fast_train.cu).  ftr_dbn: d bn_out [Ts, B*M] = ReLU'(bn_out) * sum of the up-sampled
+// half (columns M..2M-1) of d dec_in [Tp,B,2M] over the frames that read each shrunk step.  ftr_cum_suffix (cumulative
+// norm): suffix [Ts, B*M] of the second norm's backward from dX, X [Ts, B*M, K] and scaleT [Ts, B*M].  ftr_denc: d encT
+// [Tp,B,M] through the second norm, down-sampling and unfold (offline: inv2 [B], dot [B], cnt2 = M K Ts; cum: scaleT,
+// suffix) plus the decoder-input half ddec[., :M], times ReLU'(encT)
+int ftr_dbn_launch(const float* ddec, const float* bn_out, int B, int Tp, int M, int S, int Ts, float* dbn, cudaStream_t st);
+int ftr_cum_suffix_launch(const float* dX, const float* X, const float* scaleT, int Ts, int R, int K, float* suffix,
+                          cudaStream_t st);
+int ftr_denc_launch(bool cum, const float* ddec, const float* dX, const float* encT, const float* inv2, const float* dot,
+                    const float* scaleT, const float* suffix, int B, int Tp, int M, int Nn, int Ne, int S, float cnt2,
+                    float* denc, cudaStream_t st);
 // fast_fullsubnet decoder input (model.py:191-194): dec_in row (b,t) = [encoder output (M) | up-sampled bottleneck output
 // (M)].  Row (b,t) of encT [., M] and dec_in [., 2M] is b*rbs + t*rts (clip-major: Tp, 1; time-major: 1, B); frame t reads
 // shrunk step min(t/S, Ts-1) of bn_out, element (b, m, ts) at b*nbs + m*nms + ts*nts
@@ -352,8 +376,18 @@ struct SecGeom { int lo, N, cs, ns, cf, nf, W; };  // section rows [lo, lo + N*c
 struct ImpDims { int B, L, T, F, Fu, S; SecGeom sec[FSN_IMP_MAX_SECTIONS]; int maxRW, maxR; };
 int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m);
 __global__ void imp_compress_kernel(const float* __restrict__ mag, float* __restrict__ out, int F, int T, float fdrc, bool tm);
-__global__ void imp_section_input_kernel(const float* __restrict__ magc, const float* __restrict__ fbT, int B, int T,
-                                         int Fu, SecGeom g, float* __restrict__ X, float2* __restrict__ fs, bool tm);
+// section input (model.py:321-443): X [T, B*N, W] of the reflected noisy rows of magc and full-band rows of fbT ([B,T,Fu],
+// or [T,B,Fu] when tm), and fs[b*T + t] = the sum of the (b, t) block (.x and .y alike), one CTA per (b, t)
+int imp_section_input_launch(const float* magc, const float* fbT, int B, int T, int Fu, const SecGeom& g, float* X, float2* fs,
+                             bool tm, cudaStream_t st);
+// section rows [lo, hi) of Fu with sub-band / full-band centre widths cs / cf and neighbours ns / nf -> g, with the checks
+// of imp_dims (FSN_ERR_SHAPE / FSN_ERR_UNSUPPORTED)
+int sec_geom(int lo, int hi, int cs, int ns, int cf, int nf, int Fu, SecGeom& g);
+// backward of section g's norm and full-band unfold (fsn_improved_train.cu): dfb [T,B,Fu] = (first ? 0 : dfb) + the
+// gradient through the section input dX [T, B*N, W] with inv_s = invs [B], dot [B] (train_dot_launch), cnt = N W T;
+// then act' of the kept full-band output y (FSN_ACT_NONE / FSN_ACT_RELU)
+int imp_unfold_bwd_launch(const float* dX, const float* invs, const float* dot, float cnt, const SecGeom& g, int B, int T,
+                          int Fu, bool first, int act, const float* y, float* dfb, cudaStream_t st);
 // where section g's Linear(H -> 2c) writes in the cRM [B,2,F,T]
 inline HeadGeom imp_head_geom(const SecGeom& g, int F, int T) { return HeadGeom{g.N, g.cs, g.lo, F, (size_t)T}; }
 

@@ -544,9 +544,7 @@ int clip_stats_launch(const float* x, int B, int T_pad, int F, int N, float2* fs
                       const int* lens, int hop, int la) {
   int rc;
   if ((rc = frame_stats_launch(x, B, T_pad, F, N, (size_t)T_pad * F, F, fs, st))) return rc;
-  clip_reduce_kernel<<<B, 256, 0, st>>>(fs, T_pad, sums, lens, hop, la);
-  FSN_CHECK_LAUNCH("clip_reduce_kernel");
-  return FSN_OK;
+  return clip_reduce_only_launch(fs, B, T_pad, sums, st, lens, hop, la);
 }
 
 int clip_reduce_only_launch(const float2* fs, int B, int T_pad, float2* sums, cudaStream_t st, const int* lens, int hop,
@@ -564,3 +562,38 @@ int norm_scales_launch(const float2* mag_sums, const float2* fb_sums, int B, flo
 }
 
 }  // namespace fsn
+
+using namespace fsn;
+
+// ---- unit-test hook of the frame / clip statistics and the offline-norm scales (include/fsn_b200.h): the launchers the
+// inference forwards run, every argument checked before any CUDA call; host lengths go to lens_dev through wav_prologue
+extern "C" int fsn_debug_norm_stats(const float* x, int B, int T_pad, int F, int N, int64_t bs, int64_t ts,
+                                    const int32_t* lengths, int* lens_dev, int hop, int la, const float* fb_sums, float cnt1,
+                                    float cnt2, float eps, float* fs, float* sums, float* inv1, float* inv2,
+                                    fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(x && fs && sums, FSN_ERR_SHAPE, "norm stats hook: null argument");
+  FSN_REQUIRE(B > 0 && T_pad > 0 && F > 0 && bs >= 0 && ts >= 0, FSN_ERR_SHAPE,
+              "norm stats hook: bad shape B=%d T_pad=%d F=%d", B, T_pad, F);
+  FSN_REQUIRE(N >= 0 && N < F, FSN_ERR_SHAPE, "norm stats hook: reflect padding needs 0 <= N < F");
+  FSN_REQUIRE((size_t)B * T_pad < ((size_t)1 << 31), FSN_ERR_SHAPE, "norm stats hook: B*T_pad must stay below 2^31");
+  FSN_REQUIRE(!inv1 || cnt1 > 0.f, FSN_ERR_SHAPE, "norm stats hook: cnt1 must be positive");
+  FSN_REQUIRE(!inv2 || cnt2 > 0.f, FSN_ERR_SHAPE, "norm stats hook: cnt2 must be positive");
+  if (lengths) {
+    FSN_REQUIRE(lens_dev && hop > 0 && la >= 0, FSN_ERR_SHAPE, "norm stats hook: lengths need lens_dev, hop > 0, la >= 0");
+    for (int b = 0; b < B; ++b)
+      FSN_REQUIRE(lengths[b] >= 0 && 1 + lengths[b] / hop + la <= T_pad, FSN_ERR_SHAPE,
+                  "norm stats hook: clip %d has more than T_pad frames", b);
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  WavWs w = {nullptr, nullptr, nullptr, nullptr, lens_dev};
+  int rc = wav_prologue(lengths, B, w, st);
+  if (rc) return rc;
+  float2* fs2 = reinterpret_cast<float2*>(fs);
+  float2* sums2 = reinterpret_cast<float2*>(sums);
+  if ((rc = frame_stats_launch(x, B, T_pad, F, N, (size_t)bs, (size_t)ts, fs2, st))) return rc;
+  if ((rc = clip_reduce_only_launch(fs2, B, T_pad, sums2, st, w.lens, hop, la))) return rc;
+  if (!inv1 && !inv2) return FSN_OK;
+  return norm_scales_launch(sums2, fb_sums ? reinterpret_cast<const float2*>(fb_sums) : sums2, B, cnt1, cnt2, inv1, inv2,
+                            st, eps, w.lens, hop, la);
+}

@@ -244,6 +244,18 @@ __global__ void train_tm_stats_kernel(const float* __restrict__ x, int B, int F,
   if (threadIdx.x == 0) sums[b] = sh[0];
 }
 
+int train_mag_stats_launch(const float* mag, int B, int F, int T, int Ns, float2* sums, cudaStream_t st) {
+  train_mag_stats_kernel<<<B, 256, 0, st>>>(mag, F, T, Ns, sums);
+  FSN_CHECK_LAUNCH("train_mag_stats_kernel");
+  return FSN_OK;
+}
+
+int train_tm_stats_launch(const float* x, int B, int F, int Tp, int N, float2* sums, cudaStream_t st) {
+  train_tm_stats_kernel<<<B, 256, 0, st>>>(x, B, F, Tp, N, sums);
+  FSN_CHECK_LAUNCH("train_tm_stats_kernel");
+  return FSN_OK;
+}
+
 // sub-band input X[t,r,k] (base_model.py:13-46 + model.py:98-119): unit (b,f) of row r, scaled by inv2[b]
 __global__ void train_gather_kernel(const float* __restrict__ raw, const float* __restrict__ fbz,
                                     const float* __restrict__ inv2, const float* __restrict__ unit_scale,
@@ -294,6 +306,20 @@ __global__ void train_dfbz_cum_kernel(const float* __restrict__ dunit, const flo
     const int r = unit_to_row(map, b, f);
     dz[i] = act_grad(r >= 0 ? dunit[(size_t)t * R + r] : 0.f, fbz, i, act);
   }
+}
+
+int train_cum_unit_bwd_launch(const float* dX, const float* X, const float* scaleT, int Tp, int R, int K, float* dunit,
+                              cudaStream_t st) {
+  train_cum_unit_bwd_kernel<<<cdiv(R, 128), 128, 0, st>>>(dX, X, scaleT, Tp, R, K, dunit);
+  FSN_CHECK_LAUNCH("train_cum_unit_bwd_kernel");
+  return FSN_OK;
+}
+
+int train_dfbz_cum_launch(const float* dunit, const float* fbz, RowMap map, int Tp, int R, int act, float* dz,
+                          cudaStream_t st) {
+  train_dfbz_cum_kernel<<<132 * 8, 256, 0, st>>>(dunit, fbz, map, Tp, R, act, dz);
+  FSN_CHECK_LAUNCH("train_dfbz_cum_kernel");
+  return FSN_OK;
 }
 
 // LSTM cell of one step (tensor-core path): G_t [R,4H] holds x_t W_ih^T (all steps from one hoisted GEMM), rec the
@@ -425,6 +451,19 @@ __global__ void train_dfbz_kernel(const float* __restrict__ dX, const float* __r
     else if (act == FSN_ACT_RELU6) v = (y > 0.f && y < 6.f) ? v : 0.f;
     dz[i] = v;
   }
+}
+
+int train_dot_launch(const float* dX, const float* X, int Tp, int R, int Fsub, int K, int clips, float* dot, cudaStream_t st) {
+  train_dot_kernel<<<clips, 256, 0, st>>>(dX, X, Tp, R, Fsub, K, dot);
+  FSN_CHECK_LAUNCH("train_dot_kernel");
+  return FSN_OK;
+}
+
+int train_dfbz_launch(const float* dX, const float* fbz, const float* inv2, const float* dot, RowMap map, int Tp, int R, int K,
+                      float cnt2, int act, float* dz, cudaStream_t st) {
+  train_dfbz_kernel<<<132 * 8, 256, 0, st>>>(dX, fbz, inv2, dot, map, Tp, R, K, cnt2, act, dz);
+  FSN_CHECK_LAUNCH("train_dfbz_kernel");
+  return FSN_OK;
 }
 
 // ------------------------------------------------------------------------------------------ workspace
@@ -708,9 +747,8 @@ int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const 
 // ------------------------------------------------------------------------------------------ shared by the training steps
 int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, bool cum, float2* sums, float* inv1,
                        float* raw, float* scaled, float2* fs, float* cum1, cudaStream_t st) {
-  train_mag_stats_kernel<<<B, 256, 0, st>>>(noisy_mag, F, T, Ns, sums);
-  FSN_CHECK_LAUNCH("train_mag_stats_kernel");
   int rc;
+  if ((rc = train_mag_stats_launch(noisy_mag, B, F, T, Ns, sums, st))) return rc;
   if ((rc = norm_scales_launch(sums, sums, B, (float)F * Tp, 1.f, inv1, nullptr, st))) return rc;
   // raw [Tp,B,F] and scaled = raw * inv1[b]
   if ((rc = transpose_mag_launch(noisy_mag, B, F, T, Tp, F, (size_t)B * F, raw, inv1, scaled, st))) return rc;
@@ -781,8 +819,7 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   if ((rc = layer_forward(prec, seq_layer(*fb, 1), w.fb[0].H, B, Hf, Hf, Tp, w.fb[1], w.rec, w.splitk, &hf1, st))) return rc;
   if ((rc = fc_gemm_launch(w.fb[1].H, fb->fc_w, fb->fc_b, w.fbz, Tp * B, Hf, F, d->fb_activation, st))) return rc;
   // second norm in closed form (model.py:110-111)
-  train_tm_stats_kernel<<<B, 256, 0, st>>>(w.fbz, B, F, Tp, d->fb_num_neighbors, w.sums_fb);
-  FSN_CHECK_LAUNCH("train_tm_stats_kernel");
+  if ((rc = train_tm_stats_launch(w.fbz, B, F, Tp, d->fb_num_neighbors, w.sums_fb, st))) return rc;
   if ((rc = norm_scales_launch(w.sums_mag, w.sums_fb, B, 1.f, (float)F * m.Ksb * Tp, nullptr, w.inv2, st))) return rc;
   // sub-band units (unfold + concat + norm + drop_band as one gather), then the sub-band stack (model.py:98-128)
   RowMap map{B, F, m.Fsub, m.G};
@@ -884,16 +921,13 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   if ((rc = layer_weight_grads(sbL[0], Tp, w.xsb, gsb->w_ih[0], gsb->w_hh[0], gsb->b_ih[0], gsb->b_hh[0], wg, st))) return rc;
   // ---- second norm + drop_band + full-band Linear/activation
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
-    train_cum_unit_bwd_kernel<<<cdiv(R, 128), 128, 0, st2>>>(w.dxsb, w.xsb, w.cum2, Tp, R, K, w.dunit);
-    FSN_CHECK_LAUNCH("train_cum_unit_bwd_kernel");
-    train_dfbz_cum_kernel<<<132 * 8, 256, 0, st2>>>(w.dunit, w.fbz, map, Tp, R, d->fb_activation, w.dz);
-    FSN_CHECK_LAUNCH("train_dfbz_cum_kernel");
+    if ((rc = train_cum_unit_bwd_launch(w.dxsb, w.xsb, w.cum2, Tp, R, K, w.dunit, st2))) return rc;
+    if ((rc = train_dfbz_cum_launch(w.dunit, w.fbz, map, Tp, R, d->fb_activation, w.dz, st2))) return rc;
   } else {
-    train_dot_kernel<<<B, 256, 0, st2>>>(w.dxsb, w.xsb, Tp, R, m.Fsub, K, w.dot);
-    FSN_CHECK_LAUNCH("train_dot_kernel");
-    train_dfbz_kernel<<<132 * 8, 256, 0, st2>>>(w.dxsb, w.fbz, w.inv2, w.dot, map, Tp, R, K, (float)F * K * Tp,
-                                                d->fb_activation, w.dz);
-    FSN_CHECK_LAUNCH("train_dfbz_kernel");
+    if ((rc = train_dot_launch(w.dxsb, w.xsb, Tp, R, m.Fsub, K, B, w.dot, st2))) return rc;
+    if ((rc = train_dfbz_launch(w.dxsb, w.fbz, w.inv2, w.dot, map, Tp, R, K, (float)F * K * Tp, d->fb_activation, w.dz,
+                                st2)))
+      return rc;
   }
   if ((rc = linear_bwd(w.dz, w.fb[1].H, fb->fc_w, Tp * B, F, Hf, gfb->fc_w, gfb->fc_b, w.dfh1, w.splitk2, w.colsum2, st2)))
     return rc;
@@ -1280,4 +1314,43 @@ extern "C" int fsn_clip_adam(const fsn_param_list* L, float max_norm, float grad
   for (int i = 0; i < L->n; ++i) steps[i] = step;
   return fsn_clip_adam_steps(L, max_norm, grad_scale, lr, beta1, beta2, eps, steps, norm_out, scratch, scratch_bytes,
                              stream);
+}
+
+// ---- unit-test hook of the second norm + drop_band backward (include/fsn_b200.h): the launchers fsn_train_backward
+// runs, every argument checked before any CUDA call
+extern "C" int fsn_debug_norm_unfold_bwd(const float* dX, const float* X, const float* fbz, const float* scale, int cum,
+                                         int B, int F, int G, int Tp, int Ns, float cnt2, int act, float* mid, float* dz,
+                                         fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(dX && X && fbz && scale && mid && dz, FSN_ERR_SHAPE, "norm/unfold backward hook: null argument");
+  FSN_REQUIRE(B > 0 && F > 0 && Tp > 0 && G >= 0, FSN_ERR_SHAPE, "norm/unfold backward hook: bad shape B=%d F=%d Tp=%d G=%d",
+              B, F, Tp, G);
+  FSN_REQUIRE(G <= 1 || (B > G && F >= G), FSN_ERR_SHAPE, "norm/unfold backward hook: drop_band needs B > G and F >= G");
+  FSN_REQUIRE(Ns >= 0 && Ns < F, FSN_ERR_SHAPE, "norm/unfold backward hook: reflect padding needs 0 <= Ns < F");
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "norm/unfold backward hook: unknown act %d", act);
+  FSN_REQUIRE(cum || cnt2 > 0.f, FSN_ERR_SHAPE, "norm/unfold backward hook: cnt2 must be positive");
+  const int Fsub = G > 1 ? F / G : F, R = B * Fsub, K = 2 * Ns + 2;
+  FSN_REQUIRE((size_t)Tp * R * K < ((size_t)1 << 31) && (size_t)Tp * B * F < ((size_t)1 << 31), FSN_ERR_SHAPE,
+              "norm/unfold backward hook: tensors must stay below 2^31 elements");
+  const RowMap map{B, F, Fsub, G > 1 ? G : 1};
+  const cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (cum) {
+    if ((rc = train_cum_unit_bwd_launch(dX, X, scale, Tp, R, K, mid, st))) return rc;
+    return train_dfbz_cum_launch(mid, fbz, map, Tp, R, act, dz, st);
+  }
+  if ((rc = train_dot_launch(dX, X, Tp, R, Fsub, K, B, mid, st))) return rc;
+  return train_dfbz_launch(dX, fbz, scale, mid, map, Tp, R, K, cnt2, act, dz, st);
+}
+
+// ---- unit-test hook of the per-clip statistics of the training steps (include/fsn_b200.h)
+extern "C" int fsn_debug_train_stats(const float* x, int tm, int B, int F, int T, int N, float* sums, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(x && sums, FSN_ERR_SHAPE, "train stats hook: null argument");
+  FSN_REQUIRE(B > 0 && F > 0 && T > 0 && (size_t)B * F * T < ((size_t)1 << 31) && (size_t)F * T < ((size_t)1 << 31),
+              FSN_ERR_SHAPE, "train stats hook: bad shape B=%d F=%d T=%d", B, F, T);
+  FSN_REQUIRE(N >= 0 && N < F, FSN_ERR_SHAPE, "train stats hook: reflect padding needs 0 <= N < F");
+  float2* s = reinterpret_cast<float2*>(sums);
+  const cudaStream_t st = (cudaStream_t)stream;
+  return tm ? train_tm_stats_launch(x, B, F, T, N, s, st) : train_mag_stats_launch(x, B, F, T, N, s, st);
 }

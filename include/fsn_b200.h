@@ -627,6 +627,56 @@ int fsn_debug_wav_epilogue(const float* enhanced, const unsigned int* peak_bits,
                            int* lens_dev, float gain, int16_t* pcm, float* crm_out, int F, int T, int hop,
                            fsn_stream_t stream);
 
+/* unit-test hooks for the backward of the second norm and the frequency unfold of the training steps (fsn_train.cu,
+ * fsn_fast_train.cu, fsn_improved_train.cu): the launchers of the fsn_*_train_backward entry points on caller buffers.
+ * Tensors are time-major as in the training steps; act (FSN_ACT_*) is the activation of the kept output whose derivative
+ * is taken from that output.
+ *   fsn_debug_norm_unfold_bwd (fullsubnet, model.py:98-119): sub-band input X and its gradient dX [Tp, R, K], K = 2Ns+2
+ *     (the full-band unit in column K-1), R = B*Fsub rows of the drop_band map with G groups (G <= 1: none, Fsub = F;
+ *     else B > G, Fsub = F/G); full-band output fbz [Tp,B,F].  cum = 0: offline norm, scale = inv2 [B], mid = dot [B],
+ *     cnt2 = F K Tp in the step; cum != 0: cumulative norm, scale = scaleT [Tp,R], mid = dunit [Tp,R].  dz [Tp,B,F] is
+ *     the gradient at the full-band Linear's output (drop_band's removed units keep the offline norm-mean term).
+ *   fsn_debug_fast_norm_unfold_bwd (fast_fullsubnet, model.py:174-194): Ts = 1 + ceil((Tp-1)/S) shrunk steps,
+ *     K = (2Nn+1)+(2Ne+1), R = B*M.  dbn (nullable) [Ts,R] <- the up-sampling transpose of the columns M..2M-1 of ddec
+ *     [Tp,B,2M] times ReLU' of bn_out [Ts,R].  denc (nullable) [Tp,B,M] <- the gradient at the encoder output encT [Tp,B,M]
+ *     (post-ReLU) through the second norm, down-sampling and unfold of dX, X [Ts,R,K], plus ddec's columns < M; cum = 0:
+ *     scale = inv2 [B], mid = dot [B], cnt2 = M K Ts in the step; cum != 0: scale = scaleT [Ts,R], mid = suffix [Ts,R].
+ *   fsn_debug_imp_unfold_bwd (improved_fullsubnet, model.py:321-443): section rows [lo, hi) of Fu with centre widths cs
+ *     = cf and neighbours ns, nf (checked as the model descriptor's sections are), N = (hi-lo)/cs units of width
+ *     W = (cs+2ns)+(cf+2nf); dX, Xn [T, B*N, W], invs [B].  dot [B] <- <dX, Xn> per clip; dfb [T,B,Fu] <- (first ? 0 : dfb)
+ *     + the gradient at the full-band output through the section's norm and unfold, then ReLU' of y [T,B,Fu] when act is
+ *     FSN_ACT_RELU (the last section in the step).
+ *   fsn_debug_imp_section_input (improved_fullsubnet's forward, the same section): X [T, B*N, W] <- unit n of clip b at
+ *     frame t, the noisy rows lo+n*cs-ns .. of magc then the full-band rows lo+n*cf-nf .. of fbT, reflected at rows 0 and
+ *     Fu-1 (magc, fbT [B,T,Fu], or [T,B,Fu] when tm); fs [B*T] (float2) <- the sum of each (b, t) block in .x and .y.
+ * Arguments are checked before any CUDA call. */
+int fsn_debug_norm_unfold_bwd(const float* dX, const float* X, const float* fbz, const float* scale, int cum, int B, int F,
+                              int G, int Tp, int Ns, float cnt2, int act, float* mid, float* dz, fsn_stream_t stream);
+int fsn_debug_fast_norm_unfold_bwd(const float* ddec, const float* dX, const float* X, const float* encT,
+                                   const float* bn_out, const float* scale, int cum, int B, int Tp, int M, int Nn, int Ne,
+                                   int S, float cnt2, float* mid, float* denc, float* dbn, fsn_stream_t stream);
+int fsn_debug_imp_unfold_bwd(const float* dX, const float* Xn, const float* invs, const float* y, int B, int T, int Fu,
+                             int lo, int hi, int cs, int ns, int cf, int nf, int first, int act, float* dot, float* dfb,
+                             fsn_stream_t stream);
+int fsn_debug_imp_section_input(const float* magc, const float* fbT, int B, int T, int Fu, int lo, int hi, int cs, int ns,
+                                int cf, int nf, int tm, float* X, float* fs, fsn_stream_t stream);
+
+/* unit-test hooks for the statistics of the offline norms (fsn_lstm_simt.cu, fsn_train.cu; base_model.py:203-218 with
+ * the closed-form second-norm mean of model.py:98-111).  float2 outputs are pairs of floats.
+ *   fsn_debug_norm_stats: fs [B*T_pad] (float2) <- per frame (sum_f x, sum_f c_N[f] x) of x, element (b,t,f) at
+ *     b*bs + t*ts + f, c_N the reflect multiplicity of row f in the N-neighbour unfold; sums [B] (float2) <- the clip's
+ *     sums over its frames: all T_pad, or with lengths (nullable, host [B], copied to lens_dev) the first 1 +
+ *     lengths[b]/hop + la (<= T_pad), in the order and tree of a call on that clip alone with T_pad = its frames.
+ *     inv1 / inv2 (nullable, [B]) <- 1 / (sums.x / cnt1 + eps) and 1 / ((sums.y + fb_sums.y) / cnt2 + eps), fb_sums
+ *     (nullable, float2 [B] of another call; NULL: sums), the counts per frame times the clip's frames with lengths.
+ *   fsn_debug_train_stats: sums [B] (float2) <- (sum, sum c_N[f] x) of each clip of x [B,F,T] (tm = 0) or [T,B,F]
+ *     (tm != 0), one CTA per clip.
+ * Arguments are checked before any CUDA call. */
+int fsn_debug_norm_stats(const float* x, int B, int T_pad, int F, int N, int64_t bs, int64_t ts, const int32_t* lengths,
+                         int* lens_dev, int hop, int la, const float* fb_sums, float cnt1, float cnt2, float eps, float* fs,
+                         float* sums, float* inv1, float* inv2, fsn_stream_t stream);
+int fsn_debug_train_stats(const float* x, int tm, int B, int F, int T, int N, float* sums, fsn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
