@@ -162,6 +162,8 @@ _SIGNATURES = {
     "fsn_peak_normalize_int16": (C.c_int, [_P, _I, _I, _F, _P, _P]),
     "fsn_si_sdr": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "fsn_si_sdr_lengths": (C.c_int, [_P, _P, _P, _I, _I, _P, _P]),
+    "fsn_stoi_workspace_bytes": (_S, [_I, _I, _I]),
+    "fsn_stoi": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _S, _P]),
     "fsn_rir_convolve": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P]),
     "fsn_snr_mix": (C.c_int, [_P, _P, _P, _P, _F, _F, _I, _I, _P, _P, _P]),
     "fsn_debug_row_to_unit": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
@@ -195,6 +197,7 @@ _SIGNATURES = {
     "fsn_debug_imp_section_input": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "fsn_debug_norm_stats": (C.c_int, [_P, _I, _I, _I, _I, _L, _L, _P, _P, _I, _I, _P, _F, _F, _F, _P, _P, _P, _P, _P]),
     "fsn_debug_train_stats": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P]),
+    "fsn_debug_stoi_stages": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _S, _P]),
     "fsn_last_error_code": (C.c_int, []),
     "fsn_last_launch_count": (C.c_int64, []),
     "fsn_total_launch_count": (C.c_int64, []),

@@ -9,7 +9,9 @@ Same constructor arguments and config keys as the reference, so `train.py:65-80`
 (``meta.use_amp`` is accepted: the kernels compute in fp32 / tf32, at least the precision of the reference's fp16
 autocast, so the GradScaler is the identity and ``scaler`` stays an empty dict in the checkpoint schema
 {epoch, best_score, optimizer, scaler, model} of base_trainer.py:208-218).  TensorBoard, audio / spectrogram
-visualisation and the third-party CPU metrics STOI / PESQ (base_trainer.py:277-370) are outside the hot path.
+visualisation and PESQ (base_trainer.py:277-370) are outside the hot path.  STOI is computed on the device
+(``metrics.stoi``) for the noisy and the enhanced clip of every validation item when the recipe's
+``[trainer.visualization] metrics`` list names it, as base_trainer.py:316-370 does.
 
 Two gradient paths, both ONE all-reduce of gradients per step (SURVEY 8e):
   * ``model`` wrapped in DistributedDataParallel exactly like base_trainer.py:32 - the autograd Function behind
@@ -31,6 +33,7 @@ from .acoustics.mask import build_complex_ideal_ratio_mask
 from .dataset import mix_batch
 from .inferencer import Inferencer, plan_batches
 from .loss import MSELoss, cirm_mse_per_clip
+from .metrics import stoi
 from .optim import FusedClipAdam
 
 
@@ -100,6 +103,10 @@ class Trainer:
         self.validation_batch_size = self.validation_config.get("batch_size", 32)
         self.validation_max_padding = self.validation_config.get("max_padding", 0.25)
         plan_batches([], self.validation_batch_size, self.validation_max_padding)  # refuses bad values here
+        # the recipes' [trainer.visualization] metrics list: "STOI" there adds the STOI of noisy and enhanced speech
+        visualization = config["trainer"].get("visualization", {}) or {}
+        self.validation_stoi = "STOI" in (visualization.get("metrics") or ())
+        self.last_validation_stoi = None  # per-item (enhanced, noisy) STOI of the last validation, dataloader order
         self.only_validation = only_validation
         self.start_epoch = 1
         self.best_score = float("-inf") if self.save_max_metric_score else float("inf")
@@ -152,9 +159,11 @@ class Trainer:
     def _validation_items(self):
         """The validation dataloader's items (noisy [1,L], clean [1,L], name, speech_type) evaluated in groups
         (``validation_groups``): one fused enhance call per group (the model's mask + iSTFT, as
-        Inferencer.enhance_batch), then ``cirm_mse_per_clip`` and ``si_sdr`` over each clip's own length.  Returns
-        (loss float32 [N], SI-SDR float32 [N], speech types) in dataloader order, after ONE device-to-host copy.  Each
-        loss equals the reference's B=1 ``loss_function(cIRM, cRM)`` on that item alone (no drop_band), bit for bit."""
+        Inferencer.enhance_batch), then ``cirm_mse_per_clip`` and ``si_sdr`` over each clip's own length, and with
+        ``validation_stoi`` the STOI of the enhanced and of the noisy clip (``metrics.stoi``).  Returns (loss float32 [N],
+        SI-SDR float32 [N], speech types) in dataloader order, after ONE device-to-host copy; the STOI rows go to
+        ``last_validation_stoi`` ({"enhanced": [N], "noisy": [N]}, None without STOI).  Each loss equals the reference's
+        B=1 ``loss_function(cIRM, cRM)`` on that item alone (no drop_band), bit for bit."""
         if not isinstance(self.loss_function, (MSELoss, torch.nn.MSELoss)) or \
                 getattr(self.loss_function, "reduction", "mean") != "mean":
             raise NotImplementedError("fullsubnet_b200: validation computes the recipes' mean-squared cIRM loss only")
@@ -171,7 +180,9 @@ class Trainer:
         lens = [x.numel() for x in noisy_items]
         groups = validation_groups(inferencer, lens, self.validation_batch_size, self.validation_max_padding)
         order = [i for g in groups for i in g]
-        values = torch.empty(2, len(order), dtype=torch.float32, device=self.device)  # loss, SI-SDR in group order
+        rows = 4 if self.validation_stoi else 2
+        # loss, SI-SDR (, STOI enhanced, STOI noisy) in group order
+        values = torch.empty(rows, len(order), dtype=torch.float32, device=self.device)
         pos = 0
         for g in groups:
             g_lens = [lens[i] for i in g]
@@ -181,15 +192,20 @@ class Trainer:
             enhanced, crm = inferencer.enhance_batch(noisy, lengths=lengths, return_crm=True)
             values[0, pos:pos + len(g)] = cirm_mse_per_clip(noisy, clean, crm, n_fft, hop, win, lengths)
             values[1, pos:pos + len(g)] = si_sdr(clean, enhanced, lengths)
+            if self.validation_stoi:
+                values[2, pos:pos + len(g)] = stoi(clean, enhanced, lengths)
+                values[3, pos:pos + len(g)] = stoi(clean, noisy, lengths)
             pos += len(g)
-        per_item = np.empty((2, len(order)), dtype=np.float32)
+        per_item = np.empty((rows, len(order)), dtype=np.float32)
         per_item[:, order] = values.cpu().numpy()
+        self.last_validation_stoi = {"enhanced": per_item[2], "noisy": per_item[3]} if self.validation_stoi else None
         return per_item[0], per_item[1], item_types
 
     def _validation_epoch(self, epoch):
         """Loss and SI-SDR of every validation item (``_validation_items``), summed per speech type in float32 in
         dataloader order like the reference's B=1 loop.  Returns the mean SI-SDR of the "With_reverb" items (the
-        reference's score, trainer.py:181); per-type losses and scores stay in ``self.last_validation``."""
+        reference's score, trainer.py:181); per-type losses and scores stay in ``self.last_validation``, with the per-type
+        mean STOI of the noisy and the enhanced items under "stoi" when the recipe's visualization metrics name STOI."""
         types = ("With_reverb", "No_reverb")
         model = self.core
         was_training = model.training
@@ -212,6 +228,14 @@ class Trainer:
             "loss": {k: float(loss_list[k]) / n for k in types},  # divided by len(dataloader) like trainer.py:163-168
             "si_sdr": {k: (float(score_list[k]) / count[k] if count[k] else 0.0) for k in types},
             "items": dict(count)}
+        if self.validation_stoi:
+            st = self.last_validation_stoi
+            sums = {k: {"noisy": zero, "enhanced": zero} for k in types}
+            for i, speech_type in enumerate(item_types):
+                sums[speech_type]["noisy"] += st["noisy"][i]
+                sums[speech_type]["enhanced"] += st["enhanced"][i]
+            self.last_validation["stoi"] = {
+                k: {w: (float(sums[k][w]) / count[k] if count[k] else 0.0) for w in ("noisy", "enhanced")} for k in types}
         return self.last_validation["si_sdr"]["With_reverb"]
 
     def _is_best_epoch(self, score, save_max_metric_score=True):

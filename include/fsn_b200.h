@@ -63,8 +63,8 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
 /* ABI version: 101 changed fsn_enhance's argument list; 102 appended norm_type to fsn_fast_desc, so that struct grew.
  * The version counts changes that break an existing caller.  Entry points added since 102 leave every earlier argument
  * list and struct as it was, so the version stays 102; a caller finds them by symbol: fsn_cirm_mse_per_clip (+ its
- * workspace query), fsn_si_sdr_lengths (the grouped validation loss and SI-SDR) and fsn_clip_adam_steps (one Adam step
- * count per tensor). */
+ * workspace query), fsn_si_sdr_lengths (the grouped validation loss and SI-SDR), fsn_clip_adam_steps (one Adam step
+ * count per tensor) and fsn_stoi (+ its workspace query and the fsn_debug_stoi_stages hook). */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -475,7 +475,7 @@ int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn_improved_w
 int fsn_peak_normalize_int16(const float* wav, int B, int L, float gain, int16_t* out, fsn_stream_t stream);
 
 /* audio_zen/metrics.py:6-31  SI_SDR(reference, estimation) (SURVEY 8f rank 4: the validation metric of
- * fullsubnet/trainer.py:78-181 that is pure arithmetic; STOI / PESQ are third-party CPU packages and stay out).
+ * fullsubnet/trainer.py:78-181; STOI is fsn_stoi below, PESQ (ITU-T P.862) stays out).
  * reference, estimation [B,L] -> out[B] in dB; fixed-order reductions. */
 int fsn_si_sdr(const float* reference, const float* estimation, int B, int L, float* out, fsn_stream_t stream);
 /* fsn_si_sdr over the first lengths[b] samples of each row of [B,L_max] (lengths: host int32 [B], 0 < lengths[b] <=
@@ -483,6 +483,25 @@ int fsn_si_sdr(const float* reference, const float* estimation, int B, int L, fl
  * An addition at version 102 (see fsn_version). */
 int fsn_si_sdr_lengths(const float* reference, const float* estimation, const int32_t* lengths, int B, int L_max,
                        float* out, fsn_stream_t stream);
+
+/* audio_zen/metrics.py:STOI  pystoi 0.3.3 stoi(clean, estimate, sr, extended=False) (Taal et al., 2011) per clip:
+ * resampling to 10 kHz (Octave-style Kaiser-windowed sinc, scipy resample_poly), silent-frame removal at 40 dB below the
+ * clean clip's loudest 256-sample frame, 512-point spectra of the rebuilt signals, 15 one-third-octave bands from 150 Hz,
+ * clipped (-15 dB) and normalised correlations over 30-frame segments.  Fewer than 30 frames after the removal give
+ * 1e-5, as pystoi returns.  Computed in float64 from the widened inputs; out[b] float32.
+ *   clean, estimate [B,L_max]; out [B]; sr 16000 or 10000 (other rates FSN_ERR_UNSUPPORTED).
+ *   lengths (nullable, host int32 [B], read during the call through kernel parameters, not kept): clip b is the first
+ *     lengths[b] samples of its rows, samples from there on are never read; NULL = every clip L_max.  Each clip needs one
+ *     frame: at least 410 samples at 16 kHz, 257 at 10 kHz (shorter: FSN_ERR_SHAPE naming the clip).
+ *   out[b] is bit-identical to the call on clip b alone with L_max = lengths[b], whatever B and the clip's position
+ *   (one CTA per clip for every reduction, fixed orders, the kept frames compacted by a per-clip scan), and two calls
+ *   give the same bits.  Never allocates or synchronises; every argument (B > 0, pointers, lengths, workspace size:
+ *   FSN_ERR_WORKSPACE) is checked before any CUDA call.
+ * fsn_stoi_workspace_bytes: the workspace of any call with these B, L_max and sr (~32 * B * L_max * 10000/sr bytes); 0
+ * with fsn_last_error set on bad arguments; needs no GPU.  An addition at version 102 (see fsn_version). */
+size_t fsn_stoi_workspace_bytes(int B, int L_max, int sr);
+int fsn_stoi(const float* clean, const float* estimate, const int32_t* lengths, int B, int L_max, int sr, float* out,
+             void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 /* recipes/dns_interspeech_2020/dataset_train.py:136-199  Dataset.snr_mix for a batch (SURVEY 8f rank 4): the random
  * draws (snr, noisy target dBFS, which RIR) are made by the caller and passed in.
@@ -676,6 +695,17 @@ int fsn_debug_norm_stats(const float* x, int B, int T_pad, int F, int N, int64_t
                          int* lens_dev, int hop, int la, const float* fb_sums, float cnt1, float cnt2, float eps, float* fs,
                          float* sums, float* inv1, float* inv2, fsn_stream_t stream);
 int fsn_debug_train_stats(const float* x, int tm, int B, int F, int T, int N, float* sums, fsn_stream_t stream);
+
+/* unit-test hook of fsn_stoi (fsn_stoi.cu): the same kernels, with the intermediate buffers the caller's.  With Lr_max =
+ * ceil(L_max * 10000 / sr) samples at 10 kHz and nf_max = its frames (len(range(0, Lr_max - 256, 128))):
+ *   resampled [2,B,Lr_max] (float64; clean then estimate, zero past each clip's own resampled length);
+ *   keep [B,nf_max] (1 = the frame survives silent-frame removal, for the clip's own frames), n_kept [B];
+ *   compacted [2,B,Lr_max] (float64; the overlap-added kept frames, (n_kept + 1) * 128 samples, zero after);
+ *   bands [2,B,15,nf_max] (float64; the band magnitudes of the clip's n_kept - 1 frames of the compacted signals);
+ *   out [B] as fsn_stoi.  Workspace: fsn_stoi_workspace_bytes.  Arguments are checked as fsn_stoi checks them. */
+int fsn_debug_stoi_stages(const float* clean, const float* estimate, const int32_t* lengths, int B, int L_max, int sr,
+                          double* resampled, int32_t* keep, int32_t* n_kept, double* compacted, double* bands, float* out,
+                          void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 #ifdef __cplusplus
 }
