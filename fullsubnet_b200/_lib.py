@@ -197,6 +197,8 @@ _SIGNATURES = {
     "fsn_debug_imp_section_input": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "fsn_debug_norm_stats": (C.c_int, [_P, _I, _I, _I, _I, _L, _L, _P, _P, _I, _I, _P, _F, _F, _F, _P, _P, _P, _P, _P]),
     "fsn_debug_train_stats": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P]),
+    "fsn_debug_forgetting_scale": (C.c_int, [_P, _I, _P, _I, _I, _I, _I, _L, _L, _F, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
+    "fsn_debug_forgetting_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "fsn_debug_stoi_stages": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _S, _P]),
     "fsn_last_error_code": (C.c_int, []),
     "fsn_last_launch_count": (C.c_int64, []),

@@ -21,8 +21,10 @@ static int fbb_check(const fsn_fullband_desc* d, int B, int T) {
   FSN_REQUIRE(d->num_layers >= 1 && d->num_layers <= SEQ_MAX_LAYERS, FSN_ERR_UNSUPPORTED, "fullband: 1..8 LSTM layers");
   FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "fullband: the GRU cell is not built");
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "fullband: empty input (B=%d, T=%d)", B, T);
-  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE,
-              FSN_ERR_UNSUPPORTED, "You must set up a type of Norm. (offline_laplace_norm / cumulative_laplace_norm are built)");
+  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE ||
+                  d->norm_type == FSN_NORM_FORGETTING,
+              FSN_ERR_UNSUPPORTED,
+              "You must set up a type of Norm. (offline_laplace_norm / cumulative_laplace_norm / forgetting_norm are built)");
   // the tensor-core stack misses the reference gates on this model (DESIGN 4.9): f16x3_tc 1.8e-4 waveform max-abs on
   // the clipping weight set, f16_tc 1.6e-3 relative cRM
   FSN_REQUIRE(d->precision != FSN_PREC_F16X3_TC && d->precision != FSN_PREC_F16_TC, FSN_ERR_UNSUPPORTED,
@@ -37,7 +39,7 @@ static SeqStack fbb_stack(const fsn_fullband_desc* d, int B, int T) {
   memset(&s, 0, sizeof(s));
   s.R = B; s.Tp = T + d->look_ahead; s.K0 = d->num_freqs; s.n = d->num_layers; s.O = 2 * d->num_freqs; s.act = d->activation;
   for (int l = 0; l < s.n; ++l) s.H[l] = d->hidden;
-  s.step_scale = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
+  s.step_scale = norm_per_step(d->norm_type);
   return s;
 }
 
@@ -58,20 +60,21 @@ static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbW
 
 // everything after the time-major, look-ahead-padded magnitude w.magT exists: norm -> stack -> out [B,2,F,T].  lens
 // (nullable, device [B] samples): the offline norm of clip b covers only its own Tp_b = 1 + lens[b]/hop + look_ahead
-// frames; the cumulative norm and the stack are causal and run over all Tp steps.
+// frames; the cumulative and forgetting norms and the stack are causal and run over all Tp steps.
 static int fbb_core(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w, const float* fc_b, int B,
                     int T, const FbbWs& w, float* out, cudaStream_t st, const int* lens = nullptr, int hop = 0) {
   int rc;
   const int F = d->num_freqs, Tp = T + d->look_ahead, la = d->look_ahead;
-  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
+  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, fgt = d->norm_type == FSN_NORM_FORGETTING;
   if ((rc = clip_stats_launch(w.magT, B, Tp, F, 0, w.fs, w.sums, st, lens, hop, la))) return rc;
   if ((rc = norm_scales_launch(w.sums, w.sums, B, lens ? (float)F : (float)F * Tp, 1.f, w.inv1, nullptr, st, 1e-5f, lens,
                                hop, la)))
     return rc;
   if (cum && (rc = cum_clip_scale_launch(w.fs, B, Tp, F, 1.1920928955078125e-07f, w.cum1, st))) return rc;
+  if (fgt && (rc = forget_scale_launch(w.fs, nullptr, B, Tp, (float)F, w.cum1, nullptr, st))) return rc;
   SeqStack s = fbb_stack(d, B, T);
   for (int l = 0; l < s.n; ++l) s.L[l] = layers[l];
-  s.x = w.magT; s.scale = cum ? w.cum1 : w.inv1; s.fc_w = fc_w; s.fc_b = fc_b; s.out = w.y;
+  s.x = w.magT; s.scale = (cum || fgt) ? w.cum1 : w.inv1; s.fc_w = fc_w; s.fc_b = fc_b; s.out = w.y;
   if ((rc = seq_stack_forward(s, w.seq, st))) return rc;
   return crm_output_launch(w.y, (size_t)Tp * 2 * F, 2 * F, B, Tp, F, la, out, st);
 }

@@ -35,7 +35,7 @@ static void carve_fbb_train(const fsn_fullband_desc* d, int B, int T, void* base
   w.inv1 = c.take<float>(B);
   w.sums = c.take<float2>(B);
   w.fs = nullptr; w.cum1 = nullptr;
-  if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
+  if (norm_per_step(d->norm_type)) {
     w.fs = c.take<float2>(rows);
     w.cum1 = c.take<float>(rows);
   }
@@ -75,7 +75,9 @@ static int fbb_train_check(const fsn_fullband_desc* d, int B, int T) {
   FSN_REQUIRE(d->precision == FSN_PREC_FP32 || d->precision == FSN_PREC_TF32_TC, FSN_ERR_UNSUPPORTED,
               "fullband training: precision must be fp32 or tf32_tc");
   FSN_REQUIRE(d->num_layers >= 1 && d->num_layers <= FBB_MAX_LAYERS, FSN_ERR_UNSUPPORTED, "fullband training: 1..8 LSTM layers");
-  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, FSN_ERR_UNSUPPORTED,
+  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE ||
+                  d->norm_type == FSN_NORM_FORGETTING,
+              FSN_ERR_UNSUPPORTED,
               "fullband training: offline_laplace_norm and cumulative_laplace_norm are built");
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "fullband training: empty input (B=%d, T=%d)", B, T);
   return FSN_OK;
@@ -106,7 +108,7 @@ extern "C" int fsn_fullband_train_forward(const fsn_fullband_desc* d, const fsn_
   cudaStream_t st = (cudaStream_t)stream;
   const int F = d->num_freqs, H = d->hidden, Tp = T + d->look_ahead, NL = d->num_layers;
   // look-ahead pad, norm and the time-major copies (model.py:50-56)
-  if ((rc = train_input_launch(noisy_mag, B, F, T, Tp, 0, d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, w.sums, w.inv1, w.raw,
+  if ((rc = train_input_launch(noisy_mag, B, F, T, Tp, 0, d->norm_type, w.sums, w.inv1, w.raw,
                                w.xfb, w.fs, w.cum1, st)))
     return rc;
   // num_layers x LSTM (model.py:57); on tf32_tc layer l's fp16 hidden states are layer l+1's fp16 input

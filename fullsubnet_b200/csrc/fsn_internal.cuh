@@ -99,6 +99,26 @@ int lstm_step2_launch(StepParams p, int mode, int t, const fsn_lstm_layer& w1, c
 int cum_clip_scale_launch(const float2* fs, int B, int Tp, int F, float eps, float* scale1T, cudaStream_t st);
 int cum_unit_scale_launch(const float* magT, const float* fbT, RowMap map, int R, int Tp, int Ns, int Nf, float eps,
                           float* scaleT, cudaStream_t st, bool time_major = false);
+// forgetting_norm (base_model.py:102-151): mu_t = a_t mu_{t-1} + b_t m_t per clip, m_t the mean of frame t over the
+// features, scale 1 / (mu_t + 1e-10).  The coefficients are rounded as the reference rounds them: for t < 192,
+// a_t = float32(min((t-1)/(t+1), alpha)) and b_t = 1 - a_t in float32 (a_0 = -1, b_0 = 2; a_1 = 0); from t = 192 on,
+// a = float32(alpha) and b = float32(1 - alpha) rounded from the double.  Entry min(t, 192) holds frame t's pair.
+static const int FORGET_LEN = 192;
+static const float FORGET_EPS = 1e-10f;
+struct ForgetCoef { float a[FORGET_LEN + 1], b[FORGET_LEN + 1]; };
+ForgetCoef forget_coef();
+// the norms whose first-norm scale is per (step, clip) rather than per clip
+inline bool norm_per_step(int norm_type) { return norm_type != FSN_NORM_OFFLINE_LAPLACE; }
+// scaleT[t*B + b] = 1 / (mu_t + 1e-10) and muT[t*B + b] = mu_t (nullable) of clip b, one thread per clip in the exact
+// float32 operation order of the reference (no contraction).  fs2 == nullptr: m_t = fs[b*Tp + t].x / cnt (first norm:
+// the plain frame sum); else m_t = (fs[.].y + fs2[.].y) / cnt (second norm: the reflect-weighted sums of the noisy and
+// full-band unfolds, cnt = F K).  lens (nullable, device [B] samples): clip b scans only its own Tp_b = 1 + lens[b]/hop
+// + la frames and leaves the rest of its entries unwritten; those frames equal the unbounded scan's (it is causal).
+int forget_scale_launch(const float2* fs, const float2* fs2, int B, int Tp, float cnt, float* scaleT, float* muT,
+                        cudaStream_t st, const int* lens = nullptr, int hop = 0, int la = 0);
+// unit_scale[t*R + r] = scaleT[t*B + clip(r)]: the per-(step, clip) table in the per-(step, row) layout the sub-band
+// consumers read (the tensor-core kernel's unit_scale, the fp32 loop's unit_scale, the training gather)
+int forget_unit_broadcast_launch(const float* scaleT, RowMap map, int R, int Tp, float* unit_scale, cudaStream_t st);
 
 // TMA tensor maps (fsn_tgemm.cu).  tmap_encoder: cuTensorMapEncodeTiled through the runtime's driver entry point (no link
 // against libcuda), nullptr when the driver lacks it.  encode_tmap_2d: a row-major 2-D array of `inner` elements per row,
@@ -194,9 +214,9 @@ int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const 
 // input of a training step (fullsubnet/model.py:85-92, fullband_baseline/model.py:46-56): look-ahead pad, first norm and
 // the time-major copies raw [Tp,B,F] (unscaled) and scaled [Tp,B,F] (normalised); sums[b] = per-clip (sum, sum_f c_Ns[f]
 // * row sum), inv1[b] = 1 / (mean + eps).  cum: causal running mean instead, fs [B*Tp] frame sums, cum1 [Tp*B] scales
-// (fs / cum1 unused otherwise).
+// (fs / cum1 unused otherwise).  norm_type (FSN_NORM_*) picks the running mean: cumulative or forgetting.
 static const float TRAIN_CUM_EPS = 1.1920928955078125e-07f;  // audio_zen/constant.py:9
-int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, bool cum, float2* sums, float* inv1,
+int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, int norm_type, float2* sums, float* inv1,
                        float* raw, float* scaled, float2* fs, float* cum1, cudaStream_t st);
 // its backward: dY [Tp,B,2F] = dout [B,2,F,T] re-laid out, zero on the first `la` frames, times act'(y) (FSN_ACT_*) from
 // the kept post-activation output y (unread for FSN_ACT_NONE)
@@ -231,6 +251,13 @@ int train_cum_unit_bwd_launch(const float* dX, const float* X, const float* scal
                               cudaStream_t st);
 int train_dfbz_cum_launch(const float* dunit, const float* fbz, RowMap map, int Tp, int R, int act, float* dz,
                           cudaStream_t st);
+// the same for the second forgetting norm (scale2T [Tp,B], one scale per (step, clip) over all F K features; Nf = 0):
+//   dot[t,b] = <dX, X> over the kept rows of clip b at step t (one CTA per (t, b), fixed tree);
+//   reverse recurrence per clip: g_t = -s_t dot[t,b] + a_{t+1} g_{t+1}, mid[t,b] = b_t g_t / cnt  (d loss / d m_t over
+//   the cnt = F K features the mean averages; dot and mid share the buffer mid [Tp,B]);
+//   dz[t,b,f] = act'(fbz) * (dX[t, row(b,f), K-1] s_t + mid[t,b])  (a unit drop_band removed still feeds the mean).
+int train_forget_bwd_launch(const float* dX, const float* X, const float* fbz, const float* scale2T, RowMap map, int Tp,
+                            int R, int K, float cnt, int act, float* mid, float* dz, cudaStream_t st);
 
 // shapes of one fast_fullsubnet Model.forward call (fsn_fast_model.cu): Ts = shrunk steps of the bottleneck; cum: the
 // descriptor asks for the cumulative norm

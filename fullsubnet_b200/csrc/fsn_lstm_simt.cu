@@ -348,6 +348,65 @@ int cum_unit_scale_launch(const float* magT, const float* fbT, RowMap map, int R
   return FSN_OK;
 }
 
+// ---- forgetting_norm (base_model.py:102-151): the reference's per-frame loop in float32, one thread per clip
+ForgetCoef forget_coef() {
+  ForgetCoef c;
+  const double alpha = (double)(FORGET_LEN - 1) / (double)(FORGET_LEN + 1);
+  const float alpha32 = (float)alpha;
+  for (int t = 0; t < FORGET_LEN; ++t) {
+    // alp = torch.min(torch.tensor([(t-1)/(t+1), alpha])): both rounded to float32 first; 1 - alp in float32
+    const float r = (float)((double)(t - 1) / (double)(t + 1));
+    const float a = r < alpha32 ? r : alpha32;
+    c.a[t] = a;
+    c.b[t] = 1.0f - a;
+  }
+  c.a[FORGET_LEN] = alpha32;            // alpha * mu: the double applied to a float32 tensor
+  c.b[FORGET_LEN] = (float)(1.0 - alpha);  // (1 - alpha) evaluated in double, then applied
+  return c;
+}
+
+__global__ void forget_scale_kernel(const float2* __restrict__ fs, const float2* __restrict__ fs2, int B, int Tp, float cnt,
+                                    const ForgetCoef c, float* __restrict__ scaleT, float* __restrict__ muT,
+                                    const int* __restrict__ lens, int hop, int la) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int Tb = lens ? min(Tp, 1 + lens[b] / hop + la) : Tp;
+  float mu = 0.f;
+  for (int t = 0; t < Tb; ++t) {
+    const float2 v = fs[(size_t)b * Tp + t];
+    const float s = fs2 ? __fadd_rn(v.y, fs2[(size_t)b * Tp + t].y) : v.x;
+    const float m = __fdiv_rn(s, cnt);  // torch.mean: sum / count
+    const int i = t < FORGET_LEN ? t : FORGET_LEN;
+    mu = __fadd_rn(__fmul_rn(c.a[i], mu), __fmul_rn(c.b[i], m));
+    if (muT) muT[(size_t)t * B + b] = mu;
+    scaleT[(size_t)t * B + b] = __fdiv_rn(1.0f, __fadd_rn(mu, FORGET_EPS));
+  }
+}
+
+__global__ void forget_unit_broadcast_kernel(const float* __restrict__ scaleT, RowMap map, int R, int Tp,
+                                             float* __restrict__ unit_scale) {
+  const size_t n = (size_t)Tp * R;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int r = (int)(i % R), t = (int)(i / R);
+    int b, f;
+    row_to_unit(map, r, b, f);
+    unit_scale[i] = scaleT[(size_t)t * map.B + b];
+  }
+}
+
+int forget_scale_launch(const float2* fs, const float2* fs2, int B, int Tp, float cnt, float* scaleT, float* muT,
+                        cudaStream_t st, const int* lens, int hop, int la) {
+  forget_scale_kernel<<<cdiv(B, 64), 64, 0, st>>>(fs, fs2, B, Tp, cnt, forget_coef(), scaleT, muT, lens, hop, la);
+  FSN_CHECK_LAUNCH("forget_scale_kernel");
+  return FSN_OK;
+}
+
+int forget_unit_broadcast_launch(const float* scaleT, RowMap map, int R, int Tp, float* unit_scale, cudaStream_t st) {
+  forget_unit_broadcast_kernel<<<ew_grid((size_t)Tp * R), 256, 0, st>>>(scaleT, map, R, Tp, unit_scale);
+  FSN_CHECK_LAUNCH("forget_unit_broadcast_kernel");
+  return FSN_OK;
+}
+
 int lstm_step_launch(const StepParams& p, int mode, cudaStream_t st) {
   dim3 grid(cdiv(p.R, BM), cdiv(p.H, BU));
   if (mode == SEG0_DENSE) lstm_step_kernel<SEG0_DENSE><<<grid, 256, 0, st>>>(p);
@@ -596,4 +655,35 @@ extern "C" int fsn_debug_norm_stats(const float* x, int B, int T_pad, int F, int
   if (!inv1 && !inv2) return FSN_OK;
   return norm_scales_launch(sums2, fb_sums ? reinterpret_cast<const float2*>(fb_sums) : sums2, B, cnt1, cnt2, inv1, inv2,
                             st, eps, w.lens, hop, la);
+}
+
+// ---- unit-test hook of the forgetting norm's forward scan (include/fsn_b200.h): frame_stats + forget_scale_launch as the
+// forwards run them, every argument checked before any CUDA call
+extern "C" int fsn_debug_forgetting_scale(const float* x, int N, const float* x2, int N2, int B, int T_pad, int F,
+                                          int64_t bs, int64_t ts, float cnt, const int32_t* lengths, int* lens_dev, int hop,
+                                          int la, float* fs, float* fs2, float* scale, float* mu, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(x && fs && scale && (!x2 || fs2), FSN_ERR_SHAPE, "forgetting scale hook: null argument");
+  FSN_REQUIRE(B > 0 && T_pad > 0 && F > 0 && bs >= 0 && ts >= 0, FSN_ERR_SHAPE,
+              "forgetting scale hook: bad shape B=%d T_pad=%d F=%d", B, T_pad, F);
+  FSN_REQUIRE(N >= 0 && N < F && (!x2 || (N2 >= 0 && N2 < F)), FSN_ERR_SHAPE,
+              "forgetting scale hook: reflect padding needs 0 <= N < F");
+  FSN_REQUIRE((size_t)B * T_pad < ((size_t)1 << 31), FSN_ERR_SHAPE, "forgetting scale hook: B*T_pad must stay below 2^31");
+  FSN_REQUIRE(cnt > 0.f, FSN_ERR_SHAPE, "forgetting scale hook: cnt must be positive");
+  if (lengths) {
+    FSN_REQUIRE(lens_dev && hop > 0 && la >= 0, FSN_ERR_SHAPE,
+                "forgetting scale hook: lengths need lens_dev, hop > 0, la >= 0");
+    for (int b = 0; b < B; ++b)
+      FSN_REQUIRE(lengths[b] >= 0 && 1 + lengths[b] / hop + la <= T_pad, FSN_ERR_SHAPE,
+                  "forgetting scale hook: clip %d has more than T_pad frames", b);
+  }
+  const cudaStream_t st = (cudaStream_t)stream;
+  WavWs w = {nullptr, nullptr, nullptr, nullptr, lens_dev};
+  int rc = wav_prologue(lengths, B, w, st);
+  if (rc) return rc;
+  float2* f1 = reinterpret_cast<float2*>(fs);
+  float2* f2 = x2 ? reinterpret_cast<float2*>(fs2) : nullptr;
+  if ((rc = frame_stats_launch(x, B, T_pad, F, N, (size_t)bs, (size_t)ts, f1, st))) return rc;
+  if (x2 && (rc = frame_stats_launch(x2, B, T_pad, F, N2, (size_t)bs, (size_t)ts, f2, st))) return rc;
+  return forget_scale_launch(f1, f2, B, T_pad, cnt, scale, mu, st, w.lens, hop, la);
 }

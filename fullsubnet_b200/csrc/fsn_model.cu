@@ -38,7 +38,8 @@ static void prof_reset() { for (int i = 0; i < 5; ++i) g_ev_valid[i] = false; }
 struct ModelWs {
   float *magT, *fbT, *inv1, *inv2;
   float2 *fs, *sums_mag, *sums_fb;
-  float *cum1, *cum2;  // cumulative norm: per-(step, clip) and per-(step, unit) scales
+  float *cum1, *cum2;  // cumulative / forgetting norm: per-(step, clip) and per-(step, unit) scales
+  float2* fs2;         // forgetting norm: frame sums of the full-band output (fs keeps the noisy magnitude's)
   SeqStackWs fb;
   float *sb_h0[2], *sb_h1[2], *sb_c0, *sb_c1;
   size_t bytes;
@@ -52,7 +53,7 @@ static SeqStack fb_stack(const fsn_model_desc* d, const Dims& m) {
   memset(&s, 0, sizeof(s));
   s.R = m.B; s.Tp = m.Tp; s.K0 = m.F; s.n = 2; s.H[0] = s.H[1] = d->fb_hidden; s.O = m.F; s.act = d->fb_activation;
   s.gru = d->cell_type == FSN_CELL_GRU;
-  s.step_scale = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
+  s.step_scale = norm_per_step(d->norm_type);
   s.x3 = d->precision == FSN_PREC_F16X3_TC;
   s.tc = (s.x3 || d->precision == FSN_PREC_F16_TC) && !s.gru && lstm_rec_tc_supported(d->fb_hidden, s.x3);
   return s;
@@ -62,8 +63,10 @@ int make_dims(const fsn_model_desc* d, int B, int T, Dims& m) {
   FSN_REQUIRE(d && d->num_freqs > 1 && d->fb_hidden > 0 && d->sb_hidden > 0 && d->look_ahead >= 0, FSN_ERR_SHAPE,
               "model: bad descriptor");
   FSN_REQUIRE(B > 0 && T > 0, FSN_ERR_SHAPE, "model: empty input (B=%d, T=%d)", B, T);
-  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE,
-              FSN_ERR_UNSUPPORTED, "You must set up a type of Norm. (offline_laplace_norm / cumulative_laplace_norm are built)");
+  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE ||
+                  d->norm_type == FSN_NORM_FORGETTING,
+              FSN_ERR_UNSUPPORTED,
+              "You must set up a type of Norm. (offline_laplace_norm / cumulative_laplace_norm / forgetting_norm are built)");
   FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM || (d->cell_type == FSN_CELL_GRU && d->precision == FSN_PREC_FP32),
               FSN_ERR_UNSUPPORTED, "model: sequence_model must be LSTM, or GRU on the fp32 kernels (precision fp32)");
   FSN_REQUIRE(d->sb_num_neighbors >= 0 && d->fb_num_neighbors >= 0 && d->sb_num_neighbors < d->num_freqs &&
@@ -100,10 +103,12 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
     w.sb_c1 = c.take<float>(RH);
   }
   w.cum1 = w.cum2 = nullptr;
-  if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
+  w.fs2 = nullptr;
+  if (norm_per_step(d->norm_type)) {
     w.cum1 = c.take<float>((size_t)m.Tp * m.B);
     w.cum2 = c.take<float>((size_t)m.Tp * m.R);
   }
+  if (d->norm_type == FSN_NORM_FORGETTING) w.fs2 = c.take<float2>((size_t)m.B * m.Tp);
   w.bytes = c.off;
 }
 
@@ -122,19 +127,23 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
   if ((rc = norm_scales_launch(w.sums_mag, w.sums_mag, B, (float)F * tp_cnt, 1.f, w.inv1, nullptr, st, 1e-5f, lens, hop,
                                la)))
     return rc;
-  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
+  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, fgt = d->norm_type == FSN_NORM_FORGETTING;
   const float cum_eps = 1.1920928955078125e-07f;  // audio_zen/constant.py:9 (np.finfo(np.float32).eps)
   if (cum && (rc = cum_clip_scale_launch(w.fs, B, Tp, F, cum_eps, w.cum1, st))) return rc;
+  // forgetting norm (base_model.py:102-151): exponential running mean of the frame means, no bound needed with lens
+  if (fgt && (rc = forget_scale_launch(w.fs, nullptr, B, Tp, (float)F, w.cum1, nullptr, st))) return rc;
 
   // ---- full-band stack -> fbT [B, Tp, F]; x = magT * 1/(mu + 1e-5) of the clip (model.py:92) or, cumulative norm, the
-  // scale of (step, clip) from the time-major table cum1[t*B + b] (base_model.py:220-251)
+  // scale of (step, clip) from the time-major table cum1[t*B + b] (base_model.py:220-251), or the forgetting norm's
   SeqStack s = fb_stack(d, m);
   s.L[0] = seq_layer(*fb, 0); s.L[1] = seq_layer(*fb, 1);
-  s.x = w.magT; s.scale = cum ? w.cum1 : w.inv1; s.fc_w = fb->fc_w; s.fc_b = fb->fc_b; s.out = w.fbT;
+  s.x = w.magT; s.scale = (cum || fgt) ? w.cum1 : w.inv1; s.fc_w = fb->fc_w; s.fc_b = fb->fc_b; s.out = w.fbT;
   if ((rc = seq_stack_forward(s, w.fb, st))) return rc;
 
   // ---- second norm (model.py:110-111) in closed form: never materialise [B,F,Ksb,T']
-  if ((rc = clip_stats_launch(w.fbT, B, Tp, F, d->fb_num_neighbors, w.fs, w.sums_fb, st, lens, hop, la))) return rc;
+  // (the forgetting norm keeps the noisy magnitude's frame sums in fs and takes the full-band output's in fs2)
+  if ((rc = clip_stats_launch(w.fbT, B, Tp, F, d->fb_num_neighbors, fgt ? w.fs2 : w.fs, w.sums_fb, st, lens, hop, la)))
+    return rc;
   if ((rc = norm_scales_launch(w.sums_mag, w.sums_fb, B, 1.f, (float)F * m.Ksb * tp_cnt, nullptr, w.inv2, st, 1e-5f, lens,
                                hop, la)))
     return rc;
@@ -144,6 +153,13 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
   if (cum && (rc = cum_unit_scale_launch(w.magT, w.fbT, map, m.R, Tp, d->sb_num_neighbors, d->fb_num_neighbors, cum_eps,
                                          w.cum2, st)))
     return rc;
+  // forgetting norm: one scale per (step, clip) over all F Ksb features of sb_input (model.py:111), mean from the
+  // reflect-weighted frame sums of both unfolds; cum1 (the first norm's table, already consumed) holds it before the
+  // broadcast to the per-(step, row) layout of the sub-band kernels
+  if (fgt) {
+    if ((rc = forget_scale_launch(w.fs, w.fs2, B, Tp, (float)F * m.Ksb, w.cum1, nullptr, st))) return rc;
+    if ((rc = forget_unit_broadcast_launch(w.cum1, map, m.R, Tp, w.cum2, st))) return rc;
+  }
   if (d->precision == FSN_PREC_F16_TC || d->precision == FSN_PREC_F16X3_TC) {
     FSN_REQUIRE(sb_packed, FSN_ERR_SHAPE, "model: the tensor-core precisions need packed sub-band weights");
     SbTcArgs a;
@@ -151,7 +167,7 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
     a.packed = sb_packed; a.magT = w.magT; a.fbT = w.fbT; a.inv2 = w.inv2; a.crm = crm;
     a.B = B; a.F = F; a.Tp = Tp; a.la = d->look_ahead; a.Ns = d->sb_num_neighbors; a.Nf = d->fb_num_neighbors;
     a.H = Hs; a.act = d->sb_activation; a.map = map; a.x3 = d->precision == FSN_PREC_F16X3_TC;
-    a.unit_scale = cum ? w.cum2 : nullptr;
+    a.unit_scale = (cum || fgt) ? w.cum2 : nullptr;
     rc = sb_tc_forward(a, st);
     prof_mark(3, st);
     return rc;
@@ -166,7 +182,7 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
     p.K0 = m.Ksb;
     p.w_ih = sb->w_ih[0]; p.w_hh = sb->w_hh[0]; p.b_ih = sb->b_ih[0]; p.b_hh = sb->b_hh[0];
     p.magT = w.magT; p.fbT = w.fbT; p.inv2 = w.inv2;
-    p.unit_scale = cum ? w.cum2 + (size_t)t * m.R : nullptr;
+    p.unit_scale = (cum || fgt) ? w.cum2 + (size_t)t * m.R : nullptr;
     p.F = F; p.Tp = Tp; p.t = t; p.Ns = d->sb_num_neighbors; p.Nf = d->fb_num_neighbors; p.map = map;
     if ((rc = lstm_step2_launch(p, SEG0_GATHER, t, seq_layer(*sb, 1), s2, st))) return rc;
     if (t >= d->look_ahead)

@@ -322,6 +322,71 @@ int train_dfbz_cum_launch(const float* dunit, const float* fbz, RowMap map, int 
   return FSN_OK;
 }
 
+// ---- forgetting_norm at the second norm (base_model.py:102-151 on sb_input [B,F,K,T'], one scale per (clip, step))
+// Backward of X[t,r,k] = u[t,r,k] s_t, s_t = 1/(mu_t + eps), mu_t = a_t mu_{t-1} + b_t m_t, m_t = sum_{f,k} u / cnt over
+// all F units of the clip (drop_band comes after the norm):
+//   d mu_t (direct) = -s_t^2 <dX, u>_t = -s_t <dX, X>_t,  g_t = d mu_t + a_{t+1} g_{t+1},  d m_t = b_t g_t,
+//   d u[t,r,k] = dX[t,r,k] s_t + d m_t / cnt.
+// dot[t*B + b] <- <dX, X> over the Fsub rows of output clip bq at step t; one CTA per (t, bq), fixed-order tree.
+__global__ void train_forget_dot_kernel(const float* __restrict__ dX, const float* __restrict__ X, RowMap map, int Tp,
+                                        int R, int K, float* __restrict__ dot) {
+  __shared__ float sh[256];
+  const int bq = blockIdx.x % map.B, t = blockIdx.x / map.B;
+  const size_t base = ((size_t)t * R + (size_t)bq * map.Fsub) * K, n = (size_t)map.Fsub * K;
+  float a = 0.f;
+  for (size_t i = threadIdx.x; i < n; i += 256) a = fmaf(dX[base + i], X[base + i], a);
+  sh[threadIdx.x] = a;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    int b, f;
+    row_to_unit(map, bq * map.Fsub, b, f);  // source clip of output clip bq
+    dot[(size_t)t * map.B + b] = sh[0];
+  }
+}
+// the reverse recurrence, one thread per clip, in place: mid[t*B + b] holds <dX, X>_t on entry, d m_t / cnt on exit
+__global__ void train_forget_scan_bwd_kernel(const float* __restrict__ scale2T, int B, int Tp, float cnt, const ForgetCoef c,
+                                             float* __restrict__ mid) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  float g = 0.f;
+  for (int t = Tp - 1; t >= 0; --t) {
+    const size_t i = (size_t)t * B + b;
+    const float a_next = t + 1 < FORGET_LEN ? c.a[t + 1] : c.a[FORGET_LEN];
+    g = fmaf(a_next, g, -scale2T[i] * mid[i]);  // a_{t+1} g_{t+1} + d mu_t; g_{Tp} = 0
+    mid[i] = c.b[t < FORGET_LEN ? t : FORGET_LEN] * g / cnt;
+  }
+}
+// dz[t,b,f] = act'(fbz) (dX[t, row(b,f), K-1] s_t + mid[t,b])  (Nf = 0: the full-band row f enters the mean once)
+__global__ void train_dfbz_forget_kernel(const float* __restrict__ dX, const float* __restrict__ fbz,
+                                         const float* __restrict__ scale2T, const float* __restrict__ mid, RowMap map,
+                                         int Tp, int R, int K, int act, float* __restrict__ dz) {
+  const size_t n = (size_t)Tp * map.B * map.F;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int f = (int)(i % map.F);
+    const size_t tb = i / map.F;
+    const int b = (int)(tb % map.B), t = (int)(tb / map.B);
+    float v = mid[tb];
+    const int r = unit_to_row(map, b, f);
+    if (r >= 0) v = fmaf(dX[((size_t)t * R + r) * K + (K - 1)], scale2T[tb], v);
+    dz[i] = act_grad(v, fbz, i, act);
+  }
+}
+
+int train_forget_bwd_launch(const float* dX, const float* X, const float* fbz, const float* scale2T, RowMap map, int Tp,
+                            int R, int K, float cnt, int act, float* mid, float* dz, cudaStream_t st) {
+  train_forget_dot_kernel<<<(unsigned)((size_t)Tp * map.B), 256, 0, st>>>(dX, X, map, Tp, R, K, mid);
+  FSN_CHECK_LAUNCH("train_forget_dot_kernel");
+  train_forget_scan_bwd_kernel<<<cdiv(map.B, 64), 64, 0, st>>>(scale2T, map.B, Tp, cnt, forget_coef(), mid);
+  FSN_CHECK_LAUNCH("train_forget_scan_bwd_kernel");
+  train_dfbz_forget_kernel<<<132 * 8, 256, 0, st>>>(dX, fbz, scale2T, mid, map, Tp, R, K, act, dz);
+  FSN_CHECK_LAUNCH("train_dfbz_forget_kernel");
+  return FSN_OK;
+}
+
 // LSTM cell of one step (tensor-core path): G_t [R,4H] holds x_t W_ih^T (all steps from one hoisted GEMM), rec the
 // recurrent product of this step; G_t is overwritten with the post-activation gates (i,f,g,o); writes c_t and h_t
 __global__ void lstm_cell_fwd_kernel(float* __restrict__ G, const float* __restrict__ rec, const float* __restrict__ b_ih,
@@ -482,6 +547,10 @@ struct TrainWs {
   __half *fb_h16[2], *sb_h16[2], *w16;  // fp16 MMA operands of the forward step kernel (hidden states, weights)
   float *cum1, *cum2, *dunit;  // cumulative norm: scale of (step, clip), of (step, unit); gradient of the fb row per unit
   float2* fs;
+  // forgetting norm: cum1 / cum2 as above (cum2 the broadcast of fg2), fs the frame sums of the noisy magnitude; fs2 those
+  // of the full-band output, fg2 [Tp,B] the second norm's scale of (step, clip), fmid [Tp,B] its backward's d m_t / cnt
+  float *fg2, *fmid;
+  float2* fs2;
   size_t bytes;
 };
 
@@ -502,10 +571,14 @@ static void carve_train(const fsn_model_desc* d, const Dims& m, void* base, Trai
   for (int i = 0; i < 2; ++i) { w.dh_rec[i] = c.take<float>(RH); w.dc[i] = c.take<float>(RH); }
   w.dh_mid = c.take<float>(RH);
   w.dot = c.take<float>(B);
-  w.cum1 = w.cum2 = w.dunit = nullptr; w.fs = nullptr;
+  w.cum1 = w.cum2 = w.dunit = w.fg2 = w.fmid = nullptr; w.fs = w.fs2 = nullptr;
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
     w.cum1 = c.take<float>(Tp * B); w.cum2 = c.take<float>(Tp * R); w.dunit = c.take<float>(Tp * R);
     w.fs = c.take<float2>(Tp * B);
+  } else if (d->norm_type == FSN_NORM_FORGETTING) {
+    w.cum1 = c.take<float>(Tp * B); w.cum2 = c.take<float>(Tp * R); w.fg2 = c.take<float>(Tp * B);
+    w.fmid = c.take<float>(Tp * B);
+    w.fs = c.take<float2>(Tp * B); w.fs2 = c.take<float2>(Tp * B);
   }
   w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
   const size_t maxcols = 4 * (Hf > Hs ? Hf : Hs) > F ? 4 * (Hf > Hs ? Hf : Hs) : F;
@@ -539,8 +612,9 @@ static void carve_train(const fsn_model_desc* d, const Dims& m, void* base, Trai
 }
 
 static int train_check(const fsn_model_desc* d) {
-  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, FSN_ERR_UNSUPPORTED,
-              "training: offline_laplace_norm and cumulative_laplace_norm are built");
+  FSN_REQUIRE(d->norm_type == FSN_NORM_OFFLINE_LAPLACE || d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE ||
+                  d->norm_type == FSN_NORM_FORGETTING,
+              FSN_ERR_UNSUPPORTED, "training: offline_laplace_norm, cumulative_laplace_norm and forgetting_norm are built");
   FSN_REQUIRE(d->fb_num_neighbors == 0, FSN_ERR_UNSUPPORTED,
               "training: fb_num_neighbors > 0 is not built (every shipped recipe uses 0)");
   FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "training: the GRU cell is built for inference only");
@@ -745,16 +819,18 @@ int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const 
 }
 
 // ------------------------------------------------------------------------------------------ shared by the training steps
-int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, bool cum, float2* sums, float* inv1,
+int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, int norm_type, float2* sums, float* inv1,
                        float* raw, float* scaled, float2* fs, float* cum1, cudaStream_t st) {
   int rc;
   if ((rc = train_mag_stats_launch(noisy_mag, B, F, T, Ns, sums, st))) return rc;
   if ((rc = norm_scales_launch(sums, sums, B, (float)F * Tp, 1.f, inv1, nullptr, st))) return rc;
   // raw [Tp,B,F] and scaled = raw * inv1[b]
   if ((rc = transpose_mag_launch(noisy_mag, B, F, T, Tp, F, (size_t)B * F, raw, inv1, scaled, st))) return rc;
-  if (cum) {  // causal running mean per clip instead of the clip mean (base_model.py:220-251)
+  if (norm_per_step(norm_type)) {  // causal running mean per clip instead of the clip mean
     if ((rc = frame_stats_launch(raw, B, Tp, F, 0, F, (size_t)B * F, fs, st))) return rc;
-    if ((rc = cum_clip_scale_launch(fs, B, Tp, F, TRAIN_CUM_EPS, cum1, st))) return rc;
+    if (norm_type == FSN_NORM_FORGETTING) rc = forget_scale_launch(fs, nullptr, B, Tp, (float)F, cum1, nullptr, st);
+    else rc = cum_clip_scale_launch(fs, B, Tp, F, TRAIN_CUM_EPS, cum1, st);  // base_model.py:220-251
+    if (rc) return rc;
     if ((rc = scale_rows_launch(raw, cum1, (size_t)Tp * B * F, F, Tp * B, 1, scaled, st))) return rc;  // scale of (t, b)
   }
   return FSN_OK;
@@ -806,9 +882,9 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   cudaStream_t st = (cudaStream_t)stream;
   const int Tp = m.Tp, F = m.F, Hf = d->fb_hidden, Hs = d->sb_hidden;
   // first norm (model.py:92) and the time-major copies
-  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
-  if ((rc = train_input_launch(noisy_mag, B, F, T, Tp, d->sb_num_neighbors, cum, w.sums_mag, w.inv1, w.raw, w.xfb, w.fs,
-                               w.cum1, st)))
+  const bool cum = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, fgt = d->norm_type == FSN_NORM_FORGETTING;
+  if ((rc = train_input_launch(noisy_mag, B, F, T, Tp, d->sb_num_neighbors, d->norm_type, w.sums_mag, w.inv1, w.raw, w.xfb,
+                               w.fs, w.cum1, st)))
     return rc;
   // full-band stack + Linear/activation (model.py:92-95)
   // fp16 operand copies: layer 0's hidden states double as layer 1's input
@@ -826,7 +902,13 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   if (cum && (rc = cum_unit_scale_launch(w.raw, w.fbz, map, m.R, Tp, d->sb_num_neighbors, d->fb_num_neighbors, TRAIN_CUM_EPS, w.cum2,
                                          st, /*time_major=*/true)))
     return rc;
-  train_gather_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.fbz, w.inv2, cum ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,
+  if (fgt) {  // one scale per (step, clip) over all F K features: the reflect-weighted frame sums of both unfolds
+    if ((rc = frame_stats_launch(w.raw, B, Tp, F, d->sb_num_neighbors, F, (size_t)B * F, w.fs, st))) return rc;
+    if ((rc = frame_stats_launch(w.fbz, B, Tp, F, d->fb_num_neighbors, F, (size_t)B * F, w.fs2, st))) return rc;
+    if ((rc = forget_scale_launch(w.fs, w.fs2, B, Tp, (float)F * m.Ksb, w.fg2, nullptr, st))) return rc;
+    if ((rc = forget_unit_broadcast_launch(w.fg2, map, m.R, Tp, w.cum2, st))) return rc;
+  }
+  train_gather_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.fbz, w.inv2, (cum || fgt) ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,
                                                d->sb_num_neighbors, d->fb_num_neighbors);
   FSN_CHECK_LAUNCH("train_gather_kernel");
   if ((rc = layer_forward(prec, seq_layer(*sb, 0), w.xsb, m.R, m.Ksb, Hs, Tp, w.sb[0], w.rec, w.splitk, &hs0, st))) return rc;
@@ -923,6 +1005,10 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   if (d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE) {
     if ((rc = train_cum_unit_bwd_launch(w.dxsb, w.xsb, w.cum2, Tp, R, K, w.dunit, st2))) return rc;
     if ((rc = train_dfbz_cum_launch(w.dunit, w.fbz, map, Tp, R, d->fb_activation, w.dz, st2))) return rc;
+  } else if (d->norm_type == FSN_NORM_FORGETTING) {
+    if ((rc = train_forget_bwd_launch(w.dxsb, w.xsb, w.fbz, w.fg2, map, Tp, R, K, (float)F * K, d->fb_activation, w.fmid,
+                                      w.dz, st2)))
+      return rc;
   } else {
     if ((rc = train_dot_launch(w.dxsb, w.xsb, Tp, R, m.Fsub, K, B, w.dot, st2))) return rc;
     if ((rc = train_dfbz_launch(w.dxsb, w.fbz, w.inv2, w.dot, map, Tp, R, K, (float)F * K * Tp, d->fb_activation, w.dz,
@@ -1341,6 +1427,24 @@ extern "C" int fsn_debug_norm_unfold_bwd(const float* dX, const float* X, const 
   }
   if ((rc = train_dot_launch(dX, X, Tp, R, Fsub, K, B, mid, st))) return rc;
   return train_dfbz_launch(dX, fbz, scale, mid, map, Tp, R, K, cnt2, act, dz, st);
+}
+
+// ---- unit-test hook of the second forgetting norm + drop_band backward (include/fsn_b200.h): train_forget_bwd_launch as
+// fsn_train_backward runs it, every argument checked before any CUDA call
+extern "C" int fsn_debug_forgetting_bwd(const float* dX, const float* X, const float* fbz, const float* scale, int B, int F,
+                                        int G, int Tp, int Ns, int act, float* mid, float* dz, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(dX && X && fbz && scale && mid && dz, FSN_ERR_SHAPE, "forgetting backward hook: null argument");
+  FSN_REQUIRE(B > 0 && F > 0 && Tp > 0 && G >= 0, FSN_ERR_SHAPE, "forgetting backward hook: bad shape B=%d F=%d Tp=%d G=%d",
+              B, F, Tp, G);
+  FSN_REQUIRE(G <= 1 || (B > G && F >= G), FSN_ERR_SHAPE, "forgetting backward hook: drop_band needs B > G and F >= G");
+  FSN_REQUIRE(Ns >= 0 && Ns < F, FSN_ERR_SHAPE, "forgetting backward hook: reflect padding needs 0 <= Ns < F");
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "forgetting backward hook: unknown act %d", act);
+  const int Fsub = G > 1 ? F / G : F, R = B * Fsub, K = 2 * Ns + 2;
+  FSN_REQUIRE((size_t)Tp * R * K < ((size_t)1 << 31) && (size_t)Tp * B * F < ((size_t)1 << 31), FSN_ERR_SHAPE,
+              "forgetting backward hook: tensors must stay below 2^31 elements");
+  const RowMap map{B, F, Fsub, G > 1 ? G : 1};
+  return train_forget_bwd_launch(dX, X, fbz, scale, map, Tp, R, K, (float)F * K, act, mid, dz, (cudaStream_t)stream);
 }
 
 // ---- unit-test hook of the per-clip statistics of the training steps (include/fsn_b200.h)

@@ -57,6 +57,8 @@ class _MelScale(nn.Module):
 
 
 class Model(BaseModel):
+    # forgetting_norm is built for fullsubnet and fullband_baseline only: it stays an unbuilt upstream norm here
+    NORM_TYPES = {"offline_laplace_norm": 0, "cumulative_laplace_norm": 1}
     # training step (fast_fullsubnet/trainer.py:45-56): fsn_fast_train_forward keeps the activations,
     # fsn_fast_train_backward runs BPTT
     TRAIN_ENTRY_POINTS = ("fsn_fast_train_workspace_bytes", "fsn_fast_train_forward", "fsn_fast_train_backward")

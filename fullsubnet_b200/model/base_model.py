@@ -59,7 +59,7 @@ class TrainStep(torch.autograd.Function):
 
 
 class BaseModel(nn.Module):
-    NORM_TYPES = {"offline_laplace_norm": 0, "cumulative_laplace_norm": 1}
+    NORM_TYPES = {"offline_laplace_norm": 0, "cumulative_laplace_norm": 1, "forgetting_norm": 4}
     _UPSTREAM_NORMS = ("offline_laplace_norm", "cumulative_laplace_norm", "offline_gaussian_norm",
                        "cumulative_layer_norm", "forgetting_norm")
 

@@ -44,8 +44,17 @@ enum {
 enum { FSN_ACT_NONE = 0, FSN_ACT_RELU = 1, FSN_ACT_TANH = 2, FSN_ACT_RELU6 = 3 };
 /* FSN_NORM_CUMULATIVE_LAPLACE (audio_zen/model/base_model.py:220-251): causal running mean per clip (first norm) and
  * per sub-band unit (second norm); built for the fp32 inference path of fsn_model_forward / fsn_enhance, and for
- * fast_fullsubnet (fsn_fast_desc.norm_type) on every precision of inference and training */
-enum { FSN_NORM_OFFLINE_LAPLACE = 0, FSN_NORM_CUMULATIVE_LAPLACE = 1 };
+ * fast_fullsubnet (fsn_fast_desc.norm_type) on every precision of inference and training.
+ * FSN_NORM_FORGETTING (base_model.py:102-151, forgetting_norm): causal exponential running mean per clip, mu_t =
+ * a_t mu_{t-1} + b_t m_t with alpha = 191/193 from frame 192 on (a_0 = -1, so mu_0 = 2 m_0; a_1 = 0), x / (mu_t + 1e-10),
+ * computed in the reference's float32 operation order.  One scale per (clip, frame) at both sites: over the F bins for
+ * the first norm, over all F * (2Ns+1 + 2Nf+1) unfolded features for fullsubnet's second norm.  Built for fullsubnet
+ * (fsn_model_desc) and fullband_baseline (fsn_fullband_desc) wherever FSN_NORM_CUMULATIVE_LAPLACE runs: every inference
+ * precision and cell, the training steps on fp32 and tf32.  fsn_fast_desc and the improved_fullsubnet paths refuse it
+ * (FSN_ERR_UNSUPPORTED before any CUDA call).  An addition at version 102 (see fsn_version). */
+/* The values follow the order of the reference's norm_wrapper (base_model.py:356-372); 2 (offline_gaussian_norm) and 3
+ * (cumulative_layer_norm) are not built and are refused everywhere. */
+enum { FSN_NORM_OFFLINE_LAPLACE = 0, FSN_NORM_CUMULATIVE_LAPLACE = 1, FSN_NORM_FORGETTING = 4 };
 enum { FSN_CELL_LSTM = 0, FSN_CELL_GRU = 1 };
 /* arithmetic of the sub-band LSTM stack (99 % of the FLOPs):
  *   FSN_PREC_FP32     - fp32 FMA everywhere (bit-for-bit class of the reference CPU path, ~1e-6)
@@ -64,7 +73,9 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
  * The version counts changes that break an existing caller.  Entry points added since 102 leave every earlier argument
  * list and struct as it was, so the version stays 102; a caller finds them by symbol: fsn_cirm_mse_per_clip (+ its
  * workspace query), fsn_si_sdr_lengths (the grouped validation loss and SI-SDR), fsn_clip_adam_steps (one Adam step
- * count per tensor) and fsn_stoi (+ its workspace query and the fsn_debug_stoi_stages hook). */
+ * count per tensor) and fsn_stoi (+ its workspace query and the fsn_debug_stoi_stages hook).  FSN_NORM_FORGETTING is a new
+ * value of an existing field, refused by every older entry point it does not apply to, with the fsn_debug_forgetting_*
+ * hooks. */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -121,7 +132,8 @@ typedef struct fsn_model_desc {
   int32_t sb_hidden;        /* 384 */
   int32_t fb_activation;    /* FSN_ACT_* (fb_output_activate_function) */
   int32_t sb_activation;    /* FSN_ACT_* (sb_output_activate_function) */
-  int32_t norm_type;        /* FSN_NORM_* */
+  int32_t norm_type;        /* FSN_NORM_*: offline, cumulative or forgetting (inference on every precision and cell,
+                             * training on fp32 and tf32) */
   int32_t num_groups_in_drop_band; /* applied when B > 1 (model.py:114), 1 = off */
   int32_t precision;        /* FSN_PREC_* for the sub-band stack */
   int32_t cell_type;        /* FSN_CELL_*: `sequence_model` = "LSTM" | "GRU" (sequence_model.py:52-66); GRU: weights
@@ -396,7 +408,7 @@ typedef struct fsn_fullband_desc {
   int32_t num_layers; /* the reference builds 3 */
   int32_t look_ahead;
   int32_t activation; /* FSN_ACT_* */
-  int32_t norm_type;  /* FSN_NORM_* */
+  int32_t norm_type;  /* FSN_NORM_*: offline, cumulative or forgetting, inference and training */
   int32_t precision;  /* FSN_PREC_FP32 (0) or FSN_PREC_TF32_TC (training: the tf32 GEMMs; inference: fp32 kernels) */
   int32_t cell_type;  /* FSN_CELL_* (0 = LSTM; inference and training are built for LSTM only) */
 } fsn_fullband_desc;
@@ -695,6 +707,28 @@ int fsn_debug_norm_stats(const float* x, int B, int T_pad, int F, int N, int64_t
                          int* lens_dev, int hop, int la, const float* fb_sums, float cnt1, float cnt2, float eps, float* fs,
                          float* sums, float* inv1, float* inv2, fsn_stream_t stream);
 int fsn_debug_train_stats(const float* x, int tm, int B, int F, int T, int N, float* sums, fsn_stream_t stream);
+
+/* unit-test hooks of forgetting_norm (FSN_NORM_FORGETTING; fsn_lstm_simt.cu, fsn_train.cu): the launchers the forwards and
+ * fsn_train_backward run, on caller buffers.  Additions at version 102 (see fsn_version).
+ *   fsn_debug_forgetting_scale: the forward scan.  x [B,T_pad,F] with element (b,t,f) at b*bs + t*ts + f (x2 the same
+ *     layout, nullable).  fs (float2 [B*T_pad]) <- frame_stats of x with N neighbours, fs2 (needed with x2) <- those of x2
+ *     with N2.  m_t = (sum_f x) / cnt without x2 (the first norm, cnt = F), else (sum_f c_N[f] x + sum_f c_N2[f] x2) / cnt
+ *     (fullsubnet's second norm over the unfolded noisy and full-band rows, cnt = F K).  scale [T_pad,B] <- 1 / (mu_t +
+ *     1e-10), mu (nullable, [T_pad,B]) <- mu_t.  lengths (nullable, host [B], copied to lens_dev): clip b is scanned over
+ *     its own 1 + lengths[b]/hop + la (<= T_pad) frames only and its later entries are left unwritten; its frames get the
+ *     bits of the unbounded scan, which is why fsn_enhance / fsn_fullband_enhance scan every clip over all T_max +
+ *     look_ahead steps.
+ *   fsn_debug_forgetting_bwd: the adjoint of the second norm and drop_band with respect to the full-band output (Nf = 0),
+ *     tensors time-major as in the training step: sub-band input X and its gradient dX [Tp,R,K], K = 2Ns+2, R = B*Fsub rows
+ *     of the drop_band map with G groups (G <= 1: none), full-band output fbz [Tp,B,F], scale [Tp,B] the forward's.  mid
+ *     [Tp,B] <- d loss / d m_t / (F K) (the reverse recurrence g_t = -scale_t <dX,X>_t + a_{t+1} g_{t+1}, times b_t);
+ *     dz [Tp,B,F] <- act'(fbz) (dX[t, row(b,f), K-1] scale[t,b] + mid[t,b]), the gradient at the full-band Linear's output.
+ * Arguments are checked before any CUDA call. */
+int fsn_debug_forgetting_scale(const float* x, int N, const float* x2, int N2, int B, int T_pad, int F, int64_t bs,
+                               int64_t ts, float cnt, const int32_t* lengths, int* lens_dev, int hop, int la, float* fs,
+                               float* fs2, float* scale, float* mu, fsn_stream_t stream);
+int fsn_debug_forgetting_bwd(const float* dX, const float* X, const float* fbz, const float* scale, int B, int F, int G,
+                             int Tp, int Ns, int act, float* mid, float* dz, fsn_stream_t stream);
 
 /* unit-test hook of fsn_stoi (fsn_stoi.cu): the same kernels, with the intermediate buffers the caller's.  With Lr_max =
  * ceil(L_max * 10000 / sr) samples at 10 kHz and nf_max = its frames (len(range(0, Lr_max - 256, 128))):
