@@ -1,0 +1,84 @@
+"""Chunked streaming throughput of fullband_baseline (fsn_fullband_stream_step): ms per call, audio seconds enhanced per
+wall second and concurrent real-time streams for slots x K, with the whole-clip fsn_fullband_enhance rate of the same
+process beside it.  Prints one JSON line per configuration and a header line with the GPU, power limit and clocks.
+
+    python bench_stream.py [--slots 1 64 256] [--ks 1 4 16 64] [--calls 20] [--warmup 3]"""
+from __future__ import annotations
+
+import argparse
+import json
+import subprocess
+
+import torch
+
+SR, HOP = 16000, 256
+
+
+def gpu_info():
+    try:
+        q = "name,power.limit,clocks.max.sm,clocks.sm"
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True,
+                             timeout=30).stdout.strip().splitlines()[0]
+        return dict(zip(q.split(","), [v.strip() for v in out.split(",")]))
+    except Exception as e:  # the numbers still stand; say the query failed
+        return {"error": str(e)}
+
+
+def model(norm, dev):
+    from fullsubnet_b200.fullband_baseline.model import Model
+    from oracle import fullband_baseline_oracle as BO
+    args = dict(BO.DEFAULT_FBB_ARGS, norm_type=norm)
+    m = Model(**args)
+    m.load_state_dict(BO.make_fbb_state_dict(seed=11, args=args), strict=True)
+    return m.to(dev).eval()
+
+
+def time_ms(fn, calls, warmup):
+    for _ in range(warmup):
+        fn()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    a.record()
+    for _ in range(calls):
+        fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b) / calls
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--slots", type=int, nargs="+", default=[1, 64, 256])
+    ap.add_argument("--ks", type=int, nargs="+", default=[1, 4, 16, 64])
+    ap.add_argument("--calls", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--norm", default="cumulative_laplace_norm")
+    a = ap.parse_args()
+    assert torch.cuda.is_available(), "bench_stream.py needs a CUDA device"
+    dev = torch.device("cuda:0")
+    from fullsubnet_b200.stream import Streamer
+    m = model(a.norm, dev)
+    print(json.dumps({"gpu": gpu_info(), "model": "fullband_baseline", "precision": "fp32", "norm": a.norm}))
+    g = torch.Generator(device="cpu").manual_seed(0)
+    for slots in a.slots:
+        s = Streamer(m, slots)
+        for K in a.ks:
+            x = (0.1 * torch.randn(slots, K * HOP, generator=g)).to(dev)
+            s.step(x, [1] * slots)
+            ms = time_ms(lambda: s.step(x), a.calls, a.warmup)
+            chunk_ms = 1000.0 * K * HOP / SR
+            audio_rate = slots * chunk_ms / ms
+            rt = slots if ms <= chunk_ms else int(slots * chunk_ms / ms)
+            print(json.dumps({"slots": slots, "K": K, "ms_per_call": round(ms, 3), "chunk_ms": chunk_ms,
+                              "audio_s_per_s": round(audio_rate, 1), "realtime_streams": rt, "delay": s.delay}))
+        del s
+        torch.cuda.empty_cache()
+    for B in (1, 64):
+        y = (0.1 * torch.randn(B, 4 * SR, generator=g)).to(dev)
+        ms = time_ms(lambda: m.enhance(y), max(3, a.calls // 4), a.warmup)
+        print(json.dumps({"whole_clip": True, "B": B, "clip_s": 4.0, "ms_per_call": round(ms, 3),
+                          "audio_s_per_s": round(B * 4000.0 / ms, 1)}))
+
+
+if __name__ == "__main__":
+    main()

@@ -11,6 +11,7 @@
 //              hop = 480: recipes/dns_interspeech_2020/improved_fullsubnet/model.py:603-620): a direct O(n^2) DFT in
 //              shared memory against a full-circle twiddle table.  At n = 960 that is 3.7 MFLOP per frame, i.e. < 1 %
 //              of the model's 217 MFLOP per frame, so a mixed-radix FFT would not move the step time.
+#include <limits.h>
 #include <string.h>
 
 #include "fsn_internal.cuh"
@@ -594,6 +595,161 @@ int istft_launch(const float* real, const float* imag, int cstride, const float*
   return dsp_launch(dft_size_ok(n_fft) ? istft_kernel<DirectDft> : istft_kernel<Radix2>, dim3(cdiv(out_len, seg), B),
                     istft_smem_bytes(n_fft, hop), st, "istft_kernel", real, imag, cstride, crm, mask_mode, T, n_fft, hop,
                     win_length, out_len, seg, istft_np_max(n_fft, hop), wav, peak_bits, lens);
+}
+
+// ---- streaming STFT / iSTFT (DESIGN 4.14).  Both compute every frame pair and every output sample with the code and
+// the operation order of stft_kernel / istft_kernel: a frame's transform depends only on its absolute pair (2k, 2k+1)
+// (STFT) or on the absolute segment tiling (iSTFT), never on where a call starts.
+
+// Step j of slot b is frame m = pos0[b]/hop - c + j (negative: a step before the clip's first frame).  win [B, Wn] holds
+// the slot's samples from pos0[b] - Hs on.  Writes magT [B, S, F] (0 outside [0, T_b)) and the spectrum (re | im, 2F
+// per frame) of step j at frame Q + j of spec [B, Q + S, 2F].  tail[b] >= 0: the clip has pos0[b] + tail[b] samples.
+template <class P>
+__global__ void __launch_bounds__(kDspThreads)
+stft_stream_kernel(const float* __restrict__ win, int Wn, int Hs, const int* __restrict__ pos0, const int* __restrict__ tail,
+                   int n, int hop, int win_length, int c, int S, int Q, float* __restrict__ magT, float* __restrict__ spec) {
+  extern __shared__ float2 smem2[];
+  constexpr int NP = kFR / 2;
+  const P tr(smem2, n, NP);
+  const int b = blockIdx.y;
+  const int F = n / 2 + 1;
+  const int p0 = pos0[b], m0 = p0 / hop - c, tl = tail[b];
+  const int Lb = tl >= 0 ? p0 + tl : INT_MAX;
+  const int Tb = tl >= 0 ? 1 + Lb / hop : INT_MAX;
+  const int t0 = (m0 >= 0 ? m0 / 2 : -((1 - m0) / 2)) * 2 + blockIdx.x * kFR;  // pairs start on even frames
+  init_tables(tr.tw, tr.tw_len, tr.win, n, win_length);
+  __syncthreads();
+  const float* x = win + (size_t)b * Wn;
+  fill_frame_pairs(tr, NP, t0, Tb, [&](int t, int i) {
+    if (t < 0) return 0.f;
+    const int w = reflect_idx(t * hop + i - n / 2, Lb) - (p0 - Hs);
+    return x[min(max(w, 0), Wn - 1)];
+  });
+  __syncthreads();
+  const float2* z = tr.template transform<false>(NP);
+  for (int idx = threadIdx.x; idx < F * kFR; idx += blockDim.x) {
+    const int j = idx / F;
+    const int k = idx - j * F;
+    const int t = t0 + j, js = t - m0;
+    if (js < 0 || js >= S) continue;
+    const bool in = t >= 0 && t < Tb;
+    const float2 cb = in ? unpack_bin(z, tr.stride, n, j, k) : make_float2(0.f, 0.f);
+    magT[((size_t)b * S + js) * F + k] = in ? hypotf(cb.x, cb.y) : 0.f;
+    float* sp = spec + ((size_t)b * (Q + S) + Q + js) * 2 * F;
+    sp[k] = cb.x;
+    sp[F + k] = cb.y;
+  }
+}
+
+// Output row b of wav [B, K*hop + D] holds clip samples [pos0 - D, pos0 - D + K*hop), or on the clip's last call
+// [pos0 - D, pos0 + tail); 0 elsewhere.  spec / crm [B, W, 2F] hold frames T0 + i, T0 = pos0/hop - c - la - Rc, with
+// W = Q + S (spectrum) and Rc + S (cRM).  CTA x covers the row's samples in absolute iSTFT segment g0 + x.
+template <class P>
+__global__ void __launch_bounds__(kDspThreads)
+istft_stream_kernel(const float* __restrict__ spec, const float* __restrict__ crm, const int* __restrict__ pos0,
+                    const int* __restrict__ act0, const int* __restrict__ tail, int K, int D, int n, int hop,
+                    int win_length, int seg, int np_max, int c, int la, int Rc, int Q, int S, float* __restrict__ wav) {
+  extern __shared__ float2 smem2[];
+  const P tr(smem2, n, np_max);
+  const int b = blockIdx.y;
+  const int F = n / 2 + 1;
+  const int p0 = pos0[b], tl = tail[b], rowlen = K * hop + D;
+  const int x_lo = p0 - D;
+  const int x_hi = !act0[b] ? x_lo : (tl >= 0 ? p0 + tl : x_lo + K * hop);
+  const int Lb = tl >= 0 ? p0 + tl : INT_MAX / 2;
+  const int Tb = tl >= 0 ? 1 + Lb / hop : INT_MAX / 2;
+  float* out = wav + (size_t)b * rowlen;
+  if (blockIdx.x == 0)
+    for (int j = threadIdx.x; j < rowlen; j += blockDim.x)
+      if (x_lo + j < 0 || x_lo + j >= x_hi) out[j] = 0.f;
+  const int g = max(x_lo, 0) / seg + blockIdx.x;
+  const int s_begin = n / 2 + g * seg;
+  const int s_end = min(s_begin + seg, n / 2 + Lb);
+  const int a = max(s_begin, n / 2 + max(x_lo, 0)), e = min(s_end, n / 2 + x_hi);
+  if (a >= e) return;
+  const int t_min = (s_begin >= n) ? (s_begin - n) / hop + 1 : 0;
+  const int t_max = min(Tb - 1, (s_end - 1) / hop);
+  const int tlo = max(t_min, (a >= n) ? (a - n) / hop + 1 : 0), thi = min(t_max, (e - 1) / hop);
+  const int pb = t_min + 2 * ((tlo - t_min) / 2);  // first frame of the first pair the samples read
+  const int np = thi >= tlo ? (thi - pb) / 2 + 1 : 0;
+  const int T0 = p0 / hop - c - la - Rc;
+  init_tables(tr.tw, tr.tw_len, tr.win, n, win_length);
+  const float* xs = spec + (size_t)b * (Q + S) * 2 * F;
+  const float* xc = crm + (size_t)b * (Rc + S) * 2 * F;
+  for (int idx = threadIdx.x; idx < F * np; idx += blockDim.x) {
+    const int k = idx / np;
+    const int p = idx - k * np;
+    float ev[2][2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int t = pb + 2 * p + q;
+      float r = 0.f, i = 0.f;
+      if (t <= t_max) {
+        const float* sp = xs + (size_t)(t - T0) * 2 * F;
+        const float* cp = xc + (size_t)(t - T0) * 2 * F;
+        r = sp[k];
+        i = sp[F + k];
+        const float mr = decompress_cirm_f(cp[k], 10.0f, 9.9f);
+        const float mi = decompress_cirm_f(cp[F + k], 10.0f, 9.9f);
+        const float er = mr * r - mi * i;
+        const float ei = mi * r + mr * i;
+        r = er; i = ei;
+      }
+      ev[q][0] = r;
+      ev[q][1] = (k == 0 || k == n / 2) ? 0.f : i;
+    }
+    tr.in[p * tr.stride + tr.slot(k)] = make_float2(ev[0][0] - ev[1][1], ev[0][1] + ev[1][0]);
+    if (k > 0 && k < n / 2)
+      tr.in[p * tr.stride + tr.slot(n - k)] = make_float2(ev[0][0] + ev[1][1], -ev[0][1] + ev[1][0]);
+  }
+  __syncthreads();
+  const float2* z = tr.template transform<true>(np);
+  const int full = tl >= 0 ? n + hop * (Tb - 1) : INT_MAX;
+  const float inv_n = 1.0f / (float)n;
+  for (int s = a + threadIdx.x; s < e; s += blockDim.x) {
+    float acc = 0.f, env = 0.f;
+    if (s < full) {
+      const int t_lo = max(t_min, (s >= n) ? (s - n) / hop + 1 : 0);
+      const int t_hi = min(t_max, s / hop);
+      for (int t = t_lo; t <= t_hi; ++t) {
+        const int i = s - t * hop;
+        const int q = t - pb;
+        const float2 v = z[(q >> 1) * tr.stride + i];
+        const float w = tr.win[i];
+        acc += ((q & 1) ? v.y : v.x) * inv_n * w;
+        env += w * w;
+      }
+    }
+    const float y = (env > 1e-11f) ? acc / env : 0.f;
+    out[s - n / 2 - x_lo] = y;
+  }
+}
+
+static int stream_np_max(int n_fft, int hop) { return istft_np_max(n_fft, hop) + 1; }
+
+int stream_dsp_check(int n_fft, int hop, int win_length) {
+  FSN_REQUIRE(is_pow2(n_fft) && n_fft >= 16 && n_fft <= 2048, FSN_ERR_UNSUPPORTED,
+              "stream: n_fft=%d: streaming is built for the power-of-two (radix-2) transform in [16, 2048]", n_fft);
+  FSN_REQUIRE(hop > 0 && hop <= n_fft && win_length > 0 && win_length <= n_fft, FSN_ERR_SHAPE,
+              "stream: bad hop/win_length");
+  FSN_REQUIRE(Radix2::smem_bytes(n_fft, stream_np_max(n_fft, hop)) <= kSmemOptin, FSN_ERR_UNSUPPORTED,
+              "stream: n_fft=%d with hop=%d needs too much shared memory", n_fft, hop);
+  return FSN_OK;
+}
+
+int stft_stream_launch(const float* win, int Wn, int Hs, const int* pos0, const int* tail, int B, int n_fft, int hop,
+                       int win_length, int c, int S, int Q, float* magT, float* spec, cudaStream_t st) {
+  return dsp_launch(stft_stream_kernel<Radix2>, dim3(cdiv(S + 1, kFR), B), Radix2::smem_bytes(n_fft, kFR / 2), st,
+                    "stft_stream_kernel", win, Wn, Hs, pos0, tail, n_fft, hop, win_length, c, S, Q, magT, spec);
+}
+
+int istft_stream_launch(const float* spec, const float* crm, const int* pos0, const int* act0, const int* tail, int B,
+                        int K, int D, int n_fft, int hop, int win_length, int c, int la, int Rc, int Q, int S, float* wav,
+                        cudaStream_t st) {
+  const int seg = kFR * hop, np_max = stream_np_max(n_fft, hop);
+  return dsp_launch(istft_stream_kernel<Radix2>, dim3(cdiv(K * hop + D, seg) + 1, B), Radix2::smem_bytes(n_fft, np_max),
+                    st, "istft_stream_kernel", spec, crm, pos0, act0, tail, K, D, n_fft, hop, win_length, seg, np_max, c,
+                    la, Rc, Q, S, wav);
 }
 
 }  // namespace fsn

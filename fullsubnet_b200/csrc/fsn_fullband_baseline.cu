@@ -153,3 +153,172 @@ extern "C" int fsn_fullband_enhance(const fsn_fullband_desc* d, const fsn_lstm_l
     return rc;
   return wav_epilogue(e, enhanced, B, L_max, pcm, gain, crm_out, d->num_freqs, T, hop, st);
 }
+
+// ---- chunked streaming (DESIGN 4.14).  Slot state block, floats: meta (4), sample history Hs, spectrum Q x 2F, cRM
+// Rc x 2F, then h and c of every layer (num_layers x H each); each section starts on 16 bytes, blocks 256 bytes apart.
+namespace fsn {
+
+struct FbbStreamLayout { size_t hist, spec, crm, h, c, slot; };
+
+static FbbStreamLayout fbb_stream_layout(const fsn_fullband_desc* d, const StreamGeom& g) {
+  const size_t F2 = 2 * (size_t)d->num_freqs, nH = (size_t)d->num_layers * d->hidden;
+  FbbStreamLayout s;
+  size_t o = sizeof(StreamMeta);
+  s.hist = o; o = align_up(o + (size_t)g.Hs * 4, 16);
+  s.spec = o; o = align_up(o + (size_t)g.Q * F2 * 4, 16);
+  s.crm = o;  o = align_up(o + (size_t)g.Rc * F2 * 4, 16);
+  s.h = o;    o = align_up(o + nH * 4, 16);
+  s.c = o;    o = align_up(o + nH * 4, 16);
+  s.slot = align_up(o, 256);
+  return s;
+}
+
+static int fbb_stream_check(const fsn_fullband_desc* d, int n_fft, int hop, int win_length, StreamGeom& g) {
+  int rc = fbb_check(d, 1, 1);
+  if (rc) return rc;
+  FSN_REQUIRE(d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE || d->norm_type == FSN_NORM_FORGETTING, FSN_ERR_UNSUPPORTED,
+              "fullband_stream: the offline norm needs the whole clip; streaming is built for cumulative_laplace_norm and "
+              "forgetting_norm");
+  FSN_REQUIRE(n_fft / 2 + 1 == d->num_freqs, FSN_ERR_SHAPE, "fullband_stream: n_fft/2+1 = %d != num_freqs = %d",
+              n_fft / 2 + 1, d->num_freqs);
+  return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
+}
+
+struct FbbStreamWs {
+  int *pos0, *act0, *tail;
+  float *wav, *magT, *spec, *scale, *y, *crm;
+  float2* fs;
+  float *h[SEQ_MAX_LAYERS], *c[SEQ_MAX_LAYERS], *hall[2];
+  size_t bytes;
+};
+
+// S = K + E steps: a call with a clip's last chunk runs E steps past the K of the others
+static void fbb_stream_carve(const fsn_fullband_desc* d, const StreamGeom& g, int B, int K, void* base, FbbStreamWs& w) {
+  Carver c(base);
+  const size_t F = d->num_freqs, H = d->hidden, S = (size_t)K + g.E;
+  w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B);
+  w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
+  w.magT = c.take<float>(B * S * F);
+  w.spec = c.take<float>(B * ((size_t)g.Q + S) * 2 * F);
+  w.fs = c.take<float2>(B * S);
+  w.scale = c.take<float>(S * B);
+  for (int l = 0; l < d->num_layers; ++l) { w.h[l] = c.take<float>(B * H); w.c[l] = c.take<float>(B * H); }
+  w.hall[0] = c.take<float>(B * S * H); w.hall[1] = c.take<float>(B * S * H);
+  w.y = c.take<float>(B * S * 2 * F);
+  w.crm = c.take<float>(B * ((size_t)g.Rc + S) * 2 * F);
+  w.bytes = c.off;
+}
+
+}  // namespace fsn
+
+extern "C" size_t fsn_fullband_stream_state_bytes(const fsn_fullband_desc* d, int B, int n_fft, int hop) {
+  StreamGeom g;
+  if (fbb_stream_check(d, n_fft, hop, n_fft, g)) return 0;
+  if (B <= 0) { set_error("fullband_stream: B=%d slots", B); last_error_code() = FSN_ERR_SHAPE; return 0; }
+  return fbb_stream_layout(d, g).slot * (size_t)B;
+}
+
+extern "C" size_t fsn_fullband_stream_workspace_bytes(const fsn_fullband_desc* d, int B, int K_max, int n_fft, int hop) {
+  StreamGeom g;
+  if (fbb_stream_check(d, n_fft, hop, n_fft, g)) return 0;
+  if (B <= 0 || K_max <= 0) {
+    set_error("fullband_stream: B=%d slots, K_max=%d hops", B, K_max);
+    last_error_code() = FSN_ERR_SHAPE;
+    return 0;
+  }
+  FbbStreamWs w;
+  fbb_stream_carve(d, g, B, K_max, nullptr, w);
+  return w.bytes;
+}
+
+extern "C" int fsn_fullband_stream_delay(const fsn_fullband_desc* d, int n_fft, int hop) {
+  StreamGeom g;
+  const int rc = fbb_stream_check(d, n_fft, hop, n_fft, g);
+  return rc ? -rc : g.D;
+}
+
+extern "C" int fsn_fullband_stream_step(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,
+                                        const float* fc_b, const float* wav, const int32_t* start, const int32_t* tail,
+                                        int B, int K, int n_fft, int hop, int win_length, float* enhanced, void* state,
+                                        size_t state_bytes, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  StreamGeom g;
+  int rc = fbb_stream_check(d, n_fft, hop, win_length, g);
+  if (rc) return rc;
+  FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "fullband_stream: B=%d slots, K=%d hops", B, K);
+  FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "fullband_stream: B=%d slots, at most 65535", B);
+  FSN_REQUIRE((long long)K * hop + g.D < (1 << 30), FSN_ERR_SHAPE, "fullband_stream: K=%d hops too long", K);
+  FSN_REQUIRE(layers && fc_w && fc_b && wav && enhanced, FSN_ERR_SHAPE, "fullband_stream: null argument");
+  bool any_tail = false;
+  for (int b = 0; tail && b < B; ++b) {
+    FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * hop, FSN_ERR_SHAPE,
+                "fullband_stream: tail[%d] = %d, outside [0, K*hop] = [0, %d] and not -1", b, tail[b], K * hop);
+    any_tail |= tail[b] >= 0;
+  }
+  const FbbStreamLayout sl = fbb_stream_layout(d, g);
+  FSN_REQUIRE(state && state_bytes >= sl.slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
+              state_bytes, sl.slot * (size_t)B);
+  FbbStreamWs w;
+  fbb_stream_carve(d, g, B, K, workspace, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, w.bytes);
+  // laid out for K + E steps from the workspace's start (a workspace queried for a larger K_max also fits); a call
+  // without a clip's last chunk runs S = K steps and strides its buffers by S
+  const cudaStream_t st = (cudaStream_t)stream;
+  char* sb = (char*)state;
+  const size_t ss = sl.slot;
+  const int F = d->num_freqs, H = d->hidden, n = d->num_layers, S = K + (any_tail ? g.E : 0);
+  const int Kh = K * hop, Wn = g.Hs + Kh;
+  const size_t F2 = 2 * (size_t)F;
+  if ((rc = stream_prologue(start, tail, B, sb, ss, w.pos0, w.act0, w.tail, st))) return rc;
+  // samples: the carried history, then the chunk
+  if ((rc = copy_rows(w.wav, (size_t)Wn * 4, sb + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
+  // spectrum: the carried Q frames, then the S frames of this call
+  if ((rc = copy_rows(w.spec, (g.Q + S) * F2 * 4, sb + sl.spec, ss, g.Q * F2 * 4, B, st))) return rc;
+  if ((rc = stft_stream_launch(w.wav, Wn, g.Hs, w.pos0, w.tail, B, n_fft, hop, win_length, g.c, S, g.Q, w.magT, w.spec,
+                               st)))
+    return rc;
+  // first norm (fbb_core): frame sums, then the running scale of each step
+  if ((rc = frame_stats_launch(w.magT, B, S, F, 0, (size_t)S * F, F, w.fs, st))) return rc;
+  if ((rc = stream_norm_launch(w.fs, B, S, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale, st))) return rc;
+  // the stack, layer by layer, on the per-step kernels seq_stack_forward runs for the causal norms; (h, c) of each layer
+  // start from the slot's state and are stored back after step K - 1
+  for (int l = 0; l < n; ++l) {
+    float* hl = w.hall[l & 1];
+    const size_t hrow = (size_t)S * H;
+    if ((rc = copy_rows(w.h[l], (size_t)H * 4, sb + sl.h + (size_t)l * H * 4, ss, (size_t)H * 4, B, st))) return rc;
+    if ((rc = copy_rows(w.c[l], (size_t)H * 4, sb + sl.c + (size_t)l * H * 4, ss, (size_t)H * 4, B, st))) return rc;
+    for (int j = 0; j < S; ++j) {
+      float* hp = j ? hl + (size_t)(j - 1) * H : w.h[l];
+      if (j <= g.c && (rc = stream_reset_launch(w.pos0, B, g, j, H, hp, j ? hrow : (size_t)H, w.c[l], st))) return rc;
+      StepParams p;
+      memset(&p, 0, sizeof(p));
+      p.R = B; p.H = H; p.first = 0; p.gru = 0;
+      p.w_ih = layers[l].w_ih; p.w_hh = layers[l].w_hh; p.b_ih = layers[l].b_ih; p.b_hh = layers[l].b_hh;
+      p.K0 = l ? H : F;
+      p.x0 = l ? w.hall[(l - 1) & 1] + (size_t)j * H : w.magT + (size_t)j * F;
+      p.x0_row_stride = (size_t)S * p.K0;
+      p.row_scale = l ? nullptr : w.scale + (size_t)j * B;
+      p.h_prev = hp; p.h_prev_stride = j ? hrow : (size_t)H;
+      p.h_out = hl + (size_t)j * H; p.h_out_stride = hrow;
+      p.c = w.c[l];
+      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+      if (j == K - 1) {
+        if ((rc = copy_rows(sb + sl.h + (size_t)l * H * 4, ss, p.h_out, hrow * 4, (size_t)H * 4, B, st))) return rc;
+        if ((rc = copy_rows(sb + sl.c + (size_t)l * H * 4, ss, w.c[l], (size_t)H * 4, (size_t)H * 4, B, st))) return rc;
+      }
+    }
+  }
+  if ((rc = fc_gemm_launch(w.hall[(n - 1) & 1], fc_w, fc_b, w.y, B * S, H, 2 * F, d->activation, st))) return rc;
+  // cRM: the carried Rc frames, then step j's output as frame pos0/hop - c + j - la
+  if ((rc = copy_rows(w.crm, (g.Rc + S) * F2 * 4, sb + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.crm + g.Rc * F2, (g.Rc + S) * F2 * 4, w.y, S * F2 * 4, S * F2 * 4, B, st))) return rc;
+  if ((rc = istft_stream_launch(w.spec, w.crm, w.pos0, w.act0, w.tail, B, K, g.D, n_fft, hop, win_length, g.c, g.la, g.Rc,
+                                g.Q, S, enhanced, st)))
+    return rc;
+  // carry what the next call reads: the windows as of step K
+  if ((rc = copy_rows(sb + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(sb + sl.spec, ss, w.spec + K * F2, (g.Q + S) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
+  return copy_rows(sb + sl.crm, ss, w.crm + K * F2, (g.Rc + S) * F2 * 4, g.Rc * F2 * 4, B, st);
+}

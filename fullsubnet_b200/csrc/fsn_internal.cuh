@@ -483,6 +483,36 @@ struct SeqStackWs {
 void seq_stack_carve(Carver& c, const SeqStack& s, SeqStackWs& w);
 int seq_stack_forward(const SeqStack& s, const SeqStackWs& w, cudaStream_t st);
 
+// ---- chunked streaming (DESIGN 4.14).  Per (n_fft, hop, look_ahead): c = ceil((n/2) / hop) steps of framing lag (a
+// step's frame and its pair partner are complete c hops before the chunk ends), the delay D = n/2 + (la + 1 + c) hop,
+// Hs samples of history, Rc cRM frames and Q = Rc + la spectrum frames carried per slot, E extra steps on a clip's
+// last call (its last frames, the look-ahead pad and the lag).
+struct StreamGeom { int n, hop, la, c, D, Hs, Rc, Q, E; };
+int stream_geom(int n_fft, int hop, int win_length, int la, StreamGeom& g);
+// per-slot bookkeeping at the start of each slot's state block
+struct StreamMeta { int pos, active; float acc; int pad; };
+// host (start, tail) tables -> the call's device tables pos0 / act0 / tail (slot b: samples before the call, whether a
+// clip is running, tail or -1), re-initialising the meta of slots that start; the tables travel in kernel parameters
+int stream_prologue(const int32_t* start, const int32_t* tail, int B, char* state, size_t slot_bytes, int* pos0, int* act0,
+                    int* tail_dev, cudaStream_t st);
+// first norm of the causal norms over the call's S steps: scaleT [S, B] from the frame sums fs [B, S] and the carried
+// accumulator (cumulative: running sum, forgetting: mu), frames counted from the clip start; the meta of active slots
+// then advances by K steps (pos += K hop, accumulator after step K-1, inactive after a tail)
+int stream_norm_launch(const float2* fs, int B, int S, int K, int F, const StreamGeom& g, int norm_type, const int* pos0,
+                       const int* act0, const int* tail, char* state, size_t slot_bytes, float* scaleT, cudaStream_t st);
+// before step j: zero h [B rows h_row apart, H] and c [B, H] of the slots whose step j is their clip's frame 0
+int stream_reset_launch(const int* pos0, int B, const StreamGeom& g, int j, int H, float* h, size_t h_row, float* c,
+                        cudaStream_t st);
+// signal layer of the streaming calls (fsn_dsp.cu), power-of-two n_fft only
+int stream_dsp_check(int n_fft, int hop, int win_length);
+int stft_stream_launch(const float* win, int Wn, int Hs, const int* pos0, const int* tail, int B, int n_fft, int hop,
+                       int win_length, int c, int S, int Q, float* magT, float* spec, cudaStream_t st);
+int istft_stream_launch(const float* spec, const float* crm, const int* pos0, const int* act0, const int* tail, int B,
+                        int K, int D, int n_fft, int hop, int win_length, int c, int la, int Rc, int Q, int S, float* wav,
+                        cudaStream_t st);
+// rows of `width` bytes: dst row b (pitch dp) <- src row b (pitch sp), B rows, on the stream
+int copy_rows(void* dst, size_t dp, const void* src, size_t sp, size_t width, int B, cudaStream_t st);
+
 // tensor-core sub-band stack (fsn_subband_tc.cu)
 struct SbTcArgs {
   const void* packed;       // tile-ordered fp16 weights (fsn_pack_sb_weights / sb_tc_pack_raw)

@@ -1,0 +1,119 @@
+// Chunked streaming (DESIGN 4.14): the per-slot bookkeeping, the causal first norm with a carried accumulator and the
+// recurrent-state reset of a clip's first frame.  The signal layer's streaming kernels are in fsn_dsp.cu; the model
+// orchestration and the entry points beside each model's enhance call.
+#include <string.h>
+
+#include "fsn_internal.cuh"
+
+namespace fsn {
+
+int stream_geom(int n_fft, int hop, int win_length, int la, StreamGeom& g) {
+  int rc = stream_dsp_check(n_fft, hop, win_length);
+  if (rc) return rc;
+  FSN_REQUIRE(la >= 0, FSN_ERR_SHAPE, "stream: look_ahead %d", la);
+  g.n = n_fft; g.hop = hop; g.la = la;
+  g.c = cdiv(n_fft / 2, hop);
+  g.D = n_fft / 2 + (la + 1 + g.c) * hop;
+  g.Hs = (g.c + 1) * hop + n_fft / 2;
+  g.Rc = cdiv(n_fft, hop) + 2;
+  g.Q = g.Rc + la;
+  g.E = 1 + la + g.c;
+  return FSN_OK;
+}
+
+constexpr int kStreamChunk = 500;  // 4 KB parameter block with the two counts
+struct StreamChunk { int off, n; int start[kStreamChunk], tail[kStreamChunk]; };
+
+__global__ void stream_prologue_kernel(const __grid_constant__ StreamChunk c, char* __restrict__ state, size_t slot_bytes,
+                                       int* __restrict__ pos0, int* __restrict__ act0, int* __restrict__ tail) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.n) return;
+  const int b = c.off + i;
+  StreamMeta* m = reinterpret_cast<StreamMeta*>(state + (size_t)b * slot_bytes);
+  if (c.start[i]) { m->pos = 0; m->active = 1; m->acc = 0.f; }
+  pos0[b] = m->pos;
+  act0[b] = m->active;
+  tail[b] = m->active ? c.tail[i] : -1;
+}
+
+int stream_prologue(const int32_t* start, const int32_t* tail, int B, char* state, size_t slot_bytes, int* pos0, int* act0,
+                    int* tail_dev, cudaStream_t st) {
+  StreamChunk c;
+  for (int off = 0; off < B; off += kStreamChunk) {
+    c.off = off;
+    c.n = B - off < kStreamChunk ? B - off : kStreamChunk;
+    for (int i = 0; i < c.n; ++i) {
+      c.start[i] = start ? start[off + i] != 0 : 0;
+      c.tail[i] = tail ? tail[off + i] : -1;
+    }
+    stream_prologue_kernel<<<cdiv(c.n, 128), 128, 0, st>>>(c, state, slot_bytes, pos0, act0, tail_dev);
+    FSN_CHECK_LAUNCH("stream_prologue_kernel");
+  }
+  return FSN_OK;
+}
+
+// the arithmetic of cum_clip_scale_kernel / forget_scale_kernel (first norm), frame m of the clip at step j
+__global__ void stream_norm_kernel(const float2* __restrict__ fs, int B, int S, int K, int F, int hop, int c, int fgt,
+                                   const ForgetCoef cf, float eps, const int* __restrict__ pos0, const int* __restrict__ act0,
+                                   const int* __restrict__ tail, char* __restrict__ state, size_t slot_bytes,
+                                   float* __restrict__ scaleT) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  StreamMeta* mt = reinterpret_cast<StreamMeta*>(state + (size_t)b * slot_bytes);
+  const int m0 = pos0[b] / hop - c;
+  float acc = mt->acc, acc_k = acc;
+  for (int j = 0; j < S; ++j) {
+    const int m = m0 + j;
+    float sc = 1.f;
+    if (m >= 0) {
+      const float s = fs[(size_t)b * S + j].x;
+      if (fgt) {
+        const float mean = __fdiv_rn(s, (float)F);
+        const int i = m < FORGET_LEN ? m : FORGET_LEN;
+        acc = __fadd_rn(__fmul_rn(cf.a[i], acc), __fmul_rn(cf.b[i], mean));
+        sc = __fdiv_rn(1.0f, __fadd_rn(acc, FORGET_EPS));
+      } else {
+        acc += s;
+        sc = 1.0f / (acc / ((float)F * (float)(m + 1)) + eps);
+      }
+    }
+    scaleT[(size_t)j * B + b] = sc;
+    if (j == K - 1) acc_k = acc;
+  }
+  if (act0[b]) {
+    mt->acc = acc_k;
+    mt->pos = pos0[b] + K * hop;
+    mt->active = tail[b] < 0;
+  }
+}
+
+int stream_norm_launch(const float2* fs, int B, int S, int K, int F, const StreamGeom& g, int norm_type, const int* pos0,
+                       const int* act0, const int* tail, char* state, size_t slot_bytes, float* scaleT, cudaStream_t st) {
+  stream_norm_kernel<<<cdiv(B, 64), 64, 0, st>>>(fs, B, S, K, F, g.hop, g.c, norm_type == FSN_NORM_FORGETTING, forget_coef(),
+                                                 1.1920928955078125e-07f, pos0, act0, tail, state, slot_bytes, scaleT);
+  FSN_CHECK_LAUNCH("stream_norm_kernel");
+  return FSN_OK;
+}
+
+__global__ void stream_reset_kernel(const int* __restrict__ pos0, int B, int hop, int c, int j, int H, float* __restrict__ h,
+                                    size_t h_row, float* __restrict__ cs) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * H) return;
+  const int b = i / H, u = i - b * H;
+  if (pos0[b] / hop - c + j != 0) return;
+  h[(size_t)b * h_row + u] = 0.f;
+  cs[i] = 0.f;
+}
+
+int stream_reset_launch(const int* pos0, int B, const StreamGeom& g, int j, int H, float* h, size_t h_row, float* c,
+                        cudaStream_t st) {
+  stream_reset_kernel<<<cdiv(B * H, 256), 256, 0, st>>>(pos0, B, g.hop, g.c, j, H, h, h_row, c);
+  FSN_CHECK_LAUNCH("stream_reset_kernel");
+  return FSN_OK;
+}
+
+int copy_rows(void* dst, size_t dp, const void* src, size_t sp, size_t width, int B, cudaStream_t st) {
+  return check_cuda(cudaMemcpy2DAsync(dst, dp, src, sp, width, (size_t)B, cudaMemcpyDeviceToDevice, st), "stream copy");
+}
+
+}  // namespace fsn

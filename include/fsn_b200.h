@@ -438,6 +438,44 @@ int fsn_fullband_enhance(const fsn_fullband_desc* d, const fsn_lstm_layer* layer
                          float* enhanced, float* crm_out, int16_t* pcm, float gain, void* workspace,
                          size_t workspace_bytes, fsn_stream_t stream);
 
+/* Chunked streaming enhancement of fullband_baseline (DESIGN 4.14): many streams, each advanced by K hops per call, with
+ * the output of every clip bit-identical to fsn_fullband_enhance on the whole clip (lengths NULL, B = 1).  Appended in
+ * ABI version 102.
+ *
+ * A stream state is a caller-allocated device buffer of B slots, fsn_fullband_stream_state_bytes(d, B, n_fft, hop)
+ * bytes, ZERO-FILLED before its first use (every slot then holds no clip).  Slot b's state is the contiguous block of
+ * state_bytes / B bytes at b * state_bytes / B, so checkpointing or moving a stream is a device copy of its block.  A
+ * block holds: the slot's position and whether a clip runs (16 bytes); the last (c+1) hop + n_fft/2 input samples; the
+ * spectrum of the last Rc + look_ahead frames and the cRM of the last Rc frames (Rc = ceil(n_fft/hop) + 2); the norm's
+ * accumulator (cumulative: running frame sum, forgetting: mu); h and c of every LSTM layer (2 x num_layers x hidden
+ * floats).  Here c = ceil((n_fft/2) / hop).
+ *
+ * fsn_fullband_stream_step: wav [B, K*hop], the next K hops of every slot.  start / tail: HOST int32 [B], nullable,
+ * copied through kernel parameters (not retained):
+ *   start[b] != 0  slot b begins a new clip with this chunk (its state is re-initialised inside the call);
+ *   tail[b] >= 0   slot b's clip ends after tail[b] <= K*hop samples of this chunk; the slot is free afterwards.
+ *                  -1: the clip goes on.  Anything else -> FSN_ERR_SHAPE.  Ignored on a slot without a clip.
+ * enhanced [B, K*hop + D]: for a slot whose clip is at sample pos before the call, the first K*hop samples of its row
+ * are clip samples [pos - D, pos - D + K*hop) (negative indices as 0) and the rest 0; on the call that ends the clip,
+ * the row holds clip samples [pos - D, pos + tail[b]) and 0 after them.  A slot without a clip gets a row of 0.
+ * D = fsn_fullband_stream_delay(d, n_fft, hop) = n_fft/2 + (look_ahead + 1 + c) hop samples, the same for every K and
+ * schedule (a negative return is minus the FSN_ERR_* code).  A clip must have more than n_fft/2 samples and at most
+ * 2^30 (18.6 h at 16 kHz): the position is an int32 sample count.  The call cannot check either (the position lives on
+ * the device); a shorter clip reflects at a clamped index and a longer one wraps, so the output of such a clip is
+ * undefined, and the other slots are unaffected.  B > 65535 slots -> FSN_ERR_UNSUPPORTED.
+ * The workspace is fsn_fullband_stream_workspace_bytes(d, B, K_max, n_fft, hop) bytes; it serves every K <= K_max.
+ * Built for the cumulative_laplace_norm and forgetting_norm models, LSTM cell, FSN_PREC_FP32, power-of-two n_fft in
+ * [16, 2048]; the offline norm (it needs the whole clip), the GRU cell, other precisions and other n_fft ->
+ * FSN_ERR_UNSUPPORTED before any CUDA call, from the queries (which return 0) as from the call.  Never allocates,
+ * never synchronises the host; one call may be captured in a CUDA graph. */
+size_t fsn_fullband_stream_state_bytes(const fsn_fullband_desc* d, int B, int n_fft, int hop);
+size_t fsn_fullband_stream_workspace_bytes(const fsn_fullband_desc* d, int B, int K_max, int n_fft, int hop);
+int fsn_fullband_stream_delay(const fsn_fullband_desc* d, int n_fft, int hop);
+int fsn_fullband_stream_step(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,
+                             const float* fc_b, const float* wav, const int32_t* start, const int32_t* tail, int B, int K,
+                             int n_fft, int hop, int win_length, float* enhanced, void* state, size_t state_bytes,
+                             void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+
 /* Training step of recipes/dns_interspeech_2020/fullband_baseline/trainer.py:32-71, same conventions as fsn_train_*: the
  * caller allocates the workspace and passes the same untouched buffer from forward to backward; the gradients of all
  * 4 * num_layers + 2 parameters are OVERWRITTEN; no host synchronisation; arguments are checked before any CUDA call;
