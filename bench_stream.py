@@ -1,8 +1,11 @@
-"""Chunked streaming throughput of fullband_baseline (fsn_fullband_stream_step): ms per call, audio seconds enhanced per
-wall second and concurrent real-time streams for slots x K, with the whole-clip fsn_fullband_enhance rate of the same
-process beside it.  Prints one JSON line per configuration and a header line with the GPU, power limit and clocks.
+"""Chunked streaming throughput of fullband_baseline (fsn_fullband_stream_step) or fast_fullsubnet (fsn_fast_stream_step,
+--model fast_fullsubnet): ms per call, audio seconds enhanced per wall second and concurrent real-time streams for
+slots x K, with the whole-clip fp32 rate of the same process beside it (fsn_fullband_enhance; fast_fullsubnet:
+Inferencer.enhance_batch).  For fast_fullsubnet each line also gives the bottleneck's share of the call's GPU time, from
+a torch.profiler pass of its own after the timed calls.  Prints one JSON line per configuration and a header line with
+the GPU, power limit and clocks.
 
-    python bench_stream.py [--slots 1 64 256] [--ks 1 4 16 64] [--calls 20] [--warmup 3]"""
+    python bench_stream.py [--model fullband_baseline] [--slots 1 64 256] [--ks 1 4 16 64] [--calls 20] [--warmup 3]"""
 from __future__ import annotations
 
 import argparse
@@ -24,13 +27,43 @@ def gpu_info():
         return {"error": str(e)}
 
 
-def model(norm, dev):
+def model(name, norm, dev):
+    if name == "fast_fullsubnet":
+        from fullsubnet_b200.fast_fullsubnet.model import Model
+        from oracle import fast_fullsubnet_oracle as FO
+        args = dict(FO.DEFAULT_FAST_ARGS, norm_type=norm)
+        m = Model(**args, precision="fp32")
+        m.load_state_dict(FO.make_fast_state_dict(seed=11, args=args), strict=True)
+        return m.to(dev).eval()
     from fullsubnet_b200.fullband_baseline.model import Model
     from oracle import fullband_baseline_oracle as BO
     args = dict(BO.DEFAULT_FBB_ARGS, norm_type=norm)
     m = Model(**args)
     m.load_state_dict(BO.make_fbb_state_dict(seed=11, args=args), strict=True)
     return m.to(dev).eval()
+
+
+def bottleneck_share(step, calls=3):
+    """Share of the GPU time of `calls` streaming calls spent in fast_fullsubnet's bottleneck: the kernels and copies
+    from fast_stream_open_kernel up to fast_stream_dec_input_kernel, over all of them."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            step()
+        torch.cuda.synchronize()
+    evs = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA),
+                 key=lambda e: e.time_range.start)
+    total = inside = 0.0
+    on = False
+    for e in evs:
+        if "fast_stream_open_kernel" in e.name:
+            on = True
+        elif "fast_stream_dec_input_kernel" in e.name:
+            on = False
+        d = e.time_range.elapsed_us()
+        total += d
+        inside += d if on else 0.0
+    return round(inside / total, 3) if total > 0 else None
 
 
 def time_ms(fn, calls, warmup):
@@ -53,12 +86,14 @@ def main():
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--norm", default="cumulative_laplace_norm")
+    ap.add_argument("--model", default="fullband_baseline", choices=["fullband_baseline", "fast_fullsubnet"])
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_stream.py needs a CUDA device"
     dev = torch.device("cuda:0")
     from fullsubnet_b200.stream import Streamer
-    m = model(a.norm, dev)
-    print(json.dumps({"gpu": gpu_info(), "model": "fullband_baseline", "precision": "fp32", "norm": a.norm}))
+    fast = a.model == "fast_fullsubnet"
+    m = model(a.model, a.norm, dev)
+    print(json.dumps({"gpu": gpu_info(), "model": a.model, "precision": "fp32", "norm": a.norm}))
     g = torch.Generator(device="cpu").manual_seed(0)
     for slots in a.slots:
         s = Streamer(m, slots)
@@ -69,13 +104,22 @@ def main():
             chunk_ms = 1000.0 * K * HOP / SR
             audio_rate = slots * chunk_ms / ms
             rt = slots if ms <= chunk_ms else int(slots * chunk_ms / ms)
-            print(json.dumps({"slots": slots, "K": K, "ms_per_call": round(ms, 3), "chunk_ms": chunk_ms,
-                              "audio_s_per_s": round(audio_rate, 1), "realtime_streams": rt, "delay": s.delay}))
+            line = {"slots": slots, "K": K, "ms_per_call": round(ms, 3), "chunk_ms": chunk_ms,
+                    "audio_s_per_s": round(audio_rate, 1), "realtime_streams": rt, "delay": s.delay}
+            if fast:
+                line["all_realtime"] = ms <= chunk_ms
+                line["bottleneck_share"] = bottleneck_share(lambda: s.step(x))
+            print(json.dumps(line))
         del s
         torch.cuda.empty_cache()
+    if fast:
+        from fullsubnet_b200.inferencer import Inferencer
+        whole = Inferencer(model=m, device=dev).enhance_batch
+    else:
+        whole = m.enhance
     for B in (1, 64):
         y = (0.1 * torch.randn(B, 4 * SR, generator=g)).to(dev)
-        ms = time_ms(lambda: m.enhance(y), max(3, a.calls // 4), a.warmup)
+        ms = time_ms(lambda: whole(y), max(3, a.calls // 4), a.warmup)
         print(json.dumps({"whole_clip": True, "B": B, "clip_s": 4.0, "ms_per_call": round(ms, 3),
                           "audio_s_per_s": round(B * 4000.0 / ms, 1)}))
 

@@ -220,3 +220,409 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   if ((rc = seq_stack_forward(dec, w.seq, st))) return rc;
   return crm_output_launch(w.dec_out, (size_t)Tp * 2 * F, 2 * F, B, Tp, F, d->look_ahead, out, st);
 }
+
+// ---- chunked streaming (DESIGN 4.14).  Slot state block (each section on 16 bytes, blocks 256 bytes apart): meta (16
+// bytes), sample history Hs, spectrum Q x 2F, cRM Rc x 2F, the last S-1 frames of the mel spectrogram and of the encoder
+// output (M each), encoder (h | c) of both layers, the second norm's running sum and the latest bottleneck output of the
+// M rows, bottleneck (h | c) of both layers (M x Hb each), decoder (h | c) of both layers.
+namespace fsn {
+
+struct FastStreamLayout { size_t hist, spec, crm, mel, enc, eh, ec, run, bo, bh, bc, dh, dc, slot; };
+
+static FastStreamLayout fast_stream_layout(const fsn_fast_desc* d, const StreamGeom& g) {
+  const size_t F2 = 2 * (size_t)d->num_freqs, M = d->num_mels, Hm = d->shrink_size - 1;
+  const size_t He = (size_t)d->enc1_hidden + d->enc2_hidden, Hb = 2 * M * d->bn_hidden, Hd = 2 * (size_t)d->dec_hidden;
+  FastStreamLayout s;
+  size_t o = sizeof(StreamMeta);
+  auto sec = [&](size_t& at, size_t floats) { at = o; o = align_up(o + floats * 4, 16); };
+  sec(s.hist, g.Hs); sec(s.spec, g.Q * F2); sec(s.crm, g.Rc * F2);
+  sec(s.mel, Hm * M); sec(s.enc, Hm * M);
+  sec(s.eh, He); sec(s.ec, He);
+  sec(s.run, M); sec(s.bo, M);
+  sec(s.bh, Hb); sec(s.bc, Hb);
+  sec(s.dh, Hd); sec(s.dc, Hd);
+  s.slot = align_up(o, 256);
+  return s;
+}
+
+static int fast_stream_check(const fsn_fast_desc* d, int n_fft, int hop, int win_length, FastDims& m, StreamGeom& g) {
+  int rc = fast_dims(d, 1, 2, m);
+  if (rc) return rc;
+  FSN_REQUIRE(d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, FSN_ERR_UNSUPPORTED,
+              "fast_stream: the offline norm needs the whole clip; streaming is built for cumulative_laplace_norm");
+  FSN_REQUIRE(d->precision == FSN_PREC_FP32, FSN_ERR_UNSUPPORTED,
+              "fast_stream: streaming is built for FSN_PREC_FP32 (precision %d)", d->precision);
+  FSN_REQUIRE(n_fft / 2 + 1 == d->num_freqs, FSN_ERR_SHAPE, "fast_stream: n_fft/2+1 = %d != num_freqs = %d", n_fft / 2 + 1,
+              d->num_freqs);
+  return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
+}
+
+struct FastStreamWs {
+  int *pos0, *act0, *tail, *rst;
+  float *wav, *magT, *spec, *melT, *scale1, *encT, *catM, *catE, *bn, *scale2, *bo, *dec_in, *y, *crm, *pp;
+  float2* fs;
+  float *eh[2], *ec[2], *ehall[2];            // encoder state and layer outputs
+  float *bh0[2], *bh1[2], *bc0, *bc1;         // bottleneck state, h ping-pong per layer
+  float *dh[2], *dc[2], *dfh[2], *dfc[2], *dhall[2];  // decoder state (entering the call / after step K-1), outputs
+  unsigned int* barrier;
+  size_t bytes;
+};
+
+// St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others; nb = ceil(St / S) bottleneck
+// steps, the most block ends St consecutive frames can hold
+static void fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const StreamGeom& g, int B, int K, void* base,
+                              FastStreamWs& w) {
+  Carver c(base);
+  const size_t F = m.F, M = m.M, St = (size_t)K + g.E, Hm = m.S - 1, nb = cdiv((int)St, m.S), R = (size_t)B * M;
+  const size_t He0 = d->enc1_hidden, He1 = d->enc2_hidden, Hb = d->bn_hidden, Hd = d->dec_hidden;
+  w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B); w.rst = c.take<int>(B);
+  w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
+  w.magT = c.take<float>(B * St * F);
+  w.spec = c.take<float>(B * ((size_t)g.Q + St) * 2 * F);
+  w.melT = c.take<float>(B * St * M);
+  w.fs = c.take<float2>(B * St);
+  w.scale1 = c.take<float>(St * B);
+  for (int l = 0; l < 2; ++l) {
+    const size_t H = l ? He1 : He0;
+    w.eh[l] = c.take<float>(B * H); w.ec[l] = c.take<float>(B * H);
+    w.ehall[l] = c.take<float>(B * St * H);
+  }
+  w.encT = c.take<float>(B * St * M);
+  w.catM = c.take<float>(B * (Hm + St) * M);
+  w.catE = c.take<float>(B * (Hm + St) * M);
+  w.bn = c.take<float>(nb * R * m.K);
+  w.scale2 = c.take<float>(nb * R);
+  w.bo = c.take<float>(R * (nb + 1));
+  for (int i = 0; i < 2; ++i) { w.bh0[i] = c.take<float>(R * Hb); w.bh1[i] = c.take<float>(R * Hb); }
+  w.bc0 = c.take<float>(R * Hb); w.bc1 = c.take<float>(R * Hb);
+  w.dec_in = c.take<float>(B * St * 2 * M);
+  for (int l = 0; l < 2; ++l) {
+    w.dh[l] = c.take<float>(B * Hd); w.dc[l] = c.take<float>(B * Hd);
+    w.dfh[l] = c.take<float>(B * Hd); w.dfc[l] = c.take<float>(B * Hd);
+    w.dhall[l] = c.take<float>(B * St * Hd);
+  }
+  w.pp = c.take<float>((size_t)2 * 256 * Hd);  // fb::ROWS rows of the persistent kernel's h0 ping-pong
+  w.barrier = c.take<unsigned int>(64);
+  w.y = c.take<float>(B * St * 2 * F);
+  w.crm = c.take<float>(B * ((size_t)g.Rc + St) * 2 * F);
+  w.bytes = c.off;
+}
+
+// Block ends of slot b in the call: the steps j < St whose frame m0 + j is a multiple of S and >= 0 (block m/S, shrunk
+// step m/S of the whole clip, is complete at frame m).  First such step, and how many lie in [0, lim).
+__device__ __forceinline__ int fs_first_end(int m0, int S) {
+  const int m = m0 > 0 ? m0 : 0;
+  return (m + S - 1) / S * S - m0;
+}
+__device__ __forceinline__ int fs_ends_before(int jf, int S, int lim) { return lim > jf ? (lim - 1 - jf) / S + 1 : 0; }
+
+// Before the bottleneck: per slot b (grid.y), the bottleneck's h / c entering the call into h0p / h1p (the ping-pong
+// halves step 0 reads) and c0 / c1, zero when the clip's frame 0 is in the call (its first block end is block 0); the
+// latest bottleneck output into column 0 of bo [R, nb+1]; the decoder's restart step rst[b] (frame 0 at step rst).
+__global__ void fast_stream_open_kernel(const int* __restrict__ pos0, int hop, int c, int St, int M, int Hb, int nb,
+                                        const char* __restrict__ state, size_t slot_bytes, size_t bh, size_t bc, size_t bo_off,
+                                        float* __restrict__ h0p, float* __restrict__ h1p, float* __restrict__ c0,
+                                        float* __restrict__ c1, float* __restrict__ bo, int* __restrict__ rst) {
+  const int b = blockIdx.y;
+  const int m0 = pos0[b] / hop - c;
+  const bool fresh = m0 <= 0 && -m0 < St;
+  const size_t n = (size_t)M * Hb, o = (size_t)b * n;
+  const char* sb = state + (size_t)b * slot_bytes;
+  const float* sh = reinterpret_cast<const float*>(sb + bh);
+  const float* sc = reinterpret_cast<const float*>(sb + bc);
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
+    h0p[o + e] = fresh ? 0.f : sh[e];
+    h1p[o + e] = fresh ? 0.f : sh[n + e];
+    c0[o + e] = fresh ? 0.f : sc[e];
+    c1[o + e] = fresh ? 0.f : sc[n + e];
+  }
+  if (blockIdx.x == 0) {
+    const float* sbo = reinterpret_cast<const float*>(sb + bo_off);
+    for (int r = threadIdx.x; r < M; r += blockDim.x) bo[((size_t)b * M + r) * (nb + 1)] = sbo[r];
+    if (threadIdx.x == 0) rst[b] = -m0;
+  }
+}
+
+// Bottleneck input of the i-th block end of slot b (grid (nb, B)): fast_bn_input_kernel's arithmetic on the block's frames,
+// read from catM / catE [B, S-1+St, M] (the carried S-1 frames, then the call's), into bn [nb, B*M, K]; 0 past the slot's
+// last block end in the call
+__global__ void fast_stream_bn_input_kernel(const float* __restrict__ catM, const float* __restrict__ catE,
+                                            const int* __restrict__ pos0, int hop, int c, int St, int M, int Nn, int Ne,
+                                            int S, float* __restrict__ bn) {
+  const int i = blockIdx.x, b = blockIdx.y, B = gridDim.y;
+  const int K = (2 * Nn + 1) + (2 * Ne + 1);
+  const int m0 = pos0[b] / hop - c;
+  const int j = fs_first_end(m0, S) + i * S;
+  const bool ok = j < St;
+  const int len = (m0 + j == 0) ? 1 : S;  // block 0 is frame 0 alone (model.py real_time_downsampling)
+  const float inv = 1.0f / (float)len;
+  const size_t W = (size_t)(S - 1 + St);
+  const int q0 = S - 1 + j - (len - 1);  // first frame of the block in the cat rows
+  for (int idx = threadIdx.x; idx < M * K; idx += blockDim.x) {
+    const int mm = idx / K, k = idx - mm * K;
+    float v = 0.f;
+    if (ok) {
+      float acc = 0.f;
+      for (int q = q0; q < q0 + len; ++q) {
+        const size_t base = ((size_t)b * W + q) * M;
+        acc += (k < 2 * Nn + 1) ? catM[base + reflect_idx(mm + k - Nn, M)]
+                                : catE[base + reflect_idx(mm + (k - (2 * Nn + 1)) - Ne, M)];
+      }
+      v = acc * inv;
+    }
+    bn[((size_t)i * B * M + (size_t)b * M + mm) * K + k] = v;
+  }
+}
+
+// Second cumulative norm over the call's block ends: fast_cum_bn_scale_kernel's recurrence per row r = b*M + mm with the
+// running sum carried in the slot state (reset at block 0, stored as of the last block end before step K); scaleT [nb, R]
+__global__ void fast_stream_bn_scale_kernel(const float* __restrict__ bn, const int* __restrict__ pos0,
+                                            const int* __restrict__ act0, int hop, int c, int St, int K, int R, int M, int Kf,
+                                            int S, int nb, float eps, char* __restrict__ state, size_t slot_bytes,
+                                            size_t run_off, float* __restrict__ scaleT) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  const int b = r / M, mm = r - b * M;
+  float* srun = reinterpret_cast<float*>(state + (size_t)b * slot_bytes + run_off) + mm;
+  const int m0 = pos0[b] / hop - c, jf = fs_first_end(m0, S);
+  const int commit = act0[b] ? fs_ends_before(jf, S, K) - 1 : -1;
+  float run = *srun;
+  for (int i = 0; i < nb; ++i) {
+    const int j = jf + i * S;
+    float sc = 1.f;
+    if (j < St) {
+      const int ts = (m0 + j) / S;
+      if (ts == 0) run = 0.f;
+      const float* x = bn + ((size_t)i * R + r) * Kf;
+      float s = 0.f;
+      for (int k = 0; k < Kf; ++k) s += x[k];
+      run += s;
+      sc = 1.0f / (run / ((float)Kf * (float)(ts + 1)) + eps);
+    }
+    scaleT[(size_t)i * R + r] = sc;
+    if (i == commit) *srun = run;
+  }
+}
+
+// After bottleneck step i: the slots whose last block end before step K is their i-th store the bottleneck's (h, c) and
+// output (column i + 1 of bo) in their state
+__global__ void fast_stream_commit_kernel(const int* __restrict__ pos0, const int* __restrict__ act0, int hop, int c, int K,
+                                          int S, int M, int Hb, int nb, int i, const float* __restrict__ h0,
+                                          const float* __restrict__ h1, const float* __restrict__ c0,
+                                          const float* __restrict__ c1, const float* __restrict__ bo, char* __restrict__ state,
+                                          size_t slot_bytes, size_t bh, size_t bc, size_t bo_off) {
+  const int b = blockIdx.y;
+  if (!act0[b] || fs_ends_before(fs_first_end(pos0[b] / hop - c, S), S, K) - 1 != i) return;
+  const size_t n = (size_t)M * Hb, o = (size_t)b * n;
+  char* sb = state + (size_t)b * slot_bytes;
+  float* sh = reinterpret_cast<float*>(sb + bh);
+  float* sc = reinterpret_cast<float*>(sb + bc);
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
+    sh[e] = h0[o + e]; sh[n + e] = h1[o + e];
+    sc[e] = c0[o + e]; sc[n + e] = c1[o + e];
+  }
+  if (blockIdx.x == 0) {
+    float* sbo = reinterpret_cast<float*>(sb + bo_off);
+    for (int r = threadIdx.x; r < M; r += blockDim.x) sbo[r] = bo[((size_t)b * M + r) * (nb + 1) + i + 1];
+  }
+}
+
+// Decoder input (fast_dec_input_kernel's concatenation): dec_in [B, St, 2M] row (b, j) = encoder output of step j | the
+// bottleneck output of the latest block end at or before step j (column 0 of bo: the one carried into the call)
+__global__ void fast_stream_dec_input_kernel(const float* __restrict__ encT, const float* __restrict__ bo,
+                                             const int* __restrict__ pos0, int hop, int c, int B, int St, int M, int S, int nb,
+                                             float* __restrict__ dec_in) {
+  const size_t n = (size_t)B * St * 2 * M;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int col = (int)(i % (2 * M));
+    const size_t q = i / (2 * M);
+    const int b = (int)(q / St), j = (int)(q % St);
+    if (col < M) {
+      dec_in[i] = encT[q * M + col];
+    } else {
+      const int e = fs_ends_before(fs_first_end(pos0[b] / hop - c, S), S, j + 1);
+      dec_in[i] = bo[((size_t)b * M + (col - M)) * (nb + 1) + e];
+    }
+  }
+}
+
+}  // namespace fsn
+
+extern "C" size_t fsn_fast_stream_state_bytes(const fsn_fast_desc* d, int B, int n_fft, int hop) {
+  FastDims m;
+  StreamGeom g;
+  if (fast_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
+  if (B <= 0) { set_error("fast_stream: B=%d slots", B); last_error_code() = FSN_ERR_SHAPE; return 0; }
+  return fast_stream_layout(d, g).slot * (size_t)B;
+}
+
+extern "C" size_t fsn_fast_stream_workspace_bytes(const fsn_fast_desc* d, int B, int K_max, int n_fft, int hop) {
+  FastDims m;
+  StreamGeom g;
+  if (fast_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
+  if (B <= 0 || K_max <= 0) {
+    set_error("fast_stream: B=%d slots, K_max=%d hops", B, K_max);
+    last_error_code() = FSN_ERR_SHAPE;
+    return 0;
+  }
+  FastStreamWs w;
+  fast_stream_carve(d, m, g, B, K_max, nullptr, w);
+  return w.bytes;
+}
+
+extern "C" int fsn_fast_stream_delay(const fsn_fast_desc* d, int n_fft, int hop) {
+  FastDims m;
+  StreamGeom g;
+  const int rc = fast_stream_check(d, n_fft, hop, n_fft, m, g);
+  return rc ? -rc : g.D;
+}
+
+extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* wav,
+                                    const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
+                                    int win_length, float* enhanced, void* state, size_t state_bytes, void* workspace,
+                                    size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FastDims m;
+  StreamGeom g;
+  int rc = fast_stream_check(d, n_fft, hop, win_length, m, g);
+  if (rc) return rc;
+  FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "fast_stream: B=%d slots, K=%d hops", B, K);
+  FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "fast_stream: B=%d slots, at most 65535", B);
+  FSN_REQUIRE((long long)K * hop + g.D < (1 << 30), FSN_ERR_SHAPE, "fast_stream: K=%d hops too long", K);
+  FSN_REQUIRE(wt && wav && enhanced, FSN_ERR_SHAPE, "fast_stream: null argument");
+  bool any_tail = false;
+  for (int b = 0; tail && b < B; ++b) {
+    FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * hop, FSN_ERR_SHAPE,
+                "fast_stream: tail[%d] = %d, outside [0, K*hop] = [0, %d] and not -1", b, tail[b], K * hop);
+    any_tail |= tail[b] >= 0;
+  }
+  const FastStreamLayout sl = fast_stream_layout(d, g);
+  FSN_REQUIRE(state && state_bytes >= sl.slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
+              state_bytes, sl.slot * (size_t)B);
+  FastStreamWs w;
+  fast_stream_carve(d, m, g, B, K, workspace, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, w.bytes);
+  // laid out for K + E steps (a workspace queried for a larger K_max also fits); a call without a clip's last chunk runs
+  // St = K steps and strides its buffers by St
+  const cudaStream_t st = (cudaStream_t)stream;
+  char* sb = (char*)state;
+  const size_t ss = sl.slot;
+  const int F = m.F, M = m.M, S = m.S, Kf = m.K, Hm = S - 1, R = B * M;
+  const int St = K + (any_tail ? g.E : 0), nb = cdiv(St, S);
+  const int Hb = d->bn_hidden, Hd = d->dec_hidden;
+  const int Kh = K * hop, Wn = g.Hs + Kh;
+  const size_t F2 = 2 * (size_t)F, catw = (size_t)(Hm + St) * M * 4;
+  if ((rc = stream_prologue(start, tail, B, sb, ss, w.pos0, w.act0, w.tail, st))) return rc;
+  // samples: the carried history, then the chunk; spectrum: the carried Q frames, then the St frames of this call
+  if ((rc = copy_rows(w.wav, (size_t)Wn * 4, sb + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.spec, (g.Q + St) * F2 * 4, sb + sl.spec, ss, g.Q * F2 * 4, B, st))) return rc;
+  if ((rc = stft_stream_launch(w.wav, Wn, g.Hs, w.pos0, w.tail, B, n_fft, hop, win_length, g.c, St, g.Q, w.magT, w.spec,
+                               st)))
+    return rc;
+  // Mel filtering and the first norm over the mel frame sums (model.py:161-170)
+  if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, B * St, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true))) return rc;
+  if ((rc = frame_stats_launch(w.melT, B, St, M, 0, (size_t)St * M, M, w.fs, st))) return rc;
+  if ((rc = stream_norm_launch(w.fs, B, St, K, M, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale1, st))) return rc;
+  // encoder: the per-step kernels the whole-clip call runs for its per-step scale, (h, c) carried; Linear(M) + ReLU
+  const fsn_lstm_layer enc[2] = {wt->enc1, wt->enc2};
+  const int He[2] = {d->enc1_hidden, d->enc2_hidden};
+  if ((rc = stream_lstm_layers(enc, 2, He, M, w.melT, w.scale1, B, St, K, g, w.pos0, sb, ss, sl.eh, sl.ec, w.eh, w.ec,
+                               w.ehall, st)))
+    return rc;
+  if ((rc = fc_gemm_launch(w.ehall[1], wt->enc_fc_w, wt->enc_fc_b, w.encT, B * St, He[1], M, FSN_ACT_RELU, st))) return rc;
+  // the carried S-1 frames, then the call's, of the mel spectrogram and the encoder output: the frames the blocks average
+  if (Hm > 0) {
+    if ((rc = copy_rows(w.catM, catw, sb + sl.mel, ss, (size_t)Hm * M * 4, B, st))) return rc;
+    if ((rc = copy_rows(w.catE, catw, sb + sl.enc, ss, (size_t)Hm * M * 4, B, st))) return rc;
+  }
+  if ((rc = copy_rows(w.catM + (size_t)Hm * M, catw, w.melT, (size_t)St * M * 4, (size_t)St * M * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.catE + (size_t)Hm * M, catw, w.encT, (size_t)St * M * 4, (size_t)St * M * 4, B, st))) return rc;
+  // bottleneck: one step per block end, every row at its slot's i-th block end of the call (model.py:174-189)
+  const dim3 sgrid(cdiv(M * Hb, 256), B);
+  fast_stream_open_kernel<<<sgrid, 256, 0, st>>>(w.pos0, hop, g.c, St, M, Hb, nb, sb, ss, sl.bh, sl.bc, sl.bo, w.bh0[1],
+                                                w.bh1[1], w.bc0, w.bc1, w.bo, w.rst);
+  FSN_CHECK_LAUNCH("fast_stream_open_kernel");
+  fast_stream_bn_input_kernel<<<dim3(nb, B), 256, 0, st>>>(w.catM, w.catE, w.pos0, hop, g.c, St, M, d->noisy_num_neighbors,
+                                                            d->enc_num_neighbors, S, w.bn);
+  FSN_CHECK_LAUNCH("fast_stream_bn_input_kernel");
+  fast_stream_bn_scale_kernel<<<cdiv(R, 128), 128, 0, st>>>(w.bn, w.pos0, w.act0, hop, g.c, St, K, R, M, Kf, S, nb,
+                                                             TRAIN_CUM_EPS, sb, ss, sl.run, w.scale2);
+  FSN_CHECK_LAUNCH("fast_stream_bn_scale_kernel");
+  for (int i = 0; i < nb; ++i) {
+    StepParams p;
+    memset(&p, 0, sizeof(p));
+    p.R = R; p.K0 = Kf; p.H = Hb;
+    p.w_ih = wt->bn[0].w_ih; p.w_hh = wt->bn[0].w_hh; p.b_ih = wt->bn[0].b_ih; p.b_hh = wt->bn[0].b_hh;
+    p.x0 = w.bn + (size_t)i * R * Kf; p.x0_row_stride = Kf;
+    p.row_scale = w.scale2 + (size_t)i * R; p.row_scale_div = 1;
+    p.h_prev = w.bh0[(i + 1) & 1]; p.h_out = w.bh0[i & 1]; p.h_prev_stride = p.h_out_stride = Hb;
+    p.c = w.bc0;
+    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+    p.K0 = Hb;
+    p.w_ih = wt->bn[1].w_ih; p.w_hh = wt->bn[1].w_hh; p.b_ih = wt->bn[1].b_ih; p.b_hh = wt->bn[1].b_hh;
+    p.x0 = w.bh0[i & 1]; p.x0_row_stride = Hb; p.row_scale = nullptr; p.row_scale_div = 0;
+    p.h_prev = w.bh1[(i + 1) & 1]; p.h_out = w.bh1[i & 1];
+    p.c = w.bc1;
+    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+    if ((rc = sb_head_launch(w.bh1[i & 1], R, Hb, 1, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bo,
+                             HeadGeom{R, 1, 0, 0, (size_t)nb + 1}, i + 1, st)))
+      return rc;
+    fast_stream_commit_kernel<<<sgrid, 256, 0, st>>>(w.pos0, w.act0, hop, g.c, K, S, M, Hb, nb, i, w.bh0[i & 1],
+                                                     w.bh1[i & 1], w.bc0, w.bc1, w.bo, sb, ss, sl.bh, sl.bc, sl.bo);
+    FSN_CHECK_LAUNCH("fast_stream_commit_kernel");
+  }
+  // decoder input: encoder output | up-sampled bottleneck output (model.py:191-194)
+  fast_stream_dec_input_kernel<<<ew_grid((size_t)B * St * 2 * M), 256, 0, st>>>(w.encT, w.bo, w.pos0, hop, g.c, B, St, M, S,
+                                                                                 nb, w.dec_in);
+  FSN_CHECK_LAUNCH("fast_stream_dec_input_kernel");
+  // decoder on the path seq_stack_forward takes for this stack shape, (h, c) carried; then Linear(2F)
+  SeqStack dec;
+  memset(&dec, 0, sizeof(dec));
+  dec.R = B; dec.Tp = St; dec.K0 = 2 * M; dec.n = 2; dec.H[0] = Hd; dec.H[1] = Hd; dec.O = 2 * F;
+  const fsn_lstm_layer dl[2] = {wt->dec1, wt->dec2};
+  const int Hdl[2] = {Hd, Hd};
+  if (seq_stack_path(dec) == SEQ_PATH_PERSISTENT) {
+    // the state entering the call (zero for a clip whose frame 0 is step 0; a later frame 0 restarts inside the kernel),
+    // stored after step K - 1
+    for (int l = 0; l < 2; ++l) {
+      const size_t hb = (size_t)Hd * 4, lo = (size_t)l * hb;
+      if ((rc = copy_rows(w.dh[l], hb, sb + sl.dh + lo, ss, hb, B, st))) return rc;
+      if ((rc = copy_rows(w.dc[l], hb, sb + sl.dc + lo, ss, hb, B, st))) return rc;
+      if ((rc = stream_reset_launch(w.pos0, B, g, 0, Hd, w.dh[l], Hd, w.dc[l], st))) return rc;
+    }
+    FbState io;
+    memset(&io, 0, sizeof(io));
+    for (int l = 0; l < 2; ++l) {
+      io.h_init[l] = w.dh[l]; io.c_init[l] = w.dc[l]; io.h_fin[l] = w.dfh[l]; io.c_fin[l] = w.dfc[l];
+    }
+    io.restart = w.rst;
+    io.fin_step = K - 1;
+    if ((rc = fb_persistent_launch(dl, w.dec_in, nullptr, w.pp, w.dhall[1], w.barrier, B, 2 * M, Hd, Hd, St, st, &io)))
+      return rc;
+    for (int l = 0; l < 2; ++l) {
+      const size_t hb = (size_t)Hd * 4, lo = (size_t)l * hb;
+      if ((rc = copy_rows(sb + sl.dh + lo, ss, w.dfh[l], hb, hb, B, st))) return rc;
+      if ((rc = copy_rows(sb + sl.dc + lo, ss, w.dfc[l], hb, hb, B, st))) return rc;
+    }
+  } else if ((rc = stream_lstm_layers(dl, 2, Hdl, 2 * M, w.dec_in, nullptr, B, St, K, g, w.pos0, sb, ss, sl.dh, sl.dc, w.dh,
+                                      w.dc, w.dhall, st))) {
+    return rc;
+  }
+  if ((rc = fc_gemm_launch(w.dhall[1], wt->dec_fc_w, wt->dec_fc_b, w.y, B * St, Hd, 2 * F, FSN_ACT_NONE, st))) return rc;
+  // cRM: the carried Rc frames, then step j's output as frame pos0/hop - c + j - la
+  if ((rc = copy_rows(w.crm, (g.Rc + St) * F2 * 4, sb + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.crm + g.Rc * F2, (g.Rc + St) * F2 * 4, w.y, St * F2 * 4, St * F2 * 4, B, st))) return rc;
+  if ((rc = istft_stream_launch(w.spec, w.crm, w.pos0, w.act0, w.tail, B, K, g.D, n_fft, hop, win_length, g.c, g.la, g.Rc,
+                                g.Q, St, enhanced, st)))
+    return rc;
+  // carry what the next call reads: the windows as of step K
+  if ((rc = copy_rows(sb + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(sb + sl.spec, ss, w.spec + K * F2, (g.Q + St) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
+  if (Hm > 0) {
+    if ((rc = copy_rows(sb + sl.mel, ss, w.catM + (size_t)K * M, catw, (size_t)Hm * M * 4, B, st))) return rc;
+    if ((rc = copy_rows(sb + sl.enc, ss, w.catE + (size_t)K * M, catw, (size_t)Hm * M * 4, B, st))) return rc;
+  }
+  return copy_rows(sb + sl.crm, ss, w.crm + K * F2, (g.Rc + St) * F2 * 4, g.Rc * F2 * 4, B, st);
+}

@@ -43,6 +43,7 @@ struct Args {
   float* h1all;          // [B][Tp][H]
   unsigned int* barrier; // grid barrier counter (zeroed by the host before launch)
   int B, F, H0, H1, Tp, upc, G;  // layer 0: F -> H0, layer 1: H0 -> H1
+  FbState io;            // streaming: carried state (all null / fin_step -1 for a whole sequence)
 };
 
 __device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int target) {
@@ -122,6 +123,13 @@ __global__ void __launch_bounds__(THREADS, 1) fb_lstm_kernel(const Args a) {
     bias1[g] = unit_ok1 ? a.b_ih[1][g * H1 + u] + a.b_hh[1][g * H1 + u] : 0.f;
   }
   float c0[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};  // cell state: 4 rows, both layers
+  if (a.io.c_init[0])
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int row = row_base + 8 * r;
+      if (row < B && unit_ok0) c0[r] = a.io.c_init[0][(size_t)row * H0 + u];
+      if (row < B && unit_ok1) c1[r] = a.io.c_init[1][(size_t)row * H1 + u];
+    }
   float rs[4];  // 1/(mu+1e-5) of the thread's 4 clips (model.py:92), applied to the x segment
 #pragma unroll
   for (int r = 0; r < 4; ++r) rs[r] = (row_base + 8 * r < B) ? (a.inv1 ? a.inv1[row_base + 8 * r] : 1.f) : 0.f;
@@ -142,15 +150,18 @@ __global__ void __launch_bounds__(THREADS, 1) fb_lstm_kernel(const Args a) {
     for (int r = 0; r < 4; ++r)
 #pragma unroll
       for (int g = 0; g < 4; ++g) { acc0[r * 4 + g] = bias0[g]; acc1[r * 4 + g] = bias1[g]; }
-    const float* h0_prev = a.h0buf + (size_t)((p + 1) & 1) * B * H0;      // h0_{p-1}
-    const float* h1_prev = a.h1all + (size_t)(p >= 2 ? p - 2 : 0) * H1;   // h1_{p-2}, row stride Tp*H1
+    // h0_{p-1} (row stride H0) and h1_{p-2} (row stride h1_rs); the state entering step 0 from io.h_init when given
+    const bool init0 = p == 0 && a.io.h_init[0], init1 = p == 1 && a.io.h_init[1];
+    const float* h0_prev = init0 ? a.io.h_init[0] : a.h0buf + (size_t)((p + 1) & 1) * B * H0;
+    const float* h1_prev = init1 ? a.io.h_init[1] : a.h1all + (size_t)(p >= 2 ? p - 2 : 0) * H1;
+    const size_t h1_rs = init1 ? (size_t)H1 : (size_t)Tp * H1;
     // three k segments: x_p (F, layer 0), h0_{p-1} (H, both layers), h1_{p-2} (H, layer 1), walked as one
     // flat list of KC-wide chunks through a cp.async ring of NSTAGE tiles (NSTAGE-1 chunks in flight hide
     // the L2 latency; out-of-range elements are zero-filled with src-size 0).  Plain (non-.cg) loads are
     // correct here: every phase starts after the acquire of the grid barrier.
     const int nch_f = (F + KC - 1) / KC, nch_h = (H0 + KC - 1) / KC, nch_h1 = (H1 + KC - 1) / KC;
     const int c_begin = do0 ? 0 : nch_f;                       // skip x when layer 0 is finished
-    const int c_end = nch_f + (p >= 1 ? nch_h : 0) + (p >= 2 ? nch_h1 : 0);
+    const int c_end = nch_f + (p >= 1 || init0 ? nch_h : 0) + (p >= 2 || init1 ? nch_h1 : 0);
     auto issue = [&](int ci) {
       if (ci < c_end) {
         int seg = 0, k0 = ci * KC;
@@ -159,7 +170,7 @@ __global__ void __launch_bounds__(THREADS, 1) fb_lstm_kernel(const Args a) {
         const uint32_t Ab = At_s + (uint32_t)((ci - c_begin) % NSTAGE) * (ROWS * RS * 4);
         if ((seg == 1 && vec_ok1) || (seg == 2 && vec_ok2)) {
           const float* base = (seg == 1) ? h0_prev + k0 : h1_prev + k0;
-          const unsigned rstride = (seg == 1) ? (unsigned)H0 : (unsigned)(Tp * H1);
+          const unsigned rstride = (seg == 1) ? (unsigned)H0 : (unsigned)h1_rs;
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const int r = v_row0 + 64 * j;
@@ -174,7 +185,7 @@ __global__ void __launch_bounds__(THREADS, 1) fb_lstm_kernel(const Args a) {
           const int k = k0 + l_k;
           const bool kok = k < klen;
           const float* base = (seg == 0) ? a.x + (size_t)p * F + k : ((seg == 1) ? h0_prev + k : h1_prev + k);
-          const size_t rstride = (seg == 0) ? (size_t)Tp * F : ((seg == 1) ? (size_t)H0 : (size_t)Tp * H1);
+          const size_t rstride = (seg == 0) ? (size_t)Tp * F : ((seg == 1) ? (size_t)H0 : h1_rs);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const int r = l_row0 + 2 * j;
@@ -239,15 +250,23 @@ __global__ void __launch_bounds__(THREADS, 1) fb_lstm_kernel(const Args a) {
       for (int r = 0; r < 4; ++r) {
         const int row = row_base + 8 * r;
         if (row >= B) continue;
+        // io.restart: the row's state after step restart - 1 is zero (its sequence starts again at that step)
+        const int rst = a.io.restart ? a.io.restart[row] : -1;
         if (do0 && unit_ok0) {
-          const float c = sigmoidf_(acc0[r * 4 + 1]) * c0[r] + sigmoidf_(acc0[r * 4 + 0]) * tanhf(acc0[r * 4 + 2]);
+          float c = sigmoidf_(acc0[r * 4 + 1]) * c0[r] + sigmoidf_(acc0[r * 4 + 0]) * tanhf(acc0[r * 4 + 2]);
+          float h = sigmoidf_(acc0[r * 4 + 3]) * tanhf(c);
+          if (p + 1 == rst) c = h = 0.f;
           c0[r] = c;
-          a.h0buf[(size_t)(p & 1) * B * H0 + (size_t)row * H0 + u] = sigmoidf_(acc0[r * 4 + 3]) * tanhf(c);
+          a.h0buf[(size_t)(p & 1) * B * H0 + (size_t)row * H0 + u] = h;
+          if (p == a.io.fin_step) { a.io.h_fin[0][(size_t)row * H0 + u] = h; a.io.c_fin[0][(size_t)row * H0 + u] = c; }
         }
         if (do1 && unit_ok1) {
-          const float c = sigmoidf_(acc1[r * 4 + 1]) * c1[r] + sigmoidf_(acc1[r * 4 + 0]) * tanhf(acc1[r * 4 + 2]);
+          float c = sigmoidf_(acc1[r * 4 + 1]) * c1[r] + sigmoidf_(acc1[r * 4 + 0]) * tanhf(acc1[r * 4 + 2]);
+          float h = sigmoidf_(acc1[r * 4 + 3]) * tanhf(c);
+          if (p == rst) c = h = 0.f;
           c1[r] = c;
-          a.h1all[((size_t)row * Tp + (p - 1)) * H1 + u] = sigmoidf_(acc1[r * 4 + 3]) * tanhf(c);
+          a.h1all[((size_t)row * Tp + (p - 1)) * H1 + u] = h;
+          if (p - 1 == a.io.fin_step) { a.io.h_fin[1][(size_t)row * H1 + u] = h; a.io.c_fin[1][(size_t)row * H1 + u] = c; }
         }
       }
     }
@@ -276,8 +295,10 @@ bool fb_persistent_supported(int F, int H0, int H1) {
 
 // The 2-layer LSTM wavefront, one persistent launch per chunk of <= 256 rows (fb::ROWS).
 int fb_persistent_launch(const fsn_lstm_layer* L, const float* x, const float* inv1, float* h0buf, float* h1all,
-                         unsigned int* barrier, int R, int F, int H0, int H1, int Tp, cudaStream_t st) {
+                         unsigned int* barrier, int R, int F, int H0, int H1, int Tp, cudaStream_t st, const FbState* io) {
   fb::Args a;
+  memset(&a.io, 0, sizeof(a.io));
+  a.io.fin_step = -1;
   for (int l = 0; l < 2; ++l) { a.w_ih[l] = L[l].w_ih; a.w_hh[l] = L[l].w_hh; a.b_ih[l] = L[l].b_ih; a.b_hh[l] = L[l].b_hh; }
   a.h0buf = h0buf; a.barrier = barrier;
   a.F = F; a.H0 = H0; a.H1 = H1; a.Tp = Tp;
@@ -295,6 +316,17 @@ int fb_persistent_launch(const fsn_lstm_layer* L, const float* x, const float* i
   for (int r0 = 0; r0 < R; r0 += fb::ROWS) {
     a.B = (R - r0 < fb::ROWS) ? R - r0 : fb::ROWS;
     a.x = x + (size_t)r0 * Tp * F; a.inv1 = inv1 ? inv1 + r0 : nullptr; a.h1all = h1all + (size_t)r0 * Tp * H1;
+    if (io) {  // the chunk's rows of every state table
+      const int Hl[2] = {H0, H1};
+      for (int l = 0; l < 2; ++l) {
+        a.io.h_init[l] = io->h_init[l] ? io->h_init[l] + (size_t)r0 * Hl[l] : nullptr;
+        a.io.c_init[l] = io->c_init[l] ? io->c_init[l] + (size_t)r0 * Hl[l] : nullptr;
+        a.io.h_fin[l] = io->h_fin[l] ? io->h_fin[l] + (size_t)r0 * Hl[l] : nullptr;
+        a.io.c_fin[l] = io->c_fin[l] ? io->c_fin[l] + (size_t)r0 * Hl[l] : nullptr;
+      }
+      a.io.restart = io->restart ? io->restart + r0 : nullptr;
+      a.io.fin_step = io->fin_step;
+    }
     rc = check_cuda(cudaMemsetAsync(barrier, 0, sizeof(unsigned int), st), "fb barrier memset");
     if (rc) return rc;
     void* params[] = {(void*)&a};

@@ -282,34 +282,12 @@ extern "C" int fsn_fullband_stream_step(const fsn_fullband_desc* d, const fsn_ls
   // first norm (fbb_core): frame sums, then the running scale of each step
   if ((rc = frame_stats_launch(w.magT, B, S, F, 0, (size_t)S * F, F, w.fs, st))) return rc;
   if ((rc = stream_norm_launch(w.fs, B, S, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale, st))) return rc;
-  // the stack, layer by layer, on the per-step kernels seq_stack_forward runs for the causal norms; (h, c) of each layer
-  // start from the slot's state and are stored back after step K - 1
-  for (int l = 0; l < n; ++l) {
-    float* hl = w.hall[l & 1];
-    const size_t hrow = (size_t)S * H;
-    if ((rc = copy_rows(w.h[l], (size_t)H * 4, sb + sl.h + (size_t)l * H * 4, ss, (size_t)H * 4, B, st))) return rc;
-    if ((rc = copy_rows(w.c[l], (size_t)H * 4, sb + sl.c + (size_t)l * H * 4, ss, (size_t)H * 4, B, st))) return rc;
-    for (int j = 0; j < S; ++j) {
-      float* hp = j ? hl + (size_t)(j - 1) * H : w.h[l];
-      if (j <= g.c && (rc = stream_reset_launch(w.pos0, B, g, j, H, hp, j ? hrow : (size_t)H, w.c[l], st))) return rc;
-      StepParams p;
-      memset(&p, 0, sizeof(p));
-      p.R = B; p.H = H; p.first = 0; p.gru = 0;
-      p.w_ih = layers[l].w_ih; p.w_hh = layers[l].w_hh; p.b_ih = layers[l].b_ih; p.b_hh = layers[l].b_hh;
-      p.K0 = l ? H : F;
-      p.x0 = l ? w.hall[(l - 1) & 1] + (size_t)j * H : w.magT + (size_t)j * F;
-      p.x0_row_stride = (size_t)S * p.K0;
-      p.row_scale = l ? nullptr : w.scale + (size_t)j * B;
-      p.h_prev = hp; p.h_prev_stride = j ? hrow : (size_t)H;
-      p.h_out = hl + (size_t)j * H; p.h_out_stride = hrow;
-      p.c = w.c[l];
-      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-      if (j == K - 1) {
-        if ((rc = copy_rows(sb + sl.h + (size_t)l * H * 4, ss, p.h_out, hrow * 4, (size_t)H * 4, B, st))) return rc;
-        if ((rc = copy_rows(sb + sl.c + (size_t)l * H * 4, ss, w.c[l], (size_t)H * 4, (size_t)H * 4, B, st))) return rc;
-      }
-    }
-  }
+  // the stack on the per-step kernels seq_stack_forward runs for the causal norms, (h, c) carried in the slot state
+  int Hs[SEQ_MAX_LAYERS];
+  for (int l = 0; l < n; ++l) Hs[l] = H;
+  if ((rc = stream_lstm_layers(layers, n, Hs, F, w.magT, w.scale, B, S, K, g, w.pos0, sb, ss, sl.h, sl.c, w.h, w.c, w.hall,
+                               st)))
+    return rc;
   if ((rc = fc_gemm_launch(w.hall[(n - 1) & 1], fc_w, fc_b, w.y, B * S, H, 2 * F, d->activation, st))) return rc;
   // cRM: the carried Rc frames, then step j's output as frame pos0/hop - c + j - la
   if ((rc = copy_rows(w.crm, (g.Rc + S) * F2 * 4, sb + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;

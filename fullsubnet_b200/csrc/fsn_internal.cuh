@@ -419,10 +419,20 @@ int imp_unfold_bwd_launch(const float* dX, const float* invs, const float* dot, 
 inline HeadGeom imp_head_geom(const SecGeom& g, int F, int T) { return HeadGeom{g.N, g.cs, g.lo, F, (size_t)T}; }
 
 // persistent cooperative full-band LSTM (fsn_fullband.cu): layers L[0] (F -> H0, input x [R,Tp,F] times inv1[r] when
-// given) and L[1] (H0 -> H1) of R rows into h1all [R,Tp,H1]; h0buf [2][256][H0] scratch
+// given) and L[1] (H0 -> H1) of R rows into h1all [R,Tp,H1]; h0buf [2][256][H0] scratch.
+// io (nullable, chunked streaming): per layer l, h_init / c_init [R, H_l] the state entering step 0 (null: zero; the c_init
+// pair and the h_init pair are given or null together); h_fin / c_fin [R, H_l] receive the state after step fin_step
+// (-1: none); restart [R] (nullable): row r's state after step restart[r] - 1 is zero, as at a sequence's first step
+struct FbState {
+  const float* h_init[2]; const float* c_init[2];
+  float* h_fin[2]; float* c_fin[2];
+  const int* restart;
+  int fin_step;
+};
 bool fb_persistent_supported(int F, int H0, int H1);
 int fb_persistent_launch(const fsn_lstm_layer* L, const float* x, const float* inv1, float* h0buf, float* h1all,
-                         unsigned int* barrier, int R, int F, int H0, int H1, int Tp, cudaStream_t st);
+                         unsigned int* barrier, int R, int F, int H0, int H1, int Tp, cudaStream_t st,
+                         const FbState* io = nullptr);
 
 // tensor-core LSTM layer for a small batch of sequences (fsn_lstm_rec_tc.cu): hoisted input projection on the tf32
 // GEMM (x3: three passes on tf32 hi/lo splits) + persistent cooperative wgmma recurrence (x3: fp16 hi/lo splits)
@@ -510,6 +520,14 @@ int stft_stream_launch(const float* win, int Wn, int Hs, const int* pos0, const 
 int istft_stream_launch(const float* spec, const float* crm, const int* pos0, const int* act0, const int* tail, int B,
                         int K, int D, int n_fft, int hop, int win_length, int c, int la, int Rc, int Q, int S, float* wav,
                         cudaStream_t st);
+// n LSTM layers (hidden sizes H[l]) over the call's S steps on the per-step kernels, as seq_stack_forward runs a stack with
+// a per-step scale: layer 0 reads x [B, S, K0] times scaleT[j*B + b] (nullable), layer l writes h of every step to
+// hall[l & 1] [B, S, H[l]].  Layer l's (h, c) start from the slot state (h at h_off, c at c_off bytes into each block, the
+// layers one after the other) through h[l] / c[l] [B, H[l]], are zeroed at a clip's frame 0 and are stored back after
+// step K - 1
+int stream_lstm_layers(const fsn_lstm_layer* L, int n, const int* H, int K0, const float* x, const float* scaleT, int B,
+                       int S, int K, const StreamGeom& g, const int* pos0, char* state, size_t slot_bytes, size_t h_off,
+                       size_t c_off, float* const* h, float* const* c, float* const* hall, cudaStream_t st);
 // rows of `width` bytes: dst row b (pitch dp) <- src row b (pitch sp), B rows, on the stream
 int copy_rows(void* dst, size_t dp, const void* src, size_t sp, size_t width, int B, cudaStream_t st);
 

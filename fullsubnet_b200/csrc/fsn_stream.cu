@@ -112,6 +112,44 @@ int stream_reset_launch(const int* pos0, int B, const StreamGeom& g, int j, int 
   return FSN_OK;
 }
 
+int stream_lstm_layers(const fsn_lstm_layer* L, int n, const int* H, int K0, const float* x, const float* scaleT, int B,
+                       int S, int K, const StreamGeom& g, const int* pos0, char* state, size_t slot_bytes, size_t h_off,
+                       size_t c_off, float* const* h, float* const* c, float* const* hall, cudaStream_t st) {
+  int rc;
+  size_t off = 0;  // floats of the layers below in the h and c sections
+  for (int l = 0; l < n; ++l) {
+    const int Hl = H[l];
+    float* hl = hall[l & 1];
+    const size_t hrow = (size_t)S * Hl, hb = (size_t)Hl * 4;
+    char* sh = state + h_off + off * 4;
+    char* sc = state + c_off + off * 4;
+    if ((rc = copy_rows(h[l], hb, sh, slot_bytes, hb, B, st))) return rc;
+    if ((rc = copy_rows(c[l], hb, sc, slot_bytes, hb, B, st))) return rc;
+    for (int j = 0; j < S; ++j) {
+      float* hp = j ? hl + (size_t)(j - 1) * Hl : h[l];
+      if (j <= g.c && (rc = stream_reset_launch(pos0, B, g, j, Hl, hp, j ? hrow : (size_t)Hl, c[l], st))) return rc;
+      StepParams p;
+      memset(&p, 0, sizeof(p));
+      p.R = B; p.H = Hl; p.first = 0; p.gru = 0;
+      p.w_ih = L[l].w_ih; p.w_hh = L[l].w_hh; p.b_ih = L[l].b_ih; p.b_hh = L[l].b_hh;
+      p.K0 = l ? H[l - 1] : K0;
+      p.x0 = l ? hall[(l - 1) & 1] + (size_t)j * H[l - 1] : x + (size_t)j * K0;
+      p.x0_row_stride = (size_t)S * p.K0;
+      p.row_scale = (l || !scaleT) ? nullptr : scaleT + (size_t)j * B;
+      p.h_prev = hp; p.h_prev_stride = j ? hrow : (size_t)Hl;
+      p.h_out = hl + (size_t)j * Hl; p.h_out_stride = hrow;
+      p.c = c[l];
+      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+      if (j == K - 1) {
+        if ((rc = copy_rows(sh, slot_bytes, p.h_out, hrow * 4, hb, B, st))) return rc;
+        if ((rc = copy_rows(sc, slot_bytes, c[l], hb, hb, B, st))) return rc;
+      }
+    }
+    off += Hl;
+  }
+  return FSN_OK;
+}
+
 int copy_rows(void* dst, size_t dp, const void* src, size_t sp, size_t width, int B, cudaStream_t st) {
   return check_cuda(cudaMemcpy2DAsync(dst, dp, src, sp, width, (size_t)B, cudaMemcpyDeviceToDevice, st), "stream copy");
 }

@@ -63,6 +63,10 @@ class Model(BaseModel):
     # fsn_fast_train_backward runs BPTT
     TRAIN_ENTRY_POINTS = ("fsn_fast_train_workspace_bytes", "fsn_fast_train_forward", "fsn_fast_train_backward")
     TRAIN_TF32_STACKS = ("bottleneck",)
+    # chunked streaming (fullsubnet_b200.stream.Streamer, precision="fp32" with cumulative_laplace_norm): state /
+    # workspace queries, delay, step
+    STREAM_ENTRY_POINTS = ("fsn_fast_stream_state_bytes", "fsn_fast_stream_workspace_bytes", "fsn_fast_stream_delay",
+                           "fsn_fast_stream_step")
 
     def __init__(self, look_ahead, shrink_size, sequence_model, num_mels, encoder_input_size, bottleneck_hidden_size,
                  bottleneck_num_layers, noisy_input_num_neighbors, encoder_output_num_neighbors,
@@ -119,6 +123,17 @@ class Model(BaseModel):
         if self.precision != "fp32" and not ok:
             raise NotImplementedError("the tensor-core precisions need bottleneck_hidden_size = 384, 2 layers and input width <= 32")
         return self.precision
+
+    def _stream_desc(self):
+        """Descriptor of the streaming calls: the fp32 kernels only, so an explicit precision="fp32" (under "auto" the
+        whole-clip call runs the tensor cores, which a stream could not match)."""
+        if self.precision != "fp32":
+            raise NotImplementedError(f"fullsubnet_b200: fast_fullsubnet streaming is built for precision=\"fp32\" "
+                                      f"(this model has precision={self.precision!r})")
+        return self._desc(_lib.PREC["fp32"])
+
+    def _stream_weights(self):
+        return (C.byref(self._weight_struct()),)
 
     def _train_desc(self):
         return self._desc(_lib.PREC[self._resolve_train_precision()])

@@ -25,6 +25,9 @@ class Model(SpectrogramEnhance, BaseModel):
     # fsn_fullband_train_backward runs BPTT
     TRAIN_ENTRY_POINTS = ("fsn_fullband_train_workspace_bytes", "fsn_fullband_train_forward", "fsn_fullband_train_backward")
     TRAIN_TF32_STACKS = ("fullband_model",)
+    # chunked streaming (fullsubnet_b200.stream.Streamer): state / workspace queries, delay, step
+    STREAM_ENTRY_POINTS = ("fsn_fullband_stream_state_bytes", "fsn_fullband_stream_workspace_bytes",
+                           "fsn_fullband_stream_delay", "fsn_fullband_stream_step")
 
     def __init__(self, num_freqs, hidden_size, sequence_model, output_activate_function, look_ahead,
                  norm_type="offline_laplace_norm", weight_init=True, precision=None):
@@ -56,6 +59,12 @@ class Model(SpectrogramEnhance, BaseModel):
 
     def _enhance_args(self, device):
         return self._infer_desc(), self._weight_ptrs()
+
+    def _stream_desc(self):
+        return self._infer_desc()
+
+    def _stream_weights(self):
+        return self._weight_ptrs()
 
     def _train_desc(self):
         return self._desc(_lib.PREC[self._resolve_train_precision()])

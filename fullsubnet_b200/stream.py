@@ -1,7 +1,9 @@
 """Chunked streaming enhancement (DESIGN 4.14): ``Streamer`` advances many streams by K hops per call and returns, for
 each clip, the samples of the whole-clip ``enhance`` call bit for bit, ``delay`` samples later.
 
-Built for fullband_baseline with ``cumulative_laplace_norm`` or ``forgetting_norm`` (LSTM, fp32)."""
+Built for fullband_baseline with ``cumulative_laplace_norm`` or ``forgetting_norm`` (LSTM, fp32) and for fast_fullsubnet
+with ``cumulative_laplace_norm`` (LSTM, ``precision="fp32"``).  Each model names its library calls in
+``STREAM_ENTRY_POINTS`` and gives their arguments through ``_stream_desc()`` and ``_stream_weights()``."""
 from __future__ import annotations
 
 import ctypes as C
@@ -23,18 +25,20 @@ class Streamer:
     ends the clip the row holds the samples from pos - delay to the clip's end, then 0."""
 
     def __init__(self, model, slots: int, n_fft: int = 512, hop: int = 256, win_length: int = 512):
-        from .fullband_baseline.model import Model as FullbandBaseline
-        if not isinstance(model, FullbandBaseline):
-            raise NotImplementedError("fullsubnet_b200: chunked streaming is built for fullband_baseline")
+        names = getattr(type(model), "STREAM_ENTRY_POINTS", ())
+        if not names:
+            raise NotImplementedError("fullsubnet_b200: chunked streaming is built for fullband_baseline and "
+                                      "fast_fullsubnet")
         self.model, self.slots, self.n_fft, self.hop, self.win_length = model, int(slots), n_fft, hop, win_length
         self.device = next(model.parameters()).device
         lib = _lib.load()
-        d = model._infer_desc()
-        delay = lib.fsn_fullband_stream_delay(C.byref(d), n_fft, hop)
+        self._state_bytes, self._workspace_bytes, self._delay, self._step = (getattr(lib, n) for n in names)
+        d = model._stream_desc()
+        delay = self._delay(C.byref(d), n_fft, hop)
         if delay < 0:
             _lib.check(-delay)
         self.delay = int(delay)
-        n = _lib.check_workspace(lib.fsn_fullband_stream_state_bytes(C.byref(d), self.slots, n_fft, hop))
+        n = _lib.check_workspace(self._state_bytes(C.byref(d), self.slots, n_fft, hop))
         self.state = torch.zeros(n, dtype=torch.uint8, device=self.device)
         self._ws = None
         self._pos = [None] * self.slots  # each slot's clip position as far as the host knows it
@@ -58,8 +62,7 @@ class Streamer:
 
     def _workspace(self, d, K: int) -> torch.Tensor:
         """One workspace, sized for the largest K so far: a workspace for K_max serves every K <= K_max."""
-        lib = _lib.load()
-        n = _lib.check_workspace(lib.fsn_fullband_stream_workspace_bytes(C.byref(d), self.slots, K, self.n_fft, self.hop))
+        n = _lib.check_workspace(self._workspace_bytes(C.byref(d), self.slots, K, self.n_fft, self.hop))
         if self._ws is None or self._ws.numel() < n:
             self._ws = None
             self._ws = torch.empty(n, dtype=torch.uint8, device=self.device)
@@ -98,15 +101,13 @@ class Streamer:
         assert chunk.shape[1] % self.hop == 0, f"a chunk is a whole number of hops ({self.hop} samples)"
         K = chunk.shape[1] // self.hop
         x = _lib.require_cuda(chunk, "chunk")
-        lib = _lib.load()
-        d = self.model._infer_desc()
-        layers, fc_w, fc_b = self.model._weight_ptrs()
+        d, weights = self.model._stream_desc(), self.model._stream_weights()
         ws = self._workspace(d, K)
         st, tl = self._table(start, 0), self._table(tail, -1)
         pos = self._check_lengths(K, st, tl)
         out = torch.empty(self.slots, K * self.hop + self.delay, dtype=torch.float32, device=self.device)
-        _lib.check(lib.fsn_fullband_stream_step(
-            C.byref(d), layers, fc_w, fc_b, x.data_ptr(),
+        _lib.check(self._step(
+            C.byref(d), *weights, x.data_ptr(),
             None if st is None else st.ctypes.data_as(C.c_void_p), None if tl is None else tl.ctypes.data_as(C.c_void_p),
             self.slots, K, self.n_fft, self.hop, self.win_length, out.data_ptr(), self.state.data_ptr(),
             self.state.numel(), ws.data_ptr(), ws.numel(), _lib.stream_ptr(self.device)))
