@@ -10,10 +10,11 @@ wav -> enhanced wav + int16 PCM (what the file loop writes).  Two schedules of t
               most a fraction x of the batch's samples, one fsn_enhance call with per-clip lengths per batch.
 
 --model improved_fullsubnet --variant k16|k48|k48_960: the same schedules for improved_fullsubnet with bench.py's
-constructor arguments and weights of that variant, the default precision ("auto": tf32_tc), clip lengths distinct and
-uniform in 1 - 10 s at the variant's sample rate (16 or 48 kHz), fsn_improved_enhance for every call.  Its sections
-launch kernels once per frame, and one call on a 10 s clip keeps every step's gates, so the defaults are --clips 256
-and --batch 64.
+constructor arguments and weights of that variant, the precision of --precision (default "auto": tf32_tc), clip
+lengths distinct and uniform in 1 - 10 s at the variant's sample rate (16 or 48 kHz), fsn_improved_enhance for every
+call.  On tf32_tc its sections launch kernels once per frame, and one call on a 10 s clip keeps every step's gates, so
+the defaults are --clips 256 and --batch 64; f16x3_tc / f16_tc run each section in one launch and keep only the input
+projection and layer 1's output of every step.
 
 --model fullband_baseline: the same schedules and clips as fullsubnet for the paper's baseline (its full-size constructor
 arguments, seed-11 weights, fp32), fsn_fullband_enhance for every call.  The JSON line also carries "per_call_64x10s":
@@ -115,6 +116,7 @@ def make_model(a, dev):
     imp_args = {"k48": IO.ARGS_48K_1024, "k48_960": IO.ARGS_48K_960, "k16": IO.DEFAULT_IMPROVED_ARGS}[a.variant]
     m = ImpModel(**imp_args)  # the constructor arguments and weights of bench.py --variant
     m.load_state_dict(IO.make_improved_state_dict(seed=5, args=imp_args), strict=True)
+    m.precision = a.precision
     sr = 16000 if a.variant == "k16" else 48000
     return m.to(dev).eval(), sr, (f"improved_fullsubnet {a.variant} (n_fft={imp_args['n_fft']}, "
                                   f"hop={imp_args['hop_length']})")
@@ -145,6 +147,8 @@ def main():
     ap.add_argument("--model", default="fullsubnet", choices=["fullsubnet", "improved_fullsubnet", "fullband_baseline"])
     ap.add_argument("--variant", default="k48", choices=["k48", "k48_960", "k16"],
                     help="improved_fullsubnet constructor args (as bench.py --variant)")
+    ap.add_argument("--precision", default="auto", choices=["auto", "fp32", "tf32_tc", "f16x3_tc", "f16_tc"],
+                    help="improved_fullsubnet's precision (auto: tf32_tc)")
     ap.add_argument("--clips", type=int, default=None, help="default 1024 (fullsubnet), 256 (improved_fullsubnet)")
     ap.add_argument("--batch", type=int, default=None, help="default 256 (fullsubnet), 64 (improved_fullsubnet)")
     ap.add_argument("--max-padding", type=float, nargs="+", default=[0.05, 0.1, 0.25])
@@ -153,6 +157,7 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     a = ap.parse_args()
     improved = a.model == "improved_fullsubnet"
+    assert improved or a.precision == "auto", "--precision applies to --model improved_fullsubnet"
     a.clips = a.clips or (256 if improved else 1024)
     a.batch = a.batch or (64 if improved else 256)
     assert a.gpus == 1, "bench_varlen.py measures one GPU"

@@ -93,7 +93,7 @@ class ImprovedDesc(C.Structure):
 
 
 class ImprovedWeights(C.Structure):
-    _fields_ = [("fb", SeqWeights), ("sb", SeqWeights * IMP_MAX_SECTIONS)]
+    _fields_ = [("fb", SeqWeights), ("sb", SeqWeights * IMP_MAX_SECTIONS), ("sb_packed", C.c_void_p * IMP_MAX_SECTIONS)]
 
 
 class ImprovedGrads(C.Structure):
@@ -129,6 +129,8 @@ _SIGNATURES = {
     "fsn_improved_enhance_workspace_bytes": (_S, [C.POINTER(ImprovedDesc), _I, _I]),
     "fsn_improved_enhance": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _P, _I, _I, _P, _P, _P, _F,
                                        _P, _S, _P]),
+    "fsn_improved_packed_bytes": (_S, [C.POINTER(ImprovedDesc), _I]),
+    "fsn_improved_pack_sb_weights": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _I, _P, _P]),
     "fsn_improved_train_workspace_bytes": (_S, [C.POINTER(ImprovedDesc), _I, _I]),
     "fsn_improved_train_forward": (C.c_int, [C.POINTER(ImprovedDesc), C.POINTER(ImprovedWeights), _P, _I, _I, _P, _P, _S,
                                              _P]),
@@ -205,6 +207,8 @@ _SIGNATURES = {
     "fsn_debug_fast_norm_unfold_bwd": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P, _P, _P, _P]),
     "fsn_debug_imp_unfold_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "fsn_debug_imp_section_input": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "fsn_debug_imp_section_lstm_tc_workspace_bytes": (_S, [_I, _I, _I, _I, _I]),
+    "fsn_debug_imp_section_lstm_tc": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _P, _I, _I, _I, _I, _P, _P, _P, _S, _P]),
     "fsn_debug_norm_stats": (C.c_int, [_P, _I, _I, _I, _I, _L, _L, _P, _P, _I, _I, _P, _F, _F, _F, _P, _P, _P, _P, _P]),
     "fsn_debug_train_stats": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P]),
     "fsn_debug_forgetting_scale": (C.c_int, [_P, _I, _P, _I, _I, _I, _I, _L, _L, _F, _P, _P, _I, _I, _P, _P, _P, _P, _P]),

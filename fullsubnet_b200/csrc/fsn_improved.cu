@@ -73,18 +73,52 @@ struct ImpWs {
   float *h0[2], *h1[2], *c0, *c1;
   LayerSave tc;                        // FSN_PREC_TF32_TC: gates / cell / hidden of every step of one layer
   float *tc_h1, *tc_rec;
+  ImpSecTcWs f16;                      // FSN_PREC_F16X3_TC / FSN_PREC_F16_TC: GEMM operands, P and h1 of one section
   WavWs wav;                           // fsn_improved_enhance: peak and length table (spectrum and cRM above)
   size_t bytes;
 };
 
-// full band (model.py:567): 2 x LSTM(Fu -> Hf -> Hf) + Linear(Hf -> Fu), rows = clips; FSN_PREC_TF32_TC runs it on the
-// single-pass tensor-core layers
+static bool imp_f16(const fsn_improved_desc* d) {
+  return d->precision == FSN_PREC_F16X3_TC || d->precision == FSN_PREC_F16_TC;
+}
+
+// full band (model.py:567): 2 x LSTM(Fu -> Hf -> Hf) + Linear(Hf -> Fu), rows = clips; FSN_PREC_TF32_TC and
+// FSN_PREC_F16_TC run it on the single-pass tensor-core layers, FSN_PREC_F16X3_TC on the compensated ones (as
+// fullsubnet's full band)
 static SeqStack imp_fb_stack(const fsn_improved_desc* d, const ImpDims& m) {
   SeqStack s;
   memset(&s, 0, sizeof(s));
   s.R = m.B; s.Tp = m.T; s.K0 = m.Fu; s.n = 2; s.H[0] = s.H[1] = d->fb_hidden; s.O = m.Fu; s.act = d->fb_activation;
-  s.tc = d->precision == FSN_PREC_TF32_TC && lstm_rec_tc_supported(d->fb_hidden, false);
+  s.x3 = d->precision == FSN_PREC_F16X3_TC;
+  s.tc = (d->precision == FSN_PREC_TF32_TC || imp_f16(d)) && lstm_rec_tc_supported(d->fb_hidden, s.x3);
   return s;
+}
+
+// the sub-band stack shape the f16 section kernel runs: sb_hidden in {128, 256, 384}
+static bool imp_sb_f16_ok(int H) { return H % 128 == 0 && H >= 128 && H <= 384; }
+
+void imp_section_tc_carve(Carver& c, size_t rows_T, int Wmax, int H, bool x3, ImpSecTcWs& w) {
+  const size_t wa = (size_t)((Wmax + 3) & ~3) * (x3 ? 3 : 1);
+  w.gemm.a = c.take<float>(rows_T * wa);
+  w.gemm.w = c.take<float>((size_t)4 * H * wa);
+  w.gemm.P = nullptr; w.gemm.rec = nullptr;
+  w.P = c.take<float>(rows_T * 4 * H);
+  w.h1 = c.take<float>(rows_T * H);
+}
+
+int imp_section_lstm_tc(const fsn_seq_weights& sw, const void* packed, const float* X, int R, int T, int W, int H, bool x3,
+                        const ImpSecTcWs& w, cudaStream_t st, int stages, int cluster) {
+  const size_t rows = (size_t)T * R;
+  int rc;
+  // P = (X W_ih0^T + b_ih0) + b_hh0, [T*R, 4H]: the compensated (x3) or single-pass tf32 GEMM
+  if ((rc = linear_tc(X, (size_t)W, W, sw.w_ih[0], sw.b_ih[0], 4 * H, FSN_ACT_NONE, w.P, (size_t)4 * H, rows, x3, w.gemm,
+                      st)))
+    return rc;
+  if ((rc = bias_act_launch(w.P, rows, 4 * H, (size_t)4 * H, sw.b_hh[0], FSN_ACT_NONE, st))) return rc;
+  SbProjArgs a;
+  memset(&a, 0, sizeof(a));
+  a.packed = packed; a.P = w.P; a.h1 = w.h1; a.R = R; a.T = T; a.H = H; a.x3 = x3; a.stages = stages; a.cluster = cluster;
+  return sb_proj_forward(a, st);
 }
 
 int sec_geom(int lo, int hi, int cs, int ns, int cf, int nf, int Fu, SecGeom& g) {
@@ -104,8 +138,11 @@ int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m) {
               "improved model: n_fft=%d unsupported (power of two <= 2048, or even and <= 1200)", d->n_fft);
   FSN_REQUIRE(d->num_freqs == d->n_fft / 2 + 1, FSN_ERR_SHAPE, "improved model: num_freqs != n_fft/2+1");
   FSN_REQUIRE(d->num_sections >= 1 && d->num_sections <= FSN_IMP_MAX_SECTIONS, FSN_ERR_SHAPE, "improved model: sections");
-  FSN_REQUIRE(d->precision == FSN_PREC_FP32 || (d->precision == FSN_PREC_TF32_TC && (d->sb_hidden & 3) == 0),
-              FSN_ERR_UNSUPPORTED, "improved model: precision must be FSN_PREC_FP32 or FSN_PREC_TF32_TC (sb_hidden %% 4 == 0)");
+  FSN_REQUIRE(d->precision == FSN_PREC_FP32 || (d->precision == FSN_PREC_TF32_TC && (d->sb_hidden & 3) == 0) ||
+                  (imp_f16(d) && imp_sb_f16_ok(d->sb_hidden)),
+              FSN_ERR_UNSUPPORTED,
+              "improved model: precision must be FSN_PREC_FP32, FSN_PREC_TF32_TC (sb_hidden %% 4 == 0), or FSN_PREC_F16X3_TC "
+              "/ FSN_PREC_F16_TC (sb_hidden in {128, 256, 384})");
   m.B = B; m.L = L; m.T = 1 + L / d->hop_length; m.F = d->num_freqs; m.Fu = m.F - 1; m.S = d->num_sections;
   m.maxRW = 0; m.maxR = 0;
   for (int s = 0; s < m.S; ++s) {
@@ -135,6 +172,12 @@ static void imp_carve(const fsn_improved_desc* d, const ImpDims& m, void* base, 
   for (int i = 0; i < 2; ++i) { w.h0[i] = c.take<float>(RH); w.h1[i] = c.take<float>(RH); }
   w.c0 = c.take<float>(RH); w.c1 = c.take<float>(RH);
   w.tc.G = w.tc.C = w.tc.H = w.tc_h1 = w.tc_rec = nullptr;
+  memset(&w.f16, 0, sizeof(w.f16));
+  if (imp_f16(d)) {
+    int maxW = 0;
+    for (int s = 0; s < m.S; ++s) maxW = m.sec[s].W > maxW ? m.sec[s].W : maxW;
+    imp_section_tc_carve(c, (size_t)m.T * m.B * m.maxR, maxW, d->sb_hidden, d->precision == FSN_PREC_F16X3_TC, w.f16);
+  }
   if (d->precision == FSN_PREC_TF32_TC) {
     const size_t TR = (size_t)m.T * m.B * m.maxR;
     w.tc.G = c.take<float>(TR * 4 * d->sb_hidden);
@@ -187,6 +230,18 @@ static int imp_forward(const fsn_improved_desc* d, const fsn_improved_weights* w
                                  st, eps, lens, hop, 0)))
       return rc;
     const fsn_seq_weights& sw = wt->sb[s];
+    if (imp_f16(d)) {
+      // the section on the fp16 tensor cores: P of all steps on the tf32 GEMM, both layers of all steps in one
+      // persistent launch, then the head over all steps (DESIGN 4.3)
+      FSN_REQUIRE(wt->sb_packed[s], FSN_ERR_SHAPE, "improved model: section %d has no packed weights (fsn_improved_pack_sb_weights)", s);
+      if ((rc = scale_rows_launch(w.X, w.invs, (size_t)T * R * g.W, g.W, R, g.N, w.X, st))) return rc;
+      if ((rc = imp_section_lstm_tc(sw, wt->sb_packed[s], w.X, R, T, g.W, Hs, d->precision == FSN_PREC_F16X3_TC, w.f16, st)))
+        return rc;
+      if ((rc = sb_head_launch(w.f16.h1, R, Hs, T, sw.fc_w, sw.fc_b, 2 * g.cs, d->sb_activation, crm, imp_head_geom(g, F, T), 0,
+                               st)))
+        return rc;
+      continue;
+    }
     if (d->precision == FSN_PREC_TF32_TC) {
       // layer by layer over all steps: hoisted input projection + per-step recurrent GEMM on wgmma (tf32), fused cell
       LayerSave l1{w.tc.G, w.tc.C, w.tc_h1};
@@ -286,4 +341,71 @@ extern "C" int fsn_debug_imp_section_input(const float* magc, const float* fbT, 
   FSN_REQUIRE((size_t)T * B * g.N * g.W < ((size_t)1 << 31) && (size_t)B * T < ((size_t)1 << 31), FSN_ERR_SHAPE,
               "section input hook: tensors must stay below 2^31 elements");
   return imp_section_input_launch(magc, fbT, B, T, Fu, g, X, reinterpret_cast<float2*>(fs), tm != 0, (cudaStream_t)stream);
+}
+
+// ---- packed section weights of the fp16 tensor-core precisions (include/fsn_b200.h)
+static int imp_pack_check(const fsn_improved_desc* d, int section) {
+  ImpDims m;
+  int rc = imp_dims(d, 1, 1, m);
+  if (rc) return rc;
+  FSN_REQUIRE(imp_f16(d), FSN_ERR_UNSUPPORTED,
+              "improved model: packed section weights exist for FSN_PREC_F16X3_TC / FSN_PREC_F16_TC only");
+  FSN_REQUIRE(section >= 0 && section < m.S, FSN_ERR_SHAPE, "improved model: section %d of %d", section, m.S);
+  return FSN_OK;
+}
+
+extern "C" size_t fsn_improved_packed_bytes(const fsn_improved_desc* d, int section) {
+  if (imp_pack_check(d, section)) return 0;
+  return sb_tc_packed_bytes_raw(d->sb_hidden, d->precision == FSN_PREC_F16X3_TC, true);
+}
+
+extern "C" int fsn_improved_pack_sb_weights(const fsn_improved_desc* d, const fsn_improved_weights* w, int section,
+                                            void* packed, fsn_stream_t stream) {
+  launch_counter() = 0;
+  int rc = imp_pack_check(d, section);
+  if (rc) return rc;
+  FSN_REQUIRE(w && packed, FSN_ERR_SHAPE, "improved model: missing weights or packed buffer");
+  const fsn_seq_weights& sw = w->sb[section];
+  FSN_REQUIRE(sw.w_hh[0] && sw.w_ih[1] && sw.w_hh[1] && sw.b_ih[1] && sw.b_hh[1], FSN_ERR_SHAPE,
+              "improved model: section %d has missing weights", section);
+  return sb_tc_pack_raw(&sw, d->sb_hidden, 0, 0, packed, (cudaStream_t)stream, d->precision == FSN_PREC_F16X3_TC, true);
+}
+
+// ---- unit-test hook of the section recurrence alone: X [T, R, W] -> h1 [T, R, H] (layer 1's hidden state of every
+// step) through the GEMM and the persistent kernel the f16 precisions run; packed receives the section image
+static int imp_sec_hook_check(int R, int T, int W, int H) {
+  FSN_REQUIRE(R > 0 && T > 0 && W > 0 && W <= 4096 && (size_t)T * R * 4 * H < ((size_t)1 << 31), FSN_ERR_SHAPE,
+              "section recurrence hook: bad shape R=%d T=%d W=%d H=%d", R, T, W, H);
+  FSN_REQUIRE(imp_sb_f16_ok(H), FSN_ERR_UNSUPPORTED, "section recurrence hook: hidden size %d (128, 256 or 384)", H);
+  return FSN_OK;
+}
+
+extern "C" size_t fsn_debug_imp_section_lstm_tc_workspace_bytes(int R, int T, int W, int H, int x3) {
+  if (imp_sec_hook_check(R, T, W, H)) return 0;
+  Carver c(nullptr);
+  ImpSecTcWs w;
+  imp_section_tc_carve(c, (size_t)T * R, W, H, x3 != 0, w);
+  return c.off;
+}
+
+extern "C" int fsn_debug_imp_section_lstm_tc(const fsn_seq_weights* sw, int W, int H, int x3, const float* X, int R, int T,
+                                             int stages, int cluster, void* packed, float* h1, void* workspace,
+                                             size_t workspace_bytes, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(sw && X && packed && h1, FSN_ERR_SHAPE, "section recurrence hook: null argument");
+  int rc = imp_sec_hook_check(R, T, W, H);
+  if (rc) return rc;
+  FSN_REQUIRE(cluster == 0 || cluster == 1 || cluster == 2 || cluster == 4, FSN_ERR_UNSUPPORTED,
+              "section recurrence hook: cluster size %d (0, 1, 2 or 4)", cluster);
+  FSN_REQUIRE(stages == 0 || (stages >= 2 && stages <= 4), FSN_ERR_UNSUPPORTED,
+              "section recurrence hook: ring depth %d (0, 2, 3 or 4)", stages);
+  Carver c(workspace);
+  ImpSecTcWs w;
+  imp_section_tc_carve(c, (size_t)T * R, W, H, x3 != 0, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes,
+              c.off);
+  w.h1 = h1;
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = sb_tc_pack_raw(sw, H, 0, 0, packed, st, x3 != 0, true))) return rc;
+  return imp_section_lstm_tc(*sw, packed, X, R, T, W, H, x3 != 0, w, st, stages, cluster);
 }

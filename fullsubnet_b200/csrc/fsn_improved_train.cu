@@ -99,6 +99,9 @@ static int imp_train_check(const fsn_improved_desc* d, int B, int L, ImpDims& m)
   FSN_REQUIRE(d && d->hop_length > 0 && d->win_length > 0 && d->win_length <= d->n_fft && d->fb_hidden > 0 &&
                   d->sb_hidden > 0,
               FSN_ERR_SHAPE, "improved training: bad descriptor");
+  // the fp16 precisions are built for inference only (imp_dims accepts them for fsn_improved_forward / _enhance)
+  FSN_REQUIRE(d->precision == FSN_PREC_FP32 || d->precision == FSN_PREC_TF32_TC, FSN_ERR_UNSUPPORTED,
+              "improved training: precision must be FSN_PREC_FP32 or FSN_PREC_TF32_TC");
   int rc = imp_dims(d, B, L, m);
   if (rc) return rc;
   FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "improved training: the GRU cell is not built");

@@ -548,11 +548,33 @@ struct SbTcArgs {
   int stamp_ctas, stamp_its;
 };
 size_t sb_tc_packed_bytes(const fsn_model_desc* d);
-size_t sb_tc_packed_bytes_raw(int H, bool x3);
+// proj: the image sb_proj_forward streams (W_hh0, W_ih1, W_hh1 and layer 1's biases; no W_ih0 and no Linear)
+size_t sb_tc_packed_bytes_raw(int H, bool x3, bool proj = false);
 int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed, cudaStream_t st);
-// weights of a 2-layer stack of hidden size H over Ksb inputs with a Linear(H -> fc_out <= 2) on top
-int sb_tc_pack_raw(const fsn_seq_weights* sb, int H, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3);
+// weights of a 2-layer stack of hidden size H over Ksb inputs with a Linear(H -> fc_out <= 2) on top; proj: the
+// sb_proj_forward image (w_ih[0], fc_w and fc_b are not read, Ksb and fc_out are ignored)
+int sb_tc_pack_raw(const fsn_seq_weights* sb, int H, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3,
+                   bool proj = false);
 int sb_tc_forward(const SbTcArgs& a, cudaStream_t st);
 bool sb_tc_supported(const fsn_model_desc* d);
+// FSN_TC_STAGES / FSN_TC_CLUSTER (defaults 4 / 1), read once
+void sb_tc_ring_defaults(int& stages, int& cluster);
+// the same kernel with a precomputed layer-0 input (sb_proj_lstm_tc_kernel): R independent rows over T steps,
+// P [T, R, 4H] = x W_ih0^T + b_ih0 + b_hh0 (fp32) -> h1 [T, R, H] (fp32), layer 1's hidden state of every step
+struct SbProjArgs {
+  const void* packed;       // sb_tc_pack_raw(..., proj = true) image
+  const float* P;
+  float* h1;
+  int R, T, H;
+  bool x3;
+  int stages, cluster;      // 0 = FSN_TC_STAGES / FSN_TC_CLUSTER
+};
+int sb_proj_forward(const SbProjArgs& a, cudaStream_t st);
+// improved_fullsubnet's section recurrence on the f16 precisions (fsn_improved.cu): P = (X W_ih0^T + b_ih0) + b_hh0 on the
+// tf32 GEMM (x3: compensated) over X [T, R, W], then sb_proj_forward into h1 [T, R, H].  ws: imp_section_tc_carve.
+struct ImpSecTcWs { LstmTcWs gemm; float *P, *h1; };
+void imp_section_tc_carve(Carver& c, size_t rows_T, int Wmax, int H, bool x3, ImpSecTcWs& w);
+int imp_section_lstm_tc(const fsn_seq_weights& sw, const void* packed, const float* X, int R, int T, int W, int H, bool x3,
+                        const ImpSecTcWs& w, cudaStream_t st, int stages = 0, int cluster = 0);
 
 }  // namespace fsn

@@ -33,6 +33,12 @@
 //
 // Warp roles (128 + 128 MT threads): 0 = weight-stage producer, 1 = idle, 2 = x_t gather, 3 = Linear(H->2) + output
 // staging (half 0) or the half's Linear partial sums sent to half 0 (half 1), 4.. = consumer warpgroups.
+//
+// PROJ (sb_proj_lstm_tc_kernel, improved_fullsubnet's sections, DESIGN 4.3): the same stack over rows whose layer-0
+// input is too wide for a 32-wide x_t.  The caller computes P = X W_ih0^T + b_ih0 + b_hh0 [T, R, 4H] (fp32) for all
+// steps first; the ring streams only W_hh0, W_ih1 and W_hh1 (packer mode `proj`), each layer-0 accumulator starts from
+// the cell's four gate values of P[t] instead of zero, and layer 1 stores h1_t (fp32) to h1 [T, R, H] instead of
+// running a Linear.  Warps 2 and 3 idle.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -66,10 +72,11 @@ struct PackedLayout {
   size_t off_bias, off_fcw, off_fcb, bytes;
 };
 
-__host__ __device__ inline PackedLayout packed_layout(int H, bool x3) {
+// proj: layer 0 streams W_hh0 only (its input projection is precomputed), and the Linear block stays zero
+__host__ __device__ inline PackedLayout packed_layout(int H, bool x3, bool proj = false) {
   PackedLayout L;
   L.H = H; L.MT = H / 128;
-  L.nkb0 = 1 + H / KS; L.nkb1 = 2 * H / KS;  // k ranges of 32 per slice
+  L.nkb0 = (proj ? 0 : 1) + H / KS; L.nkb1 = 2 * H / KS;  // k ranges of 32 per slice
   L.parts = x3 ? 2 : 1;
   L.tiles0 = (size_t)L.MT * L.nkb0 * L.parts;
   L.tiles1 = (size_t)L.MT * L.nkb1 * L.parts;
@@ -88,8 +95,8 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
                             const float* __restrict__ bih0, const float* __restrict__ bhh0,
                             const float* __restrict__ bih1, const float* __restrict__ bhh1,
                             const float* __restrict__ fcw, const float* __restrict__ fcb, int H, int Ksb, int x3,
-                            int fc_out, uint8_t* __restrict__ out) {
-  const PackedLayout L = packed_layout(H, x3 != 0);
+                            int fc_out, int proj, uint8_t* __restrict__ out) {
+  const PackedLayout L = packed_layout(H, x3 != 0, proj != 0);
   const size_t per_half = L.tiles0 + L.tiles1;
   const size_t total = 2 * per_half * 4 * US * 4;  // one thread per (stage, gate, row, 16-byte chunk)
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -112,7 +119,9 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
     for (int e = 0; e < 8; ++e) {
       const int kk = c * 8 + e;
       float w = 0.f;
-      if (layer == 0) {
+      if (layer == 0 && proj) {
+        w = whh0[(size_t)wrow * H + kb * KS + kk];
+      } else if (layer == 0) {
         if (kb == 0) { if (kk < Ksb) w = wih0[(size_t)wrow * Ksb + kk]; }
         else w = whh0[(size_t)wrow * H + (kb - 1) * KS + kk];
       } else {
@@ -125,17 +134,19 @@ __global__ void pack_kernel(const float* __restrict__ wih0, const float* __restr
     uint8_t* dst = out + st_abs * W_TILE + g * W_SUB + swz64_off(r, c * 8);
     *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(v);
   }
-  // biases (b_ih + b_hh, fp32) and the Linear layer (outputs beyond fc_out are zero)
+  // biases (b_ih + b_hh, fp32) and the Linear layer (outputs beyond fc_out are zero); proj: layer 0's biases are in P
+  // and there is no Linear, so both stay zero
   float* bias = reinterpret_cast<float*>(out + L.off_bias);
   float* pfcw = reinterpret_cast<float*>(out + L.off_fcw);
   float* pfcb = reinterpret_cast<float*>(out + L.off_fcb);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 4 * H; i += gridDim.x * blockDim.x) {
-    bias[i] = bih0[i] + bhh0[i];
+    bias[i] = proj ? 0.f : bih0[i] + bhh0[i];
     bias[4 * H + i] = bih1[i] + bhh1[i];
   }
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * H; i += gridDim.x * blockDim.x)
-    pfcw[i] = (i < fc_out * H) ? fcw[i] : 0.f;
-  if (blockIdx.x == 0 && threadIdx.x < 2) pfcb[threadIdx.x] = ((int)threadIdx.x < fc_out) ? fcb[threadIdx.x] : 0.f;
+    pfcw[i] = (!proj && i < fc_out * H) ? fcw[i] : 0.f;
+  if (blockIdx.x == 0 && threadIdx.x < 2)
+    pfcb[threadIdx.x] = (!proj && (int)threadIdx.x < fc_out) ? fcb[threadIdx.x] : 0.f;
 }
 
 // ---------------------------------------------------------------- shared-memory plan
@@ -197,6 +208,8 @@ struct KArgs {
   RowMap map;
   long long* stamps;  // PROBE instantiation only: records of CTAs [0, stamp_ctas), iterations [0, stamp_its)
   int stamp_ctas, stamp_its;
+  // PROJ instantiation only: layer 0's input projection P [Tp, R, 4H] and the layer-1 output h1 [Tp, R, H] (fp32)
+  const float* proj; float* h1;
 };
 
 // ---------------------------------------------------------------- cycle stamps (PROBE instantiation)
@@ -263,10 +276,24 @@ __device__ __forceinline__ void release_stage(uint32_t bar, uint32_t pred, uint3
   mbar_arrive_remote_elect_if(bar, rank, pred & remote);
 }
 
+// PROJ: gate g of layer 0 for accumulator register i of consumer thread (warp q, lane) of slice s at step t, P[t][row0 +
+// n][g H + u] with unit u = 64 s + 16 q + lane/4 + 8 hh and row n = 8 j + 2 (lane % 4) + e for i = 4 j + 2 hh + e (rows
+// past R read row R - 1; their results are never stored).  x3 starts the accumulators from it, which hides the load
+// behind the ring waits; the single pass adds it after the MMAs, because there the loaded accumulators make ptxas
+// serialise the MMAs (C7515), and with x3 the later add costs 120 bytes of spills instead of none (DESIGN 4.3)
+__device__ __forceinline__ float proj_at(const KArgs& a, int t, int row0, int s, int q, int lane, int g, int i) {
+  const int j = i >> 2, hh = (i >> 1) & 1, e = i & 1;
+  const int u = s * US + 16 * q + (lane >> 2) + 8 * hh;
+  const int r = min(row0 + 8 * j + 2 * (lane & 3) + e, a.R - 1);
+  return __ldg(a.proj + ((size_t)t * a.R + r) * 4 * a.H + g * a.H + u);
+}
+
 // PROBE: the same kernel with cycle stamps (ProbeField) written to a.stamps; the production launches use PROBE = false,
-// where every stamp below compiles away
-template <bool X3, bool PROBE>
-__global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_constant__ KArgs a) {
+// where every stamp below compiles away.  PROJ: the precomputed layer-0 projection and stored h1 (see the top of the
+// file); every PROJ branch below is `if constexpr` or folds away, so the sb_lstm_tc_kernel instantiations are the code
+// they were before the policy existed
+template <bool X3, bool PROBE, bool PROJ>
+__device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
   constexpr int PARTS = X3 ? 2 : 1;
   // probe clock: cycles since the previous mark (0 and no code without PROBE)
   long long pt = 0;
@@ -299,7 +326,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
   const uint16_t cl_mask = (uint16_t)((0x55u & ((1u << (2 * CL)) - 1u)) << half);
   const Smem sp = smem_plan(H, STAGES, X3);
   const uint32_t LO = sp.lo - sp.x;  // byte offset of a lo copy from its hi copy
-  const PackedLayout PL = packed_layout(H, X3);
+  const PackedLayout PL = packed_layout(H, X3, PROJ);
   Bars& bars = *reinterpret_cast<Bars*>(smem + sp.bars);
   RowInfo* rows = reinterpret_cast<RowInfo*>(smem + sp.rows);
   float* fc_part = reinterpret_cast<float*>(smem + sp.fcw);
@@ -325,7 +352,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
     for (int m = 0; m < MAX_MT; ++m) mbar_init(&bars.turn[m], 4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (threadIdx.x < NB) {
+  if (!PROJ && threadIdx.x < NB) {
     RowInfo ri;
     const int r = row0 + threadIdx.x;
     ri.src_b = -1; ri.src_f = 0; ri.scale = 0.f; ri.out_idx = 0;
@@ -383,7 +410,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
         r[PF_STAGES] = (long long)(t_end - t_begin); r[PF_GT_BEGIN] = p_g0;
       }
     }
-  } else if (warp == 2) {
+  } else if (!PROJ && warp == 2) {
     // ================= x_t gather: sub-band unit = 2Ns+1 reflected magnitude rows + 2Nf+1 full-band rows,
     // scaled by 1/(mu'+1e-5)  (base_model.py:35-44, model.py:98-111), fp16 (X3: + lo), B-operand layout.
     // Both CTAs of a pair gather all NB rows (a duplicated L2 read is cheaper than an exchange)
@@ -420,7 +447,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars.x_full[t & 1]);
     }
-  } else if (warp == 3) {
+  } else if (!PROJ && warp == 3) {
     // ================= Linear(H -> 2), one row per lane: sums the fp32 partial dot products of the consumer warps.
     // Half 1 sends its sums to half 0; half 0 adds the bias, its own sums and half 1's (one fixed association
     // order), stages OUT_T frames and stores crm[b', o, f', t - la]  (model.py:129-135 fused)
@@ -512,7 +539,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
           // kernel's waits on the weight ring and the state are CTA-scope: each of those barriers guards data written
           // by this CTA or by an async-proxy copy with complete_tx (TMA from L2, the peer's DSMEM bulk copy)
           if (layer == 0) {
-            mbar_wait_cta<false>(&bars.x_full[t & 1], (t >> 1) & 1);
+            if constexpr (!PROJ) mbar_wait_cta<false>(&bars.x_full[t & 1], (t >> 1) & 1);
             for (; h0_seen < t; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready[h0_seen & 1], (h0_seen >> 1) & 1);      // h0_{t-1}
           } else {
             for (; h0_seen < t + 1; ++h0_seen) mbar_wait_cta<false>(&bars.h0_ready[h0_seen & 1], (h0_seen >> 1) & 1);  // h0_t
@@ -530,7 +557,26 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
           for (int g = 0; g < 4; ++g) {
 #pragma unroll
             for (int i = 0; i < 16; ++i) acc[g][i] = 0.f;
+            if constexpr (PROJ && X3) {
+              if (layer == 0) {
+#pragma unroll
+                for (int i = 0; i < 16; ++i) acc[g][i] = proj_at(a, t, row0, s, q, lane, g, i);
+              }
+            }
             wg::fence_operand(acc[g]);
+          }
+          if constexpr (PROJ && !X3) {
+            // single pass: layer 0 adds P[t] after its MMAs (see proj_at); pull this warp's P lines into L2 now, 32
+            // rows x 4 gates of 16 units (64 B) each
+            if (layer == 0) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const int idx = lane + 32 * i;
+                const int r = min(row0 + (idx & 31), a.R - 1);
+                const float* p = a.proj + ((size_t)t * a.R + r) * 4 * H + (idx >> 5) * H + s * US + 16 * q;
+                asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+              }
+            }
           }
           int prev_stage = -1;
           if (m > 0 || !first_block) { mbar_wait_cta<false>(&bars.turn[m], turns & 1); ++turns; }
@@ -575,7 +621,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
           };
           // B operand k ranges: layer 0: [x_t (32 k, one 64B-swizzled block)] [h0_{t-1} (H)]; layer 1: [h0_t (H)]
           // [h1_{t-1} (H)].  A k-block of h (64 k, 128B-swizzled) is two k ranges, 64 B apart in the swizzle row
-          if (layer == 0) {
+          if (!PROJ && layer == 0) {
 #pragma unroll
             for (int part = 0; part < PARTS; ++part) issue_stage(part, wg::desc_lo(x_addr), wg::DESC_SW64_HI, 0u);
           }
@@ -599,18 +645,26 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
           wg::wait<0>();
 #pragma unroll
           for (int g = 0; g < 4; ++g) wg::fence_operand(acc[g]);
+          if constexpr (PROJ && !X3) {
+            if (layer == 0) {
+#pragma unroll
+              for (int g = 0; g < 4; ++g)
+#pragma unroll
+                for (int i = 0; i < 16; ++i) acc[g][i] += proj_at(a, t, row0, s, q, lane, g, i);
+            }
+          }
           p_wgw += mark();
           if constexpr (PROBE) { p_lat += (uint32_t)(pt - p_commit_prev); p_mma1 = pt; }
           release_stage(w_empty0 + 8 * prev_stage, 1u, rel_local, rel_remote, rel_rank);
           // this warpgroup's MMAs of the step have consumed x_t / h1_{t-1}
-          if (lane == 0) mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
+          if (lane == 0 && (!PROJ || layer)) mbar_arrive(layer ? &bars.l1_done : &bars.x_empty[t & 1]);
           if (layer == 1 && lane == 0) {
             // ... and h0_t / h1_{t-1}, including the peer's half that the peer copied in: the peer may copy again
             if (q == 2) mbar_arrive_remote(&bars.h0_empty[t & 1], peer);
             if (q == 3) mbar_arrive_remote(&bars.h1_empty, peer);
           }
           p_cell += mark();
-          if (layer == 1 && t >= 1) mbar_wait_cta<false>(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
+          if (!PROJ && layer == 1 && t >= 1) mbar_wait_cta<false>(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
           p_fc += mark();
           float fsum[2][8];  // Linear partials [o][row slot j*2+e]
 #pragma unroll
@@ -637,26 +691,32 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
                 const __half hi = __float2half_rn(h);
                 hv[hh][j * 2 + e] = hi;
                 lv[hh][j * 2 + e] = __float2half_rn(h - __half2float(hi));
-                if (layer) { fsum[0][j * 2 + e] += h * w0; fsum[1][j * 2 + e] += h * w1; }
+                if (!PROJ && layer) { fsum[0][j * 2 + e] += h * w0; fsum[1][j * 2 + e] += h * w1; }
+                if constexpr (PROJ) {
+                  const int r = row0 + 8 * j + 2 * (lane & 3) + e;
+                  if (layer && r < a.R) a.h1[((size_t)t * a.R + r) * H + u] = h;
+                }
               }
           }
           if (layer == 1) {
-            // Linear(H->2) in fp32: sum over the warp's units (lanes with equal lane % 4 hold the same rows)
-#pragma unroll
-            for (int o = 0; o < 2; ++o)
-#pragma unroll
-              for (int r = 0; r < 8; ++r) {
-                float v = fsum[o][r];
-                v += __shfl_xor_sync(0xffffffffu, v, 4);
-                v += __shfl_xor_sync(0xffffffffu, v, 8);
-                v += __shfl_xor_sync(0xffffffffu, v, 16);
-                fsum[o][r] = v;
-              }
-            if (lane < 4) {
+            if constexpr (!PROJ) {
+              // Linear(H->2) in fp32: sum over the warp's units (lanes with equal lane % 4 hold the same rows)
 #pragma unroll
               for (int o = 0; o < 2; ++o)
 #pragma unroll
-                for (int r = 0; r < 8; ++r) my_part[o * NB + 8 * (r >> 1) + 2 * lane + (r & 1)] = fsum[o][r];
+                for (int r = 0; r < 8; ++r) {
+                  float v = fsum[o][r];
+                  v += __shfl_xor_sync(0xffffffffu, v, 4);
+                  v += __shfl_xor_sync(0xffffffffu, v, 8);
+                  v += __shfl_xor_sync(0xffffffffu, v, 16);
+                  fsum[o][r] = v;
+                }
+              if (lane < 4) {
+#pragma unroll
+                for (int o = 0; o < 2; ++o)
+#pragma unroll
+                  for (int r = 0; r < 8; ++r) my_part[o * NB + 8 * (r >> 1) + 2 * lane + (r & 1)] = fsum[o][r];
+              }
             }
             p_cell += mark();
             // every layer-1 MMA of this step in this CTA has consumed h1_{t-1}: overwrite it with h1_t
@@ -719,6 +779,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_co
   cluster_sync_all();  // no CTA leaves while a peer may still signal its barriers or copy into it
 }
 
+// fullsubnet's sub-band stack and fast_fullsubnet's bottleneck: gathered x_t, fused Linear
+template <bool X3, bool PROBE>
+__global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_constant__ KArgs a) {
+  sb_lstm_tc_body<X3, PROBE, false>(a);
+}
+
+// improved_fullsubnet's sections: precomputed layer-0 projection, h1 stored for the caller's head
+template <bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) sb_proj_lstm_tc_kernel(const __grid_constant__ KArgs a) {
+  sb_lstm_tc_body<X3, false, true>(a);
+}
+
 }  // namespace tc
 
 static int sb_ksb(const fsn_model_desc* d) { return (2 * d->sb_num_neighbors + 1) + (2 * d->fb_num_neighbors + 1); }
@@ -730,22 +802,23 @@ bool sb_tc_supported(const fsn_model_desc* d) {
   return sb_tc_shape_ok(d->sb_hidden, sb_ksb(d));
 }
 
-size_t sb_tc_packed_bytes_raw(int H, bool x3) { return tc::packed_layout(H, x3).bytes; }
+size_t sb_tc_packed_bytes_raw(int H, bool x3, bool proj) { return tc::packed_layout(H, x3, proj).bytes; }
 
 size_t sb_tc_packed_bytes(const fsn_model_desc* d) {
   if (!sb_tc_supported(d)) return 0;
   return sb_tc_packed_bytes_raw(d->sb_hidden, d->precision == FSN_PREC_F16X3_TC);
 }
 
-int sb_tc_pack_raw(const fsn_seq_weights* sb, int H, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3) {
-  FSN_REQUIRE(sb_tc_shape_ok(H, Ksb), FSN_ERR_UNSUPPORTED,
+int sb_tc_pack_raw(const fsn_seq_weights* sb, int H, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3,
+                   bool proj) {
+  FSN_REQUIRE(sb_tc_shape_ok(H, proj ? 0 : Ksb), FSN_ERR_UNSUPPORTED,
               "the fp16 tensor-core LSTM stack needs a hidden size in {128,256,384} and an input width <= 32");
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   tc::pack_kernel<<<sms * 4, 256, 0, st>>>(sb->w_ih[0], sb->w_hh[0], sb->w_ih[1], sb->w_hh[1], sb->b_ih[0], sb->b_hh[0],
                                            sb->b_ih[1], sb->b_hh[1], sb->fc_w, sb->fc_b, H, Ksb, x3 ? 1 : 0, fc_out,
-                                           (uint8_t*)packed);
+                                           proj ? 1 : 0, (uint8_t*)packed);
   FSN_CHECK_LAUNCH("sb pack_kernel");
   return FSN_OK;
 }
@@ -760,11 +833,11 @@ int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed,
 // alive while cfg is used)
 template <bool X3, bool PROBE = false>
 static int sb_tc_config(int H, int stages, int cluster, int pairs, cudaStream_t st, cudaLaunchConfig_t& cfg,
-                        cudaLaunchAttribute* attr) {
+                        cudaLaunchAttribute* attr, const void* kern = (const void*)tc::sb_lstm_tc_kernel<X3, PROBE>) {
   const tc::Smem sp = tc::smem_plan(H, stages, X3);
   const size_t smem = sp.total + 1024;  // slack for the 1024-byte alignment of the dynamic segment
-  int rc = check_cuda(cudaFuncSetAttribute(tc::sb_lstm_tc_kernel<X3, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)smem), "sb_lstm_tc smem attr");
+  int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                      "sb_lstm_tc smem attr");
   if (rc) return rc;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(2 * pairs);
@@ -804,6 +877,44 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
   a.stamps = s.stamps; a.stamp_ctas = s.stamp_ctas; a.stamp_its = s.stamp_its;
   FSN_REQUIRE(sb_tc_shape_ok(a.H, a.Ksb), FSN_ERR_UNSUPPORTED, "sb_lstm_tc: unsupported hidden size %d / input width %d",
               a.H, a.Ksb);
+  a.proj = nullptr; a.h1 = nullptr;
+  int stages = 0, cluster = 0;
+  sb_tc_ring_defaults(stages, cluster);
+  // an explicit launch configuration (the unit-test hook) overrides the environment
+  a.stages = s.stages ? s.stages : stages;
+  a.cluster = s.cluster ? s.cluster : cluster;
+  if (s.stamps) return s.x3 ? sb_tc_launch<true, true>(a, s.H, st) : sb_tc_launch<false, true>(a, s.H, st);
+  return s.x3 ? sb_tc_launch<true, false>(a, s.H, st) : sb_tc_launch<false, false>(a, s.H, st);
+}
+
+int sb_proj_forward(const SbProjArgs& s, cudaStream_t st) {
+  FSN_REQUIRE(s.R > 0 && s.T > 0 && sb_tc_shape_ok(s.H, 0), FSN_ERR_UNSUPPORTED,
+              "sb_proj_lstm_tc: unsupported hidden size %d (R=%d, T=%d)", s.H, s.R, s.T);
+  FSN_REQUIRE(s.packed && s.P && s.h1, FSN_ERR_SHAPE, "sb_proj_lstm_tc: missing buffer");
+  tc::KArgs a;
+  memset(&a, 0, sizeof(a));
+  a.packed = (const uint8_t*)s.packed; a.proj = s.P; a.h1 = s.h1;
+  a.R = s.R; a.Tp = s.T; a.T = s.T; a.H = s.H;
+  int stages = 0, cluster = 0;
+  sb_tc_ring_defaults(stages, cluster);
+  a.stages = s.stages ? s.stages : stages;
+  a.cluster = s.cluster ? s.cluster : cluster;
+  const int pairs = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  const void* kern = s.x3 ? (const void*)tc::sb_proj_lstm_tc_kernel<true> : (const void*)tc::sb_proj_lstm_tc_kernel<false>;
+  int rc = s.x3 ? sb_tc_config<true>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, kern)
+                : sb_tc_config<false>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, kern);
+  if (rc) return rc;
+  rc = s.x3 ? check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_proj_lstm_tc_kernel<true>, a), "sb_proj_lstm_tc_kernel launch")
+            : check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_proj_lstm_tc_kernel<false>, a), "sb_proj_lstm_tc_kernel launch");
+  if (rc) return rc;
+  FSN_CHECK_LAUNCH("sb_proj_lstm_tc_kernel");
+  return FSN_OK;
+}
+
+// weight ring depth and cluster size of the production launches: FSN_TC_STAGES / FSN_TC_CLUSTER, read once
+void sb_tc_ring_defaults(int& stages, int& cluster) {
   static int stages_env = -1;
   if (stages_env < 0) {
     const char* e = getenv("FSN_TC_STAGES");
@@ -819,11 +930,8 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
     cluster_env = e ? atoi(e) : 1;
     if (cluster_env != 1 && cluster_env != 2 && cluster_env != 4) cluster_env = 1;
   }
-  // an explicit launch configuration (the unit-test hook) overrides the environment
-  a.stages = s.stages ? s.stages : stages_env;
-  a.cluster = s.cluster ? s.cluster : cluster_env;
-  if (s.stamps) return s.x3 ? sb_tc_launch<true, true>(a, s.H, st) : sb_tc_launch<false, true>(a, s.H, st);
-  return s.x3 ? sb_tc_launch<true, false>(a, s.H, st) : sb_tc_launch<false, false>(a, s.H, st);
+  stages = stages_env;
+  cluster = cluster_env;
 }
 
 }  // namespace fsn

@@ -71,9 +71,15 @@ class Model(BaseModel):
             # model.py:226-236 also offers cumulative_laplace_norm / offline_gaussian_norm
             raise NotImplementedError("libfsn_b200 builds offline_laplace_norm for improved_fullsubnet")
         self.norm_type = norm_type
-        # arithmetic of the sub-band sections (98 % of the FLOPs): "fp32" (FMA kernels), "tf32_tc" (wgmma tf32
-        # GEMMs, fp32 accumulate; waveform within 1e-4 of the reference) or "auto" (= tf32_tc when sb_hidden % 4 == 0)
+        # arithmetic of the sub-band sections (98 % of the FLOPs):
+        #   "fp32"     FMA kernels
+        #   "tf32_tc"  wgmma tf32 GEMMs, fp32 accumulate, one launch per layer and step (waveform within 1e-4)
+        #   "f16x3_tc" each section in one persistent wgmma launch, fp16 hi+lo split of weights and state: the fp32
+        #              error class (sb_hidden in {128, 256, 384}); the full band on the compensated tensor-core layers
+        #   "f16_tc"   the same with single fp16 / tf32 passes
+        #   "auto"     tf32_tc when sb_hidden % 4 == 0, else fp32
         self.precision = os.environ.get("FSN_IMPROVED_PRECISION", "auto")
+        self._packed = {}  # section -> (key, fsn_improved_pack_sb_weights image)
         # arithmetic of the training step's GEMMs: "fp32" (FMA) | "tf32_tc" (wgmma tf32 for the LSTM layers) | "auto" =
         # tf32_tc when fb_hidden_size and sb_hidden_size are multiples of 4
         self.train_precision = os.environ.get("FSN_TRAIN_PRECISION", "auto")
@@ -82,16 +88,34 @@ class Model(BaseModel):
         ok = self.sb_model.sb_models[0].hidden_size % 4 == 0
         if self.precision == "auto":
             return "tf32_tc" if ok else "fp32"
-        if self.precision not in ("fp32", "tf32_tc"):
-            raise ValueError("precision must be 'fp32', 'tf32_tc' or 'auto'")
+        if self.precision not in ("fp32", "tf32_tc", "f16x3_tc", "f16_tc"):
+            raise ValueError("precision must be 'fp32', 'tf32_tc', 'f16x3_tc', 'f16_tc' or 'auto'")
         return self.precision
 
-    def _structs(self):
-        return self._desc(self._resolve_precision()), self._weights()
+    def _structs(self, device=None):
+        d, w = self._desc(self._resolve_precision()), self._weights()
+        if d.precision in (_lib.PREC["f16x3_tc"], _lib.PREC["f16_tc"]):
+            for s in range(d.num_sections):
+                w.sb_packed[s] = self._packed_section(d, w, s, device)
+        return d, w
+
+    def _packed_section(self, desc, w, s, device):
+        """fp16 image of section s's recurrent weights (fsn_improved_pack_sb_weights), rebuilt when any of its parameters
+        changes."""
+        key = (self.sb_model.sb_models[s].version_key(), str(device), int(desc.precision), int(desc.sb_hidden))
+        hit = self._packed.get(s)
+        if hit is None or hit[0] != key:
+            lib = _lib.load()
+            n = _lib.check_workspace(lib.fsn_improved_packed_bytes(C.byref(desc), s))
+            buf = torch.empty(n, dtype=torch.uint8, device=device)
+            _lib.check(lib.fsn_improved_pack_sb_weights(C.byref(desc), C.byref(w), s, buf.data_ptr(),
+                                                        _lib.stream_ptr(device)))
+            hit = self._packed[s] = (key, buf)
+        return hit[1].data_ptr()
 
     def _enhance_args(self, device):
         self._check_sections()
-        d, w = self._structs()
+        d, w = self._structs(device)
         return d, (C.byref(w),)
 
     def _desc(self, precision: str) -> "_lib.ImprovedDesc":
@@ -166,7 +190,7 @@ class Model(BaseModel):
             return TrainStep.apply(self, x, *self.parameters())
         lib = _lib.load()
         with torch.cuda.device(x.device):
-            d, w = self._structs()
+            d, w = self._structs(x.device)
             n = _lib.check_workspace(lib.fsn_improved_workspace_bytes(C.byref(d), B, L))
             ws = torch.empty(n, dtype=torch.uint8, device=x.device)
             out = torch.empty(B, 1, L, dtype=torch.float32, device=x.device)

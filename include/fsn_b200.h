@@ -75,7 +75,9 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
  * workspace query), fsn_si_sdr_lengths (the grouped validation loss and SI-SDR), fsn_clip_adam_steps (one Adam step
  * count per tensor) and fsn_stoi (+ its workspace query and the fsn_debug_stoi_stages hook).  FSN_NORM_FORGETTING is a new
  * value of an existing field, refused by every older entry point it does not apply to, with the fsn_debug_forgetting_*
- * hooks. */
+ * hooks.  fsn_improved_weights grew sb_packed, read only by the FSN_PREC_F16X3_TC / FSN_PREC_F16_TC precisions that
+ * fsn_improved_forward / _enhance accept since, with fsn_improved_packed_bytes / fsn_improved_pack_sb_weights and the
+ * fsn_debug_imp_section_lstm_tc hook: a caller of the shorter struct never selects them, so the version stays 102. */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -259,14 +261,36 @@ typedef struct fsn_improved_desc {
   int32_t sb_num_center[FSN_IMP_MAX_SECTIONS], sb_num_neighbor[FSN_IMP_MAX_SECTIONS];
   int32_t fb_num_center[FSN_IMP_MAX_SECTIONS], fb_num_neighbor[FSN_IMP_MAX_SECTIONS];
   int32_t fb_hidden, sb_hidden, fb_activation, sb_activation;
-  int32_t precision; /* FSN_PREC_FP32, or FSN_PREC_TF32_TC: the sub-band sections' GEMMs on wgmma tf32 */
+  int32_t precision; /* inference (fsn_improved_forward / _enhance):
+                      *   FSN_PREC_FP32     - fp32 FMA kernels
+                      *   FSN_PREC_TF32_TC  - the sections' layers on wgmma tf32, one launch per layer and step
+                      *                       (sb_hidden % 4 == 0)
+                      *   FSN_PREC_F16X3_TC - each section's input projection on the compensated tf32 GEMM, both LSTM
+                      *                       layers of all steps in one persistent fp16 hi+lo wgmma launch, the head once
+                      *                       over all steps; the full band on the compensated tensor-core layers.
+                      *                       sb_hidden in {128, 256, 384}; needs w->sb_packed (the fp32 error class)
+                      *   FSN_PREC_F16_TC   - the same with single fp16 / tf32 passes (cRM within 1e-3 rel)
+                      * training (fsn_improved_train_*): FSN_PREC_FP32 or FSN_PREC_TF32_TC only */
   int32_t cell_type; /* FSN_CELL_* (`sequence_model`); read by the training step only, which is built for LSTM */
 } fsn_improved_desc;
 
 typedef struct fsn_improved_weights {
   fsn_seq_weights fb;                          /* fb_model */
   fsn_seq_weights sb[FSN_IMP_MAX_SECTIONS];    /* sb_model.sb_models[s] */
+  /* FSN_PREC_F16X3_TC / FSN_PREC_F16_TC: fsn_improved_pack_sb_weights() image of section s, else unread (NULL).
+   * Appended after 102: only those precisions read it, so a caller built against the shorter struct is unaffected. */
+  const void* sb_packed[FSN_IMP_MAX_SECTIONS];
 } fsn_improved_weights;
+
+/* Packed section weights of the fp16 tensor-core precisions, mirroring fsn_fast_pack_bn_weights: the tile-ordered fp16
+ * (x3: hi + lo) image of section s's W_hh0, W_ih1, W_hh1 and layer-1 biases that its persistent kernel streams (W_ih0 and
+ * the Linear run outside it).  fsn_improved_packed_bytes: 0 (fsn_last_error_code set, no CUDA call) for other precisions,
+ * unsupported shapes or section outside [0, num_sections).  fsn_improved_pack_sb_weights fills `packed` on `stream`
+ * from w->sb[section]; rebuild it whenever those weights change (cache it keyed on their version and the precision).
+ * No allocation, no host synchronisation. */
+size_t fsn_improved_packed_bytes(const fsn_improved_desc* d, int section);
+int fsn_improved_pack_sb_weights(const fsn_improved_desc* d, const fsn_improved_weights* w, int section, void* packed,
+                                 fsn_stream_t stream);
 
 size_t fsn_improved_workspace_bytes(const fsn_improved_desc* d, int B, int L);
 /* Model.forward (improved_fullsubnet/model.py:541-591): wav [B,L] -> enhanced [B,L] (the reference returns
@@ -755,6 +779,16 @@ int fsn_debug_imp_unfold_bwd(const float* dX, const float* Xn, const float* invs
                              fsn_stream_t stream);
 int fsn_debug_imp_section_input(const float* magc, const float* fbT, int B, int T, int Fu, int lo, int hi, int cs, int ns,
                                 int cf, int nf, int tm, float* X, float* fs, fsn_stream_t stream);
+/* unit-test hook of improved_fullsubnet's section recurrence on FSN_PREC_F16X3_TC (x3 = 1) / FSN_PREC_F16_TC (x3 = 0):
+ * R independent rows of X [T, R, W] through the 2-layer LSTM of `sw` (w_ih[0] [4H, W]; fc_w / fc_b unread) -> h1 [T, R, H],
+ * layer 1's hidden state of every step, by the path fsn_improved_forward runs (input projection on the tf32 GEMM, then
+ * the persistent kernel).  packed receives the section image (fsn_debug_sb_lstm_tc_packed_bytes is not its size: use
+ * fsn_improved_packed_bytes).  stages / cluster: weight ring depth (0, 2, 3, 4) and pairs per cluster (0, 1, 2, 4), 0 =
+ * the production default.  H in {128, 256, 384}; every check precedes the first CUDA call. */
+size_t fsn_debug_imp_section_lstm_tc_workspace_bytes(int R, int T, int W, int H, int x3);
+int fsn_debug_imp_section_lstm_tc(const fsn_seq_weights* sw, int W, int H, int x3, const float* X, int R, int T, int stages,
+                                  int cluster, void* packed, float* h1, void* workspace, size_t workspace_bytes,
+                                  fsn_stream_t stream);
 
 /* unit-test hooks for the statistics of the offline norms (fsn_lstm_simt.cu, fsn_train.cu; base_model.py:203-218 with
  * the closed-form second-norm mean of model.py:98-111).  float2 outputs are pairs of floats.
