@@ -1,9 +1,10 @@
-"""Chunked streaming throughput of fullband_baseline (fsn_fullband_stream_step) or fast_fullsubnet (fsn_fast_stream_step,
---model fast_fullsubnet): ms per call, audio seconds enhanced per wall second and concurrent real-time streams for
-slots x K, with the whole-clip fp32 rate of the same process beside it (fsn_fullband_enhance; fast_fullsubnet:
-Inferencer.enhance_batch).  For fast_fullsubnet each line also gives the bottleneck's share of the call's GPU time, from
-a torch.profiler pass of its own after the timed calls.  Prints one JSON line per configuration and a header line with
-the GPU, power limit and clocks.
+"""Chunked streaming throughput of fullband_baseline (fsn_fullband_stream_step), fullsubnet (fsn_stream_step, --model
+fullsubnet, precision="fp32") or fast_fullsubnet (fsn_fast_stream_step, --model fast_fullsubnet): ms per call, audio
+seconds enhanced per wall second and concurrent real-time streams for slots x K, with the whole-clip fp32 rate of the
+same process beside it (fsn_fullband_enhance; fullsubnet: fsn_enhance; fast_fullsubnet: Inferencer.enhance_batch).  For
+fullsubnet and fast_fullsubnet each line also says whether every slot stays real-time; for fast_fullsubnet it gives the
+bottleneck's share of the call's GPU time, from a torch.profiler pass of its own after the timed calls.  Prints one
+JSON line per configuration and a header line with the GPU, power limit and clocks.
 
     python bench_stream.py [--model fullband_baseline] [--slots 1 64 256] [--ks 1 4 16 64] [--calls 20] [--warmup 3]"""
 from __future__ import annotations
@@ -34,6 +35,13 @@ def model(name, norm, dev):
         args = dict(FO.DEFAULT_FAST_ARGS, norm_type=norm)
         m = Model(**args, precision="fp32")
         m.load_state_dict(FO.make_fast_state_dict(seed=11, args=args), strict=True)
+        return m.to(dev).eval()
+    if name == "fullsubnet":
+        from fullsubnet_b200.fullsubnet.model import Model
+        from oracle import fullsubnet_oracle as O
+        args = dict(O.DEFAULT_MODEL_ARGS, norm_type=norm)
+        m = Model(**args, precision="fp32")
+        m.load_state_dict(O.make_state_dict(seed=11, args=args), strict=True)
         return m.to(dev).eval()
     from fullsubnet_b200.fullband_baseline.model import Model
     from oracle import fullband_baseline_oracle as BO
@@ -86,7 +94,7 @@ def main():
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--norm", default="cumulative_laplace_norm")
-    ap.add_argument("--model", default="fullband_baseline", choices=["fullband_baseline", "fast_fullsubnet"])
+    ap.add_argument("--model", default="fullband_baseline", choices=["fullband_baseline", "fullsubnet", "fast_fullsubnet"])
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_stream.py needs a CUDA device"
     dev = torch.device("cuda:0")
@@ -106,8 +114,9 @@ def main():
             rt = slots if ms <= chunk_ms else int(slots * chunk_ms / ms)
             line = {"slots": slots, "K": K, "ms_per_call": round(ms, 3), "chunk_ms": chunk_ms,
                     "audio_s_per_s": round(audio_rate, 1), "realtime_streams": rt, "delay": s.delay}
-            if fast:
+            if a.model != "fullband_baseline":
                 line["all_realtime"] = ms <= chunk_ms
+            if fast:
                 line["bottleneck_share"] = bottleneck_share(lambda: s.step(x))
             print(json.dumps(line))
         del s

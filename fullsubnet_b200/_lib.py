@@ -167,6 +167,11 @@ _SIGNATURES = {
     "fsn_fast_stream_delay": (C.c_int, [C.POINTER(FastDesc), _I, _I]),
     "fsn_fast_stream_step": (C.c_int, [C.POINTER(FastDesc), C.POINTER(FastWeights), _P, _P, _P, _I, _I, _I, _I, _I, _P, _P,
                                        _S, _P, _S, _P]),
+    "fsn_stream_state_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I]),
+    "fsn_stream_workspace_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I, _I]),
+    "fsn_stream_delay": (C.c_int, [C.POINTER(ModelDesc), _I, _I]),
+    "fsn_stream_step": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P, _P, _I, _I,
+                                  _I, _I, _I, _P, _P, _S, _P, _S, _P]),
     "fsn_fullband_train_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
     "fsn_fullband_train_forward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, _P, _P, _S, _P]),
     "fsn_fullband_train_backward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, C.POINTER(FullbandGrads), _P,

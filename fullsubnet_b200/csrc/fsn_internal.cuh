@@ -83,10 +83,12 @@ struct StepParams {
 
 int lstm_step_launch(const StepParams& p, int mode, cudaStream_t st);
 // per-step state of a two-layer stack: layer 0's h ping-pong h0[2] [R,H0] and cell c0; layer 1's cell c1 and its h, either
-// a ping-pong h1[2] [R,H1] (keep_steps = 0) or one [R, keep_steps, H1] tensor h1[0] that keeps every step
+// a ping-pong h1[2] [R,H1] (keep_steps = 0) or one [R, keep_steps, H1] tensor h1[0] that keeps every step.  carry (chunked
+// streaming): step 0 continues from the state in h0[1], c0, h1_at(-1) and c1 instead of starting from zero.
 struct Step2State {
   float *h0[2], *c0, *h1[2], *c1;
   int H1, keep_steps;
+  bool carry;
   float* h1_at(int t) const { return keep_steps ? h1[0] + (size_t)(t > 0 ? t : 0) * H1 : h1[t & 1]; }
   size_t h1_stride() const { return (size_t)(keep_steps ? keep_steps : 1) * H1; }
 };
@@ -99,6 +101,14 @@ int lstm_step2_launch(StepParams p, int mode, int t, const fsn_lstm_layer& w1, c
 int cum_clip_scale_launch(const float2* fs, int B, int Tp, int F, float eps, float* scale1T, cudaStream_t st);
 int cum_unit_scale_launch(const float* magT, const float* fbT, RowMap map, int R, int Tp, int Ns, int Nf, float eps,
                           float* scaleT, cudaStream_t st, bool time_major = false);
+// one frame's sum over the features of sub-band unit f, in the order of cum_unit_scale_kernel and its streaming variant:
+// the 2Ns+1 reflected rows of mag, then the 2Nf+1 reflected rows of fb (both [F] of that frame)
+__device__ __forceinline__ float unit_frame_sum(const float* mag, const float* fb, int f, int F, int Ns, int Nf) {
+  float s = 0.f;
+  for (int k = -Ns; k <= Ns; ++k) s += mag[reflect_idx(f + k, F)];
+  for (int k = -Nf; k <= Nf; ++k) s += fb[reflect_idx(f + k, F)];
+  return s;
+}
 // forgetting_norm (base_model.py:102-151): mu_t = a_t mu_{t-1} + b_t m_t per clip, m_t the mean of frame t over the
 // features, scale 1 / (mu_t + 1e-10).  The coefficients are rounded as the reference rounds them: for t < 192,
 // a_t = float32(min((t-1)/(t+1), alpha)) and b_t = 1 - a_t in float32 (a_0 = -1, b_0 = 2; a_1 = 0); from t = 192 on,
@@ -320,11 +330,18 @@ int fc_gemm_launch(const float* A, const float* W, const float* bias, float* out
 // Where a sub-band head Linear(H -> O <= 2c) writes: row r = b*N + n of the sub-band batch, output o = ch*c + j goes to
 // out[((b*2 + ch)*rows + lo + n*c + j)*rs + t] at frame t, i.e. a [B, 2, rows, frames] cRM with rows rs apart and
 // contiguous frames (fullsubnet/model.py:129-135: c = 1; improved_fullsubnet/model.py:239-247: one section, c its centre
-// width; with N = R every row is clip 0 and channel 0 is a plain [rows, frames] table)
+// width; with N = R every row is clip 0 and channel 0 is a plain [rows, frames] table).  bs (0 = 2 rows rs, the layout
+// above): clips bs elements apart instead, e.g. the frame-major [B, frames, 2, rows] cRM of the streaming call with rs = 1
 struct HeadGeom {
   int N, c, lo, rows;
-  size_t rs;
+  size_t rs, bs;
 };
+// element of the cRM that output o of sub-band row r goes to at frame t
+__device__ __forceinline__ size_t head_index(const HeadGeom& g, int r, int o, int t) {
+  const int b = r / g.N, n = r - b * g.N, ch = o / g.c, j = o - ch * g.c;
+  const size_t bs = g.bs ? g.bs : 2 * (size_t)g.rows * g.rs;
+  return (size_t)b * bs + ((size_t)ch * g.rows + g.lo + n * g.c + j) * g.rs + t;
+}
 // out = act(h W^T + b) for `steps` frames of h [steps, R, H] into frames t0 .. t0+steps-1 of g; one warp per (step, row,
 // output): lane-strided fmaf over H, warp_sum, + bias, act (FSN_ACT_*)
 int sb_head_launch(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act, float* out,
@@ -507,9 +524,18 @@ int stream_prologue(const int32_t* start, const int32_t* tail, int B, char* stat
                     int* tail_dev, cudaStream_t st);
 // first norm of the causal norms over the call's S steps: scaleT [S, B] from the frame sums fs [B, S] and the carried
 // accumulator (cumulative: running sum, forgetting: mu), frames counted from the clip start; the meta of active slots
-// then advances by K steps (pos += K hop, accumulator after step K-1, inactive after a tail)
+// then advances by K steps (pos += K hop, accumulator after step K-1, inactive after a tail).  With fs2 (forgetting norm
+// only): fullsubnet's second norm instead, mean (fs.y + fs2.y) / F (the caller passes F := F Ksb), mu carried at acc_off
+// bytes into each block and reset at the clip's frame 0, the meta untouched
 int stream_norm_launch(const float2* fs, int B, int S, int K, int F, const StreamGeom& g, int norm_type, const int* pos0,
-                       const int* act0, const int* tail, char* state, size_t slot_bytes, float* scaleT, cudaStream_t st);
+                       const int* act0, const int* tail, char* state, size_t slot_bytes, float* scaleT, cudaStream_t st,
+                       const float2* fs2 = nullptr, size_t acc_off = 0);
+// fullsubnet's second cumulative norm over the call's S steps: scaleT [S, B*F] of row b*F + f from magT / fbT [B, S, F],
+// the running sum of each row carried at run_off bytes into each block (F floats), reset at the clip's frame 0 and
+// stored as of step K - 1 for the active slots
+int stream_cum_unit_launch(const float* magT, const float* fbT, int B, int S, int K, int F, int Ns, int Nf,
+                           const StreamGeom& g, const int* pos0, const int* act0, char* state, size_t slot_bytes,
+                           size_t run_off, float* scaleT, cudaStream_t st);
 // before step j: zero h [B rows h_row apart, H] and c [B, H] of the slots whose step j is their clip's frame 0
 int stream_reset_launch(const int* pos0, int B, const StreamGeom& g, int j, int H, float* h, size_t h_row, float* c,
                         cudaStream_t st);

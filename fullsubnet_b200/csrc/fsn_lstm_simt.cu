@@ -326,10 +326,7 @@ __global__ void cum_unit_scale_kernel(const float* __restrict__ magT, const floa
   float run = 0.f;
   for (int t = 0; t < Tp; ++t) {
     const size_t base = (size_t)b * bs + (size_t)t * ts;
-    float s = 0.f;
-    for (int k = -Ns; k <= Ns; ++k) s += magT[base + reflect_idx(f + k, map.F)];
-    for (int k = -Nf; k <= Nf; ++k) s += fbT[base + reflect_idx(f + k, map.F)];
-    run += s;
+    run += unit_frame_sum(magT + base, fbT + base, f, map.F, Ns, Nf);
     scaleT[(size_t)t * R + r] = 1.0f / (run / ((float)K * (float)(t + 1)) + eps);
   }
 }
@@ -417,7 +414,7 @@ int lstm_step_launch(const StepParams& p, int mode, cudaStream_t st) {
 
 int lstm_step2_launch(StepParams p, int mode, int t, const fsn_lstm_layer& w1, const Step2State& s, cudaStream_t st) {
   const int H0 = p.H;
-  p.first = (t == 0);
+  p.first = t == 0 && !s.carry;
   p.h_prev = s.h0[(t + 1) & 1]; p.h_prev_stride = H0;
   p.h_out = s.h0[t & 1]; p.h_out_stride = H0;
   p.c = s.c0;
@@ -511,10 +508,7 @@ __global__ void sb_head_kernel(const float* __restrict__ h, int R, int H, int st
   float s = 0.f;
   for (int k = lane; k < H; k += 32) s = fmaf(hp[k], W[(size_t)o * H + k], s);
   s = warp_sum(s);
-  if (lane == 0) {
-    const int b = row / g.N, n = row - b * g.N, ch = o / g.c, j = o - ch * g.c;
-    out[(((size_t)b * 2 + ch) * g.rows + g.lo + n * g.c + j) * g.rs + t] = apply_act(s + bias[o], ACT);
-  }
+  if (lane == 0) out[head_index(g, row, o, t)] = apply_act(s + bias[o], ACT);
 }
 
 // the inverse gather of sb_head_kernel's scatter: dY[t, r, o] = act'(y) dcrm at frame t - la, 0 for t < la
@@ -527,8 +521,7 @@ __global__ void sb_head_bwd_kernel(const float* __restrict__ dcrm, const float* 
     const int r = (int)(tr % R), t = (int)(tr / R);
     float v = 0.f;
     if (t >= la) {
-      const int b = r / g.N, u = r - b * g.N, ch = o / g.c, j = o - ch * g.c;
-      const size_t idx = (((size_t)b * 2 + ch) * g.rows + g.lo + u * g.c + j) * g.rs + (t - la);
+      const size_t idx = head_index(g, r, o, t - la);
       v = act_grad(dcrm[idx], y, idx, act);
     }
     dY[i] = v;

@@ -334,3 +334,217 @@ extern "C" int fsn_enhance(const fsn_model_desc* d, const fsn_seq_weights* fb, c
   prof_mark(4, st);
   return rc;
 }
+
+// ---- chunked streaming (DESIGN 4.14).  Slot state block (each section on 16 bytes, blocks 256 bytes apart): meta (16
+// bytes), sample history Hs, spectrum Q x 2F, cRM Rc x 2F (the sections of fullband_baseline's stream), the second norm's
+// accumulator (cumulative: the running sum of each of the F sub-band units, forgetting: mu), full-band (h | c) of both
+// layers (2 x fb_hidden each), sub-band (h | c) of both layers for every frequency (2 x F x sb_hidden each).
+namespace fsn {
+
+struct FsnStreamLayout { size_t hist, spec, crm, norm2, fbh, fbc, sbh, sbc, slot; };
+
+static FsnStreamLayout fsn_stream_layout(const fsn_model_desc* d, const StreamGeom& g) {
+  const size_t F = d->num_freqs, F2 = 2 * F, Hf = 2 * (size_t)d->fb_hidden, Hs = 2 * F * d->sb_hidden;
+  FsnStreamLayout s;
+  size_t o = sizeof(StreamMeta);
+  auto sec = [&](size_t& at, size_t floats) { at = o; o = align_up(o + floats * 4, 16); };
+  sec(s.hist, g.Hs); sec(s.spec, g.Q * F2); sec(s.crm, g.Rc * F2);
+  sec(s.norm2, d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE ? F : 1);
+  sec(s.fbh, Hf); sec(s.fbc, Hf);
+  sec(s.sbh, Hs); sec(s.sbc, Hs);
+  s.slot = align_up(o, 256);
+  return s;
+}
+
+// every slot is one clip of the B = 1 whole-clip call, so drop_band never applies, whatever num_groups_in_drop_band says
+static int fsn_stream_check(const fsn_model_desc* d, int n_fft, int hop, int win_length, Dims& m, StreamGeom& g) {
+  FSN_REQUIRE(d, FSN_ERR_SHAPE, "stream: null descriptor");
+  fsn_model_desc dd = *d;
+  dd.num_groups_in_drop_band = 1;
+  int rc = make_dims(&dd, 1, 1, m);
+  if (rc) return rc;
+  FSN_REQUIRE(norm_per_step(d->norm_type), FSN_ERR_UNSUPPORTED,
+              "stream: the offline norm needs the whole clip; streaming is built for cumulative_laplace_norm and "
+              "forgetting_norm");
+  FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "stream: streaming is built for the LSTM cell");
+  FSN_REQUIRE(d->precision == FSN_PREC_FP32, FSN_ERR_UNSUPPORTED,
+              "stream: streaming is built for FSN_PREC_FP32 (precision %d)", d->precision);
+  FSN_REQUIRE(n_fft / 2 + 1 == d->num_freqs, FSN_ERR_SHAPE, "stream: n_fft/2+1 = %d != num_freqs = %d", n_fft / 2 + 1,
+              d->num_freqs);
+  return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
+}
+
+struct FsnStreamWs {
+  int *pos0, *act0, *tail;
+  float *wav, *magT, *spec, *scale1, *fbT, *scale2, *unit, *crm;
+  float2 *fs, *fs2;
+  float *fh[2], *fc[2], *fhall[2];       // full-band state and layer outputs
+  float *sh0[2], *sh1[2], *sc0, *sc1;    // sub-band state, h ping-pong per layer
+  size_t bytes;
+};
+
+// St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others
+static void fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B, int K, void* base, FsnStreamWs& w) {
+  Carver c(base);
+  const size_t F = d->num_freqs, Hf = d->fb_hidden, St = (size_t)K + g.E, RH = (size_t)B * F * d->sb_hidden;
+  w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B);
+  w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
+  w.magT = c.take<float>(B * St * F);
+  w.spec = c.take<float>(B * ((size_t)g.Q + St) * 2 * F);
+  w.fs = c.take<float2>(B * St);
+  w.fs2 = d->norm_type == FSN_NORM_FORGETTING ? c.take<float2>(B * St) : nullptr;
+  w.scale1 = c.take<float>(St * B);
+  for (int l = 0; l < 2; ++l) {
+    w.fh[l] = c.take<float>(B * Hf); w.fc[l] = c.take<float>(B * Hf);
+    w.fhall[l] = c.take<float>(B * St * Hf);
+  }
+  w.fbT = c.take<float>(B * St * F);
+  w.scale2 = d->norm_type == FSN_NORM_FORGETTING ? c.take<float>(St * B) : nullptr;
+  w.unit = c.take<float>(St * B * F);
+  for (int i = 0; i < 2; ++i) { w.sh0[i] = c.take<float>(RH); w.sh1[i] = c.take<float>(RH); }
+  w.sc0 = c.take<float>(RH); w.sc1 = c.take<float>(RH);
+  w.crm = c.take<float>(B * ((size_t)g.Rc + St) * 2 * F);
+  w.bytes = c.off;
+}
+
+}  // namespace fsn
+
+extern "C" size_t fsn_stream_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop) {
+  Dims m;
+  StreamGeom g;
+  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
+  if (B <= 0) { set_error("stream: B=%d slots", B); last_error_code() = FSN_ERR_SHAPE; return 0; }
+  return fsn_stream_layout(d, g).slot * (size_t)B;
+}
+
+extern "C" size_t fsn_stream_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop) {
+  Dims m;
+  StreamGeom g;
+  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
+  if (B <= 0 || K_max <= 0) {
+    set_error("stream: B=%d slots, K_max=%d hops", B, K_max);
+    last_error_code() = FSN_ERR_SHAPE;
+    return 0;
+  }
+  FsnStreamWs w;
+  fsn_stream_carve(d, g, B, K_max, nullptr, w);
+  return w.bytes;
+}
+
+extern "C" int fsn_stream_delay(const fsn_model_desc* d, int n_fft, int hop) {
+  Dims m;
+  StreamGeom g;
+  const int rc = fsn_stream_check(d, n_fft, hop, n_fft, m, g);
+  return rc ? -rc : g.D;
+}
+
+extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                               const float* wav, const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
+                               int win_length, float* enhanced, void* state, size_t state_bytes, void* workspace,
+                               size_t workspace_bytes, fsn_stream_t stream) {
+  g_launches = 0;
+  Dims m;
+  StreamGeom g;
+  int rc = fsn_stream_check(d, n_fft, hop, win_length, m, g);
+  if (rc) return rc;
+  FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "stream: B=%d slots, K=%d hops", B, K);
+  FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "stream: B=%d slots, at most 65535", B);
+  // the sub-band rows' (h, c) of all slots, one int-indexed element per thread in stream_reset_kernel
+  FSN_REQUIRE((size_t)B * m.F * d->sb_hidden <= 0x7fffffff, FSN_ERR_SHAPE,
+              "stream: B=%d slots x %d frequencies x sb_hidden %d must stay below 2^31", B, m.F, d->sb_hidden);
+  FSN_REQUIRE((long long)K * hop + g.D < (1 << 30), FSN_ERR_SHAPE, "stream: K=%d hops too long", K);
+  FSN_REQUIRE(fb && sb && wav && enhanced, FSN_ERR_SHAPE, "stream: null argument");
+  bool any_tail = false;
+  for (int b = 0; tail && b < B; ++b) {
+    FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * hop, FSN_ERR_SHAPE,
+                "stream: tail[%d] = %d, outside [0, K*hop] = [0, %d] and not -1", b, tail[b], K * hop);
+    any_tail |= tail[b] >= 0;
+  }
+  const FsnStreamLayout sl = fsn_stream_layout(d, g);
+  FSN_REQUIRE(state && state_bytes >= sl.slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
+              state_bytes, sl.slot * (size_t)B);
+  FsnStreamWs w;
+  fsn_stream_carve(d, g, B, K, workspace, w);
+  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, w.bytes);
+  // laid out for K + E steps from the workspace's start (a workspace queried for a larger K_max also fits); a call
+  // without a clip's last chunk runs St = K steps and strides its buffers by St
+  const cudaStream_t st = (cudaStream_t)stream;
+  char* sbase = (char*)state;
+  const size_t ss = sl.slot;
+  const int F = m.F, Hf = d->fb_hidden, Hs = d->sb_hidden, Ns = d->sb_num_neighbors, Nf = d->fb_num_neighbors;
+  const int St = K + (any_tail ? g.E : 0), R = B * F, Kh = K * hop, Wn = g.Hs + Kh;
+  const bool fgt = d->norm_type == FSN_NORM_FORGETTING;
+  const size_t F2 = 2 * (size_t)F;
+  if ((rc = stream_prologue(start, tail, B, sbase, ss, w.pos0, w.act0, w.tail, st))) return rc;
+  // samples: the carried history, then the chunk; spectrum: the carried Q frames, then the St frames of this call
+  if ((rc = copy_rows(w.wav, (size_t)Wn * 4, sbase + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.spec, (g.Q + St) * F2 * 4, sbase + sl.spec, ss, g.Q * F2 * 4, B, st))) return rc;
+  if ((rc = stft_stream_launch(w.wav, Wn, g.Hs, w.pos0, w.tail, B, n_fft, hop, win_length, g.c, St, g.Q, w.magT, w.spec,
+                               st)))
+    return rc;
+  // first norm (model_core): frame sums (.y reflect-weighted with Ns, for the second forgetting norm), running scale
+  if ((rc = frame_stats_launch(w.magT, B, St, F, Ns, (size_t)St * F, F, w.fs, st))) return rc;
+  if ((rc = stream_norm_launch(w.fs, B, St, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sbase, ss, w.scale1, st)))
+    return rc;
+  // full band on the per-step kernels seq_stack_forward runs for the per-step scale, (h, c) carried; Linear(F) + act
+  const fsn_lstm_layer fl[2] = {seq_layer(*fb, 0), seq_layer(*fb, 1)};
+  const int Hfl[2] = {Hf, Hf};
+  if ((rc = stream_lstm_layers(fl, 2, Hfl, F, w.magT, w.scale1, B, St, K, g, w.pos0, sbase, ss, sl.fbh, sl.fbc, w.fh, w.fc,
+                               w.fhall, st)))
+    return rc;
+  if ((rc = fc_gemm_launch(w.fhall[1], fb->fc_w, fb->fc_b, w.fbT, B * St, Hf, F, d->fb_activation, st))) return rc;
+  // second norm, one scale per (step, row), rows b*F + f
+  const RowMap map{B, F, F, 1};
+  if (fgt) {
+    if ((rc = frame_stats_launch(w.fbT, B, St, F, Nf, (size_t)St * F, F, w.fs2, st))) return rc;
+    if ((rc = stream_norm_launch(w.fs, B, St, K, F * m.Ksb, g, d->norm_type, w.pos0, w.act0, w.tail, sbase, ss, w.scale2,
+                                 st, w.fs2, sl.norm2)))
+      return rc;
+    if ((rc = forget_unit_broadcast_launch(w.scale2, map, R, St, w.unit, st))) return rc;
+  } else if ((rc = stream_cum_unit_launch(w.magT, w.fbT, B, St, K, F, Ns, Nf, g, w.pos0, w.act0, sbase, ss, sl.norm2, w.unit,
+                                          st))) {
+    return rc;
+  }
+  // sub band on the B*F rows, (h, c) of every row from the state (into the halves step 0 reads), stored after step K - 1;
+  // step j's cRM is frame Rc + j of w.crm [B, Rc + St, 2F]
+  const size_t sbw = (size_t)F * Hs * 4;
+  const Step2State s2{{w.sh0[0], w.sh0[1]}, w.sc0, {w.sh1[0], w.sh1[1]}, w.sc1, Hs, 0, true};
+  if ((rc = copy_rows(w.sh0[1], sbw, sbase + sl.sbh, ss, sbw, B, st))) return rc;
+  if ((rc = copy_rows(w.sh1[1], sbw, sbase + sl.sbh + sbw, ss, sbw, B, st))) return rc;
+  if ((rc = copy_rows(w.sc0, sbw, sbase + sl.sbc, ss, sbw, B, st))) return rc;
+  if ((rc = copy_rows(w.sc1, sbw, sbase + sl.sbc + sbw, ss, sbw, B, st))) return rc;
+  const HeadGeom hg{F, 1, 0, F, 1, ((size_t)g.Rc + St) * F2};
+  for (int j = 0; j < St; ++j) {
+    if (j <= g.c) {  // a clip's frame 0 is one of the first c + 1 steps
+      if ((rc = stream_reset_launch(w.pos0, B, g, j, F * Hs, w.sh0[(j + 1) & 1], (size_t)F * Hs, w.sc0, st))) return rc;
+      if ((rc = stream_reset_launch(w.pos0, B, g, j, F * Hs, w.sh1[(j + 1) & 1], (size_t)F * Hs, w.sc1, st))) return rc;
+    }
+    StepParams p;
+    memset(&p, 0, sizeof(p));
+    p.R = R; p.H = Hs; p.K0 = m.Ksb;
+    p.w_ih = sb->w_ih[0]; p.w_hh = sb->w_hh[0]; p.b_ih = sb->b_ih[0]; p.b_hh = sb->b_hh[0];
+    p.magT = w.magT; p.fbT = w.fbT; p.unit_scale = w.unit + (size_t)j * R;
+    p.F = F; p.Tp = St; p.t = j; p.Ns = Ns; p.Nf = Nf; p.map = map;
+    if ((rc = lstm_step2_launch(p, SEG0_GATHER, j, seq_layer(*sb, 1), s2, st))) return rc;
+    if ((rc = sb_head_launch(s2.h1_at(j), R, Hs, 1, sb->fc_w, sb->fc_b, 2, d->sb_activation, w.crm + (g.Rc + j) * F2, hg, 0,
+                             st)))
+      return rc;
+    if (j == K - 1) {
+      if ((rc = copy_rows(sbase + sl.sbh, ss, w.sh0[j & 1], sbw, sbw, B, st))) return rc;
+      if ((rc = copy_rows(sbase + sl.sbh + sbw, ss, w.sh1[j & 1], sbw, sbw, B, st))) return rc;
+      if ((rc = copy_rows(sbase + sl.sbc, ss, w.sc0, sbw, sbw, B, st))) return rc;
+      if ((rc = copy_rows(sbase + sl.sbc + sbw, ss, w.sc1, sbw, sbw, B, st))) return rc;
+    }
+  }
+  // cRM: the carried Rc frames before the call's; iSTFT
+  if ((rc = copy_rows(w.crm, (g.Rc + St) * F2 * 4, sbase + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;
+  if ((rc = istft_stream_launch(w.spec, w.crm, w.pos0, w.act0, w.tail, B, K, g.D, n_fft, hop, win_length, g.c, g.la, g.Rc,
+                                g.Q, St, enhanced, st)))
+    return rc;
+  // carry what the next call reads: the windows as of step K
+  if ((rc = copy_rows(sbase + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(sbase + sl.spec, ss, w.spec + K * F2, (g.Q + St) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
+  return copy_rows(sbase + sl.crm, ss, w.crm + K * F2, (g.Rc + St) * F2 * 4, g.Rc * F2 * 4, B, st);
+}

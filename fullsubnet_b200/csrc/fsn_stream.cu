@@ -52,21 +52,25 @@ int stream_prologue(const int32_t* start, const int32_t* tail, int B, char* stat
   return FSN_OK;
 }
 
-// the arithmetic of cum_clip_scale_kernel / forget_scale_kernel (first norm), frame m of the clip at step j
-__global__ void stream_norm_kernel(const float2* __restrict__ fs, int B, int S, int K, int F, int hop, int c, int fgt,
-                                   const ForgetCoef cf, float eps, const int* __restrict__ pos0, const int* __restrict__ act0,
-                                   const int* __restrict__ tail, char* __restrict__ state, size_t slot_bytes,
-                                   float* __restrict__ scaleT) {
+// the arithmetic of cum_clip_scale_kernel / forget_scale_kernel, frame m of the clip at step j: the first norm (fs2 null,
+// accumulator in the meta) or fullsubnet's second forgetting norm (mean of fs.y + fs2.y, mu at acc_off)
+__global__ void stream_norm_kernel(const float2* __restrict__ fs, const float2* __restrict__ fs2, int B, int S, int K, int F,
+                                   int hop, int c, int fgt, const ForgetCoef cf, float eps, const int* __restrict__ pos0,
+                                   const int* __restrict__ act0, const int* __restrict__ tail, char* __restrict__ state,
+                                   size_t slot_bytes, size_t acc_off, float* __restrict__ scaleT) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   StreamMeta* mt = reinterpret_cast<StreamMeta*>(state + (size_t)b * slot_bytes);
+  float* accp = fs2 ? reinterpret_cast<float*>(state + (size_t)b * slot_bytes + acc_off) : &mt->acc;
   const int m0 = pos0[b] / hop - c;
-  float acc = mt->acc, acc_k = acc;
+  float acc = *accp, acc_k = acc;
   for (int j = 0; j < S; ++j) {
     const int m = m0 + j;
     float sc = 1.f;
     if (m >= 0) {
-      const float s = fs[(size_t)b * S + j].x;
+      if (m == 0) acc = 0.f;
+      const float2 v = fs[(size_t)b * S + j];
+      const float s = fs2 ? __fadd_rn(v.y, fs2[(size_t)b * S + j].y) : v.x;
       if (fgt) {
         const float mean = __fdiv_rn(s, (float)F);
         const int i = m < FORGET_LEN ? m : FORGET_LEN;
@@ -81,17 +85,57 @@ __global__ void stream_norm_kernel(const float2* __restrict__ fs, int B, int S, 
     if (j == K - 1) acc_k = acc;
   }
   if (act0[b]) {
-    mt->acc = acc_k;
-    mt->pos = pos0[b] + K * hop;
-    mt->active = tail[b] < 0;
+    *accp = acc_k;
+    if (!fs2) {
+      mt->pos = pos0[b] + K * hop;
+      mt->active = tail[b] < 0;
+    }
   }
 }
 
 int stream_norm_launch(const float2* fs, int B, int S, int K, int F, const StreamGeom& g, int norm_type, const int* pos0,
-                       const int* act0, const int* tail, char* state, size_t slot_bytes, float* scaleT, cudaStream_t st) {
-  stream_norm_kernel<<<cdiv(B, 64), 64, 0, st>>>(fs, B, S, K, F, g.hop, g.c, norm_type == FSN_NORM_FORGETTING, forget_coef(),
-                                                 1.1920928955078125e-07f, pos0, act0, tail, state, slot_bytes, scaleT);
+                       const int* act0, const int* tail, char* state, size_t slot_bytes, float* scaleT, cudaStream_t st,
+                       const float2* fs2, size_t acc_off) {
+  stream_norm_kernel<<<cdiv(B, 64), 64, 0, st>>>(fs, fs2, B, S, K, F, g.hop, g.c, norm_type == FSN_NORM_FORGETTING,
+                                                 forget_coef(), 1.1920928955078125e-07f, pos0, act0, tail, state, slot_bytes,
+                                                 acc_off, scaleT);
   FSN_CHECK_LAUNCH("stream_norm_kernel");
+  return FSN_OK;
+}
+
+// cum_unit_scale_kernel on the call's S steps, one thread per row r = b*F + f
+__global__ void stream_cum_unit_kernel(const float* __restrict__ magT, const float* __restrict__ fbT, int B, int S, int K,
+                                       int F, int Ns, int Nf, int hop, int c, float eps, const int* __restrict__ pos0,
+                                       const int* __restrict__ act0, char* __restrict__ state, size_t slot_bytes,
+                                       size_t run_off, float* __restrict__ scaleT) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= B * F) return;
+  const int b = r / F, f = r - b * F;
+  const int Kf = 2 * Ns + 1 + 2 * Nf + 1;
+  float* srun = reinterpret_cast<float*>(state + (size_t)b * slot_bytes + run_off) + f;
+  const int m0 = pos0[b] / hop - c;
+  float run = *srun, run_k = run;
+  for (int j = 0; j < S; ++j) {
+    const int m = m0 + j;
+    float sc = 1.f;
+    if (m >= 0) {
+      if (m == 0) run = 0.f;
+      const size_t base = ((size_t)b * S + j) * F;
+      run += unit_frame_sum(magT + base, fbT + base, f, F, Ns, Nf);
+      sc = 1.0f / (run / ((float)Kf * (float)(m + 1)) + eps);
+    }
+    scaleT[(size_t)j * B * F + r] = sc;
+    if (j == K - 1) run_k = run;
+  }
+  if (act0[b]) *srun = run_k;
+}
+
+int stream_cum_unit_launch(const float* magT, const float* fbT, int B, int S, int K, int F, int Ns, int Nf,
+                           const StreamGeom& g, const int* pos0, const int* act0, char* state, size_t slot_bytes,
+                           size_t run_off, float* scaleT, cudaStream_t st) {
+  stream_cum_unit_kernel<<<cdiv(B * F, 128), 128, 0, st>>>(magT, fbT, B, S, K, F, Ns, Nf, g.hop, g.c, 1.1920928955078125e-07f,
+                                                           pos0, act0, state, slot_bytes, run_off, scaleT);
+  FSN_CHECK_LAUNCH("stream_cum_unit_kernel");
   return FSN_OK;
 }
 

@@ -24,6 +24,9 @@ class Model(SpectrogramEnhance, BaseModel):
     # training step (trainer.py:56-63): fsn_train_forward keeps the activations, fsn_train_backward runs BPTT
     TRAIN_ENTRY_POINTS = ("fsn_train_workspace_bytes", "fsn_train_forward", "fsn_train_backward")
     TRAIN_TF32_STACKS = ("fb_model", "sb_model")
+    # chunked streaming (fullsubnet_b200.stream.Streamer, precision="fp32" with cumulative_laplace_norm or
+    # forgetting_norm): state / workspace queries, delay, step
+    STREAM_ENTRY_POINTS = ("fsn_stream_state_bytes", "fsn_stream_workspace_bytes", "fsn_stream_delay", "fsn_stream_step")
 
     def __init__(self, num_freqs, look_ahead, sequence_model, fb_num_neighbors, sb_num_neighbors,
                  fb_output_activate_function, sb_output_activate_function, fb_model_hidden_size,
@@ -71,6 +74,17 @@ class Model(SpectrogramEnhance, BaseModel):
             return "fp32"
         d = self._desc("f16x3_tc", 1)
         return "f16x3_tc" if _lib.load().fsn_sb_packed_bytes(C.byref(d)) > 0 else "fp32"
+
+    def _stream_desc(self):
+        """Descriptor of the streaming calls: the fp32 kernels only, so an explicit precision="fp32" (under "auto" the
+        whole-clip call runs the sub band on the tensor cores, which a stream could not match)."""
+        if self.precision != "fp32":
+            raise NotImplementedError(f"fullsubnet_b200: fullsubnet streaming is built for precision=\"fp32\" "
+                                      f"(this model has precision={self.precision!r})")
+        return self._desc("fp32", int(self.num_groups_in_drop_band))
+
+    def _stream_weights(self):
+        return C.byref(self.fb_model.weight_struct()), C.byref(self.sb_model.weight_struct())
 
     def _train_desc(self):
         return self._desc(self._resolve_train_precision(), int(self.num_groups_in_drop_band))

@@ -1,8 +1,9 @@
 """Chunked streaming enhancement (DESIGN 4.14): ``Streamer`` advances many streams by K hops per call and returns, for
 each clip, the samples of the whole-clip ``enhance`` call bit for bit, ``delay`` samples later.
 
-Built for fullband_baseline with ``cumulative_laplace_norm`` or ``forgetting_norm`` (LSTM, fp32) and for fast_fullsubnet
-with ``cumulative_laplace_norm`` (LSTM, ``precision="fp32"``).  Each model names its library calls in
+Built for fullband_baseline with ``cumulative_laplace_norm`` or ``forgetting_norm`` (LSTM, fp32), for fullsubnet with
+``cumulative_laplace_norm`` or ``forgetting_norm`` (LSTM, ``precision="fp32"``) and for fast_fullsubnet with
+``cumulative_laplace_norm`` (LSTM, ``precision="fp32"``).  Each model names its library calls in
 ``STREAM_ENTRY_POINTS`` and gives their arguments through ``_stream_desc()`` and ``_stream_weights()``."""
 from __future__ import annotations
 
@@ -27,8 +28,8 @@ class Streamer:
     def __init__(self, model, slots: int, n_fft: int = 512, hop: int = 256, win_length: int = 512):
         names = getattr(type(model), "STREAM_ENTRY_POINTS", ())
         if not names:
-            raise NotImplementedError("fullsubnet_b200: chunked streaming is built for fullband_baseline and "
-                                      "fast_fullsubnet")
+            raise NotImplementedError("fullsubnet_b200: chunked streaming is built for fullband_baseline, fullsubnet "
+                                      "and fast_fullsubnet")
         self.model, self.slots, self.n_fft, self.hop, self.win_length = model, int(slots), n_fft, hop, win_length
         self.device = next(model.parameters()).device
         lib = _lib.load()

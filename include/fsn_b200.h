@@ -526,6 +526,33 @@ int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weights* w, cons
                          const int32_t* tail, int B, int K, int n_fft, int hop, int win_length, float* enhanced,
                          void* state, size_t state_bytes, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
+/* Chunked streaming enhancement of fullsubnet (DESIGN 4.14), with the semantics of the fullband_baseline calls above:
+ * many streams, each advanced by K hops per call, the output of every clip bit-identical to fsn_enhance on the whole
+ * clip (lengths NULL, B = 1), delayed by D = fsn_stream_delay(d, n_fft, hop) = n_fft/2 + (look_ahead + 1 + c) hop
+ * samples, c = ceil((n_fft/2) / hop).  Every slot is a B = 1 clip, so drop_band never applies, whatever
+ * num_groups_in_drop_band says.  Appended in ABI version 102.
+ *
+ * State: fsn_stream_state_bytes(d, B, n_fft, hop) bytes, ZERO-FILLED before its first use, slot b's block at
+ * b * state_bytes / B.  A block holds the slot's position and the first norm's accumulator (16 bytes), the last (c+1) hop
+ * + n_fft/2 input samples, the spectrum of the last Rc + look_ahead frames and the cRM of the last Rc frames (Rc =
+ * ceil(n_fft/hop) + 2), the second norm's accumulator (cumulative: one running sum per frequency, forgetting: mu), h and
+ * c of both full-band layers, and h and c of both sub-band layers for every frequency (2 x 2 x num_freqs x sb_hidden
+ * floats: 1 579 008 of the recipe's 1 612 032 bytes per slot with the cumulative norm).  fsn_stream_step: wav, start, tail, enhanced, workspace
+ * (fsn_stream_workspace_bytes(d, B, K_max, n_fft, hop), every K <= K_max) and the clip-length limits as
+ * fsn_fullband_stream_step; fb / sb as fsn_enhance.  Built for the cumulative_laplace_norm and forgetting_norm models,
+ * LSTM cell, FSN_PREC_FP32, power-of-two n_fft in [16, 2048] with n_fft/2 + 1 = num_freqs; the offline norm, the GRU
+ * cell, the tensor-core precisions, other n_fft and B > 65535 -> FSN_ERR_UNSUPPORTED (n_fft/2 + 1 != num_freqs:
+ * FSN_ERR_SHAPE) before any CUDA call, from the queries (which return 0) as from the call; B x num_freqs x sb_hidden >=
+ * 2^31 -> FSN_ERR_SHAPE from the call.  Never allocates, never synchronises the host; one call may be captured in a
+ * CUDA graph. */
+size_t fsn_stream_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop);
+size_t fsn_stream_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop);
+int fsn_stream_delay(const fsn_model_desc* d, int n_fft, int hop);
+int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb, const float* wav,
+                    const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop, int win_length,
+                    float* enhanced, void* state, size_t state_bytes, void* workspace, size_t workspace_bytes,
+                    fsn_stream_t stream);
+
 /* Training step of recipes/dns_interspeech_2020/fullband_baseline/trainer.py:32-71, same conventions as fsn_train_*: the
  * caller allocates the workspace and passes the same untouched buffer from forward to backward; the gradients of all
  * 4 * num_layers + 2 parameters are OVERWRITTEN; no host synchronisation; arguments are checked before any CUDA call;
