@@ -3,10 +3,13 @@ fullsubnet, precision="fp32") or fast_fullsubnet (fsn_fast_stream_step, --model 
 seconds enhanced per wall second and concurrent real-time streams for slots x K, with the whole-clip fp32 rate of the
 same process beside it (fsn_fullband_enhance; fullsubnet: fsn_enhance; fast_fullsubnet: Inferencer.enhance_batch).  For
 fullsubnet and fast_fullsubnet each line also says whether every slot stays real-time; for fast_fullsubnet it gives the
-bottleneck's share of the call's GPU time, from a torch.profiler pass of its own after the timed calls.  Prints one
-JSON line per configuration and a header line with the GPU, power limit and clocks.
+bottleneck's share of the call's GPU time, from a torch.profiler pass of its own after the timed calls.  fullsubnet with
+--precision f16x3_tc / f16_tc streams on the tensor cores (fsn_stream_tc_step), gives the launches per call, and the
+whole-clip rate beside it is of that precision.  Prints one JSON line per configuration and a header line with the GPU,
+power limit and clocks.
 
-    python bench_stream.py [--model fullband_baseline] [--slots 1 64 256] [--ks 1 4 16 64] [--calls 20] [--warmup 3]"""
+    python bench_stream.py [--model fullband_baseline] [--precision fp32] [--slots 1 64 256] [--ks 1 4 16 64]
+                           [--calls 20] [--warmup 3]"""
 from __future__ import annotations
 
 import argparse
@@ -14,6 +17,8 @@ import json
 import subprocess
 
 import torch
+
+from fullsubnet_b200 import _lib
 
 SR, HOP = 16000, 256
 
@@ -28,7 +33,7 @@ def gpu_info():
         return {"error": str(e)}
 
 
-def model(name, norm, dev):
+def model(name, norm, dev, precision="fp32"):
     if name == "fast_fullsubnet":
         from fullsubnet_b200.fast_fullsubnet.model import Model
         from oracle import fast_fullsubnet_oracle as FO
@@ -40,7 +45,7 @@ def model(name, norm, dev):
         from fullsubnet_b200.fullsubnet.model import Model
         from oracle import fullsubnet_oracle as O
         args = dict(O.DEFAULT_MODEL_ARGS, norm_type=norm)
-        m = Model(**args, precision="fp32")
+        m = Model(**args, precision=precision)
         m.load_state_dict(O.make_state_dict(seed=11, args=args), strict=True)
         return m.to(dev).eval()
     from fullsubnet_b200.fullband_baseline.model import Model
@@ -95,16 +100,22 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--norm", default="cumulative_laplace_norm")
     ap.add_argument("--model", default="fullband_baseline", choices=["fullband_baseline", "fullsubnet", "fast_fullsubnet"])
+    # fullsubnet only: f16x3_tc / f16_tc stream on the tensor cores (Streamer(tensor_cores=True)), and the whole-clip rate
+    # is of the same precision
+    ap.add_argument("--precision", default="fp32", choices=["fp32", "f16x3_tc", "f16_tc"])
     a = ap.parse_args()
+    assert a.precision == "fp32" or a.model == "fullsubnet", "--precision is for --model fullsubnet"
+    tc = a.precision != "fp32"
     assert torch.cuda.is_available(), "bench_stream.py needs a CUDA device"
     dev = torch.device("cuda:0")
     from fullsubnet_b200.stream import Streamer
     fast = a.model == "fast_fullsubnet"
-    m = model(a.model, a.norm, dev)
-    print(json.dumps({"gpu": gpu_info(), "model": a.model, "precision": "fp32", "norm": a.norm}))
+    m = model(a.model, a.norm, dev, a.precision)
+    print(json.dumps({"gpu": gpu_info(), "model": a.model, "precision": a.precision, "norm": a.norm}))
+    lib = _lib.load()
     g = torch.Generator(device="cpu").manual_seed(0)
     for slots in a.slots:
-        s = Streamer(m, slots)
+        s = Streamer(m, slots, tensor_cores=tc)
         for K in a.ks:
             x = (0.1 * torch.randn(slots, K * HOP, generator=g)).to(dev)
             s.step(x, [1] * slots)
@@ -116,6 +127,8 @@ def main():
                     "audio_s_per_s": round(audio_rate, 1), "realtime_streams": rt, "delay": s.delay}
             if a.model != "fullband_baseline":
                 line["all_realtime"] = ms <= chunk_ms
+            if tc:
+                line["launches_per_call"] = int(lib.fsn_last_launch_count())
             if fast:
                 line["bottleneck_share"] = bottleneck_share(lambda: s.step(x))
             print(json.dumps(line))

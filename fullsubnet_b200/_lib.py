@@ -172,6 +172,11 @@ _SIGNATURES = {
     "fsn_stream_delay": (C.c_int, [C.POINTER(ModelDesc), _I, _I]),
     "fsn_stream_step": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P, _P, _I, _I,
                                   _I, _I, _I, _P, _P, _S, _P, _S, _P]),
+    "fsn_stream_tc_state_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I]),
+    "fsn_stream_tc_workspace_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I, _I]),
+    "fsn_stream_tc_delay": (C.c_int, [C.POINTER(ModelDesc), _I, _I]),
+    "fsn_stream_tc_step": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(SeqWeights), C.POINTER(SeqWeights), _P, _P, _P, _P,
+                                     _I, _I, _I, _I, _I, _P, _P, _S, _P, _S, _P]),
     "fsn_fullband_train_workspace_bytes": (_S, [C.POINTER(FullbandDesc), _I, _I]),
     "fsn_fullband_train_forward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, _P, _P, _S, _P]),
     "fsn_fullband_train_backward": (C.c_int, [C.POINTER(FullbandDesc), _P, _P, _P, _P, _I, _I, C.POINTER(FullbandGrads), _P,
@@ -188,11 +193,14 @@ _SIGNATURES = {
     "fsn_debug_reflect_count": (C.c_int, [_I, _I, _I]),
     "fsn_debug_lstm_tc_workspace_bytes": (_S, [_I, _I, _I, _I, _I]),
     "fsn_debug_lstm_layer_tc": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _S, _P]),
+    "fsn_debug_lstm_tc_carry": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _I, _P, _P, _S, _P]),
     "fsn_debug_linear_tc": (C.c_int, [_P, _I, _I, _P, _P, _I, _I, _I, _P, _P, _S, _P]),
     "fsn_debug_sb_lstm_tc_packed_bytes": (_S, [_I, _I]),
     "fsn_debug_sb_lstm_tc_max_clusters": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int)]),
     "fsn_debug_sb_lstm_tc": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _I,
                                        _I, _I, _I, _I, _P, _P, _P]),
+    "fsn_debug_sb_lstm_tc_carry": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _I, _P,
+                                             _I, _P, _P, _P, _P, _P]),
     "fsn_debug_sb_lstm_tc_probe": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P,
                                              _I, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P]),
     "fsn_debug_tgemm": (C.c_int, [_P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _P, _L, _P]),

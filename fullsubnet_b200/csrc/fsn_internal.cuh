@@ -456,9 +456,18 @@ int fb_persistent_launch(const fsn_lstm_layer* L, const float* x, const float* i
 bool lstm_rec_tc_supported(int H, bool x3);
 int lstm_rec_tc_rows_per_launch(int H);
 size_t lstm_rec_tc_scratch_bytes(int H, bool x3);
+// chunked streaming (lstm_rec_tc_carry_kernel): row r enters step 0 with h_init / c_init [r * row + u] and step
+// restart[r] with zero state; c after step fin_step (-1: none) goes to c_fin (may be c_init)
+struct RecCarry {
+  const float *h_init, *c_init;
+  float* c_fin;
+  size_t row;
+  const int* restart;
+  int fin_step;
+};
 int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, const float* P, size_t p_row, size_t p_t,
                        float* hall, size_t h_row, size_t h_t, int R, int T, int H, bool x3, void* scratch,
-                       cudaStream_t st);
+                       cudaStream_t st, const RecCarry* io = nullptr);
 int split_tf32_launch(const float* in, size_t rows, int K, size_t ldi, const float* row_scale, int rows_per_scale,
                       float* out, int Kp, int cat, cudaStream_t st, int scale_B = 0);
 int bias_act_launch(float* x, size_t rows, int N, size_t ld, const float* bias, int act, cudaStream_t st);
@@ -467,7 +476,8 @@ int bias_act_launch(float* x, size_t rows, int N, size_t ld, const float* bias, 
 struct LstmTcWs { float *a, *w, *P; void* rec; };
 void lstm_tc_carve(Carver& c, size_t rows_T, int Kmax, int Hmax, bool x3, LstmTcWs& ws);
 int lstm_layer_tc(const fsn_lstm_layer& L, const float* x, size_t ldx, int K, const float* row_scale, int rows_per_scale,
-                  int scale_B, int R, int T, int H, bool x3, const LstmTcWs& ws, float* hall, cudaStream_t st);
+                  int scale_B, int R, int T, int H, bool x3, const LstmTcWs& ws, float* hall, cudaStream_t st,
+                  const RecCarry* io = nullptr);
 int linear_tc(const float* x, size_t ldx, int K, const float* W, const float* bias, int N, int act, float* out, size_t ldo,
               size_t rows, bool x3, const LstmTcWs& ws, cudaStream_t st);
 int gemm_tc_split_launch(const float* a, size_t lda, const float* W, int N, int K, float* w, float* C, size_t ldc, size_t M,
@@ -539,6 +549,9 @@ int stream_cum_unit_launch(const float* magT, const float* fbT, int B, int S, in
 // before step j: zero h [B rows h_row apart, H] and c [B, H] of the slots whose step j is their clip's frame 0
 int stream_reset_launch(const int* pos0, int B, const StreamGeom& g, int j, int H, float* h, size_t h_row, float* c,
                         cudaStream_t st);
+// restart[b] = the step of the call that is slot b's clip frame 0 (c - pos0[b] / hop; outside [0, c] when none is):
+// the tensor-core stream's kernels enter it with zero state, where the per-step kernels run stream_reset_launch
+int stream_restart_launch(const int* pos0, int B, const StreamGeom& g, int* restart, cudaStream_t st);
 // signal layer of the streaming calls (fsn_dsp.cu), power-of-two n_fft only
 int stream_dsp_check(int n_fft, int hop, int win_length);
 int stft_stream_launch(const float* win, int Wn, int Hs, const int* pos0, const int* tail, int B, int n_fft, int hop,
@@ -582,6 +595,20 @@ int sb_tc_pack(const fsn_model_desc* d, const fsn_seq_weights* sb, void* packed,
 int sb_tc_pack_raw(const fsn_seq_weights* sb, int H, int Ksb, int fc_out, void* packed, cudaStream_t st, bool x3,
                    bool proj = false);
 int sb_tc_forward(const SbTcArgs& a, cudaStream_t st);
+// chunked streaming (sb_carry_lstm_tc_kernel): the stack continued from a carried state.  (h, c) of row r, layer l, unit u
+// at h / c [(r / rps) slot + l layer + (r % rps) H + u] (floats) are read before step 0 and written after store_step;
+// row r enters step restart[r / rps] with zero state; step t's output o of row r = b F + f goes to crm[b crm_bs +
+// (crm_t0 + t) 2F + o F + f].  a: unit_scale given, la = 0, no drop_band, no down-sampling.
+struct SbCarry {
+  float *h, *c;
+  size_t slot, layer;
+  int rps;
+  const int* restart;
+  int store_step;
+  size_t crm_bs;
+  int crm_t0;
+};
+int sb_tc_carry_forward(const SbTcArgs& a, const SbCarry& io, cudaStream_t st);
 bool sb_tc_supported(const fsn_model_desc* d);
 // FSN_TC_STAGES / FSN_TC_CLUSTER (defaults 4 / 1), read once
 void sb_tc_ring_defaults(int& stages, int& cluster);

@@ -17,6 +17,11 @@
 // Column block j (8 columns) of D is gate j % 4, so the thread that holds a row's fragment holds all four gates of
 // the same two units: c stays in 8 registers (4 rows x 2 units), no exchange.  Groups of 64 CTAs cover 128 clips
 // each with H = 512.
+//
+// CARRY (lstm_rec_tc_carry_kernel, chunked streaming, DESIGN 4.14): the recurrence continued from a carried state.  The
+// host writes h_{-1} as hi [/ lo] into the parity buffer step 0 reads (rec_carry_init_kernel, instead of the memset
+// zeros), so step 0 runs its MMAs like every later step; c_{-1} is loaded into the consumer registers.  A row restarting
+// at step j drops its c there and publishes a zero h_{j-1}; c after step fin_step is stored (h is in hall anyway).
 #include <string.h>
 #include <stdlib.h>
 
@@ -48,6 +53,12 @@ struct Args {
   unsigned int* barrier;                                      // one counter per group, 32 words apart
   int R, T, H, Kp, Rpad, C, stages, fence_all;
 };
+// CARRY only: c of row r at c_init / c_fin [r * c_row + u], restart step of row r at restart[r], c stored after fin_step
+struct CarryArgs {
+  const float* c_init; float* c_fin; size_t c_row;
+  const int* restart;
+  int fin_step;
+};
 
 template <bool X3> __device__ __forceinline__ float act_sigmoid(float x) {
   return X3 ? 1.0f / (1.0f + expf(-x)) : fast_sigmoid(x);
@@ -56,8 +67,9 @@ template <bool X3> __device__ __forceinline__ float act_tanh(float x) {
   return X3 ? 1.0f - 2.0f / (1.0f + expf(2.0f * x)) : fast_tanh(x);
 }
 
-template <bool X3>
-__global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_constant__ CUtensorMap tmap, const Args a) {
+// every CARRY branch below is `if constexpr` or folds away: lstm_rec_tc_kernel is the code it was before the policy
+template <bool X3, bool CARRY>
+__device__ __forceinline__ void lstm_rec_tc_body(const CUtensorMap& tmap, const Args& a, const CarryArgs& io) {
   constexpr int PARTS = X3 ? 2 : 1;
   constexpr int STAGE_BYTES = PARTS * A_TILE;
   constexpr int WB_ROWS = PARTS * NG;          // rows of the resident weight operand per k-block: [W_hi ; W_lo]
@@ -104,7 +116,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
   if (warp == 4) {
     // ================= producer: after the group has published h_{p-1}, stream it through the ring
     uint32_t it = 0;
-    for (int p = 1; p < T; ++p) {
+    for (int p = CARRY ? 0 : 1; p < T; ++p) {
       if (lane == 0) {
         const unsigned int target = (unsigned int)a.C * (unsigned int)p;
         unsigned int v, spins = 0;
@@ -115,7 +127,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
       }
       __syncwarp();
       fence_proxy_async();  // the TMA (async proxy) reads below come after the acquire above
-      const int par = (p - 1) & 1;
+      const int par = CARRY ? ((p + 1) & 1) : ((p - 1) & 1);
       for (int kb = 0; kb < nkb; ++kb, ++it) {
         const uint32_t s = it % (uint32_t)a.stages, use = it / (uint32_t)a.stages;
         mbar_wait<false>(&bars.empty[s], (use & 1) ^ 1);
@@ -148,6 +160,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
     for (int i = 0; i < 4; ++i) c[i][0] = c[i][1] = 0.f;
     const int nu = (H - u0 < U) ? (H - u0) : U;  // real units of this CTA
     const bool u_ok0 = ul0 < nu, u_ok1 = ul0 + 1 < nu;
+    int rst[4] = {-1, -1, -1, -1};
+    if constexpr (CARRY) {
+#pragma unroll
+      for (int rs = 0; rs < 4; ++rs) {
+        const int r = g * MR + 64 * (rs >> 1) + 16 * q + (lane >> 2) + 8 * (rs & 1);
+        if (r < a.R) {
+          rst[rs] = io.restart[r];
+          const float* cp = io.c_init + (size_t)r * io.c_row + u0 + ul0;
+          if (u_ok0) c[rs][0] = cp[0];
+          if (u_ok1) c[rs][1] = cp[1];
+        }
+      }
+    }
     uint32_t it = 0;
     const uint32_t wbase = smem_u32(wsm), rbase = smem_u32(ring);
     for (int p = 0; p < T; ++p) {
@@ -168,7 +193,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
           }
         }
       }
-      if (p > 0) {
+      if (CARRY || p > 0) {
         float acc[2][NACC];
         float accl[2][NG / 2];
 #pragma unroll
@@ -227,7 +252,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
         for (int e = 0; e < 2; ++e) {
           const float gi = pre[rs][0][e] + bias[0][e], gf = pre[rs][1][e] + bias[1][e];
           const float gg = pre[rs][2][e] + bias[2][e], go = pre[rs][3][e] + bias[3][e];
-          const float cn = act_sigmoid<X3>(gf) * c[rs][e] + act_sigmoid<X3>(gi) * act_tanh<X3>(gg);
+          const float cp = (CARRY && p == rst[rs]) ? 0.f : c[rs][e];
+          const float cn = act_sigmoid<X3>(gf) * cp + act_sigmoid<X3>(gi) * act_tanh<X3>(gg);
           c[rs][e] = cn;
           h[e] = act_sigmoid<X3>(go) * act_tanh<X3>(cn);
         }
@@ -239,8 +265,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
             if (u_ok0) hp[0] = h[0];
             if (u_ok1) hp[1] = h[1];
           }
+          if constexpr (CARRY) {
+            if (p == io.fin_step) {
+              float* cf = io.c_fin + (size_t)r * io.c_row + u0 + ul0;
+              if (u_ok0) cf[0] = c[rs][0];
+              if (u_ok1) cf[1] = c[rs][1];
+            }
+          }
           if (p + 1 < T) {  // publish h_p for the next step: fp16 hi (and lo)
-            const float v0 = u_ok0 ? h[0] : 0.f, v1 = u_ok1 ? h[1] : 0.f;
+            const bool zero = CARRY && rst[rs] == p + 1;  // the row enters step p + 1 with zero state
+            const float v0 = (u_ok0 && !zero) ? h[0] : 0.f, v1 = (u_ok1 && !zero) ? h[1] : 0.f;
             const __half2 hi = __floats2half2_rn(v0, v1);
             const __half2 lo = __floats2half2_rn(v0 - __low2float(hi), v1 - __high2float(hi));
             __half* sp = a.state + ((size_t)((p & 1) * PARTS) * a.Rpad + r) * a.Kp + u0 + ul0;
@@ -262,6 +296,32 @@ __global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_c
         }
       }
     }
+  }
+}
+
+template <bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_kernel(const __grid_constant__ CUtensorMap tmap, const Args a) {
+  lstm_rec_tc_body<X3, false>(tmap, a, CarryArgs{});
+}
+
+template <bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) lstm_rec_tc_carry_kernel(const __grid_constant__ CUtensorMap tmap,
+                                                                       const Args a, const CarryArgs io) {
+  lstm_rec_tc_body<X3, true>(tmap, a, io);
+}
+
+// h_{-1} of rows [0, R) (row r at h[r * h_row], zero where the row restarts at step 0) into parity 1 of the fp16 state
+// [2 parity][parts][Rpad][Kp]: hi = rn(h), lo = rn(h - hi), the split the consumers publish h with
+__global__ void rec_carry_init_kernel(const float* __restrict__ h, size_t h_row, const int* __restrict__ restart, int R, int H,
+                                      int Kp, int Rpad, int parts, __half* __restrict__ state) {
+  const size_t n = (size_t)R * H;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int r = (int)(i / H), k = (int)(i - (size_t)r * H);
+    const float v = restart[r] == 0 ? 0.f : h[(size_t)r * h_row + k];
+    const __half hi = __float2half_rn(v);
+    __half* sp = state + ((size_t)parts * Rpad + r) * Kp + k;
+    sp[0] = hi;
+    if (parts > 1) sp[(size_t)Rpad * Kp] = __float2half_rn(v - __half2float(hi));
   }
 }
 
@@ -363,7 +423,7 @@ size_t lstm_rec_tc_scratch_bytes(int H, bool x3) {
 // count: chunks of lstm_rec_tc_rows_per_launch are launched back to back)
 int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, const float* P, size_t p_row, size_t p_t,
                        float* hall, size_t h_row, size_t h_t, int R, int T, int H, bool x3, void* scratch,
-                       cudaStream_t st) {
+                       cudaStream_t st, const RecCarry* io) {
   FSN_REQUIRE(lstm_rec_tc_supported(H, x3), FSN_ERR_UNSUPPORTED, "lstm_rec_tc: hidden size %d not supported", H);
   const int Kp = (H + rec::KB - 1) / rec::KB * rec::KB;
   const int C = cdiv(H, rec::U);
@@ -380,7 +440,8 @@ int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, 
   FSN_REQUIRE(state_bytes <= rec_state_capacity_bytes(), FSN_ERR_UNSUPPORTED, "lstm_rec_tc: state of H=%d exceeds the scratch", H);
   unsigned int* barrier = (unsigned int*)((uint8_t*)scratch + rec_state_capacity_bytes());  // fixed place, whatever H
   int rc;
-  const void* kern = x3 ? (const void*)rec::lstm_rec_tc_kernel<true> : (const void*)rec::lstm_rec_tc_kernel<false>;
+  const void* kern = io ? (x3 ? (const void*)rec::lstm_rec_tc_carry_kernel<true> : (const void*)rec::lstm_rec_tc_carry_kernel<false>)
+                        : (x3 ? (const void*)rec::lstm_rec_tc_kernel<true> : (const void*)rec::lstm_rec_tc_kernel<false>);
   if ((rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "lstm_rec_tc smem attr")))
     return rc;
   for (int r0 = 0; r0 < R; r0 += rows_max) {
@@ -390,6 +451,11 @@ int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, 
     // state of padded rows / padded k stays zero for the whole launch; counters start at zero
     if ((rc = check_cuda(cudaMemsetAsync(scratch, 0, state_bytes, st), "lstm_rec_tc memset"))) return rc;
     if ((rc = check_cuda(cudaMemsetAsync(barrier, 0, 64 * 32 * sizeof(unsigned int), st), "lstm_rec_tc memset"))) return rc;
+    if (io) {
+      rec::rec_carry_init_kernel<<<ew_grid((size_t)nr * H), 256, 0, st>>>(io->h_init + (size_t)r0 * io->row, io->row,
+                                                                          io->restart + r0, nr, H, Kp, Rpad, parts, state);
+      FSN_CHECK_LAUNCH("rec_carry_init_kernel");
+    }
     CUtensorMap tm;
     FSN_REQUIRE(encode_tmap_2d(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, state, Kp, 2 * parts * Rpad, Kp * sizeof(__half), rec::KB,
                                rec::MR),
@@ -401,7 +467,12 @@ int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, 
     a.state = state; a.barrier = barrier;
     a.R = nr; a.T = T; a.H = H; a.Kp = Kp; a.Rpad = Rpad; a.C = C; a.stages = stages;
     a.fence_all = getenv("FSN_REC_FENCE_ALL") != nullptr;
-    void* params[] = {(void*)&tm, (void*)&a};
+    rec::CarryArgs ca{};
+    if (io) {
+      ca.c_init = io->c_init + (size_t)r0 * io->row; ca.c_fin = io->c_fin + (size_t)r0 * io->row; ca.c_row = io->row;
+      ca.restart = io->restart + r0; ca.fin_step = io->fin_step;
+    }
+    void* params[] = {(void*)&tm, (void*)&a, (void*)&ca};
     if ((rc = check_cuda(cudaLaunchCooperativeKernel(kern, dim3(G * C), dim3(rec::NTHREADS), params, smem, st),
                          "lstm_rec_tc cooperative launch")))
       return rc;
@@ -468,7 +539,8 @@ static int prep_operand(const float* x, size_t ldx, int K, size_t rows, const fl
 
 // hall[r, t, :] (row stride T*H) of one LSTM layer over x[(r*T + t), :K] * scale
 int lstm_layer_tc(const fsn_lstm_layer& L, const float* x, size_t ldx, int K, const float* row_scale, int rows_per_scale,
-                  int scale_B, int R, int T, int H, bool x3, const LstmTcWs& ws, float* hall, cudaStream_t st) {
+                  int scale_B, int R, int T, int H, bool x3, const LstmTcWs& ws, float* hall, cudaStream_t st,
+                  const RecCarry* io) {
   const size_t rows = (size_t)R * T;
   const float* a;
   size_t lda;
@@ -476,7 +548,7 @@ int lstm_layer_tc(const fsn_lstm_layer& L, const float* x, size_t ldx, int K, co
   if ((rc = prep_operand(x, ldx, K, rows, row_scale, rows_per_scale, scale_B, x3, ws, a, lda, st))) return rc;
   if ((rc = gemm_tc_split_launch(a, lda, L.w_ih, 4 * H, K, ws.w, ws.P, (size_t)4 * H, rows, x3, st))) return rc;
   return lstm_rec_tc_launch(L.w_hh, L.b_ih, L.b_hh, ws.P, (size_t)T * 4 * H, (size_t)4 * H, hall, (size_t)T * H, (size_t)H, R, T,
-                            H, x3, ws.rec, st);
+                            H, x3, ws.rec, st, io);
 }
 
 // out[rows, :N] (row stride ldo) = act(x[rows, :K] W[N,K]^T + bias)
@@ -519,4 +591,19 @@ extern "C" int fsn_debug_linear_tc(const float* x, int rows, int K, const float*
   fsn::lstm_tc_carve(c, (size_t)rows, K, Hm, x3 != 0, ws);
   FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, c.off);
   return fsn::linear_tc(x, (size_t)K, K, W, bias, N, act, out, (size_t)N, (size_t)rows, x3 != 0, ws, (cudaStream_t)stream);
+}
+extern "C" int fsn_debug_lstm_tc_carry(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
+                                       const float* x, int R, int T, int K, int H, int x3, const float* h_init, float* c,
+                                       const int32_t* restart, int fin_step, float* hall, void* workspace,
+                                       size_t workspace_bytes, fsn_stream_t stream) {
+  FSN_REQUIRE(fsn::lstm_rec_tc_supported(H, x3 != 0), FSN_ERR_UNSUPPORTED, "lstm_layer_tc: hidden size %d not supported", H);
+  FSN_REQUIRE(h_init && c && restart && hall && R > 0 && T > 0 && fin_step >= -1 && fin_step < T, FSN_ERR_SHAPE,
+              "lstm_tc_carry: bad argument (R=%d, T=%d, fin_step=%d)", R, T, fin_step);
+  fsn::Carver cv(workspace);
+  fsn::LstmTcWs ws;
+  fsn::lstm_tc_carve(cv, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
+  FSN_REQUIRE(workspace && workspace_bytes >= cv.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, cv.off);
+  fsn_lstm_layer L{w_ih, w_hh, b_ih, b_hh};
+  const fsn::RecCarry io{h_init, c, c, (size_t)H, restart, fin_step};
+  return fsn::lstm_layer_tc(L, x, (size_t)K, K, nullptr, 1, 0, R, T, H, x3 != 0, ws, hall, (cudaStream_t)stream, &io);
 }

@@ -356,8 +356,10 @@ static FsnStreamLayout fsn_stream_layout(const fsn_model_desc* d, const StreamGe
   return s;
 }
 
-// every slot is one clip of the B = 1 whole-clip call, so drop_band never applies, whatever num_groups_in_drop_band says
-static int fsn_stream_check(const fsn_model_desc* d, int n_fft, int hop, int win_length, Dims& m, StreamGeom& g) {
+// every slot is one clip of the B = 1 whole-clip call, so drop_band never applies, whatever num_groups_in_drop_band says.
+// tc: the tensor-core stream (fsn_stream_tc_*), which takes FSN_PREC_F16X3_TC / FSN_PREC_F16_TC instead of FSN_PREC_FP32
+static int fsn_stream_check(const fsn_model_desc* d, int n_fft, int hop, int win_length, Dims& m, StreamGeom& g,
+                            bool tc = false) {
   FSN_REQUIRE(d, FSN_ERR_SHAPE, "stream: null descriptor");
   fsn_model_desc dd = *d;
   dd.num_groups_in_drop_band = 1;
@@ -367,27 +369,47 @@ static int fsn_stream_check(const fsn_model_desc* d, int n_fft, int hop, int win
               "stream: the offline norm needs the whole clip; streaming is built for cumulative_laplace_norm and "
               "forgetting_norm");
   FSN_REQUIRE(d->cell_type == FSN_CELL_LSTM, FSN_ERR_UNSUPPORTED, "stream: streaming is built for the LSTM cell");
-  FSN_REQUIRE(d->precision == FSN_PREC_FP32, FSN_ERR_UNSUPPORTED,
-              "stream: streaming is built for FSN_PREC_FP32 (precision %d)", d->precision);
+  if (tc) {
+    FSN_REQUIRE(d->precision == FSN_PREC_F16X3_TC || d->precision == FSN_PREC_F16_TC, FSN_ERR_UNSUPPORTED,
+                "stream_tc: the tensor-core stream is built for FSN_PREC_F16X3_TC and FSN_PREC_F16_TC (precision %d); "
+                "the fp32 kernels stream through fsn_stream_step", d->precision);
+    FSN_REQUIRE(sb_tc_supported(d), FSN_ERR_UNSUPPORTED,
+                "stream_tc: the tensor-core sub band needs sb_hidden in {128,256,384} and sub-band input width <= 32");
+  } else {
+    FSN_REQUIRE(d->precision == FSN_PREC_FP32, FSN_ERR_UNSUPPORTED,
+                "stream: streaming is built for FSN_PREC_FP32 (precision %d)", d->precision);
+  }
   FSN_REQUIRE(n_fft / 2 + 1 == d->num_freqs, FSN_ERR_SHAPE, "stream: n_fft/2+1 = %d != num_freqs = %d", n_fft / 2 + 1,
               d->num_freqs);
   return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
 }
 
 struct FsnStreamWs {
-  int *pos0, *act0, *tail;
+  int *pos0, *act0, *tail, *restart;
   float *wav, *magT, *spec, *scale1, *fbT, *scale2, *unit, *crm;
   float2 *fs, *fs2;
   float *fh[2], *fc[2], *fhall[2];       // full-band state and layer outputs
-  float *sh0[2], *sh1[2], *sc0, *sc1;    // sub-band state, h ping-pong per layer
+  float *sh0[2], *sh1[2], *sc0, *sc1;    // sub-band state, h ping-pong per layer (fp32 stream)
+  LstmTcWs ftc;                          // tensor-core full band (tensor-core stream on SEQ_PATH_TC)
   size_t bytes;
 };
 
-// St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others
-static void fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B, int K, void* base, FsnStreamWs& w) {
+// the full-band stack of a call over B slots and St steps, as the whole-clip call builds it (fb_stack)
+static SeqStack fsn_stream_fb(const fsn_model_desc* d, int B, int St) {
+  Dims m;
+  memset(&m, 0, sizeof(m));
+  m.B = B; m.Tp = St; m.F = d->num_freqs;
+  return fb_stack(d, m);
+}
+
+// St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others.  tc: the sub band's state
+// stays in the slot state (no per-row buffers), the full band gets the tensor-core workspace when it runs there
+static void fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B, int K, void* base, FsnStreamWs& w,
+                             bool tc = false) {
   Carver c(base);
   const size_t F = d->num_freqs, Hf = d->fb_hidden, St = (size_t)K + g.E, RH = (size_t)B * F * d->sb_hidden;
   w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B);
+  w.restart = tc ? c.take<int>(B) : nullptr;
   w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
   w.magT = c.take<float>(B * St * F);
   w.spec = c.take<float>(B * ((size_t)g.Q + St) * 2 * F);
@@ -401,51 +423,64 @@ static void fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B
   w.fbT = c.take<float>(B * St * F);
   w.scale2 = d->norm_type == FSN_NORM_FORGETTING ? c.take<float>(St * B) : nullptr;
   w.unit = c.take<float>(St * B * F);
-  for (int i = 0; i < 2; ++i) { w.sh0[i] = c.take<float>(RH); w.sh1[i] = c.take<float>(RH); }
-  w.sc0 = c.take<float>(RH); w.sc1 = c.take<float>(RH);
+  memset(&w.ftc, 0, sizeof(w.ftc));
+  memset(w.sh0, 0, sizeof(w.sh0)); memset(w.sh1, 0, sizeof(w.sh1));
+  w.sc0 = w.sc1 = nullptr;
+  if (!tc) {
+    for (int i = 0; i < 2; ++i) { w.sh0[i] = c.take<float>(RH); w.sh1[i] = c.take<float>(RH); }
+    w.sc0 = c.take<float>(RH); w.sc1 = c.take<float>(RH);
+  } else if (fsn_stream_fb(d, B, (int)St).tc) {
+    const int Hw = (int)Hf > cdiv((int)F, 4) ? (int)Hf : cdiv((int)F, 4);  // the Linear's prepared weights share the rows
+    lstm_tc_carve(c, (size_t)B * St, (int)(F > Hf ? F : Hf), Hw, d->precision == FSN_PREC_F16X3_TC, w.ftc);
+  }
   w.crm = c.take<float>(B * ((size_t)g.Rc + St) * 2 * F);
   w.bytes = c.off;
 }
 
 }  // namespace fsn
 
-extern "C" size_t fsn_stream_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop) {
+namespace fsn {
+
+static size_t fsn_stream_state_query(const fsn_model_desc* d, int B, int n_fft, int hop, bool tc) {
   Dims m;
   StreamGeom g;
-  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
+  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g, tc)) return 0;
   if (B <= 0) { set_error("stream: B=%d slots", B); last_error_code() = FSN_ERR_SHAPE; return 0; }
   return fsn_stream_layout(d, g).slot * (size_t)B;
 }
 
-extern "C" size_t fsn_stream_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop) {
+static size_t fsn_stream_workspace_query(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop, bool tc) {
   Dims m;
   StreamGeom g;
-  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
+  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g, tc)) return 0;
   if (B <= 0 || K_max <= 0) {
     set_error("stream: B=%d slots, K_max=%d hops", B, K_max);
     last_error_code() = FSN_ERR_SHAPE;
     return 0;
   }
   FsnStreamWs w;
-  fsn_stream_carve(d, g, B, K_max, nullptr, w);
+  fsn_stream_carve(d, g, B, K_max, nullptr, w, tc);
   return w.bytes;
 }
 
-extern "C" int fsn_stream_delay(const fsn_model_desc* d, int n_fft, int hop) {
+static int fsn_stream_delay_query(const fsn_model_desc* d, int n_fft, int hop, bool tc) {
   Dims m;
   StreamGeom g;
-  const int rc = fsn_stream_check(d, n_fft, hop, n_fft, m, g);
+  const int rc = fsn_stream_check(d, n_fft, hop, n_fft, m, g, tc);
   return rc ? -rc : g.D;
 }
 
-extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
-                               const float* wav, const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
-                               int win_length, float* enhanced, void* state, size_t state_bytes, void* workspace,
-                               size_t workspace_bytes, fsn_stream_t stream) {
-  g_launches = 0;
+// one call of either stream.  tc: the full band on the tensor cores where the whole-clip call runs it there
+// (SEQ_PATH_TC: lstm_layer_tc per layer with carried (h, c), then linear_tc), else on the per-step kernels as the fp32
+// stream; the sub band in one sb_carry_lstm_tc_kernel launch over all St steps
+static int fsn_stream_run(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                          const void* sb_packed, bool tc, const float* wav, const int32_t* start, const int32_t* tail,
+                          int B, int K, int n_fft, int hop, int win_length, float* enhanced, void* state,
+                          size_t state_bytes, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  launch_counter() = 0;
   Dims m;
   StreamGeom g;
-  int rc = fsn_stream_check(d, n_fft, hop, win_length, m, g);
+  int rc = fsn_stream_check(d, n_fft, hop, win_length, m, g, tc);
   if (rc) return rc;
   FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "stream: B=%d slots, K=%d hops", B, K);
   FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "stream: B=%d slots, at most 65535", B);
@@ -454,6 +489,7 @@ extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* f
               "stream: B=%d slots x %d frequencies x sb_hidden %d must stay below 2^31", B, m.F, d->sb_hidden);
   FSN_REQUIRE((long long)K * hop + g.D < (1 << 30), FSN_ERR_SHAPE, "stream: K=%d hops too long", K);
   FSN_REQUIRE(fb && sb && wav && enhanced, FSN_ERR_SHAPE, "stream: null argument");
+  FSN_REQUIRE(!tc || sb_packed, FSN_ERR_SHAPE, "stream_tc: the tensor-core stream needs packed sub-band weights");
   bool any_tail = false;
   for (int b = 0; tail && b < B; ++b) {
     FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * hop, FSN_ERR_SHAPE,
@@ -464,19 +500,19 @@ extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* f
   FSN_REQUIRE(state && state_bytes >= sl.slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
               state_bytes, sl.slot * (size_t)B);
   FsnStreamWs w;
-  fsn_stream_carve(d, g, B, K, workspace, w);
+  fsn_stream_carve(d, g, B, K, workspace, w, tc);
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
               workspace_bytes, w.bytes);
   // laid out for K + E steps from the workspace's start (a workspace queried for a larger K_max also fits); a call
   // without a clip's last chunk runs St = K steps and strides its buffers by St
-  const cudaStream_t st = (cudaStream_t)stream;
   char* sbase = (char*)state;
   const size_t ss = sl.slot;
   const int F = m.F, Hf = d->fb_hidden, Hs = d->sb_hidden, Ns = d->sb_num_neighbors, Nf = d->fb_num_neighbors;
   const int St = K + (any_tail ? g.E : 0), R = B * F, Kh = K * hop, Wn = g.Hs + Kh;
-  const bool fgt = d->norm_type == FSN_NORM_FORGETTING;
+  const bool fgt = d->norm_type == FSN_NORM_FORGETTING, x3 = d->precision == FSN_PREC_F16X3_TC;
   const size_t F2 = 2 * (size_t)F;
   if ((rc = stream_prologue(start, tail, B, sbase, ss, w.pos0, w.act0, w.tail, st))) return rc;
+  if (tc && (rc = stream_restart_launch(w.pos0, B, g, w.restart, st))) return rc;
   // samples: the carried history, then the chunk; spectrum: the carried Q frames, then the St frames of this call
   if ((rc = copy_rows(w.wav, (size_t)Wn * 4, sbase + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
   if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
@@ -488,13 +524,31 @@ extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* f
   if ((rc = frame_stats_launch(w.magT, B, St, F, Ns, (size_t)St * F, F, w.fs, st))) return rc;
   if ((rc = stream_norm_launch(w.fs, B, St, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sbase, ss, w.scale1, st)))
     return rc;
-  // full band on the per-step kernels seq_stack_forward runs for the per-step scale, (h, c) carried; Linear(F) + act
   const fsn_lstm_layer fl[2] = {seq_layer(*fb, 0), seq_layer(*fb, 1)};
-  const int Hfl[2] = {Hf, Hf};
-  if ((rc = stream_lstm_layers(fl, 2, Hfl, F, w.magT, w.scale1, B, St, K, g, w.pos0, sbase, ss, sl.fbh, sl.fbc, w.fh, w.fc,
-                               w.fhall, st)))
-    return rc;
-  if ((rc = fc_gemm_launch(w.fhall[1], fb->fc_w, fb->fc_b, w.fbT, B * St, Hf, F, d->fb_activation, st))) return rc;
+  if (tc && seq_stack_path(fsn_stream_fb(d, B, St)) == SEQ_PATH_TC) {
+    // full band as seq_stack_forward runs it on the tensor cores over the call's B*St rows, per-(step, clip) scale;
+    // each layer's (h, c) from the state, c stored after step K - 1 by the recurrence, h from its output at K - 1
+    for (int l = 0; l < 2; ++l) {
+      float* fh = (float*)(sbase + sl.fbh) + (size_t)l * Hf;
+      float* fc = (float*)(sbase + sl.fbc) + (size_t)l * Hf;
+      const RecCarry io{fh, fc, fc, ss / 4, w.restart, K - 1};
+      const int Kl = l ? Hf : F;
+      if ((rc = lstm_layer_tc(fl[l], l ? w.fhall[0] : w.magT, (size_t)Kl, Kl, l ? nullptr : w.scale1, St, l ? 0 : B, B, St,
+                              Hf, x3, w.ftc, w.fhall[l], st, &io)))
+        return rc;
+      if ((rc = copy_rows(fh, ss, w.fhall[l] + (size_t)(K - 1) * Hf, (size_t)St * Hf * 4, (size_t)Hf * 4, B, st))) return rc;
+    }
+    if ((rc = linear_tc(w.fhall[1], (size_t)Hf, Hf, fb->fc_w, fb->fc_b, F, d->fb_activation, w.fbT, (size_t)F,
+                        (size_t)B * St, x3, w.ftc, st)))
+      return rc;
+  } else {
+    // full band on the per-step kernels seq_stack_forward runs for the per-step scale, (h, c) carried; Linear(F) + act
+    const int Hfl[2] = {Hf, Hf};
+    if ((rc = stream_lstm_layers(fl, 2, Hfl, F, w.magT, w.scale1, B, St, K, g, w.pos0, sbase, ss, sl.fbh, sl.fbc, w.fh,
+                                 w.fc, w.fhall, st)))
+      return rc;
+    if ((rc = fc_gemm_launch(w.fhall[1], fb->fc_w, fb->fc_b, w.fbT, B * St, Hf, F, d->fb_activation, st))) return rc;
+  }
   // second norm, one scale per (step, row), rows b*F + f
   const RowMap map{B, F, F, 1};
   if (fgt) {
@@ -507,35 +561,47 @@ extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* f
                                           st))) {
     return rc;
   }
-  // sub band on the B*F rows, (h, c) of every row from the state (into the halves step 0 reads), stored after step K - 1;
-  // step j's cRM is frame Rc + j of w.crm [B, Rc + St, 2F]
-  const size_t sbw = (size_t)F * Hs * 4;
-  const Step2State s2{{w.sh0[0], w.sh0[1]}, w.sc0, {w.sh1[0], w.sh1[1]}, w.sc1, Hs, 0, true};
-  if ((rc = copy_rows(w.sh0[1], sbw, sbase + sl.sbh, ss, sbw, B, st))) return rc;
-  if ((rc = copy_rows(w.sh1[1], sbw, sbase + sl.sbh + sbw, ss, sbw, B, st))) return rc;
-  if ((rc = copy_rows(w.sc0, sbw, sbase + sl.sbc, ss, sbw, B, st))) return rc;
-  if ((rc = copy_rows(w.sc1, sbw, sbase + sl.sbc + sbw, ss, sbw, B, st))) return rc;
-  const HeadGeom hg{F, 1, 0, F, 1, ((size_t)g.Rc + St) * F2};
-  for (int j = 0; j < St; ++j) {
-    if (j <= g.c) {  // a clip's frame 0 is one of the first c + 1 steps
-      if ((rc = stream_reset_launch(w.pos0, B, g, j, F * Hs, w.sh0[(j + 1) & 1], (size_t)F * Hs, w.sc0, st))) return rc;
-      if ((rc = stream_reset_launch(w.pos0, B, g, j, F * Hs, w.sh1[(j + 1) & 1], (size_t)F * Hs, w.sc1, st))) return rc;
-    }
-    StepParams p;
-    memset(&p, 0, sizeof(p));
-    p.R = R; p.H = Hs; p.K0 = m.Ksb;
-    p.w_ih = sb->w_ih[0]; p.w_hh = sb->w_hh[0]; p.b_ih = sb->b_ih[0]; p.b_hh = sb->b_hh[0];
-    p.magT = w.magT; p.fbT = w.fbT; p.unit_scale = w.unit + (size_t)j * R;
-    p.F = F; p.Tp = St; p.t = j; p.Ns = Ns; p.Nf = Nf; p.map = map;
-    if ((rc = lstm_step2_launch(p, SEG0_GATHER, j, seq_layer(*sb, 1), s2, st))) return rc;
-    if ((rc = sb_head_launch(s2.h1_at(j), R, Hs, 1, sb->fc_w, sb->fc_b, 2, d->sb_activation, w.crm + (g.Rc + j) * F2, hg, 0,
-                             st)))
-      return rc;
-    if (j == K - 1) {
-      if ((rc = copy_rows(sbase + sl.sbh, ss, w.sh0[j & 1], sbw, sbw, B, st))) return rc;
-      if ((rc = copy_rows(sbase + sl.sbh + sbw, ss, w.sh1[j & 1], sbw, sbw, B, st))) return rc;
-      if ((rc = copy_rows(sbase + sl.sbc, ss, w.sc0, sbw, sbw, B, st))) return rc;
-      if ((rc = copy_rows(sbase + sl.sbc + sbw, ss, w.sc1, sbw, sbw, B, st))) return rc;
+  // sub band on the B*F rows, (h, c) of every row from the state, stored after step K - 1; step j's cRM is frame Rc + j
+  // of w.crm [B, Rc + St, 2F]
+  if (tc) {
+    SbTcArgs a;
+    memset(&a, 0, sizeof(a));
+    a.packed = sb_packed; a.magT = w.magT; a.fbT = w.fbT; a.unit_scale = w.unit; a.crm = w.crm;
+    a.B = B; a.F = F; a.Tp = St; a.la = 0; a.Ns = Ns; a.Nf = Nf; a.H = Hs; a.act = d->sb_activation; a.map = map;
+    a.x3 = x3;
+    const SbCarry io{(float*)(sbase + sl.sbh), (float*)(sbase + sl.sbc), ss / 4, (size_t)F * Hs, F, w.restart, K - 1,
+                     ((size_t)g.Rc + St) * F2, g.Rc};
+    if ((rc = sb_tc_carry_forward(a, io, st))) return rc;
+  } else {
+    // (h, c) into the halves step 0 reads
+    const size_t sbw = (size_t)F * Hs * 4;
+    const Step2State s2{{w.sh0[0], w.sh0[1]}, w.sc0, {w.sh1[0], w.sh1[1]}, w.sc1, Hs, 0, true};
+    if ((rc = copy_rows(w.sh0[1], sbw, sbase + sl.sbh, ss, sbw, B, st))) return rc;
+    if ((rc = copy_rows(w.sh1[1], sbw, sbase + sl.sbh + sbw, ss, sbw, B, st))) return rc;
+    if ((rc = copy_rows(w.sc0, sbw, sbase + sl.sbc, ss, sbw, B, st))) return rc;
+    if ((rc = copy_rows(w.sc1, sbw, sbase + sl.sbc + sbw, ss, sbw, B, st))) return rc;
+    const HeadGeom hg{F, 1, 0, F, 1, ((size_t)g.Rc + St) * F2};
+    for (int j = 0; j < St; ++j) {
+      if (j <= g.c) {  // a clip's frame 0 is one of the first c + 1 steps
+        if ((rc = stream_reset_launch(w.pos0, B, g, j, F * Hs, w.sh0[(j + 1) & 1], (size_t)F * Hs, w.sc0, st))) return rc;
+        if ((rc = stream_reset_launch(w.pos0, B, g, j, F * Hs, w.sh1[(j + 1) & 1], (size_t)F * Hs, w.sc1, st))) return rc;
+      }
+      StepParams p;
+      memset(&p, 0, sizeof(p));
+      p.R = R; p.H = Hs; p.K0 = m.Ksb;
+      p.w_ih = sb->w_ih[0]; p.w_hh = sb->w_hh[0]; p.b_ih = sb->b_ih[0]; p.b_hh = sb->b_hh[0];
+      p.magT = w.magT; p.fbT = w.fbT; p.unit_scale = w.unit + (size_t)j * R;
+      p.F = F; p.Tp = St; p.t = j; p.Ns = Ns; p.Nf = Nf; p.map = map;
+      if ((rc = lstm_step2_launch(p, SEG0_GATHER, j, seq_layer(*sb, 1), s2, st))) return rc;
+      if ((rc = sb_head_launch(s2.h1_at(j), R, Hs, 1, sb->fc_w, sb->fc_b, 2, d->sb_activation, w.crm + (g.Rc + j) * F2, hg,
+                               0, st)))
+        return rc;
+      if (j == K - 1) {
+        if ((rc = copy_rows(sbase + sl.sbh, ss, w.sh0[j & 1], sbw, sbw, B, st))) return rc;
+        if ((rc = copy_rows(sbase + sl.sbh + sbw, ss, w.sh1[j & 1], sbw, sbw, B, st))) return rc;
+        if ((rc = copy_rows(sbase + sl.sbc, ss, w.sc0, sbw, sbw, B, st))) return rc;
+        if ((rc = copy_rows(sbase + sl.sbc + sbw, ss, w.sc1, sbw, sbw, B, st))) return rc;
+      }
     }
   }
   // cRM: the carried Rc frames before the call's; iSTFT
@@ -547,4 +613,44 @@ extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* f
   if ((rc = copy_rows(sbase + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
   if ((rc = copy_rows(sbase + sl.spec, ss, w.spec + K * F2, (g.Q + St) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
   return copy_rows(sbase + sl.crm, ss, w.crm + K * F2, (g.Rc + St) * F2 * 4, g.Rc * F2 * 4, B, st);
+}
+
+}  // namespace fsn
+
+extern "C" size_t fsn_stream_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop) {
+  return fsn_stream_state_query(d, B, n_fft, hop, false);
+}
+
+extern "C" size_t fsn_stream_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop) {
+  return fsn_stream_workspace_query(d, B, K_max, n_fft, hop, false);
+}
+
+extern "C" int fsn_stream_delay(const fsn_model_desc* d, int n_fft, int hop) { return fsn_stream_delay_query(d, n_fft, hop, false); }
+
+extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                               const float* wav, const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
+                               int win_length, float* enhanced, void* state, size_t state_bytes, void* workspace,
+                               size_t workspace_bytes, fsn_stream_t stream) {
+  return fsn_stream_run(d, fb, sb, nullptr, false, wav, start, tail, B, K, n_fft, hop, win_length, enhanced, state,
+                        state_bytes, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t fsn_stream_tc_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop) {
+  return fsn_stream_state_query(d, B, n_fft, hop, true);
+}
+
+extern "C" size_t fsn_stream_tc_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop) {
+  return fsn_stream_workspace_query(d, B, K_max, n_fft, hop, true);
+}
+
+extern "C" int fsn_stream_tc_delay(const fsn_model_desc* d, int n_fft, int hop) {
+  return fsn_stream_delay_query(d, n_fft, hop, true);
+}
+
+extern "C" int fsn_stream_tc_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                                  const void* sb_packed, const float* wav, const int32_t* start, const int32_t* tail, int B,
+                                  int K, int n_fft, int hop, int win_length, float* enhanced, void* state,
+                                  size_t state_bytes, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  return fsn_stream_run(d, fb, sb, sb_packed, true, wav, start, tail, B, K, n_fft, hop, win_length, enhanced, state,
+                        state_bytes, workspace, workspace_bytes, (cudaStream_t)stream);
 }

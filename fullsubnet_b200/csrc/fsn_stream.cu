@@ -156,6 +156,17 @@ int stream_reset_launch(const int* pos0, int B, const StreamGeom& g, int j, int 
   return FSN_OK;
 }
 
+__global__ void stream_restart_kernel(const int* __restrict__ pos0, int B, int hop, int c, int* __restrict__ restart) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) restart[b] = c - pos0[b] / hop;
+}
+
+int stream_restart_launch(const int* pos0, int B, const StreamGeom& g, int* restart, cudaStream_t st) {
+  stream_restart_kernel<<<cdiv(B, 128), 128, 0, st>>>(pos0, B, g.hop, g.c, restart);
+  FSN_CHECK_LAUNCH("stream_restart_kernel");
+  return FSN_OK;
+}
+
 int stream_lstm_layers(const fsn_lstm_layer* L, int n, const int* H, int K0, const float* x, const float* scaleT, int B,
                        int S, int K, const StreamGeom& g, const int* pos0, char* state, size_t slot_bytes, size_t h_off,
                        size_t c_off, float* const* h, float* const* c, float* const* hall, cudaStream_t st) {

@@ -39,6 +39,14 @@
 // steps first; the ring streams only W_hh0, W_ih1 and W_hh1 (packer mode `proj`), each layer-0 accumulator starts from
 // the cell's four gate values of P[t] instead of zero, and layer 1 stores h1_t (fp32) to h1 [T, R, H] instead of
 // running a Linear.  Warps 2 and 3 idle.
+//
+// CARRY (sb_carry_lstm_tc_kernel, chunked streaming, DESIGN 4.14): the same stack continued from a carried state.  Before
+// step 0 each row's fp32 (h, c) of both layers is read from a.io_h / a.io_c: h split into hi / lo into the h0 buffer step 0
+// reads and into h1 (the split the cell applies to h, so the MMAs see the bits an uninterrupted run would), c into the
+// consumers' registers.  A row whose slot restarts at step j (a.restart) enters step j with zero state: its c is dropped
+// there and its h of step j - 1 is written to shared memory as zero (j = 0: not loaded).  After step a.store_step the
+// fp32 (h, c) go back to io_h / io_c while the kernel runs on; step t's Linear output goes to frame crm_t0 + t of a
+// frame-major [clips, frames, 2F] cRM.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -189,7 +197,10 @@ static_assert(sizeof(Bars) <= 256, "barrier block too large");
 struct RowInfo {
   int src_b, src_f;   // source clip / frequency (drop_band map), src_b < 0: row beyond the batch
   float scale;        // 1 / (mu' + 1e-5) of the source clip
-  int out_idx;        // crm index of (b', o=0, f', t=0) divided by T  (= (b'*2)*Fsub + f')
+  union {
+    int out_idx;      // crm index of (b', o=0, f', t=0) divided by T  (= (b'*2)*Fsub + f')
+    int restart;      // CARRY: the step at which the row enters with zero state (none when outside [0, Tp))
+  };
 };
 
 // The kernel takes KArgs as a __grid_constant__ parameter: its fields stay in parameter (constant-bank) space and are
@@ -210,6 +221,13 @@ struct KArgs {
   int stamp_ctas, stamp_its;
   // PROJ instantiation only: layer 0's input projection P [Tp, R, 4H] and the layer-1 output h1 [Tp, R, H] (fp32)
   const float* proj; float* h1;
+  // CARRY instantiation only: (h, c) of row r, layer l, unit u at io_h / io_c [(r / io_rps) io_slot + l io_layer +
+  // (r % io_rps) H + u] (floats), restart step of row r at restart[r / io_rps], state stored after step store_step;
+  // output o of row r = b F + f at step t to crm[b crm_bs + (crm_t0 + t) 2F + o F + f]
+  float* io_h; float* io_c;
+  size_t io_slot, io_layer, crm_bs;
+  const int* restart;
+  int io_rps, store_step, crm_t0;
 };
 
 // ---------------------------------------------------------------- cycle stamps (PROBE instantiation)
@@ -288,11 +306,17 @@ __device__ __forceinline__ float proj_at(const KArgs& a, int t, int row0, int s,
   return __ldg(a.proj + ((size_t)t * a.R + r) * 4 * a.H + g * a.H + u);
 }
 
+// CARRY: offset of row r's unit u in the layer-0 block of io_h / io_c
+__device__ __forceinline__ size_t carry_idx(const KArgs& a, int r, int u) {
+  const int sl = r / a.io_rps;
+  return (size_t)sl * a.io_slot + (size_t)(r - sl * a.io_rps) * a.H + u;
+}
+
 // PROBE: the same kernel with cycle stamps (ProbeField) written to a.stamps; the production launches use PROBE = false,
 // where every stamp below compiles away.  PROJ: the precomputed layer-0 projection and stored h1 (see the top of the
-// file); every PROJ branch below is `if constexpr` or folds away, so the sb_lstm_tc_kernel instantiations are the code
-// they were before the policy existed
-template <bool X3, bool PROBE, bool PROJ>
+// file); every PROJ and CARRY branch below is `if constexpr` or folds away, so the sb_lstm_tc_kernel instantiations are
+// the code they were before the policies existed
+template <bool X3, bool PROBE, bool PROJ, bool CARRY>
 __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
   constexpr int PARTS = X3 ? 2 : 1;
   // probe clock: cycles since the previous mark (0 and no code without PROBE)
@@ -358,9 +382,13 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
     ri.src_b = -1; ri.src_f = 0; ri.scale = 0.f; ri.out_idx = 0;
     if (r < a.R) {
       row_to_unit(a.map, r, ri.src_b, ri.src_f);
-      ri.scale = a.inv2[ri.src_b];
-      const int bq = r / a.Fsub, fq = r - bq * a.Fsub;
-      ri.out_idx = bq * 2 * a.Fsub + fq;
+      if constexpr (CARRY) {
+        ri.restart = a.restart[r / a.io_rps];
+      } else {
+        ri.scale = a.inv2[ri.src_b];
+        const int bq = r / a.Fsub, fq = r - bq * a.Fsub;
+        ri.out_idx = bq * 2 * a.Fsub + fq;
+      }
     }
     rows[threadIdx.x] = ri;
   }
@@ -368,6 +396,23 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
     uint4* z = reinterpret_cast<uint4*>(smem + sp.x);
     const int n16 = (sp.fcw - sp.x) / 16;
     for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
+  }
+  if constexpr (CARRY) {
+    // h_{-1} of both layers for all H units of the pair's rows: layer 0 into the h0 buffer step 0 reads (buffer 1),
+    // layer 1 into h1, in the B-operand layout the consumers write (unit U = 64 s + u of row n)
+    __syncthreads();
+    const int nkh0 = H / KB;
+    for (int i = threadIdx.x; i < 2 * NB * H; i += blockDim.x) {
+      const int l = i / (NB * H), n = (i / H) % NB, U = i % H;
+      const int r = row0 + n;
+      if (r >= a.R || a.restart[r / a.io_rps] == 0) continue;
+      const float v = a.io_h[carry_idx(a, r, U) + l * a.io_layer];
+      uint8_t* p = smem + (l ? sp.h1 : sp.h0 + nkh0 * S_KBLK) + (U >> 6) * S_KBLK + (n >> 3) * 1024 + (n & 7) * 128 +
+                   ((((U & 63) >> 3) ^ (n & 7)) << 4) + (U & 7) * 2;
+      const __half hi = __float2half_rn(v);
+      *reinterpret_cast<__half*>(p) = hi;
+      if (X3) *reinterpret_cast<__half*>(p + (sp.lo - sp.x)) = __float2half_rn(v - __half2float(hi));
+    }
   }
   fence_proxy_async_smem();
   __syncthreads();
@@ -491,8 +536,14 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
         if (ri.src_b >= 0) {
 #pragma unroll
           for (int o = 0; o < 2; ++o) {
-            float* dst = a.crm + ((size_t)ri.out_idx + (size_t)o * a.Fsub) * a.T + t_stage0;
-            for (int i = 0; i < staged; ++i) dst[i] = outst[(lane * 2 + o) * OUT_T + i];
+            if constexpr (CARRY) {
+              const size_t F2 = 2 * (size_t)a.F;
+              float* dst = a.crm + (size_t)ri.src_b * a.crm_bs + ((size_t)a.crm_t0 + t_stage0) * F2 + (size_t)o * a.F + ri.src_f;
+              for (int i = 0; i < staged; ++i) dst[i * F2] = outst[(lane * 2 + o) * OUT_T + i];
+            } else {
+              float* dst = a.crm + ((size_t)ri.out_idx + (size_t)o * a.Fsub) * a.T + t_stage0;
+              for (int i = 0; i < staged; ++i) dst[i] = outst[(lane * 2 + o) * OUT_T + i];
+            }
           }
         }
         staged = 0;
@@ -516,6 +567,19 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
       float c0[16], c1[16];
 #pragma unroll
       for (int i = 0; i < 16; ++i) c0[i] = c1[i] = 0.f;
+      if constexpr (CARRY) {
+        // c_{-1} of this thread's fragment (a row restarting at step 0 drops it in its first cell)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int hh = i >> 3, j = (i >> 1) & 3, e = i & 1;
+          const int r = row0 + 8 * j + 2 * (lane & 3) + e;
+          if (r < a.R) {
+            const float* p = a.io_c + carry_idx(a, r, s * US + 16 * q + (lane >> 2) + 8 * hh);
+            c0[i] = p[0];
+            c1[i] = p[a.io_layer];
+          }
+        }
+      }
       // per-kernel constants of the stage loop: the A descriptor of ring slot 0 (a slot is W_TILE >> 4 further), the
       // barriers, and which warps release a stage where (see release_stage)
       const uint32_t a_lo0 = wg::desc_lo(smem_u32(smem + sp.w));
@@ -684,13 +748,30 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
               for (int e = 0; e < 2; ++e) {
                 const int ri = 4 * j + 2 * hh + e;
                 const int ci = hh * 8 + j * 2 + e;
-                const float cp = layer ? c1[ci] : c0[ci];
+                float cp = layer ? c1[ci] : c0[ci];
+                if constexpr (CARRY) {
+                  if (rows[8 * j + 2 * (lane & 3) + e].restart == t) cp = 0.f;
+                }
                 const float cn = sg<X3>(acc[1][ri] + bff) * cp + sg<X3>(acc[0][ri] + bi) * th<X3>(acc[2][ri] + bg);
                 if (layer) c1[ci] = cn; else c0[ci] = cn;
                 const float h = sg<X3>(acc[3][ri] + bo) * th<X3>(cn);
-                const __half hi = __float2half_rn(h);
+                __half hi = __float2half_rn(h);
+                __half lo = __float2half_rn(h - __half2float(hi));
+                if constexpr (CARRY) {
+                  const int n = 8 * j + 2 * (lane & 3) + e, r = row0 + n;
+                  if (t == a.store_step && r < a.R) {
+                    const size_t o = carry_idx(a, r, u) + layer * a.io_layer;
+                    a.io_h[o] = h;
+                    a.io_c[o] = cn;
+                  }
+                  // the row enters step t + 1 with zero state: its h_t operand is zero.  Layer 1 of step t then reads a
+                  // zero h0_t, so this row's output at step t is wrong.  Exactness needs that output never read: step t
+                  // is frame -1 of the slot's new clip, its cRM is frame -1 - look_ahead, and istft_stream_kernel reads
+                  // frames >= 0 only (the fp32 stream's stream_reset_kernel zeroes the same operand)
+                  if (rows[n].restart == t + 1) hi = lo = __float2half_rn(0.f);
+                }
                 hv[hh][j * 2 + e] = hi;
-                lv[hh][j * 2 + e] = __float2half_rn(h - __half2float(hi));
+                lv[hh][j * 2 + e] = lo;
                 if (!PROJ && layer) { fsum[0][j * 2 + e] += h * w0; fsum[1][j * 2 + e] += h * w1; }
                 if constexpr (PROJ) {
                   const int r = row0 + 8 * j + 2 * (lane & 3) + e;
@@ -782,13 +863,19 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
 // fullsubnet's sub-band stack and fast_fullsubnet's bottleneck: gathered x_t, fused Linear
 template <bool X3, bool PROBE>
 __global__ void __launch_bounds__(NTHREADS, 1) sb_lstm_tc_kernel(const __grid_constant__ KArgs a) {
-  sb_lstm_tc_body<X3, PROBE, false>(a);
+  sb_lstm_tc_body<X3, PROBE, false, false>(a);
 }
 
 // improved_fullsubnet's sections: precomputed layer-0 projection, h1 stored for the caller's head
 template <bool X3>
 __global__ void __launch_bounds__(NTHREADS, 1) sb_proj_lstm_tc_kernel(const __grid_constant__ KArgs a) {
-  sb_lstm_tc_body<X3, false, true>(a);
+  sb_lstm_tc_body<X3, false, true, false>(a);
+}
+
+// chunked streaming: fullsubnet's sub-band stack continued from a carried (h, c), frame-major cRM
+template <bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) sb_carry_lstm_tc_kernel(const __grid_constant__ KArgs a) {
+  sb_lstm_tc_body<X3, false, false, true>(a);
 }
 
 }  // namespace tc
@@ -866,8 +953,8 @@ static int sb_tc_launch(const tc::KArgs& a, int H, cudaStream_t st) {
   return FSN_OK;
 }
 
-int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
-  tc::KArgs a;
+static int sb_tc_kargs(const SbTcArgs& s, tc::KArgs& a) {
+  memset(&a, 0, sizeof(a));
   a.packed = (const uint8_t*)s.packed;
   a.magT = s.magT; a.fbT = s.fbT; a.inv2 = s.inv2; a.unit_scale = s.unit_scale; a.crm = s.crm;
   a.R = s.map.B * s.map.Fsub; a.F = s.F; a.Tp = s.steps > 0 ? s.steps : s.Tp; a.la = s.la; a.T = a.Tp - s.la;
@@ -883,8 +970,37 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
   // an explicit launch configuration (the unit-test hook) overrides the environment
   a.stages = s.stages ? s.stages : stages;
   a.cluster = s.cluster ? s.cluster : cluster;
+  return FSN_OK;
+}
+
+int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
+  tc::KArgs a;
+  int rc = sb_tc_kargs(s, a);
+  if (rc) return rc;
   if (s.stamps) return s.x3 ? sb_tc_launch<true, true>(a, s.H, st) : sb_tc_launch<false, true>(a, s.H, st);
   return s.x3 ? sb_tc_launch<true, false>(a, s.H, st) : sb_tc_launch<false, false>(a, s.H, st);
+}
+
+int sb_tc_carry_forward(const SbTcArgs& s, const SbCarry& io, cudaStream_t st) {
+  FSN_REQUIRE(s.unit_scale && io.h && io.c && io.restart && io.rps > 0 && s.la == 0 && s.shrink <= 1 && s.map.G <= 1,
+              FSN_ERR_SHAPE, "sb_carry_lstm_tc: per-row scales, state, restart steps, la = 0 and no drop_band / shrink");
+  tc::KArgs a;
+  int rc = sb_tc_kargs(s, a);
+  if (rc) return rc;
+  a.io_h = io.h; a.io_c = io.c; a.io_slot = io.slot; a.io_layer = io.layer; a.io_rps = io.rps;
+  a.restart = io.restart; a.store_step = io.store_step; a.crm_bs = io.crm_bs; a.crm_t0 = io.crm_t0;
+  const int pairs = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  const void* kern = s.x3 ? (const void*)tc::sb_carry_lstm_tc_kernel<true> : (const void*)tc::sb_carry_lstm_tc_kernel<false>;
+  rc = s.x3 ? sb_tc_config<true>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, kern)
+            : sb_tc_config<false>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, kern);
+  if (rc) return rc;
+  rc = s.x3 ? check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_carry_lstm_tc_kernel<true>, a), "sb_carry_lstm_tc_kernel launch")
+            : check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_carry_lstm_tc_kernel<false>, a), "sb_carry_lstm_tc_kernel launch");
+  if (rc) return rc;
+  FSN_CHECK_LAUNCH("sb_carry_lstm_tc_kernel");
+  return FSN_OK;
 }
 
 int sb_proj_forward(const SbProjArgs& s, cudaStream_t st) {
@@ -1025,4 +1141,34 @@ extern "C" int fsn_debug_sb_lstm_tc_probe(const fsn_seq_weights* sb, int H, int 
   FSN_REQUIRE(stamps, FSN_ERR_SHAPE, "sb_lstm_tc probe: missing stamp buffer");
   return sb_lstm_tc_hook(sb, H, Ns, Nf, fc_out, act, x3, magT, fbT, B, F, src_T, G, inv2, unit_scale, la, steps, shrink,
                          stages, cluster, packed, crm, stamps, stamp_ctas, stamp_steps, stream);
+}
+
+// unit-test hook (tests/test_gpu_fsn_stream_tc.py): the carry instantiation on caller-provided inputs.  B clips of F rows
+// (rows b F + f), per-(step, row) scales unit_scale [steps, B F], magT / fbT [B, src_T, F]; h / c [2, B F, H] hold the
+// state entering step 0 and receive the state after store_step (-1: none); restart [B F] per row; crm [B, steps, 2F]
+extern "C" int fsn_debug_sb_lstm_tc_carry(const fsn_seq_weights* sb, int H, int Ns, int Nf, int act, int x3,
+                                          const float* magT, const float* fbT, int B, int F, int src_T,
+                                          const float* unit_scale, int steps, const int32_t* restart, int store_step,
+                                          float* h, float* c, void* packed, float* crm, fsn_stream_t stream) {
+  using namespace fsn;
+  FSN_REQUIRE(sb && magT && fbT && unit_scale && restart && h && c && packed && crm, FSN_ERR_SHAPE,
+              "sb_carry_lstm_tc: missing buffer");
+  FSN_REQUIRE(B > 0 && F > 1 && src_T > 0 && Ns >= 0 && Nf >= 0 && Ns < F && Nf < F && steps > 0 && steps <= src_T &&
+                  store_step >= -1 && store_step < steps,
+              FSN_ERR_SHAPE, "sb_carry_lstm_tc: bad shape B=%d F=%d src_T=%d steps=%d store_step=%d", B, F, src_T, steps,
+              store_step);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "sb_carry_lstm_tc: activation %d", act);
+  FSN_REQUIRE(sb_tc_shape_ok(H, (2 * Ns + 1) + (2 * Nf + 1)), FSN_ERR_UNSUPPORTED,
+              "sb_carry_lstm_tc: unsupported hidden size %d / input width %d", H, (2 * Ns + 1) + (2 * Nf + 1));
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = sb_tc_pack_raw(sb, H, (2 * Ns + 1) + (2 * Nf + 1), 2, packed, st, x3 != 0);
+  if (rc) return rc;
+  SbTcArgs a;
+  memset(&a, 0, sizeof(a));
+  a.packed = packed; a.magT = magT; a.fbT = fbT; a.unit_scale = unit_scale; a.crm = crm;
+  a.B = B; a.F = F; a.Tp = src_T; a.Ns = Ns; a.Nf = Nf; a.H = H; a.act = act; a.steps = steps; a.x3 = x3 != 0;
+  a.map = RowMap{B, F, F, 1};
+  const size_t R = (size_t)B * F;
+  const SbCarry io{h, c, (size_t)H, R * H, 1, restart, store_step, (size_t)steps * 2 * F, 0};
+  return sb_tc_carry_forward(a, io, st);
 }

@@ -27,6 +27,9 @@ class Model(SpectrogramEnhance, BaseModel):
     # chunked streaming (fullsubnet_b200.stream.Streamer, precision="fp32" with cumulative_laplace_norm or
     # forgetting_norm): state / workspace queries, delay, step
     STREAM_ENTRY_POINTS = ("fsn_stream_state_bytes", "fsn_stream_workspace_bytes", "fsn_stream_delay", "fsn_stream_step")
+    # the same on the fp16 tensor cores (Streamer(tensor_cores=True), the model's f16x3_tc / f16_tc precision)
+    STREAM_TC_ENTRY_POINTS = ("fsn_stream_tc_state_bytes", "fsn_stream_tc_workspace_bytes", "fsn_stream_tc_delay",
+                              "fsn_stream_tc_step")
 
     def __init__(self, num_freqs, look_ahead, sequence_model, fb_num_neighbors, sb_num_neighbors,
                  fb_output_activate_function, sb_output_activate_function, fb_model_hidden_size,
@@ -85,6 +88,22 @@ class Model(SpectrogramEnhance, BaseModel):
 
     def _stream_weights(self):
         return C.byref(self.fb_model.weight_struct()), C.byref(self.sb_model.weight_struct())
+
+    def _stream_tc_desc(self):
+        """Descriptor of the tensor-core streaming calls: the model's resolved precision, which must be f16x3_tc or
+        f16_tc (so "auto" streams the bits of the whole-clip call wherever that call runs the tensor cores)."""
+        prec = self._resolve_precision()
+        if prec == "fp32":
+            raise NotImplementedError("fullsubnet_b200: this model resolves to precision=\"fp32\"; stream it with the "
+                                      "default Streamer(model, slots) (tensor_cores=False)")
+        return self._desc(prec, 1)
+
+    def _stream_tc_weights(self):
+        desc = self._stream_tc_desc()
+        device = next(self.parameters()).device
+        fb_w, sb_w = self.fb_model.weight_struct(), self.sb_model.weight_struct()
+        packed = self._packed_sb(desc, sb_w, device)
+        return C.byref(fb_w), C.byref(sb_w), _lib.ptr(packed)
 
     def _train_desc(self):
         return self._desc(self._resolve_train_precision(), int(self.num_groups_in_drop_band))

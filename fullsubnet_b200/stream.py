@@ -4,7 +4,11 @@ each clip, the samples of the whole-clip ``enhance`` call bit for bit, ``delay``
 Built for fullband_baseline with ``cumulative_laplace_norm`` or ``forgetting_norm`` (LSTM, fp32), for fullsubnet with
 ``cumulative_laplace_norm`` or ``forgetting_norm`` (LSTM, ``precision="fp32"``) and for fast_fullsubnet with
 ``cumulative_laplace_norm`` (LSTM, ``precision="fp32"``).  Each model names its library calls in
-``STREAM_ENTRY_POINTS`` and gives their arguments through ``_stream_desc()`` and ``_stream_weights()``."""
+``STREAM_ENTRY_POINTS`` and gives their arguments through ``_stream_desc()`` and ``_stream_weights()``.
+
+``tensor_cores=True`` streams fullsubnet on its fp16 tensor-core precision (``f16x3_tc`` or ``f16_tc``, what the model
+resolves to), bit for bit the whole-clip call of that precision, through ``STREAM_TC_ENTRY_POINTS``,
+``_stream_tc_desc()`` and ``_stream_tc_weights()``."""
 from __future__ import annotations
 
 import ctypes as C
@@ -25,16 +29,25 @@ class Streamer:
     pos - delay + K*hop), pos being the clip's position before the call (negative positions as 0); on the call that
     ends the clip the row holds the samples from pos - delay to the clip's end, then 0."""
 
-    def __init__(self, model, slots: int, n_fft: int = 512, hop: int = 256, win_length: int = 512):
-        names = getattr(type(model), "STREAM_ENTRY_POINTS", ())
-        if not names:
-            raise NotImplementedError("fullsubnet_b200: chunked streaming is built for fullband_baseline, fullsubnet "
-                                      "and fast_fullsubnet")
+    def __init__(self, model, slots: int, n_fft: int = 512, hop: int = 256, win_length: int = 512,
+                 tensor_cores: bool = False):
+        if tensor_cores:
+            names = getattr(type(model), "STREAM_TC_ENTRY_POINTS", ())
+            if not names:
+                raise NotImplementedError("fullsubnet_b200: tensor-core streaming (tensor_cores=True) is built for "
+                                          "fullsubnet")
+            self._desc_of, self._weights_of = model._stream_tc_desc, model._stream_tc_weights
+        else:
+            names = getattr(type(model), "STREAM_ENTRY_POINTS", ())
+            if not names:
+                raise NotImplementedError("fullsubnet_b200: chunked streaming is built for fullband_baseline, fullsubnet "
+                                          "and fast_fullsubnet")
+            self._desc_of, self._weights_of = model._stream_desc, model._stream_weights
         self.model, self.slots, self.n_fft, self.hop, self.win_length = model, int(slots), n_fft, hop, win_length
         self.device = next(model.parameters()).device
         lib = _lib.load()
         self._state_bytes, self._workspace_bytes, self._delay, self._step = (getattr(lib, n) for n in names)
-        d = model._stream_desc()
+        d = self._desc_of()
         delay = self._delay(C.byref(d), n_fft, hop)
         if delay < 0:
             _lib.check(-delay)
@@ -102,7 +115,7 @@ class Streamer:
         assert chunk.shape[1] % self.hop == 0, f"a chunk is a whole number of hops ({self.hop} samples)"
         K = chunk.shape[1] // self.hop
         x = _lib.require_cuda(chunk, "chunk")
-        d, weights = self.model._stream_desc(), self.model._stream_weights()
+        d, weights = self._desc_of(), self._weights_of()
         ws = self._workspace(d, K)
         st, tl = self._table(start, 0), self._table(tail, -1)
         pos = self._check_lengths(K, st, tl)

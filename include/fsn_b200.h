@@ -553,6 +553,22 @@ int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fs
                     float* enhanced, void* state, size_t state_bytes, void* workspace, size_t workspace_bytes,
                     fsn_stream_t stream);
 
+/* The same stream on the fp16 tensor cores (DESIGN 4.14.1): d->precision FSN_PREC_F16X3_TC or FSN_PREC_F16_TC, the
+ * output of every clip bit-identical to fsn_enhance of that precision on the whole clip (lengths NULL, B = 1), delayed
+ * by D = fsn_stream_tc_delay(d, n_fft, hop), the fsn_stream_delay of the same shape.  The state is the fp32 stream's
+ * slot layout, byte for byte (fsn_stream_tc_state_bytes = fsn_stream_state_bytes of the FSN_PREC_FP32 descriptor): h and
+ * c stay fp32, and the kernels split h into fp16 hi / lo on load as they do after every step.  sb_packed: the
+ * fsn_pack_sb_weights image fsn_enhance takes.  Semantics, limits and buffers as fsn_stream_step; FSN_PREC_FP32, the
+ * offline norm, the GRU cell, sub-band shapes the tensor-core kernel cannot take, other n_fft and B > 65535 ->
+ * FSN_ERR_UNSUPPORTED, a null sb_packed -> FSN_ERR_SHAPE, before any CUDA call.  Appended in ABI version 102. */
+size_t fsn_stream_tc_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop);
+size_t fsn_stream_tc_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop);
+int fsn_stream_tc_delay(const fsn_model_desc* d, int n_fft, int hop);
+int fsn_stream_tc_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
+                       const void* sb_packed, const float* wav, const int32_t* start, const int32_t* tail, int B, int K,
+                       int n_fft, int hop, int win_length, float* enhanced, void* state, size_t state_bytes,
+                       void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+
 /* Training step of recipes/dns_interspeech_2020/fullband_baseline/trainer.py:32-71, same conventions as fsn_train_*: the
  * caller allocates the workspace and passes the same untouched buffer from forward to backward; the gradients of all
  * 4 * num_layers + 2 parameters are OVERWRITTEN; no host synchronisation; arguments are checked before any CUDA call;
@@ -680,6 +696,12 @@ int fsn_debug_lstm_layer_tc(const float* w_ih, const float* w_hh, const float* b
                             fsn_stream_t stream);
 int fsn_debug_linear_tc(const float* x, int rows, int K, const float* W, const float* bias, int N, int act, int x3,
                         float* out, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+/* the same layer continued from a carried state (the tensor-core stream's full band): row r enters step 0 with h_init /
+ * c [r*H + u] and step restart[r] with zero state (restart[r] = 0: they are ignored); c after step fin_step (-1: none) is
+ * written back to c, h of every step is in hall.  Workspace: fsn_debug_lstm_tc_workspace_bytes. */
+int fsn_debug_lstm_tc_carry(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* x,
+                            int R, int T, int K, int H, int x3, const float* h_init, float* c, const int32_t* restart,
+                            int fin_step, float* hall, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 /* unit-test hook for the sub-band tensor-core stack (fsn_subband_tc.cu; model.py:98-135): packs sb (2 LSTM layers of
  * hidden size H over Ksb = (2Ns+1)+(2Nf+1) inputs, Linear(H -> fc_out <= 2)) into `packed`
@@ -698,6 +720,15 @@ int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int f
                          const float* magT, const float* fbT, int B, int F, int src_T, int G,
                          const float* inv2, const float* unit_scale, int la, int steps, int shrink,
                          int stages, int cluster, void* packed, float* crm, fsn_stream_t stream);
+/* the carry instantiation of the kernel (the tensor-core stream's sub band): B clips of F rows r = b*F + f, no
+ * drop_band, look-ahead 0, fc_out 2, unit_scale [steps, B*F] required.  h / c [2 layers, B*F, H] hold the state entering
+ * step 0 and receive the state after store_step (-1: none); row r enters step restart[r] with zero state (0: its h / c
+ * are ignored); crm [B, steps, 2F] receives act(Linear) of every step, channel-major per frame.  Arguments are checked before
+ * any CUDA call. */
+int fsn_debug_sb_lstm_tc_carry(const fsn_seq_weights* sb, int H, int Ns, int Nf, int act, int x3, const float* magT,
+                               const float* fbT, int B, int F, int src_T, const float* unit_scale, int steps,
+                               const int32_t* restart, int store_step, float* h, float* c, void* packed, float* crm,
+                               fsn_stream_t stream);
 /* the same run through the cycle-stamp instantiation of the kernel (same output bits): CTAs [0, stamp_ctas) (at most
  * the 2 * ceil(B * Fsub / 32) CTAs that own rows) record, for the loop iterations [0, stamp_steps) (stamp_steps <=
  * steps + 1: layer 1 runs one iteration behind layer 0), FSN_SB_PROBE_FIELDS int64 per (CTA, iteration, layer, slot)
