@@ -221,27 +221,23 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   return crm_output_launch(w.dec_out, (size_t)Tp * 2 * F, 2 * F, B, Tp, F, d->look_ahead, out, st);
 }
 
-// ---- chunked streaming (DESIGN 4.14).  Slot state block (each section on 16 bytes, blocks 256 bytes apart): meta (16
-// bytes), sample history Hs, spectrum Q x 2F, cRM Rc x 2F, the last S-1 frames of the mel spectrogram and of the encoder
-// output (M each), encoder (h | c) of both layers, the second norm's running sum and the latest bottleneck output of the
-// M rows, bottleneck (h | c) of both layers (M x Hb each), decoder (h | c) of both layers.
+// ---- chunked streaming (DESIGN 4.14).  Slot state block: the stream header (StreamSlot), then the last S-1 frames of
+// the mel spectrogram and of the encoder output (M each), encoder (h | c) of both layers, the second norm's running sum
+// and the latest bottleneck output of the M rows, bottleneck (h | c) of both layers (M x Hb each), decoder (h | c) of
+// both layers.
 namespace fsn {
 
-struct FastStreamLayout { size_t hist, spec, crm, mel, enc, eh, ec, run, bo, bh, bc, dh, dc, slot; };
+struct FastStreamLayout : StreamSlot { size_t mel, enc, eh, ec, run, bo, bh, bc, dh, dc; };
 
 static FastStreamLayout fast_stream_layout(const fsn_fast_desc* d, const StreamGeom& g) {
-  const size_t F2 = 2 * (size_t)d->num_freqs, M = d->num_mels, Hm = d->shrink_size - 1;
+  const size_t M = d->num_mels, Hm = d->shrink_size - 1;
   const size_t He = (size_t)d->enc1_hidden + d->enc2_hidden, Hb = 2 * M * d->bn_hidden, Hd = 2 * (size_t)d->dec_hidden;
-  FastStreamLayout s;
-  size_t o = sizeof(StreamMeta);
-  auto sec = [&](size_t& at, size_t floats) { at = o; o = align_up(o + floats * 4, 16); };
-  sec(s.hist, g.Hs); sec(s.spec, g.Q * F2); sec(s.crm, g.Rc * F2);
-  sec(s.mel, Hm * M); sec(s.enc, Hm * M);
-  sec(s.eh, He); sec(s.ec, He);
-  sec(s.run, M); sec(s.bo, M);
-  sec(s.bh, Hb); sec(s.bc, Hb);
-  sec(s.dh, Hd); sec(s.dc, Hd);
-  s.slot = align_up(o, 256);
+  FastStreamLayout s{StreamSlot(g, d->num_freqs)};
+  s.mel = s.sec(Hm * M); s.enc = s.sec(Hm * M);
+  s.eh = s.sec(He); s.ec = s.sec(He);
+  s.run = s.sec(M); s.bo = s.sec(M);
+  s.bh = s.sec(Hb); s.bc = s.sec(Hb);
+  s.dh = s.sec(Hd); s.dc = s.sec(Hd);
   return s;
 }
 
@@ -257,28 +253,25 @@ static int fast_stream_check(const fsn_fast_desc* d, int n_fft, int hop, int win
   return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
 }
 
-struct FastStreamWs {
-  int *pos0, *act0, *tail, *rst;
-  float *wav, *magT, *spec, *melT, *scale1, *encT, *catM, *catE, *bn, *scale2, *bo, *dec_in, *y, *crm, *pp;
+struct FastStreamWs : StreamWs {
+  int* rst;
+  float *melT, *scale1, *encT, *catM, *catE, *bn, *scale2, *bo, *dec_in, *y, *pp;
   float2* fs;
   float *eh[2], *ec[2], *ehall[2];            // encoder state and layer outputs
   float *bh0[2], *bh1[2], *bc0, *bc1;         // bottleneck state, h ping-pong per layer
   float *dh[2], *dc[2], *dfh[2], *dfc[2], *dhall[2];  // decoder state (entering the call / after step K-1), outputs
   unsigned int* barrier;
-  size_t bytes;
 };
 
 // St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others; nb = ceil(St / S) bottleneck
-// steps, the most block ends St consecutive frames can hold
-static void fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const StreamGeom& g, int B, int K, void* base,
-                              FastStreamWs& w) {
+// steps, the most block ends St consecutive frames can hold.  Returns the bytes
+static size_t fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const StreamGeom& g, int B, int K, void* base,
+                                FastStreamWs& w) {
   Carver c(base);
   const size_t F = m.F, M = m.M, St = (size_t)K + g.E, Hm = m.S - 1, nb = cdiv((int)St, m.S), R = (size_t)B * M;
   const size_t He0 = d->enc1_hidden, He1 = d->enc2_hidden, Hb = d->bn_hidden, Hd = d->dec_hidden;
-  w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B); w.rst = c.take<int>(B);
-  w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
-  w.magT = c.take<float>(B * St * F);
-  w.spec = c.take<float>(B * ((size_t)g.Q + St) * 2 * F);
+  stream_carve(c, g, B, K, m.F, w);
+  w.rst = c.take<int>(B);
   w.melT = c.take<float>(B * St * M);
   w.fs = c.take<float2>(B * St);
   w.scale1 = c.take<float>(St * B);
@@ -304,8 +297,7 @@ static void fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const S
   w.pp = c.take<float>((size_t)2 * 256 * Hd);  // fb::ROWS rows of the persistent kernel's h0 ping-pong
   w.barrier = c.take<unsigned int>(64);
   w.y = c.take<float>(B * St * 2 * F);
-  w.crm = c.take<float>(B * ((size_t)g.Rc + St) * 2 * F);
-  w.bytes = c.off;
+  return c.off;
 }
 
 // Block ends of slot b in the call: the steps j < St whose frame m0 + j is a multiple of S and >= 0 (block m/S, shrunk
@@ -451,30 +443,22 @@ __global__ void fast_stream_dec_input_kernel(const float* __restrict__ encT, con
 extern "C" size_t fsn_fast_stream_state_bytes(const fsn_fast_desc* d, int B, int n_fft, int hop) {
   FastDims m;
   StreamGeom g;
-  if (fast_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
-  if (B <= 0) { set_error("fast_stream: B=%d slots", B); last_error_code() = FSN_ERR_SHAPE; return 0; }
-  return fast_stream_layout(d, g).slot * (size_t)B;
+  return stream_query_check(fast_stream_check(d, n_fft, hop, n_fft, m, g), "fast_stream", B, 1)
+             ? 0 : fast_stream_layout(d, g).slot() * (size_t)B;
 }
 
 extern "C" size_t fsn_fast_stream_workspace_bytes(const fsn_fast_desc* d, int B, int K_max, int n_fft, int hop) {
   FastDims m;
   StreamGeom g;
-  if (fast_stream_check(d, n_fft, hop, n_fft, m, g)) return 0;
-  if (B <= 0 || K_max <= 0) {
-    set_error("fast_stream: B=%d slots, K_max=%d hops", B, K_max);
-    last_error_code() = FSN_ERR_SHAPE;
-    return 0;
-  }
   FastStreamWs w;
-  fast_stream_carve(d, m, g, B, K_max, nullptr, w);
-  return w.bytes;
+  return stream_query_check(fast_stream_check(d, n_fft, hop, n_fft, m, g), "fast_stream", B, K_max)
+             ? 0 : fast_stream_carve(d, m, g, B, K_max, nullptr, w);
 }
 
 extern "C" int fsn_fast_stream_delay(const fsn_fast_desc* d, int n_fft, int hop) {
   FastDims m;
   StreamGeom g;
-  const int rc = fast_stream_check(d, n_fft, hop, n_fft, m, g);
-  return rc ? -rc : g.D;
+  return stream_delay(fast_stream_check(d, n_fft, hop, n_fft, m, g), g);
 }
 
 extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* wav,
@@ -484,43 +468,20 @@ extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weigh
   launch_counter() = 0;
   FastDims m;
   StreamGeom g;
-  int rc = fast_stream_check(d, n_fft, hop, win_length, m, g);
-  if (rc) return rc;
-  FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "fast_stream: B=%d slots, K=%d hops", B, K);
-  FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "fast_stream: B=%d slots, at most 65535", B);
-  FSN_REQUIRE((long long)K * hop + g.D < (1 << 30), FSN_ERR_SHAPE, "fast_stream: K=%d hops too long", K);
-  FSN_REQUIRE(wt && wav && enhanced, FSN_ERR_SHAPE, "fast_stream: null argument");
-  bool any_tail = false;
-  for (int b = 0; tail && b < B; ++b) {
-    FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * hop, FSN_ERR_SHAPE,
-                "fast_stream: tail[%d] = %d, outside [0, K*hop] = [0, %d] and not -1", b, tail[b], K * hop);
-    any_tail |= tail[b] >= 0;
-  }
+  int St, rc = fast_stream_check(d, n_fft, hop, win_length, m, g);
+  if (rc || (rc = stream_check("fast_stream", g, B, K, tail, wav, enhanced, St))) return rc;
+  FSN_REQUIRE(wt, FSN_ERR_SHAPE, "fast_stream: null weights");
   const FastStreamLayout sl = fast_stream_layout(d, g);
-  FSN_REQUIRE(state && state_bytes >= sl.slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
-              state_bytes, sl.slot * (size_t)B);
   FastStreamWs w;
-  fast_stream_carve(d, m, g, B, K, workspace, w);
-  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
-              workspace_bytes, w.bytes);
-  // laid out for K + E steps (a workspace queried for a larger K_max also fits); a call without a clip's last chunk runs
-  // St = K steps and strides its buffers by St
+  const size_t ws = fast_stream_carve(d, m, g, B, K, workspace, w);
+  if ((rc = stream_check_sizes(state, state_bytes, sl.slot(), B, workspace, workspace_bytes, ws))) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
   char* sb = (char*)state;
-  const size_t ss = sl.slot;
-  const int F = m.F, M = m.M, S = m.S, Kf = m.K, Hm = S - 1, R = B * M;
-  const int St = K + (any_tail ? g.E : 0), nb = cdiv(St, S);
+  const size_t ss = sl.slot();
+  const int F = m.F, M = m.M, S = m.S, Kf = m.K, Hm = S - 1, R = B * M, nb = cdiv(St, S);
   const int Hb = d->bn_hidden, Hd = d->dec_hidden;
-  const int Kh = K * hop, Wn = g.Hs + Kh;
-  const size_t F2 = 2 * (size_t)F, catw = (size_t)(Hm + St) * M * 4;
-  if ((rc = stream_prologue(start, tail, B, sb, ss, w.pos0, w.act0, w.tail, st))) return rc;
-  // samples: the carried history, then the chunk; spectrum: the carried Q frames, then the St frames of this call
-  if ((rc = copy_rows(w.wav, (size_t)Wn * 4, sb + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
-  if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
-  if ((rc = copy_rows(w.spec, (g.Q + St) * F2 * 4, sb + sl.spec, ss, g.Q * F2 * 4, B, st))) return rc;
-  if ((rc = stft_stream_launch(w.wav, Wn, g.Hs, w.pos0, w.tail, B, n_fft, hop, win_length, g.c, St, g.Q, w.magT, w.spec,
-                               st)))
-    return rc;
+  const size_t catw = (size_t)(Hm + St) * M * 4;
+  if ((rc = stream_open(g, sl, w, F, B, K, St, win_length, start, tail, wav, sb, nullptr, st))) return rc;
   // Mel filtering and the first norm over the mel frame sums (model.py:161-170)
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, B * St, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true))) return rc;
   if ((rc = frame_stats_launch(w.melT, B, St, M, 0, (size_t)St * M, M, w.fs, st))) return rc;
@@ -611,18 +572,10 @@ extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weigh
     return rc;
   }
   if ((rc = fc_gemm_launch(w.dhall[1], wt->dec_fc_w, wt->dec_fc_b, w.y, B * St, Hd, 2 * F, FSN_ACT_NONE, st))) return rc;
-  // cRM: the carried Rc frames, then step j's output as frame pos0/hop - c + j - la
-  if ((rc = copy_rows(w.crm, (g.Rc + St) * F2 * 4, sb + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;
-  if ((rc = copy_rows(w.crm + g.Rc * F2, (g.Rc + St) * F2 * 4, w.y, St * F2 * 4, St * F2 * 4, B, st))) return rc;
-  if ((rc = istft_stream_launch(w.spec, w.crm, w.pos0, w.act0, w.tail, B, K, g.D, n_fft, hop, win_length, g.c, g.la, g.Rc,
-                                g.Q, St, enhanced, st)))
-    return rc;
-  // carry what the next call reads: the windows as of step K
-  if ((rc = copy_rows(sb + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
-  if ((rc = copy_rows(sb + sl.spec, ss, w.spec + K * F2, (g.Q + St) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
+  // carry the last S-1 frames of the mel spectrogram and the encoder output as of step K
   if (Hm > 0) {
     if ((rc = copy_rows(sb + sl.mel, ss, w.catM + (size_t)K * M, catw, (size_t)Hm * M * 4, B, st))) return rc;
     if ((rc = copy_rows(sb + sl.enc, ss, w.catE + (size_t)K * M, catw, (size_t)Hm * M * 4, B, st))) return rc;
   }
-  return copy_rows(sb + sl.crm, ss, w.crm + K * F2, (g.Rc + St) * F2 * 4, g.Rc * F2 * 4, B, st);
+  return stream_close(g, sl, w, F, B, K, St, win_length, w.y, enhanced, sb, st);
 }

@@ -154,22 +154,17 @@ extern "C" int fsn_fullband_enhance(const fsn_fullband_desc* d, const fsn_lstm_l
   return wav_epilogue(e, enhanced, B, L_max, pcm, gain, crm_out, d->num_freqs, T, hop, st);
 }
 
-// ---- chunked streaming (DESIGN 4.14).  Slot state block, floats: meta (4), sample history Hs, spectrum Q x 2F, cRM
-// Rc x 2F, then h and c of every layer (num_layers x H each); each section starts on 16 bytes, blocks 256 bytes apart.
+// ---- chunked streaming (DESIGN 4.14).  Slot state block: the stream header (StreamSlot), then h and c of every layer
+// (num_layers x H floats each).
 namespace fsn {
 
-struct FbbStreamLayout { size_t hist, spec, crm, h, c, slot; };
+struct FbbStreamLayout : StreamSlot { size_t h, c; };
 
 static FbbStreamLayout fbb_stream_layout(const fsn_fullband_desc* d, const StreamGeom& g) {
-  const size_t F2 = 2 * (size_t)d->num_freqs, nH = (size_t)d->num_layers * d->hidden;
-  FbbStreamLayout s;
-  size_t o = sizeof(StreamMeta);
-  s.hist = o; o = align_up(o + (size_t)g.Hs * 4, 16);
-  s.spec = o; o = align_up(o + (size_t)g.Q * F2 * 4, 16);
-  s.crm = o;  o = align_up(o + (size_t)g.Rc * F2 * 4, 16);
-  s.h = o;    o = align_up(o + nH * 4, 16);
-  s.c = o;    o = align_up(o + nH * 4, 16);
-  s.slot = align_up(o, 256);
+  const size_t nH = (size_t)d->num_layers * d->hidden;
+  FbbStreamLayout s{StreamSlot(g, d->num_freqs)};
+  s.h = s.sec(nH);
+  s.c = s.sec(nH);
   return s;
 }
 
@@ -184,57 +179,43 @@ static int fbb_stream_check(const fsn_fullband_desc* d, int n_fft, int hop, int 
   return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
 }
 
-struct FbbStreamWs {
-  int *pos0, *act0, *tail;
-  float *wav, *magT, *spec, *scale, *y, *crm;
+struct FbbStreamWs : StreamWs {
+  float *scale, *y;
   float2* fs;
   float *h[SEQ_MAX_LAYERS], *c[SEQ_MAX_LAYERS], *hall[2];
-  size_t bytes;
 };
 
-// S = K + E steps: a call with a clip's last chunk runs E steps past the K of the others
-static void fbb_stream_carve(const fsn_fullband_desc* d, const StreamGeom& g, int B, int K, void* base, FbbStreamWs& w) {
+// St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others; returns the bytes
+static size_t fbb_stream_carve(const fsn_fullband_desc* d, const StreamGeom& g, int B, int K, void* base, FbbStreamWs& w) {
   Carver c(base);
-  const size_t F = d->num_freqs, H = d->hidden, S = (size_t)K + g.E;
-  w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B);
-  w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
-  w.magT = c.take<float>(B * S * F);
-  w.spec = c.take<float>(B * ((size_t)g.Q + S) * 2 * F);
-  w.fs = c.take<float2>(B * S);
-  w.scale = c.take<float>(S * B);
+  const size_t H = d->hidden, St = (size_t)K + g.E;
+  stream_carve(c, g, B, K, d->num_freqs, w);
+  w.fs = c.take<float2>(B * St);
+  w.scale = c.take<float>(St * B);
   for (int l = 0; l < d->num_layers; ++l) { w.h[l] = c.take<float>(B * H); w.c[l] = c.take<float>(B * H); }
-  w.hall[0] = c.take<float>(B * S * H); w.hall[1] = c.take<float>(B * S * H);
-  w.y = c.take<float>(B * S * 2 * F);
-  w.crm = c.take<float>(B * ((size_t)g.Rc + S) * 2 * F);
-  w.bytes = c.off;
+  w.hall[0] = c.take<float>(B * St * H); w.hall[1] = c.take<float>(B * St * H);
+  w.y = c.take<float>(B * St * 2 * d->num_freqs);
+  return c.off;
 }
 
 }  // namespace fsn
 
 extern "C" size_t fsn_fullband_stream_state_bytes(const fsn_fullband_desc* d, int B, int n_fft, int hop) {
   StreamGeom g;
-  if (fbb_stream_check(d, n_fft, hop, n_fft, g)) return 0;
-  if (B <= 0) { set_error("fullband_stream: B=%d slots", B); last_error_code() = FSN_ERR_SHAPE; return 0; }
-  return fbb_stream_layout(d, g).slot * (size_t)B;
+  return stream_query_check(fbb_stream_check(d, n_fft, hop, n_fft, g), "fullband_stream", B, 1)
+             ? 0 : fbb_stream_layout(d, g).slot() * (size_t)B;
 }
 
 extern "C" size_t fsn_fullband_stream_workspace_bytes(const fsn_fullband_desc* d, int B, int K_max, int n_fft, int hop) {
   StreamGeom g;
-  if (fbb_stream_check(d, n_fft, hop, n_fft, g)) return 0;
-  if (B <= 0 || K_max <= 0) {
-    set_error("fullband_stream: B=%d slots, K_max=%d hops", B, K_max);
-    last_error_code() = FSN_ERR_SHAPE;
-    return 0;
-  }
   FbbStreamWs w;
-  fbb_stream_carve(d, g, B, K_max, nullptr, w);
-  return w.bytes;
+  return stream_query_check(fbb_stream_check(d, n_fft, hop, n_fft, g), "fullband_stream", B, K_max)
+             ? 0 : fbb_stream_carve(d, g, B, K_max, nullptr, w);
 }
 
 extern "C" int fsn_fullband_stream_delay(const fsn_fullband_desc* d, int n_fft, int hop) {
   StreamGeom g;
-  const int rc = fbb_stream_check(d, n_fft, hop, n_fft, g);
-  return rc ? -rc : g.D;
+  return stream_delay(fbb_stream_check(d, n_fft, hop, n_fft, g), g);
 }
 
 extern "C" int fsn_fullband_stream_step(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, const float* fc_w,
@@ -243,60 +224,27 @@ extern "C" int fsn_fullband_stream_step(const fsn_fullband_desc* d, const fsn_ls
                                         size_t state_bytes, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
   launch_counter() = 0;
   StreamGeom g;
-  int rc = fbb_stream_check(d, n_fft, hop, win_length, g);
-  if (rc) return rc;
-  FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "fullband_stream: B=%d slots, K=%d hops", B, K);
-  FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "fullband_stream: B=%d slots, at most 65535", B);
-  FSN_REQUIRE((long long)K * hop + g.D < (1 << 30), FSN_ERR_SHAPE, "fullband_stream: K=%d hops too long", K);
-  FSN_REQUIRE(layers && fc_w && fc_b && wav && enhanced, FSN_ERR_SHAPE, "fullband_stream: null argument");
-  bool any_tail = false;
-  for (int b = 0; tail && b < B; ++b) {
-    FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * hop, FSN_ERR_SHAPE,
-                "fullband_stream: tail[%d] = %d, outside [0, K*hop] = [0, %d] and not -1", b, tail[b], K * hop);
-    any_tail |= tail[b] >= 0;
-  }
+  int St, rc = fbb_stream_check(d, n_fft, hop, win_length, g);
+  if (rc || (rc = stream_check("fullband_stream", g, B, K, tail, wav, enhanced, St))) return rc;
+  FSN_REQUIRE(layers && fc_w && fc_b, FSN_ERR_SHAPE, "fullband_stream: null weights");
   const FbbStreamLayout sl = fbb_stream_layout(d, g);
-  FSN_REQUIRE(state && state_bytes >= sl.slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
-              state_bytes, sl.slot * (size_t)B);
   FbbStreamWs w;
-  fbb_stream_carve(d, g, B, K, workspace, w);
-  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
-              workspace_bytes, w.bytes);
-  // laid out for K + E steps from the workspace's start (a workspace queried for a larger K_max also fits); a call
-  // without a clip's last chunk runs S = K steps and strides its buffers by S
+  const size_t ws = fbb_stream_carve(d, g, B, K, workspace, w);
+  if ((rc = stream_check_sizes(state, state_bytes, sl.slot(), B, workspace, workspace_bytes, ws))) return rc;
   const cudaStream_t st = (cudaStream_t)stream;
   char* sb = (char*)state;
-  const size_t ss = sl.slot;
-  const int F = d->num_freqs, H = d->hidden, n = d->num_layers, S = K + (any_tail ? g.E : 0);
-  const int Kh = K * hop, Wn = g.Hs + Kh;
-  const size_t F2 = 2 * (size_t)F;
-  if ((rc = stream_prologue(start, tail, B, sb, ss, w.pos0, w.act0, w.tail, st))) return rc;
-  // samples: the carried history, then the chunk
-  if ((rc = copy_rows(w.wav, (size_t)Wn * 4, sb + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
-  if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
-  // spectrum: the carried Q frames, then the S frames of this call
-  if ((rc = copy_rows(w.spec, (g.Q + S) * F2 * 4, sb + sl.spec, ss, g.Q * F2 * 4, B, st))) return rc;
-  if ((rc = stft_stream_launch(w.wav, Wn, g.Hs, w.pos0, w.tail, B, n_fft, hop, win_length, g.c, S, g.Q, w.magT, w.spec,
-                               st)))
-    return rc;
+  const size_t ss = sl.slot();
+  const int F = d->num_freqs, H = d->hidden, n = d->num_layers;
+  if ((rc = stream_open(g, sl, w, F, B, K, St, win_length, start, tail, wav, sb, nullptr, st))) return rc;
   // first norm (fbb_core): frame sums, then the running scale of each step
-  if ((rc = frame_stats_launch(w.magT, B, S, F, 0, (size_t)S * F, F, w.fs, st))) return rc;
-  if ((rc = stream_norm_launch(w.fs, B, S, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale, st))) return rc;
+  if ((rc = frame_stats_launch(w.magT, B, St, F, 0, (size_t)St * F, F, w.fs, st))) return rc;
+  if ((rc = stream_norm_launch(w.fs, B, St, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale, st))) return rc;
   // the stack on the per-step kernels seq_stack_forward runs for the causal norms, (h, c) carried in the slot state
   int Hs[SEQ_MAX_LAYERS];
   for (int l = 0; l < n; ++l) Hs[l] = H;
-  if ((rc = stream_lstm_layers(layers, n, Hs, F, w.magT, w.scale, B, S, K, g, w.pos0, sb, ss, sl.h, sl.c, w.h, w.c, w.hall,
-                               st)))
+  if ((rc = stream_lstm_layers(layers, n, Hs, F, w.magT, w.scale, B, St, K, g, w.pos0, sb, ss, sl.h, sl.c, w.h, w.c,
+                               w.hall, st)))
     return rc;
-  if ((rc = fc_gemm_launch(w.hall[(n - 1) & 1], fc_w, fc_b, w.y, B * S, H, 2 * F, d->activation, st))) return rc;
-  // cRM: the carried Rc frames, then step j's output as frame pos0/hop - c + j - la
-  if ((rc = copy_rows(w.crm, (g.Rc + S) * F2 * 4, sb + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;
-  if ((rc = copy_rows(w.crm + g.Rc * F2, (g.Rc + S) * F2 * 4, w.y, S * F2 * 4, S * F2 * 4, B, st))) return rc;
-  if ((rc = istft_stream_launch(w.spec, w.crm, w.pos0, w.act0, w.tail, B, K, g.D, n_fft, hop, win_length, g.c, g.la, g.Rc,
-                                g.Q, S, enhanced, st)))
-    return rc;
-  // carry what the next call reads: the windows as of step K
-  if ((rc = copy_rows(sb + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
-  if ((rc = copy_rows(sb + sl.spec, ss, w.spec + K * F2, (g.Q + S) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
-  return copy_rows(sb + sl.crm, ss, w.crm + K * F2, (g.Rc + S) * F2 * 4, g.Rc * F2 * 4, B, st);
+  if ((rc = fc_gemm_launch(w.hall[(n - 1) & 1], fc_w, fc_b, w.y, B * St, H, 2 * F, d->activation, st))) return rc;
+  return stream_close(g, sl, w, F, B, K, St, win_length, w.y, enhanced, sb, st);
 }

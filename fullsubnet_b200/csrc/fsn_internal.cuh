@@ -570,6 +570,45 @@ int stream_lstm_layers(const fsn_lstm_layer* L, int n, const int* H, int K0, con
 // rows of `width` bytes: dst row b (pitch dp) <- src row b (pitch sp), B rows, on the stream
 int copy_rows(void* dst, size_t dp, const void* src, size_t sp, size_t width, int B, cudaStream_t st);
 
+// ---- the host skeleton of every model's streaming step.  Each step reads its descriptor / geometry check ->
+// stream_check -> its own argument checks -> layout -> carve -> stream_check_sizes -> stream_open -> its own norms and
+// stacks -> stream_close; its size queries are stream_query_check, then the layout or the carve.
+// Slot state block: the meta, the sample history Hs, the spectrum Q x 2F and the cRM Rc x 2F, then the model's sections
+// appended with sec; every section starts on 16 bytes and slot() closes the block on 256
+struct StreamSlot {
+  size_t hist, spec, crm, end;
+  StreamSlot(const StreamGeom& g, int F);
+  size_t sec(size_t floats) { const size_t at = end; end = align_up(end + floats * 4, 16); return at; }
+  size_t slot() const { return align_up(end, 256); }
+};
+// the workspace every step starts with, laid out for K + E steps: stream_prologue's device tables, the samples
+// [B, Hs + K hop], the magnitude [B, St, F], the spectrum [B, Q + St, 2F] and the cRM [B, Rc + St, 2F]
+struct StreamWs {
+  int *pos0, *act0, *tail;
+  float *wav, *magT, *spec, *crm;
+};
+void stream_carve(Carver& c, const StreamGeom& g, int B, int K, int F, StreamWs& w);
+// the state / workspace queries after the model's check rc: refuse B <= 0 or K_max <= 0 (FSN_ERR_SHAPE)
+int stream_query_check(int rc, const char* who, int B, int K_max);
+inline int stream_delay(int rc, const StreamGeom& g) { return rc ? -rc : g.D; }
+// host checks of a call before any CUDA call and before its layout and carve: B, K > 0 (FSN_ERR_SHAPE), B <= 65535
+// (FSN_ERR_UNSUPPORTED; the DSP kernels put the slot in gridDim.y), K hop + D < 2^30, non-null chunk and output, tail
+// (host [B], nullable) -1 or in [0, K hop] (FSN_ERR_SHAPE).  St: the call's steps, K + E when a slot's clip ends in it,
+// else K.  `who` prefixes the messages
+int stream_check(const char* who, const StreamGeom& g, int B, int K, const int32_t* tail, const float* wav,
+                 const float* enhanced, int& St);
+// after the layout and carve: B blocks of `slot` bytes of state, then ws_need bytes of workspace (FSN_ERR_WORKSPACE)
+int stream_check_sizes(const void* state, size_t state_bytes, size_t slot, int B, const void* workspace,
+                       size_t workspace_bytes, size_t ws_need);
+// signal front end: stream_prologue (with restart non-null, stream_restart_launch into it), the carried history and the
+// chunk wav [B, K hop] into w.wav, the carried spectrum into w.spec, the STFT of the St steps into w.magT and w.spec
+int stream_open(const StreamGeom& g, const StreamSlot& sl, const StreamWs& w, int F, int B, int K, int St, int win_length,
+                const int32_t* start, const int32_t* tail, const float* wav, char* state, int* restart, cudaStream_t st);
+// signal back end: the carried cRM into w.crm, then the model's output y [B, St, 2F] behind it (nullable: the model
+// wrote w.crm itself), the iSTFT into enhanced and the carry of history, spectrum and cRM as of step K
+int stream_close(const StreamGeom& g, const StreamSlot& sl, const StreamWs& w, int F, int B, int K, int St, int win_length,
+                 const float* y, float* enhanced, char* state, cudaStream_t st);
+
 // tensor-core sub-band stack (fsn_subband_tc.cu)
 struct SbTcArgs {
   const void* packed;       // tile-ordered fp16 weights (fsn_pack_sb_weights / sb_tc_pack_raw)

@@ -335,31 +335,26 @@ extern "C" int fsn_enhance(const fsn_model_desc* d, const fsn_seq_weights* fb, c
   return rc;
 }
 
-// ---- chunked streaming (DESIGN 4.14).  Slot state block (each section on 16 bytes, blocks 256 bytes apart): meta (16
-// bytes), sample history Hs, spectrum Q x 2F, cRM Rc x 2F (the sections of fullband_baseline's stream), the second norm's
+// ---- chunked streaming (DESIGN 4.14).  Slot state block: the stream header (StreamSlot), then the second norm's
 // accumulator (cumulative: the running sum of each of the F sub-band units, forgetting: mu), full-band (h | c) of both
 // layers (2 x fb_hidden each), sub-band (h | c) of both layers for every frequency (2 x F x sb_hidden each).
 namespace fsn {
 
-struct FsnStreamLayout { size_t hist, spec, crm, norm2, fbh, fbc, sbh, sbc, slot; };
+struct FsnStreamLayout : StreamSlot { size_t norm2, fbh, fbc, sbh, sbc; };
 
 static FsnStreamLayout fsn_stream_layout(const fsn_model_desc* d, const StreamGeom& g) {
-  const size_t F = d->num_freqs, F2 = 2 * F, Hf = 2 * (size_t)d->fb_hidden, Hs = 2 * F * d->sb_hidden;
-  FsnStreamLayout s;
-  size_t o = sizeof(StreamMeta);
-  auto sec = [&](size_t& at, size_t floats) { at = o; o = align_up(o + floats * 4, 16); };
-  sec(s.hist, g.Hs); sec(s.spec, g.Q * F2); sec(s.crm, g.Rc * F2);
-  sec(s.norm2, d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE ? F : 1);
-  sec(s.fbh, Hf); sec(s.fbc, Hf);
-  sec(s.sbh, Hs); sec(s.sbc, Hs);
-  s.slot = align_up(o, 256);
+  const size_t F = d->num_freqs, Hf = 2 * (size_t)d->fb_hidden, Hs = 2 * F * d->sb_hidden;
+  FsnStreamLayout s{StreamSlot(g, d->num_freqs)};
+  s.norm2 = s.sec(d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE ? F : 1);
+  s.fbh = s.sec(Hf); s.fbc = s.sec(Hf);
+  s.sbh = s.sec(Hs); s.sbc = s.sec(Hs);
   return s;
 }
 
 // every slot is one clip of the B = 1 whole-clip call, so drop_band never applies, whatever num_groups_in_drop_band says.
 // tc: the tensor-core stream (fsn_stream_tc_*), which takes FSN_PREC_F16X3_TC / FSN_PREC_F16_TC instead of FSN_PREC_FP32
 static int fsn_stream_check(const fsn_model_desc* d, int n_fft, int hop, int win_length, Dims& m, StreamGeom& g,
-                            bool tc = false) {
+                            bool tc) {
   FSN_REQUIRE(d, FSN_ERR_SHAPE, "stream: null descriptor");
   fsn_model_desc dd = *d;
   dd.num_groups_in_drop_band = 1;
@@ -384,14 +379,13 @@ static int fsn_stream_check(const fsn_model_desc* d, int n_fft, int hop, int win
   return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
 }
 
-struct FsnStreamWs {
-  int *pos0, *act0, *tail, *restart;
-  float *wav, *magT, *spec, *scale1, *fbT, *scale2, *unit, *crm;
+struct FsnStreamWs : StreamWs {
+  int* restart;
+  float *scale1, *fbT, *scale2, *unit;
   float2 *fs, *fs2;
   float *fh[2], *fc[2], *fhall[2];       // full-band state and layer outputs
   float *sh0[2], *sh1[2], *sc0, *sc1;    // sub-band state, h ping-pong per layer (fp32 stream)
   LstmTcWs ftc;                          // tensor-core full band (tensor-core stream on SEQ_PATH_TC)
-  size_t bytes;
 };
 
 // the full-band stack of a call over B slots and St steps, as the whole-clip call builds it (fb_stack)
@@ -403,16 +397,14 @@ static SeqStack fsn_stream_fb(const fsn_model_desc* d, int B, int St) {
 }
 
 // St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others.  tc: the sub band's state
-// stays in the slot state (no per-row buffers), the full band gets the tensor-core workspace when it runs there
-static void fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B, int K, void* base, FsnStreamWs& w,
-                             bool tc = false) {
+// stays in the slot state (no per-row buffers), the full band gets the tensor-core workspace when it runs there.
+// Returns the bytes
+static size_t fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B, int K, void* base, FsnStreamWs& w,
+                               bool tc) {
   Carver c(base);
   const size_t F = d->num_freqs, Hf = d->fb_hidden, St = (size_t)K + g.E, RH = (size_t)B * F * d->sb_hidden;
-  w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B);
+  stream_carve(c, g, B, K, d->num_freqs, w);
   w.restart = tc ? c.take<int>(B) : nullptr;
-  w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
-  w.magT = c.take<float>(B * St * F);
-  w.spec = c.take<float>(B * ((size_t)g.Q + St) * 2 * F);
   w.fs = c.take<float2>(B * St);
   w.fs2 = d->norm_type == FSN_NORM_FORGETTING ? c.take<float2>(B * St) : nullptr;
   w.scale1 = c.take<float>(St * B);
@@ -433,41 +425,7 @@ static void fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B
     const int Hw = (int)Hf > cdiv((int)F, 4) ? (int)Hf : cdiv((int)F, 4);  // the Linear's prepared weights share the rows
     lstm_tc_carve(c, (size_t)B * St, (int)(F > Hf ? F : Hf), Hw, d->precision == FSN_PREC_F16X3_TC, w.ftc);
   }
-  w.crm = c.take<float>(B * ((size_t)g.Rc + St) * 2 * F);
-  w.bytes = c.off;
-}
-
-}  // namespace fsn
-
-namespace fsn {
-
-static size_t fsn_stream_state_query(const fsn_model_desc* d, int B, int n_fft, int hop, bool tc) {
-  Dims m;
-  StreamGeom g;
-  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g, tc)) return 0;
-  if (B <= 0) { set_error("stream: B=%d slots", B); last_error_code() = FSN_ERR_SHAPE; return 0; }
-  return fsn_stream_layout(d, g).slot * (size_t)B;
-}
-
-static size_t fsn_stream_workspace_query(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop, bool tc) {
-  Dims m;
-  StreamGeom g;
-  if (fsn_stream_check(d, n_fft, hop, n_fft, m, g, tc)) return 0;
-  if (B <= 0 || K_max <= 0) {
-    set_error("stream: B=%d slots, K_max=%d hops", B, K_max);
-    last_error_code() = FSN_ERR_SHAPE;
-    return 0;
-  }
-  FsnStreamWs w;
-  fsn_stream_carve(d, g, B, K_max, nullptr, w, tc);
-  return w.bytes;
-}
-
-static int fsn_stream_delay_query(const fsn_model_desc* d, int n_fft, int hop, bool tc) {
-  Dims m;
-  StreamGeom g;
-  const int rc = fsn_stream_check(d, n_fft, hop, n_fft, m, g, tc);
-  return rc ? -rc : g.D;
+  return c.off;
 }
 
 // one call of either stream.  tc: the full band on the tensor cores where the whole-clip call runs it there
@@ -480,46 +438,24 @@ static int fsn_stream_run(const fsn_model_desc* d, const fsn_seq_weights* fb, co
   launch_counter() = 0;
   Dims m;
   StreamGeom g;
-  int rc = fsn_stream_check(d, n_fft, hop, win_length, m, g, tc);
-  if (rc) return rc;
-  FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "stream: B=%d slots, K=%d hops", B, K);
-  FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "stream: B=%d slots, at most 65535", B);
+  int St, rc = fsn_stream_check(d, n_fft, hop, win_length, m, g, tc);
+  if (rc || (rc = stream_check("stream", g, B, K, tail, wav, enhanced, St))) return rc;
   // the sub-band rows' (h, c) of all slots, one int-indexed element per thread in stream_reset_kernel
   FSN_REQUIRE((size_t)B * m.F * d->sb_hidden <= 0x7fffffff, FSN_ERR_SHAPE,
               "stream: B=%d slots x %d frequencies x sb_hidden %d must stay below 2^31", B, m.F, d->sb_hidden);
-  FSN_REQUIRE((long long)K * hop + g.D < (1 << 30), FSN_ERR_SHAPE, "stream: K=%d hops too long", K);
-  FSN_REQUIRE(fb && sb && wav && enhanced, FSN_ERR_SHAPE, "stream: null argument");
+  FSN_REQUIRE(fb && sb, FSN_ERR_SHAPE, "stream: null weights");
   FSN_REQUIRE(!tc || sb_packed, FSN_ERR_SHAPE, "stream_tc: the tensor-core stream needs packed sub-band weights");
-  bool any_tail = false;
-  for (int b = 0; tail && b < B; ++b) {
-    FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * hop, FSN_ERR_SHAPE,
-                "stream: tail[%d] = %d, outside [0, K*hop] = [0, %d] and not -1", b, tail[b], K * hop);
-    any_tail |= tail[b] >= 0;
-  }
   const FsnStreamLayout sl = fsn_stream_layout(d, g);
-  FSN_REQUIRE(state && state_bytes >= sl.slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
-              state_bytes, sl.slot * (size_t)B);
   FsnStreamWs w;
-  fsn_stream_carve(d, g, B, K, workspace, w, tc);
-  FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
-              workspace_bytes, w.bytes);
-  // laid out for K + E steps from the workspace's start (a workspace queried for a larger K_max also fits); a call
-  // without a clip's last chunk runs St = K steps and strides its buffers by St
+  const size_t ws = fsn_stream_carve(d, g, B, K, workspace, w, tc);
+  if ((rc = stream_check_sizes(state, state_bytes, sl.slot(), B, workspace, workspace_bytes, ws))) return rc;
   char* sbase = (char*)state;
-  const size_t ss = sl.slot;
+  const size_t ss = sl.slot();
   const int F = m.F, Hf = d->fb_hidden, Hs = d->sb_hidden, Ns = d->sb_num_neighbors, Nf = d->fb_num_neighbors;
-  const int St = K + (any_tail ? g.E : 0), R = B * F, Kh = K * hop, Wn = g.Hs + Kh;
+  const int R = B * F;
   const bool fgt = d->norm_type == FSN_NORM_FORGETTING, x3 = d->precision == FSN_PREC_F16X3_TC;
   const size_t F2 = 2 * (size_t)F;
-  if ((rc = stream_prologue(start, tail, B, sbase, ss, w.pos0, w.act0, w.tail, st))) return rc;
-  if (tc && (rc = stream_restart_launch(w.pos0, B, g, w.restart, st))) return rc;
-  // samples: the carried history, then the chunk; spectrum: the carried Q frames, then the St frames of this call
-  if ((rc = copy_rows(w.wav, (size_t)Wn * 4, sbase + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
-  if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
-  if ((rc = copy_rows(w.spec, (g.Q + St) * F2 * 4, sbase + sl.spec, ss, g.Q * F2 * 4, B, st))) return rc;
-  if ((rc = stft_stream_launch(w.wav, Wn, g.Hs, w.pos0, w.tail, B, n_fft, hop, win_length, g.c, St, g.Q, w.magT, w.spec,
-                               st)))
-    return rc;
+  if ((rc = stream_open(g, sl, w, F, B, K, St, win_length, start, tail, wav, sbase, w.restart, st))) return rc;
   // first norm (model_core): frame sums (.y reflect-weighted with Ns, for the second forgetting norm), running scale
   if ((rc = frame_stats_launch(w.magT, B, St, F, Ns, (size_t)St * F, F, w.fs, st))) return rc;
   if ((rc = stream_norm_launch(w.fs, B, St, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sbase, ss, w.scale1, st)))
@@ -604,28 +540,31 @@ static int fsn_stream_run(const fsn_model_desc* d, const fsn_seq_weights* fb, co
       }
     }
   }
-  // cRM: the carried Rc frames before the call's; iSTFT
-  if ((rc = copy_rows(w.crm, (g.Rc + St) * F2 * 4, sbase + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;
-  if ((rc = istft_stream_launch(w.spec, w.crm, w.pos0, w.act0, w.tail, B, K, g.D, n_fft, hop, win_length, g.c, g.la, g.Rc,
-                                g.Q, St, enhanced, st)))
-    return rc;
-  // carry what the next call reads: the windows as of step K
-  if ((rc = copy_rows(sbase + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
-  if ((rc = copy_rows(sbase + sl.spec, ss, w.spec + K * F2, (g.Q + St) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
-  return copy_rows(sbase + sl.crm, ss, w.crm + K * F2, (g.Rc + St) * F2 * 4, g.Rc * F2 * 4, B, st);
+  return stream_close(g, sl, w, F, B, K, St, win_length, nullptr, enhanced, sbase, st);
 }
 
 }  // namespace fsn
 
 extern "C" size_t fsn_stream_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop) {
-  return fsn_stream_state_query(d, B, n_fft, hop, false);
+  Dims m;
+  StreamGeom g;
+  return stream_query_check(fsn_stream_check(d, n_fft, hop, n_fft, m, g, false), "stream", B, 1)
+             ? 0 : fsn_stream_layout(d, g).slot() * (size_t)B;
 }
 
 extern "C" size_t fsn_stream_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop) {
-  return fsn_stream_workspace_query(d, B, K_max, n_fft, hop, false);
+  Dims m;
+  StreamGeom g;
+  FsnStreamWs w;
+  return stream_query_check(fsn_stream_check(d, n_fft, hop, n_fft, m, g, false), "stream", B, K_max)
+             ? 0 : fsn_stream_carve(d, g, B, K_max, nullptr, w, false);
 }
 
-extern "C" int fsn_stream_delay(const fsn_model_desc* d, int n_fft, int hop) { return fsn_stream_delay_query(d, n_fft, hop, false); }
+extern "C" int fsn_stream_delay(const fsn_model_desc* d, int n_fft, int hop) {
+  Dims m;
+  StreamGeom g;
+  return stream_delay(fsn_stream_check(d, n_fft, hop, n_fft, m, g, false), g);
+}
 
 extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
                                const float* wav, const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
@@ -636,15 +575,24 @@ extern "C" int fsn_stream_step(const fsn_model_desc* d, const fsn_seq_weights* f
 }
 
 extern "C" size_t fsn_stream_tc_state_bytes(const fsn_model_desc* d, int B, int n_fft, int hop) {
-  return fsn_stream_state_query(d, B, n_fft, hop, true);
+  Dims m;
+  StreamGeom g;
+  return stream_query_check(fsn_stream_check(d, n_fft, hop, n_fft, m, g, true), "stream", B, 1)
+             ? 0 : fsn_stream_layout(d, g).slot() * (size_t)B;
 }
 
 extern "C" size_t fsn_stream_tc_workspace_bytes(const fsn_model_desc* d, int B, int K_max, int n_fft, int hop) {
-  return fsn_stream_workspace_query(d, B, K_max, n_fft, hop, true);
+  Dims m;
+  StreamGeom g;
+  FsnStreamWs w;
+  return stream_query_check(fsn_stream_check(d, n_fft, hop, n_fft, m, g, true), "stream", B, K_max)
+             ? 0 : fsn_stream_carve(d, g, B, K_max, nullptr, w, true);
 }
 
 extern "C" int fsn_stream_tc_delay(const fsn_model_desc* d, int n_fft, int hop) {
-  return fsn_stream_delay_query(d, n_fft, hop, true);
+  Dims m;
+  StreamGeom g;
+  return stream_delay(fsn_stream_check(d, n_fft, hop, n_fft, m, g, true), g);
 }
 
 extern "C" int fsn_stream_tc_step(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,

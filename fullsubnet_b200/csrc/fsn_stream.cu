@@ -1,11 +1,91 @@
 // Chunked streaming (DESIGN 4.14): the per-slot bookkeeping, the causal first norm with a carried accumulator and the
-// recurrent-state reset of a clip's first frame.  The signal layer's streaming kernels are in fsn_dsp.cu; the model
-// orchestration and the entry points beside each model's enhance call.
+// recurrent-state reset of a clip's first frame, and the host skeleton every model's step is built from (the call
+// checks, the slot-state header, the workspace head and the signal front and back end).  The signal layer's streaming
+// kernels are in fsn_dsp.cu; each model's sections, the middle of its step and its entry points beside its enhance call.
 #include <string.h>
 
 #include "fsn_internal.cuh"
 
 namespace fsn {
+
+StreamSlot::StreamSlot(const StreamGeom& g, int F) : end(sizeof(StreamMeta)) {
+  hist = sec(g.Hs);
+  spec = sec((size_t)g.Q * 2 * F);
+  crm = sec((size_t)g.Rc * 2 * F);
+}
+
+void stream_carve(Carver& c, const StreamGeom& g, int B, int K, int F, StreamWs& w) {
+  const size_t St = (size_t)K + g.E;
+  w.pos0 = c.take<int>(B); w.act0 = c.take<int>(B); w.tail = c.take<int>(B);
+  w.wav = c.take<float>(B * ((size_t)g.Hs + (size_t)K * g.hop));
+  w.magT = c.take<float>(B * St * F);
+  w.spec = c.take<float>(B * ((size_t)g.Q + St) * 2 * F);
+  w.crm = c.take<float>(B * ((size_t)g.Rc + St) * 2 * F);
+}
+
+int stream_query_check(int rc, const char* who, int B, int K_max) {
+  if (rc) return rc;
+  FSN_REQUIRE(B > 0 && K_max > 0, FSN_ERR_SHAPE, "%s: B=%d slots, K_max=%d hops", who, B, K_max);
+  return FSN_OK;
+}
+
+int stream_check(const char* who, const StreamGeom& g, int B, int K, const int32_t* tail, const float* wav,
+                 const float* enhanced, int& St) {
+  FSN_REQUIRE(B > 0 && K > 0, FSN_ERR_SHAPE, "%s: B=%d slots, K=%d hops", who, B, K);
+  FSN_REQUIRE(B <= 65535, FSN_ERR_UNSUPPORTED, "%s: B=%d slots, at most 65535", who, B);
+  FSN_REQUIRE((long long)K * g.hop + g.D < (1 << 30), FSN_ERR_SHAPE, "%s: K=%d hops too long", who, K);
+  FSN_REQUIRE(wav && enhanced, FSN_ERR_SHAPE, "%s: null chunk or output", who);
+  bool any_tail = false;
+  for (int b = 0; tail && b < B; ++b) {
+    FSN_REQUIRE(tail[b] >= -1 && tail[b] <= K * g.hop, FSN_ERR_SHAPE,
+                "%s: tail[%d] = %d, outside [0, K*hop] = [0, %d] and not -1", who, b, tail[b], K * g.hop);
+    any_tail |= tail[b] >= 0;
+  }
+  St = K + (any_tail ? g.E : 0);
+  return FSN_OK;
+}
+
+int stream_check_sizes(const void* state, size_t state_bytes, size_t slot, int B, const void* workspace,
+                       size_t workspace_bytes, size_t ws_need) {
+  FSN_REQUIRE(state && state_bytes >= slot * (size_t)B, FSN_ERR_WORKSPACE, "stream state too small: %zu < %zu",
+              state_bytes, slot * (size_t)B);
+  FSN_REQUIRE(workspace && workspace_bytes >= ws_need, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
+              workspace_bytes, ws_need);
+  return FSN_OK;
+}
+
+// buffers laid out for K + E steps from the workspace's start (a workspace queried for a larger K_max also fits); a
+// call without a clip's last chunk runs St = K steps and strides its buffers by St
+int stream_open(const StreamGeom& g, const StreamSlot& sl, const StreamWs& w, int F, int B, int K, int St, int win_length,
+                const int32_t* start, const int32_t* tail, const float* wav, char* state, int* restart, cudaStream_t st) {
+  int rc;
+  const size_t ss = sl.slot(), F2 = 2 * (size_t)F;
+  const int Kh = K * g.hop, Wn = g.Hs + Kh;
+  if ((rc = stream_prologue(start, tail, B, state, ss, w.pos0, w.act0, w.tail, st))) return rc;
+  if (restart && (rc = stream_restart_launch(w.pos0, B, g, restart, st))) return rc;
+  // samples: the carried history, then the chunk; spectrum: the carried Q frames, then the St frames of this call
+  if ((rc = copy_rows(w.wav, (size_t)Wn * 4, state + sl.hist, ss, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.wav + g.Hs, (size_t)Wn * 4, wav, (size_t)Kh * 4, (size_t)Kh * 4, B, st))) return rc;
+  if ((rc = copy_rows(w.spec, (g.Q + St) * F2 * 4, state + sl.spec, ss, g.Q * F2 * 4, B, st))) return rc;
+  return stft_stream_launch(w.wav, Wn, g.Hs, w.pos0, w.tail, B, g.n, g.hop, win_length, g.c, St, g.Q, w.magT, w.spec, st);
+}
+
+int stream_close(const StreamGeom& g, const StreamSlot& sl, const StreamWs& w, int F, int B, int K, int St, int win_length,
+                 const float* y, float* enhanced, char* state, cudaStream_t st) {
+  int rc;
+  const size_t ss = sl.slot(), F2 = 2 * (size_t)F;
+  const int Kh = K * g.hop, Wn = g.Hs + Kh;
+  // cRM: the carried Rc frames, then step j's output as frame pos0/hop - c + j - la
+  if ((rc = copy_rows(w.crm, (g.Rc + St) * F2 * 4, state + sl.crm, ss, g.Rc * F2 * 4, B, st))) return rc;
+  if (y && (rc = copy_rows(w.crm + g.Rc * F2, (g.Rc + St) * F2 * 4, y, St * F2 * 4, St * F2 * 4, B, st))) return rc;
+  if ((rc = istft_stream_launch(w.spec, w.crm, w.pos0, w.act0, w.tail, B, K, g.D, g.n, g.hop, win_length, g.c, g.la, g.Rc,
+                                g.Q, St, enhanced, st)))
+    return rc;
+  // carry what the next call reads: the windows as of step K
+  if ((rc = copy_rows(state + sl.hist, ss, w.wav + Kh, (size_t)Wn * 4, (size_t)g.Hs * 4, B, st))) return rc;
+  if ((rc = copy_rows(state + sl.spec, ss, w.spec + K * F2, (g.Q + St) * F2 * 4, g.Q * F2 * 4, B, st))) return rc;
+  return copy_rows(state + sl.crm, ss, w.crm + K * F2, (g.Rc + St) * F2 * 4, g.Rc * F2 * 4, B, st);
+}
 
 int stream_geom(int n_fft, int hop, int win_length, int la, StreamGeom& g) {
   int rc = stream_dsp_check(n_fft, hop, win_length);

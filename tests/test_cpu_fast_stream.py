@@ -122,50 +122,6 @@ def test_refusals_before_any_cuda_call(kw, n_fft, code):
     assert lib.fsn_last_launch_count() == 0
 
 
-def _step(lib, d, start, tail, B=2, K=4, state_bytes=1 << 40, ws_bytes=1 << 40):
-    s = (C.c_int32 * B)(*start) if start is not None else None
-    t = (C.c_int32 * B)(*tail) if tail is not None else None
-    w = _lib.FastWeights()
-    # non-null dummy pointers: a refusal must come before anything reads them
-    return lib.fsn_fast_stream_step(C.byref(d), C.byref(w), 1, s, t, B, K, 512, 256, 512, 1, 1, state_bytes, 1,
-                                    ws_bytes, None)
-
-
-@pytest.mark.parametrize("tail", [[-2, -1], [0, 4 * 256 + 1]])
-def test_tail_out_of_range_refused(tail):
-    lib = _lib.load()
-    assert _step(lib, _desc(), [1, 1], tail) == _lib.FSN_ERR_SHAPE
-    assert lib.fsn_last_launch_count() == 0
-
-
-def test_zero_hops_refused():
-    lib = _lib.load()
-    assert _step(lib, _desc(), None, None, K=0) == _lib.FSN_ERR_SHAPE
-    assert lib.fsn_last_launch_count() == 0
-
-
-def test_small_state_or_workspace_refused():
-    lib = _lib.load()
-    d = _desc()
-    need_s = lib.fsn_fast_stream_state_bytes(C.byref(d), 2, 512, 256)
-    need_w = lib.fsn_fast_stream_workspace_bytes(C.byref(d), 2, 4, 512, 256)
-    assert _step(lib, d, None, None, state_bytes=need_s - 1) == _lib.FSN_ERR_WORKSPACE
-    assert lib.fsn_last_launch_count() == 0
-    assert _step(lib, d, None, None, ws_bytes=need_w - 1) == _lib.FSN_ERR_WORKSPACE
-    assert lib.fsn_last_launch_count() == 0
-
-
-def test_too_many_slots_refused():
-    lib = _lib.load()
-    B = 65536
-    s = (C.c_int32 * B)()
-    w = _lib.FastWeights()
-    rc = lib.fsn_fast_stream_step(C.byref(_desc()), C.byref(w), 1, s, None, B, 4, 512, 256, 512, 1, 1, 1 << 40, 1,
-                                  1 << 40, None)
-    assert rc == _lib.FSN_ERR_UNSUPPORTED
-    assert lib.fsn_last_launch_count() == 0
-
-
 def _fast_model(**kw):
     from fullsubnet_b200.fast_fullsubnet.model import Model
     precision = kw.pop("precision", "fp32")

@@ -110,38 +110,6 @@ def _step(lib, d, start=None, tail=None, B=2, K=4, state_bytes=1 << 40, ws_bytes
                                ws_bytes, None)
 
 
-@pytest.mark.parametrize("tail", [[-2, -1], [0, 4 * 256 + 1]])
-def test_tail_out_of_range_refused(tail):
-    lib = _lib.load()
-    assert _step(lib, _desc(), [1, 1], tail) == _lib.FSN_ERR_SHAPE
-    assert lib.fsn_last_launch_count() == 0
-
-
-def test_zero_hops_refused():
-    lib = _lib.load()
-    assert _step(lib, _desc(), K=0) == _lib.FSN_ERR_SHAPE
-    assert lib.fsn_last_launch_count() == 0
-
-
-@pytest.mark.parametrize("norm", [CUM, FGT])
-def test_small_state_or_workspace_refused(norm):
-    lib = _lib.load()
-    d = _desc(norm)
-    need_s = lib.fsn_stream_state_bytes(C.byref(d), 2, 512, 256)
-    need_w = lib.fsn_stream_workspace_bytes(C.byref(d), 2, 4, 512, 256)
-    assert _step(lib, d, state_bytes=need_s - 1) == _lib.FSN_ERR_WORKSPACE
-    assert lib.fsn_last_launch_count() == 0
-    assert _step(lib, d, ws_bytes=need_w - 1) == _lib.FSN_ERR_WORKSPACE
-    assert lib.fsn_last_launch_count() == 0
-
-
-def test_too_many_slots_refused():
-    lib = _lib.load()
-    B = 65536
-    assert _step(lib, _desc(), [0] * B, B=B) == _lib.FSN_ERR_UNSUPPORTED
-    assert lib.fsn_last_launch_count() == 0
-
-
 def test_too_many_sub_band_rows_refused():
     """B x F x sb_hidden elements of sub-band state must stay int-indexable: 21 760 slots of the recipe fit, 21 761 not."""
     lib = _lib.load()

@@ -94,26 +94,6 @@ def test_null_packed_weights_refused(prec):
     assert lib.fsn_last_launch_count() == 0
 
 
-def test_too_many_slots_refused():
-    lib = _lib.load()
-    B = 65536
-    assert _tc_step(lib, _desc(prec="f16x3_tc"), [0] * B, B=B) == _lib.FSN_ERR_UNSUPPORTED
-    assert lib.fsn_last_launch_count() == 0
-
-
-@pytest.mark.parametrize("norm", [CUM, FGT])
-@pytest.mark.parametrize("prec", TC_PRECS)
-def test_small_state_or_workspace_refused(norm, prec):
-    lib = _lib.load()
-    d = _desc(norm, prec=prec)
-    need_s = lib.fsn_stream_tc_state_bytes(C.byref(d), 2, 512, 256)
-    need_w = lib.fsn_stream_tc_workspace_bytes(C.byref(d), 2, 4, 512, 256)
-    assert _tc_step(lib, d, state_bytes=need_s - 1) == _lib.FSN_ERR_WORKSPACE
-    assert lib.fsn_last_launch_count() == 0
-    assert _tc_step(lib, d, ws_bytes=need_w - 1) == _lib.FSN_ERR_WORKSPACE
-    assert lib.fsn_last_launch_count() == 0
-
-
 @pytest.mark.parametrize("norm", [CUM, FGT])
 @pytest.mark.parametrize("precision", ["auto", "f16x3_tc", "f16_tc"])
 def test_streamer_tensor_cores_accepts_fullsubnet(precision, norm):
