@@ -206,6 +206,13 @@ _SIGNATURES = {
     "fsn_debug_tgemm": (C.c_int, [_P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _P, _L, _P]),
     "fsn_debug_tgemm_blocked": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _L, _P]),
     "fsn_debug_lstm_fwd_step": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _L, _P]),
+    "fsn_debug_fc_gemm": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "fsn_debug_sgemm": (C.c_int, [_I, _P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _P, _L, _P]),
+    "fsn_debug_colsum": (C.c_int, [_P, _L, _I, _L, _P, _P, _P, _L, _P]),
+    "fsn_debug_small_out_wgrad": (C.c_int, [_P, _P, _L, _I, _P, _P, _L, _P]),
+    "fsn_debug_transpose": (C.c_int, [_P, _L, _I, _P, _P]),
+    "fsn_debug_transpose_blocked": (C.c_int, [_P, _L, _I, _L, _P, _P, _I, C.POINTER(C.c_int), _P, _P]),
+    "fsn_debug_gemm_tc": (C.c_int, [_P, _L, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P, _L, _L, _P, _S, _P]),
     "fsn_debug_lstm_train_workspace_bytes": (_S, [_I, _I, _I, _I, _I, _I]),
     "fsn_debug_lstm_train": (C.c_int, [C.POINTER(LstmLayer), _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P,
                                        C.POINTER(LstmGrads), _P, _P, _S, _P]),

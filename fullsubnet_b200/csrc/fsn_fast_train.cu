@@ -130,6 +130,7 @@ struct FastTrainWs {
   float *dY, *dH, *ddec, *dbn, *dxbn, *denc;
   float *dh_rec[2], *dc[2], *dh_mid;
   float *splitk, *colsum, *gT, *xT, *rec;
+  size_t colsum_floats;
   float *whhT[NL], *wihT[NL];  // FSN_PREC_TF32_TC: transposed weights of the tensor-core layers
   __half *h16[NL], *w16;       // fp16 MMA operands of the forward step kernel
   size_t bytes;
@@ -188,7 +189,8 @@ static void carve_fast_train(const fsn_fast_desc* d, const FastDims& m, void* ba
   for (int i = 0; i < 2; ++i) { w.dh_rec[i] = c.take<float>(rh); w.dc[i] = c.take<float>(rh); }
   w.dh_mid = c.take<float>(rh);
   w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
-  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * smax(4 * hmax, 2 * F));
+  w.colsum_floats = (size_t)COLSUM_MAX_S * smax(4 * hmax, 2 * F);
+  w.colsum = c.take<float>(w.colsum_floats);
   w.gT = w.xT = w.rec = nullptr;
   w.w16 = nullptr;
   for (int l = 0; l < NL; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
@@ -336,7 +338,7 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   const int Hd = d->dec_hidden, He2 = d->enc2_hidden, Hb = d->bn_hidden;
   LayerShape s[NL];
   layer_shapes(d, m, s);
-  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum, w.colsum_floats};
   // the lower layer of each pair keeps its BPTT state in dh_rec[0] / dc[0], the upper one in dh_rec[1] / dc[1]
   LayerBwd L[NL];
   for (int l = 0; l < NL; ++l) {
@@ -348,7 +350,7 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   // ---- decoder Linear(2F) (model.py:196-200 backwards)
   if ((rc = train_dy_launch(dout, nullptr, FSN_ACT_NONE, B, F, T, Tp, d->look_ahead, w.dY, st))) return rc;
   if ((rc = linear_bwd(w.dY, w.L[L_DEC2].H, wt->dec_fc_w, Tp * B, 2 * F, Hd, g->dec_fc_w, g->dec_fc_b, w.dH, w.splitk,
-                       w.colsum, st)))
+                       w.colsum, w.colsum_floats, st)))
     return rc;
   // ---- decoder BPTT, d dec_in
   if ((rc = stack_bwd(L + L_DEC1, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, w.ddec, st))) return rc;
@@ -359,7 +361,7 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
   // ---- up-sampling transpose + ReLU' of the bottleneck output, its Linear(1)
   if ((rc = ftr_dbn_launch(w.ddec, w.bn_out, B, Tp, M, m.S, Ts, w.dbn, st))) return rc;
   if ((rc = linear_bwd(w.dbn, w.L[L_BN1].H, wt->bn_fc_w, Ts * R, 1, Hb, g->bn_fc_w, g->bn_fc_b, nullptr, w.splitk, w.colsum,
-                       st)))
+                       w.colsum_floats, st)))
     return rc;
   // ---- bottleneck BPTT (the Linear(1) backward folded into layer 1's point kernel), d X_bn
   if ((rc = stack_bwd(L + L_BN0, 2, Ts, nullptr, w.dbn, wt->bn_fc_w, 1, w.dh_mid, nullptr, w.dxbn, st))) return rc;
@@ -380,7 +382,7 @@ extern "C" int fsn_fast_train_backward(const fsn_fast_desc* d, const fsn_fast_we
       return rc;
   }
   if ((rc = linear_bwd(w.denc, w.L[L_ENC2].H, wt->enc_fc_w, Tp * B, M, He2, g->enc_fc_w, g->enc_fc_b, w.dH, w.splitk, w.colsum,
-                       st)))
+                       w.colsum_floats, st)))
     return rc;
   // ---- encoder BPTT (its input is the normalised mel spectrogram: no dx)
   if ((rc = stack_bwd(L + L_ENC1, 2, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st))) return rc;

@@ -19,6 +19,7 @@ struct FbbTrainWs {
   float *dY, *dH;
   float *dh_rec[FBB_MAX_LAYERS], *dc[FBB_MAX_LAYERS], *dh_mid[2];
   float *splitk, *colsum, *gT, *xT, *rec;
+  size_t colsum_floats;
   float *whhT[FBB_MAX_LAYERS], *wihT[FBB_MAX_LAYERS];  // FSN_PREC_TF32_TC: transposed weights
   __half *h16[FBB_MAX_LAYERS], *w16;                   // fp16 MMA operands of the forward step kernel
   size_t bytes;
@@ -49,7 +50,8 @@ static void carve_fbb_train(const fsn_fullband_desc* d, int B, int T, void* base
   w.dh_mid[0] = c.take<float>((size_t)B * H);
   w.dh_mid[1] = NL > 2 ? c.take<float>((size_t)B * H) : nullptr;
   w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
-  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * (4 * H > 2 * F ? 4 * H : 2 * F));
+  w.colsum_floats = (size_t)COLSUM_MAX_S * (4 * H > 2 * F ? 4 * H : 2 * F);
+  w.colsum = c.take<float>(w.colsum_floats);
   w.gT = w.xT = w.rec = nullptr;
   w.w16 = nullptr;
   for (int l = 0; l < FBB_MAX_LAYERS; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
@@ -144,11 +146,12 @@ extern "C" int fsn_fullband_train_backward(const fsn_fullband_desc* d, const fsn
   }
   // ---- output re-layout + act', Linear(2F)
   if ((rc = train_dy_launch(dout, w.y, d->activation, B, F, T, Tp, d->look_ahead, w.dY, st))) return rc;
-  if ((rc = linear_bwd(w.dY, w.L[NL - 1].H, fc_w, Tp * B, 2 * F, H, g->fc_w, g->fc_b, w.dH, w.splitk, w.colsum, st))) return rc;
+  if ((rc = linear_bwd(w.dY, w.L[NL - 1].H, fc_w, Tp * B, 2 * F, H, g->fc_w, g->fc_b, w.dH, w.splitk, w.colsum, w.colsum_floats, st)))
+    return rc;
   // ---- BPTT of the stack from the top, one step at a time (the input is the normalised spectrogram: no dx)
   if ((rc = stack_bwd(L, NL, Tp, w.dH, nullptr, nullptr, 0, w.dh_mid[0], w.dh_mid[1], nullptr, st))) return rc;
   // ---- weight gradients: layer 0 reads the normalised input, layer l the hidden states of layer l-1
-  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum, w.colsum_floats};
   for (int l = NL - 1; l >= 0; --l) {
     const fsn_lstm_grads& q = g->layer[l];
     if ((rc = layer_weight_grads(L[l], Tp, l == 0 ? w.xfb : w.L[l - 1].H, q.w_ih, q.w_hh, q.b_ih, q.b_hh, wg, st))) return rc;

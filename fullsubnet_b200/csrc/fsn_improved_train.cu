@@ -27,6 +27,7 @@ struct ImpTrainWs {
   float *dcrm, *dY, *dH, *dX, *dfb, *dot;
   float *dh_rec[2], *dc[2], *dh_mid;
   float *splitk, *colsum;
+  size_t colsum_floats;
   // tf32 layers: transposed weights of the stack being differentiated (a section's, then the full band's), K-major
   // copies for the weight gradients, the recurrent product of the unfused step, fp16 operands of the forward step kernel
   float *whhT[2], *wihT[2], *gT, *xT, *rec;
@@ -74,7 +75,8 @@ static void carve_imp_train(const fsn_improved_desc* d, const ImpDims& m, void* 
   for (int l = 0; l < 2; ++l) { w.dh_rec[l] = c.take<float>(RH); w.dc[l] = c.take<float>(RH); }
   w.dh_mid = c.take<float>(RH);
   w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
-  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * zmax(4 * zmax(Hf, Hs), maxO));
+  w.colsum_floats = (size_t)COLSUM_MAX_S * zmax(4 * zmax(Hf, Hs), maxO);
+  w.colsum = c.take<float>(w.colsum_floats);
   for (int l = 0; l < 2; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
   w.gT = w.xT = w.rec = nullptr;
   w.w16 = nullptr;
@@ -231,7 +233,7 @@ extern "C" int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn
   cudaStream_t st = (cudaStream_t)stream;
   const int T = m.T, F = m.F, Fu = m.Fu, Hf = d->fb_hidden, Hs = d->sb_hidden;
   const bool tf = tf32_layer(d->precision, Hf), ts = tf32_layer(d->precision, Hs);
-  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum, w.colsum_floats};
   // ---- mask + iSTFT adjoint: d loss / d cRM
   if ((rc = istft_mask_adjoint_launch(d_enhanced, w.real, w.imag, B, L, T, d->n_fft, d->hop_length, d->win_length, w.dcrm, st)))
     return rc;
@@ -250,7 +252,8 @@ extern "C" int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn
     for (int l = 0; l < 2; ++l)
       if ((rc = layer_bwd_transpose_weights(Ls[l], st))) return rc;
     if ((rc = sb_head_bwd_launch(w.dcrm, w.crm, d->sb_activation, R, O, T, 0, imp_head_geom(sg, F, T), w.dY, st))) return rc;
-    if ((rc = linear_bwd(w.dY, q.L[1].H, sw.fc_w, T * R, O, Hs, sgr.fc_w, sgr.fc_b, w.dH, w.splitk, w.colsum, st))) return rc;
+    if ((rc = linear_bwd(w.dY, q.L[1].H, sw.fc_w, T * R, O, Hs, sgr.fc_w, sgr.fc_b, w.dH, w.splitk, w.colsum, w.colsum_floats, st)))
+      return rc;
     // BPTT down to the normalised section input
     if ((rc = stack_bwd(Ls, 2, T, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, w.dX, st))) return rc;
     if ((rc = train_dot_launch(w.dX, q.Xn, T, R, sg.N, sg.W, B, w.dot, st))) return rc;
@@ -269,7 +272,8 @@ extern "C" int fsn_improved_train_backward(const fsn_improved_desc* d, const fsn
                tf ? w.wihT[1] : nullptr, w.splitk}};
   for (int l = 0; l < 2; ++l)
     if ((rc = layer_bwd_transpose_weights(Lf[l], st))) return rc;
-  if ((rc = linear_bwd(w.dfb, w.fb[1].H, fw.fc_w, T * B, Fu, Hf, fg.fc_w, fg.fc_b, w.dH, w.splitk, w.colsum, st))) return rc;
+  if ((rc = linear_bwd(w.dfb, w.fb[1].H, fw.fc_w, T * B, Fu, Hf, fg.fc_w, fg.fc_b, w.dH, w.splitk, w.colsum, w.colsum_floats, st)))
+    return rc;
   if ((rc = stack_bwd(Lf, 2, T, w.dH, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st))) return rc;
   if ((rc = layer_weight_grads(Lf[1], T, w.fb[0].H, fg.w_ih[1], fg.w_hh[1], fg.b_ih[1], fg.b_hh[1], wg, st))) return rc;
   return layer_weight_grads(Lf[0], T, w.xfb, fg.w_ih[0], fg.w_hh[0], fg.b_ih[0], fg.b_hh[0], wg, st);

@@ -150,6 +150,9 @@ int tgemm_launch(const float* A, size_t lda, const float* Bm, size_t ldb, float*
 size_t tgemm_blocked_floats(size_t K, int M);
 int transpose_blocked_launch(const float* in, size_t K, int M, size_t ld, float* out, cudaStream_t st, float* colsum_part,
                              int max_slabs, int* slabs);
+// out[c] (and out2[c] when given) = sum_{z < S} part[z * cols + c] in a fixed order (fsn_train.cu): the second pass of
+// a column sum, e.g. over the colsum_part slabs of transpose_blocked_launch
+int colsum_final_launch(const float* part, int S, int cols, float* out, float* out2, cudaStream_t st);
 int tgemm_blocked_launch(const float* Ablk, int nkb_a, int a_kb0, const float* Bblk, int nkb_b, int b_kb0, float* C, size_t ldc,
                          int M, int N, int K, bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st);
 
@@ -204,8 +207,8 @@ struct LayerBwd {
   float* splitk;               // split-K space of the per-step GEMMs (used when the layer has only a few tiles)
 };
 // scratch of layer_weight_grads: K-major copies of dG / layer input (tensor-core path, tgemm_blocked_floats of the largest
-// layer), split-K space (SPLITK_SCRATCH_FLOATS) and column-sum partials (COLSUM_MAX_S x 4H)
-struct WgradScratch { float *gT, *xT, *splitk, *colsum; };
+// layer), split-K space (SPLITK_SCRATCH_FLOATS) and column-sum partials (colsum_floats, COLSUM_MAX_S x 4H for full slabs)
+struct WgradScratch { float *gT, *xT, *splitk, *colsum; size_t colsum_floats; };
 // tensor-core path: writes L.w_hhT, and L.w_ihT when the layer has one (it computes a dx); nothing when L.w_hhT is null
 int layer_bwd_transpose_weights(const LayerBwd& L, cudaStream_t st);
 // step t of one layer: pointwise gate gradients (d h from above = dh_above + dout W_fc for an O-output Linear on top),
@@ -232,15 +235,22 @@ int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int 
 // the kept post-activation output y (unread for FSN_ACT_NONE)
 int train_dy_launch(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
                     cudaStream_t st);
-// fp32 SIMT GEMM C[M,N] (+)= op(A) B (op(A) = A^T when ta), split-K over `scratch` for long K (deterministic)
+// fp32 SIMT GEMM C[M,N] (+)= op(A) B (op(A) = A^T when ta), split-K over `scratch` (scratch_floats; S M N partial sums
+// must fit, S drops until they do) for long K (deterministic)
 int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M, int N, int K,
-                 bool accumulate, float* scratch, cudaStream_t st);
-// out[c] (and out2[c] when given) = sum_r X[r*ldx + c], fixed order
-int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch, cudaStream_t st);
+                 bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st);
+// out[c] (and out2[c] when given) = sum_r X[r*ldx + c], fixed order; S = min(ceil(rows / 2048), COLSUM_MAX_S) row slabs
+// of partials in scratch: FSN_ERR_WORKSPACE when S * cols > scratch_floats
+int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch,
+                  size_t scratch_floats, cudaStream_t st);
+// dW [2,H] = dout^T Hm of the 2-output sub-band Linear (dout [rows,2], Hm [rows,H]), partials in scratch (S 2 H floats,
+// S dropping until they fit; FSN_ERR_WORKSPACE when even 2 H do not)
+int small_out_wgrad_launch(const float* dout, const float* Hm, size_t rows, int H, float* dW, float* scratch,
+                           size_t scratch_floats, cudaStream_t st);
 // backward of a Linear Y = X W^T + b over `rows` rows, dY [rows,N], X [rows,K], W [N,K]: dW = dY^T X (split-K over
 // `splitk`), db = colsum dY (partials in `colsum`) and, when dX != nullptr, dX = dY W
 int linear_bwd(const float* dY, const float* X, const float* W, int rows, int N, int K, float* dW, float* db, float* dX,
-               float* splitk, float* colsum, cudaStream_t st);
+               float* splitk, float* colsum, size_t colsum_floats, cudaStream_t st);
 // out [cols, rows] = in [rows, cols]^T
 int transpose_launch(const float* in, size_t rows, int cols, float* out, cudaStream_t st);
 // per-clip (sum, sum_f c_N[f] * row sum) of a time-major x [Tp,B,F] (train_tm_stats) or of mag [B,F,T]

@@ -607,3 +607,36 @@ extern "C" int fsn_debug_lstm_tc_carry(const float* w_ih, const float* w_hh, con
   const fsn::RecCarry io{h_init, c, c, (size_t)H, restart, fin_step};
   return fsn::lstm_layer_tc(L, x, (size_t)K, K, nullptr, 1, 0, R, T, H, x3 != 0, ws, hall, (cudaStream_t)stream, &io);
 }
+// unit-test hook of the tf32 GEMM path of the full-band stacks: out[rows, :N] (row stride ldo) = act(x' W^T + bias) with
+// x' = x[rows, :K] (row stride ldx) times its row scale, i.e. the input projection of lstm_layer_tc (prep_operand,
+// gemm_tc_split_launch) and the epilogue of linear_tc (bias_act_launch).  Workspace: the prepared A and W operands only,
+// carved as lstm_tc_carve lays them out (so fsn_debug_lstm_tc_workspace_bytes(rows, 1, K, max(8, ceil(N / 4)), x3) is
+// always enough) and sized in host arithmetic.  Every argument is checked before any CUDA call.
+extern "C" int fsn_debug_gemm_tc(const float* x, int64_t ldx, int K, const float* row_scale, int rows_per_scale, int scale_B,
+                                 const float* W, int N, const float* bias, int act, int x3, float* out, int64_t ldo, int64_t rows,
+                                 void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  fsn::launch_counter() = 0;
+  FSN_REQUIRE(x && W && out, FSN_ERR_SHAPE, "gemm_tc hook: null argument");
+  FSN_REQUIRE(K > 0 && N > 0 && rows > 0 && rows < ((int64_t)1 << 31) && ldx >= K && ldo >= N, FSN_ERR_SHAPE,
+              "gemm_tc hook: bad shape rows=%lld K=%d N=%d ldx=%lld ldo=%lld", (long long)rows, K, N, (long long)ldx,
+              (long long)ldo);
+  FSN_REQUIRE(!row_scale || (rows_per_scale >= 1 && scale_B >= 0), FSN_ERR_SHAPE,
+              "gemm_tc hook: a row scale needs rows_per_scale >= 1 and scale_B >= 0");
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "gemm_tc hook: unknown act %d", act);
+  FSN_REQUIRE((N + 127) / 128 <= 65535, FSN_ERR_SHAPE, "gemm_tc hook: N=%d exceeds the grid", N);
+  fsn::Carver c(workspace);
+  const size_t wa = (size_t)((K + 3) & ~3) * (x3 ? 3 : 1);
+  const int Hm = (N + 3) / 4 > 8 ? (N + 3) / 4 : 8;
+  fsn::LstmTcWs ws{};
+  ws.a = c.take<float>((size_t)rows * wa);
+  ws.w = c.take<float>((size_t)4 * Hm * wa);
+  FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, c.off);
+  cudaStream_t st = (cudaStream_t)stream;
+  const float* a;
+  size_t lda;
+  int rc;
+  if ((rc = fsn::prep_operand(x, (size_t)ldx, K, (size_t)rows, row_scale, rows_per_scale, scale_B, x3 != 0, ws, a, lda, st)))
+    return rc;
+  if ((rc = fsn::gemm_tc_split_launch(a, lda, W, N, K, ws.w, out, (size_t)ldo, (size_t)rows, x3 != 0, st))) return rc;
+  return fsn::bias_act_launch(out, (size_t)rows, N, (size_t)ldo, bias, act, st);
+}

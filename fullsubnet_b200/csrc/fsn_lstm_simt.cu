@@ -680,3 +680,14 @@ extern "C" int fsn_debug_forgetting_scale(const float* x, int N, const float* x2
   if (x2 && (rc = frame_stats_launch(x2, B, T_pad, F, N2, (size_t)bs, (size_t)ts, f2, st))) return rc;
   return forget_scale_launch(f1, f2, B, T_pad, cnt, scale, mu, st, w.lens, hop, la);
 }
+
+// ---- unit-test hook of the fp32 Linear (include/fsn_b200.h): fc_gemm_launch, every argument checked before any CUDA call
+extern "C" int fsn_debug_fc_gemm(const float* A, const float* W, const float* bias, float* out, int M, int K, int O, int act,
+                                 int w_kmajor, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(A && W && out, FSN_ERR_SHAPE, "fc_gemm hook: null argument");
+  FSN_REQUIRE(M > 0 && K > 0 && O > 0, FSN_ERR_SHAPE, "fc_gemm hook: bad shape M=%d K=%d O=%d", M, K, O);
+  FSN_REQUIRE(O <= 65535 * 64, FSN_ERR_SHAPE, "fc_gemm hook: O=%d exceeds the grid", O);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "fc_gemm hook: unknown act %d", act);
+  return fc_gemm_launch(A, W, bias, out, M, K, O, act, (cudaStream_t)stream, w_kmajor != 0);
+}

@@ -627,10 +627,30 @@ extern "C" int fsn_debug_tgemm_blocked(const float* A, const float* B, float* C,
                                    false, scratch + fa + fb, (size_t)scratch_floats - fa - fb, st);
 }
 
+// unit-test hook: the block-tiled transposed copy of in [K, M] (row stride ld) into out (tgemm_blocked_floats(K, M)
+// floats); with colsum_part (>= max_slabs * M floats) also the per-slab column sums and their fixed-order total into
+// bias_out [M], as layer_weight_grads takes the bias gradients; *slabs (nullable) receives the slab count
+extern "C" int fsn_debug_transpose_blocked(const float* in, int64_t K, int M, int64_t ld, float* out, float* colsum_part,
+                                           int max_slabs, int* slabs, float* bias_out, fsn_stream_t stream) {
+  fsn::launch_counter() = 0;
+  FSN_REQUIRE(in && out, FSN_ERR_SHAPE, "transpose_blocked hook: null argument");
+  FSN_REQUIRE(K > 0 && M > 0 && ld >= M, FSN_ERR_SHAPE, "transpose_blocked hook: bad shape K=%lld M=%d ld=%lld", (long long)K,
+              M, (long long)ld);
+  FSN_REQUIRE(!colsum_part || (bias_out && max_slabs > 0), FSN_ERR_SHAPE,
+              "transpose_blocked hook: column sums need bias_out and max_slabs >= 1");
+  cudaStream_t st = (cudaStream_t)stream;
+  int S = 0;
+  int rc = fsn::transpose_blocked_launch(in, (size_t)K, M, (size_t)ld, out, st, colsum_part, max_slabs, &S);
+  if (rc) return rc;
+  if (slabs) *slabs = S;
+  return colsum_part ? fsn::colsum_final_launch(colsum_part, S, M, bias_out, nullptr, st) : FSN_OK;
+}
+
 // unit-test hook for the fused training-forward step (tg::lstm_fwd_step_kernel; torch.nn.LSTM cell math): one step
 //   z = [X W_ih^T  or  the P already in G] + b_ih + b_hh + Hprev W_hh^T;  G <- act(z) (i,f,g,o), C_out, H_out
 // Hprev nullable (first step), X nullable (then G [R,4H] holds the hoisted projection on entry).  half != 0: fp16 MMA
-// operands, converted here into `scratch` (>= 2 * (2 R H + 4 H (H + K0) + R K0) bytes)
+// operands for h and the weights, converted here into `scratch` (>= 2 * (2 R H + 4 H (H + K0) + R K0) bytes); X and W_ih
+// too when K0 % 8 == 0 (16-byte fp16 rows), else they stay tf32 in the same k loop, the rule of layer_forward_save_tc
 extern "C" int fsn_debug_lstm_fwd_step(const float* Hprev, const float* w_hh, const float* X, const float* w_ih, int K0, float* G,
                                        const float* b_ih, const float* b_hh, const float* C_prev, float* C_out, float* H_out,
                                        int R, int H, int half, void* scratch, int64_t scratch_bytes, fsn_stream_t stream) {
@@ -642,7 +662,8 @@ extern "C" int fsn_debug_lstm_fwd_step(const float* Hprev, const float* w_hh, co
   FSN_REQUIRE(!X || fsn::tgemm_supported(X, K0, w_ih, K0, K0), FSN_ERR_UNSUPPORTED, "lstm_fwd_step hook: X rows must be 16-byte aligned");
   if (!half) return fsn::lstm_fwd_step_launch(Hprev, w_hh, X, w_ih, K0, G, b_ih, b_hh, C_prev, C_out, H_out, R, H, st, nullptr);
   const size_t nh = (size_t)R * H, nw = (size_t)4 * H * H, nx = X ? (size_t)R * K0 : 0, nwx = X ? (size_t)4 * H * K0 : 0;
-  FSN_REQUIRE((H % 8) == 0 && (!X || (K0 % 8) == 0), FSN_ERR_UNSUPPORTED, "lstm_fwd_step hook: fp16 rows must be 16-byte aligned");
+  FSN_REQUIRE((H % 8) == 0, FSN_ERR_UNSUPPORTED, "lstm_fwd_step hook: fp16 rows must be 16-byte aligned");
+  const bool x16 = X && (K0 % 8) == 0;
   FSN_REQUIRE(scratch && (size_t)scratch_bytes >= 2 * (2 * nh + nw + nx + nwx) + 1024, FSN_ERR_WORKSPACE,
               "lstm_fwd_step hook: scratch too small");
   auto up = [](size_t n) { return (n + 127) & ~(size_t)127; };  // keep every block 256-byte aligned
@@ -656,7 +677,7 @@ extern "C" int fsn_debug_lstm_fwd_step(const float* Hprev, const float* w_hh, co
   int rc;
   if (Hprev && (rc = fsn::to_half_launch(Hprev, nh, hp, st))) return rc;
   if ((rc = fsn::to_half_launch(w_hh, nw, wh, st))) return rc;
-  if (X && ((rc = fsn::to_half_launch(X, nx, xx, st)) || (rc = fsn::to_half_launch(w_ih, nwx, wx, st)))) return rc;
-  fsn::LstmStepHalf hs{Hprev ? hp : nullptr, wh, X ? xx : nullptr, X ? wx : nullptr, ho};
+  if (x16 && ((rc = fsn::to_half_launch(X, nx, xx, st)) || (rc = fsn::to_half_launch(w_ih, nwx, wx, st)))) return rc;
+  fsn::LstmStepHalf hs{Hprev ? hp : nullptr, wh, x16 ? xx : nullptr, x16 ? wx : nullptr, ho};
   return fsn::lstm_fwd_step_launch(Hprev, w_hh, X, w_ih, K0, G, b_ih, b_hh, C_prev, C_out, H_out, R, H, st, &hs);
 }

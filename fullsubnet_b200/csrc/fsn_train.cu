@@ -103,14 +103,14 @@ int splitk_reduce_launch(const float* part, int S, int M, int N, float* C, size_
 }
 
 int sgemm_launch(bool ta, const float* A, size_t lda, const float* Bm, size_t ldb, float* C, size_t ldc, int M,
-                        int N, int K, bool accumulate, float* scratch, cudaStream_t st) {
+                        int N, int K, bool accumulate, float* scratch, size_t scratch_floats, cudaStream_t st) {
   if (M <= 0 || N <= 0 || K <= 0) return FSN_OK;
   const int tiles = cdiv(M, 64) * cdiv(N, 64);
   int S = 1;
   if (scratch && K >= 4096 && tiles < 528) {  // fill 132 SMs x 4 CTAs; slices of >= 1024 k
     S = cdiv(592, tiles);
     if (S > cdiv(K, 1024)) S = cdiv(K, 1024);
-    while (S > 1 && (size_t)S * M * N > SPLITK_SCRATCH_FLOATS) --S;
+    while (S > 1 && (size_t)S * M * N > scratch_floats) --S;
   }
   const int kps = cdiv(cdiv(K, S), 16) * 16;
   S = cdiv(K, kps);
@@ -157,6 +157,11 @@ __global__ void colsum_final_kernel(const float* __restrict__ part, int S, int c
   out[c] = s;
   if (out2) out2[c] = s;
 }
+int colsum_final_launch(const float* part, int S, int cols, float* out, float* out2, cudaStream_t st) {
+  colsum_final_kernel<<<cdiv(cols, 128), 128, 0, st>>>(part, S, cols, out, out2);
+  FSN_CHECK_LAUNCH("colsum_final_kernel");
+  return FSN_OK;
+}
 
 // dW [O,H] = dout^T Hm for a Linear with a few outputs (the sub-band Linear, O = 2; model.py:129-135 backwards):
 // dout [rows,O], Hm [rows,H].  One pass over Hm: a CTA owns a slab of rows, a thread one column; part [S][O][H], then
@@ -190,15 +195,38 @@ __global__ void __launch_bounds__(128) small_out_wgrad_kernel(const float* __res
     for (int o = 0; o < O; ++o) part[((size_t)blockIdx.y * O + o) * H + c] = acc[o];
   }
 }
-int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch,
-                         cudaStream_t st) {
+// row slabs of a column sum over `rows` rows: one per 2048 rows, at most COLSUM_MAX_S
+static int colsum_slabs(size_t rows) {
   int S = (int)((rows + 2047) / 2048);
   if (S > COLSUM_MAX_S) S = COLSUM_MAX_S;
-  if (S < 1) S = 1;
+  return S < 1 ? 1 : S;
+}
+int colsum_launch(const float* X, size_t rows, int cols, size_t ldx, float* out, float* out2, float* scratch,
+                  size_t scratch_floats, cudaStream_t st) {
+  const int S = colsum_slabs(rows);
+  FSN_REQUIRE((size_t)S * cols <= scratch_floats, FSN_ERR_WORKSPACE, "colsum: %d slabs x %d columns exceed the %zu-float scratch",
+              S, cols, scratch_floats);
   const size_t rows_per = (rows + S - 1) / S;
   colsum_part_kernel<<<dim3(cdiv(cols, 32), S), dim3(32, 8), 0, st>>>(X, rows, cols, ldx, rows_per, scratch);
   FSN_CHECK_LAUNCH("colsum_part_kernel");
   colsum_final_kernel<<<cdiv(cols, 128), 128, 0, st>>>(scratch, S, cols, out, out2);
+  FSN_CHECK_LAUNCH("colsum_final_kernel");
+  return FSN_OK;
+}
+
+// dW [2,H] of the 2-output sub-band Linear from dout [rows,2] and Hm [rows,H]: one streaming pass over Hm (2.4 GB at
+// config 3), partials [S][2][H] in scratch, then their fixed-order sum.  S drops until the partials fit scratch_floats.
+int small_out_wgrad_launch(const float* dout, const float* Hm, size_t rows, int H, float* dW, float* scratch,
+                           size_t scratch_floats, cudaStream_t st) {
+  int S = (int)((rows + 2047) / 2048);
+  if (S > COLSUM_MAX_S) S = COLSUM_MAX_S;
+  while (S > 1 && (size_t)S * 2 * H > scratch_floats) --S;
+  FSN_REQUIRE((size_t)S * 2 * H <= scratch_floats, FSN_ERR_WORKSPACE, "small_out_wgrad: %d floats of partials exceed the %zu-float scratch",
+              2 * H, scratch_floats);
+  const size_t rows_per = (rows + S - 1) / S;
+  small_out_wgrad_kernel<2><<<dim3(cdiv(H, 128), S), 128, 0, st>>>(dout, Hm, rows, H, rows_per, scratch);
+  FSN_CHECK_LAUNCH("small_out_wgrad_kernel");
+  colsum_final_kernel<<<cdiv(2 * H, 128), 128, 0, st>>>(scratch, S, 2 * H, dW, nullptr);
   FSN_CHECK_LAUNCH("colsum_final_kernel");
   return FSN_OK;
 }
@@ -541,6 +569,7 @@ struct TrainWs {
   float *dh_rec[2], *dc[2], *dh_mid, *dot;
   float *splitk, *colsum;
   float *splitk2, *colsum2;  // scratch of the side stream (full-band backward overlapped with the sub-band weight gradients)
+  size_t colsum_floats;       // floats of colsum and of colsum2
   // FSN_PREC_TF32_TC: transposed weights ([H,4H], [K0,4H]) and transposed dG / layer inputs for the weight gradients
   float *sb_whhT[2], *sb_wihT[2], *fb_whhT[2], *fb_wihT1;
   float *gT, *xT, *rec;
@@ -582,9 +611,10 @@ static void carve_train(const fsn_model_desc* d, const Dims& m, void* base, Trai
   }
   w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
   const size_t maxcols = 4 * (Hf > Hs ? Hf : Hs) > F ? 4 * (Hf > Hs ? Hf : Hs) : F;
-  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * maxcols);
+  w.colsum_floats = (size_t)COLSUM_MAX_S * maxcols;  // each of colsum, colsum2
+  w.colsum = c.take<float>(w.colsum_floats);
   w.splitk2 = c.take<float>(SPLITK_SCRATCH_FLOATS);
-  w.colsum2 = c.take<float>((size_t)COLSUM_MAX_S * maxcols);
+  w.colsum2 = c.take<float>(w.colsum_floats);
   if (d->precision == FSN_PREC_TF32_TC) {
     for (int l = 0; l < 2; ++l) {
       w.sb_whhT[l] = c.take<float>(Hs * 4 * Hs);
@@ -719,11 +749,11 @@ int layer_bwd_transpose_weights(const LayerBwd& L, cudaStream_t st) {
 }
 
 int linear_bwd(const float* dY, const float* X, const float* W, int rows, int N, int K, float* dW, float* db, float* dX,
-               float* splitk, float* colsum, cudaStream_t st) {
+               float* splitk, float* colsum, size_t colsum_floats, cudaStream_t st) {
   int rc;
-  if ((rc = sgemm_launch(true, dY, N, X, K, dW, K, N, K, rows, false, splitk, st))) return rc;
-  if ((rc = colsum_launch(dY, (size_t)rows, N, N, db, nullptr, colsum, st))) return rc;
-  if (dX && (rc = sgemm_launch(false, dY, N, W, K, dX, K, rows, K, N, false, nullptr, st))) return rc;
+  if ((rc = sgemm_launch(true, dY, N, X, K, dW, K, N, K, rows, false, splitk, SPLITK_SCRATCH_FLOATS, st))) return rc;
+  if ((rc = colsum_launch(dY, (size_t)rows, N, N, db, nullptr, colsum, colsum_floats, st))) return rc;
+  if (dX && (rc = sgemm_launch(false, dY, N, W, K, dX, K, rows, K, N, false, nullptr, 0, st))) return rc;
   return FSN_OK;
 }
 
@@ -746,12 +776,12 @@ int layer_bwd_step(const LayerBwd& L, int t, int Tp, const float* dh_above, cons
   const bool tc = tc_bwd(L);
   if (t > 0) {
     if (tc) rc = tgemm_launch(p.G, 4 * L.H, L.w_hhT, 4 * L.H, L.dh_rec, L.H, L.R, L.H, 4 * L.H, false, L.splitk, SPLITK_SCRATCH_FLOATS, st);
-    else         rc = sgemm_launch(false, p.G, 4 * L.H, L.w_hh, L.H, L.dh_rec, L.H, L.R, L.H, 4 * L.H, false, nullptr, st);
+    else         rc = sgemm_launch(false, p.G, 4 * L.H, L.w_hh, L.H, L.dh_rec, L.H, L.R, L.H, 4 * L.H, false, nullptr, 0, st);
     if (rc) return rc;
   }
   if (dx) {
     if (tc && L.w_ihT) rc = tgemm_launch(p.G, 4 * L.H, L.w_ihT, 4 * L.H, dx, L.K0, L.R, L.K0, 4 * L.H, false, L.splitk, SPLITK_SCRATCH_FLOATS, st);
-    else         rc = sgemm_launch(false, p.G, 4 * L.H, L.w_ih, L.K0, dx, L.K0, L.R, L.K0, 4 * L.H, false, nullptr, st);
+    else         rc = sgemm_launch(false, p.G, 4 * L.H, L.w_ih, L.K0, dx, L.K0, L.R, L.K0, 4 * L.H, false, nullptr, 0, st);
     if (rc) return rc;
   }
   return FSN_OK;
@@ -768,7 +798,12 @@ int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih,
     // pitch of `rows` floats): dW_ih = dG^T X, dW_hh = dG[1:]^T H[:-1]
     const int nkb = (rows + 31) / 32;
     int slabs = 0;  // bias gradients = column sums of dG, taken while its tiles pass through shared memory
-    if ((rc = transpose_blocked_launch(L.s.G, (size_t)rows, H4, (size_t)H4, w.gT, st, w.colsum, COLSUM_MAX_S, &slabs))) return rc;
+    // at most COLSUM_MAX_S slabs of H4 partial sums, fewer when the scratch holds fewer
+    const size_t fit = w.colsum_floats / H4;
+    FSN_REQUIRE(fit >= 1, FSN_ERR_WORKSPACE, "weight gradients: %zu floats of column-sum scratch for %d columns", w.colsum_floats, H4);
+    if ((rc = transpose_blocked_launch(L.s.G, (size_t)rows, H4, (size_t)H4, w.gT, st, w.colsum,
+                                       fit < (size_t)COLSUM_MAX_S ? (int)fit : COLSUM_MAX_S, &slabs)))
+      return rc;
     colsum_final_kernel<<<cdiv(H4, 128), 128, 0, st>>>(w.colsum, slabs, H4, g_b_ih, g_b_hh);
     FSN_CHECK_LAUNCH("colsum_final_kernel");
     if ((rc = transpose_blocked_launch(X, (size_t)rows, L.K0, (size_t)L.K0, w.xT, st, nullptr, 0, nullptr))) return rc;
@@ -790,15 +825,17 @@ int layer_weight_grads(const LayerBwd& L, int Tp, const float* X, float* g_w_ih,
     }
     return FSN_OK;
   }
-  if ((rc = sgemm_launch(true, L.s.G, H4, X, L.K0, g_w_ih, L.K0, H4, L.K0, rows, false, w.splitk, st))) return rc;
+  if ((rc = sgemm_launch(true, L.s.G, H4, X, L.K0, g_w_ih, L.K0, H4, L.K0, rows, false, w.splitk, SPLITK_SCRATCH_FLOATS,
+                         st)))
+    return rc;
   if (Tp > 1) {
     if ((rc = sgemm_launch(true, L.s.G + (size_t)L.R * H4, H4, L.s.H, L.H, g_w_hh, L.H, H4, L.H, rows - L.R, false,
-                           w.splitk, st)))
+                           w.splitk, SPLITK_SCRATCH_FLOATS, st)))
       return rc;
   } else if ((rc = check_cuda(cudaMemsetAsync(g_w_hh, 0, (size_t)H4 * L.H * sizeof(float), st), "memset"))) {
     return rc;
   }
-  return colsum_launch(L.s.G, (size_t)rows, H4, H4, g_b_ih, g_b_hh, w.colsum, st);
+  return colsum_launch(L.s.G, (size_t)rows, H4, H4, g_b_ih, g_b_hh, w.colsum, w.colsum_floats, st);
 }
 
 int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const float* dout, const float* fc_w, int O,
@@ -962,18 +999,10 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   // ---- sub-band Linear (model.py:129-135 backwards)
   if ((rc = sb_head_bwd_launch(dcrm, nullptr, FSN_ACT_NONE, R, 2, Tp, d->look_ahead, fsn_head_geom(m.Fsub, T), w.dout, st)))
     return rc;
-  {  // dW of the 2-output Linear: one streaming pass over h1 (2.4 GB at config 3)
-    const size_t rows = (size_t)Tp * R;
-    int S = (int)((rows + 2047) / 2048);
-    if (S > COLSUM_MAX_S) S = COLSUM_MAX_S;
-    while (S > 1 && (size_t)S * 2 * Hs > SPLITK_SCRATCH_FLOATS) --S;
-    const size_t rows_per = (rows + S - 1) / S;
-    small_out_wgrad_kernel<2><<<dim3(cdiv(Hs, 128), S), 128, 0, st>>>(w.dout, w.sb[1].H, rows, Hs, rows_per, w.splitk);
-    FSN_CHECK_LAUNCH("small_out_wgrad_kernel");
-    colsum_final_kernel<<<cdiv(2 * Hs, 128), 128, 0, st>>>(w.splitk, S, 2 * Hs, gsb->fc_w, nullptr);
-    FSN_CHECK_LAUNCH("colsum_final_kernel");
-  }
-  if ((rc = colsum_launch(w.dout, (size_t)Tp * R, 2, 2, gsb->fc_b, nullptr, w.colsum, st))) return rc;
+  // dW of the 2-output Linear: one streaming pass over h1
+  if ((rc = small_out_wgrad_launch(w.dout, w.sb[1].H, (size_t)Tp * R, Hs, gsb->fc_w, w.splitk, SPLITK_SCRATCH_FLOATS, st)))
+    return rc;
+  if ((rc = colsum_launch(w.dout, (size_t)Tp * R, 2, 2, gsb->fc_b, nullptr, w.colsum, w.colsum_floats, st))) return rc;
   const bool tc_fb = tf32_layer(d->precision, Hf), tc_sb = tf32_layer(d->precision, Hs);
   // the full-band chain (second norm, full-band Linear, full-band BPTT) runs on the side stream st2, with its own split-K /
   // column-sum scratch
@@ -997,7 +1026,7 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
   // ---- fork: sub-band weight gradients on the caller's stream, the rest of the chain on st2
   if ((rc = check_cuda(cudaEventRecord(side->fork, st), "event record"))) return rc;
   if ((rc = check_cuda(cudaStreamWaitEvent(st2, side->fork, 0), "stream wait"))) return rc;
-  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum, w.colsum_floats};
   if ((rc = layer_weight_grads(sbL[1], Tp, w.sb[0].H, gsb->w_ih[1], gsb->w_hh[1], gsb->b_ih[1], gsb->b_hh[1], wg, st)))
     return rc;
   if ((rc = layer_weight_grads(sbL[0], Tp, w.xsb, gsb->w_ih[0], gsb->w_hh[0], gsb->b_ih[0], gsb->b_hh[0], wg, st))) return rc;
@@ -1015,7 +1044,8 @@ extern "C" int fsn_train_backward(const fsn_model_desc* d, const fsn_seq_weights
                                 st2)))
       return rc;
   }
-  if ((rc = linear_bwd(w.dz, w.fb[1].H, fb->fc_w, Tp * B, F, Hf, gfb->fc_w, gfb->fc_b, w.dfh1, w.splitk2, w.colsum2, st2)))
+  if ((rc = linear_bwd(w.dz, w.fb[1].H, fb->fc_w, Tp * B, F, Hf, gfb->fc_w, gfb->fc_b, w.dfh1, w.splitk2, w.colsum2,
+                       w.colsum_floats, st2)))
     return rc;
   // ---- full-band stack
   if ((rc = stack_bwd(fbL, 2, Tp, w.dfh1, nullptr, nullptr, 0, w.dh_mid, nullptr, nullptr, st2))) return rc;
@@ -1038,6 +1068,7 @@ struct DbgLstmWs {
   LayerSave L[DBG_MAX_LAYERS];
   float *dh_rec[DBG_MAX_LAYERS], *dc[DBG_MAX_LAYERS], *dh_mid[2];
   float *splitk, *colsum, *gT, *xT, *rec;
+  size_t colsum_floats;
   float *whhT[DBG_MAX_LAYERS], *wihT[DBG_MAX_LAYERS];
   __half *h16[DBG_MAX_LAYERS], *w16;
   size_t bytes;
@@ -1053,7 +1084,8 @@ static void carve_dbg_lstm(int n, int R, int T, int K0, int H, int precision, vo
   w.dh_mid[0] = c.take<float>(RH);
   w.dh_mid[1] = c.take<float>(RH);
   w.splitk = c.take<float>(SPLITK_SCRATCH_FLOATS);
-  w.colsum = c.take<float>((size_t)COLSUM_MAX_S * 4 * Hs);
+  w.colsum_floats = (size_t)COLSUM_MAX_S * 4 * Hs;
+  w.colsum = c.take<float>(w.colsum_floats);
   w.gT = w.xT = w.rec = nullptr;
   w.w16 = nullptr;
   for (int l = 0; l < DBG_MAX_LAYERS; ++l) { w.whhT[l] = w.wihT[l] = nullptr; w.h16[l] = nullptr; }
@@ -1128,7 +1160,7 @@ extern "C" int fsn_debug_lstm_train(const fsn_lstm_layer* layers, int n_layers, 
     if ((rc = layer_bwd_transpose_weights(L[l], st))) return rc;
   }
   if ((rc = stack_bwd(L, n, T, dh_top, dout, fc_w, O, w.dh_mid[0], w.dh_mid[1], dx, st))) return rc;
-  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum};
+  const WgradScratch wg{w.gT, w.xT, w.splitk, w.colsum, w.colsum_floats};
   for (int l = n - 1; l >= 0; --l)
     if ((rc = layer_weight_grads(L[l], T, l == 0 ? x : w.L[l - 1].H, g[l].w_ih, g[l].w_hh, g[l].b_ih, g[l].b_hh, wg, st)))
       return rc;
@@ -1457,4 +1489,46 @@ extern "C" int fsn_debug_train_stats(const float* x, int tm, int B, int F, int T
   float2* s = reinterpret_cast<float2*>(sums);
   const cudaStream_t st = (cudaStream_t)stream;
   return tm ? train_tm_stats_launch(x, B, F, T, N, s, st) : train_mag_stats_launch(x, B, F, T, N, s, st);
+}
+
+// ---- unit-test hooks of the fp32 GEMM layer of the training steps (include/fsn_b200.h): each runs the launch function
+// its callers use, every argument checked before any CUDA call
+extern "C" int fsn_debug_sgemm(int ta, const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M,
+                               int N, int K, int accumulate, float* scratch, int64_t scratch_floats, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(A && B && C, FSN_ERR_SHAPE, "sgemm hook: null argument");
+  FSN_REQUIRE(M > 0 && N > 0 && K > 0, FSN_ERR_SHAPE, "sgemm hook: bad shape M=%d N=%d K=%d", M, N, K);
+  FSN_REQUIRE(lda >= (ta ? M : K) && ldb >= N && ldc >= N, FSN_ERR_SHAPE, "sgemm hook: a leading dimension is below its row");
+  FSN_REQUIRE((N + 63) / 64 <= 65535, FSN_ERR_SHAPE, "sgemm hook: N=%d exceeds the grid", N);
+  FSN_REQUIRE(scratch_floats >= 0 && (scratch || scratch_floats == 0), FSN_ERR_WORKSPACE,
+              "sgemm hook: scratch_floats without scratch");
+  return sgemm_launch(ta != 0, A, (size_t)lda, B, (size_t)ldb, C, (size_t)ldc, M, N, K, accumulate != 0, scratch,
+                      (size_t)scratch_floats, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_colsum(const float* X, int64_t rows, int cols, int64_t ldx, float* out, float* out2, float* scratch,
+                                int64_t scratch_floats, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(X && out, FSN_ERR_SHAPE, "colsum hook: null argument");
+  FSN_REQUIRE(rows > 0 && cols > 0 && ldx >= cols, FSN_ERR_SHAPE, "colsum hook: bad shape rows=%lld cols=%d ldx=%lld",
+              (long long)rows, cols, (long long)ldx);
+  FSN_REQUIRE(scratch && scratch_floats > 0, FSN_ERR_WORKSPACE, "colsum hook: no scratch");
+  return colsum_launch(X, (size_t)rows, cols, (size_t)ldx, out, out2, scratch, (size_t)scratch_floats, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_small_out_wgrad(const float* dout, const float* Hm, int64_t rows, int H, float* dW, float* scratch,
+                                         int64_t scratch_floats, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(dout && Hm && dW, FSN_ERR_SHAPE, "small_out_wgrad hook: null argument");
+  FSN_REQUIRE(rows > 0 && H > 0, FSN_ERR_SHAPE, "small_out_wgrad hook: bad shape rows=%lld H=%d", (long long)rows, H);
+  FSN_REQUIRE(scratch && scratch_floats > 0, FSN_ERR_WORKSPACE, "small_out_wgrad hook: no scratch");
+  return small_out_wgrad_launch(dout, Hm, (size_t)rows, H, dW, scratch, (size_t)scratch_floats, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_transpose(const float* in, int64_t rows, int cols, float* out, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(in && out, FSN_ERR_SHAPE, "transpose hook: null argument");
+  FSN_REQUIRE(rows > 0 && cols > 0 && (rows + 31) / 32 < ((int64_t)1 << 31) && (cols + 31) / 32 <= 65535, FSN_ERR_SHAPE,
+              "transpose hook: bad shape rows=%lld cols=%d", (long long)rows, cols);
+  return transpose_launch(in, (size_t)rows, cols, out, (cudaStream_t)stream);
 }

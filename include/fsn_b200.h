@@ -77,7 +77,9 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
  * value of an existing field, refused by every older entry point it does not apply to, with the fsn_debug_forgetting_*
  * hooks.  fsn_improved_weights grew sb_packed, read only by the FSN_PREC_F16X3_TC / FSN_PREC_F16_TC precisions that
  * fsn_improved_forward / _enhance accept since, with fsn_improved_packed_bytes / fsn_improved_pack_sb_weights and the
- * fsn_debug_imp_section_lstm_tc hook: a caller of the shorter struct never selects them, so the version stays 102. */
+ * fsn_debug_imp_section_lstm_tc hook: a caller of the shorter struct never selects them, so the version stays 102.  The
+ * dense GEMM layer's unit-test hooks fsn_debug_fc_gemm, fsn_debug_sgemm, fsn_debug_colsum, fsn_debug_small_out_wgrad,
+ * fsn_debug_transpose, fsn_debug_transpose_blocked and fsn_debug_gemm_tc are new symbols only. */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -680,10 +682,46 @@ int fsn_debug_tgemm_blocked(const float* A, const float* B, float* C, int M, int
  * audio_zen/model/module/sequence_model.py:52-58): z = x W_ih^T (or the projection already in G) + b_ih + b_hh +
  * h_prev W_hh^T; G [R,4H] <- post-activation gates (i,f,g,o), c_out = f c_prev + i g, h_out = o tanh(c_out).
  * h_prev, c_prev nullable (first step); x nullable (G then holds x W_ih^T on entry).  half != 0: fp16 MMA operands
- * (converted into scratch, >= 2 * (2 R H + 4 H (H + K0) + R K0) + 1024 bytes); H % 32 == 0 */
+ * for h and W_hh, and for x and W_ih when K0 % 8 == 0 (else those stay tf32 in the same k loop, as in the training
+ * forward); converted into scratch, >= 2 * (2 R H + 4 H (H + K0) + R K0) + 1024 bytes; H % 32 == 0 */
 int fsn_debug_lstm_fwd_step(const float* h_prev, const float* w_hh, const float* x, const float* w_ih, int K0, float* G,
                             const float* b_ih, const float* b_hh, const float* c_prev, float* c_out, float* h_out, int R,
                             int H, int half, void* scratch, int64_t scratch_bytes, fsn_stream_t stream);
+
+/* unit-test hooks of the dense GEMM layer, each running the launch function its callers use; every argument (null
+ * pointers, non-positive sizes, leading dimensions, short scratch: FSN_ERR_WORKSPACE) is checked before any CUDA call.
+ *   fsn_debug_fc_gemm:   out[M,O] = act(A[M,K] W^T + bias) in fp32 (bias nullable); W [O,K], or [K,O] with w_kmajor
+ *   fsn_debug_sgemm:     C[M,N] (+)= op(A) B in fp32, op(A) = A [M,K] (lda) or, ta != 0, A stored [K,M]; B [K,N] (ldb);
+ *                        long K with few tiles splits K over scratch (fewer slices when scratch_floats is short)
+ *   fsn_debug_colsum:    out[c] (and out2[c] when given) = sum_r X[r*ldx + c]; scratch >= min(ceil(rows/2048), 512) *
+ *                        cols floats
+ *   fsn_debug_small_out_wgrad: dW [2,H] = dout[rows,2]^T Hm[rows,H] (the sub-band Linear's weight gradient); scratch
+ *                        >= 2 H floats (more lets it split the rows)
+ *   fsn_debug_transpose: out [cols,rows] = in [rows,cols]^T
+ *   fsn_debug_transpose_blocked: the block-tiled K-major copy of in [K,M] (row stride ld) that the weight-gradient
+ *                        GEMMs stream: element (k, m) at ((m/128 * ceil(K/32) + k/32) * 128 + m%128) * 32 + k%32, zero
+ *                        padded to whole 128 x 32 tiles; colsum_part (nullable, >= max_slabs * M floats): also the
+ *                        column sums of in into bias_out [M] over at most max_slabs slabs (*slabs, nullable, = count)
+ *   fsn_debug_gemm_tc:   out[rows, :N] (row stride ldo) = act(x' W^T + bias) on the tf32 tensor cores (x3: hi/lo
+ *                        compensated), x' = x[rows, :K] (row stride ldx) times row_scale[r / rows_per_scale] or, with
+ *                        scale_B > 0, row_scale[(r % rows_per_scale) * scale_B + r / rows_per_scale] (row_scale
+ *                        nullable); workspace: the prepared operands, align256(rows Kp p 4) + align256(4 max(8, ceil(N/4)) Kp p 4)
+ *                        bytes with Kp = K rounded up to 4, p = 3 for x3 else 1 (fsn_debug_lstm_tc_workspace_bytes(rows,
+ *                        1, K, max(8, ceil(N/4)), x3) is more than that) */
+int fsn_debug_fc_gemm(const float* A, const float* W, const float* bias, float* out, int M, int K, int O, int act,
+                      int w_kmajor, fsn_stream_t stream);
+int fsn_debug_sgemm(int ta, const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N,
+                    int K, int accumulate, float* scratch, int64_t scratch_floats, fsn_stream_t stream);
+int fsn_debug_colsum(const float* X, int64_t rows, int cols, int64_t ldx, float* out, float* out2, float* scratch,
+                     int64_t scratch_floats, fsn_stream_t stream);
+int fsn_debug_small_out_wgrad(const float* dout, const float* Hm, int64_t rows, int H, float* dW, float* scratch,
+                              int64_t scratch_floats, fsn_stream_t stream);
+int fsn_debug_transpose(const float* in, int64_t rows, int cols, float* out, fsn_stream_t stream);
+int fsn_debug_transpose_blocked(const float* in, int64_t K, int M, int64_t ld, float* out, float* colsum_part,
+                                int max_slabs, int* slabs, float* bias_out, fsn_stream_t stream);
+int fsn_debug_gemm_tc(const float* x, int64_t ldx, int K, const float* row_scale, int rows_per_scale, int scale_B,
+                      const float* W, int N, const float* bias, int act, int x3, float* out, int64_t ldo, int64_t rows,
+                      void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 /* unit-test hooks for the tensor-core LSTM layer of the full-band stacks (fsn_lstm_rec_tc.cu;
  * audio_zen/model/module/sequence_model.py:52-58,117): hall[r,t,:] of nn.LSTM(K -> H, 1 layer) over x [R,T,K]
