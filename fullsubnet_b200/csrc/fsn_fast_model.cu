@@ -48,15 +48,32 @@ struct FastWs {
 
 static bool fast_is_tc(const fsn_fast_desc* d) { return d->precision == FSN_PREC_F16_TC || d->precision == FSN_PREC_F16X3_TC; }
 
-// encoder / decoder pair: LSTM(K0 -> H0), LSTM(H0 -> H1) + Linear(O) over B rows of Tp steps; on the tensor cores with
-// the tensor-core precisions when all three encoder / decoder hidden sizes are supported there
-static SeqStack fast_pair(const fsn_fast_desc* d, const FastDims& m, int K0, int H0, int H1, int O, int act) {
+// encoder / decoder pair over B rows of Tp steps; on the tensor cores with the tensor-core precisions when all three
+// encoder / decoder hidden sizes are supported there.  dec = false: F_l2m, LSTM(M -> He1), LSTM(He1 -> He2) + Linear(M) +
+// ReLU (model.py:35-54,171), per-step scale with the cumulative norm; dec: F_m2l, LSTM(2M -> Hd), LSTM(Hd -> Hd) +
+// Linear(2F) (model.py:77-96,196)
+static SeqStack fast_pair(const fsn_fast_desc* d, int B, int Tp, bool dec) {
   SeqStack s;
   memset(&s, 0, sizeof(s));
-  s.R = m.B; s.Tp = m.Tp; s.K0 = K0; s.n = 2; s.H[0] = H0; s.H[1] = H1; s.O = O; s.act = act;
+  const int M = d->num_mels;
+  s.R = B; s.Tp = Tp; s.n = 2;
+  if (dec) {
+    s.K0 = 2 * M; s.H[0] = s.H[1] = d->dec_hidden; s.O = 2 * d->num_freqs; s.act = FSN_ACT_NONE;
+  } else {
+    s.K0 = M; s.H[0] = d->enc1_hidden; s.H[1] = d->enc2_hidden; s.O = M; s.act = FSN_ACT_RELU;
+    s.step_scale = d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE;
+  }
   s.x3 = fast_x3(d);
   s.tc = fast_is_tc(d) && lstm_rec_tc_supported(d->enc1_hidden, s.x3) && lstm_rec_tc_supported(d->enc2_hidden, s.x3) &&
          lstm_rec_tc_supported(d->dec_hidden, s.x3);
+  return s;
+}
+
+// the encoder and the decoder run one after the other on one stack workspace, carved for the larger of the two
+static SeqStack fast_pair_ws(const fsn_fast_desc* d, int B, int Tp) {
+  auto mx = [](int a, int b) { return a > b ? a : b; };
+  SeqStack s = fast_pair(d, B, Tp, true);
+  s.H[0] = mx(d->enc1_hidden, d->dec_hidden); s.H[1] = mx(d->enc2_hidden, d->dec_hidden); s.O = mx(d->num_mels, s.O);
   return s;
 }
 
@@ -102,9 +119,7 @@ static void fast_carve(const fsn_fast_desc* d, const FastDims& m, void* base, Fa
     w.bn_c0 = c.take<float>(R * d->bn_hidden);
     w.bn_c1 = c.take<float>(R * d->bn_hidden);
   }
-  auto mx = [](int a, int b) { return a > b ? a : b; };
-  seq_stack_carve(c, fast_pair(d, m, 2 * m.M, mx(d->enc1_hidden, d->dec_hidden), mx(d->enc2_hidden, d->dec_hidden),
-                               mx(m.M, 2 * m.F), 0), w.seq);
+  seq_stack_carve(c, fast_pair_ws(d, m.B, m.Tp), w.seq);
   w.bytes = c.off;
 }
 
@@ -156,10 +171,10 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   } else if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)M * Tp, 1.f, w.inv1, nullptr, st))) {
     return rc;
   }
-  // F_l2m: LSTM(M->He1), LSTM(He1->He2) + Linear(M) + ReLU (model.py:35-54,171)
-  SeqStack enc = fast_pair(d, m, M, d->enc1_hidden, d->enc2_hidden, M, FSN_ACT_RELU);
+  // F_l2m (model.py:171)
+  SeqStack enc = fast_pair(d, B, Tp, false);
   enc.L[0] = wt->enc1; enc.L[1] = wt->enc2;
-  enc.x = w.melT; enc.scale = m.cum ? w.cum1 : w.inv1; enc.step_scale = m.cum;
+  enc.x = w.melT; enc.scale = m.cum ? w.cum1 : w.inv1;
   enc.fc_w = wt->enc_fc_w; enc.fc_b = wt->enc_fc_b; enc.out = w.encT;
   if ((rc = seq_stack_forward(enc, w.seq, st))) return rc;
   // bottleneck input: unfold + concat + real-time down-sampling, then its norm (model.py:174-187)
@@ -213,8 +228,8 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   if ((rc = fast_dec_input_launch(w.encT, w.bn_out, (size_t)bn_bstride * m.Ts, m.Ts, 1, B, Tp, M, m.S, m.Ts, Tp, 1, w.dec_in,
                                   st)))
     return rc;
-  // F_m2l: LSTM(2M->Hd), LSTM(Hd->Hd) + Linear(2F) (model.py:77-96,196)
-  SeqStack dec = fast_pair(d, m, 2 * M, d->dec_hidden, d->dec_hidden, 2 * F, FSN_ACT_NONE);
+  // F_m2l (model.py:196)
+  SeqStack dec = fast_pair(d, B, Tp, true);
   dec.L[0] = wt->dec1; dec.L[1] = wt->dec2;
   dec.x = w.dec_in; dec.fc_w = wt->dec_fc_w; dec.fc_b = wt->dec_fc_b; dec.out = w.dec_out;
   if ((rc = seq_stack_forward(dec, w.seq, st))) return rc;
@@ -255,12 +270,10 @@ static int fast_stream_check(const fsn_fast_desc* d, int n_fft, int hop, int win
 
 struct FastStreamWs : StreamWs {
   int* rst;
-  float *melT, *scale1, *encT, *catM, *catE, *bn, *scale2, *bo, *dec_in, *y, *pp;
+  float *melT, *scale1, *encT, *catM, *catE, *bn, *scale2, *bo, *dec_in, *y;
   float2* fs;
-  float *eh[2], *ec[2], *ehall[2];            // encoder state and layer outputs
+  StreamStackWs stack;                        // encoder and decoder, one after the other
   float *bh0[2], *bh1[2], *bc0, *bc1;         // bottleneck state, h ping-pong per layer
-  float *dh[2], *dc[2], *dfh[2], *dfc[2], *dhall[2];  // decoder state (entering the call / after step K-1), outputs
-  unsigned int* barrier;
 };
 
 // St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others; nb = ceil(St / S) bottleneck
@@ -269,17 +282,13 @@ static size_t fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const
                                 FastStreamWs& w) {
   Carver c(base);
   const size_t F = m.F, M = m.M, St = (size_t)K + g.E, Hm = m.S - 1, nb = cdiv((int)St, m.S), R = (size_t)B * M;
-  const size_t He0 = d->enc1_hidden, He1 = d->enc2_hidden, Hb = d->bn_hidden, Hd = d->dec_hidden;
+  const size_t Hb = d->bn_hidden;
   stream_carve(c, g, B, K, m.F, w);
   w.rst = c.take<int>(B);
   w.melT = c.take<float>(B * St * M);
   w.fs = c.take<float2>(B * St);
   w.scale1 = c.take<float>(St * B);
-  for (int l = 0; l < 2; ++l) {
-    const size_t H = l ? He1 : He0;
-    w.eh[l] = c.take<float>(B * H); w.ec[l] = c.take<float>(B * H);
-    w.ehall[l] = c.take<float>(B * St * H);
-  }
+  stream_stack_carve(c, fast_pair_ws(d, B, (int)St), w.stack);
   w.encT = c.take<float>(B * St * M);
   w.catM = c.take<float>(B * (Hm + St) * M);
   w.catE = c.take<float>(B * (Hm + St) * M);
@@ -289,13 +298,6 @@ static size_t fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const
   for (int i = 0; i < 2; ++i) { w.bh0[i] = c.take<float>(R * Hb); w.bh1[i] = c.take<float>(R * Hb); }
   w.bc0 = c.take<float>(R * Hb); w.bc1 = c.take<float>(R * Hb);
   w.dec_in = c.take<float>(B * St * 2 * M);
-  for (int l = 0; l < 2; ++l) {
-    w.dh[l] = c.take<float>(B * Hd); w.dc[l] = c.take<float>(B * Hd);
-    w.dfh[l] = c.take<float>(B * Hd); w.dfc[l] = c.take<float>(B * Hd);
-    w.dhall[l] = c.take<float>(B * St * Hd);
-  }
-  w.pp = c.take<float>((size_t)2 * 256 * Hd);  // fb::ROWS rows of the persistent kernel's h0 ping-pong
-  w.barrier = c.take<unsigned int>(64);
   w.y = c.take<float>(B * St * 2 * F);
   return c.off;
 }
@@ -479,20 +481,19 @@ extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weigh
   char* sb = (char*)state;
   const size_t ss = sl.slot();
   const int F = m.F, M = m.M, S = m.S, Kf = m.K, Hm = S - 1, R = B * M, nb = cdiv(St, S);
-  const int Hb = d->bn_hidden, Hd = d->dec_hidden;
+  const int Hb = d->bn_hidden;
   const size_t catw = (size_t)(Hm + St) * M * 4;
   if ((rc = stream_open(g, sl, w, F, B, K, St, win_length, start, tail, wav, sb, nullptr, st))) return rc;
   // Mel filtering and the first norm over the mel frame sums (model.py:161-170)
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, B * St, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true))) return rc;
   if ((rc = frame_stats_launch(w.melT, B, St, M, 0, (size_t)St * M, M, w.fs, st))) return rc;
   if ((rc = stream_norm_launch(w.fs, B, St, K, M, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale1, st))) return rc;
-  // encoder: the per-step kernels the whole-clip call runs for its per-step scale, (h, c) carried; Linear(M) + ReLU
-  const fsn_lstm_layer enc[2] = {wt->enc1, wt->enc2};
-  const int He[2] = {d->enc1_hidden, d->enc2_hidden};
-  if ((rc = stream_lstm_layers(enc, 2, He, M, w.melT, w.scale1, B, St, K, g, w.pos0, sb, ss, sl.eh, sl.ec, w.eh, w.ec,
-                               w.ehall, st)))
-    return rc;
-  if ((rc = fc_gemm_launch(w.ehall[1], wt->enc_fc_w, wt->enc_fc_b, w.encT, B * St, He[1], M, FSN_ACT_RELU, st))) return rc;
+  // encoder, (h, c) carried; its per-step scale keeps it off the paths that read the restart table, which
+  // fast_stream_open_kernel writes only later in the call
+  SeqStack enc = fast_pair(d, B, St, false);
+  enc.L[0] = wt->enc1; enc.L[1] = wt->enc2;
+  enc.x = w.melT; enc.scale = w.scale1; enc.fc_w = wt->enc_fc_w; enc.fc_b = wt->enc_fc_b; enc.out = w.encT;
+  if ((rc = stream_seq_stack(enc, w.stack, StackCarry{sb, ss, sl.eh, sl.ec, w.pos0, g, nullptr, K}, st))) return rc;
   // the carried S-1 frames, then the call's, of the mel spectrogram and the encoder output: the frames the blocks average
   if (Hm > 0) {
     if ((rc = copy_rows(w.catM, catw, sb + sl.mel, ss, (size_t)Hm * M * 4, B, st))) return rc;
@@ -538,40 +539,11 @@ extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weigh
   fast_stream_dec_input_kernel<<<ew_grid((size_t)B * St * 2 * M), 256, 0, st>>>(w.encT, w.bo, w.pos0, hop, g.c, B, St, M, S,
                                                                                  nb, w.dec_in);
   FSN_CHECK_LAUNCH("fast_stream_dec_input_kernel");
-  // decoder on the path seq_stack_forward takes for this stack shape, (h, c) carried; then Linear(2F)
-  SeqStack dec;
-  memset(&dec, 0, sizeof(dec));
-  dec.R = B; dec.Tp = St; dec.K0 = 2 * M; dec.n = 2; dec.H[0] = Hd; dec.H[1] = Hd; dec.O = 2 * F;
-  const fsn_lstm_layer dl[2] = {wt->dec1, wt->dec2};
-  const int Hdl[2] = {Hd, Hd};
-  if (seq_stack_path(dec) == SEQ_PATH_PERSISTENT) {
-    // the state entering the call (zero for a clip whose frame 0 is step 0; a later frame 0 restarts inside the kernel),
-    // stored after step K - 1
-    for (int l = 0; l < 2; ++l) {
-      const size_t hb = (size_t)Hd * 4, lo = (size_t)l * hb;
-      if ((rc = copy_rows(w.dh[l], hb, sb + sl.dh + lo, ss, hb, B, st))) return rc;
-      if ((rc = copy_rows(w.dc[l], hb, sb + sl.dc + lo, ss, hb, B, st))) return rc;
-      if ((rc = stream_reset_launch(w.pos0, B, g, 0, Hd, w.dh[l], Hd, w.dc[l], st))) return rc;
-    }
-    FbState io;
-    memset(&io, 0, sizeof(io));
-    for (int l = 0; l < 2; ++l) {
-      io.h_init[l] = w.dh[l]; io.c_init[l] = w.dc[l]; io.h_fin[l] = w.dfh[l]; io.c_fin[l] = w.dfc[l];
-    }
-    io.restart = w.rst;
-    io.fin_step = K - 1;
-    if ((rc = fb_persistent_launch(dl, w.dec_in, nullptr, w.pp, w.dhall[1], w.barrier, B, 2 * M, Hd, Hd, St, st, &io)))
-      return rc;
-    for (int l = 0; l < 2; ++l) {
-      const size_t hb = (size_t)Hd * 4, lo = (size_t)l * hb;
-      if ((rc = copy_rows(sb + sl.dh + lo, ss, w.dfh[l], hb, hb, B, st))) return rc;
-      if ((rc = copy_rows(sb + sl.dc + lo, ss, w.dfc[l], hb, hb, B, st))) return rc;
-    }
-  } else if ((rc = stream_lstm_layers(dl, 2, Hdl, 2 * M, w.dec_in, nullptr, B, St, K, g, w.pos0, sb, ss, sl.dh, sl.dc, w.dh,
-                                      w.dc, w.dhall, st))) {
-    return rc;
-  }
-  if ((rc = fc_gemm_launch(w.dhall[1], wt->dec_fc_w, wt->dec_fc_b, w.y, B * St, Hd, 2 * F, FSN_ACT_NONE, st))) return rc;
+  // decoder, (h, c) carried, restarting at rst
+  SeqStack dec = fast_pair(d, B, St, true);
+  dec.L[0] = wt->dec1; dec.L[1] = wt->dec2;
+  dec.x = w.dec_in; dec.fc_w = wt->dec_fc_w; dec.fc_b = wt->dec_fc_b; dec.out = w.y;
+  if ((rc = stream_seq_stack(dec, w.stack, StackCarry{sb, ss, sl.dh, sl.dc, w.pos0, g, w.rst, K}, st))) return rc;
   // carry the last S-1 frames of the mel spectrogram and the encoder output as of step K
   if (Hm > 0) {
     if ((rc = copy_rows(sb + sl.mel, ss, w.catM + (size_t)K * M, catw, (size_t)Hm * M * 4, B, st))) return rc;

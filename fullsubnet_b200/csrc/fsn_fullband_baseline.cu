@@ -34,10 +34,10 @@ static int fbb_check(const fsn_fullband_desc* d, int B, int T) {
 
 // num_layers x LSTM(F -> H) + Linear(H -> 2F), rows = clips, fp32 kernels (also for the training precision
 // FSN_PREC_TF32_TC).  The path does not depend on B, so a clip gets the same bits in any batch.
-static SeqStack fbb_stack(const fsn_fullband_desc* d, int B, int T) {
+static SeqStack fbb_stack(const fsn_fullband_desc* d, int B, int Tp) {
   SeqStack s;
   memset(&s, 0, sizeof(s));
-  s.R = B; s.Tp = T + d->look_ahead; s.K0 = d->num_freqs; s.n = d->num_layers; s.O = 2 * d->num_freqs; s.act = d->activation;
+  s.R = B; s.Tp = Tp; s.K0 = d->num_freqs; s.n = d->num_layers; s.O = 2 * d->num_freqs; s.act = d->activation;
   for (int l = 0; l < s.n; ++l) s.H[l] = d->hidden;
   s.step_scale = norm_per_step(d->norm_type);
   return s;
@@ -52,7 +52,7 @@ static void fbb_carve(const fsn_fullband_desc* d, int B, int T, void* base, FbbW
   w.sums = c.take<float2>(B);
   w.inv1 = c.take<float>(B);
   w.cum1 = c.take<float>(B * Tp);
-  seq_stack_carve(c, fbb_stack(d, B, T), w.seq);
+  seq_stack_carve(c, fbb_stack(d, B, (int)Tp), w.seq);
   w.y = c.take<float>(B * Tp * 2 * F);
   if (enhance) wav_carve(c, B, (int)F, T, w.wav);
   w.bytes = c.off;
@@ -72,7 +72,7 @@ static int fbb_core(const fsn_fullband_desc* d, const fsn_lstm_layer* layers, co
     return rc;
   if (cum && (rc = cum_clip_scale_launch(w.fs, B, Tp, F, 1.1920928955078125e-07f, w.cum1, st))) return rc;
   if (fgt && (rc = forget_scale_launch(w.fs, nullptr, B, Tp, (float)F, w.cum1, nullptr, st))) return rc;
-  SeqStack s = fbb_stack(d, B, T);
+  SeqStack s = fbb_stack(d, B, Tp);
   for (int l = 0; l < s.n; ++l) s.L[l] = layers[l];
   s.x = w.magT; s.scale = (cum || fgt) ? w.cum1 : w.inv1; s.fc_w = fc_w; s.fc_b = fc_b; s.out = w.y;
   if ((rc = seq_stack_forward(s, w.seq, st))) return rc;
@@ -182,18 +182,17 @@ static int fbb_stream_check(const fsn_fullband_desc* d, int n_fft, int hop, int 
 struct FbbStreamWs : StreamWs {
   float *scale, *y;
   float2* fs;
-  float *h[SEQ_MAX_LAYERS], *c[SEQ_MAX_LAYERS], *hall[2];
+  StreamStackWs stack;
 };
 
 // St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others; returns the bytes
 static size_t fbb_stream_carve(const fsn_fullband_desc* d, const StreamGeom& g, int B, int K, void* base, FbbStreamWs& w) {
   Carver c(base);
-  const size_t H = d->hidden, St = (size_t)K + g.E;
+  const size_t St = (size_t)K + g.E;
   stream_carve(c, g, B, K, d->num_freqs, w);
   w.fs = c.take<float2>(B * St);
   w.scale = c.take<float>(St * B);
-  for (int l = 0; l < d->num_layers; ++l) { w.h[l] = c.take<float>(B * H); w.c[l] = c.take<float>(B * H); }
-  w.hall[0] = c.take<float>(B * St * H); w.hall[1] = c.take<float>(B * St * H);
+  stream_stack_carve(c, fbb_stack(d, B, (int)St), w.stack);
   w.y = c.take<float>(B * St * 2 * d->num_freqs);
   return c.off;
 }
@@ -234,17 +233,15 @@ extern "C" int fsn_fullband_stream_step(const fsn_fullband_desc* d, const fsn_ls
   const cudaStream_t st = (cudaStream_t)stream;
   char* sb = (char*)state;
   const size_t ss = sl.slot();
-  const int F = d->num_freqs, H = d->hidden, n = d->num_layers;
+  const int F = d->num_freqs;
   if ((rc = stream_open(g, sl, w, F, B, K, St, win_length, start, tail, wav, sb, nullptr, st))) return rc;
   // first norm (fbb_core): frame sums, then the running scale of each step
   if ((rc = frame_stats_launch(w.magT, B, St, F, 0, (size_t)St * F, F, w.fs, st))) return rc;
   if ((rc = stream_norm_launch(w.fs, B, St, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale, st))) return rc;
-  // the stack on the per-step kernels seq_stack_forward runs for the causal norms, (h, c) carried in the slot state
-  int Hs[SEQ_MAX_LAYERS];
-  for (int l = 0; l < n; ++l) Hs[l] = H;
-  if ((rc = stream_lstm_layers(layers, n, Hs, F, w.magT, w.scale, B, St, K, g, w.pos0, sb, ss, sl.h, sl.c, w.h, w.c,
-                               w.hall, st)))
-    return rc;
-  if ((rc = fc_gemm_launch(w.hall[(n - 1) & 1], fc_w, fc_b, w.y, B * St, H, 2 * F, d->activation, st))) return rc;
+  // the stack, (h, c) carried in the slot state; its per-step scale keeps it off the paths that read a restart table
+  SeqStack s = fbb_stack(d, B, St);
+  for (int l = 0; l < s.n; ++l) s.L[l] = layers[l];
+  s.x = w.magT; s.scale = w.scale; s.fc_w = fc_w; s.fc_b = fc_b; s.out = w.y;
+  if ((rc = stream_seq_stack(s, w.stack, StackCarry{sb, ss, sl.h, sl.c, w.pos0, g, nullptr, K}, st))) return rc;
   return stream_close(g, sl, w, F, B, K, St, win_length, w.y, enhanced, sb, st);
 }

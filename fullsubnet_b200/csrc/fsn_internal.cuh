@@ -569,14 +569,20 @@ int stft_stream_launch(const float* win, int Wn, int Hs, const int* pos0, const 
 int istft_stream_launch(const float* spec, const float* crm, const int* pos0, const int* act0, const int* tail, int B,
                         int K, int D, int n_fft, int hop, int win_length, int c, int la, int Rc, int Q, int S, float* wav,
                         cudaStream_t st);
-// n LSTM layers (hidden sizes H[l]) over the call's S steps on the per-step kernels, as seq_stack_forward runs a stack with
-// a per-step scale: layer 0 reads x [B, S, K0] times scaleT[j*B + b] (nullable), layer l writes h of every step to
-// hall[l & 1] [B, S, H[l]].  Layer l's (h, c) start from the slot state (h at h_off, c at c_off bytes into each block, the
-// layers one after the other) through h[l] / c[l] [B, H[l]], are zeroed at a clip's frame 0 and are stored back after
-// step K - 1
-int stream_lstm_layers(const fsn_lstm_layer* L, int n, const int* H, int K0, const float* x, const float* scaleT, int B,
-                       int S, int K, const StreamGeom& g, const int* pos0, char* state, size_t slot_bytes, size_t h_off,
-                       size_t c_off, float* const* h, float* const* c, float* const* hall, cudaStream_t st);
+// An LSTM SequenceModel over a streaming call (R = B slots, Tp = the call's St steps, from the whole-clip call's builder)
+// with each layer's (h, c) carried in the slot state, on the path seq_stack_path picks for the whole-clip stack, so a clip
+// streams to the whole-clip bits.  TC: lstm_layer_tc with RecCarry, then linear_tc.  PERSISTENT: layers 0-1 on
+// fb_persistent_launch with FbState.  Otherwise, and for layers past the second, one layer after the other on the
+// per-step kernels, (h, c) zeroed before the step that is a clip's frame 0.  (h, c) after step K - 1 go back to the
+// state.  Layer l's h / c are at the h / c byte offsets of each slot's block plus the floats of the layers below.
+// restart (slot b's frame-0 step, stream_restart_launch) is read on the TC and persistent paths only: a stream whose
+// stacks always have a per-step scale (fullband_baseline, fast_fullsubnet's encoder) never takes them and passes none.
+struct StackCarry { char* state; size_t slot, h, c; const int* pos0; StreamGeom g; const int* restart; int K; };
+// seq_stack_carve plus what only the carry needs: the per-step layers' output ping-pong and entering h (their c in
+// seq.c0), the persistent kernel's (h, c) after step K - 1 (its entering state goes to seq.h0 / c0 / c1)
+struct StreamStackWs { SeqStackWs seq; float* h; float *h_fin[2], *c_fin[2]; };
+void stream_stack_carve(Carver& c, const SeqStack& s, StreamStackWs& w);
+int stream_seq_stack(const SeqStack& s, const StreamStackWs& w, const StackCarry& io, cudaStream_t st);
 // rows of `width` bytes: dst row b (pitch dp) <- src row b (pitch sp), B rows, on the stream
 int copy_rows(void* dst, size_t dp, const void* src, size_t sp, size_t width, int B, cudaStream_t st);
 

@@ -45,13 +45,14 @@ struct ModelWs {
   size_t bytes;
 };
 
-// full-band stack (model.py:92-95): 2-layer LSTM / GRU (F -> Hf -> Hf) + Linear(Hf -> F), rows = clips.  On the tensor
-// cores with the tensor-core precisions and LSTM, for every batch size, so a clip's result does not depend on the batch
-// it is enhanced in.
-static SeqStack fb_stack(const fsn_model_desc* d, const Dims& m) {
+// full-band stack (model.py:92-95): 2-layer LSTM / GRU (F -> Hf -> Hf) + Linear(Hf -> F), rows = B clips of Tp steps.
+// On the tensor cores with the tensor-core precisions and LSTM, for every batch size, so a clip's result does not depend
+// on the batch it is enhanced in.
+static SeqStack fb_stack(const fsn_model_desc* d, int B, int Tp) {
   SeqStack s;
   memset(&s, 0, sizeof(s));
-  s.R = m.B; s.Tp = m.Tp; s.K0 = m.F; s.n = 2; s.H[0] = s.H[1] = d->fb_hidden; s.O = m.F; s.act = d->fb_activation;
+  const int F = d->num_freqs;
+  s.R = B; s.Tp = Tp; s.K0 = F; s.n = 2; s.H[0] = s.H[1] = d->fb_hidden; s.O = F; s.act = d->fb_activation;
   s.gru = d->cell_type == FSN_CELL_GRU;
   s.step_scale = norm_per_step(d->norm_type);
   s.x3 = d->precision == FSN_PREC_F16X3_TC;
@@ -95,7 +96,7 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
   w.sums_fb = c.take<float2>(m.B);
   w.inv1 = c.take<float>(m.B);
   w.inv2 = c.take<float>(m.B);
-  seq_stack_carve(c, fb_stack(d, m), w.fb);
+  seq_stack_carve(c, fb_stack(d, m.B, m.Tp), w.fb);
   if (d->precision == FSN_PREC_FP32) {
     const size_t RH = (size_t)m.R * d->sb_hidden;
     for (int i = 0; i < 2; ++i) { w.sb_h0[i] = c.take<float>(RH); w.sb_h1[i] = c.take<float>(RH); }
@@ -135,7 +136,7 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
 
   // ---- full-band stack -> fbT [B, Tp, F]; x = magT * 1/(mu + 1e-5) of the clip (model.py:92) or, cumulative norm, the
   // scale of (step, clip) from the time-major table cum1[t*B + b] (base_model.py:220-251), or the forgetting norm's
-  SeqStack s = fb_stack(d, m);
+  SeqStack s = fb_stack(d, B, Tp);
   s.L[0] = seq_layer(*fb, 0); s.L[1] = seq_layer(*fb, 1);
   s.x = w.magT; s.scale = (cum || fgt) ? w.cum1 : w.inv1; s.fc_w = fb->fc_w; s.fc_b = fb->fc_b; s.out = w.fbT;
   if ((rc = seq_stack_forward(s, w.fb, st))) return rc;
@@ -383,54 +384,36 @@ struct FsnStreamWs : StreamWs {
   int* restart;
   float *scale1, *fbT, *scale2, *unit;
   float2 *fs, *fs2;
-  float *fh[2], *fc[2], *fhall[2];       // full-band state and layer outputs
+  StreamStackWs fb;                      // full band
   float *sh0[2], *sh1[2], *sc0, *sc1;    // sub-band state, h ping-pong per layer (fp32 stream)
-  LstmTcWs ftc;                          // tensor-core full band (tensor-core stream on SEQ_PATH_TC)
 };
 
-// the full-band stack of a call over B slots and St steps, as the whole-clip call builds it (fb_stack)
-static SeqStack fsn_stream_fb(const fsn_model_desc* d, int B, int St) {
-  Dims m;
-  memset(&m, 0, sizeof(m));
-  m.B = B; m.Tp = St; m.F = d->num_freqs;
-  return fb_stack(d, m);
-}
-
 // St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others.  tc: the sub band's state
-// stays in the slot state (no per-row buffers), the full band gets the tensor-core workspace when it runs there.
-// Returns the bytes
+// stays in the slot state (no per-row buffers).  Returns the bytes
 static size_t fsn_stream_carve(const fsn_model_desc* d, const StreamGeom& g, int B, int K, void* base, FsnStreamWs& w,
                                bool tc) {
   Carver c(base);
-  const size_t F = d->num_freqs, Hf = d->fb_hidden, St = (size_t)K + g.E, RH = (size_t)B * F * d->sb_hidden;
+  const size_t F = d->num_freqs, St = (size_t)K + g.E, RH = (size_t)B * F * d->sb_hidden;
   stream_carve(c, g, B, K, d->num_freqs, w);
   w.restart = tc ? c.take<int>(B) : nullptr;
   w.fs = c.take<float2>(B * St);
   w.fs2 = d->norm_type == FSN_NORM_FORGETTING ? c.take<float2>(B * St) : nullptr;
   w.scale1 = c.take<float>(St * B);
-  for (int l = 0; l < 2; ++l) {
-    w.fh[l] = c.take<float>(B * Hf); w.fc[l] = c.take<float>(B * Hf);
-    w.fhall[l] = c.take<float>(B * St * Hf);
-  }
+  stream_stack_carve(c, fb_stack(d, B, (int)St), w.fb);
   w.fbT = c.take<float>(B * St * F);
   w.scale2 = d->norm_type == FSN_NORM_FORGETTING ? c.take<float>(St * B) : nullptr;
   w.unit = c.take<float>(St * B * F);
-  memset(&w.ftc, 0, sizeof(w.ftc));
   memset(w.sh0, 0, sizeof(w.sh0)); memset(w.sh1, 0, sizeof(w.sh1));
   w.sc0 = w.sc1 = nullptr;
   if (!tc) {
     for (int i = 0; i < 2; ++i) { w.sh0[i] = c.take<float>(RH); w.sh1[i] = c.take<float>(RH); }
     w.sc0 = c.take<float>(RH); w.sc1 = c.take<float>(RH);
-  } else if (fsn_stream_fb(d, B, (int)St).tc) {
-    const int Hw = (int)Hf > cdiv((int)F, 4) ? (int)Hf : cdiv((int)F, 4);  // the Linear's prepared weights share the rows
-    lstm_tc_carve(c, (size_t)B * St, (int)(F > Hf ? F : Hf), Hw, d->precision == FSN_PREC_F16X3_TC, w.ftc);
   }
   return c.off;
 }
 
-// one call of either stream.  tc: the full band on the tensor cores where the whole-clip call runs it there
-// (SEQ_PATH_TC: lstm_layer_tc per layer with carried (h, c), then linear_tc), else on the per-step kernels as the fp32
-// stream; the sub band in one sb_carry_lstm_tc_kernel launch over all St steps
+// one call of either stream.  The full band on the kernels of the whole-clip call (stream_seq_stack); tc: the sub band in
+// one sb_carry_lstm_tc_kernel launch over all St steps
 static int fsn_stream_run(const fsn_model_desc* d, const fsn_seq_weights* fb, const fsn_seq_weights* sb,
                           const void* sb_packed, bool tc, const float* wav, const int32_t* start, const int32_t* tail,
                           int B, int K, int n_fft, int hop, int win_length, float* enhanced, void* state,
@@ -451,7 +434,7 @@ static int fsn_stream_run(const fsn_model_desc* d, const fsn_seq_weights* fb, co
   if ((rc = stream_check_sizes(state, state_bytes, sl.slot(), B, workspace, workspace_bytes, ws))) return rc;
   char* sbase = (char*)state;
   const size_t ss = sl.slot();
-  const int F = m.F, Hf = d->fb_hidden, Hs = d->sb_hidden, Ns = d->sb_num_neighbors, Nf = d->fb_num_neighbors;
+  const int F = m.F, Hs = d->sb_hidden, Ns = d->sb_num_neighbors, Nf = d->fb_num_neighbors;
   const int R = B * F;
   const bool fgt = d->norm_type == FSN_NORM_FORGETTING, x3 = d->precision == FSN_PREC_F16X3_TC;
   const size_t F2 = 2 * (size_t)F;
@@ -460,31 +443,12 @@ static int fsn_stream_run(const fsn_model_desc* d, const fsn_seq_weights* fb, co
   if ((rc = frame_stats_launch(w.magT, B, St, F, Ns, (size_t)St * F, F, w.fs, st))) return rc;
   if ((rc = stream_norm_launch(w.fs, B, St, K, F, g, d->norm_type, w.pos0, w.act0, w.tail, sbase, ss, w.scale1, st)))
     return rc;
-  const fsn_lstm_layer fl[2] = {seq_layer(*fb, 0), seq_layer(*fb, 1)};
-  if (tc && seq_stack_path(fsn_stream_fb(d, B, St)) == SEQ_PATH_TC) {
-    // full band as seq_stack_forward runs it on the tensor cores over the call's B*St rows, per-(step, clip) scale;
-    // each layer's (h, c) from the state, c stored after step K - 1 by the recurrence, h from its output at K - 1
-    for (int l = 0; l < 2; ++l) {
-      float* fh = (float*)(sbase + sl.fbh) + (size_t)l * Hf;
-      float* fc = (float*)(sbase + sl.fbc) + (size_t)l * Hf;
-      const RecCarry io{fh, fc, fc, ss / 4, w.restart, K - 1};
-      const int Kl = l ? Hf : F;
-      if ((rc = lstm_layer_tc(fl[l], l ? w.fhall[0] : w.magT, (size_t)Kl, Kl, l ? nullptr : w.scale1, St, l ? 0 : B, B, St,
-                              Hf, x3, w.ftc, w.fhall[l], st, &io)))
-        return rc;
-      if ((rc = copy_rows(fh, ss, w.fhall[l] + (size_t)(K - 1) * Hf, (size_t)St * Hf * 4, (size_t)Hf * 4, B, st))) return rc;
-    }
-    if ((rc = linear_tc(w.fhall[1], (size_t)Hf, Hf, fb->fc_w, fb->fc_b, F, d->fb_activation, w.fbT, (size_t)F,
-                        (size_t)B * St, x3, w.ftc, st)))
-      return rc;
-  } else {
-    // full band on the per-step kernels seq_stack_forward runs for the per-step scale, (h, c) carried; Linear(F) + act
-    const int Hfl[2] = {Hf, Hf};
-    if ((rc = stream_lstm_layers(fl, 2, Hfl, F, w.magT, w.scale1, B, St, K, g, w.pos0, sbase, ss, sl.fbh, sl.fbc, w.fh,
-                                 w.fc, w.fhall, st)))
-      return rc;
-    if ((rc = fc_gemm_launch(w.fhall[1], fb->fc_w, fb->fc_b, w.fbT, B * St, Hf, F, d->fb_activation, st))) return rc;
-  }
+  // full band, (h, c) carried; only the tensor-core stream has a restart table, and only its stack can take a path that
+  // reads one (the fp32 stream's per-step scale keeps it on the per-step kernels)
+  SeqStack fbs = fb_stack(d, B, St);
+  fbs.L[0] = seq_layer(*fb, 0); fbs.L[1] = seq_layer(*fb, 1);
+  fbs.x = w.magT; fbs.scale = w.scale1; fbs.fc_w = fb->fc_w; fbs.fc_b = fb->fc_b; fbs.out = w.fbT;
+  if ((rc = stream_seq_stack(fbs, w.fb, StackCarry{sbase, ss, sl.fbh, sl.fbc, w.pos0, g, w.restart, K}, st))) return rc;
   // second norm, one scale per (step, row), rows b*F + f
   const RowMap map{B, F, F, 1};
   if (fgt) {

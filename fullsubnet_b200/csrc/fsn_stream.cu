@@ -247,42 +247,101 @@ int stream_restart_launch(const int* pos0, int B, const StreamGeom& g, int* rest
   return FSN_OK;
 }
 
-int stream_lstm_layers(const fsn_lstm_layer* L, int n, const int* H, int K0, const float* x, const float* scaleT, int B,
-                       int S, int K, const StreamGeom& g, const int* pos0, char* state, size_t slot_bytes, size_t h_off,
-                       size_t c_off, float* const* h, float* const* c, float* const* hall, cudaStream_t st) {
+void stream_stack_carve(Carver& c, const SeqStack& s, StreamStackWs& w) {
+  seq_stack_carve(c, s, w.seq);
+  int Hm = 0;
+  for (int l = 0; l < s.n; ++l) Hm = s.H[l] > Hm ? s.H[l] : Hm;
+  // seq_stack_carve's conditions: seq_stack_forward keeps only the top layer's output of a two-layer stack off the
+  // tensor cores, and the persistent kernel runs stacks of two or more LSTM layers without a per-step scale
+  if (s.n == 2 && !s.tc) w.seq.hall[1] = c.take<float>((size_t)s.R * s.Tp * Hm);
+  w.h = (s.n >= 2 && s.H[0] == Hm) ? w.seq.h0[0] : c.take<float>((size_t)s.R * Hm);
+  w.h_fin[0] = w.h_fin[1] = w.c_fin[0] = w.c_fin[1] = nullptr;
+  for (int l = 0; s.n >= 2 && !s.gru && !s.step_scale && l < 2; ++l) {
+    w.h_fin[l] = c.take<float>((size_t)s.R * s.H[l]);
+    w.c_fin[l] = c.take<float>((size_t)s.R * s.H[l]);
+  }
+}
+
+int stream_seq_stack(const SeqStack& s, const StreamStackWs& w, const StackCarry& io, cudaStream_t st) {
+  const SeqPath path = seq_stack_path(s);
+  const int R = s.R, S = s.Tp, n = s.n, Ht = s.H[n - 1];
+  auto hall = [&](int l) { return w.seq.hall[(n - 1 - l) & 1]; };  // as in seq_stack_forward: the top one in hall[0]
+  // layer l's h / c section in slot 0's block
+  auto sec = [&](size_t off, int l) {
+    size_t f = 0;
+    for (int i = 0; i < l; ++i) f += s.H[i];
+    return io.state + off + f * 4;
+  };
   int rc;
-  size_t off = 0;  // floats of the layers below in the h and c sections
-  for (int l = 0; l < n; ++l) {
-    const int Hl = H[l];
-    float* hl = hall[l & 1];
+  FSN_REQUIRE(io.restart || (path != SEQ_PATH_TC && path != SEQ_PATH_PERSISTENT), FSN_ERR_UNSUPPORTED,
+              "stream: the stack's path (%d) restarts inside its kernels and the stream gives no restart table", (int)path);
+  if (path == SEQ_PATH_TC) {
+    for (int l = 0; l < n; ++l) {
+      const int K = l ? s.H[l - 1] : s.K0, Hl = s.H[l];
+      float* h = (float*)sec(io.h, l);
+      float* c = (float*)sec(io.c, l);
+      const RecCarry carry{h, c, c, io.slot / 4, io.restart, io.K - 1};
+      if ((rc = lstm_layer_tc(s.L[l], l ? hall(l - 1) : s.x, (size_t)K, K, l ? nullptr : s.scale, S,
+                              (!l && s.step_scale) ? R : 0, R, S, Hl, s.x3, w.seq.tc, hall(l), st, &carry)))
+        return rc;
+      if ((rc = copy_rows(h, io.slot, hall(l) + (size_t)(io.K - 1) * Hl, (size_t)S * Hl * 4, (size_t)Hl * 4, R, st)))
+        return rc;
+    }
+    return linear_tc(hall(n - 1), (size_t)Ht, Ht, s.fc_w, s.fc_b, s.O, s.act, s.out, (size_t)s.O, (size_t)R * S, s.x3,
+                     w.seq.tc, st);
+  }
+  int l = 0;  // first layer left for the per-step loop
+  if (path == SEQ_PATH_PERSISTENT) {
+    // the state entering the call (zero for a clip whose frame 0 is step 0; a later frame 0 restarts inside the kernel)
+    float* h_init[2] = {w.seq.h0[0], w.seq.c0};
+    float* c_init[2] = {w.seq.h0[1], w.seq.c1};
+    for (int i = 0; i < 2; ++i) {
+      const size_t hb = (size_t)s.H[i] * 4;
+      if ((rc = copy_rows(h_init[i], hb, sec(io.h, i), io.slot, hb, R, st))) return rc;
+      if ((rc = copy_rows(c_init[i], hb, sec(io.c, i), io.slot, hb, R, st))) return rc;
+      if ((rc = stream_reset_launch(io.pos0, R, io.g, 0, s.H[i], h_init[i], s.H[i], c_init[i], st))) return rc;
+    }
+    const FbState fs{{h_init[0], h_init[1]}, {c_init[0], c_init[1]}, {w.h_fin[0], w.h_fin[1]}, {w.c_fin[0], w.c_fin[1]},
+                     io.restart, io.K - 1};
+    if ((rc = fb_persistent_launch(s.L, s.x, s.scale, w.seq.pp, hall(1), w.seq.barrier, R, s.K0, s.H[0], s.H[1], S, st, &fs)))
+      return rc;
+    for (int i = 0; i < 2; ++i) {
+      const size_t hb = (size_t)s.H[i] * 4;
+      if ((rc = copy_rows(sec(io.h, i), io.slot, w.h_fin[i], hb, hb, R, st))) return rc;
+      if ((rc = copy_rows(sec(io.c, i), io.slot, w.c_fin[i], hb, hb, R, st))) return rc;
+    }
+    l = 2;
+  }
+  for (; l < n; ++l) {
+    const int Hl = s.H[l];
+    float* hl = hall(l);
     const size_t hrow = (size_t)S * Hl, hb = (size_t)Hl * 4;
-    char* sh = state + h_off + off * 4;
-    char* sc = state + c_off + off * 4;
-    if ((rc = copy_rows(h[l], hb, sh, slot_bytes, hb, B, st))) return rc;
-    if ((rc = copy_rows(c[l], hb, sc, slot_bytes, hb, B, st))) return rc;
+    char* sh = sec(io.h, l);
+    char* sc = sec(io.c, l);
+    if ((rc = copy_rows(w.h, hb, sh, io.slot, hb, R, st))) return rc;
+    if ((rc = copy_rows(w.seq.c0, hb, sc, io.slot, hb, R, st))) return rc;
     for (int j = 0; j < S; ++j) {
-      float* hp = j ? hl + (size_t)(j - 1) * Hl : h[l];
-      if (j <= g.c && (rc = stream_reset_launch(pos0, B, g, j, Hl, hp, j ? hrow : (size_t)Hl, c[l], st))) return rc;
+      float* hp = j ? hl + (size_t)(j - 1) * Hl : w.h;
+      if (j <= io.g.c && (rc = stream_reset_launch(io.pos0, R, io.g, j, Hl, hp, j ? hrow : (size_t)Hl, w.seq.c0, st)))
+        return rc;
       StepParams p;
       memset(&p, 0, sizeof(p));
-      p.R = B; p.H = Hl; p.first = 0; p.gru = 0;
-      p.w_ih = L[l].w_ih; p.w_hh = L[l].w_hh; p.b_ih = L[l].b_ih; p.b_hh = L[l].b_hh;
-      p.K0 = l ? H[l - 1] : K0;
-      p.x0 = l ? hall[(l - 1) & 1] + (size_t)j * H[l - 1] : x + (size_t)j * K0;
-      p.x0_row_stride = (size_t)S * p.K0;
-      p.row_scale = (l || !scaleT) ? nullptr : scaleT + (size_t)j * B;
+      p.R = R; p.H = Hl; p.first = 0; p.gru = 0;
+      p.w_ih = s.L[l].w_ih; p.w_hh = s.L[l].w_hh; p.b_ih = s.L[l].b_ih; p.b_hh = s.L[l].b_hh;
+      p.K0 = l ? s.H[l - 1] : s.K0;
+      p.x0 = (l ? hall(l - 1) : s.x) + (size_t)j * p.K0; p.x0_row_stride = (size_t)S * p.K0;
+      if (!l) p.row_scale = (s.scale && s.step_scale) ? s.scale + (size_t)j * R : s.scale;
       p.h_prev = hp; p.h_prev_stride = j ? hrow : (size_t)Hl;
       p.h_out = hl + (size_t)j * Hl; p.h_out_stride = hrow;
-      p.c = c[l];
+      p.c = w.seq.c0;
       if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-      if (j == K - 1) {
-        if ((rc = copy_rows(sh, slot_bytes, p.h_out, hrow * 4, hb, B, st))) return rc;
-        if ((rc = copy_rows(sc, slot_bytes, c[l], hb, hb, B, st))) return rc;
+      if (j == io.K - 1) {
+        if ((rc = copy_rows(sh, io.slot, p.h_out, hrow * 4, hb, R, st))) return rc;
+        if ((rc = copy_rows(sc, io.slot, w.seq.c0, hb, hb, R, st))) return rc;
       }
     }
-    off += Hl;
   }
-  return FSN_OK;
+  return fc_gemm_launch(hall(n - 1), s.fc_w, s.fc_b, s.out, R * S, Ht, s.O, s.act, st);
 }
 
 int copy_rows(void* dst, size_t dp, const void* src, size_t sp, size_t width, int B, cudaStream_t st) {

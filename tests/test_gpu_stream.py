@@ -20,14 +20,22 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _model(norm, dev, fc_gain=1.0):
+def _model(norm, dev, fc_gain=1.0, layers=3):
     from fullsubnet_b200.fullband_baseline.model import Model
+    from fullsubnet_b200.model.module.sequence_model import SequenceModel
     from oracle import fullband_baseline_oracle as BO
     args = dict(BO.DEFAULT_FBB_ARGS, norm_type=norm)
     sd = BO.make_fbb_state_dict(seed=11, args=args)
+    m = Model(**args)
+    if layers != 3:  # the recipe's Model fixes 3 layers; the library reads the depth from its SequenceModel
+        F, H = args["num_freqs"], args["hidden_size"]
+        m.fullband_model = SequenceModel(input_size=F, output_size=2 * F, hidden_size=H, num_layers=layers,
+                                         bidirectional=False, sequence_model=args["sequence_model"],
+                                         output_activate_function=args["output_activate_function"])
+        g = torch.Generator().manual_seed(11 + layers)
+        sd = {k: (torch.rand(v.shape, generator=g) * 2 - 1) / H ** 0.5 for k, v in m.state_dict().items()}
     for k in ("fullband_model.fc_output_layer.weight", "fullband_model.fc_output_layer.bias"):
         sd[k] = sd[k] * fc_gain
-    m = Model(**args)
     m.load_state_dict(sd, strict=True)
     return m.to(dev).eval()
 
@@ -92,12 +100,17 @@ def _whole(m, clip):
     return m.enhance(clip[None])[0]
 
 
-@pytest.mark.parametrize("fc_gain", [1.0, 8.0], ids=["Wa", "Wb"])
-@pytest.mark.parametrize("norm", NORMS)
-def test_stream_bit_identical_to_whole_clip(norm, fc_gain, dev):
+@pytest.mark.parametrize("norm,fc_gain,layers", [
+    pytest.param(norm, gain, 3, id=f"{norm}-{w}") for norm in NORMS for gain, w in ((1.0, "Wa"), (8.0, "Wb"))
+] + [
+    # depth 1 runs one layer alone; depth 4 puts the top layer in the other half of the layer-output ping-pong
+    pytest.param("cumulative_laplace_norm", 1.0, n, id=f"cumulative_laplace_norm-Wa-depth{n}") for n in (1, 4)
+])
+def test_stream_bit_identical_to_whole_clip(norm, fc_gain, layers, dev):
     from fullsubnet_b200.stream import Streamer
-    m = _model(norm, dev, fc_gain)
-    rng = random.Random(NORMS.index(norm) * 10 + int(fc_gain))
+    m = _model(norm, dev, fc_gain, layers)
+    assert m.fullband_model.num_layers == layers
+    rng = random.Random(NORMS.index(norm) * 10 + int(fc_gain) + (0 if layers == 3 else 100 * layers))
     slots = 4
     s = Streamer(m, slots)
     assert s.delay == 256 + (m.look_ahead + 2) * HOP
