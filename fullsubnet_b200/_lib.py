@@ -234,6 +234,19 @@ _SIGNATURES = {
     "fsn_debug_forgetting_scale": (C.c_int, [_P, _I, _P, _I, _I, _I, _I, _L, _L, _F, _P, _P, _I, _I, _P, _P, _P, _P, _P]),
     "fsn_debug_forgetting_bwd": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "fsn_debug_stoi_stages": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _S, _P]),
+    "fsn_debug_cum_clip_scale": (C.c_int, [_P, _I, _I, _I, _L, _L, _F, _P, _P, _P]),
+    "fsn_debug_cum_unit_scale": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _P, _P]),
+    "fsn_debug_forget_unit_broadcast": (C.c_int, [_P, _I, _I, _I, _I, _P, _P]),
+    "fsn_debug_fast_bn": (C.c_int, [_P, _P, _L, _L, _I, _I, _I, _I, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
+    "fsn_debug_fast_dec_input": (C.c_int, [_P, _P, _L, _L, _L, _I, _I, _I, _I, _I, _L, _L, _P, _P]),
+    "fsn_debug_transpose_mag": (C.c_int, [_P, _I, _I, _I, _I, _L, _L, _P, _P, _P, _P]),
+    "fsn_debug_crm_output": (C.c_int, [_P, _L, _L, _I, _I, _I, _I, _P, _P]),
+    "fsn_debug_scale_rows": (C.c_int, [_P, _P, _L, _I, _I, _I, _P, _P]),
+    "fsn_debug_imp_compress": (C.c_int, [_P, _I, _I, _I, _F, _I, _P, _P]),
+    "fsn_debug_train_gather": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "fsn_debug_sb_head": (C.c_int, [_P, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _L, _L, _I, _P, _P]),
+    "fsn_debug_sb_head_bwd": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _L, _L, _P, _P]),
+    "fsn_debug_train_dy": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
     "fsn_last_error_code": (C.c_int, []),
     "fsn_last_launch_count": (C.c_int64, []),
     "fsn_total_launch_count": (C.c_int64, []),

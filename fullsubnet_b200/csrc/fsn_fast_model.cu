@@ -153,6 +153,7 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
   FastDims m;
   int rc = fast_dims(d, B, T, m);
   if (rc) return rc;
+  if ((rc = layout_clips_check(B, true, "fast model"))) return rc;
   FastWs w;
   fast_carve(d, m, workspace, w);
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",

@@ -261,6 +261,7 @@ extern "C" int fsn_fast_train_forward(const fsn_fast_desc* d, const fsn_fast_wei
   FastDims m;
   int rc = fast_train_check(d, B, T, m);
   if (rc) return rc;
+  if ((rc = layout_clips_check(B, true, "fast training"))) return rc;
   FSN_REQUIRE(wt && mix_mag && out, FSN_ERR_SHAPE, "fast training: null argument");
   FastTrainWs w;
   carve_fast_train(d, m, workspace, w);

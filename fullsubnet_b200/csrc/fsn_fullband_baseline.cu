@@ -106,6 +106,7 @@ extern "C" int fsn_fullband_forward(const fsn_fullband_desc* d, const fsn_lstm_l
   launch_counter() = 0;
   int rc = fbb_check(d, B, T);
   if (rc) return rc;
+  if ((rc = layout_clips_check(B, true, "fullband"))) return rc;
   FbbWs w;
   fbb_carve(d, B, T, workspace, w);
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
@@ -133,6 +134,7 @@ extern "C" int fsn_fullband_enhance(const fsn_fullband_desc* d, const fsn_lstm_l
   launch_counter() = 0;
   int T, rc = fbb_enhance_dims(d, B, L_max, n_fft, hop, T);
   if (rc) return rc;
+  if ((rc = layout_clips_check(B, true, "fullband_enhance"))) return rc;
   if ((rc = wav_check(lengths, B, L_max, n_fft, true, enhanced, "fullband_enhance"))) return rc;
   FbbWs w;
   fbb_carve(d, B, T, workspace, w, true);

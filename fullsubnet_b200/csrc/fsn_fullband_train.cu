@@ -102,6 +102,7 @@ extern "C" int fsn_fullband_train_forward(const fsn_fullband_desc* d, const fsn_
   launch_counter() = 0;
   int rc = fbb_train_check(d, B, T);
   if (rc) return rc;
+  if ((rc = layout_clips_check(B, true, "fullband training"))) return rc;
   FSN_REQUIRE(layers && fc_w && fc_b && noisy_mag && out, FSN_ERR_SHAPE, "fullband training: null argument");
   FbbTrainWs w;
   carve_fbb_train(d, B, T, workspace, w);

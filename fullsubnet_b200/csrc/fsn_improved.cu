@@ -29,6 +29,12 @@ __global__ void imp_compress_kernel(const float* __restrict__ mag, float* __rest
   }
 }
 
+int imp_compress_launch(const float* mag, int B, int F, int T, float fdrc, bool tm, float* out, cudaStream_t st) {
+  imp_compress_kernel<<<dim3(cdiv(T, 32), cdiv(F - 1, 32), B), dim3(32, 8), 0, st>>>(mag, out, F, T, fdrc, tm);
+  FSN_CHECK_LAUNCH("imp_compress_kernel");
+  return FSN_OK;
+}
+
 // section input (model.py:321-405, 425-442): unit n of clip b at frame t = noisy rows lo+n*cs-ns .. (+cs+2ns) and
 // full-band rows lo+n*cf-nf .. (+cf+2nf), reflected (no edge repeat) at row 0 / row Fu-1.  One CTA per (b,t):
 // writes X[t][b*N+n][w] and the per-(b,t) sum (for the section norm).  magc / fbT are [B,T,Fu], or [T,B,Fu] when tm.
@@ -204,11 +210,7 @@ static int imp_forward(const fsn_improved_desc* d, const fsn_improved_weights* w
   // STFT (model.py:550-557), |X|^fdrc without the Nyquist bin (564-565)
   if ((rc = stft_launch(wav, B, L, d->n_fft, hop, d->win_length, w.mag, nullptr, w.real, w.imag, nullptr, 0, st, lens)))
     return rc;
-  {
-    dim3 grid(cdiv(T, 32), cdiv(Fu, 32), B);
-    imp_compress_kernel<<<grid, dim3(32, 8), 0, st>>>(w.mag, w.magc, F, T, d->fdrc, false);
-    FSN_CHECK_LAUNCH("imp_compress_kernel");
-  }
+  if ((rc = imp_compress_launch(w.mag, B, F, T, d->fdrc, false, w.magc, st))) return rc;
   // full band: norm (566) -> 2xLSTM + Linear (567); with lens the counts are per frame, times the clip's own frames
   if ((rc = clip_stats_launch(w.magc, B, T, Fu, 0, w.fs, w.sums, st, lens, hop, 0))) return rc;
   if ((rc = norm_scales_launch(w.sums, w.sums, B, lens ? (float)Fu : (float)Fu * T, 1.f, w.inv1, nullptr, st, eps, lens,

@@ -183,8 +183,7 @@ extern "C" int fsn_improved_train_forward(const fsn_improved_desc* d, const fsn_
   // STFT (model.py:550-557), |X|^fdrc without the Nyquist bin (564-565), time-major
   if ((rc = stft_launch(wav, B, L, d->n_fft, d->hop_length, d->win_length, w.mag, nullptr, w.real, w.imag, nullptr, 0, st)))
     return rc;
-  imp_compress_kernel<<<dim3(cdiv(T, 32), cdiv(Fu, 32), B), dim3(32, 8), 0, st>>>(w.mag, w.raw, F, T, d->fdrc, true);
-  FSN_CHECK_LAUNCH("imp_compress_kernel");
+  if ((rc = imp_compress_launch(w.mag, B, F, T, d->fdrc, true, w.raw, st))) return rc;
   // full band: norm (566) -> 2xLSTM + Linear + act (567), y kept for act'
   if ((rc = train_tm_stats_launch(w.raw, B, Fu, T, 0, w.sums, st))) return rc;
   if ((rc = norm_scales_launch(w.sums, w.sums, B, (float)Fu * T, 1.f, w.inv1, nullptr, st, IMP_EPS))) return rc;

@@ -231,6 +231,11 @@ int stack_bwd(const LayerBwd* L, int n, int steps, const float* dh_above, const 
 static const float TRAIN_CUM_EPS = 1.1920928955078125e-07f;  // audio_zen/constant.py:9
 int train_input_launch(const float* noisy_mag, int B, int F, int T, int Tp, int Ns, int norm_type, float2* sums, float* inv1,
                        float* raw, float* scaled, float2* fs, float* cum1, cudaStream_t st);
+// sub-band input of a training step X [Tp, R, K] (base_model.py:13-46 + model.py:98-119) from the time-major raw / fbz
+// [Tp,B,F]: unit (b,f) of row r (map), 2Ns+1 reflected raw rows || 2Nf+1 reflected fbz rows, times inv2[b], or
+// unit_scale[t*R + r] when given (the causal norms); a grid-stride kernel of 132 * 8 CTAs
+int train_gather_launch(const float* raw, const float* fbz, const float* inv2, const float* unit_scale, float* X, RowMap map,
+                        int Tp, int R, int Ns, int Nf, cudaStream_t st);
 // its backward: dY [Tp,B,2F] = dout [B,2,F,T] re-laid out, zero on the first `la` frames, times act'(y) (FSN_ACT_*) from
 // the kept post-activation output y (unread for FSN_ACT_NONE)
 int train_dy_launch(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
@@ -369,6 +374,11 @@ int crm_output_launch(const float* y, size_t bs, size_t ts, int B, int Tp, int F
 // scaled (nullable) receives the same elements times scale[b]
 int transpose_mag_launch(const float* in, int B, int F, int T, int Tp, size_t bs, size_t ts, float* out,
                          const float* scale, float* scaled, cudaStream_t st);
+// transpose_mag_launch and imp_compress_launch put the clip in gridDim.z, crm_output_launch the (clip, channel) pair:
+// an entry point that reaches them checks B with layout_clips_check (crm: it runs crm_output_launch) before any CUDA
+// call, FSN_ERR_UNSUPPORTED beyond the grid.  `who` prefixes the message.
+static const int LAYOUT_MAX_GRID_Z = 65535;
+int layout_clips_check(int B, bool crm, const char* who);
 // fs[b*Tp + t] = (sum_f x, sum_f c_N[f] x) of the frames of x, element (b,t,f) at b*bs + t*ts + f
 int frame_stats_launch(const float* x, int B, int Tp, int F, int N, size_t bs, size_t ts, float2* fs, cudaStream_t st);
 // Per-clip lengths (lens non-null, device [B] samples): clip b sums only its own Tp_b = 1 + lens[b]/hop + la frames of
@@ -429,7 +439,8 @@ int istft_mask_adjoint_launch(const float* dwav, const float* real, const float*
 struct SecGeom { int lo, N, cs, ns, cf, nf, W; };  // section rows [lo, lo + N*cs), unit width W
 struct ImpDims { int B, L, T, F, Fu, S; SecGeom sec[FSN_IMP_MAX_SECTIONS]; int maxRW, maxR; };
 int imp_dims(const fsn_improved_desc* d, int B, int L, ImpDims& m);
-__global__ void imp_compress_kernel(const float* __restrict__ mag, float* __restrict__ out, int F, int T, float fdrc, bool tm);
+// |X|^fdrc with the Nyquist bin dropped (model.py:564-565): mag [B,F,T] -> out [B,T,F-1], or [T,B,F-1] when tm
+int imp_compress_launch(const float* mag, int B, int F, int T, float fdrc, bool tm, float* out, cudaStream_t st);
 // section input (model.py:321-443): X [T, B*N, W] of the reflected noisy rows of magc and full-band rows of fbT ([B,T,Fu],
 // or [T,B,Fu] when tm), and fs[b*T + t] = the sum of the (b, t) block (.x and .y alike), one CTA per (b, t)
 int imp_section_input_launch(const float* magc, const float* fbT, int B, int T, int Fu, const SecGeom& g, float* X, float2* fs,

@@ -586,6 +586,12 @@ int scale_rows_launch(const float* in, const float* scale, size_t n, int cols, i
   return FSN_OK;
 }
 
+int layout_clips_check(int B, bool crm, const char* who) {
+  const int most = crm ? LAYOUT_MAX_GRID_Z / 2 : LAYOUT_MAX_GRID_Z;
+  FSN_REQUIRE(B <= most, FSN_ERR_UNSUPPORTED, "%s: B=%d clips, at most %d", who, B, most);
+  return FSN_OK;
+}
+
 int frame_stats_launch(const float* x, int B, int Tp, int F, int N, size_t bs, size_t ts, float2* fs, cudaStream_t st) {
   frame_stats_kernel<<<cdiv(B * Tp, 8), 256, 0, st>>>(x, B, Tp, F, N, bs, ts, fs);
   FSN_CHECK_LAUNCH("frame_stats_kernel");
@@ -690,4 +696,206 @@ extern "C" int fsn_debug_fc_gemm(const float* A, const float* W, const float* bi
   FSN_REQUIRE(O <= 65535 * 64, FSN_ERR_SHAPE, "fc_gemm hook: O=%d exceeds the grid", O);
   FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "fc_gemm hook: unknown act %d", act);
   return fc_gemm_launch(A, W, bias, out, M, K, O, act, (cudaStream_t)stream, w_kmajor != 0);
+}
+
+// ---- unit-test hooks of the causal-norm scales, the layout kernels and the sub-band heads (include/fsn_b200.h): each
+// reaches its kernels through the launchers the forwards and training steps run, every argument checked before any CUDA
+// call
+static const size_t HOOK_MAX_ELEMS = (size_t)1 << 31;
+
+// the sub-band row map of B clips of F bins with drop_band groups G (<= 1: none); R = B * Fsub
+static int hook_row_map(const char* who, int B, int F, int G, RowMap& map, int& R) {
+  FSN_REQUIRE(B > 0 && F > 0 && G >= 0, FSN_ERR_SHAPE, "%s: bad shape B=%d F=%d G=%d", who, B, F, G);
+  FSN_REQUIRE(G <= 1 || (B > G && F >= G), FSN_ERR_SHAPE, "%s: drop_band needs B > G and F >= G", who);
+  const int Fsub = G > 1 ? F / G : F;
+  map = RowMap{B, F, Fsub, G > 1 ? G : 1};
+  R = B * Fsub;
+  return FSN_OK;
+}
+
+extern "C" int fsn_debug_cum_clip_scale(const float* x, int B, int Tp, int F, int64_t bs, int64_t ts, float eps, float* fs,
+                                        float* scale1T, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(x && fs && scale1T, FSN_ERR_SHAPE, "cum clip scale hook: null argument");
+  FSN_REQUIRE(B > 0 && Tp > 0 && F > 0 && bs >= 0 && ts >= 0, FSN_ERR_SHAPE, "cum clip scale hook: bad shape B=%d Tp=%d F=%d",
+              B, Tp, F);
+  FSN_REQUIRE((size_t)B * Tp < HOOK_MAX_ELEMS, FSN_ERR_SHAPE, "cum clip scale hook: B*Tp must stay below 2^31");
+  const cudaStream_t st = (cudaStream_t)stream;
+  float2* f2 = reinterpret_cast<float2*>(fs);
+  int rc;
+  if ((rc = frame_stats_launch(x, B, Tp, F, 0, (size_t)bs, (size_t)ts, f2, st))) return rc;
+  return cum_clip_scale_launch(f2, B, Tp, F, eps, scale1T, st);
+}
+
+extern "C" int fsn_debug_cum_unit_scale(const float* magT, const float* fbT, int B, int F, int G, int Tp, int Ns, int Nf,
+                                        float eps, int time_major, float* scaleT, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(magT && fbT && scaleT, FSN_ERR_SHAPE, "cum unit scale hook: null argument");
+  RowMap map;
+  int R, rc;
+  if ((rc = hook_row_map("cum unit scale hook", B, F, G, map, R))) return rc;
+  FSN_REQUIRE(Tp > 0, FSN_ERR_SHAPE, "cum unit scale hook: bad shape Tp=%d", Tp);
+  FSN_REQUIRE(Ns >= 0 && Ns < F && Nf >= 0 && Nf < F, FSN_ERR_SHAPE, "cum unit scale hook: reflect padding needs 0 <= Ns, Nf < F");
+  FSN_REQUIRE((size_t)Tp * R < HOOK_MAX_ELEMS && (size_t)Tp * B * F < HOOK_MAX_ELEMS, FSN_ERR_SHAPE,
+              "cum unit scale hook: tensors must stay below 2^31 elements");
+  return cum_unit_scale_launch(magT, fbT, map, R, Tp, Ns, Nf, eps, scaleT, (cudaStream_t)stream, time_major != 0);
+}
+
+extern "C" int fsn_debug_forget_unit_broadcast(const float* scaleT, int B, int F, int G, int Tp, float* unit_scale,
+                                               fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(scaleT && unit_scale, FSN_ERR_SHAPE, "unit broadcast hook: null argument");
+  RowMap map;
+  int R, rc;
+  if ((rc = hook_row_map("unit broadcast hook", B, F, G, map, R))) return rc;
+  FSN_REQUIRE(Tp > 0 && (size_t)Tp * R < HOOK_MAX_ELEMS, FSN_ERR_SHAPE, "unit broadcast hook: bad shape Tp=%d", Tp);
+  return forget_unit_broadcast_launch(scaleT, map, R, Tp, unit_scale, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_fast_bn(const float* melT, const float* encT, int64_t bs, int64_t ts, int B, int Tp, int M, int Nn,
+                                 int Ne, int S, int cum, float eps, float* bn, float* fs, float* sums, float* scale,
+                                 fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(melT && encT && bn && fs && scale && (cum || sums), FSN_ERR_SHAPE, "fast bottleneck hook: null argument");
+  FSN_REQUIRE(B > 0 && Tp > 0 && M > 0 && S >= 1 && bs >= 0 && ts >= 0, FSN_ERR_SHAPE,
+              "fast bottleneck hook: bad shape B=%d Tp=%d M=%d S=%d", B, Tp, M, S);
+  FSN_REQUIRE(Nn >= 0 && Nn < M && Ne >= 0 && Ne < M, FSN_ERR_SHAPE, "fast bottleneck hook: reflect padding needs 0 <= Nn, Ne < M");
+  const int K = (2 * Nn + 1) + (2 * Ne + 1), Ts = 1 + cdiv(Tp - 1, S), R = B * M;
+  FSN_REQUIRE((size_t)Ts * R * K < HOOK_MAX_ELEMS && (size_t)B * Ts < HOOK_MAX_ELEMS, FSN_ERR_SHAPE,
+              "fast bottleneck hook: tensors must stay below 2^31 elements");
+  const cudaStream_t st = (cudaStream_t)stream;
+  float2* f2 = reinterpret_cast<float2*>(fs);
+  float2* s2 = reinterpret_cast<float2*>(sums);
+  int rc;
+  // as fsn_fast_model_forward and fsn_fast_train_forward run them
+  if ((rc = fast_bn_input_launch(melT, encT, (size_t)bs, (size_t)ts, B, Tp, M, Nn, Ne, S, Ts, bn, f2, st))) return rc;
+  if (cum) return fast_cum_bn_scale_launch(bn, R, K, Ts, eps, scale, st);
+  if ((rc = clip_reduce_only_launch(f2, B, Ts, s2, st))) return rc;
+  return norm_scales_launch(s2, s2, B, (float)M * K * Ts, 1.f, scale, nullptr, st, eps);
+}
+
+extern "C" int fsn_debug_fast_dec_input(const float* encT, const float* bn_out, int64_t nbs, int64_t nms, int64_t nts, int B,
+                                        int Tp, int M, int S, int Ts, int64_t rbs, int64_t rts, float* dec_in,
+                                        fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(encT && bn_out && dec_in, FSN_ERR_SHAPE, "decoder input hook: null argument");
+  FSN_REQUIRE(B > 0 && Tp > 0 && M > 0 && S >= 1 && Ts > 0 && nbs >= 0 && nms >= 0 && nts >= 0, FSN_ERR_SHAPE,
+              "decoder input hook: bad shape B=%d Tp=%d M=%d S=%d Ts=%d", B, Tp, M, S, Ts);
+  FSN_REQUIRE((rbs == Tp && rts == 1) || (rbs == 1 && rts == B), FSN_ERR_SHAPE,
+              "decoder input hook: rows clip-major (rbs = Tp, rts = 1) or time-major (rbs = 1, rts = B)");
+  FSN_REQUIRE((size_t)B * Tp * 2 * M < HOOK_MAX_ELEMS, FSN_ERR_SHAPE, "decoder input hook: tensors must stay below 2^31");
+  return fast_dec_input_launch(encT, bn_out, (size_t)nbs, (size_t)nms, (size_t)nts, B, Tp, M, S, Ts, (size_t)rbs, (size_t)rts,
+                               dec_in, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_transpose_mag(const float* in, int B, int F, int T, int Tp, int64_t bs, int64_t ts, float* out,
+                                       const float* scale, float* scaled, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(in && out && (!scaled || scale), FSN_ERR_SHAPE, "transpose_mag hook: null argument");
+  FSN_REQUIRE(B > 0 && F > 0 && T > 0 && Tp >= T && bs >= 0 && ts >= 0, FSN_ERR_SHAPE,
+              "transpose_mag hook: bad shape B=%d F=%d T=%d Tp=%d", B, F, T, Tp);
+  FSN_REQUIRE(cdiv(F, 32) <= LAYOUT_MAX_GRID_Z, FSN_ERR_UNSUPPORTED, "transpose_mag hook: F=%d exceeds the grid", F);
+  int rc;
+  if ((rc = layout_clips_check(B, false, "transpose_mag hook"))) return rc;
+  return transpose_mag_launch(in, B, F, T, Tp, (size_t)bs, (size_t)ts, out, scale, scaled, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_crm_output(const float* y, int64_t bs, int64_t ts, int B, int Tp, int F, int la, float* out,
+                                    fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(y && out, FSN_ERR_SHAPE, "crm_output hook: null argument");
+  FSN_REQUIRE(B > 0 && F > 0 && la >= 0 && Tp > la && bs >= 0 && ts >= 0, FSN_ERR_SHAPE,
+              "crm_output hook: bad shape B=%d Tp=%d F=%d la=%d", B, Tp, F, la);
+  FSN_REQUIRE(cdiv(F, 32) <= LAYOUT_MAX_GRID_Z, FSN_ERR_UNSUPPORTED, "crm_output hook: F=%d exceeds the grid", F);
+  int rc;
+  if ((rc = layout_clips_check(B, true, "crm_output hook"))) return rc;
+  return crm_output_launch(y, (size_t)bs, (size_t)ts, B, Tp, F, la, out, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_scale_rows(const float* in, const float* scale, int64_t n, int cols, int rows, int div, float* out,
+                                    fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(in && scale && out, FSN_ERR_SHAPE, "scale_rows hook: null argument");
+  FSN_REQUIRE(n > 0 && cols > 0 && rows > 0 && div > 0, FSN_ERR_SHAPE,
+              "scale_rows hook: bad shape n=%lld cols=%d rows=%d div=%d", (long long)n, cols, rows, div);
+  return scale_rows_launch(in, scale, (size_t)n, cols, rows, div, out, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_imp_compress(const float* mag, int B, int F, int T, float fdrc, int tm, float* out,
+                                      fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(mag && out, FSN_ERR_SHAPE, "imp_compress hook: null argument");
+  FSN_REQUIRE(B > 0 && F >= 2 && T > 0, FSN_ERR_SHAPE, "imp_compress hook: bad shape B=%d F=%d T=%d", B, F, T);
+  FSN_REQUIRE(cdiv(F - 1, 32) <= LAYOUT_MAX_GRID_Z, FSN_ERR_UNSUPPORTED, "imp_compress hook: F=%d exceeds the grid", F);
+  FSN_REQUIRE((size_t)B * T * F < HOOK_MAX_ELEMS, FSN_ERR_SHAPE, "imp_compress hook: tensors must stay below 2^31");
+  int rc;
+  if ((rc = layout_clips_check(B, false, "imp_compress hook"))) return rc;
+  return imp_compress_launch(mag, B, F, T, fdrc, tm != 0, out, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_train_gather(const float* raw, const float* fbz, const float* inv2, const float* unit_scale, int B,
+                                      int F, int G, int Tp, int Ns, int Nf, float* X, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(raw && fbz && X && (inv2 || unit_scale), FSN_ERR_SHAPE, "train_gather hook: null argument");
+  RowMap map;
+  int R, rc;
+  if ((rc = hook_row_map("train_gather hook", B, F, G, map, R))) return rc;
+  FSN_REQUIRE(Tp > 0, FSN_ERR_SHAPE, "train_gather hook: bad shape Tp=%d", Tp);
+  FSN_REQUIRE(Ns >= 0 && Ns < F && Nf >= 0 && Nf < F, FSN_ERR_SHAPE, "train_gather hook: reflect padding needs 0 <= Ns, Nf < F");
+  FSN_REQUIRE((size_t)Tp * R * (2 * Ns + 2 * Nf + 2) < HOOK_MAX_ELEMS && (size_t)Tp * B * F < HOOK_MAX_ELEMS, FSN_ERR_SHAPE,
+              "train_gather hook: tensors must stay below 2^31 elements");
+  return train_gather_launch(raw, fbz, inv2, unit_scale, X, map, Tp, R, Ns, Nf, (cudaStream_t)stream);
+}
+
+// the cRM geometry of a head: R rows of N units per clip, O <= 2c outputs, section rows [lo, lo + N c) of `rows`
+// (rows = 0: one channel, a plain [R, frames] table)
+static int hook_head_geom(const char* who, int R, int O, int N, int c, int lo, int rows, int64_t rs, int64_t bs,
+                          HeadGeom& g) {
+  FSN_REQUIRE(R > 0 && O > 0 && N > 0 && c > 0 && lo >= 0 && rows >= 0 && rs > 0 && bs >= 0, FSN_ERR_SHAPE,
+              "%s: bad geometry R=%d O=%d N=%d c=%d lo=%d rows=%d", who, R, O, N, c, lo, rows);
+  FSN_REQUIRE(R % N == 0, FSN_ERR_SHAPE, "%s: R=%d rows are not whole clips of N=%d units", who, R, N);
+  FSN_REQUIRE(O <= 2 * c, FSN_ERR_SHAPE, "%s: O=%d outputs exceed 2c = %d", who, O, 2 * c);
+  FSN_REQUIRE(rows == 0 ? O <= c : (size_t)lo + (size_t)N * c <= (size_t)rows, FSN_ERR_SHAPE,
+              "%s: section rows [%d, %d + N c) exceed rows=%d", who, lo, lo, rows);
+  g = HeadGeom{N, c, lo, rows, (size_t)rs, (size_t)bs};
+  return FSN_OK;
+}
+
+extern "C" int fsn_debug_sb_head(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act,
+                                 int N, int c, int lo, int rows, int64_t rs, int64_t bs, int t0, float* out,
+                                 fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(h && W && bias && out, FSN_ERR_SHAPE, "sub-band head hook: null argument");
+  FSN_REQUIRE(H > 0 && steps > 0 && t0 >= 0, FSN_ERR_SHAPE, "sub-band head hook: bad shape H=%d steps=%d t0=%d", H, steps, t0);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "sub-band head hook: unknown act %d", act);
+  HeadGeom g;
+  int rc;
+  if ((rc = hook_head_geom("sub-band head hook", R, O, N, c, lo, rows, rs, bs, g))) return rc;
+  FSN_REQUIRE(((size_t)steps * R * O + 7) / 8 <= 0x7fffffff && (size_t)steps * R * H < HOOK_MAX_ELEMS, FSN_ERR_SHAPE,
+              "sub-band head hook: steps * R * O exceeds the grid");
+  return sb_head_launch(h, R, H, steps, W, bias, O, act, out, g, t0, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_sb_head_bwd(const float* dcrm, const float* y, int act, int R, int O, int steps, int la, int N, int c,
+                                     int lo, int rows, int64_t rs, int64_t bs, float* dY, fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(dcrm && dY && (act == FSN_ACT_NONE || y), FSN_ERR_SHAPE, "sub-band head backward hook: null argument");
+  FSN_REQUIRE(steps > 0 && la >= 0, FSN_ERR_SHAPE, "sub-band head backward hook: bad shape steps=%d la=%d", steps, la);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "sub-band head backward hook: unknown act %d", act);
+  HeadGeom g;
+  int rc;
+  if ((rc = hook_head_geom("sub-band head backward hook", R, O, N, c, lo, rows, rs, bs, g))) return rc;
+  FSN_REQUIRE((size_t)steps * R * O < HOOK_MAX_ELEMS, FSN_ERR_SHAPE, "sub-band head backward hook: tensors must stay below 2^31");
+  return sb_head_bwd_launch(dcrm, y, act, R, O, steps, la, g, dY, (cudaStream_t)stream);
+}
+
+extern "C" int fsn_debug_train_dy(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
+                                  fsn_stream_t stream) {
+  launch_counter() = 0;
+  FSN_REQUIRE(dout && dY && (act == FSN_ACT_NONE || y), FSN_ERR_SHAPE, "train_dy hook: null argument");
+  FSN_REQUIRE(B > 0 && F > 0 && T > 0 && la >= 0 && Tp == T + la, FSN_ERR_SHAPE,
+              "train_dy hook: bad shape B=%d F=%d T=%d Tp=%d la=%d (Tp = T + la)", B, F, T, Tp, la);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "train_dy hook: unknown act %d", act);
+  FSN_REQUIRE((size_t)Tp * B * 2 * F < HOOK_MAX_ELEMS, FSN_ERR_SHAPE, "train_dy hook: tensors must stay below 2^31");
+  return train_dy_launch(dout, y, act, B, F, T, Tp, la, dY, (cudaStream_t)stream);
 }

@@ -256,6 +256,7 @@ extern "C" int fsn_model_forward(const fsn_model_desc* d, const fsn_seq_weights*
   Dims m;
   int rc = make_dims(d, B, T, m);
   if (rc) return rc;
+  if ((rc = layout_clips_check(B, false, "model"))) return rc;
   FSN_REQUIRE(d->precision == FSN_PREC_FP32 || sb_tc_supported(d), FSN_ERR_UNSUPPORTED,
               "FSN_PREC_F16_TC / FSN_PREC_F16X3_TC need sb_hidden in {128,256,384} and sub-band input width <= 32");
   ModelWs w;

@@ -304,6 +304,13 @@ __global__ void train_gather_kernel(const float* __restrict__ raw, const float* 
   }
 }
 
+int train_gather_launch(const float* raw, const float* fbz, const float* inv2, const float* unit_scale, float* X, RowMap map,
+                        int Tp, int R, int Ns, int Nf, cudaStream_t st) {
+  train_gather_kernel<<<132 * 8, 256, 0, st>>>(raw, fbz, inv2, unit_scale, X, map, Tp, R, Ns, Nf);
+  FSN_CHECK_LAUNCH("train_gather_kernel");
+  return FSN_OK;
+}
+
 // ---- cumulative_laplace_norm in the training step (audio_zen/model/base_model.py:220-251)
 // Backward of X[t,r,k] = u[t,r,k] * s[t,r], s = 1/(m + eps), m[t,r] = sum_{t'<=t} sum_k u[t',r,k] / (K (t+1)):
 //   d u[t,r,k] = dX[t,r,k] s[t,r] + sum_{t''>=t} q[t'',r],   q[t,r] = -s[t,r] <dX[t,r,:], X[t,r,:]> / (K (t+1)).
@@ -912,6 +919,7 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
   int rc = make_dims(d, B, T, m);
   if (rc) return rc;
   if ((rc = train_check(d))) return rc;
+  if ((rc = layout_clips_check(B, false, "training"))) return rc;
   TrainWs w;
   carve_train(d, m, workspace, w);
   FSN_REQUIRE(workspace && workspace_bytes >= w.bytes, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu",
@@ -945,9 +953,9 @@ extern "C" int fsn_train_forward(const fsn_model_desc* d, const fsn_seq_weights*
     if ((rc = forget_scale_launch(w.fs, w.fs2, B, Tp, (float)F * m.Ksb, w.fg2, nullptr, st))) return rc;
     if ((rc = forget_unit_broadcast_launch(w.fg2, map, m.R, Tp, w.cum2, st))) return rc;
   }
-  train_gather_kernel<<<132 * 8, 256, 0, st>>>(w.raw, w.fbz, w.inv2, (cum || fgt) ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,
-                                               d->sb_num_neighbors, d->fb_num_neighbors);
-  FSN_CHECK_LAUNCH("train_gather_kernel");
+  if ((rc = train_gather_launch(w.raw, w.fbz, w.inv2, (cum || fgt) ? w.cum2 : nullptr, w.xsb, map, Tp, m.R,
+                                d->sb_num_neighbors, d->fb_num_neighbors, st)))
+    return rc;
   if ((rc = layer_forward(prec, seq_layer(*sb, 0), w.xsb, m.R, m.Ksb, Hs, Tp, w.sb[0], w.rec, w.splitk, &hs0, st))) return rc;
   if ((rc = layer_forward(prec, seq_layer(*sb, 1), w.sb[0].H, m.R, Hs, Hs, Tp, w.sb[1], w.rec, w.splitk, &hs1, st))) return rc;
   // sub-band Linear of every output frame in one launch (model.py:129-135; the first look_ahead steps have no frame)

@@ -79,7 +79,8 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
  * fsn_improved_forward / _enhance accept since, with fsn_improved_packed_bytes / fsn_improved_pack_sb_weights and the
  * fsn_debug_imp_section_lstm_tc hook: a caller of the shorter struct never selects them, so the version stays 102.  The
  * dense GEMM layer's unit-test hooks fsn_debug_fc_gemm, fsn_debug_sgemm, fsn_debug_colsum, fsn_debug_small_out_wgrad,
- * fsn_debug_transpose, fsn_debug_transpose_blocked and fsn_debug_gemm_tc are new symbols only. */
+ * fsn_debug_transpose, fsn_debug_transpose_blocked and fsn_debug_gemm_tc are new symbols only, and so are the hooks of the
+ * causal-norm scales, the layout kernels and the sub-band heads (fsn_debug_cum_clip_scale .. fsn_debug_train_dy). */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -875,6 +876,60 @@ int fsn_debug_imp_unfold_bwd(const float* dX, const float* Xn, const float* invs
                              fsn_stream_t stream);
 int fsn_debug_imp_section_input(const float* magc, const float* fbT, int B, int T, int Fu, int lo, int hi, int cs, int ns,
                                 int cf, int nf, int tm, float* X, float* fs, fsn_stream_t stream);
+/* unit-test hooks of the causal-norm forward scales, the layout kernels and the sub-band heads (fsn_lstm_simt.cu,
+ * fsn_fast_model.cu, fsn_improved.cu, fsn_train.cu): the launchers the forwards and training steps run, on caller
+ * buffers.  Every argument is checked before any CUDA call; fsn_last_launch_count() gives the kernels a call launched.
+ *   fsn_debug_cum_clip_scale: fs [B*Tp] (float2) <- the frame sums of x (element (b,t,f) at b*bs + t*ts + f), then
+ *     scale1T [Tp,B] <- 1 / (running mean over the F bins of the frames so far + eps) (cumulative_laplace_norm).
+ *   fsn_debug_cum_unit_scale: scaleT [Tp,R] of every sub-band unit of the drop_band map (G <= 1: none; else B > G,
+ *     Fsub = F/G, R = B*Fsub): the running mean over its 2Ns+1 reflected magT rows and 2Nf+1 reflected fbT rows; magT /
+ *     fbT [B,Tp,F], or [Tp,B,F] with time_major.
+ *   fsn_debug_forget_unit_broadcast: unit_scale [Tp,R] <- scaleT [Tp,B] of each row's clip (same map).
+ *   fsn_debug_fast_bn: fast_fullsubnet's bottleneck input bn [Ts, B*M, K] (Ts = 1 + ceil((Tp-1)/S), K = 2Nn+2Ne+2) and
+ *     its (b, ts) block sums fs [B*Ts] (float2) from melT / encT (element (b,t,m) at b*bs + t*ts + m); cum: scale [Ts,B*M]
+ *     <- the second cumulative norm's scales; else sums [B] (float2) and scale [B] <- 1 / (mean over M K Ts + eps).
+ *   fsn_debug_fast_dec_input: dec_in rows (b,t) of 2M at b*rbs + t*rts (clip-major rbs = Tp, rts = 1; time-major rbs = 1,
+ *     rts = B) <- encT row || the bottleneck output (b, m, min(t/S, Ts-1)) at b*nbs + m*nms + ts*nts.
+ *   fsn_debug_transpose_mag: mag [B,F,T] -> out (b,t,f) at b*bs + t*ts + f for t < Tp (frames >= T zero); scaled
+ *     (nullable) the same times scale[b].  B <= 65535.
+ *   fsn_debug_crm_output: y rows (b,t) of 2F at b*bs + t*ts -> out [B,2,F,Tp-la], dropping the first la frames.
+ *     B <= 32767.
+ *   fsn_debug_scale_rows: out[i] = in[i] * scale[((i / cols) % rows) / div] for i < n; in may be out.
+ *   fsn_debug_imp_compress: mag [B,F,T] -> |mag|^fdrc without the Nyquist bin, [B,T,F-1], or [T,B,F-1] with tm.
+ *   fsn_debug_train_gather: X [Tp, R, K] (K = 2Ns+2Nf+2) of the training step's sub-band input from raw / fbz [Tp,B,F]
+ *     (same map), times inv2[b], or unit_scale [Tp,R] when given.
+ *   fsn_debug_sb_head: act(h W^T + bias) of h [steps, R, H], W [O,H], into frames t0 .. t0+steps-1 of the cRM: output
+ *     o = ch*c + j of row r = b*N + n at out[b*bs' + (ch*rows + lo + n*c + j)*rs + t], bs' = bs or (bs = 0) 2*rows*rs;
+ *     O <= 2c, R a multiple of N, lo + N c <= rows (rows = 0: one channel, O <= c).
+ *   fsn_debug_sb_head_bwd: dY [steps, R, O] <- act'(y) dcrm at frame t - la of the same geometry, 0 for t < la (y, laid
+ *     out like dcrm, unread for FSN_ACT_NONE).
+ *   fsn_debug_train_dy: dY [Tp,B,2F] <- dout [B,2,F,T] at frame t - la (0 for t < la, Tp = T + la) times act'(y [Tp,B,2F]).
+ */
+int fsn_debug_cum_clip_scale(const float* x, int B, int Tp, int F, int64_t bs, int64_t ts, float eps, float* fs,
+                             float* scale1T, fsn_stream_t stream);
+int fsn_debug_cum_unit_scale(const float* magT, const float* fbT, int B, int F, int G, int Tp, int Ns, int Nf, float eps,
+                             int time_major, float* scaleT, fsn_stream_t stream);
+int fsn_debug_forget_unit_broadcast(const float* scaleT, int B, int F, int G, int Tp, float* unit_scale, fsn_stream_t stream);
+int fsn_debug_fast_bn(const float* melT, const float* encT, int64_t bs, int64_t ts, int B, int Tp, int M, int Nn, int Ne,
+                      int S, int cum, float eps, float* bn, float* fs, float* sums, float* scale, fsn_stream_t stream);
+int fsn_debug_fast_dec_input(const float* encT, const float* bn_out, int64_t nbs, int64_t nms, int64_t nts, int B, int Tp,
+                             int M, int S, int Ts, int64_t rbs, int64_t rts, float* dec_in, fsn_stream_t stream);
+int fsn_debug_transpose_mag(const float* in, int B, int F, int T, int Tp, int64_t bs, int64_t ts, float* out,
+                            const float* scale, float* scaled, fsn_stream_t stream);
+int fsn_debug_crm_output(const float* y, int64_t bs, int64_t ts, int B, int Tp, int F, int la, float* out,
+                         fsn_stream_t stream);
+int fsn_debug_scale_rows(const float* in, const float* scale, int64_t n, int cols, int rows, int div, float* out,
+                         fsn_stream_t stream);
+int fsn_debug_imp_compress(const float* mag, int B, int F, int T, float fdrc, int tm, float* out, fsn_stream_t stream);
+int fsn_debug_train_gather(const float* raw, const float* fbz, const float* inv2, const float* unit_scale, int B, int F, int G,
+                           int Tp, int Ns, int Nf, float* X, fsn_stream_t stream);
+int fsn_debug_sb_head(const float* h, int R, int H, int steps, const float* W, const float* bias, int O, int act, int N,
+                      int c, int lo, int rows, int64_t rs, int64_t bs, int t0, float* out, fsn_stream_t stream);
+int fsn_debug_sb_head_bwd(const float* dcrm, const float* y, int act, int R, int O, int steps, int la, int N, int c, int lo,
+                          int rows, int64_t rs, int64_t bs, float* dY, fsn_stream_t stream);
+int fsn_debug_train_dy(const float* dout, const float* y, int act, int B, int F, int T, int Tp, int la, float* dY,
+                       fsn_stream_t stream);
+
 /* unit-test hook of improved_fullsubnet's section recurrence on FSN_PREC_F16X3_TC (x3 = 1) / FSN_PREC_F16_TC (x3 = 0):
  * R independent rows of X [T, R, W] through the 2-layer LSTM of `sw` (w_ih[0] [4H, W]; fc_w / fc_b unread) -> h1 [T, R, H],
  * layer 1's hidden state of every step, by the path fsn_improved_forward runs (input projection on the tf32 GEMM, then
