@@ -195,6 +195,9 @@ _SIGNATURES = {
     "fsn_debug_lstm_layer_tc": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _S, _P]),
     "fsn_debug_lstm_tc_carry": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _I, _P, _P, _S, _P]),
     "fsn_debug_linear_tc": (C.c_int, [_P, _I, _I, _P, _P, _I, _I, _I, _P, _P, _S, _P]),
+    "fsn_debug_lstm_rec_tc_scratch_bytes": (_S, [_I, _I]),
+    "fsn_debug_lstm_rec_tc": (C.c_int, [_P, _P, _P, _P, _L, _L, _P, _L, _L, _I, _I, _I, _I, _P, _P, _P, _L, _P, _I, _P, _P,
+                                        _S, _P]),
     "fsn_debug_sb_lstm_tc_packed_bytes": (_S, [_I, _I]),
     "fsn_debug_sb_lstm_tc_max_clusters": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int)]),
     "fsn_debug_sb_lstm_tc": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _I,

@@ -486,9 +486,14 @@ struct RecCarry {
   const int* restart;
   int fin_step;
 };
+// what lstm_rec_tc_launch chose for a call (unit tests): rows per cooperative launch, TMA ring stages, launches, dynamic
+// shared memory bytes per CTA
+struct RecTcInfo {
+  int rows_per_launch, stages, launches, smem_bytes;
+};
 int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, const float* P, size_t p_row, size_t p_t,
                        float* hall, size_t h_row, size_t h_t, int R, int T, int H, bool x3, void* scratch,
-                       cudaStream_t st, const RecCarry* io = nullptr);
+                       cudaStream_t st, const RecCarry* io = nullptr, RecTcInfo* info = nullptr);
 int split_tf32_launch(const float* in, size_t rows, int K, size_t ldi, const float* row_scale, int rows_per_scale,
                       float* out, int Kp, int cat, cudaStream_t st, int scale_B = 0);
 int bias_act_launch(float* x, size_t rows, int N, size_t ld, const float* bias, int act, cudaStream_t st);

@@ -40,6 +40,7 @@ constexpr int KB = 64;                // k-block: one 128-byte swizzled row of f
 constexpr int A_TILE = MR * KB * 2;   // 16 KB
 constexpr int NTHREADS = 160;         // warps 0-3: MMA + cell (one warpgroup), warp 4: TMA producer
 constexpr int MAX_STAGES = 6;
+constexpr int MIN_H = 64;             // smallest hidden size: see lstm_rec_tc_scratch_bytes
 
 struct Bars {
   uint64_t full[MAX_STAGES], empty[MAX_STAGES];
@@ -392,7 +393,7 @@ static int rec_sm_count() {
 // tensor-core recurrence available for hidden size H on this device?
 bool lstm_rec_tc_supported(int H, bool x3) {
   static const bool off = getenv("FSN_NO_REC_TC") != nullptr;
-  if (off || H < 64 || !tmap_encoder()) return false;  // H >= 64: see lstm_rec_tc_scratch_bytes
+  if (off || H < rec::MIN_H || !tmap_encoder()) return false;
   int dev = 0, coop = 0, max_smem = 0, major = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
@@ -420,10 +421,14 @@ size_t lstm_rec_tc_scratch_bytes(int H, bool x3) {
 }
 
 // h_t for every step of one layer, given the hoisted input projection P (see Args for the strides); R rows (any
-// count: chunks of lstm_rec_tc_rows_per_launch are launched back to back)
+// count: chunks of lstm_rec_tc_rows_per_launch are launched back to back).  P and hall must be 8-byte aligned: with H
+// and the strides even the kernel reads P and writes hall as float2 (vec_ok), so a base at 4 mod 8 is refused
+// (FSN_ERR_SHAPE) before any CUDA call rather than faulting in the kernel.  info (nullable) receives the launch choices.
 int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, const float* P, size_t p_row, size_t p_t,
                        float* hall, size_t h_row, size_t h_t, int R, int T, int H, bool x3, void* scratch,
-                       cudaStream_t st, const RecCarry* io) {
+                       cudaStream_t st, const RecCarry* io, RecTcInfo* info) {
+  FSN_REQUIRE((reinterpret_cast<uintptr_t>(P) & 7) == 0 && (reinterpret_cast<uintptr_t>(hall) & 7) == 0, FSN_ERR_SHAPE,
+              "lstm_rec_tc: P (%p) and hall (%p) must be 8-byte aligned", (const void*)P, (void*)hall);
   FSN_REQUIRE(lstm_rec_tc_supported(H, x3), FSN_ERR_UNSUPPORTED, "lstm_rec_tc: hidden size %d not supported", H);
   const int Kp = (H + rec::KB - 1) / rec::KB * rec::KB;
   const int C = cdiv(H, rec::U);
@@ -444,6 +449,7 @@ int lstm_rec_tc_launch(const float* w_hh, const float* b_ih, const float* b_hh, 
                         : (x3 ? (const void*)rec::lstm_rec_tc_kernel<true> : (const void*)rec::lstm_rec_tc_kernel<false>);
   if ((rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "lstm_rec_tc smem attr")))
     return rc;
+  if (info) *info = RecTcInfo{rows_max, stages, cdiv(R, rows_max), (int)smem};
   for (int r0 = 0; r0 < R; r0 += rows_max) {
     const int nr = (R - r0 < rows_max) ? R - r0 : rows_max;
     const int G = cdiv(nr, rec::MR);
@@ -565,26 +571,47 @@ int linear_tc(const float* x, size_t ldx, int K, const float* W, const float* bi
 
 }  // namespace fsn
 
-// unit-test hooks (tests/test_gpu_rec_tc.py): one LSTM layer / one Linear layer on the tensor-core path
+// unit-test hooks (tests/test_gpu_rec_tc.py): one LSTM layer / one Linear layer on the tensor-core path, and the
+// recurrence alone.  Every argument is checked before any CUDA call (the scratch sizes read the device's SM count only);
+// what the device supports (FSN_ERR_UNSUPPORTED) is reported after those checks.  The layer hooks report a hidden size
+// below the kernel's minimum as unsupported right after the pointer and shape checks, before the workspace, whose size
+// means nothing for such an H: a caller probing H gets FSN_ERR_UNSUPPORTED whatever workspace it passes.
 extern "C" size_t fsn_debug_lstm_tc_workspace_bytes(int R, int T, int K, int H, int x3) {
   fsn::Carver c(nullptr);
   fsn::LstmTcWs ws;
   fsn::lstm_tc_carve(c, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
   return c.off;
 }
+// the argument checks shared by the two LSTM layer hooks, before any CUDA call: pointers, sizes, the minimum H, workspace
+static int lstm_layer_hook_check(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* x,
+                                 int R, int T, int K, int H, int x3, float* hall, void* workspace, size_t workspace_bytes,
+                                 fsn::LstmTcWs& ws) {
+  FSN_REQUIRE(w_ih && w_hh && b_ih && b_hh && x && hall, FSN_ERR_SHAPE, "lstm_layer_tc hook: null argument");
+  FSN_REQUIRE(R > 0 && T > 0 && K > 0 && H > 0 && (int64_t)R * T < ((int64_t)1 << 31), FSN_ERR_SHAPE,
+              "lstm_layer_tc hook: bad shape R=%d T=%d K=%d H=%d", R, T, K, H);
+  FSN_REQUIRE(H >= fsn::rec::MIN_H, FSN_ERR_UNSUPPORTED, "lstm_layer_tc: hidden size %d not supported (< %d)", H,
+              fsn::rec::MIN_H);
+  fsn::Carver c(workspace);
+  fsn::lstm_tc_carve(c, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
+  FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, c.off);
+  return FSN_OK;
+}
 extern "C" int fsn_debug_lstm_layer_tc(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh,
                                        const float* x, int R, int T, int K, int H, int x3, float* hall, void* workspace,
                                        size_t workspace_bytes, fsn_stream_t stream) {
-  FSN_REQUIRE(fsn::lstm_rec_tc_supported(H, x3 != 0), FSN_ERR_UNSUPPORTED, "lstm_layer_tc: hidden size %d not supported", H);
-  fsn::Carver c(workspace);
   fsn::LstmTcWs ws;
-  fsn::lstm_tc_carve(c, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
-  FSN_REQUIRE(workspace && workspace_bytes >= c.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, c.off);
+  int rc;
+  if ((rc = lstm_layer_hook_check(w_ih, w_hh, b_ih, b_hh, x, R, T, K, H, x3, hall, workspace, workspace_bytes, ws))) return rc;
+  FSN_REQUIRE(fsn::lstm_rec_tc_supported(H, x3 != 0), FSN_ERR_UNSUPPORTED, "lstm_layer_tc: hidden size %d not supported", H);
   fsn_lstm_layer L{w_ih, w_hh, b_ih, b_hh};
   return fsn::lstm_layer_tc(L, x, (size_t)K, K, nullptr, 1, 0, R, T, H, x3 != 0, ws, hall, (cudaStream_t)stream);
 }
 extern "C" int fsn_debug_linear_tc(const float* x, int rows, int K, const float* W, const float* bias, int N, int act, int x3,
                                    float* out, void* workspace, size_t workspace_bytes, fsn_stream_t stream) {
+  FSN_REQUIRE(x && W && out, FSN_ERR_SHAPE, "linear_tc hook: null argument");
+  FSN_REQUIRE(rows > 0 && K > 0 && N > 0 && (N + 127) / 128 <= 65535, FSN_ERR_SHAPE, "linear_tc hook: bad shape rows=%d K=%d N=%d",
+              rows, K, N);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "linear_tc hook: unknown act %d", act);
   fsn::Carver c(workspace);
   fsn::LstmTcWs ws;
   const int Hm = (N + 3) / 4 > 8 ? (N + 3) / 4 : 8;
@@ -596,16 +623,50 @@ extern "C" int fsn_debug_lstm_tc_carry(const float* w_ih, const float* w_hh, con
                                        const float* x, int R, int T, int K, int H, int x3, const float* h_init, float* c,
                                        const int32_t* restart, int fin_step, float* hall, void* workspace,
                                        size_t workspace_bytes, fsn_stream_t stream) {
-  FSN_REQUIRE(fsn::lstm_rec_tc_supported(H, x3 != 0), FSN_ERR_UNSUPPORTED, "lstm_layer_tc: hidden size %d not supported", H);
-  FSN_REQUIRE(h_init && c && restart && hall && R > 0 && T > 0 && fin_step >= -1 && fin_step < T, FSN_ERR_SHAPE,
-              "lstm_tc_carry: bad argument (R=%d, T=%d, fin_step=%d)", R, T, fin_step);
-  fsn::Carver cv(workspace);
+  FSN_REQUIRE(h_init && c && restart, FSN_ERR_SHAPE, "lstm_tc_carry hook: null carry argument");
+  FSN_REQUIRE(fin_step >= -1 && fin_step < T, FSN_ERR_SHAPE, "lstm_tc_carry hook: fin_step %d outside [-1, T=%d)", fin_step, T);
   fsn::LstmTcWs ws;
-  fsn::lstm_tc_carve(cv, (size_t)R * T, K > H ? K : H, H, x3 != 0, ws);
-  FSN_REQUIRE(workspace && workspace_bytes >= cv.off, FSN_ERR_WORKSPACE, "workspace too small: %zu < %zu", workspace_bytes, cv.off);
+  int rc;
+  if ((rc = lstm_layer_hook_check(w_ih, w_hh, b_ih, b_hh, x, R, T, K, H, x3, hall, workspace, workspace_bytes, ws))) return rc;
+  FSN_REQUIRE(fsn::lstm_rec_tc_supported(H, x3 != 0), FSN_ERR_UNSUPPORTED, "lstm_layer_tc: hidden size %d not supported", H);
   fsn_lstm_layer L{w_ih, w_hh, b_ih, b_hh};
   const fsn::RecCarry io{h_init, c, c, (size_t)H, restart, fin_step};
   return fsn::lstm_layer_tc(L, x, (size_t)K, K, nullptr, 1, 0, R, T, H, x3 != 0, ws, hall, (cudaStream_t)stream, &io);
+}
+extern "C" size_t fsn_debug_lstm_rec_tc_scratch_bytes(int H, int x3) { return fsn::lstm_rec_tc_scratch_bytes(H, x3 != 0); }
+// the recurrence alone, on a given input projection P[r * p_row + t * p_t + gate * H + u], into hall[r * h_row + t * h_t
+// + u], as the layers call lstm_rec_tc_launch.  restart == nullptr: the plain kernel (zero initial state; h_init, c_init
+// and c_fin must be null); otherwise the carried-state kernel with RecCarry{h_init, c_init, c_fin, c_row, restart,
+// fin_step} (c_fin may be c_init).  info (nullable, 4 ints): rows per launch, ring stages, launches, dynamic shared memory.
+extern "C" int fsn_debug_lstm_rec_tc(const float* w_hh, const float* b_ih, const float* b_hh, const float* P, int64_t p_row,
+                                     int64_t p_t, float* hall, int64_t h_row, int64_t h_t, int R, int T, int H, int x3,
+                                     const float* h_init, const float* c_init, float* c_fin, int64_t c_row,
+                                     const int32_t* restart, int fin_step, int* info, void* scratch, size_t scratch_bytes,
+                                     fsn_stream_t stream) {
+  FSN_REQUIRE(w_hh && b_ih && b_hh && P && hall, FSN_ERR_SHAPE, "lstm_rec_tc hook: null argument");
+  FSN_REQUIRE(R > 0 && T > 0 && H > 0, FSN_ERR_SHAPE, "lstm_rec_tc hook: bad shape R=%d T=%d H=%d", R, T, H);
+  // a row of n floats per step, steps t_stride apart, rows row_stride apart: no two (row, step) blocks overlap
+  auto covers = [T](int64_t row_stride, int64_t t_stride, int64_t n) {
+    return t_stride >= n && t_stride <= (INT64_MAX - n) / T && row_stride >= (T - 1) * t_stride + n;
+  };
+  FSN_REQUIRE(covers(p_row, p_t, (int64_t)4 * H) && covers(h_row, h_t, H), FSN_ERR_SHAPE,
+              "lstm_rec_tc hook: strides P (%lld, %lld) / hall (%lld, %lld) do not cover T=%d steps of 4H / H (H=%d)",
+              (long long)p_row, (long long)p_t, (long long)h_row, (long long)h_t, T, H);
+  if (restart) {
+    FSN_REQUIRE(h_init && c_init && c_fin, FSN_ERR_SHAPE, "lstm_rec_tc hook: a carried state needs h_init, c_init and c_fin");
+    FSN_REQUIRE(c_row >= H, FSN_ERR_SHAPE, "lstm_rec_tc hook: c_row %lld < H=%d", (long long)c_row, H);
+    FSN_REQUIRE(fin_step >= -1 && fin_step < T, FSN_ERR_SHAPE, "lstm_rec_tc hook: fin_step %d outside [-1, T=%d)", fin_step, T);
+  } else {
+    FSN_REQUIRE(!h_init && !c_init && !c_fin, FSN_ERR_SHAPE, "lstm_rec_tc hook: carry pointers without a restart table");
+  }
+  const size_t need = fsn::lstm_rec_tc_scratch_bytes(H, x3 != 0);
+  FSN_REQUIRE(scratch && scratch_bytes >= need, FSN_ERR_WORKSPACE, "scratch too small: %zu < %zu", scratch_bytes, need);
+  const fsn::RecCarry io{h_init, c_init, c_fin, (size_t)c_row, restart, fin_step};
+  fsn::RecTcInfo got{};
+  const int rc = fsn::lstm_rec_tc_launch(w_hh, b_ih, b_hh, P, (size_t)p_row, (size_t)p_t, hall, (size_t)h_row, (size_t)h_t, R, T,
+                                         H, x3 != 0, scratch, (cudaStream_t)stream, restart ? &io : nullptr, &got);
+  if (info) memcpy(info, &got, sizeof(got));
+  return rc;
 }
 // unit-test hook of the tf32 GEMM path of the full-band stacks: out[rows, :N] (row stride ldo) = act(x' W^T + bias) with
 // x' = x[rows, :K] (row stride ldx) times its row scale, i.e. the input projection of lstm_layer_tc (prep_operand,

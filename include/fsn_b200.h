@@ -80,7 +80,8 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
  * fsn_debug_imp_section_lstm_tc hook: a caller of the shorter struct never selects them, so the version stays 102.  The
  * dense GEMM layer's unit-test hooks fsn_debug_fc_gemm, fsn_debug_sgemm, fsn_debug_colsum, fsn_debug_small_out_wgrad,
  * fsn_debug_transpose, fsn_debug_transpose_blocked and fsn_debug_gemm_tc are new symbols only, and so are the hooks of the
- * causal-norm scales, the layout kernels and the sub-band heads (fsn_debug_cum_clip_scale .. fsn_debug_train_dy). */
+ * causal-norm scales, the layout kernels and the sub-band heads (fsn_debug_cum_clip_scale .. fsn_debug_train_dy), and of
+ * the full-band recurrence alone (fsn_debug_lstm_rec_tc + its scratch query). */
 int fsn_version(void);
 const char* fsn_last_error(void);
 /* status code (FSN_ERR_*) of the last failed call on this thread: lets the *_workspace_bytes() functions, which
@@ -741,6 +742,21 @@ int fsn_debug_linear_tc(const float* x, int rows, int K, const float* W, const f
 int fsn_debug_lstm_tc_carry(const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* x,
                             int R, int T, int K, int H, int x3, const float* h_init, float* c, const int32_t* restart,
                             int fin_step, float* hall, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+/* the recurrence of that layer alone (lstm_rec_tc_kernel / lstm_rec_tc_carry_kernel), on a given input projection
+ * P[r*p_row + t*p_t + gate*H + u] (gate order i, f, g, o), h_t into hall[r*h_row + t*h_t + u]; P and hall 8-byte aligned,
+ * p_t >= 4H, p_row >= (T-1) p_t + 4H, h_t >= H, h_row >= (T-1) h_t + H.  restart NULL: zero initial state (h_init,
+ * c_init, c_fin must be NULL); otherwise row r enters step 0 with h_init / c_init [r*c_row + u] (c_row >= H) and step
+ * restart[r] with zero state, and c after step fin_step (-1: none) goes to c_fin [r*c_row + u] (c_fin may be c_init).
+ * info (nullable, 4 ints): rows per cooperative launch, TMA ring stages, launches, dynamic shared memory bytes.  Scratch:
+ * fsn_debug_lstm_rec_tc_scratch_bytes, the same for every H.  Every argument is checked before any CUDA call; an
+ * unsupported H (FSN_ERR_UNSUPPORTED) is reported after those checks.  fsn_debug_lstm_layer_tc, fsn_debug_lstm_tc_carry
+ * and fsn_debug_linear_tc check theirs the same way, except that the layer hooks report H below the kernel's minimum
+ * (64) as unsupported before they look at the workspace. */
+size_t fsn_debug_lstm_rec_tc_scratch_bytes(int H, int x3);
+int fsn_debug_lstm_rec_tc(const float* w_hh, const float* b_ih, const float* b_hh, const float* P, int64_t p_row, int64_t p_t,
+                          float* hall, int64_t h_row, int64_t h_t, int R, int T, int H, int x3, const float* h_init,
+                          const float* c_init, float* c_fin, int64_t c_row, const int32_t* restart, int fin_step, int* info,
+                          void* scratch, size_t scratch_bytes, fsn_stream_t stream);
 
 /* unit-test hook for the sub-band tensor-core stack (fsn_subband_tc.cu; model.py:98-135): packs sb (2 LSTM layers of
  * hidden size H over Ksb = (2Ns+1)+(2Nf+1) inputs, Linear(H -> fc_out <= 2)) into `packed`
