@@ -3,9 +3,9 @@ fullsubnet, precision="fp32") or fast_fullsubnet (fsn_fast_stream_step, --model 
 seconds enhanced per wall second and concurrent real-time streams for slots x K, with the whole-clip fp32 rate of the
 same process beside it (fsn_fullband_enhance; fullsubnet: fsn_enhance; fast_fullsubnet: Inferencer.enhance_batch).  For
 fullsubnet and fast_fullsubnet each line also says whether every slot stays real-time; for fast_fullsubnet it gives the
-bottleneck's share of the call's GPU time, from a torch.profiler pass of its own after the timed calls.  fullsubnet with
---precision f16x3_tc / f16_tc streams on the tensor cores (fsn_stream_tc_step), gives the launches per call, and the
-whole-clip rate beside it is of that precision.  Prints one JSON line per configuration and a header line with the GPU,
+bottleneck's share of the call's GPU time, from a torch.profiler pass of its own after the timed calls.  fullsubnet and
+fast_fullsubnet with --precision f16x3_tc / f16_tc stream on the tensor cores (fsn_stream_tc_step, fsn_fast_stream_tc_step),
+give the launches per call, and the whole-clip rate beside them is of that precision (fast_fullsubnet: also at B = 256).  Prints one JSON line per configuration and a header line with the GPU,
 power limit and clocks.
 
     python bench_stream.py [--model fullband_baseline] [--precision fp32] [--slots 1 64 256] [--ks 1 4 16 64]
@@ -38,7 +38,7 @@ def model(name, norm, dev, precision="fp32"):
         from fullsubnet_b200.fast_fullsubnet.model import Model
         from oracle import fast_fullsubnet_oracle as FO
         args = dict(FO.DEFAULT_FAST_ARGS, norm_type=norm)
-        m = Model(**args, precision="fp32")
+        m = Model(**args, precision=precision)
         m.load_state_dict(FO.make_fast_state_dict(seed=11, args=args), strict=True)
         return m.to(dev).eval()
     if name == "fullsubnet":
@@ -58,7 +58,8 @@ def model(name, norm, dev, precision="fp32"):
 
 def bottleneck_share(step, calls=3):
     """Share of the GPU time of `calls` streaming calls spent in fast_fullsubnet's bottleneck: the kernels and copies
-    from fast_stream_open_kernel up to fast_stream_dec_input_kernel, over all of them."""
+    from fast_stream_open_kernel up to fast_stream_dec_input_kernel, over all of them (on the tensor cores: the input
+    and norm kernels, the one sb_phased_lstm_tc_kernel launch and the output carry)."""
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(calls):
@@ -100,11 +101,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--norm", default="cumulative_laplace_norm")
     ap.add_argument("--model", default="fullband_baseline", choices=["fullband_baseline", "fullsubnet", "fast_fullsubnet"])
-    # fullsubnet only: f16x3_tc / f16_tc stream on the tensor cores (Streamer(tensor_cores=True)), and the whole-clip rate
-    # is of the same precision
+    # fullsubnet and fast_fullsubnet: f16x3_tc / f16_tc stream on the tensor cores (Streamer(tensor_cores=True)), and
+    # the whole-clip rate is of the same precision
     ap.add_argument("--precision", default="fp32", choices=["fp32", "f16x3_tc", "f16_tc"])
     a = ap.parse_args()
-    assert a.precision == "fp32" or a.model == "fullsubnet", "--precision is for --model fullsubnet"
+    assert a.precision == "fp32" or a.model != "fullband_baseline", "--precision is for fullsubnet and fast_fullsubnet"
     tc = a.precision != "fp32"
     assert torch.cuda.is_available(), "bench_stream.py needs a CUDA device"
     dev = torch.device("cuda:0")
@@ -139,7 +140,7 @@ def main():
         whole = Inferencer(model=m, device=dev).enhance_batch
     else:
         whole = m.enhance
-    for B in (1, 64):
+    for B in ((1, 64, 256) if fast and tc else (1, 64)):
         y = (0.1 * torch.randn(B, 4 * SR, generator=g)).to(dev)
         ms = time_ms(lambda: whole(y), max(3, a.calls // 4), a.warmup)
         print(json.dumps({"whole_clip": True, "B": B, "clip_s": 4.0, "ms_per_call": round(ms, 3),

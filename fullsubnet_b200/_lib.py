@@ -167,6 +167,11 @@ _SIGNATURES = {
     "fsn_fast_stream_delay": (C.c_int, [C.POINTER(FastDesc), _I, _I]),
     "fsn_fast_stream_step": (C.c_int, [C.POINTER(FastDesc), C.POINTER(FastWeights), _P, _P, _P, _I, _I, _I, _I, _I, _P, _P,
                                        _S, _P, _S, _P]),
+    "fsn_fast_stream_tc_state_bytes": (_S, [C.POINTER(FastDesc), _I, _I, _I]),
+    "fsn_fast_stream_tc_workspace_bytes": (_S, [C.POINTER(FastDesc), _I, _I, _I, _I]),
+    "fsn_fast_stream_tc_delay": (C.c_int, [C.POINTER(FastDesc), _I, _I]),
+    "fsn_fast_stream_tc_step": (C.c_int, [C.POINTER(FastDesc), C.POINTER(FastWeights), _P, _P, _P, _I, _I, _I, _I, _I, _P,
+                                          _P, _S, _P, _S, _P]),
     "fsn_stream_state_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I]),
     "fsn_stream_workspace_bytes": (_S, [C.POINTER(ModelDesc), _I, _I, _I, _I]),
     "fsn_stream_delay": (C.c_int, [C.POINTER(ModelDesc), _I, _I]),
@@ -204,6 +209,8 @@ _SIGNATURES = {
                                        _I, _I, _I, _I, _P, _P, _P]),
     "fsn_debug_sb_lstm_tc_carry": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _I, _P,
                                              _I, _P, _P, _P, _P, _P]),
+    "fsn_debug_sb_lstm_tc_phased": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _P,
+                                              _P, _P, _P, _P, _P, _P, _P]),
     "fsn_debug_sb_lstm_tc_probe": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P,
                                              _I, _I, _I, _I, _I, _P, _P, _P, _I, _I, _P]),
     "fsn_debug_tgemm": (C.c_int, [_P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _P, _L, _P]),

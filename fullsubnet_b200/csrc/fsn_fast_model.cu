@@ -240,7 +240,8 @@ extern "C" int fsn_fast_model_forward(const fsn_fast_desc* d, const fsn_fast_wei
 // ---- chunked streaming (DESIGN 4.14).  Slot state block: the stream header (StreamSlot), then the last S-1 frames of
 // the mel spectrogram and of the encoder output (M each), encoder (h | c) of both layers, the second norm's running sum
 // and the latest bottleneck output of the M rows, bottleneck (h | c) of both layers (M x Hb each), decoder (h | c) of
-// both layers.
+// both layers.  The tensor-core stream (fsn_fast_stream_tc_*, DESIGN 4.14.2) keeps the same block; its bottleneck is one
+// sb_phased_lstm_tc_kernel launch over all block ends of the call instead of the per-step loop.
 namespace fsn {
 
 struct FastStreamLayout : StreamSlot { size_t mel, enc, eh, ec, run, bo, bh, bc, dh, dc; };
@@ -257,13 +258,24 @@ static FastStreamLayout fast_stream_layout(const fsn_fast_desc* d, const StreamG
   return s;
 }
 
-static int fast_stream_check(const fsn_fast_desc* d, int n_fft, int hop, int win_length, FastDims& m, StreamGeom& g) {
+// tc: the tensor-core stream (fsn_fast_stream_tc_*), which takes FSN_PREC_F16X3_TC / FSN_PREC_F16_TC instead of
+// FSN_PREC_FP32 and the bottleneck shapes the wgmma kernel takes
+static int fast_stream_check(const fsn_fast_desc* d, int n_fft, int hop, int win_length, FastDims& m, StreamGeom& g,
+                             bool tc = false) {
   int rc = fast_dims(d, 1, 2, m);
   if (rc) return rc;
   FSN_REQUIRE(d->norm_type == FSN_NORM_CUMULATIVE_LAPLACE, FSN_ERR_UNSUPPORTED,
               "fast_stream: the offline norm needs the whole clip; streaming is built for cumulative_laplace_norm");
-  FSN_REQUIRE(d->precision == FSN_PREC_FP32, FSN_ERR_UNSUPPORTED,
-              "fast_stream: streaming is built for FSN_PREC_FP32 (precision %d)", d->precision);
+  if (tc) {
+    FSN_REQUIRE(fast_is_tc(d), FSN_ERR_UNSUPPORTED,
+                "fast_stream_tc: the tensor-core stream is built for FSN_PREC_F16X3_TC and FSN_PREC_F16_TC (precision %d); "
+                "the fp32 kernels stream through fsn_fast_stream_step", d->precision);
+    FSN_REQUIRE(fast_tc_ok(d), FSN_ERR_UNSUPPORTED,
+                "fast_stream_tc: the tensor-core bottleneck needs bn_hidden = 384, 2 layers and input width <= 32");
+  } else {
+    FSN_REQUIRE(d->precision == FSN_PREC_FP32, FSN_ERR_UNSUPPORTED,
+                "fast_stream: streaming is built for FSN_PREC_FP32 (precision %d)", d->precision);
+  }
   FSN_REQUIRE(n_fft / 2 + 1 == d->num_freqs, FSN_ERR_SHAPE, "fast_stream: n_fft/2+1 = %d != num_freqs = %d", n_fft / 2 + 1,
               d->num_freqs);
   return stream_geom(n_fft, hop, win_length, d->look_ahead, g);
@@ -274,13 +286,24 @@ struct FastStreamWs : StreamWs {
   float *melT, *scale1, *encT, *catM, *catE, *bn, *scale2, *bo, *dec_in, *y;
   float2* fs;
   StreamStackWs stack;                        // encoder and decoder, one after the other
-  float *bh0[2], *bh1[2], *bc0, *bc1;         // bottleneck state, h ping-pong per layer
+  float *bh0[2], *bh1[2], *bc0, *bc1;         // bottleneck state, h ping-pong per layer (fp32 stream)
+  float* x;                                   // tensor-core stream: the bottleneck's scaled input [nb, R, K]
+  int *sb_rst, *store;                        // ... and per slot its restart step (0 or none) and its store step
 };
 
+// element (b, m, col) of the bottleneck outputs bo at b bs + m ms + col cs; column 0 is the output carried into the call,
+// column i + 1 that of bottleneck step i.  fp32 stream: [B, M, nb + 1]; tensor-core stream: the frame-major [B, nb + 1, 2M]
+// the sub-band kernel's carry output writes (its second, zero-padded output row at columns M .. 2M)
+struct BoGeom { size_t bs, ms, cs; };
+static BoGeom fast_bo_geom(bool tc, int M, int nb) {
+  return tc ? BoGeom{(size_t)(nb + 1) * 2 * M, 1, 2 * (size_t)M} : BoGeom{(size_t)M * (nb + 1), (size_t)nb + 1, 1};
+}
+
 // St = K + E steps: a call with a clip's last chunk runs E steps past the K of the others; nb = ceil(St / S) bottleneck
-// steps, the most block ends St consecutive frames can hold.  Returns the bytes
+// steps, the most block ends St consecutive frames can hold.  tc: the bottleneck's state stays in the slot state (no
+// per-row buffers), its input is carved instead.  Returns the bytes
 static size_t fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const StreamGeom& g, int B, int K, void* base,
-                                FastStreamWs& w) {
+                                FastStreamWs& w, bool tc = false) {
   Carver c(base);
   const size_t F = m.F, M = m.M, St = (size_t)K + g.E, Hm = m.S - 1, nb = cdiv((int)St, m.S), R = (size_t)B * M;
   const size_t Hb = d->bn_hidden;
@@ -295,9 +318,19 @@ static size_t fast_stream_carve(const fsn_fast_desc* d, const FastDims& m, const
   w.catE = c.take<float>(B * (Hm + St) * M);
   w.bn = c.take<float>(nb * R * m.K);
   w.scale2 = c.take<float>(nb * R);
-  w.bo = c.take<float>(R * (nb + 1));
-  for (int i = 0; i < 2; ++i) { w.bh0[i] = c.take<float>(R * Hb); w.bh1[i] = c.take<float>(R * Hb); }
-  w.bc0 = c.take<float>(R * Hb); w.bc1 = c.take<float>(R * Hb);
+  memset(w.bh0, 0, sizeof(w.bh0)); memset(w.bh1, 0, sizeof(w.bh1));
+  w.bc0 = w.bc1 = w.x = nullptr;
+  w.sb_rst = w.store = nullptr;
+  if (tc) {
+    w.bo = c.take<float>(R * 2 * (nb + 1));
+    w.x = c.take<float>(nb * R * m.K);
+    w.sb_rst = c.take<int>(B);
+    w.store = c.take<int>(B);
+  } else {
+    w.bo = c.take<float>(R * (nb + 1));
+    for (int i = 0; i < 2; ++i) { w.bh0[i] = c.take<float>(R * Hb); w.bh1[i] = c.take<float>(R * Hb); }
+    w.bc0 = c.take<float>(R * Hb); w.bc1 = c.take<float>(R * Hb);
+  }
   w.dec_in = c.take<float>(B * St * 2 * M);
   w.y = c.take<float>(B * St * 2 * F);
   return c.off;
@@ -313,11 +346,15 @@ __device__ __forceinline__ int fs_ends_before(int jf, int S, int lim) { return l
 
 // Before the bottleneck: per slot b (grid.y), the bottleneck's h / c entering the call into h0p / h1p (the ping-pong
 // halves step 0 reads) and c0 / c1, zero when the clip's frame 0 is in the call (its first block end is block 0); the
-// latest bottleneck output into column 0 of bo [R, nb+1]; the decoder's restart step rst[b] (frame 0 at step rst).
-__global__ void fast_stream_open_kernel(const int* __restrict__ pos0, int hop, int c, int St, int M, int Hb, int nb,
-                                        const char* __restrict__ state, size_t slot_bytes, size_t bh, size_t bc, size_t bo_off,
-                                        float* __restrict__ h0p, float* __restrict__ h1p, float* __restrict__ c0,
-                                        float* __restrict__ c1, float* __restrict__ bo, int* __restrict__ rst) {
+// latest bottleneck output into column 0 of bo; the decoder's restart step rst[b] (frame 0 at step rst).  Tensor-core
+// stream (h0p null, sb_rst non-null): the kernel reads h / c from the state itself, so instead its restart step sb_rst[b]
+// (0 when the first block end is block 0, else none) and its store step store[b] (fast_stream_commit_kernel's rule)
+__global__ void fast_stream_open_kernel(const int* __restrict__ pos0, const int* __restrict__ act0, int hop, int c, int St,
+                                        int K, int S, int M, int Hb, const char* __restrict__ state, size_t slot_bytes,
+                                        size_t bh, size_t bc, size_t bo_off, float* __restrict__ h0p, float* __restrict__ h1p,
+                                        float* __restrict__ c0, float* __restrict__ c1, float* __restrict__ bo,
+                                        const BoGeom bg, int* __restrict__ rst, int* __restrict__ sb_rst,
+                                        int* __restrict__ store) {
   const int b = blockIdx.y;
   const int m0 = pos0[b] / hop - c;
   const bool fresh = m0 <= 0 && -m0 < St;
@@ -325,7 +362,7 @@ __global__ void fast_stream_open_kernel(const int* __restrict__ pos0, int hop, i
   const char* sb = state + (size_t)b * slot_bytes;
   const float* sh = reinterpret_cast<const float*>(sb + bh);
   const float* sc = reinterpret_cast<const float*>(sb + bc);
-  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; h0p && e < n; e += (size_t)gridDim.x * blockDim.x) {
     h0p[o + e] = fresh ? 0.f : sh[e];
     h1p[o + e] = fresh ? 0.f : sh[n + e];
     c0[o + e] = fresh ? 0.f : sc[e];
@@ -333,17 +370,24 @@ __global__ void fast_stream_open_kernel(const int* __restrict__ pos0, int hop, i
   }
   if (blockIdx.x == 0) {
     const float* sbo = reinterpret_cast<const float*>(sb + bo_off);
-    for (int r = threadIdx.x; r < M; r += blockDim.x) bo[((size_t)b * M + r) * (nb + 1)] = sbo[r];
-    if (threadIdx.x == 0) rst[b] = -m0;
+    for (int r = threadIdx.x; r < M; r += blockDim.x) bo[(size_t)b * bg.bs + (size_t)r * bg.ms] = sbo[r];
+    if (threadIdx.x == 0) {
+      rst[b] = -m0;
+      if (sb_rst) {
+        sb_rst[b] = fresh ? 0 : -1;
+        store[b] = act0[b] ? fs_ends_before(fs_first_end(m0, S), S, K) - 1 : -1;
+      }
+    }
   }
 }
 
 // Bottleneck input of the i-th block end of slot b (grid (nb, B)): fast_bn_input_kernel's arithmetic on the block's frames,
 // read from catM / catE [B, S-1+St, M] (the carried S-1 frames, then the call's), into bn [nb, B*M, K]; 0 past the slot's
-// last block end in the call
+// last block end in the call.  scale non-null (the tensor-core stream): the input the sub-band kernel's gather forms
+// with `shrink`, the block sum times (1/len * scale [nb, B*M] of the row), instead of the block mean
 __global__ void fast_stream_bn_input_kernel(const float* __restrict__ catM, const float* __restrict__ catE,
                                             const int* __restrict__ pos0, int hop, int c, int St, int M, int Nn, int Ne,
-                                            int S, float* __restrict__ bn) {
+                                            int S, float* __restrict__ bn, const float* __restrict__ scale) {
   const int i = blockIdx.x, b = blockIdx.y, B = gridDim.y;
   const int K = (2 * Nn + 1) + (2 * Ne + 1);
   const int m0 = pos0[b] / hop - c;
@@ -363,7 +407,7 @@ __global__ void fast_stream_bn_input_kernel(const float* __restrict__ catM, cons
         acc += (k < 2 * Nn + 1) ? catM[base + reflect_idx(mm + k - Nn, M)]
                                 : catE[base + reflect_idx(mm + (k - (2 * Nn + 1)) - Ne, M)];
       }
-      v = acc * inv;
+      v = scale ? acc * (inv * scale[(size_t)i * B * M + (size_t)b * M + mm]) : acc * inv;
     }
     bn[((size_t)i * B * M + (size_t)b * M + mm) * K + k] = v;
   }
@@ -422,10 +466,20 @@ __global__ void fast_stream_commit_kernel(const int* __restrict__ pos0, const in
   }
 }
 
+// Tensor-core stream, after the bottleneck: slot b (block b) stores the output of its store step store[b] as its latest
+// bottleneck output (the sub-band kernel stored its (h, c) after that step)
+__global__ void fast_stream_bo_store_kernel(const int* __restrict__ store, int M, const float* __restrict__ bo,
+                                            const BoGeom bg, char* __restrict__ state, size_t slot_bytes, size_t bo_off) {
+  const int b = blockIdx.x, i = store[b];
+  if (i < 0) return;
+  float* sbo = reinterpret_cast<float*>(state + (size_t)b * slot_bytes + bo_off);
+  for (int r = threadIdx.x; r < M; r += blockDim.x) sbo[r] = bo[(size_t)b * bg.bs + (size_t)r * bg.ms + (size_t)(i + 1) * bg.cs];
+}
+
 // Decoder input (fast_dec_input_kernel's concatenation): dec_in [B, St, 2M] row (b, j) = encoder output of step j | the
 // bottleneck output of the latest block end at or before step j (column 0 of bo: the one carried into the call)
-__global__ void fast_stream_dec_input_kernel(const float* __restrict__ encT, const float* __restrict__ bo,
-                                             const int* __restrict__ pos0, int hop, int c, int B, int St, int M, int S, int nb,
+__global__ void fast_stream_dec_input_kernel(const float* __restrict__ encT, const float* __restrict__ bo, const BoGeom bg,
+                                             const int* __restrict__ pos0, int hop, int c, int B, int St, int M, int S,
                                              float* __restrict__ dec_in) {
   const size_t n = (size_t)B * St * 2 * M;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -436,65 +490,73 @@ __global__ void fast_stream_dec_input_kernel(const float* __restrict__ encT, con
       dec_in[i] = encT[q * M + col];
     } else {
       const int e = fs_ends_before(fs_first_end(pos0[b] / hop - c, S), S, j + 1);
-      dec_in[i] = bo[((size_t)b * M + (col - M)) * (nb + 1) + e];
+      dec_in[i] = bo[(size_t)b * bg.bs + (size_t)(col - M) * bg.ms + (size_t)e * bg.cs];
     }
   }
 }
 
 }  // namespace fsn
 
-extern "C" size_t fsn_fast_stream_state_bytes(const fsn_fast_desc* d, int B, int n_fft, int hop) {
+namespace fsn {
+
+static size_t fast_stream_state_query(const fsn_fast_desc* d, int B, int n_fft, int hop, bool tc) {
   FastDims m;
   StreamGeom g;
-  return stream_query_check(fast_stream_check(d, n_fft, hop, n_fft, m, g), "fast_stream", B, 1)
+  return stream_query_check(fast_stream_check(d, n_fft, hop, n_fft, m, g, tc), tc ? "fast_stream_tc" : "fast_stream", B, 1)
              ? 0 : fast_stream_layout(d, g).slot() * (size_t)B;
 }
 
-extern "C" size_t fsn_fast_stream_workspace_bytes(const fsn_fast_desc* d, int B, int K_max, int n_fft, int hop) {
+static size_t fast_stream_workspace_query(const fsn_fast_desc* d, int B, int K_max, int n_fft, int hop, bool tc) {
   FastDims m;
   StreamGeom g;
   FastStreamWs w;
-  return stream_query_check(fast_stream_check(d, n_fft, hop, n_fft, m, g), "fast_stream", B, K_max)
-             ? 0 : fast_stream_carve(d, m, g, B, K_max, nullptr, w);
+  return stream_query_check(fast_stream_check(d, n_fft, hop, n_fft, m, g, tc), tc ? "fast_stream_tc" : "fast_stream", B,
+                            K_max)
+             ? 0 : fast_stream_carve(d, m, g, B, K_max, nullptr, w, tc);
 }
 
-extern "C" int fsn_fast_stream_delay(const fsn_fast_desc* d, int n_fft, int hop) {
+static int fast_stream_delay_query(const fsn_fast_desc* d, int n_fft, int hop, bool tc) {
   FastDims m;
   StreamGeom g;
-  return stream_delay(fast_stream_check(d, n_fft, hop, n_fft, m, g), g);
+  return stream_delay(fast_stream_check(d, n_fft, hop, n_fft, m, g, tc), g);
 }
 
-extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* wav,
-                                    const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
-                                    int win_length, float* enhanced, void* state, size_t state_bytes, void* workspace,
-                                    size_t workspace_bytes, fsn_stream_t stream) {
+// one call of either stream.  tc: the encoder and decoder on the path the whole-clip call takes (SEQ_PATH_TC with the
+// restart table stream_open writes), and the bottleneck in one sb_phased_lstm_tc_kernel launch over all nb steps of
+// every row, its input formed first by fast_stream_bn_input_kernel with the second norm's scales
+static int fast_stream_run(const fsn_fast_desc* d, const fsn_fast_weights* wt, bool tc, const float* wav,
+                           const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop, int win_length,
+                           float* enhanced, void* state, size_t state_bytes, void* workspace, size_t workspace_bytes,
+                           cudaStream_t st) {
   launch_counter() = 0;
   FastDims m;
   StreamGeom g;
-  int St, rc = fast_stream_check(d, n_fft, hop, win_length, m, g);
-  if (rc || (rc = stream_check("fast_stream", g, B, K, tail, wav, enhanced, St))) return rc;
+  int St, rc = fast_stream_check(d, n_fft, hop, win_length, m, g, tc);
+  if (rc || (rc = stream_check(tc ? "fast_stream_tc" : "fast_stream", g, B, K, tail, wav, enhanced, St))) return rc;
   FSN_REQUIRE(wt, FSN_ERR_SHAPE, "fast_stream: null weights");
+  FSN_REQUIRE(!tc || wt->bn_packed, FSN_ERR_SHAPE,
+              "fast_stream_tc: the tensor-core stream needs the packed bottleneck weights (fsn_fast_pack_bn_weights)");
   const FastStreamLayout sl = fast_stream_layout(d, g);
   FastStreamWs w;
-  const size_t ws = fast_stream_carve(d, m, g, B, K, workspace, w);
+  const size_t ws = fast_stream_carve(d, m, g, B, K, workspace, w, tc);
   if ((rc = stream_check_sizes(state, state_bytes, sl.slot(), B, workspace, workspace_bytes, ws))) return rc;
-  const cudaStream_t st = (cudaStream_t)stream;
   char* sb = (char*)state;
   const size_t ss = sl.slot();
   const int F = m.F, M = m.M, S = m.S, Kf = m.K, Hm = S - 1, R = B * M, nb = cdiv(St, S);
   const int Hb = d->bn_hidden;
   const size_t catw = (size_t)(Hm + St) * M * 4;
-  if ((rc = stream_open(g, sl, w, F, B, K, St, win_length, start, tail, wav, sb, nullptr, st))) return rc;
+  if ((rc = stream_open(g, sl, w, F, B, K, St, win_length, start, tail, wav, sb, tc ? w.rst : nullptr, st))) return rc;
   // Mel filtering and the first norm over the mel frame sums (model.py:161-170)
   if ((rc = fc_gemm_launch(w.magT, wt->mel_fb, nullptr, w.melT, B * St, F, M, FSN_ACT_NONE, st, /*w_kmajor=*/true))) return rc;
   if ((rc = frame_stats_launch(w.melT, B, St, M, 0, (size_t)St * M, M, w.fs, st))) return rc;
   if ((rc = stream_norm_launch(w.fs, B, St, K, M, g, d->norm_type, w.pos0, w.act0, w.tail, sb, ss, w.scale1, st))) return rc;
-  // encoder, (h, c) carried; its per-step scale keeps it off the paths that read the restart table, which
-  // fast_stream_open_kernel writes only later in the call
+  // encoder, (h, c) carried.  fp32: its per-step scale keeps it off the paths that read the restart table, which
+  // fast_stream_open_kernel writes only later in the call; tc: on SEQ_PATH_TC it reads the table stream_open wrote
   SeqStack enc = fast_pair(d, B, St, false);
   enc.L[0] = wt->enc1; enc.L[1] = wt->enc2;
   enc.x = w.melT; enc.scale = w.scale1; enc.fc_w = wt->enc_fc_w; enc.fc_b = wt->enc_fc_b; enc.out = w.encT;
-  if ((rc = stream_seq_stack(enc, w.stack, StackCarry{sb, ss, sl.eh, sl.ec, w.pos0, g, nullptr, K}, st))) return rc;
+  if ((rc = stream_seq_stack(enc, w.stack, StackCarry{sb, ss, sl.eh, sl.ec, w.pos0, g, tc ? w.rst : nullptr, K}, st)))
+    return rc;
   // the carried S-1 frames, then the call's, of the mel spectrogram and the encoder output: the frames the blocks average
   if (Hm > 0) {
     if ((rc = copy_rows(w.catM, catw, sb + sl.mel, ss, (size_t)Hm * M * 4, B, st))) return rc;
@@ -503,42 +565,61 @@ extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weigh
   if ((rc = copy_rows(w.catM + (size_t)Hm * M, catw, w.melT, (size_t)St * M * 4, (size_t)St * M * 4, B, st))) return rc;
   if ((rc = copy_rows(w.catE + (size_t)Hm * M, catw, w.encT, (size_t)St * M * 4, (size_t)St * M * 4, B, st))) return rc;
   // bottleneck: one step per block end, every row at its slot's i-th block end of the call (model.py:174-189)
-  const dim3 sgrid(cdiv(M * Hb, 256), B);
-  fast_stream_open_kernel<<<sgrid, 256, 0, st>>>(w.pos0, hop, g.c, St, M, Hb, nb, sb, ss, sl.bh, sl.bc, sl.bo, w.bh0[1],
-                                                w.bh1[1], w.bc0, w.bc1, w.bo, w.rst);
+  const BoGeom bg = fast_bo_geom(tc, M, nb);
+  const dim3 sgrid(tc ? 1 : cdiv(M * Hb, 256), B);
+  fast_stream_open_kernel<<<sgrid, 256, 0, st>>>(w.pos0, w.act0, hop, g.c, St, K, S, M, Hb, sb, ss, sl.bh, sl.bc, sl.bo,
+                                                w.bh0[1], w.bh1[1], w.bc0, w.bc1, w.bo, bg, w.rst, w.sb_rst, w.store);
   FSN_CHECK_LAUNCH("fast_stream_open_kernel");
   fast_stream_bn_input_kernel<<<dim3(nb, B), 256, 0, st>>>(w.catM, w.catE, w.pos0, hop, g.c, St, M, d->noisy_num_neighbors,
-                                                            d->enc_num_neighbors, S, w.bn);
+                                                            d->enc_num_neighbors, S, w.bn, nullptr);
   FSN_CHECK_LAUNCH("fast_stream_bn_input_kernel");
   fast_stream_bn_scale_kernel<<<cdiv(R, 128), 128, 0, st>>>(w.bn, w.pos0, w.act0, hop, g.c, St, K, R, M, Kf, S, nb,
                                                              TRAIN_CUM_EPS, sb, ss, sl.run, w.scale2);
   FSN_CHECK_LAUNCH("fast_stream_bn_scale_kernel");
-  for (int i = 0; i < nb; ++i) {
-    StepParams p;
-    memset(&p, 0, sizeof(p));
-    p.R = R; p.K0 = Kf; p.H = Hb;
-    p.w_ih = wt->bn[0].w_ih; p.w_hh = wt->bn[0].w_hh; p.b_ih = wt->bn[0].b_ih; p.b_hh = wt->bn[0].b_hh;
-    p.x0 = w.bn + (size_t)i * R * Kf; p.x0_row_stride = Kf;
-    p.row_scale = w.scale2 + (size_t)i * R; p.row_scale_div = 1;
-    p.h_prev = w.bh0[(i + 1) & 1]; p.h_out = w.bh0[i & 1]; p.h_prev_stride = p.h_out_stride = Hb;
-    p.c = w.bc0;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-    p.K0 = Hb;
-    p.w_ih = wt->bn[1].w_ih; p.w_hh = wt->bn[1].w_hh; p.b_ih = wt->bn[1].b_ih; p.b_hh = wt->bn[1].b_hh;
-    p.x0 = w.bh0[i & 1]; p.x0_row_stride = Hb; p.row_scale = nullptr; p.row_scale_div = 0;
-    p.h_prev = w.bh1[(i + 1) & 1]; p.h_out = w.bh1[i & 1];
-    p.c = w.bc1;
-    if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
-    if ((rc = sb_head_launch(w.bh1[i & 1], R, Hb, 1, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bo,
-                             HeadGeom{R, 1, 0, 0, (size_t)nb + 1}, i + 1, st)))
-      return rc;
-    fast_stream_commit_kernel<<<sgrid, 256, 0, st>>>(w.pos0, w.act0, hop, g.c, K, S, M, Hb, nb, i, w.bh0[i & 1],
-                                                     w.bh1[i & 1], w.bc0, w.bc1, w.bo, sb, ss, sl.bh, sl.bc, sl.bo);
-    FSN_CHECK_LAUNCH("fast_stream_commit_kernel");
+  if (tc) {
+    // the input the whole-clip gather forms for each block, then all nb steps in one launch: (h, c) from and back to the
+    // state, step i's output (and the zero-padded second one) into column i + 1 of bo
+    fast_stream_bn_input_kernel<<<dim3(nb, B), 256, 0, st>>>(w.catM, w.catE, w.pos0, hop, g.c, St, M,
+                                                              d->noisy_num_neighbors, d->enc_num_neighbors, S, w.x, w.scale2);
+    FSN_CHECK_LAUNCH("fast_stream_bn_input_kernel");
+    SbTcArgs a;
+    memset(&a, 0, sizeof(a));
+    a.packed = wt->bn_packed; a.crm = w.bo;
+    a.B = B; a.F = M; a.Tp = nb; a.la = 0; a.Ns = d->noisy_num_neighbors; a.Nf = d->enc_num_neighbors; a.H = Hb;
+    a.act = FSN_ACT_RELU; a.x3 = fast_x3(d); a.map = RowMap{B, M, M, 1};
+    const SbCarry io{(float*)(sb + sl.bh), (float*)(sb + sl.bc), ss / 4, (size_t)M * Hb, M, w.sb_rst, -1, bg.bs, 1, w.x,
+                     w.store};
+    if ((rc = sb_tc_carry_forward(a, io, st))) return rc;
+    fast_stream_bo_store_kernel<<<B, 64, 0, st>>>(w.store, M, w.bo, bg, sb, ss, sl.bo);
+    FSN_CHECK_LAUNCH("fast_stream_bo_store_kernel");
+  } else {
+    for (int i = 0; i < nb; ++i) {
+      StepParams p;
+      memset(&p, 0, sizeof(p));
+      p.R = R; p.K0 = Kf; p.H = Hb;
+      p.w_ih = wt->bn[0].w_ih; p.w_hh = wt->bn[0].w_hh; p.b_ih = wt->bn[0].b_ih; p.b_hh = wt->bn[0].b_hh;
+      p.x0 = w.bn + (size_t)i * R * Kf; p.x0_row_stride = Kf;
+      p.row_scale = w.scale2 + (size_t)i * R; p.row_scale_div = 1;
+      p.h_prev = w.bh0[(i + 1) & 1]; p.h_out = w.bh0[i & 1]; p.h_prev_stride = p.h_out_stride = Hb;
+      p.c = w.bc0;
+      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+      p.K0 = Hb;
+      p.w_ih = wt->bn[1].w_ih; p.w_hh = wt->bn[1].w_hh; p.b_ih = wt->bn[1].b_ih; p.b_hh = wt->bn[1].b_hh;
+      p.x0 = w.bh0[i & 1]; p.x0_row_stride = Hb; p.row_scale = nullptr; p.row_scale_div = 0;
+      p.h_prev = w.bh1[(i + 1) & 1]; p.h_out = w.bh1[i & 1];
+      p.c = w.bc1;
+      if ((rc = lstm_step_launch(p, SEG0_DENSE, st))) return rc;
+      if ((rc = sb_head_launch(w.bh1[i & 1], R, Hb, 1, wt->bn_fc_w, wt->bn_fc_b, 1, FSN_ACT_RELU, w.bo,
+                               HeadGeom{R, 1, 0, 0, (size_t)nb + 1}, i + 1, st)))
+        return rc;
+      fast_stream_commit_kernel<<<sgrid, 256, 0, st>>>(w.pos0, w.act0, hop, g.c, K, S, M, Hb, nb, i, w.bh0[i & 1],
+                                                       w.bh1[i & 1], w.bc0, w.bc1, w.bo, sb, ss, sl.bh, sl.bc, sl.bo);
+      FSN_CHECK_LAUNCH("fast_stream_commit_kernel");
+    }
   }
   // decoder input: encoder output | up-sampled bottleneck output (model.py:191-194)
-  fast_stream_dec_input_kernel<<<ew_grid((size_t)B * St * 2 * M), 256, 0, st>>>(w.encT, w.bo, w.pos0, hop, g.c, B, St, M, S,
-                                                                                 nb, w.dec_in);
+  fast_stream_dec_input_kernel<<<ew_grid((size_t)B * St * 2 * M), 256, 0, st>>>(w.encT, w.bo, bg, w.pos0, hop, g.c, B, St, M,
+                                                                                 S, w.dec_in);
   FSN_CHECK_LAUNCH("fast_stream_dec_input_kernel");
   // decoder, (h, c) carried, restarting at rst
   SeqStack dec = fast_pair(d, B, St, true);
@@ -551,4 +632,80 @@ extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weigh
     if ((rc = copy_rows(sb + sl.enc, ss, w.catE + (size_t)K * M, catw, (size_t)Hm * M * 4, B, st))) return rc;
   }
   return stream_close(g, sl, w, F, B, K, St, win_length, w.y, enhanced, sb, st);
+}
+
+}  // namespace fsn
+
+extern "C" size_t fsn_fast_stream_state_bytes(const fsn_fast_desc* d, int B, int n_fft, int hop) {
+  return fast_stream_state_query(d, B, n_fft, hop, false);
+}
+
+extern "C" size_t fsn_fast_stream_workspace_bytes(const fsn_fast_desc* d, int B, int K_max, int n_fft, int hop) {
+  return fast_stream_workspace_query(d, B, K_max, n_fft, hop, false);
+}
+
+extern "C" int fsn_fast_stream_delay(const fsn_fast_desc* d, int n_fft, int hop) {
+  return fast_stream_delay_query(d, n_fft, hop, false);
+}
+
+extern "C" int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* wav,
+                                    const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
+                                    int win_length, float* enhanced, void* state, size_t state_bytes, void* workspace,
+                                    size_t workspace_bytes, fsn_stream_t stream) {
+  return fast_stream_run(d, wt, false, wav, start, tail, B, K, n_fft, hop, win_length, enhanced, state, state_bytes,
+                         workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t fsn_fast_stream_tc_state_bytes(const fsn_fast_desc* d, int B, int n_fft, int hop) {
+  return fast_stream_state_query(d, B, n_fft, hop, true);
+}
+
+extern "C" size_t fsn_fast_stream_tc_workspace_bytes(const fsn_fast_desc* d, int B, int K_max, int n_fft, int hop) {
+  return fast_stream_workspace_query(d, B, K_max, n_fft, hop, true);
+}
+
+extern "C" int fsn_fast_stream_tc_delay(const fsn_fast_desc* d, int n_fft, int hop) {
+  return fast_stream_delay_query(d, n_fft, hop, true);
+}
+
+extern "C" int fsn_fast_stream_tc_step(const fsn_fast_desc* d, const fsn_fast_weights* wt, const float* wav,
+                                       const int32_t* start, const int32_t* tail, int B, int K, int n_fft, int hop,
+                                       int win_length, float* enhanced, void* state, size_t state_bytes, void* workspace,
+                                       size_t workspace_bytes, fsn_stream_t stream) {
+  return fast_stream_run(d, wt, true, wav, start, tail, B, K, n_fft, hop, win_length, enhanced, state, state_bytes,
+                         workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// unit-test hook (tests/test_gpu_fast_stream_tc.py): the block-phased bottleneck on caller inputs.  B slots of M rows
+// (rows b M + m); slot b's call step j is frame m0[b] + j of its clip, and row q of catM / catE [B, S-1+St, M] is call
+// step q - (S-1).  fast_stream_bn_input_kernel forms the input of the nb = ceil(St / S) block ends into x [nb, B M, K] with
+// the scales scale [nb, B M], then sb_phased_lstm_tc_kernel runs: h / c [2, B M, H] hold the state entering step 0 and
+// receive slot b's state after step store[b] (-1: none); slot b enters step restart[b] with zero state; step i's output
+// of row b M + m goes to out [B, nb, 2M] at (b, i, m) (and the zero-padded second output at (b, i, M + m)).  m0, restart
+// and store are device tables [B]
+extern "C" int fsn_debug_sb_lstm_tc_phased(const fsn_seq_weights* bn, int H, int Ns, int Nf, int x3, const float* catM,
+                                           const float* catE, int B, int M, int S, int St, const int32_t* m0,
+                                           const float* scale, const int32_t* restart, const int32_t* store, float* h,
+                                           float* c, void* packed, float* x, float* out, fsn_stream_t stream) {
+  using namespace fsn;
+  FSN_REQUIRE(bn && catM && catE && m0 && scale && restart && store && h && c && packed && x && out, FSN_ERR_SHAPE,
+              "sb_phased_lstm_tc: missing buffer");
+  FSN_REQUIRE(B > 0 && M > 1 && S >= 1 && St > 0 && Ns >= 0 && Nf >= 0 && Ns < M && Nf < M, FSN_ERR_SHAPE,
+              "sb_phased_lstm_tc: bad shape B=%d M=%d S=%d St=%d Ns=%d Nf=%d", B, M, S, St, Ns, Nf);
+  FSN_REQUIRE(H == 128 || H == 256 || H == 384, FSN_ERR_UNSUPPORTED, "sb_phased_lstm_tc: hidden size %d", H);
+  const int Ksb = (2 * Ns + 1) + (2 * Nf + 1), nb = cdiv(St, S);
+  FSN_REQUIRE(Ksb <= 32, FSN_ERR_UNSUPPORTED, "sb_phased_lstm_tc: input width %d > 32", Ksb);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = sb_tc_pack_raw(bn, H, Ksb, 1, packed, st, x3 != 0);
+  if (rc) return rc;
+  fast_stream_bn_input_kernel<<<dim3(nb, B), 256, 0, st>>>(catM, catE, m0, 1, 0, St, M, Ns, Nf, S, x, scale);
+  FSN_CHECK_LAUNCH("fast_stream_bn_input_kernel");
+  SbTcArgs a;
+  memset(&a, 0, sizeof(a));
+  a.packed = packed; a.crm = out;
+  a.B = B; a.F = M; a.Tp = nb; a.Ns = Ns; a.Nf = Nf; a.H = H; a.act = FSN_ACT_RELU; a.x3 = x3 != 0;
+  a.map = RowMap{B, M, M, 1};
+  const size_t R = (size_t)B * M;
+  const SbCarry io{h, c, (size_t)M * H, R * H, M, restart, -1, (size_t)nb * 2 * M, 0, x, store};
+  return sb_tc_carry_forward(a, io, st);
 }

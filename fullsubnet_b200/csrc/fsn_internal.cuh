@@ -670,6 +670,9 @@ int sb_tc_forward(const SbTcArgs& a, cudaStream_t st);
 // at h / c [(r / rps) slot + l layer + (r % rps) H + u] (floats) are read before step 0 and written after store_step;
 // row r enters step restart[r / rps] with zero state; step t's output o of row r = b F + f goes to crm[b crm_bs +
 // (crm_t0 + t) 2F + o F + f].  a: unit_scale given, la = 0, no drop_band, no down-sampling.
+// store_at non-null: the block-phased instantiation (sb_phased_lstm_tc_kernel, fast_fullsubnet's stream): step t's input
+// of row r is x [(t R + r) Ksb + k], already down-sampled and scaled (a.unit_scale unused), and row r's state is stored
+// after step store_at[r / rps] (store_step unused)
 struct SbCarry {
   float *h, *c;
   size_t slot, layer;
@@ -678,6 +681,8 @@ struct SbCarry {
   int store_step;
   size_t crm_bs;
   int crm_t0;
+  const float* x;
+  const int* store_at;
 };
 int sb_tc_carry_forward(const SbTcArgs& a, const SbCarry& io, cudaStream_t st);
 bool sb_tc_supported(const fsn_model_desc* d);

@@ -47,6 +47,12 @@
 // there and its h of step j - 1 is written to shared memory as zero (j = 0: not loaded).  After step a.store_step the
 // fp32 (h, c) go back to io_h / io_c while the kernel runs on; step t's Linear output goes to frame crm_t0 + t of a
 // frame-major [clips, frames, 2F] cRM.
+//
+// PHASED (sb_phased_lstm_tc_kernel, fast_fullsubnet's chunked stream, DESIGN 4.14.2): CARRY over rows whose steps are
+// block ends at a phase of their own slot, so step t of row r is its slot's t-th block end in the call.  The gather warp
+// reads x_t dense from a.xin, which the caller wrote with the whole-clip gather's expression (so the operand bits are
+// those of the whole-clip call), and row r's state goes back to io_h / io_c after step store_at[r / io_rps] instead of
+// one store_step for all rows.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -196,7 +202,10 @@ static_assert(sizeof(Bars) <= 256, "barrier block too large");
 
 struct RowInfo {
   int src_b, src_f;   // source clip / frequency (drop_band map), src_b < 0: row beyond the batch
-  float scale;        // 1 / (mu' + 1e-5) of the source clip
+  // 1 / (mu' + 1e-5) of the source clip.  Block-phased CARRY: the bits of the step after which the row's state is
+  // stored (the carry policies read no scale here; making this a union with an int changes the code of the production
+  // instantiations)
+  float scale;
   union {
     int out_idx;      // crm index of (b', o=0, f', t=0) divided by T  (= (b'*2)*Fsub + f')
     int restart;      // CARRY: the step at which the row enters with zero state (none when outside [0, Tp))
@@ -228,6 +237,10 @@ struct KArgs {
   size_t io_slot, io_layer, crm_bs;
   const int* restart;
   int io_rps, store_step, crm_t0;
+  // block-phased CARRY instantiation only: the input x_t of row r at xin [(t R + r) Ksb + k], gathered, down-sampled and
+  // scaled by the caller; the state of row r stored after step store_at[r / io_rps] (none when outside [0, Tp))
+  const float* xin;
+  const int* store_at;
 };
 
 // ---------------------------------------------------------------- cycle stamps (PROBE instantiation)
@@ -315,9 +328,10 @@ __device__ __forceinline__ size_t carry_idx(const KArgs& a, int r, int u) {
 // PROBE: the same kernel with cycle stamps (ProbeField) written to a.stamps; the production launches use PROBE = false,
 // where every stamp below compiles away.  PROJ: the precomputed layer-0 projection and stored h1 (see the top of the
 // file); every PROJ and CARRY branch below is `if constexpr` or folds away, so the sb_lstm_tc_kernel instantiations are
-// the code they were before the policies existed
-template <bool X3, bool PROBE, bool PROJ, bool CARRY>
+// the code they were before the policies existed.  PHASED (only with CARRY): dense input and per-slot store steps
+template <bool X3, bool PROBE, bool PROJ, bool CARRY, bool PHASED = false>
 __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
+  static_assert(!PHASED || CARRY, "the block-phased policy is a carry policy");
   constexpr int PARTS = X3 ? 2 : 1;
   // probe clock: cycles since the previous mark (0 and no code without PROBE)
   long long pt = 0;
@@ -384,6 +398,7 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
       row_to_unit(a.map, r, ri.src_b, ri.src_f);
       if constexpr (CARRY) {
         ri.restart = a.restart[r / a.io_rps];
+        if constexpr (PHASED) ri.scale = __int_as_float(a.store_at[r / a.io_rps]);
       } else {
         ri.scale = a.inv2[ri.src_b];
         const int bq = r / a.Fsub, fq = r - bq * a.Fsub;
@@ -472,7 +487,9 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
       for (int n = 0; n < NB; ++n) {
         const RowInfo ri = rows[n];
         float v = 0.f;
-        if (ri.src_b >= 0 && lane < a.Ksb) {
+        if constexpr (PHASED) {
+          if (ri.src_b >= 0 && lane < a.Ksb) v = a.xin[((size_t)t * a.R + row0 + n) * a.Ksb + lane];
+        } else if (ri.src_b >= 0 && lane < a.Ksb) {
           const int col = (lane < nmag) ? reflect_idx(ri.src_f + lane - a.Ns, a.F)
                                         : reflect_idx(ri.src_f + (lane - nmag) - a.Nf, a.F);
           const float* src = (lane < nmag) ? a.magT : a.fbT;
@@ -759,7 +776,9 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
                 __half lo = __float2half_rn(h - __half2float(hi));
                 if constexpr (CARRY) {
                   const int n = 8 * j + 2 * (lane & 3) + e, r = row0 + n;
-                  if (t == a.store_step && r < a.R) {
+                  int store_t;
+                  if constexpr (PHASED) store_t = __float_as_int(rows[n].scale); else store_t = a.store_step;
+                  if (t == store_t && r < a.R) {
                     const size_t o = carry_idx(a, r, u) + layer * a.io_layer;
                     a.io_h[o] = h;
                     a.io_c[o] = cn;
@@ -878,6 +897,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_carry_lstm_tc_kernel(const __g
   sb_lstm_tc_body<X3, false, false, true>(a);
 }
 
+// chunked streaming: fast_fullsubnet's bottleneck continued from a carried (h, c), every row at its own block phase
+template <bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) sb_phased_lstm_tc_kernel(const __grid_constant__ KArgs a) {
+  sb_lstm_tc_body<X3, false, false, true, true>(a);
+}
+
 }  // namespace tc
 
 static int sb_ksb(const fsn_model_desc* d) { return (2 * d->sb_num_neighbors + 1) + (2 * d->fb_num_neighbors + 1); }
@@ -982,24 +1007,30 @@ int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
 }
 
 int sb_tc_carry_forward(const SbTcArgs& s, const SbCarry& io, cudaStream_t st) {
-  FSN_REQUIRE(s.unit_scale && io.h && io.c && io.restart && io.rps > 0 && s.la == 0 && s.shrink <= 1 && s.map.G <= 1,
-              FSN_ERR_SHAPE, "sb_carry_lstm_tc: per-row scales, state, restart steps, la = 0 and no drop_band / shrink");
+  const bool phased = io.store_at != nullptr;
+  FSN_REQUIRE((phased ? io.x != nullptr : s.unit_scale != nullptr) && io.h && io.c && io.restart && io.rps > 0 && s.la == 0 &&
+                  s.shrink <= 1 && s.map.G <= 1,
+              FSN_ERR_SHAPE,
+              "sb_carry_lstm_tc: per-row scales (block-phased: the input), state, restart steps, la = 0 and no drop_band / "
+              "shrink");
   tc::KArgs a;
   int rc = sb_tc_kargs(s, a);
   if (rc) return rc;
   a.io_h = io.h; a.io_c = io.c; a.io_slot = io.slot; a.io_layer = io.layer; a.io_rps = io.rps;
   a.restart = io.restart; a.store_step = io.store_step; a.crm_bs = io.crm_bs; a.crm_t0 = io.crm_t0;
+  a.xin = io.x; a.store_at = io.store_at;
   const int pairs = cdiv(cdiv(a.R, tc::NB), a.cluster) * a.cluster;
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
-  const void* kern = s.x3 ? (const void*)tc::sb_carry_lstm_tc_kernel<true> : (const void*)tc::sb_carry_lstm_tc_kernel<false>;
-  rc = s.x3 ? sb_tc_config<true>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, kern)
-            : sb_tc_config<false>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, kern);
+  void (*kern)(tc::KArgs);
+  if (phased) kern = s.x3 ? tc::sb_phased_lstm_tc_kernel<true> : tc::sb_phased_lstm_tc_kernel<false>;
+  else        kern = s.x3 ? tc::sb_carry_lstm_tc_kernel<true> : tc::sb_carry_lstm_tc_kernel<false>;
+  rc = s.x3 ? sb_tc_config<true>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, (const void*)kern)
+            : sb_tc_config<false>(s.H, a.stages, a.cluster, pairs, st, cfg, attr, (const void*)kern);
   if (rc) return rc;
-  rc = s.x3 ? check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_carry_lstm_tc_kernel<true>, a), "sb_carry_lstm_tc_kernel launch")
-            : check_cuda(cudaLaunchKernelEx(&cfg, tc::sb_carry_lstm_tc_kernel<false>, a), "sb_carry_lstm_tc_kernel launch");
-  if (rc) return rc;
-  FSN_CHECK_LAUNCH("sb_carry_lstm_tc_kernel");
+  const char* name = phased ? "sb_phased_lstm_tc_kernel" : "sb_carry_lstm_tc_kernel";
+  if ((rc = check_cuda(cudaLaunchKernelEx(&cfg, kern, a), name))) return rc;
+  FSN_CHECK_LAUNCH(name);
   return FSN_OK;
 }
 

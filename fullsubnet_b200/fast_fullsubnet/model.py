@@ -67,6 +67,9 @@ class Model(BaseModel):
     # workspace queries, delay, step
     STREAM_ENTRY_POINTS = ("fsn_fast_stream_state_bytes", "fsn_fast_stream_workspace_bytes", "fsn_fast_stream_delay",
                            "fsn_fast_stream_step")
+    # the same on the fp16 tensor cores (Streamer(tensor_cores=True), the model's f16x3_tc / f16_tc precision)
+    STREAM_TC_ENTRY_POINTS = ("fsn_fast_stream_tc_state_bytes", "fsn_fast_stream_tc_workspace_bytes",
+                              "fsn_fast_stream_tc_delay", "fsn_fast_stream_tc_step")
 
     def __init__(self, look_ahead, shrink_size, sequence_model, num_mels, encoder_input_size, bottleneck_hidden_size,
                  bottleneck_num_layers, noisy_input_num_neighbors, encoder_output_num_neighbors,
@@ -134,6 +137,21 @@ class Model(BaseModel):
 
     def _stream_weights(self):
         return (C.byref(self._weight_struct()),)
+
+    def _stream_tc_desc(self):
+        """Descriptor of the tensor-core streaming calls: the model's resolved precision, which must be f16x3_tc or
+        f16_tc (so "auto" streams the bits of the whole-clip call wherever that call runs the tensor cores)."""
+        prec = self._resolve_precision()
+        if prec == "fp32":
+            raise NotImplementedError("fullsubnet_b200: this model resolves to precision=\"fp32\", and tensor-core "
+                                      "streaming (tensor_cores=True) needs f16x3_tc or f16_tc; stream it with the default "
+                                      "Streamer(model, slots) (tensor_cores=False)")
+        return self._desc(_lib.PREC[prec])
+
+    def _stream_tc_weights(self):
+        self._stream_tc_desc()
+        _, w = self._structs(next(self.parameters()).device)  # with the cached packed bottleneck image
+        return (C.byref(w),)
 
     def _train_desc(self):
         return self._desc(_lib.PREC[self._resolve_train_precision()])

@@ -6,9 +6,9 @@ Built for fullband_baseline with ``cumulative_laplace_norm`` or ``forgetting_nor
 ``cumulative_laplace_norm`` (LSTM, ``precision="fp32"``).  Each model names its library calls in
 ``STREAM_ENTRY_POINTS`` and gives their arguments through ``_stream_desc()`` and ``_stream_weights()``.
 
-``tensor_cores=True`` streams fullsubnet on its fp16 tensor-core precision (``f16x3_tc`` or ``f16_tc``, what the model
-resolves to), bit for bit the whole-clip call of that precision, through ``STREAM_TC_ENTRY_POINTS``,
-``_stream_tc_desc()`` and ``_stream_tc_weights()``."""
+``tensor_cores=True`` streams fullsubnet and fast_fullsubnet on their fp16 tensor-core precision (``f16x3_tc`` or
+``f16_tc``, what the model resolves to, so ``precision="auto"`` too), bit for bit the whole-clip call of that precision,
+through ``STREAM_TC_ENTRY_POINTS``, ``_stream_tc_desc()`` and ``_stream_tc_weights()``."""
 from __future__ import annotations
 
 import ctypes as C
@@ -27,7 +27,12 @@ class Streamer:
     ``start[b]`` truthy begins a new clip in slot b with this chunk; ``tail[b] >= 0`` ends slot b's clip after that many
     samples of the chunk (-1 or None: it goes on).  Row b's first K*hop samples are the clip's samples [pos - delay,
     pos - delay + K*hop), pos being the clip's position before the call (negative positions as 0); on the call that
-    ends the clip the row holds the samples from pos - delay to the clip's end, then 0."""
+    ends the clip the row holds the samples from pos - delay to the clip's end, then 0.
+
+    ``tensor_cores=False`` (default): the fp32 kernels, for models built with ``precision="fp32"`` (fullsubnet,
+    fast_fullsubnet) and for fullband_baseline.  ``tensor_cores=True``: fullsubnet and fast_fullsubnet on the fp16 tensor
+    cores, for models that resolve to ``f16x3_tc`` or ``f16_tc`` (``precision="auto"`` included); the output matches the
+    whole-clip call of that precision, the delay and the state size are those of the fp32 stream."""
 
     def __init__(self, model, slots: int, n_fft: int = 512, hop: int = 256, win_length: int = 512,
                  tensor_cores: bool = False):
@@ -35,7 +40,7 @@ class Streamer:
             names = getattr(type(model), "STREAM_TC_ENTRY_POINTS", ())
             if not names:
                 raise NotImplementedError("fullsubnet_b200: tensor-core streaming (tensor_cores=True) is built for "
-                                          "fullsubnet")
+                                          "fullsubnet and fast_fullsubnet; stream this model with tensor_cores=False")
             self._desc_of, self._weights_of = model._stream_tc_desc, model._stream_tc_weights
         else:
             names = getattr(type(model), "STREAM_ENTRY_POINTS", ())

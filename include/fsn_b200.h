@@ -530,6 +530,23 @@ int fsn_fast_stream_step(const fsn_fast_desc* d, const fsn_fast_weights* w, cons
                          const int32_t* tail, int B, int K, int n_fft, int hop, int win_length, float* enhanced,
                          void* state, size_t state_bytes, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
+/* The same stream on the fp16 tensor cores (DESIGN 4.14.2): d->precision FSN_PREC_F16X3_TC or FSN_PREC_F16_TC, the output
+ * of every clip bit-identical to fsn_stft -> fsn_fast_model_forward -> fsn_istft of that precision on the whole clip
+ * (B = 1), delayed by D = fsn_fast_stream_tc_delay(d, n_fft, hop), the fsn_fast_stream_delay of the same shape.  The state
+ * is the fp32 stream's slot layout, byte for byte (fsn_fast_stream_tc_state_bytes = fsn_fast_stream_state_bytes of the
+ * FSN_PREC_FP32 descriptor): h and c stay fp32, and the bottleneck kernel splits h into fp16 hi / lo on load as it does
+ * after every step.  w->bn_packed: the fsn_fast_pack_bn_weights image fsn_fast_model_forward takes.  Semantics, limits
+ * and buffers as fsn_fast_stream_step; FSN_PREC_FP32, the offline norm, the GRU cell, bottleneck shapes the tensor-core
+ * kernel cannot take (bn_hidden != 384, bn_layers != 2, input width > 32), other n_fft and B > 65535 ->
+ * FSN_ERR_UNSUPPORTED (n_fft/2 + 1 != num_freqs: FSN_ERR_SHAPE), a null bn_packed -> FSN_ERR_SHAPE, before any CUDA
+ * call.  The number of kernel launches of a call does not depend on K.  Appended in ABI version 102. */
+size_t fsn_fast_stream_tc_state_bytes(const fsn_fast_desc* d, int B, int n_fft, int hop);
+size_t fsn_fast_stream_tc_workspace_bytes(const fsn_fast_desc* d, int B, int K_max, int n_fft, int hop);
+int fsn_fast_stream_tc_delay(const fsn_fast_desc* d, int n_fft, int hop);
+int fsn_fast_stream_tc_step(const fsn_fast_desc* d, const fsn_fast_weights* w, const float* wav, const int32_t* start,
+                            const int32_t* tail, int B, int K, int n_fft, int hop, int win_length, float* enhanced,
+                            void* state, size_t state_bytes, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+
 /* Chunked streaming enhancement of fullsubnet (DESIGN 4.14), with the semantics of the fullband_baseline calls above:
  * many streams, each advanced by K hops per call, the output of every clip bit-identical to fsn_enhance on the whole
  * clip (lengths NULL, B = 1), delayed by D = fsn_stream_delay(d, n_fft, hop) = n_fft/2 + (look_ahead + 1 + c) hop
@@ -784,6 +801,18 @@ int fsn_debug_sb_lstm_tc_carry(const fsn_seq_weights* sb, int H, int Ns, int Nf,
                                const float* fbT, int B, int F, int src_T, const float* unit_scale, int steps,
                                const int32_t* restart, int store_step, float* h, float* c, void* packed, float* crm,
                                fsn_stream_t stream);
+/* the block-phased carry instantiation (fast_fullsubnet's tensor-core stream bottleneck): B slots of M rows r = b*M + m,
+ * fc_out 1, ReLU.  Slot b's call step j is frame m0[b] + j of its clip; row q of catM / catE [B, S-1+St, M] is call
+ * step q - (S-1).  The input of the nb = ceil(St / S) block ends (frame 0 alone, then blocks of S frames ending on
+ * multiples of S) is formed into x [nb, B*M, K] as the whole-clip gather forms it with shrink = S, scaled by scale
+ * [nb, B*M] (0 past a slot's last block end in the call); then all nb steps run in one launch.  h / c [2 layers, B*M, H]
+ * hold the state entering step 0 and receive slot b's state after step store[b] (-1: none); slot b enters step restart[b]
+ * with zero state; out [B, nb, 2M] receives step i's output of row b*M + m at (b, i, m) and the zero-padded second
+ * output at (b, i, M + m).  m0, restart and store are device tables [B].  Arguments are checked before any CUDA call. */
+int fsn_debug_sb_lstm_tc_phased(const fsn_seq_weights* bn, int H, int Ns, int Nf, int x3, const float* catM,
+                                const float* catE, int B, int M, int S, int St, const int32_t* m0, const float* scale,
+                                const int32_t* restart, const int32_t* store, float* h, float* c, void* packed, float* x,
+                                float* out, fsn_stream_t stream);
 /* the same run through the cycle-stamp instantiation of the kernel (same output bits): CTAs [0, stamp_ctas) (at most
  * the 2 * ceil(B * Fsub / 32) CTAs that own rows) record, for the loop iterations [0, stamp_steps) (stamp_steps <=
  * steps + 1: layer 1 runs one iteration behind layer 0), FSN_SB_PROBE_FIELDS int64 per (CTA, iteration, layer, slot)
