@@ -207,6 +207,9 @@ _SIGNATURES = {
     "fsn_debug_sb_lstm_tc_max_clusters": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int)]),
     "fsn_debug_sb_lstm_tc": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _I,
                                        _I, _I, _I, _I, _P, _P, _P]),
+    "fsn_debug_sb_lstm_tc2_ws_bytes": (_S, [_I, _I, _I, _I, _I]),
+    "fsn_debug_sb_lstm_tc2": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _I, _I,
+                                        _I, _I, _P, _P, _P, _P]),
     "fsn_debug_sb_lstm_tc_carry": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _I, _P,
                                              _I, _P, _P, _P, _P, _P]),
     "fsn_debug_sb_lstm_tc_phased": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _P,

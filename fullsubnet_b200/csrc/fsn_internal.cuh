@@ -656,7 +656,12 @@ struct SbTcArgs {
   // iterations [0, stamp_its); the production launches leave it null
   long long* stamps;
   int stamp_ctas, stamp_its;
+  // non-null (and no stamps): the two-pass path (sb_l0_tc_kernel, sb_l1_tc_kernel), h0 of split_chunk pairs at a time
+  // (0: the default chunk) through this buffer of sb_tc_split_ws_bytes
+  void* h0ws;
+  int split_chunk;
 };
+size_t sb_tc_split_ws_bytes(int R, int Tp, int H, bool x3, int chunk_pairs = 0);
 size_t sb_tc_packed_bytes(const fsn_model_desc* d);
 // proj: the image sb_proj_forward streams (W_hh0, W_ih1, W_hh1 and layer 1's biases; no W_ih0 and no Linear)
 size_t sb_tc_packed_bytes_raw(int H, bool x3, bool proj = false);

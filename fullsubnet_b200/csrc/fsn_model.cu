@@ -42,6 +42,7 @@ struct ModelWs {
   float2* fs2;         // forgetting norm: frame sums of the full-band output (fs keeps the noisy magnitude's)
   SeqStackWs fb;
   float *sb_h0[2], *sb_h1[2], *sb_c0, *sb_c1;
+  void* sb_h0ws;  // tensor-core precisions: layer 0's output for the two-pass sub-band stack
   size_t bytes;
 };
 
@@ -103,6 +104,9 @@ static void carve_model(const fsn_model_desc* d, const Dims& m, void* base, Mode
     w.sb_c0 = c.take<float>(RH);
     w.sb_c1 = c.take<float>(RH);
   }
+  w.sb_h0ws = nullptr;
+  if (d->precision == FSN_PREC_F16_TC || d->precision == FSN_PREC_F16X3_TC)
+    w.sb_h0ws = c.take<uint8_t>(sb_tc_split_ws_bytes(m.R, m.Tp, d->sb_hidden, d->precision == FSN_PREC_F16X3_TC));
   w.cum1 = w.cum2 = nullptr;
   w.fs2 = nullptr;
   if (norm_per_step(d->norm_type)) {
@@ -169,6 +173,7 @@ static int model_core(const fsn_model_desc* d, const fsn_seq_weights* fb, const 
     a.B = B; a.F = F; a.Tp = Tp; a.la = d->look_ahead; a.Ns = d->sb_num_neighbors; a.Nf = d->fb_num_neighbors;
     a.H = Hs; a.act = d->sb_activation; a.map = map; a.x3 = d->precision == FSN_PREC_F16X3_TC;
     a.unit_scale = (cum || fgt) ? w.cum2 : nullptr;
+    a.h0ws = w.sb_h0ws;
     rc = sb_tc_forward(a, st);
     prof_mark(3, st);
     return rc;

@@ -54,6 +54,8 @@
 // those of the whole-clip call), and row r's state goes back to io_h / io_c after step store_at[r / io_rps] instead of
 // one store_step for all rows.
 #include <cuda_fp16.h>
+
+#include <algorithm>
 #include <stdlib.h>
 #include <string.h>
 
@@ -290,6 +292,15 @@ __device__ __forceinline__ float act_apply(float v, int act) {
 // for the compensated one, whose whole point is the fp32 error class
 template <bool X3> __device__ __forceinline__ float sg(float x) { return X3 ? 1.0f / (1.0f + expf(-x)) : fast_sigmoid(x); }
 template <bool X3> __device__ __forceinline__ float th(float x) { return X3 ? 1.0f - 2.0f / (1.0f + expf(2.0f * x)) : fast_tanh(x); }
+// LSTM cell of one (unit, row) from its gate pre-activations (MMA sums, gate order i, f, g, o) and biases b[4]: returns
+// the new c and sets h
+template <bool X3>
+__device__ __forceinline__ float lstm_cell(float ai, float af, float ag, float ao, const float (&b)[4], float cp,
+                                           float& h) {
+  const float cn = sg<X3>(af + b[1]) * cp + sg<X3>(ai + b[0]) * th<X3>(ag + b[2]);
+  h = sg<X3>(ao + b[3]) * th<X3>(cn);
+  return cn;
+}
 
 // Consumer warpgroup releases weight stage `bar` to the producers of the CL CTAs that share the stream (the CTAs of
 // the same half, ranks 2 q + half): one arrive per warpgroup and destination CTA (w_empty counts CL), warp q
@@ -757,7 +768,7 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
           for (int hh = 0; hh < 2; ++hh) {
             const int u = s * US + 16 * q + (lane >> 2) + 8 * hh;
             const float* bl = bias_g + (layer ? 4 * H : 0);
-            const float bi = bl[u], bff = bl[H + u], bg = bl[2 * H + u], bo = bl[3 * H + u];
+            const float b4[4] = {bl[u], bl[H + u], bl[2 * H + u], bl[3 * H + u]};
             const float w0 = fcw[u], w1 = fcw[H + u];
 #pragma unroll
             for (int j = 0; j < 4; ++j)
@@ -769,9 +780,9 @@ __device__ __forceinline__ void sb_lstm_tc_body(const KArgs& a) {
                 if constexpr (CARRY) {
                   if (rows[8 * j + 2 * (lane & 3) + e].restart == t) cp = 0.f;
                 }
-                const float cn = sg<X3>(acc[1][ri] + bff) * cp + sg<X3>(acc[0][ri] + bi) * th<X3>(acc[2][ri] + bg);
+                float h;
+                const float cn = lstm_cell<X3>(acc[0][ri], acc[1][ri], acc[2][ri], acc[3][ri], b4, cp, h);
                 if (layer) c1[ci] = cn; else c0[ci] = cn;
-                const float h = sg<X3>(acc[3][ri] + bo) * th<X3>(cn);
                 __half hi = __float2half_rn(h);
                 __half lo = __float2half_rn(h - __half2float(hi));
                 if constexpr (CARRY) {
@@ -903,6 +914,460 @@ __global__ void __launch_bounds__(NTHREADS, 1) sb_phased_lstm_tc_kernel(const __
   sb_lstm_tc_body<X3, false, false, true, true>(a);
 }
 
+// ---------------------------------------------------------------- two-pass stack (DESIGN 4.1.1)
+// The whole-clip stack as two persistent kernels over the same packed image, one per layer, with h0_t handed over
+// through global memory: a CTA then holds one layer's state only, which makes room for NB2 = 48 rows per pair, so each
+// streamed weight byte meets 48 rows instead of 32.  Per (gate, unit, row) both passes issue the fused kernel's MMAs in
+// its k order and part order into the same accumulator, apply its cell math and sum the Linear in its order; m64n48k16
+// computes every element as m64n32k16 does, so the result is the fused kernel's, bit for bit.
+//   layer 0 (sb_l0_tc_kernel): gathered x_t and h0_{t-1} -> h0_t, written to the B-operand image (hi, lo) in shared
+//           memory as in the fused kernel and from there by a bulk store to h0ws;
+//   layer 1 (sb_l1_tc_kernel): h0_t bulk-loaded from h0ws into a single buffer, h1 single-buffered as in the fused kernel,
+//           Linear(H -> 2) and the output store of the fused kernel.
+// h0ws holds the image of pair p (of the launch), step t at [(p Tp + t) img], img = PARTS nkh S_KBLK2 bytes: the hi
+// k-blocks of all H units, then the lo k-blocks.  Clusters are one pair, the ring is FSN_TC_STAGES deep.
+constexpr int NB2 = 48;                 // rows per CTA pair (MMA N)
+constexpr int S_KBLK2 = NB2 * KB * 2;   // 6144 B: one k-block of the state operand
+constexpr int X_BLK2 = NB2 * KS * 2;    // 3072 B: x_t
+// pairs per launch, fixed so that the workspace size does not depend on the device: two full waves of 66 resident
+// pairs on the 132-SM H100 SXM (a part with fewer SMs ends each chunk in a partial wave)
+constexpr int SPLIT_CHUNK_PAIRS = 132;
+
+__host__ __device__ inline Smem smem_plan2(int H, int stages, bool x3, int layer) {
+  Smem s;
+  const int nkh = H / KB;
+  uint32_t o = 0;
+  s.w = o; o += stages * W_TILE;
+  s.x = o; o += layer ? 0 : 2 * X_BLK2;
+  s.h0 = o; o += (layer ? 1 : 2) * nkh * S_KBLK2;  // layer 1: h0_t as loaded; layer 0: double-buffered as in the fused kernel
+  s.h1 = o; o += layer ? nkh * S_KBLK2 : 0;
+  s.lo = o; o += x3 ? (o - s.x) : 0;
+  s.fcw = o; o += layer ? 4 * MAX_MT * 2 * NB2 * 4 : 0;
+  s.fcp = o; o += layer ? 2 * 2 * NB2 * 4 : 0;
+  s.outst = o; o += layer ? NB2 * 2 * OUT_T * 4 : 0;
+  s.rows = o; o += NB2 * 16;
+  s.bars = o; o += 256;
+  s.total = o;
+  return s;
+}
+
+struct Bars2 {
+  uint64_t w_full[MAX_STAGES], w_empty[MAX_STAGES];
+  uint64_t x_full[2], x_empty[2];       // layer 0: the gathered x_t
+  uint64_t h_ready[2], h_empty[2];      // the pass's own state (layer 0: h0 buffers, layer 1: h1 in [0])
+  uint64_t h0_full, h0_free;            // layer 1: h0_t loaded / read by every MMA of this CTA
+  uint64_t l1_done, fc_done;
+  uint64_t fcp_full[2], fcp_empty[2];
+  uint64_t turn[MAX_MT];
+};
+static_assert(sizeof(Bars2) <= 256, "barrier block too large");
+
+struct SplitArgs {
+  KArgs k;
+  uint8_t* h0ws;
+  int row_base;  // first row of this launch's pair 0
+};
+
+template <bool X3, int LAYER>
+__device__ __forceinline__ void sb_split_body(const SplitArgs& sa) {
+  constexpr int PARTS = X3 ? 2 : 1;
+  constexpr int NJ = NB2 / 8;  // accumulator row groups
+  const KArgs& a = sa.k;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  const int H = a.H;
+  const int MT = H / 128;
+  const int nkh = H / KB;
+  const int STAGES = a.stages;
+  const uint32_t cl_rank = cluster_ctarank();
+  const int half = (int)(cl_rank & 1u);
+  const uint32_t peer = cl_rank ^ 1u;
+  const Smem sp = smem_plan2(H, STAGES, X3, LAYER);
+  const uint32_t LO = sp.lo - sp.x;
+  const PackedLayout PL = packed_layout(H, X3);
+  Bars2& bars = *reinterpret_cast<Bars2*>(smem + sp.bars);
+  RowInfo* rows = reinterpret_cast<RowInfo*>(smem + sp.rows);
+  float* fc_part = reinterpret_cast<float*>(smem + sp.fcw);
+  float* fcp = reinterpret_cast<float*>(smem + sp.fcp);
+  float* outst = reinterpret_cast<float*>(smem + sp.outst);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int pair = blockIdx.x >> 1;
+  const int row0 = sa.row_base + pair * NB2;
+  const int Tp = a.Tp;
+  const uint32_t img = PARTS * nkh * S_KBLK2;
+  uint8_t* ws_pair = sa.h0ws + (size_t)pair * Tp * img;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.w_full[s], 1); mbar_init(&bars.w_empty[s], 1); }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&bars.x_full[i], 1); mbar_init(&bars.x_empty[i], 4 * MT);
+      mbar_init(&bars.h_ready[i], 5 * MT);  // 4 MT local warps + MT peer copies
+      mbar_init(&bars.h_empty[i], MT);
+      mbar_init(&bars.fcp_full[i], 1); mbar_init(&bars.fcp_empty[i], 1);
+    }
+    mbar_init(&bars.h0_full, 1);
+    mbar_init(&bars.h0_free, 4 * MT);
+    mbar_init(&bars.fc_done, 1);
+    mbar_init(&bars.l1_done, 4 * MT);
+    for (int m = 0; m < MAX_MT; ++m) mbar_init(&bars.turn[m], 4);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (threadIdx.x < NB2) {
+    RowInfo ri;
+    const int r = row0 + threadIdx.x;
+    ri.src_b = -1; ri.src_f = 0; ri.scale = 0.f; ri.out_idx = 0;
+    if (r < a.R) {
+      row_to_unit(a.map, r, ri.src_b, ri.src_f);
+      ri.scale = a.inv2[ri.src_b];
+      const int bq = r / a.Fsub, fq = r - bq * a.Fsub;
+      ri.out_idx = bq * 2 * a.Fsub + fq;
+    }
+    rows[threadIdx.x] = ri;
+  }
+  {  // zero the state (h_{-1} = 0, x padding)
+    uint4* z = reinterpret_cast<uint4*>(smem + sp.x);
+    const int n16 = (sp.fcw - sp.x) / 16;
+    for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+  cluster_sync_all();
+
+  // registers of warpgroup 0 / of each consumer thread (4 x 128 x REG0 + 12 x 128 x REG1 <= 65536).  x3 layer 1 spills
+  // least with 160 for its consumers (Linear partial sums and cell state at 48 rows); everywhere else 56 / 152 spill
+  // least (DESIGN 4.1.1)
+  constexpr int REG0 = (LAYER == 1 && X3) ? 32 : 56, REG1 = (LAYER == 1 && X3) ? 160 : 152;
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REG0));
+    if (warp == 0) {
+      // ================= weight-stage producer: this half's stream of this layer, the same every step
+      const uint8_t* stream = a.packed + ((size_t)half * (PL.tiles0 + PL.tiles1) + (LAYER ? PL.tiles0 : 0)) * W_TILE;
+      const size_t tiles = LAYER ? PL.tiles1 : PL.tiles0;
+      uint32_t stage = 0, phase = 0;
+      for (int t = 0; t < Tp; ++t) {
+        const uint8_t* src = stream;
+        for (size_t tile = 0; tile < tiles; ++tile, src += W_TILE) {
+          mbar_wait_cta<false>(&bars.w_empty[stage], phase ^ 1);
+          if (elect_one()) {
+            mbar_expect_tx(&bars.w_full[stage], W_TILE);
+            bulk_g2s(smem + sp.w + stage * W_TILE, src, W_TILE, &bars.w_full[stage]);
+          }
+          __syncwarp();
+          if (++stage == (uint32_t)STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    } else if (LAYER == 0 && warp == 2) {
+      // ================= x_t gather, as in the fused kernel
+      const int nmag = 2 * a.Ns + 1;
+      for (int t = 0; t < Tp; ++t) {
+        mbar_wait_cta<true>(&bars.x_empty[t & 1], ((t >> 1) & 1) ^ 1);
+        uint8_t* xb = smem + sp.x + (t & 1) * X_BLK2;
+#pragma unroll 4
+        for (int n = 0; n < NB2; ++n) {
+          const RowInfo ri = rows[n];
+          float v = 0.f;
+          if (ri.src_b >= 0 && lane < a.Ksb) {
+            const int col = (lane < nmag) ? reflect_idx(ri.src_f + lane - a.Ns, a.F)
+                                          : reflect_idx(ri.src_f + (lane - nmag) - a.Nf, a.F);
+            const float* src = (lane < nmag) ? a.magT : a.fbT;
+            v = src[((size_t)ri.src_b * a.src_T + t) * a.F + col];
+            v *= a.unit_scale ? a.unit_scale[(size_t)t * a.R + row0 + n] : ri.scale;
+          }
+          const __half hi = __float2half_rn(v);
+          *reinterpret_cast<__half*>(xb + swz64_off(n, lane)) = hi;
+          if (X3) *reinterpret_cast<__half*>(xb + LO + swz64_off(n, lane)) = __float2half_rn(v - __half2float(hi));
+        }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.x_full[t & 1]);
+      }
+    } else if (LAYER == 1 && warp == 2) {
+      // ================= h0_t loader: the pair's image of step t, once every MMA of this CTA has read h0_{t-1}
+      for (int t = 0; t < Tp; ++t) {
+        if (t > 0) mbar_wait_cta<false>(&bars.h0_free, (t - 1) & 1);
+        if (elect_one()) {
+          const uint8_t* src = ws_pair + (size_t)t * img;
+          mbar_expect_tx(&bars.h0_full, img);
+          bulk_g2s(smem + sp.h0, src, nkh * S_KBLK2, &bars.h0_full);
+          if (X3) bulk_g2s(smem + sp.h0 + LO, src + nkh * S_KBLK2, nkh * S_KBLK2, &bars.h0_full);
+        }
+        __syncwarp();
+      }
+    } else if (LAYER == 1 && warp == 3) {
+      // ================= Linear(H -> 2) and output staging, as in the fused kernel (rows lane and lane + 32)
+      const float fcb0 = half ? 0.f : reinterpret_cast<const float*>(a.packed + PL.off_fcb)[0];
+      const float fcb1 = half ? 0.f : reinterpret_cast<const float*>(a.packed + PL.off_fcb)[1];
+      int staged = 0, t_stage0 = 0;
+      for (int t = 0; t < Tp; ++t) {
+        mbar_wait_cta<true>(&bars.h_ready[0], t & 1);
+        float s0[2], s1[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int n = lane + 32 * k;
+          s0[k] = fcb0; s1[k] = fcb1;
+          if (t >= a.la && n < NB2) {
+            for (int w = 0; w < 4 * MT; ++w) {
+              s0[k] += fc_part[(w * 2 + 0) * NB2 + n];
+              s1[k] += fc_part[(w * 2 + 1) * NB2 + n];
+            }
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.fc_done);
+        if (t < a.la) continue;
+        const int u = t - a.la, b = u & 1;
+        float* pb = fcp + b * 2 * NB2;
+        if (half) {
+          mbar_wait<true>(&bars.fcp_empty[b], ((u >> 1) & 1) ^ 1);
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            const int n = lane + 32 * k;
+            if (n < NB2) { st_remote_f32(pb + n, peer, s0[k]); st_remote_f32(pb + NB2 + n, peer, s1[k]); }
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive_cluster(&bars.fcp_full[b], peer);
+          continue;
+        }
+        mbar_wait<true>(&bars.fcp_full[b], (u >> 1) & 1);
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int n = lane + 32 * k;
+          if (n < NB2) { s0[k] += pb[n]; s1[k] += pb[NB2 + n]; }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive_cluster(&bars.fcp_empty[b], peer);
+        if (staged == 0) t_stage0 = u;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int n = lane + 32 * k;
+          if (n < NB2) {
+            outst[(n * 2 + 0) * OUT_T + staged] = act_apply(s0[k], a.act);
+            outst[(n * 2 + 1) * OUT_T + staged] = act_apply(s1[k], a.act);
+          }
+        }
+        ++staged;
+        if (staged == OUT_T || t == Tp - 1) {
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            const int n = lane + 32 * k;
+            if (n >= NB2) continue;
+            const RowInfo ri = rows[n];
+            if (ri.src_b < 0) continue;
+#pragma unroll
+            for (int o = 0; o < 2; ++o) {
+              float* dst = a.crm + ((size_t)ri.out_idx + (size_t)o * a.Fsub) * a.T + t_stage0;
+              for (int i = 0; i < staged; ++i) dst[i] = outst[(n * 2 + o) * OUT_T + i];
+            }
+          }
+          staged = 0;
+        }
+      }
+    }
+  } else {
+    // ================= consumer warpgroup m: slice s = MT half + m of this layer.  Fragment of thread (warp q, lane l):
+    // unit 64 s + 16 q + l/4 + 8 hh, row n = 8 j + 2 (l%4) + e, register acc[g][4 j + 2 hh + e]
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REG1));
+    const int m = __shfl_sync(0xffffffffu, (warp - 4) >> 2, 0);
+    const int q = __shfl_sync(0xffffffffu, warp & 3, 0);
+    const int s = half * MT + m;
+    if (m < MT) {
+      const float* bias_g = reinterpret_cast<const float*>(a.packed + PL.off_bias) + (LAYER ? 4 * H : 0);
+      const float* fcw = reinterpret_cast<const float*>(a.packed + PL.off_fcw);
+      float* my_part = fc_part + (size_t)(warp - 4) * 2 * NB2;
+      float c[4 * NJ];
+#pragma unroll
+      for (int i = 0; i < 4 * NJ; ++i) c[i] = 0.f;
+      const uint32_t a_lo0 = wg::desc_lo(smem_u32(smem + sp.w));
+      const uint32_t w_full0 = smem_u32(&bars.w_full[0]), w_empty0 = smem_u32(&bars.w_empty[0]);
+      const uint32_t turn_next = smem_u32(&bars.turn[m + 1 < MT ? m + 1 : 0]);
+      const uint32_t rel_local = q == 0;
+      const int nkb = LAYER ? PL.nkb1 : PL.nkb0;
+      const size_t tiles = LAYER ? PL.tiles1 : PL.tiles0;
+      int h_seen = 0, turns = 0;
+      for (int t = 0; t < Tp; ++t) {
+        if (LAYER == 0) {
+          mbar_wait_cta<false>(&bars.x_full[t & 1], (t >> 1) & 1);
+          for (; h_seen < t; ++h_seen) mbar_wait_cta<false>(&bars.h_ready[h_seen & 1], (h_seen >> 1) & 1);  // h0_{t-1}
+        } else {
+          mbar_wait_cta<false>(&bars.h0_full, t & 1);  // h0_t; h1_{t-1} is waited for after the h0_t k ranges
+        }
+        const uint32_t x_addr = smem_u32(smem + sp.x + (t & 1) * X_BLK2);
+        const uint32_t h0_cur = smem_u32(smem + sp.h0);
+        const uint32_t h0_prev = smem_u32(smem + sp.h0 + ((t + 1) & 1) * nkh * S_KBLK2);
+        const uint32_t h1_prev = smem_u32(smem + sp.h1);
+        const size_t first = (size_t)t * tiles + (size_t)m * nkb * PARTS;
+        float acc[4][4 * NJ];
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+#pragma unroll
+          for (int i = 0; i < 4 * NJ; ++i) acc[g][i] = 0.f;
+          wg::fence_operand(acc[g]);
+        }
+        int prev_stage = -1;
+        if (m > 0 || t > 0) { mbar_wait_cta<false>(&bars.turn[m], turns & 1); ++turns; }
+        int stage = __shfl_sync(0xffffffffu, (int)(first % (size_t)STAGES), 0);
+        uint32_t wphase = __shfl_sync(0xffffffffu, (uint32_t)((first / (size_t)STAGES) & 1), 0);
+        auto issue_stage = [&](int part, uint32_t bd, uint32_t b_hi, uint32_t ends_block) {
+          mbar_wait_cta_warp(w_full0 + 8 * stage, wphase);
+          mbar_arrive_elect_if(turn_next, ends_block);
+          wg::fence();
+          const uint32_t ad = a_lo0 + stage * (W_TILE >> 4);
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+            for (int g = 0; g < 4; ++g) {
+              const uint32_t a_off = g * (W_SUB >> 4) + kk * 2;
+              wg::mma_f16_n48_w(acc[g], ad, a_off, wg::DESC_SW64_HI, bd, kk * 2, b_hi);
+              if (X3 && part == 0) wg::mma_f16_n48_w(acc[g], ad, a_off, wg::DESC_SW64_HI, bd, (LO >> 4) + kk * 2, b_hi);
+            }
+          wg::commit();
+          wg::wait<1>();
+          release_stage(w_empty0 + 8 * prev_stage, prev_stage >= 0, rel_local, 0u, 0u);
+          prev_stage = stage;
+          if (++stage == STAGES) { stage = 0; wphase ^= 1; }
+        };
+        // B operand k ranges: layer 0: [x_t] [h0_{t-1} (H)]; layer 1: [h0_t (H)] [h1_{t-1} (H)] (the fused kernel's)
+        if (LAYER == 0) {
+#pragma unroll
+          for (int part = 0; part < PARTS; ++part) issue_stage(part, wg::desc_lo(x_addr), wg::DESC_SW64_HI, 0u);
+        }
+        const int nseg = LAYER ? 2 : 1;
+        int seg = 0;
+        do {
+          if (LAYER == 1 && seg == 1)
+            for (; h_seen < t; ++h_seen) mbar_wait_cta<false>(&bars.h_ready[0], h_seen & 1);  // h1_{t-1}
+          uint32_t bd = wg::desc_lo(LAYER == 0 ? h0_prev : seg == 0 ? h0_cur : h1_prev);
+          int kb = 0;
+          do {
+            const uint32_t ends_block = seg == nseg - 1 && kb == nkh - 1;
+#pragma unroll
+            for (int part = 0; part < PARTS; ++part) issue_stage(part, bd, wg::DESC_SW128_HI, 0u);
+            // layer 1: the first h1 stage's wait retired the last h0_t stage - this warp is done with h0_t
+            if (LAYER == 1 && seg == 1 && kb == 0 && lane == 0) mbar_arrive(&bars.h0_free);
+#pragma unroll
+            for (int part = 0; part < PARTS; ++part)
+              issue_stage(part, bd + (64 >> 4), wg::DESC_SW128_HI, part == PARTS - 1 ? ends_block : 0u);
+            bd += S_KBLK2 >> 4;
+          } while (++kb < nkh);
+        } while (++seg < nseg);
+        wg::wait<0>();
+#pragma unroll
+        for (int g = 0; g < 4; ++g) wg::fence_operand(acc[g]);
+        release_stage(w_empty0 + 8 * prev_stage, 1u, rel_local, 0u, 0u);
+        if (lane == 0) mbar_arrive(LAYER ? &bars.l1_done : &bars.x_empty[t & 1]);
+        // this warpgroup's MMAs have read the state the peer copied in (layer 0: h0_{t-1}, buffer (t + 1) & 1)
+        if (q == 2 && lane == 0) mbar_arrive_remote(&bars.h_empty[LAYER ? 0 : (t + 1) & 1], peer);
+        if (LAYER == 1 && t >= 1) mbar_wait_cta<false>(&bars.fc_done, (t - 1) & 1);  // FC(t-1) has read the partials
+        __half hv[2][2 * NJ], lv[2][2 * NJ];
+        uint8_t* hb = smem + (LAYER ? sp.h1 : sp.h0 + (t & 1) * nkh * S_KBLK2) + s * S_KBLK2;
+        float bias[2][4], fw[2][2];  // biases and Linear weights of the thread's units u(hh), hh = 0, 1
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int u = s * US + 16 * q + (lane >> 2) + 8 * hh;
+#pragma unroll
+          for (int g = 0; g < 4; ++g) bias[hh][g] = bias_g[g * H + u];
+          fw[hh][0] = LAYER ? fcw[u] : 0.f;
+          fw[hh][1] = LAYER ? fcw[H + u] : 0.f;
+        }
+        // row slot by row slot, both units of the slot, so that a slot's Linear partial sum (the fused kernel's: its
+        // unit hh = 0 term, then hh = 1, then the warp's lane sums) is stored before the next slot's cells run
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float f0 = 0.f, f1 = 0.f;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int ri = 4 * j + 2 * hh + e;
+              const int ci = hh * 2 * NJ + j * 2 + e;
+              float h;
+              c[ci] = lstm_cell<X3>(acc[0][ri], acc[1][ri], acc[2][ri], acc[3][ri], bias[hh], c[ci], h);
+              const __half hi = __float2half_rn(h);
+              hv[hh][j * 2 + e] = hi;
+              lv[hh][j * 2 + e] = __float2half_rn(h - __half2float(hi));
+              if (LAYER == 1) { f0 += h * fw[hh][0]; f1 += h * fw[hh][1]; }
+            }
+            if (LAYER == 1) {
+              // Linear(H->2) in fp32: sum over the warp's units (lanes with equal lane % 4 hold the same rows)
+              f0 += __shfl_xor_sync(0xffffffffu, f0, 4);
+              f0 += __shfl_xor_sync(0xffffffffu, f0, 8);
+              f0 += __shfl_xor_sync(0xffffffffu, f0, 16);
+              f1 += __shfl_xor_sync(0xffffffffu, f1, 4);
+              f1 += __shfl_xor_sync(0xffffffffu, f1, 8);
+              f1 += __shfl_xor_sync(0xffffffffu, f1, 16);
+              if (lane < 4) {
+                my_part[8 * j + 2 * lane + e] = f0;
+                my_part[NB2 + 8 * j + 2 * lane + e] = f1;
+              }
+            }
+          }
+        if (LAYER == 1) {
+          // every layer-1 MMA of step t in this CTA, and in the peer, has read h1_{t-1}: overwrite it with h1_t
+          mbar_wait_cta<false>(&bars.l1_done, t & 1);
+          mbar_wait_cta<false>(&bars.h_empty[0], t & 1);
+        } else if (t >= 1) {
+          // the peer's MMAs of step t - 1 have read h0_{t-2} in buffer t & 1; this CTA's own readers of the buffer are
+          // ordered by the ring turn, as in the fused kernel
+          mbar_wait_cta<false>(&bars.h_empty[t & 1], ((t - 1) >> 1) & 1);
+        }
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int u = 16 * q + (lane >> 2) + 8 * hh;
+          uint8_t* ub = hb + (u & 7) * 2;
+          const int chunk = u >> 3;
+#pragma unroll
+          for (int j = 0; j < NJ; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int n = 8 * j + 2 * (lane & 3) + e;
+              uint8_t* p = ub + (n >> 3) * 1024 + (n & 7) * 128 + ((chunk ^ (n & 7)) << 4);
+              *reinterpret_cast<__half*>(p) = hv[hh][j * 2 + e];
+              if (X3) *reinterpret_cast<__half*>(p + LO) = lv[hh][j * 2 + e];
+            }
+        }
+        fence_proxy_async_smem();
+        __syncwarp();
+        // h_t to the peer (and this CTA's readers), except layer 0's last h0, which no MMA of the pass reads: the peer
+        // never waits for that copy, so it could still be in flight when the pair leaves the SMs (layer 1's last copy
+        // is waited for by the peer's Linear warp before its teardown)
+        const bool exchange = LAYER == 1 || t < Tp - 1;
+        uint64_t* ready = &bars.h_ready[LAYER ? 0 : t & 1];
+        if (exchange && lane == 0) mbar_arrive(ready);
+        // layer 0: the store of step t - 1 has read its buffer, which the writes of step t + 1 reuse (they follow the
+        // named barrier below)
+        if (LAYER == 0 && q == 0 && lane == 0) bulk_wait_read_all();
+        named_sync(1 + m, 128);
+        if (q == 0 && lane == 0) {
+          if (exchange) {
+            mbar_arrive_expect_tx_remote(ready, peer, PARTS * S_KBLK2);
+            bulk_s2s_remote(hb, S_KBLK2, ready, peer);
+            if (X3) bulk_s2s_remote(hb + LO, S_KBLK2, ready, peer);
+          }
+          if (LAYER == 0) {
+            uint8_t* dst = ws_pair + (size_t)t * img + s * S_KBLK2;
+            bulk_s2g(dst, hb, S_KBLK2);
+            if (X3) bulk_s2g(dst + nkh * S_KBLK2, hb + LO, S_KBLK2);
+            bulk_commit();
+          }
+        }
+      }
+      if (LAYER == 0 && q == 0 && lane == 0) bulk_wait_all();
+    }
+  }
+
+  __syncthreads();
+  cluster_sync_all();
+}
+
+template <bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) sb_l0_tc_kernel(const __grid_constant__ SplitArgs a) {
+  sb_split_body<X3, 0>(a);
+}
+template <bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) sb_l1_tc_kernel(const __grid_constant__ SplitArgs a) {
+  sb_split_body<X3, 1>(a);
+}
+
 }  // namespace tc
 
 static int sb_ksb(const fsn_model_desc* d) { return (2 * d->sb_num_neighbors + 1) + (2 * d->fb_num_neighbors + 1); }
@@ -998,7 +1463,61 @@ static int sb_tc_kargs(const SbTcArgs& s, tc::KArgs& a) {
   return FSN_OK;
 }
 
+size_t sb_tc_split_ws_bytes(int R, int Tp, int H, bool x3, int chunk_pairs) {
+  if (!sb_tc_shape_ok(H, 0) || R <= 0 || Tp <= 0) return 0;
+  const int pairs = std::min(cdiv(R, tc::NB2), chunk_pairs > 0 ? chunk_pairs : tc::SPLIT_CHUNK_PAIRS);
+  return (size_t)pairs * Tp * (x3 ? 2 : 1) * (H / tc::KB) * tc::S_KBLK2;
+}
+
+template <bool X3>
+static int sb_split_launch(const tc::SplitArgs& sa, int pairs, int layer, cudaStream_t st) {
+  void (*kern)(tc::SplitArgs) = layer ? tc::sb_l1_tc_kernel<X3> : tc::sb_l0_tc_kernel<X3>;
+  const size_t smem = tc::smem_plan2(sa.k.H, sa.k.stages, X3, layer).total + 1024;
+  const char* name = layer ? "sb_l1_tc_kernel" : "sb_l0_tc_kernel";
+  int rc = check_cuda(cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), name);
+  if (rc) return rc;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(2 * pairs);
+  cfg.blockDim = dim3(128 + 128 * (sa.k.H / 128));
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if ((rc = check_cuda(cudaLaunchKernelEx(&cfg, kern, sa), name))) return rc;
+  FSN_CHECK_LAUNCH(name);
+  return FSN_OK;
+}
+
+// the two-pass stack (sb_l0_tc_kernel, sb_l1_tc_kernel) over chunks of s.split_chunk pairs (0: SPLIT_CHUNK_PAIRS), each
+// chunk's h0 through s.h0ws (sb_tc_split_ws_bytes)
+static int sb_tc_split_forward(const SbTcArgs& s, cudaStream_t st) {
+  FSN_REQUIRE(s.shrink <= 1, FSN_ERR_UNSUPPORTED, "sb_lstm_tc two-pass: no time down-sampling");
+  tc::SplitArgs sa;
+  memset(&sa, 0, sizeof(sa));
+  int rc = sb_tc_kargs(s, sa.k);
+  if (rc) return rc;
+  sa.k.cluster = 1;
+  sa.h0ws = (uint8_t*)s.h0ws;
+  const int total = cdiv(sa.k.R, tc::NB2);
+  const int chunk = s.split_chunk > 0 ? s.split_chunk : tc::SPLIT_CHUNK_PAIRS;
+  for (int p0 = 0; p0 < total; p0 += chunk) {
+    const int pairs = std::min(chunk, total - p0);
+    sa.row_base = p0 * tc::NB2;
+    for (int layer = 0; layer < 2; ++layer)
+      if ((rc = s.x3 ? sb_split_launch<true>(sa, pairs, layer, st) : sb_split_launch<false>(sa, pairs, layer, st)))
+        return rc;
+  }
+  return FSN_OK;
+}
+
 int sb_tc_forward(const SbTcArgs& s, cudaStream_t st) {
+  if (s.h0ws && !s.stamps) return sb_tc_split_forward(s, st);
   tc::KArgs a;
   int rc = sb_tc_kargs(s, a);
   if (rc) return rc;
@@ -1161,6 +1680,46 @@ extern "C" int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, in
                                     int cluster, void* packed, float* crm, fsn_stream_t stream) {
   return sb_lstm_tc_hook(sb, H, Ns, Nf, fc_out, act, x3, magT, fbT, B, F, src_T, G, inv2, unit_scale, la, steps, shrink,
                          stages, cluster, packed, crm, nullptr, 0, 0, stream);
+}
+
+// unit-test hook (tests/test_gpu_subband_two_pass.py): the two-pass stack on the inputs of fsn_debug_sb_lstm_tc, in
+// chunks of chunk_pairs pairs (0: the production chunk), with h0ws of fsn_debug_sb_lstm_tc2_ws_bytes
+extern "C" size_t fsn_debug_sb_lstm_tc2_ws_bytes(int R, int steps, int H, int x3, int chunk_pairs) {
+  return fsn::sb_tc_split_ws_bytes(R, steps, H, x3 != 0, chunk_pairs);
+}
+
+extern "C" int fsn_debug_sb_lstm_tc2(const fsn_seq_weights* sb, int H, int Ns, int Nf, int act, int x3, const float* magT,
+                                     const float* fbT, int B, int F, int src_T, int G, const float* inv2,
+                                     const float* unit_scale, int la, int steps, int stages, int chunk_pairs, void* packed,
+                                     void* h0ws, float* crm, fsn_stream_t stream) {
+  using namespace fsn;
+  FSN_REQUIRE(stages == 0 || (stages >= 2 && stages <= tc::MAX_STAGES), FSN_ERR_UNSUPPORTED,
+              "sb_lstm_tc2: ring depth %d (0, 2, 3 or 4)", stages);
+  FSN_REQUIRE(sb && magT && fbT && inv2 && packed && h0ws && crm && chunk_pairs >= 0, FSN_ERR_SHAPE,
+              "sb_lstm_tc2: missing buffer");
+  FSN_REQUIRE(B > 0 && F > 1 && src_T > 0 && Ns >= 0 && Nf >= 0 && Ns < F && Nf < F && G >= 1, FSN_ERR_SHAPE,
+              "sb_lstm_tc2: bad shape B=%d F=%d src_T=%d Ns=%d Nf=%d", B, F, src_T, Ns, Nf);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "sb_lstm_tc2: activation %d", act);
+  const int g = (B > 1 && G > 1) ? G : 1;
+  FSN_REQUIRE(B == 1 || B > G, FSN_ERR_SHAPE, "sb_lstm_tc2: batch size %d <= num_groups %d", B, G);
+  const int Fsub = g > 1 ? F / g : F;
+  FSN_REQUIRE(Fsub > 0, FSN_ERR_SHAPE, "sb_lstm_tc2: num_freqs < num_groups");
+  FSN_REQUIRE(steps > 0 && steps <= src_T && la >= 0 && la < steps, FSN_ERR_SHAPE,
+              "sb_lstm_tc2: steps %d / look-ahead %d for %d source frames", steps, la, src_T);
+  FSN_REQUIRE(sb_tc_shape_ok(H, (2 * Ns + 1) + (2 * Nf + 1)), FSN_ERR_UNSUPPORTED,
+              "sb_lstm_tc2: unsupported hidden size %d / input width %d", H, (2 * Ns + 1) + (2 * Nf + 1));
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = sb_tc_pack_raw(sb, H, (2 * Ns + 1) + (2 * Nf + 1), 2, packed, st, x3 != 0);
+  if (rc) return rc;
+  SbTcArgs a;
+  memset(&a, 0, sizeof(a));
+  a.packed = packed; a.magT = magT; a.fbT = fbT; a.inv2 = inv2; a.unit_scale = unit_scale; a.crm = crm;
+  a.B = B; a.F = F; a.Tp = src_T; a.la = la; a.Ns = Ns; a.Nf = Nf; a.H = H; a.act = act;
+  a.steps = steps; a.shrink = 1; a.x3 = x3 != 0;
+  a.map = RowMap{B, F, Fsub, g};
+  a.stages = stages;
+  a.h0ws = h0ws; a.split_chunk = chunk_pairs;
+  return sb_tc_forward(a, st);
 }
 
 extern "C" int fsn_debug_sb_lstm_tc_probe(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,

@@ -69,6 +69,21 @@ __device__ __forceinline__ void mma_f16_n32_w(float (&d)[16], uint32_t a_lo, uin
       : "memory");
 }
 
+// m64n48k16, otherwise mma_f16_n32_w
+__device__ __forceinline__ void mma_f16_n48_w(float (&d)[24], uint32_t a_lo, uint32_t a_off, uint32_t a_hi,
+                                              uint32_t b_lo, uint32_t b_off, uint32_t b_hi) {
+  asm volatile(
+      "{\n\t.reg .b32 al, bl;\n\t.reg .b64 a, b;\n\t"
+      "add.u32 al, %24, %25;\n\tadd.u32 bl, %27, %28;\n\t"
+      "mov.b64 a, {al, %26};\n\tmov.b64 b, {bl, %29};\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,"
+      "%18,%19,%20,%21,%22,%23}, a, b, 1, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "r"(a_lo), "r"(a_off), "r"(a_hi), "r"(b_lo), "r"(b_off), "r"(b_hi)
+      : "memory");
+}
+
 // m64n64k16, f16 operands; scale_d = 0 overwrites D
 __device__ __forceinline__ void mma_f16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(

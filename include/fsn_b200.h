@@ -792,6 +792,15 @@ int fsn_debug_sb_lstm_tc(const fsn_seq_weights* sb, int H, int Ns, int Nf, int f
                          const float* magT, const float* fbT, int B, int F, int src_T, int G,
                          const float* inv2, const float* unit_scale, int la, int steps, int shrink,
                          int stages, int cluster, void* packed, float* crm, fsn_stream_t stream);
+/* the two-pass stack of the whole-clip fullsubnet enhance (one kernel per layer, 48 rows per CTA pair, h0 through h0ws)
+ * on the inputs of fsn_debug_sb_lstm_tc with fc_out 2 and no down-sampling; rows run chunk_pairs x 48 at a time
+ * (0 = the production chunk), h0ws holds fsn_debug_sb_lstm_tc2_ws_bytes(B*Fsub, steps, H, x3, chunk_pairs) bytes (0 =
+ * unsupported H).  Same bits as fsn_debug_sb_lstm_tc.  Arguments are checked before any CUDA call. */
+size_t fsn_debug_sb_lstm_tc2_ws_bytes(int R, int steps, int H, int x3, int chunk_pairs);
+int fsn_debug_sb_lstm_tc2(const fsn_seq_weights* sb, int H, int Ns, int Nf, int act, int x3, const float* magT,
+                          const float* fbT, int B, int F, int src_T, int G, const float* inv2, const float* unit_scale,
+                          int la, int steps, int stages, int chunk_pairs, void* packed, void* h0ws, float* crm,
+                          fsn_stream_t stream);
 /* the carry instantiation of the kernel (the tensor-core stream's sub band): B clips of F rows r = b*F + f, no
  * drop_band, look-ahead 0, fc_out 2, unit_scale [steps, B*F] required.  h / c [2 layers, B*F, H] hold the state entering
  * step 0 and receive the state after store_step (-1: none); row r enters step restart[r] with zero state (0: its h / c
