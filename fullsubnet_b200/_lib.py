@@ -210,6 +210,8 @@ _SIGNATURES = {
     "fsn_debug_sb_lstm_tc2_ws_bytes": (_S, [_I, _I, _I, _I, _I]),
     "fsn_debug_sb_lstm_tc2": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _I, _I,
                                         _I, _I, _P, _P, _P, _P]),
+    "fsn_debug_sb_tc2_pass": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _I, _I,
+                                        _I, _I, _I, _I, _P, _P, _S, _P, _P]),
     "fsn_debug_sb_lstm_tc_carry": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _I, _P,
                                              _I, _P, _P, _P, _P, _P]),
     "fsn_debug_sb_lstm_tc_phased": (C.c_int, [C.POINTER(SeqWeights), _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _P,

@@ -1722,6 +1722,57 @@ extern "C" int fsn_debug_sb_lstm_tc2(const fsn_seq_weights* sb, int H, int Ns, i
   return sb_tc_forward(a, st);
 }
 
+// unit-test hook (tests/test_gpu_subband_two_pass_layers.py): one pass of the two-pass stack over one chunk, the launch
+// sb_tc_split_forward makes for it.  Layer 0 writes the images of pairs [pair0, pair0 + pairs) to h0ws (image of the
+// chunk's pair p, step t at (p steps + t) img); layer 1 reads them from h0ws as the caller left it and writes those
+// pairs' rows of crm.  h0ws_bytes must cover pairs x fsn_debug_sb_lstm_tc2_ws_bytes(48, steps, H, x3, 0)
+extern "C" int fsn_debug_sb_tc2_pass(const fsn_seq_weights* sb, int H, int Ns, int Nf, int act, int x3, const float* magT,
+                                     const float* fbT, int B, int F, int src_T, int G, const float* inv2,
+                                     const float* unit_scale, int la, int steps, int stages, int layer, int pair0,
+                                     int pairs, void* packed, void* h0ws, size_t h0ws_bytes, float* crm,
+                                     fsn_stream_t stream) {
+  using namespace fsn;
+  // every check precedes the first CUDA call
+  FSN_REQUIRE(stages == 0 || (stages >= 2 && stages <= tc::MAX_STAGES), FSN_ERR_UNSUPPORTED,
+              "sb_tc2_pass: ring depth %d (0, 2, 3 or 4)", stages);
+  FSN_REQUIRE(layer == 0 || layer == 1, FSN_ERR_SHAPE, "sb_tc2_pass: layer %d (0 or 1)", layer);
+  FSN_REQUIRE(sb && magT && fbT && inv2 && packed && crm, FSN_ERR_SHAPE, "sb_tc2_pass: missing buffer");
+  FSN_REQUIRE(B > 0 && F > 1 && src_T > 0 && Ns >= 0 && Nf >= 0 && Ns < F && Nf < F && G >= 1, FSN_ERR_SHAPE,
+              "sb_tc2_pass: bad shape B=%d F=%d src_T=%d Ns=%d Nf=%d", B, F, src_T, Ns, Nf);
+  FSN_REQUIRE(act >= FSN_ACT_NONE && act <= FSN_ACT_RELU6, FSN_ERR_SHAPE, "sb_tc2_pass: activation %d", act);
+  const int g = (B > 1 && G > 1) ? G : 1;
+  FSN_REQUIRE(B == 1 || B > G, FSN_ERR_SHAPE, "sb_tc2_pass: batch size %d <= num_groups %d", B, G);
+  const int Fsub = g > 1 ? F / g : F;
+  FSN_REQUIRE(Fsub > 0, FSN_ERR_SHAPE, "sb_tc2_pass: num_freqs < num_groups");
+  FSN_REQUIRE(steps > 0 && steps <= src_T && la >= 0 && la < steps, FSN_ERR_SHAPE,
+              "sb_tc2_pass: steps %d / look-ahead %d for %d source frames", steps, la, src_T);
+  const int total = cdiv(B * Fsub, tc::NB2);
+  FSN_REQUIRE(pair0 >= 0 && pairs > 0 && pair0 < total && pairs <= total - pair0, FSN_ERR_SHAPE,
+              "sb_tc2_pass: pairs [%d, %d + %d) outside the %d pairs of %d rows", pair0, pair0, pairs, total, B * Fsub);
+  FSN_REQUIRE(sb_tc_shape_ok(H, (2 * Ns + 1) + (2 * Nf + 1)), FSN_ERR_UNSUPPORTED,
+              "sb_tc2_pass: unsupported hidden size %d / input width %d", H, (2 * Ns + 1) + (2 * Nf + 1));
+  const size_t need = (size_t)pairs * sb_tc_split_ws_bytes(tc::NB2, steps, H, x3 != 0, 1);
+  FSN_REQUIRE(h0ws && h0ws_bytes >= need, FSN_ERR_WORKSPACE, "sb_tc2_pass: h0ws of %zu bytes, %zu needed", h0ws_bytes,
+              need);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = sb_tc_pack_raw(sb, H, (2 * Ns + 1) + (2 * Nf + 1), 2, packed, st, x3 != 0);
+  if (rc) return rc;
+  SbTcArgs a;
+  memset(&a, 0, sizeof(a));
+  a.packed = packed; a.magT = magT; a.fbT = fbT; a.inv2 = inv2; a.unit_scale = unit_scale; a.crm = crm;
+  a.B = B; a.F = F; a.Tp = src_T; a.la = la; a.Ns = Ns; a.Nf = Nf; a.H = H; a.act = act;
+  a.steps = steps; a.shrink = 1; a.x3 = x3 != 0;
+  a.map = RowMap{B, F, Fsub, g};
+  a.stages = stages;
+  tc::SplitArgs sa;
+  memset(&sa, 0, sizeof(sa));
+  if ((rc = sb_tc_kargs(a, sa.k))) return rc;
+  sa.k.cluster = 1;
+  sa.h0ws = (uint8_t*)h0ws;
+  sa.row_base = pair0 * tc::NB2;
+  return x3 ? sb_split_launch<true>(sa, pairs, layer, st) : sb_split_launch<false>(sa, pairs, layer, st);
+}
+
 extern "C" int fsn_debug_sb_lstm_tc_probe(const fsn_seq_weights* sb, int H, int Ns, int Nf, int fc_out, int act, int x3,
                                           const float* magT, const float* fbT, int B, int F, int src_T, int G,
                                           const float* inv2, const float* unit_scale, int la, int steps, int shrink,

@@ -801,6 +801,16 @@ int fsn_debug_sb_lstm_tc2(const fsn_seq_weights* sb, int H, int Ns, int Nf, int 
                           const float* fbT, int B, int F, int src_T, int G, const float* inv2, const float* unit_scale,
                           int la, int steps, int stages, int chunk_pairs, void* packed, void* h0ws, float* crm,
                           fsn_stream_t stream);
+/* one pass (layer 0 or 1) of that stack over one chunk: the CTA pairs [pair0, pair0 + pairs) of 48 rows, launched as
+ * the production loop launches a chunk.  Layer 0 writes only h0ws: the fp16 image of the chunk's pair p at step t at
+ * byte (p*steps + t)*img, img = (x3 ? 2 : 1) * H * 96, the 128B-swizzled k-blocks of 64 units x 48 rows, hi blocks
+ * before lo blocks.  Layer 1 reads h0ws as given and writes only those pairs' rows of crm.  h0ws_bytes >= pairs *
+ * steps * img.  Errors: FSN_ERR_SHAPE (layer, shape, pairs beyond the rows, missing buffer), FSN_ERR_WORKSPACE (h0ws),
+ * FSN_ERR_UNSUPPORTED (stages, H, input width), each before any CUDA call. */
+int fsn_debug_sb_tc2_pass(const fsn_seq_weights* sb, int H, int Ns, int Nf, int act, int x3, const float* magT,
+                          const float* fbT, int B, int F, int src_T, int G, const float* inv2, const float* unit_scale,
+                          int la, int steps, int stages, int layer, int pair0, int pairs, void* packed, void* h0ws,
+                          size_t h0ws_bytes, float* crm, fsn_stream_t stream);
 /* the carry instantiation of the kernel (the tensor-core stream's sub band): B clips of F rows r = b*F + f, no
  * drop_band, look-ahead 0, fc_out 2, unit_scale [steps, B*F] required.  h / c [2 layers, B*F, H] hold the state entering
  * step 0 and receive the state after store_step (-1: none); row r enters step restart[r] with zero state (0: its h / c

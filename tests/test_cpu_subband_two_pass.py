@@ -66,11 +66,9 @@ def test_hook_rejects_bad_arguments_before_any_cuda_call():
         return lib.fsn_debug_sb_lstm_tc2(C.byref(s), H, 15, 0, act, 1, p, p, B, 33, 10, G, p, None, la, steps, stages,
                                          chunk, p, ws, p, None)
 
-    assert call(H=192) != 0
-    assert call(act=7) != 0
-    assert call(B=2, G=2) != 0
-    assert call(la=10) != 0
-    assert call(steps=11) != 0
-    assert call(stages=5) != 0
-    assert call(chunk=-1) != 0
-    assert call(ws=None) != 0
+    SH, UN = _l.FSN_ERR_SHAPE, _l.FSN_ERR_UNSUPPORTED
+    for kw, code in ((dict(H=192), UN), (dict(act=7), SH), (dict(B=2, G=2), SH), (dict(la=10), SH),
+                     (dict(steps=11), SH), (dict(stages=5), UN), (dict(stages=1), UN), (dict(chunk=-1), SH),
+                     (dict(ws=None), SH)):
+        assert call(**kw) == code, kw
+        assert lib.fsn_last_error_code() == code, kw
