@@ -191,6 +191,8 @@ _SIGNATURES = {
     "fsn_si_sdr_lengths": (C.c_int, [_P, _P, _P, _I, _I, _P, _P]),
     "fsn_stoi_workspace_bytes": (_S, [_I, _I, _I]),
     "fsn_stoi": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _S, _P]),
+    "fsn_resample_workspace_bytes": (_S, [_I, _I, _I, _I, _I]),
+    "fsn_resample": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _P, _I, _P, _S, _P]),
     "fsn_rir_convolve": (C.c_int, [_P, _P, _P, _I, _I, _I, _P, _P]),
     "fsn_snr_mix": (C.c_int, [_P, _P, _P, _P, _F, _F, _I, _I, _P, _P, _P]),
     "fsn_debug_row_to_unit": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -7,7 +7,7 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["fsn_dsp.cu", "fsn_lstm_simt.cu", "fsn_subband_tc.cu", "fsn_fullband.cu", "fsn_lstm_rec_tc.cu", "fsn_fast_model.cu", "fsn_improved.cu", "fsn_fullband_baseline.cu", "fsn_train.cu", "fsn_fast_train.cu", "fsn_fullband_train.cu", "fsn_improved_train.cu", "fsn_mix.cu", "fsn_stoi.cu", "fsn_stream.cu", "fsn_tgemm.cu", "fsn_model.cu"]
+SOURCES = ["fsn_dsp.cu", "fsn_lstm_simt.cu", "fsn_subband_tc.cu", "fsn_fullband.cu", "fsn_lstm_rec_tc.cu", "fsn_fast_model.cu", "fsn_improved.cu", "fsn_fullband_baseline.cu", "fsn_train.cu", "fsn_fast_train.cu", "fsn_fullband_train.cu", "fsn_improved_train.cu", "fsn_mix.cu", "fsn_stoi.cu", "fsn_resample.cu", "fsn_stream.cu", "fsn_tgemm.cu", "fsn_model.cu"]
 LIB = os.path.join(HERE, "libfsn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -65,7 +65,8 @@ def _resampled_length(n: int, rate: int, sr: int) -> int:
 def load_wav(path, sr: int = 16000) -> np.ndarray:
     """float32 [C, N] at ``sr`` from a PCM wav file, every channel kept (``librosa.load(path, mono=False, sr=sr)``, with
     librosa's int -> float scaling).  When the file's rate differs, each channel goes through the windowed-sinc resampler
-    of ``Inferencer.resample``, which stands in for librosa's soxr and is not bit-identical to it."""
+    of ``Inferencer.resample`` on the host, which stands in for librosa's soxr and is not bit-identical to it
+    (``Dataset(resample_on_device=True)`` runs the same filter on the device for the preloaded lists)."""
     y, rate = read_wav(_expand(path))
     if rate != sr:
         from .inferencer import Inferencer
@@ -90,15 +91,21 @@ class Dataset(torch.utils.data.Dataset):
     ``Trainer`` turns such a batch into ``(noisy, clean)`` on the device with ``snr_mix``.  A clean or noise file with
     more than one channel is refused (the reference asserts on the first and silently interleaves the second); a RIR
     file may have several channels, one of which each reverberant item draws.  ``pre_load_*`` holds the waveforms in host
-    memory, read by ``num_workers`` threads.  Files at another sample rate are resampled as ``load_wav`` says."""
+    memory, read by ``num_workers`` threads.  Files at another sample rate are resampled as ``load_wav`` says.
+
+    ``resample_on_device`` (a keyword after the reference's arguments): the preloaded lists are resampled on the current
+    CUDA device by ``resample_batch`` (fsn_resample, every RIR channel a clip), equal to the host resampler to float32
+    rounding, and kept as host arrays as before; lengths, and so every draw, are the host's.  Lists that are not
+    preloaded load in the DataLoader workers, where CUDA cannot run, and keep the host resampler."""
 
     def __init__(self, clean_dataset, clean_dataset_limit, clean_dataset_offset, noise_dataset, noise_dataset_limit,
                  noise_dataset_offset, rir_dataset, rir_dataset_limit, rir_dataset_offset, snr_range, reverb_proportion,
                  silence_length, target_dB_FS, target_dB_FS_floating_value, sub_sample_length, sr,
-                 pre_load_clean_dataset, pre_load_noise, pre_load_rir, num_workers):
+                 pre_load_clean_dataset, pre_load_noise, pre_load_rir, num_workers, resample_on_device=False):
         super().__init__()
         self.sr = sr
         self.num_workers = num_workers
+        self.resample_on_device = bool(resample_on_device)
         clean = self._offset_and_limit(self._read_list(clean_dataset), clean_dataset_offset, clean_dataset_limit)
         noise = self._offset_and_limit(self._read_list(noise_dataset), noise_dataset_offset, noise_dataset_limit)
         rir = self._offset_and_limit(self._read_list(rir_dataset), rir_dataset_offset, rir_dataset_limit)
@@ -137,10 +144,28 @@ class Dataset(torch.utils.data.Dataset):
     def _preload(self, paths, kind):
         from concurrent.futures import ThreadPoolExecutor
         with ThreadPoolExecutor(max_workers=max(1, int(self.num_workers or 1))) as pool:
-            waves = list(pool.map(lambda p: load_wav(p, self.sr), paths))
+            if self.resample_on_device:
+                waves = self._resample_on_device(list(pool.map(lambda p: read_wav(_expand(p)), paths)))
+            else:
+                waves = list(pool.map(lambda p: load_wav(p, self.sr), paths))
         if kind != "rir":
             waves = [self._mono(w, p, kind) for p, w in zip(paths, waves)]
         return [(p, w) for p, w in zip(paths, waves)]
+
+    def _resample_on_device(self, files, batch_size: int = 32):
+        """(float32 [C, N], rate) per file -> float32 [C, n] at ``sr``: the channels of files at another rate go through
+        ``resample_batch`` on the current CUDA device, in batches of clips of similar length (``plan_batches``)."""
+        from .acoustics.resample import resample_batch
+        from .inferencer import plan_batches
+        clips = [(f, c) for f, (w, rate) in enumerate(files) if rate != self.sr for c in range(w.shape[0])]
+        device = torch.device("cuda", torch.cuda.current_device())
+        out = {}
+        for chunk in plan_batches([files[f][0].shape[1] for f, _ in clips], batch_size, 0.5):
+            picked = [clips[i] for i in chunk]
+            ys = resample_batch([files[f][0][c] for f, c in picked], [files[f][1] for f, _ in picked], self.sr, device)
+            out.update((fc, y.cpu().numpy()) for fc, y in zip(picked, ys))
+        return [w if rate == self.sr else np.stack([out[f, c] for c in range(w.shape[0])])
+                for f, (w, rate) in enumerate(files)]
 
     @staticmethod
     def _mono(wav, path, kind) -> np.ndarray:

@@ -189,20 +189,28 @@ class Inferencer:
 
     # ------------------------------------------------------------------ wav files (base_inferencer.py:163-195, dataset_inference.py:39-43)
     @staticmethod
+    def mono(wav: np.ndarray) -> np.ndarray:
+        """float32 [C, N] -> [N]: the channels averaged like librosa.load(mono=True)."""
+        return wav[0] if len(wav) == 1 else np.ascontiguousarray(wav.T).mean(axis=1).astype(np.float32)
+
+    @staticmethod
     def load_wav(path, sr: int = 16000) -> np.ndarray:
         """Mono float32 waveform at ``sr`` from a PCM wav file (8/16/24/32-bit; channels averaged like librosa).  The reference calls
         ``librosa.load(path, sr=sr)`` (dataset_inference.py:41): same int -> float scaling (1/32768 for 16-bit); when the
         file's rate differs, a windowed-sinc polyphase resampler stands in for librosa's soxr (not bit-identical to it -
-        the hot-path parity contract starts at the 16 kHz waveform)."""
+        the hot-path parity contract starts at the 16 kHz waveform).  The resampling here is ``resample`` on the host;
+        ``enhance_files(..., resample_on_device=True)`` runs the same filter on the device instead."""
         wav, rate = read_wav(path)
-        y = wav[0] if len(wav) == 1 else np.ascontiguousarray(wav.T).mean(axis=1).astype(np.float32)  # librosa(mono=True)
+        y = Inferencer.mono(wav)
         if rate != sr:
             y = Inferencer.resample(y, rate, sr)
         return np.ascontiguousarray(y, dtype=np.float32)
 
     @staticmethod
     def resample(y: np.ndarray, sr_in: int, sr_out: int, zeros: int = 24) -> np.ndarray:
-        """Band-limited (hann-windowed sinc) polyphase resampling, host side."""
+        """Band-limited (hann-windowed sinc) polyphase resampling on the host, in float64 with [n_out, 2 * half]
+        temporaries.  ``acoustics.resample.resample_batch`` computes the same outputs for a batch of clips on the device
+        (fsn_resample), equal to these to float32 rounding."""
         from math import gcd
         g = gcd(int(sr_in), int(sr_out))
         up, down = sr_out // g, sr_in // g
@@ -220,7 +228,8 @@ class Inferencer:
         return (vals * w).sum(axis=1).astype(np.float32)
 
     @torch.no_grad()
-    def enhance_files(self, paths, output_dir, batch_size: int = 64, sr=None, max_padding: float = 0.0):
+    def enhance_files(self, paths, output_dir, batch_size: int = 64, sr=None, max_padding: float = 0.0,
+                      resample_on_device: bool = False):
         """Batched form of the host loop of base_inferencer.py:163-195: ``plan_batches`` groups the files, each batch
         goes through ONE fused library call (pinned staging buffer -> H2D -> the model's enhance_pcm -> int16 D2H), and
         ``<output_dir>/<stem>.wav`` is written as 16-bit PCM like the reference.  Returns the written paths.
@@ -229,20 +238,39 @@ class Inferencer:
         and fullsubnet and fullband_baseline with a power-of-two n_fft; other models keep equal-length batches): clips of
         different lengths share a batch, padded to its longest clip by at most that fraction of the batch's samples,
         through fsn_enhance / fsn_improved_enhance / fsn_fullband_enhance.  Every file is bit-identical either way: each
-        clip is bounded by its own length in the length-dependent kernels."""
+        clip is bounded by its own length in the length-dependent kernels.
+
+        ``resample_on_device``: files are read and mixed to mono on the host as ``load_wav`` does, and each batch is
+        assembled on the device by ``resample_batch`` (fsn_resample, one call per input rate): files at another rate are
+        resampled there, in float64 like ``resample`` and equal to it to float32 rounding, and files at ``sr`` are copied
+        with their bits.  Batches are planned on the same lengths, so files at ``sr`` come out byte-identical to the
+        default, and resampled ones within an int16 step of it."""
         from pathlib import Path
         sr = int(sr or self.sr)
         out_dir = Path(output_dir)
         out_dir.mkdir(parents=True, exist_ok=True)
-        clips = [(Path(p), self.load_wav(p, sr)) for p in paths]
-        lens = [len(y) for _, y in clips]
+        if resample_on_device:
+            from .acoustics.resample import resample_batch, resampled_length
+            clips, rates = [], []
+            for p in paths:
+                wav, rate = read_wav(p)
+                clips.append((Path(p), self.mono(wav)))
+                rates.append(rate)
+            lens = [resampled_length(len(y), rate, sr) for (_, y), rate in zip(clips, rates)]
+        else:
+            clips = [(Path(p), self.load_wav(p, sr)) for p in paths]
+            lens = [len(y) for _, y in clips]
         written = [None] * len(clips)
         for chunk in plan_batches(lens, batch_size, max_padding if self.supports_lengths() else 0.0):
             L = max(lens[i] for i in chunk)
             mixed = any(lens[i] != L for i in chunk)
-            stage = (torch.zeros if mixed else torch.empty)(len(chunk), L, dtype=torch.float32).pin_memory()
-            for r, i in enumerate(chunk):
-                stage[r, :lens[i]] = torch.from_numpy(clips[i][1])
+            if resample_on_device:  # every row written, 0 past each clip
+                stage = torch.empty(len(chunk), L, dtype=torch.float32, device=self.device)
+                resample_batch([clips[i][1] for i in chunk], [rates[i] for i in chunk], sr, self.device, out=stage)
+            else:
+                stage = (torch.zeros if mixed else torch.empty)(len(chunk), L, dtype=torch.float32).pin_memory()
+                for r, i in enumerate(chunk):
+                    stage[r, :lens[i]] = torch.from_numpy(clips[i][1])
             pcm = self.enhance_to_pcm(stage, lengths=[lens[i] for i in chunk] if mixed else None).cpu().numpy()
             for r, i in enumerate(chunk):
                 dst = out_dir / f"{clips[i][0].stem}.wav"

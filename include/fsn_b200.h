@@ -73,7 +73,8 @@ enum { FSN_PREC_FP32 = 0, FSN_PREC_F16_TC = 1, FSN_PREC_TF32_TC = 2, FSN_PREC_F1
  * The version counts changes that break an existing caller.  Entry points added since 102 leave every earlier argument
  * list and struct as it was, so the version stays 102; a caller finds them by symbol: fsn_cirm_mse_per_clip (+ its
  * workspace query), fsn_si_sdr_lengths (the grouped validation loss and SI-SDR), fsn_clip_adam_steps (one Adam step
- * count per tensor) and fsn_stoi (+ its workspace query and the fsn_debug_stoi_stages hook).  FSN_NORM_FORGETTING is a new
+ * count per tensor), fsn_stoi (+ its workspace query and the fsn_debug_stoi_stages hook) and fsn_resample (+ its
+ * workspace query).  FSN_NORM_FORGETTING is a new
  * value of an existing field, refused by every older entry point it does not apply to, with the fsn_debug_forgetting_*
  * hooks.  fsn_improved_weights grew sb_packed, read only by the FSN_PREC_F16X3_TC / FSN_PREC_F16_TC precisions that
  * fsn_improved_forward / _enhance accept since, with fsn_improved_packed_bytes / fsn_improved_pack_sb_weights and the
@@ -666,6 +667,27 @@ int fsn_si_sdr_lengths(const float* reference, const float* estimation, const in
 size_t fsn_stoi_workspace_bytes(int B, int L_max, int sr);
 int fsn_stoi(const float* clean, const float* estimate, const int32_t* lengths, int B, int L_max, int sr, float* out,
              void* workspace, size_t workspace_bytes, fsn_stream_t stream);
+
+/* fullsubnet_b200/inferencer.py  Inferencer.resample(y, sr_in, sr_out, zeros) per clip: the hann-windowed sinc that brings
+ * a wav file at another rate to the model's (the stand-in for librosa.load(path, sr=sr)'s soxr, not bit-identical to
+ * soxr).  g = gcd(sr_in, sr_out), up = sr_out/g, down = sr_in/g, cutoff = min(1, up/down), half = ceil(zeros/cutoff).
+ *   x [B, N_max]; clip b is its first N_b = lengths[b] samples (lengths: nullable, host int32 [B], read during the call
+ *     through kernel parameters, not kept; NULL = every clip N_max; 1 <= lengths[b] <= N_max).
+ *   y [B, N_out_max]: row b holds n_out_b = ceil(N_b * up / down) samples (integer arithmetic: the host's float64
+ *     ceiling for N_b * up < 2^53), 0 from there on; N_out_max must be at least the largest n_out_b.
+ *   Output n, in float64 as the host: t = n * down / up, taps idx = floor(t) + k for k in [-half + 1, half], d = t - idx,
+ *     w = cutoff * sinc(cutoff * d) * (0.5 + 0.5 * cos(pi * clip(d / half, -1, 1))) (numpy's sinc), taps outside
+ *     [0, N_b) contribute 0; the products are summed in float64 in ascending k and the sum is rounded once to float32.
+ *     CUDA's sin / cos differ from the host's libm by up to 2 ulp, so an output can differ from the host's by one float32
+ *     rounding step; almost all are bit-identical (DESIGN 4.10.1).  sr_in == sr_out copies the input bits.
+ *   Checks, all before any CUDA call: B > 0, N_max > 0, positive rates, zeros >= 1, x, y non-null, the lengths and
+ *   N_out_max (FSN_ERR_SHAPE); B > 65535 or half > 2^29 (FSN_ERR_UNSUPPORTED); the workspace (FSN_ERR_WORKSPACE).
+ *   Never allocates, never synchronises the host; one call may be captured in a CUDA graph.
+ * fsn_resample_workspace_bytes: the workspace of any call with these arguments (the device length table, 256-byte
+ * aligned); 0 with fsn_last_error set on bad arguments; needs no GPU.  An addition at version 102 (see fsn_version). */
+size_t fsn_resample_workspace_bytes(int B, int N_max, int sr_in, int sr_out, int zeros);
+int fsn_resample(const float* x, const int32_t* lengths, int B, int N_max, int sr_in, int sr_out, int zeros, float* y,
+                 int N_out_max, void* workspace, size_t workspace_bytes, fsn_stream_t stream);
 
 /* recipes/dns_interspeech_2020/dataset_train.py:136-199  Dataset.snr_mix for a batch (SURVEY 8f rank 4): the random
  * draws (snr, noisy target dBFS, which RIR) are made by the caller and passed in.
